@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- headline benchmark of the B200-native association engine.
+"""bench.py -- headline benchmark of the H100-native association engine.
 
 Metric (BASELINE.json): pair-associations/s of BatchVisualSORT on 256 scenes x 512 tracks x 512 detections x 512-dim
 features (cfg5), one `predict` per step.  pair-associations = sum over scenes of N_s * M_s per frame.
@@ -49,6 +49,9 @@ def parse():
                     help="override the visual metric's threshold: a float, or 'max' = the reference's default Euclidean(f32::MAX)")
     ap.add_argument("--feat-noise", type=float, default=None, help="override the workload's feature noise (sensitivity sweeps)")
     ap.add_argument("--no-scatter", action="store_true", help="N > 1: skip the ingest-rank scatter arm (sb200_shard_*)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the outputs of the last timed step to DIR/<name>.npy (float32 / float64), so that two builds "
+                         "can be compared output for output on the same seeded inputs")
     return ap.parse_args()
 
 
@@ -299,17 +302,13 @@ def run_reference(args):
     return 0
 
 
-def newest_traffic():
-    """DRAM bytes per launch of the dominant kernel from the newest ncu --set full capture under profiles/."""
-    import glob
-
-    best = None
-    for fn in sorted(glob.glob(os.path.join(ROOT, "profiles", "r*_dominant_kernel_traffic*.json"))):
-        try:
-            best = (fn, json.load(open(fn)))
-        except Exception:
-            pass
-    return best
+def dump_outputs(out_dir, arrays):
+    """Writes each array as out_dir/<name>.npy in float64 (integers: exact up to 2^53) or float32 (floating point)."""
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        a = np.asarray(a)
+        a = a.astype(np.float32 if a.dtype.kind == "f" and a.itemsize <= 4 else np.float64)
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def run_scatter_arm(eng, torch, dist, new_tracker, frames, dboxes, dfeats, W, K, D, visual, max_total, rank, world, local,
@@ -543,6 +542,7 @@ def main():
     sampler.mark_end()
     e2e_total_ms = float(ev0.elapsed_time(ev1))
     ids_e2e_last = out_ring[(W + K - 1) % RING]["ids"][: len(frames[W + K - 1]["boxes"])].copy()
+    e2e_last = {k_: v_[: len(frames[W + K - 1]["boxes"])].copy() for k_, v_ in out_ring[(W + K - 1) % RING].items()}
     t_e2e.close()
 
     # ---------------------------------------------------------------- value: inputs resident in HBM
@@ -620,6 +620,16 @@ def main():
     launches = eng.launch_count() - l0
     c1 = t_dev.work_counters()
     ids_dev_last = d_ids[(W + K - 1) & 1][: len(frames[W + K - 1]["boxes"])].cpu().numpy().astype(np.uint64)
+    if args.dump_outputs:
+        # what the callers of the two timed paths received for the last timed frame (this rank's scenes); a few MB
+        n_last = len(frames[W + K - 1]["boxes"])
+        b = (W + K - 1) & 1
+        dump_outputs(os.path.join(args.dump_outputs, f"rank{rank}") if world > 1 else args.dump_outputs, {
+            "ids": d_ids[b][:n_last].cpu().numpy(), "epochs": d_ep[b][:n_last].cpu().numpy(),
+            "lengths": d_len[b][:n_last].cpu().numpy(), "voting_types": d_vt[b][:n_last].cpu().numpy(),
+            "e2e_ids": e2e_last["ids"], "e2e_epochs": e2e_last["epochs"], "e2e_lengths": e2e_last["lengths"],
+            "e2e_voting_types": e2e_last["voting_types"], "e2e_predicted_boxes": e2e_last["predicted"],
+            "e2e_observed_boxes": e2e_last["observed"]})
     assert np.array_equal(ids_dev_last, ids_e2e_last), "device-pointer and host-pointer paths disagree"
     if gather is not None:   # every rank holds every shard's ids of the last step
         gl = gather["buf"][(W + K - 1) & 1].view(world, max_total)[rank][: len(ids_dev_last)].cpu().numpy().astype(np.uint64)
@@ -664,25 +674,18 @@ def main():
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception:
             pass
-        hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
-        tf_peak = float(peaks.get("bf16_tflops", 1590.0))
-        peak_src = "measured (MEASURED_PEAKS.json, burst)" if peaks else "fallback (B200_PROFILING.md)"
+        hbm_peak = float(peaks.get("hbm_gbs", 3350.0))
+        tf_peak = float(peaks.get("bf16_tflops", 989.0))
+        peak_src = "measured (MEASURED_PEAKS.json, burst)" if peaks else "H100 SXM data sheet (dense BF16, HBM3; 700 W card)"
         Kobs = 3 if visual else 1
-        tr = newest_traffic()
         if visual and tc_frames:
             fl = 2.0 * dots * D / K                       # algorithmic FLOP per launch: 2 * M * (feature rows) * D
             m_tot = float(np.mean([len(frames[i]["boxes"]) for i in range(W, W + K)]))
             kms = stage_ms["vis_screen"]
             achieved = fl / (kms * 1e-3) / 1e12
-            floor_bytes = None
-            traffic = None
-            if tr:
-                traffic = tr[1].get("dram_bytes_per_launch")
-                floor_bytes = tr[1].get("operand_floor_bytes")
-            roof = {"kernel": "tensor-core visual cost kernel (tcgen05 BF16, kernels_feat_tc.cu)", "bound": "tensor",
+            roof = {"kernel": "tensor-core visual cost kernel (wgmma BF16, kernels_feat_tc.cu)", "bound": "tensor",
                     "achieved": achieved, "peak": tf_peak, "unit": "TFLOP/s", "frac": achieved / tf_peak,
-                    "traffic": traffic, "traffic_source": os.path.basename(tr[0]) if tr else None,
-                    "traffic_over_operand_floor": (traffic / floor_bytes) if traffic and floor_bytes else None,
+                    "traffic": None,
                     "peak_source": peak_src, "algorithmic_flops_per_launch": fl,
                     # the kernel runs a fraction of a millisecond inside a ~1 ms step at full clocks, so the burst peak is
                     # the denominator; against the sustained figure of MEASURED_PEAKS.json the fraction would be:
@@ -696,8 +699,8 @@ def main():
             fl = 3.0 * dots * D / K
             kms = stage_ms["visual_cost"]
             roof = {"kernel": "vis_cost_kernel (exact f32 SIMT)", "bound": "fp32", "achieved": fl / (kms * 1e-3) / 1e12,
-                    "peak": 75.0, "unit": "TFLOP/s", "frac": fl / (kms * 1e-3) / 1e12 / 75.0, "traffic": None,
-                    "peak_source": "nominal FP32 (no measured figure)", "kernel_ms": kms}
+                    "peak": 67.0, "unit": "TFLOP/s", "frac": fl / (kms * 1e-3) / 1e12 / 67.0, "traffic": None,
+                    "peak_source": "H100 SXM data sheet FP32 (no measured figure)", "kernel_ms": kms}
         else:
             m_l = np.concatenate([np.diff(frames[i]["det_offsets"]) for i in range(W, W + K)]).astype(np.float64)
             n_mean = units / max(1.0, float(m_l.sum()))       # mean tracks per scene over the timed steps

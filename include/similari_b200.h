@@ -1,5 +1,5 @@
 /*
- * similari_b200.h -- C ABI of the B200-native association engine (libsimilari_b200.so).
+ * similari_b200.h -- C ABI of the H100-native association engine (libsimilari_b200.so).
  *
  * Drop-in boundary for Similari's per-frame cost-matrix + assignment hot path.  The reference has no C ABI
  * (it is a Rust crate with PyO3 classes); these entry points are what a Rust `extern "C"` block inside

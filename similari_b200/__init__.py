@@ -1,4 +1,4 @@
-"""similari_b200 -- B200-native association engine for Similari's cost-matrix + assignment hot path.
+"""similari_b200 -- H100-native association engine for Similari's cost-matrix + assignment hot path.
 
 `similari_b200.engine`  array-level interface (numpy in / numpy out) over the C ABI of libsimilari_b200.so
 `similari_b200.api`     the reference's Python class names (Sort, BatchSort, VisualSort, BatchVisualSort, nms, ...)

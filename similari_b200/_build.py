@@ -1,4 +1,4 @@
-"""Builds libsimilari_b200.so (hand-written sm_100a CUDA + the C ABI) in-tree with nvcc.
+"""Builds libsimilari_b200.so (hand-written sm_90a CUDA + the C ABI) in-tree with nvcc.
 
 nvcc cross-compiles without a GPU; the built .so travels to the GPU box with the repo snapshot."""
 from __future__ import annotations
@@ -15,7 +15,7 @@ HEADERS = ["sb_engine.cuh", "sb_math.cuh", "sb_own_area.cuh", "sb_tc.cuh", "sb_s
 
 # --fmad=false: the reference (Rust) never contracts a*b+c; parity of the i64 weights depends on it.
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "--fmad=false",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "--fmad=false",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-fno-fast-math", "-Xptxas", "-v",
 ]
 
@@ -57,7 +57,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         f.write("\n".join(logs))
     if verbose:
         print("\n".join(logs))
-    cmd = [nvcc(), "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_100a,code=sm_100a", "-cudart", "static", "-ldl"]
+    cmd = [nvcc(), "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_90a,code=sm_90a", "-cudart", "static", "-ldl"]
     subprocess.check_call(cmd)
     return LIB
 

@@ -1,6 +1,6 @@
 """ctypes binding of libsimilari_b200.so (the C ABI declared in include/similari_b200.h).
 
-The library is the product: hand-written sm_100a CUDA kernels behind an extern "C" boundary.  There is no CPU
+The library is the product: hand-written sm_90a CUDA kernels behind an extern "C" boundary.  There is no CPU
 fallback -- if the shared library is missing this module raises, and every compute call raises without a GPU.
 """
 from __future__ import annotations
@@ -94,7 +94,7 @@ def lib():
         return _lib
     if not os.path.exists(LIB_PATH):
         raise Sb200Error(
-            f"{LIB_PATH} is missing: build it with `python -m similari_b200._build` (nvcc, sm_100a). "
+            f"{LIB_PATH} is missing: build it with `python -m similari_b200._build` (nvcc, sm_90a). "
             "similari_b200 has no CPU fallback.")
     L = C.CDLL(LIB_PATH)
     vp, i32, i64, u64, f32 = C.c_void_p, C.c_int32, C.c_int64, C.c_uint64, C.c_float

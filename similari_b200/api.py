@@ -1,4 +1,4 @@
-"""The reference's Python surface (PyO3 module `similari`, src/lib.rs:117-161) over the B200 engine.
+"""The reference's Python surface (PyO3 module `similari`, src/lib.rs:117-161) over the H100 engine.
 
 Class names, constructor defaults and method names follow the reference so that `import similari_b200.api as similari`
 is a drop-in for scripts using the cost-matrix + assignment trackers.  Each class cites the PyO3 definition it mirrors.

@@ -2,7 +2,7 @@
 // request from an ingest rank to the ranks that own its scenes and to gather the assigned track records back.
 //
 // Scenes are independent (`compatible()` needs equal scene ids, src/trackers/sort.rs:250-251) and track state is sticky per
-// GPU, so a multi-GPU tracker is N independent single-GPU trackers plus this exchange -- the B200 counterpart of the
+// GPU, so a multi-GPU tracker is N independent single-GPU trackers plus this exchange -- the GPU counterpart of the
 // reference's voting-shard fan-out (src/trackers/sort/batch_api.rs:197-207: one channel per voting thread, results collected
 // on PredictionBatchResult's channel).  One process per GPU; the caller (bench.py under torchrun, or a Rust host) ships the
 // 128-byte NCCL unique id from rank 0 to the other ranks over whatever control channel it has.

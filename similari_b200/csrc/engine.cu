@@ -256,7 +256,7 @@ struct sb200_tracker {
   DBuf f_winner, f_cvt, f_pos, f_vis, f_scenes, f_newcount,
       f_status, f_featdst, f_apprank, f_appmeta, f_posgq, f_frameout, f_excl, f_prewin, f_own, f_ownovf, f_dyn, f_ws, f_tmeta, f_rowinfo, f_slabc, f_slabm, f_slabmask,
       f_dscene, f_maxc, f_maxcval, f_drowb, f_dcolb, f_slabk, f_scene_max, f_tiles, f_pairs, f_colmeta, f_colgeo, f_colb, f_colvalid, f_rowmeta, f_poslist, f_counters, f_visval;
-  int num_sms = 148;
+  int num_sms = 132;
   DBuf o_ids, o_epochs, o_lengths, o_vt, o_pred, o_obs;
   HBuf h_small;
   bool adapt_dense = false;     // a nominally selective threshold whose survivor lists overflow: treat it as non-selective
@@ -861,10 +861,9 @@ int sb200_tracker::predict(int32_t n_scenes, const uint64_t* scene_ids, const in
     tc.use_tc = true;
     tc.dense = want_dense;
     {
-      // SB200_SCREEN = single | multicast | pair (default): CTA organisation of the screen kernel (the dense kernel: pairs)
+      // SB200_SCREEN = single | multicast (default): CTA organisation of the screen kernel (the dense kernel: multicast)
       const char* e = getenv("SB200_SCREEN");
       tc.cluster2 = want_dense || (!(e && !strcmp(e, "single")) && getenv("SB200_SCREEN_SINGLE") == nullptr);
-      tc.pair = want_dense || (tc.cluster2 && !(e && !strcmp(e, "multicast")));
     }
     mstep = tc.cluster2 ? 256 : 128;   // a cluster covers two 128-row candidate tiles
     if (want_dense) cstep = (256 / K) * K;   // column tiles end at block boundaries: a track's observations stay together
@@ -1142,8 +1141,8 @@ int sb200_tracker::predict(int32_t n_scenes, const uint64_t* scene_ids, const in
     }
   }
   const bool prep_ahead = prep_stream != nullptr && !derive_own && total > 0;
-  // (measured: keeping the tables on the work stream when the preparation runs ahead saves nothing -- 0.873 vs 0.875 ms -- and
-  // moves the next frame's preparation squarely under the screen kernel, 0.260 vs 0.248 ms; the side stream stays)
+  // (the tables go to the side stream: on the work stream they would move the next frame's preparation squarely under the
+  // screen kernel)
   const bool side_setup = side_ok && !derive_own && total > 0;
   cudaStream_t s_setup = stream;
   if (side_setup) {
@@ -1178,11 +1177,9 @@ int sb200_tracker::predict(int32_t n_scenes, const uint64_t* scene_ids, const in
       else { CU(cudaEventRecord(ev_inputs, stream)); CU(cudaStreamWaitEvent(prep_stream, ev_inputs, 0)); }
     }
     if (set_busy[cset]) CU(cudaStreamWaitEvent(prep_stream, ev_set_free[cset], 0));
-    // ... and not before the frame in front has left its cost kernels: the preparation is HBM traffic; under that frame's
-    // tensor-core screen it costs the screen 3-6 % (0.248-0.26 ms instead of 0.243), under its voting / apply / feature store it
-    // costs those ~40 us.  Measured at cfg5: 0.897 ms/step with the screen at 0.717 of the BF16 peak here, against 0.875-0.88
-    // ms/step with the screen at 0.67-0.70 for SB200_PREP_AFTER=none (as early as possible).  The default keeps the
-    // tensor-core kernel undisturbed and the step time reproducible; a deployment that only counts frames sets "none".
+    // ... and not before the frame in front has left its cost kernels: the preparation is HBM traffic that would slow that
+    // frame's tensor-core screen.  SB200_PREP_AFTER=none starts it as early as possible instead, which may shorten the step
+    // at the screen's expense.  The default keeps the tensor-core kernel undisturbed and the step time reproducible.
     static const bool after_cost = [] { const char* e = getenv("SB200_PREP_AFTER"); return !(e && !strcmp(e, "none")); }();
     if (after_cost && cost_done_valid) CU(cudaStreamWaitEvent(prep_stream, ev_cost_done, 0));
     sb::launch_prep(Pf, f, n_scenes, max_m, prep_stream);

@@ -526,11 +526,11 @@ static void pos_scan_impl(const Params& p, const TrackStore& ts, const Frame& f,
   while (Np < max_n) Np <<= 1;
   size_t smem = (size_t)Np * 8 + (size_t)max_n * 12 + (size_t)PS_QCAP * 8 + 64;
   // two CTAs fit an SM: with fewer scenes than that, several CTAs per scene (each at least 64 candidates)
-  int nsplit = std::max(1, std::min(std::min(16, (max_m + 63) / 64), (2 * 148) / std::max(1, n_scenes)));
+  int nsplit = std::max(1, std::min(std::min(16, (max_m + 63) / 64), (2 * kNumSms) / std::max(1, n_scenes)));
   dim3 grid(n_scenes, nsplit);
   // optional: the gated pairs of passes -1 / 0 go to one queue of the frame and pos_eval_kernel evaluates them
-  // (SB200_POS_GQ=1; measured slower on B200 -- cfg4 positional stage 0.142 vs 0.063 ms, cfg2 0.078 vs 0.070 -- the pairs of
-  // a scene evaluate faster next to the shared-memory copy of its tracks than spread over the device: kept for experiments)
+  // (SB200_POS_GQ=1, off by default: the pairs of a scene are expected to evaluate faster next to the shared-memory copy of its
+  // tracks than spread over the device; kept for experiments)
   const char* gq_env = getenv("SB200_POS_GQ");   // read per launch: the parity test switches it on inside a running process
   const bool gq_on = gq_env != nullptr && gq_env[0] == '1';
   const int use_gq = (gq_on && f.pos_gq != nullptr && lazy_pass != 1) ? 1 : 0;
@@ -539,12 +539,12 @@ static void pos_scan_impl(const Params& p, const TrackStore& ts, const Frame& f,
     cudaFuncSetAttribute(pos_scan_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     pos_scan_kernel<0><<<grid, PS_THREADS, smem, st>>>(p, ts, f, lazy_pass, use_gq);
     note_launch();
-    if (use_gq) { pos_eval_kernel<0><<<148 * 8, 256, 0, st>>>(p, ts, f, wdense, wlist); note_launch(); }
+    if (use_gq) { pos_eval_kernel<0><<<kNumSms * 8, 256, 0, st>>>(p, ts, f, wdense, wlist); note_launch(); }
   } else {
     cudaFuncSetAttribute(pos_scan_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     pos_scan_kernel<1><<<grid, PS_THREADS, smem, st>>>(p, ts, f, lazy_pass, use_gq);
     note_launch();
-    if (use_gq) { pos_eval_kernel<1><<<148 * 8, 256, 0, st>>>(p, ts, f, wdense, wlist); note_launch(); }
+    if (use_gq) { pos_eval_kernel<1><<<kNumSms * 8, 256, 0, st>>>(p, ts, f, wdense, wlist); note_launch(); }
   }
 }
 
@@ -753,7 +753,7 @@ int launch_vis_cost_b(const Params& p, const TrackStore& ts, const Frame& f, int
     // a scene in dense mode is recomputed whole by the exact kernel (whatever the refinement did for it before)
     const int tx = (max_n * p.max_obs + VN - 1) / VN, ty = (max_m + VM - 1) / VM;
     const long long want = (long long)tx * ty * (use_tc ? 1 : n_scenes);
-    const int grid = (int)std::min<long long>(want, 148 * 8);
+    const int grid = (int)std::min<long long>(want, kNumSms * 8);
     vis_cost_kernel<<<grid, VT, 0, st>>>(p, ts, f, n_scenes, tx, ty);
     note_launch();
     launch_scene_max(p, f, n_scenes, /*init_only=*/false, st);

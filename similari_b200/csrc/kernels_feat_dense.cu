@@ -8,7 +8,7 @@
 // every (candidate q, track t) group the weight W(q,t) = sum_k (max_dist - d(q,t,k)), a candidate's decision is its row
 // maximum and it wins that track iff it is also the column maximum (kernels_assign.cu).  So:
 //
-//   1. vis_wsum_kernel  : C~ = A B^T on the tensor cores (tcgen05 BF16, the same TMA / TMEM pipeline as the screen).  The
+//   1. vis_wsum_kernel  : C~ = A B^T on the tensor cores (wgmma BF16, the same TMA / mbarrier pipeline as the screen).  The
 //                         epilogue turns every accumulator into an approximate distance d~ with a rigorous error bound
 //                         (BF16 operand rounding, kScreenRelErr), sums the observations of a track -- the column tiles are
 //                         cut at track boundaries -- and stores {S~(q,t), bound} once per (candidate, track): 8 B per
@@ -46,9 +46,10 @@ namespace sb {
 constexpr float kDenseErrE = kScreenRelErr + 2e-4f;
 constexpr float kDenseErrC = kScreenRelErr + 2e-4f;
 
-constexpr int DS_STAGES = 6;
-constexpr int DS_STAGE_BYTES = 32768;   // A tile (128 x 64 bf16) + half of the B tile (128 x 64 bf16) per CTA of the pair
-constexpr int DS_THREADS = 320;         // TMA warp, MMA warp, 2 x 4 epilogue warps
+constexpr int DS_STAGES = 4;
+constexpr int DS_STAGE_BYTES = TC_A_BYTES + TC_B_BYTES;   // A tile (128 x 64 bf16) + B tile (256 x 64 bf16, half from each CTA)
+constexpr int DS_CH = 16;                                 // accumulator columns per epilogue chunk
+constexpr int DS_PITCH = DS_CH + 1;                       // +1: the row owners read column cc of 32 rows from 32 banks
 
 struct DsHdr {
   int scene, m0, m, det_base;
@@ -67,15 +68,14 @@ struct DsSmem {
   VisRowMeta rowm[4][TC_BM];
   unsigned int vmask[4][TC_BN / 32];
   unsigned int bmask[4][TC_BN / 32];
+  float dist[2][TC_WG_ROWS][DS_PITCH];   // per consumer warpgroup: one chunk of approximate distances, row-major
   DsHdr hdr[4];
   unsigned long long full_bar[DS_STAGES];
   unsigned long long empty_bar[DS_STAGES];
-  unsigned long long tmem_full[2];
-  unsigned long long tmem_empty[2];
   unsigned long long meta_full[4];
   unsigned long long meta_empty[4];
-  unsigned int tmem_base;
 };
+static_assert(sizeof(DsSmem) + 1024 <= 227 * 1024, "weight-sum kernel exceeds the shared memory of an SM");
 
 constexpr int kDenseKClasses = 5;   // observation counts the fused row bounds distinguish (templated kernels: K <= 5)
 constexpr float kHalfRel = 4.9e-4f; // 2^-11 (+): relative rounding error of a sum stored as fp16
@@ -102,8 +102,8 @@ struct DenseDev {   // device pointers of the path (TcArgs subset, passed by val
 };
 
 // ------------------------------------------------------------------------------------------------ weight-sum kernel
-// CTA pairs (cta_group::2): one 256 x 256 x 16 MMA per instruction issued by the leader, each CTA stages its own 128
-// candidate rows and half of the B tile; accumulator rows 0-127 / 128-255 in the two CTAs' TMEM; double-buffered accumulators.
+// Clusters of two CTAs: each CTA takes 128 candidate rows of the cluster's 256 and loads half of the shared B tile,
+// multicast into both CTAs' shared memory.  Two consumer warpgroups per CTA, 64 rows x 256 columns of accumulators each.
 // approximate MUFU operations (2 ulp), one instruction each: only upper bounds and the approximate distances use them
 __device__ __forceinline__ float rsqrt_approx(float x) { float r; asm("rsqrt.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x)); return r; }
 __device__ __forceinline__ float rcp_approx(float x) { float r; asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x)); return r; }
@@ -118,38 +118,11 @@ __device__ __noinline__ void dense_append_candidate(VisPair* maxc, int* maxc_cnt
   }
 }
 
-// (superseded by the per-element test above; kept for the any-K kernel)
-// Rare path of the weight-sum epilogue, one copy of code: some element of a 32-column chunk may be the scene's maximal
-// distance.  The whole warp re-reads the chunk from TMEM (the accumulator buffer is still owned by this warp's group) and
-// every lane appends its own candidates (feature row = row0 + column) for the exact pass.
-template <bool COSINE>
-__device__ __noinline__ void dense_max_candidates(uint32_t taddr_chunk, float rowc, const float* colc32, unsigned int vm, float T,
-                                                  int g, int row0, int scene, int lbase, int lcap, VisPair* maxc, int* maxc_cnt) {
-  uint32_t av[32];
-  tc_ld32(taddr_chunk, av);
-#pragma unroll
-  for (int jj = 0; jj < 32; ++jj) {
-    if (!((vm >> jj) & 1u)) continue;
-    const float a = __uint_as_float(av[jj]);
-    float key;
-    if (COSINE) key = __fsub_rn(1.0f, __fmul_rn(__fmul_rn(a, rowc), colc32[jj]));
-    else key = fmaxf(__fmaf_rn(-2.0f, a, __fadd_rn(rowc, colc32[jj])), 1e-30f);
-    if (key >= T) {
-      const int slot = atomicAdd(&maxc_cnt[scene], 1);
-      if (slot < lcap) {
-        VisPair vp;
-        vp.g = g; vp.row = row0 + jj; vp.scene = scene; vp.outcol = -1;
-        maxc[lbase + slot] = vp;
-      }
-    }
-  }
-}
-
 // KT > 0: the number of observations per track is a compile-time constant, so the positions where a block of the
 // accumulator ends (every KT-th column: tiles start at block boundaries) are too and the epilogue is straight-line code.
 // KT == 0: any K, block ends come from the bmask slab (uniform branches).
 template <bool COSINE, int KT>
-__global__ void __launch_bounds__(DS_THREADS, 1)
+__global__ void __launch_bounds__(TC_THREADS, 1)
 vis_wsum_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB, Params p, TrackStore ts,
                 Frame f, const TcTile* tiles, const int* n_tiles_dev, DenseDev dd) {
   extern __shared__ unsigned char smem_raw_[];
@@ -162,25 +135,19 @@ vis_wsum_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
   const int cta_first = (int)(blockIdx.x >> 1);
   const int cta_step = (int)(gridDim.x >> 1);
   unsigned char* const stage_base = &S.stage[0][0];
-  if (threadIdx.x == 32) {
-    for (int s = 0; s < DS_STAGES; ++s) { mbar_init(&S.full_bar[s], 1); mbar_init(&S.empty_bar[s], 1); }
-    for (int b = 0; b < 2; ++b) { mbar_init(&S.tmem_full[b], 1); mbar_init(&S.tmem_empty[b], 8); }
-    for (int b = 0; b < 4; ++b) { mbar_init(&S.meta_full[b], 1); mbar_init(&S.meta_empty[b], 4); }
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < DS_STAGES; ++s) { mbar_init(&S.full_bar[s], 1); mbar_init(&S.empty_bar[s], 4); }
+    for (int b = 0; b < 4; ++b) { mbar_init(&S.meta_full[b], 1); mbar_init(&S.meta_empty[b], 8); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&S.tmem_base)), "r"(512));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::);
-  }
-  tc_fence_before();
   __syncthreads();
   cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = S.tmem_base;
 
-  if (warp == 0) {
-    // ===================================================================== TMA producer
-    if (lane == 0) {
+  if (warp < 4) {
+    // ===================================================================== TMA producer (one thread); the warpgroup hands
+    // most of its registers to the consumers, whose accumulators alone take 128 per thread
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (warp == 0 && lane == 0) {
       asm volatile("prefetch.tensormap [%0];" ::"l"((uint64_t)&mapA) : "memory");
       asm volatile("prefetch.tensormap [%0];" ::"l"((uint64_t)&mapB) : "memory");
       int stage = 0;
@@ -214,67 +181,64 @@ vis_wsum_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
           bulk_load(S.bmask[g], dd.slab_bmask + slab * (TC_BN / 32), TC_BN / 8, &S.meta_full[g]);
         }
         for (int kb = 0; kb < KB; ++kb) {
-          mbar_wait(&S.empty_bar[stage], phase ^ 1);
+          mbar_wait(&S.empty_bar[stage], phase ^ 1);   // both CTAs have released the stage
           unsigned char* base = stage_base + stage * DS_STAGE_BYTES;
-          const uint32_t lbar = leader_addr(&S.full_bar[stage]);
-          if (crank == 0) mbar_expect_tx(&S.full_bar[stage], 2 * DS_STAGE_BYTES);
-          tma_load_2d_pair(base, &mapA, kb * TC_BK, rowA, lbar);
-          tma_load_2d_pair(base + TC_A_BYTES, &mapB, kb * TC_BK, rowB + (int)crank * (TC_BN / 2), lbar);
+          mbar_expect_tx(&S.full_bar[stage], DS_STAGE_BYTES);
+          tma_load_2d(base, &mapA, kb * TC_BK, rowA, &S.full_bar[stage]);
+          tma_load_2d_mc(base + TC_A_BYTES + crank * (TC_B_BYTES / 2), &mapB, kb * TC_BK, rowB + (int)crank * (TC_BN / 2),
+                         &S.full_bar[stage], (uint16_t)0x3);
           if (++stage == DS_STAGES) { stage = 0; phase ^= 1; }
         }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================================================================== MMA issuer (one elected lane of the leader CTA)
-    if (lane == 0 && crank == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      int it = 0;
-      for (int t = cta_first; t < n_tiles; t += cta_step, ++it) {
-        const int buf = it & 1;
-        mbar_wait(&S.tmem_empty[buf], ((it >> 1) & 1) ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(buf * TC_BN);
-        for (int kb = 0; kb < KB; ++kb) {
-          mbar_wait(&S.full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t a0 = smem_u32(stage_base + stage * DS_STAGE_BYTES);
-          const uint32_t b0 = a0 + TC_A_BYTES;
-#pragma unroll
-          for (int k = 0; k < TC_BK / 16; ++k) {
-            const uint32_t off = k * 32;
-            tc_mma_bf16_pair(d_tmem, umma_desc(a0 + off), umma_desc(b0 + off), kIdescBf16Pair, (kb | k) != 0 ? 1u : 0u);
-          }
-          tc_commit_pair_mc(&S.empty_bar[stage], (uint16_t)0x3);
-          if (++stage == DS_STAGES) { stage = 0; phase ^= 1; }
-        }
-        tc_commit_pair_mc(&S.tmem_full[buf], (uint16_t)0x3);
       }
     }
   } else {
-    // ===================================================================== epilogue warps 2..9 (two groups of four)
-    const int q = warp & 3;
-    const int grp = (warp - 2) >> 2;
-    const int r = q * 32 + lane;
+    // ===================================================================== consumer warpgroups 1 and 2
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    // Per 16-column chunk: every thread turns its accumulators (wgmma layout: register i is row er[(i >> 1) & 1], column
+    // 8 * (i >> 2) + 2 * (lane & 3) + (i & 1)) into approximate distances in place and parks them in S.dist; then the
+    // warpgroup's first two warps, one thread per row, add them up block by block in column order.
+    const int wg = (warp >> 2) - 1;
+    const int wtid = threadIdx.x & 127;
+    const bool owner = wtid < TC_WG_ROWS;   // warp-uniform
+    const int er[2] = {(warp & 3) * 16 + (lane >> 2), (warp & 3) * 16 + (lane >> 2) + 8};   // rows inside the warpgroup
+    const int q2 = 2 * (lane & 3);
     const float finf = __int_as_float(0x7f800000);
-    int it = grp;
-    for (int t = cta_first + grp * cta_step; t < n_tiles; t += 2 * cta_step, it += 2) {
-      const int buf = grp;
+    float (*dist)[DS_PITCH] = S.dist[wg];
+    int stage = 0;
+    uint32_t phase = 0;
+    int it = 0;
+    for (int t = cta_first; t < n_tiles; t += cta_step, ++it) {
+      float acc[128];
+      tc_consume_tile<2, DS_STAGES, DS_STAGE_BYTES>(acc, stage_base, S.full_bar, S.empty_bar, KB, wg, stage, phase);
       const int ms = it & 3;
       mbar_wait(&S.meta_full[ms], (it >> 2) & 1);
       const DsHdr h = S.hdr[ms];
-      const VisRowMeta rm = S.rowm[ms][r];
-      const int m = h.m0 + r;
-      const bool row_ok = m < h.m && rm.ok;
-      const int g = h.det_base + m;
-      const float rowc = rm.rowk;   // |a|^2 (euclidean) or 1 / |a| (cosine)
-      // an element can be the scene's maximal distance only above the sampled lower bound minus the error bound
-      float T = COSINE ? h.l0 - kDenseErrC : h.l0 - kDenseErrE * (rowc + h.scmax);
-      if (!row_ok) T = finf;
-      __half2* wsp = dd.ws + h.ws_base + m;
       const float* gcolc = S.colc[ms];
       const float* gcmax = S.cmax[ms];
       const float* gktf = S.ktf[ms];
+      // element view: the two rows of this thread's accumulators
+      float erowc[2], eTd[2];
+      int eg[2];
+#pragma unroll
+      for (int hr = 0; hr < 2; ++hr) {
+        const int r = wg * TC_WG_ROWS + er[hr];
+        const VisRowMeta rm = S.rowm[ms][r];
+        const int m = h.m0 + r;
+        erowc[hr] = rm.rowk;   // |a|^2 (euclidean) or 1 / |a| (cosine)
+        eg[hr] = h.det_base + m;
+        // an element can be the scene's maximal distance only above the sampled lower bound minus the error bound
+        float T = COSINE ? h.l0 - kDenseErrC : h.l0 - kDenseErrE * (erowc[hr] + h.scmax);
+        if (!(m < h.m && rm.ok)) T = finf;
+        eTd[hr] = COSINE ? T : (T > 0.0f ? T * rsqrt_approx(T) * (1.0f - 1e-6f) : -1.0f);   // sqrt(T), a hair low
+      }
+      // row view (owners): the row this thread sums
+      const int rrow = wg * TC_WG_ROWS + (wtid & (TC_WG_ROWS - 1));
+      const VisRowMeta rm = S.rowm[ms][rrow];
+      const int m = h.m0 + rrow;
+      const bool row_ok = m < h.m && rm.ok;
+      const int g = h.det_base + m;
+      const float rowc = rm.rowk;
+      __half2* wsp = dd.ws + h.ws_base + m;
       float s_acc = 0.0f, dmin = finf;
       // fused "pass A" of the selection (templated kernels): best lower bound of the maxd-independent part of the weight,
       // -(S + k del), per observation count for this row, per block over the rows (warp maximum + one atomic)
@@ -283,11 +247,6 @@ vis_wsum_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
 #pragma unroll
       for (int kc = 0; kc < kDenseKClasses; ++kc) lrow[kc] = -finf;
       int bidx = h.blk0;
-      mbar_wait(&S.tmem_full[buf], (it >> 1) & 1);
-      tc_fence_after();
-      uint32_t acc[2][32];
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(buf * TC_BN);
-      tc_ld32_issue(taddr, acc[0]);
       // one flush per block: {sum of the block's distances, per-observation error bound}
       auto flush = [&](int col) {
         const float cmx = gcmax[col];
@@ -296,9 +255,6 @@ vis_wsum_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
         else {
           const float rc = rowc + cmx;
           const float e = kDenseErrE * rc;
-          // |d - d~| <= e / (d + d~) <= 0.536 e / d~ once d~^2 >= 4 e; both d, d~ <= sqrt(5 e) otherwise.  Only an upper
-          // bound is needed: approximate reciprocal / rsqrt (2 ulp) under a 1.0001 safety factor, and 1e-6 (rc + 1) >=
-          // 1e-6 sqrt(rc) for the rsqrt approximation of d~ itself.
           // |d - d~| <= |d^2 - d~^2| / (d + d~) <= e / d~ always, <= 0.536 e / d~ once d~^2 >= 4 e (then d >= 0.866 d~),
           // and <= sqrt(e) always.  Approximate reciprocal / rsqrt (2 ulp) under a 1.0001 safety factor; 1e-6 (rc + 1) >=
           // 1e-6 sqrt(rc) covers the rsqrt approximation of d~ itself.
@@ -321,54 +277,49 @@ vis_wsum_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
         ++bidx;
         s_acc = 0.0f; dmin = finf;
       };
-      // distances of one 32-column chunk in place; an element that can be the scene's maximal distance (approximate distance
-      // above the bound Td, valid column) is appended to the candidate list on the spot
-      const float Td = COSINE ? T : (T > 0.0f ? T * rsqrt_approx(T) * (1.0f - 1e-6f) : -1.0f);   // sqrt(T), a hair low
-      auto distances = [&](uint32_t* av, int ch, unsigned int vm) {
-        unsigned int cmask = 0u;
+      // distances of one chunk in place (accumulator groups j = 2 ch, 2 ch + 1); an element that can be the scene's maximal
+      // distance (approximate distance above the bound Td, valid column) is appended to the candidate list on the spot;
+      // then the chunk goes to S.dist
+      auto distances = [&](int ch, unsigned int vm) {
 #pragma unroll
-        for (int jj = 0; jj < 32; jj += 4) {
-          const float4 c4 = *reinterpret_cast<const float4*>(gcolc + ch * 32 + jj);
-          const float cc[4] = {c4.x, c4.y, c4.z, c4.w};
+        for (int jj = 0; jj < 2; ++jj) {
+          const int j = 2 * ch + jj;
+          const int cc = 8 * jj + q2;   // column inside the chunk
+          const float2 c2 = *reinterpret_cast<const float2*>(gcolc + 8 * j + q2);
 #pragma unroll
-          for (int u = 0; u < 4; ++u) {
-            const float a = __uint_as_float(av[jj + u]);
+          for (int e = 0; e < 4; ++e) {
+            const int hr = e >> 1, cl = e & 1;
+            const float a = acc[4 * j + e];
+            const float cv = cl ? c2.y : c2.x;
             float dval;
-            if (COSINE) dval = __fsub_rn(1.0f, __fmul_rn(__fmul_rn(a, rowc), cc[u]));
+            if (COSINE) dval = __fsub_rn(1.0f, __fmul_rn(__fmul_rn(a, erowc[hr]), cv));
             else {
-              float x = __fmaf_rn(-2.0f, a, __fadd_rn(rowc, cc[u]));
+              float x = __fmaf_rn(-2.0f, a, __fadd_rn(erowc[hr], cv));
               x = fmaxf(x, 1e-30f);
               dval = __fmul_rn(x, rsqrt_approx(x));
             }
-            if (dval >= Td) cmask |= 1u << (jj + u);
-            av[jj + u] = __float_as_uint(dval);
+            // about one element in a thousand
+            if (dval >= eTd[hr] && ((vm >> (cc + cl)) & 1u) && !(dd.dbg & 2))
+              dense_append_candidate(dd.maxc, dd.maxc_cnt, h.scene, h.vis_lbase, h.vis_lcap, eg[hr], h.rowB + 8 * j + q2 + cl);
+            dist[er[hr]][cc + cl] = dval;
           }
-        }
-        cmask &= vm;
-        if (dd.dbg & 2) cmask = 0u;
-        while (cmask) {   // about one element in a thousand
-          const int jj = __ffs(cmask) - 1;
-          cmask &= cmask - 1;
-          dense_append_candidate(dd.maxc, dd.maxc_cnt, h.scene, h.vis_lbase, h.vis_lcap, g, h.rowB + ch * 32 + jj);
         }
       };
       if (KT > 0) {
         constexpr int KC = KT > 0 ? KT : 1;
         constexpr int CSTEP = (TC_BN / KC) * KC;   // columns of the tile that belong to whole blocks
 #pragma unroll
-        for (int ch = 0; ch < TC_BN / 32; ++ch) {
-          uint32_t* av = acc[ch & 1];
-          tc_ld_wait32(av);
-          if (ch + 1 < TC_BN / 32) tc_ld32_issue(taddr + (ch + 1) * 32, acc[(ch + 1) & 1]);
-          const unsigned int vm = S.vmask[ms][ch];
-          distances(av, ch, vm);
-          if (!(dd.dbg & 4)) {
+        for (int ch = 0; ch < TC_BN / DS_CH; ++ch) {
+          const unsigned int vm = (S.vmask[ms][ch >> 1] >> ((ch & 1) * DS_CH)) & 0xffffu;
+          distances(ch, vm);
+          wg_bar(1 + wg);
+          if (owner && !(dd.dbg & 4)) {
 #pragma unroll
-            for (int jj = 0; jj < 32; ++jj) {
-              const int col = ch * 32 + jj;
+            for (int cc = 0; cc < DS_CH; ++cc) {
+              const int col = ch * DS_CH + cc;
               if (col < CSTEP) {   // compile time
-                const bool valid = (vm >> jj) & 1u;
-                const float dval = __uint_as_float(av[jj]);
+                const bool valid = (vm >> cc) & 1u;
+                const float dval = dist[wtid][cc];
                 s_acc = __fadd_rn(s_acc, valid ? dval : 0.0f);
                 dmin = fminf(dmin, valid ? dval : finf);
                 // compile-time position: last physical slot of a block (the per-scene arrays are padded to whole tiles, so a
@@ -377,52 +328,40 @@ vis_wsum_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
               }
             }
           }
+          wg_bar(1 + wg);   // S.dist may be overwritten
         }
       } else {
-#pragma unroll 1
-        for (int ch2 = 0; ch2 < TC_BN / 32; ch2 += 2) {
 #pragma unroll
-          for (int par = 0; par < 2; ++par) {
-            const int ch = ch2 + par;
-            tc_ld_wait32(acc[par]);
-            if (ch + 1 < TC_BN / 32) tc_ld32_issue(taddr + (ch + 1) * 32, acc[par ^ 1]);
-            const unsigned int vm = S.vmask[ms][ch], bm = S.bmask[ms][ch];
-            if ((vm | bm) != 0u) {   // warp-uniform, like every test on vm / bm below: column properties
-              distances(acc[par], ch, vm);
-              if (!(dd.dbg & 4)) {
+        for (int ch = 0; ch < TC_BN / DS_CH; ++ch) {   // unrolled: the accumulators are indexed at compile time
+          const unsigned int vm = (S.vmask[ms][ch >> 1] >> ((ch & 1) * DS_CH)) & 0xffffu;
+          const unsigned int bm = (S.bmask[ms][ch >> 1] >> ((ch & 1) * DS_CH)) & 0xffffu;
+          if ((vm | bm) == 0u) continue;   // uniform over the warpgroup, like every test on vm / bm below: column properties
+          distances(ch, vm);
+          wg_bar(1 + wg);
+          if (owner && !(dd.dbg & 4)) {
 #pragma unroll
-                for (int jj = 0; jj < 32; ++jj) {
-                  const bool valid = (vm >> jj) & 1u;
-                  const float dval = __uint_as_float(acc[par][jj]);
-                  s_acc = __fadd_rn(s_acc, valid ? dval : 0.0f);
-                  dmin = fminf(dmin, valid ? dval : finf);
-                  if (bm & (1u << jj)) flush(ch * 32 + jj);
-                }
-              }
+            for (int cc = 0; cc < DS_CH; ++cc) {
+              const bool valid = (vm >> cc) & 1u;
+              const float dval = dist[wtid][cc];
+              s_acc = __fadd_rn(s_acc, valid ? dval : 0.0f);
+              dmin = fminf(dmin, valid ? dval : finf);
+              if (bm & (1u << cc)) flush(ch * DS_CH + cc);
             }
           }
+          wg_bar(1 + wg);
         }
       }
-      tc_fence_before();
       __syncwarp();
-      if (lane == 0) {
-        mbar_arrive_cluster(leader_addr(&S.tmem_empty[buf]));
-        mbar_arrive(&S.meta_empty[ms]);
-      }
-      if (FUSED && row_ok) {
+      if (lane == 0) mbar_arrive(&S.meta_empty[ms]);
+      if (FUSED && owner && row_ok) {
 #pragma unroll
         for (int kc = 0; kc < (KT > 0 ? KT : 1); ++kc)
           if (lrow[kc] > -finf) atomicMax(&dd.rowb[(size_t)g * kDenseKClasses + kc], enc_ord(lrow[kc]));
       }
     }
   }
-  tc_fence_before();
   __syncthreads();
-  cluster_sync_all();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512));
-  }
+  cluster_sync_all();   // no CTA leaves while its peer may still multicast into / arrive on its smem
 }
 
 // ------------------------------------------------------------------------------------------------ per-frame metadata
@@ -766,7 +705,7 @@ int launch_vis_dense(const Params& p, const TrackStore& ts, const Frame& f, int 
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
     cfg.gridDim = dim3(ncta);
-    cfg.blockDim = dim3(DS_THREADS);
+    cfg.blockDim = dim3(TC_THREADS);
     cfg.dynamicSmemBytes = smem;
     cfg.stream = st;
     cudaLaunchAttribute attr[1];

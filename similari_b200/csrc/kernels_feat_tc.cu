@@ -1,4 +1,4 @@
-// kernels_feat_tc.cu -- visual (ReID feature) cost matrix: tensor-core screen (tcgen05.mma + TMEM + TMA) followed by
+// kernels_feat_tc.cu -- visual (ReID feature) cost matrix: tensor-core screen (wgmma + TMA + mbarrier) followed by
 // an exact f32 refinement of the surviving pairs.
 //
 // What the reference computes (src/distance.rs:9-47, src/trackers/visual_sort/metric.rs:200-295): for every
@@ -7,21 +7,21 @@
 // handful of observations of "its" track and far from everything else.
 //
 // GPU shape:
-//   1. screen  : C~[m][c] = sum_d A[m][d] * B[c][d] with BF16 operand copies on the 5th-gen tensor cores
-//                (one tcgen05.mma.kind::f16 chain, fp32 accumulation in TMEM).  The BF16 rounding error of the dot
-//                product is bounded by E = 2^-8 * ||a|| * ||b|| (Cauchy-Schwarz), so a pair can only pass the
-//                threshold if its screened value is within E of it.  Everything else is written as None (NaN)
-//                straight from the epilogue; survivors are appended to a compact pair list.
+//   1. screen  : C~[m][c] = sum_d A[m][d] * B[c][d] with BF16 operand copies on the tensor cores (wgmma m64n256k16,
+//                fp32 accumulation in registers).  The BF16 rounding error of the dot product is bounded by
+//                E = 2^-8 * ||a|| * ||b|| (Cauchy-Schwarz), so a pair can only pass the threshold if its screened value is
+//                within E of it.  Everything else is written as None (NaN) straight from the epilogue; survivors are
+//                appended to a compact pair list.
 //   2. refine  : one warp per surviving pair recomputes the distance in f32 in the reference's exact summation order
 //                (8-lane blocks, horizontal reduce_add, sequential block accumulation) and applies is_ok /
 //                distance_to_weight.  Every value that reaches the voting stage is therefore bit-identical to the
 //                CPU reference -- the tensor cores only decide which pairs are worth computing.
 //   If the pair list overflows (a non-selective threshold) the caller falls back to the dense exact SIMT kernel.
 //
-// Screen kernel: persistent CTAs (one per SM), 192 threads = TMA producer warp, MMA issuer warp, 4 epilogue warps.
-// Tile 128 (candidates) x 256 (track-observation rows) x 64 (features = one 128-byte swizzle atom of bf16);
-// 4 smem stages of 48 KB; the 512 TMEM columns hold two 128x256 fp32 accumulators so the epilogue of tile i overlaps
-// the MMAs of tile i+1.
+// Screen kernel: persistent CTAs (one per SM), 384 threads = a producer warpgroup (one TMA warp) and two consumer
+// warpgroups.  Tile 128 (candidates) x 256 (track-observation rows) x 64 (features = one 128-byte swizzle atom of bf16);
+// 4 smem stages of 48 KB, so the loads of the next tile run while the consumers screen this one.  Each consumer
+// warpgroup accumulates 64 candidate rows x 256 columns in registers and screens them in place.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -37,38 +37,28 @@
 namespace sb {
 
 constexpr int TC_STAGES = 4;          // 48 KB stages (A tile + whole B tile)
-constexpr int TC_STAGES_PAIR = 6;     // 32 KB stages of the cta_group::2 variant (A tile + half of the B tile)
-constexpr int TC_STAGE_BYTES_PAIR = 32768;
 constexpr int TC_STAGE_BYTES = TC_A_BYTES + TC_B_BYTES;  // 48 KB
-constexpr int TC_THREADS = 320;  // TMA warp, MMA warp, 2 x 4 epilogue warps (the two groups alternate tiles)
 
 struct TcHdr { int scene, m0, ncols_left, m, det_base, col0, epoch, vis_lbase, vis_lcap, pad; };
 struct TcSmem {
   unsigned char stage[TC_STAGES][TC_STAGE_BYTES];  // 1024-byte aligned operand stages first
-  // per epilogue group: the metadata slabs of its current tile, bulk-copied by the producer warp
-  // four slab sets (two per group): the producer runs up to two tile pairs ahead of the epilogue
+  // four slab sets of per-tile metadata, bulk-copied by the producer warp: it runs up to three tiles ahead
   VisColMeta meta[4][TC_BN];
   VisRowMeta rowm[4][TC_BM];
   float colb[4][TC_BN];
   unsigned int colvalid[4][TC_BN / 32];
   TcHdr hdr[4];
-  unsigned long long full_bar[TC_STAGES_PAIR];
-  unsigned long long empty_bar[TC_STAGES_PAIR];
-  unsigned long long tmem_full[2];
-  unsigned long long tmem_empty[2];
+  unsigned long long full_bar[TC_STAGES];
+  unsigned long long empty_bar[TC_STAGES];
   unsigned long long meta_full[4];
   unsigned long long meta_empty[4];
-  unsigned int tmem_base;
 };
+static_assert(sizeof(TcSmem) + 1024 <= 227 * 1024, "screen kernel exceeds the shared memory of an SM");
 
 
 // ------------------------------------------------------------------------------------------------ screen kernel
 // CL == 2: clusters of two CTAs work on two candidate tiles (m0, m0 + 128) of the same track-row tile; each CTA loads
 // its own A tile and HALF of the B tile, multicast into both CTAs' shared memory, so B crosses L2 -> SM once per pair.
-// CL == 3: the two CTAs form a cta_group::2 pair: one 256 x 256 x 16 MMA per instruction, issued by the leader CTA only.
-// Each CTA stages its own A tile and HALF of the B tile (no multicast: the tensor cores read the peer's half), which
-// halves the shared-memory bytes written and read per MMA -- with 128 x 256 single-CTA tiles every operand byte is
-// written once by TMA and read once by the MMA, 192 B/clk against the 128 B/clk an SM's shared memory delivers.
 template <int CL, bool COSINE>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 vis_screen_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB, Params p,
@@ -84,40 +74,24 @@ vis_screen_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
   const int K = p.max_obs;
   const int KB = (p.d8 + TC_BK - 1) / TC_BK;
 
-  constexpr bool PAIR = CL == 3;
-  constexpr int NST = PAIR ? TC_STAGES_PAIR : TC_STAGES;
-  constexpr int STAGE_B = PAIR ? TC_STAGE_BYTES_PAIR : TC_STAGE_BYTES;
-  unsigned char* const stage_base = &S.stage[0][0];   // NST stages of STAGE_B bytes (192 KB either way)
+  unsigned char* const stage_base = &S.stage[0][0];
   const uint32_t crank = CL >= 2 ? cluster_rank() : 0u;
   const int cta_first = CL >= 2 ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;   // first (cluster) tile of this CTA
   const int cta_step = CL >= 2 ? (int)(gridDim.x >> 1) : (int)gridDim.x;
-  if (threadIdx.x == 32) {
-    for (int s = 0; s < NST; ++s) { mbar_init(&S.full_bar[s], 1); mbar_init(&S.empty_bar[s], CL == 2 ? 2 : 1); }
-    for (int b = 0; b < 2; ++b) {
-      // PAIR: the leader's tmem_empty collects the epilogue warps of both CTAs
-      mbar_init(&S.tmem_full[b], 1); mbar_init(&S.tmem_empty[b], PAIR ? 8 : 4);
-    }
-    for (int b = 0; b < 4; ++b) { mbar_init(&S.meta_full[b], 1); mbar_init(&S.meta_empty[b], 4); }
+  if (threadIdx.x == 0) {
+    // empty: one arrival per consumer warpgroup of every CTA that reads the stage's bytes; meta_empty: the 8 consumer warps
+    for (int s = 0; s < TC_STAGES; ++s) { mbar_init(&S.full_bar[s], 1); mbar_init(&S.empty_bar[s], 2 * CL); }
+    for (int b = 0; b < 4; ++b) { mbar_init(&S.meta_full[b], 1); mbar_init(&S.meta_empty[b], 8); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    if (PAIR) {   // both CTAs of the pair allocate, same warp, same destination
-      asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&S.tmem_base)), "r"(512));
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::);
-    } else {
-      asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&S.tmem_base)), "r"(512));
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-    }
-  }
-  tc_fence_before();
   __syncthreads();
   if (CL >= 2) cluster_sync_all();   // the peer's barriers are initialised before anything is multicast into them
-  tc_fence_after();
-  const uint32_t tmem_base = S.tmem_base;
 
-  if (warp == 0) {
-    // ===================================================================== TMA producer
-    if (lane == 0) {
+  if (warp < 4) {
+    // ===================================================================== TMA producer (one thread); the warpgroup hands
+    // most of its registers to the consumers, whose accumulators alone take 128 per thread
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (warp == 0 && lane == 0) {
       asm volatile("prefetch.tensormap [%0];" ::"l"((uint64_t)&mapA) : "memory");
       asm volatile("prefetch.tensormap [%0];" ::"l"((uint64_t)&mapB) : "memory");
       int stage = 0;
@@ -135,9 +109,9 @@ vis_screen_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
         const int rowA = sc.det_base + m0;
         const int rowB = sc.slot * ts.track_cap * K + tl.c0;
         {
-          // metadata of this tile for the epilogue group that will drain it: header by plain stores (published by the
-          // release of the arrive below), column / row slabs by bulk copies that complete on the same barrier
-          const int g = it & 3;   // slab set: tile parity picks the group, bit 1 alternates the group's two sets
+          // metadata of this tile: header by plain stores (published by the release of the arrive below), column / row
+          // slabs by bulk copies that complete on the same barrier
+          const int g = it & 3;
           mbar_wait(&S.meta_empty[g], ((it >> 2) & 1) ^ 1);
           TcHdr h;
           h.scene = tl.scene; h.m0 = m0; h.ncols_left = sc.nb * K - tl.c0; h.m = sc.m; h.det_base = sc.det_base;
@@ -152,139 +126,96 @@ vis_screen_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
         }
         for (int kb = 0; kb < KB; ++kb) {
           mbar_wait(&S.empty_bar[stage], phase ^ 1);   // CL == 2: both CTAs have released the stage
-          unsigned char* base = stage_base + stage * STAGE_B;
-          if (PAIR) {
-            // both CTAs' bytes are counted on the leader's barrier, which the leader arms for the whole pair
-            const uint32_t lbar = leader_addr(&S.full_bar[stage]);
-            if (crank == 0) mbar_expect_tx(&S.full_bar[stage], 2 * TC_STAGE_BYTES_PAIR);
-            tma_load_2d_pair(base, &mapA, kb * TC_BK, rowA, lbar);
-            tma_load_2d_pair(base + TC_A_BYTES, &mapB, kb * TC_BK, rowB + (int)crank * (TC_BN / 2), lbar);
+          unsigned char* base = stage_base + stage * TC_STAGE_BYTES;
+          mbar_expect_tx(&S.full_bar[stage], TC_STAGE_BYTES);
+          tma_load_2d(base, &mapA, kb * TC_BK, rowA, &S.full_bar[stage]);
+          if (CL == 2) {
+            // this CTA's half of the B tile (rows rank*128 .. +128), delivered to both CTAs
+            tma_load_2d_mc(base + TC_A_BYTES + crank * (TC_B_BYTES / 2), &mapB, kb * TC_BK, rowB + (int)crank * (TC_BN / 2),
+                           &S.full_bar[stage], (uint16_t)0x3);
           } else {
-            mbar_expect_tx(&S.full_bar[stage], TC_STAGE_BYTES);
-            tma_load_2d(base, &mapA, kb * TC_BK, rowA, &S.full_bar[stage]);
-            if (CL == 2) {
-              // this CTA's half of the B tile (rows rank*128 .. +128), delivered to both CTAs
-              tma_load_2d_mc(base + TC_A_BYTES + crank * (TC_B_BYTES / 2), &mapB, kb * TC_BK, rowB + (int)crank * (TC_BN / 2),
-                             &S.full_bar[stage], (uint16_t)0x3);
-            } else {
-              tma_load_2d(base + TC_A_BYTES, &mapB, kb * TC_BK, rowB, &S.full_bar[stage]);
-            }
+            tma_load_2d(base + TC_A_BYTES, &mapB, kb * TC_BK, rowB, &S.full_bar[stage]);
           }
-          if (++stage == NST) { stage = 0; phase ^= 1; }
+          if (++stage == TC_STAGES) { stage = 0; phase ^= 1; }
         }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================================================================== MMA issuer (one elected lane; PAIR: leader CTA)
-    if (lane == 0 && (!PAIR || crank == 0)) {
-      int stage = 0;
-      uint32_t phase = 0;
-      int it = 0;
-      for (int t = cta_first; t < n_tiles; t += cta_step, ++it) {
-        const int buf = it & 1;
-        mbar_wait(&S.tmem_empty[buf], ((it >> 1) & 1) ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(buf * TC_BN);
-        for (int kb = 0; kb < KB; ++kb) {
-          mbar_wait(&S.full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t a0 = smem_u32(stage_base + stage * STAGE_B);
-          const uint32_t b0 = a0 + TC_A_BYTES;
-#pragma unroll
-          for (int k = 0; k < TC_BK / 16; ++k) {
-            const uint32_t off = k * 32;  // 16 bf16 = 32 bytes inside the 128-byte swizzle atom
-            if (PAIR) tc_mma_bf16_pair(d_tmem, umma_desc(a0 + off), umma_desc(b0 + off), kIdescBf16Pair, (kb | k) != 0 ? 1u : 0u);
-            else tc_mma_bf16(d_tmem, umma_desc(a0 + off), umma_desc(b0 + off), kIdescBf16, (kb | k) != 0 ? 1u : 0u);
-          }
-          // frees the smem stage once the MMAs above retire, in both CTAs when they share the stage's data
-          if (PAIR) tc_commit_pair_mc(&S.empty_bar[stage], (uint16_t)0x3);
-          else if (CL == 2) tc_commit_mc(&S.empty_bar[stage], (uint16_t)0x3);
-          else tc_commit(&S.empty_bar[stage]);
-          if (++stage == NST) { stage = 0; phase ^= 1; }
-        }
-        if (PAIR) tc_commit_pair_mc(&S.tmem_full[buf], (uint16_t)0x3);   // both CTAs' epilogues drain their half
-        else tc_commit(&S.tmem_full[buf]);
       }
     }
   } else {
-    // ===================================================================== epilogue warps 2..9
-    // Two groups of four warps; group g drains accumulator buffer g, i.e. the tiles with (iteration & 1) == g, so each
-    // group has two tile-times per tile.  All per-tile metadata arrives in shared memory through the producer warp's
-    // bulk copies: the epilogue issues no global load between the TMEM drain and the survivor append.
-    const int q = warp & 3;           // TMEM lane quarter this warp may read
-    const int grp = (warp - 2) >> 2;  // 0 or 1
+    // ===================================================================== consumer warpgroups 1 and 2
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    // Warpgroup wg owns candidate rows wg*64 .. +64 of every tile.  Thread layout of the accumulators (wgmma): register i
+    // holds row rr[(i >> 1) & 1] and column 8 * (i >> 2) + 2 * (lane & 3) + (i & 1).  All per-tile metadata arrives in
+    // shared memory through the producer warp's bulk copies: the epilogue issues no global load on its common path.
+    const int wg = (warp >> 2) - 1;
+    const int rr[2] = {wg * TC_WG_ROWS + (warp & 3) * 16 + (lane >> 2), wg * TC_WG_ROWS + (warp & 3) * 16 + (lane >> 2) + 8};
+    const int q2 = 2 * (lane & 3);
     const bool geo = p.n_constraints > 0;
-    const int r = q * 32 + lane;      // accumulator row (candidate) of this thread
-    int it = grp;
-    for (int t = cta_first + grp * cta_step; t < n_tiles; t += 2 * cta_step, it += 2) {
-      const int buf = grp;
+    int stage = 0;
+    uint32_t phase = 0;
+    int it = 0;
+    for (int t = cta_first; t < n_tiles; t += cta_step, ++it) {
+      float acc[128];
+      tc_consume_tile<CL, TC_STAGES, TC_STAGE_BYTES>(acc, stage_base, S.full_bar, S.empty_bar, KB, wg, stage, phase);
       const int ms = it & 3;   // slab set of this tile (same rule as the producer)
       mbar_wait(&S.meta_full[ms], (it >> 2) & 1);
       const VisColMeta* gmeta = S.meta[ms];
       const TcHdr h = S.hdr[ms];
-      const VisRowMeta rm = S.rowm[ms][r];
-      const int m = h.m0 + r;
-      const bool row_ok = m < h.m && rm.ok;
-      const int g = h.det_base + m;
-      float cx = 0.0f, cy = 0.0f, cr = 0.0f;
-      if (geo && row_ok) { cx = f.c_box[(size_t)g * 6]; cy = f.c_box[(size_t)g * 6 + 1]; cr = f.c_radius[g]; }
+      const float* gcolb = S.colb[ms];
       // Screen test, E = kScreenRelErr bounds the BF16 operand rounding (|dot~ - dot| <= E |a||b| <= E (|a|^2 + |b|^2) / 2):
       //   cosine: cos >= thr possible   <=>  dot~ >= (thr - 1e-5 - E) |a| * |b|                                = rowk * colb
       //   euclid: d^2 <= thr^2 possible <=>  dot~ >= 0.5 ((1 - 1e-5 - E)(|a|^2 + |b|^2) - thr^2 (1 + 1e-5))   = rowk + colb
-      const float rowk = rm.rowk;
-      const float* gcolb = S.colb[ms];
-      mbar_wait(&S.tmem_full[buf], (it >> 1) & 1);
-      tc_fence_after();
-      // ---- phase A: drain the accumulator into per-thread survivor masks, then hand the TMEM buffer back at once
-      unsigned int keep[TC_BN / 32];
-      uint32_t acc[2][32];
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(buf * TC_BN);
-      const int nch = min(TC_BN / 32, (h.ncols_left + 31) / 32);   // chunks that hold tracks of this scene
-      tc_ld32_issue(taddr, acc[0]);
+      float rowk[2];
+      bool row_ok[2];
+      int g[2];
 #pragma unroll
-      for (int ch = 0; ch < TC_BN / 32; ++ch) {
-        keep[ch] = 0;
-        if (ch < nch) {  // warp-uniform
-          tc_ld_wait32(acc[ch & 1]);                                     // chunk ch has landed
-          if (ch + 1 < nch) tc_ld32_issue(taddr + (ch + 1) * 32, acc[(ch + 1) & 1]);   // in flight while ch is screened
-          unsigned int kb = 0;  // bit jj: pair (row, column ch*32+jj) survives the screen
+      for (int hr = 0; hr < 2; ++hr) {
+        const VisRowMeta rm = S.rowm[ms][rr[hr]];
+        const int m = h.m0 + rr[hr];
+        row_ok[hr] = m < h.m && rm.ok;
+        g[hr] = h.det_base + m;
+        rowk[hr] = rm.rowk;
+      }
+      // bit i of keep[i >> 5]: the pair of accumulator register i survives the screen
+      unsigned int keep[4] = {0u, 0u, 0u, 0u};
 #pragma unroll
-          for (int jj = 0; jj < 32; jj += 4) {
-            const float4 cb = *reinterpret_cast<const float4*>(gcolb + ch * 32 + jj);
-            const float b0 = COSINE ? rowk * cb.x : rowk + cb.x, b1 = COSINE ? rowk * cb.y : rowk + cb.y;
-            const float b2 = COSINE ? rowk * cb.z : rowk + cb.z, b3 = COSINE ? rowk * cb.w : rowk + cb.w;
-            // a NaN anywhere keeps the pair: the exact pass decides
-            if (!(__uint_as_float(acc[ch & 1][jj]) < b0)) kb |= 1u << jj;
-            if (!(__uint_as_float(acc[ch & 1][jj + 1]) < b1)) kb |= 2u << jj;
-            if (!(__uint_as_float(acc[ch & 1][jj + 2]) < b2)) kb |= 4u << jj;
-            if (!(__uint_as_float(acc[ch & 1][jj + 3]) < b3)) kb |= 8u << jj;
-          }
-          kb &= S.colvalid[ms][ch];   // columns without a usable observation never survive
-          const int left = h.ncols_left - ch * 32;   // columns past the scene's last track row hold foreign metadata
-          if (left < 32) kb &= (1u << left) - 1u;
-          if (!row_ok) kb = 0;
-          if (geo && kb) {
-            unsigned int kk = kb;
-            while (kk) {
-              const int jj = __ffs(kk) - 1;
-              kk &= kk - 1;
-              const VisColGeo cg = colgeo[h.col0 + ch * 32 + jj];   // rare path: straight from global memory
-              if (!compat_ok(p, (unsigned int)h.epoch, cg.tep, cx, cy, cr, cg.tx, cg.ty, cg.tr)) kb &= ~(1u << jj);
-            }
-          }
-          keep[ch] = kb;
+      for (int j = 0; j < TC_BN / 8; ++j) {
+        const int c0 = 8 * j + q2;
+        const float2 cb = *reinterpret_cast<const float2*>(gcolb + c0);
+        const unsigned int vw = S.colvalid[ms][c0 >> 5] >> (c0 & 31);   // columns without a usable observation never survive
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int hr = e >> 1, cl = e & 1;
+          const float b = COSINE ? rowk[hr] * (cl ? cb.y : cb.x) : rowk[hr] + (cl ? cb.y : cb.x);
+          // a NaN anywhere keeps the pair: the exact pass decides; columns past the scene's last track row hold foreign
+          // metadata
+          const bool k = !(acc[4 * j + e] < b) && ((vw >> cl) & 1u) && c0 + cl < h.ncols_left && row_ok[hr];
+          if (k) keep[j >> 3] |= 1u << (((4 * j) & 31) + e);
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {   // accumulator buffer drained: the next MMA may start
-        if (PAIR) mbar_arrive_cluster(leader_addr(&S.tmem_empty[buf]));
-        else mbar_arrive(&S.tmem_empty[buf]);
+      if (geo) {
+        float cx[2], cy[2], cr[2];
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+          cx[hr] = 0.0f; cy[hr] = 0.0f; cr[hr] = 0.0f;
+          if (row_ok[hr]) { cx[hr] = f.c_box[(size_t)g[hr] * 6]; cy[hr] = f.c_box[(size_t)g[hr] * 6 + 1]; cr[hr] = f.c_radius[g[hr]]; }
+        }
+#pragma unroll
+        for (int w = 0; w < 4; ++w) {
+          unsigned int kk = keep[w];
+          while (kk) {
+            const int b = __ffs(kk) - 1;
+            kk &= kk - 1;
+            const int i = w * 32 + b, hr = (i >> 1) & 1;
+            const int col = 8 * (i >> 2) + q2 + (i & 1);
+            const VisColGeo cg = colgeo[h.col0 + col];   // rare path: straight from global memory
+            if (!compat_ok(p, (unsigned int)h.epoch, cg.tep, cx[hr], cy[hr], cr[hr], cg.tx, cg.ty, cg.tr)) keep[w] &= ~(1u << b);
+          }
+        }
       }
-      // ---- phase B: survivors -> pair list, ONE warp-aggregated append per tile; everything else is None
+      // survivors -> pair list, ONE warp-aggregated append per tile (a thread's pairs row by row); everything else is None
       int cnt = 0;
 #pragma unroll
-      for (int ch = 0; ch < TC_BN / 32; ++ch) cnt += __popc(keep[ch]);
+      for (int w = 0; w < 4; ++w) cnt += __popc(keep[w]);
       if (__any_sync(0xffffffffu, cnt != 0)) {
         int incl = cnt;
 #pragma unroll
@@ -298,18 +229,22 @@ vis_screen_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
         base = __shfl_sync(0xffffffffu, base, 31);
         int pos = base + incl - cnt;
 #pragma unroll
-        for (int ch = 0; ch < TC_BN / 32; ++ch) {
-          unsigned int kk = keep[ch];
-          while (kk) {
-            const int jj = __ffs(kk) - 1;
-            kk &= kk - 1;
-            if (pos < h.vis_lcap) {
-              const VisColMeta cm = gmeta[ch * 32 + jj];
-              VisPair vp;
-              vp.g = g; vp.row = cm.row; vp.scene = h.scene; vp.outcol = cm.outcol;
-              f.vis_pairs[h.vis_lbase + pos] = vp;
+        for (int hr = 0; hr < 2; ++hr) {
+#pragma unroll
+          for (int w = 0; w < 4; ++w) {
+            unsigned int kk = keep[w] & (hr ? 0xccccccccu : 0x33333333u);
+            while (kk) {
+              const int b = __ffs(kk) - 1;
+              kk &= kk - 1;
+              if (pos < h.vis_lcap) {
+                const int i = w * 32 + b;
+                const VisColMeta cm = gmeta[8 * (i >> 2) + q2 + (i & 1)];
+                VisPair vp;
+                vp.g = g[hr]; vp.row = cm.row; vp.scene = h.scene; vp.outcol = cm.outcol;
+                f.vis_pairs[h.vis_lbase + pos] = vp;
+              }
+              ++pos;
             }
-            ++pos;
           }
         }
       }
@@ -317,14 +252,8 @@ vis_screen_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
       if (lane == 0) mbar_arrive(&S.meta_empty[ms]);   // the slabs of this tile may be overwritten
     }
   }
-  tc_fence_before();
   __syncthreads();
   if (CL >= 2) cluster_sync_all();   // no CTA leaves while its peer may still multicast into / arrive on its smem
-  if (warp == 1) {
-    tc_fence_after();
-    if (PAIR) asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512));
-    else asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512));
-  }
 }
 
 // ------------------------------------------------------------------------------------------------ refine kernel
@@ -449,8 +378,7 @@ __global__ void __launch_bounds__(RF_WARPS * 32, RP == 32 ? 6 : 8) vis_refine_ke
 
 // ------------------------------------------------------------------------------------------------ refine, asynchronous copies
 // Same arithmetic, different data movement.  The register-staged kernel above keeps about 4 KB per warp in flight and has
-// none in flight while a warp adds its serial chains; ncu (round 1) showed it latency-bound (DRAM 47 %, 23 % of the warp
-// slots active).  Here every warp owns a ring of three shared-memory stages and feeds it with cp.async (16-byte chunks, no
+// none in flight while a warp adds its serial chains, so it tends to be latency-bound.  Here every warp owns a ring of three shared-memory stages and feeds it with cp.async (16-byte chunks, no
 // registers held): while it turns the rows of stage s into block sums, the copies of stages s+1 and s+2 -- 16 KB -- are in
 // flight, whatever the warp is doing.  A stage holds the 512-float segments of both rows of two pairs; chunks are stored
 // half-block-major so that the 16-byte reads of the block sums hit 32 different banks.  The 64 block sums of 32 pairs are
@@ -742,8 +670,8 @@ int launch_vis_refine(const Params& p, const TrackStore& ts, const Frame& f, int
   dim3 grid(16, n_scenes);   // 64 warps x 32 survivors per scene in flight; more survivors are claimed in further rounds
   // the vector path needs 16-byte aligned input rows (a caller-owned device pointer on the device-io path)
   const bool tail = p.feature_dim != p.d8 || (reinterpret_cast<uintptr_t>(f.in_feat) & 15) != 0;
-  // SB200_REFINE=async: the cp.async variant (measured slower on B200: 0.39 vs 0.25 ms at cfg5 -- one CTA of six warps per
-  // SM cannot keep the block-sum arithmetic fed; kept for experiments)
+  // SB200_REFINE=async: the cp.async variant (one CTA of six warps per SM may not keep the block-sum arithmetic fed; kept
+  // for experiments)
   static const bool async_copy = getenv("SB200_REFINE") != nullptr && !strcmp(getenv("SB200_REFINE"), "async");
   if (!tail && async_copy) {
     // asynchronous-copy kernel: 3 x 8 KB stages + the parked block sums per warp
@@ -757,8 +685,8 @@ int launch_vis_refine(const Params& p, const TrackStore& ts, const Frame& f, int
     note_launch();
     return 0;
   }
-  // 16 survivors per claim: half the parked block sums of 32, eight CTAs per SM instead of six (0.182 vs 0.200 ms at cfg5);
-  // SB200_REFINE_PAIRS=32 selects the wider claim
+  // 16 survivors per claim: half the parked block sums of 32, eight CTAs per SM instead of six; SB200_REFINE_PAIRS=32
+  // selects the wider claim
   static const bool rp16 = !(getenv("SB200_REFINE_PAIRS") != nullptr && atoi(getenv("SB200_REFINE_PAIRS")) == 32);
 #define SB_RF(C, T)                                                                        \
   do {                                                                                     \
@@ -799,9 +727,8 @@ int launch_vis_cost_tc(const Params& p, const TrackStore& ts, const Frame& f, in
   size_t smem = sizeof(TcSmem) + 1024;
   const bool cosine = p.visual_kind == 1;
   cudaError_t e = cudaSuccess;
-  const void* fn = tc.pair ? (cosine ? (const void*)vis_screen_kernel<3, true> : (const void*)vis_screen_kernel<3, false>)
-                   : cluster ? (cosine ? (const void*)vis_screen_kernel<2, true> : (const void*)vis_screen_kernel<2, false>)
-                             : (cosine ? (const void*)vis_screen_kernel<1, true> : (const void*)vis_screen_kernel<1, false>);
+  const void* fn = cluster ? (cosine ? (const void*)vis_screen_kernel<2, true> : (const void*)vis_screen_kernel<2, false>)
+                           : (cosine ? (const void*)vis_screen_kernel<1, true> : (const void*)vis_screen_kernel<1, false>);
   e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return (int)e;
   if (!tc.colmeta_done) launch_vis_colmeta(p, ts, f, n_scenes, max_n, tc, st);

@@ -151,7 +151,7 @@ void launch_own_area(const Frame& f, int n_scenes, int max_m, const float* d_box
   own_area_kernel<<<grid, OW_WARPS * 32, 0, st>>>(f, d_boxes, d_out, d_ovf_cnt, d_ovf);
   const size_t smem = (size_t)(kOwnBigNb + 1) * 8 * sizeof(double);
   cudaFuncSetAttribute(own_area_big_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  own_area_big_kernel<<<148, OB_T, smem, st>>>(f, d_boxes, d_out, d_ovf_cnt, d_ovf);
+  own_area_big_kernel<<<kNumSms, OB_T, smem, st>>>(f, d_boxes, d_out, d_ovf_cnt, d_ovf);
   note_launch(2);
 }
 

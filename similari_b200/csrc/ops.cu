@@ -235,10 +235,9 @@ int sb200_visual_cost_matrix(int32_t visual_kind, float threshold, const float* 
   if (tc.use_tc) {
     std::vector<sb::TcTile> tiles;
     {
-        // SB200_SCREEN = single | multicast | pair (default): CTA organisation of the screen kernel
+        // SB200_SCREEN = single | multicast (default): CTA organisation of the screen kernel
         const char* e = getenv("SB200_SCREEN");
         tc.cluster2 = !(e && !strcmp(e, "single")) && getenv("SB200_SCREEN_SINGLE") == nullptr;
-        tc.pair = tc.cluster2 && !(e && !strcmp(e, "multicast"));
       }
     for (int m0 = 0; m0 < m; m0 += (tc.cluster2 ? 256 : 128))
       for (int c0 = 0; c0 < n; c0 += 256) tiles.push_back(sb::TcTile{0, m0, c0, 0});

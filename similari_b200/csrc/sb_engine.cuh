@@ -19,6 +19,7 @@
 namespace sb {
 
 constexpr int kMaxConstraints = 8;
+constexpr int kNumSms = 132;  // H100 SXM: grid sizes of the launches that do not query the device
 constexpr int kMaxObs = 8;  // visual_max_observations supported on device (reference default 5)
 constexpr int kStateStride = 32;   // floats per Kalman state row in the tracker's store (kStateFloats padded to 128 bytes)
 constexpr int kMaxHist = 64;  // box history kept per track on the device (history_length above it, or 0 = unlimited, is capped)
@@ -231,13 +232,12 @@ void note_launch(int n = 1);
 unsigned long long launch_count();
 void launch_pos_cost(const Params& p, const TrackStore& ts, const Frame& f, int n_scenes, int max_m, int max_n,
                      cudaStream_t st);
-// visual cost: fp32 SIMT kernel in the reference's summation order (use_tc == false) or the tcgen05 3xTF32 kernel
+// visual cost: fp32 SIMT kernel in the reference's summation order (use_tc == false) or the tensor-core screen
 struct TcArgs {
   int max_init_done;   // the frame's setup kernel already reset scene_max
   int colmeta_done;    // the column metadata of the screen was launched by the caller (side stream)  // tensor-core screen resources (all null / 0 when the dense exact kernel is used)
   bool use_tc;
-  bool cluster2;   // tiles describe candidate-tile PAIRS processed by 2-CTA clusters (multicast B loads, or pair MMAs)
-  bool pair;       // with cluster2: cta_group::2 MMAs (256 x 256 x 16 across the CTA pair)
+  bool cluster2;   // tiles describe candidate-tile PAIRS processed by 2-CTA clusters (multicast B loads)
   const TcTile* d_tiles;
   int n_tiles;            // tiles (stateless operators) or an upper bound of them (trackers: the count is d_n_tiles[0])
   const int* d_n_tiles;   // device-side tile count (null: n_tiles is exact)

@@ -1,6 +1,6 @@
-// sb_tc.cuh -- tcgen05 / TMEM / TMA / mbarrier PTX helpers shared by the tensor-core kernels of the visual cost
+// sb_tc.cuh -- wgmma / TMA / mbarrier / cluster PTX helpers shared by the tensor-core kernels of the visual cost
 // (kernels_feat_tc.cu: screen + refine for selective thresholds; kernels_feat_dense.cu: the dense weight-sum kernel).
-// sm_100a only: every wrapper is one inline-PTX instruction (or a try_wait loop).
+// sm_90a only: every wrapper is one inline-PTX instruction (or a try_wait loop).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -8,10 +8,13 @@
 
 namespace sb {
 
-// tile of the tensor-core kernels: 128 candidate rows (x2 for a CTA pair) x 256 feature rows x 64 features per stage
+// tile of the tensor-core kernels: 128 candidate rows x 256 feature rows x 64 features per stage.  Two consumer
+// warpgroups share a tile, each holds the fp32 accumulators of 64 rows x 256 columns in registers (wgmma m64n256k16).
 constexpr int TC_BM = 128, TC_BN = 256, TC_BK = 64;
 constexpr int TC_A_BYTES = TC_BM * TC_BK * 2;  // 16 KB
 constexpr int TC_B_BYTES = TC_BN * TC_BK * 2;  // 32 KB
+constexpr int TC_WG_ROWS = 64;                 // accumulator rows of one consumer warpgroup
+constexpr int TC_THREADS = 384;                // producer warpgroup (one TMA warp) + two consumer warpgroups
 
 // ------------------------------------------------------------------------------------------------ PTX helpers
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -46,33 +49,11 @@ __device__ __forceinline__ void tma_load_2d_mc(void* dst, const CUtensorMap* map
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%4, %5}], [%2], %3;"
       ::"r"(smem_u32(dst)), "l"((uint64_t)map), "r"(smem_u32(bar)), "h"(mask), "r"(c0), "r"(c1) : "memory");
 }
-__device__ __forceinline__ void tc_commit_mc(void* bar, uint16_t mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(smem_u32(bar)), "h"(mask) : "memory");
-}
-// ---- cta_group::2 (CTA pair) helpers.  leader_addr(): the shared::cluster address of the same variable in CTA rank 0.
-__device__ __forceinline__ uint32_t leader_addr(const void* p) {
+// shared::cluster address of the same variable in CTA `rank` of the cluster
+__device__ __forceinline__ uint32_t cluster_addr(const void* p, uint32_t rank) {
   uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, 0;" : "=r"(r) : "r"(smem_u32(p)));
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_u32(p)), "r"(rank));
   return r;
-}
-__device__ __forceinline__ void tma_load_2d_pair(void* dst, const CUtensorMap* map, int c0, int c1, uint32_t leader_bar) {
-  // the bytes land in THIS CTA's shared memory, the transaction count on the LEADER's barrier
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(dst)), "l"((uint64_t)map), "r"(leader_bar), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ void tc_mma_bf16_pair(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum) : "memory");
-}
-__device__ __forceinline__ void tc_commit_pair_mc(void* bar, uint16_t mask) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(smem_u32(bar)), "h"(mask) : "memory");
 }
 __device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_bar) {
   asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_bar) : "memory");
@@ -89,64 +70,99 @@ __device__ __forceinline__ void bulk_load(void* dst, const void* src, uint32_t b
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                ::"r"(smem_u32(dst)), "l"((uint64_t)src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(void* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tc_mma_bf16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
+// named barrier of the 128 threads of one warpgroup (id 0 is __syncthreads)
+__device__ __forceinline__ void wg_bar(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
+
+// ---- wgmma (asynchronous warpgroup MMA): A and B from shared memory, D in registers
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// D[64 x 256] (+)= A[64 x 16] * B[256 x 16]^T, BF16 operands, fp32 accumulators.  Register i of a thread holds row
+// (warp % 4) * 16 + lane / 4 + 8 * ((i >> 1) & 1), column 8 * (i >> 2) + 2 * (lane % 4) + (i & 1).
+__device__ __forceinline__ void wgmma_bf16_m64n256(float* d, uint64_t adesc, uint64_t bdesc, uint32_t accum) {
   asm volatile(
       "{\n\t"
       ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum) : "memory");
+      "setp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127 "
+      "}, %128, %129, p, 1, 1, 0, 0;\n\t"
+      "}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
+        "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
+        "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(adesc), "l"(bdesc), "r"(accum));
 }
-__device__ __forceinline__ void tc_ld32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// Asynchronous TMEM load split in two: the issue, and a wait that names the destination registers as in/out operands so the
-// compiler cannot move a consumer of r[] above it.
-__device__ __forceinline__ void tc_ld32_issue(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tc_ld_wait32(uint32_t* r) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]), "+r"(r[8]), "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15]), "+r"(r[16]), "+r"(r[17]), "+r"(r[18]), "+r"(r[19]), "+r"(r[20]), "+r"(r[21]), "+r"(r[22]), "+r"(r[23]), "+r"(r[24]), "+r"(r[25]), "+r"(r[26]), "+r"(r[27]), "+r"(r[28]), "+r"(r[29]), "+r"(r[30]), "+r"(r[31])
+// keeps the compiler from moving accesses of the accumulators across a wgmma issue / wait
+__device__ __forceinline__ void wgmma_fence_acc(float* d) {
+  asm volatile("" : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+                 "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+                 "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+                 "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+                 "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+                 "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
+                 "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
+                 "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
                :: "memory");
 }
 
-// K-major, 128-byte swizzle shared-memory matrix descriptor (cute::UMMA::SmemDescriptor layout):
-// start>>4 | LBO(=1, ignored for swizzled K-major)<<16 | SBO(8 rows x 128 B = 1024 B)>>4 <<32 | version 1 <<46 | SW128 (2) <<61
-__device__ __forceinline__ uint64_t umma_desc(uint32_t smem_addr) {
-  return (uint64_t)((smem_addr & 0x3ffffu) >> 4) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) | (2ull << 61);
+// K-major, 128-byte swizzle shared-memory matrix descriptor (sm_90 wgmma layout):
+// start>>4 | LBO(=1, ignored for swizzled K-major)<<16 | SBO(8 rows x 128 B = 1024 B)>>4 <<32 | SW128 (1) <<62
+__device__ __forceinline__ uint64_t wgmma_desc(uint32_t smem_addr) {
+  return (uint64_t)((smem_addr & 0x3ffffu) >> 4) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);
 }
-// instruction descriptor: D = F32 (1<<4), A = B = BF16 (1<<7, 1<<10), K-major both, N>>3 at bit 17, M>>4 at bit 24
-constexpr uint32_t kIdescBf16 = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(TC_BN >> 3) << 17) | ((uint32_t)(TC_BM >> 4) << 24);
 
-// cta_group::2: one MMA spans the CTA pair, M = 256 (128 accumulator rows in each CTA's TMEM), N = 256
-constexpr uint32_t kIdescBf16Pair = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(TC_BN >> 3) << 17) | ((uint32_t)(256 >> 4) << 24);
+// Consumer side of the operand pipeline for one tile: acc (the 64 x 256 accumulators of warpgroup `wg`) = A B^T over KB
+// stages of 64 features.  Stage s holds the A tile (128 rows) at offset 0 and the B tile (256 rows) at TC_A_BYTES.  A
+// stage is handed back one stage behind the issue, once the wgmma that reads it has completed: one arrival per warpgroup
+// on the empty barrier of every CTA of the cluster (CL) whose producer writes into it.
+template <int CL, int NST, int STAGE_B>
+__device__ __forceinline__ void tc_consume_tile(float* acc, unsigned char* stage_base, unsigned long long* full_bar,
+                                                unsigned long long* empty_bar, int KB, int wg, int& stage, uint32_t& phase) {
+  const bool elected = (threadIdx.x & 127) == 0;
+  auto release = [&](int s) {
+    if (!elected) return;
+    if (CL == 1) mbar_arrive(&empty_bar[s]);
+    else
+      for (uint32_t r = 0; r < (uint32_t)CL; ++r) mbar_arrive_cluster(cluster_addr(&empty_bar[s], r));
+  };
+  int prev = -1;
+  for (int kb = 0; kb < KB; ++kb) {
+    mbar_wait(&full_bar[stage], phase);
+    const uint32_t a0 = smem_u32(stage_base + stage * STAGE_B) + (uint32_t)(wg * TC_WG_ROWS * 128);
+    const uint32_t b0 = smem_u32(stage_base + stage * STAGE_B) + TC_A_BYTES;
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < TC_BK / 16; ++k)   // 16 bf16 = 32 bytes inside the 128-byte swizzle atom
+      wgmma_bf16_m64n256(acc, wgmma_desc(a0 + k * 32), wgmma_desc(b0 + k * 32), (kb | k) != 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<1>();   // the previous stage's wgmma has completed
+    if (prev >= 0) release(prev);
+    prev = stage;
+    if (++stage == NST) { stage = 0; phase ^= 1; }
+  }
+  wgmma_wait<0>();
+  wgmma_fence_acc(acc);
+  if (prev >= 0) release(prev);
+}
 
 // BF16 operand rounding bound on a dot product.  BF16 keeps 8 significant bits; round-to-nearest leaves a relative error
 // of at most u = 2^-8 per operand (a value just above a power of two sits half a 2^-7 spacing from its neighbours).
 // Two rounded operands: |a~ b~ - a b| <= (2u + u^2) |a b|, hence by Cauchy-Schwarz
 //   |dot~ - dot| <= (2^-7 + 2^-16) * sum|a_i b_i| <= (2^-7 + 2^-16) * ||a|| ||b||.
-// The fp32 accumulation in TMEM adds at most D * 2^-24 relative (truncation; D <= 4096: 2^-12).  Together
-// 2^-7 + 2^-16 + 2^-12 = 2.066 * 2^-8 <= kScreenRelErr = 2.1 * 2^-8.  (Round 1 used 1.5 * 2^-8: fine for the rounding
-// errors of real feature vectors, which average out, but below the adversarial worst case -- the screen must never drop
-// a pair the exact metric keeps.)
+// The fp32 accumulation of the tensor cores adds at most D * 2^-24 relative (truncation; D <= 4096: 2^-12).  Together
+// 2^-7 + 2^-16 + 2^-12 = 2.066 * 2^-8 <= kScreenRelErr = 2.1 * 2^-8.  (1.5 * 2^-8 would cover the rounding errors of real
+// feature vectors, which average out, but not the adversarial worst case -- the screen must never drop a pair the exact
+// metric keeps.)
 constexpr float kScreenRelErr = 2.1f / 256.0f;
 
 }  // namespace sb

@@ -14,7 +14,7 @@ def eng():
     from similari_b200._lib import lib
 
     if lib().sb200_device_count() <= 0:
-        pytest.fail("no CUDA device: the gpu-marked tests must run on the B200 box")
+        pytest.fail("no CUDA device: the gpu-marked tests must run on an H100")
     return e
 
 
@@ -132,7 +132,7 @@ def test_cfg5_scene_with_degenerate_features_overflows_its_list_mid_batch(eng, o
 @pytest.mark.parametrize("gate", ["quality", "area", "has_feature", "own_area"])
 def test_visual_gates_on_the_tensor_core_path_at_baseline_size(eng, oracle, gate, monkeypatch):
     """The gates of VisualMetric::metric (src/trackers/visual_sort/metric.rs:227-249, 280-290) -- candidate quality,
-    minimal box area, feature present, own-area share -- at 512 x 512 x 512-d with the tcgen05 path forced: candidates the
+    minimal box area, feature present, own-area share -- at 512 x 512 x 512-d with the tensor-core path forced: candidates the
     gate rejects must not vote visually (row mask of the screen), tracks below the minimal feature count must not be
     scored (column mask), and rejected features must not be collected."""
     from similari_b200._lib import default_options

@@ -17,7 +17,7 @@ def eng():
     from similari_b200._lib import lib
 
     if lib().sb200_device_count() <= 0:
-        pytest.fail("no CUDA device: the gpu-marked tests must run on the B200 box")
+        pytest.fail("no CUDA device: the gpu-marked tests must run on an H100")
     return e
 
 
@@ -286,7 +286,7 @@ def _tc_inputs(m, n, d, seed):
 @pytest.mark.parametrize("kind", ["euclid", "cosine"])
 @pytest.mark.parametrize("m,n,d", [(64, 64, 64), (129, 257, 72), (300, 700, 512), (130, 1000, 2048), (500, 1536, 512)])
 def test_visual_cost_matrix_tensor_core_bit_exact(eng, oracle, kind, m, n, d, monkeypatch):
-    """tcgen05 BF16 screen + exact f32 refinement: every emitted value is bit-identical to the oracle and no pair
+    """Tensor-core BF16 screen + exact f32 refinement: every emitted value is bit-identical to the oracle and no pair
     that passes the threshold is lost by the screen."""
     monkeypatch.setenv("SB200_VIS_KERNEL", "tc")
     cf, tf = _tc_inputs(m, n, d, 400 + d + m)

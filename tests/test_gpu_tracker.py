@@ -13,7 +13,7 @@ def eng():
     from similari_b200._lib import lib
 
     if lib().sb200_device_count() <= 0:
-        pytest.fail("no CUDA device: the gpu-marked tests must run on the B200 box")
+        pytest.fail("no CUDA device: the gpu-marked tests must run on an H100")
     return e
 
 
@@ -111,7 +111,7 @@ def test_visual_trackers_match_oracle(eng, oracle, kind, pos, vis):
 @pytest.mark.parametrize("kind", [2, 3])
 @pytest.mark.parametrize("vis", [0, 1])
 def test_visual_trackers_tensor_core_path_match_oracle(eng, oracle, kind, vis, monkeypatch):
-    """Same end-to-end comparison with the tcgen05 visual-cost kernel forced on (the default for large frames)."""
+    """Same end-to-end comparison with the tensor-core visual-cost kernel forced on (the default for large frames)."""
     monkeypatch.setenv("SB200_VIS_KERNEL", "tc")
     cfg = small("cfg5", n_scenes=1 if kind == 2 else 3, n_objects=150, oriented=False, canvas=(1400.0, 900.0),
                 feature_dim=128)
@@ -121,12 +121,12 @@ def test_visual_trackers_tensor_core_path_match_oracle(eng, oracle, kind, vis, m
                     visual_min_votes=2, visual_minimal_track_length=1, min_confidence=0.1))
 
 
-@pytest.mark.parametrize("mode", ["single", "multicast", "pair"])
+@pytest.mark.parametrize("mode", ["single", "multicast"])
 @pytest.mark.parametrize("vis", [0, 1])
 def test_screen_kernel_cta_organisations_match_oracle(eng, oracle, mode, vis, monkeypatch):
-    """The three CTA organisations of the screen kernel (one CTA per tile, 2-CTA cluster with multicast B loads,
-    cta_group::2 pair MMAs -- the default) against the oracle; 300 candidates per scene exercise the ragged second
-    candidate tile of a pair (rows 256..299 valid, the rest masked) and D = 96 the zero-filled K tail."""
+    """The two CTA organisations of the screen kernel (one CTA per tile; 2-CTA cluster with multicast B loads, the
+    default) against the oracle; 300 candidates per scene exercise the ragged second candidate tile of a cluster
+    (rows 256..299 valid, the rest masked) and D = 96 the zero-filled K tail."""
     monkeypatch.setenv("SB200_VIS_KERNEL", "tc")
     monkeypatch.setenv("SB200_SCREEN", mode)
     cfg = small("cfg5", n_scenes=3, n_objects=300, oriented=False, canvas=(2200.0, 1400.0), feature_dim=96)
@@ -457,7 +457,7 @@ F32MAX = float(np.finfo(np.float32).max)
 @pytest.mark.parametrize("kobs,min_votes", [(3, 2), (5, 1), (2, 2), (4, 3)])
 def test_dense_tensor_core_path_matches_oracle(eng, oracle, kind, vis, thr, kobs, min_votes, monkeypatch):
     """Thresholds that cut nothing -- the reference's default Euclidean(f32::MAX), cosine(-1), the published bench's
-    Euclidean(10.0) on unit vectors -- on the dense tensor-core path (kernels_feat_dense.cu): tcgen05 weight sums with error
+    Euclidean(10.0) on unit vectors -- on the dense tensor-core path (kernels_feat_dense.cu): wgmma weight sums with error
     bounds, exact max_dist, selection of the groups that can be a BestFit row / column maximum, exact refinement, voting.
     Every id / voting type must be the oracle's.  K = 2..5 observations exercise column tiles of 256, 255, 256 and 255
     feature rows (tiles end at block boundaries), min_votes the block filter."""
