@@ -860,13 +860,10 @@ int sb200_tracker::predict(int32_t n_scenes, const uint64_t* scene_ids, const in
   if (want_tc || want_dense) {
     tc.use_tc = true;
     tc.dense = want_dense;
-    {
-      // SB200_SCREEN = single | multicast (default): CTA organisation of the screen kernel (the dense kernel: multicast)
-      const char* e = getenv("SB200_SCREEN");
-      tc.cluster2 = want_dense || (!(e && !strcmp(e, "single")) && getenv("SB200_SCREEN_SINGLE") == nullptr);
-    }
-    mstep = tc.cluster2 ? 256 : 128;   // a cluster covers two 128-row candidate tiles
-    if (want_dense) cstep = (256 / K) * K;   // column tiles end at block boundaries: a track's observations stay together
+    mstep = 256;   // a cluster covers two 128-row candidate tiles
+    // dense: column tiles end at block boundaries, a track's observations stay together
+    cstep = want_dense ? (256 / K) * K : sb::vis_screen_ucols(P.d8, num_sms, n_scenes, m_of.data(), nb_ub.data(), K);
+    tc.cstep = cstep;
     long long tiles_ub = 0, slabs_ub = 0, ws_ub = 0, blk_ub = 0;
     for (int s = 0; s < n_scenes; ++s) {
       const long long ct = ((long long)nb_ub[s] * K + cstep - 1) / cstep;
@@ -921,7 +918,6 @@ int sb200_tracker::predict(int32_t n_scenes, const uint64_t* scene_ids, const in
           (rc = ENS(f_dscene, 4 * 6 * (size_t)n_scenes + 128)) || (rc = ENS(f_maxc, sizeof(sb::VisPair) * (size_t)std::max<long long>(1, visl_alloc))) ||
           (rc = ENS(f_maxcval, 4 * (size_t)std::max<long long>(1, visl_alloc))))
         return rc;
-      tc.cstep = cstep;
       tc.max_blocks = max_nb;
       tc.n_slabs_ub = (int)slabs_ub;
       tc.ws = f_ws.p;

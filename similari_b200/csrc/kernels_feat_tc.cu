@@ -18,10 +18,12 @@
 //                CPU reference -- the tensor cores only decide which pairs are worth computing.
 //   If the pair list overflows (a non-selective threshold) the caller falls back to the dense exact SIMT kernel.
 //
-// Screen kernel: persistent CTAs (one per SM), 384 threads = a producer warpgroup (one TMA warp) and two consumer
-// warpgroups.  Tile 128 (candidates) x 256 (track-observation rows) x 64 (features = one 128-byte swizzle atom of bf16);
-// 4 smem stages of 48 KB, so the loads of the next tile run while the consumers screen this one.  Each consumer
-// warpgroup accumulates 64 candidate rows x 256 columns in registers and screens them in place.
+// Screen kernels: persistent 2-CTA clusters (one CTA per SM), 384 threads = a producer warpgroup (one TMA thread) and two
+// consumer warpgroups.  d8 <= 512 (vis_screen_sa_kernel): the cluster's candidate rows stay in shared memory for a whole
+// work unit and only the track-observation rows stream; each consumer warpgroup owns whole 128 x 128 output tiles and the
+// two take turns on the tensor pipe.  d8 > 512 (vis_screen_kernel): tile 128 (candidates) x 256 (track-observation rows)
+// x 64 (features = one 128-byte swizzle atom of bf16), both operands streamed through 4 smem stages of 48 KB; each
+// consumer warpgroup accumulates 64 candidate rows x 256 columns in registers and screens them in place.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -56,10 +58,10 @@ struct TcSmem {
 static_assert(sizeof(TcSmem) + 1024 <= 227 * 1024, "screen kernel exceeds the shared memory of an SM");
 
 
-// ------------------------------------------------------------------------------------------------ screen kernel
-// CL == 2: clusters of two CTAs work on two candidate tiles (m0, m0 + 128) of the same track-row tile; each CTA loads
-// its own A tile and HALF of the B tile, multicast into both CTAs' shared memory, so B crosses L2 -> SM once per pair.
-template <int CL, bool COSINE>
+// ------------------------------------------------------------------------------------------------ screen kernel, d8 > 512
+// Clusters of two CTAs work on two candidate tiles (m0, m0 + 128) of the same track-row tile; each CTA loads its own A
+// tile and HALF of the B tile, multicast into both CTAs' shared memory, so B crosses L2 -> SM once per pair.
+template <bool COSINE>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 vis_screen_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB, Params p,
                   TrackStore ts, Frame f, const TcTile* tiles, int n_tiles_host, const int* n_tiles_dev,
@@ -75,17 +77,17 @@ vis_screen_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
   const int KB = (p.d8 + TC_BK - 1) / TC_BK;
 
   unsigned char* const stage_base = &S.stage[0][0];
-  const uint32_t crank = CL >= 2 ? cluster_rank() : 0u;
-  const int cta_first = CL >= 2 ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;   // first (cluster) tile of this CTA
-  const int cta_step = CL >= 2 ? (int)(gridDim.x >> 1) : (int)gridDim.x;
+  const uint32_t crank = cluster_rank();
+  const int cta_first = (int)(blockIdx.x >> 1);   // first (cluster) tile of this CTA
+  const int cta_step = (int)(gridDim.x >> 1);
   if (threadIdx.x == 0) {
     // empty: one arrival per consumer warpgroup of every CTA that reads the stage's bytes; meta_empty: the 8 consumer warps
-    for (int s = 0; s < TC_STAGES; ++s) { mbar_init(&S.full_bar[s], 1); mbar_init(&S.empty_bar[s], 2 * CL); }
+    for (int s = 0; s < TC_STAGES; ++s) { mbar_init(&S.full_bar[s], 1); mbar_init(&S.empty_bar[s], 4); }
     for (int b = 0; b < 4; ++b) { mbar_init(&S.meta_full[b], 1); mbar_init(&S.meta_empty[b], 8); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
-  if (CL >= 2) cluster_sync_all();   // the peer's barriers are initialised before anything is multicast into them
+  cluster_sync_all();   // the peer's barriers are initialised before anything is multicast into them
 
   if (warp < 4) {
     // ===================================================================== TMA producer (one thread); the warpgroup hands
@@ -125,17 +127,13 @@ vis_screen_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
           bulk_load(S.colvalid[g], colvalid + (h.col0 >> 5), TC_BN / 8, &S.meta_full[g]);   // col0 is a multiple of 128
         }
         for (int kb = 0; kb < KB; ++kb) {
-          mbar_wait(&S.empty_bar[stage], phase ^ 1);   // CL == 2: both CTAs have released the stage
+          mbar_wait(&S.empty_bar[stage], phase ^ 1);   // both CTAs have released the stage
           unsigned char* base = stage_base + stage * TC_STAGE_BYTES;
           mbar_expect_tx(&S.full_bar[stage], TC_STAGE_BYTES);
           tma_load_2d(base, &mapA, kb * TC_BK, rowA, &S.full_bar[stage]);
-          if (CL == 2) {
-            // this CTA's half of the B tile (rows rank*128 .. +128), delivered to both CTAs
-            tma_load_2d_mc(base + TC_A_BYTES + crank * (TC_B_BYTES / 2), &mapB, kb * TC_BK, rowB + (int)crank * (TC_BN / 2),
-                           &S.full_bar[stage], (uint16_t)0x3);
-          } else {
-            tma_load_2d(base + TC_A_BYTES, &mapB, kb * TC_BK, rowB, &S.full_bar[stage]);
-          }
+          // this CTA's half of the B tile (rows rank*128 .. +128), delivered to both CTAs
+          tma_load_2d_mc(base + TC_A_BYTES + crank * (TC_B_BYTES / 2), &mapB, kb * TC_BK, rowB + (int)crank * (TC_BN / 2),
+                         &S.full_bar[stage], (uint16_t)0x3);
           if (++stage == TC_STAGES) { stage = 0; phase ^= 1; }
         }
       }
@@ -155,7 +153,7 @@ vis_screen_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
     int it = 0;
     for (int t = cta_first; t < n_tiles; t += cta_step, ++it) {
       float acc[128];
-      tc_consume_tile<CL, TC_STAGES, TC_STAGE_BYTES>(acc, stage_base, S.full_bar, S.empty_bar, KB, wg, stage, phase);
+      tc_consume_tile<2, TC_STAGES, TC_STAGE_BYTES>(acc, stage_base, S.full_bar, S.empty_bar, KB, wg, stage, phase);
       const int ms = it & 3;   // slab set of this tile (same rule as the producer)
       mbar_wait(&S.meta_full[ms], (it >> 2) & 1);
       const VisColMeta* gmeta = S.meta[ms];
@@ -253,7 +251,294 @@ vis_screen_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
     }
   }
   __syncthreads();
-  if (CL >= 2) cluster_sync_all();   // no CTA leaves while its peer may still multicast into / arrive on its smem
+  cluster_sync_all();   // no CTA leaves while its peer may still multicast into / arrive on its smem
+}
+
+// ------------------------------------------------------------------------------------------------ screen kernel, d8 <= 512
+// A-stationary organisation.  A work unit is (scene, pair of 128-row candidate tiles, range of track-observation rows)
+// and one 2-CTA cluster runs it: each CTA keeps its 128 candidate rows x d8 resident in shared memory (loaded once per
+// unit, each 64-feature block on its own barrier so the first column tile starts on the first block) and streams the
+// unit's B rows through a FIFO ring of 128-row x 64-feature stages, half of every stage loaded by each CTA and multicast
+// to both.  Only B crosses L2 -> SM per output tile: 64 KB per CTA per 128 x 128 x 512 tile.
+//
+// Ping-pong consumers: the column tiles of the cluster's units form one sequence; consumer warpgroup 0 takes the even
+// positions, warpgroup 1 the odd ones, and each holds a whole 128 x 128 tile (two m64n128 MMAs per k16 step, 128 fp32
+// accumulators).  A pair of named barriers hands the tensor pipe from one warpgroup's mainloop to the other's, so one
+// warpgroup screens its tile while the other's MMAs run.
+constexpr int SA_BN = 128;                          // track-observation rows per column tile (one warpgroup's tile)
+constexpr int SA_KMAX = 8;                          // 64-feature blocks of A kept resident: d8 <= 512
+constexpr int SA_A_BLOCK = TC_BM * TC_BK * 2;       // 16 KB
+constexpr int SA_B_STAGE = SA_BN * TC_BK * 2;       // 16 KB
+constexpr int SA_STAGES = 5;
+constexpr int SA_SLABS = 4;                         // column-tile metadata slabs in flight
+struct SaHdr { int scene, m0, ncols, m, det_base, col0, epoch, vis_lbase, vis_lcap, unit, last, pad; };
+struct SaSmem {
+  unsigned char a[SA_KMAX][SA_A_BLOCK];             // 1024-byte aligned operand buffers first
+  unsigned char b[SA_STAGES][SA_B_STAGE];
+  VisColMeta meta[SA_SLABS][SA_BN];
+  float colb[SA_SLABS][SA_BN];
+  unsigned int colvalid[SA_SLABS][SA_BN / 32];
+  SaHdr hdr[SA_SLABS];
+  unsigned long long a_full[SA_KMAX];
+  unsigned long long a_empty;
+  unsigned long long full_bar[SA_STAGES];
+  unsigned long long empty_bar[SA_STAGES];
+  unsigned long long meta_full[SA_SLABS];
+  unsigned long long meta_empty[SA_SLABS];
+};
+static_assert(sizeof(SaSmem) + 1024 <= 227 * 1024, "A-stationary screen kernel exceeds the shared memory of an SM");
+constexpr int kScreenStationaryMaxD8 = SA_KMAX * TC_BK;
+
+// units: TcTile (scene, m0, c0) with m0 a multiple of 256 and c0 a multiple of ucols; the unit covers the scene's rows
+// c0 .. min(c0 + ucols, nb * K)
+template <bool COSINE>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+vis_screen_sa_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB, Params p,
+                     TrackStore ts, Frame f, const TcTile* units, int n_units_host, const int* n_units_dev, int ucols,
+                     const VisColMeta* colmeta, const VisColGeo* colgeo, const VisRowMeta* rowmeta, const float* colb,
+                     const unsigned int* colvalid) {
+  const int n_units = n_units_dev ? *n_units_dev : n_units_host;
+  extern __shared__ unsigned char smem_raw_[];
+  SaSmem& S = *reinterpret_cast<SaSmem*>(smem_raw_ + ((1024u - (smem_u32(smem_raw_) & 1023u)) & 1023u));
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int K = p.max_obs;
+  const int KB = (p.d8 + TC_BK - 1) / TC_BK;
+  const uint32_t crank = cluster_rank();
+  if (threadIdx.x == 0) {
+    // full: the local producer's expect_tx; empty: the consuming warpgroup of each CTA; a_empty: both local consumer
+    // warpgroups (or the producer for a warpgroup without a tile in the unit); meta_empty: the 4 warps of the consumer
+    for (int kb = 0; kb < SA_KMAX; ++kb) mbar_init(&S.a_full[kb], 1);
+    mbar_init(&S.a_empty, 2);
+    for (int s = 0; s < SA_STAGES; ++s) { mbar_init(&S.full_bar[s], 1); mbar_init(&S.empty_bar[s], 2); }
+    for (int b = 0; b < SA_SLABS; ++b) { mbar_init(&S.meta_full[b], 1); mbar_init(&S.meta_empty[b], 4); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+  cluster_sync_all();   // the peer's barriers are initialised before anything is multicast into them
+
+  if (warp < 4) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (warp == 0 && lane == 0) {
+      asm volatile("prefetch.tensormap [%0];" ::"l"((uint64_t)&mapA) : "memory");
+      asm volatile("prefetch.tensormap [%0];" ::"l"((uint64_t)&mapB) : "memory");
+      int seq = 0, gk = 0, unit = 0;
+      for (int u = (int)(blockIdx.x >> 1); u < n_units; u += (int)(gridDim.x >> 1), ++unit) {
+        const TcTile tl = units[u];
+        const SceneDesc sc = f.scenes[tl.scene];
+        const int m0 = tl.m0 + (int)crank * TC_BM;
+        const int rowA = sc.det_base + m0;
+        const int cols = min(ucols, sc.nb * K - tl.c0);
+        const int nct = (cols + SA_BN - 1) / SA_BN;
+        const int rowB = sc.slot * ts.track_cap * K + tl.c0;
+        // A stays until both warpgroups have completed the MMAs of the previous unit
+        if (unit > 0) mbar_wait(&S.a_empty, (unit - 1) & 1);
+        if (nct == 1) mbar_arrive(&S.a_empty);   // on behalf of the warpgroup without a tile in this unit
+        for (int ct = 0; ct < nct; ++ct, ++seq) {
+          const int g = seq % SA_SLABS;
+          mbar_wait(&S.meta_empty[g], ((seq / SA_SLABS) & 1) ^ 1);
+          SaHdr h;
+          h.scene = tl.scene; h.m0 = m0; h.ncols = min(SA_BN, cols - ct * SA_BN); h.m = sc.m; h.det_base = sc.det_base;
+          h.col0 = sc.col_off + tl.c0 + ct * SA_BN; h.epoch = (int)sc.epoch; h.vis_lbase = sc.vis_lbase;
+          h.vis_lcap = sc.vis_lcap; h.unit = unit; h.last = ct + 2 >= nct; h.pad = 0;
+          S.hdr[g] = h;   // published by the release of the arrive below
+          mbar_expect_tx(&S.meta_full[g], (uint32_t)(sizeof(VisColMeta) * SA_BN + 4 * SA_BN + SA_BN / 8));
+          bulk_load(S.meta[g], colmeta + h.col0, (uint32_t)(sizeof(VisColMeta) * SA_BN), &S.meta_full[g]);
+          bulk_load(S.colb[g], colb + h.col0, 4 * SA_BN, &S.meta_full[g]);
+          bulk_load(S.colvalid[g], colvalid + (h.col0 >> 5), SA_BN / 8, &S.meta_full[g]);   // col0 is a multiple of 128
+          for (int kb = 0; kb < KB; ++kb, ++gk) {
+            if (ct == 0) {
+              mbar_expect_tx(&S.a_full[kb], SA_A_BLOCK);
+              tma_load_2d(S.a[kb], &mapA, kb * TC_BK, rowA, &S.a_full[kb]);
+            }
+            const int s = gk % SA_STAGES;
+            mbar_wait(&S.empty_bar[s], ((gk / SA_STAGES) & 1) ^ 1);   // both CTAs have released the stage
+            mbar_expect_tx(&S.full_bar[s], SA_B_STAGE);
+            // this CTA's half of the stage (rows rank*64 .. +64), delivered to both CTAs
+            tma_load_2d_mc(S.b[s] + crank * (SA_B_STAGE / 2), &mapB, kb * TC_BK, rowB + ct * SA_BN + (int)crank * (SA_BN / 2),
+                           &S.full_bar[s], (uint16_t)0x3);
+          }
+        }
+      }
+      // two end markers: one for each consumer warpgroup
+      for (int e = 0; e < 2; ++e, ++seq) {
+        const int g = seq % SA_SLABS;
+        mbar_wait(&S.meta_empty[g], ((seq / SA_SLABS) & 1) ^ 1);
+        S.hdr[g].scene = -1 - e;
+        mbar_arrive(&S.meta_full[g]);
+      }
+    }
+  } else {
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    // Warpgroup wg screens the column tiles at positions wg, wg + 2, ... of the cluster's sequence.  Accumulator register
+    // i (0..127) holds row 64 * (i >> 6) + rr[(i >> 1) & 1] and column 8 * ((i & 63) >> 2) + q2 + (i & 1).
+    const int wg = (warp >> 2) - 1;
+    const int rr[2] = {(warp & 3) * 16 + (lane >> 2), (warp & 3) * 16 + (lane >> 2) + 8};
+    const int q2 = 2 * (lane & 3);
+    const bool geo = p.n_constraints > 0;
+    const bool elected = (threadIdx.x & 127) == 0;
+    for (int pos = wg;; pos += 2) {
+      const int ms = pos % SA_SLABS;
+      mbar_wait(&S.meta_full[ms], (pos / SA_SLABS) & 1);
+      const SaHdr h = S.hdr[ms];
+      // named barriers 1 + (pos & 1): the warpgroup at position pos waits for the mainloop of position pos - 1
+      if (pos > 0) wg2_bar_sync(1 + (pos & 1));
+      if (h.scene < 0) {
+        if (h.scene == -1) wg2_bar_arrive(1 + ((pos + 1) & 1));   // lets the other warpgroup reach its end marker
+        break;
+      }
+      // row constants of the 4 rows of this thread (rows past the tile's candidates read padding and are masked)
+      float rowk[2][2];
+      bool row_ok[2][2];
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+          const int m = h.m0 + 64 * hh + rr[hr];
+          const VisRowMeta rm = rowmeta[h.det_base + m];
+          rowk[hh][hr] = rm.rowk;
+          row_ok[hh][hr] = m < h.m && rm.ok;
+        }
+
+      float acc[128];
+      {
+        const int g0 = pos * KB;
+        int stage = g0 % SA_STAGES;
+        uint32_t phase = (g0 / SA_STAGES) & 1;
+        int prev = -1;
+        auto release = [&](int s) {
+          if (elected)
+            for (uint32_t r = 0; r < 2; ++r) mbar_arrive_cluster(cluster_addr(&S.empty_bar[s], r));
+        };
+        for (int kb = 0; kb < KB; ++kb) {
+          mbar_wait(&S.a_full[kb], (uint32_t)h.unit & 1u);
+          mbar_wait(&S.full_bar[stage], phase);
+          const uint32_t a0 = smem_u32(S.a[kb]);
+          const uint32_t b0 = smem_u32(S.b[stage]);
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < TC_BK / 16; ++k) {
+            const uint32_t acc_on = (kb | k) != 0 ? 1u : 0u;
+            wgmma_bf16_m64n128(acc, wgmma_desc(a0 + k * 32), wgmma_desc(b0 + k * 32), acc_on);
+            wgmma_bf16_m64n128(acc + 64, wgmma_desc(a0 + 64 * 128 + k * 32), wgmma_desc(b0 + k * 32), acc_on);
+          }
+          wgmma_commit();
+          wgmma_wait<1>();   // the previous stage's MMAs have completed
+          if (prev >= 0) release(prev);
+          prev = stage;
+          if (++stage == SA_STAGES) { stage = 0; phase ^= 1; }
+        }
+        wg2_bar_arrive(1 + ((pos + 1) & 1));   // the other warpgroup's mainloop may start
+        wgmma_wait<0>();
+        wgmma_fence_acc(acc);
+        release(prev);
+        if (h.last && elected) mbar_arrive(&S.a_empty);   // this warpgroup's last MMAs on the unit's A have completed
+      }
+
+      // Screen test (see vis_screen_kernel).  Column and row conditions are folded into masks built once per tile, so
+      // the inner loop is the test alone; a NaN accumulator keeps the pair.
+      const VisColMeta* gmeta = S.meta[ms];
+      const float* gcolb = S.colb[ms];
+      unsigned int colm[2] = {0u, 0u};   // bit i & 31 of colm[i >> 5] (i = register index within a 64-row half)
+#pragma unroll
+      for (int j = 0; j < SA_BN / 8; ++j) {
+        const int c0 = 8 * j + q2;
+        unsigned int m2 = (S.colvalid[ms][c0 >> 5] >> (c0 & 31)) & 3u;
+        m2 &= (c0 < h.ncols ? 1u : 0u) | (c0 + 1 < h.ncols ? 2u : 0u);
+        colm[j >> 3] |= (m2 | (m2 << 2)) << ((4 * j) & 31);
+      }
+      unsigned int keep[4];
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const unsigned int rowm = (row_ok[hh][0] ? 0x33333333u : 0u) | (row_ok[hh][1] ? 0xccccccccu : 0u);
+        keep[2 * hh] = 0u;
+        keep[2 * hh + 1] = 0u;
+#pragma unroll
+        for (int j = 0; j < SA_BN / 8; ++j) {
+          const float2 cb = *reinterpret_cast<const float2*>(gcolb + 8 * j + q2);
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            const float rk = rowk[hh][e >> 1], c = (e & 1) ? cb.y : cb.x;
+            const float b = COSINE ? rk * c : rk + c;
+            if (!(acc[64 * hh + 4 * j + e] < b)) keep[2 * hh + (j >> 3)] |= 1u << ((4 * j + e) & 31);
+          }
+        }
+        keep[2 * hh] &= colm[0] & rowm;
+        keep[2 * hh + 1] &= colm[1] & rowm;
+      }
+      if (geo) {
+        float cx[2][2], cy[2][2], cr[2][2];
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+          for (int hr = 0; hr < 2; ++hr) {
+            cx[hh][hr] = 0.0f; cy[hh][hr] = 0.0f; cr[hh][hr] = 0.0f;
+            if (row_ok[hh][hr]) {
+              const size_t g = (size_t)h.det_base + h.m0 + 64 * hh + rr[hr];
+              cx[hh][hr] = f.c_box[g * 6]; cy[hh][hr] = f.c_box[g * 6 + 1]; cr[hh][hr] = f.c_radius[g];
+            }
+          }
+#pragma unroll
+        for (int w = 0; w < 4; ++w) {
+          unsigned int kk = keep[w];
+          while (kk) {
+            const int b = __ffs(kk) - 1;
+            kk &= kk - 1;
+            const int i = (w & 1) * 32 + b, hh = w >> 1;
+            const bool r8 = (i >> 1) & 1;   // selects, not an index: the row arrays stay in registers
+            const int col = 8 * (i >> 2) + q2 + (i & 1);
+            const VisColGeo cg = colgeo[h.col0 + col];   // rare path: straight from global memory
+            if (!compat_ok(p, (unsigned int)h.epoch, cg.tep, r8 ? cx[hh][1] : cx[hh][0], r8 ? cy[hh][1] : cy[hh][0],
+                           r8 ? cr[hh][1] : cr[hh][0], cg.tx, cg.ty, cg.tr))
+              keep[w] &= ~(1u << b);
+          }
+        }
+      }
+      // survivors -> pair list, ONE warp-aggregated append per tile (a thread's pairs row by row)
+      int cnt = 0;
+#pragma unroll
+      for (int w = 0; w < 4; ++w) cnt += __popc(keep[w]);
+      if (__any_sync(0xffffffffu, cnt != 0)) {
+        int incl = cnt;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+          int tt = __shfl_up_sync(0xffffffffu, incl, o);
+          if (lane >= o) incl += tt;
+        }
+        const int total = __shfl_sync(0xffffffffu, incl, 31);
+        int base = 0;
+        if (lane == 31) base = atomicAdd(&f.vis_cnt[h.scene], total);
+        base = __shfl_sync(0xffffffffu, base, 31);
+        int at = base + incl - cnt;
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+#pragma unroll
+          for (int hr = 0; hr < 2; ++hr) {
+            const int g = h.det_base + h.m0 + 64 * hh + rr[hr];
+#pragma unroll
+            for (int w = 0; w < 2; ++w) {
+              unsigned int kk = keep[2 * hh + w] & (hr ? 0xccccccccu : 0x33333333u);
+              while (kk) {
+                const int b = __ffs(kk) - 1;
+                kk &= kk - 1;
+                if (at < h.vis_lcap) {
+                  const int i = w * 32 + b;
+                  const VisColMeta cm = gmeta[8 * (i >> 2) + q2 + (i & 1)];
+                  VisPair vp;
+                  vp.g = g; vp.row = cm.row; vp.scene = h.scene; vp.outcol = cm.outcol;
+                  f.vis_pairs[h.vis_lbase + at] = vp;
+                }
+                ++at;
+              }
+            }
+          }
+        }
+      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&S.meta_empty[ms]);   // the slabs of this tile may be overwritten
+    }
+  }
+  __syncthreads();
+  cluster_sync_all();   // no CTA leaves while its peer may still multicast into / arrive on its smem
 }
 
 // ------------------------------------------------------------------------------------------------ refine kernel
@@ -712,6 +997,24 @@ void launch_vis_colmeta(const Params& p, const TrackStore& ts, const Frame& f, i
   note_launch();
 }
 
+int vis_screen_ucols(int d8, int num_sms, int n_scenes, const int* m, const int* nb, int K) {
+  if (d8 > kScreenStationaryMaxD8) return TC_BN;
+  long long pairs = 0, pair_tiles = 0;
+  int max_ct = 1;
+  for (int s = 0; s < n_scenes; ++s) {
+    const int ct = (nb[s] * K + SA_BN - 1) / SA_BN, rp = (m[s] + 2 * TC_BM - 1) / (2 * TC_BM);
+    pairs += rp;
+    pair_tiles += (long long)rp * ct;
+    max_ct = std::max(max_ct, ct);
+  }
+  // whole scenes when the candidate-tile pairs alone give every cluster two units; else split the columns until they do,
+  // but not below two column tiles, one for each consumer warpgroup
+  const long long units = 2ll * std::max(1, num_sms / 2);
+  if (pairs >= units) return max_ct * SA_BN;
+  const long long per = (pair_tiles + units - 1) / units;
+  return (int)std::max<long long>(2, std::min<long long>(per, max_ct)) * SA_BN;
+}
+
 int launch_vis_cost_tc(const Params& p, const TrackStore& ts, const Frame& f, int n_scenes, int max_n, const TcArgs& tc,
                        int phase, cudaStream_t st) {
   if (tc.n_tiles == 0) return 0;
@@ -720,15 +1023,18 @@ int launch_vis_cost_tc(const Params& p, const TrackStore& ts, const Frame& f, in
     if (tc.ev_refine1) cudaEventRecord(tc.ev_refine1, st);
     return rc;
   }
-  const bool cluster = tc.cluster2;
+  // d8 <= 512: the A-stationary kernel over work units of tc.cstep columns; wider features do not fit A in shared
+  // memory, they take the streaming kernel over 256-column tiles
+  const bool stationary = p.d8 <= kScreenStationaryMaxD8;
   CUtensorMap mA, mB;
-  if (make_map(&mA, f.c_bf16, tc.a_rows, p.d8, TC_BM) || make_map(&mB, ts.feat_bf16, tc.b_rows, p.d8, cluster ? TC_BN / 2 : TC_BN))
+  if (make_map(&mA, f.c_bf16, tc.a_rows, p.d8, TC_BM) ||
+      make_map(&mB, ts.feat_bf16, tc.b_rows, p.d8, stationary ? SA_BN / 2 : TC_BN / 2))
     return -1;
-  size_t smem = sizeof(TcSmem) + 1024;
+  const size_t smem = (stationary ? sizeof(SaSmem) : sizeof(TcSmem)) + 1024;
   const bool cosine = p.visual_kind == 1;
   cudaError_t e = cudaSuccess;
-  const void* fn = cluster ? (cosine ? (const void*)vis_screen_kernel<2, true> : (const void*)vis_screen_kernel<2, false>)
-                           : (cosine ? (const void*)vis_screen_kernel<1, true> : (const void*)vis_screen_kernel<1, false>);
+  const void* fn = stationary ? (cosine ? (const void*)vis_screen_sa_kernel<true> : (const void*)vis_screen_sa_kernel<false>)
+                              : (cosine ? (const void*)vis_screen_kernel<true> : (const void*)vis_screen_kernel<false>);
   e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return (int)e;
   if (!tc.colmeta_done) launch_vis_colmeta(p, ts, f, n_scenes, max_n, tc, st);
@@ -736,7 +1042,7 @@ int launch_vis_cost_tc(const Params& p, const TrackStore& ts, const Frame& f, in
   note_launch();
   if (tc.ev_screen0) cudaEventRecord(tc.ev_screen0, st);
   {
-    const int ncta = cluster ? 2 * std::min(tc.n_tiles, tc.num_sms / 2) : std::min(tc.n_tiles, tc.num_sms);
+    const int ncta = 2 * std::min(tc.n_tiles, tc.num_sms / 2);
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
     cfg.gridDim = dim3(ncta);
@@ -745,7 +1051,7 @@ int launch_vis_cost_tc(const Params& p, const TrackStore& ts, const Frame& f, in
     cfg.stream = st;
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = cluster ? 2 : 1; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+    attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
     const TcTile* d_tiles = tc.d_tiles;
@@ -756,9 +1062,12 @@ int launch_vis_cost_tc(const Params& p, const TrackStore& ts, const Frame& f, in
     const VisRowMeta* rmeta = tc.rowmeta;
     const float* cb = tc.colb;
     const unsigned int* cv = tc.colvalid;
+    int ucols = tc.cstep;
     void* args[] = {(void*)&mA, (void*)&mB, (void*)&p, (void*)&ts, (void*)&f, (void*)&d_tiles, (void*)&n_tiles,
                     (void*)&d_n_tiles, (void*)&cmeta, (void*)&cgeo, (void*)&rmeta, (void*)&cb, (void*)&cv};
-    e = cudaLaunchKernelExC(&cfg, fn, args);
+    void* args_sa[] = {(void*)&mA, (void*)&mB, (void*)&p, (void*)&ts, (void*)&f, (void*)&d_tiles, (void*)&n_tiles,
+                       (void*)&d_n_tiles, (void*)&ucols, (void*)&cmeta, (void*)&cgeo, (void*)&rmeta, (void*)&cb, (void*)&cv};
+    e = cudaLaunchKernelExC(&cfg, fn, stationary ? args_sa : args);
     if (e != cudaSuccess) return (int)e;
     note_launch();
   }

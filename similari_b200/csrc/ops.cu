@@ -234,13 +234,9 @@ int sb200_visual_cost_matrix(int32_t visual_kind, float threshold, const float* 
   }
   if (tc.use_tc) {
     std::vector<sb::TcTile> tiles;
-    {
-        // SB200_SCREEN = single | multicast (default): CTA organisation of the screen kernel
-        const char* e = getenv("SB200_SCREEN");
-        tc.cluster2 = !(e && !strcmp(e, "single")) && getenv("SB200_SCREEN_SINGLE") == nullptr;
-      }
-    for (int m0 = 0; m0 < m; m0 += (tc.cluster2 ? 256 : 128))
-      for (int c0 = 0; c0 < n; c0 += 256) tiles.push_back(sb::TcTile{0, m0, c0, 0});
+    tc.cstep = sb::vis_screen_ucols(p.d8, tc.num_sms, 1, &m, &n, 1);
+    for (int m0 = 0; m0 < m; m0 += 256)
+      for (int c0 = 0; c0 < n; c0 += tc.cstep) tiles.push_back(sb::TcTile{0, m0, c0, 0});
     tc.n_tiles = (int)tiles.size();
     tc.d_tiles = sc.upload(tiles.data(), tiles.size());
     tc.a_rows = m;

@@ -220,10 +220,11 @@ void launch_own_area(const Frame& f, int n_scenes, int max_m, const float* d_box
 // dst (device) <- src (device alias of mapped pinned host memory), bytes a multiple of 4; a kernel instead of a DMA
 void launch_pull(void* dst, const void* src, size_t bytes, cudaStream_t st);
 // Per-frame tables built on the device: scene descriptors (request half from `req`, a device alias of mapped pinned host
-// memory; store half from d_n_tracks / ts.arena_top), the tile list of the tensor-core visual cost kernel (mstep = 128 or
-// 256 candidate rows per tile, 0: none) and the frame scalars; also zeroes the `n_zero` ints at `zero` (list counters, status).
-// cstep: feature rows per column tile (256 for the screen; (256 / K) * K for the dense kernel, which also gets ws_off /
-// blk_off / slab_off and one metadata slab per column tile instead of 128-padded columns)
+// memory; store half from d_n_tracks / ts.arena_top), the tile list of the tensor-core visual cost kernel (mstep = 256
+// candidate rows per entry: a 2-CTA cluster's pair of 128-row tiles; 0: none) and the frame scalars; also zeroes the
+// `n_zero` ints at `zero` (list counters, status).
+// cstep: feature rows per entry (the screen: vis_screen_ucols(); (256 / K) * K for the dense kernel, which also gets
+// ws_off / blk_off / slab_off and one metadata slab per column tile instead of 128-padded columns)
 void launch_frame_setup(const Params& p, const TrackStore& ts, const Frame& f, const SceneReq* req, int n_scenes,
                         const int* d_n_tracks, int mstep, int cstep, bool dense, TcTile* tiles, FrameDyn* dyn, int* zero,
                         int n_zero, cudaStream_t st);
@@ -237,8 +238,7 @@ struct TcArgs {
   int max_init_done;   // the frame's setup kernel already reset scene_max
   int colmeta_done;    // the column metadata of the screen was launched by the caller (side stream)  // tensor-core screen resources (all null / 0 when the dense exact kernel is used)
   bool use_tc;
-  bool cluster2;   // tiles describe candidate-tile PAIRS processed by 2-CTA clusters (multicast B loads)
-  const TcTile* d_tiles;
+  const TcTile* d_tiles;  // candidate-tile PAIRS (m0 step 256) x column ranges of cstep rows, run by 2-CTA clusters
   int n_tiles;            // tiles (stateless operators) or an upper bound of them (trackers: the count is d_n_tiles[0])
   const int* d_n_tiles;   // device-side tile count (null: n_tiles is exact)
   long long a_rows, b_rows;
@@ -253,7 +253,9 @@ struct TcArgs {
   int max_rows;          // max over the scenes of nb * K
   // ---- dense weight-sum path (mode 2)
   bool dense;            // run launch_vis_dense instead of the screen
-  int cstep;             // feature rows per column tile: (256 / K) * K, so that no track straddles two tiles
+  // feature rows per entry of d_tiles: dense, (256 / K) * K, so that no track straddles two tiles; screen,
+  // vis_screen_ucols()
+  int cstep;
   int max_blocks;        // upper bound of nb over the scenes
   int n_slabs_ub;        // upper bound of the 256-column metadata slabs of the frame
   void* ws;              // weight sums {S~, per-observation error bound} per (block, candidate), packed as half2
@@ -307,6 +309,9 @@ int launch_vote_masks(const Params& p, const TrackStore& ts, const Frame& f, int
 // screen metadata of the stored feature rows (needs the frame tables and the store, not the candidates)
 void launch_vis_colmeta(const Params& p, const TrackStore& ts, const Frame& f, int n_scenes, int max_n, const TcArgs& tc,
                         cudaStream_t st);
+// feature rows per work unit of the screen (TcArgs::cstep), from each scene's candidates m[s] and (an upper bound of) its
+// arena blocks nb[s]
+int vis_screen_ucols(int d8, int num_sms, int n_scenes, const int* m, const int* nb, int K);
 int launch_vis_cost_tc(const Params& p, const TrackStore& ts, const Frame& f, int n_scenes, int max_n, const TcArgs& tc,
                        int phase, cudaStream_t st);
 // materialises the dense visual matrix of the sparse scenes (operators / debugging only)
