@@ -264,9 +264,29 @@ int sb200_kalman_update(float pos_weight, float vel_weight, const float* in30, c
 int sb200_own_area_shares(const float* boxes, int32_t n, float* out, int32_t device);
 
 /* nms (src/utils/nms.rs:32-72): scores NULL or NaN entries == None; out_idx = kept input indices in rank order;
- * returns kept count or negative status. */
+ * returns kept count or negative status.  The one-set case of sb200_nms_batch; at most 1,638,400 boxes
+ * (SB200_ERR_CAPACITY above: the suppressed-box bitmap, ceil(n / 64) * 8 bytes, must fit in 200 KB of shared memory). */
 int64_t sb200_nms(const float* boxes, const float* scores, int32_t n, float nms_threshold, float score_threshold,
                   int32_t has_score_threshold, int32_t* out_idx, int32_t device);
+/* nms (src/utils/nms.rs:32-72) applied independently to each of n_sets sets; set s = rows [offsets[s], offsets[s+1]).
+ * keep_idx[offsets[s] .. offsets[s] + keep_counts[s]) = kept row indices RELATIVE to the set, in rank order; the rest of
+ * the set's range = -1.  keep_mask (optional) [total] = 1 for kept rows, input order.  scores NULL or NaN == None.
+ * Returns the total kept count or a negative status. Host pointers; offsets[n_sets + 1] host.
+ * Checks, before anything is launched or written: n_sets >= 0, offsets[0] == 0, offsets non-decreasing, keep_counts
+ * non-NULL when n_sets > 0 and boxes / keep_idx non-NULL when the total is above 0 (else SB200_ERR_INVALID); a CUDA
+ * device (SB200_ERR_CUDA); every set within sb200_nms's limit (SB200_ERR_CAPACITY, naming the set).  Empty sets and
+ * n_sets == 0 are valid.  All sets run in one fixed sequence of kernel launches, whatever their number. */
+int64_t sb200_nms_batch(int32_t n_sets, const int32_t* offsets, const float* boxes, const float* scores,
+                        float nms_threshold, float score_threshold, int32_t has_score_threshold,
+                        int32_t* keep_idx, int32_t* keep_counts, uint8_t* keep_mask, int32_t device);
+/* The same with boxes / scores / keep_idx / keep_counts / keep_mask as DEVICE pointers, enqueued on cuda_stream (NULL:
+ * the legacy default stream); offsets stays a host pointer and may be reused as soon as the call returns.  Returns after
+ * the enqueue (0 or a negative status); no host synchronisation, except that a call waits when eight earlier calls on
+ * the device still have the copy of their (pinned) set tables queued.  The workspace is allocated and freed
+ * stream-ordered on cuda_stream. */
+int sb200_nms_batch_device(int32_t n_sets, const int32_t* offsets, const float* boxes, const float* scores,
+                           float nms_threshold, float score_threshold, int32_t has_score_threshold,
+                           int32_t* keep_idx, int32_t* keep_counts, uint8_t* keep_mask, int32_t device, void* cuda_stream);
 
 /* ---- multi-GPU: the one exchange step of the scene-sharded path (csrc/comm.cu) ----
  * Scenes are independent and track state is sticky per GPU (rank = scene shard), so N GPUs run N independent trackers; the

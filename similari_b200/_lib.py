@@ -84,6 +84,7 @@ EXPORTS = [
     "sb200_predict_batch_async", "sb200_sync", "sb200_frames_in_flight", "sb200_work_counters", "sb200_launch_count",
     "sb200_set_feature_dim", "sb200_comm_unique_id", "sb200_comm_create", "sb200_comm_destroy", "sb200_shard_scatter",
     "sb200_shard_gather", "sb200_wasted_history", "sb200_host_counters", "sb200_set_stream_join", "sb200_stream_join",
+    "sb200_nms_batch", "sb200_nms_batch_device",
 ]
 
 
@@ -144,6 +145,8 @@ def lib():
         "sb200_kalman_predict": (C.c_int, [f32, f32, vp, i32, vp, i32]),
         "sb200_kalman_update": (C.c_int, [f32, f32, vp, vp, i32, vp, i32]),
         "sb200_nms": (i64, [vp, vp, i32, f32, f32, i32, vp, i32]),
+        "sb200_nms_batch": (i64, [i32, vp, vp, vp, f32, f32, i32, vp, vp, vp, i32]),
+        "sb200_nms_batch_device": (C.c_int, [i32, vp, vp, vp, f32, f32, i32, vp, vp, vp, i32, vp]),
         "sb200_own_area_shares": (C.c_int, [vp, i32, vp, i32]),
         "sb200_host_alloc": (vp, [C.c_size_t]),
         "sb200_host_free": (None, [vp]),

@@ -525,5 +525,18 @@ def nms(detections, nms_threshold, score_threshold):
     return [detections[i][0] for i in idx]
 
 
+def nms_batch(detections_by_scene, nms_threshold, score_threshold):
+    """`nms` of every scene in one GPU call: {scene_id: [(Universal2DBox, score or None), ...]} -> {scene_id: kept boxes
+    in rank order}.  An extension with no PyO3 counterpart in the reference; for each scene the result equals
+    nms(detections_by_scene[scene_id], nms_threshold, score_threshold)."""
+    scenes = list(detections_by_scene.keys())
+    dets = [d for s in scenes for d in detections_by_scene[s]]
+    offsets = np.cumsum([0] + [len(detections_by_scene[s]) for s in scenes])
+    boxes = np.array([b._row() for b, _ in dets], dtype=np.float32).reshape(-1, 6)
+    scores = np.array([math.nan if s is None else s for _, s in dets], dtype=np.float32)
+    kept = engine.nms_batch(boxes, scores, offsets, nms_threshold, score_threshold)
+    return {s: [detections_by_scene[s][i][0] for i in k] for s, k in zip(scenes, kept)}
+
+
 def version():
     return "0.26.12-b200"

@@ -358,8 +358,6 @@ void launch_frame_sweep(const Params& p, const TrackStore& ts, const Frame& f, i
 // stateless operators
 void launch_kalman_ops(int op, float pw, float vw, const float* in30, const float* boxes, int n, float* out30,
                        cudaStream_t st);
-int launch_nms(const float* d_boxes, const float* d_scores, int n, float nms_thr, float score_thr, int has_score_thr,
-               int* d_out_idx, int* d_out_count, cudaStream_t st);
 
 // shared device helpers
 __device__ __forceinline__ bool compat_ok(const Params& p, unsigned int cand_epoch, unsigned int trk_epoch, float cx,

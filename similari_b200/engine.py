@@ -337,3 +337,34 @@ def nms_indices(boxes, scores, nms_threshold, score_threshold=None, device=0):
     n = check(lib().sb200_nms(ptr(b), ptr(s), len(b), nms_threshold, 0.0 if score_threshold is None else score_threshold,
                               int(score_threshold is not None), ptr(out), device))
     return out[:n].copy()
+
+
+def nms_batch(boxes, scores, offsets, nms_threshold, score_threshold=None, device=0):
+    """sb200_nms_batch: nms of every set s = rows [offsets[s], offsets[s+1]) of `boxes` in one call.  Returns one int32
+    array per set: the kept indices relative to the set, in rank order (what nms_indices returns for the set alone)."""
+    b = _f32(boxes).reshape(-1, 6)
+    offs = np.ascontiguousarray(offsets, dtype=np.int32)
+    if offs.ndim != 1 or len(offs) == 0 or int(offs[-1]) != len(b):
+        raise ValueError("offsets needs n_sets + 1 entries ending at the number of boxes")
+    s = _f32(scores) if scores is not None else None
+    if s is not None and len(s) != len(b):
+        raise ValueError("scores and boxes differ in length")
+    n_sets = len(offs) - 1
+    idx = np.empty(max(1, len(b)), np.int32)
+    counts = np.zeros(max(1, n_sets), np.int32)
+    check(lib().sb200_nms_batch(n_sets, ptr(offs), ptr(b), ptr(s), nms_threshold,
+                                0.0 if score_threshold is None else score_threshold, int(score_threshold is not None),
+                                ptr(idx), ptr(counts), None, device))
+    return [idx[offs[i]: offs[i] + counts[i]].copy() for i in range(n_sets)]
+
+
+def nms_batch_device(offsets, d_boxes, d_scores, nms_threshold, score_threshold, d_keep_idx, d_keep_counts, d_keep_mask=0,
+                     stream=0, device=0):
+    """sb200_nms_batch_device: d_* are raw device addresses (0 == NULL), `stream` a cudaStream_t (0: the legacy default
+    stream).  Stream-ordered: returns as soon as the work is enqueued on `stream`."""
+    offs = np.ascontiguousarray(offsets, dtype=np.int32)
+    vp = lambda a: C.c_void_p(a) if a else None  # noqa: E731
+    check(lib().sb200_nms_batch_device(len(offs) - 1, ptr(offs), vp(d_boxes), vp(d_scores), nms_threshold,
+                                       0.0 if score_threshold is None else score_threshold,
+                                       int(score_threshold is not None), vp(d_keep_idx), vp(d_keep_counts),
+                                       vp(d_keep_mask), device, vp(stream)))
