@@ -137,6 +137,7 @@ int make_params(const sb200_options& o, sb::Params* out) {
     p.visual_threshold = o.visual_threshold;
     p.feature_dim = o.feature_dim;
     p.d8 = (o.feature_dim + 7) / 8 * 8;
+    p.vis_rel_err = sb::screen_rel_err(o.feature_dim);
     p.max_obs = o.visual_max_observations;
     p.min_votes = o.visual_min_votes;
     p.min_track_length = o.visual_minimal_track_length;
@@ -1418,6 +1419,7 @@ int sb200_set_feature_dim(sb200_tracker* t, int32_t feature_dim) {
   // no track holds a feature yet (obs_hasf == 0 everywhere): the feature arena is simply re-created for the new row size
   t->P.feature_dim = feature_dim;
   t->P.d8 = (feature_dim + 7) / 8 * 8;
+  t->P.vis_rel_err = sb::screen_rel_err(feature_dim);
   t->opts.feature_dim = feature_dim;
   t->b_feat.release(); t->b_feat_bf16.release(); t->f_cbf162[0].release(); t->f_cbf162[1].release();
   t->ts.feat = nullptr; t->ts.feat_bf16 = nullptr;

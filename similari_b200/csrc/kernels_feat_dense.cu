@@ -10,7 +10,7 @@
 //
 //   1. vis_wsum_kernel  : C~ = A B^T on the tensor cores (wgmma BF16, the same TMA / mbarrier pipeline as the screen).  The
 //                         epilogue turns every accumulator into an approximate distance d~ with a rigorous error bound
-//                         (BF16 operand rounding, kScreenRelErr), sums the observations of a track -- the column tiles are
+//                         (BF16 operand rounding, screen_rel_err), sums the observations of a track -- the column tiles are
 //                         cut at track boundaries -- and stores {S~(q,t), bound} once per (candidate, track): 8 B per
 //                         3 * 512 MACs.  Elements that can be the scene's maximal distance (needed exactly: it is best.rs's
 //                         max_dist) are appended to a short list, found with a lower bound sampled beforehand.
@@ -23,8 +23,11 @@
 //                         worth computing exactly, so assignments stay bit-identical to the CPU reference.
 //
 // Preconditions checked on the device per scene (else dense_bad -> the exact SIMT kernels take the scene): the exact max_dist
-// passes the threshold (then every entry does), the lists did not overflow.  Spatio-temporal constraints switch the path off
-// on the host (they make the matrix sparse in a way only the per-pair gate knows).
+// passes the threshold (then every entry does), every feature norm is in the range of dense_norm_ok, the lists did not
+// overflow.
+// The final refinement also sends a scene to the exact kernels when one of its exact values is cut by the threshold.
+// Spatio-temporal constraints switch the path off on the host (they make the matrix sparse in a way only the per-pair gate
+// knows).
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -41,10 +44,18 @@
 namespace sb {
 
 // error of x~ = |a|^2 + |b|^2 - 2 dot~ against the reference's f32 squared distance, relative to (|a|^2 + |b|^2):
-// 2 E |a||b| <= E (|a|^2 + |b|^2) for the BF16 dot product, plus 2e-4 for the f32 roundings of the norms, of x~ itself and
-// of the reference's own 512-term summation.  Cosine: |cos~ - cos| <= E + 2e-4 absolute.
-constexpr float kDenseErrE = kScreenRelErr + 2e-4f;
-constexpr float kDenseErrC = kScreenRelErr + 2e-4f;
+// 2 E |a||b| <= E (|a|^2 + |b|^2) for the BF16 dot product (E = p.vis_rel_err, screen_rel_err), plus 2e-4 for the f32
+// roundings of the norms, of x~ itself and of the reference's own 512-term summation.  Cosine: |cos~ - cos| <= E + 2e-4
+// absolute.
+__device__ __forceinline__ float dense_err(const Params& p) { return p.vis_rel_err + 2e-4f; }
+
+// The bounds above hold for finite operands whose squared norms stay below FLT_MAX / 4 (then neither |a|^2 + |b|^2 nor
+// 2 dot~ overflows) and, under cosine, are not zero.  A scene with any other feature (a NaN or infinite component, a zero
+// vector under cosine, an overflowing norm) goes to the exact kernels: its approximate distances bound nothing, and a
+// NaN among them would poison the order-preserving row and column maxima of the selection.
+__device__ __forceinline__ bool dense_norm_ok(const Params& p, float n2) {
+  return n2 <= 0.25f * 3.402823466e38f && (p.visual_kind != 1 || n2 > 0.0f);
+}
 
 constexpr int DS_STAGES = 4;
 constexpr int DS_STAGE_BYTES = TC_A_BYTES + TC_B_BYTES;   // A tile (128 x 64 bf16) + B tile (256 x 64 bf16, half from each CTA)
@@ -227,7 +238,7 @@ vis_wsum_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
         erowc[hr] = rm.rowk;   // |a|^2 (euclidean) or 1 / |a| (cosine)
         eg[hr] = h.det_base + m;
         // an element can be the scene's maximal distance only above the sampled lower bound minus the error bound
-        float T = COSINE ? h.l0 - kDenseErrC : h.l0 - kDenseErrE * (erowc[hr] + h.scmax);
+        float T = COSINE ? h.l0 - dense_err(p) : h.l0 - dense_err(p) * (erowc[hr] + h.scmax);
         if (!(m < h.m && rm.ok)) T = finf;
         eTd[hr] = COSINE ? T : (T > 0.0f ? T * rsqrt_approx(T) * (1.0f - 1e-6f) : -1.0f);   // sqrt(T), a hair low
       }
@@ -251,10 +262,10 @@ vis_wsum_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
       auto flush = [&](int col) {
         const float cmx = gcmax[col];
         float del;
-        if (COSINE) del = kDenseErrC;
+        if (COSINE) del = dense_err(p);
         else {
           const float rc = rowc + cmx;
-          const float e = kDenseErrE * rc;
+          const float e = dense_err(p) * rc;
           // |d - d~| <= |d^2 - d~^2| / (d + d~) <= e / d~ always, <= 0.536 e / d~ once d~^2 >= 4 e (then d >= 0.866 d~),
           // and <= sqrt(e) always.  Approximate reciprocal / rsqrt (2 ulp) under a 1.0001 safety factor; 1e-6 (rc + 1) >=
           // 1e-6 sqrt(rc) covers the rsqrt approximation of d~ itself.
@@ -370,7 +381,8 @@ vis_wsum_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
 // the block record of the selection kernel (owner, valid observations).  Same validity rule as vis_meta_kernel.
 __global__ void vis_dense_meta_kernel(Params p, TrackStore ts, Frame f, int max_blocks, int cstep, DenseTrackMeta* tmeta,
                                       int2* rowinfo, float* slab_colc, float* slab_cmax, float* slab_ktf,
-                                      unsigned int* slab_vmask, unsigned int* slab_bmask, float* scene_cmax) {
+                                      unsigned int* slab_vmask, unsigned int* slab_bmask, float* scene_cmax,
+                                      int* dense_bad) {
   const int s = blockIdx.y;
   const SceneDesc sc = f.scenes[s];
   const int K = p.max_obs;
@@ -398,6 +410,7 @@ __global__ void vis_dense_meta_kernel(Params p, TrackStore ts, Frame f, int max_
           if (valid) {
             frow_of[ph] = (int)frow;
             const float nb2 = ts.fnorm2[frow];
+            if (!dense_norm_ok(p, nb2)) dense_bad[s] = 1;
             colc[ph] = p.visual_kind == 1 ? rsqrtf(nb2) : nb2;
             cmax = fmaxf(cmax, nb2);
             tm.kt += 1;
@@ -442,7 +455,8 @@ __global__ void vis_dense_rowmeta_kernel(Params p, Frame f, VisRowMeta* rowmeta)
 // up to 64 candidates x 64 valid feature rows, plain f32 dot products.  Any real element bounds the maximum from below, so
 // whatever the sample is, the candidates the weight-sum kernel keeps (x~ >= l0 - bound) contain the true maximum.
 constexpr int DSAMP = 32;
-__global__ void __launch_bounds__(256) vis_dense_sample_kernel(Params p, TrackStore ts, Frame f, const int2* rowinfo, float* scene_l0) {
+__global__ void __launch_bounds__(256) vis_dense_sample_kernel(Params p, TrackStore ts, Frame f, const int2* rowinfo, float* scene_l0,
+                                                                int* dense_bad) {
   __shared__ int s_q[DSAMP], s_r[DSAMP];
   __shared__ int s_nq, s_nr;
   __shared__ float s_w[8];
@@ -453,6 +467,10 @@ __global__ void __launch_bounds__(256) vis_dense_sample_kernel(Params p, TrackSt
   if (tid == 0) { s_nq = 0; s_nr = 0; }
   __syncthreads();
   const int rows = sc.nb * K;
+  for (int i = tid; i < sc.m; i += 256) {   // the candidate side of the dense_norm_ok rule
+    const int g = sc.det_base + i;
+    if ((f.c_flags[g] & 2) && !dense_norm_ok(p, f.c_norm2[g])) dense_bad[s] = 1;
+  }
   if (tid < DSAMP) {
     if (sc.m > 0) {
       const int m = (int)(((long long)tid * sc.m) / DSAMP);
@@ -517,7 +535,8 @@ __global__ void __launch_bounds__(SEL_T) vis_dense_select_kernel(Params p, Frame
   // preconditions of the dense result
   const unsigned int um = f.scene_max[s];
   const float maxd = __uint_as_float((um & 0x80000000u) ? (um & 0x7fffffffu) : ~um);
-  // reasons: 1 an entry the threshold cuts (set by the max refinement), 2 max-candidate list overflow, 4 no maximum found
+  // reasons: 1 an entry the threshold cuts (set by the max refinement and the final refinement) or a feature norm outside
+  // dense_norm_ok (set by the metadata and sample kernels), 2 max-candidate list overflow, 4 no maximum found
   const int reason = (max_nan[s] != 0 ? 1 : 0) | (maxc_cnt[s] > sc.vis_lcap ? 2 : 0) | (!(maxd >= 0.0f) ? 4 : 0);
   if (tid == 0) {   // diagnostics of the frame (SB200_TRACE): fallback reasons, list lengths
     if (reason & 1) atomicAdd(&dbg_counts[0], 1);
@@ -678,11 +697,12 @@ int launch_vis_dense(const Params& p, const TrackStore& ts, const Frame& f, int 
   if (tc.max_blocks > 0) {
     dim3 grid((tc.max_blocks + 127) / 128, n_scenes);
     vis_dense_meta_kernel<<<grid, 128, 0, st>>>(p, ts, f, tc.max_blocks, tc.cstep, tc.tmeta, tc.rowinfo, tc.slab_colc, tc.slab_cmax,
-                                                tc.slab_ktf, tc.slab_vmask, tc.slab_bmask, tc.scene_cmax);
+                                                tc.slab_ktf, tc.slab_vmask, tc.slab_bmask, tc.scene_cmax,
+                                                tc.dense_bad);
     note_launch();
   }
   vis_dense_rowmeta_kernel<<<(f.total + 255) / 256, 256, 0, st>>>(p, f, tc.rowmeta);
-  vis_dense_sample_kernel<<<n_scenes, 256, 0, st>>>(p, ts, f, tc.rowinfo, tc.scene_l0);
+  vis_dense_sample_kernel<<<n_scenes, 256, 0, st>>>(p, ts, f, tc.rowinfo, tc.scene_l0, tc.dense_bad);
   note_launch(2);
   if (tc.ev_screen0) cudaEventRecord(tc.ev_screen0, st);
   {

@@ -159,7 +159,7 @@ vis_screen_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
       const VisColMeta* gmeta = S.meta[ms];
       const TcHdr h = S.hdr[ms];
       const float* gcolb = S.colb[ms];
-      // Screen test, E = kScreenRelErr bounds the BF16 operand rounding (|dot~ - dot| <= E |a||b| <= E (|a|^2 + |b|^2) / 2):
+      // Screen test, E = p.vis_rel_err (screen_rel_err) bounds the BF16 operand rounding (|dot~ - dot| <= E |a||b| <= E (|a|^2 + |b|^2) / 2):
       //   cosine: cos >= thr possible   <=>  dot~ >= (thr - 1e-5 - E) |a| * |b|                                = rowk * colb
       //   euclid: d^2 <= thr^2 possible <=>  dot~ >= 0.5 ((1 - 1e-5 - E)(|a|^2 + |b|^2) - thr^2 (1 + 1e-5))   = rowk + colb
       float rowk[2];
@@ -908,7 +908,7 @@ __global__ void vis_meta_kernel(Params p, TrackStore ts, Frame f, int n_scenes, 
         cm.outcol = n * K + k_of;
         const bool valid = (ts.feat_cnt[ti] >= p.min_track_length) && ((unsigned int)p.max_idle_epochs >= delta);
         const float nb = ts.fnorm2[frow];
-        cm.colb = p.visual_kind == 1 ? sqrtf(nb) : 0.5f * nb * (1.0f - 1e-5f - kScreenRelErr);
+        cm.colb = p.visual_kind == 1 ? sqrtf(nb) : 0.5f * nb * (1.0f - 1e-5f - p.vis_rel_err);
         cm.row = valid ? (int)frow : -1;
       } else {
         // dead physical slot -> owns the dead_rank-th logical column without a feature (written as None)
@@ -944,8 +944,8 @@ __global__ void vis_rowmeta_kernel(Params p, Frame f, VisRowMeta* rowmeta) {
   VisRowMeta rm;
   rm.ok = (f.c_flags[g] & 2) ? 1 : 0;
   const float thr = p.visual_threshold;
-  if (p.visual_kind == 1) rm.rowk = (thr - 1e-5f - kScreenRelErr) * sqrtf(na);
-  else rm.rowk = 0.5f * (na * (1.0f - 1e-5f - kScreenRelErr) - thr * thr * (1.0f + 1e-5f));
+  if (p.visual_kind == 1) rm.rowk = (thr - 1e-5f - p.vis_rel_err) * sqrtf(na);
+  else rm.rowk = 0.5f * (na * (1.0f - 1e-5f - p.vis_rel_err) - thr * thr * (1.0f + 1e-5f));
   rowmeta[g] = rm;
 }
 
@@ -1019,7 +1019,8 @@ int launch_vis_cost_tc(const Params& p, const TrackStore& ts, const Frame& f, in
                        int phase, cudaStream_t st) {
   if (tc.n_tiles == 0) return 0;
   if (phase == 1) {
-    int rc = launch_vis_refine(p, ts, f, n_scenes, nullptr, st);
+    // dense path: an exact value the threshold cuts (a NaN or infinite distance) voids the scene's dense result too
+    int rc = launch_vis_refine(p, ts, f, n_scenes, tc.dense ? tc.dense_bad : nullptr, st);
     if (tc.ev_refine1) cudaEventRecord(tc.ev_refine1, st);
     return rc;
   }

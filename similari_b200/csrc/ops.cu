@@ -153,6 +153,7 @@ int sb200_visual_cost_matrix(int32_t visual_kind, float threshold, const float* 
   p.visual_threshold = threshold;
   p.feature_dim = d;
   p.d8 = (d + 7) / 8 * 8;
+  p.vis_rel_err = sb::screen_rel_err(d);
   p.max_obs = 1;
   p.min_track_length = 0;
   // track side: norms through the candidate-norm kernel on a scratch frame

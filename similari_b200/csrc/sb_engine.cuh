@@ -24,6 +24,21 @@ constexpr int kMaxObs = 8;  // visual_max_observations supported on device (refe
 constexpr int kStateStride = 32;   // floats per Kalman state row in the tracker's store (kStateFloats padded to 128 bytes)
 constexpr int kMaxHist = 64;  // box history kept per track on the device (history_length above it, or 0 = unlimited, is capped)
 
+// BF16 operand rounding bound on a dot product of width d, relative to ||a|| ||b||.  BF16 keeps 8 significant bits;
+// round-to-nearest leaves a relative error of at most u = 2^-8 per operand (a value just above a power of two sits half a
+// 2^-7 spacing from its neighbours).  Two rounded operands: |a~ b~ - a b| <= (2u + u^2) |a b|, hence by Cauchy-Schwarz
+//   |dot~ - dot| <= (2^-7 + 2^-16) * sum|a_i b_i| <= (2^-7 + 2^-16) * ||a|| ||b||.
+// Products of BF16 operands are exact in fp32.  The fp32 accumulation of the tensor cores is modelled as one truncation per
+// addition, at most d * 2^-23 relative to sum|a_i b_i|; that model has not been measured on the H100.  The slack is
+// 2.1 * 2^-8, which covers 2^-7 + 2^-16 + d * 2^-23 up to d = 3148, and that sum for wider features.  (1.5 * 2^-8 would
+// cover the rounding errors of real feature vectors, which average out, but not the adversarial worst case -- the screen
+// must never drop a pair the exact metric keeps.)
+inline float screen_rel_err(int d) {
+  const double e = 0x1p-7 + 0x1p-16 + (double)d * 0x1p-23;
+  const float floor_e = 2.1f / 256.0f;
+  return e <= (double)floor_e ? floor_e : (float)(e * (1.0 + 0x1p-20));   // rounded up past the f32 conversion
+}
+
 struct Params {  // immutable per tracker, passed by value to kernels
   int kind, positional_kind, visual_kind;
   float iou_threshold, min_confidence, pos_weight, vel_weight;
@@ -32,6 +47,7 @@ struct Params {  // immutable per tracker, passed by value to kernels
   int constraint_epochs[kMaxConstraints];
   float constraint_max_dist[kMaxConstraints];
   float visual_threshold;
+  float vis_rel_err;  // screen_rel_err(feature_dim): the BF16 slack of the tensor-core visual kernels
   int feature_dim, d8, max_obs, min_votes, min_track_length;
   int vote_vis_cap;   // visual entries per scene the sparse voting kernel keeps in shared memory (0: kVoteVisCap)
   float min_area, min_quality_use, min_quality_collect, min_own_use, min_own_collect;

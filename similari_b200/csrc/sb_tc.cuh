@@ -180,14 +180,4 @@ __device__ __forceinline__ void tc_consume_tile(float* acc, unsigned char* stage
   if (prev >= 0) release(prev);
 }
 
-// BF16 operand rounding bound on a dot product.  BF16 keeps 8 significant bits; round-to-nearest leaves a relative error
-// of at most u = 2^-8 per operand (a value just above a power of two sits half a 2^-7 spacing from its neighbours).
-// Two rounded operands: |a~ b~ - a b| <= (2u + u^2) |a b|, hence by Cauchy-Schwarz
-//   |dot~ - dot| <= (2^-7 + 2^-16) * sum|a_i b_i| <= (2^-7 + 2^-16) * ||a|| ||b||.
-// The fp32 accumulation of the tensor cores adds at most D * 2^-24 relative (truncation; D <= 4096: 2^-12).  Together
-// 2^-7 + 2^-16 + 2^-12 = 2.066 * 2^-8 <= kScreenRelErr = 2.1 * 2^-8.  (1.5 * 2^-8 would cover the rounding errors of real
-// feature vectors, which average out, but not the adversarial worst case -- the screen must never drop a pair the exact
-// metric keeps.)
-constexpr float kScreenRelErr = 2.1f / 256.0f;
-
 }  // namespace sb
