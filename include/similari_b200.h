@@ -256,6 +256,31 @@ int sb200_kalman_initiate(float pos_weight, float vel_weight, const float* boxes
 int sb200_kalman_predict(float pos_weight, float vel_weight, const float* in30, int32_t n, float* out30, int32_t device);
 int sb200_kalman_update(float pos_weight, float vel_weight, const float* in30, const float* boxes, int32_t n,
                         float* out30, int32_t device);
+/* Universal2DBoxKalmanFilter::distance (kalman_2d_box.rs:150-170): out[i] = squared Mahalanobis distance of boxes[i]
+ * from states30[i] (vel_weight is accepted for symmetry and unused: the distance reads the position weight only). */
+int sb200_kalman_distance(float pos_weight, float vel_weight, const float* states30, const float* boxes, int32_t n,
+                          float* out, int32_t device);
+/* Point2DKalmanFilter (src/utils/kalman/kalman_2d_point.rs:51-137) on n packed 12-float states: mean (x, y, vx, vy),
+ * then for i in {x, y} the covariance block P[i][i], P[i][i+2], P[i+2][i], P[i+2][i+2].  points2 = (x, y) pairs. */
+int sb200_point_kalman_initiate(float pos_weight, float vel_weight, const float* points2, int32_t n, float* states12,
+                                int32_t device);
+int sb200_point_kalman_predict(float pos_weight, float vel_weight, const float* in12, int32_t n, float* out12,
+                               int32_t device);
+int sb200_point_kalman_update(float pos_weight, float vel_weight, const float* in12, const float* points2, int32_t n,
+                              float* out12, int32_t device);
+int sb200_point_kalman_distance(float pos_weight, float vel_weight, const float* states12, const float* points2,
+                                int32_t n, float* out, int32_t device);
+/* Universal2DBox::get_vertices (src/utils/bbox.rs:169-171,287-330): out8[n][4][2] f64, angle NaN == 0. */
+int sb200_box_vertices(const float* boxes, int32_t n, double* out8, int32_t device);
+/* sutherland_hodgman_clip_py / intersection_area_py (src/utils/clipping/clipping_py.rs:29-46) of n (subject, clipping)
+ * box pairs: out_vertices[n][16][2] f64 = the clipped ring without its closing repeat (slots past the count are 0),
+ * out_counts[n] = its vertex count, out_areas[n] = its unsigned area.  SB200_ERR_CAPACITY, with no output written, when a
+ * pair's clip would need more than 16 vertices (the reference's Vec has no bound). */
+int sb200_clip_polygons(const float* subjects, const float* clippings, int32_t n, double* out_vertices,
+                        int32_t* out_counts, double* out_areas, int32_t device);
+/* out_mn[i][j] = intersection_area_py(a[i], b[j]) (f64; no too_far and no IoU gate).  SB200_ERR_CAPACITY, with no output
+ * written, as for sb200_clip_polygons. */
+int sb200_intersection_areas(const float* a, int32_t m, const float* b, int32_t n, double* out_mn, int32_t device);
 /* exclusively_owned_areas + exclusively_owned_areas_normalized_shares (src/utils/clipping/bbox_own_areas.rs:8-46) for the
  * boxes of ONE scene: out[i] = share of box i that no other box covers, in [0, 1].  The visual trackers call the same
  * kernel themselves when an own-area threshold is set and the request carries no `own_area` column

@@ -84,7 +84,9 @@ EXPORTS = [
     "sb200_predict_batch_async", "sb200_sync", "sb200_frames_in_flight", "sb200_work_counters", "sb200_launch_count",
     "sb200_set_feature_dim", "sb200_comm_unique_id", "sb200_comm_create", "sb200_comm_destroy", "sb200_shard_scatter",
     "sb200_shard_gather", "sb200_wasted_history", "sb200_host_counters", "sb200_set_stream_join", "sb200_stream_join",
-    "sb200_nms_batch", "sb200_nms_batch_device",
+    "sb200_nms_batch", "sb200_nms_batch_device", "sb200_kalman_distance", "sb200_point_kalman_initiate",
+    "sb200_point_kalman_predict", "sb200_point_kalman_update", "sb200_point_kalman_distance", "sb200_box_vertices",
+    "sb200_clip_polygons", "sb200_intersection_areas",
 ]
 
 
@@ -144,6 +146,14 @@ def lib():
         "sb200_kalman_initiate": (C.c_int, [f32, f32, vp, i32, vp, i32]),
         "sb200_kalman_predict": (C.c_int, [f32, f32, vp, i32, vp, i32]),
         "sb200_kalman_update": (C.c_int, [f32, f32, vp, vp, i32, vp, i32]),
+        "sb200_kalman_distance": (C.c_int, [f32, f32, vp, vp, i32, vp, i32]),
+        "sb200_point_kalman_initiate": (C.c_int, [f32, f32, vp, i32, vp, i32]),
+        "sb200_point_kalman_predict": (C.c_int, [f32, f32, vp, i32, vp, i32]),
+        "sb200_point_kalman_update": (C.c_int, [f32, f32, vp, vp, i32, vp, i32]),
+        "sb200_point_kalman_distance": (C.c_int, [f32, f32, vp, vp, i32, vp, i32]),
+        "sb200_box_vertices": (C.c_int, [vp, i32, vp, i32]),
+        "sb200_clip_polygons": (C.c_int, [vp, vp, i32, vp, vp, vp, i32]),
+        "sb200_intersection_areas": (C.c_int, [vp, i32, vp, i32, vp, i32]),
         "sb200_nms": (i64, [vp, vp, i32, f32, f32, i32, vp, i32]),
         "sb200_nms_batch": (i64, [i32, vp, vp, vp, f32, f32, i32, vp, vp, vp, i32]),
         "sb200_nms_batch_device": (C.c_int, [i32, vp, vp, vp, f32, f32, i32, vp, vp, vp, i32, vp]),

@@ -7,6 +7,7 @@ Objects here are thin: all state lives on the GPU inside `engine.Tracker`.
 from __future__ import annotations
 
 import math
+from collections.abc import Sequence
 from typing import List, Optional, Tuple
 
 import numpy as np
@@ -78,6 +79,13 @@ class Universal2DBox:
 
     def rotate(self, angle):
         self.angle = F32(angle)
+
+    def gen_vertices(self):
+        """Accepted for compatibility: the reference fills a vertex cache that no Python-visible result depends on."""
+
+    def get_vertices(self) -> "Polygon":
+        """src/utils/bbox.rs:685-687: the four vertices (angle None == 0) as a closed Polygon."""
+        return Polygon._from_ring(engine.box_vertices(np.array([self._row()], dtype=np.float32))[0])
 
     def _row(self):
         return [self.xc, self.yc, math.nan if self.angle is None else self.angle, self.aspect, self.height, self.confidence]
@@ -536,6 +544,205 @@ def nms_batch(detections_by_scene, nms_threshold, score_threshold):
     scores = np.array([math.nan if s is None else s for _, s in dets], dtype=np.float32)
     kept = engine.nms_batch(boxes, scores, offsets, nms_threshold, score_threshold)
     return {s: [detections_by_scene[s][i][0] for i in k] for s, k in zip(scenes, kept)}
+
+
+class Polygon:
+    """src/utils/clipping/clipping_py.rs:5-27 `PyPolygon` (a geo::Polygon<f64> without interiors)."""
+
+    def __init__(self, points):
+        self._points = [(float(x), float(y)) for x, y in points]
+
+    @staticmethod
+    def _from_ring(xy) -> "Polygon":
+        # geo::Polygon::new closes the exterior ring: the first coordinate is repeated unless the last already equals it
+        pts = [(float(x), float(y)) for x, y in xy]
+        if pts and pts[0] != pts[-1]:
+            pts.append(pts[0])
+        return Polygon(pts)
+
+    def get_points(self) -> List[Tuple[float, float]]:
+        return list(self._points)
+
+    def __repr__(self):
+        coords = ", ".join(f"Coord {{ x: {x!r}, y: {y!r} }}" for x, y in self._points)
+        return f"PyPolygon(Polygon {{ exterior: LineString([{coords}]), interiors: [] }})"
+
+
+def _clip_one(subject: Universal2DBox, clipping: Universal2DBox):
+    v, n, a = engine.clip_polygons(np.array([subject._row()], dtype=np.float32),
+                                   np.array([clipping._row()], dtype=np.float32))
+    return v[0, : n[0]], float(a[0])
+
+
+def sutherland_hodgman_clip(subject: Universal2DBox, clipping: Universal2DBox) -> Polygon:
+    """src/utils/clipping/clipping_py.rs:29-39 (Universal2DBox::sutherland_hodgman_clip, src/utils/bbox.rs:216-238: a
+    None angle is 0)."""
+    return Polygon._from_ring(_clip_one(subject, clipping)[0])
+
+
+def intersection_area(subject: Universal2DBox, clipping: Universal2DBox) -> float:
+    """src/utils/clipping/clipping_py.rs:41-46: unsigned area of sutherland_hodgman_clip(subject, clipping)."""
+    return _clip_one(subject, clipping)[1]
+
+
+def intersection_areas(subjects, clippings) -> np.ndarray:
+    """intersection_area of every (subjects[i], clippings[j]) pair in one GPU call: an [m][n] float64 matrix.  An
+    extension with no PyO3 counterpart in the reference; element (i, j) equals intersection_area(subjects[i],
+    clippings[j])."""
+    a = np.array([b._row() for b in subjects], dtype=np.float32).reshape(-1, 6)
+    b = np.array([c._row() for c in clippings], dtype=np.float32).reshape(-1, 6)
+    return engine.intersection_areas(a, b)
+
+
+# CHI2INV95 and CHI2_UPPER_BOUND, src/utils/kalman.rs:16-20
+_CHI2INV95 = np.array([3.8415, 5.9915, 7.8147, 9.4877, 11.070, 12.592, 14.067, 15.507, 16.919], dtype=np.float32)
+_CHI2_UPPER = F32(100.0)
+
+
+def _cost(distance, inverted, plain_index):
+    """calculate_cost of the Kalman filters in f32: the non-inverted branch compares with CHI2INV95[plain_index] (4 for
+    the box filter, kalman_2d_box.rs:172-184; 1 for the point filter, kalman_2d_point.rs:139-151), the inverted one
+    with CHI2INV95[4] in both."""
+    d = F32(distance)
+    if not inverted:
+        return float(_CHI2_UPPER if d > _CHI2INV95[plain_index] else d)
+    return float(F32(0.0) if d > _CHI2INV95[4] else _CHI2_UPPER - d)
+
+
+class Universal2DBoxKalmanFilterState:
+    """src/utils/kalman/kalman_2d_box.rs:267-284 `PyUniversal2DBoxKalmanFilterState`.  Holds the packed 30-float state
+    (mean[10], then five 2x2 covariance blocks; DESIGN.md)."""
+
+    __slots__ = ("_st",)
+
+    def __init__(self, st):
+        self._st = st
+
+    def universal_bbox(self) -> Universal2DBox:
+        # TryFrom<KalmanState> for Universal2DBox, src/utils/kalman.rs:72-92: angle None when mean[2] == 0, confidence 1
+        m = self._st
+        return Universal2DBox(m[0], m[1], None if m[2] == 0.0 else m[2], m[3], m[4])
+
+    def bbox(self) -> BoundingBox:
+        return self.universal_bbox().as_ltwh()
+
+
+class Universal2DBoxKalmanFilter:
+    """src/utils/kalman/kalman_2d_box.rs:260-265,286-338 `PyUniversal2DBoxKalmanFilter`.  Each call is one GPU call over one
+    state; for many states use engine.kalman_* on packed arrays."""
+
+    def __init__(self, position_weight=0.05, velocity_weight=0.00625):
+        self._pw, self._vw = float(F32(position_weight)), float(F32(velocity_weight))
+
+    def initiate(self, bbox: Universal2DBox) -> Universal2DBoxKalmanFilterState:
+        return Universal2DBoxKalmanFilterState(engine.kalman_initiate([bbox._row()], self._pw, self._vw)[0])
+
+    def predict(self, state: Universal2DBoxKalmanFilterState) -> Universal2DBoxKalmanFilterState:
+        return Universal2DBoxKalmanFilterState(engine.kalman_predict(state._st, self._pw, self._vw)[0])
+
+    def update(self, state: Universal2DBoxKalmanFilterState, bbox: Universal2DBox) -> Universal2DBoxKalmanFilterState:
+        return Universal2DBoxKalmanFilterState(engine.kalman_update(state._st, [bbox._row()], self._pw, self._vw)[0])
+
+    def distance(self, state: Universal2DBoxKalmanFilterState, bbox: Universal2DBox) -> float:
+        return float(engine.kalman_distance(state._st, [bbox._row()], self._pw, self._vw)[0])
+
+    @staticmethod
+    def calculate_cost(distance, inverted) -> float:
+        return _cost(distance, inverted, 4)
+
+
+class Point2DKalmanFilterState:
+    """src/utils/kalman/kalman_2d_point.rs:237-264 `PyPoint2DKalmanFilterState`.  Holds the packed 12-float state
+    (x, y, vx, vy, then the x and y covariance blocks; DESIGN.md)."""
+
+    __slots__ = ("_st",)
+
+    def __init__(self, st):
+        self._st = st
+
+    def x(self) -> float:
+        return float(self._st[0])
+
+    def y(self) -> float:
+        return float(self._st[1])
+
+
+class Point2DKalmanFilter:
+    """src/utils/kalman/kalman_2d_point.rs:230-234,266-312 `PyPoint2DKalmanFilter`.  Each call is one GPU call over one state."""
+
+    def __init__(self, position_weight=0.05, velocity_weight=0.00625):
+        self._pw, self._vw = float(F32(position_weight)), float(F32(velocity_weight))
+
+    def initiate(self, x, y) -> Point2DKalmanFilterState:
+        return Point2DKalmanFilterState(engine.point_kalman_initiate([[x, y]], self._pw, self._vw)[0])
+
+    def predict(self, state: Point2DKalmanFilterState) -> Point2DKalmanFilterState:
+        return Point2DKalmanFilterState(engine.point_kalman_predict(state._st, self._pw, self._vw)[0])
+
+    def update(self, state: Point2DKalmanFilterState, x, y) -> Point2DKalmanFilterState:
+        return Point2DKalmanFilterState(engine.point_kalman_update(state._st, [[x, y]], self._pw, self._vw)[0])
+
+    def distance(self, state: Point2DKalmanFilterState, x, y) -> float:
+        return float(engine.point_kalman_distance(state._st, [[x, y]], self._pw, self._vw)[0])
+
+    @staticmethod
+    def calculate_cost(distance, inverted) -> float:
+        return _cost(distance, inverted, 1)
+
+
+class Point2DKalmanFilterStates(Sequence):
+    """What Vec2DKalmanFilter.initiate / predict / update return: a read-only sequence of Point2DKalmanFilterState over
+    one packed [n][12] array.  The reference returns a list; indexing, len() and iteration behave the same, and passing
+    the sequence back to Vec2DKalmanFilter hands the packed array to the GPU without touching the elements."""
+
+    __slots__ = ("_a",)
+
+    def __init__(self, a):
+        self._a = a
+
+    def __len__(self):
+        return len(self._a)
+
+    def __getitem__(self, i):
+        if isinstance(i, slice):
+            return Point2DKalmanFilterStates(self._a[i])
+        return Point2DKalmanFilterState(self._a[i])
+
+
+def _pack_points(states) -> np.ndarray:
+    if isinstance(states, Point2DKalmanFilterStates):
+        return states._a
+    return np.array([s._st for s in states], dtype=np.float32).reshape(-1, 12)
+
+
+def _xy(points) -> np.ndarray:
+    return np.array(points, dtype=np.float32).reshape(-1, 2)
+
+
+class Vec2DKalmanFilter:
+    """src/utils/kalman/kalman_2d_point_vec.rs:86-166 `PyVec2DKalmanFilter`: every call is one GPU launch over the whole
+    list of states."""
+
+    def __init__(self, position_weight=0.05, velocity_weight=0.00625):
+        self._pw, self._vw = float(F32(position_weight)), float(F32(velocity_weight))
+
+    def initiate(self, points) -> Point2DKalmanFilterStates:
+        return Point2DKalmanFilterStates(engine.point_kalman_initiate(_xy(points), self._pw, self._vw))
+
+    def predict(self, state) -> Point2DKalmanFilterStates:
+        return Point2DKalmanFilterStates(engine.point_kalman_predict(_pack_points(state), self._pw, self._vw))
+
+    def update(self, state, points) -> Point2DKalmanFilterStates:
+        assert len(state) == len(points), "Lengths of state and points must match"
+        return Point2DKalmanFilterStates(engine.point_kalman_update(_pack_points(state), _xy(points), self._pw, self._vw))
+
+    def distance(self, state, points) -> List[float]:
+        assert len(state) == len(points), "Lengths of state and points must match"
+        return engine.point_kalman_distance(_pack_points(state), _xy(points), self._pw, self._vw).tolist()
+
+    @staticmethod
+    def calculate_cost(distances, inverted) -> List[float]:
+        return [_cost(d, inverted, 1) for d in distances]
 
 
 def version():

@@ -578,6 +578,56 @@ void launch_kalman_ops(int op, float pw, float vw, const float* in30, const floa
   note_launch();
 }
 
+// Universal2DBoxKalmanFilter::distance over n (state, box) pairs
+__global__ void kalman_distance_kernel(float pw, const float* __restrict__ in30, const float* __restrict__ boxes, int n,
+                                       float* __restrict__ out) {
+  int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  float a[kStateFloats];
+  for (int k = 0; k < kStateFloats; ++k) a[k] = in30[(size_t)i * kStateFloats + k];
+  const float* q = boxes + (size_t)i * 6;
+  out[i] = kalman_distance(pw, a, Box{q[0], q[1], q[2], q[3], q[4], q[5]});
+}
+
+void launch_kalman_distance(float pw, const float* in30, const float* boxes, int n, float* out, cudaStream_t st) {
+  if (n == 0) return;
+  kalman_distance_kernel<<<(n + 127) / 128, 128, 0, st>>>(pw, in30, boxes, n, out);
+  note_launch();
+}
+
+// Point2DKalmanFilter over n packed 12-float states, one thread per state.  op: 0 initiate (points -> out12),
+// 1 predict (in12 -> out12), 2 update (in12, points -> out12), 3 distance (in12, points -> out_f32).
+__global__ void point_kalman_kernel(int op, float pw, float vw, const float* __restrict__ in12,
+                                    const float* __restrict__ points, int n, float* __restrict__ out) {
+  int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  float a[kPointStateFloats], b[kPointStateFloats];
+  float x = 0.0f, y = 0.0f;
+  if (points) { x = points[(size_t)i * 2]; y = points[(size_t)i * 2 + 1]; }
+  if (op != 0) {
+    const float4* s4 = reinterpret_cast<const float4*>(in12 + (size_t)i * kPointStateFloats);
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+      const float4 v = s4[k];
+      a[4 * k] = v.x; a[4 * k + 1] = v.y; a[4 * k + 2] = v.z; a[4 * k + 3] = v.w;
+    }
+  }
+  if (op == 3) { out[i] = point_kalman_distance(pw, a, x, y); return; }
+  if (op == 0) point_kalman_initiate(pw, vw, x, y, b);
+  else if (op == 1) point_kalman_predict(pw, vw, a, b);
+  else point_kalman_update(pw, a, x, y, b);
+  float4* o4 = reinterpret_cast<float4*>(out + (size_t)i * kPointStateFloats);
+#pragma unroll
+  for (int k = 0; k < 3; ++k) o4[k] = make_float4(b[4 * k], b[4 * k + 1], b[4 * k + 2], b[4 * k + 3]);
+}
+
+void launch_point_kalman(int op, float pw, float vw, const float* in12, const float* points, int n, float* out,
+                         cudaStream_t st) {
+  if (n == 0) return;
+  point_kalman_kernel<<<(n + 255) / 256, 256, 0, st>>>(op, pw, vw, in12, points, n, out);
+  note_launch();
+}
+
 // ------------------------------------------------------------------------------------------------------------
 // Small per-frame tables (scene descriptors, tile list) are read straight from mapped pinned host memory.
 __global__ void pull_kernel(unsigned int* __restrict__ dst, const unsigned int* __restrict__ src, size_t n4, size_t n1) {

@@ -377,4 +377,135 @@ int sb200_kalman_update(float pw, float vw, const float* in30, const float* boxe
   return kalman_op(2, pw, vw, in30, boxes, n, out30, device);
 }
 
+// Universal2DBoxKalmanFilter::distance, src/utils/kalman/kalman_2d_box.rs:150-170
+int sb200_kalman_distance(float pw, float vw, const float* states30, const float* boxes, int32_t n, float* out,
+                          int32_t device) {
+  (void)vw;   // the distance reads only the position weight (project, :104-120)
+  if (n < 0 || (n > 0 && (!states30 || !boxes || !out))) return ops_fail(SB200_ERR_INVALID, "bad arguments");
+  Scratch sc;
+  int rc = begin(sc, device);
+  if (rc) return rc;
+  if (n == 0) return 0;
+  float* din = sc.upload(states30, (size_t)n * 30);
+  float* db = sc.upload(boxes, (size_t)n * 6);
+  float* dout = sc.alloc<float>(n);
+  if (!din || !db || !dout) return ops_fail(SB200_ERR_CUDA, "cudaMalloc failed");
+  sb::launch_kalman_distance(pw, din, db, n, dout, sc.st);
+  cudaMemcpyAsync(out, dout, (size_t)n * 4, cudaMemcpyDeviceToHost, sc.st);
+  return finish(sc);
+}
+
+// op as launch_point_kalman: 0 initiate, 1 predict, 2 update, 3 distance
+static int point_kalman_op(int op, float pw, float vw, const float* in12, const float* points, int n, float* out,
+                           int device) {
+  const bool need_in = op != 0, need_pts = op != 1;
+  if (n < 0 || (n > 0 && (!out || (need_in && !in12) || (need_pts && !points))))
+    return ops_fail(SB200_ERR_INVALID, "bad arguments");
+  Scratch sc;
+  int rc = begin(sc, device);
+  if (rc) return rc;
+  if (n == 0) return 0;
+  const size_t out_floats = op == 3 ? (size_t)n : (size_t)n * 12;
+  float* din = need_in ? sc.upload(in12, (size_t)n * 12) : nullptr;
+  float* dp = need_pts ? sc.upload(points, (size_t)n * 2) : nullptr;
+  float* dout = sc.alloc<float>(out_floats);
+  if ((need_in && !din) || (need_pts && !dp) || !dout) return ops_fail(SB200_ERR_CUDA, "cudaMalloc failed");
+  sb::launch_point_kalman(op, pw, vw, din, dp, n, dout, sc.st);
+  cudaMemcpyAsync(out, dout, out_floats * 4, cudaMemcpyDeviceToHost, sc.st);
+  return finish(sc);
+}
+// Point2DKalmanFilter::initiate, src/utils/kalman/kalman_2d_point.rs:51-65
+int sb200_point_kalman_initiate(float pw, float vw, const float* points2, int32_t n, float* states12, int32_t device) {
+  return point_kalman_op(0, pw, vw, nullptr, points2, n, states12, device);
+}
+// Point2DKalmanFilter::predict, src/utils/kalman/kalman_2d_point.rs:67-84
+int sb200_point_kalman_predict(float pw, float vw, const float* in12, int32_t n, float* out12, int32_t device) {
+  return point_kalman_op(1, pw, vw, in12, nullptr, n, out12, device);
+}
+// Point2DKalmanFilter::update, src/utils/kalman/kalman_2d_point.rs:103-121
+int sb200_point_kalman_update(float pw, float vw, const float* in12, const float* points2, int32_t n, float* out12,
+                              int32_t device) {
+  return point_kalman_op(2, pw, vw, in12, points2, n, out12, device);
+}
+// Point2DKalmanFilter::distance, src/utils/kalman/kalman_2d_point.rs:123-137
+int sb200_point_kalman_distance(float pw, float vw, const float* states12, const float* points2, int32_t n, float* out,
+                                int32_t device) {
+  return point_kalman_op(3, pw, vw, states12, points2, n, out, device);
+}
+
+// Universal2DBox::get_vertices, src/utils/bbox.rs:169-171,287-330
+int sb200_box_vertices(const float* boxes, int32_t n, double* out8, int32_t device) {
+  if (n < 0 || (n > 0 && (!boxes || !out8))) return ops_fail(SB200_ERR_INVALID, "bad arguments");
+  Scratch sc;
+  int rc = begin(sc, device);
+  if (rc) return rc;
+  if (n == 0) return 0;
+  float* db = sc.upload(boxes, (size_t)n * 6);
+  double* dv = sc.alloc<double>((size_t)n * 8);
+  if (!db || !dv) return ops_fail(SB200_ERR_CUDA, "cudaMalloc failed");
+  sb::launch_box_vertices(db, n, dv, sc.st);
+  cudaMemcpyAsync(out8, dv, (size_t)n * 64, cudaMemcpyDeviceToHost, sc.st);
+  return finish(sc);
+}
+
+// sutherland_hodgman_clip_py + intersection_area_py, src/utils/clipping/clipping_py.rs:29-46
+int sb200_clip_polygons(const float* subjects, const float* clippings, int32_t n, double* out_vertices,
+                        int32_t* out_counts, double* out_areas, int32_t device) {
+  if (n < 0 || (n > 0 && (!subjects || !clippings || !out_vertices || !out_counts || !out_areas)))
+    return ops_fail(SB200_ERR_INVALID, "bad arguments");
+  Scratch sc;
+  int rc = begin(sc, device);
+  if (rc) return rc;
+  if (n == 0) return 0;
+  const size_t nv = (size_t)n * sb::kMaxPoly * 2;
+  float* ds = sc.upload(subjects, (size_t)n * 6);
+  float* dc = sc.upload(clippings, (size_t)n * 6);
+  double* dv = sc.alloc<double>(nv, true);
+  int* dn = sc.alloc<int>(n);
+  double* da = sc.alloc<double>(n);
+  int* dst = sc.alloc<int>(1, true);
+  if (!ds || !dc || !dv || !dn || !da || !dst) return ops_fail(SB200_ERR_CUDA, "cudaMalloc failed");
+  sb::launch_clip_polygons(ds, dc, n, dv, dn, da, dst, sc.st);
+  int status = 0;
+  cudaMemcpyAsync(&status, dst, sizeof(int), cudaMemcpyDeviceToHost, sc.st);
+  rc = finish(sc);
+  if (rc) return rc;
+  if (status & 1) return ops_fail(SB200_ERR_CAPACITY, "a clipped polygon would have more than 16 vertices");
+  // outputs are written only when every pair fits
+  cudaMemcpy(out_vertices, dv, nv * sizeof(double), cudaMemcpyDeviceToHost);
+  cudaMemcpy(out_counts, dn, (size_t)n * 4, cudaMemcpyDeviceToHost);
+  cudaMemcpy(out_areas, da, (size_t)n * 8, cudaMemcpyDeviceToHost);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return ops_fail(SB200_ERR_CUDA, std::string("CUDA error: ") + cudaGetErrorString(e));
+  return 0;
+}
+
+// intersection_area_py (src/utils/clipping/clipping_py.rs:41-46) of every (a[i], b[j]) pair
+int sb200_intersection_areas(const float* a, int32_t m, const float* b, int32_t n, double* out_mn, int32_t device) {
+  if (m < 0 || n < 0 || (m > 0 && !a) || (n > 0 && !b) || (m > 0 && n > 0 && !out_mn))
+    return ops_fail(SB200_ERR_INVALID, "bad arguments");
+  Scratch sc;
+  int rc = begin(sc, device);
+  if (rc) return rc;
+  if (m == 0 || n == 0) return 0;
+  float* da = sc.upload(a, (size_t)m * 6);
+  float* db = sc.upload(b, (size_t)n * 6);
+  double* va = sc.alloc<double>((size_t)m * 8);
+  double* vb = sc.alloc<double>((size_t)n * 8);
+  double* dout = sc.alloc<double>((size_t)m * n);
+  int* dst = sc.alloc<int>(1, true);
+  if (!da || !db || !va || !vb || !dout || !dst) return ops_fail(SB200_ERR_CUDA, "cudaMalloc failed");
+  sb::launch_box_vertices(da, m, va, sc.st);
+  sb::launch_box_vertices(db, n, vb, sc.st);
+  sb::launch_intersection_areas(va, m, vb, n, dout, dst, sc.st);
+  int status = 0;
+  cudaMemcpyAsync(&status, dst, sizeof(int), cudaMemcpyDeviceToHost, sc.st);
+  rc = finish(sc);
+  if (rc) return rc;
+  if (status & 1) return ops_fail(SB200_ERR_CAPACITY, "a clipped polygon would have more than 16 vertices");
+  cudaError_t e = cudaMemcpy(out_mn, dout, (size_t)m * n * sizeof(double), cudaMemcpyDeviceToHost);
+  if (e != cudaSuccess) return ops_fail(SB200_ERR_CUDA, std::string("CUDA error: ") + cudaGetErrorString(e));
+  return 0;
+}
+
 }  // extern "C"

@@ -374,6 +374,20 @@ void launch_frame_sweep(const Params& p, const TrackStore& ts, const Frame& f, i
 // stateless operators
 void launch_kalman_ops(int op, float pw, float vw, const float* in30, const float* boxes, int n, float* out30,
                        cudaStream_t st);
+void launch_kalman_distance(float pw, const float* in30, const float* boxes, int n, float* out, cudaStream_t st);
+// op: 0 initiate, 1 predict, 2 update (out = 12-float states), 3 distance (out = one float per state); in12 16-byte aligned
+void launch_point_kalman(int op, float pw, float vw, const float* in12, const float* points, int n, float* out,
+                         cudaStream_t st);
+// kernels_geom.cu
+void launch_box_vertices(const float* boxes6, int n, double* out8, cudaStream_t st);
+// n (subject, clipping) pairs: ring [n][kMaxPoly][2], counts (-1: more than kMaxPoly vertices), areas; *d_status |= 1
+// when any count is -1
+void launch_clip_polygons(const float* subjects6, const float* clippings6, int n, double* out_xy, int* out_counts,
+                          double* out_areas, int* d_status, cudaStream_t st);
+// m x n intersection areas from the boxes' vertices (launch_box_vertices); *d_status |= 1 when a pair would need more
+// than kMaxPoly vertices
+void launch_intersection_areas(const double* a_vert, int m, const double* b_vert, int n, double* out_mn, int* d_status,
+                               cudaStream_t st);
 
 // shared device helpers
 __device__ __forceinline__ bool compat_ok(const Params& p, unsigned int cand_epoch, unsigned int trk_epoch, float cx,

@@ -89,10 +89,21 @@ SB_HD void box_vertices(float xc, float yc, float angle, float aspect_f, float h
   out[6] = x - r2x; out[7] = y - r2y;
 }
 
-// Area of sutherland_hodgman_clip(subject, clip) (src/utils/clipping.rs:12-91) followed by geo's
-// Area::unsigned_area (shoelace on coordinates shifted by the first vertex).  Ping-pong buffers, no heap.
-SB_HD double clip_area(const double* subj, const double* clp) {
+// sutherland_hodgman_clip(subject, clip) (src/utils/clipping.rs:12-91) followed by geo's Area::unsigned_area (shoelace
+// on coordinates shifted by the first vertex).  Ping-pong buffers, no heap.  What else it reports is chosen at compile
+// time, so the area-only instantiation (clip_area) carries none of it:
+//   kClipArea   the area only;
+//   kClipCount  also *out_n = number of vertices of the clipped ring, or -1 when the reference's unbounded Vec would have
+//               held more than kMaxPoly vertices at some step (the area is then that of a truncated ring: not the
+//               reference's);
+//   kClipRing   also the ring itself, out_xy = (x, y) pairs of the first *out_n vertices, in the reference's order and
+//               without the closing repeat that geo::Polygon::new adds.
+enum ClipOut { kClipArea = 0, kClipCount = 1, kClipRing = 2 };
+
+template <int kOut>
+SB_HD double clip_poly(const double* subj, const double* clp, double* out_xy, int* out_n) {
   double ax[kMaxPoly], ay[kMaxPoly], bx[kMaxPoly], by[kMaxPoly];
+  [[maybe_unused]] bool over = false;
   int na = 4;
 #pragma unroll
   for (int i = 0; i < 4; ++i) { ax[i] = subj[2 * i]; ay[i] = subj[2 * i + 1]; }
@@ -117,8 +128,10 @@ SB_HD double clip_area(const double* subj, const double* clp) {
           const double n1 = psx * qy - psy * qx;
           const double n2 = c1x * c2y - c1y * c2x;
           const double n3 = 1.0 / (dcx * dpy - dcy * dpx);
+          if constexpr (kOut != kClipArea) over = over || nd >= kMaxPoly;
           if (nd < kMaxPoly) { dx[nd] = (n1 * dpx - n2 * dcx) * n3; dy[nd] = (n1 * dpy - n2 * dcy) * n3; ++nd; }
         }
+        if constexpr (kOut != kClipArea) over = over || (q_in && nd >= kMaxPoly);
         if (q_in && nd < kMaxPoly) { dx[nd] = qx; dy[nd] = qy; ++nd; }
         psx = qx; psy = qy; p_in = q_in;
       }
@@ -127,6 +140,10 @@ SB_HD double clip_area(const double* subj, const double* clp) {
     t = sx; sx = dx; dx = t;
     t = sy; sy = dy; dy = t;
     na = nd;
+  }
+  if constexpr (kOut != kClipArea) *out_n = over ? -1 : na;
+  if constexpr (kOut == kClipRing) {
+    for (int j = 0; j < na; ++j) { out_xy[2 * j] = sx[j]; out_xy[2 * j + 1] = sy[j]; }
   }
   if (na < 3) return 0.0;
   // geo: ring closed by Polygon::new; shift by first coord; sum of determinants over ring lines; |sum / 2|
@@ -141,6 +158,7 @@ SB_HD double clip_area(const double* subj, const double* clp) {
   }
   return fabs(tmp / 2.0);
 }
+SB_HD double clip_area(const double* subj, const double* clp) { return clip_poly<kClipArea>(subj, clp, nullptr, nullptr); }
 
 // Conservative pre-gates of the IoU metric: they decide "certainly None" for any threshold above ~1e-6, so that the f64
 // clip can be skipped.  Pairs they cannot decide go through clip_area unchanged.
@@ -295,6 +313,90 @@ SB_HD Box state_box(const float* st, float conf) {
   b.angle = (st[2] == 0.0f) ? nanf("") : st[2];
   b.aspect = st[3]; b.height = st[4]; b.conf = conf;
   return b;
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// Kalman filter of a 2-D point, src/utils/kalman/kalman_2d_point.rs.  State = mean[4] + cov[8] where
+// mean = (x, y, vx, vy) and cov[4*i + {0,1,2,3}] = P[i][i], P[i][i+2], P[i+2][i], P[i+2][i+2]  (i = x, y): the box
+// state's layout with two blocks.  The reference's 4x4 matrices never couple x with y either, so the same argument
+// holds: S is exactly diagonal and every entry of the full products has at most two non-zero terms.
+constexpr int kPointStateFloats = 12;
+
+SB_HD void point_kalman_initiate(float pw, float vw, float x, float y, float* st) {  // initiate, :51-65
+  st[0] = x; st[1] = y; st[2] = 0.0f; st[3] = 0.0f;
+  const float sp = 2.0f * pw;   // std_position(2.0) = k * w, :41-44 (no height factor, unlike the box filter)
+  const float sv = 10.0f * vw;  // std_velocity(10.0), :46-49
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    st[4 + 4 * i + 0] = sp * sp;
+    st[4 + 4 * i + 1] = 0.0f;
+    st[4 + 4 * i + 2] = 0.0f;
+    st[4 + 4 * i + 3] = sv * sv;
+  }
+}
+
+SB_HD void point_kalman_predict(float pw, float vw, const float* in, float* out) {  // predict, :67-84
+  const float p = 1.0f * pw;  // std_position(1.0)
+  const float q = 1.0f * vw;  // std_velocity(1.0)
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const float m = in[i], v = in[2 + i];
+    const float a = in[4 + 4 * i], b = in[4 + 4 * i + 1], c = in[4 + 4 * i + 2], d = in[4 + 4 * i + 3];
+    out[i] = m + v;      // F * mean, F = [[I, I], [0, I]] (DT = 1)
+    out[2 + i] = v;
+    const float fa = a + c, fb = b + d;      // (F P) row i
+    out[4 + 4 * i + 0] = (fa + fb) + p * p;  // (F P F^T)[i][i] + motion_cov
+    out[4 + 4 * i + 1] = fb;                 // [i][i+2]
+    out[4 + 4 * i + 2] = c + d;              // [i+2][i]
+    out[4 + 4 * i + 3] = d + q * q;          // [i+2][i+2]
+  }
+}
+
+// project (:86-101): S_ii = P_ii + std_position(1.0)^2 (S is exactly diagonal)
+SB_HD float point_kalman_proj_var(float pw, float pii) {
+  const float p = 1.0f * pw;
+  return pii + p * p;
+}
+
+SB_HD void point_kalman_update(float pw, const float* in, float x, float y, float* out) {  // update, :103-121
+  const float meas[2] = {x, y};
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const float m = in[i], v = in[2 + i];
+    const float a = in[4 + 4 * i], b = in[4 + 4 * i + 1], c = in[4 + 4 * i + 2], d = in[4 + 4 * i + 3];
+    const float s = point_kalman_proj_var(pw, a);
+    const float kp = a / s;   // kalman_gain[i][i]   = P[i][i]   / S_ii  (solve_lower_triangular on the diagonal S)
+    const float kv = c / s;   // kalman_gain[i][i+2] = P[i+2][i] / S_ii
+    const float innov = meas[i] - m;
+    out[i] = m + innov * kp;
+    out[2 + i] = v + innov * kv;
+    const float kps = kp * s, kvs = kv * s;  // (K^T S)
+    out[4 + 4 * i + 0] = a - kps * kp;
+    out[4 + 4 * i + 1] = b - kps * kv;
+    out[4 + 4 * i + 2] = c - kvs * kp;
+    out[4 + 4 * i + 3] = d - kvs * kv;
+  }
+}
+
+// distance (:123-137): the Cholesky factor of the diagonal S is diag(sqrt(S_ii)); sum of squares in index order
+SB_HD float point_kalman_distance(float pw, const float* st, float x, float y) {
+  const float l0 = sqrtf(point_kalman_proj_var(pw, st[4]));
+  const float l1 = sqrtf(point_kalman_proj_var(pw, st[8]));
+  const float y0 = (x - st[0]) / l0;
+  const float y1 = (y - st[1]) / l1;
+  float s = y0 * y0;
+  s = s + y1 * y1;
+  return s;
+}
+
+// Universal2DBoxKalmanFilter::distance (src/utils/kalman/kalman_2d_box.rs:150-170) of a packed 30-float state: the
+// same l5 as the positional cost kernel's Mahalanobis pair (kernels_cost.cu, pos_eval_pair)
+SB_HD float kalman_distance(float pw, const float* st, const Box& z) {
+  float l5[5];
+  const float hh = st[4];
+#pragma unroll
+  for (int q = 0; q < 5; ++q) l5[q] = sqrtf(kalman_proj_var(pw, hh, st[10 + 4 * q], q));
+  return maha_distance(st, l5, z.xc, z.yc, angle_or0(z.angle), z.aspect, z.height);
 }
 
 // Rust `f32 as i64` (saturating, NaN -> 0) of value * 1e6, src/trackers/sort/voting.rs:20,59

@@ -322,6 +322,79 @@ def kalman_update(states30, boxes, pw=1 / 20, vw=1 / 160, device=0):
     return out
 
 
+def kalman_distance(states30, boxes, pw=1 / 20, vw=1 / 160, device=0):
+    """sb200_kalman_distance: squared Mahalanobis distance of boxes[i] ([n][6]) from states30[i] ([n][30])."""
+    s, b = _f32(states30).reshape(-1, 30), _f32(boxes).reshape(-1, 6)
+    if len(s) != len(b):
+        raise ValueError("states and boxes differ in length")
+    out = np.empty(len(s), np.float32)
+    check(lib().sb200_kalman_distance(pw, vw, ptr(s), ptr(b), len(s), ptr(out), device))
+    return out
+
+
+def point_kalman_initiate(points, pw=1 / 20, vw=1 / 160, device=0):
+    """sb200_point_kalman_initiate: points [n][2] -> packed states [n][12] (mean x, y, vx, vy; then the x and y blocks
+    P[i][i], P[i][i+2], P[i+2][i], P[i+2][i+2])."""
+    p = _f32(points).reshape(-1, 2)
+    out = np.empty((len(p), 12), np.float32)
+    check(lib().sb200_point_kalman_initiate(pw, vw, ptr(p), len(p), ptr(out), device))
+    return out
+
+
+def point_kalman_predict(states12, pw=1 / 20, vw=1 / 160, device=0):
+    s = _f32(states12).reshape(-1, 12)
+    out = np.empty_like(s)
+    check(lib().sb200_point_kalman_predict(pw, vw, ptr(s), len(s), ptr(out), device))
+    return out
+
+
+def point_kalman_update(states12, points, pw=1 / 20, vw=1 / 160, device=0):
+    s, p = _f32(states12).reshape(-1, 12), _f32(points).reshape(-1, 2)
+    if len(s) != len(p):
+        raise ValueError("states and points differ in length")
+    out = np.empty_like(s)
+    check(lib().sb200_point_kalman_update(pw, vw, ptr(s), ptr(p), len(s), ptr(out), device))
+    return out
+
+
+def point_kalman_distance(states12, points, pw=1 / 20, vw=1 / 160, device=0):
+    s, p = _f32(states12).reshape(-1, 12), _f32(points).reshape(-1, 2)
+    if len(s) != len(p):
+        raise ValueError("states and points differ in length")
+    out = np.empty(len(s), np.float32)
+    check(lib().sb200_point_kalman_distance(pw, vw, ptr(s), ptr(p), len(s), ptr(out), device))
+    return out
+
+
+def box_vertices(boxes, device=0):
+    """sb200_box_vertices: boxes [n][6] -> vertices [n][4][2] (f64)."""
+    b = _f32(boxes).reshape(-1, 6)
+    out = np.empty((len(b), 4, 2), np.float64)
+    check(lib().sb200_box_vertices(ptr(b), len(b), ptr(out), device))
+    return out
+
+
+def clip_polygons(subjects, clippings, device=0):
+    """sb200_clip_polygons: Sutherland-Hodgman clip of subjects[i] by clippings[i] ([n][6] each).  Returns
+    (vertices [n][16][2] f64, counts [n] int32, areas [n] f64); ring i is vertices[i, :counts[i]] (not closed)."""
+    s, c = _f32(subjects).reshape(-1, 6), _f32(clippings).reshape(-1, 6)
+    if len(s) != len(c):
+        raise ValueError("subjects and clippings differ in length")
+    v = np.empty((len(s), 16, 2), np.float64)
+    n = np.empty(len(s), np.int32)
+    a = np.empty(len(s), np.float64)
+    check(lib().sb200_clip_polygons(ptr(s), ptr(c), len(s), ptr(v), ptr(n), ptr(a), device))
+    return v, n, a
+
+
+def intersection_areas(a, b, device=0):
+    """sb200_intersection_areas: [m][n] f64 matrix of the clipped areas of every (a[i], b[j]) box pair."""
+    a, b = _f32(a).reshape(-1, 6), _f32(b).reshape(-1, 6)
+    out = np.zeros((len(a), len(b)), np.float64)
+    check(lib().sb200_intersection_areas(ptr(a), len(a), ptr(b), len(b), ptr(out), device))
+    return out
+
+
 def own_area_shares(boxes, device=0):
     """exclusively_owned_areas_normalized_shares of ONE scene's boxes ([n][6]) on the GPU."""
     b = _f32(boxes).reshape(-1, 6)
