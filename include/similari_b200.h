@@ -210,6 +210,23 @@ int64_t sb200_wasted(sb200_tracker* t, int64_t cap, uint64_t* ids, uint64_t* sce
 int64_t sb200_wasted_history(sb200_tracker* t, int64_t cap, uint64_t* ids, uint64_t* scene_ids, uint32_t* epochs,
                              uint32_t* lengths, float* predicted_boxes, float* observed_boxes, int32_t history_cap,
                              float* predicted_history, float* observed_history, int32_t* history_counts);
+/* Feature history of the visual trackers (WastedVisualSortTrack::observed_features, src/trackers/visual_sort.rs:117-119,
+ * 210-213): the input feature of each of a track's last history_length observations (capped at 64 like the box history),
+ * kept on the device while the track lives and until its wasted record is collected.  Off by default; on == 1 switches
+ * it on.  SB200_ERR_INVALID for a non-visual tracker or once a predict has been enqueued. */
+int sb200_set_feature_history(sb200_tracker* t, int32_t on);
+/* Size of the feature-history pool (waits for the frames in flight): out3 = {blocks allocated, blocks ever handed out,
+ * free blocks}.  A block holds history_length * (4 * d8 + 1) bytes.  SB200_ERR_INVALID when the history is off. */
+int sb200_feature_history_pool(sb200_tracker* t, int64_t* out3);
+/* sb200_wasted_history (same records, same order, same "newest history_cap entries" rule) plus each entry's feature:
+ * features[cap][history_cap][d8] f32 (d8 = feature_dim rounded up to 8, zero-padded as Feature::from_vec does) and
+ * feature_present[cap][history_cap] (0: the observation had no feature; also 0 past history_counts[i]).  Every row of
+ * the first returned-count records is written: rows whose present byte is 0 are all zero.  SB200_ERR_INVALID when the
+ * feature history is off or an output is NULL. */
+int64_t sb200_wasted_visual(sb200_tracker* t, int64_t cap, uint64_t* ids, uint64_t* scene_ids, uint32_t* epochs,
+                            uint32_t* lengths, float* predicted_boxes, float* observed_boxes, int32_t history_cap,
+                            float* predicted_history, float* observed_history, int32_t* history_counts, float* features,
+                            uint8_t* feature_present);
 /* idle_tracks_with_scene() (src/trackers/sort/simple_api.rs:198-215) */
 int64_t sb200_idle_tracks(sb200_tracker* t, uint64_t scene_id, int64_t cap, uint64_t* ids, uint32_t* epochs,
                           uint32_t* lengths, float* predicted_boxes, float* observed_boxes);

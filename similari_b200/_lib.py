@@ -86,7 +86,8 @@ EXPORTS = [
     "sb200_shard_gather", "sb200_wasted_history", "sb200_host_counters", "sb200_set_stream_join", "sb200_stream_join",
     "sb200_nms_batch", "sb200_nms_batch_device", "sb200_kalman_distance", "sb200_point_kalman_initiate",
     "sb200_point_kalman_predict", "sb200_point_kalman_update", "sb200_point_kalman_distance", "sb200_box_vertices",
-    "sb200_clip_polygons", "sb200_intersection_areas",
+    "sb200_clip_polygons", "sb200_intersection_areas", "sb200_set_feature_history", "sb200_wasted_visual",
+    "sb200_feature_history_pool",
 ]
 
 
@@ -134,6 +135,9 @@ def lib():
         "sb200_clear_wasted": (C.c_int, [vp]),
         "sb200_wasted": (i64, [vp, i64, vp, vp, vp, vp, vp, vp]),
         "sb200_wasted_history": (i64, [vp, i64, vp, vp, vp, vp, vp, vp, i32, vp, vp, vp]),
+        "sb200_set_feature_history": (C.c_int, [vp, i32]),
+        "sb200_feature_history_pool": (C.c_int, [vp, vp]),
+        "sb200_wasted_visual": (i64, [vp, i64, vp, vp, vp, vp, vp, vp, i32, vp, vp, vp, vp, vp]),
         "sb200_idle_tracks": (i64, [vp, u64, i64, vp, vp, vp, vp, vp]),
         "sb200_scene_tracks": (i64, [vp, u64, i64, vp, vp, vp, vp]),
         "sb200_last_costs": (i64, [vp, u64, i64, vp, C.POINTER(i32), C.POINTER(i32)]),

@@ -187,7 +187,26 @@ class WastedSortTrack:
         self.observed_boxes = observed_boxes if observed_boxes is not None else [observed_bbox]
 
 
-WastedVisualSortTrack = WastedSortTrack
+class WastedVisualSortTrack(WastedSortTrack):
+    """src/trackers/visual_sort.rs:195-224 `PyWastedVisualSortTrack`: a WastedSortTrack plus observed_features, the feature
+    of each of the track's last kept_history_length observations (oldest first; None for an observation without one).
+    Each feature is its f32 values zero-padded to a multiple of 8 (Vec::from_vec(&Feature), src/track/utils.rs:25-33)."""
+
+    __slots__ = ("_feat_rows", "_feat_present", "_observed_features")
+
+    def __init__(self, id, epoch, predicted_bbox, observed_bbox, scene_id, length, predicted_boxes=None,
+                 observed_boxes=None, feature_rows=None, feature_present=None):
+        super().__init__(id, epoch, predicted_bbox, observed_bbox, scene_id, length, predicted_boxes, observed_boxes)
+        self._feat_rows = np.zeros((0, 8), np.float32) if feature_rows is None else feature_rows
+        self._feat_present = np.zeros(len(self._feat_rows), bool) if feature_present is None else feature_present
+        self._observed_features = None
+
+    @property
+    def observed_features(self) -> List[Optional[List[float]]]:
+        # built from the packed [count][d8] rows when first read: most users of wasted() never look at it
+        if self._observed_features is None:
+            self._observed_features = [row.tolist() if p else None for row, p in zip(self._feat_rows, self._feat_present)]
+        return self._observed_features
 
 
 def _tracks_from(out, scene_id, custom_ids=None) -> List[SortTrack]:
@@ -447,6 +466,7 @@ class _VisualBase(_TrackerBase):
                 dim = 8  # no feature seen yet (feature is an Option in the reference): provisional until one arrives
                 self._dim_provisional = True
             self._t = engine.Tracker(self._opts._build(kind, dim))
+            self._t.set_feature_history(True)   # the reference always keeps it (kept_history_length is its memory knob)
             self._dim = dim
         elif self._dim_provisional and dim > 0:
             # first featured observation: the tracker keeps its tracks, ids, epochs and Kalman state, only the (still
@@ -474,6 +494,17 @@ class _VisualBase(_TrackerBase):
         q = np.array([1.0 if o.feature_quality is None else o.feature_quality for o in observations], dtype=np.float32)
         custom = np.array([NONE_ID if o.custom_object_id is None else o.custom_object_id for o in observations], dtype=np.int64)
         return boxes, feats, has, q, custom
+
+    def wasted(self) -> List[WastedVisualSortTrack]:
+        if self._t is None:
+            return []
+        w = self._t.wasted_visual()
+        return [WastedVisualSortTrack(w["ids"][i], w["epochs"][i], Universal2DBox._from_row(w["predicted"][i]),
+                                      Universal2DBox._from_row(w["observed"][i]), w["scene_ids"][i], w["lengths"][i],
+                                      [Universal2DBox._from_row(r) for r in w["predicted_history"][i]],
+                                      [Universal2DBox._from_row(r) for r in w["observed_history"][i]],
+                                      w["features"][i], w["feature_present"][i])
+                for i in range(len(w["ids"]))]
 
 
 class VisualSort(_VisualBase):

@@ -240,6 +240,14 @@ struct sb200_tracker {
   sb::WastedBuf wb{};
   DBuf w_count, w_id, w_scene, w_epoch, w_length, w_pred, w_obs, w_hpred, w_hobs;
   int hist_len = 1;   // boxes of history kept per track (1: only the last ones, the SortTrack columns)
+  // feature history of the visual trackers (sb200_set_feature_history): hist_len features per track in a pool of history
+  // blocks (TrackStore::hblk ...), owned by the live track, then by its wasted record until the record is collected
+  bool fhist_on = false;
+  DBuf b_hblk, b_hrows, b_hpresent, b_hfree, b_hpool, w_hblk, f_histdst;
+  long long hpool_cap = 0;    // blocks the pool can hold
+  long long hpool_top = 0;    // blocks ever handed out, as of the last absorbed frame (exact when nothing is in flight)
+  long long hpool_free = 0;   // free blocks, as of the last absorbed frame or the last collection (exact likewise)
+  long long hpool_pend = 0;   // detections of the frames in flight (each can take at most one block)
   // frame buffers
   // two input staging sets: sb200_prefetch_inputs() fills one while the kernels of the previous frame read the other
   struct Staging {
@@ -272,7 +280,8 @@ struct sb200_tracker {
                    &b_feat_bf16, &f_scene_max, &f_tiles, &f_pairs, &f_colmeta, &f_colgeo, &f_colb, &f_colvalid, &f_rowmeta, &f_poslist, &f_counters, &f_visval, &b_fnorm2, &b_obs_phys, &b_obs_hasf, &b_obs_q, &b_obs_n, &b_feat_cnt, &b_ntracks, &b_cur_epoch,
                    &b_fblk, &b_blk_owner, &b_blk_free, &b_nfree, &b_atop, &f_frameout, &f_excl, &f_prewin, &f_own, &f_ownovf, &f_dyn, &b_idc, &f_ws, &f_tmeta, &f_rowinfo, &f_slabc, &f_slabm, &f_slabmask, &f_dscene, &f_maxc, &f_maxcval, &f_drowb, &f_dcolb, &f_slabk,
                    &b_scene_ids, &w_count, &w_id, &w_scene, &w_epoch, &w_length, &w_pred, &w_obs, &f_winner, &f_cvt, &f_pos, &f_vis, &f_scenes, &f_newcount, &f_status,
-                   &f_featdst, &f_apprank, &f_appmeta, &f_posgq, &o_ids, &o_epochs, &o_lengths, &o_vt, &o_pred, &o_obs};
+                   &f_featdst, &f_apprank, &f_appmeta, &f_posgq, &o_ids, &o_epochs, &o_lengths, &o_vt, &o_pred, &o_obs,
+                   &b_hblk, &b_hrows, &b_hpresent, &b_hfree, &b_hpool, &w_hblk, &f_histdst};
     for (DBuf* b : all) b->release();
     for (int k = 0; k < 2; ++k) {
       f_cbox2[k].release(); f_cradius2[k].release(); f_cconf2[k].release(); f_cvert2[k].release(); f_cflags2[k].release();
@@ -366,6 +375,8 @@ struct sb200_tracker {
       if ((rc = regrow(b_fblk, &ts.fblk, 1, ns, nt))) return rc;
       if ((rc = regrow(b_blk_owner, &ts.blk_owner, 1, ns, nt))) return rc;
       if ((rc = regrow(b_blk_free, &ts.blk_free, 1, ns, nt))) return rc;
+      // the history pool is not indexed by slot: only the tracks' block indices move with the store
+      if (fhist_on && (rc = regrow(b_hblk, &ts.hblk, 1, ns, nt))) return rc;
     }
     if (ns != scene_cap) {
       // per-slot small arrays
@@ -414,11 +425,12 @@ struct sb200_tracker {
     if (need <= wb.cap) return 0;
     int64_t ncap = std::max<int64_t>(need, std::max<int64_t>(1024, (int64_t)wb.cap * 3));
     // wasted records are drained by sb200_wasted; growing preserves the pending ones
-    DBuf nid, nsc, nep, nle, npr, nob, nhp, nho;
+    DBuf nid, nsc, nep, nle, npr, nob, nhp, nho, nhb;
     int rc;
     if ((rc = nid.ensure(8 * ncap)) || (rc = nsc.ensure(8 * ncap)) || (rc = nep.ensure(4 * ncap)) ||
         (rc = nle.ensure(4 * ncap)) || (rc = npr.ensure(24 * ncap)) || (rc = nob.ensure(24 * ncap)))
       return rc;
+    if (fhist_on && (rc = nhb.ensure(4 * ncap))) return rc;
     const size_t hrow = (size_t)24 * hist_len;
     if (hist_len > 1 && ((rc = nhp.ensure(hrow * ncap)) || (rc = nho.ensure(hrow * ncap)))) return rc;
     if (wasted_count > 0) {
@@ -432,11 +444,14 @@ struct sb200_tracker {
         CU(cudaMemcpyAsync(nhp.p, w_hpred.p, hrow * wasted_count, cudaMemcpyDeviceToDevice, stream));
         CU(cudaMemcpyAsync(nho.p, w_hobs.p, hrow * wasted_count, cudaMemcpyDeviceToDevice, stream));
       }
+      if (fhist_on) CU(cudaMemcpyAsync(nhb.p, w_hblk.p, 4 * wasted_count, cudaMemcpyDeviceToDevice, stream));
       CU(cudaStreamSynchronize(stream));
     }
     w_id.release(); w_scene.release(); w_epoch.release(); w_length.release(); w_pred.release(); w_obs.release();
-    w_hpred.release(); w_hobs.release();
+    w_hpred.release(); w_hobs.release(); w_hblk.release();
     w_id = nid; w_scene = nsc; w_epoch = nep; w_length = nle; w_pred = npr; w_obs = nob; w_hpred = nhp; w_hobs = nho;
+    w_hblk = nhb;
+    wb.hblk = w_hblk.as<int>();
     wb.hist_pred = w_hpred.as<float>();
     wb.hist_obs = w_hobs.as<float>();
     if (!w_count.p) {
@@ -500,6 +515,18 @@ struct sb200_tracker {
     const int64_t rest = wasted_count - n;
     cudaStream_t st = stream;
     int rc = 0;
+    if (fhist_on) {
+      // the collected records' history blocks go back on the pool's free list.  Every caller has drained: no frame in
+      // flight reads the list, and a block pushed here is handed out only by a frame enqueued after this point.
+      int nf = 0;
+      CU(cudaMemcpyAsync(&nf, ts.hpool, sizeof(int), cudaMemcpyDeviceToHost, st));
+      CU(cudaStreamSynchronize(st));
+      CU(cudaMemcpyAsync(ts.hfree + nf, wb.hblk, 4 * (size_t)n, cudaMemcpyDeviceToDevice, st));
+      nf += (int)n;
+      CU(cudaMemcpyAsync(ts.hpool, &nf, sizeof(int), cudaMemcpyHostToDevice, st));
+      CU(cudaStreamSynchronize(st));
+      hpool_free = nf;
+    }
     if (rest > 0) {
       DBuf tmp;   // overlapping device-to-device moves are done through a temporary
       if ((rc = tmp.ensure((size_t)rest * 24))) return rc;
@@ -511,6 +538,7 @@ struct sb200_tracker {
       if ((rc = shift(wb.id, 8)) || (rc = shift(wb.scene, 8)) || (rc = shift(wb.epoch, 4)) || (rc = shift(wb.length, 4)) ||
           (rc = shift(wb.pred, 24)) || (rc = shift(wb.obs, 24)))
         return rc;
+      if (fhist_on && (rc = shift(wb.hblk, 4))) return rc;
       if (hist_len > 1) {
         tmp.release();
         if ((rc = tmp.ensure((size_t)rest * 24 * hist_len))) return rc;
@@ -524,6 +552,64 @@ struct sb200_tracker {
     CU(cudaStreamSynchronize(st));
     wasted_count = rest;
     revealed = std::max<int64_t>(0, revealed - n);
+    return 0;
+  }
+
+  // (re)allocates the feature-history pool for exactly `need` blocks (at least 256), preserving the blocks handed out so
+  // far [0, hpool_top) and the free list.  Nothing may be in flight.
+  int ensure_hpool(long long need) {
+    if (need <= hpool_cap) return 0;
+    const long long ncap = std::max<long long>(need, 256);
+    const size_t H = (size_t)hist_len, d8 = (size_t)P.d8;
+    DBuf nr, np, nf;
+    int rc;
+    if ((rc = nr.ensure((size_t)ncap * H * d8 * 4)) || (rc = np.ensure((size_t)ncap * H)) || (rc = nf.ensure((size_t)ncap * 4)))
+      return rc;
+    CU(cudaMemsetAsync(np.p, 0, (size_t)ncap * H, stream));
+    if (hpool_top > 0) {
+      CU(cudaMemcpyAsync(nr.p, b_hrows.p, (size_t)hpool_top * H * d8 * 4, cudaMemcpyDeviceToDevice, stream));
+      CU(cudaMemcpyAsync(np.p, b_hpresent.p, (size_t)hpool_top * H, cudaMemcpyDeviceToDevice, stream));
+      CU(cudaMemcpyAsync(nf.p, b_hfree.p, (size_t)hpool_top * 4, cudaMemcpyDeviceToDevice, stream));   // free <= top
+    }
+    CU(cudaStreamSynchronize(stream));
+    b_hrows.release(); b_hpresent.release(); b_hfree.release();
+    b_hrows = nr; b_hpresent = np; b_hfree = nf;
+    ts.hrows = b_hrows.as<float>();
+    ts.hpresent = b_hpresent.as<unsigned char>();
+    ts.hfree = b_hfree.as<int>();
+    hpool_cap = ncap;
+    return 0;
+  }
+
+  int set_feature_history(bool on) {
+    if (on == fhist_on) return 0;
+    CU(cudaSetDevice(device));
+    CU(cudaStreamSynchronize(stream));
+    if (!on) {
+      b_hblk.release(); b_hrows.release(); b_hpresent.release(); b_hfree.release(); b_hpool.release(); w_hblk.release();
+      f_histdst.release();
+      ts.hblk = nullptr; ts.hrows = nullptr; ts.hpresent = nullptr; ts.hfree = nullptr; ts.hpool = nullptr;
+      ts.fhist_len = 0;
+      wb.hblk = nullptr;
+      fhist_on = false;
+      hpool_cap = hpool_top = hpool_free = hpool_pend = 0;
+      return 0;
+    }
+    int rc;
+    if ((rc = b_hpool.ensure(2 * sizeof(int)))) return rc;
+    CU(cudaMemsetAsync(b_hpool.p, 0, 2 * sizeof(int), stream));
+    if (scene_cap > 0 && track_cap > 0) {
+      if ((rc = b_hblk.ensure((size_t)scene_cap * track_cap * sizeof(int)))) return rc;
+      ts.hblk = b_hblk.as<int>();
+    }
+    if (wb.cap > 0) {   // no record exists before the first frame
+      if ((rc = w_hblk.ensure((size_t)wb.cap * sizeof(int)))) return rc;
+      wb.hblk = w_hblk.as<int>();
+    }
+    CU(cudaStreamSynchronize(stream));
+    ts.hpool = b_hpool.as<int>();
+    ts.fhist_len = hist_len;
+    fhist_on = true;
     return 0;
   }
 
@@ -583,6 +669,11 @@ int sb200_tracker::absorb_oldest(bool block) {
       n_hidden[slot] += h_fo[3 * s + 2];   // swept from the device store, not yet collected in the reference's sense
       wasted_count += h_fo[3 * s + 2];
     }
+    if (fhist_on) {   // the history pool's counters {free, handed out} as the frame's sweep left them
+      const int* hp = reinterpret_cast<const int*>(reinterpret_cast<const char*>(dyn) + sizeof(sb::FrameDyn) + 2 * sizeof(int));
+      hpool_free = hp[0];
+      hpool_top = hp[1];
+    }
     acc_units_mn += dyn->units_mn;
     acc_units_rows += dyn->units_rows;
     acc_frames += 1;
@@ -616,6 +707,7 @@ int sb200_tracker::absorb_oldest(bool block) {
   }
   for (int s = 0; s < n; ++s) pending_add[q.slots[s]] -= q.m[s];
   inflight_live_ub -= q.live_ub;
+  if (fhist_on) hpool_pend -= q.total;
   q.active = false;
   pend_head = (pend_head + 1) % kDepth;
   pend_count -= 1;
@@ -775,6 +867,19 @@ int sb200_tracker::predict(int32_t n_scenes, const uint64_t* scene_ids, const in
       const long long mult = std::max<long long>(1, std::min<long long>(8, (2ll << 30) / std::max<long long>(1, base_need * rec_bytes)));
       if ((rc = ensure_wasted(2 * wasted_count + mult * base_need + 1))) return rc;
     }
+    // Feature-history pool.  New tracks take free blocks first, so the blocks handed out after this frame are at most
+    //   top + max(0, detections queued since - free)      (top, free: as of the last absorbed frame or collection).
+    // When that bound exceeds the pool, meet the device (the counts become exact) and grow, if needed, to
+    //   top + max(0, f * detections of this frame - free),   f = the frames the bound covered (in flight + this one),
+    // and at least half again as much as before.  So the pool is at most 1.5 x (live + uncollected wasted tracks + the
+    // detections of the frames actually queued together, less the free blocks): a caller that waits for every frame (the
+    // Python API) has f = 1, and only a caller that really queues f frames gets room for f frames of new tracks.
+    if (fhist_on && total > 0 && hpool_top + std::max<long long>(0, hpool_pend + total - hpool_free) > hpool_cap) {
+      const long long frames = pend_count + 1;
+      if ((rc = drain("feature history pool bound"))) return rc;   // hpool_top / hpool_free are exact from here on
+      const long long want = hpool_top + std::max<long long>(0, frames * total - hpool_free);
+      if (want > hpool_cap && (rc = ensure_hpool(std::max<long long>(want, hpool_cap + hpool_cap / 2)))) return rc;
+    }
     if (!b_idc.p) {
       if ((rc = b_idc.ensure(8))) return rc;
       CU(cudaMemsetAsync(b_idc.p, 0, 8, stream));
@@ -849,6 +954,7 @@ int sb200_tracker::predict(int32_t n_scenes, const uint64_t* scene_ids, const in
     return rc;
   if (P.positional_kind == SB200_POS_IOU && (rc = ENS(f_cvert, T * 64))) return rc;
   if (P.is_visual) {
+    if (fhist_on && (rc = ENS(f_histdst, T * 4))) return rc;
     if ((rc = ENS(f_cflags, T)) || (rc = ENS(f_cnorm2, T * 4)) || (rc = ENS(f_featdst, T * 4)) ||
         (rc = ENS(f_vis, std::max<size_t>(4, (size_t)vis_total * 4))) || (rc = ENS(f_scene_max, 4 * (size_t)n_scenes)))
       return rc;
@@ -1002,6 +1108,7 @@ int sb200_tracker::predict(int32_t n_scenes, const uint64_t* scene_ids, const in
   f.scenes = f_scenes.as<sb::SceneDesc>(); f.new_count = f_newcount.as<int>();
   f.new_count_all = f.new_count;
   f.feat_dst = P.is_visual ? f_featdst.as<int>() : nullptr;
+  f.hist_dst = fhist_on ? f_histdst.as<int>() : nullptr;
   f.app_rank = f_apprank.as<int2>(); f.app_meta = f_appmeta.as<int4>();
   if ((rc = ENS(f_frameout, sizeof(int) * 3 * (size_t)n_scenes))) return rc;
   f.frame_out = f_frameout.as<int>();
@@ -1080,6 +1187,7 @@ int sb200_tracker::predict(int32_t n_scenes, const uint64_t* scene_ids, const in
   q.mode = tc.dense ? 2 : (tc.use_tc ? 1 : 0);
   for (int s = 0; s < n_scenes; ++s) pending_add[last_req_slots[s]] += m_of[s];
   inflight_live_ub += live_ub;
+  if (fhist_on) hpool_pend += total;
   pend_count += 1;
   last_n_scenes = n_scenes;
   // a CUDA failure while the frame is being enqueued takes it out of the ring again (the context is lost anyway)
@@ -1089,6 +1197,7 @@ int sb200_tracker::predict(int32_t n_scenes, const uint64_t* scene_ids, const in
       if (!armed) return;
       for (int s = 0; s < q->n_scenes; ++s) t->pending_add[q->slots[s]] -= q->m[s];
       t->inflight_live_ub -= q->live_ub;
+      if (t->fhist_on) t->hpool_pend -= q->total;
       q->active = false;
       t->pend_count -= 1;
     }
@@ -1254,6 +1363,8 @@ int sb200_tracker::predict(int32_t n_scenes, const uint64_t* scene_ids, const in
     CU(cudaMemcpyAsync(ho + 12 * (size_t)n_scenes, f.status, 4 * (size_t)n_scenes, cudaMemcpyDeviceToHost, stream));
     CU(cudaMemcpyAsync(ho + dyn_offset(n_scenes), f_dyn.p, sizeof(sb::FrameDyn), cudaMemcpyDeviceToHost, stream));
     CU(cudaMemcpyAsync(ho + dyn_offset(n_scenes) + sizeof(sb::FrameDyn), f.dense_cnt, 4, cudaMemcpyDeviceToHost, stream));
+    if (fhist_on)
+      CU(cudaMemcpyAsync(ho + dyn_offset(n_scenes) + sizeof(sb::FrameDyn) + 8, ts.hpool, 8, cudaMemcpyDeviceToHost, stream));
   }
   static const bool trace_dense = trace && atoi(getenv("SB200_TRACE")) >= 2;   // synchronises: level 2 only
   if (trace_dense && tc.dense && tc.n_tiles > 0) {
@@ -1430,7 +1541,35 @@ int sb200_set_feature_dim(sb200_tracker* t, int32_t feature_dim) {
     t->ts.feat_bf16 = t->b_feat_bf16.p;
   }
   for (auto& g : t->stg) g.feat.release();
+  if (t->fhist_on && t->hpool_cap > 0) {
+    // the history rows are re-created for the new row size; the present bytes (all zero so far) and the tracks' blocks stay
+    t->b_hrows.release();
+    t->ts.hrows = nullptr;
+    if ((rc = t->b_hrows.ensure((size_t)t->hpool_cap * t->hist_len * t->P.d8 * 4))) return rc;
+    t->ts.hrows = t->b_hrows.as<float>();
+  }
   return 0;
+}
+
+int sb200_feature_history_pool(sb200_tracker* t, int64_t* out3) {
+  if (!t || !out3) return fail(SB200_ERR_INVALID, "bad arguments");
+  if (!t->fhist_on) return fail(SB200_ERR_INVALID, "the feature history is off (sb200_set_feature_history)");
+  CU(cudaSetDevice(t->device));
+  { int rc_ = t->drain(); if (rc_) return rc_; }
+  int h[2] = {0, 0};
+  CU(cudaMemcpyAsync(h, t->ts.hpool, sizeof(h), cudaMemcpyDeviceToHost, t->stream));
+  CU(cudaStreamSynchronize(t->stream));
+  out3[0] = t->hpool_cap;
+  out3[1] = h[1];
+  out3[2] = h[0];
+  return 0;
+}
+
+int sb200_set_feature_history(sb200_tracker* t, int32_t on) {
+  if (!t) return fail(SB200_ERR_INVALID, "tracker is NULL");
+  if (!t->P.is_visual) return fail(SB200_ERR_INVALID, "the feature history belongs to the visual trackers");
+  if (t->frame_seq > 0) return fail(SB200_ERR_INVALID, "the feature history is switched before the first predict");
+  return t->set_feature_history(on != 0);
 }
 
 int sb200_sync(sb200_tracker* t) {
@@ -1601,10 +1740,15 @@ int64_t sb200_wasted(sb200_tracker* t, int64_t cap, uint64_t* ids, uint64_t* sce
   return n;
 }
 
-int64_t sb200_wasted_history(sb200_tracker* t, int64_t cap, uint64_t* ids, uint64_t* scene_ids, uint32_t* epochs, uint32_t* lengths,
-                             float* predicted_boxes, float* observed_boxes, int32_t history_cap, float* predicted_history,
-                             float* observed_history, int32_t* history_counts) {
+// sb200_wasted_history, and sb200_wasted_visual when `features` / `feature_present` are given
+static int64_t wasted_records(sb200_tracker* t, int64_t cap, uint64_t* ids, uint64_t* scene_ids, uint32_t* epochs,
+                              uint32_t* lengths, float* predicted_boxes, float* observed_boxes, int32_t history_cap,
+                              float* predicted_history, float* observed_history, int32_t* history_counts, float* features,
+                              uint8_t* feature_present) {
   if (!t || cap < 0 || history_cap < 0) return fail(SB200_ERR_INVALID, "bad arguments");
+  const bool want_feat = features != nullptr || feature_present != nullptr;
+  if (want_feat && !(features && feature_present)) return fail(SB200_ERR_INVALID, "features and feature_present go together");
+  if (want_feat && !t->fhist_on) return fail(SB200_ERR_INVALID, "the feature history is off (sb200_set_feature_history)");
   CU(cudaSetDevice(t->device));
   { int rc_ = t->drain(); if (rc_) return rc_; }
   int rc = t->run_waste();  // wasted() starts with auto_waste (tracker_api.rs:90-91)
@@ -1646,8 +1790,42 @@ int64_t sb200_wasted_history(sb200_tracker* t, int64_t cap, uint64_t* ids, uint6
       if (observed_history) memcpy(observed_history + ((size_t)i * history_cap + c) * 6, so, 24);
     }
   }
+  if (want_feat && history_cap > 0) {
+    // the records' rings are gathered on the device in the same order, a chunk of records at a time, and copied back once
+    const size_t rec_bytes = (size_t)history_cap * t->P.d8 * 4;
+    const int64_t chunk = std::max<int64_t>(1, std::min<int64_t>(n, (int64_t)((64u << 20) / rec_bytes)));
+    DBuf rows, pres;
+    if ((rc = rows.ensure((size_t)chunk * rec_bytes)) || (rc = pres.ensure((size_t)chunk * history_cap))) return rc;
+    for (int64_t i0 = 0; i0 < n; i0 += chunk) {
+      const int c = (int)std::min<int64_t>(chunk, n - i0);
+      sb::launch_hist_gather(t->ts, t->P.d8, t->wb.hblk + i0, t->wb.length + i0, c, history_cap, rows.as<float>(),
+                             pres.as<unsigned char>(), st);
+      CU(cudaGetLastError());
+      CU(cudaMemcpyAsync(features + (size_t)i0 * history_cap * t->P.d8, rows.p, (size_t)c * rec_bytes, cudaMemcpyDeviceToHost, st));
+      CU(cudaMemcpyAsync(feature_present + (size_t)i0 * history_cap, pres.p, (size_t)c * history_cap, cudaMemcpyDeviceToHost, st));
+      CU(cudaStreamSynchronize(st));
+    }
+    rows.release(); pres.release();
+  }
   if ((rc = t->drop_wasted_front(n))) return rc;   // drain
   return n;
+}
+
+int64_t sb200_wasted_history(sb200_tracker* t, int64_t cap, uint64_t* ids, uint64_t* scene_ids, uint32_t* epochs, uint32_t* lengths,
+                             float* predicted_boxes, float* observed_boxes, int32_t history_cap, float* predicted_history,
+                             float* observed_history, int32_t* history_counts) {
+  return wasted_records(t, cap, ids, scene_ids, epochs, lengths, predicted_boxes, observed_boxes, history_cap,
+                        predicted_history, observed_history, history_counts, nullptr, nullptr);
+}
+
+int64_t sb200_wasted_visual(sb200_tracker* t, int64_t cap, uint64_t* ids, uint64_t* scene_ids, uint32_t* epochs, uint32_t* lengths,
+                            float* predicted_boxes, float* observed_boxes, int32_t history_cap, float* predicted_history,
+                            float* observed_history, int32_t* history_counts, float* features, uint8_t* feature_present) {
+  if (!t) return fail(SB200_ERR_INVALID, "tracker is NULL");
+  if (!t->fhist_on) return fail(SB200_ERR_INVALID, "the feature history is off (sb200_set_feature_history)");
+  if (!features || !feature_present) return fail(SB200_ERR_INVALID, "features / feature_present is NULL");
+  return wasted_records(t, cap, ids, scene_ids, epochs, lengths, predicted_boxes, observed_boxes, history_cap,
+                        predicted_history, observed_history, history_counts, features, feature_present);
 }
 
 static int64_t dump_scene(sb200_tracker* t, uint64_t scene_id, int64_t cap, bool idle_only, uint64_t* ids,

@@ -35,8 +35,10 @@ __global__ void __launch_bounds__(AT) apply_rank_kernel(Params p, TrackStore ts,
   const int sidx = blockIdx.x;
   const SceneDesc sc = f.scenes[sidx];
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-  // ids of non-batch trackers are consumed by new tracks only, in request order => prefix over earlier scenes
-  if (!p.is_batch) {
+  // ids of non-batch trackers are consumed by new tracks only, in request order => prefix over earlier scenes; the
+  // feature-history pool hands out blocks by the same frame-wide rank, for every kind
+  const bool need_before = !p.is_batch || ts.hblk != nullptr;
+  if (need_before) {
     int c = 0;
     for (int s2 = tid; s2 < f.scene0 + sidx; s2 += AT) c += f.new_count_all[s2];
 #pragma unroll
@@ -49,7 +51,7 @@ __global__ void __launch_bounds__(AT) apply_rank_kernel(Params p, TrackStore ts,
       s_newbefore = t;
     }
   }
-  if (tid == 0) { s_carry = 0; if (p.is_batch) s_newbefore = 0; }
+  if (tid == 0) { s_carry = 0; if (!need_before) s_newbefore = 0; }
   __syncthreads();
   const int* winner = f.winner + sc.det_base;
   for (int base = 0; base < sc.m; base += AT) {
@@ -121,7 +123,12 @@ __global__ void __launch_bounds__(256) apply_kernel(Params p, TrackStore ts, Fra
     unsigned long long o_id = 0; unsigned int o_len = 0; signed char o_vt = -1;   // SortTrack columns of this detection
     if (isnew) {
       const int j = sc.n + rank;
-      if (j >= ts.track_cap) { atomicOr(&f.status[sidx], 1); return; }
+      if (j >= ts.track_cap) {   // store overflow: the frame fails; nothing of this detection may be stored later
+        atomicOr(&f.status[sidx], 1);
+        if (f.feat_dst) f.feat_dst[g] = -1;
+        if (f.hist_dst) f.hist_dst[g] = -1;
+        return;
+      }
       idx = (size_t)sc.slot * ts.track_cap + j;
       const float* rb = f.in_boxes + (size_t)g * 6;
       const Box raw{rb[0], rb[1], rb[2], rb[3], rb[4], rb[5]};
@@ -259,6 +266,22 @@ __global__ void __launch_bounds__(256) apply_kernel(Params p, TrackStore ts, Fra
       for (int i = 0; i < 4; ++i) v2[i] = make_double2(vx[2 * i], vx[2 * i + 1]);
     }
     if (f.feat_dst) f.feat_dst[g] = fdst;
+    if (ts.hblk) {
+      // feature history: every observation pushes its feature, or None, before the collect gate
+      // (VisualMetric::optimize, visual_sort/metric.rs:319-324).  A new track takes the pool block of its frame-wide rank:
+      // the free list first, then fresh blocks.  The sweep at the end of the frame advances hpool by the same count.
+      int hb;
+      if (isnew) {
+        const int r = s_newbefore + rank, hn0 = ts.hpool[0];
+        hb = r < hn0 ? ts.hfree[hn0 - 1 - r] : ts.hpool[1] + (r - hn0);
+        ts.hblk[idx] = hb;
+      } else {
+        hb = ts.hblk[idx];
+      }
+      const size_t hrow = (size_t)hb * ts.fhist_len + (o_len - 1u) % (unsigned int)ts.fhist_len;
+      ts.hpresent[hrow] = flags & 1;
+      f.hist_dst[g] = (flags & 1) ? (int)hrow : -1;
+    }
     if (ts.hist_len > 1) {   // update_history: observation number o_len - 1 goes to ring slot (o_len - 1) % hist_len
       const size_t hslot = (idx * ts.hist_len + (size_t)((o_len - 1u) % (unsigned int)ts.hist_len)) * 6;
       write_box_row(ts.hist_pred + hslot, pred);
@@ -277,21 +300,29 @@ __global__ void __launch_bounds__(256) apply_kernel(Params p, TrackStore ts, Fra
   }
 }
 
-// copies the features that VisualMetric::optimize keeps into the track's free physical slot (warp per detection)
+// copies the features that VisualMetric::optimize keeps into the track's free physical slot (warp per detection), and
+// every present feature -- kept or dropped by the collect gate -- into the track's history ring when history is on.
+// This kernel runs beside the end-of-frame sweep (side stream).  It writes history rows only of the blocks of tracks
+// updated in this frame (epoch == the scene's new epoch); the sweep moves only the block indices of tracks with
+// epoch + max_idle < that epoch, and no block changes hands in between (blocks are freed on the host, after a drain, and
+// reused only by frames enqueued after it).  The two sets are disjoint.
 __global__ void feat_store_kernel(Params p, TrackStore ts, Frame f) {
   int w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   int lane = threadIdx.x & 31;
   if (w >= f.total) return;
   w += f.det0;
-  int dst = f.feat_dst[w];
-  if (dst < 0) return;
+  const int dst = f.feat_dst[w];
+  const int hdst = f.hist_dst ? f.hist_dst[w] : -1;
+  if (dst < 0 && hdst < 0) return;
   const float* src = f.in_feat + (size_t)w * p.feature_dim;
-  float* d = ts.feat + (size_t)dst * p.d8;
-  __nv_bfloat16* db = reinterpret_cast<__nv_bfloat16*>(ts.feat_bf16) + (size_t)dst * p.d8;
+  float* d = ts.feat + (size_t)max(dst, 0) * p.d8;
+  __nv_bfloat16* db = reinterpret_cast<__nv_bfloat16*>(ts.feat_bf16) + (size_t)max(dst, 0) * p.d8;
+  float* hd = hdst >= 0 ? ts.hrows + (size_t)hdst * p.d8 : nullptr;
   if (p.feature_dim == p.d8 && (reinterpret_cast<uintptr_t>(f.in_feat) & 15) == 0) {
     // rows are 32-byte multiples: 16-byte vectors, four in flight per lane
     const float4* s4 = reinterpret_cast<const float4*>(src);
     float4* d4 = reinterpret_cast<float4*>(d);
+    float4* h4 = reinterpret_cast<float4*>(hd);
     uint2* b4 = reinterpret_cast<uint2*>(db);
     const int n4 = p.d8 >> 2;
     for (int i0 = 0; i0 < n4; i0 += 128) {
@@ -305,23 +336,61 @@ __global__ void feat_store_kernel(Params p, TrackStore ts, Frame f) {
       for (int u = 0; u < 4; ++u) {
         const int i = i0 + u * 32 + lane;
         if (i < n4) {
-          d4[i] = v[u];
-          const __nv_bfloat162 lo = __floats2bfloat162_rn(v[u].x, v[u].y), hi = __floats2bfloat162_rn(v[u].z, v[u].w);
-          uint2 pk;
-          pk.x = *reinterpret_cast<const unsigned int*>(&lo);
-          pk.y = *reinterpret_cast<const unsigned int*>(&hi);
-          b4[i] = pk;   // B operand of the tensor-core screen
+          if (dst >= 0) {
+            d4[i] = v[u];
+            const __nv_bfloat162 lo = __floats2bfloat162_rn(v[u].x, v[u].y), hi = __floats2bfloat162_rn(v[u].z, v[u].w);
+            uint2 pk;
+            pk.x = *reinterpret_cast<const unsigned int*>(&lo);
+            pk.y = *reinterpret_cast<const unsigned int*>(&hi);
+            b4[i] = pk;   // B operand of the tensor-core screen
+          }
+          if (h4) __stcs(h4 + i, v[u]);   // read back only when the track is collected: streaming store
         }
       }
     }
   } else {
     for (int i = lane; i < p.d8; i += 32) {
-      float x = i < p.feature_dim ? src[i] : 0.0f;
-      d[i] = x;
-      db[i] = __float2bfloat16_rn(x);
+      float x = i < p.feature_dim ? src[i] : 0.0f;   // Feature::from_vec zero-pads to the 8-lane multiple
+      if (dst >= 0) {
+        d[i] = x;
+        db[i] = __float2bfloat16_rn(x);
+      }
+      if (hd) hd[i] = x;
     }
   }
-  if (lane == 0) ts.fnorm2[dst] = f.c_norm2[w];
+  if (lane == 0 && dst >= 0) ts.fnorm2[dst] = f.c_norm2[w];
+}
+
+// feature histories of wasted records, one warp per (record, entry)
+__global__ void hist_gather_kernel(TrackStore ts, int d8, const int* __restrict__ blk, const unsigned int* __restrict__ lengths,
+                                   int n, int hist_cap, float* __restrict__ out_rows, unsigned char* __restrict__ out_present) {
+  const long long w = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (w >= (long long)n * hist_cap) return;
+  const int i = (int)(w / hist_cap), c = (int)(w - (long long)i * hist_cap);
+  const unsigned int len = lengths[i], H = (unsigned int)ts.fhist_len;
+  const int cnt = (int)min(min(len, H), (unsigned int)hist_cap);
+  // every output row is written: the entry's feature, or zeros (no feature, or past the record's count)
+  unsigned char present = 0;
+  size_t row = 0;
+  if (c < cnt) {
+    const unsigned int j = len - (unsigned int)cnt + (unsigned int)c;   // observation number, oldest kept first
+    row = (size_t)blk[i] * H + j % H;
+    present = ts.hpresent[row];
+  }
+  if (lane == 0) out_present[w] = present;
+  const float4* s4 = reinterpret_cast<const float4*>(ts.hrows + row * d8);
+  float4* d4 = reinterpret_cast<float4*>(out_rows + (size_t)w * d8);
+  for (int k = lane; k < (d8 >> 2); k += 32) d4[k] = present ? s4[k] : make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+}
+
+void launch_hist_gather(const TrackStore& ts, int d8, const int* blk, const unsigned int* lengths, int n, int hist_cap,
+                        float* out_rows, unsigned char* out_present, cudaStream_t st) {
+  const long long threads = (long long)n * hist_cap * 32;
+  if (threads == 0) return;
+  hist_gather_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(ts, d8, blk, lengths, n, hist_cap, out_rows,
+                                                                        out_present);
+  note_launch();
 }
 
 void launch_apply(const Params& p, const TrackStore& ts, const Frame& f, int n_scenes, int max_m,
@@ -398,6 +467,15 @@ __global__ void __launch_bounds__(WT) waste_kernel(Params p, TrackStore ts, cons
     else for (int s2 = 0; s2 < n_scenes; ++s2) add += (unsigned long long)new_count[s2];
     *id_counter += add;
   }
+  if (ts.hblk && scenes && blockIdx.x == 0 && threadIdx.x == 0) {
+    // feature-history pool: the new tracks of this frame took its first free blocks, then fresh ones (apply_kernel, which
+    // completed before this kernel started, read the old values)
+    int add = 0;
+    for (int s2 = 0; s2 < n_scenes; ++s2) add += new_count[s2];
+    const int nf = ts.hpool[0];
+    ts.hpool[0] = nf - min(nf, add);
+    ts.hpool[1] += max(0, add - nf);
+  }
   const int slot = scenes ? scenes[blockIdx.x].slot : (int)blockIdx.x;
   const int n = n_tracks[slot];
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
@@ -469,6 +547,7 @@ __global__ void __launch_bounds__(WT) waste_kernel(Params p, TrackStore ts, cons
           wb.hist_obs[(size_t)o * hw + c] = ts.hist_obs[(base + j) * hw + c];
         }
       }
+      if (ts.hblk) wb.hblk[o] = ts.hblk[base + j];   // the feature history stays in the pool: only its block moves
     }
     if (arena) {
       const int b = ts.fblk[base + j];
@@ -483,7 +562,7 @@ __global__ void __launch_bounds__(WT) waste_kernel(Params p, TrackStore ts, cons
     const int j = j0 + tid;
     int d = -1;
     unsigned long long v_id = 0; unsigned int v_ep = 0, v_len = 0; long long v_cu = 0; signed char v_vt = 0; float v_r = 0.0f;
-    unsigned char v_on = 0, v_fc = 0, v_ph[kMaxObs], v_hf[kMaxObs]; float v_q[kMaxObs]; int v_fb = 0;
+    unsigned char v_on = 0, v_fc = 0, v_ph[kMaxObs], v_hf[kMaxObs]; float v_q[kMaxObs]; int v_fb = 0, v_hb = 0;
     if (j < n) {
       d = s_dst[j];
       if (d >= 0 && d != j) {
@@ -492,6 +571,7 @@ __global__ void __launch_bounds__(WT) waste_kernel(Params p, TrackStore ts, cons
         if (p.is_visual) {
           v_on = ts.obs_n[t]; v_fc = ts.feat_cnt[t];
           if (arena) v_fb = ts.fblk[t];
+          if (ts.hblk) v_hb = ts.hblk[t];
           for (int k = 0; k < K; ++k) {   // slots at and beyond obs_n were never written
             const bool have = k < (int)v_on;
             v_ph[k] = have ? ts.obs_phys[t * K + k] : (unsigned char)0; v_hf[k] = have ? ts.obs_hasf[t * K + k] : (unsigned char)0;
@@ -507,6 +587,7 @@ __global__ void __launch_bounds__(WT) waste_kernel(Params p, TrackStore ts, cons
       if (p.is_visual) {
         ts.obs_n[t] = v_on; ts.feat_cnt[t] = v_fc;
         if (arena) ts.fblk[t] = v_fb;
+        if (ts.hblk) ts.hblk[t] = v_hb;
         for (int k = 0; k < K; ++k) { ts.obs_phys[t * K + k] = v_ph[k]; ts.obs_hasf[t * K + k] = v_hf[k]; ts.obs_q[t * K + k] = v_q[k]; }
       }
     }

@@ -139,6 +139,18 @@ struct TrackStore {
   int* blk_free;    // [slot * track_cap + i] free-list stack
   int* n_free;      // [slot]
   int* arena_top;   // [slot] blocks ever handed out (== live tracks + free blocks)
+  // Feature history (VisualAttributes::update_history, src/trackers/visual_sort/track_attributes.rs:73-90): the input
+  // feature of each of the last fhist_len observations, kept for the wasted tracks (sb200_wasted_visual).  One
+  // tracker-wide pool of history blocks, not indexed by scene slot: block b = fhist_len rings of d8 floats plus a present
+  // byte each, observation number j (0-based) in ring slot j % fhist_len.  A live track owns the block in hblk; when it
+  // expires only the index moves into its wasted record (WastedBuf::hblk), and the host puts the block back on the free
+  // list when the record leaves the wasted buffer.  All null (history off): the kernels take no extra memory traffic.
+  int fhist_len;
+  int* hblk;                // [idx] history block of the track
+  float* hrows;             // [block][fhist_len][d8]
+  unsigned char* hpresent;  // [block][fhist_len] the observation had a feature
+  int* hfree;               // free-list stack of blocks
+  int* hpool;               // [2] free blocks, blocks ever handed out (advanced once per frame by the sweep)
 };
 
 // first feature row of track `ti` (absolute store index) of scene slot `slot`, divided by K
@@ -179,6 +191,7 @@ struct Frame {  // per-request transient device buffers (a request may be proces
   int* new_count;          // [n_scenes] new tracks per scene (written by voting)
   int* status;             // [n_scenes] per-scene status flags (capacity overflow etc.)
   int* feat_dst;           // [total] destination feature row (block*K + phys) or -1
+  int* hist_dst;           // [total] destination history row (block*fhist_len + ring slot) or -1 (null: history off)
   int2* app_rank;          // [total] apply phase 1: (scene of the detection, rank among the scene's new tracks)
   int4* app_meta;          // [scenes] apply phase 1: (new tracks of earlier scenes, free blocks, arena top) before the frame
   int* frame_out;          // [n_scenes][3] written by the end-of-frame sweep: live tracks, arena blocks, newly expired
@@ -360,6 +373,7 @@ struct WastedBuf {
   float* obs;
   float* hist_pred;   // [cap][hist_len][6] rings of the wasted tracks (null unless history_length > 1)
   float* hist_obs;
+  int* hblk;          // [cap] feature-history block of the record (null: history off)
 };
 void launch_waste(const Params& p, const TrackStore& ts, int n_slots, const unsigned int* d_cur_epoch,
                   const unsigned long long* d_scene_ids, int* d_n_tracks, const WastedBuf& wb, int max_n,
@@ -370,6 +384,11 @@ void launch_waste(const Params& p, const TrackStore& ts, int n_slots, const unsi
 // frame_out[s] = {live tracks, arena blocks, newly expired} is written for the host mirror.
 void launch_frame_sweep(const Params& p, const TrackStore& ts, const Frame& f, int n_scenes, int* d_n_tracks,
                         const WastedBuf& wb, cudaStream_t st);
+// feature histories of n wasted records (their blocks `blk`, observation counts `lengths`) in the order of
+// sb200_wasted_visual: entry c of record i (oldest first, at most hist_cap) -> out_rows[i][c][d8], out_present[i][c];
+// entries without a feature, and entries past a record's count, get present 0 and a zero row
+void launch_hist_gather(const TrackStore& ts, int d8, const int* blk, const unsigned int* lengths, int n, int hist_cap,
+                        float* out_rows, unsigned char* out_present, cudaStream_t st);
 
 // stateless operators
 void launch_kalman_ops(int op, float pw, float vw, const float* in30, const float* boxes, int n, float* out30,

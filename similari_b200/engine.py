@@ -92,6 +92,7 @@ class Tracker:
     def set_feature_dim(self, dim):
         """sb200_set_feature_dim: fixes the feature length of a visual tracker that has not stored a feature yet."""
         check(self._L.sb200_set_feature_dim(self._h, int(dim)))
+        self.opts.feature_dim = int(dim)
 
     def sync(self):
         """sb200_sync: waits for every frame in flight; raises the first error an asynchronous frame produced."""
@@ -190,6 +191,54 @@ class Tracker:
         return {"ids": ids[:n], "scene_ids": sc[:n], "epochs": ep[:n], "lengths": ln[:n], "predicted": pr[:n],
                 "observed": ob[:n], "predicted_history": [hp[i, : hc[i]].copy() for i in range(n)],
                 "observed_history": [ho[i, : hc[i]].copy() for i in range(n)]}
+
+    def set_feature_history(self, on=True):
+        """sb200_set_feature_history: keep the feature of each of a visual track's last history_length observations for
+        wasted_visual().  Only before the first predict."""
+        check(self._L.sb200_set_feature_history(self._h, 1 if on else 0))
+
+    def feature_history_pool(self):
+        """sb200_feature_history_pool: {"capacity", "handed_out", "free"} blocks of the feature-history pool."""
+        o = np.zeros(3, np.int64)
+        check(self._L.sb200_feature_history_pool(self._h, ptr(o)))
+        return {"capacity": int(o[0]), "handed_out": int(o[1]), "free": int(o[2])}
+
+    def wasted_visual(self, history_cap=None, chunk_bytes=64 << 20):
+        """wasted_history() of every wasted record plus its feature history: `features` is a list of [count][d8]
+        float32 arrays (oldest first, zero-padded to 8 lanes), `feature_present` a list of [count] bool arrays (False: that
+        observation had no feature; its row is zero).  The records are drained in chunks of about `chunk_bytes` of
+        features each."""
+        if history_cap is None:
+            history_cap = max(1, min(64, self.opts.history_length or 64))
+        H = int(history_cap)
+        if H < 0:
+            raise ValueError("history_cap must be >= 0")
+        d8 = (int(self.opts.feature_dim) + 7) // 8 * 8
+        cap = max(1, min(1 << 14, int(chunk_bytes) // max(1, H * d8 * 4)))
+        res = {k: [] for k in ("ids", "scene_ids", "epochs", "lengths", "predicted", "observed", "predicted_history",
+                               "observed_history", "features", "feature_present")}
+        while True:
+            ids, sc = np.zeros(cap, np.uint64), np.zeros(cap, np.uint64)
+            ep, ln = np.zeros(cap, np.uint32), np.zeros(cap, np.uint32)
+            pr, ob = np.zeros((cap, 6), np.float32), np.zeros((cap, 6), np.float32)
+            hp, ho = np.zeros((cap, H, 6), np.float32), np.zeros((cap, H, 6), np.float32)
+            hc = np.zeros(cap, np.int32)
+            ft, fp = np.zeros((cap, H, d8), np.float32), np.zeros((cap, H), np.uint8)
+            n = check(self._L.sb200_wasted_visual(self._h, cap, ptr(ids), ptr(sc), ptr(ep), ptr(ln), ptr(pr), ptr(ob), H,
+                                                  ptr(hp), ptr(ho), ptr(hc), ptr(ft), ptr(fp)))
+            for k, a in (("ids", ids), ("scene_ids", sc), ("epochs", ep), ("lengths", ln), ("predicted", pr), ("observed", ob)):
+                res[k].append(a[:n])
+            for i in range(n):
+                c = hc[i]
+                res["predicted_history"].append(hp[i, :c].copy())
+                res["observed_history"].append(ho[i, :c].copy())
+                res["features"].append(ft[i, :c].copy())
+                res["feature_present"].append(fp[i, :c].astype(bool))
+            if n < cap:
+                break
+        for k in ("ids", "scene_ids", "epochs", "lengths", "predicted", "observed"):
+            res[k] = np.concatenate(res[k])
+        return res
 
     def idle_tracks(self, scene_id=0, cap=1 << 16):
         ids = np.zeros(cap, np.uint64)
