@@ -253,6 +253,41 @@ int sb200_last_stage_ms(sb200_tracker* t, float* out5);
  * [1] scene-mode + exact refinement kernels; 0 when the tensor-core path was not used. */
 int sb200_last_kernel_ms(sb200_tracker* t, float* out2);
 
+/* ---- state blob: save / restore a tracker, move scenes between trackers and GPUs (no reference counterpart: the
+ * reference's state lives in host memory).  One versioned binary format; DESIGN.md section 3b describes it.
+ * `dst` / `src` may be host memory or device memory on any device.  Every entry first waits for the frames in flight
+ * (an error of an asynchronous frame is returned there).  Size query: with dst == NULL or cap too small, save and export
+ * write nothing, set *bytes to the size they need and return SB200_ERR_CAPACITY.  A rejected call changes nothing.
+ * Stream order of a device blob: save, export and import are ordered after what the stream named with
+ * sb200_tracker_set_stream holds when the call is made (a blob the caller is still receiving on that stream is read
+ * after the receive; pending reads of the destination come before it is written) and return after the blob work is
+ * done.  load has no tracker stream yet, and a tracker without a named stream has none to wait for: there a device blob
+ * must be complete when the call is made (e.g. cudaStreamSynchronize on the stream of the receive).
+ * A blob is checked before anything is copied: header, section bounds, alignment and sizes, and every index it carries
+ * (arena blocks, free lists, block owners, observation slots, history blocks) against the counts it declares.
+ * sb200_set_feature_history is refused on a loaded tracker and after an import, as after a predict.
+ *
+ * Whole tracker: options, every scene slot in slot order, the wasted buffer (revealed and hidden records, with box and
+ * feature histories), the id counter, the auto-waste counter and periodicity, the feature dimension state, adapt_dense.
+ * A loaded tracker fed the same requests returns the same results, bit for bit.  load builds its tracker from the
+ * blob's options on `device` (the capacity hints are the blob's); it rejects a scene blob. */
+int sb200_tracker_save(sb200_tracker* t, void* dst, size_t cap, size_t* bytes);
+int sb200_tracker_load(const void* src, size_t bytes, int32_t device, sb200_tracker** out);
+/* Scenes: the live tracks and the epoch of each listed scene (SB200_ERR_INVALID for an unknown id).  remove != 0 takes
+ * them out of the source: the slot starts over (no tracks, epoch 0) and the scene's hidden wasted records stay with the
+ * source until its next collection point.  import checks the format, that every option but the capacity hints and
+ * `device` matches (the constraints up to n_constraints), the feature-history flag, and that no imported scene already
+ * holds tracks or epochs here; the id counter becomes max(its own, the source's at export), so a new id never repeats an
+ * imported one.  The ids the destination's own scenes already hold come from its own counter and may equal imported ids
+ * of other scenes.  import rejects a whole-tracker blob. */
+int sb200_scenes_export(sb200_tracker* t, int32_t n_scenes, const uint64_t* scene_ids, int32_t remove,
+                        void* dst, size_t cap, size_t* bytes);
+int sb200_scenes_import(sb200_tracker* t, const void* src, size_t bytes);
+/* The tracker's options as they stand (feature_dim after sb200_set_feature_dim; a loaded tracker's from its blob) and,
+ * if `feature_dim_fixed` is not NULL, whether a request has carried feature rows (sb200_set_feature_dim then refuses a
+ * change).  No device call. */
+int sb200_tracker_options(sb200_tracker* t, sb200_options* out, int32_t* feature_dim_fixed);
+
 /* ---- stateless operators (host pointers) used by parity tests and by callers that keep their own state ----
  * Positional cost matrix = SortMetric::metric over all pairs (src/trackers/sort/metric.rs:38-77):
  * out[m][n] = IoU*conf (>= thr) or (100 - d^2)/conf, NaN == None.  track_states30 only for Mahalanobis. */

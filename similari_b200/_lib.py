@@ -87,7 +87,8 @@ EXPORTS = [
     "sb200_nms_batch", "sb200_nms_batch_device", "sb200_kalman_distance", "sb200_point_kalman_initiate",
     "sb200_point_kalman_predict", "sb200_point_kalman_update", "sb200_point_kalman_distance", "sb200_box_vertices",
     "sb200_clip_polygons", "sb200_intersection_areas", "sb200_set_feature_history", "sb200_wasted_visual",
-    "sb200_feature_history_pool",
+    "sb200_feature_history_pool", "sb200_tracker_save", "sb200_tracker_load", "sb200_scenes_export",
+    "sb200_scenes_import", "sb200_tracker_options",
 ]
 
 
@@ -138,6 +139,11 @@ def lib():
         "sb200_set_feature_history": (C.c_int, [vp, i32]),
         "sb200_feature_history_pool": (C.c_int, [vp, vp]),
         "sb200_wasted_visual": (i64, [vp, i64, vp, vp, vp, vp, vp, vp, i32, vp, vp, vp, vp, vp]),
+        "sb200_tracker_save": (C.c_int, [vp, vp, C.c_size_t, C.POINTER(C.c_size_t)]),
+        "sb200_tracker_load": (C.c_int, [vp, C.c_size_t, i32, C.POINTER(vp)]),
+        "sb200_scenes_export": (C.c_int, [vp, i32, vp, i32, vp, C.c_size_t, C.POINTER(C.c_size_t)]),
+        "sb200_scenes_import": (C.c_int, [vp, vp, C.c_size_t]),
+        "sb200_tracker_options": (C.c_int, [vp, C.POINTER(Options), C.POINTER(i32)]),
         "sb200_idle_tracks": (i64, [vp, u64, i64, vp, vp, vp, vp, vp]),
         "sb200_scene_tracks": (i64, [vp, u64, i64, vp, vp, vp, vp]),
         "sb200_last_costs": (i64, [vp, u64, i64, vp, C.POINTER(i32), C.POINTER(i32)]),

@@ -259,6 +259,23 @@ class _TrackerBase:
                           Universal2DBox._from_row(w["observed"][i]), scene_id, w["lengths"][i], VotingType.Positional, None)
                 for i in range(len(w["ids"]))]
 
+    def save_state(self) -> np.ndarray:
+        """The whole tracker as a uint8 array (sb200_tracker_save); `load_state` continues it exactly.  An extension with
+        no PyO3 counterpart in the reference."""
+        return self._t.save()
+
+
+class _SceneTransfer:
+    def export_scenes(self, scene_ids, remove=False) -> np.ndarray:
+        """The live tracks and epochs of `scene_ids` as a uint8 array (sb200_scenes_export); remove=True takes the
+        scenes out of this tracker.  An extension with no PyO3 counterpart in the reference."""
+        return self._t.export_scenes([int(s) for s in scene_ids], remove=remove)
+
+    def import_scenes(self, blob):
+        """Adds the scenes of an export_scenes() blob of a tracker with the same options (sb200_scenes_import).  An
+        extension with no PyO3 counterpart in the reference."""
+        self._t.import_scenes(blob)
+
 
 def _sort_options(kind, bbox_history, max_idle_epochs, method, min_confidence, constraints, pw, vw):
     method = method or PositionalMetricType.maha()
@@ -325,7 +342,7 @@ class SortPredictionBatchRequest:
         return None
 
 
-class BatchSort(_TrackerBase):
+class BatchSort(_SceneTransfer, _TrackerBase):
     """src/trackers/sort/batch_api.rs `PyBatchSort` (defaults :391-401)."""
 
     def __init__(self, distance_shards=4, voting_shards=4, bbox_history=1, max_idle_epochs=5, method=None,
@@ -495,6 +512,15 @@ class _VisualBase(_TrackerBase):
         custom = np.array([NONE_ID if o.custom_object_id is None else o.custom_object_id for o in observations], dtype=np.int64)
         return boxes, feats, has, q, custom
 
+    def _kind(self):
+        return _lib.KIND_BATCH_VISUAL_SORT if isinstance(self, BatchVisualSort) else _lib.KIND_VISUAL_SORT
+
+    def save_state(self) -> np.ndarray:
+        """See _TrackerBase.save_state; a tracker that has seen no observation yet saves an empty state."""
+        if self._t is None:
+            self._ensure(self._kind(), [])
+        return self._t.save()
+
     def wasted(self) -> List[WastedVisualSortTrack]:
         if self._t is None:
             return []
@@ -531,7 +557,7 @@ class VisualSort(_VisualBase):
         return self._idle(scene_id)
 
 
-class BatchVisualSort(_VisualBase):
+class BatchVisualSort(_SceneTransfer, _VisualBase):
     """src/trackers/visual_sort/batch_api.rs `PyBatchVisualSort`."""
 
     def __init__(self, distance_shards: int, voting_shards: int, opts: VisualSortOptions):
@@ -554,6 +580,43 @@ class BatchVisualSort(_VisualBase):
 
     def idle_tracks(self, scene_id):
         return self._idle(scene_id)
+
+    def export_scenes(self, scene_ids, remove=False) -> np.ndarray:
+        if self._t is None:
+            self._ensure(self._kind(), [])
+        return _SceneTransfer.export_scenes(self, scene_ids, remove)
+
+    def import_scenes(self, blob):
+        if self._t is None:
+            # the engine tracker is created with the blob's feature length (the options must match anyway)
+            dim = int(engine.blob_options(blob).feature_dim)
+            self._t = engine.Tracker(self._opts._build(self._kind(), dim))
+            self._t.set_feature_history(True)
+            self._dim = dim
+        self._t.import_scenes(blob)
+        # the source's dimension may still have been provisional (no feature seen): then so is this one
+        self._dim_provisional = not self._t.feature_dim_fixed()
+
+
+def load_state(blob, device=0):
+    """A Sort / BatchSort / VisualSort / BatchVisualSort restored from a save_state() blob on `device`, options
+    included; it continues exactly where the saved tracker stood.  An extension with no PyO3 counterpart in the
+    reference."""
+    t = engine.Tracker.load(blob, device=device)
+    o = t.opts
+    cls = {_lib.KIND_SORT: Sort, _lib.KIND_BATCH_SORT: BatchSort, _lib.KIND_VISUAL_SORT: VisualSort,
+           _lib.KIND_BATCH_VISUAL_SORT: BatchVisualSort}[int(o.kind)]
+    obj = cls.__new__(cls)
+    obj._t = t
+    if cls in (VisualSort, BatchVisualSort):
+        opts = VisualSortOptions()
+        for k in opts._kw:
+            opts._kw[k] = getattr(o, k)
+        n = int(o.n_constraints)
+        opts._constraints = [(int(o.constraint_epochs[i]), float(o.constraint_max_dist[i])) for i in range(n)] or None
+        obj._opts, obj._dim = opts, int(o.feature_dim)
+        obj._dim_provisional = not t.feature_dim_fixed()
+    return obj
 
 
 def nms(detections, nms_threshold, score_threshold):

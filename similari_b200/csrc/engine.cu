@@ -272,6 +272,7 @@ struct sb200_tracker {
   unsigned long long acc_dense_scenes = 0;   // scenes the exact SIMT fallback had to take (over all absorbed frames)
   int last_dense_scenes = 0;
   bool seen_features = false;   // a request has carried feature rows (the feature dimension is fixed from then on)
+  bool transferred = false;     // built by sb200_tracker_load or filled by sb200_scenes_import: holds state without a frame
   int last_n_scenes = 0;   // scenes of the last frame (sb200_last_costs reads its scene table back from the device)
 
   ~sb200_tracker() {
@@ -1568,7 +1569,9 @@ int sb200_feature_history_pool(sb200_tracker* t, int64_t* out3) {
 int sb200_set_feature_history(sb200_tracker* t, int32_t on) {
   if (!t) return fail(SB200_ERR_INVALID, "tracker is NULL");
   if (!t->P.is_visual) return fail(SB200_ERR_INVALID, "the feature history belongs to the visual trackers");
-  if (t->frame_seq > 0) return fail(SB200_ERR_INVALID, "the feature history is switched before the first predict");
+  // tracks (and their history blocks) exist once a frame has run or a blob has been loaded / imported
+  if (t->frame_seq > 0 || t->transferred)
+    return fail(SB200_ERR_INVALID, "the feature history is switched before the first predict, load or import");
   return t->set_feature_history(on != 0);
 }
 
@@ -1968,6 +1971,664 @@ int sb200_last_kernel_ms(sb200_tracker* t, float* out2) {
   { int rc_ = t->drain(); if (rc_) return rc_; }
   out2[0] = t->kernel_ms[0];
   out2[1] = t->kernel_ms[1];
+  return 0;
+}
+
+}  // extern "C"
+
+// =============================================================================================== state blob
+// One versioned format for sb200_tracker_save / _load (the whole tracker) and sb200_scenes_export / _import (the live
+// tracks of some scenes).  Layout: BlobHeader, then sections at 256-byte aligned offsets: the scene table (BlobScene per
+// scene, in slot order for a tracker blob), one section per store column holding the listed scenes' rows back to back
+// (live tracks, arena blocks or free-list entries: scene i's rows start at the prefix of the counts before it), then,
+// for a tracker blob, the wasted buffer's records [0, wasted_count) and the feature-history pool (blocks [0, top), free
+// stack [0, free)), or, for a scene blob with the feature history on, the history block of every live track in the
+// order of the track columns.  Rows are copied as they are (BF16 copies, norms, permutations and vertex caches included),
+// so a loaded tracker continues bit for bit.
+namespace {
+
+constexpr uint32_t kBlobMagic = 0x42534253u;   // "SBSB"
+constexpr uint32_t kBlobVersion = 1;
+constexpr uint32_t kBlobTracker = 1, kBlobScenes = 2;
+constexpr int kMaxSections = 48;
+constexpr uint64_t kSecAlign = 256;
+
+struct BlobHeader {
+  uint32_t magic, version, type, n_sections;
+  uint64_t total_bytes;
+  sb200_options opts;
+  int32_t feature_history, hist_len, d8, n_scenes;
+  int32_t seen_features, adapt_dense, auto_waste_counter, auto_waste_periodicity;
+  int32_t scene_cap, track_cap, pad0, pad1;
+  int64_t live_total, blk_total, free_total, wasted_count, revealed, hpool_top, hpool_free, hpool_cap;
+  uint64_t id_counter;   // ids handed out by the source (at export, for a scene blob)
+  uint64_t sec_off[kMaxSections], sec_bytes[kMaxSections];
+};
+struct TmpBuf : DBuf { ~TmpBuf() { release(); } };   // a DBuf freed when it goes out of scope
+struct BlobScene { uint64_t scene_id; uint32_t epoch; int32_t n_tracks, n_hidden, arena_top; };
+
+// a column of the store: rows of `w` bytes per live track (0), per arena block (1) or per free-list entry (2)
+enum ColTag { kTagNone, kTagFblk, kTagHblk, kTagObsN, kTagObsPhys, kTagOwner, kTagFree };
+struct Col { char* base; size_t w; int kind; int tag = kTagNone; };   // tag: index-valued columns a load checks
+
+std::vector<Col> store_cols(const sb200_tracker* t, bool tracker_blob) {
+  const sb::TrackStore& ts = t->ts;
+  const size_t K = (size_t)t->P.max_obs, d8 = (size_t)t->P.d8, H = (size_t)t->hist_len;
+  std::vector<Col> c = {{(char*)ts.id, 8, 0}, {(char*)ts.epoch, 4, 0}, {(char*)ts.length, 4, 0}, {(char*)ts.custom, 8, 0},
+                        {(char*)ts.vt, 1, 0}, {(char*)ts.pred, 24, 0}, {(char*)ts.obs, 24, 0}, {(char*)ts.radius, 4, 0},
+                        {(char*)ts.kst, 4 * (size_t)sb::kStateStride, 0}};
+  if (t->P.positional_kind == SB200_POS_IOU) c.push_back({(char*)ts.vert, 64, 0});
+  if (H > 1) { c.push_back({(char*)ts.hist_pred, 24 * H, 0}); c.push_back({(char*)ts.hist_obs, 24 * H, 0}); }
+  if (t->P.is_visual) {
+    c.push_back({(char*)ts.obs_phys, K, 0, kTagObsPhys}); c.push_back({(char*)ts.obs_hasf, K, 0});
+    c.push_back({(char*)ts.obs_q, 4 * K, 0});
+    c.push_back({(char*)ts.obs_n, 1, 0, kTagObsN}); c.push_back({(char*)ts.feat_cnt, 1, 0});
+    c.push_back({(char*)ts.fblk, 4, 0, kTagFblk});
+    // a scene blob carries the history rows themselves (renumbered on import), a tracker blob the pool and the indices
+    if (t->fhist_on && tracker_blob) c.push_back({(char*)ts.hblk, 4, 0, kTagHblk});
+    c.push_back({(char*)ts.feat, 4 * K * d8, 1}); c.push_back({(char*)ts.feat_bf16, 2 * K * d8, 1});
+    c.push_back({(char*)ts.fnorm2, 4 * K, 1}); c.push_back({(char*)ts.blk_owner, 4, 1, kTagOwner});
+    c.push_back({(char*)ts.blk_free, 4, 2, kTagFree});
+  }
+  return c;
+}
+
+// byte sizes of every section after the scene table, in blob order (the structure depends on the options only)
+std::vector<uint64_t> section_bytes(const sb200_tracker* t, uint32_t type, int64_t n_scenes, int64_t live, int64_t blk,
+                                    int64_t fre, int64_t wasted, int64_t top, int64_t hfree) {
+  std::vector<uint64_t> b = {(uint64_t)n_scenes * sizeof(BlobScene)};
+  const int64_t cnt[3] = {live, blk, fre};
+  for (const Col& c : store_cols(t, type == kBlobTracker)) b.push_back((uint64_t)cnt[c.kind] * c.w);
+  const uint64_t H = (uint64_t)t->hist_len, hrow = H * (uint64_t)t->P.d8 * 4;
+  if (type == kBlobTracker) {
+    for (uint64_t w : {8, 8, 4, 4, 24, 24}) b.push_back((uint64_t)wasted * w);
+    if (H > 1) { b.push_back((uint64_t)wasted * 24 * H); b.push_back((uint64_t)wasted * 24 * H); }
+    if (t->fhist_on) {
+      b.push_back((uint64_t)wasted * 4);
+      b.push_back((uint64_t)top * hrow); b.push_back((uint64_t)top * H); b.push_back((uint64_t)hfree * 4);
+    }
+  } else if (t->fhist_on) {
+    b.push_back((uint64_t)live * hrow); b.push_back((uint64_t)live * H);
+  }
+  return b;
+}
+
+// header sections from their sizes; returns the blob's total size
+uint64_t lay_out(BlobHeader& h, const std::vector<uint64_t>& sec) {
+  uint64_t off = (sizeof(BlobHeader) + kSecAlign - 1) / kSecAlign * kSecAlign;
+  h.n_sections = (uint32_t)sec.size();
+  for (size_t i = 0; i < sec.size(); ++i) {
+    h.sec_off[i] = off;
+    h.sec_bytes[i] = sec[i];
+    off += (sec[i] + kSecAlign - 1) / kSecAlign * kSecAlign;
+  }
+  return off;
+}
+
+// where a blob lives: -1 host memory, else the ordinal of the device that holds it
+int blob_device(const void* p) {
+  cudaPointerAttributes a;
+  if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return -1; }
+  return (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) ? a.device : -1;
+}
+
+// host <-> device copy of a blob through two pinned staging buffers (the copy of one chunk overlaps the host copy of the
+// other); memory that is pinned already is copied in one piece
+int host_copy(cudaStream_t st, void* host, void* dev, size_t n, bool to_host) {
+  cudaPointerAttributes a;
+  const bool pinned = cudaPointerGetAttributes(&a, host) == cudaSuccess && a.type == cudaMemoryTypeHost;
+  cudaGetLastError();
+  if (pinned || n <= (1u << 20)) {
+    CU(to_host ? cudaMemcpyAsync(host, dev, n, cudaMemcpyDeviceToHost, st) : cudaMemcpyAsync(dev, host, n, cudaMemcpyHostToDevice, st));
+    CU(cudaStreamSynchronize(st));
+    return 0;
+  }
+  constexpr size_t kStage = 32u << 20;
+  struct Stage {
+    void* p[2] = {nullptr, nullptr};
+    cudaEvent_t ev[2] = {nullptr, nullptr};
+    ~Stage() { for (int i = 0; i < 2; ++i) { if (p[i]) cudaFreeHost(p[i]); if (ev[i]) cudaEventDestroy(ev[i]); } }
+  } sg;
+  for (int i = 0; i < 2; ++i) {
+    CU(cudaHostAlloc(&sg.p[i], kStage, cudaHostAllocDefault));
+    CU(cudaEventCreateWithFlags(&sg.ev[i], cudaEventDisableTiming));
+  }
+  char* h = static_cast<char*>(host);
+  char* d = static_cast<char*>(dev);
+  const size_t nch = (n + kStage - 1) / kStage;
+  auto len = [&](size_t i) { return std::min(kStage, n - i * kStage); };
+  if (to_host) {
+    CU(cudaMemcpyAsync(sg.p[0], d, len(0), cudaMemcpyDeviceToHost, st));
+    CU(cudaEventRecord(sg.ev[0], st));
+    for (size_t i = 0; i < nch; ++i) {
+      if (i + 1 < nch) {
+        CU(cudaMemcpyAsync(sg.p[(i + 1) & 1], d + (i + 1) * kStage, len(i + 1), cudaMemcpyDeviceToHost, st));
+        CU(cudaEventRecord(sg.ev[(i + 1) & 1], st));
+      }
+      CU(cudaEventSynchronize(sg.ev[i & 1]));
+      memcpy(h + i * kStage, sg.p[i & 1], len(i));
+    }
+  } else {
+    for (size_t i = 0; i < nch; ++i) {
+      if (i >= 2) CU(cudaEventSynchronize(sg.ev[i & 1]));   // the copy out of this buffer two chunks ago has finished
+      memcpy(sg.p[i & 1], h + i * kStage, len(i));
+      CU(cudaMemcpyAsync(d + i * kStage, sg.p[i & 1], len(i), cudaMemcpyHostToDevice, st));
+      CU(cudaEventRecord(sg.ev[i & 1], st));
+    }
+  }
+  CU(cudaStreamSynchronize(st));
+  return 0;
+}
+
+struct SlotRows { int slot, n, blk, fre; };
+
+// Pack (dir 0: store -> blob) or unpack (dir 1: blob -> store) of the store columns of `rows` (one per scene, in blob
+// order) and, for a tracker blob, of the wasted buffer and the history pool; `dblob` is on the tracker's device.  For a
+// scene blob with the feature history on, unpack hands the tracks the fresh pool blocks [hist_base, hist_base + live).
+int move_store(sb200_tracker* t, int dir, uint32_t type, const BlobHeader& h, char* dblob, const std::vector<SlotRows>& rows,
+               int hist_base) {
+  const size_t tc = (size_t)t->track_cap;
+  std::vector<sb::XferSeg> segs;
+  auto add = [&](char* store, char* blob, uint64_t bytes) {
+    if (bytes == 0) return;
+    if (dir == 0) segs.push_back({store, blob, bytes});
+    else segs.push_back({blob, store, bytes});
+  };
+  const std::vector<Col> cols = store_cols(t, type == kBlobTracker);
+  for (size_t c = 0; c < cols.size(); ++c) {
+    int64_t pre = 0;
+    for (const SlotRows& r : rows) {
+      const int64_t cnt = cols[c].kind == 0 ? r.n : (cols[c].kind == 1 ? r.blk : r.fre);
+      add(cols[c].base + (size_t)r.slot * tc * cols[c].w, dblob + h.sec_off[1 + c] + (uint64_t)pre * cols[c].w,
+          (uint64_t)cnt * cols[c].w);
+      pre += cnt;
+    }
+  }
+  size_t sec = 1 + cols.size();
+  const uint64_t H = (uint64_t)t->hist_len, hrow = H * (uint64_t)t->P.d8 * 4;
+  if (type == kBlobTracker) {
+    const uint64_t wn = (uint64_t)h.wasted_count;
+    const sb::WastedBuf& wb = t->wb;
+    add((char*)wb.id, dblob + h.sec_off[sec++], wn * 8);
+    add((char*)wb.scene, dblob + h.sec_off[sec++], wn * 8);
+    add((char*)wb.epoch, dblob + h.sec_off[sec++], wn * 4);
+    add((char*)wb.length, dblob + h.sec_off[sec++], wn * 4);
+    add((char*)wb.pred, dblob + h.sec_off[sec++], wn * 24);
+    add((char*)wb.obs, dblob + h.sec_off[sec++], wn * 24);
+    if (H > 1) {
+      add((char*)wb.hist_pred, dblob + h.sec_off[sec++], wn * 24 * H);
+      add((char*)wb.hist_obs, dblob + h.sec_off[sec++], wn * 24 * H);
+    }
+    if (t->fhist_on) {
+      add((char*)wb.hblk, dblob + h.sec_off[sec++], wn * 4);
+      add((char*)t->ts.hrows, dblob + h.sec_off[sec++], (uint64_t)h.hpool_top * hrow);
+      add((char*)t->ts.hpresent, dblob + h.sec_off[sec++], (uint64_t)h.hpool_top * H);
+      add((char*)t->ts.hfree, dblob + h.sec_off[sec++], (uint64_t)h.hpool_free * 4);
+    }
+  }
+  const cudaStream_t st = t->stream;
+  if (!segs.empty()) {
+    std::vector<long long> cpre(segs.size() + 1, 0);
+    for (size_t i = 0; i < segs.size(); ++i)
+      cpre[i + 1] = cpre[i] + (long long)((segs[i].bytes + sb::kXferChunk - 1) / sb::kXferChunk);
+    TmpBuf d_tab;
+    const size_t sb_ = segs.size() * sizeof(sb::XferSeg);
+    int rc = d_tab.ensure(sb_ + cpre.size() * sizeof(long long));
+    if (rc) return rc;
+    CU(cudaMemcpyAsync(d_tab.p, segs.data(), sb_, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(d_tab.as<char>() + sb_, cpre.data(), cpre.size() * sizeof(long long), cudaMemcpyHostToDevice, st));
+    const int e = sb::launch_xfer_copy(d_tab.as<sb::XferSeg>(), reinterpret_cast<const long long*>(d_tab.as<char>() + sb_),
+                                       (int)segs.size(), cpre.back(), t->num_sms, st);
+    if (e) return fail(SB200_ERR_CUDA, "state copy launch failed: %s", cudaGetErrorString((cudaError_t)e));
+    CU(cudaStreamSynchronize(st));
+  }
+  if (type == kBlobScenes && t->fhist_on && h.live_total > 0) {
+    std::vector<int> tab(2 * rows.size() + 1, 0);   // slots | prefix of the live tracks
+    for (size_t i = 0; i < rows.size(); ++i) { tab[i] = rows[i].slot; tab[rows.size() + i + 1] = tab[rows.size() + i] + rows[i].n; }
+    TmpBuf d_tab;
+    int rc = d_tab.ensure(tab.size() * sizeof(int));
+    if (rc) return rc;
+    CU(cudaMemcpyAsync(d_tab.p, tab.data(), tab.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+    const int e = sb::launch_xfer_hist(t->ts, t->P.d8, d_tab.as<int>(), d_tab.as<int>() + rows.size(), (int)rows.size(),
+                                       (int)h.live_total, dir, reinterpret_cast<float*>(dblob + h.sec_off[sec]),
+                                       reinterpret_cast<unsigned char*>(dblob + h.sec_off[sec + 1]), hist_base, t->num_sms, st);
+    if (e) return fail(SB200_ERR_CUDA, "history copy launch failed: %s", cudaGetErrorString((cudaError_t)e));
+    CU(cudaStreamSynchronize(st));
+  }
+  return 0;
+}
+
+// Checks, on the device, every index a blob carries before anything is copied into the store: a track's arena block,
+// the free list and the block owners against the scene's arena, observation counts and permutations against K, history
+// block indices against the pool.  A damaged blob is refused instead of turning into out-of-bounds accesses later.
+int check_indices(sb200_tracker* t, uint32_t type, const BlobHeader& h, const char* dblob,
+                  const std::vector<BlobScene>& table) {
+  std::vector<sb::XferCheck> ck;
+  const std::vector<Col> cols = store_cols(t, type == kBlobTracker);
+  const int K = t->P.max_obs;
+  const char* obs_n_sec = nullptr;
+  for (size_t c = 0; c < cols.size(); ++c)
+    if (cols[c].tag == kTagObsN) obs_n_sec = dblob + h.sec_off[1 + c];
+  for (size_t c = 0; c < cols.size(); ++c) {
+    if (cols[c].tag == kTagNone) continue;
+    const char* sec = dblob + h.sec_off[1 + c];
+    int64_t pre = 0;
+    for (const BlobScene& s : table) {
+      const int fre = s.arena_top - s.n_tracks;
+      const int64_t cnt = cols[c].kind == 0 ? s.n_tracks : (cols[c].kind == 1 ? s.arena_top : fre);
+      const char* p = sec + (uint64_t)pre * cols[c].w;
+      switch (cols[c].tag) {
+        case kTagFblk: case kTagFree: ck.push_back({p, nullptr, cnt, 0, s.arena_top, 0}); break;
+        case kTagOwner: ck.push_back({p, nullptr, cnt, -1, s.n_tracks, 0}); break;
+        case kTagHblk: ck.push_back({p, nullptr, cnt, 0, (int)h.hpool_top, 0}); break;
+        case kTagObsN: ck.push_back({p, nullptr, cnt, 0, K + 1, 1}); break;
+        case kTagObsPhys: ck.push_back({p, reinterpret_cast<const unsigned char*>(obs_n_sec) + pre, cnt, 0, K, 2}); break;
+        default: break;
+      }
+      pre += cnt;
+    }
+  }
+  if (type == kBlobTracker && t->fhist_on) {
+    const size_t sec = 1 + cols.size() + 6 + (t->hist_len > 1 ? 2 : 0);   // wasted hblk, then rows, present, free stack
+    ck.push_back({dblob + h.sec_off[sec], nullptr, h.wasted_count, 0, (int)h.hpool_top, 0});
+    ck.push_back({dblob + h.sec_off[sec + 3], nullptr, h.hpool_free, 0, (int)h.hpool_top, 0});
+  }
+  ck.erase(std::remove_if(ck.begin(), ck.end(), [](const sb::XferCheck& x) { return x.n <= 0; }), ck.end());
+  if (ck.empty()) return 0;
+  TmpBuf d;
+  int rc = d.ensure(ck.size() * sizeof(sb::XferCheck) + 16);
+  if (rc) return rc;
+  int* d_bad = reinterpret_cast<int*>(d.as<char>() + ck.size() * sizeof(sb::XferCheck));
+  CU(cudaMemcpyAsync(d.p, ck.data(), ck.size() * sizeof(sb::XferCheck), cudaMemcpyHostToDevice, t->stream));
+  CU(cudaMemsetAsync(d_bad, 0, sizeof(int), t->stream));
+  const int e = sb::launch_xfer_check(d.as<sb::XferCheck>(), (int)ck.size(), K, d_bad, t->stream);
+  if (e) return fail(SB200_ERR_CUDA, "index check launch failed: %s", cudaGetErrorString((cudaError_t)e));
+  int bad = 0;
+  CU(cudaMemcpyAsync(&bad, d_bad, sizeof(int), cudaMemcpyDeviceToHost, t->stream));
+  CU(cudaStreamSynchronize(t->stream));
+  if (bad) return fail(SB200_ERR_INVALID, "the blob holds %d out-of-range block or observation indices", bad);
+  return 0;
+}
+
+// sets the device counters of the listed slots (and, for removed scenes, frees their history blocks); see XferSlot
+int set_slots(sb200_tracker* t, const std::vector<sb::XferSlot>& tab, int free0, int free_add, int top_add,
+              unsigned long long id_min, bool raise_ids) {
+  if (tab.empty()) return 0;
+  TmpBuf d_tab;
+  int rc = d_tab.ensure(tab.size() * sizeof(sb::XferSlot));
+  if (rc) return rc;
+  CU(cudaMemcpyAsync(d_tab.p, tab.data(), tab.size() * sizeof(sb::XferSlot), cudaMemcpyHostToDevice, t->stream));
+  const int e = sb::launch_xfer_slots(d_tab.as<sb::XferSlot>(), (int)tab.size(), t->b_ntracks.as<int>(), t->ts.n_free,
+                                      t->ts.arena_top, t->ts, free0, free_add, top_add,
+                                      raise_ids ? t->b_idc.as<unsigned long long>() : nullptr, id_min, t->stream);
+  if (e) return fail(SB200_ERR_CUDA, "slot update launch failed: %s", cudaGetErrorString((cudaError_t)e));
+  CU(cudaStreamSynchronize(t->stream));
+  return 0;
+}
+
+uint64_t read_id_counter(sb200_tracker* t, int* rc) {
+  uint64_t v = 0;
+  *rc = 0;
+  if (!t->b_idc.p) return 0;
+  cudaError_t e = cudaMemcpyAsync(&v, t->b_idc.p, 8, cudaMemcpyDeviceToHost, t->stream);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(t->stream);
+  if (e != cudaSuccess) *rc = fail(SB200_ERR_CUDA, "id counter read failed: %s", cudaGetErrorString(e));
+  return v;
+}
+
+// Writes the blob of `slots` (type kBlobScenes) or of the whole tracker to `dst` (host, or device memory on any device).
+int save_blob(sb200_tracker* t, uint32_t type, const std::vector<int>& slots, void* dst, size_t cap, size_t* bytes) {
+  BlobHeader h;
+  memset(&h, 0, sizeof(h));
+  h.magic = kBlobMagic; h.version = kBlobVersion; h.type = type;
+  h.opts = t->opts;
+  h.feature_history = t->fhist_on; h.hist_len = t->hist_len; h.d8 = t->P.d8; h.n_scenes = (int32_t)slots.size();
+  h.seen_features = t->seen_features;
+  if (type == kBlobTracker) {   // tracker-wide state: a scene blob carries the scenes alone
+    h.adapt_dense = t->adapt_dense;
+    h.auto_waste_counter = t->auto_waste_counter; h.auto_waste_periodicity = t->auto_waste_periodicity;
+    h.scene_cap = t->scene_cap; h.track_cap = t->track_cap;
+  }
+  std::vector<BlobScene> table(slots.size());
+  std::vector<SlotRows> rows(slots.size());
+  for (size_t i = 0; i < slots.size(); ++i) {
+    const int s = slots[i];
+    const int blk = t->P.is_visual ? t->arena_top[s] : 0;
+    table[i] = {t->scene_of_slot[s], t->epoch[s], t->n_tracks[s], type == kBlobTracker ? t->n_hidden[s] : 0, blk};
+    rows[i] = {s, t->n_tracks[s], blk, t->P.is_visual ? blk - t->n_tracks[s] : 0};
+    h.live_total += rows[i].n; h.blk_total += rows[i].blk; h.free_total += rows[i].fre;
+  }
+  if (type == kBlobTracker) {
+    h.wasted_count = t->wasted_count; h.revealed = t->revealed;
+    h.hpool_top = t->fhist_on ? t->hpool_top : 0; h.hpool_free = t->fhist_on ? t->hpool_free : 0;
+    h.hpool_cap = t->fhist_on ? t->hpool_cap : 0;
+  }
+  int rc = 0;
+  h.id_counter = read_id_counter(t, &rc);
+  if (rc) return rc;
+  const uint64_t total = lay_out(h, section_bytes(t, type, h.n_scenes, h.live_total, h.blk_total, h.free_total,
+                                                  h.wasted_count, h.hpool_top, h.hpool_free));
+  h.total_bytes = total;
+  *bytes = (size_t)total;
+  if (!dst || cap < total) return fail(SB200_ERR_CAPACITY, "the blob needs %llu bytes", (unsigned long long)total);
+  const int where = blob_device(dst);
+  TmpBuf tmp;
+  char* dblob = static_cast<char*>(dst);
+  if (where != t->device) {
+    if ((rc = tmp.ensure(total))) return rc;
+    dblob = tmp.as<char>();
+  }
+  CU(cudaMemcpyAsync(dblob, &h, sizeof(h), cudaMemcpyHostToDevice, t->stream));
+  {   // the alignment gaps after the header and every section are zero (equal states give equal blobs)
+    uint64_t end = sizeof(h);
+    for (uint32_t i = 0; i <= h.n_sections; ++i) {
+      const uint64_t next = i < h.n_sections ? h.sec_off[i] : total;
+      if (next > end) CU(cudaMemsetAsync(dblob + end, 0, next - end, t->stream));
+      if (i < h.n_sections) end = h.sec_off[i] + h.sec_bytes[i];
+    }
+  }
+  if (!table.empty())
+    CU(cudaMemcpyAsync(dblob + h.sec_off[0], table.data(), table.size() * sizeof(BlobScene), cudaMemcpyHostToDevice, t->stream));
+  if ((rc = move_store(t, 0, type, h, dblob, rows, 0))) return rc;
+  if (where == t->device) return 0;
+  if (where >= 0) {
+    CU(cudaMemcpyPeerAsync(dst, where, dblob, t->device, total, t->stream));
+    CU(cudaStreamSynchronize(t->stream));
+    return 0;
+  }
+  return host_copy(t->stream, dst, dblob, total, true);
+}
+
+// Orders the tracker's work after what the caller's stream (sb200_tracker_set_stream) holds now, as predict does: a device
+// blob that the caller's stream is still writing (a receive) or reading (a send) is complete before the blob calls touch it.
+int join_caller(sb200_tracker* t) {
+  if (!t->has_user_stream) return 0;
+  if (!t->ev_user_in) {
+    CU(cudaEventCreateWithFlags(&t->ev_user_in, cudaEventDisableTiming));
+    CU(cudaEventCreateWithFlags(&t->ev_user_out, cudaEventDisableTiming));
+  }
+  CU(cudaEventRecord(t->ev_user_in, t->user_stream));
+  CU(cudaStreamWaitEvent(t->stream, t->ev_user_in, 0));
+  return 0;
+}
+
+// every option an import compares: all but the capacity hints and the device; the constraints up to n_constraints
+bool same_options(const sb200_options& a, const sb200_options& b) {
+  auto f = [](float x, float y) { return x == y || (x != x && y != y); };
+  if (a.kind != b.kind || a.positional_kind != b.positional_kind || !f(a.iou_threshold, b.iou_threshold) ||
+      !f(a.min_confidence, b.min_confidence) || a.max_idle_epochs != b.max_idle_epochs || a.history_length != b.history_length ||
+      !f(a.kalman_position_weight, b.kalman_position_weight) || !f(a.kalman_velocity_weight, b.kalman_velocity_weight) ||
+      a.n_constraints != b.n_constraints || a.visual_kind != b.visual_kind || !f(a.visual_threshold, b.visual_threshold) ||
+      a.feature_dim != b.feature_dim || a.visual_max_observations != b.visual_max_observations ||
+      a.visual_min_votes != b.visual_min_votes || a.visual_minimal_track_length != b.visual_minimal_track_length ||
+      !f(a.visual_minimal_area, b.visual_minimal_area) || !f(a.visual_minimal_quality_use, b.visual_minimal_quality_use) ||
+      !f(a.visual_minimal_quality_collect, b.visual_minimal_quality_collect) ||
+      !f(a.visual_minimal_own_area_percentage_use, b.visual_minimal_own_area_percentage_use) ||
+      !f(a.visual_minimal_own_area_percentage_collect, b.visual_minimal_own_area_percentage_collect))
+    return false;
+  const int n = std::min(std::max(a.n_constraints, 0), SB200_MAX_CONSTRAINTS);
+  for (int i = 0; i < n; ++i)
+    if (a.constraint_epochs[i] != b.constraint_epochs[i] || !f(a.constraint_max_dist[i], b.constraint_max_dist[i])) return false;
+  return true;
+}
+
+// Reads and checks the header and the scene table of a blob (host or device memory): magic, version, type, the
+// section table against the sizes the counts imply, and the bounds of every section.
+int parse_blob(const void* src, size_t bytes, uint32_t want_type, cudaStream_t st, BlobHeader* h,
+               std::vector<BlobScene>* table) {
+  if (bytes < sizeof(BlobHeader)) return fail(SB200_ERR_INVALID, "the blob is truncated (%zu bytes)", bytes);
+  CU(cudaMemcpyAsync(h, src, sizeof(BlobHeader), cudaMemcpyDefault, st));
+  CU(cudaStreamSynchronize(st));
+  if (h->magic != kBlobMagic) return fail(SB200_ERR_INVALID, "not a state blob (bad magic)");
+  if (h->version != kBlobVersion) return fail(SB200_ERR_INVALID, "state blob version %u (this library reads %u)", h->version, kBlobVersion);
+  if (h->type != want_type)
+    return fail(SB200_ERR_INVALID, h->type == kBlobTracker ? "a whole-tracker blob: use sb200_tracker_load"
+                                                           : "a scene blob: use sb200_scenes_import");
+  if (h->total_bytes > bytes) return fail(SB200_ERR_INVALID, "the blob is truncated (%zu of %llu bytes)", bytes, (unsigned long long)h->total_bytes);
+  if (h->n_sections < 1 || h->n_sections > (uint32_t)kMaxSections) return fail(SB200_ERR_INVALID, "bad section count");
+  // sections in order, aligned as the writer lays them out (the kernels read them with 16-byte accesses), disjoint
+  uint64_t end = sizeof(BlobHeader);
+  for (uint32_t i = 0; i < h->n_sections; ++i) {
+    if (h->sec_off[i] < end || h->sec_off[i] > h->total_bytes || h->sec_bytes[i] > h->total_bytes - h->sec_off[i])
+      return fail(SB200_ERR_INVALID, "section %u lies outside the blob or overlaps the one before", i);
+    if (h->sec_off[i] % kSecAlign != 0) return fail(SB200_ERR_INVALID, "section %u is not aligned", i);
+    end = h->sec_off[i] + h->sec_bytes[i];
+  }
+  if (h->n_scenes < 0 || h->live_total < 0 || h->blk_total < 0 || h->free_total < 0 || h->wasted_count < 0 ||
+      h->revealed < 0 || h->revealed > h->wasted_count || h->hpool_top < 0 || h->hpool_free < 0 || h->hpool_free > h->hpool_top ||
+      h->hpool_cap < 0 || (h->hpool_cap > 0 && h->hpool_cap < h->hpool_top) ||
+      h->sec_bytes[0] != (uint64_t)h->n_scenes * sizeof(BlobScene))
+    return fail(SB200_ERR_INVALID, "inconsistent blob counts");
+  table->resize((size_t)h->n_scenes);
+  if (h->n_scenes > 0)
+  {
+    CU(cudaMemcpyAsync(table->data(), static_cast<const char*>(src) + h->sec_off[0], h->sec_bytes[0], cudaMemcpyDefault, st));
+    CU(cudaStreamSynchronize(st));
+  }
+  int64_t live = 0, blk = 0, hidden = 0;
+  const bool visual = h->opts.kind == SB200_KIND_VISUAL_SORT || h->opts.kind == SB200_KIND_BATCH_VISUAL_SORT;
+  std::unordered_map<uint64_t, int> seen;
+  for (const BlobScene& s : *table) {
+    if (s.n_tracks < 0 || s.n_hidden < 0 || (visual ? s.arena_top < s.n_tracks : s.arena_top != 0))
+      return fail(SB200_ERR_INVALID, "inconsistent counts of scene %llu", (unsigned long long)s.scene_id);
+    if (!seen.emplace(s.scene_id, 1).second) return fail(SB200_ERR_INVALID, "scene %llu appears twice in the blob", (unsigned long long)s.scene_id);
+    live += s.n_tracks; blk += s.arena_top; hidden += s.n_hidden;
+  }
+  if (live != h->live_total || blk != h->blk_total || (visual && h->free_total != blk - live) ||
+      (h->type == kBlobScenes && hidden != 0) || hidden > h->wasted_count - h->revealed)
+    return fail(SB200_ERR_INVALID, "inconsistent blob counts");
+  return 0;
+}
+
+// the section sizes the tracker `t` (built with the blob's options) expects for the blob's counts
+int check_sections(const sb200_tracker* t, const BlobHeader& h) {
+  const std::vector<uint64_t> sec = section_bytes(t, h.type, h.n_scenes, h.live_total, h.blk_total, h.free_total,
+                                                  h.wasted_count, h.hpool_top, h.hpool_free);
+  if (sec.size() != h.n_sections) return fail(SB200_ERR_INVALID, "the blob has %u sections, %zu expected", h.n_sections, sec.size());
+  for (size_t i = 0; i < sec.size(); ++i)
+    if (sec[i] != h.sec_bytes[i]) return fail(SB200_ERR_INVALID, "section %zu holds %llu bytes, %llu expected", i,
+                                              (unsigned long long)h.sec_bytes[i], (unsigned long long)sec[i]);
+  return 0;
+}
+
+// the blob on the tracker's device: `src` itself, or a copy in `tmp`
+int blob_on_device(sb200_tracker* t, const void* src, size_t bytes, DBuf& tmp, const char** out) {
+  const int where = blob_device(src);
+  if (where == t->device) { *out = static_cast<const char*>(src); return 0; }
+  int rc = tmp.ensure(bytes);
+  if (rc) return rc;
+  if (where >= 0) {
+    CU(cudaMemcpyPeerAsync(tmp.p, t->device, src, where, bytes, t->stream));
+    CU(cudaStreamSynchronize(t->stream));
+  } else if ((rc = host_copy(t->stream, const_cast<void*>(src), tmp.p, bytes, false))) {
+    return rc;
+  }
+  *out = tmp.as<const char>();
+  return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int sb200_tracker_save(sb200_tracker* t, void* dst, size_t cap, size_t* bytes) {
+  if (!t || !bytes) return fail(SB200_ERR_INVALID, "tracker / bytes is NULL");
+  if (sb200_device_count() <= 0) return fail(SB200_ERR_CUDA, "no CUDA device available");
+  CU(cudaSetDevice(t->device));
+  int rc = t->drain();
+  if (rc) return rc;
+  if ((rc = join_caller(t))) return rc;   // the caller's pending work on the destination comes first
+  std::vector<int> slots(t->scene_of_slot.size());
+  for (size_t i = 0; i < slots.size(); ++i) slots[i] = (int)i;
+  return save_blob(t, kBlobTracker, slots, dst, cap, bytes);
+}
+
+int sb200_tracker_load(const void* src, size_t bytes, int32_t device, sb200_tracker** out) {
+  if (!src || !out) return fail(SB200_ERR_INVALID, "src / out is NULL");
+  *out = nullptr;
+  const int ndev = sb200_device_count();
+  if (ndev <= 0) return fail(SB200_ERR_CUDA, "no CUDA device available (this library has no CPU execution path)");
+  if (device < 0 || device >= ndev) return fail(SB200_ERR_INVALID, "device %d out of range (%d devices)", device, ndev);
+  BlobHeader h;
+  std::vector<BlobScene> table;
+  // no tracker (and no caller stream) yet: a device blob must be complete when the call is made
+  int rc = parse_blob(src, bytes, kBlobTracker, nullptr, &h, &table);
+  if (rc) return rc;
+  // created without the capacity hints, then sized to the source's store exactly (a save of the loaded tracker is the
+  // same blob), then the hints restored for the growth of later frames
+  sb200_options o = h.opts;
+  o.device = device;
+  o.max_scenes_hint = o.max_tracks_per_scene_hint = o.max_dets_per_scene_hint = 0;
+  sb200_tracker* t = nullptr;
+  if ((rc = sb200_tracker_create(&o, &t))) return rc;
+  struct Guard { sb200_tracker* t; ~Guard() { if (t) sb200_tracker_destroy(t); } } guard{t};
+  t->opts = h.opts;
+  t->opts.device = device;
+  if (h.feature_history && !t->P.is_visual) return fail(SB200_ERR_INVALID, "feature history on a non-visual tracker");
+  if (h.feature_history && (rc = t->set_feature_history(true))) return rc;
+  if (h.hist_len != t->hist_len || h.d8 != t->P.d8) return fail(SB200_ERR_INVALID, "the blob's row sizes do not match its options");
+  if ((rc = check_sections(t, h))) return rc;
+  int max_rows = 0;
+  for (const BlobScene& s : table) max_rows = std::max(max_rows, std::max(s.n_tracks, s.arena_top));
+  if ((h.scene_cap > 0 || !table.empty()) &&
+      (rc = t->ensure_store(std::max<int>(h.scene_cap, (int)table.size()), std::max(std::max(h.track_cap, max_rows), 64))))
+    return rc;
+  if (h.wasted_count > 0 && (rc = t->ensure_wasted(h.wasted_count))) return rc;
+  if (t->fhist_on && h.hpool_cap > 0 && (rc = t->ensure_hpool(std::max(h.hpool_cap, h.hpool_top)))) return rc;
+  if ((rc = t->b_idc.ensure(8))) return rc;
+  const char* dblob = nullptr;
+  TmpBuf tmp;
+  if ((rc = blob_on_device(t, src, (size_t)h.total_bytes, tmp, &dblob))) return rc;
+  if ((rc = check_indices(t, h.type, h, dblob, table))) return rc;
+  std::vector<SlotRows> rows(table.size());
+  std::vector<sb::XferSlot> st(table.size());
+  for (size_t i = 0; i < table.size(); ++i) {
+    const BlobScene& s = table[i];
+    const int fre = t->P.is_visual ? s.arena_top - s.n_tracks : 0;
+    rows[i] = {(int)i, s.n_tracks, s.arena_top, fre};
+    st[i] = {(int)i, s.n_tracks, fre, s.arena_top, 0, 0};
+  }
+  if ((rc = move_store(t, 1, kBlobTracker, h, const_cast<char*>(dblob), rows, 0))) return rc;
+  if ((rc = set_slots(t, st, 0, 0, 0, 0, false))) return rc;
+  CU(cudaMemcpyAsync(t->b_idc.p, &h.id_counter, 8, cudaMemcpyHostToDevice, t->stream));
+  if (h.wasted_count > 0) {
+    const int wc = (int)h.wasted_count;
+    CU(cudaMemcpyAsync(t->w_count.p, &wc, sizeof(int), cudaMemcpyHostToDevice, t->stream));
+  }
+  if (t->fhist_on) {
+    const int hp[2] = {(int)h.hpool_free, (int)h.hpool_top};
+    CU(cudaMemcpyAsync(t->ts.hpool, hp, sizeof(hp), cudaMemcpyHostToDevice, t->stream));
+  }
+  CU(cudaStreamSynchronize(t->stream));
+  // host side: the scene table in slot order and the scalars
+  for (const BlobScene& s : table) {
+    const int slot = t->slot_for(s.scene_id, true);
+    t->epoch[slot] = s.epoch; t->n_tracks[slot] = s.n_tracks; t->n_hidden[slot] = s.n_hidden; t->arena_top[slot] = s.arena_top;
+  }
+  t->wasted_count = h.wasted_count; t->revealed = h.revealed;
+  t->hpool_top = h.hpool_top; t->hpool_free = h.hpool_free;
+  t->auto_waste_counter = h.auto_waste_counter; t->auto_waste_periodicity = h.auto_waste_periodicity;
+  t->adapt_dense = h.adapt_dense != 0; t->seen_features = h.seen_features != 0;
+  t->transferred = true;
+  guard.t = nullptr;
+  *out = t;
+  return 0;
+}
+
+int sb200_scenes_export(sb200_tracker* t, int32_t n_scenes, const uint64_t* scene_ids, int32_t remove, void* dst,
+                        size_t cap, size_t* bytes) {
+  if (!t || !bytes || n_scenes < 1 || !scene_ids) return fail(SB200_ERR_INVALID, "bad arguments");
+  if (sb200_device_count() <= 0) return fail(SB200_ERR_CUDA, "no CUDA device available");
+  CU(cudaSetDevice(t->device));
+  int rc = t->drain();
+  if (rc) return rc;
+  std::vector<int> slots((size_t)n_scenes);
+  std::unordered_map<uint64_t, int> seen;
+  for (int i = 0; i < n_scenes; ++i) {
+    if (!seen.emplace(scene_ids[i], i).second) return fail(SB200_ERR_INVALID, "scene %llu is listed twice", (unsigned long long)scene_ids[i]);
+    slots[i] = t->slot_for(scene_ids[i], false);
+    if (slots[i] < 0) return fail(SB200_ERR_INVALID, "unknown scene %llu", (unsigned long long)scene_ids[i]);
+  }
+  if ((rc = join_caller(t))) return rc;   // the caller's pending work on the destination comes first
+  if ((rc = save_blob(t, kBlobScenes, slots, dst, cap, bytes))) return rc;
+  if (!remove) return 0;
+  // the slots start over: no tracks, no arena, epoch 0; the live tracks' history blocks go back on the pool's free list
+  // (the hidden records of the scenes stay here, with their blocks, until this tracker's next collection point)
+  std::vector<sb::XferSlot> st((size_t)n_scenes);
+  int pushed = 0;
+  for (int i = 0; i < n_scenes; ++i) {
+    const int n = t->fhist_on ? t->n_tracks[slots[i]] : 0;
+    st[i] = {slots[i], 0, 0, 0, n, pushed};
+    pushed += n;
+  }
+  if ((rc = set_slots(t, st, (int)t->hpool_free, pushed, 0, 0, false))) return rc;
+  for (int s : slots) { t->n_tracks[s] = 0; t->arena_top[s] = 0; t->epoch[s] = 0; }
+  t->hpool_free += pushed;
+  return 0;
+}
+
+int sb200_scenes_import(sb200_tracker* t, const void* src, size_t bytes) {
+  if (!t || !src) return fail(SB200_ERR_INVALID, "tracker / src is NULL");
+  if (sb200_device_count() <= 0) return fail(SB200_ERR_CUDA, "no CUDA device available");
+  CU(cudaSetDevice(t->device));
+  int rc = t->drain();
+  if (rc) return rc;
+  BlobHeader h;
+  std::vector<BlobScene> table;
+  if ((rc = join_caller(t))) return rc;   // a blob the caller's stream is still writing is complete from here on
+  if ((rc = parse_blob(src, bytes, kBlobScenes, t->stream, &h, &table))) return rc;
+  if (!same_options(h.opts, t->opts)) return fail(SB200_ERR_INVALID, "the blob's tracker options differ from this tracker's");
+  if ((h.feature_history != 0) != t->fhist_on)
+    return fail(SB200_ERR_INVALID, "the feature history is %s in the blob and %s here", h.feature_history ? "on" : "off", t->fhist_on ? "on" : "off");
+  if ((rc = check_sections(t, h))) return rc;
+  // a scene id that exists here is refused, unless its slot is empty (epoch 0, no tracks: a scene exported with `remove`)
+  std::vector<int> dst_slot(table.size());
+  int next = (int)t->scene_of_slot.size(), max_rows = 0;
+  for (size_t i = 0; i < table.size(); ++i) {
+    const int s = t->slot_for(table[i].scene_id, false);
+    if (s >= 0 && (t->epoch[s] != 0 || t->n_tracks[s] != 0 || t->arena_top[s] != 0))
+      return fail(SB200_ERR_INVALID, "scene %llu already exists in this tracker", (unsigned long long)table[i].scene_id);
+    dst_slot[i] = s >= 0 ? s : next++;
+    max_rows = std::max(max_rows, std::max(table[i].n_tracks, table[i].arena_top));
+  }
+  // ---- checks done: from here on only growth (which preserves the state) can fail before the copies
+  if ((rc = t->ensure_store(std::max(next, t->scene_cap), std::max(std::max(max_rows, t->track_cap), 64)))) return rc;
+  if (!t->b_idc.p) {
+    if ((rc = t->b_idc.ensure(8))) return rc;
+    CU(cudaMemsetAsync(t->b_idc.p, 0, 8, t->stream));
+  }
+  const long long hist_base = t->fhist_on ? t->hpool_top : 0;
+  if (t->fhist_on && hist_base + h.live_total > t->hpool_cap &&
+      (rc = t->ensure_hpool(std::max(hist_base + h.live_total, t->hpool_cap + t->hpool_cap / 2))))
+    return rc;
+  const char* dblob = nullptr;
+  TmpBuf tmp;
+  if ((rc = blob_on_device(t, src, (size_t)h.total_bytes, tmp, &dblob))) return rc;
+  if ((rc = check_indices(t, h.type, h, dblob, table))) return rc;
+  std::vector<SlotRows> rows(table.size());
+  std::vector<sb::XferSlot> st(table.size());
+  for (size_t i = 0; i < table.size(); ++i) {
+    const BlobScene& s = table[i];
+    const int fre = t->P.is_visual ? s.arena_top - s.n_tracks : 0;
+    rows[i] = {dst_slot[i], s.n_tracks, s.arena_top, fre};
+    st[i] = {dst_slot[i], s.n_tracks, fre, s.arena_top, 0, 0};
+  }
+  if ((rc = move_store(t, 1, kBlobScenes, h, const_cast<char*>(dblob), rows, (int)hist_base))) return rc;
+  if ((rc = set_slots(t, st, 0, 0, t->fhist_on ? (int)h.live_total : 0, h.id_counter, true))) return rc;
+  for (size_t i = 0; i < table.size(); ++i) {
+    const int slot = t->slot_for(table[i].scene_id, true);
+    t->epoch[slot] = table[i].epoch; t->n_tracks[slot] = table[i].n_tracks; t->arena_top[slot] = table[i].arena_top;
+  }
+  if (t->fhist_on) t->hpool_top += h.live_total;
+  if (h.seen_features) t->seen_features = true;
+  t->transferred = true;
+  return 0;
+}
+
+int sb200_tracker_options(sb200_tracker* t, sb200_options* out, int32_t* feature_dim_fixed) {
+  if (!t || !out) return fail(SB200_ERR_INVALID, "tracker / out is NULL");
+  *out = t->opts;
+  if (feature_dim_fixed) *feature_dim_fixed = t->seen_features ? 1 : 0;
   return 0;
 }
 

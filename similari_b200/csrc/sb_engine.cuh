@@ -390,6 +390,28 @@ void launch_frame_sweep(const Params& p, const TrackStore& ts, const Frame& f, i
 void launch_hist_gather(const TrackStore& ts, int d8, const int* blk, const unsigned int* lengths, int n, int hist_cap,
                         float* out_rows, unsigned char* out_present, cudaStream_t st);
 
+// state blob (kernels_xfer.cu): pack / unpack as lists of contiguous segments, each cut into kXferChunk-byte chunks;
+// d_cpre[i] = chunks of the segments before i (n_seg + 1 entries)
+constexpr int kXferChunk = 32 * 1024;
+struct XferSeg { const char* src; char* dst; unsigned long long bytes; };
+int launch_xfer_copy(const XferSeg* d_segs, const long long* d_cpre, int n_seg, long long chunks, int num_sms,
+                     cudaStream_t st);
+// feature-history blocks of the tracks of the listed slots (d_pre: prefix of their live tracks, n + 1 entries) in store
+// order: dir 0 gathers them from the pool into rows / pres, dir 1 scatters them to the fresh blocks [base, base + total)
+// and points the tracks' hblk there
+int launch_xfer_hist(const TrackStore& ts, int d8, const int* d_slots, const int* d_pre, int n, int total, int dir,
+                     float* rows, unsigned char* pres, int base, int num_sms, cudaStream_t st);
+// per slot: push the history blocks of its first `push` tracks onto the free list at free0 + push_off (a removed scene),
+// then set its device counters; once: id counter = max(itself, id_min), pool counters {free, top} += {free_add, top_add}
+struct XferSlot { int slot, n_tracks, n_free, arena_top, push, push_off; };
+// range checks of index columns of a blob: kind 0 int32 values in [lo, hi); kind 1 uint8 values in [lo, hi); kind 2
+// rows of K uint8 (observation permutations) whose first aux[i] entries lie in [lo, hi).  *bad counts the violations.
+struct XferCheck { const void* p; const unsigned char* aux; long long n; int lo, hi, kind; };
+int launch_xfer_check(const XferCheck* d_ck, int n, int K, int* bad, cudaStream_t st);
+int launch_xfer_slots(const XferSlot* d_tab, int n, int* d_n_tracks, int* d_n_free, int* d_arena_top,
+                      const TrackStore& ts, int free0, int free_add, int top_add, unsigned long long* id_counter,
+                      unsigned long long id_min, cudaStream_t st);
+
 // stateless operators
 void launch_kalman_ops(int op, float pw, float vw, const float* in30, const float* boxes, int n, float* out30,
                        cudaStream_t st);

@@ -271,6 +271,99 @@ class Tracker:
         check(self._L.sb200_last_kernel_ms(self._h, ptr(out)))
         return {"vis_screen": float(out[0]), "vis_refine": float(out[1])}
 
+    # ---- state blob: save / restore the whole tracker, move scenes between trackers and GPUs
+    def feature_dim_fixed(self):
+        """True once a request has carried feature rows (set_feature_dim then refuses a change)."""
+        o, fixed = Options(), C.c_int32(0)
+        check(self._L.sb200_tracker_options(self._h, C.byref(o), C.byref(fixed)))
+        return bool(fixed.value)
+
+    def save(self):
+        """sb200_tracker_save into host memory: the whole tracker as a uint8 array."""
+        return _host_blob(lambda p, cap, n: self._L.sb200_tracker_save(self._h, p, cap, n))
+
+    def save_device(self, d_ptr, cap):
+        """sb200_tracker_save into device memory (any device) at raw address `d_ptr` of `cap` bytes; returns the bytes
+        written.  d_ptr == 0 returns the size the blob needs and writes nothing."""
+        return _device_blob(lambda p, c, n: self._L.sb200_tracker_save(self._h, p, c, n), d_ptr, cap)
+
+    @classmethod
+    def load(cls, blob_or_ptr, nbytes=None, device=0):
+        """sb200_tracker_load: a new tracker on `device` from a blob of save() (a uint8 array / bytes) or at a raw device
+        address `blob_or_ptr` of `nbytes` bytes.  The options are the blob's."""
+        p, n, keep = _blob_src(blob_or_ptr, nbytes)
+        L = lib()
+        h = C.c_void_p()
+        check(L.sb200_tracker_load(p, n, int(device), C.byref(h)))
+        del keep
+        self = cls.__new__(cls)
+        self._L, self._h = L, h
+        self.opts = Options()
+        check(L.sb200_tracker_options(h, C.byref(self.opts), None))
+        return self
+
+    def export_scenes(self, scene_ids, remove=False, d_ptr=None, cap=None):
+        """sb200_scenes_export: the live tracks and epochs of `scene_ids` as a uint8 array, or, with `d_ptr` (a raw
+        device address of `cap` bytes), into device memory, returning the bytes written (d_ptr == 0: the size needed).
+        remove=True takes the scenes out of this tracker."""
+        sc = np.ascontiguousarray(scene_ids, dtype=np.uint64)
+        fn = lambda p, c, n: self._L.sb200_scenes_export(self._h, len(sc), ptr(sc), 1 if remove else 0, p, c, n)  # noqa: E731
+        if d_ptr is None:
+            return _host_blob(fn)
+        return _device_blob(fn, d_ptr, cap)
+
+    def import_scenes(self, blob_or_ptr, nbytes=None):
+        """sb200_scenes_import of a blob of export_scenes() (uint8 array / bytes, or a raw device address and size)."""
+        p, n, keep = _blob_src(blob_or_ptr, nbytes)
+        check(self._L.sb200_scenes_import(self._h, p, n))
+        del keep
+
+
+_ERR_CAPACITY = -3
+
+
+def _host_blob(call):
+    """Size query, then the blob into a uint8 array."""
+    n = C.c_size_t(0)
+    rc = call(None, 0, C.byref(n))
+    if rc != _ERR_CAPACITY:
+        check(rc)
+    out = np.empty(n.value, np.uint8)
+    check(call(ptr(out), n.value, C.byref(n)))
+    return out[: n.value]
+
+
+def _device_blob(call, d_ptr, cap):
+    n = C.c_size_t(0)
+    if not d_ptr:
+        rc = call(None, 0, C.byref(n))
+        if rc != _ERR_CAPACITY:
+            check(rc)
+        return int(n.value)
+    check(call(C.c_void_p(d_ptr), int(cap), C.byref(n)))
+    return int(n.value)
+
+
+def _blob_src(blob_or_ptr, nbytes):
+    """(void*, size, object to keep alive) of a host blob or a raw device address."""
+    if isinstance(blob_or_ptr, (int, np.integer)):
+        if nbytes is None:
+            raise ValueError("a device blob needs its size (nbytes)")
+        return C.c_void_p(int(blob_or_ptr)), int(nbytes), None
+    a = np.frombuffer(blob_or_ptr, dtype=np.uint8) if isinstance(blob_or_ptr, (bytes, bytearray)) else \
+        np.ascontiguousarray(blob_or_ptr).view(np.uint8).reshape(-1)
+    n = len(a) if nbytes is None else int(nbytes)
+    return ptr(a), n, a
+
+
+def blob_options(blob) -> Options:
+    """The tracker options embedded in a host state blob (save() / export_scenes()); no device call."""
+    a = np.ascontiguousarray(blob).view(np.uint8).reshape(-1)
+    off = 24   # magic, version, type, section count, total size
+    if len(a) < off + C.sizeof(Options):
+        raise _lib.Sb200Error("the blob is truncated")
+    return Options.from_buffer_copy(a[off: off + C.sizeof(Options)].tobytes())
+
 
 class Comm:
     """NCCL communicator of the scene-sharded path (sb200_comm_*): scatter a request from an ingest rank to the ranks that
