@@ -179,7 +179,6 @@ struct sb200_tracker {
   cudaEvent_t ev_cost_done = nullptr;   // the cost kernels of the newest frame have been issued up to here (work stream)
   bool cost_done_valid = false;
   bool set_busy[2]{};
-  bool prep_off = false;
   unsigned long long frame_seq = 0;
   float kernel_ms[2]{};    // screen, refine(+mode) of the last absorbed frame
   bool tc_timed = false;
@@ -211,10 +210,9 @@ struct sb200_tracker {
   unsigned long long host_calls = 0;
   double acc_stage_ms[5]{}, acc_kernel_ms[2]{};
   unsigned long long acc_tc_frames = 0;
-  // side stream of the positional stage (visual trackers): the culled scan runs next to the refinement of the visual
-  // survivors instead of in front of the screen
-  cudaStream_t pos_stream = nullptr;   // side stream: frame tables beside the candidate preparation, sweep beside the feature store
-  bool side_off = false;
+  // high-priority side stream: the frame tables and the screen's column metadata beside the candidate preparation, the
+  // end-of-frame sweep beside the feature store
+  cudaStream_t side_stream = nullptr;
   cudaEvent_t ev_fork[2]{}, ev_join = nullptr;
   float stage_ms[5]{};
   // scene table
@@ -263,7 +261,7 @@ struct sb200_tracker {
   int stg_last = 1;   // staging set used by the most recent predict
   DBuf f_cbox2[2], f_cradius2[2], f_cconf2[2], f_cvert2[2], f_cflags2[2], f_cnorm22[2], f_cbf162[2], f_decided2[2];   // candidate side, two sets
   DBuf f_winner, f_cvt, f_pos, f_vis, f_scenes, f_newcount,
-      f_status, f_featdst, f_apprank, f_appmeta, f_posgq, f_frameout, f_excl, f_prewin, f_own, f_ownovf, f_dyn, f_ws, f_tmeta, f_rowinfo, f_slabc, f_slabm, f_slabmask,
+      f_status, f_featdst, f_apprank, f_appmeta, f_frameout, f_excl, f_prewin, f_own, f_ownovf, f_dyn, f_ws, f_tmeta, f_rowinfo, f_slabc, f_slabm, f_slabmask,
       f_dscene, f_maxc, f_maxcval, f_drowb, f_dcolb, f_slabk, f_scene_max, f_tiles, f_pairs, f_colmeta, f_colgeo, f_colb, f_colvalid, f_rowmeta, f_poslist, f_counters, f_visval;
   int num_sms = 132;
   DBuf o_ids, o_epochs, o_lengths, o_vt, o_pred, o_obs;
@@ -281,7 +279,7 @@ struct sb200_tracker {
                    &b_feat_bf16, &f_scene_max, &f_tiles, &f_pairs, &f_colmeta, &f_colgeo, &f_colb, &f_colvalid, &f_rowmeta, &f_poslist, &f_counters, &f_visval, &b_fnorm2, &b_obs_phys, &b_obs_hasf, &b_obs_q, &b_obs_n, &b_feat_cnt, &b_ntracks, &b_cur_epoch,
                    &b_fblk, &b_blk_owner, &b_blk_free, &b_nfree, &b_atop, &f_frameout, &f_excl, &f_prewin, &f_own, &f_ownovf, &f_dyn, &b_idc, &f_ws, &f_tmeta, &f_rowinfo, &f_slabc, &f_slabm, &f_slabmask, &f_dscene, &f_maxc, &f_maxcval, &f_drowb, &f_dcolb, &f_slabk,
                    &b_scene_ids, &w_count, &w_id, &w_scene, &w_epoch, &w_length, &w_pred, &w_obs, &f_winner, &f_cvt, &f_pos, &f_vis, &f_scenes, &f_newcount, &f_status,
-                   &f_featdst, &f_apprank, &f_appmeta, &f_posgq, &o_ids, &o_epochs, &o_lengths, &o_vt, &o_pred, &o_obs,
+                   &f_featdst, &f_apprank, &f_appmeta, &o_ids, &o_epochs, &o_lengths, &o_vt, &o_pred, &o_obs,
                    &b_hblk, &b_hrows, &b_hpresent, &b_hfree, &b_hpool, &w_hblk, &f_histdst};
     for (DBuf* b : all) b->release();
     for (int k = 0; k < 2; ++k) {
@@ -304,7 +302,7 @@ struct sb200_tracker {
       for (auto& e : q.ev_pos) if (e) cudaEventDestroy(e);
     }
     if (copy_stream) cudaStreamDestroy(copy_stream);
-    if (pos_stream) cudaStreamDestroy(pos_stream);
+    if (side_stream) cudaStreamDestroy(side_stream);
     if (prep_stream) cudaStreamDestroy(prep_stream);
     for (cudaEvent_t e : {ev_user_in, ev_user_out, ev_prep_done, ev_set_free[0], ev_set_free[1], ev_inputs, ev_join_req, ev_cost_done}) if (e) cudaEventDestroy(e);
     for (auto& e : ev_fork) if (e) cudaEventDestroy(e);
@@ -1059,8 +1057,8 @@ int sb200_tracker::predict(int32_t n_scenes, const uint64_t* scene_ids, const in
   f.id_counter = b_idc.as<unsigned long long>();
   f.id_add = P.is_batch ? (long long)total : -1;
   f.dense_bad = tc.dense ? tc.dense_bad : nullptr;
-  // dense positional matrices for every scene only on request (SB200_FULL_COSTS / SB200_NO_FORK: parity of sb200_last_costs)
-  f.pos_dense_all = getenv("SB200_FULL_COSTS") != nullptr || getenv("SB200_NO_FORK") != nullptr;
+  // dense positional matrices for every scene only on request (SB200_FULL_COSTS: parity of sb200_last_costs)
+  f.pos_dense_all = getenv("SB200_FULL_COSTS") != nullptr;
   bool prefetched = false;
   Staging* sin = nullptr;
   // inputs
@@ -1131,15 +1129,6 @@ int sb200_tracker::predict(int32_t n_scenes, const uint64_t* scene_ids, const in
   f.refine_next = f.pos_cnt + 4 * n_scenes;
   f.status = f.pos_cnt + 5 * n_scenes;
   f.dense_cnt = f.pos_cnt + 6 * n_scenes;
-  // SB200_POS_GQ=1 (experiment): gated positional pairs of the frame in one queue, evaluated by a kernel of their own
-  if (getenv("SB200_POS_GQ") != nullptr) {
-    size_t gq_cap = (size_t)std::min<long long>(std::max<long long>(1, std::max<long long>(total, hint_dets) * 24), 1ll << 26);
-    if (const char* e = getenv("SB200_POS_GQ_CAP")) gq_cap = (size_t)std::max(1, atoi(e));   // tests: force the overflow path
-    if ((rc = ENS(f_posgq, 8 * gq_cap))) return rc;
-    f.pos_gq = f_posgq.as<int2>();
-    f.pos_gq_cnt = f.pos_cnt + 6 * n_scenes + 1;
-    f.pos_gq_cap = (int)gq_cap;
-  }
   f.vis_pairs = f_pairs.as<sb::VisPair>();
   f.vis_val = f_visval.as<float>();
   // outputs
@@ -1158,11 +1147,9 @@ int sb200_tracker::predict(int32_t n_scenes, const uint64_t* scene_ids, const in
   }
   // Visual trackers on the tensor-core path evaluate the positional metric lazily: VisualVoting only consults it for
   // candidates the visual BestFit pass left undecided, against tracks that pass did not claim, so the order is
-  // screen -> refine -> BestFit pre-pass (masks) -> culled scan of what is still open -> full voting.  The dense None
-  // fill of the positional matrices runs on a side stream next to the screen.  SB200_FULL_COSTS=1 (every pair is
-  // evaluated, sb200_last_costs is complete) and SB200_NO_FORK=1 keep the plain order.
-  const bool full_costs = getenv("SB200_FULL_COSTS") != nullptr || getenv("SB200_NO_FORK") != nullptr;
-  const bool fork = P.is_visual && tc.use_tc && tc.n_tiles > 0 && !full_costs;
+  // screen -> refine -> BestFit pre-pass (masks) -> culled scan of what is still open -> full voting.
+  // SB200_FULL_COSTS=1 (every pair is evaluated, sb200_last_costs is complete) keeps the plain order.
+  const bool fork = P.is_visual && tc.use_tc && tc.n_tiles > 0 && !f.pos_dense_all;
   if (fork) {
     if ((rc = ENS(f_decided, T)) || (rc = ENS(f_excl, (size_t)scene_cap * track_cap + 16)) || (rc = ENS(f_prewin, T * 4))) return rc;
     f.decided = f_decided.as<unsigned char>();
@@ -1222,50 +1209,41 @@ int sb200_tracker::predict(int32_t n_scenes, const uint64_t* scene_ids, const in
     if (f.in_own) CU(cudaMemcpyAsync(sin->own.p, own_area, n * 4, cudaMemcpyHostToDevice, stream));
   }
   // scene descriptors, tile list, frame scalars; list counters and status words zeroed
-  if (!pos_stream && !side_off) {
-    static const bool off = [] { const char* e = getenv("SB200_SIDE_STREAM"); return e && e[0] == '0'; }();
-    side_off = off;
-    if (!side_off) {
-      int lo = 0, hi = 0;
-      CU(cudaDeviceGetStreamPriorityRange(&lo, &hi));
-      CU(cudaStreamCreateWithPriority(&pos_stream, cudaStreamNonBlocking, hi));
-      for (auto& e : ev_fork) CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-      CU(cudaEventCreateWithFlags(&ev_join, cudaEventDisableTiming));
-    }
+  if (!side_stream) {
+    int lo = 0, hi = 0;
+    CU(cudaDeviceGetStreamPriorityRange(&lo, &hi));
+    CU(cudaStreamCreateWithPriority(&side_stream, cudaStreamNonBlocking, hi));
+    for (auto& e : ev_fork) CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    CU(cudaEventCreateWithFlags(&ev_join, cudaEventDisableTiming));
   }
-  const bool side_ok = pos_stream != nullptr;
   // The frame's tables come from one small CTA: with nothing else to wait for (no own-area derivation, which reads them) it
   // runs beside the candidate preparation, on the side stream, and the main stream joins before the first kernel that reads them.
-  if (!prep_stream && !prep_off) {
-    static const bool off = [] { const char* e = getenv("SB200_PREP_AHEAD"); return e && e[0] == '0'; }();
-    prep_off = off;
-    if (!prep_off) {
-      int lo = 0, hi = 0;
-      CU(cudaDeviceGetStreamPriorityRange(&lo, &hi));
-      CU(cudaStreamCreateWithPriority(&prep_stream, cudaStreamNonBlocking, lo));
-      CU(cudaEventCreateWithFlags(&ev_prep_done, cudaEventDisableTiming));
-      CU(cudaEventCreateWithFlags(&ev_inputs, cudaEventDisableTiming));
-    }
+  if (!prep_stream) {
+    int lo = 0, hi = 0;
+    CU(cudaDeviceGetStreamPriorityRange(&lo, &hi));
+    CU(cudaStreamCreateWithPriority(&prep_stream, cudaStreamNonBlocking, lo));
+    CU(cudaEventCreateWithFlags(&ev_prep_done, cudaEventDisableTiming));
+    CU(cudaEventCreateWithFlags(&ev_inputs, cudaEventDisableTiming));
   }
-  const bool prep_ahead = prep_stream != nullptr && !derive_own && total > 0;
+  const bool prep_ahead = !derive_own && total > 0;
   // (the tables go to the side stream: on the work stream they would move the next frame's preparation squarely under the
   // screen kernel)
-  const bool side_setup = side_ok && !derive_own && total > 0;
+  const bool side_setup = !derive_own && total > 0;
   cudaStream_t s_setup = stream;
   if (side_setup) {
     CU(cudaEventRecord(ev_fork[0], stream));
-    CU(cudaStreamWaitEvent(pos_stream, ev_fork[0], 0));
-    s_setup = pos_stream;
+    CU(cudaStreamWaitEvent(side_stream, ev_fork[0], 0));
+    s_setup = side_stream;
   }
   sb::launch_frame_setup(P, ts, f, reinterpret_cast<const sb::SceneReq*>(q.h_req.dp), n_scenes, b_ntracks.as<int>(), mstep,
                          cstep, tc.dense, f_tiles.as<sb::TcTile>(), f_dyn.as<sb::FrameDyn>(), f_counters.as<int>(), (int)n_counters, s_setup);
   tc.max_init_done = 1;   // frame_setup resets scene_max
   if (side_setup && Pf.is_visual && tc.use_tc && !tc.dense && tc.n_tiles > 0 && max_m > 0 && max_n > 0 && f.in_feat) {
     // the screen's column metadata reads the tables and the store only: it follows the setup on the side stream
-    sb::launch_vis_colmeta(Pf, ts, f, n_scenes, max_n, tc, pos_stream);
+    sb::launch_vis_colmeta(Pf, ts, f, n_scenes, max_n, tc, side_stream);
     tc.colmeta_done = 1;
   }
-  if (side_setup) CU(cudaEventRecord(ev_join, pos_stream));
+  if (side_setup) CU(cudaEventRecord(ev_join, side_stream));
   CU(cudaEventRecord(q.ev[0], stream));
   if (derive_own) {
     // visual_sort/simple_api.rs:110-127: with an own-area threshold and no shares supplied by the caller, the shares come
@@ -1285,10 +1263,8 @@ int sb200_tracker::predict(int32_t n_scenes, const uint64_t* scene_ids, const in
     }
     if (set_busy[cset]) CU(cudaStreamWaitEvent(prep_stream, ev_set_free[cset], 0));
     // ... and not before the frame in front has left its cost kernels: the preparation is HBM traffic that would slow that
-    // frame's tensor-core screen.  SB200_PREP_AFTER=none starts it as early as possible instead, which may shorten the step
-    // at the screen's expense.  The default keeps the tensor-core kernel undisturbed and the step time reproducible.
-    static const bool after_cost = [] { const char* e = getenv("SB200_PREP_AFTER"); return !(e && !strcmp(e, "none")); }();
-    if (after_cost && cost_done_valid) CU(cudaStreamWaitEvent(prep_stream, ev_cost_done, 0));
+    // frame's tensor-core screen.  Waiting keeps the tensor-core kernel undisturbed and the step time reproducible.
+    if (cost_done_valid) CU(cudaStreamWaitEvent(prep_stream, ev_cost_done, 0));
     sb::launch_prep(Pf, f, n_scenes, max_m, prep_stream);
     CU(cudaEventRecord(ev_prep_done, prep_stream));
     CU(cudaStreamWaitEvent(stream, ev_prep_done, 0));
@@ -1323,23 +1299,21 @@ int sb200_tracker::predict(int32_t n_scenes, const uint64_t* scene_ids, const in
     q.pos_forked = true;
   }
   CU(cudaEventRecord(q.ev[3], stream));
-  if (prep_stream) {
-    if (!ev_cost_done) CU(cudaEventCreateWithFlags(&ev_cost_done, cudaEventDisableTiming));
-    CU(cudaEventRecord(ev_cost_done, stream));
-    cost_done_valid = true;
-  }
+  if (!ev_cost_done) CU(cudaEventCreateWithFlags(&ev_cost_done, cudaEventDisableTiming));
+  CU(cudaEventRecord(ev_cost_done, stream));
+  cost_done_valid = true;
   int vr = sb::launch_voting(Pf, ts, f, n_scenes, max_m, max_n, stream);
   if (vr != 0) return fail(SB200_ERR_CUDA, "voting launch failed: %s", cudaGetErrorString((cudaError_t)vr));
   CU(cudaEventRecord(q.ev[4], stream));
   sb::launch_apply(Pf, ts, f, n_scenes, max_m, 0ull, b_ntracks.as<int>(), stream);
   // The sweep (latency-bound, one CTA per scene) and the feature store (HBM-bound) touch disjoint arrays -- a track's feature
   // block is not moved by the compaction -- so the sweep runs on the side stream beside the store; the frame ends at the join.
-  const bool side_sweep = side_ok && Pf.is_visual && f.in_feat && total > 0;
+  const bool side_sweep = Pf.is_visual && f.in_feat && total > 0;
   if (side_sweep) {
     CU(cudaEventRecord(ev_fork[1], stream));
-    CU(cudaStreamWaitEvent(pos_stream, ev_fork[1], 0));
-    sb::launch_frame_sweep(Pf, ts, f, n_scenes, b_ntracks.as<int>(), wb, pos_stream);
-    CU(cudaEventRecord(ev_join, pos_stream));
+    CU(cudaStreamWaitEvent(side_stream, ev_fork[1], 0));
+    sb::launch_frame_sweep(Pf, ts, f, n_scenes, b_ntracks.as<int>(), wb, side_stream);
+    CU(cudaEventRecord(ev_join, side_stream));
     sb::launch_feat_store(Pf, ts, f, stream);
     CU(cudaStreamWaitEvent(stream, ev_join, 0));
   } else {
@@ -1935,7 +1909,7 @@ int64_t sb200_last_costs(sb200_tracker* t, uint64_t scene_id, int64_t cap, float
     CU(cudaMemcpyAsync(&h[0], t->f_counters.as<int>() + si, 4, cudaMemcpyDeviceToHost, t->stream));
     CU(cudaMemcpyAsync(&h[1], t->f_counters.as<int>() + 2 * (size_t)ns + si, 4, cudaMemcpyDeviceToHost, t->stream));
     CU(cudaStreamSynchronize(t->stream));
-    const bool dense_exists = h[1] != 0 || getenv("SB200_FULL_COSTS") != nullptr || getenv("SB200_NO_FORK") != nullptr;
+    const bool dense_exists = h[1] != 0 || getenv("SB200_FULL_COSTS") != nullptr;
     if (dense_exists) {
       CU(cudaMemcpyAsync(out, t->f_pos.as<float>() + d.pos_off, 4 * (size_t)cnt, cudaMemcpyDeviceToHost, t->stream));
       CU(cudaStreamSynchronize(t->stream));

@@ -298,54 +298,29 @@ __device__ __forceinline__ void pos_eval_pair(const Params& p, const TrackStore&
   }
 }
 
-// Hands the CTA's gated pairs to the frame's global queue (one reservation per CTA, coalesced copy); without a global queue,
-// or when it is full, the CTA evaluates them itself, one pair per thread.  All threads of the CTA call this.
+// The CTA evaluates its queue of gated pairs, one pair per thread.  All threads of the CTA call this.
 template <int POS>
 __device__ __forceinline__ void pos_flush_queue(const Params& p, const TrackStore& ts, const Frame& f, const SceneDesc& sc,
-                                                int sidx, size_t tbase, const int2* queue, int qn, bool use_gq, float* out,
-                                                bool wdense, bool wlist, int* s_base) {
-  const int tid = threadIdx.x;
-  int fit = 0;
-  if (use_gq) {
-    // one reservation per CTA; what does not fit any more (the counter only ever grows: no holes) stays with the CTA
-    if (tid == 0) *s_base = qn > 0 ? atomicAdd(f.pos_gq_cnt, qn) : 0;
-    __syncthreads();
-    const int b = *s_base;
-    fit = b >= 0 ? max(0, min(qn, f.pos_gq_cap - b)) : 0;
-    for (int e = tid; e < fit; e += blockDim.x) f.pos_gq[b + e] = make_int2(sidx, (queue[e].x << 16) | queue[e].y);
-  }
-  for (int e = fit + tid; e < qn; e += blockDim.x) {
+                                                int sidx, size_t tbase, const int2* queue, int qn, float* out, bool wdense,
+                                                bool wlist) {
+  for (int e = threadIdx.x; e < qn; e += blockDim.x) {
     const int2 q = queue[e];
     pos_eval_pair<POS>(p, ts, f, sc, sidx, tbase, q.x, q.y, out, wdense, wlist);
   }
   __syncthreads();
 }
 
-// the pairs of the frame's global queue, one per thread
-template <int POS>
-__global__ void __launch_bounds__(256) pos_eval_kernel(Params p, TrackStore ts, Frame f, int wdense_i, int wlist_i) {
-  const int cnt = min(*f.pos_gq_cnt, f.pos_gq_cap);
-  for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < cnt; e += gridDim.x * blockDim.x) {
-    const int2 q = f.pos_gq[e];
-    const SceneDesc& sc = f.scenes[q.x];
-    pos_eval_pair<POS>(p, ts, f, sc, q.x, (size_t)sc.slot * ts.track_cap, q.y >> 16, q.y & 0xffff, f.pos + sc.pos_off, wdense_i != 0,
-                       wlist_i != 0);
-  }
-}
-
 // lazy_pass < 0: plain scan.  0: lazy (visual trackers) -- in scenes whose visual lists are complete only candidates the
 // visual pass left undecided and tracks it did not claim take part; 1: full scan of the scenes that ended in dense mode
 // although their visual lists were complete (their first scan was a lazy one).
 template <int POS>
-__global__ void __launch_bounds__(PS_THREADS, 2) pos_scan_kernel(Params p, TrackStore ts, Frame f, int lazy_pass, int use_gq_i) {
+__global__ void __launch_bounds__(PS_THREADS, 2) pos_scan_kernel(Params p, TrackStore ts, Frame f, int lazy_pass) {
   extern __shared__ __align__(16) unsigned char ps_smem[];
   __shared__ float s_rmax[PS_THREADS / 32];
   __shared__ int s_bad;
   __shared__ int s_qn;
   __shared__ int s_nund;
-  __shared__ int s_gbase;
   __shared__ int s_und[PS_UND];
-  const bool use_gq = use_gq_i != 0 && f.pos_gq != nullptr;
   const int sidx = blockIdx.x;
   const SceneDesc sc = f.scenes[sidx];
   const int N = sc.n, M = sc.m;
@@ -408,7 +383,7 @@ __global__ void __launch_bounds__(PS_THREADS, 2) pos_scan_kernel(Params p, Track
         }
       }
       __syncthreads();
-      pos_flush_queue<POS>(p, ts, f, sc, sidx, tbase, queue, min(s_qn, PS_QCAP), use_gq, out, wdense, wlist, &s_gbase);
+      pos_flush_queue<POS>(p, ts, f, sc, sidx, tbase, queue, min(s_qn, PS_QCAP), out, wdense, wlist);
       return;
     }
     __syncthreads();
@@ -493,12 +468,12 @@ __global__ void __launch_bounds__(PS_THREADS, 2) pos_scan_kernel(Params p, Track
       }
     }
     __syncthreads();
-    // ---- phase 2: the survivors go to the frame's queue (or, without one, are evaluated here, one per thread)
-    pos_flush_queue<POS>(p, ts, f, sc, sidx, tbase, queue, min(s_qn, PS_QCAP), use_gq, out, wdense, wlist, &s_gbase);
+    // ---- phase 2: the survivors are evaluated, one per thread
+    pos_flush_queue<POS>(p, ts, f, sc, sidx, tbase, queue, min(s_qn, PS_QCAP), out, wdense, wlist);
   }
 }
 
-static bool pos_use_dense(int max_n) { return max_n > PS_MAXN || getenv("SB200_POS_DENSE") != nullptr; }
+static bool pos_use_dense(int max_n) { return max_n > PS_MAXN; }
 
 void launch_pos_fill(const Params& p, const Frame& f, int n_scenes, int max_m, int max_n, cudaStream_t st) {
   (void)p;
@@ -528,24 +503,14 @@ static void pos_scan_impl(const Params& p, const TrackStore& ts, const Frame& f,
   // two CTAs fit an SM: with fewer scenes than that, several CTAs per scene (each at least 64 candidates)
   int nsplit = std::max(1, std::min(std::min(16, (max_m + 63) / 64), (2 * kNumSms) / std::max(1, n_scenes)));
   dim3 grid(n_scenes, nsplit);
-  // optional: the gated pairs of passes -1 / 0 go to one queue of the frame and pos_eval_kernel evaluates them
-  // (SB200_POS_GQ=1, off by default: the pairs of a scene are expected to evaluate faster next to the shared-memory copy of its
-  // tracks than spread over the device; kept for experiments)
-  const char* gq_env = getenv("SB200_POS_GQ");   // read per launch: the parity test switches it on inside a running process
-  const bool gq_on = gq_env != nullptr && gq_env[0] == '1';
-  const int use_gq = (gq_on && f.pos_gq != nullptr && lazy_pass != 1) ? 1 : 0;
-  const int wdense = (f.pos_dense_all || lazy_pass == 1) ? 1 : 0, wlist = lazy_pass != 1 ? 1 : 0;
   if (p.positional_kind == 0) {
     cudaFuncSetAttribute(pos_scan_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    pos_scan_kernel<0><<<grid, PS_THREADS, smem, st>>>(p, ts, f, lazy_pass, use_gq);
-    note_launch();
-    if (use_gq) { pos_eval_kernel<0><<<kNumSms * 8, 256, 0, st>>>(p, ts, f, wdense, wlist); note_launch(); }
+    pos_scan_kernel<0><<<grid, PS_THREADS, smem, st>>>(p, ts, f, lazy_pass);
   } else {
     cudaFuncSetAttribute(pos_scan_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    pos_scan_kernel<1><<<grid, PS_THREADS, smem, st>>>(p, ts, f, lazy_pass, use_gq);
-    note_launch();
-    if (use_gq) { pos_eval_kernel<1><<<kNumSms * 8, 256, 0, st>>>(p, ts, f, wdense, wlist); note_launch(); }
+    pos_scan_kernel<1><<<grid, PS_THREADS, smem, st>>>(p, ts, f, lazy_pass);
   }
+  note_launch();
 }
 
 void launch_pos_scan(const Params& p, const TrackStore& ts, const Frame& f, int n_scenes, int max_m, int max_n,

@@ -109,7 +109,6 @@ struct DenseDev {   // device pointers of the path (TcArgs subset, passed by val
   const float* scene_l0; const float* scene_cmax;
   VisPair* maxc; int* maxc_cnt;
   const VisRowMeta* rowmeta;
-  int dbg;   // SB200_DENSE_DBG (timing experiments only, results are wrong): 1 no ws stores, 2 no max candidates, 4 no phase 2
 };
 
 // ------------------------------------------------------------------------------------------------ weight-sum kernel
@@ -274,7 +273,7 @@ vis_wsum_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
           del = fminf(dm * dm >= 4.0f * e ? 0.536f * q : q, e * rsqrt_approx(e));
           del = __fmaf_rn(del, 1.0001f, 1e-6f * (rc + 1.0f));
         }
-        if (row_ok && !(dd.dbg & 1)) *wsp = __halves2half2(__float2half_rn(s_acc), __float2half_ru(del));
+        if (row_ok) *wsp = __halves2half2(__float2half_rn(s_acc), __float2half_ru(del));
         wsp += h.mpad;
         if (FUSED) {
           const float kf = gktf[col];   // block-uniform; 0: the block takes no part in the voting
@@ -310,7 +309,7 @@ vis_wsum_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
               dval = __fmul_rn(x, rsqrt_approx(x));
             }
             // about one element in a thousand
-            if (dval >= eTd[hr] && ((vm >> (cc + cl)) & 1u) && !(dd.dbg & 2))
+            if (dval >= eTd[hr] && ((vm >> (cc + cl)) & 1u))
               dense_append_candidate(dd.maxc, dd.maxc_cnt, h.scene, h.vis_lbase, h.vis_lcap, eg[hr], h.rowB + 8 * j + q2 + cl);
             dist[er[hr]][cc + cl] = dval;
           }
@@ -324,7 +323,7 @@ vis_wsum_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
           const unsigned int vm = (S.vmask[ms][ch >> 1] >> ((ch & 1) * DS_CH)) & 0xffffu;
           distances(ch, vm);
           wg_bar(1 + wg);
-          if (owner && !(dd.dbg & 4)) {
+          if (owner) {
 #pragma unroll
             for (int cc = 0; cc < DS_CH; ++cc) {
               const int col = ch * DS_CH + cc;
@@ -349,7 +348,7 @@ vis_wsum_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
           if ((vm | bm) == 0u) continue;   // uniform over the warpgroup, like every test on vm / bm below: column properties
           distances(ch, vm);
           wg_bar(1 + wg);
-          if (owner && !(dd.dbg & 4)) {
+          if (owner) {
 #pragma unroll
             for (int cc = 0; cc < DS_CH; ++cc) {
               const bool valid = (vm >> cc) & 1u;
@@ -647,30 +646,6 @@ __global__ void __launch_bounds__(SEL_T) vis_dense_select_kernel(Params p, Frame
 }
 
 // ------------------------------------------------------------------------------------------------ host launcher
-typedef CUresult (*EncodeTiledFnD)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                   const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                   CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static EncodeTiledFnD get_encode_d() {
-  static EncodeTiledFnD fn = nullptr;
-  if (!fn) {
-    void* q = nullptr;
-    cudaDriverEntryPointQueryResult qr;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &q, cudaEnableDefault, &qr) == cudaSuccess && q) fn = (EncodeTiledFnD)q;
-  }
-  return fn;
-}
-static int make_map_d(CUtensorMap* m, const void* base, long long rows, int d8, int box_rows) {
-  EncodeTiledFnD enc = get_encode_d();
-  if (!enc) return -1;
-  cuuint64_t dims[2] = {(cuuint64_t)d8, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)d8 * 2};
-  cuuint32_t box[2] = {(cuuint32_t)TC_BK, (cuuint32_t)box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (void*)base, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS ? 0 : -2;
-}
-
 // the max-candidate refinement reuses the refine kernel of kernels_feat_tc.cu on a view of the frame
 int launch_vis_refine(const Params& p, const TrackStore& ts, const Frame& f, int n_scenes, int* nan_flag, cudaStream_t st);
 
@@ -681,7 +656,7 @@ int launch_vis_dense(const Params& p, const TrackStore& ts, const Frame& f, int 
   cudaMemsetAsync(tc.dbg_counts, 0, 8 * 4, st);
   if (tc.n_tiles == 0 || max_m == 0) return 0;
   CUtensorMap mA, mB;
-  if (make_map_d(&mA, f.c_bf16, tc.a_rows, p.d8, TC_BM) || make_map_d(&mB, ts.feat_bf16, tc.b_rows, p.d8, TC_BN / 2)) return -1;
+  if (make_map(&mA, f.c_bf16, tc.a_rows, p.d8, TC_BM) || make_map(&mB, ts.feat_bf16, tc.b_rows, p.d8, TC_BN / 2)) return -1;
   const bool cosine = p.visual_kind == 1;
   // metadata: zeroed masks / maxima, then one thread per arena block
   cudaMemsetAsync(tc.slab_vmask, 0, (size_t)tc.n_slabs_ub * (TC_BN / 32) * 4, st);
@@ -689,6 +664,7 @@ int launch_vis_dense(const Params& p, const TrackStore& ts, const Frame& f, int 
   cudaMemsetAsync(tc.scene_cmax, 0, (size_t)n_scenes * 4, st);
   // block positions past a scene's arena (the last column tile is padded to whole blocks) must read "no voting observations"
   cudaMemsetAsync(tc.slab_ktf, 0, (size_t)tc.n_slabs_ub * TC_BN * 4, st);
+  // SB200_DENSE_GENERIC (tests): the any-K epilogue also for K <= kDenseKClasses
   const bool fused = p.max_obs <= kDenseKClasses && getenv("SB200_DENSE_GENERIC") == nullptr;
   if (fused) {
     cudaMemsetAsync(tc.d_rowb, 0, (size_t)f.total * kDenseKClasses * 4, st);
@@ -709,7 +685,7 @@ int launch_vis_dense(const Params& p, const TrackStore& ts, const Frame& f, int 
     const size_t smem = sizeof(DsSmem) + 1024;
     const void* fn = nullptr;
 #define SB_WSUM(KT) (cosine ? (const void*)vis_wsum_kernel<true, KT> : (const void*)vis_wsum_kernel<false, KT>)
-    switch (p.max_obs) {   // the reference's default is 5 observations per track, its published bench uses 3
+    switch (fused ? p.max_obs : 0) {   // the reference's default is 5 observations per track, its published bench uses 3
       case 1: fn = SB_WSUM(1); break;
       case 2: fn = SB_WSUM(2); break;
       case 3: fn = SB_WSUM(3); break;
@@ -717,7 +693,6 @@ int launch_vis_dense(const Params& p, const TrackStore& ts, const Frame& f, int 
       case 5: fn = SB_WSUM(5); break;
       default: fn = SB_WSUM(0); break;
     }
-    if (getenv("SB200_DENSE_GENERIC")) fn = SB_WSUM(0);   // the any-K epilogue (tests)
 #undef SB_WSUM
     cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return (int)e;
@@ -738,8 +713,6 @@ int launch_vis_dense(const Params& p, const TrackStore& ts, const Frame& f, int 
     dd.slab_colc = tc.slab_colc; dd.slab_cmax = tc.slab_cmax; dd.slab_vmask = tc.slab_vmask;
     dd.slab_bmask = tc.slab_bmask; dd.scene_l0 = tc.scene_l0; dd.scene_cmax = tc.scene_cmax; dd.maxc = tc.maxc;
     dd.maxc_cnt = tc.maxc_cnt; dd.rowmeta = tc.rowmeta;
-    static const int dbg = getenv("SB200_DENSE_DBG") ? atoi(getenv("SB200_DENSE_DBG")) : 0;
-    dd.dbg = dbg;
     const TcTile* d_tiles = tc.d_tiles;
     const int* d_n_tiles = tc.d_n_tiles;
     void* args[] = {(void*)&mA, (void*)&mB, (void*)&p, (void*)&ts, (void*)&f, (void*)&d_tiles, (void*)&d_n_tiles, (void*)&dd};

@@ -549,13 +549,15 @@ __device__ __forceinline__ float reduce_add8_tc(const float* t) {
   return d0 + d1;
 }
 
-// A warp takes 32 pairs at a time.  Phase 1 (cooperative, coalesced): for every pair the lanes compute the 8-element
+// A warp takes RF_CLAIM pairs at a time.  Phase 1 (cooperative, coalesced): for every pair the lanes compute the 8-element
 // block sums s_blk = reduce_add8(...) of up to 64 blocks and park them in shared memory.  Phase 2: lane p owns pair p and
-// adds its block sums strictly in block order, acc = (..((0 + s_0) + s_1) + ..), which is the reference's order; the 32
+// adds its block sums strictly in block order, acc = (..((0 + s_0) + s_1) + ..), which is the reference's order; the
 // serial chains run side by side instead of one 64-step shuffle chain per pair.
 constexpr int RF_WARPS = 4;
 constexpr int RF_SEG = 64;             // blocks per segment
 constexpr int RF_PITCH = RF_SEG + 1;   // +1: lane p reads row p, rows must start in different banks
+// 16 survivors per claim rather than 32: half the parked block sums, so eight CTAs fit an SM instead of six
+constexpr int RF_CLAIM = 16;
 
 // a-side of a block sum: the candidate's 8 features of block `blk` (zero padded past D on the TAIL path)
 template <bool TAIL>
@@ -583,9 +585,9 @@ __device__ __forceinline__ float refine_block_sum(const float* av, const float* 
   return reduce_add8_tc(t);
 }
 
-template <bool COSINE, bool TAIL, int RP>
-__global__ void __launch_bounds__(RF_WARPS * 32, RP == 32 ? 6 : 8) vis_refine_kernel(Params p, TrackStore ts, Frame f, int* nan_flag) {
-  __shared__ float s_bs[RF_WARPS][RP][RF_PITCH];
+template <bool COSINE, bool TAIL>
+__global__ void __launch_bounds__(RF_WARPS * 32, 8) vis_refine_kernel(Params p, TrackStore ts, Frame f, int* nan_flag) {
+  __shared__ float s_bs[RF_WARPS][RF_CLAIM][RF_PITCH];
   const int scene = blockIdx.y;
   if (f.vis_mode[scene] != 0) return;  // survivor list overflowed: this scene is computed densely
   const SceneDesc sc = f.scenes[scene];
@@ -595,13 +597,13 @@ __global__ void __launch_bounds__(RF_WARPS * 32, RP == 32 ? 6 : 8) vis_refine_ke
   const int D = p.feature_dim;
   float (*bs)[RF_PITCH] = s_bs[w];
   float vmax = nanf("");
-  // warps claim RP survivors at a time from the scene's counter: however many survive, the scene's warps finish together
+  // warps claim RF_CLAIM survivors at a time from the scene's counter: however many survive, the scene's warps finish together
   for (;;) {
     int i0 = 0;
-    if (lane == 0) i0 = atomicAdd(f.refine_next + scene, RP);
+    if (lane == 0) i0 = atomicAdd(f.refine_next + scene, RF_CLAIM);
     i0 = __shfl_sync(0xffffffffu, i0, 0);
     if (i0 >= n_pairs) break;
-    const int npair = min(RP, n_pairs - i0);
+    const int npair = min(RF_CLAIM, n_pairs - i0);
     VisPair mine;
     mine.g = 0; mine.row = 0; mine.scene = 0; mine.outcol = 0;
     if (lane < npair) mine = f.vis_pairs[sc.vis_lbase + i0 + lane];
@@ -651,145 +653,6 @@ __global__ void __launch_bounds__(RF_WARPS * 32, RP == 32 ? 6 : 8) vis_refine_ke
     }
   }
   // one atomic per warp
-  unsigned int u = 0u;
-  if (!is_nan(vmax)) {
-    u = __float_as_uint(vmax);
-    u = (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) u = max(u, __shfl_xor_sync(0xffffffffu, u, o));
-  if (lane == 0 && u != 0u) atomicMax(f.scene_max + scene, u);
-}
-
-// ------------------------------------------------------------------------------------------------ refine, asynchronous copies
-// Same arithmetic, different data movement.  The register-staged kernel above keeps about 4 KB per warp in flight and has
-// none in flight while a warp adds its serial chains, so it tends to be latency-bound.  Here every warp owns a ring of three shared-memory stages and feeds it with cp.async (16-byte chunks, no
-// registers held): while it turns the rows of stage s into block sums, the copies of stages s+1 and s+2 -- 16 KB -- are in
-// flight, whatever the warp is doing.  A stage holds the 512-float segments of both rows of two pairs; chunks are stored
-// half-block-major so that the 16-byte reads of the block sums hit 32 different banks.  The 64 block sums of 32 pairs are
-// parked as before and added in the reference's order by 32 lanes side by side.
-constexpr int RA_WARPS = 6;
-constexpr int RA_STAGES = 3;
-constexpr int RA_PAIRS = 2;                        // pairs per stage
-constexpr int RA_SEGF = RF_SEG * 8;                // floats per row segment (512)
-constexpr int RA_STAGE_FLOATS = RA_PAIRS * 2 * RA_SEGF;   // 2048 floats = 8 KB
-
-__device__ __forceinline__ void cp_async16(void* smem_dst, const void* gsrc) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(smem_dst)), "l"(gsrc) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
-
-template <bool COSINE>
-__global__ void __launch_bounds__(RA_WARPS * 32) vis_refine_async_kernel(Params p, TrackStore ts, Frame f, int* nan_flag) {
-  extern __shared__ __align__(16) unsigned char ra_smem[];
-  const int scene = blockIdx.y;
-  if (f.vis_mode[scene] != 0) return;  // survivor list overflowed: this scene is computed densely
-  const SceneDesc sc = f.scenes[scene];
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  float* stage0 = reinterpret_cast<float*>(ra_smem) + (size_t)w * (RA_STAGES * RA_STAGE_FLOATS + 32 * RF_PITCH);
-  float (*bs)[RF_PITCH] = reinterpret_cast<float (*)[RF_PITCH]>(stage0 + RA_STAGES * RA_STAGE_FLOATS);
-  const int n_pairs = min(f.vis_cnt[scene], sc.vis_lcap);
-  const int nblk = p.d8 / 8;
-  const int D = p.feature_dim;   // == d8 on this path, rows 16-byte aligned
-  float vmax = nanf("");
-  for (;;) {
-    int i0 = 0;
-    if (lane == 0) i0 = atomicAdd(f.refine_next + scene, 32);
-    i0 = __shfl_sync(0xffffffffu, i0, 0);
-    if (i0 >= n_pairs) break;
-    const int npair = min(32, n_pairs - i0);
-    VisPair mine;
-    mine.g = 0; mine.row = 0; mine.scene = 0; mine.outcol = 0;
-    if (lane < npair) mine = f.vis_pairs[sc.vis_lbase + i0 + lane];
-    float acc = 0.0f;
-    const int nst = (npair + RA_PAIRS - 1) / RA_PAIRS;   // stages of this batch
-    for (int seg0 = 0; seg0 < nblk; seg0 += RF_SEG) {
-      const int segn = min(RF_SEG, nblk - seg0);          // blocks of this segment
-      const int nchunk = segn * 2;                        // 16-byte chunks per row segment
-      auto issue = [&](int st) {
-        if (st < nst) {
-          float* dst = stage0 + (st % RA_STAGES) * RA_STAGE_FLOATS;
-#pragma unroll
-          for (int pi = 0; pi < RA_PAIRS; ++pi) {
-            const int pp = st * RA_PAIRS + pi;
-            const int g = __shfl_sync(0xffffffffu, mine.g, pp & 31);
-            const int row = __shfl_sync(0xffffffffu, mine.row, pp & 31);
-            if (pp < npair) {
-              const float* a = f.in_feat + (size_t)g * D + seg0 * 8;
-              const float* b = ts.feat + (size_t)row * p.d8 + seg0 * 8;
-              float* da = dst + (pi * 2) * RA_SEGF;
-              float* db = da + RA_SEGF;
-#pragma unroll
-              for (int c = 0; c < RA_SEGF / 4 / 32; ++c) {
-                const int q = c * 32 + lane;   // chunk q = half (q & 1) of block (q >> 1); stored half-major
-                if (q < nchunk) {
-                  const int pos = ((q & 1) * RF_SEG + (q >> 1)) * 4;
-                  cp_async16(da + pos, a + q * 4);
-                  cp_async16(db + pos, b + q * 4);
-                }
-              }
-            }
-          }
-        }
-        cp_async_commit();   // always: the group count stays in step with the stage count
-      };
-      issue(0);
-      issue(1);
-      for (int st = 0; st < nst; ++st) {
-        issue(st + 2);
-        cp_async_wait<2>();
-        __syncwarp();
-        const float* src = stage0 + (st % RA_STAGES) * RA_STAGE_FLOATS;
-#pragma unroll
-        for (int pi = 0; pi < RA_PAIRS; ++pi) {
-          const int pp = st * RA_PAIRS + pi;
-          if (pp < npair) {   // warp-uniform
-            const float* sa = src + (pi * 2) * RA_SEGF;
-            const float* sb2 = sa + RA_SEGF;
-#pragma unroll
-            for (int h = 0; h < RF_SEG / 32; ++h) {
-              const int j = h * 32 + lane;
-              if (j < segn) {
-                const float4 a0 = *reinterpret_cast<const float4*>(sa + j * 4);
-                const float4 a1 = *reinterpret_cast<const float4*>(sa + (RF_SEG + j) * 4);
-                const float4 b0 = *reinterpret_cast<const float4*>(sb2 + j * 4);
-                const float4 b1 = *reinterpret_cast<const float4*>(sb2 + (RF_SEG + j) * 4);
-                const float av[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
-                const float bv[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-                float t[8];
-#pragma unroll
-                for (int l = 0; l < 8; ++l) {
-                  if (COSINE) t[l] = av[l] * bv[l];
-                  else { const float df = av[l] - bv[l]; t[l] = df * df; }
-                }
-                bs[pp][j] = reduce_add8_tc(t);
-              }
-            }
-          }
-        }
-        __syncwarp();   // the stage may be refilled (two iterations ahead), the block sums are visible
-      }
-      cp_async_wait<0>();
-      if (lane < npair)
-        for (int j = 0; j < segn; ++j) acc = acc + bs[lane][j];
-      __syncwarp();
-    }
-    if (lane < npair) {
-      float v = nanf("");
-      if (COSINE) {
-        const float d = acc / sqrtf(f.c_norm2[mine.g] * ts.fnorm2[mine.row]);
-        if (d >= p.visual_threshold) v = 1.0f - d;       // is_ok + distance_to_weight
-      } else {
-        const float d = sqrtf(acc);
-        if (d <= p.visual_threshold) v = d;
-      }
-      f.vis_val[sc.vis_lbase + i0 + lane] = v;
-      if (!is_nan(v) && !(v <= vmax)) vmax = v;   // best.rs "max_dist": maximum over the entries that exist
-      if (nan_flag && is_nan(v)) nan_flag[scene] = 1;
-    }
-  }
   unsigned int u = 0u;
   if (!is_nan(vmax)) {
     u = __float_as_uint(vmax);
@@ -861,7 +724,7 @@ static EncodeTiledFn get_encode() {
   return fn;
 }
 
-static int make_map(CUtensorMap* m, const void* base, long long rows, int d8, int box_rows) {
+int make_map(CUtensorMap* m, const void* base, long long rows, int d8, int box_rows) {
   EncodeTiledFn enc = get_encode();
   if (!enc) return -1;
   cuuint64_t dims[2] = {(cuuint64_t)d8, (cuuint64_t)rows};
@@ -952,38 +815,16 @@ __global__ void vis_rowmeta_kernel(Params p, Frame f, VisRowMeta* rowmeta) {
 // exact refinement of the scene pair lists (f.vis_pairs / vis_cnt / refine_next / vis_val; scenes with vis_mode != 0 skipped)
 int launch_vis_refine(const Params& p, const TrackStore& ts, const Frame& f, int n_scenes, int* nan_flag, cudaStream_t st) {
   if (n_scenes == 0) return 0;
-  dim3 grid(16, n_scenes);   // 64 warps x 32 survivors per scene in flight; more survivors are claimed in further rounds
+  dim3 grid(16, n_scenes);   // 64 warps x RF_CLAIM survivors per scene in flight; more survivors are claimed in further rounds
   // the vector path needs 16-byte aligned input rows (a caller-owned device pointer on the device-io path)
   const bool tail = p.feature_dim != p.d8 || (reinterpret_cast<uintptr_t>(f.in_feat) & 15) != 0;
-  // SB200_REFINE=async: the cp.async variant (one CTA of six warps per SM may not keep the block-sum arithmetic fed; kept
-  // for experiments)
-  static const bool async_copy = getenv("SB200_REFINE") != nullptr && !strcmp(getenv("SB200_REFINE"), "async");
-  if (!tail && async_copy) {
-    // asynchronous-copy kernel: 3 x 8 KB stages + the parked block sums per warp
-    const size_t smem = (size_t)RA_WARPS * (RA_STAGES * RA_STAGE_FLOATS + 32 * RF_PITCH) * sizeof(float);
-    const void* fn = p.visual_kind == 1 ? (const void*)vis_refine_async_kernel<true> : (const void*)vis_refine_async_kernel<false>;
-    cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return (int)e;
-    dim3 grid2(8, n_scenes);
-    if (p.visual_kind == 1) vis_refine_async_kernel<true><<<grid2, RA_WARPS * 32, smem, st>>>(p, ts, f, nan_flag);
-    else vis_refine_async_kernel<false><<<grid2, RA_WARPS * 32, smem, st>>>(p, ts, f, nan_flag);
-    note_launch();
-    return 0;
-  }
-  // 16 survivors per claim: half the parked block sums of 32, eight CTAs per SM instead of six; SB200_REFINE_PAIRS=32
-  // selects the wider claim
-  static const bool rp16 = !(getenv("SB200_REFINE_PAIRS") != nullptr && atoi(getenv("SB200_REFINE_PAIRS")) == 32);
-#define SB_RF(C, T)                                                                        \
-  do {                                                                                     \
-    if (rp16) vis_refine_kernel<C, T, 16><<<grid, RF_WARPS * 32, 0, st>>>(p, ts, f, nan_flag); \
-    else vis_refine_kernel<C, T, 32><<<grid, RF_WARPS * 32, 0, st>>>(p, ts, f, nan_flag);      \
-  } while (0)
   if (p.visual_kind == 1) {
-    if (tail) SB_RF(true, true); else SB_RF(true, false);
+    if (tail) vis_refine_kernel<true, true><<<grid, RF_WARPS * 32, 0, st>>>(p, ts, f, nan_flag);
+    else vis_refine_kernel<true, false><<<grid, RF_WARPS * 32, 0, st>>>(p, ts, f, nan_flag);
   } else {
-    if (tail) SB_RF(false, true); else SB_RF(false, false);
+    if (tail) vis_refine_kernel<false, true><<<grid, RF_WARPS * 32, 0, st>>>(p, ts, f, nan_flag);
+    else vis_refine_kernel<false, false><<<grid, RF_WARPS * 32, 0, st>>>(p, ts, f, nan_flag);
   }
-#undef SB_RF
   note_launch();
   return 0;
 }

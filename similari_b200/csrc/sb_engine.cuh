@@ -213,10 +213,7 @@ struct Frame {  // per-request transient device buffers (a request may be proces
   unsigned char* excl;     // [slot * track_cap + n] track was claimed by the visual pass
   int* pre_winner;         // [total] the pre-pass's decision: track index the candidate won, -1 = decided as a new track
   int* dense_cnt;          // [1] scenes of the request in dense mode (null: unknown); lets the dense kernels leave at once
-  int2* pos_gq;            // gated (candidate, track) pairs of the whole frame: x = scene, y = m << 16 | n (null: evaluate in the scan kernel)
-  int* pos_gq_cnt;         // [1] entries of pos_gq (zeroed with the frame counters)
-  int pos_gq_cap;
-  int* refine_next;        // [n_scenes] next unclaimed survivor of the scene (the refinement's warps claim 32 at a time)
+  int* refine_next;        // [n_scenes] next unclaimed survivor of the scene (the refinement's warps claim 16 at a time)
   const int* dense_bad;    // [n_scenes] dense tensor-core path only: != 0 sends the scene to the exact SIMT kernels
   // outputs (device), any may be null
   unsigned long long* o_ids;

@@ -16,6 +16,10 @@ constexpr int TC_B_BYTES = TC_BN * TC_BK * 2;  // 32 KB
 constexpr int TC_WG_ROWS = 64;                 // accumulator rows of one consumer warpgroup
 constexpr int TC_THREADS = 384;                // producer warpgroup (one TMA warp) + two consumer warpgroups
 
+// Host: tensor map of a row-major [rows][d8] BF16 matrix, boxes of TC_BK features x box_rows rows, 128-byte swizzle.
+// 0 on success, -1 without the driver's encoder, -2 when it refuses the map (kernels_feat_tc.cu).
+int make_map(CUtensorMap* m, const void* base, long long rows, int d8, int box_rows);
+
 // ------------------------------------------------------------------------------------------------ PTX helpers
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(void* bar, uint32_t count) {

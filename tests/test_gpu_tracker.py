@@ -588,24 +588,6 @@ def test_positional_list_overflow_takes_the_dense_voting_kernels(eng, oracle, ki
     assert g.active_tracks() == o.active_tracks()
 
 
-@pytest.mark.parametrize("cap", ["1", "37", "100000"])
-@pytest.mark.parametrize("kind,pos", [(1, 0), (1, 1), (3, 1)])
-def test_gated_pair_queue_overflow_is_evaluated_in_place(eng, oracle, kind, pos, cap, monkeypatch):
-    """SB200_POS_GQ=1: the positional scan hands its gated (candidate, track) pairs to one queue of the frame and a second
-    kernel evaluates them.  A queue that is too small (1 or 37 entries here) keeps what fits and leaves the rest with the scan kernel's CTAs:
-    costs and assignments must not depend on where a pair was evaluated."""
-    monkeypatch.setenv("SB200_POS_GQ", "1")   # the queue is an opt-in experiment (slower than evaluating next to the scene)
-    monkeypatch.setenv("SB200_POS_GQ_CAP", cap)
-    visual = kind == 3
-    cfg = small("cfg5" if visual else "cfg2", n_scenes=3, n_objects=70, oriented=False, canvas=(700.0, 500.0),
-                feature_dim=64 if visual else 0)
-    kw = dict(kind=kind, positional_kind=pos, iou_threshold=0.3, max_idle_epochs=3)
-    if visual:
-        kw.update(visual_kind=0, visual_threshold=0.7, feature_dim=64, visual_max_observations=3, visual_min_votes=2,
-                  visual_minimal_track_length=1, min_confidence=0.1)
-    run_frames(eng, oracle, cfg, 6, kw)
-
-
 @pytest.mark.parametrize("join_per_call", [True, False])
 def test_caller_stream_is_joined_by_events(eng, oracle, join_per_call):
     """sb200_tracker_set_stream: the tracker runs on its own streams and is ordered with the caller's by events.  Inputs are
