@@ -82,6 +82,47 @@ __global__ void fill_u8_kernel(unsigned char* p, unsigned char v, int n) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) p[i] = v;
 }
+
+// The voting operators' entry lists: the valid (non-NaN) entries of a dense row-major [rows][cols] matrix in the
+// tracker's list format -- PosEntry {row, col, v}, or VisPair {g = row, outcol = col} plus vis_val -- in REVERSE
+// row-major order.  The tracker's lists arrive in atomic order, so the sparse voting kernel must not rely on sorted
+// input, and the operator does not hand it one.  One CTA walks the matrix from its end in chunks of 1024 with a
+// block-wide scan of the valid flags; entries past `cap` are counted but not stored, as in the tracker (the count then
+// sends the scene to the dense voting kernel).
+constexpr int kListThreads = 1024;
+__global__ void __launch_bounds__(kListThreads) vote_list_kernel(const float* a, int rows, int cols, int cap,
+                                                                 sb::PosEntry* pos_out, sb::VisPair* vis_out,
+                                                                 float* vis_val, int* cnt) {
+  __shared__ int s_warp[kListThreads / 32];
+  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+  const long long total = (long long)rows * cols;
+  int carry = 0;
+  for (long long base = 0; base < total; base += kListThreads) {
+    const long long i = total - 1 - (base + tid);   // position base + tid of the reversed order
+    const float v = i >= 0 ? a[i] : 0.0f;
+    const bool ok = i >= 0 && v == v;
+    const unsigned int bal = __ballot_sync(0xffffffffu, ok);
+    if (lane == 0) s_warp[wid] = __popc(bal);
+    __syncthreads();
+    int woff = 0, chunk = 0;
+    for (int w = 0; w < kListThreads / 32; ++w) {
+      woff += w < wid ? s_warp[w] : 0;
+      chunk += s_warp[w];
+    }
+    const int slot = carry + woff + __popc(bal & ((1u << lane) - 1u));
+    if (ok && slot < cap) {
+      const int r = (int)(i / cols), c = (int)(i % cols);
+      if (pos_out) pos_out[slot] = sb::PosEntry{(unsigned short)r, (unsigned short)c, v};
+      else {
+        vis_out[slot] = sb::VisPair{r, -1, 0, c};
+        vis_val[slot] = v;
+      }
+    }
+    carry += chunk;
+    __syncthreads();
+  }
+  if (tid == 0) *cnt = carry;
+}
 }  // namespace
 
 extern "C" {
@@ -267,6 +308,17 @@ static int run_voting(bool visual, float threshold, int min_votes, const float* 
                       int k, int32_t* winner, uint8_t* voting_type, int device) {
   if (m < 0 || n < 0 || (m > 0 && !winner) || (m > 0 && n > 0 && !pos_mn)) return ops_fail(SB200_ERR_INVALID, "bad arguments");
   if (visual && (k < 1 || k > sb::kMaxObs || (m > 0 && n > 0 && !vis_mnk))) return ops_fail(SB200_ERR_INVALID, "bad arguments");
+  // Which voting kernel runs: by default the tracker's rule (the sparse kernel on the entry lists unless a list exceeds
+  // its capacity); SB200_VOTE_KERNEL=dense|sparse|prepass forces one, so that a test can hand each kernel the matrix of
+  // its choosing.  A forced kernel the rule would not allow is an error, never a silent switch to the other one.
+  enum { kRule, kDense, kSparse, kPrepass } want = kRule;
+  if (const char* ev = getenv("SB200_VOTE_KERNEL")) {
+    if (!strcmp(ev, "dense")) want = kDense;
+    else if (!strcmp(ev, "sparse")) want = kSparse;
+    else if (!strcmp(ev, "prepass")) want = kPrepass;
+    else if (*ev) return ops_fail(SB200_ERR_INVALID, "SB200_VOTE_KERNEL must be dense, sparse or prepass");
+  }
+  if (want == kPrepass && !visual) return ops_fail(SB200_ERR_INVALID, "SB200_VOTE_KERNEL=prepass applies to visual voting only");
   Scratch sc;
   int rc = begin(sc, device);
   if (rc) return rc;
@@ -277,8 +329,10 @@ static int run_voting(bool visual, float threshold, int min_votes, const float* 
   p.is_visual = visual;
   p.max_obs = visual ? k : 1;
   p.min_votes = min_votes;
+  p.vote_vis_cap = sb::kVoteVisCap;
   sb::TrackStore ts;
   memset(&ts, 0, sizeof(ts));
+  ts.track_cap = n;
   sb::Frame f;
   memset(&f, 0, sizeof(f));
   f.total = m;
@@ -288,24 +342,59 @@ static int run_voting(bool visual, float threshold, int min_votes, const float* 
   f.c_vt = sc.alloc<unsigned char>(m);
   f.new_count = sc.alloc<int>(1);
   {
-    // operators take dense matrices: scene mode 1 routes the request to the dense voting kernel
-    int hm[4] = {0, 0, 1, 0};
+    // scene mode 1 until the rule below runs: the scene-maximum reduction skips sparse scenes (the tracker's refinement
+    // reduces their maximum), and the operator has no refinement
+    int hm[4] = {0, 0, 1, 1};
     f.pos_cnt = sc.upload(hm, 4);
     if (!f.pos_cnt) return ops_fail(SB200_ERR_CUDA, "cudaMalloc failed");
     f.vis_cnt = f.pos_cnt + 1;
     f.scene_mode = f.pos_cnt + 2;
     f.vis_mode = f.pos_cnt + 3;
   }
+  // one scene, list slices sized as the tracker sizes them (engine.cu, predict)
   sb::SceneDesc sd;
   memset(&sd, 0, sizeof(sd));
   sd.m = m; sd.n = n; sd.epoch = 1;
+  sd.pos_lcap = (int)std::min<long long>((long long)m * 32, (long long)sb::kVotePosCap * 2);
+  sd.vis_lcap = visual ? (int)std::min<long long>((long long)m * 64, (long long)sb::kVoteVisCap * 4) : 0;
   f.scenes = sc.upload(&sd, 1);
-  if (!f.pos || (visual && !f.vis) || !f.winner || !f.c_vt || !f.new_count || !f.scenes) return ops_fail(SB200_ERR_CUDA, "cudaMalloc failed");
+  f.pos_list = sc.alloc<sb::PosEntry>(sd.pos_lcap);
+  if (visual) {
+    f.vis_pairs = sc.alloc<sb::VisPair>(sd.vis_lcap);
+    f.vis_val = sc.alloc<float>(sd.vis_lcap);
+  }
+  if (!f.pos || (visual && (!f.vis || !f.vis_pairs || !f.vis_val)) || !f.winner || !f.c_vt || !f.new_count || !f.scenes ||
+      !f.pos_list)
+    return ops_fail(SB200_ERR_CUDA, "cudaMalloc failed");
+  vote_list_kernel<<<1, kListThreads, 0, sc.st>>>(f.pos, m, n, sd.pos_lcap, f.pos_list, nullptr, nullptr, f.pos_cnt);
+  if (visual) vote_list_kernel<<<1, kListThreads, 0, sc.st>>>(f.vis, m, n * k, sd.vis_lcap, nullptr, f.vis_pairs, f.vis_val, f.vis_cnt);
   if (visual) {
     f.scene_max = sc.alloc<unsigned int>(1);
     if (!f.scene_max) return ops_fail(SB200_ERR_CUDA, "cudaMalloc failed");
     sb::launch_scene_max(p, f, 1, /*init_only=*/true, sc.st);
     if (n > 0) sb::launch_scene_max(p, f, 1, /*init_only=*/false, sc.st);
+  }
+  if (want != kDense) {
+    // the tracker's rule, with the list capacities above and the sparse visual lists of its tensor-core path
+    sb::launch_vis_mode(p, f, 1, /*tc_used=*/true, sc.st);
+    sb::launch_scene_mode(p, f, 1, /*tc_used=*/true, sc.st);
+  }
+  if (want == kSparse || want == kPrepass) {
+    int mode = 1;
+    cudaMemcpyAsync(&mode, f.scene_mode, sizeof(int), cudaMemcpyDeviceToHost, sc.st);
+    if ((rc = finish(sc))) return rc;
+    if (mode != 0)
+      return ops_fail(SB200_ERR_CAPACITY, "SB200_VOTE_KERNEL: the entry lists exceed the sparse voting kernel's capacity");
+  }
+  if (want == kPrepass) {
+    // the tracker's lazy positional stage: BestFit pre-pass, then the full pass reuses its decisions
+    f.decided = sc.alloc<unsigned char>(m);
+    f.excl = sc.alloc<unsigned char>(n);
+    f.pre_winner = sc.alloc<int>(m);
+    if (!f.decided || !f.excl || !f.pre_winner) return ops_fail(SB200_ERR_CUDA, "cudaMalloc failed");
+    int vr = sb::launch_vote_masks(p, ts, f, 1, m, n, sc.st);
+    if (vr == -3) return ops_fail(SB200_ERR_CAPACITY, "scene too large for the on-chip assignment solver");
+    if (vr != 0) return ops_fail(SB200_ERR_CUDA, std::string("voting launch failed: ") + cudaGetErrorString((cudaError_t)vr));
   }
   int vr = sb::launch_voting(p, ts, f, 1, m, n, sc.st);
   if (vr == -3) return ops_fail(SB200_ERR_CAPACITY, "scene too large for the on-chip assignment solver");
