@@ -29,7 +29,7 @@
 extern "C" {
 #endif
 
-#define SB200_VERSION 2
+#define SB200_VERSION 3
 
 typedef enum {
   SB200_OK = 0,
@@ -134,12 +134,27 @@ int sb200_stream_join(sb200_tracker* t, void* cuda_stream);
  * is provisional and can be changed here; afterwards a different value is SB200_ERR_INVALID. */
 int sb200_set_feature_dim(sb200_tracker* t, int32_t feature_dim);
 
+/* Element type of the `features` column of the predict entry points and sb200_prefetch_inputs.  The column stays
+ * [total][feature_dim] row-major; with F16 (IEEE binary16) or BF16 the `const float* features` parameter carries a pointer
+ * to 2-byte elements.  Widening either type to f32 is exact: a frame fed half-precision rows returns exactly what the same
+ * frame fed the widened f32 rows returns (results, stored features, wasted feature histories, state blobs). */
+#define SB200_FEATURE_F32 0
+#define SB200_FEATURE_F16 1
+#define SB200_FEATURE_BF16 2
+/* Sets the element type of the features column for every later sb200_predict_batch / _async / _device and
+ * sb200_prefetch_inputs call on the tracker.  It may change between calls: each frame keeps the type it was enqueued
+ * with, and a prefetch made under one type is not used by a predict call under another (the columns are copied again).
+ * The type is an input format, not tracker state: it is not saved in the state blob, and a new or loaded tracker reads
+ * F32.  SB200_ERR_INVALID for a NULL handle, a non-visual tracker or an unknown type. */
+int sb200_set_feature_type(sb200_tracker* t, int32_t type);
+
 /* ---- the hot path ----
  * One call == Sort::predict_with_scene (n_scenes = 1, src/trackers/sort/simple_api.rs:110-196) or
  * BatchSort::predict / BatchVisualSort::predict over a PredictionBatchRequest (src/trackers/sort/batch_api.rs:222-290,
  * src/trackers/visual_sort/batch_api.rs:213-317, src/trackers/batch.rs:12-38) flattened as:
  *   scene_ids[n_scenes], det_offsets[n_scenes+1] (CSR over detections),
- *   boxes[total][6], features[total][D] or NULL, has_feature[total] or NULL (all present),
+ *   boxes[total][6], features[total][D] or NULL (f32, or the type set by sb200_set_feature_type), has_feature[total]
+ *   or NULL (all present),
  *   quality[total] or NULL, custom_ids[total] or NULL, own_area[total] or NULL
  *   (own-area shares of exclusively_owned_areas, computed by the caller; src/utils/clipping/bbox_own_areas.rs).
  * All pointers are HOST pointers; inputs are copied to the device and the requested result columns copied back

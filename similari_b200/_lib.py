@@ -19,6 +19,7 @@ KIND_SORT, KIND_BATCH_SORT, KIND_VISUAL_SORT, KIND_BATCH_VISUAL_SORT = 0, 1, 2, 
 POS_MAHA, POS_IOU = 0, 1
 VIS_EUCLIDEAN, VIS_COSINE = 0, 1
 VOTING_VISUAL, VOTING_POSITIONAL = 0, 1
+FEATURE_F32, FEATURE_F16, FEATURE_BF16 = 0, 1, 2
 
 
 class Sb200Error(RuntimeError):
@@ -88,7 +89,7 @@ EXPORTS = [
     "sb200_point_kalman_predict", "sb200_point_kalman_update", "sb200_point_kalman_distance", "sb200_box_vertices",
     "sb200_clip_polygons", "sb200_intersection_areas", "sb200_set_feature_history", "sb200_wasted_visual",
     "sb200_feature_history_pool", "sb200_tracker_save", "sb200_tracker_load", "sb200_scenes_export",
-    "sb200_scenes_import", "sb200_tracker_options",
+    "sb200_scenes_import", "sb200_tracker_options", "sb200_set_feature_type",
 ]
 
 
@@ -117,6 +118,7 @@ def lib():
         "sb200_predict_batch_async": (C.c_int, [vp, i32, vp, vp, vp, vp, vp, vp, vp, vp, C.POINTER(PredictOut)]),
         "sb200_sync": (C.c_int, [vp]),
         "sb200_set_feature_dim": (C.c_int, [vp, i32]),
+        "sb200_set_feature_type": (C.c_int, [vp, i32]),
         "sb200_comm_unique_id": (C.c_int, [vp]),
         "sb200_comm_create": (C.c_int, [i32, i32, vp, i32, C.POINTER(vp)]),
         "sb200_comm_destroy": (None, [vp]),

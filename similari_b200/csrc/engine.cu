@@ -252,6 +252,7 @@ struct sb200_tracker {
     DBuf boxes, feat, hasf, quality, custom, own;
     const void* key[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};   // the six host columns of the prefetch
     int total = -1;
+    int type = sb::kFeatF32;   // element type of the prefetched features column
     bool pending = false;   // holds a prefetched request that no predict call has consumed yet
     cudaEvent_t ev = nullptr;
     cudaEvent_t ev0 = nullptr;   // start of the set's prefetch copy (SB200_TRACE timing)
@@ -270,6 +271,10 @@ struct sb200_tracker {
   unsigned long long acc_dense_scenes = 0;   // scenes the exact SIMT fallback had to take (over all absorbed frames)
   int last_dense_scenes = 0;
   bool seen_features = false;   // a request has carried feature rows (the feature dimension is fixed from then on)
+  // element type of the features column of the calls that follow (sb200_set_feature_type): an input format, not state --
+  // each frame copies it at enqueue, and it is not part of the state blob
+  int feat_type = sb::kFeatF32;
+  size_t feat_bytes() const { return feat_type == sb::kFeatF32 ? 4 : 2; }
   bool transferred = false;     // built by sb200_tracker_load or filled by sb200_scenes_import: holds state without a frame
   int last_n_scenes = 0;   // scenes of the last frame (sb200_last_costs reads its scene table back from the device)
 
@@ -1059,6 +1064,7 @@ int sb200_tracker::predict(int32_t n_scenes, const uint64_t* scene_ids, const in
   f.dense_bad = tc.dense ? tc.dense_bad : nullptr;
   // dense positional matrices for every scene only on request (SB200_FULL_COSTS: parity of sb200_last_costs)
   f.pos_dense_all = getenv("SB200_FULL_COSTS") != nullptr;
+  f.feat_type = feat_type;
   bool prefetched = false;
   Staging* sin = nullptr;
   // inputs
@@ -1071,7 +1077,8 @@ int sb200_tracker::predict(int32_t n_scenes, const uint64_t* scene_ids, const in
     const void* key[6] = {boxes, features, features ? has_feature : nullptr, quality, custom_ids, own_area};
     int use = -1;
     for (int k = 0; k < 2; ++k)
-      if (stg[k].pending && stg[k].total == total && memcmp(stg[k].key, key, sizeof(key)) == 0) use = k;
+      if (stg[k].pending && stg[k].total == total && stg[k].type == feat_type && memcmp(stg[k].key, key, sizeof(key)) == 0)
+        use = k;
     if (use >= 0) {
       prefetched = true;
       stg[use].pending = false;
@@ -1083,15 +1090,15 @@ int sb200_tracker::predict(int32_t n_scenes, const uint64_t* scene_ids, const in
     stg_last = use;
     Staging& S = stg[use];
     sin = &S;
-    if (prefetched && (S.boxes.bytes < T * 24 || (features && S.feat.bytes < T * (size_t)P.feature_dim * 4))) {
+    if (prefetched && (S.boxes.bytes < T * 24 || (features && S.feat.bytes < T * (size_t)P.feature_dim * feat_bytes()))) {
       // the filled set is smaller than this frame's sizing rule (hints changed?): re-copy instead of reallocating
       prefetched = false;
     }
     if ((rc = ENS(S.boxes, T * 24))) return rc;
     f.in_boxes = S.boxes.as<float>();
     if (features && total > 0) {
-      if ((rc = ENS(S.feat, T * (size_t)P.feature_dim * 4))) return rc;
-      f.in_feat = S.feat.as<float>();
+      if ((rc = ENS(S.feat, T * (size_t)P.feature_dim * feat_bytes()))) return rc;
+      f.in_feat = S.feat.p;
       if (has_feature) {
         if ((rc = ENS(S.hasf, T))) return rc;
         f.in_hasf = S.hasf.as<unsigned char>();
@@ -1201,7 +1208,7 @@ int sb200_tracker::predict(int32_t n_scenes, const uint64_t* scene_ids, const in
     const size_t n = (size_t)total;
     CU(cudaMemcpyAsync(sin->boxes.p, boxes, n * 24, cudaMemcpyHostToDevice, stream));
     if (f.in_feat) {
-      CU(cudaMemcpyAsync(sin->feat.p, features, n * (size_t)P.feature_dim * 4, cudaMemcpyHostToDevice, stream));
+      CU(cudaMemcpyAsync(sin->feat.p, features, n * (size_t)P.feature_dim * feat_bytes(), cudaMemcpyHostToDevice, stream));
       if (f.in_hasf) CU(cudaMemcpyAsync(sin->hasf.p, has_feature, n, cudaMemcpyHostToDevice, stream));
     }
     if (f.in_quality) CU(cudaMemcpyAsync(sin->quality.p, quality, n * 4, cudaMemcpyHostToDevice, stream));
@@ -1549,6 +1556,18 @@ int sb200_set_feature_history(sb200_tracker* t, int32_t on) {
   return t->set_feature_history(on != 0);
 }
 
+static_assert(SB200_FEATURE_F32 == sb::kFeatF32 && SB200_FEATURE_F16 == sb::kFeatF16 && SB200_FEATURE_BF16 == sb::kFeatBF16,
+              "feature type codes of the ABI and the kernels differ");
+
+int sb200_set_feature_type(sb200_tracker* t, int32_t type) {
+  if (!t) return fail(SB200_ERR_INVALID, "tracker is NULL");
+  if (!t->P.is_visual) return fail(SB200_ERR_INVALID, "the feature type belongs to the visual trackers");
+  if (type != SB200_FEATURE_F32 && type != SB200_FEATURE_F16 && type != SB200_FEATURE_BF16)
+    return fail(SB200_ERR_INVALID, "unknown feature type %d", (int)type);
+  t->feat_type = type;   // frames already enqueued keep the type they were enqueued with (Frame::feat_type)
+  return 0;
+}
+
 int sb200_sync(sb200_tracker* t) {
   if (!t) return fail(SB200_ERR_INVALID, "tracker is NULL");
   CU(cudaSetDevice(t->device));
@@ -1603,7 +1622,8 @@ int sb200_prefetch_inputs(sb200_tracker* t, int32_t total, const float* boxes, c
   cudaStream_t cs = t->copy_stream;
   if (features == nullptr) has_feature = nullptr;
   // the set's previous reader (a frame that may still be in flight) finishes first; a reallocation meets the device
-  if (S.boxes.bytes < T * 24 || (features && S.feat.bytes < T * (size_t)t->P.feature_dim * 4) || (has_feature && S.hasf.bytes < T) ||
+  const size_t fbytes = t->feat_bytes();
+  if (S.boxes.bytes < T * 24 || (features && S.feat.bytes < T * (size_t)t->P.feature_dim * fbytes) || (has_feature && S.hasf.bytes < T) ||
       (quality && S.quality.bytes < T * 4) || (custom_ids && S.custom.bytes < T * 8) || (own_area && S.own.bytes < T * 4)) {
     if ((rc = t->drain())) return rc;
   }
@@ -1612,8 +1632,8 @@ int sb200_prefetch_inputs(sb200_tracker* t, int32_t total, const float* boxes, c
   CU(cudaEventRecord(S.ev0, cs));
   CU(cudaMemcpyAsync(S.boxes.p, boxes, n * 24, cudaMemcpyHostToDevice, cs));
   if (features) {
-    if ((rc = S.feat.ensure(T * (size_t)t->P.feature_dim * 4))) return rc;
-    CU(cudaMemcpyAsync(S.feat.p, features, n * (size_t)t->P.feature_dim * 4, cudaMemcpyHostToDevice, cs));
+    if ((rc = S.feat.ensure(T * (size_t)t->P.feature_dim * fbytes))) return rc;
+    CU(cudaMemcpyAsync(S.feat.p, features, n * (size_t)t->P.feature_dim * fbytes, cudaMemcpyHostToDevice, cs));
     if (has_feature) { if ((rc = S.hasf.ensure(T))) return rc; CU(cudaMemcpyAsync(S.hasf.p, has_feature, n, cudaMemcpyHostToDevice, cs)); }
   }
   if (quality) { if ((rc = S.quality.ensure(T * 4))) return rc; CU(cudaMemcpyAsync(S.quality.p, quality, n * 4, cudaMemcpyHostToDevice, cs)); }
@@ -1621,7 +1641,7 @@ int sb200_prefetch_inputs(sb200_tracker* t, int32_t total, const float* boxes, c
   if (own_area) { if ((rc = S.own.ensure(T * 4))) return rc; CU(cudaMemcpyAsync(S.own.p, own_area, n * 4, cudaMemcpyHostToDevice, cs)); }
   CU(cudaEventRecord(S.ev, cs));
   S.key[0] = boxes; S.key[1] = features; S.key[2] = has_feature; S.key[3] = quality; S.key[4] = custom_ids; S.key[5] = own_area;
-  S.total = total; S.pending = true;
+  S.total = total; S.type = t->feat_type; S.pending = true;
   return 0;
 }
 

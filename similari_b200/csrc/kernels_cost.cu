@@ -9,6 +9,7 @@
 
 #include <algorithm>
 #include <cstdlib>
+#include <type_traits>
 
 #include "sb_engine.cuh"
 
@@ -52,15 +53,18 @@ __device__ __forceinline__ float reduce_add8(const float* t) {
 
 // One warp per detection: squared norm in the reference's order (per 8-lane block reduce_add, blocks accumulated
 // sequentially) and, when the tensor-core screen will run, the BF16 operand copy of the row -- the feature row is
-// read from HBM once for both.
+// read from HBM once for both.  T: element type of the request's feature column (f32, or a 2-byte type widened on load,
+// where one 16-byte load is a whole 8-lane block).
+template <class T>
 __global__ void cand_norm_kernel(Params p, Frame f, __nv_bfloat16* __restrict__ bf16_out) {
   int w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   int lane = threadIdx.x & 31;
   if (w >= f.total) return;
   w += f.det0;
   const int nblk = p.d8 / 8;
-  const float* __restrict__ row = f.in_feat + (size_t)w * p.feature_dim;
-  const bool vec = (p.feature_dim % 4 == 0) && (reinterpret_cast<uintptr_t>(f.in_feat) & 15) == 0;
+  const T* __restrict__ row = static_cast<const T*>(f.in_feat) + (size_t)w * p.feature_dim;
+  constexpr bool kF32 = std::is_same<T, float>::value;
+  const bool vec = (p.feature_dim % (kF32 ? 4 : 8) == 0) && (reinterpret_cast<uintptr_t>(f.in_feat) & 15) == 0;
   float acc = 0.0f;
   // two rounds of 32 blocks per step: the loads of both are issued before anything waits for them (2 KB in flight per warp)
   for (int base = 0; base < nblk; base += 64) {
@@ -72,12 +76,16 @@ __global__ void cand_norm_kernel(Params p, Frame f, __nv_bfloat16* __restrict__ 
       have[h] = blk < nblk;
       if (have[h]) {
         if (vec && blk * 8 + 8 <= p.feature_dim) {
-          const float4 a = __ldcs(reinterpret_cast<const float4*>(row + blk * 8));
-          const float4 b = __ldcs(reinterpret_cast<const float4*>(row + blk * 8 + 4));
-          x[h][0] = a.x; x[h][1] = a.y; x[h][2] = a.z; x[h][3] = a.w; x[h][4] = b.x; x[h][5] = b.y; x[h][6] = b.z; x[h][7] = b.w;
+          if constexpr (kF32) {
+            const float4 a = __ldcs(reinterpret_cast<const float4*>(row + blk * 8));
+            const float4 b = __ldcs(reinterpret_cast<const float4*>(row + blk * 8 + 4));
+            x[h][0] = a.x; x[h][1] = a.y; x[h][2] = a.z; x[h][3] = a.w; x[h][4] = b.x; x[h][5] = b.y; x[h][6] = b.z; x[h][7] = b.w;
+          } else {
+            feat_widen8(__ldcs(reinterpret_cast<const uint4*>(row + blk * 8)), row, x[h]);
+          }
         } else {
 #pragma unroll
-          for (int l = 0; l < 8; ++l) { int d = blk * 8 + l; x[h][l] = d < p.feature_dim ? row[d] : 0.0f; }
+          for (int l = 0; l < 8; ++l) { int d = blk * 8 + l; x[h][l] = d < p.feature_dim ? feat_elem(row, d) : 0.0f; }
         }
       }
     }
@@ -114,7 +122,9 @@ void launch_prep(const Params& p, const Frame& f, int n_scenes, int max_m, cudaS
   note_launch();
   if (p.is_visual && f.in_feat) {  // squared norms (+ BF16 operand rows when f.c_bf16 is set for this frame)
     long long threads = (long long)f.total * 32;
-    cand_norm_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(p, f, reinterpret_cast<__nv_bfloat16*>(f.c_bf16));
+    feat_dispatch(f.feat_type, [&](auto t) {
+      cand_norm_kernel<decltype(t)><<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(p, f, reinterpret_cast<__nv_bfloat16*>(f.c_bf16));
+    });
     note_launch();
   }
 }
@@ -537,22 +547,26 @@ void launch_pos_cost(const Params& p, const TrackStore& ts, const Frame& f, int 
 constexpr int VM = 64, VN = 64, VK = 32, VT = 256;  // 4x4 pairs per thread
 
 // tile body; `scene`, `bx`, `by` identify the VM x VN tile
+template <class T>
 __device__ void vis_cost_tile(const Params& p, const TrackStore& ts, const Frame& f, int scene, int bx, int by);
 
 // Dense kernel over the scenes in dense mode.  The grid is a fixed number of CTAs that walk (scene, tile) pairs, so
 // when every scene took the screen + refine path (the common case) the launch costs a few microseconds.
+// T: element type of the request's feature column.
+template <class T>
 __global__ void __launch_bounds__(VT) vis_cost_kernel(Params p, TrackStore ts, Frame f, int n_scenes, int tiles_x, int tiles_y) {
   if (f.dense_cnt && *f.dense_cnt == 0) return;   // the common case: every scene took the screen + refine path
   const long long per_scene = (long long)tiles_x * tiles_y;
   for (int scene = 0; scene < n_scenes; ++scene) {
     if (f.scene_mode[scene] == 0) continue;  // this scene's visual entries come from the screen + refine path
     for (long long t = blockIdx.x; t < per_scene; t += gridDim.x) {
-      vis_cost_tile(p, ts, f, scene, (int)(t % tiles_x), (int)(t / tiles_x));
+      vis_cost_tile<T>(p, ts, f, scene, (int)(t % tiles_x), (int)(t / tiles_x));
       __syncthreads();
     }
   }
 }
 
+template <class T>
 __device__ void vis_cost_tile(const Params& p, const TrackStore& ts, const Frame& f, int scene, int bx, int by) {
   const SceneDesc sc = f.scenes[scene];
   const int K = p.max_obs;
@@ -608,7 +622,7 @@ __device__ void vis_cost_tile(const Params& p, const TrackStore& ts, const Frame
       int r = e / VK, c = e % VK;
       int m = m0 + r, d = k0 + c;
       float v = 0.0f;
-      if (m < sc.m && d < D && row_ok[r]) v = f.in_feat[(size_t)(sc.det_base + m) * D + d];
+      if (m < sc.m && d < D && row_ok[r]) v = feat_elem(static_cast<const T*>(f.in_feat), (size_t)(sc.det_base + m) * D + d);
       sa[r][c] = v;
     }
     for (int e = tid; e < VN * VK; e += VT) {
@@ -719,7 +733,7 @@ int launch_vis_cost_b(const Params& p, const TrackStore& ts, const Frame& f, int
     const int tx = (max_n * p.max_obs + VN - 1) / VN, ty = (max_m + VM - 1) / VM;
     const long long want = (long long)tx * ty * (use_tc ? 1 : n_scenes);
     const int grid = (int)std::min<long long>(want, kNumSms * 8);
-    vis_cost_kernel<<<grid, VT, 0, st>>>(p, ts, f, n_scenes, tx, ty);
+    feat_dispatch(f.feat_type, [&](auto t) { vis_cost_kernel<decltype(t)><<<grid, VT, 0, st>>>(p, ts, f, n_scenes, tx, ty); });
     note_launch();
     launch_scene_max(p, f, n_scenes, /*init_only=*/false, st);
   }

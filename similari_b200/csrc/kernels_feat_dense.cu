@@ -453,7 +453,9 @@ __global__ void vis_dense_rowmeta_kernel(Params p, Frame f, VisRowMeta* rowmeta)
 // Sampled lower bound of the scene's maximal distance (in the weight-sum kernel's domain: squared distance, or 1 - cos):
 // up to 64 candidates x 64 valid feature rows, plain f32 dot products.  Any real element bounds the maximum from below, so
 // whatever the sample is, the candidates the weight-sum kernel keeps (x~ >= l0 - bound) contain the true maximum.
+// T: element type of the request's feature column (widened on load).
 constexpr int DSAMP = 32;
+template <class T>
 __global__ void __launch_bounds__(256) vis_dense_sample_kernel(Params p, TrackStore ts, Frame f, const int2* rowinfo, float* scene_l0,
                                                                 int* dense_bad) {
   __shared__ int s_q[DSAMP], s_r[DSAMP];
@@ -496,10 +498,10 @@ __global__ void __launch_bounds__(256) vis_dense_sample_kernel(Params p, TrackSt
   // one warp per sampled pair: the lanes stride over the features (coalesced), shuffle tree at the end
   for (int pi = wid; pi < nq * nr; pi += 8) {
     const int g = s_q[pi / nr], fr = s_r[pi % nr];
-    const float* a = f.in_feat + (size_t)g * D;
+    const T* a = static_cast<const T*>(f.in_feat) + (size_t)g * D;
     const float* b = ts.feat + (size_t)fr * p.d8;
     float dot = 0.0f;
-    for (int d = lane; d < D; d += 32) dot = __fmaf_rn(a[d], b[d], dot);
+    for (int d = lane; d < D; d += 32) dot = __fmaf_rn(feat_elem(a, d), b[d], dot);
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) dot += __shfl_xor_sync(0xffffffffu, dot, o);
     const float na = f.c_norm2[g], nb2 = ts.fnorm2[fr];
@@ -678,7 +680,9 @@ int launch_vis_dense(const Params& p, const TrackStore& ts, const Frame& f, int 
     note_launch();
   }
   vis_dense_rowmeta_kernel<<<(f.total + 255) / 256, 256, 0, st>>>(p, f, tc.rowmeta);
-  vis_dense_sample_kernel<<<n_scenes, 256, 0, st>>>(p, ts, f, tc.rowinfo, tc.scene_l0, tc.dense_bad);
+  feat_dispatch(f.feat_type, [&](auto t) {
+    vis_dense_sample_kernel<decltype(t)><<<n_scenes, 256, 0, st>>>(p, ts, f, tc.rowinfo, tc.scene_l0, tc.dense_bad);
+  });
   note_launch(2);
   if (tc.ev_screen0) cudaEventRecord(tc.ev_screen0, st);
   {

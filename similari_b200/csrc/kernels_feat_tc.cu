@@ -559,7 +559,8 @@ constexpr int RF_PITCH = RF_SEG + 1;   // +1: lane p reads row p, rows must star
 // 16 survivors per claim rather than 32: half the parked block sums, so eight CTAs fit an SM instead of six
 constexpr int RF_CLAIM = 16;
 
-// a-side of a block sum: the candidate's 8 features of block `blk` (zero padded past D on the TAIL path)
+// a-side of a block sum: the candidate's 8 features of block `blk` (zero padded past D on the TAIL path), widened to f32
+// when the request's column is a 2-byte type (one 16-byte load per block)
 template <bool TAIL>
 __device__ __forceinline__ void refine_load_a(const float* __restrict__ a, int blk, int D, float* av) {
   if (!TAIL) {
@@ -569,6 +570,15 @@ __device__ __forceinline__ void refine_load_a(const float* __restrict__ a, int b
   } else {
 #pragma unroll
     for (int l = 0; l < 8; ++l) av[l] = blk * 8 + l < D ? a[blk * 8 + l] : 0.0f;   // the input row has D, not d8, floats
+  }
+}
+template <bool TAIL, class T>
+__device__ __forceinline__ void refine_load_a(const T* __restrict__ a, int blk, int D, float* av) {
+  if (!TAIL) {
+    feat_widen8(*reinterpret_cast<const uint4*>(a + blk * 8), a, av);
+  } else {
+#pragma unroll
+    for (int l = 0; l < 8; ++l) av[l] = blk * 8 + l < D ? feat_elem(a, blk * 8 + l) : 0.0f;
   }
 }
 template <bool COSINE>
@@ -585,7 +595,8 @@ __device__ __forceinline__ float refine_block_sum(const float* av, const float* 
   return reduce_add8_tc(t);
 }
 
-template <bool COSINE, bool TAIL>
+// T: element type of the request's feature column
+template <bool COSINE, bool TAIL, class T>
 __global__ void __launch_bounds__(RF_WARPS * 32, 8) vis_refine_kernel(Params p, TrackStore ts, Frame f, int* nan_flag) {
   __shared__ float s_bs[RF_WARPS][RF_CLAIM][RF_PITCH];
   const int scene = blockIdx.y;
@@ -621,7 +632,7 @@ __global__ void __launch_bounds__(RF_WARPS * 32, 8) vis_refine_kernel(Params p, 
         const int row = __shfl_sync(0xffffffffu, mine.row, pp);
         const float* b = ts.feat + (size_t)row * p.d8;
         if (g != g_prev) {   // warp-uniform
-          const float* a = f.in_feat + (size_t)g * D;
+          const T* a = static_cast<const T*>(f.in_feat) + (size_t)g * D;
 #pragma unroll
           for (int h = 0; h < RF_SEG / 32; ++h)
             if (h * 32 + lane < segn) refine_load_a<TAIL>(a, seg0 + h * 32 + lane, D, av[h]);
@@ -816,15 +827,19 @@ __global__ void vis_rowmeta_kernel(Params p, Frame f, VisRowMeta* rowmeta) {
 int launch_vis_refine(const Params& p, const TrackStore& ts, const Frame& f, int n_scenes, int* nan_flag, cudaStream_t st) {
   if (n_scenes == 0) return 0;
   dim3 grid(16, n_scenes);   // 64 warps x RF_CLAIM survivors per scene in flight; more survivors are claimed in further rounds
-  // the vector path needs 16-byte aligned input rows (a caller-owned device pointer on the device-io path)
+  // the vector path needs 16-byte aligned input rows (a caller-owned device pointer on the device-io path); rows of d8
+  // elements are 16-byte multiples for every element type
   const bool tail = p.feature_dim != p.d8 || (reinterpret_cast<uintptr_t>(f.in_feat) & 15) != 0;
-  if (p.visual_kind == 1) {
-    if (tail) vis_refine_kernel<true, true><<<grid, RF_WARPS * 32, 0, st>>>(p, ts, f, nan_flag);
-    else vis_refine_kernel<true, false><<<grid, RF_WARPS * 32, 0, st>>>(p, ts, f, nan_flag);
-  } else {
-    if (tail) vis_refine_kernel<false, true><<<grid, RF_WARPS * 32, 0, st>>>(p, ts, f, nan_flag);
-    else vis_refine_kernel<false, false><<<grid, RF_WARPS * 32, 0, st>>>(p, ts, f, nan_flag);
-  }
+  feat_dispatch(f.feat_type, [&](auto t) {
+    using T = decltype(t);
+    if (p.visual_kind == 1) {
+      if (tail) vis_refine_kernel<true, true, T><<<grid, RF_WARPS * 32, 0, st>>>(p, ts, f, nan_flag);
+      else vis_refine_kernel<true, false, T><<<grid, RF_WARPS * 32, 0, st>>>(p, ts, f, nan_flag);
+    } else {
+      if (tail) vis_refine_kernel<false, true, T><<<grid, RF_WARPS * 32, 0, st>>>(p, ts, f, nan_flag);
+      else vis_refine_kernel<false, false, T><<<grid, RF_WARPS * 32, 0, st>>>(p, ts, f, nan_flag);
+    }
+  });
   note_launch();
   return 0;
 }

@@ -10,6 +10,7 @@
 #include <cuda_bf16.h>
 
 #include <algorithm>
+#include <type_traits>
 
 #include "sb_engine.cuh"
 
@@ -306,6 +307,9 @@ __global__ void __launch_bounds__(256) apply_kernel(Params p, TrackStore ts, Fra
 // updated in this frame (epoch == the scene's new epoch); the sweep moves only the block indices of tracks with
 // epoch + max_idle < that epoch, and no block changes hands in between (blocks are freed on the host, after a drain, and
 // reused only by frames enqueued after it).  The two sets are disjoint.
+// T: element type of the request's feature column; a 2-byte row is widened to f32 where it is loaded, and the arena row,
+// its BF16 copy and the history row are written from the widened values.
+template <class T>
 __global__ void feat_store_kernel(Params p, TrackStore ts, Frame f) {
   int w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   int lane = threadIdx.x & 31;
@@ -314,11 +318,55 @@ __global__ void feat_store_kernel(Params p, TrackStore ts, Frame f) {
   const int dst = f.feat_dst[w];
   const int hdst = f.hist_dst ? f.hist_dst[w] : -1;
   if (dst < 0 && hdst < 0) return;
-  const float* src = f.in_feat + (size_t)w * p.feature_dim;
+  const T* src = static_cast<const T*>(f.in_feat) + (size_t)w * p.feature_dim;
   float* d = ts.feat + (size_t)max(dst, 0) * p.d8;
   __nv_bfloat16* db = reinterpret_cast<__nv_bfloat16*>(ts.feat_bf16) + (size_t)max(dst, 0) * p.d8;
   float* hd = hdst >= 0 ? ts.hrows + (size_t)hdst * p.d8 : nullptr;
-  if (p.feature_dim == p.d8 && (reinterpret_cast<uintptr_t>(f.in_feat) & 15) == 0) {
+  if constexpr (!std::is_same<T, float>::value) {
+    if (p.feature_dim == p.d8 && (reinterpret_cast<uintptr_t>(f.in_feat) & 15) == 0) {
+      // rows are 16-byte multiples: one 16-byte load is 8 elements, four in flight per lane
+      const uint4* s8 = reinterpret_cast<const uint4*>(src);
+      float4* d4 = reinterpret_cast<float4*>(d);
+      float4* h4 = reinterpret_cast<float4*>(hd);
+      uint4* b8 = reinterpret_cast<uint4*>(db);
+      const int n8 = p.d8 >> 3;
+      for (int i0 = 0; i0 < n8; i0 += 128) {
+        uint4 r[4];
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+          const int i = i0 + u * 32 + lane;
+          if (i < n8) r[u] = __ldcs(s8 + i);   // the input row is dead after this kernel
+        }
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+          const int i = i0 + u * 32 + lane;
+          if (i < n8) {
+            float x[8];
+            feat_widen8(r[u], src, x);
+            const float4 lo = make_float4(x[0], x[1], x[2], x[3]), hi = make_float4(x[4], x[5], x[6], x[7]);
+            if (dst >= 0) {
+              d4[2 * i] = lo;
+              d4[2 * i + 1] = hi;
+              __nv_bfloat162 bb[4];
+#pragma unroll
+              for (int l = 0; l < 4; ++l) bb[l] = __floats2bfloat162_rn(x[2 * l], x[2 * l + 1]);
+              b8[i] = *reinterpret_cast<const uint4*>(bb);   // B operand of the tensor-core screen
+            }
+            if (h4) { __stcs(h4 + 2 * i, lo); __stcs(h4 + 2 * i + 1, hi); }
+          }
+        }
+      }
+    } else {
+      for (int i = lane; i < p.d8; i += 32) {
+        float x = i < p.feature_dim ? feat_elem(src, i) : 0.0f;   // Feature::from_vec zero-pads to the 8-lane multiple
+        if (dst >= 0) {
+          d[i] = x;
+          db[i] = __float2bfloat16_rn(x);
+        }
+        if (hd) hd[i] = x;
+      }
+    }
+  } else if (p.feature_dim == p.d8 && (reinterpret_cast<uintptr_t>(f.in_feat) & 15) == 0) {
     // rows are 32-byte multiples: 16-byte vectors, four in flight per lane
     const float4* s4 = reinterpret_cast<const float4*>(src);
     float4* d4 = reinterpret_cast<float4*>(d);
@@ -408,7 +456,9 @@ void launch_apply(const Params& p, const TrackStore& ts, const Frame& f, int n_s
 bool launch_feat_store(const Params& p, const TrackStore& ts, const Frame& f, cudaStream_t st) {
   if (!(p.is_visual && f.in_feat && f.total > 0)) return false;
   long long threads = (long long)f.total * 32;
-  feat_store_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(p, ts, f);
+  feat_dispatch(f.feat_type, [&](auto t) {
+    feat_store_kernel<decltype(t)><<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(p, ts, f);
+  });
   note_launch();
   return true;
 }

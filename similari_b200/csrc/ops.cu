@@ -293,8 +293,8 @@ int sb200_visual_cost_matrix(int32_t visual_kind, float threshold, const float* 
     tc.total_cols = n;
     if (!tc.d_tiles || !f.c_bf16 || !ts.feat_bf16 || !tc.colmeta || !tc.colgeo || !tc.rowmeta || !tc.colb || !tc.colvalid)
       return ops_fail(SB200_ERR_CUDA, "cudaMalloc failed");
-    sb::launch_to_bf16(ft.in_feat, d, d, p.d8, n, ts.feat_bf16, sc.st);
-    sb::launch_to_bf16(f.in_feat, d, d, p.d8, m, f.c_bf16, sc.st);   // (the tracker fuses this into cand_norm_kernel)
+    sb::launch_to_bf16(static_cast<const float*>(ft.in_feat), d, d, p.d8, n, ts.feat_bf16, sc.st);
+    sb::launch_to_bf16(static_cast<const float*>(f.in_feat), d, d, p.d8, m, f.c_bf16, sc.st);   // (the tracker fuses this into cand_norm_kernel)
   }
   ts.fnorm2 = ft.c_norm2;
   int vr = sb::launch_vis_cost(p, ts, f, 1, m, n, tc, sc.st);

@@ -11,6 +11,8 @@
 //   per frame     : candidates in request order; cost matrices packed per scene (row-major m x n, and
 //                   m x n x K for visual distances), NaN == None.
 #pragma once
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -158,14 +160,55 @@ __device__ __forceinline__ size_t feat_block(const TrackStore& ts, int slot, siz
   return ts.fblk ? (size_t)slot * ts.track_cap + (size_t)ts.fblk[ti] : ti;
 }
 
+// Element type of the request's feature column (SB200_FEATURE_*).  The kernels that read the column are instantiated per
+// type and widen each element where they load it; widening binary16 / bfloat16 to f32 is exact, so every later step sees
+// the values of the widened f32 request.
+constexpr int kFeatF32 = 0, kFeatF16 = 1, kFeatBF16 = 2;
+
+// Widening from the bits, so that NaN payloads move as the IEEE widening (and numpy's astype) moves them: a binary16 NaN
+// keeps its sign and its 10 payload bits in the top of the f32 payload; a bfloat16 is the top half of its f32.
+__device__ __forceinline__ float widen_f16(unsigned int h) {
+  if ((h & 0x7c00u) == 0x7c00u) return __uint_as_float(((h & 0x8000u) << 16) | 0x7f800000u | ((h & 0x3ffu) << 13));
+  return __half2float(__ushort_as_half((unsigned short)h));   // finite values (subnormals included): exact
+}
+__device__ __forceinline__ float widen_bf16(unsigned int b) { return __uint_as_float(b << 16); }
+
+__device__ __forceinline__ float feat_elem(const float* p, size_t i) { return p[i]; }
+__device__ __forceinline__ float feat_elem(const __half* p, size_t i) {
+  return widen_f16(reinterpret_cast<const unsigned short*>(p)[i]);
+}
+__device__ __forceinline__ float feat_elem(const __nv_bfloat16* p, size_t i) {
+  return widen_bf16(reinterpret_cast<const unsigned short*>(p)[i]);
+}
+// the 8 elements of one 16-byte load of a 2-byte column, widened
+__device__ __forceinline__ void feat_widen8(const uint4& r, const __half*, float* x) {
+  const unsigned int w[4] = {r.x, r.y, r.z, r.w};
+#pragma unroll
+  for (int i = 0; i < 4; ++i) { x[2 * i] = widen_f16(w[i] & 0xffffu); x[2 * i + 1] = widen_f16(w[i] >> 16); }
+}
+__device__ __forceinline__ void feat_widen8(const uint4& r, const __nv_bfloat16*, float* x) {
+  const unsigned int w[4] = {r.x, r.y, r.z, r.w};
+#pragma unroll
+  for (int i = 0; i < 4; ++i) { x[2 * i] = widen_bf16(w[i] & 0xffffu); x[2 * i + 1] = __uint_as_float(w[i] & 0xffff0000u); }
+}
+// Host side: calls fn(T{}) with T the element type of `type` (float, __half or __nv_bfloat16), so that a launcher can
+// start the kernel instance of the frame's type.
+template <class Fn>
+inline void feat_dispatch(int type, Fn&& fn) {
+  if (type == kFeatF16) fn(__half());
+  else if (type == kFeatBF16) fn(__nv_bfloat16());
+  else fn(float());
+}
+
 struct Frame {  // per-request transient device buffers (a request may be processed in scene chunks)
   int total;               // detections of this chunk
   int det0;                // first detection of this chunk (global row of the request)
   int scene0;              // first scene of this chunk (index into the request)
+  int feat_type;           // element type of in_feat (kFeatF32 / kFeatF16 / kFeatBF16), fixed when the frame is enqueued
   const int* new_count_all;  // [all scenes of the request] (ids of non-batch trackers need the global prefix)
   long long pos_fill_off;  // offset of this chunk's positional matrices inside `pos`
   const float* in_boxes;   // [total][6] raw request boxes
-  const float* in_feat;    // [total][D] or null
+  const void* in_feat;     // [total][D] elements of type feat_type, or null
   const unsigned char* in_hasf;
   const float* in_quality;
   const long long* in_custom;

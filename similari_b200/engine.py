@@ -19,6 +19,20 @@ def _f32(a):
     return np.ascontiguousarray(a, dtype=np.float32)
 
 
+# element types of the features column (sb200_set_feature_type)
+FEATURE_TYPES = {"f32": _lib.FEATURE_F32, "f16": _lib.FEATURE_F16, "bf16": _lib.FEATURE_BF16}
+
+
+def _raw16(a, feature_type):
+    """C-contiguous array of 2-byte elements passed as the feature column of type `feature_type` without conversion."""
+    if feature_type not in FEATURE_TYPES:
+        raise ValueError(f"feature_type must be one of {sorted(FEATURE_TYPES)}")
+    a = np.ascontiguousarray(a)
+    if a.dtype.itemsize != 2:
+        raise ValueError(f"feature_type={feature_type!r} needs an array of 2-byte elements, got {a.dtype}")
+    return a
+
+
 class Tracker:
     """Device-resident Sort / BatchSort / VisualSort / BatchVisualSort (selected by opts.kind)."""
 
@@ -52,16 +66,28 @@ class Tracker:
 
     def predict_batch(self, scene_ids, det_offsets, boxes, features=None, has_feature=None, quality=None,
                       custom_ids=None, own_area=None, want=("ids", "epochs", "lengths", "voting_types", "predicted",
-                                                            "observed"), out=None, wait=True):
+                                                            "observed"), out=None, wait=True, feature_type=None):
         """Host-pointer call (sb200_predict_batch).  Returns a dict of numpy arrays (the SortTrack columns).
-        wait=False: sb200_predict_batch_async -- the arrays (pass pinned ones in `out`) are defined after sync()."""
+        wait=False: sb200_predict_batch_async -- the arrays (pass pinned ones in `out`) are defined after sync().
+        Features: a float16 array is sent as it is; any other dtype is widened to float32.  feature_type="bf16" (or
+        "f16") sends a 2-byte array (e.g. the uint16 bits of bfloat16 values) as it is, with that element type."""
         scene_ids = np.ascontiguousarray(scene_ids, dtype=np.uint64)
         det_offsets = np.ascontiguousarray(det_offsets, dtype=np.int32)
         total = int(det_offsets[-1]) if len(det_offsets) else 0
         boxes = _f32(boxes).reshape(-1, 6)
         if len(boxes) != total:
             raise ValueError("boxes rows != det_offsets[-1]")
-        features = _f32(features) if features is not None else None
+        if features is not None:
+            # float16 rows go to the device as they are (the kernels widen them exactly); anything else is widened here
+            if feature_type not in (None, "f32"):
+                features = _raw16(features, feature_type)
+                self._use_feature_type(feature_type)
+            elif feature_type is None and isinstance(features, np.ndarray) and features.dtype == np.float16:
+                features = np.ascontiguousarray(features)
+                self._use_feature_type("f16")
+            else:
+                features = _f32(features)
+                self._use_feature_type("f32")
         has_feature = np.ascontiguousarray(has_feature, dtype=np.uint8) if has_feature is not None else None
         quality = _f32(quality) if quality is not None else None
         custom_ids = np.ascontiguousarray(custom_ids, dtype=np.int64) if custom_ids is not None else None
@@ -88,6 +114,24 @@ class Tracker:
         if not wait:   # the caller's arrays must outlive the frame
             self._keep = getattr(self, "_keep", [])[-16:] + [(boxes, features, has_feature, quality, custom_ids, own_area, out)]
         return out
+
+    def set_feature_type(self, feature_type):
+        """sb200_set_feature_type: element type ("f32", "f16" or "bf16") of the features column of the calls that follow.
+        Frames already enqueued keep theirs.  A new or loaded tracker reads "f32"."""
+        if feature_type not in FEATURE_TYPES:
+            raise ValueError(f"feature_type must be one of {sorted(FEATURE_TYPES)}")
+        check(self._L.sb200_set_feature_type(self._h, FEATURE_TYPES[feature_type]))
+        self._feature_type = feature_type
+
+    @property
+    def feature_type(self):
+        return getattr(self, "_feature_type", "f32")
+
+    def _use_feature_type(self, feature_type):
+        # (Sort / BatchSort ignore the features column, so their type never needs setting)
+        visual = self.opts.kind in (_lib.KIND_VISUAL_SORT, _lib.KIND_BATCH_VISUAL_SORT)
+        if visual and feature_type != self.feature_type:
+            self.set_feature_type(feature_type)
 
     def set_feature_dim(self, dim):
         """sb200_set_feature_dim: fixes the feature length of a visual tracker that has not stored a feature yet."""
@@ -116,22 +160,39 @@ class Tracker:
         check(self._L.sb200_host_counters(self._h, ptr(o)))
         return {"calls": int(o[0]), "ms_total": float(o[1]), "ms_blocked": float(o[2])}
 
-    def prefetch_inputs(self, boxes, features=None, has_feature=None, quality=None, custom_ids=None, own_area=None):
+    def prefetch_inputs(self, boxes, features=None, has_feature=None, quality=None, custom_ids=None, own_area=None,
+                        feature_type=None):
         """sb200_prefetch_inputs: start the H2D copy of a future request.  The arrays must be the very objects later
-        passed to predict_batch (same memory) and C-contiguous with the right dtype (no conversion copies)."""
-        for a, dt in ((boxes, np.float32), (features, np.float32), (has_feature, np.uint8), (quality, np.float32),
+        passed to predict_batch (same memory) and C-contiguous with the right dtype (no conversion copies).  Features
+        may be float32 or float16; the tracker's feature type follows them, and the later predict_batch must pass the
+        same array (a predict under another type copies the columns again)."""
+        if feature_type is None:
+            feature_type = "f16" if isinstance(features, np.ndarray) and features.dtype == np.float16 else "f32"
+        if feature_type not in FEATURE_TYPES:
+            raise ValueError(f"feature_type must be one of {sorted(FEATURE_TYPES)}")
+        fdt = np.float32 if feature_type == "f32" else (features.dtype if isinstance(features, np.ndarray) else np.float16)
+        if fdt != np.float32 and np.dtype(fdt).itemsize != 2:
+            raise ValueError("f16 / bf16 features need an array of 2-byte elements")
+        for a, dt in ((boxes, np.float32), (features, fdt), (has_feature, np.uint8), (quality, np.float32),
                       (custom_ids, np.int64), (own_area, np.float32)):
             if a is not None and not (isinstance(a, np.ndarray) and a.dtype == dt and a.flags["C_CONTIGUOUS"]):
                 raise ValueError("prefetch_inputs needs C-contiguous numpy arrays of the exact dtype")
+        if features is not None:
+            self._use_feature_type(feature_type)
         total = int(np.prod(boxes.shape)) // 6
         check(self._L.sb200_prefetch_inputs(self._h, total, ptr(boxes), ptr(features), ptr(has_feature), ptr(quality),
                                             ptr(custom_ids), ptr(own_area)))
 
     def predict_batch_device(self, scene_ids, det_offsets, d_boxes, d_features=0, d_has_feature=0, d_quality=0,
                              d_custom_ids=0, d_own_area=0, d_ids=0, d_epochs=0, d_lengths=0, d_voting_types=0,
-                             d_predicted=0, d_observed=0):
+                             d_predicted=0, d_observed=0, feature_type="f32"):
         """Device-pointer call (sb200_predict_batch_device); d_* are raw device addresses (0 == NULL).  Stream-ordered:
-        returns as soon as the frame is enqueued."""
+        returns as soon as the frame is enqueued.  feature_type: element type of d_features ("f32", "f16" or "bf16",
+        e.g. the data_ptr() of a torch float16 / bfloat16 CUDA tensor)."""
+        if d_features:
+            if feature_type not in FEATURE_TYPES:
+                raise ValueError(f"feature_type must be one of {sorted(FEATURE_TYPES)}")
+            self._use_feature_type(feature_type)
         scene_ids = np.ascontiguousarray(scene_ids, dtype=np.uint64)
         det_offsets = np.ascontiguousarray(det_offsets, dtype=np.int32)
         vp = lambda a: C.c_void_p(a) if a else None  # noqa: E731
