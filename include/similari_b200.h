@@ -260,6 +260,9 @@ int64_t sb200_last_costs(sb200_tracker* t, uint64_t scene_id, int64_t cap, float
  * summed times of the dominant visual-cost kernel and of the refinement; frames in which those two ran }.  Either may
  * be NULL.  bench.py reads it before and after its timed region. */
 int sb200_work_counters(sb200_tracker* t, uint64_t* counters4, double* ms8);
+/* Screen precision counters, cumulative over the frames absorbed so far: frames screened on e4m3 operands, frames screened
+   on BF16 operands, survivors of those screens refined, survivors the exact test cut.  Waits for the frames in flight. */
+int sb200_screen_counters(sb200_tracker* t, uint64_t* counters4);
 /* Kernels this library has launched since it was loaded (every launch site counts itself). */
 uint64_t sb200_launch_count(void);
 /* Per-stage device times (ms) of the last completed predict call: prep, positional cost, visual cost, voting, apply. */

@@ -82,7 +82,7 @@ EXPORTS = [
     "sb200_idle_tracks", "sb200_scene_tracks", "sb200_last_costs", "sb200_last_stage_ms", "sb200_last_kernel_ms", "sb200_sort_cost_matrix",
     "sb200_visual_cost_matrix", "sb200_sort_voting", "sb200_visual_voting", "sb200_kalman_initiate",
     "sb200_kalman_predict", "sb200_kalman_update", "sb200_nms", "sb200_own_area_shares", "sb200_host_alloc", "sb200_host_free",
-    "sb200_predict_batch_async", "sb200_sync", "sb200_frames_in_flight", "sb200_work_counters", "sb200_launch_count",
+    "sb200_predict_batch_async", "sb200_sync", "sb200_frames_in_flight", "sb200_work_counters", "sb200_screen_counters", "sb200_launch_count",
     "sb200_set_feature_dim", "sb200_comm_unique_id", "sb200_comm_create", "sb200_comm_destroy", "sb200_shard_scatter",
     "sb200_shard_gather", "sb200_wasted_history", "sb200_host_counters", "sb200_set_stream_join", "sb200_stream_join",
     "sb200_nms_batch", "sb200_nms_batch_device", "sb200_kalman_distance", "sb200_point_kalman_initiate",
@@ -126,6 +126,7 @@ def lib():
         "sb200_shard_gather": (C.c_int, [vp, i32, vp, C.POINTER(PredictOut), C.POINTER(PredictOut), vp]),
         "sb200_frames_in_flight": (C.c_int, [vp]),
         "sb200_work_counters": (C.c_int, [vp, vp, vp]),
+        "sb200_screen_counters": (C.c_int, [vp, vp]),
         "sb200_launch_count": (u64, []),
         "sb200_host_counters": (C.c_int, [vp, vp]),
         "sb200_predict_batch_device": (C.c_int, [vp, i32, vp, vp, vp, vp, vp, vp, vp, vp, C.POINTER(PredictOut)]),

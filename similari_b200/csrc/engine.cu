@@ -138,6 +138,7 @@ int make_params(const sb200_options& o, sb::Params* out) {
     p.feature_dim = o.feature_dim;
     p.d8 = (o.feature_dim + 7) / 8 * 8;
     p.vis_rel_err = sb::screen_rel_err(o.feature_dim);
+    p.vis_rel_err8 = sb::screen_rel_err_fp8(o.feature_dim);
     p.max_obs = o.visual_max_observations;
     p.min_votes = o.visual_min_votes;
     p.min_track_length = o.visual_minimal_track_length;
@@ -198,6 +199,7 @@ struct sb200_tracker {
     cudaEvent_t ev[6]{}, ev_k[3]{}, ev_pos[2]{};
     bool tc_timed = false, pos_forked = false;
     int mode = 0;              // visual cost path of the frame: 0 none / exact SIMT, 1 screen + refine, 2 dense tensor-core
+    bool fp8 = false;          // mode 1 on the e4m3 screen
   } pend[kDepth];
   int pend_head = 0, pend_count = 0;
   std::vector<int> pending_add;   // per slot: detections of the frames in flight (each can add at most that many tracks)
@@ -210,6 +212,14 @@ struct sb200_tracker {
   unsigned long long host_calls = 0;
   double acc_stage_ms[5]{}, acc_kernel_ms[2]{};
   unsigned long long acc_tc_frames = 0;
+  // Screen precision.  The e4m3 screen (twice the tensor rate of BF16) is the default where d8 <= 512; its slack is ~30x
+  // the BF16 one, too wide when the threshold sits in the bulk of the distance distribution.  After a frame on it where
+  // most survivors failed the exact test, or a survivor list overflowed, the next kFp8Hold screened frames take the BF16
+  // screen, then e4m3 is tried again.
+  static constexpr int kFp8Hold = 64;
+  int fp8_hold = 0;
+  // cumulative over the absorbed screened frames: frames on e4m3, frames on BF16, survivors refined, survivors cut
+  unsigned long long acc_screen[4] = {0, 0, 0, 0};
   // high-priority side stream: the frame tables and the screen's column metadata beside the candidate preparation, the
   // end-of-frame sweep beside the feature store
   cudaStream_t side_stream = nullptr;
@@ -232,7 +242,7 @@ struct sb200_tracker {
   // device track store
   sb::TrackStore ts{};
   DBuf b_id, b_epoch, b_length, b_custom, b_vt, b_pred, b_obs, b_radius, b_kst, b_vert, b_hpred, b_hobs, b_feat, b_feat_bf16, b_fnorm2, b_obs_phys,
-      b_obs_hasf, b_obs_q, b_obs_n, b_feat_cnt, b_fblk, b_blk_owner, b_blk_free;
+      b_feat_fp8, b_fscale, b_obs_hasf, b_obs_q, b_obs_n, b_feat_cnt, b_fblk, b_blk_owner, b_blk_free;
   DBuf b_ntracks, b_cur_epoch, b_scene_ids, b_nfree, b_atop;
   // wasted
   sb::WastedBuf wb{};
@@ -261,9 +271,10 @@ struct sb200_tracker {
   } stg[2];
   int stg_last = 1;   // staging set used by the most recent predict
   DBuf f_cbox2[2], f_cradius2[2], f_cconf2[2], f_cvert2[2], f_cflags2[2], f_cnorm22[2], f_cbf162[2], f_decided2[2];   // candidate side, two sets
+  DBuf f_cfp82[2], f_cscale2[2];
   DBuf f_winner, f_cvt, f_pos, f_vis, f_scenes, f_newcount,
       f_status, f_featdst, f_apprank, f_appmeta, f_frameout, f_excl, f_prewin, f_own, f_ownovf, f_dyn, f_ws, f_tmeta, f_rowinfo, f_slabc, f_slabm, f_slabmask,
-      f_dscene, f_maxc, f_maxcval, f_drowb, f_dcolb, f_slabk, f_scene_max, f_tiles, f_pairs, f_colmeta, f_colgeo, f_colb, f_colvalid, f_rowmeta, f_poslist, f_counters, f_visval;
+      f_dscene, f_maxc, f_maxcval, f_drowb, f_dcolb, f_slabk, f_scene_max, f_tiles, f_pairs, f_colmeta, f_colgeo, f_colb, f_colvalid, f_rowmeta, f_poslist, f_counters, f_visval, f_colsb;
   int num_sms = 132;
   DBuf o_ids, o_epochs, o_lengths, o_vt, o_pred, o_obs;
   HBuf h_small;
@@ -285,11 +296,11 @@ struct sb200_tracker {
                    &b_fblk, &b_blk_owner, &b_blk_free, &b_nfree, &b_atop, &f_frameout, &f_excl, &f_prewin, &f_own, &f_ownovf, &f_dyn, &b_idc, &f_ws, &f_tmeta, &f_rowinfo, &f_slabc, &f_slabm, &f_slabmask, &f_dscene, &f_maxc, &f_maxcval, &f_drowb, &f_dcolb, &f_slabk,
                    &b_scene_ids, &w_count, &w_id, &w_scene, &w_epoch, &w_length, &w_pred, &w_obs, &f_winner, &f_cvt, &f_pos, &f_vis, &f_scenes, &f_newcount, &f_status,
                    &f_featdst, &f_apprank, &f_appmeta, &o_ids, &o_epochs, &o_lengths, &o_vt, &o_pred, &o_obs,
-                   &b_hblk, &b_hrows, &b_hpresent, &b_hfree, &b_hpool, &w_hblk, &f_histdst};
+                   &b_hblk, &b_hrows, &b_hpresent, &b_hfree, &b_hpool, &w_hblk, &f_histdst, &b_feat_fp8, &b_fscale, &f_colsb};
     for (DBuf* b : all) b->release();
     for (int k = 0; k < 2; ++k) {
       f_cbox2[k].release(); f_cradius2[k].release(); f_cconf2[k].release(); f_cvert2[k].release(); f_cflags2[k].release();
-      f_cnorm22[k].release(); f_cbf162[k].release(); f_decided2[k].release();
+      f_cnorm22[k].release(); f_cbf162[k].release(); f_decided2[k].release(); f_cfp82[k].release(); f_cscale2[k].release();
     }
     if (stream) cudaStreamSynchronize(stream);
     h_small.release();
@@ -339,6 +350,15 @@ struct sb200_tracker {
     return 0;
   }
 
+  // The e4m3 copies of the feature rows are not part of the state blob: after a load / import they are converted again from
+  // the f32 rows of the arena blocks [0, top) of each listed slot (one launch per slot).
+  int regen_fp8(int slot, int top) {
+    if (!ts.feat_fp8 || top <= 0) return 0;
+    const long long r0 = (long long)slot * track_cap * P.max_obs, rows = (long long)top * P.max_obs;
+    sb::launch_to_fp8(ts.feat + r0 * P.d8, P.d8, P.d8, P.d8, rows, ts.feat_fp8 + r0 * sb::fp8_pitch(P.d8), ts.fscale + r0, stream);
+    return cudaGetLastError() == cudaSuccess ? 0 : fail(SB200_ERR_CUDA, "e4m3 row conversion failed");
+  }
+
   int ensure_store(int need_scenes, int need_tracks) {
     if (need_scenes <= scene_cap && need_tracks <= track_cap) return 0;
     int ns = scene_cap, nt = track_cap;
@@ -371,6 +391,10 @@ struct sb200_tracker {
         ts.feat_bf16 = tmp;
       }
       if ((rc = regrow(b_fnorm2, &ts.fnorm2, K, ns, nt))) return rc;
+      if (P.d8 <= sb::kFp8MaxD8) {   // the e4m3 copies: only the A-stationary screen (d8 <= 512) reads them
+        if ((rc = regrow(b_feat_fp8, &ts.feat_fp8, K * sb::fp8_pitch(P.d8), ns, nt))) return rc;
+        if ((rc = regrow(b_fscale, &ts.fscale, K, ns, nt))) return rc;
+      }
       if ((rc = regrow(b_obs_phys, &ts.obs_phys, K, ns, nt))) return rc;
       if ((rc = regrow(b_obs_hasf, &ts.obs_hasf, K, ns, nt))) return rc;
       if ((rc = regrow(b_obs_q, &ts.obs_q, K, ns, nt))) return rc;
@@ -687,8 +711,17 @@ int sb200_tracker::absorb_oldest(bool block) {
       last_dense_scenes = dense_scenes;
       // most scenes of a screened frame overflowed their survivor lists: the threshold cuts (almost) nothing, so the
       // following frames take the dense tensor-core path; and back, if that path's precondition keeps failing
-      if (q.mode == 1 && n >= 1 && dense_scenes * 4 > n) adapt_dense = true;
+      // (an overflow of the e4m3 screen says that its slack is too wide, not that the threshold cuts nothing)
+      if (q.mode == 1 && !q.fp8 && n >= 1 && dense_scenes * 4 > n) adapt_dense = true;
       if (q.mode == 2 && n >= 1 && dense_scenes * 4 > n) adapt_dense = false;
+      if (q.mode == 1) {
+        const int* sc = reinterpret_cast<const int*>(reinterpret_cast<const char*>(dyn) + sizeof(sb::FrameDyn) + 16);
+        const unsigned long long kept = (unsigned int)sc[0], cut = (unsigned int)sc[1], ovf = (unsigned int)sc[2];
+        acc_screen[q.fp8 ? 0 : 1] += 1;
+        acc_screen[2] += kept;
+        acc_screen[3] += cut;
+        if (q.fp8 && (ovf > 0 || 2 * cut > kept)) fp8_hold = kFp8Hold;
+      }
     }
     for (int i = 0; i < 5; ++i) cudaEventElapsedTime(&stage_ms[i], q.ev[i], q.ev[i + 1]);
     if (q.pos_forked) {
@@ -898,12 +931,12 @@ int sb200_tracker::predict(int32_t n_scenes, const uint64_t* scene_ids, const in
     for (auto& e : q.ev_pos) CU(cudaEventCreate(&e));
   }
   if ((rc = q.h_req.ensure(sizeof(sb::SceneReq) * (size_t)n_scenes)) ||
-      (rc = q.h_out.ensure(dyn_offset(n_scenes) + sizeof(sb::FrameDyn) + 16)))
+      (rc = q.h_out.ensure(dyn_offset(n_scenes) + sizeof(sb::FrameDyn) + 32)))
     return rc;
   // visual cost path of this frame: tensor-core screen + exact refinement for large frames with a selective threshold, the
   // dense tensor-core weight sums for thresholds that cut nothing, the exact SIMT kernel otherwise (small frames, and as the
   // device-side fallback of single scenes)
-  bool want_tc = false, want_dense = false;
+  bool want_tc = false, want_dense = false, want_fp8 = false;
   if (P.is_visual && features != nullptr && total > 0) {
     const bool selective = P.visual_kind == SB200_VIS_EUCLIDEAN ? (P.visual_threshold < 1e18f) : (P.visual_threshold > -1.0f);
     const bool big = P.d8 >= 64 && work * P.d8 >= (1ll << 28);
@@ -915,6 +948,17 @@ int sb200_tracker::predict(int32_t n_scenes, const uint64_t* scene_ids, const in
       if (!strcmp(e, "simt")) { want_tc = false; want_dense = false; }
       else if (!strcmp(e, "tc")) { want_tc = work > 0; want_dense = false; }
       else if (!strcmp(e, "dense")) { want_dense = work > 0 && dense_ok; want_tc = work > 0 && !want_dense; }
+      else if (!strcmp(e, "tc8") || !strcmp(e, "tc16")) { want_tc = work > 0; want_dense = false; }
+    }
+    // screen precision (d8 <= 512): e4m3 unless a recent e4m3 frame showed its slack to be too wide; SB200_VIS_KERNEL=tc8 /
+    // tc16 force one
+    const char* ek = getenv("SB200_VIS_KERNEL");
+    const bool can8 = want_tc && P.d8 <= sb::kFp8MaxD8 && ts.feat_fp8 != nullptr;
+    if (ek && !strcmp(ek, "tc8")) want_fp8 = can8;
+    else if (ek && !strcmp(ek, "tc16")) want_fp8 = false;
+    else {
+      want_fp8 = can8 && fp8_hold == 0;
+      if (can8 && fp8_hold > 0) fp8_hold -= 1;
     }
   }
   const int vote_cap = want_dense ? kDenseVoteCap : sb::kVoteVisCap;
@@ -949,7 +993,8 @@ int sb200_tracker::predict(int32_t n_scenes, const uint64_t* scene_ids, const in
   // candidate-side buffers: the set of this frame (the other one may still be read by the frame in front of it)
   const int cset = (int)(frame_seq & 1);
   DBuf &f_cbox = f_cbox2[cset], &f_cradius = f_cradius2[cset], &f_cconf = f_cconf2[cset], &f_cvert = f_cvert2[cset],
-       &f_cflags = f_cflags2[cset], &f_cnorm2 = f_cnorm22[cset], &f_cbf16 = f_cbf162[cset], &f_decided = f_decided2[cset];
+       &f_cflags = f_cflags2[cset], &f_cnorm2 = f_cnorm22[cset], &f_cbf16 = f_cbf162[cset], &f_decided = f_decided2[cset],
+       &f_cfp8 = f_cfp82[cset], &f_cscale = f_cscale2[cset];
   if ((rc = ENS(f_cbox, T * 24)) || (rc = ENS(f_cradius, T * 4)) || (rc = ENS(f_cconf, T * 4)) ||
       (rc = ENS(f_winner, T * 4)) || (rc = ENS(f_cvt, T)) || (rc = ENS(f_scenes, sizeof(sb::SceneDesc) * n_scenes)) ||
       (rc = ENS(f_newcount, 4 * (size_t)n_scenes)) || (rc = ENS(f_dyn, sizeof(sb::FrameDyn))) ||
@@ -993,6 +1038,10 @@ int sb200_tracker::predict(int32_t n_scenes, const uint64_t* scene_ids, const in
       tiles_alloc = std::max(tiles_alloc, hs * ((hd + mstep - 1) / mstep) * ((ht * K + cstep - 1) / cstep + 1));
       if (f_tiles.bytes > 0 && sizeof(sb::TcTile) * (size_t)tiles_alloc > f_tiles.bytes) tiles_alloc += tiles_alloc / 2;
     }
+    // both operand copies of the candidates whenever the e4m3 screen can run: a switch between the precisions must not
+    // allocate (and synchronise) in the middle of a stream of frames
+    const bool alloc8 = !want_dense && P.d8 <= sb::kFp8MaxD8 && ts.feat_fp8 != nullptr;
+    if (alloc8 && ((rc = ENS(f_cfp8, T * sb::fp8_pitch(P.d8))) || (rc = ENS(f_cscale, T * 4)))) return rc;
     if ((rc = ENS(f_cbf16, T * P.d8 * 2)) || (rc = ENS(f_tiles, sizeof(sb::TcTile) * (size_t)std::max<long long>(1, tiles_alloc))) ||
         (rc = ENS(f_rowmeta, sizeof(sb::VisRowMeta) * (T + 256))))
       return rc;
@@ -1013,6 +1062,11 @@ int sb200_tracker::predict(int32_t n_scenes, const uint64_t* scene_ids, const in
       tc.colb = f_colb.as<float>();
       tc.colvalid = f_colvalid.as<unsigned int>();
       tc.total_cols = (int)col_total;
+      if (alloc8 && P.visual_kind != SB200_VIS_COSINE) {
+        if ((rc = ENS(f_colsb, 4 * (size_t)(std::max(col_total, hint_cols) + 256)))) return rc;
+        if (want_fp8) tc.colsb = f_colsb.as<float>();
+      }
+      tc.fp8 = want_fp8;
     } else {
       // sized from the hints like the other frame buffers, so steady-state frames never reallocate
       const long long hs = std::max(opts.max_scenes_hint, n_scenes), ht = hint_tracks;
@@ -1118,7 +1172,9 @@ int sb200_tracker::predict(int32_t n_scenes, const uint64_t* scene_ids, const in
   f.app_rank = f_apprank.as<int2>(); f.app_meta = f_appmeta.as<int4>();
   if ((rc = ENS(f_frameout, sizeof(int) * 3 * (size_t)n_scenes))) return rc;
   f.frame_out = f_frameout.as<int>();
-  f.c_bf16 = tc.use_tc ? f_cbf16.p : nullptr; f.scene_max = f_scene_max.as<unsigned int>();
+  f.c_bf16 = tc.use_tc && !tc.fp8 ? f_cbf16.p : nullptr; f.scene_max = f_scene_max.as<unsigned int>();
+  f.c_fp8 = tc.fp8 ? f_cfp8.as<unsigned char>() : nullptr;
+  f.c_scale = tc.fp8 ? f_cscale.as<float>() : nullptr;
   // sparse entry lists + per-scene counters (pos_cnt | vis_cnt | scene_mode | vis_mode | refine_next | dense_cnt | status),
   // zeroed every frame by frame_setup_kernel
   const size_t n_counters = 6 * (size_t)n_scenes + 4;
@@ -1136,6 +1192,7 @@ int sb200_tracker::predict(int32_t n_scenes, const uint64_t* scene_ids, const in
   f.refine_next = f.pos_cnt + 4 * n_scenes;
   f.status = f.pos_cnt + 5 * n_scenes;
   f.dense_cnt = f.pos_cnt + 6 * n_scenes;
+  f.screen_cnt = tc.use_tc && !tc.dense ? f.dense_cnt + 1 : nullptr;   // the 3 ints after it: zeroed with the counters
   f.vis_pairs = f_pairs.as<sb::VisPair>();
   f.vis_val = f_visval.as<float>();
   // outputs
@@ -1180,6 +1237,7 @@ int sb200_tracker::predict(int32_t n_scenes, const uint64_t* scene_ids, const in
   q.tc_timed = false;
   q.pos_forked = false;
   q.mode = tc.dense ? 2 : (tc.use_tc ? 1 : 0);
+  q.fp8 = tc.use_tc && !tc.dense && tc.fp8;
   for (int s = 0; s < n_scenes; ++s) pending_add[last_req_slots[s]] += m_of[s];
   inflight_live_ub += live_ub;
   if (fhist_on) hpool_pend += total;
@@ -1347,6 +1405,8 @@ int sb200_tracker::predict(int32_t n_scenes, const uint64_t* scene_ids, const in
     CU(cudaMemcpyAsync(ho + dyn_offset(n_scenes) + sizeof(sb::FrameDyn), f.dense_cnt, 4, cudaMemcpyDeviceToHost, stream));
     if (fhist_on)
       CU(cudaMemcpyAsync(ho + dyn_offset(n_scenes) + sizeof(sb::FrameDyn) + 8, ts.hpool, 8, cudaMemcpyDeviceToHost, stream));
+    // the screen's survivors, the part of them the exact test cut, the scenes whose list overflowed (zeros on other paths)
+    CU(cudaMemcpyAsync(ho + dyn_offset(n_scenes) + sizeof(sb::FrameDyn) + 16, f.dense_cnt + 1, 12, cudaMemcpyDeviceToHost, stream));
   }
   static const bool trace_dense = trace && atoi(getenv("SB200_TRACE")) >= 2;   // synchronises: level 2 only
   if (trace_dense && tc.dense && tc.n_tiles > 0) {
@@ -1513,14 +1573,21 @@ int sb200_set_feature_dim(sb200_tracker* t, int32_t feature_dim) {
   t->P.feature_dim = feature_dim;
   t->P.d8 = (feature_dim + 7) / 8 * 8;
   t->P.vis_rel_err = sb::screen_rel_err(feature_dim);
+  t->P.vis_rel_err8 = sb::screen_rel_err_fp8(feature_dim);
   t->opts.feature_dim = feature_dim;
   t->b_feat.release(); t->b_feat_bf16.release(); t->f_cbf162[0].release(); t->f_cbf162[1].release();
-  t->ts.feat = nullptr; t->ts.feat_bf16 = nullptr;
+  t->b_feat_fp8.release(); t->b_fscale.release(); t->f_cfp82[0].release(); t->f_cfp82[1].release();
+  t->ts.feat = nullptr; t->ts.feat_bf16 = nullptr; t->ts.feat_fp8 = nullptr; t->ts.fscale = nullptr;
   const size_t rows = (size_t)t->scene_cap * t->track_cap * t->P.max_obs;
   if (rows > 0) {
     if ((rc = t->b_feat.ensure(rows * t->P.d8 * 4)) || (rc = t->b_feat_bf16.ensure(rows * t->P.d8 * 2))) return rc;
     t->ts.feat = t->b_feat.as<float>();
     t->ts.feat_bf16 = t->b_feat_bf16.p;
+    if (t->P.d8 <= sb::kFp8MaxD8) {
+      if ((rc = t->b_feat_fp8.ensure(rows * sb::fp8_pitch(t->P.d8))) || (rc = t->b_fscale.ensure(rows * 4))) return rc;
+      t->ts.feat_fp8 = t->b_feat_fp8.as<unsigned char>();
+      t->ts.fscale = t->b_fscale.as<float>();
+    }
   }
   for (auto& g : t->stg) g.feat.release();
   if (t->fhist_on && t->hpool_cap > 0) {
@@ -1591,6 +1658,15 @@ int sb200_work_counters(sb200_tracker* t, uint64_t* out3 /* [4] */, double* ms7 
     for (int i = 0; i < 5; ++i) ms7[i] = t->acc_stage_ms[i];
     ms7[5] = t->acc_kernel_ms[0]; ms7[6] = t->acc_kernel_ms[1]; ms7[7] = (double)t->acc_tc_frames;
   }
+  return 0;
+}
+
+int sb200_screen_counters(sb200_tracker* t, uint64_t* out4) {
+  if (!t || !out4) return fail(SB200_ERR_INVALID, "bad arguments");
+  CU(cudaSetDevice(t->device));
+  int rc = t->drain();
+  if (rc) return rc;
+  for (int i = 0; i < 4; ++i) out4[i] = t->acc_screen[i];
   return 0;
 }
 
@@ -2504,6 +2580,8 @@ int sb200_tracker_load(const void* src, size_t bytes, int32_t device, sb200_trac
   }
   if ((rc = move_store(t, 1, kBlobTracker, h, const_cast<char*>(dblob), rows, 0))) return rc;
   if ((rc = set_slots(t, st, 0, 0, 0, 0, false))) return rc;
+  for (size_t i = 0; i < table.size(); ++i)
+    if ((rc = t->regen_fp8((int)i, table[i].arena_top))) return rc;
   CU(cudaMemcpyAsync(t->b_idc.p, &h.id_counter, 8, cudaMemcpyHostToDevice, t->stream));
   if (h.wasted_count > 0) {
     const int wc = (int)h.wasted_count;
@@ -2609,6 +2687,8 @@ int sb200_scenes_import(sb200_tracker* t, const void* src, size_t bytes) {
   }
   if ((rc = move_store(t, 1, kBlobScenes, h, const_cast<char*>(dblob), rows, (int)hist_base))) return rc;
   if ((rc = set_slots(t, st, 0, 0, t->fhist_on ? (int)h.live_total : 0, h.id_counter, true))) return rc;
+  for (size_t i = 0; i < table.size(); ++i)
+    if ((rc = t->regen_fp8(dst_slot[i], table[i].arena_top))) return rc;
   for (size_t i = 0; i < table.size(); ++i) {
     const int slot = t->slot_for(table[i].scene_id, true);
     t->epoch[slot] = table[i].epoch; t->n_tracks[slot] = table[i].n_tracks; t->arena_top[slot] = table[i].arena_top;

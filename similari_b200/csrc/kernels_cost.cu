@@ -52,8 +52,8 @@ __device__ __forceinline__ float reduce_add8(const float* t) {
 }
 
 // One warp per detection: squared norm in the reference's order (per 8-lane block reduce_add, blocks accumulated
-// sequentially) and, when the tensor-core screen will run, the BF16 operand copy of the row -- the feature row is
-// read from HBM once for both.  T: element type of the request's feature column (f32, or a 2-byte type widened on load,
+// sequentially) and, when the tensor-core screen will run, the BF16 or the e4m3 operand copy of the row (f.c_bf16 /
+// f.c_fp8, whichever the frame's screen reads) -- the feature row is read from HBM once for all.  T: element type of the request's feature column (f32, or a 2-byte type widened on load,
 // where one 16-byte load is a whole 8-lane block).
 template <class T>
 __global__ void cand_norm_kernel(Params p, Frame f, __nv_bfloat16* __restrict__ bf16_out) {
@@ -74,6 +74,8 @@ __global__ void cand_norm_kernel(Params p, Frame f, __nv_bfloat16* __restrict__ 
     for (int h = 0; h < 2; ++h) {
       const int blk = base + h * 32 + lane;
       have[h] = blk < nblk;
+#pragma unroll
+      for (int l = 0; l < 8; ++l) x[h][l] = 0.0f;
       if (have[h]) {
         if (vec && blk * 8 + 8 <= p.feature_dim) {
           if constexpr (kF32) {
@@ -88,6 +90,10 @@ __global__ void cand_norm_kernel(Params p, Frame f, __nv_bfloat16* __restrict__ 
           for (int l = 0; l < 8; ++l) { int d = blk * 8 + l; x[h][l] = d < p.feature_dim ? feat_elem(row, d) : 0.0f; }
         }
       }
+    }
+    if (f.c_fp8) {   // d8 <= 512 (kFp8MaxD8): this round holds the whole row
+      const float s = fp8_row_store(x, p.d8, f.c_fp8 + (size_t)w * fp8_pitch(p.d8));
+      if (lane == 0) f.c_scale[w] = s;
     }
 #pragma unroll
     for (int h = 0; h < 2; ++h) {

@@ -446,7 +446,7 @@ __global__ void vis_dense_rowmeta_kernel(Params p, Frame f, VisRowMeta* rowmeta)
   VisRowMeta rm;
   rm.ok = (f.c_flags[g] & 2) ? 1 : 0;
   rm.rowk = p.visual_kind == 1 ? rsqrtf(na) : na;
-  rm.pad0 = 0; rm.pad1 = 0;
+  rm.rowi = 1.0f; rm.pad = 0;
   rowmeta[g] = rm;
 }
 

@@ -277,6 +277,7 @@ struct SaSmem {
   unsigned char b[SA_STAGES][SA_B_STAGE];
   VisColMeta meta[SA_SLABS][SA_BN];
   float colb[SA_SLABS][SA_BN];
+  float colsb[SA_SLABS][SA_BN];                     // e4m3 Euclidean screen only: the columns' scales
   unsigned int colvalid[SA_SLABS][SA_BN / 32];
   SaHdr hdr[SA_SLABS];
   unsigned long long a_full[SA_KMAX];
@@ -291,18 +292,25 @@ constexpr int kScreenStationaryMaxD8 = SA_KMAX * TC_BK;
 
 // units: TcTile (scene, m0, c0) with m0 a multiple of 256 and c0 a multiple of ucols; the unit covers the scene's rows
 // c0 .. min(c0 + ucols, nb * K)
-template <bool COSINE>
+//
+// FP8: the operands are the e4m3 copies (f.c_fp8, ts.feat_fp8) and every MMA is m64n128k32.e4m3.  A 128-byte swizzle row
+// then holds 128 features instead of 64: the same 16 KB blocks and stages carry twice the features, so A takes half the
+// blocks and the k-loop half the trips.  The row and column constants carry the rows' scales (vis_rowmeta_kernel,
+// vis_meta_kernel): the cosine test stays rowk * colb, the Euclidean one becomes acc * rowi >= fma(colsb, rowk, colb).
+template <bool COSINE, bool FP8>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 vis_screen_sa_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB, Params p,
                      TrackStore ts, Frame f, const TcTile* units, int n_units_host, const int* n_units_dev, int ucols,
                      const VisColMeta* colmeta, const VisColGeo* colgeo, const VisRowMeta* rowmeta, const float* colb,
-                     const unsigned int* colvalid) {
+                     const float* colsb, const unsigned int* colvalid) {
+  constexpr bool kScaled = FP8 && !COSINE;   // the Euclidean e4m3 test needs the columns' scales
+  constexpr int BKF = FP8 ? 2 * TC_BK : TC_BK;   // features per 128-byte swizzle row
   const int n_units = n_units_dev ? *n_units_dev : n_units_host;
   extern __shared__ unsigned char smem_raw_[];
   SaSmem& S = *reinterpret_cast<SaSmem*>(smem_raw_ + ((1024u - (smem_u32(smem_raw_) & 1023u)) & 1023u));
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int K = p.max_obs;
-  const int KB = (p.d8 + TC_BK - 1) / TC_BK;
+  const int KB = (p.d8 + BKF - 1) / BKF;
   const uint32_t crank = cluster_rank();
   if (threadIdx.x == 0) {
     // full: the local producer's expect_tx; empty: the consuming warpgroup of each CTA; a_empty: both local consumer
@@ -341,20 +349,21 @@ vis_screen_sa_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_cons
           h.col0 = sc.col_off + tl.c0 + ct * SA_BN; h.epoch = (int)sc.epoch; h.vis_lbase = sc.vis_lbase;
           h.vis_lcap = sc.vis_lcap; h.unit = unit; h.last = ct + 2 >= nct; h.pad = 0;
           S.hdr[g] = h;   // published by the release of the arrive below
-          mbar_expect_tx(&S.meta_full[g], (uint32_t)(sizeof(VisColMeta) * SA_BN + 4 * SA_BN + SA_BN / 8));
+          mbar_expect_tx(&S.meta_full[g], (uint32_t)(sizeof(VisColMeta) * SA_BN + (kScaled ? 8 : 4) * SA_BN + SA_BN / 8));
           bulk_load(S.meta[g], colmeta + h.col0, (uint32_t)(sizeof(VisColMeta) * SA_BN), &S.meta_full[g]);
           bulk_load(S.colb[g], colb + h.col0, 4 * SA_BN, &S.meta_full[g]);
+          if (kScaled) bulk_load(S.colsb[g], colsb + h.col0, 4 * SA_BN, &S.meta_full[g]);
           bulk_load(S.colvalid[g], colvalid + (h.col0 >> 5), SA_BN / 8, &S.meta_full[g]);   // col0 is a multiple of 128
           for (int kb = 0; kb < KB; ++kb, ++gk) {
             if (ct == 0) {
               mbar_expect_tx(&S.a_full[kb], SA_A_BLOCK);
-              tma_load_2d(S.a[kb], &mapA, kb * TC_BK, rowA, &S.a_full[kb]);
+              tma_load_2d(S.a[kb], &mapA, kb * BKF, rowA, &S.a_full[kb]);
             }
             const int s = gk % SA_STAGES;
             mbar_wait(&S.empty_bar[s], ((gk / SA_STAGES) & 1) ^ 1);   // both CTAs have released the stage
             mbar_expect_tx(&S.full_bar[s], SA_B_STAGE);
             // this CTA's half of the stage (rows rank*64 .. +64), delivered to both CTAs
-            tma_load_2d_mc(S.b[s] + crank * (SA_B_STAGE / 2), &mapB, kb * TC_BK, rowB + ct * SA_BN + (int)crank * (SA_BN / 2),
+            tma_load_2d_mc(S.b[s] + crank * (SA_B_STAGE / 2), &mapB, kb * BKF, rowB + ct * SA_BN + (int)crank * (SA_BN / 2),
                            &S.full_bar[s], (uint16_t)0x3);
           }
         }
@@ -387,7 +396,7 @@ vis_screen_sa_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_cons
         break;
       }
       // row constants of the 4 rows of this thread (rows past the tile's candidates read padding and are masked)
-      float rowk[2][2];
+      float rowk[2][2], rowi[2][2];
       bool row_ok[2][2];
 #pragma unroll
       for (int hh = 0; hh < 2; ++hh)
@@ -396,6 +405,7 @@ vis_screen_sa_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_cons
           const int m = h.m0 + 64 * hh + rr[hr];
           const VisRowMeta rm = rowmeta[h.det_base + m];
           rowk[hh][hr] = rm.rowk;
+          rowi[hh][hr] = rm.rowi;
           row_ok[hh][hr] = m < h.m && rm.ok;
         }
 
@@ -416,10 +426,15 @@ vis_screen_sa_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_cons
           const uint32_t b0 = smem_u32(S.b[stage]);
           wgmma_fence();
 #pragma unroll
-          for (int k = 0; k < TC_BK / 16; ++k) {
+          for (int k = 0; k < 4; ++k) {   // 32 bytes of the 128-byte swizzle row per MMA: k16 of BF16, k32 of e4m3
             const uint32_t acc_on = (kb | k) != 0 ? 1u : 0u;
-            wgmma_bf16_m64n128(acc, wgmma_desc(a0 + k * 32), wgmma_desc(b0 + k * 32), acc_on);
-            wgmma_bf16_m64n128(acc + 64, wgmma_desc(a0 + 64 * 128 + k * 32), wgmma_desc(b0 + k * 32), acc_on);
+            if (FP8) {
+              wgmma_e4m3_m64n128(acc, wgmma_desc(a0 + k * 32), wgmma_desc(b0 + k * 32), acc_on);
+              wgmma_e4m3_m64n128(acc + 64, wgmma_desc(a0 + 64 * 128 + k * 32), wgmma_desc(b0 + k * 32), acc_on);
+            } else {
+              wgmma_bf16_m64n128(acc, wgmma_desc(a0 + k * 32), wgmma_desc(b0 + k * 32), acc_on);
+              wgmma_bf16_m64n128(acc + 64, wgmma_desc(a0 + 64 * 128 + k * 32), wgmma_desc(b0 + k * 32), acc_on);
+            }
           }
           wgmma_commit();
           wgmma_wait<1>();   // the previous stage's MMAs have completed
@@ -455,11 +470,19 @@ vis_screen_sa_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_cons
 #pragma unroll
         for (int j = 0; j < SA_BN / 8; ++j) {
           const float2 cb = *reinterpret_cast<const float2*>(gcolb + 8 * j + q2);
+          float2 cs = make_float2(1.0f, 1.0f);
+          if (kScaled) cs = *reinterpret_cast<const float2*>(&S.colsb[ms][8 * j + q2]);
 #pragma unroll
           for (int e = 0; e < 4; ++e) {
             const float rk = rowk[hh][e >> 1], c = (e & 1) ? cb.y : cb.x;
-            const float b = COSINE ? rk * c : rk + c;
-            if (!(acc[64 * hh + 4 * j + e] < b)) keep[2 * hh + (j >> 3)] |= 1u << ((4 * j + e) & 31);
+            if (kScaled) {
+              // acc = 2^(ka + kb) dot~: acc 2^-ka >= 2^kb (rowk + colb), both sides exact scalings of the BF16 test's
+              const float b = __fmaf_rn((e & 1) ? cs.y : cs.x, rk, c);
+              if (!(acc[64 * hh + 4 * j + e] * rowi[hh][e >> 1] < b)) keep[2 * hh + (j >> 3)] |= 1u << ((4 * j + e) & 31);
+            } else {
+              const float b = COSINE ? rk * c : rk + c;
+              if (!(acc[64 * hh + 4 * j + e] < b)) keep[2 * hh + (j >> 3)] |= 1u << ((4 * j + e) & 31);
+            }
           }
         }
         keep[2 * hh] &= colm[0] & rowm;
@@ -599,10 +622,19 @@ __device__ __forceinline__ float refine_block_sum(const float* av, const float* 
 template <bool COSINE, bool TAIL, class T>
 __global__ void __launch_bounds__(RF_WARPS * 32, 8) vis_refine_kernel(Params p, TrackStore ts, Frame f, int* nan_flag) {
   __shared__ float s_bs[RF_WARPS][RF_CLAIM][RF_PITCH];
+  __shared__ int s_cnt[2];
   const int scene = blockIdx.y;
-  if (f.vis_mode[scene] != 0) return;  // survivor list overflowed: this scene is computed densely
+  if (f.vis_mode[scene] != 0) {   // survivor list overflowed: this scene is computed densely
+    if (f.screen_cnt && blockIdx.x == 0 && threadIdx.x == 0) atomicAdd(f.screen_cnt + 2, 1);
+    return;
+  }
   const SceneDesc sc = f.scenes[scene];
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  if (f.screen_cnt) {
+    if (threadIdx.x < 2) s_cnt[threadIdx.x] = 0;
+    __syncthreads();
+  }
+  int n_ref = 0, n_cut = 0;   // survivors this lane refined, and how many of them the exact test cut
   const int n_pairs = min(f.vis_cnt[scene], sc.vis_lcap);
   const int nblk = p.d8 / 8;
   const int D = p.feature_dim;
@@ -659,6 +691,8 @@ __global__ void __launch_bounds__(RF_WARPS * 32, 8) vis_refine_kernel(Params p, 
         if (d <= p.visual_threshold) v = d;
       }
       f.vis_val[sc.vis_lbase + i0 + lane] = v;
+      n_ref += 1;
+      n_cut += is_nan(v) ? 1 : 0;
       if (!is_nan(v) && !(v <= vmax)) vmax = v;   // best.rs "max_dist": maximum over the entries that exist
       if (nan_flag && is_nan(v)) nan_flag[scene] = 1;   // dense path: an entry the threshold cuts voids its precondition
     }
@@ -672,6 +706,13 @@ __global__ void __launch_bounds__(RF_WARPS * 32, 8) vis_refine_kernel(Params p, 
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) u = max(u, __shfl_xor_sync(0xffffffffu, u, o));
   if (lane == 0 && u != 0u) atomicMax(f.scene_max + scene, u);
+  if (f.screen_cnt) {   // the screen's selectivity: one shared atomic per warp, one global atomic per CTA
+    n_ref = __reduce_add_sync(0xffffffffu, n_ref);
+    n_cut = __reduce_add_sync(0xffffffffu, n_cut);
+    if (lane == 0 && n_ref) { atomicAdd(&s_cnt[0], n_ref); atomicAdd(&s_cnt[1], n_cut); }
+    __syncthreads();
+    if (threadIdx.x == 0 && s_cnt[0]) { atomicAdd(f.screen_cnt, s_cnt[0]); if (s_cnt[1]) atomicAdd(f.screen_cnt + 1, s_cnt[1]); }
+  }
 }
 
 // dense view of the sparse scenes' visual entries (operators / debugging): None everywhere, then the refined survivors
@@ -720,6 +761,21 @@ void launch_to_bf16(const float* src, int src_pitch, int d, int d8, long long ro
   note_launch();
 }
 
+// e4m3 operand copies: one warp per row (d8 <= 512)
+__global__ void to_fp8_kernel(const float* src, int src_pitch, int d, int d8, long long rows, unsigned char* dst, float* scale) {
+  const long long r = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  if (r >= rows) return;
+  const float s = fp8_row_from(src + r * src_pitch, d, d8, dst + r * fp8_pitch(d8));
+  if ((threadIdx.x & 31) == 0) scale[r] = s;
+}
+
+void launch_to_fp8(const float* src, int src_pitch, int d, int d8, long long rows, unsigned char* dst, float* scale,
+                   cudaStream_t st) {
+  if (rows == 0) return;
+  to_fp8_kernel<<<(unsigned)((rows * 32 + 255) / 256), 256, 0, st>>>(src, src_pitch, d, d8, rows, dst, scale);
+  note_launch();
+}
+
 // ------------------------------------------------------------------------------------------------ host launcher
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                   const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
@@ -735,22 +791,28 @@ static EncodeTiledFn get_encode() {
   return fn;
 }
 
-int make_map(CUtensorMap* m, const void* base, long long rows, int d8, int box_rows) {
+int make_map(CUtensorMap* m, const void* base, long long rows, int d8, int box_rows, bool fp8) {
   EncodeTiledFn enc = get_encode();
   if (!enc) return -1;
+  // a box row is one 128-byte swizzle row: 64 BF16 or 128 e4m3 features; past d8 the box is zero-filled
   cuuint64_t dims[2] = {(cuuint64_t)d8, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)d8 * 2};
-  cuuint32_t box[2] = {(cuuint32_t)TC_BK, (cuuint32_t)box_rows};
+  cuuint64_t strides[1] = {fp8 ? (cuuint64_t)fp8_pitch(d8) : (cuuint64_t)d8 * 2};
+  cuuint32_t box[2] = {(cuuint32_t)(fp8 ? 2 * TC_BK : TC_BK), (cuuint32_t)box_rows};
   cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (void*)base, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+  CUresult r = enc(m, fp8 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (void*)base, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                    CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   return r == CUDA_SUCCESS ? 0 : -2;
 }
 
+// the frame's screen runs on the e4m3 copies
+static bool screen_fp8(const Params& p, const TcArgs& tc) { return tc.fp8 && !tc.dense && p.d8 <= kFp8MaxD8; }
+
 // per-frame metadata: one thread per physical feature row (scene, arena block b, physical slot p) and per candidate.
 // A block without an owner (free list) is an invalid column; otherwise the row belongs to track n = blk_owner[b].
+// fp8: the constants of the e4m3 screen -- colb scaled by the row's 2^k (NaN, which keeps every pair, for a row outside
+// fp8_norm_ok), and the scale itself in colsb.
 __global__ void vis_meta_kernel(Params p, TrackStore ts, Frame f, int n_scenes, int max_rows, VisColMeta* colmeta,
-                                VisColGeo* colgeo, float* colb, unsigned int* colvalid) {
+                                VisColGeo* colgeo, float* colb, float* colsb, unsigned int* colvalid, bool fp8) {
   const int s = blockIdx.y;
   const SceneDesc sc = f.scenes[s];
   const int K = p.max_obs;
@@ -758,6 +820,7 @@ __global__ void vis_meta_kernel(Params p, TrackStore ts, Frame f, int n_scenes, 
   const bool in = prow < sc.nb * K && prow < max_rows;
   VisColMeta cm;
   cm.colb = 0.0f; cm.colc = 0.0f; cm.outcol = -1; cm.row = -1;
+  float csb = 1.0f;
   if (in) {
     const int b = prow / K, ph = prow - b * K;
     const size_t sbase = (size_t)sc.slot * ts.track_cap;
@@ -782,7 +845,12 @@ __global__ void vis_meta_kernel(Params p, TrackStore ts, Frame f, int n_scenes, 
         cm.outcol = n * K + k_of;
         const bool valid = (ts.feat_cnt[ti] >= p.min_track_length) && ((unsigned int)p.max_idle_epochs >= delta);
         const float nb = ts.fnorm2[frow];
-        cm.colb = p.visual_kind == 1 ? sqrtf(nb) : 0.5f * nb * (1.0f - 1e-5f - p.vis_rel_err);
+        const float E = fp8 ? p.vis_rel_err8 : p.vis_rel_err;
+        cm.colb = p.visual_kind == 1 ? sqrtf(nb) : 0.5f * nb * (1.0f - 1e-5f - E);
+        if (fp8) {
+          if (fp8_norm_ok(nb)) { csb = ts.fscale[frow]; cm.colb *= csb; }
+          else cm.colb = nanf("");
+        }
         cm.row = valid ? (int)frow : -1;
       } else {
         // dead physical slot -> owns the dead_rank-th logical column without a feature (written as None)
@@ -797,6 +865,7 @@ __global__ void vis_meta_kernel(Params p, TrackStore ts, Frame f, int n_scenes, 
     }
     colmeta[sc.col_off + prow] = cm;
     colb[sc.col_off + prow] = cm.colb;
+    if (fp8 && p.visual_kind != 1) colsb[sc.col_off + prow] = csb;
     if (p.n_constraints > 0) {
       VisColGeo cg;
       cg.tx = 0.0f; cg.ty = 0.0f; cg.tr = 0.0f; cg.tep = tep;
@@ -810,16 +879,26 @@ __global__ void vis_meta_kernel(Params p, TrackStore ts, Frame f, int n_scenes, 
   else if ((threadIdx.x & 31) == 0 && in) colvalid[(sc.col_off + prow) >> 5] = 0u;
 }
 
-__global__ void vis_rowmeta_kernel(Params p, Frame f, VisRowMeta* rowmeta) {
+// fp8: cosine rowk carries the row's 2^k, Euclidean rowi = 2^-k; NaN rowk (every pair kept) outside fp8_norm_ok
+__global__ void vis_rowmeta_kernel(Params p, Frame f, VisRowMeta* rowmeta, bool fp8) {
   int g = blockIdx.x * blockDim.x + threadIdx.x;
   if (g >= f.total) return;
   g += f.det0;
   const float na = f.c_norm2[g];
   VisRowMeta rm;
   rm.ok = (f.c_flags[g] & 2) ? 1 : 0;
+  rm.rowi = 1.0f;
+  rm.pad = 0;
   const float thr = p.visual_threshold;
-  if (p.visual_kind == 1) rm.rowk = (thr - 1e-5f - p.vis_rel_err) * sqrtf(na);
-  else rm.rowk = 0.5f * (na * (1.0f - 1e-5f - p.vis_rel_err) - thr * thr * (1.0f + 1e-5f));
+  const float E = fp8 ? p.vis_rel_err8 : p.vis_rel_err;
+  if (p.visual_kind == 1) rm.rowk = (thr - 1e-5f - E) * sqrtf(na);
+  else rm.rowk = 0.5f * (na * (1.0f - 1e-5f - E) - thr * thr * (1.0f + 1e-5f));
+  if (fp8) {
+    const float s = f.c_scale[g];
+    if (!fp8_norm_ok(na)) rm.rowk = nanf("");
+    else if (p.visual_kind == 1) rm.rowk *= s;
+    else rm.rowi = 1.0f / s;
+  }
   rowmeta[g] = rm;
 }
 
@@ -849,7 +928,8 @@ void launch_vis_colmeta(const Params& p, const TrackStore& ts, const Frame& f, i
   const int max_rows = tc.max_rows > 0 ? tc.max_rows : max_n * p.max_obs;
   if (tc.n_tiles == 0 || max_rows <= 0) return;
   dim3 grid((max_rows + 255) / 256, n_scenes);
-  vis_meta_kernel<<<grid, 256, 0, st>>>(p, ts, f, n_scenes, max_rows, tc.colmeta, tc.colgeo, tc.colb, tc.colvalid);
+  vis_meta_kernel<<<grid, 256, 0, st>>>(p, ts, f, n_scenes, max_rows, tc.colmeta, tc.colgeo, tc.colb, tc.colsb, tc.colvalid,
+                                        screen_fp8(p, tc));
   note_launch();
 }
 
@@ -883,19 +963,24 @@ int launch_vis_cost_tc(const Params& p, const TrackStore& ts, const Frame& f, in
   // d8 <= 512: the A-stationary kernel over work units of tc.cstep columns; wider features do not fit A in shared
   // memory, they take the streaming kernel over 256-column tiles
   const bool stationary = p.d8 <= kScreenStationaryMaxD8;
+  // e4m3 operands (TcArgs::fp8): the A-stationary kernel only; a missing copy is an error, not a quiet BF16 run
+  const bool fp8 = screen_fp8(p, tc);
+  if (fp8 && (!f.c_fp8 || !f.c_scale || !ts.feat_fp8 || !ts.fscale || (p.visual_kind != 1 && !tc.colsb))) return -3;
   CUtensorMap mA, mB;
-  if (make_map(&mA, f.c_bf16, tc.a_rows, p.d8, TC_BM) ||
-      make_map(&mB, ts.feat_bf16, tc.b_rows, p.d8, stationary ? SA_BN / 2 : TC_BN / 2))
+  if (make_map(&mA, fp8 ? (const void*)f.c_fp8 : f.c_bf16, tc.a_rows, p.d8, TC_BM, fp8) ||
+      make_map(&mB, fp8 ? (const void*)ts.feat_fp8 : ts.feat_bf16, tc.b_rows, p.d8, stationary ? SA_BN / 2 : TC_BN / 2, fp8))
     return -1;
   const size_t smem = (stationary ? sizeof(SaSmem) : sizeof(TcSmem)) + 1024;
   const bool cosine = p.visual_kind == 1;
   cudaError_t e = cudaSuccess;
-  const void* fn = stationary ? (cosine ? (const void*)vis_screen_sa_kernel<true> : (const void*)vis_screen_sa_kernel<false>)
-                              : (cosine ? (const void*)vis_screen_kernel<true> : (const void*)vis_screen_kernel<false>);
+  const void* fn;
+  if (!stationary) fn = cosine ? (const void*)vis_screen_kernel<true> : (const void*)vis_screen_kernel<false>;
+  else if (fp8) fn = cosine ? (const void*)vis_screen_sa_kernel<true, true> : (const void*)vis_screen_sa_kernel<false, true>;
+  else fn = cosine ? (const void*)vis_screen_sa_kernel<true, false> : (const void*)vis_screen_sa_kernel<false, false>;
   e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return (int)e;
   if (!tc.colmeta_done) launch_vis_colmeta(p, ts, f, n_scenes, max_n, tc, st);
-  vis_rowmeta_kernel<<<(f.total + 255) / 256, 256, 0, st>>>(p, f, tc.rowmeta);
+  vis_rowmeta_kernel<<<(f.total + 255) / 256, 256, 0, st>>>(p, f, tc.rowmeta, fp8);
   note_launch();
   if (tc.ev_screen0) cudaEventRecord(tc.ev_screen0, st);
   {
@@ -918,12 +1003,14 @@ int launch_vis_cost_tc(const Params& p, const TrackStore& ts, const Frame& f, in
     const VisColGeo* cgeo = tc.colgeo;
     const VisRowMeta* rmeta = tc.rowmeta;
     const float* cb = tc.colb;
+    const float* csb = tc.colsb;
     const unsigned int* cv = tc.colvalid;
     int ucols = tc.cstep;
     void* args[] = {(void*)&mA, (void*)&mB, (void*)&p, (void*)&ts, (void*)&f, (void*)&d_tiles, (void*)&n_tiles,
                     (void*)&d_n_tiles, (void*)&cmeta, (void*)&cgeo, (void*)&rmeta, (void*)&cb, (void*)&cv};
     void* args_sa[] = {(void*)&mA, (void*)&mB, (void*)&p, (void*)&ts, (void*)&f, (void*)&d_tiles, (void*)&n_tiles,
-                       (void*)&d_n_tiles, (void*)&ucols, (void*)&cmeta, (void*)&cgeo, (void*)&rmeta, (void*)&cb, (void*)&cv};
+                       (void*)&d_n_tiles, (void*)&ucols, (void*)&cmeta, (void*)&cgeo, (void*)&rmeta, (void*)&cb, (void*)&csb,
+                       (void*)&cv};
     e = cudaLaunchKernelExC(&cfg, fn, stationary ? args_sa : args);
     if (e != cudaSuccess) return (int)e;
     note_launch();

@@ -308,7 +308,7 @@ __global__ void __launch_bounds__(256) apply_kernel(Params p, TrackStore ts, Fra
 // epoch + max_idle < that epoch, and no block changes hands in between (blocks are freed on the host, after a drain, and
 // reused only by frames enqueued after it).  The two sets are disjoint.
 // T: element type of the request's feature column; a 2-byte row is widened to f32 where it is loaded, and the arena row,
-// its BF16 copy and the history row are written from the widened values.
+// its BF16 and e4m3 copies and the history row are written from the widened values.
 template <class T>
 __global__ void feat_store_kernel(Params p, TrackStore ts, Frame f) {
   int w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -405,6 +405,12 @@ __global__ void feat_store_kernel(Params p, TrackStore ts, Frame f) {
       }
       if (hd) hd[i] = x;
     }
+  }
+  if (dst >= 0 && ts.feat_fp8) {
+    // the e4m3 copy (d8 <= 512) from the f32 row this warp has just written
+    __syncwarp();
+    const float s = fp8_row_from(d, p.d8, p.d8, ts.feat_fp8 + (size_t)dst * fp8_pitch(p.d8));
+    if (lane == 0) ts.fscale[dst] = s;
   }
   if (lane == 0 && dst >= 0) ts.fnorm2[dst] = f.c_norm2[w];
 }

@@ -195,6 +195,7 @@ int sb200_visual_cost_matrix(int32_t visual_kind, float threshold, const float* 
   p.feature_dim = d;
   p.d8 = (d + 7) / 8 * 8;
   p.vis_rel_err = sb::screen_rel_err(d);
+  p.vis_rel_err8 = sb::screen_rel_err_fp8(d);
   p.max_obs = 1;
   p.min_track_length = 0;
   // track side: norms through the candidate-norm kernel on a scratch frame
@@ -247,14 +248,16 @@ int sb200_visual_cost_matrix(int32_t visual_kind, float threshold, const float* 
   sb::launch_prep(p, f, 1, m, sc.st);
   fill_u8_kernel<<<(m + 255) / 256, 256, 0, sc.st>>>(f.c_flags, 3, m);
   // same kernel selection rule as the tracker (engine.cu): tensor-core screen + exact refinement for large
-  // contractions with a selective threshold; SB200_VIS_KERNEL=simt|tc overrides
+  // contractions with a selective threshold; SB200_VIS_KERNEL=simt|tc|tc16|tc8 overrides.  The operator has no frames to
+  // learn the e4m3 screen's selectivity from: it screens on BF16 unless tc8 asks for e4m3 operands (d8 <= 512).
   sb::TcArgs tc;
   memset(&tc, 0, sizeof(tc));
   const bool selective = visual_kind == SB200_VIS_EUCLIDEAN ? (threshold < 1e18f) : (threshold > -1.0f);
   tc.use_tc = selective && p.d8 >= 64 && (long long)m * n * p.d8 >= (1ll << 28);
   if (const char* ev = getenv("SB200_VIS_KERNEL")) {
     if (!strcmp(ev, "simt")) tc.use_tc = false;
-    else if (!strcmp(ev, "tc")) tc.use_tc = true;
+    else if (!strcmp(ev, "tc") || !strcmp(ev, "tc16")) tc.use_tc = true;
+    else if (!strcmp(ev, "tc8")) { tc.use_tc = true; tc.fp8 = p.d8 <= sb::kFp8MaxD8; }
   }
   f.scene_max = sc.alloc<unsigned int>(1);
   cudaDeviceGetAttribute(&tc.num_sms, cudaDevAttrMultiProcessorCount, device);
@@ -283,18 +286,34 @@ int sb200_visual_cost_matrix(int32_t visual_kind, float threshold, const float* 
     tc.d_tiles = sc.upload(tiles.data(), tiles.size());
     tc.a_rows = m;
     tc.b_rows = n;
-    f.c_bf16 = sc.alloc<unsigned short>((size_t)m * p.d8);
-    ts.feat_bf16 = sc.alloc<unsigned short>((size_t)n * p.d8);
+    if (tc.fp8) {
+      const int p8 = sb::fp8_pitch(p.d8);
+      f.c_fp8 = sc.alloc<unsigned char>((size_t)m * p8);
+      f.c_scale = sc.alloc<float>(m);
+      ts.feat_fp8 = sc.alloc<unsigned char>((size_t)n * p8);
+      ts.fscale = sc.alloc<float>(n);
+      tc.colsb = sc.alloc<float>(n + 256);
+      if (!f.c_fp8 || !f.c_scale || !ts.feat_fp8 || !ts.fscale || !tc.colsb) return ops_fail(SB200_ERR_CUDA, "cudaMalloc failed");
+    } else {
+      f.c_bf16 = sc.alloc<unsigned short>((size_t)m * p.d8);
+      ts.feat_bf16 = sc.alloc<unsigned short>((size_t)n * p.d8);
+    }
     tc.colmeta = sc.alloc<sb::VisColMeta>(n + 256);   // the screen kernel bulk-copies whole 256-column slabs
     tc.colgeo = sc.alloc<sb::VisColGeo>(n);
     tc.colb = sc.alloc<float>(n + 256);
     tc.colvalid = sc.alloc<unsigned int>((n + 256) / 32 + 4);
     tc.rowmeta = sc.alloc<sb::VisRowMeta>(m + 256);
     tc.total_cols = n;
-    if (!tc.d_tiles || !f.c_bf16 || !ts.feat_bf16 || !tc.colmeta || !tc.colgeo || !tc.rowmeta || !tc.colb || !tc.colvalid)
+    if (!tc.d_tiles || (!tc.fp8 && (!f.c_bf16 || !ts.feat_bf16)) || !tc.colmeta || !tc.colgeo || !tc.rowmeta || !tc.colb || !tc.colvalid)
       return ops_fail(SB200_ERR_CUDA, "cudaMalloc failed");
-    sb::launch_to_bf16(static_cast<const float*>(ft.in_feat), d, d, p.d8, n, ts.feat_bf16, sc.st);
-    sb::launch_to_bf16(static_cast<const float*>(f.in_feat), d, d, p.d8, m, f.c_bf16, sc.st);   // (the tracker fuses this into cand_norm_kernel)
+    // (the tracker fuses these into cand_norm_kernel and feat_store_kernel)
+    if (tc.fp8) {
+      sb::launch_to_fp8(static_cast<const float*>(ft.in_feat), d, d, p.d8, n, ts.feat_fp8, ts.fscale, sc.st);
+      sb::launch_to_fp8(static_cast<const float*>(f.in_feat), d, d, p.d8, m, f.c_fp8, f.c_scale, sc.st);
+    } else {
+      sb::launch_to_bf16(static_cast<const float*>(ft.in_feat), d, d, p.d8, n, ts.feat_bf16, sc.st);
+      sb::launch_to_bf16(static_cast<const float*>(f.in_feat), d, d, p.d8, m, f.c_bf16, sc.st);
+    }
   }
   ts.fnorm2 = ft.c_norm2;
   int vr = sb::launch_vis_cost(p, ts, f, 1, m, n, tc, sc.st);

@@ -13,6 +13,7 @@
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
+#include <cuda_fp8.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -41,6 +42,90 @@ inline float screen_rel_err(int d) {
   return e <= (double)floor_e ? floor_e : (float)(e * (1.0 + 0x1p-20));   // rounded up past the f32 conversion
 }
 
+// The same bound for the e4m3 screen (FP8 operands, fp32 accumulation), relative to ||a|| ||b|| of the UNSCALED rows.  Each
+// row r is stored as x~ = e4m3(2^k_r x) with 2^k_r the power of two that puts max|x| in [224, 448) (fp8_row_scale): the
+// scaling is exact and saturation cannot occur, so only the e4m3 rounding and the accumulation add error.
+//   1. Operand rounding.  e4m3 keeps 4 significant bits: for a normal value |x~ - x| <= u |x|, u = 2^-4.  As above,
+//      sum |a~_i b~_i - a_i b_i| <= (2u + u^2) sum|a_i b_i| for the normal part.
+//   2. Subnormal floor.  Below 2^-6 the spacing is 2^-9, so |x~ - x| <= 2^-10 in scaled units.  Its share of the dot product
+//      is at most 2^-10 (1 + u) (sum|a_i| + sum|b_i|) + d 2^-20 <= 2^-10 (1 + u) sqrt(d) (||a|| + ||b||) + d 2^-20; both
+//      scaled norms are >= max|x| >= 224, so relative to ||a|| ||b|| it is <= 2 (1 + u) sqrt(d) 2^-10 / 224 + d 2^-20 / 224^2.
+//   3. Accumulation.  Products of e4m3 values are exact in fp32.  The FP8 tensor cores of the H100 are publicly reported to
+//      keep only about 14 bits when they add a k32 group of products to the accumulator.  Model (NOT measured here, wide
+//      margin): every k32 step aligns its 32 products and the accumulator to the largest of them and truncates each to
+//      13 significant bits, then rounds the sum.  Each of those 34 operations errs by less than 2^-12 of the step's largest
+//      term, which is at most sum|a~_i b~_i| <= (1 + u)^2 ||a|| ||b|| (plus the floor, covered by the 1.01 below), so
+//      ceil(d / 32) steps add at most ceil(d / 32) * 34 * 2^-12 * (1 + u)^2 * 1.01.
+// At d = 512 the sum is 0.129 + 0.0003 + 0.150 = 0.280: on unit-norm features the Euclidean screen keeps d <= 0.7 pairs
+// up to d~ = sqrt(0.49 + 2 E) ~ 1.04, the cosine screen keeps cos >= thr pairs down to cos~ = thr - 0.28.  Selective enough
+// for thresholds in the tail of the distance distribution; where it is not, the tracker goes back to the BF16 screen.
+inline float screen_rel_err_fp8(int d) {
+  const double u = 0x1p-4;
+  const double rnd = 2.0 * u + u * u;
+  const double sub = 2.0 * (1.0 + u) * __builtin_sqrt((double)d) * 0x1p-10 / 224.0 + (double)d * 0x1p-20 / (224.0 * 224.0);
+  const double acc = (double)((d + 31) / 32) * 34.0 * 0x1p-12 * (1.0 + u) * (1.0 + u) * 1.01;
+  return (float)((rnd + sub + acc) * (1.0 + 0x1p-20));   // rounded up past the f32 conversion
+}
+
+// Rows whose squared norm lies outside [2^-60, 2^60] (zero, tiny, huge, inf or NaN features) keep every pair in the e4m3
+// screen: the exact pass decides.  Inside that range max|x| lies in [2^-35, 2^30], the scale 2^k_r is a normal float and
+// the folded screen constants neither overflow nor lose bits to subnormals.
+__host__ __device__ __forceinline__ bool fp8_norm_ok(float n2) { return n2 >= 0x1p-60f && n2 <= 0x1p60f; }
+// 2^k with max|x| * 2^k in [224, 448), exact; 1 for a row without a usable maximum (such rows fail fp8_norm_ok)
+__host__ __device__ __forceinline__ float fp8_row_scale(float amax) {
+  if (!(amax >= 0x1p-100f && amax <= 0x1p100f)) return 1.0f;
+  int e = 0;
+  const float m = frexpf(amax, &e);   // amax = m 2^e, m in [0.5, 1)
+  return ldexpf(1.0f, (m >= 0.875f ? 8 : 9) - e);
+}
+// bytes per row of the e4m3 copies: d8 rounded up to 16 (the tensor maps need 16-byte row pitches)
+__host__ __device__ __forceinline__ int fp8_pitch(int d8) { return (d8 + 15) & ~15; }
+
+// 8 consecutive values of a row -> their e4m3 bytes of s x (cvt.rn.satfinite.e4m3x2.f32: round to nearest even)
+__device__ __forceinline__ uint2 fp8_pack8(const float* x, float s) {
+  unsigned int w[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const unsigned int lo = __nv_cvt_float2_to_fp8x2(make_float2(x[4 * h] * s, x[4 * h + 1] * s), __NV_SATFINITE, __NV_E4M3);
+    const unsigned int hi = __nv_cvt_float2_to_fp8x2(make_float2(x[4 * h + 2] * s, x[4 * h + 3] * s), __NV_SATFINITE, __NV_E4M3);
+    w[h] = lo | (hi << 16);
+  }
+  return make_uint2(w[0], w[1]);
+}
+// One warp, a row of d8 <= 512 values held as blocks lane and lane + 32 (x[h], zero past the row): writes the e4m3 copy
+// to out (fp8_pitch(d8) bytes) and returns the row's scale.  NaN elements do not enter the maximum; such rows fail
+// fp8_norm_ok and keep every pair.
+__device__ __forceinline__ float fp8_row_store(const float (&x)[2][8], int d8, unsigned char* out) {
+  const int lane = threadIdx.x & 31;
+  float amax = 0.0f;
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int l = 0; l < 8; ++l) amax = fmaxf(amax, fabsf(x[h][l]));
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+  const float s = fp8_row_scale(amax);
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int blk = h * 32 + lane;
+    if (blk * 8 < d8) *reinterpret_cast<uint2*>(out + blk * 8) = fp8_pack8(x[h], s);
+  }
+  return s;
+}
+// the same from a f32 row in memory (d values, zero padded to d8)
+__device__ __forceinline__ float fp8_row_from(const float* src, int d, int d8, unsigned char* out) {
+  const int lane = threadIdx.x & 31;
+  float x[2][8];
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int l = 0; l < 8; ++l) {
+      const int c = (h * 32 + lane) * 8 + l;
+      x[h][l] = c < d ? src[c] : 0.0f;
+    }
+  return fp8_row_store(x, d8, out);
+}
+
 struct Params {  // immutable per tracker, passed by value to kernels
   int kind, positional_kind, visual_kind;
   float iou_threshold, min_confidence, pos_weight, vel_weight;
@@ -50,6 +135,7 @@ struct Params {  // immutable per tracker, passed by value to kernels
   float constraint_max_dist[kMaxConstraints];
   float visual_threshold;
   float vis_rel_err;  // screen_rel_err(feature_dim): the BF16 slack of the tensor-core visual kernels
+  float vis_rel_err8; // screen_rel_err_fp8(feature_dim): the slack of the e4m3 screen
   int feature_dim, d8, max_obs, min_votes, min_track_length;
   int vote_vis_cap;   // visual entries per scene the sparse voting kernel keeps in shared memory (0: kVoteVisCap)
   float min_area, min_quality_use, min_quality_collect, min_own_use, min_own_collect;
@@ -126,6 +212,8 @@ struct TrackStore {
   // visual
   float* feat;           // [idx][K][d8]
   void* feat_bf16;       // [idx][K][d8] bf16 copy of feat: B operand of the tensor-core screen
+  unsigned char* feat_fp8;  // [idx][K][fp8_pitch(d8)] e4m3 copy of 2^k feat (d8 <= 512 only, else null): B operand of the e4m3 screen
+  float* fscale;            // [idx][K] the row's 2^k (fp8_row_scale)
   float* fnorm2;         // [idx][K] by physical slot
   unsigned char* obs_phys;  // [idx][K] logical -> physical
   unsigned char* obs_hasf;  // [idx][K] logical: feature present
@@ -220,6 +308,10 @@ struct Frame {  // per-request transient device buffers (a request may be proces
   unsigned char* c_flags;  // bit0 has feature, bit1 feature usable (feature_can_be_used with *_use thresholds)
   float* c_norm2;
   void* c_bf16;            // [total][d8] bf16 copy of the candidate features (A operand of the screen)
+  unsigned char* c_fp8;    // [total][fp8_pitch(d8)] e4m3 copy of 2^k x (A operand of the e4m3 screen), or null
+  float* c_scale;          // [total] the row's 2^k
+  int* screen_cnt;         // [3] survivors refined, how many of them the exact test cut, scenes whose survivor list
+                           // overflowed (null: not counted)
   unsigned int* scene_max; // [n_scenes] order-preserving encoding of best.rs "max_dist"
   int* winner;             // [total] track index within the scene or -1
   unsigned char* c_vt;     // voting type of the decision
@@ -276,7 +368,8 @@ struct VisColMeta {
   int row;       // feature row idx*K + phys when the observation takes part in the metric, else -1
 };
 struct VisColGeo { float tx, ty, tr; unsigned int tep; };  // only read when spatio-temporal constraints exist
-struct VisRowMeta { float rowk; int ok, pad0, pad1; };   // row constant of the screen test, candidate may vote visually
+// row constant of the screen test, candidate may vote visually, e4m3 Euclidean screen: 2^-k of the candidate row
+struct VisRowMeta { float rowk; int ok; float rowi; int pad; };
 struct DenseTrackMeta { int n; int kt; float cmax; int pad; };   // arena block: owner (store index, -1: none), valid observations
 
 // ---- kernel launchers (each in its own .cu) ----
@@ -318,6 +411,8 @@ struct TcArgs {
   float* colb;                // [sum n_s*K (+pad)] column constant of the screen test
   unsigned int* colvalid;     // bit per column: the observation takes part in the metric
   VisRowMeta* rowmeta;   // [total]
+  bool fp8;              // the A-stationary screen runs on the e4m3 copies (d8 <= 512)
+  float* colsb;          // [like colb] e4m3 Euclidean screen: the column's 2^k
   int total_cols;
   int max_rows;          // max over the scenes of nb * K
   // ---- dense weight-sum path (mode 2)
@@ -386,6 +481,11 @@ int launch_vis_cost_tc(const Params& p, const TrackStore& ts, const Frame& f, in
 // materialises the dense visual matrix of the sparse scenes (operators / debugging only)
 void launch_vis_densify(const Params& p, const Frame& f, int n_scenes, cudaStream_t st);
 void launch_to_bf16(const float* src, int src_pitch, int d, int d8, long long rows, void* dst, cudaStream_t st);
+// e4m3 copies of f32 rows (d8 <= 512): dst[r][fp8_pitch(d8)] = e4m3(2^k_r src[r]), scale[r] = 2^k_r; one warp per row
+void launch_to_fp8(const float* src, int src_pitch, int d, int d8, long long rows, unsigned char* dst, float* scale,
+                   cudaStream_t st);
+// largest d8 the e4m3 (A-stationary) screen takes
+constexpr int kFp8MaxD8 = 512;
 // scene_max init (all scenes) and, unless init_only, the dense reduction for the scenes whose mode has bit1 set
 void launch_scene_max(const Params& p, const Frame& f, int n_scenes, bool init_only, cudaStream_t st);
 // per-scene voting mode from the list counters (runs after the cost kernels); launch_vis_mode: the visual half of it

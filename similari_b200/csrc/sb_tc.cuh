@@ -16,9 +16,10 @@ constexpr int TC_B_BYTES = TC_BN * TC_BK * 2;  // 32 KB
 constexpr int TC_WG_ROWS = 64;                 // accumulator rows of one consumer warpgroup
 constexpr int TC_THREADS = 384;                // producer warpgroup (one TMA warp) + two consumer warpgroups
 
-// Host: tensor map of a row-major [rows][d8] BF16 matrix, boxes of TC_BK features x box_rows rows, 128-byte swizzle.
+// Host: tensor map of a row-major [rows][d8] BF16 matrix, boxes of TC_BK features x box_rows rows, 128-byte swizzle; fp8:
+// of a [rows][fp8_pitch(d8)] byte matrix (the e4m3 copies), boxes of 128 features.
 // 0 on success, -1 without the driver's encoder, -2 when it refuses the map (kernels_feat_tc.cu).
-int make_map(CUtensorMap* m, const void* base, long long rows, int d8, int box_rows);
+int make_map(CUtensorMap* m, const void* base, long long rows, int d8, int box_rows, bool fp8 = false);
 
 // ------------------------------------------------------------------------------------------------ PTX helpers
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -124,6 +125,24 @@ __device__ __forceinline__ void wgmma_bf16_m64n128(float* d, uint64_t adesc, uin
       "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
       "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63 "
       "}, %64, %65, p, 1, 1, 0, 0;\n\t"
+      "}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(accum));
+}
+// D[64 x 128] (+)= A[64 x 32] * B[128 x 32]^T with e4m3 operands (32 bytes of each row, as a k16 step of BF16), fp32
+// accumulators in the layout of wgmma_bf16_m64n128.
+__device__ __forceinline__ void wgmma_e4m3_m64n128(float* d, uint64_t adesc, uint64_t bdesc, uint32_t accum) {
+  asm volatile(
+      "{\n\t"
+      ".reg .pred p;\n\t"
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k32.f32.e4m3.e4m3 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63 "
+      "}, %64, %65, p, 1, 1;\n\t"
       "}"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
         "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),

@@ -154,6 +154,13 @@ class Tracker:
                 "stage_ms": dict(zip(("prep", "positional_cost", "visual_cost", "voting", "apply"), map(float, ms[:5]))),
                 "vis_screen_ms": float(ms[5]), "vis_refine_ms": float(ms[6]), "tc_frames": int(ms[7])}
 
+    def screen_counters(self):
+        """sb200_screen_counters: frames screened on e4m3 and on BF16 operands, survivors of those screens that were
+        refined, and survivors the exact test cut (cumulative; waits for the frames in flight)."""
+        c = np.zeros(4, np.uint64)
+        check(self._L.sb200_screen_counters(self._h, ptr(c)))
+        return {"fp8_frames": int(c[0]), "bf16_frames": int(c[1]), "survivors": int(c[2]), "cut": int(c[3])}
+
     def host_counters(self):
         """sb200_host_counters: calls of the predict entry points, wall ms inside them, ms of that blocked on the device."""
         o = np.zeros(3, np.float64)
