@@ -12,7 +12,9 @@
 #include <cstring>
 #include <map>
 #include <string>
+#include <type_traits>
 #include <unordered_map>
+#include <utility>
 #include <vector>
 
 #include "../../include/similari_b200.h"
@@ -47,10 +49,19 @@ int fail(int code, const char* fmt, ...) {
       return fail(SB200_ERR_CUDA, "%s failed: %s (%s:%d)", #x, cudaGetErrorString(e_), __FILE__, __LINE__); \
   } while (0)
 
-// grow-only device buffer
+// grow-only device buffer; it owns its memory (move-only, freed by the destructor)
 struct DBuf {
   void* p = nullptr;
   size_t bytes = 0;
+  DBuf() = default;
+  DBuf(const DBuf&) = delete;
+  DBuf& operator=(const DBuf&) = delete;
+  DBuf(DBuf&& o) noexcept : p(o.p), bytes(o.bytes) { o.p = nullptr; o.bytes = 0; }
+  DBuf& operator=(DBuf&& o) noexcept {
+    if (this != &o) { release(); p = o.p; bytes = o.bytes; o.p = nullptr; o.bytes = 0; }
+    return *this;
+  }
+  ~DBuf() { release(); }
   int ensure(size_t need) {
     if (need <= bytes) return 0;
     size_t nb = std::max(need, bytes + bytes / 2);
@@ -70,23 +81,31 @@ struct DBuf {
   template <typename T> T* as() const { return reinterpret_cast<T*>(p); }
 };
 
-struct HBuf {  // grow-only pinned host buffer, mapped into the device address space (dp)
+struct HBuf {  // grow-only pinned host buffer, mapped into the device address space (dp); owns its memory like DBuf
   void* p = nullptr;
   void* dp = nullptr;   // device-side alias: kernels can read the buffer over PCIe without a copy-engine transfer
   size_t bytes = 0;
+  HBuf() = default;
+  HBuf(const HBuf&) = delete;
+  HBuf& operator=(const HBuf&) = delete;
+  HBuf(HBuf&& o) noexcept : p(o.p), dp(o.dp), bytes(o.bytes) { o.p = o.dp = nullptr; o.bytes = 0; }
+  HBuf& operator=(HBuf&& o) noexcept {
+    if (this != &o) { release(); p = o.p; dp = o.dp; bytes = o.bytes; o.p = o.dp = nullptr; o.bytes = 0; }
+    return *this;
+  }
+  ~HBuf() { release(); }
   int ensure(size_t need) {
     if (need <= bytes) return 0;
-    size_t nb = std::max(need, bytes + bytes / 2);
+    HBuf nb;   // freed on failure
+    const size_t n = std::max(need, bytes + bytes / 2);
     void* np = nullptr;
-    cudaError_t e = cudaHostAlloc(&np, nb, cudaHostAllocMapped);
-    if (e != cudaSuccess) return fail(SB200_ERR_CUDA, "cudaHostAlloc(%zu) failed: %s", nb, cudaGetErrorString(e));
-    void* ndp = nullptr;
-    e = cudaHostGetDevicePointer(&ndp, np, 0);
-    if (e != cudaSuccess) { cudaFreeHost(np); return fail(SB200_ERR_CUDA, "cudaHostGetDevicePointer failed: %s", cudaGetErrorString(e)); }
-    if (p) cudaFreeHost(p);
-    p = np;
-    dp = ndp;
-    bytes = nb;
+    cudaError_t e = cudaHostAlloc(&np, n, cudaHostAllocMapped);
+    if (e != cudaSuccess) return fail(SB200_ERR_CUDA, "cudaHostAlloc(%zu) failed: %s", n, cudaGetErrorString(e));
+    nb.p = np;
+    e = cudaHostGetDevicePointer(&nb.dp, nb.p, 0);
+    if (e != cudaSuccess) return fail(SB200_ERR_CUDA, "cudaHostGetDevicePointer failed: %s", cudaGetErrorString(e));
+    nb.bytes = n;
+    *this = std::move(nb);
     return 0;
   }
   void release() {
@@ -96,6 +115,25 @@ struct HBuf {  // grow-only pinned host buffer, mapped into the device address s
     bytes = 0;
   }
   template <typename T> T* as() const { return reinterpret_cast<T*>(p); }
+};
+
+// A column of the tracker's device state (sb200_tracker::store_table, slot_table, wasted_table, pool_table): the buffer
+// that owns it, the TrackStore / WastedBuf pointer the kernels read it through, and its row width.  `rows` says what a
+// row counts, and so how many rows a state-blob section of the column holds: live tracks, arena blocks or free-list
+// entries of each listed scene; the records of the wasted buffer; the history blocks handed out or the pool's free stack;
+// or, in a scene blob, the history rows of the live tracks.
+enum ColRows { kRowTrack, kRowBlock, kRowFree, kRowWasted, kRowHistTop, kRowHistFree, kRowTrackHist };
+enum ColBlob { kBlobNo, kBlobAll, kBlobTrackerOnly };
+// index-valued columns that a load checks against the blob's counts (kTagHblk: a history block, below the pool's top)
+enum ColTag { kTagNone, kTagFblk, kTagHblk, kTagObsN, kTagObsPhys, kTagOwner, kTagFree };
+struct Col {
+  DBuf* buf;
+  void (*point)(sb200_tracker&, void*);   // sets the column's pointer in the TrackStore / WastedBuf (null: there is none)
+  size_t w;                                // bytes per row
+  bool zero = false;   // growth zero-fills the column: rows moved whole although only partly written (history rings)
+  int rows = kRowTrack;
+  int blob = kBlobAll;   // which state blobs carry the column
+  int tag = kTagNone;
 };
 
 int make_params(const sb200_options& o, sb::Params* out) {
@@ -270,8 +308,7 @@ struct sb200_tracker {
     bool read_pending = false;
   } stg[2];
   int stg_last = 1;   // staging set used by the most recent predict
-  DBuf f_cbox2[2], f_cradius2[2], f_cconf2[2], f_cvert2[2], f_cflags2[2], f_cnorm22[2], f_cbf162[2], f_decided2[2];   // candidate side, two sets
-  DBuf f_cfp82[2], f_cscale2[2];
+  struct CandBufs { DBuf box, radius, conf, vert, flags, norm2, bf16, decided, fp8, scale; } cand[2];   // candidate side, two sets
   DBuf f_winner, f_cvt, f_pos, f_vis, f_scenes, f_newcount,
       f_status, f_featdst, f_apprank, f_appmeta, f_frameout, f_excl, f_prewin, f_own, f_ownovf, f_dyn, f_ws, f_tmeta, f_rowinfo, f_slabc, f_slabm, f_slabmask,
       f_dscene, f_maxc, f_maxcval, f_drowb, f_dcolb, f_slabk, f_scene_max, f_tiles, f_pairs, f_colmeta, f_colgeo, f_colb, f_colvalid, f_rowmeta, f_poslist, f_counters, f_visval, f_colsb;
@@ -289,29 +326,14 @@ struct sb200_tracker {
   bool transferred = false;     // built by sb200_tracker_load or filled by sb200_scenes_import: holds state without a frame
   int last_n_scenes = 0;   // scenes of the last frame (sb200_last_costs reads its scene table back from the device)
 
+  // The buffers free themselves after this body, so every stream the tracker owns is drained first (a caller's stream,
+  // which the tracker only joins, is not).
   ~sb200_tracker() {
     cudaSetDevice(device);
-    DBuf* all[] = {&b_id, &b_epoch, &b_length, &b_custom, &b_vt, &b_pred, &b_obs, &b_radius, &b_kst, &b_vert, &b_hpred, &b_hobs, &w_hpred, &w_hobs, &b_feat,
-                   &b_feat_bf16, &f_scene_max, &f_tiles, &f_pairs, &f_colmeta, &f_colgeo, &f_colb, &f_colvalid, &f_rowmeta, &f_poslist, &f_counters, &f_visval, &b_fnorm2, &b_obs_phys, &b_obs_hasf, &b_obs_q, &b_obs_n, &b_feat_cnt, &b_ntracks, &b_cur_epoch,
-                   &b_fblk, &b_blk_owner, &b_blk_free, &b_nfree, &b_atop, &f_frameout, &f_excl, &f_prewin, &f_own, &f_ownovf, &f_dyn, &b_idc, &f_ws, &f_tmeta, &f_rowinfo, &f_slabc, &f_slabm, &f_slabmask, &f_dscene, &f_maxc, &f_maxcval, &f_drowb, &f_dcolb, &f_slabk,
-                   &b_scene_ids, &w_count, &w_id, &w_scene, &w_epoch, &w_length, &w_pred, &w_obs, &f_winner, &f_cvt, &f_pos, &f_vis, &f_scenes, &f_newcount, &f_status,
-                   &f_featdst, &f_apprank, &f_appmeta, &o_ids, &o_epochs, &o_lengths, &o_vt, &o_pred, &o_obs,
-                   &b_hblk, &b_hrows, &b_hpresent, &b_hfree, &b_hpool, &w_hblk, &f_histdst, &b_feat_fp8, &b_fscale, &f_colsb};
-    for (DBuf* b : all) b->release();
-    for (int k = 0; k < 2; ++k) {
-      f_cbox2[k].release(); f_cradius2[k].release(); f_cconf2[k].release(); f_cvert2[k].release(); f_cflags2[k].release();
-      f_cnorm22[k].release(); f_cbf162[k].release(); f_decided2[k].release(); f_cfp82[k].release(); f_cscale2[k].release();
-    }
-    if (stream) cudaStreamSynchronize(stream);
-    h_small.release();
-    for (auto& g : stg) {
-      g.boxes.release(); g.feat.release(); g.hasf.release(); g.quality.release(); g.custom.release(); g.own.release();
-      if (g.ev) cudaEventDestroy(g.ev);
-      if (g.ev0) cudaEventDestroy(g.ev0);
-      if (g.ev_read) cudaEventDestroy(g.ev_read);
-    }
+    for (cudaStream_t s : {stream, prep_stream, side_stream, copy_stream}) if (s) cudaStreamSynchronize(s);
+    for (auto& g : stg)
+      for (cudaEvent_t e : {g.ev, g.ev0, g.ev_read}) if (e) cudaEventDestroy(e);
     for (auto& q : pend) {
-      q.h_req.release(); q.h_out.release();
       if (q.done) cudaEventDestroy(q.done);
       for (auto& e : q.ev) if (e) cudaEventDestroy(e);
       for (auto& e : q.ev_k) if (e) cudaEventDestroy(e);
@@ -326,27 +348,106 @@ struct sb200_tracker {
     if (own_stream && stream) cudaStreamDestroy(stream);
   }
 
-  // (re)allocates the track store for scene_cap x track_cap rows, preserving the live rows
-  template <typename T>
-  int regrow(DBuf& b, T** field, int width, int new_scenes, int new_tracks, bool zero = false) {
-    size_t row = (size_t)width * sizeof(T);
-    DBuf nb;
-    int rc = nb.ensure(std::max<size_t>(1, (size_t)new_scenes * new_tracks * row));
-    if (rc) return rc;
-    // rows that are moved whole although only partly written (the history rings of short tracks) start out defined
-    if (zero && cudaMemsetAsync(nb.p, 0, std::max<size_t>(1, (size_t)new_scenes * new_tracks * row), stream) != cudaSuccess)
-      return fail(SB200_ERR_CUDA, "store regrow memset failed");
-    if (b.p && scene_cap > 0 && track_cap > 0) {
-      cudaError_t e = cudaMemcpy2DAsync(nb.p, (size_t)new_tracks * row, b.p, (size_t)track_cap * row,
-                                        (size_t)std::min(track_cap, new_tracks) * row, (size_t)scene_cap,
-                                        cudaMemcpyDeviceToDevice, stream);
-      if (e != cudaSuccess) return fail(SB200_ERR_CUDA, "store regrow copy failed: %s", cudaGetErrorString(e));
-      e = cudaStreamSynchronize(stream);
-      if (e != cudaSuccess) return fail(SB200_ERR_CUDA, "store regrow sync failed: %s", cudaGetErrorString(e));
+  template <auto F> static void in_ts(sb200_tracker& t, void* p) { t.ts.*F = static_cast<std::remove_reference_t<decltype(t.ts.*F)>>(p); }
+  template <auto F> static void in_wb(sb200_tracker& t, void* p) { t.wb.*F = static_cast<std::remove_reference_t<decltype(t.wb.*F)>>(p); }
+
+  // The device track store: scene_cap x track_cap rows per column, in blob order.
+  std::vector<Col> store_table() {
+    using TS = sb::TrackStore;
+    const size_t K = (size_t)P.max_obs, d8 = (size_t)P.d8, H = (size_t)hist_len;
+    std::vector<Col> c = {{&b_id, in_ts<&TS::id>, 8}, {&b_epoch, in_ts<&TS::epoch>, 4}, {&b_length, in_ts<&TS::length>, 4},
+                          {&b_custom, in_ts<&TS::custom>, 8}, {&b_vt, in_ts<&TS::vt>, 1}, {&b_pred, in_ts<&TS::pred>, 24},
+                          {&b_obs, in_ts<&TS::obs>, 24}, {&b_radius, in_ts<&TS::radius>, 4},
+                          {&b_kst, in_ts<&TS::kst>, 4 * (size_t)sb::kStateStride}};
+    if (P.positional_kind == SB200_POS_IOU) c.push_back({&b_vert, in_ts<&TS::vert>, 64});
+    if (H > 1) {
+      c.push_back({&b_hpred, in_ts<&TS::hist_pred>, 24 * H, true});
+      c.push_back({&b_hobs, in_ts<&TS::hist_obs>, 24 * H, true});
     }
-    b.release();
-    b = nb;
-    *field = b.as<T>();
+    if (P.is_visual) {
+      c.push_back({&b_obs_phys, in_ts<&TS::obs_phys>, K, false, kRowTrack, kBlobAll, kTagObsPhys});
+      c.push_back({&b_obs_hasf, in_ts<&TS::obs_hasf>, K});
+      c.push_back({&b_obs_q, in_ts<&TS::obs_q>, 4 * K});
+      c.push_back({&b_obs_n, in_ts<&TS::obs_n>, 1, false, kRowTrack, kBlobAll, kTagObsN});
+      c.push_back({&b_feat_cnt, in_ts<&TS::feat_cnt>, 1});
+      c.push_back({&b_fblk, in_ts<&TS::fblk>, 4, false, kRowTrack, kBlobAll, kTagFblk});
+      // the history pool is not indexed by slot: only the tracks' block indices move with the store.  A scene blob carries
+      // the history rows themselves (renumbered on import), a tracker blob the pool and the indices.
+      if (fhist_on) c.push_back({&b_hblk, in_ts<&TS::hblk>, 4, false, kRowTrack, kBlobTrackerOnly, kTagHblk});
+      c.push_back({&b_feat, in_ts<&TS::feat>, 4 * K * d8, false, kRowBlock});
+      c.push_back({&b_feat_bf16, in_ts<&TS::feat_bf16>, 2 * K * d8, false, kRowBlock});
+      c.push_back({&b_fnorm2, in_ts<&TS::fnorm2>, 4 * K, false, kRowBlock});
+      // the e4m3 copies: only the A-stationary screen (d8 <= 512) reads them.  Not in the blob: a load converts the f32
+      // rows again (regen_fp8).
+      if (P.d8 <= sb::kFp8MaxD8) {
+        c.push_back({&b_feat_fp8, in_ts<&TS::feat_fp8>, K * sb::fp8_pitch(P.d8), false, kRowBlock, kBlobNo});
+        c.push_back({&b_fscale, in_ts<&TS::fscale>, 4 * K, false, kRowBlock, kBlobNo});
+      }
+      c.push_back({&b_blk_owner, in_ts<&TS::blk_owner>, 4, false, kRowBlock, kBlobAll, kTagOwner});
+      c.push_back({&b_blk_free, in_ts<&TS::blk_free>, 4, false, kRowFree, kBlobAll, kTagFree});
+    }
+    return c;
+  }
+
+  // per-slot arrays (scene_cap rows; not in the blob): live tracks, the epochs and scene ids run_waste uploads, free
+  // blocks, arena top
+  std::vector<Col> slot_table() {
+    using TS = sb::TrackStore;
+    return {{&b_ntracks, nullptr, 4, true}, {&b_cur_epoch, nullptr, 4, true}, {&b_scene_ids, nullptr, 8, true},
+            {&b_nfree, in_ts<&TS::n_free>, 4, true}, {&b_atop, in_ts<&TS::arena_top>, 4, true}};
+  }
+
+  // the wasted-track buffer: one row per record, in blob order
+  std::vector<Col> wasted_table() {
+    using WB = sb::WastedBuf;
+    const size_t H = (size_t)hist_len;
+    std::vector<Col> c = {{&w_id, in_wb<&WB::id>, 8, false, kRowWasted}, {&w_scene, in_wb<&WB::scene>, 8, false, kRowWasted},
+                          {&w_epoch, in_wb<&WB::epoch>, 4, false, kRowWasted}, {&w_length, in_wb<&WB::length>, 4, false, kRowWasted},
+                          {&w_pred, in_wb<&WB::pred>, 24, false, kRowWasted}, {&w_obs, in_wb<&WB::obs>, 24, false, kRowWasted}};
+    if (H > 1) {
+      c.push_back({&w_hpred, in_wb<&WB::hist_pred>, 24 * H, false, kRowWasted});
+      c.push_back({&w_hobs, in_wb<&WB::hist_obs>, 24 * H, false, kRowWasted});
+    }
+    if (fhist_on) c.push_back({&w_hblk, in_wb<&WB::hblk>, 4, false, kRowWasted, kBlobAll, kTagHblk});
+    return c;
+  }
+
+  // the feature-history pool (only with the feature history on): one row per block, in blob order
+  std::vector<Col> pool_table() {
+    using TS = sb::TrackStore;
+    const size_t H = (size_t)hist_len;
+    return {{&b_hrows, in_ts<&TS::hrows>, H * (size_t)P.d8 * 4, false, kRowHistTop},
+            {&b_hpresent, in_ts<&TS::hpresent>, H, true, kRowHistTop},
+            {&b_hfree, in_ts<&TS::hfree>, 4, false, kRowHistFree, kBlobAll, kTagHblk}};
+  }
+
+  // Re-creates column `b` with `groups` x `rows` rows of `w` bytes, keeping the first `old_rows` rows of each of the first
+  // `old_groups` groups (old pitch: `old_rows` rows).  Allocate, zero-fill if asked, copy, synchronise, free the old one.
+  int regrow(DBuf& b, size_t w, size_t groups, size_t rows, size_t old_groups, size_t old_rows, bool zero) {
+    const size_t bytes = std::max<size_t>(1, groups * rows * w);
+    DBuf nb;
+    int rc = nb.ensure(bytes);
+    if (rc) return rc;
+    if (zero) CU(cudaMemsetAsync(nb.p, 0, bytes, stream));
+    if (b.p && old_groups > 0 && old_rows > 0) {
+      if (old_groups == 1)   // one contiguous run: a plain copy, which has no pitch limit
+        CU(cudaMemcpyAsync(nb.p, b.p, old_rows * w, cudaMemcpyDeviceToDevice, stream));
+      else
+        CU(cudaMemcpy2DAsync(nb.p, rows * w, b.p, old_rows * w, old_rows * w, old_groups, cudaMemcpyDeviceToDevice, stream));
+      CU(cudaStreamSynchronize(stream));
+    }
+    b = std::move(nb);
+    return 0;
+  }
+
+  // Grows every column of `cols` (see regrow) and re-points it.  One column at a time: memory peaks at the old columns
+  // plus one, where allocating all first would hold two whole stores at once.
+  int grow(const std::vector<Col>& cols, size_t groups, size_t rows, size_t old_groups, size_t old_rows) {
+    for (const Col& c : cols) {
+      const int rc = regrow(*c.buf, c.w, groups, rows, old_groups, old_rows, c.zero);
+      if (rc) return rc;
+      if (c.point) c.point(*this, c.buf->p);
+    }
     return 0;
   }
 
@@ -359,75 +460,17 @@ struct sb200_tracker {
     return cudaGetLastError() == cudaSuccess ? 0 : fail(SB200_ERR_CUDA, "e4m3 row conversion failed");
   }
 
+  // (re)allocates the track store for scene_cap x track_cap rows, preserving the live rows
   int ensure_store(int need_scenes, int need_tracks) {
     if (need_scenes <= scene_cap && need_tracks <= track_cap) return 0;
     int ns = scene_cap, nt = track_cap;
     if (need_scenes > ns) ns = std::max(need_scenes, std::max(4, ns * 2));
     if (need_tracks > nt) nt = std::max(need_tracks, std::max(64, nt * 2));
-    const int K = P.max_obs;
-    int rc = 0;
-    if ((rc = regrow(b_id, &ts.id, 1, ns, nt))) return rc;
-    if ((rc = regrow(b_epoch, &ts.epoch, 1, ns, nt))) return rc;
-    if ((rc = regrow(b_length, &ts.length, 1, ns, nt))) return rc;
-    if ((rc = regrow(b_custom, &ts.custom, 1, ns, nt))) return rc;
-    if ((rc = regrow(b_vt, &ts.vt, 1, ns, nt))) return rc;
-    if ((rc = regrow(b_pred, &ts.pred, 6, ns, nt))) return rc;
-    if ((rc = regrow(b_obs, &ts.obs, 6, ns, nt))) return rc;
-    if ((rc = regrow(b_radius, &ts.radius, 1, ns, nt))) return rc;
-    if ((rc = regrow(b_kst, &ts.kst, sb::kStateStride, ns, nt))) return rc;
+    int rc = grow(store_table(), ns, nt, scene_cap, track_cap);
+    if (rc) return rc;
+    if (ns != scene_cap && (rc = grow(slot_table(), ns, 1, scene_cap, 1))) return rc;
     ts.kst_stride = sb::kStateStride;
-    if (P.positional_kind == SB200_POS_IOU)
-      if ((rc = regrow(b_vert, &ts.vert, 8, ns, nt))) return rc;
-    if (hist_len > 1) {
-      if ((rc = regrow(b_hpred, &ts.hist_pred, 6 * hist_len, ns, nt, true))) return rc;
-      if ((rc = regrow(b_hobs, &ts.hist_obs, 6 * hist_len, ns, nt, true))) return rc;
-      ts.hist_len = hist_len;
-    }
-    if (P.is_visual) {
-      if ((rc = regrow(b_feat, &ts.feat, K * P.d8, ns, nt))) return rc;
-      {
-        unsigned short* tmp = reinterpret_cast<unsigned short*>(ts.feat_bf16);
-        if ((rc = regrow(b_feat_bf16, &tmp, K * P.d8, ns, nt))) return rc;
-        ts.feat_bf16 = tmp;
-      }
-      if ((rc = regrow(b_fnorm2, &ts.fnorm2, K, ns, nt))) return rc;
-      if (P.d8 <= sb::kFp8MaxD8) {   // the e4m3 copies: only the A-stationary screen (d8 <= 512) reads them
-        if ((rc = regrow(b_feat_fp8, &ts.feat_fp8, K * sb::fp8_pitch(P.d8), ns, nt))) return rc;
-        if ((rc = regrow(b_fscale, &ts.fscale, K, ns, nt))) return rc;
-      }
-      if ((rc = regrow(b_obs_phys, &ts.obs_phys, K, ns, nt))) return rc;
-      if ((rc = regrow(b_obs_hasf, &ts.obs_hasf, K, ns, nt))) return rc;
-      if ((rc = regrow(b_obs_q, &ts.obs_q, K, ns, nt))) return rc;
-      if ((rc = regrow(b_obs_n, &ts.obs_n, 1, ns, nt))) return rc;
-      if ((rc = regrow(b_feat_cnt, &ts.feat_cnt, 1, ns, nt))) return rc;
-      if ((rc = regrow(b_fblk, &ts.fblk, 1, ns, nt))) return rc;
-      if ((rc = regrow(b_blk_owner, &ts.blk_owner, 1, ns, nt))) return rc;
-      if ((rc = regrow(b_blk_free, &ts.blk_free, 1, ns, nt))) return rc;
-      // the history pool is not indexed by slot: only the tracks' block indices move with the store
-      if (fhist_on && (rc = regrow(b_hblk, &ts.hblk, 1, ns, nt))) return rc;
-    }
-    if (ns != scene_cap) {
-      // per-slot small arrays
-      DBuf n1, n2, n3, n4, n5;
-      if ((rc = n1.ensure(sizeof(int) * ns))) return rc;
-      if ((rc = n2.ensure(sizeof(unsigned int) * ns))) return rc;
-      if ((rc = n3.ensure(sizeof(unsigned long long) * ns))) return rc;
-      if ((rc = n4.ensure(sizeof(int) * ns))) return rc;
-      if ((rc = n5.ensure(sizeof(int) * ns))) return rc;
-      CU(cudaMemsetAsync(n1.p, 0, sizeof(int) * ns, stream));
-      CU(cudaMemsetAsync(n4.p, 0, sizeof(int) * ns, stream));
-      CU(cudaMemsetAsync(n5.p, 0, sizeof(int) * ns, stream));
-      if (b_ntracks.p && scene_cap > 0) {
-        CU(cudaMemcpyAsync(n1.p, b_ntracks.p, sizeof(int) * scene_cap, cudaMemcpyDeviceToDevice, stream));
-        CU(cudaMemcpyAsync(n4.p, b_nfree.p, sizeof(int) * scene_cap, cudaMemcpyDeviceToDevice, stream));
-        CU(cudaMemcpyAsync(n5.p, b_atop.p, sizeof(int) * scene_cap, cudaMemcpyDeviceToDevice, stream));
-      }
-      CU(cudaStreamSynchronize(stream));
-      b_ntracks.release(); b_cur_epoch.release(); b_scene_ids.release(); b_nfree.release(); b_atop.release();
-      b_ntracks = n1; b_cur_epoch = n2; b_scene_ids = n3; b_nfree = n4; b_atop = n5;
-      ts.n_free = b_nfree.as<int>();
-      ts.arena_top = b_atop.as<int>();
-    }
+    if (hist_len > 1) ts.hist_len = hist_len;
     scene_cap = ns;
     track_cap = nt;
     ts.track_cap = nt;
@@ -453,47 +496,14 @@ struct sb200_tracker {
     if (need <= wb.cap) return 0;
     int64_t ncap = std::max<int64_t>(need, std::max<int64_t>(1024, (int64_t)wb.cap * 3));
     // wasted records are drained by sb200_wasted; growing preserves the pending ones
-    DBuf nid, nsc, nep, nle, npr, nob, nhp, nho, nhb;
-    int rc;
-    if ((rc = nid.ensure(8 * ncap)) || (rc = nsc.ensure(8 * ncap)) || (rc = nep.ensure(4 * ncap)) ||
-        (rc = nle.ensure(4 * ncap)) || (rc = npr.ensure(24 * ncap)) || (rc = nob.ensure(24 * ncap)))
-      return rc;
-    if (fhist_on && (rc = nhb.ensure(4 * ncap))) return rc;
-    const size_t hrow = (size_t)24 * hist_len;
-    if (hist_len > 1 && ((rc = nhp.ensure(hrow * ncap)) || (rc = nho.ensure(hrow * ncap)))) return rc;
-    if (wasted_count > 0) {
-      CU(cudaMemcpyAsync(nid.p, w_id.p, 8 * wasted_count, cudaMemcpyDeviceToDevice, stream));
-      CU(cudaMemcpyAsync(nsc.p, w_scene.p, 8 * wasted_count, cudaMemcpyDeviceToDevice, stream));
-      CU(cudaMemcpyAsync(nep.p, w_epoch.p, 4 * wasted_count, cudaMemcpyDeviceToDevice, stream));
-      CU(cudaMemcpyAsync(nle.p, w_length.p, 4 * wasted_count, cudaMemcpyDeviceToDevice, stream));
-      CU(cudaMemcpyAsync(npr.p, w_pred.p, 24 * wasted_count, cudaMemcpyDeviceToDevice, stream));
-      CU(cudaMemcpyAsync(nob.p, w_obs.p, 24 * wasted_count, cudaMemcpyDeviceToDevice, stream));
-      if (hist_len > 1) {
-        CU(cudaMemcpyAsync(nhp.p, w_hpred.p, hrow * wasted_count, cudaMemcpyDeviceToDevice, stream));
-        CU(cudaMemcpyAsync(nho.p, w_hobs.p, hrow * wasted_count, cudaMemcpyDeviceToDevice, stream));
-      }
-      if (fhist_on) CU(cudaMemcpyAsync(nhb.p, w_hblk.p, 4 * wasted_count, cudaMemcpyDeviceToDevice, stream));
-      CU(cudaStreamSynchronize(stream));
-    }
-    w_id.release(); w_scene.release(); w_epoch.release(); w_length.release(); w_pred.release(); w_obs.release();
-    w_hpred.release(); w_hobs.release(); w_hblk.release();
-    w_id = nid; w_scene = nsc; w_epoch = nep; w_length = nle; w_pred = npr; w_obs = nob; w_hpred = nhp; w_hobs = nho;
-    w_hblk = nhb;
-    wb.hblk = w_hblk.as<int>();
-    wb.hist_pred = w_hpred.as<float>();
-    wb.hist_obs = w_hobs.as<float>();
+    int rc = grow(wasted_table(), 1, (size_t)ncap, 1, (size_t)wasted_count);
+    if (rc) return rc;
     if (!w_count.p) {
       if ((rc = w_count.ensure(sizeof(int)))) return rc;
       CU(cudaMemsetAsync(w_count.p, 0, sizeof(int), stream));
     }
     wb.cap = (int)ncap;
     wb.count = w_count.as<int>();
-    wb.id = w_id.as<unsigned long long>();
-    wb.scene = w_scene.as<unsigned long long>();
-    wb.epoch = w_epoch.as<unsigned int>();
-    wb.length = w_length.as<unsigned int>();
-    wb.pred = w_pred.as<float>();
-    wb.obs = w_obs.as<float>();
     return 0;
   }
 
@@ -556,24 +566,17 @@ struct sb200_tracker {
       hpool_free = nf;
     }
     if (rest > 0) {
+      const std::vector<Col> cols = wasted_table();
+      size_t wmax = 0;
+      for (const Col& c : cols) wmax = std::max(wmax, c.w);
       DBuf tmp;   // overlapping device-to-device moves are done through a temporary
-      if ((rc = tmp.ensure((size_t)rest * 24))) return rc;
-      auto shift = [&](void* base, size_t el) -> int {
-        CU(cudaMemcpyAsync(tmp.p, (char*)base + n * el, rest * el, cudaMemcpyDeviceToDevice, st));
-        CU(cudaMemcpyAsync(base, tmp.p, rest * el, cudaMemcpyDeviceToDevice, st));
-        return 0;
-      };
-      if ((rc = shift(wb.id, 8)) || (rc = shift(wb.scene, 8)) || (rc = shift(wb.epoch, 4)) || (rc = shift(wb.length, 4)) ||
-          (rc = shift(wb.pred, 24)) || (rc = shift(wb.obs, 24)))
-        return rc;
-      if (fhist_on && (rc = shift(wb.hblk, 4))) return rc;
-      if (hist_len > 1) {
-        tmp.release();
-        if ((rc = tmp.ensure((size_t)rest * 24 * hist_len))) return rc;
-        if ((rc = shift(wb.hist_pred, (size_t)24 * hist_len)) || (rc = shift(wb.hist_obs, (size_t)24 * hist_len))) return rc;
+      if ((rc = tmp.ensure((size_t)rest * wmax))) return rc;
+      for (const Col& c : cols) {
+        char* base = c.buf->as<char>();
+        CU(cudaMemcpyAsync(tmp.p, base + n * c.w, rest * c.w, cudaMemcpyDeviceToDevice, st));
+        CU(cudaMemcpyAsync(base, tmp.p, rest * c.w, cudaMemcpyDeviceToDevice, st));
       }
       CU(cudaStreamSynchronize(st));
-      tmp.release();
     }
     int newc = (int)rest;
     CU(cudaMemcpyAsync(w_count.p, &newc, sizeof(int), cudaMemcpyHostToDevice, st));
@@ -584,60 +587,49 @@ struct sb200_tracker {
   }
 
   // (re)allocates the feature-history pool for exactly `need` blocks (at least 256), preserving the blocks handed out so
-  // far [0, hpool_top) and the free list.  Nothing may be in flight.
+  // far [0, hpool_top) and the free list (never longer than that).  Nothing may be in flight.
   int ensure_hpool(long long need) {
     if (need <= hpool_cap) return 0;
     const long long ncap = std::max<long long>(need, 256);
-    const size_t H = (size_t)hist_len, d8 = (size_t)P.d8;
-    DBuf nr, np, nf;
-    int rc;
-    if ((rc = nr.ensure((size_t)ncap * H * d8 * 4)) || (rc = np.ensure((size_t)ncap * H)) || (rc = nf.ensure((size_t)ncap * 4)))
-      return rc;
-    CU(cudaMemsetAsync(np.p, 0, (size_t)ncap * H, stream));
-    if (hpool_top > 0) {
-      CU(cudaMemcpyAsync(nr.p, b_hrows.p, (size_t)hpool_top * H * d8 * 4, cudaMemcpyDeviceToDevice, stream));
-      CU(cudaMemcpyAsync(np.p, b_hpresent.p, (size_t)hpool_top * H, cudaMemcpyDeviceToDevice, stream));
-      CU(cudaMemcpyAsync(nf.p, b_hfree.p, (size_t)hpool_top * 4, cudaMemcpyDeviceToDevice, stream));   // free <= top
-    }
-    CU(cudaStreamSynchronize(stream));
-    b_hrows.release(); b_hpresent.release(); b_hfree.release();
-    b_hrows = nr; b_hpresent = np; b_hfree = nf;
-    ts.hrows = b_hrows.as<float>();
-    ts.hpresent = b_hpresent.as<unsigned char>();
-    ts.hfree = b_hfree.as<int>();
+    int rc = grow(pool_table(), 1, (size_t)ncap, 1, (size_t)hpool_top);
+    if (rc) return rc;
     hpool_cap = ncap;
     return 0;
   }
 
+  // Adds or drops the feature history: the block index of every store row and wasted record (the entries of those tables
+  // tagged kTagHblk), the pool's counters; the pool itself comes with the first frame that needs it (ensure_hpool).  An
+  // add that fails drops what it added.
   int set_feature_history(bool on) {
     if (on == fhist_on) return 0;
     CU(cudaSetDevice(device));
     CU(cudaStreamSynchronize(stream));
-    if (!on) {
-      b_hblk.release(); b_hrows.release(); b_hpresent.release(); b_hfree.release(); b_hpool.release(); w_hblk.release();
-      f_histdst.release();
-      ts.hblk = nullptr; ts.hrows = nullptr; ts.hpresent = nullptr; ts.hfree = nullptr; ts.hpool = nullptr;
-      ts.fhist_len = 0;
-      wb.hblk = nullptr;
-      fhist_on = false;
-      hpool_cap = hpool_top = hpool_free = hpool_pend = 0;
-      return 0;
-    }
+    fhist_on = true;   // the tables list the history columns while they are added or dropped
+    const int rc = on ? add_feature_history() : 0;
+    if (on && rc == 0) return 0;
+    std::vector<Col> cols = pool_table();
+    for (const Col& c : store_table()) if (c.tag == kTagHblk) cols.push_back(c);
+    for (const Col& c : wasted_table()) if (c.tag == kTagHblk) cols.push_back(c);
+    for (const Col& c : cols) { c.buf->release(); c.point(*this, nullptr); }
+    b_hpool.release();
+    f_histdst.release();
+    ts.hpool = nullptr;
+    ts.fhist_len = 0;
+    fhist_on = false;
+    hpool_cap = hpool_top = hpool_free = hpool_pend = 0;
+    return rc;
+  }
+  int add_feature_history() {
     int rc;
     if ((rc = b_hpool.ensure(2 * sizeof(int)))) return rc;
     CU(cudaMemsetAsync(b_hpool.p, 0, 2 * sizeof(int), stream));
-    if (scene_cap > 0 && track_cap > 0) {
-      if ((rc = b_hblk.ensure((size_t)scene_cap * track_cap * sizeof(int)))) return rc;
-      ts.hblk = b_hblk.as<int>();
-    }
-    if (wb.cap > 0) {   // no record exists before the first frame
-      if ((rc = w_hblk.ensure((size_t)wb.cap * sizeof(int)))) return rc;
-      wb.hblk = w_hblk.as<int>();
-    }
+    for (const Col& c : store_table())
+      if (c.tag == kTagHblk && scene_cap > 0 && (rc = grow({c}, scene_cap, track_cap, 0, 0))) return rc;
+    for (const Col& c : wasted_table())   // no record exists before the first frame
+      if (c.tag == kTagHblk && wb.cap > 0 && (rc = grow({c}, 1, wb.cap, 0, 0))) return rc;
     CU(cudaStreamSynchronize(stream));
     ts.hpool = b_hpool.as<int>();
     ts.fhist_len = hist_len;
-    fhist_on = true;
     return 0;
   }
 
@@ -992,19 +984,17 @@ int sb200_tracker::predict(int32_t n_scenes, const uint64_t* scene_ids, const in
   }
   // candidate-side buffers: the set of this frame (the other one may still be read by the frame in front of it)
   const int cset = (int)(frame_seq & 1);
-  DBuf &f_cbox = f_cbox2[cset], &f_cradius = f_cradius2[cset], &f_cconf = f_cconf2[cset], &f_cvert = f_cvert2[cset],
-       &f_cflags = f_cflags2[cset], &f_cnorm2 = f_cnorm22[cset], &f_cbf16 = f_cbf162[cset], &f_decided = f_decided2[cset],
-       &f_cfp8 = f_cfp82[cset], &f_cscale = f_cscale2[cset];
-  if ((rc = ENS(f_cbox, T * 24)) || (rc = ENS(f_cradius, T * 4)) || (rc = ENS(f_cconf, T * 4)) ||
+  CandBufs& cb = cand[cset];
+  if ((rc = ENS(cb.box, T * 24)) || (rc = ENS(cb.radius, T * 4)) || (rc = ENS(cb.conf, T * 4)) ||
       (rc = ENS(f_winner, T * 4)) || (rc = ENS(f_cvt, T)) || (rc = ENS(f_scenes, sizeof(sb::SceneDesc) * n_scenes)) ||
       (rc = ENS(f_newcount, 4 * (size_t)n_scenes)) || (rc = ENS(f_dyn, sizeof(sb::FrameDyn))) ||
       (rc = ENS(f_apprank, T * 8)) || (rc = ENS(f_appmeta, 16 * (size_t)n_scenes)) ||
       (rc = ENS(f_pos, std::max<size_t>(4, (size_t)pos_total * 4))))
     return rc;
-  if (P.positional_kind == SB200_POS_IOU && (rc = ENS(f_cvert, T * 64))) return rc;
+  if (P.positional_kind == SB200_POS_IOU && (rc = ENS(cb.vert, T * 64))) return rc;
   if (P.is_visual) {
     if (fhist_on && (rc = ENS(f_histdst, T * 4))) return rc;
-    if ((rc = ENS(f_cflags, T)) || (rc = ENS(f_cnorm2, T * 4)) || (rc = ENS(f_featdst, T * 4)) ||
+    if ((rc = ENS(cb.flags, T)) || (rc = ENS(cb.norm2, T * 4)) || (rc = ENS(f_featdst, T * 4)) ||
         (rc = ENS(f_vis, std::max<size_t>(4, (size_t)vis_total * 4))) || (rc = ENS(f_scene_max, 4 * (size_t)n_scenes)))
       return rc;
   }
@@ -1041,8 +1031,8 @@ int sb200_tracker::predict(int32_t n_scenes, const uint64_t* scene_ids, const in
     // both operand copies of the candidates whenever the e4m3 screen can run: a switch between the precisions must not
     // allocate (and synchronise) in the middle of a stream of frames
     const bool alloc8 = !want_dense && P.d8 <= sb::kFp8MaxD8 && ts.feat_fp8 != nullptr;
-    if (alloc8 && ((rc = ENS(f_cfp8, T * sb::fp8_pitch(P.d8))) || (rc = ENS(f_cscale, T * 4)))) return rc;
-    if ((rc = ENS(f_cbf16, T * P.d8 * 2)) || (rc = ENS(f_tiles, sizeof(sb::TcTile) * (size_t)std::max<long long>(1, tiles_alloc))) ||
+    if (alloc8 && ((rc = ENS(cb.fp8, T * sb::fp8_pitch(P.d8))) || (rc = ENS(cb.scale, T * 4)))) return rc;
+    if ((rc = ENS(cb.bf16, T * P.d8 * 2)) || (rc = ENS(f_tiles, sizeof(sb::TcTile) * (size_t)std::max<long long>(1, tiles_alloc))) ||
         (rc = ENS(f_rowmeta, sizeof(sb::VisRowMeta) * (T + 256))))
       return rc;
     tc.rowmeta = f_rowmeta.as<sb::VisRowMeta>();
@@ -1162,8 +1152,8 @@ int sb200_tracker::predict(int32_t n_scenes, const uint64_t* scene_ids, const in
     if (custom_ids && total > 0) { if ((rc = ENS(S.custom, T * 8))) return rc; f.in_custom = S.custom.as<long long>(); }
     if (own_area && total > 0) { if ((rc = ENS(S.own, T * 4))) return rc; f.in_own = S.own.as<float>(); }
   }
-  f.c_box = f_cbox.as<float>(); f.c_radius = f_cradius.as<float>(); f.c_conf = f_cconf.as<float>();
-  f.c_vert = f_cvert.as<double>(); f.c_flags = f_cflags.as<unsigned char>(); f.c_norm2 = f_cnorm2.as<float>();
+  f.c_box = cb.box.as<float>(); f.c_radius = cb.radius.as<float>(); f.c_conf = cb.conf.as<float>();
+  f.c_vert = cb.vert.as<double>(); f.c_flags = cb.flags.as<unsigned char>(); f.c_norm2 = cb.norm2.as<float>();
   f.winner = f_winner.as<int>(); f.c_vt = f_cvt.as<unsigned char>(); f.pos = f_pos.as<float>(); f.vis = f_vis.as<float>();
   f.scenes = f_scenes.as<sb::SceneDesc>(); f.new_count = f_newcount.as<int>();
   f.new_count_all = f.new_count;
@@ -1172,9 +1162,9 @@ int sb200_tracker::predict(int32_t n_scenes, const uint64_t* scene_ids, const in
   f.app_rank = f_apprank.as<int2>(); f.app_meta = f_appmeta.as<int4>();
   if ((rc = ENS(f_frameout, sizeof(int) * 3 * (size_t)n_scenes))) return rc;
   f.frame_out = f_frameout.as<int>();
-  f.c_bf16 = tc.use_tc && !tc.fp8 ? f_cbf16.p : nullptr; f.scene_max = f_scene_max.as<unsigned int>();
-  f.c_fp8 = tc.fp8 ? f_cfp8.as<unsigned char>() : nullptr;
-  f.c_scale = tc.fp8 ? f_cscale.as<float>() : nullptr;
+  f.c_bf16 = tc.use_tc && !tc.fp8 ? cb.bf16.p : nullptr; f.scene_max = f_scene_max.as<unsigned int>();
+  f.c_fp8 = tc.fp8 ? cb.fp8.as<unsigned char>() : nullptr;
+  f.c_scale = tc.fp8 ? cb.scale.as<float>() : nullptr;
   // sparse entry lists + per-scene counters (pos_cnt | vis_cnt | scene_mode | vis_mode | refine_next | dense_cnt | status),
   // zeroed every frame by frame_setup_kernel
   const size_t n_counters = 6 * (size_t)n_scenes + 4;
@@ -1215,8 +1205,8 @@ int sb200_tracker::predict(int32_t n_scenes, const uint64_t* scene_ids, const in
   // SB200_FULL_COSTS=1 (every pair is evaluated, sb200_last_costs is complete) keeps the plain order.
   const bool fork = P.is_visual && tc.use_tc && tc.n_tiles > 0 && !f.pos_dense_all;
   if (fork) {
-    if ((rc = ENS(f_decided, T)) || (rc = ENS(f_excl, (size_t)scene_cap * track_cap + 16)) || (rc = ENS(f_prewin, T * 4))) return rc;
-    f.decided = f_decided.as<unsigned char>();
+    if ((rc = ENS(cb.decided, T)) || (rc = ENS(f_excl, (size_t)scene_cap * track_cap + 16)) || (rc = ENS(f_prewin, T * 4))) return rc;
+    f.decided = cb.decided.as<unsigned char>();
     f.excl = f_excl.as<unsigned char>();
     f.pre_winner = f_prewin.as<int>();
   }
@@ -1569,34 +1559,31 @@ int sb200_set_feature_dim(sb200_tracker* t, int32_t feature_dim) {
   int rc = t->drain();
   if (rc) return rc;
   CU(cudaStreamSynchronize(t->stream));
-  // no track holds a feature yet (obs_hasf == 0 everywhere): the feature arena is simply re-created for the new row size
+  // No track holds a feature yet (obs_hasf == 0 everywhere): the columns whose rows depend on d8 are simply re-created for
+  // the new row size -- the feature rows with their BF16 and e4m3 copies (the latter exist for d8 <= 512 only) and the
+  // history rows of the pool.  The present bytes (all zero so far) and the tracks' blocks stay.
+  auto d8_cols = [t] {   // (column, rows it holds)
+    std::vector<std::pair<Col, size_t>> v;
+    for (const Col& c : t->store_table())
+      if (c.buf == &t->b_feat || c.buf == &t->b_feat_bf16 || c.buf == &t->b_feat_fp8 || c.buf == &t->b_fscale)
+        v.push_back({c, (size_t)t->scene_cap * t->track_cap});
+    if (t->fhist_on)
+      for (const Col& c : t->pool_table()) if (c.buf == &t->b_hrows) v.push_back({c, (size_t)t->hpool_cap});
+    return v;
+  };
+  for (const auto& [c, rows] : d8_cols()) { c.buf->release(); c.point(*t, nullptr); }
+  for (auto& cb : t->cand) { cb.bf16.release(); cb.fp8.release(); }
   t->P.feature_dim = feature_dim;
   t->P.d8 = (feature_dim + 7) / 8 * 8;
   t->P.vis_rel_err = sb::screen_rel_err(feature_dim);
   t->P.vis_rel_err8 = sb::screen_rel_err_fp8(feature_dim);
   t->opts.feature_dim = feature_dim;
-  t->b_feat.release(); t->b_feat_bf16.release(); t->f_cbf162[0].release(); t->f_cbf162[1].release();
-  t->b_feat_fp8.release(); t->b_fscale.release(); t->f_cfp82[0].release(); t->f_cfp82[1].release();
-  t->ts.feat = nullptr; t->ts.feat_bf16 = nullptr; t->ts.feat_fp8 = nullptr; t->ts.fscale = nullptr;
-  const size_t rows = (size_t)t->scene_cap * t->track_cap * t->P.max_obs;
-  if (rows > 0) {
-    if ((rc = t->b_feat.ensure(rows * t->P.d8 * 4)) || (rc = t->b_feat_bf16.ensure(rows * t->P.d8 * 2))) return rc;
-    t->ts.feat = t->b_feat.as<float>();
-    t->ts.feat_bf16 = t->b_feat_bf16.p;
-    if (t->P.d8 <= sb::kFp8MaxD8) {
-      if ((rc = t->b_feat_fp8.ensure(rows * sb::fp8_pitch(t->P.d8))) || (rc = t->b_fscale.ensure(rows * 4))) return rc;
-      t->ts.feat_fp8 = t->b_feat_fp8.as<unsigned char>();
-      t->ts.fscale = t->b_fscale.as<float>();
-    }
+  for (const auto& [c, rows] : d8_cols()) {
+    if (rows == 0) continue;
+    if ((rc = c.buf->ensure(rows * c.w))) return rc;
+    c.point(*t, c.buf->p);
   }
   for (auto& g : t->stg) g.feat.release();
-  if (t->fhist_on && t->hpool_cap > 0) {
-    // the history rows are re-created for the new row size; the present bytes (all zero so far) and the tracks' blocks stay
-    t->b_hrows.release();
-    t->ts.hrows = nullptr;
-    if ((rc = t->b_hrows.ensure((size_t)t->hpool_cap * t->hist_len * t->P.d8 * 4))) return rc;
-    t->ts.hrows = t->b_hrows.as<float>();
-  }
   return 0;
 }
 
@@ -1878,7 +1865,6 @@ static int64_t wasted_records(sb200_tracker* t, int64_t cap, uint64_t* ids, uint
       CU(cudaMemcpyAsync(feature_present + (size_t)i0 * history_cap, pres.p, (size_t)c * history_cap, cudaMemcpyDeviceToHost, st));
       CU(cudaStreamSynchronize(st));
     }
-    rows.release(); pres.release();
   }
   if ((rc = t->drop_wasted_front(n))) return rc;   // drain
   return n;
@@ -2074,53 +2060,36 @@ struct BlobHeader {
   uint64_t id_counter;   // ids handed out by the source (at export, for a scene blob)
   uint64_t sec_off[kMaxSections], sec_bytes[kMaxSections];
 };
-struct TmpBuf : DBuf { ~TmpBuf() { release(); } };   // a DBuf freed when it goes out of scope
 struct BlobScene { uint64_t scene_id; uint32_t epoch; int32_t n_tracks, n_hidden, arena_top; };
 
-// a column of the store: rows of `w` bytes per live track (0), per arena block (1) or per free-list entry (2)
-enum ColTag { kTagNone, kTagFblk, kTagHblk, kTagObsN, kTagObsPhys, kTagOwner, kTagFree };
-struct Col { char* base; size_t w; int kind; int tag = kTagNone; };   // tag: index-valued columns a load checks
-
-std::vector<Col> store_cols(const sb200_tracker* t, bool tracker_blob) {
-  const sb::TrackStore& ts = t->ts;
-  const size_t K = (size_t)t->P.max_obs, d8 = (size_t)t->P.d8, H = (size_t)t->hist_len;
-  std::vector<Col> c = {{(char*)ts.id, 8, 0}, {(char*)ts.epoch, 4, 0}, {(char*)ts.length, 4, 0}, {(char*)ts.custom, 8, 0},
-                        {(char*)ts.vt, 1, 0}, {(char*)ts.pred, 24, 0}, {(char*)ts.obs, 24, 0}, {(char*)ts.radius, 4, 0},
-                        {(char*)ts.kst, 4 * (size_t)sb::kStateStride, 0}};
-  if (t->P.positional_kind == SB200_POS_IOU) c.push_back({(char*)ts.vert, 64, 0});
-  if (H > 1) { c.push_back({(char*)ts.hist_pred, 24 * H, 0}); c.push_back({(char*)ts.hist_obs, 24 * H, 0}); }
-  if (t->P.is_visual) {
-    c.push_back({(char*)ts.obs_phys, K, 0, kTagObsPhys}); c.push_back({(char*)ts.obs_hasf, K, 0});
-    c.push_back({(char*)ts.obs_q, 4 * K, 0});
-    c.push_back({(char*)ts.obs_n, 1, 0, kTagObsN}); c.push_back({(char*)ts.feat_cnt, 1, 0});
-    c.push_back({(char*)ts.fblk, 4, 0, kTagFblk});
-    // a scene blob carries the history rows themselves (renumbered on import), a tracker blob the pool and the indices
-    if (t->fhist_on && tracker_blob) c.push_back({(char*)ts.hblk, 4, 0, kTagHblk});
-    c.push_back({(char*)ts.feat, 4 * K * d8, 1}); c.push_back({(char*)ts.feat_bf16, 2 * K * d8, 1});
-    c.push_back({(char*)ts.fnorm2, 4 * K, 1}); c.push_back({(char*)ts.blk_owner, 4, 1, kTagOwner});
-    c.push_back({(char*)ts.blk_free, 4, 2, kTagFree});
-  }
-  return c;
-}
-
-// byte sizes of every section after the scene table, in blob order (the structure depends on the options only)
-std::vector<uint64_t> section_bytes(const sb200_tracker* t, uint32_t type, int64_t n_scenes, int64_t live, int64_t blk,
-                                    int64_t fre, int64_t wasted, int64_t top, int64_t hfree) {
-  std::vector<uint64_t> b = {(uint64_t)n_scenes * sizeof(BlobScene)};
-  const int64_t cnt[3] = {live, blk, fre};
-  for (const Col& c : store_cols(t, type == kBlobTracker)) b.push_back((uint64_t)cnt[c.kind] * c.w);
-  const uint64_t H = (uint64_t)t->hist_len, hrow = H * (uint64_t)t->P.d8 * 4;
-  if (type == kBlobTracker) {
-    for (uint64_t w : {8, 8, 4, 4, 24, 24}) b.push_back((uint64_t)wasted * w);
-    if (H > 1) { b.push_back((uint64_t)wasted * 24 * H); b.push_back((uint64_t)wasted * 24 * H); }
-    if (t->fhist_on) {
-      b.push_back((uint64_t)wasted * 4);
-      b.push_back((uint64_t)top * hrow); b.push_back((uint64_t)top * H); b.push_back((uint64_t)hfree * 4);
-    }
+// the columns of the sections after the scene table, in blob order
+std::vector<Col> blob_cols(sb200_tracker* t, uint32_t type) {
+  const bool tracker_blob = type == kBlobTracker;
+  std::vector<Col> b;
+  for (const Col& c : t->store_table())
+    if (c.blob == kBlobAll || (c.blob == kBlobTrackerOnly && tracker_blob)) b.push_back(c);
+  if (tracker_blob) {
+    for (const Col& c : t->wasted_table()) b.push_back(c);
+    if (t->fhist_on) for (const Col& c : t->pool_table()) b.push_back(c);
   } else if (t->fhist_on) {
-    b.push_back((uint64_t)live * hrow); b.push_back((uint64_t)live * H);
+    for (const Col& c : t->pool_table())   // the history rows of each live track, gathered from the pool
+      if (c.rows == kRowHistTop) b.push_back({c.buf, nullptr, c.w, false, kRowTrackHist});
   }
   return b;
+}
+
+// byte sizes of every section, in blob order (the structure depends on the options only)
+std::vector<uint64_t> section_bytes(sb200_tracker* t, uint32_t type, int64_t n_scenes, int64_t live, int64_t blk,
+                                    int64_t fre, int64_t wasted, int64_t top, int64_t hfree) {
+  std::vector<uint64_t> b = {(uint64_t)n_scenes * sizeof(BlobScene)};
+  const int64_t cnt[] = {live, blk, fre, wasted, top, hfree, live};   // rows, by ColRows
+  for (const Col& c : blob_cols(t, type)) b.push_back((uint64_t)cnt[c.rows] * c.w);
+  return b;
+}
+
+// rows of a section that covers the whole tracker (kRowWasted, kRowHistTop, kRowHistFree)
+int64_t tracker_rows(const BlobHeader& h, int rows) {
+  return rows == kRowWasted ? h.wasted_count : (rows == kRowHistTop ? h.hpool_top : h.hpool_free);
 }
 
 // header sections from their sizes; returns the blob's total size
@@ -2204,36 +2173,24 @@ int move_store(sb200_tracker* t, int dir, uint32_t type, const BlobHeader& h, ch
     if (dir == 0) segs.push_back({store, blob, bytes});
     else segs.push_back({blob, store, bytes});
   };
-  const std::vector<Col> cols = store_cols(t, type == kBlobTracker);
+  const std::vector<Col> cols = blob_cols(t, type);
+  size_t hist_sec = 0;   // scene blob: the history rows, then the present bytes, of the live tracks (launch_xfer_hist)
   for (size_t c = 0; c < cols.size(); ++c) {
+    const Col& col = cols[c];
+    char* sec = dblob + h.sec_off[1 + c];
+    if (col.rows == kRowTrackHist) {
+      if (!hist_sec) hist_sec = 1 + c;
+      continue;
+    }
+    if (col.rows >= kRowWasted) {
+      add(col.buf->as<char>(), sec, (uint64_t)tracker_rows(h, col.rows) * col.w);
+      continue;
+    }
     int64_t pre = 0;
     for (const SlotRows& r : rows) {
-      const int64_t cnt = cols[c].kind == 0 ? r.n : (cols[c].kind == 1 ? r.blk : r.fre);
-      add(cols[c].base + (size_t)r.slot * tc * cols[c].w, dblob + h.sec_off[1 + c] + (uint64_t)pre * cols[c].w,
-          (uint64_t)cnt * cols[c].w);
+      const int64_t cnt = col.rows == kRowTrack ? r.n : (col.rows == kRowBlock ? r.blk : r.fre);
+      add(col.buf->as<char>() + (size_t)r.slot * tc * col.w, sec + (uint64_t)pre * col.w, (uint64_t)cnt * col.w);
       pre += cnt;
-    }
-  }
-  size_t sec = 1 + cols.size();
-  const uint64_t H = (uint64_t)t->hist_len, hrow = H * (uint64_t)t->P.d8 * 4;
-  if (type == kBlobTracker) {
-    const uint64_t wn = (uint64_t)h.wasted_count;
-    const sb::WastedBuf& wb = t->wb;
-    add((char*)wb.id, dblob + h.sec_off[sec++], wn * 8);
-    add((char*)wb.scene, dblob + h.sec_off[sec++], wn * 8);
-    add((char*)wb.epoch, dblob + h.sec_off[sec++], wn * 4);
-    add((char*)wb.length, dblob + h.sec_off[sec++], wn * 4);
-    add((char*)wb.pred, dblob + h.sec_off[sec++], wn * 24);
-    add((char*)wb.obs, dblob + h.sec_off[sec++], wn * 24);
-    if (H > 1) {
-      add((char*)wb.hist_pred, dblob + h.sec_off[sec++], wn * 24 * H);
-      add((char*)wb.hist_obs, dblob + h.sec_off[sec++], wn * 24 * H);
-    }
-    if (t->fhist_on) {
-      add((char*)wb.hblk, dblob + h.sec_off[sec++], wn * 4);
-      add((char*)t->ts.hrows, dblob + h.sec_off[sec++], (uint64_t)h.hpool_top * hrow);
-      add((char*)t->ts.hpresent, dblob + h.sec_off[sec++], (uint64_t)h.hpool_top * H);
-      add((char*)t->ts.hfree, dblob + h.sec_off[sec++], (uint64_t)h.hpool_free * 4);
     }
   }
   const cudaStream_t st = t->stream;
@@ -2241,7 +2198,7 @@ int move_store(sb200_tracker* t, int dir, uint32_t type, const BlobHeader& h, ch
     std::vector<long long> cpre(segs.size() + 1, 0);
     for (size_t i = 0; i < segs.size(); ++i)
       cpre[i + 1] = cpre[i] + (long long)((segs[i].bytes + sb::kXferChunk - 1) / sb::kXferChunk);
-    TmpBuf d_tab;
+    DBuf d_tab;
     const size_t sb_ = segs.size() * sizeof(sb::XferSeg);
     int rc = d_tab.ensure(sb_ + cpre.size() * sizeof(long long));
     if (rc) return rc;
@@ -2255,13 +2212,13 @@ int move_store(sb200_tracker* t, int dir, uint32_t type, const BlobHeader& h, ch
   if (type == kBlobScenes && t->fhist_on && h.live_total > 0) {
     std::vector<int> tab(2 * rows.size() + 1, 0);   // slots | prefix of the live tracks
     for (size_t i = 0; i < rows.size(); ++i) { tab[i] = rows[i].slot; tab[rows.size() + i + 1] = tab[rows.size() + i] + rows[i].n; }
-    TmpBuf d_tab;
+    DBuf d_tab;
     int rc = d_tab.ensure(tab.size() * sizeof(int));
     if (rc) return rc;
     CU(cudaMemcpyAsync(d_tab.p, tab.data(), tab.size() * sizeof(int), cudaMemcpyHostToDevice, st));
     const int e = sb::launch_xfer_hist(t->ts, t->P.d8, d_tab.as<int>(), d_tab.as<int>() + rows.size(), (int)rows.size(),
-                                       (int)h.live_total, dir, reinterpret_cast<float*>(dblob + h.sec_off[sec]),
-                                       reinterpret_cast<unsigned char*>(dblob + h.sec_off[sec + 1]), hist_base, t->num_sms, st);
+                                       (int)h.live_total, dir, reinterpret_cast<float*>(dblob + h.sec_off[hist_sec]),
+                                       reinterpret_cast<unsigned char*>(dblob + h.sec_off[hist_sec + 1]), hist_base, t->num_sms, st);
     if (e) return fail(SB200_ERR_CUDA, "history copy launch failed: %s", cudaGetErrorString((cudaError_t)e));
     CU(cudaStreamSynchronize(st));
   }
@@ -2274,20 +2231,25 @@ int move_store(sb200_tracker* t, int dir, uint32_t type, const BlobHeader& h, ch
 int check_indices(sb200_tracker* t, uint32_t type, const BlobHeader& h, const char* dblob,
                   const std::vector<BlobScene>& table) {
   std::vector<sb::XferCheck> ck;
-  const std::vector<Col> cols = store_cols(t, type == kBlobTracker);
+  const std::vector<Col> cols = blob_cols(t, type);
   const int K = t->P.max_obs;
   const char* obs_n_sec = nullptr;
   for (size_t c = 0; c < cols.size(); ++c)
     if (cols[c].tag == kTagObsN) obs_n_sec = dblob + h.sec_off[1 + c];
   for (size_t c = 0; c < cols.size(); ++c) {
-    if (cols[c].tag == kTagNone) continue;
+    const Col& col = cols[c];
+    if (col.tag == kTagNone) continue;
     const char* sec = dblob + h.sec_off[1 + c];
+    if (col.rows >= kRowWasted) {   // history block indices of the wasted records / the pool's free stack
+      ck.push_back({sec, nullptr, tracker_rows(h, col.rows), 0, (int)h.hpool_top, 0});
+      continue;
+    }
     int64_t pre = 0;
     for (const BlobScene& s : table) {
       const int fre = s.arena_top - s.n_tracks;
-      const int64_t cnt = cols[c].kind == 0 ? s.n_tracks : (cols[c].kind == 1 ? s.arena_top : fre);
-      const char* p = sec + (uint64_t)pre * cols[c].w;
-      switch (cols[c].tag) {
+      const int64_t cnt = col.rows == kRowTrack ? s.n_tracks : (col.rows == kRowBlock ? s.arena_top : fre);
+      const char* p = sec + (uint64_t)pre * col.w;
+      switch (col.tag) {
         case kTagFblk: case kTagFree: ck.push_back({p, nullptr, cnt, 0, s.arena_top, 0}); break;
         case kTagOwner: ck.push_back({p, nullptr, cnt, -1, s.n_tracks, 0}); break;
         case kTagHblk: ck.push_back({p, nullptr, cnt, 0, (int)h.hpool_top, 0}); break;
@@ -2298,14 +2260,9 @@ int check_indices(sb200_tracker* t, uint32_t type, const BlobHeader& h, const ch
       pre += cnt;
     }
   }
-  if (type == kBlobTracker && t->fhist_on) {
-    const size_t sec = 1 + cols.size() + 6 + (t->hist_len > 1 ? 2 : 0);   // wasted hblk, then rows, present, free stack
-    ck.push_back({dblob + h.sec_off[sec], nullptr, h.wasted_count, 0, (int)h.hpool_top, 0});
-    ck.push_back({dblob + h.sec_off[sec + 3], nullptr, h.hpool_free, 0, (int)h.hpool_top, 0});
-  }
   ck.erase(std::remove_if(ck.begin(), ck.end(), [](const sb::XferCheck& x) { return x.n <= 0; }), ck.end());
   if (ck.empty()) return 0;
-  TmpBuf d;
+  DBuf d;
   int rc = d.ensure(ck.size() * sizeof(sb::XferCheck) + 16);
   if (rc) return rc;
   int* d_bad = reinterpret_cast<int*>(d.as<char>() + ck.size() * sizeof(sb::XferCheck));
@@ -2324,7 +2281,7 @@ int check_indices(sb200_tracker* t, uint32_t type, const BlobHeader& h, const ch
 int set_slots(sb200_tracker* t, const std::vector<sb::XferSlot>& tab, int free0, int free_add, int top_add,
               unsigned long long id_min, bool raise_ids) {
   if (tab.empty()) return 0;
-  TmpBuf d_tab;
+  DBuf d_tab;
   int rc = d_tab.ensure(tab.size() * sizeof(sb::XferSlot));
   if (rc) return rc;
   CU(cudaMemcpyAsync(d_tab.p, tab.data(), tab.size() * sizeof(sb::XferSlot), cudaMemcpyHostToDevice, t->stream));
@@ -2382,7 +2339,7 @@ int save_blob(sb200_tracker* t, uint32_t type, const std::vector<int>& slots, vo
   *bytes = (size_t)total;
   if (!dst || cap < total) return fail(SB200_ERR_CAPACITY, "the blob needs %llu bytes", (unsigned long long)total);
   const int where = blob_device(dst);
-  TmpBuf tmp;
+  DBuf tmp;
   char* dblob = static_cast<char*>(dst);
   if (where != t->device) {
     if ((rc = tmp.ensure(total))) return rc;
@@ -2491,7 +2448,7 @@ int parse_blob(const void* src, size_t bytes, uint32_t want_type, cudaStream_t s
 }
 
 // the section sizes the tracker `t` (built with the blob's options) expects for the blob's counts
-int check_sections(const sb200_tracker* t, const BlobHeader& h) {
+int check_sections(sb200_tracker* t, const BlobHeader& h) {
   const std::vector<uint64_t> sec = section_bytes(t, h.type, h.n_scenes, h.live_total, h.blk_total, h.free_total,
                                                   h.wasted_count, h.hpool_top, h.hpool_free);
   if (sec.size() != h.n_sections) return fail(SB200_ERR_INVALID, "the blob has %u sections, %zu expected", h.n_sections, sec.size());
@@ -2567,7 +2524,7 @@ int sb200_tracker_load(const void* src, size_t bytes, int32_t device, sb200_trac
   if (t->fhist_on && h.hpool_cap > 0 && (rc = t->ensure_hpool(std::max(h.hpool_cap, h.hpool_top)))) return rc;
   if ((rc = t->b_idc.ensure(8))) return rc;
   const char* dblob = nullptr;
-  TmpBuf tmp;
+  DBuf tmp;
   if ((rc = blob_on_device(t, src, (size_t)h.total_bytes, tmp, &dblob))) return rc;
   if ((rc = check_indices(t, h.type, h, dblob, table))) return rc;
   std::vector<SlotRows> rows(table.size());
@@ -2674,7 +2631,7 @@ int sb200_scenes_import(sb200_tracker* t, const void* src, size_t bytes) {
       (rc = t->ensure_hpool(std::max(hist_base + h.live_total, t->hpool_cap + t->hpool_cap / 2))))
     return rc;
   const char* dblob = nullptr;
-  TmpBuf tmp;
+  DBuf tmp;
   if ((rc = blob_on_device(t, src, (size_t)h.total_bytes, tmp, &dblob))) return rc;
   if ((rc = check_indices(t, h.type, h, dblob, table))) return rc;
   std::vector<SlotRows> rows(table.size());
