@@ -374,8 +374,9 @@ struct sb200_tracker {
       // the history pool is not indexed by slot: only the tracks' block indices move with the store.  A scene blob carries
       // the history rows themselves (renumbered on import), a tracker blob the pool and the indices.
       if (fhist_on) c.push_back({&b_hblk, in_ts<&TS::hblk>, 4, false, kRowTrack, kBlobTrackerOnly, kTagHblk});
-      c.push_back({&b_feat, in_ts<&TS::feat>, 4 * K * d8, false, kRowBlock});
-      c.push_back({&b_feat_bf16, in_ts<&TS::feat_bf16>, 2 * K * d8, false, kRowBlock});
+      // zeroed: a block's rows past its track's observations are in the blob, and a full BF16 conversion reads them
+      c.push_back({&b_feat, in_ts<&TS::feat>, 4 * K * d8, true, kRowBlock});
+      c.push_back({&b_feat_bf16, in_ts<&TS::feat_bf16>, 2 * K * d8, true, kRowBlock});
       c.push_back({&b_fnorm2, in_ts<&TS::fnorm2>, 4 * K, false, kRowBlock});
       // the e4m3 copies: only the A-stationary screen (d8 <= 512) reads them.  Not in the blob: a load converts the f32
       // rows again (regen_fp8).
@@ -460,13 +461,33 @@ struct sb200_tracker {
     return cudaGetLastError() == cudaSuccess ? 0 : fail(SB200_ERR_CUDA, "e4m3 row conversion failed");
   }
 
+  // The BF16 rows the e4m3 frames skip (sb::Frame::skip_bf16).  Each such frame appends the rows it stores to a log of
+  // row indices; past its capacity every arena row counts as stale.  regen_bf16 converts them, in stream order, before
+  // anything reads the BF16 rows or the row indices change: a frame on the BF16 screen or the dense path, a blob, a regrow
+  // of the store.  The host decides a frame's precision while earlier frames are in flight: stream order alone makes the
+  // rows those frames store part of the conversion, with no wait for the device.
+  static constexpr long long kBf16LogCap = 1 << 18;
+  DBuf b_bf16log;
+  long long bf16_log_n = 0;     // entries in the log (each e4m3 frame adds one per detection, -1 where nothing is stored)
+  bool bf16_stale_all = false;  // the log overflowed
+  int regen_bf16() {
+    if (bf16_stale_all) sb::launch_bf16_regen(ts, P.d8, P.max_obs, nullptr, 0, scene_cap, stream);
+    else if (bf16_log_n > 0) sb::launch_bf16_regen(ts, P.d8, P.max_obs, b_bf16log.as<int>(), bf16_log_n, 0, stream);
+    else return 0;
+    bf16_log_n = 0;
+    bf16_stale_all = false;
+    return cudaGetLastError() == cudaSuccess ? 0 : fail(SB200_ERR_CUDA, "BF16 row conversion failed");
+  }
+
   // (re)allocates the track store for scene_cap x track_cap rows, preserving the live rows
   int ensure_store(int need_scenes, int need_tracks) {
     if (need_scenes <= scene_cap && need_tracks <= track_cap) return 0;
     int ns = scene_cap, nt = track_cap;
     if (need_scenes > ns) ns = std::max(need_scenes, std::max(4, ns * 2));
     if (need_tracks > nt) nt = std::max(need_tracks, std::max(64, nt * 2));
-    int rc = grow(store_table(), ns, nt, scene_cap, track_cap);
+    int rc = regen_bf16();   // the log's row indices hold for the old row pitch only
+    if (rc) return rc;
+    rc = grow(store_table(), ns, nt, scene_cap, track_cap);
     if (rc) return rc;
     if (ns != scene_cap && (rc = grow(slot_table(), ns, 1, scene_cap, 1))) return rc;
     ts.kst_stride = sb::kStateStride;
@@ -1031,7 +1052,8 @@ int sb200_tracker::predict(int32_t n_scenes, const uint64_t* scene_ids, const in
     // both operand copies of the candidates whenever the e4m3 screen can run: a switch between the precisions must not
     // allocate (and synchronise) in the middle of a stream of frames
     const bool alloc8 = !want_dense && P.d8 <= sb::kFp8MaxD8 && ts.feat_fp8 != nullptr;
-    if (alloc8 && ((rc = ENS(cb.fp8, T * sb::fp8_pitch(P.d8))) || (rc = ENS(cb.scale, T * 4)))) return rc;
+    if (alloc8 && ((rc = ENS(cb.fp8, T * sb::fp8_pitch(P.d8))) || (rc = ENS(cb.scale, T * 4)) || (rc = ENS(b_bf16log, kBf16LogCap * 4))))
+      return rc;
     if ((rc = ENS(cb.bf16, T * P.d8 * 2)) || (rc = ENS(f_tiles, sizeof(sb::TcTile) * (size_t)std::max<long long>(1, tiles_alloc))) ||
         (rc = ENS(f_rowmeta, sizeof(sb::VisRowMeta) * (T + 256))))
       return rc;
@@ -1279,6 +1301,17 @@ int sb200_tracker::predict(int32_t n_scenes, const uint64_t* scene_ids, const in
     CU(cudaStreamCreateWithPriority(&prep_stream, cudaStreamNonBlocking, lo));
     CU(cudaEventCreateWithFlags(&ev_prep_done, cudaEventDisableTiming));
     CU(cudaEventCreateWithFlags(&ev_inputs, cudaEventDisableTiming));
+  }
+  if (q.fp8 && f.in_feat) {
+    f.skip_bf16 = true;
+    if (!bf16_stale_all && bf16_log_n + total <= kBf16LogCap) {
+      f.bf16_log = b_bf16log.as<int>() + bf16_log_n;
+      bf16_log_n += total;
+    } else {
+      bf16_stale_all = true;
+    }
+  } else if (tc.use_tc && !tc.fp8) {   // the BF16 screen or the dense path reads the BF16 rows
+    if ((rc = regen_bf16())) return rc;
   }
   const bool prep_ahead = !derive_own && total > 0;
   // (the tables go to the side stream: on the work stream they would move the next frame's preparation squarely under the
@@ -2305,6 +2338,7 @@ uint64_t read_id_counter(sb200_tracker* t, int* rc) {
 
 // Writes the blob of `slots` (type kBlobScenes) or of the whole tracker to `dst` (host, or device memory on any device).
 int save_blob(sb200_tracker* t, uint32_t type, const std::vector<int>& slots, void* dst, size_t cap, size_t* bytes) {
+  if (int rc = t->regen_bf16()) return rc;   // the blob carries the BF16 rows
   BlobHeader h;
   memset(&h, 0, sizeof(h));
   h.magic = kBlobMagic; h.version = kBlobVersion; h.type = type;

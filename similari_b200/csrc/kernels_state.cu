@@ -308,12 +308,14 @@ __global__ void __launch_bounds__(256) apply_kernel(Params p, TrackStore ts, Fra
 // epoch + max_idle < that epoch, and no block changes hands in between (blocks are freed on the host, after a drain, and
 // reused only by frames enqueued after it).  The two sets are disjoint.
 // T: element type of the request's feature column; a 2-byte row is widened to f32 where it is loaded, and the arena row,
-// its BF16 and e4m3 copies and the history row are written from the widened values.
+// its BF16 and e4m3 copies and the history row are written from the widened values.  With d8 <= 512 (the only rows with
+// an e4m3 copy) the vector paths hold the whole row in registers after their first round: the e4m3 copy comes from there.
 template <class T>
 __global__ void feat_store_kernel(Params p, TrackStore ts, Frame f) {
   int w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   int lane = threadIdx.x & 31;
   if (w >= f.total) return;
+  if (lane == 0 && f.bf16_log) f.bf16_log[w] = f.feat_dst[f.det0 + w];
   w += f.det0;
   const int dst = f.feat_dst[w];
   const int hdst = f.hist_dst ? f.hist_dst[w] : -1;
@@ -321,7 +323,9 @@ __global__ void feat_store_kernel(Params p, TrackStore ts, Frame f) {
   const T* src = static_cast<const T*>(f.in_feat) + (size_t)w * p.feature_dim;
   float* d = ts.feat + (size_t)max(dst, 0) * p.d8;
   __nv_bfloat16* db = reinterpret_cast<__nv_bfloat16*>(ts.feat_bf16) + (size_t)max(dst, 0) * p.d8;
+  const bool wb = dst >= 0 && !f.skip_bf16;
   float* hd = hdst >= 0 ? ts.hrows + (size_t)hdst * p.d8 : nullptr;
+  unsigned char* d8p = dst >= 0 && ts.feat_fp8 ? ts.feat_fp8 + (size_t)dst * fp8_pitch(p.d8) : nullptr;
   if constexpr (!std::is_same<T, float>::value) {
     if (p.feature_dim == p.d8 && (reinterpret_cast<uintptr_t>(f.in_feat) & 15) == 0) {
       // rows are 16-byte multiples: one 16-byte load is 8 elements, four in flight per lane
@@ -330,8 +334,8 @@ __global__ void feat_store_kernel(Params p, TrackStore ts, Frame f) {
       float4* h4 = reinterpret_cast<float4*>(hd);
       uint4* b8 = reinterpret_cast<uint4*>(db);
       const int n8 = p.d8 >> 3;
+      uint4 r[4];
       for (int i0 = 0; i0 < n8; i0 += 128) {
-        uint4 r[4];
 #pragma unroll
         for (int u = 0; u < 4; ++u) {
           const int i = i0 + u * 32 + lane;
@@ -347,6 +351,8 @@ __global__ void feat_store_kernel(Params p, TrackStore ts, Frame f) {
             if (dst >= 0) {
               d4[2 * i] = lo;
               d4[2 * i + 1] = hi;
+            }
+            if (wb) {
               __nv_bfloat162 bb[4];
 #pragma unroll
               for (int l = 0; l < 4; ++l) bb[l] = __floats2bfloat162_rn(x[2 * l], x[2 * l + 1]);
@@ -356,14 +362,29 @@ __global__ void feat_store_kernel(Params p, TrackStore ts, Frame f) {
           }
         }
       }
+      if (d8p) {   // n8 <= 64: blocks lane and lane + 32 of the row are r[0] and r[1]
+        float x[2][8];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          if (h * 32 + lane < n8) feat_widen8(r[h], src, x[h]);
+          else
+#pragma unroll
+            for (int l = 0; l < 8; ++l) x[h][l] = 0.0f;
+        }
+        const float s = fp8_row_store(x, p.d8, d8p);
+        if (lane == 0) ts.fscale[dst] = s;
+      }
     } else {
       for (int i = lane; i < p.d8; i += 32) {
         float x = i < p.feature_dim ? feat_elem(src, i) : 0.0f;   // Feature::from_vec zero-pads to the 8-lane multiple
-        if (dst >= 0) {
-          d[i] = x;
-          db[i] = __float2bfloat16_rn(x);
-        }
+        if (dst >= 0) d[i] = x;
+        if (wb) db[i] = __float2bfloat16_rn(x);
         if (hd) hd[i] = x;
+      }
+      if (d8p) {   // from the f32 row this warp has just written
+        __syncwarp();
+        const float s = fp8_row_from(d, p.d8, p.d8, d8p);
+        if (lane == 0) ts.fscale[dst] = s;
       }
     }
   } else if (p.feature_dim == p.d8 && (reinterpret_cast<uintptr_t>(f.in_feat) & 15) == 0) {
@@ -373,8 +394,8 @@ __global__ void feat_store_kernel(Params p, TrackStore ts, Frame f) {
     float4* h4 = reinterpret_cast<float4*>(hd);
     uint2* b4 = reinterpret_cast<uint2*>(db);
     const int n4 = p.d8 >> 2;
+    float4 v[4];
     for (int i0 = 0; i0 < n4; i0 += 128) {
-      float4 v[4];
 #pragma unroll
       for (int u = 0; u < 4; ++u) {
         const int i = i0 + u * 32 + lane;
@@ -384,8 +405,8 @@ __global__ void feat_store_kernel(Params p, TrackStore ts, Frame f) {
       for (int u = 0; u < 4; ++u) {
         const int i = i0 + u * 32 + lane;
         if (i < n4) {
-          if (dst >= 0) {
-            d4[i] = v[u];
+          if (dst >= 0) d4[i] = v[u];
+          if (wb) {
             const __nv_bfloat162 lo = __floats2bfloat162_rn(v[u].x, v[u].y), hi = __floats2bfloat162_rn(v[u].z, v[u].w);
             uint2 pk;
             pk.x = *reinterpret_cast<const unsigned int*>(&lo);
@@ -396,23 +417,68 @@ __global__ void feat_store_kernel(Params p, TrackStore ts, Frame f) {
         }
       }
     }
+    if (d8p) {   // n4 <= 128: element 4 i of the row is v[i / 32] of lane i % 32
+      float amax = 0.0f;   // the maximum of fp8_row_store (NaN does not enter it)
+#pragma unroll
+      for (int u = 0; u < 4; ++u)
+        if (u * 32 + lane < n4)
+          amax = fmaxf(amax, fmaxf(fmaxf(fabsf(v[u].x), fabsf(v[u].y)), fmaxf(fabsf(v[u].z), fabsf(v[u].w))));
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+      const float s = fp8_row_scale(amax);
+      unsigned int* o4 = reinterpret_cast<unsigned int*>(d8p);
+#pragma unroll
+      for (int u = 0; u < 4; ++u) {
+        const int i = u * 32 + lane;
+        if (i < n4) o4[i] = fp8_pack4(v[u].x, v[u].y, v[u].z, v[u].w, s);
+      }
+      if (lane == 0) ts.fscale[dst] = s;
+    }
   } else {
     for (int i = lane; i < p.d8; i += 32) {
       float x = i < p.feature_dim ? src[i] : 0.0f;   // Feature::from_vec zero-pads to the 8-lane multiple
-      if (dst >= 0) {
-        d[i] = x;
-        db[i] = __float2bfloat16_rn(x);
-      }
+      if (dst >= 0) d[i] = x;
+      if (wb) db[i] = __float2bfloat16_rn(x);
       if (hd) hd[i] = x;
     }
-  }
-  if (dst >= 0 && ts.feat_fp8) {
-    // the e4m3 copy (d8 <= 512) from the f32 row this warp has just written
-    __syncwarp();
-    const float s = fp8_row_from(d, p.d8, p.d8, ts.feat_fp8 + (size_t)dst * fp8_pitch(p.d8));
-    if (lane == 0) ts.fscale[dst] = s;
+    if (d8p) {   // from the f32 row this warp has just written
+      __syncwarp();
+      const float s = fp8_row_from(d, p.d8, p.d8, d8p);
+      if (lane == 0) ts.fscale[dst] = s;
+    }
   }
   if (lane == 0 && dst >= 0) ts.fnorm2[dst] = f.c_norm2[w];
+}
+
+__global__ void bf16_regen_kernel(TrackStore ts, int d8, int K, const int* __restrict__ rows, long long n, int n_slots) {
+  const int lane = threadIdx.x & 31, wpb = blockDim.x >> 5;
+  auto convert = [&](long long r) {
+    const float4* s4 = reinterpret_cast<const float4*>(ts.feat + (size_t)r * d8);
+    uint2* b4 = reinterpret_cast<uint2*>(reinterpret_cast<__nv_bfloat16*>(ts.feat_bf16) + (size_t)r * d8);
+    for (int k = lane; k < (d8 >> 2); k += 32) {
+      const float4 v = s4[k];
+      const __nv_bfloat162 lo = __floats2bfloat162_rn(v.x, v.y), hi = __floats2bfloat162_rn(v.z, v.w);
+      b4[k] = make_uint2(*reinterpret_cast<const unsigned int*>(&lo), *reinterpret_cast<const unsigned int*>(&hi));
+    }
+  };
+  const long long w0 = (long long)blockIdx.x * wpb + (threadIdx.x >> 5), ws = (long long)gridDim.x * wpb;
+  if (rows) {
+    for (long long i = w0; i < n; i += ws)
+      if (rows[i] >= 0) convert(rows[i]);
+    return;
+  }
+  for (int s = blockIdx.y; s < n_slots; s += gridDim.y) {
+    const long long r0 = (long long)s * ts.track_cap * K, nr = (long long)ts.arena_top[s] * K;
+    for (long long i = w0; i < nr; i += ws) convert(r0 + i);
+  }
+}
+
+void launch_bf16_regen(const TrackStore& ts, int d8, int K, const int* rows, long long n, int n_slots, cudaStream_t st) {
+  if (rows ? n <= 0 : n_slots <= 0) return;
+  const long long warps = rows ? n : (long long)ts.track_cap * K;   // per slot: an upper bound of its arena rows
+  const dim3 grid((unsigned)std::min<long long>((warps + 7) / 8, 2048), rows ? 1u : (unsigned)std::min(n_slots, 65535));
+  bf16_regen_kernel<<<grid, 256, 0, st>>>(ts, d8, K, rows, n, n_slots);
+  note_launch();
 }
 
 // feature histories of wasted records, one warp per (record, entry)

@@ -81,16 +81,15 @@ __host__ __device__ __forceinline__ float fp8_row_scale(float amax) {
 // bytes per row of the e4m3 copies: d8 rounded up to 16 (the tensor maps need 16-byte row pitches)
 __host__ __device__ __forceinline__ int fp8_pitch(int d8) { return (d8 + 15) & ~15; }
 
-// 8 consecutive values of a row -> their e4m3 bytes of s x (cvt.rn.satfinite.e4m3x2.f32: round to nearest even)
+// 4 consecutive values of a row -> their e4m3 bytes of s x (cvt.rn.satfinite.e4m3x2.f32: round to nearest even)
+__device__ __forceinline__ unsigned int fp8_pack4(float a, float b, float c, float d, float s) {
+  const unsigned int lo = __nv_cvt_float2_to_fp8x2(make_float2(a * s, b * s), __NV_SATFINITE, __NV_E4M3);
+  const unsigned int hi = __nv_cvt_float2_to_fp8x2(make_float2(c * s, d * s), __NV_SATFINITE, __NV_E4M3);
+  return lo | (hi << 16);
+}
+// the same for 8 values
 __device__ __forceinline__ uint2 fp8_pack8(const float* x, float s) {
-  unsigned int w[2];
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    const unsigned int lo = __nv_cvt_float2_to_fp8x2(make_float2(x[4 * h] * s, x[4 * h + 1] * s), __NV_SATFINITE, __NV_E4M3);
-    const unsigned int hi = __nv_cvt_float2_to_fp8x2(make_float2(x[4 * h + 2] * s, x[4 * h + 3] * s), __NV_SATFINITE, __NV_E4M3);
-    w[h] = lo | (hi << 16);
-  }
-  return make_uint2(w[0], w[1]);
+  return make_uint2(fp8_pack4(x[0], x[1], x[2], x[3], s), fp8_pack4(x[4], x[5], x[6], x[7], s));
 }
 // One warp, a row of d8 <= 512 values held as blocks lane and lane + 32 (x[h], zero past the row): writes the e4m3 copy
 // to out (fp8_pitch(d8) bytes) and returns the row's scale.  NaN elements do not enter the maximum; such rows fail
@@ -326,6 +325,11 @@ struct Frame {  // per-request transient device buffers (a request may be proces
   int* new_count;          // [n_scenes] new tracks per scene (written by voting)
   int* status;             // [n_scenes] per-scene status flags (capacity overflow etc.)
   int* feat_dst;           // [total] destination feature row (block*K + phys) or -1
+  // Frames on the e4m3 screen leave the BF16 arena rows unwritten: only the BF16 screen and the dense path read them, and
+  // the tracker converts the skipped rows again, in stream order, before the first frame or blob that does.
+  bool skip_bf16;
+  int* bf16_log;           // [total] with skip_bf16: feat_dst again, this frame's part of the tracker's dirty-row log
+                           // (null: the log is full, every arena row gets converted)
   int* hist_dst;           // [total] destination history row (block*fhist_len + ring slot) or -1 (null: history off)
   int2* app_rank;          // [total] apply phase 1: (scene of the detection, rank among the scene's new tracks)
   int4* app_meta;          // [scenes] apply phase 1: (new tracks of earlier scenes, free blocks, arena top) before the frame
@@ -501,6 +505,9 @@ void launch_apply(const Params& p, const TrackStore& ts, const Frame& f, int n_s
                   unsigned long long id_base, int* d_n_tracks, cudaStream_t st);
 // the kept features of the frame -> the tracks' feature blocks; false when the frame has none (no launch)
 bool launch_feat_store(const Params& p, const TrackStore& ts, const Frame& f, cudaStream_t st);
+// BF16 arena rows again from the f32 rows, converted as feat_store_kernel converts them: the n rows listed in `rows`
+// (-1: none), or with rows == null every row of the blocks [0, arena_top[slot]) of slots [0, n_slots)
+void launch_bf16_regen(const TrackStore& ts, int d8, int K, const int* rows, long long n, int n_slots, cudaStream_t st);
 // stable compaction of wasted tracks; appends them to the wasted buffers
 struct WastedBuf {
   int cap;
