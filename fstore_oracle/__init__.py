@@ -1,0 +1,146 @@
+"""CPU oracle of the feature track store -- TEST INFRASTRUCTURE ONLY.
+
+ctypes binding of ``fstore_oracle/libfstore_oracle.so`` (built from ``feature_store.cpp`` by ``build()``), which calls
+the distance code of ``oracle/liboracle.so``.  It restates the reference's TrackStore for feature-only tracks and
+TopNVoting::winners, and defines the orders the reference leaves to its shards and HashMaps (see feature_store.cpp).
+Only ``tests/``, ``__graft_entry__`` and ``tools/feature_store_bench.py`` import it; ``similari_b200`` never does.
+"""
+from __future__ import annotations
+
+import ctypes as C
+import os
+import subprocess
+
+import numpy as np
+
+import oracle
+
+_HERE = os.path.dirname(os.path.abspath(__file__))
+_SRC = os.path.join(_HERE, "feature_store.cpp")
+_LIB_PATH = os.path.join(_HERE, "libfstore_oracle.so")
+_ORACLE_DIR = os.path.dirname(os.path.abspath(oracle.__file__))
+
+EUCLIDEAN, COSINE = 0, 1
+
+
+def build(force: bool = False) -> str:
+    """Compile libfstore_oracle.so if missing or stale (g++ only; -ffp-contract=off as for liboracle.so)."""
+    base = oracle.build()
+    deps = [_SRC, os.path.join(_ORACLE_DIR, "similari_oracle.h"), base]
+    if force or not os.path.exists(_LIB_PATH) or os.path.getmtime(_LIB_PATH) < max(os.path.getmtime(d) for d in deps):
+        subprocess.check_call([
+            "g++", "-O2", "-std=c++17", "-fPIC", "-ffp-contract=off", "-fno-fast-math", "-Wall", "-Wextra", "-pthread",
+            "-shared", "-o", _LIB_PATH, _SRC, "-L" + _ORACLE_DIR, "-l:liboracle.so", "-Wl,-rpath,$ORIGIN/../oracle"])
+    return _LIB_PATH
+
+
+_lib = None
+
+
+def lib():
+    global _lib
+    if _lib is None:
+        build()
+        L = C.CDLL(_LIB_PATH)
+        vp, i32, i64, f32 = C.c_void_p, C.c_int32, C.c_int64, C.c_float
+        sig = {
+            "ofs_create": (vp, [i32, f32, i32, i32, i32, f32, i32]),
+            "ofs_destroy": (None, [vp]),
+            "ofs_add": (C.c_int, [vp, i32, vp, vp]),
+            "ofs_search": (C.c_int, [vp, i32, vp, vp, vp, vp, vp, vp, i32]),
+            "ofs_associate": (C.c_int, [vp, i32, vp, vp, vp, vp, vp, vp, vp, vp, i32]),
+            "ofs_fetch": (i64, [vp, i32, vp, i32, vp, vp]),
+            "ofs_size": (i64, [vp]),
+            "ofs_ids": (i64, [vp, i64, vp]),
+            "ofs_topn_voting": (C.c_int, [f32, i32, i32, i32, vp, vp, vp, vp, vp, vp]),
+        }
+        for name, (res, args) in sig.items():
+            fn = getattr(L, name)
+            fn.restype = res
+            fn.argtypes = args
+        _lib = L
+    return _lib
+
+
+def _p(a):
+    return a.ctypes.data_as(C.c_void_p) if a is not None else None
+
+
+def topn_voting(topn, max_distance, min_votes, ents):
+    """TopNVoting::winners.  ents: list of (from, to, distance or None).  Returns {query: [(winner, weight), ...]}."""
+    fr = np.array([e[0] for e in ents], dtype=np.uint64)
+    to = np.array([e[1] for e in ents], dtype=np.uint64)
+    fe = np.array([np.nan if e[2] is None else e[2] for e in ents], dtype=np.float32)
+    cap = max(1, len(ents))
+    q, w, wt = np.zeros(cap, np.uint64), np.zeros(cap, np.uint64), np.zeros(cap, np.float64)
+    n = lib().ofs_topn_voting(max_distance, min_votes, topn, len(ents), _p(fr), _p(to), _p(fe), _p(q), _p(w), _p(wt))
+    res = {}
+    for i in range(n):
+        res.setdefault(int(q[i]), []).append((int(w[i]), float(wt[i])))
+    return res
+
+
+class FeatureStore:
+    """The oracle's feature track store; same calls and results as similari_b200.engine.FeatureStore."""
+
+    def __init__(self, metric=EUCLIDEAN, distance_filter=100.0, max_observations=3, feature_dim=256, topn=1,
+                 max_distance=100.0, min_votes=1, threads=1):
+        self._L = lib()
+        self.K, self.D, self.topn, self.threads = int(max_observations), int(feature_dim), int(topn), int(threads)
+        self._h = self._L.ofs_create(metric, distance_filter, self.K, self.D, self.topn, max_distance, min_votes)
+        if not self._h:
+            raise ValueError("invalid feature store options")
+
+    def __del__(self):
+        if getattr(self, "_h", None):
+            self._L.ofs_destroy(self._h)
+            self._h = None
+
+    def add(self, ids, features):
+        ids = np.ascontiguousarray(ids, dtype=np.uint64)
+        f = np.ascontiguousarray(features, dtype=np.float32).reshape(len(ids), self.D)
+        self._L.ofs_add(self._h, len(ids), _p(ids), _p(f))
+
+    def _queries(self, ids, offsets, features):
+        ids = np.ascontiguousarray(ids, dtype=np.uint64)
+        offs = np.ascontiguousarray(offsets, dtype=np.int32)
+        f = np.ascontiguousarray(features, dtype=np.float32).reshape(-1, self.D)
+        q = len(ids)
+        out = {"counts": np.zeros(q, np.int32), "winners": np.zeros((q, self.topn), np.uint64),
+               "weights": np.zeros((q, self.topn), np.float64)}
+        return ids, offs, f, out
+
+    def search(self, ids, offsets, features):
+        ids, offs, f, out = self._queries(ids, offsets, features)
+        rc = self._L.ofs_search(self._h, len(ids), _p(ids), _p(offs), _p(f), _p(out["counts"]), _p(out["winners"]),
+                                _p(out["weights"]), self.threads)
+        if rc:
+            raise ValueError("invalid search request")
+        return out
+
+    def associate(self, ids, offsets, features):
+        ids, offs, f, out = self._queries(ids, offsets, features)
+        out["track_ids"] = np.zeros(len(ids), np.uint64)
+        out["merged"] = np.zeros(len(ids), np.uint8)
+        rc = self._L.ofs_associate(self._h, len(ids), _p(ids), _p(offs), _p(f), _p(out["counts"]),
+                                   _p(out["winners"]), _p(out["weights"]), _p(out["track_ids"]), _p(out["merged"]),
+                                   self.threads)
+        if rc:
+            raise ValueError("invalid associate request")
+        return out
+
+    def fetch(self, ids, remove=False):
+        ids = np.ascontiguousarray(ids, dtype=np.uint64)
+        counts = np.zeros(len(ids), np.int32)
+        feats = np.zeros((len(ids), self.K, self.D), np.float32)
+        self._L.ofs_fetch(self._h, len(ids), _p(ids), int(bool(remove)), _p(counts), _p(feats))
+        return counts, feats
+
+    def size(self):
+        return int(self._L.ofs_size(self._h))
+
+    def ids(self):
+        n = self.size()
+        out = np.zeros(max(1, n), np.uint64)
+        self._L.ofs_ids(self._h, n, _p(out))
+        return out[:n]

@@ -1,0 +1,308 @@
+// feature_store.cpp -- CPU ORACLE of the feature track store (sb200_fstore_*), TEST INFRASTRUCTURE ONLY.
+//
+// A restatement of the reference's TrackStore for the feature-only tracks of benches/feature_tracker.rs and of
+// TopNVoting::winners (src/track/voting/topn.rs:74-138), built on the distance code of oracle/liboracle.so (the scalar /
+// AVX2 restatement of src/distance.rs, reached through its orc_euclidean_blocks / orc_cosine_blocks hooks).  It defines
+// the orders the reference leaves to its shards and HashMaps:
+//   - store order = insertion order; removal is a stable compaction;
+//   - entries are enumerated as (query, stored track in store order, query observation, track observation), oldest
+//     observations first; a group's f64 weight is summed in that order;
+//   - TopN ties (equal weights) go to the group that appeared first, i.e. the lower store position.
+// It is the parity reference of tests/test_gpu_feature_store.py and the timed CPU baseline of
+// tools/feature_store_bench.py; the product never links it.
+#include <algorithm>
+#include <cmath>
+#include <cstdint>
+#include <cstring>
+#include <functional>
+#include <thread>
+#include <unordered_map>
+#include <unordered_set>
+#include <vector>
+
+#include "../oracle/similari_oracle.h"
+
+namespace {
+
+struct Ent {
+  uint64_t from, to;
+  float d;   // NaN == None
+};
+struct Elt {
+  uint64_t query, winner;
+  double weight;
+};
+struct PairHash {
+  size_t operator()(const std::pair<uint64_t, uint64_t>& p) const {
+    return std::hash<uint64_t>()(p.first) * 0x9E3779B97F4A7C15ull ^ std::hash<uint64_t>()(p.second);
+  }
+};
+
+// TopNVoting::winners.  Returns, per query in order of first appearance, its at most `topn` elements, weight
+// descending, equal weights in order of the group's first appearance.
+std::vector<std::vector<Elt>> topn_voting(float max_distance, size_t min_votes, size_t topn, const std::vector<Ent>& ents,
+                                          std::vector<uint64_t>* queries) {
+  float max_dist = -1.0f;
+  std::vector<std::pair<std::pair<uint64_t, uint64_t>, std::vector<float>>> groups;
+  std::unordered_map<std::pair<uint64_t, uint64_t>, size_t, PairHash> gidx;
+  for (const Ent& e : ents) {
+    if (std::isnan(e.d)) continue;   // feature_distance None
+    if (max_dist < e.d) max_dist = e.d;
+    if (!(e.d <= max_distance)) continue;
+    const auto key = std::make_pair(e.from, e.to);
+    auto it = gidx.find(key);
+    if (it == gidx.end()) {
+      gidx.emplace(key, groups.size());
+      groups.push_back({key, {e.d}});
+    } else {
+      groups[it->second].second.push_back(e.d);
+    }
+  }
+  std::vector<std::vector<Elt>> res;
+  std::unordered_map<uint64_t, size_t> qidx;
+  for (auto& g : groups) {
+    if (g.second.size() < min_votes) continue;
+    double weight = 0.0;
+    for (float d : g.second) weight += (double)(max_dist - d);
+    auto it = qidx.find(g.first.first);
+    if (it == qidx.end()) {
+      it = qidx.emplace(g.first.first, res.size()).first;
+      res.emplace_back();
+      queries->push_back(g.first.first);
+    }
+    res[it->second].push_back({g.first.first, g.first.second, weight});
+  }
+  for (auto& r : res) {
+    std::stable_sort(r.begin(), r.end(), [](const Elt& a, const Elt& b) { return a.weight > b.weight; });
+    if (r.size() > topn) r.resize(topn);
+  }
+  return res;
+}
+
+void parallel_for(int n, int threads, const std::function<void(int, int)>& fn) {
+  if (threads <= 1 || n <= 1) { fn(0, n); return; }
+  threads = std::min(threads, n);
+  std::vector<std::thread> th;
+  const int chunk = (n + threads - 1) / threads;
+  for (int t = 0; t < threads; ++t) {
+    const int b = t * chunk, e = std::min(n, b + chunk);
+    if (b >= e) break;
+    th.emplace_back(fn, b, e);
+  }
+  for (auto& x : th) x.join();
+}
+
+struct Track {
+  uint64_t id;
+  std::vector<std::vector<float>> obs;   // zero-padded to d8, oldest first
+};
+
+}  // namespace
+
+struct ofs_store {
+  int metric, K, D, d8, topn, min_votes;
+  float filter, max_distance;
+  std::vector<Track> tracks;
+  std::unordered_map<uint64_t, size_t> pos;
+
+  std::vector<float> pad(const float* v) const {
+    std::vector<float> out((size_t)d8, 0.0f);
+    std::memcpy(out.data(), v, sizeof(float) * (size_t)D);
+    return out;
+  }
+  // optimize: keep the newest K in their original order (the bench's reverse / truncate(K) / reverse)
+  void keep_newest(std::vector<std::vector<float>>& o) const {
+    if ((int)o.size() > K) o.erase(o.begin(), o.end() - K);
+  }
+  float metric_of(const float* a, const float* b) const {
+    if (metric == 0) return orc_euclidean_blocks(a, b, d8 / 8);
+    return 1.0f - orc_cosine_blocks(a, b, d8 / 8);
+  }
+  void reindex() {
+    pos.clear();
+    for (size_t i = 0; i < tracks.size(); ++i) pos[tracks[i].id] = i;
+  }
+
+  // TrackBuilder: each observation through add_observation (and optimize), so only the newest K remain
+  std::vector<Track> build_queries(int Q, const uint64_t* ids, const int32_t* offs, const float* feats) const {
+    std::vector<Track> qs((size_t)Q);
+    for (int q = 0; q < Q; ++q) {
+      qs[q].id = ids[q];
+      for (int r = offs[q]; r < offs[q + 1]; ++r) {
+        qs[q].obs.push_back(pad(feats + (size_t)r * D));
+        keep_newest(qs[q].obs);
+      }
+    }
+    return qs;
+  }
+
+  int check(int Q, const uint64_t* ids, const int32_t* offs, bool assoc) const {
+    if (Q < 0) return -1;
+    if (Q == 0) return 0;
+    if (offs[0] != 0) return -1;
+    std::unordered_set<uint64_t> seen;
+    for (int q = 0; q < Q; ++q) {
+      if (offs[q + 1] <= offs[q]) return -1;
+      if (!seen.insert(ids[q]).second) return -1;
+      if (assoc && pos.count(ids[q])) return -1;
+    }
+    return 0;
+  }
+
+  // foreign_track_distances + postprocess_distances (d < filter) + TopNVoting::winners
+  std::vector<std::vector<Elt>> search(const std::vector<Track>& qs, int threads) const {
+    std::vector<std::vector<Ent>> per((size_t)qs.size());
+    parallel_for((int)qs.size(), threads, [&](int b, int e) {
+      for (int q = b; q < e; ++q)
+        for (const Track& t : tracks) {
+          if (t.id == qs[q].id) continue;   // src/track/store.rs:206
+          for (const auto& a : qs[q].obs)
+            for (const auto& o : t.obs) {
+              const float d = metric_of(a.data(), o.data());
+              if (d < filter) per[q].push_back({qs[q].id, t.id, d});
+            }
+        }
+    });
+    std::vector<Ent> ents;
+    for (auto& p : per) ents.insert(ents.end(), p.begin(), p.end());
+    std::vector<uint64_t> order;
+    auto groups = topn_voting(max_distance, (size_t)std::max(min_votes, 0), (size_t)topn, ents, &order);
+    std::unordered_map<uint64_t, size_t> at;
+    for (size_t i = 0; i < order.size(); ++i) at[order[i]] = i;
+    std::vector<std::vector<Elt>> out(qs.size());
+    for (size_t q = 0; q < qs.size(); ++q) {
+      auto it = at.find(qs[q].id);
+      if (it != at.end()) out[q] = groups[it->second];
+    }
+    return out;
+  }
+
+  void write(const std::vector<std::vector<Elt>>& r, int32_t* counts, uint64_t* winners, double* weights) const {
+    for (size_t q = 0; q < r.size(); ++q) {
+      counts[q] = (int32_t)r[q].size();
+      for (int e = 0; e < topn; ++e) {
+        const bool ok = e < (int)r[q].size();
+        winners[q * topn + e] = ok ? r[q][e].winner : 0;
+        weights[q * topn + e] = ok ? r[q][e].weight : 0.0;
+      }
+    }
+  }
+};
+
+extern "C" {
+
+ofs_store* ofs_create(int metric, float distance_filter, int max_observations, int feature_dim, int topn,
+                      float max_distance, int min_votes) {
+  if ((metric != 0 && metric != 1) || max_observations < 1 || feature_dim < 1 || topn < 1) return nullptr;
+  ofs_store* s = new ofs_store();
+  s->metric = metric;
+  s->filter = distance_filter;
+  s->K = max_observations;
+  s->D = feature_dim;
+  s->d8 = (feature_dim + 7) / 8 * 8;
+  s->topn = topn;
+  s->max_distance = max_distance;
+  s->min_votes = min_votes;
+  return s;
+}
+
+void ofs_destroy(ofs_store* s) { delete s; }
+
+// TrackStore::add, src/track/store.rs:530-568, in call order
+int ofs_add(ofs_store* s, int n, const uint64_t* ids, const float* feats) {
+  for (int i = 0; i < n; ++i) {
+    auto it = s->pos.find(ids[i]);
+    if (it == s->pos.end()) {
+      s->pos[ids[i]] = s->tracks.size();
+      s->tracks.push_back({ids[i], {s->pad(feats + (size_t)i * s->D)}});
+    } else {
+      auto& o = s->tracks[it->second].obs;
+      o.push_back(s->pad(feats + (size_t)i * s->D));
+      s->keep_newest(o);
+    }
+  }
+  return 0;
+}
+
+int ofs_search(ofs_store* s, int Q, const uint64_t* ids, const int32_t* offs, const float* feats, int32_t* counts,
+               uint64_t* winners, double* weights, int threads) {
+  if (s->check(Q, ids, offs, false)) return -1;
+  if (Q == 0) return 0;
+  s->write(s->search(s->build_queries(Q, ids, offs, feats), threads), counts, winners, weights);
+  return 0;
+}
+
+// one iteration of benches/feature_tracker.rs: search, then merge_external into results[0].winner_track or add_track
+int ofs_associate(ofs_store* s, int Q, const uint64_t* ids, const int32_t* offs, const float* feats, int32_t* counts,
+                  uint64_t* winners, double* weights, uint64_t* track_ids, uint8_t* merged, int threads) {
+  if (s->check(Q, ids, offs, true)) return -1;
+  if (Q == 0) return 0;
+  auto qs = s->build_queries(Q, ids, offs, feats);
+  const auto r = s->search(qs, threads);
+  s->write(r, counts, winners, weights);
+  for (int q = 0; q < Q; ++q) {
+    if (!r[q].empty()) {
+      // Track::merge (src/track.rs:522-600): extend, then optimize keeps the newest K
+      auto& dst = s->tracks[s->pos.at(r[q][0].winner)].obs;
+      dst.insert(dst.end(), qs[q].obs.begin(), qs[q].obs.end());
+      s->keep_newest(dst);
+      track_ids[q] = r[q][0].winner;
+      merged[q] = 1;
+    } else {
+      s->pos[qs[q].id] = s->tracks.size();
+      s->tracks.push_back(qs[q]);
+      track_ids[q] = qs[q].id;
+      merged[q] = 0;
+    }
+  }
+  return 0;
+}
+
+// fetch_tracks (src/track/store.rs:388-401) when remove != 0, else a read-only lookup; features [n][K][D]
+int64_t ofs_fetch(ofs_store* s, int n, const uint64_t* ids, int remove, int32_t* counts, float* feats) {
+  int64_t found = 0;
+  std::memset(feats, 0, sizeof(float) * (size_t)n * s->K * s->D);
+  for (int i = 0; i < n; ++i) {
+    counts[i] = 0;
+    auto it = s->pos.find(ids[i]);
+    if (it == s->pos.end()) continue;
+    const Track& t = s->tracks[it->second];
+    counts[i] = (int32_t)t.obs.size();
+    for (size_t b = 0; b < t.obs.size(); ++b)
+      std::memcpy(feats + ((size_t)i * s->K + b) * s->D, t.obs[b].data(), sizeof(float) * (size_t)s->D);
+    ++found;
+    if (remove) {
+      s->tracks.erase(s->tracks.begin() + (std::ptrdiff_t)it->second);
+      s->reindex();
+    }
+  }
+  return found;
+}
+
+int64_t ofs_size(ofs_store* s) { return (int64_t)s->tracks.size(); }
+
+int64_t ofs_ids(ofs_store* s, int64_t cap, uint64_t* ids) {
+  for (int64_t i = 0; i < std::min<int64_t>(cap, (int64_t)s->tracks.size()); ++i) ids[i] = s->tracks[i].id;
+  return (int64_t)s->tracks.size();
+}
+
+// TopNVoting::winners on an entry list (feat NaN == None).  Writes n results (query, winner, weight): queries in order
+// of first appearance, each query's results weight descending, equal weights in order of first appearance.
+int ofs_topn_voting(float max_distance, int min_votes, int topn, int n_ent, const uint64_t* from, const uint64_t* to,
+                    const float* feat, uint64_t* out_query, uint64_t* out_winner, double* out_weight) {
+  std::vector<Ent> ents((size_t)n_ent);
+  for (int i = 0; i < n_ent; ++i) ents[i] = {from[i], to[i], feat[i]};
+  std::vector<uint64_t> order;
+  const auto groups = topn_voting(max_distance, (size_t)std::max(min_votes, 0), (size_t)topn, ents, &order);
+  int n = 0;
+  for (const auto& g : groups)
+    for (const Elt& e : g) {
+      out_query[n] = e.query;
+      out_winner[n] = e.winner;
+      out_weight[n] = e.weight;
+      ++n;
+    }
+  return n;
+}
+
+}  // extern "C"

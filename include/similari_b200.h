@@ -407,6 +407,74 @@ int sb200_shard_scatter(sb200_comm* c, int32_t root, const int32_t* det_range, i
 int sb200_shard_gather(sb200_comm* c, int32_t root, const int32_t* det_range, const sb200_predict_out* mine,
                        const sb200_predict_out* all, void* cuda_stream);
 
+/* ---- feature track store: TrackStore (src/track/store.rs) for feature-only tracks, with TopNVoting on top ----
+ * The tracks of benches/feature_tracker.rs: one feature class, no track attributes (compatible is always true, baked is
+ * always Ready), every observation carries a feature.  Each track keeps its newest max_observations (K) observations in
+ * their original order (the bench's optimize: reverse / truncate(K) / reverse).  The store lives on the device.
+ *
+ * Order rules (the reference's shard / HashMap order is replaced by these, which the oracle defines):
+ *   - store order is insertion order; removal (sb200_fstore_fetch with remove) is a stable compaction;
+ *   - the entries of a search are enumerated as (query, stored track in store order, query observation, track
+ *     observation), both observation lists oldest first (cartesian_product(query, track), src/track.rs:618-645); each
+ *     group's f64 weight is summed in that order;
+ *   - TopN results are sorted by weight, descending; equal weights go to the lower store position.
+ * Bounds: topn <= 64, max_observations <= 64, feature_dim <= 8192.  One search / associate call computes a distance
+ * matrix of (query observations taking part) x (stored tracks x max_observations) entries, 4 B each; a call that needs
+ * more than 2^30 of them returns SB200_ERR_CAPACITY before anything runs.
+ * Every rejected call changes nothing.  Host pointers; the caller allocates the outputs.  A handle is single-threaded. */
+#define SB200_FSTORE_MAX_TOPN 64
+#define SB200_FSTORE_MAX_OBS 64
+#define SB200_FSTORE_MAX_DIM 8192
+typedef struct {
+  int32_t metric;           /* SB200_VIS_EUCLIDEAN: euclidean (src/distance.rs:9-19); SB200_VIS_COSINE: 1 - cosine
+                               (src/distance.rs:26-47, as VisualSortMetricType::distance_to_weight maps it) */
+  float distance_filter;    /* postprocess_distances keeps d < distance_filter (strict) */
+  int32_t max_observations; /* K, 1..64 */
+  int32_t feature_dim;      /* D, 1..8192; rows are zero-padded to a multiple of 8 as Feature::from_vec pads */
+  int32_t topn;             /* TopNVoting::new(topn, max_distance, min_votes), src/track/voting/topn.rs:37-44 */
+  float max_distance;
+  int32_t min_votes;
+  int32_t device;
+} sb200_fstore_options;
+typedef struct sb200_fstore sb200_fstore;
+/* TrackStoreBuilder::build + TopNVoting::new.  SB200_ERR_INVALID for an unknown metric or a bound outside the caps above. */
+int sb200_fstore_create(const sb200_fstore_options* opts, sb200_fstore** out);
+void sb200_fstore_destroy(sb200_fstore* s);
+/* TrackStore::add (src/track/store.rs:530-568) for each (ids[i], features[i][D]) in order: an unknown id creates a
+ * track, at the end of the store, with that one observation; a known id appends the observation and keeps the newest K. */
+int sb200_fstore_add(sb200_fstore* s, int32_t n, const uint64_t* ids, const float* features);
+/* foreign_track_distances (src/track/store.rs:429-460, Track::distances src/track.rs:604-652) + TopNVoting::winners
+ * (src/track/voting/topn.rs:74-138).  Queries in CSR form: query q has id query_ids[q] and the observations
+ * features[obs_offsets[q] .. obs_offsets[q+1])[D], oldest first; like a track built by TrackBuilder
+ * (src/track/builder.rs:168-179) only its newest K take part.  Stored tracks with the query's id are skipped
+ * (src/track/store.rs:206).  max_dist is taken over every entry of the call that passed distance_filter (all queries,
+ * also entries above max_distance and entries of groups short of min_votes, topn.rs:78-95).  Outputs: counts[q] results,
+ * winners[q][topn] their track ids and weights[q][topn] their f64 weights (entries past counts[q] are 0).
+ * SB200_ERR_INVALID for a query without observations or an id twice in the call. */
+int sb200_fstore_search(sb200_fstore* s, int32_t n_queries, const uint64_t* query_ids, const int32_t* obs_offsets,
+                        const float* features, int32_t* counts, uint64_t* winners, double* weights);
+/* One iteration of benches/feature_tracker.rs: search, then, in query order, each query with a result is merged into
+ * its first winner (merge_external -> Track::merge, src/track/store.rs:265-277, 625-691: the query's observations are
+ * appended and the newest K kept), and every other query becomes a new track under its own id at the end of the store
+ * (add_track, src/track/store.rs:510-519).  Queries never see each other within a call.  Outputs as for search, plus
+ * track_ids[q] = the id the query ended up in and merged[q] = 1 when it was merged.  SB200_ERR_INVALID, before anything
+ * changes, as for search and for a query id that is already stored (where the reference returns DuplicateTrackId after
+ * merging the queries before it). */
+int sb200_fstore_associate(sb200_fstore* s, int32_t n_queries, const uint64_t* query_ids, const int32_t* obs_offsets,
+                           const float* features, int32_t* counts, uint64_t* winners, double* weights,
+                           uint64_t* track_ids, uint8_t* merged);
+/* fetch_tracks (src/track/store.rs:388-401) when remove != 0, else a read-only lookup: counts[i] = observations of track
+ * ids[i] (0: not stored), features[i][K][D] = its observations oldest first (rows past counts[i] are 0).  Returns how
+ * many of the ids were found, or a negative status. */
+int64_t sb200_fstore_fetch(sb200_fstore* s, int32_t n, const uint64_t* ids, int32_t remove, int32_t* counts,
+                           float* features);
+/* sum(shard_stats()) (src/track/store.rs:378-384): stored tracks. */
+int64_t sb200_fstore_size(sb200_fstore* s);
+/* Ids of the stored tracks in store order; writes min(cap, size) and returns the size. */
+int64_t sb200_fstore_ids(sb200_fstore* s, int64_t cap, uint64_t* ids);
+/* Device times (ms) of the last search / associate / add call: distances, TopN, apply (0 for a stage that did not run). */
+int sb200_fstore_last_stage_ms(sb200_fstore* s, float* out3);
+
 /* Pinned host memory for callers that want the predict H2D/D2H copies to run at full PCIe speed. */
 void* sb200_host_alloc(size_t bytes);
 void sb200_host_free(void* p);

@@ -72,6 +72,21 @@ class PredictOut(C.Structure):
     ]
 
 
+class FstoreOptions(C.Structure):
+    """sb200_fstore_options."""
+
+    _fields_ = [
+        ("metric", C.c_int32),
+        ("distance_filter", C.c_float),
+        ("max_observations", C.c_int32),
+        ("feature_dim", C.c_int32),
+        ("topn", C.c_int32),
+        ("max_distance", C.c_float),
+        ("min_votes", C.c_int32),
+        ("device", C.c_int32),
+    ]
+
+
 _lib = None
 
 # every symbol include/similari_b200.h declares (checked by tests/test_abi.py without a GPU)
@@ -89,7 +104,9 @@ EXPORTS = [
     "sb200_point_kalman_predict", "sb200_point_kalman_update", "sb200_point_kalman_distance", "sb200_box_vertices",
     "sb200_clip_polygons", "sb200_intersection_areas", "sb200_set_feature_history", "sb200_wasted_visual",
     "sb200_feature_history_pool", "sb200_tracker_save", "sb200_tracker_load", "sb200_scenes_export",
-    "sb200_scenes_import", "sb200_tracker_options", "sb200_set_feature_type",
+    "sb200_scenes_import", "sb200_tracker_options", "sb200_set_feature_type", "sb200_fstore_create",
+    "sb200_fstore_destroy", "sb200_fstore_add", "sb200_fstore_search", "sb200_fstore_associate", "sb200_fstore_fetch",
+    "sb200_fstore_size", "sb200_fstore_ids", "sb200_fstore_last_stage_ms",
 ]
 
 
@@ -171,6 +188,15 @@ def lib():
         "sb200_nms_batch": (i64, [i32, vp, vp, vp, f32, f32, i32, vp, vp, vp, i32]),
         "sb200_nms_batch_device": (C.c_int, [i32, vp, vp, vp, f32, f32, i32, vp, vp, vp, i32, vp]),
         "sb200_own_area_shares": (C.c_int, [vp, i32, vp, i32]),
+        "sb200_fstore_create": (C.c_int, [C.POINTER(FstoreOptions), C.POINTER(vp)]),
+        "sb200_fstore_destroy": (None, [vp]),
+        "sb200_fstore_add": (C.c_int, [vp, i32, vp, vp]),
+        "sb200_fstore_search": (C.c_int, [vp, i32, vp, vp, vp, vp, vp, vp]),
+        "sb200_fstore_associate": (C.c_int, [vp, i32, vp, vp, vp, vp, vp, vp, vp, vp]),
+        "sb200_fstore_fetch": (i64, [vp, i32, vp, i32, vp, vp]),
+        "sb200_fstore_size": (i64, [vp]),
+        "sb200_fstore_ids": (i64, [vp, i64, vp]),
+        "sb200_fstore_last_stage_ms": (C.c_int, [vp, vp]),
         "sb200_host_alloc": (vp, [C.c_size_t]),
         "sb200_host_free": (None, [vp]),
     }

@@ -43,14 +43,6 @@ __global__ void prep_kernel(Params p, Frame f) {
   }
 }
 
-// squared norms of candidate features in the reference's order (cosine, src/distance.rs:36-44):
-// per 8-lane block reduce_add, blocks accumulated sequentially. One warp per detection.
-__device__ __forceinline__ float reduce_add8(const float* t) {
-  float q0 = t[0] + t[4], q1 = t[1] + t[5], q2 = t[2] + t[6], q3 = t[3] + t[7];
-  float d0 = q0 + q2, d1 = q1 + q3;
-  return d0 + d1;
-}
-
 // One warp per detection: squared norm in the reference's order (per 8-lane block reduce_add, blocks accumulated
 // sequentially) and, when the tensor-core screen will run, the BF16 or the e4m3 operand copy of the row (f.c_bf16 /
 // f.c_fp8, whichever the frame's screen reads) -- the feature row is read from HBM once for all.  T: element type of the request's feature column (f32, or a 2-byte type widened on load,

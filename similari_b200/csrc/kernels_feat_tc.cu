@@ -566,11 +566,6 @@ vis_screen_sa_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_cons
 
 // ------------------------------------------------------------------------------------------------ refine kernel
 // One warp per surviving pair: f32 distance in the reference's summation order (src/distance.rs:9-47).
-__device__ __forceinline__ float reduce_add8_tc(const float* t) {
-  float q0 = t[0] + t[4], q1 = t[1] + t[5], q2 = t[2] + t[6], q3 = t[3] + t[7];
-  float d0 = q0 + q2, d1 = q1 + q3;
-  return d0 + d1;
-}
 
 // A warp takes RF_CLAIM pairs at a time.  Phase 1 (cooperative, coalesced): for every pair the lanes compute the 8-element
 // block sums s_blk = reduce_add8(...) of up to 64 blocks and park them in shared memory.  Phase 2: lane p owns pair p and
@@ -615,7 +610,7 @@ __device__ __forceinline__ float refine_block_sum(const float* av, const float* 
     if (COSINE) t[l] = av[l] * bb[l];
     else { const float df = av[l] - bb[l]; t[l] = df * df; }
   }
-  return reduce_add8_tc(t);
+  return reduce_add8(t);
 }
 
 // T: element type of the request's feature column

@@ -1,0 +1,390 @@
+// kernels_fstore.cu -- the feature track store's call: distances, TopN voting, merge / append.
+//
+// Replaces, for feature-only tracks (benches/feature_tracker.rs),
+//   TrackStore::foreign_track_distances -> Track::distances -> euclidean / cosine (src/track/store.rs:199-250,
+//   src/track.rs:604-652, src/distance.rs:9-47) + postprocess_distances (d < distance_filter)
+//   TopNVoting::winners (src/track/voting/topn.rs:74-138)
+//   TrackStore::merge_external / add_track / add (src/track/store.rs:265-277, 510-580, 625-691)
+// Every value that reaches the voting stage is the oracle's f32 bit for bit: --fmad=false, 8-lane blocks reduced by
+// reduce_add8 and accumulated one after another, then sqrt (euclidean) or the quotient by sqrt(|a|^2 |b|^2) (cosine).
+#include <climits>
+
+#include "sb_engine.cuh"
+#include "sb_fstore.cuh"
+
+namespace sb {
+
+namespace {
+
+__device__ __forceinline__ float fs_unkey(int k) { return __int_as_float(k >= 0 ? k : (k ^ 0x7fffffff)); }
+
+// ------------------------------------------------------------------------------------------------ squared norms
+// One warp per row (query rows first, then every stored slot): per 8-lane block reduce_add, blocks accumulated in
+// order (src/distance.rs:36-44).  Lane l takes blocks l, l + 32, ...; lane 0 adds the block sums in block order.
+__global__ void fs_norm_kernel(FsStore s, FsCall c) {
+  const long long w = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  const long long S = (long long)s.live * s.K;
+  if (w >= c.R + S) return;
+  const float* row = w < c.R ? c.rows + (size_t)w * s.d8 : s.feat + (size_t)(w - c.R) * s.d8;
+  const int nblk = s.d8 / 8;
+  float acc = 0.0f;
+  for (int base = 0; base < nblk; base += 32) {
+    const int blk = base + lane;
+    float bs = 0.0f;
+    if (blk < nblk) {
+      const float4 x0 = *reinterpret_cast<const float4*>(row + blk * 8);
+      const float4 x1 = *reinterpret_cast<const float4*>(row + blk * 8 + 4);
+      float t[8] = {x0.x * x0.x, x0.y * x0.y, x0.z * x0.z, x0.w * x0.w, x1.x * x1.x, x1.y * x1.y, x1.z * x1.z, x1.w * x1.w};
+      bs = reduce_add8(t);
+    }
+    const int cntb = min(32, nblk - base);
+    for (int j = 0; j < cntb; ++j) acc = acc + __shfl_sync(0xffffffffu, bs, j);
+  }
+  if (lane == 0) {
+    if (w < c.R) c.qnorm[w] = acc;
+    else c.snorm[w - c.R] = acc;
+  }
+}
+
+// ------------------------------------------------------------------------------------------------ distance tiles
+// 64 query rows x 64 stored rows per CTA of 256 threads; thread (ty, tx) owns rows ty + 16 i and columns tx + 16 j
+// (i, j < 4), so the float4 reads of shared memory are broadcast (A) or conflict-free (B, pitch 36).  Operands are staged
+// kDC 8-lane blocks at a time.  Per pair and block: 8 sub + 8 mul + 7 adds of the tree + 1 accumulate (euclidean), or
+// 8 mul + 8 adds (cosine), all on the FP32 pipe.
+constexpr int kDT = 64;
+constexpr int kDC = 4;
+constexpr int kDP = kDC * 8 + 4;
+
+template <int METRIC>
+__global__ void __launch_bounds__(256) fs_dist_kernel(FsStore s, FsCall c, float filter, int tiles_s) {
+  __shared__ __align__(16) float sa[kDT][kDP];
+  __shared__ __align__(16) float sbm[kDT][kDP];
+  __shared__ int s_max[8];
+  const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
+  const int S = s.live * s.K;
+  const int r0 = (int)(blockIdx.x / tiles_s) * kDT, c0 = (int)(blockIdx.x % tiles_s) * kDT;
+  const int nblk = s.d8 / 8;
+  float acc[4][4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+#pragma unroll
+    for (int j = 0; j < 4; ++j) acc[i][j] = 0.0f;
+
+  for (int b0 = 0; b0 < nblk; b0 += kDC) {
+#pragma unroll
+    for (int k = tid; k < kDT * kDC * 2; k += 256) {
+      const int row = k / (kDC * 2), q4 = k % (kDC * 2), blk = b0 + q4 / 2;
+      float4 va = make_float4(0.f, 0.f, 0.f, 0.f), vb = va;
+      if (blk < nblk) {
+        if (r0 + row < c.R) va = *reinterpret_cast<const float4*>(c.rows + (size_t)(r0 + row) * s.d8 + q4 * 4 + b0 * 8);
+        if (c0 + row < S) vb = *reinterpret_cast<const float4*>(s.feat + (size_t)(c0 + row) * s.d8 + q4 * 4 + b0 * 8);
+      }
+      *reinterpret_cast<float4*>(&sa[row][q4 * 4]) = va;
+      *reinterpret_cast<float4*>(&sbm[row][q4 * 4]) = vb;
+    }
+    __syncthreads();
+    const int nb = min(kDC, nblk - b0);
+    for (int bb = 0; bb < nb; ++bb) {
+      float a[4][8], b[4][8];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const float4 x0 = *reinterpret_cast<const float4*>(&sa[ty + 16 * i][bb * 8]);
+        const float4 x1 = *reinterpret_cast<const float4*>(&sa[ty + 16 * i][bb * 8 + 4]);
+        a[i][0] = x0.x; a[i][1] = x0.y; a[i][2] = x0.z; a[i][3] = x0.w;
+        a[i][4] = x1.x; a[i][5] = x1.y; a[i][6] = x1.z; a[i][7] = x1.w;
+        const float4 y0 = *reinterpret_cast<const float4*>(&sbm[tx + 16 * i][bb * 8]);
+        const float4 y1 = *reinterpret_cast<const float4*>(&sbm[tx + 16 * i][bb * 8 + 4]);
+        b[i][0] = y0.x; b[i][1] = y0.y; b[i][2] = y0.z; b[i][3] = y0.w;
+        b[i][4] = y1.x; b[i][5] = y1.y; b[i][6] = y1.z; b[i][7] = y1.w;
+      }
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          float t[8];
+#pragma unroll
+          for (int l = 0; l < 8; ++l) {
+            if (METRIC == 0) {
+              const float e = a[i][l] - b[j][l];
+              t[l] = e * e;
+            } else {
+              t[l] = a[i][l] * b[j][l];
+            }
+          }
+          acc[i][j] = acc[i][j] + reduce_add8(t);
+        }
+    }
+    __syncthreads();
+  }
+
+  // epilogue: the metric, postprocess_distances (d < filter), the same-id skip and empty ring slots -> NaN
+  int kmax = INT_MIN;
+  const float nan = __int_as_float(0x7fc00000);
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const int col = c0 + tx + 16 * j;
+    if (col >= S) continue;
+    const int t = col / s.K, slot = col - t * s.K;
+    const bool filled = ((slot - s.start[t] + s.K) % s.K) < s.cnt[t];
+    const unsigned long long tid_ = s.ids[t];
+    const float sn = METRIC == 1 ? c.snorm[col] : 0.0f;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int row = r0 + ty + 16 * i;
+      if (row >= c.R) continue;
+      float d;
+      if (METRIC == 0) d = sqrtf(acc[i][j]);
+      else d = 1.0f - acc[i][j] / sqrtf(c.qnorm[row] * sn);
+      const bool keep = filled && c.qid[c.row_q[row]] != tid_ && d < filter;
+      c.dist[(size_t)row * S + col] = keep ? d : nan;
+      if (keep) kmax = max(kmax, fs_key(d));
+    }
+  }
+  kmax = __reduce_max_sync(0xffffffffu, kmax);
+  if ((tid & 31) == 0) s_max[tid >> 5] = kmax;
+  __syncthreads();
+  if (tid == 0) {
+    int m = s_max[0];
+    for (int w = 1; w < 8; ++w) m = max(m, s_max[w]);
+    if (m != INT_MIN) atomicMax(c.maxkey, m);
+  }
+}
+
+// ------------------------------------------------------------------------------------------------ TopN
+// One CTA per query; thread t takes stored tracks t, t + 256, ...  A track's group = its entries with d <= max_distance
+// in entry order (query observation outer, track observation inner, both oldest first); its weight is the sum of
+// (max_dist - d) computed in f32 and widened to f64 (topn.rs:96-108).  The CTA keeps the best `topn` (weight descending,
+// store position ascending) in shared memory; each round only the candidates that beat its last entry are ranked in.
+constexpr int kTopnThreads = 256;
+
+__device__ __forceinline__ bool fs_better(double wa, int pa, double wb, int pb) {
+  return wa > wb || (wa == wb && pa < pb);
+}
+
+__global__ void __launch_bounds__(kTopnThreads) fs_topn_kernel(FsStore s, FsCall c, float max_distance, int min_votes,
+                                                                int topn, int want_dest) {
+  __shared__ double l_w[kFsMaxTopn], n_w[kFsMaxTopn], b_w[kTopnThreads];
+  __shared__ int l_p[kFsMaxTopn], n_p[kFsMaxTopn], b_p[kTopnThreads];
+  __shared__ int s_nb;
+  const int q = blockIdx.x, tid = threadIdx.x;
+  const float maxd = fs_unkey(*c.maxkey);
+  const unsigned long long qid = c.qid[q];
+  const int a0 = c.qoff[q], na = c.qoff[q + 1] - a0;
+  const int K = s.K;
+  const size_t S = (size_t)s.live * K;
+  const int need = max(1, min_votes);
+  int nl = 0;
+  for (int base = 0; base < s.live; base += kTopnThreads) {
+    const int t = base + tid;
+    bool have = false;
+    double w = 0.0;
+    if (t < s.live && s.ids[t] != qid) {
+      const int n = s.cnt[t], st = s.start[t];
+      int votes = 0;
+      for (int a = 0; a < na; ++a) {
+        const float* dr = c.dist + (size_t)(a0 + a) * S + (size_t)t * K;
+        int slot = st;
+        for (int b = 0; b < n; ++b) {
+          const float d = dr[slot];
+          if (d <= max_distance) {   // false for NaN: dropped entries
+            ++votes;
+            w = w + (double)(maxd - d);
+          }
+          slot = slot + 1 == K ? 0 : slot + 1;
+        }
+      }
+      have = votes >= need;
+    }
+    if (tid == 0) s_nb = 0;
+    __syncthreads();
+    if (have && (nl < topn || fs_better(w, t, l_w[nl - 1], l_p[nl - 1]))) {
+      const int k = atomicAdd(&s_nb, 1);
+      b_w[k] = w;
+      b_p[k] = t;
+    }
+    __syncthreads();
+    const int nb = s_nb;
+    if (nb > 0) {
+      const int m = nl + nb;
+      for (int e = tid; e < m; e += kTopnThreads) {
+        const double we = e < nl ? l_w[e] : b_w[e - nl];
+        const int pe = e < nl ? l_p[e] : b_p[e - nl];
+        int rank = 0;
+        for (int f = 0; f < m; ++f) {
+          const double wf = f < nl ? l_w[f] : b_w[f - nl];
+          const int pf = f < nl ? l_p[f] : b_p[f - nl];
+          rank += fs_better(wf, pf, we, pe) ? 1 : 0;
+        }
+        if (rank < topn) { n_w[rank] = we; n_p[rank] = pe; }
+      }
+      __syncthreads();
+      nl = min(topn, m);
+      for (int e = tid; e < nl; e += kTopnThreads) { l_w[e] = n_w[e]; l_p[e] = n_p[e]; }
+    }
+    __syncthreads();
+  }
+  for (int e = tid; e < topn; e += kTopnThreads) {
+    c.out_pos[(size_t)q * topn + e] = e < nl ? l_p[e] : -1;
+    c.out_w[(size_t)q * topn + e] = e < nl ? l_w[e] : 0.0;
+  }
+  if (tid == 0) {
+    c.out_cnt[q] = nl;
+    if (want_dest) c.dest[q] = nl > 0 ? l_p[0] : -1;
+  }
+}
+
+// ------------------------------------------------------------------------------------------------ apply
+// Plan (one CTA, items in order): item q goes to position p = dest[q] (a stored track), or, for dest[q] == -1, to a new
+// track appended after the tracks that exist and the earlier new ones.  Appending the items of one destination one
+// after another and keeping the newest K after each append (Track::merge / add_observation + optimize) keeps the last K
+// of the concatenation; so item q's rows take combined indices c0 .. c0 + n - 1 after the track's old observations and
+// the rows of the earlier items with the same destination, and a row survives when its index is >= total - K.
+constexpr int kOrderThreads = 1024;
+
+__global__ void __launch_bounds__(kOrderThreads) fs_order_kernel(FsStore s, FsCall c) {
+  __shared__ int s_p[kOrderThreads], s_n[kOrderThreads], s_warp[kOrderThreads / 32];
+  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+  int new_base = 0;
+  for (int base = 0; base < c.Q; base += kOrderThreads) {
+    const int q = base + tid;
+    const bool in = q < c.Q;
+    const int d = in ? c.dest[q] : 0;
+    const int n = in ? c.qoff[q + 1] - c.qoff[q] : 0;
+    const bool isnew = in && d < 0;
+    const unsigned int bal = __ballot_sync(0xffffffffu, isnew);
+    if (lane == 0) s_warp[wid] = __popc(bal);
+    __syncthreads();
+    int woff = 0, chunk_new = 0;
+    for (int w = 0; w < kOrderThreads / 32; ++w) {
+      woff += w < wid ? s_warp[w] : 0;
+      chunk_new += s_warp[w];
+    }
+    const int p = isnew ? s.live + new_base + woff + __popc(bal & ((1u << lane) - 1u)) : d;
+    s_p[tid] = in ? p : -1;
+    s_n[tid] = n;
+    __syncthreads();
+    int pre = 0;
+    bool last = true;
+    for (int j = 0; j < kOrderThreads; ++j) {
+      if (s_p[j] != p) continue;
+      if (j < tid) pre += s_n[j];
+      else if (j > tid) last = false;
+    }
+    int run = 0;
+    if (in) {
+      const bool old = p < s.live;
+      run = s.run[p];
+      c.dest[q] = p;
+      c.plan[q] = make_int4(p, (old ? s.cnt[p] : 0) + run + pre, 0, old ? s.start[p] : 0);
+    }
+    __syncthreads();   // every read of run[] of this chunk precedes its update
+    if (in && last) s.run[p] = run + pre + n;
+    __syncthreads();
+    new_base += chunk_new;
+  }
+  for (int q = tid; q < c.Q; q += kOrderThreads) {
+    int4 pl = c.plan[q];
+    pl.z = (pl.x < s.live ? s.cnt[pl.x] : 0) + s.run[pl.x];
+    c.plan[q] = pl;
+  }
+  __syncthreads();   // cnt[] and run[] are read above before they are written below
+  for (int q = tid; q < c.Q; q += kOrderThreads) {
+    const int4 pl = c.plan[q];
+    if (pl.y + (c.qoff[q + 1] - c.qoff[q]) != pl.z) continue;   // not the last item of its destination
+    const int K = s.K, T = pl.z;
+    s.cnt[pl.x] = min(T, K);
+    s.start[pl.x] = (pl.w + max(0, T - K)) % K;
+    s.run[pl.x] = 0;
+    if (pl.x >= s.live) s.ids[pl.x] = c.qid[q];
+  }
+}
+
+// One CTA per item: writes the item's surviving rows into their ring slots.
+__global__ void fs_apply_kernel(FsStore s, FsCall c) {
+  const int q = blockIdx.x;
+  const int4 pl = c.plan[q];
+  const int a0 = c.qoff[q], n = c.qoff[q + 1] - a0, K = s.K, w4 = s.d8 / 4;
+  for (int k = 0; k < n; ++k) {
+    const int ci = pl.y + k;
+    if (ci < pl.z - K) continue;
+    const int slot = (pl.w + ci) % K;
+    const float4* src = reinterpret_cast<const float4*>(c.rows + (size_t)(a0 + k) * s.d8);
+    float4* dst = reinterpret_cast<float4*>(s.feat + ((size_t)pl.x * K + slot) * s.d8);
+    for (int e = threadIdx.x; e < w4; e += blockDim.x) dst[e] = src[e];
+  }
+}
+
+// ------------------------------------------------------------------------------------------------ fetch / remove
+__global__ void fs_gather_kernel(FsStore s, const int* pos, float* out, int* out_cnt) {
+  const int i = blockIdx.x, p = pos[i], K = s.K, w4 = s.d8 / 4;
+  const int n = p >= 0 ? s.cnt[p] : 0;
+  if (threadIdx.x == 0) out_cnt[i] = n;
+  for (int b = 0; b < K; ++b) {
+    float4* dst = reinterpret_cast<float4*>(out + ((size_t)i * K + b) * s.d8);
+    if (b < n) {
+      const float4* src = reinterpret_cast<const float4*>(s.feat + ((size_t)p * K + (s.start[p] + b) % K) * s.d8);
+      for (int e = threadIdx.x; e < w4; e += blockDim.x) dst[e] = src[e];
+    } else {
+      for (int e = threadIdx.x; e < w4; e += blockDim.x) dst[e] = make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+  }
+}
+
+__global__ void fs_compact_kernel(FsStore src, FsStore dst, const int* from) {
+  const int i = blockIdx.x, p = from[i];
+  const size_t w4 = (size_t)src.K * src.d8 / 4;
+  const float4* a = reinterpret_cast<const float4*>(src.feat + (size_t)p * src.K * src.d8);
+  float4* b = reinterpret_cast<float4*>(dst.feat + (size_t)i * src.K * src.d8);
+  for (size_t e = threadIdx.x; e < w4; e += blockDim.x) b[e] = a[e];
+  if (threadIdx.x == 0) {
+    dst.cnt[i] = src.cnt[p];
+    dst.start[i] = src.start[p];
+    dst.ids[i] = src.ids[p];
+  }
+}
+
+}  // namespace
+
+void fs_launch_dist(int metric, float filter, const FsStore& s, const FsCall& c, cudaStream_t st) {
+  const long long S = (long long)s.live * s.K;
+  if (c.R == 0 || S == 0) return;
+  if (metric == 1) {
+    const long long warps = c.R + S;
+    fs_norm_kernel<<<(unsigned)((warps * 32 + 255) / 256), 256, 0, st>>>(s, c);
+    note_launch();
+  }
+  const int tiles_s = (int)((S + kDT - 1) / kDT), tiles_r = (c.R + kDT - 1) / kDT;
+  const unsigned grid = (unsigned)((long long)tiles_s * tiles_r);
+  if (metric == 0) fs_dist_kernel<0><<<grid, 256, 0, st>>>(s, c, filter, tiles_s);
+  else fs_dist_kernel<1><<<grid, 256, 0, st>>>(s, c, filter, tiles_s);
+  note_launch();
+}
+
+void fs_launch_topn(float max_distance, int min_votes, int topn, bool want_dest, const FsStore& s, const FsCall& c,
+                    cudaStream_t st) {
+  if (c.Q == 0) return;
+  fs_topn_kernel<<<c.Q, kTopnThreads, 0, st>>>(s, c, max_distance, min_votes, topn, want_dest ? 1 : 0);
+  note_launch();
+}
+
+void fs_launch_apply(const FsStore& s, const FsCall& c, cudaStream_t st) {
+  if (c.Q == 0) return;
+  fs_order_kernel<<<1, kOrderThreads, 0, st>>>(s, c);
+  fs_apply_kernel<<<c.Q, 128, 0, st>>>(s, c);
+  note_launch(2);
+}
+
+void fs_launch_gather(const FsStore& s, const int* pos, int n, float* out, int* out_cnt, cudaStream_t st) {
+  if (n == 0) return;
+  fs_gather_kernel<<<n, 128, 0, st>>>(s, pos, out, out_cnt);
+  note_launch();
+}
+
+void fs_launch_compact(const FsStore& src, const FsStore& dst, const int* from, int n, cudaStream_t st) {
+  if (n == 0) return;
+  fs_compact_kernel<<<n, 128, 0, st>>>(src, dst, from);
+  note_launch();
+}
+
+}  // namespace sb

@@ -1,0 +1,63 @@
+// sb_fstore.cuh -- device side of the feature track store (csrc/kernels_fstore.cu), shared with its host side
+// (csrc/fstore.cu).  The store is the reference's TrackStore specialised to feature-only tracks: one feature class, no
+// track attributes, the newest `max_observations` (K) observations of each track (src/track/store.rs,
+// benches/feature_tracker.rs).
+#pragma once
+#include <cuda_runtime.h>
+#include <stdint.h>
+#include <string.h>
+
+namespace sb {
+
+constexpr int kFsMaxTopn = 64;
+constexpr int kFsMaxObs = 64;
+constexpr int kFsMaxDim = 8192;
+constexpr long long kFsMaxPairs = 1LL << 30;   // observation pairs of one call's distance matrix (4 B each)
+
+// The store's device columns, in store order (insertion order; removal is a stable compaction).  Observation j (oldest
+// first) of track t lives in ring slot (start[t] + j) % K of feat[t][.][.]; rows are zero-padded from D to d8 as
+// Feature::from_vec pads (src/track/utils.rs:45-71).
+struct FsStore {
+  float* feat;                // [cap][K][d8]
+  int* cnt;                   // [cap] observations held (1..K)
+  int* start;                 // [cap] ring slot of the oldest observation
+  unsigned long long* ids;    // [cap]
+  int* run;                   // [cap] scratch of the apply stage; zero between calls
+  int K, d8, live;
+};
+
+// One request on the device.  Items are the queries of search / associate, or the single observations of add.
+struct FsCall {
+  const float* rows;              // [R][d8] the items' observations (a query's newest K only), item by item
+  const unsigned long long* qid;  // [Q]
+  const int* qoff;                // [Q + 1] row ranges
+  const int* row_q;               // [R] item of each row
+  int* dest;                      // [Q] apply: store position to merge into, or -1 = new track at the end
+  int* maxkey;                    // max_dist of the call, as an order-preserving int (fs_key)
+  int4* plan;                     // [Q] apply: {position, first combined index, combined total, old ring start}
+  float* qnorm;                   // [R] squared norms (cosine)
+  float* snorm;                   // [live * K]
+  float* dist;                    // [R][live * K] NaN == dropped (filtered, empty slot or same id)
+  int* out_cnt;                   // [Q] results of TopN
+  int* out_pos;                   // [Q][topn] store positions
+  double* out_w;                  // [Q][topn]
+  int Q, R;
+};
+
+// order-preserving map of an f32 onto an int (negative values included); NaN never reaches it
+__host__ __device__ __forceinline__ int fs_key(float f) {
+  int b;
+  memcpy(&b, &f, 4);
+  return b >= 0 ? b : (b ^ 0x7fffffff);
+}
+
+void fs_launch_dist(int metric, float filter, const FsStore& s, const FsCall& c, cudaStream_t st);
+void fs_launch_topn(float max_distance, int min_votes, int topn, bool want_dest, const FsStore& s, const FsCall& c,
+                    cudaStream_t st);
+void fs_launch_apply(const FsStore& s, const FsCall& c, cudaStream_t st);
+// out[i][b][.] = observation b (oldest first) of the track at pos[i] (-1: none), out_cnt[i] its count (0 for -1)
+void fs_launch_gather(const FsStore& s, const int* pos, int n, float* out, int* out_cnt, cudaStream_t st);
+// dst[i] = src[from[i]] for the i < n kept tracks (stable compaction into fresh columns)
+void fs_launch_compact(const FsStore& src, const FsStore& dst, const int* from, int n, cudaStream_t st);
+
+}  // namespace sb

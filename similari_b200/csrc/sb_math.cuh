@@ -40,6 +40,13 @@ struct Box {
 };
 
 SB_HD bool is_nan(float v) { return v != v; }
+
+// wide::f32x8::reduce_add of one 8-lane block (src/distance.rs:9-47): lo + hi quads, then pairs, then the last add
+SB_HD float reduce_add8(const float* t) {
+  float q0 = t[0] + t[4], q1 = t[1] + t[5], q2 = t[2] + t[6], q3 = t[3] + t[7];
+  float d0 = q0 + q2, d1 = q1 + q3;
+  return d0 + d1;
+}
 SB_HD float angle_or0(float a) { return is_nan(a) ? 0.0f : a; }
 
 // Universal2DBox::get_radius, src/utils/bbox.rs:157-161

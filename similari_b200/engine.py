@@ -651,3 +651,98 @@ def nms_batch_device(offsets, d_boxes, d_scores, nms_threshold, score_threshold,
                                        0.0 if score_threshold is None else score_threshold,
                                        int(score_threshold is not None), vp(d_keep_idx), vp(d_keep_counts),
                                        vp(d_keep_mask), device, vp(stream)))
+
+
+METRICS = {"euclidean": _lib.VIS_EUCLIDEAN, "cosine": _lib.VIS_COSINE}
+
+
+class FeatureStore:
+    """Device-resident feature track store: the reference's TrackStore for feature-only tracks (one feature class, no
+    track attributes) with TopNVoting(topn, max_distance, min_votes) on top (sb200_fstore_*).  Each track keeps its
+    newest `max_observations` observations.  Queries are given in CSR form: ids[q] with the feature rows
+    features[offsets[q]:offsets[q + 1]], oldest first.  numpy in, numpy out."""
+
+    def __init__(self, metric="euclidean", distance_filter=100.0, max_observations=3, feature_dim=256, topn=1,
+                 max_distance=100.0, min_votes=1, device=0):
+        if metric not in METRICS:
+            raise ValueError(f"metric must be one of {sorted(METRICS)}")
+        self._L = lib()
+        o = _lib.FstoreOptions(METRICS[metric], distance_filter, max_observations, feature_dim, topn, max_distance,
+                               min_votes, device)
+        h = C.c_void_p()
+        check(self._L.sb200_fstore_create(C.byref(o), C.byref(h)))
+        self._h = h
+        self.K, self.D, self.topn = int(max_observations), int(feature_dim), int(topn)
+
+    def close(self):
+        if getattr(self, "_h", None):
+            self._L.sb200_fstore_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def add(self, ids, features):
+        """TrackStore::add for each (ids[i], features[i]) in order."""
+        ids = np.ascontiguousarray(ids, dtype=np.uint64)
+        f = _f32(features).reshape(len(ids), self.D)
+        check(self._L.sb200_fstore_add(self._h, len(ids), ptr(ids), ptr(f)))
+
+    def _queries(self, ids, offsets, features):
+        ids = np.ascontiguousarray(ids, dtype=np.uint64)
+        offs = np.ascontiguousarray(offsets, dtype=np.int32)
+        if len(offs) != len(ids) + 1:
+            raise ValueError("offsets must have len(ids) + 1 entries")
+        f = _f32(features).reshape(-1, self.D)
+        if len(ids) and int(offs[-1]) > len(f):
+            raise ValueError("offsets[-1] exceeds the feature rows")
+        q = len(ids)
+        out = {"counts": np.zeros(q, np.int32), "winners": np.zeros((q, self.topn), np.uint64),
+               "weights": np.zeros((q, self.topn), np.float64)}
+        return ids, offs, f, out
+
+    def search(self, ids, offsets, features):
+        """foreign_track_distances + TopNVoting::winners: counts[q], winners[q][topn] (track ids), weights[q][topn]."""
+        ids, offs, f, out = self._queries(ids, offsets, features)
+        check(self._L.sb200_fstore_search(self._h, len(ids), ptr(ids), ptr(offs), ptr(f), ptr(out["counts"]),
+                                          ptr(out["winners"]), ptr(out["weights"])))
+        return out
+
+    def associate(self, ids, offsets, features):
+        """search, then merge each query with a result into its first winner and add the others as new tracks.  Adds
+        track_ids[q] (where the query ended up) and merged[q] to the search outputs."""
+        ids, offs, f, out = self._queries(ids, offsets, features)
+        out["track_ids"] = np.zeros(len(ids), np.uint64)
+        out["merged"] = np.zeros(len(ids), np.uint8)
+        check(self._L.sb200_fstore_associate(self._h, len(ids), ptr(ids), ptr(offs), ptr(f), ptr(out["counts"]),
+                                             ptr(out["winners"]), ptr(out["weights"]), ptr(out["track_ids"]),
+                                             ptr(out["merged"])))
+        return out
+
+    def fetch(self, ids, remove=False):
+        """(counts[n], features[n][max_observations][feature_dim]) of the tracks `ids`, oldest observation first (count 0:
+        not stored); remove=True takes them out of the store (fetch_tracks)."""
+        ids = np.ascontiguousarray(ids, dtype=np.uint64)
+        counts = np.zeros(len(ids), np.int32)
+        feats = np.zeros((len(ids), self.K, self.D), np.float32)
+        check(self._L.sb200_fstore_fetch(self._h, len(ids), ptr(ids), int(bool(remove)), ptr(counts), ptr(feats)))
+        return counts, feats
+
+    def size(self):
+        return int(check(self._L.sb200_fstore_size(self._h)))
+
+    def ids(self):
+        """Stored track ids in store order."""
+        n = self.size()
+        out = np.zeros(max(1, n), np.uint64)
+        check(self._L.sb200_fstore_ids(self._h, n, ptr(out)))
+        return out[:n]
+
+    def last_stage_ms(self):
+        """Device times (ms) of the last call: distances, TopN, apply."""
+        out = np.zeros(3, np.float32)
+        check(self._L.sb200_fstore_last_stage_ms(self._h, ptr(out)))
+        return out

@@ -147,3 +147,16 @@ def tracker_options_for(name: str, make_options, **over):
         raise KeyError(name)
     kw.update(over)
     return make_options(**kw)
+
+
+class FeatGen:
+    """Seeded counterpart of the reference's FeatGen (src/examples.rs:266-293), which benches/feature_tracker.rs feeds
+    its store with: every call returns a `dim`-long row x + U(-drift, drift), f32."""
+
+    def __init__(self, x: float, dim: int, drift: float, seed: int):
+        self.x, self.dim, self.drift = np.float32(x), int(dim), float(drift)
+        self.rng = np.random.default_rng(seed)
+
+    def next(self) -> np.ndarray:
+        u = self.rng.uniform(-self.drift, self.drift, self.dim).astype(np.float32)
+        return self.x + u
