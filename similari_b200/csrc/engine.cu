@@ -4,8 +4,10 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <array>
 #include <chrono>
 #include <cmath>
+#include <cstddef>
 #include <cstdlib>
 #include <cstdarg>
 #include <cstdio>
@@ -226,13 +228,25 @@ struct sb200_tracker {
   // the call is made (tracks per scene, ids consumed, expired tracks) is joined in by frame_setup_kernel and read back
   // into the host mirrors when the frame is absorbed -- lazily, by a later call, or by sb200_sync().
   static constexpr int kDepth = 3;
+  // What a frame leaves for the host in Pending::h_out: frame_out[n][3] {live tracks, arena blocks, newly expired} and
+  // status[n] per scene, then, at back_offset(n), this record.
+  struct FrameBack {
+    sb::FrameDyn dyn;
+    int dense_scenes;   // scenes the exact SIMT kernels had to take (Frame::dense_cnt)
+    int hpool[2];       // the history pool's {free, handed out} blocks after the sweep (feature history on only)
+    int screen[3];      // screen survivors refined, how many the exact test cut, scenes whose list overflowed
+  };
+  static_assert(offsetof(FrameBack, dense_scenes) == sizeof(sb::FrameDyn) && sizeof(FrameBack) == sizeof(sb::FrameDyn) + 24,
+                "FrameBack: FrameDyn followed by the counters, without padding");
+  static size_t back_offset(int n_scenes) { return ((size_t)n_scenes * 16 + 15) / 16 * 16; }
   struct Pending {
     bool active = false;
     int n_scenes = 0, total = 0;
     std::vector<int> slots, m;
     long long live_ub = 0;     // upper bound of the records this frame's sweep appends to the wasted buffer
     HBuf h_req;                // SceneReq[n_scenes], written by the host, read by frame_setup_kernel over PCIe
-    HBuf h_out;                // frame_out[n][3] | status[n] | FrameDyn, copied back at the end of the frame
+    HBuf h_out;                // frame_out[n][3] | status[n] | FrameBack, copied back at the end of the frame
+    FrameBack* back() const { return reinterpret_cast<FrameBack*>(h_out.as<char>() + back_offset(n_scenes)); }
     cudaEvent_t done = nullptr;
     cudaEvent_t ev[6]{}, ev_k[3]{}, ev_pos[2]{};
     bool tc_timed = false, pos_forked = false;
@@ -295,10 +309,41 @@ struct sb200_tracker {
   long long hpool_free = 0;   // free blocks, as of the last absorbed frame or the last collection (exact likewise)
   long long hpool_pend = 0;   // detections of the frames in flight (each can take at most one block)
   // frame buffers
+  // The input columns of a request.  Each has a staging buffer in both sets (Staging::col), a Frame field the kernels
+  // read it through and a row width; only visual trackers read the feature-side ones, and has_feature only with features.
+  enum InColumn { kBoxes, kFeat, kHasf, kQuality, kCustom, kOwn, kInCols };
+  using InPtrs = std::array<const void*, kInCols>;
+  InPtrs in_ptrs(const void* boxes, const void* feat, const void* hasf, const void* quality, const void* custom,
+                 const void* own) const {
+    if (!P.is_visual) return {boxes, nullptr, nullptr, nullptr, custom, nullptr};
+    return {boxes, feat, feat ? hasf : nullptr, quality, custom, own};
+  }
+  template <auto F> static void to_frame(sb::Frame& f, const void* p) { f.*F = static_cast<std::remove_reference_t<decltype(f.*F)>>(const_cast<void*>(p)); }
+  struct InCol { void (*bind)(sb::Frame&, const void*); size_t w; const char* name; };   // w: bytes per row
+  std::array<InCol, kInCols> in_cols() const {
+    using F = sb::Frame;
+    return {{{to_frame<&F::in_boxes>, 24, "S.boxes"}, {to_frame<&F::in_feat>, (size_t)P.feature_dim * feat_bytes(), "S.feat"},
+             {to_frame<&F::in_hasf>, 1, "S.hasf"}, {to_frame<&F::in_quality>, 4, "S.quality"},
+             {to_frame<&F::in_custom>, 8, "S.custom"}, {to_frame<&F::in_own>, 4, "S.own"}}};
+  }
+  // The output columns (sb200_predict_out), device or staged in o_col.
+  static constexpr int kOutCols = 6;
+  struct OutCol { void* host; void (*bind)(sb::Frame&, const void*); size_t w; const char* name; };
+  static std::array<OutCol, kOutCols> out_cols(const sb200_predict_out& o) {
+    using F = sb::Frame;
+    return {{{o.ids, to_frame<&F::o_ids>, 8, "o_ids"}, {o.epochs, to_frame<&F::o_epochs>, 4, "o_epochs"},
+             {o.lengths, to_frame<&F::o_lengths>, 4, "o_lengths"}, {o.voting_types, to_frame<&F::o_vt>, 1, "o_vt"},
+             {o.predicted_boxes, to_frame<&F::o_pred>, 24, "o_pred"}, {o.observed_boxes, to_frame<&F::o_obs>, 24, "o_obs"}}};
+  }
+  // rows of the per-detection frame buffers and of the staging sets: the request's detections, or what the capacity
+  // hints allow for (n_scenes 0 when the scene count is not known), so that steady-state frames never reallocate
+  long long hint_dets(int n_scenes) const { return (long long)std::max(opts.max_scenes_hint, n_scenes) * opts.max_dets_per_scene_hint; }
+  size_t frame_rows(int total, int n_scenes) const { return (size_t)std::max<long long>(std::max(total, 1), hint_dets(n_scenes)); }
+  int hint_tracks() const { return opts.max_tracks_per_scene_hint > 0 ? track_cap : 0; }   // the store's rows per scene: hint + pipeline room
   // two input staging sets: sb200_prefetch_inputs() fills one while the kernels of the previous frame read the other
   struct Staging {
-    DBuf boxes, feat, hasf, quality, custom, own;
-    const void* key[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};   // the six host columns of the prefetch
+    DBuf col[kInCols];
+    InPtrs key{};   // the host columns of the prefetch
     int total = -1;
     int type = sb::kFeatF32;   // element type of the prefetched features column
     bool pending = false;   // holds a prefetched request that no predict call has consumed yet
@@ -313,7 +358,7 @@ struct sb200_tracker {
       f_status, f_featdst, f_apprank, f_appmeta, f_frameout, f_excl, f_prewin, f_own, f_ownovf, f_dyn, f_ws, f_tmeta, f_rowinfo, f_slabc, f_slabm, f_slabmask,
       f_dscene, f_maxc, f_maxcval, f_drowb, f_dcolb, f_slabk, f_scene_max, f_tiles, f_pairs, f_colmeta, f_colgeo, f_colb, f_colvalid, f_rowmeta, f_poslist, f_counters, f_visval, f_colsb;
   int num_sms = 132;
-  DBuf o_ids, o_epochs, o_lengths, o_vt, o_pred, o_obs;
+  DBuf o_col[kOutCols];
   HBuf h_small;
   bool adapt_dense = false;     // a nominally selective threshold whose survivor lists overflow: treat it as non-selective
   unsigned long long acc_dense_scenes = 0;   // scenes the exact SIMT fallback had to take (over all absorbed frames)
@@ -668,8 +713,596 @@ struct sb200_tracker {
     if (rc) return rc;
     return b.ensure(need);
   }
-  static size_t dyn_offset(int n_scenes) { return ((size_t)n_scenes * 16 + 15) / 16 * 16; }
+  template <class T> int ens(DBuf& b, size_t need, T*& to, const char* name) {   // ... and points `to` at the buffer
+    const int rc = ens(b, need, name);
+    if (rc == 0) to = static_cast<T*>(b.p);
+    return rc;
+  }
   static constexpr int kDenseVoteCap = 8192;   // visual entries per scene of the voting kernel on the dense path (power of two)
+
+  struct Request {   // the arguments of one predict call
+    int n_scenes = 0, total = 0;
+    const uint64_t* scene_ids = nullptr;
+    const int32_t* det_offsets = nullptr;
+    InPtrs in{};   // input columns (device pointers with device_io), null: not given
+    sb200_predict_out out{};
+    bool device_io = false, same_req = false;   // same_req (set by check_request): the previous request's scene list
+  };
+  struct FramePlan {   // what the stages derive from the request and the tracker's state
+    // bounds(): upper bounds of what the device sizes exactly (tracks per scene with frames still in flight)
+    std::vector<int> m_of, nb_ub;
+    int max_m = 0, max_n = 0, max_nb = 0, need_tracks = 0;
+    long long live_ub = 0, pos_total = 0, vis_total = 0, col_total = 0, work = 0;
+    // plan_frame: the frame's own positional elements, the list totals, the buffer rows, the visual path
+    long long pos_ub = 0, posl_total = 0, visl_total = 0;
+    size_t T = 0;
+    int cset = 0, vote_cap = 0, mstep = 0, cstep = 256;
+    bool want_tc = false, want_dense = false, want_fp8 = false;
+    // bind_frame: the staging set, whether a prefetch filled it, the lazy positional stage, derived own-area shares
+    Staging* sin = nullptr;
+    bool prefetched = false, fork = false, derive_own = false;
+  };
+  // takes a frame's share out of the bounds of the frames in flight (absorbed, or rolled back by a failed enqueue)
+  void unbook(Pending& q) {
+    for (int s = 0; s < q.n_scenes; ++s) pending_add[q.slots[s]] -= q.m[s];
+    inflight_live_ub -= q.live_ub;
+    if (fhist_on) hpool_pend -= q.total;
+    q.active = false;
+    pend_count -= 1;
+  }
+  // a CUDA failure while the frame is being enqueued takes it out of the ring again (the context is lost anyway)
+  struct Rollback { sb200_tracker* t; Pending* q; bool armed; ~Rollback() { if (armed) t->unbook(*q); } };
+  // Refuses a malformed request, or one the on-chip assignment solver cannot hold, before any tracker state changes (a
+  // drain is allowed).  Sets rq.total and rq.same_req (the slots of the previous request's scene list are reused).
+  int check_request(Request& rq) {
+    const int n_scenes = rq.n_scenes;
+    const uint64_t* scene_ids = rq.scene_ids;
+    const int32_t* det_offsets = rq.det_offsets;
+    if (n_scenes < 0) return fail(SB200_ERR_INVALID, "n_scenes must be >= 0");
+    if (n_scenes > 0 && (!scene_ids || !det_offsets)) return fail(SB200_ERR_INVALID, "scene_ids / det_offsets are NULL");
+    rq.total = n_scenes > 0 ? det_offsets[n_scenes] : 0;
+    if (n_scenes > 0 && det_offsets[0] != 0) return fail(SB200_ERR_INVALID, "det_offsets[0] must be 0");
+    for (int s = 0; s < n_scenes; ++s)
+      if (det_offsets[s + 1] < det_offsets[s]) return fail(SB200_ERR_INVALID, "det_offsets must be non-decreasing");
+    if (rq.total > 0 && !rq.in[kBoxes]) return fail(SB200_ERR_INVALID, "boxes is NULL");
+    int rc = 0;
+    // frames that have completed since the last call hand over their results; an error of an earlier asynchronous frame
+    // is reported now
+    poll();
+    if (async_rc) { if ((rc = drain("error of an earlier frame"))) return rc; }
+    rq.same_req = (int)last_req_scenes.size() == n_scenes && n_scenes > 0 &&
+                memcmp(last_req_scenes.data(), scene_ids, sizeof(uint64_t) * (size_t)n_scenes) == 0;
+    if (!rq.same_req && n_scenes > 0) {
+      std::unordered_map<uint64_t, int> seen;
+      for (int s = 0; s < n_scenes; ++s)
+        if (!seen.emplace(scene_ids[s], s).second) return fail(SB200_ERR_INVALID, "scene %llu appears twice in one request", (unsigned long long)scene_ids[s]);
+    }
+    // the on-chip assignment solver holds a scene's rows and columns in shared memory
+    int max_m0 = 0, max_n0 = 0;
+    auto fits = [&] {
+      max_m0 = max_n0 = 0;
+      for (int s = 0; s < n_scenes; ++s) {
+        int slot = -1;
+        if (rq.same_req) slot = last_req_slots[s];
+        else { auto it = slot_of.find(scene_ids[s]); if (it != slot_of.end()) slot = it->second; }
+        max_m0 = std::max(max_m0, det_offsets[s + 1] - det_offsets[s]);
+        max_n0 = std::max(max_n0, slot >= 0 ? n_tracks[slot] + pending_add[slot] : 0);
+      }
+      return sb::voting_smem_need(max_m0, max_n0, P.is_visual ? kDenseVoteCap : 0) <= sb::kVotingSmemLimit;
+    };
+    // the bound counts every detection in flight as a new track: get the exact counts first
+    bool ok = fits();
+    if (!ok && pend_count > 0) { if ((rc = drain("assignment solver bound"))) return rc; ok = fits(); }
+    if (!ok) return fail(SB200_ERR_CAPACITY, "scene too large for the on-chip assignment solver (m=%d, n=%d)", max_m0, max_n0);
+    return 0;
+  }
+
+  // upper bounds of everything the device will size exactly (tracks per scene with frames still in flight)
+  void bounds(const Request& rq, FramePlan& pl) const {
+    const int n_scenes = rq.n_scenes, K = P.max_obs;
+    pl.m_of.resize(n_scenes);
+    pl.nb_ub.resize(n_scenes);
+    pl.max_m = pl.max_n = pl.max_nb = pl.need_tracks = 0;
+    pl.live_ub = pl.pos_total = pl.vis_total = pl.col_total = pl.work = 0;
+    for (int s = 0; s < n_scenes; ++s) {
+      const int slot = last_req_slots[s];
+      const int m = rq.det_offsets[s + 1] - rq.det_offsets[s];
+      const int n = n_tracks[slot] + pending_add[slot];
+      pl.m_of[s] = m;
+      pl.nb_ub[s] = P.is_visual ? arena_top[slot] + pending_add[slot] : 0;
+      pl.live_ub += n;
+      pl.pos_total += (long long)m * n;
+      if (P.is_visual) pl.vis_total += (long long)m * n * K;
+      pl.col_total += ((long long)pl.nb_ub[s] * K + 127) / 128 * 128;
+      pl.work += (long long)m * n * K;
+      pl.max_m = std::max(pl.max_m, m);
+      pl.max_n = std::max(pl.max_n, n);
+      pl.max_nb = std::max(pl.max_nb, pl.nb_ub[s]);
+      pl.need_tracks = std::max(pl.need_tracks, n + m);
+    }
+  }
+
+  int reserve_state(const Request& rq, FramePlan& pl) {
+    const int n_scenes = rq.n_scenes, total = rq.total;
+    int rc = 0;
+    bounds(rq, pl);
+    // Capacity has to hold the UPPER BOUNDS: with frames in flight every queued detection counts as a possible new track.
+    // So the store is sized for the pipeline once -- the caller's hint (or what this frame needs) plus the detections of
+    // kDepth frames -- and later frames neither wait for the device nor reallocate.
+    const int pipe_room = kDepth * std::max(pl.max_m, opts.max_dets_per_scene_hint);
+    int hint_s = std::max((int)scene_of_slot.size(), opts.max_scenes_hint);
+    if (hint_s > scene_cap || pl.need_tracks > track_cap) {
+      // the store has to grow: meet the device first (the exact counts are the ones to grow from)
+      if ((rc = drain("track store bound"))) return rc;
+      bounds(rq, pl);
+      // grow generously (a regrow copies the whole feature arena: tens of milliseconds): what is needed now plus the
+      // pipeline's room, and at least half again as much as before
+      const int want_t = std::max(pl.need_tracks, opts.max_tracks_per_scene_hint) + pipe_room;
+      if (hint_s > scene_cap || pl.need_tracks > track_cap)
+        if ((rc = ensure_store(hint_s, std::max(want_t, track_cap + track_cap / 2)))) return rc;
+    }
+    // room for every live track of the frames in flight and of this one in the wasted buffer: the end-of-frame sweep
+    // appends without a host check
+    if (wasted_count + inflight_live_ub + pl.live_ub + 1 > wb.cap) {
+      // the bound that failed is the pipeline's (frames in flight + this one): grow for twice that, or the next frame meets
+      // the same bound again -- after the wait the exact counts alone would fit and nothing would grow
+      const long long pipe_need = inflight_live_ub + pl.live_ub;
+      if ((rc = drain("wasted buffer bound"))) return rc;
+      bounds(rq, pl);
+      // a full ring: kDepth frames in flight plus this one, each bounded by the live tracks plus every detection queued before it
+      const long long dets = std::max<long long>(total, hint_dets(n_scenes));
+      const long long ring_need = (long long)(kDepth + 1) * (pl.live_ub + (long long)kDepth * dets);
+      // and the records already waiting for collection doubled: a caller that collects rarely pays for few regrows
+      // and several times that while it is cheap (<= ~2 GB of records): a regrow drains the ring and reallocates
+      const long long rec_bytes = 72 + (hist_len > 1 ? 48ll * hist_len : 0);
+      const long long base_need = std::max<long long>(ring_need, 2 * pipe_need);
+      const long long mult = std::max<long long>(1, std::min<long long>(8, (2ll << 30) / std::max<long long>(1, base_need * rec_bytes)));
+      if ((rc = ensure_wasted(2 * wasted_count + mult * base_need + 1))) return rc;
+    }
+    // Feature-history pool.  New tracks take free blocks first, so the blocks handed out after this frame are at most
+    //   top + max(0, detections queued since - free)      (top, free: as of the last absorbed frame or collection).
+    // When that bound exceeds the pool, meet the device (the counts become exact) and grow, if needed, to
+    //   top + max(0, f * detections of this frame - free),   f = the frames the bound covered (in flight + this one),
+    // and at least half again as much as before.  So the pool is at most 1.5 x (live + uncollected wasted tracks + the
+    // detections of the frames actually queued together, less the free blocks): a caller that waits for every frame (the
+    // Python API) has f = 1, and only a caller that really queues f frames gets room for f frames of new tracks.
+    if (fhist_on && total > 0 && hpool_top + std::max<long long>(0, hpool_pend + total - hpool_free) > hpool_cap) {
+      const long long frames = pend_count + 1;
+      if ((rc = drain("feature history pool bound"))) return rc;   // hpool_top / hpool_free are exact from here on
+      const long long want = hpool_top + std::max<long long>(0, frames * total - hpool_free);
+      if (want > hpool_cap && (rc = ensure_hpool(std::max<long long>(want, hpool_cap + hpool_cap / 2)))) return rc;
+    }
+    if (!b_idc.p) {
+      if ((rc = b_idc.ensure(8))) return rc;
+      CU(cudaMemsetAsync(b_idc.p, 0, 8, stream));
+    }
+    return 0;
+  }
+
+  // The ring slot's host tables, the visual cost path, the scenes' list slices (into the request table) and the sizes.
+  int plan_frame(const Request& rq, Pending& q, FramePlan& pl) {
+    const int n_scenes = rq.n_scenes, total = rq.total, K = P.max_obs;
+    int rc = 0;
+    if ((rc = q.h_req.ensure(sizeof(sb::SceneReq) * (size_t)n_scenes)) ||
+        (rc = q.h_out.ensure(back_offset(n_scenes) + sizeof(FrameBack))))
+      return rc;
+    // visual cost path of this frame: tensor-core screen + exact refinement for large frames with a selective threshold, the
+    // dense tensor-core weight sums for thresholds that cut nothing, the exact SIMT kernel otherwise (small frames, and as the
+    // device-side fallback of single scenes)
+    if (P.is_visual && rq.in[kFeat] != nullptr && total > 0) {
+      const sb::VisKernel vk = sb::vis_kernel_env();
+      const bool selective = sb::vis_selective(P.visual_kind == SB200_VIS_EUCLIDEAN, P.visual_threshold);
+      const bool big = sb::vis_tc_worth(P.d8, pl.work);
+      const bool dense_ok = P.n_constraints == 0;
+      pl.want_dense = big && dense_ok && (!selective || adapt_dense);
+      pl.want_tc = selective && big && !pl.want_dense;
+      if (vk == sb::kVisSimt) { pl.want_tc = false; pl.want_dense = false; }
+      else if (vk == sb::kVisTc || vk == sb::kVisTc8 || vk == sb::kVisTc16) { pl.want_tc = pl.work > 0; pl.want_dense = false; }
+      else if (vk == sb::kVisDense) { pl.want_dense = pl.work > 0 && dense_ok; pl.want_tc = pl.work > 0 && !pl.want_dense; }
+      // screen precision (d8 <= 512): e4m3 unless a recent e4m3 frame showed its slack to be too wide; tc8 / tc16 force one
+      const bool can8 = pl.want_tc && P.d8 <= sb::kFp8MaxD8 && ts.feat_fp8 != nullptr;
+      const bool forced = vk == sb::kVisTc8 || vk == sb::kVisTc16;
+      pl.want_fp8 = can8 && (forced ? vk == sb::kVisTc8 : fp8_hold == 0);
+      if (!forced && can8 && fp8_hold > 0) fp8_hold -= 1;
+    }
+    pl.vote_cap = pl.want_dense ? kDenseVoteCap : sb::kVoteVisCap;
+    sb::SceneReq* hreq = q.h_req.as<sb::SceneReq>();
+    for (int s = 0; s < n_scenes; ++s) {
+      sb::SceneReq& r = hreq[s];
+      r.slot = last_req_slots[s];
+      r.m = pl.m_of[s];
+      r.det_base = rq.det_offsets[s];
+      r.epoch = epoch[r.slot] + 1;   // EpochDb::next_epoch, src/trackers/epoch_db.rs:35-49 (committed by commit())
+      r.scene_id = rq.scene_ids[s];
+      r.pos_lbase = (int)pl.posl_total;
+      r.pos_lcap = sb::pos_lcap(r.m);
+      pl.posl_total += r.pos_lcap;
+      r.vis_lbase = (int)pl.visl_total;
+      r.vis_lcap = P.is_visual ? sb::vis_lcap(r.m, pl.vote_cap) : 0;
+      pl.visl_total += r.vis_lcap;
+    }
+    // ---- frame buffers (sized once from the capacity hints when given, so steady-state frames never reallocate)
+    pl.T = frame_rows(total, n_scenes);
+    pl.pos_ub = pl.pos_total;
+    const long long hint_pos = hint_dets(n_scenes) * hint_tracks();
+    pl.pos_total = std::max(pl.pos_total, hint_pos);
+    if (P.is_visual) pl.vis_total = std::max(pl.vis_total, hint_pos * K);
+    // candidate-side buffers: the set of this frame (the other one may still be read by the frame in front of it)
+    pl.cset = (int)(frame_seq & 1);
+    if (!pl.want_tc && !pl.want_dense) return 0;
+    pl.mstep = 256;   // a cluster covers two 128-row candidate tiles
+    // dense: column tiles end at block boundaries, a track's observations stay together
+    pl.cstep = pl.want_dense ? (256 / K) * K : sb::vis_screen_ucols(P.d8, num_sms, n_scenes, pl.m_of.data(), pl.nb_ub.data(), K);
+    return 0;
+  }
+
+#define ENS(b, ...) ens(b, __VA_ARGS__, #b)
+  // Grows the frame buffers (each growth waits for the frames in flight) and points the kernels' arguments at them.
+  int bind_frame(const Request& rq, FramePlan& pl, sb::Frame& f, sb::TcArgs& tc) {
+    const int n_scenes = rq.n_scenes, total = rq.total, K = P.max_obs;
+    const size_t T = pl.T;
+    CandBufs& cb = cand[pl.cset];
+    int rc = 0;
+    if ((rc = ENS(cb.box, T * 24, f.c_box)) || (rc = ENS(cb.radius, T * 4, f.c_radius)) || (rc = ENS(cb.conf, T * 4, f.c_conf)) ||
+        (rc = ENS(f_winner, T * 4, f.winner)) || (rc = ENS(f_cvt, T, f.c_vt)) ||
+        (rc = ENS(f_scenes, sizeof(sb::SceneDesc) * n_scenes, f.scenes)) || (rc = ENS(f_newcount, 4 * (size_t)n_scenes, f.new_count)) ||
+        (rc = ENS(f_dyn, sizeof(sb::FrameDyn), f.dyn)) || (rc = ENS(f_apprank, T * 8, f.app_rank)) ||
+        (rc = ENS(f_appmeta, 16 * (size_t)n_scenes, f.app_meta)) || (rc = ENS(f_pos, std::max<size_t>(4, (size_t)pl.pos_total * 4), f.pos)))
+      return rc;
+    if (P.positional_kind == SB200_POS_IOU && (rc = ENS(cb.vert, T * 64, f.c_vert))) return rc;
+    if (P.is_visual) {
+      if (fhist_on && (rc = ENS(f_histdst, T * 4, f.hist_dst))) return rc;
+      if ((rc = ENS(cb.flags, T, f.c_flags)) || (rc = ENS(cb.norm2, T * 4, f.c_norm2)) || (rc = ENS(f_featdst, T * 4, f.feat_dst)) ||
+          (rc = ENS(f_vis, std::max<size_t>(4, (size_t)pl.vis_total * 4), f.vis)) ||
+          (rc = ENS(f_scene_max, 4 * (size_t)n_scenes, f.scene_max)))
+        return rc;
+    }
+    tc.num_sms = num_sms;
+    const int hint_tr = hint_tracks();
+    const long long hs = std::max(opts.max_scenes_hint, n_scenes), visl_alloc = std::max(pl.visl_total, hint_dets(n_scenes) * 64);
+    if (pl.want_tc || pl.want_dense) {
+      tc.use_tc = true;
+      tc.dense = pl.want_dense;
+      const int mstep = pl.mstep, cstep = tc.cstep = pl.cstep;
+      long long tiles_ub = 0, slabs_ub = 0, ws_ub = 0, blk_ub = 0;
+      for (int s = 0; s < n_scenes; ++s) {
+        const long long ct = ((long long)pl.nb_ub[s] * K + cstep - 1) / cstep;
+        tiles_ub += (long long)((pl.m_of[s] + mstep - 1) / mstep) * ct;
+        slabs_ub += ct;
+        ws_ub += ct * (cstep / K) * ((pl.m_of[s] + 127) / 128 * 128);   // blocks padded to whole column tiles
+        blk_ub += ct * (cstep / K);
+      }
+      tc.n_tiles = (int)tiles_ub;   // an upper bound: the list is built on the device
+      // the tile list is sized from the hints like the other frame buffers (the bound grows with the frames in flight: a
+      // list sized for this frame alone would be outgrown, and wait for the device, again and again)
+      const long long hd = std::max(opts.max_dets_per_scene_hint, pl.max_m), ht = std::max(hint_tr, pl.max_nb);
+      long long tiles_alloc = std::max(tiles_ub, hs * ((hd + mstep - 1) / mstep) * ((ht * K + cstep - 1) / cstep + 1));
+      if (f_tiles.bytes > 0 && sizeof(sb::TcTile) * (size_t)tiles_alloc > f_tiles.bytes) tiles_alloc += tiles_alloc / 2;
+      // both operand copies of the candidates whenever the e4m3 screen can run: a switch between the precisions must not
+      // allocate (and synchronise) in the middle of a stream of frames
+      const bool alloc8 = !pl.want_dense && P.d8 <= sb::kFp8MaxD8 && ts.feat_fp8 != nullptr;
+      if (alloc8 && ((rc = ENS(cb.fp8, T * sb::fp8_pitch(P.d8))) || (rc = ENS(cb.scale, T * 4)) || (rc = ENS(b_bf16log, kBf16LogCap * 4))))
+        return rc;
+      if ((rc = ENS(cb.bf16, T * P.d8 * 2)) ||
+          (rc = ENS(f_tiles, sizeof(sb::TcTile) * (size_t)std::max<long long>(1, tiles_alloc), tc.d_tiles)) ||
+          (rc = ENS(f_rowmeta, sizeof(sb::VisRowMeta) * (T + 256), tc.rowmeta)))
+        return rc;
+      tc.max_rows = pl.max_nb * K;
+      tc.d_n_tiles = &f_dyn.as<sb::FrameDyn>()->n_tiles;
+      tc.a_rows = total;
+      tc.b_rows = (long long)scene_cap * track_cap * K;
+      if (!tc.dense) {
+        const size_t cols = (size_t)std::max(pl.col_total, hs * (((long long)hint_tr * K + 127) / 128 * 128));
+        if ((rc = ENS(f_colmeta, sizeof(sb::VisColMeta) * (cols + 256), tc.colmeta)) || (rc = ENS(f_colb, 4 * (cols + 256), tc.colb)) ||
+            (rc = ENS(f_colvalid, (cols + 256) / 8 + 16, tc.colvalid)) ||
+            (rc = ENS(f_colgeo, sizeof(sb::VisColGeo) * std::max<size_t>(1, P.n_constraints > 0 ? cols : 1), tc.colgeo)))
+          return rc;
+        tc.total_cols = (int)pl.col_total;
+        if (alloc8 && P.visual_kind != SB200_VIS_COSINE) {
+          if ((rc = ENS(f_colsb, 4 * (cols + 256)))) return rc;
+          if (pl.want_fp8) tc.colsb = f_colsb.as<float>();
+        }
+        tc.fp8 = pl.want_fp8;
+      } else {
+        // sized from the hints like the other frame buffers, so steady-state frames never reallocate
+        const long long hd0 = std::max(opts.max_dets_per_scene_hint, 0);
+        ws_ub = std::max(ws_ub, hs * (hint_tr + 256) * ((hd0 + 127) / 128 * 128));
+        blk_ub = std::max(blk_ub, hs * (hint_tr + 256));
+        slabs_ub = std::max(slabs_ub, hs * (((long long)hint_tr * K + cstep - 1) / cstep + 1));
+        const size_t slabs = (size_t)std::max<long long>(1, slabs_ub), blks = (size_t)std::max<long long>(1, blk_ub);
+        const size_t visl = (size_t)std::max<long long>(1, visl_alloc);
+        if ((rc = ENS(f_drowb, 4 * 5 * T, tc.d_rowb)) || (rc = ENS(f_dcolb, 4 * blks, tc.d_colb)) ||
+            (rc = ENS(f_slabk, 4 * 256 * slabs, tc.slab_ktf)) || (rc = ENS(f_ws, 4 * (size_t)std::max<long long>(1, ws_ub), tc.ws)) ||
+            (rc = ENS(f_tmeta, sizeof(sb::DenseTrackMeta) * blks, tc.tmeta)) ||
+            (rc = ENS(f_rowinfo, 8 * (size_t)std::max<long long>(1, blk_ub * K), tc.rowinfo)) ||
+            (rc = ENS(f_slabc, 4 * 256 * slabs, tc.slab_colc)) || (rc = ENS(f_slabm, 4 * 256 * slabs, tc.slab_cmax)) ||
+            (rc = ENS(f_slabmask, 2 * 32 * slabs, tc.slab_vmask)) || (rc = ENS(f_dscene, dscene_bytes(n_scenes))) ||
+            (rc = ENS(f_maxc, sizeof(sb::VisPair) * visl, tc.maxc)) || (rc = ENS(f_maxcval, 4 * visl, tc.maxc_val)))
+          return rc;
+        tc.max_blocks = pl.max_nb;
+        tc.n_slabs_ub = (int)slabs_ub;
+        tc.blk_ub = blk_ub;
+        tc.slab_bmask = tc.slab_vmask + (size_t)slabs_ub * 8;
+        carve_dscene(f_dscene.p, n_scenes, tc);
+      }
+    }
+    f.total = total;
+    f.pos_total = pl.pos_ub;
+    f.id_counter = b_idc.as<unsigned long long>();
+    f.id_add = P.is_batch ? (long long)total : -1;
+    f.dense_bad = tc.dense ? tc.dense_bad : nullptr;
+    // dense positional matrices for every scene only on request (SB200_FULL_COSTS: parity of sb200_last_costs)
+    f.pos_dense_all = getenv("SB200_FULL_COSTS") != nullptr;
+    f.feat_type = feat_type;
+    // inputs: the caller's device columns, or a staging set.  A set already filled by sb200_prefetch_inputs() for exactly
+    // these host columns is used as is; otherwise enqueue() issues the H2D copies.  Boxes are always staged.
+    const std::array<InCol, kInCols> ic = in_cols();
+    if (rq.device_io) {
+      for (int c = 0; c < kInCols; ++c) ic[c].bind(f, rq.in[c]);
+    } else {
+      int use = -1;
+      for (int k = 0; k < 2; ++k)
+        if (stg[k].pending && stg[k].total == total && stg[k].type == feat_type && stg[k].key == rq.in)
+          use = k;
+      if (use >= 0) {
+        pl.prefetched = true;
+        stg[use].pending = false;
+        CU(cudaStreamWaitEvent(stream, stg[use].ev, 0));
+      } else {
+        use = stg[0].pending ? 1 : (stg[1].pending ? 0 : 1 - stg_last);
+        stg[use].pending = false;
+      }
+      stg_last = use;
+      Staging& S = stg[use];
+      pl.sin = &S;
+      for (int c = 0; c < kInCols; ++c) {
+        if (c != kBoxes && !(rq.in[c] && total > 0)) continue;
+        // a filled set smaller than this frame's sizing rule (hints changed?): re-copy instead of reallocating
+        if (S.col[c].bytes < T * ic[c].w) pl.prefetched = false;
+        if ((rc = ens(S.col[c], T * ic[c].w, ic[c].name))) return rc;
+        ic[c].bind(f, S.col[c].p);
+      }
+    }
+    f.new_count_all = f.new_count;
+    if ((rc = ENS(f_frameout, sizeof(int) * 3 * (size_t)n_scenes, f.frame_out))) return rc;
+    f.c_bf16 = tc.use_tc && !tc.fp8 ? cb.bf16.p : nullptr;
+    f.c_fp8 = tc.fp8 ? cb.fp8.as<unsigned char>() : nullptr;
+    f.c_scale = tc.fp8 ? cb.scale.as<float>() : nullptr;
+    if ((rc = ENS(f_poslist, sizeof(sb::PosEntry) * (size_t)std::max<long long>(1, std::max(pl.posl_total, hint_dets(n_scenes) * 32)), f.pos_list)) ||
+        (rc = ENS(f_counters, sizeof(int) * counter_ints(n_scenes))))
+      return rc;
+    if (P.is_visual && ((rc = ENS(f_pairs, sizeof(sb::VisPair) * (size_t)std::max<long long>(1, visl_alloc), f.vis_pairs)) ||
+                        (rc = ENS(f_visval, sizeof(float) * (size_t)std::max<long long>(1, visl_alloc), f.vis_val))))
+      return rc;
+    carve_counters(f_counters.as<int>(), n_scenes, f);
+    if (!tc.use_tc || tc.dense) f.screen_cnt = nullptr;   // only the screen counts its survivors
+    // outputs: the caller's device columns, or staged and copied back by enqueue()
+    const std::array<OutCol, kOutCols> oc = out_cols(rq.out);
+    for (int c = 0; c < kOutCols; ++c) {
+      if (!oc[c].host) continue;
+      if (rq.device_io) { oc[c].bind(f, oc[c].host); continue; }
+      if ((rc = ens(o_col[c], T * oc[c].w, oc[c].name))) return rc;
+      oc[c].bind(f, o_col[c].p);
+    }
+    // Visual trackers on the tensor-core path evaluate the positional metric lazily: VisualVoting only consults it for
+    // candidates the visual BestFit pass left undecided, against tracks it did not claim, so the order is
+    // screen -> refine -> BestFit pre-pass (masks) -> culled scan of what is still open -> full voting.
+    // SB200_FULL_COSTS=1 (every pair is evaluated, sb200_last_costs is complete) keeps the plain order.
+    pl.fork = P.is_visual && tc.use_tc && tc.n_tiles > 0 && !f.pos_dense_all;
+    if (pl.fork && ((rc = ENS(cb.decided, T, f.decided)) || (rc = ENS(f_excl, (size_t)scene_cap * track_cap + 16, f.excl)) ||
+                    (rc = ENS(f_prewin, T * 4, f.pre_winner))))
+      return rc;
+    pl.derive_own = P.is_visual && P.use_own_area && f.in_own == nullptr && total > 0;
+    if (pl.derive_own && ((rc = ENS(f_own, T * 4)) || (rc = ENS(f_ownovf, 16 + T * sizeof(int2))))) return rc;
+    return 0;
+  }
+#undef ENS
+
+  // The scenes' epochs, the ring slot and the in-flight bounds; the guard undoes the slot unless enqueue() completes.
+  Rollback commit(const Request& rq, const FramePlan& pl, Pending& q) {
+    const int n_scenes = rq.n_scenes;
+    for (int s = 0; s < n_scenes; ++s) epoch[last_req_slots[s]] += 1;
+    if (rq.in[kFeat] != nullptr && rq.total > 0) seen_features = true;
+    frame_seq += 1;
+    q.active = true;
+    q.n_scenes = n_scenes;
+    q.total = rq.total;
+    q.slots.assign(last_req_slots.begin(), last_req_slots.end());
+    q.m = pl.m_of;
+    q.live_ub = pl.live_ub;
+    q.tc_timed = false;
+    q.pos_forked = false;
+    q.mode = pl.want_dense ? 2 : (pl.want_tc ? 1 : 0);
+    q.fp8 = pl.want_fp8;
+    for (int s = 0; s < n_scenes; ++s) pending_add[last_req_slots[s]] += pl.m_of[s];
+    inflight_live_ub += pl.live_ub;
+    if (fhist_on) hpool_pend += rq.total;
+    pend_count += 1;
+    last_n_scenes = n_scenes;
+    return Rollback{this, &q, true};
+  }
+
+  // The stream joins, input copies, launches (prep -> costs -> voting -> apply -> store / sweep) and the read-back.
+  int enqueue(const Request& rq, const FramePlan& pl, Pending& q, sb::Frame& f, sb::TcArgs& tc) {
+    const int n_scenes = rq.n_scenes, total = rq.total, max_m = pl.max_m, max_n = pl.max_n, cset = pl.cset;
+    sb::Params Pf = P;
+    Pf.vote_vis_cap = pl.vote_cap;
+    if (has_user_stream) {   // everything the caller's stream holds now comes first
+      if (!ev_user_in) { CU(cudaEventCreateWithFlags(&ev_user_in, cudaEventDisableTiming)); CU(cudaEventCreateWithFlags(&ev_user_out, cudaEventDisableTiming)); }
+      CU(cudaEventRecord(ev_user_in, user_stream));
+      CU(cudaStreamWaitEvent(stream, ev_user_in, 0));
+    }
+    if (!rq.device_io && !pl.prefetched && total > 0) {
+      const std::array<InCol, kInCols> ic = in_cols();
+      for (int c = 0; c < kInCols; ++c)
+        if (rq.in[c]) CU(cudaMemcpyAsync(pl.sin->col[c].p, rq.in[c], (size_t)total * ic[c].w, cudaMemcpyHostToDevice, stream));
+    }
+    if (q.fp8 && f.in_feat) {
+      f.skip_bf16 = true;
+      if (!bf16_stale_all && bf16_log_n + total <= kBf16LogCap) {
+        f.bf16_log = b_bf16log.as<int>() + bf16_log_n;
+        bf16_log_n += total;
+      } else {
+        bf16_stale_all = true;
+      }
+    } else if (tc.use_tc && !tc.fp8) {   // the BF16 screen or the dense path reads the BF16 rows
+      if (const int rc = regen_bf16()) return rc;
+    }
+    const bool prep_ahead = !pl.derive_own && total > 0;
+    // The frame's tables (scene descriptors, tile list, frame scalars; counters zeroed) come from one small CTA: with no
+    // own-area derivation (which reads them) it runs on the side stream beside the candidate preparation -- on the work
+    // stream it would move the next frame's preparation under the screen kernel -- and the main stream joins later.
+    const bool side_setup = !pl.derive_own && total > 0;
+    cudaStream_t s_setup = stream;
+    if (side_setup) {
+      CU(cudaEventRecord(ev_fork[0], stream));
+      CU(cudaStreamWaitEvent(side_stream, ev_fork[0], 0));
+      s_setup = side_stream;
+    }
+    sb::launch_frame_setup(P, ts, f, reinterpret_cast<const sb::SceneReq*>(q.h_req.dp), n_scenes, b_ntracks.as<int>(), pl.mstep,
+                           pl.cstep, tc.dense, f_tiles.as<sb::TcTile>(), f_dyn.as<sb::FrameDyn>(), f_counters.as<int>(),
+                           (int)counter_ints(n_scenes), s_setup);
+    tc.max_init_done = 1;   // frame_setup resets scene_max
+    if (side_setup && Pf.is_visual && tc.use_tc && !tc.dense && tc.n_tiles > 0 && max_m > 0 && max_n > 0 && f.in_feat) {
+      // the screen's column metadata reads the tables and the store only: it follows the setup on the side stream
+      sb::launch_vis_colmeta(Pf, ts, f, n_scenes, max_n, tc, side_stream);
+      tc.colmeta_done = 1;
+    }
+    if (side_setup) CU(cudaEventRecord(ev_join, side_stream));
+    CU(cudaEventRecord(q.ev[0], stream));
+    if (pl.derive_own) {
+      // visual_sort/simple_api.rs:110-127: with an own-area threshold and no shares supplied by the caller, the shares come
+      // from the scene's observation boxes (exclusively_owned_areas_normalized_shares)
+      sb::launch_own_area(f, n_scenes, max_m, f.in_boxes, f_own.as<float>(), f_ownovf.as<int>(),
+                          reinterpret_cast<int2*>(f_ownovf.as<char>() + 16), stream);
+      f.in_own = f_own.as<float>();
+    }
+    // Candidate preparation needs the request only (boxes, features): it runs on its own stream as soon as the inputs are there
+    // and the frame that read this set of candidate buffers (two frames back) has ended -- in the steady state under the
+    // tensor-core kernel of the frame in front.  (With derived own-area shares it needs the frame tables: main stream.)
+    if (prep_ahead) {
+      if (has_user_stream) CU(cudaStreamWaitEvent(prep_stream, ev_user_in, 0));
+      if (!rq.device_io) {   // staged inputs: the prefetch copy, or the copies issued above on the work stream
+        if (pl.prefetched) CU(cudaStreamWaitEvent(prep_stream, pl.sin->ev, 0));
+        else { CU(cudaEventRecord(ev_inputs, stream)); CU(cudaStreamWaitEvent(prep_stream, ev_inputs, 0)); }
+      }
+      if (set_busy[cset]) CU(cudaStreamWaitEvent(prep_stream, ev_set_free[cset], 0));
+      // ... and not before the frame in front has left its cost kernels: the preparation is HBM traffic that would slow that
+      // frame's tensor-core screen.  Waiting keeps the tensor-core kernel undisturbed and the step time reproducible.
+      if (cost_done_valid) CU(cudaStreamWaitEvent(prep_stream, ev_cost_done, 0));
+      sb::launch_prep(Pf, f, n_scenes, max_m, prep_stream);
+      CU(cudaEventRecord(ev_prep_done, prep_stream));
+      CU(cudaStreamWaitEvent(stream, ev_prep_done, 0));
+    } else {
+      sb::launch_prep(Pf, f, n_scenes, max_m, stream);
+    }
+    if (side_setup) CU(cudaStreamWaitEvent(stream, ev_join, 0));
+    CU(cudaEventRecord(q.ev[1], stream));
+    sb::TcArgs tcc = tc;
+    if (tc.use_tc && tc.n_tiles > 0) { tcc.ev_screen0 = q.ev_k[0]; tcc.ev_screen1 = q.ev_k[1]; tcc.ev_refine1 = q.ev_k[2]; q.tc_timed = true; }
+    if (!pl.fork) {
+      sb::launch_pos_cost(Pf, ts, f, n_scenes, max_m, max_n, stream);
+      CU(cudaEventRecord(q.ev[2], stream));
+      int vr0 = sb::launch_vis_cost(Pf, ts, f, n_scenes, max_m, max_n, tcc, stream);
+      if (vr0 != 0) return fail(SB200_ERR_CUDA, "visual cost launch failed (%d)", vr0);
+      // scenes whose entry list overflowed vote on the dense matrix: it is filled and scanned for them alone, now
+      if (!f.pos_dense_all) sb::launch_pos_scan_lazy(Pf, ts, f, n_scenes, max_m, max_n, /*pass=*/1, stream);
+    } else {
+      CU(cudaEventRecord(q.ev[2], stream));
+      {
+        int vr0 = sb::launch_vis_cost_a(Pf, ts, f, n_scenes, max_m, max_n, tcc, stream);   // metadata, screen, vis_mode, refinement
+        if (vr0 != 0) return fail(SB200_ERR_CUDA, "visual cost launch failed (%d)", vr0);
+        vr0 = sb::launch_vote_masks(Pf, ts, f, n_scenes, max_m, max_n, stream);            // who is still open positionally
+        if (vr0 != 0) return fail(SB200_ERR_CUDA, "voting launch failed: %s", cudaGetErrorString((cudaError_t)vr0));
+      }
+      CU(cudaEventRecord(q.ev_pos[0], stream));
+      sb::launch_pos_scan_lazy(Pf, ts, f, n_scenes, max_m, max_n, /*pass=*/0, stream);
+      CU(cudaEventRecord(q.ev_pos[1], stream));
+      int vr1 = sb::launch_vis_cost_b(Pf, ts, f, n_scenes, max_m, max_n, tcc, stream);     // final scene mode, dense fallbacks
+      if (vr1 != 0) return fail(SB200_ERR_CUDA, "visual cost launch failed (%d)", vr1);
+      sb::launch_pos_scan_lazy(Pf, ts, f, n_scenes, max_m, max_n, /*pass=*/1, stream);     // scenes that fell back to dense voting
+      q.pos_forked = true;
+    }
+    CU(cudaEventRecord(q.ev[3], stream));
+    CU(cudaEventRecord(ev_cost_done, stream));
+    cost_done_valid = true;
+    int vr = sb::launch_voting(Pf, ts, f, n_scenes, max_m, max_n, stream);
+    if (vr != 0) return fail(SB200_ERR_CUDA, "voting launch failed: %s", cudaGetErrorString((cudaError_t)vr));
+    CU(cudaEventRecord(q.ev[4], stream));
+    sb::launch_apply(Pf, ts, f, n_scenes, max_m, 0ull, b_ntracks.as<int>(), stream);
+    // The sweep (latency-bound, one CTA per scene) and the feature store (HBM-bound) touch disjoint arrays -- a track's feature
+    // block is not moved by the compaction -- so the sweep runs on the side stream beside the store; the frame ends at the join.
+    const bool side_sweep = Pf.is_visual && f.in_feat && total > 0;
+    if (side_sweep) {
+      CU(cudaEventRecord(ev_fork[1], stream));
+      CU(cudaStreamWaitEvent(side_stream, ev_fork[1], 0));
+      sb::launch_frame_sweep(Pf, ts, f, n_scenes, b_ntracks.as<int>(), wb, side_stream);
+      CU(cudaEventRecord(ev_join, side_stream));
+      sb::launch_feat_store(Pf, ts, f, stream);
+      CU(cudaStreamWaitEvent(stream, ev_join, 0));
+    } else {
+      sb::launch_feat_store(Pf, ts, f, stream);
+      sb::launch_frame_sweep(Pf, ts, f, n_scenes, b_ntracks.as<int>(), wb, stream);
+    }
+    CU(cudaEventRecord(q.ev[5], stream));
+    CU(cudaGetLastError());
+
+    if (!rq.device_io && total > 0) {
+      const std::array<OutCol, kOutCols> oc = out_cols(rq.out);
+      for (int c = 0; c < kOutCols; ++c)
+        if (oc[c].host) CU(cudaMemcpyAsync(oc[c].host, o_col[c].p, (size_t)total * oc[c].w, cudaMemcpyDeviceToHost, stream));
+    }
+    FrameBack* back = q.back();
+    sb::Frame cnt{};   // the counters, screen_cnt included on every path (zeros where nothing counts)
+    carve_counters(f_counters.as<int>(), n_scenes, cnt);
+    CU(cudaMemcpyAsync(q.h_out.p, f.frame_out, 12 * (size_t)n_scenes, cudaMemcpyDeviceToHost, stream));
+    CU(cudaMemcpyAsync(q.h_out.as<char>() + 12 * (size_t)n_scenes, cnt.status, 4 * (size_t)n_scenes, cudaMemcpyDeviceToHost, stream));
+    CU(cudaMemcpyAsync(&back->dyn, f_dyn.p, sizeof(back->dyn), cudaMemcpyDeviceToHost, stream));
+    CU(cudaMemcpyAsync(&back->dense_scenes, cnt.dense_cnt, sizeof(back->dense_scenes), cudaMemcpyDeviceToHost, stream));
+    if (fhist_on) CU(cudaMemcpyAsync(back->hpool, ts.hpool, sizeof(back->hpool), cudaMemcpyDeviceToHost, stream));
+    CU(cudaMemcpyAsync(back->screen, cnt.screen_cnt, sizeof(back->screen), cudaMemcpyDeviceToHost, stream));
+    static const bool trace_dense = getenv("SB200_TRACE") != nullptr && atoi(getenv("SB200_TRACE")) >= 2;   // synchronises: level 2 only
+    if (trace_dense && tc.dense && tc.n_tiles > 0) {
+      int hc[8] = {0};
+      CU(cudaMemcpyAsync(hc, tc.dbg_counts, sizeof(hc), cudaMemcpyDeviceToHost, stream));
+      CU(cudaStreamSynchronize(stream));
+      std::vector<int> vcnt((size_t)n_scenes);
+      CU(cudaMemcpy(vcnt.data(), f.vis_cnt, 4 * (size_t)n_scenes, cudaMemcpyDeviceToHost));
+      long long tot = 0; int mx = 0;
+      for (int v : vcnt) { tot += v; mx = std::max(mx, v); }
+      fprintf(stderr, "[sb200] dense frame: fallback reasons threshold %d, max-list overflow %d, no maximum %d; max candidates %d; pairs to refine %lld (largest scene %d)\n",
+              hc[0], hc[1], hc[2], hc[3], tot, mx);
+    }
+    CU(cudaEventRecord(q.done, stream));
+    CU(cudaEventRecord(ev_set_free[cset], stream));   // this frame's candidate buffers may be rewritten after this point
+    set_busy[cset] = true;
+    if (has_user_stream && join_per_call) {   // the caller's stream continues after the frame
+      CU(cudaEventRecord(ev_user_out, stream));
+      CU(cudaStreamWaitEvent(user_stream, ev_user_out, 0));
+    }
+    return 0;
+  }
+
+  // The per-scene counters of a frame (f_counters), zeroed together by frame_setup_kernel: pos_cnt | vis_cnt | scene_mode |
+  // vis_mode | refine_next | status, [n] ints each, then dense_cnt and screen_cnt[3].
+  static size_t counter_ints(int n) { return 6 * (size_t)n + 4; }
+  static void carve_counters(int* c, int n, sb::Frame& f) {
+    using F = sb::Frame;
+    int* F::* const rows[] = {&F::pos_cnt, &F::vis_cnt, &F::scene_mode, &F::vis_mode, &F::refine_next, &F::status, &F::dense_cnt};
+    for (int i = 0; i < 7; ++i) f.*rows[i] = c + (size_t)i * n;
+    f.screen_cnt = f.dense_cnt + 1;
+  }
+  // The per-scene block of the dense path (f_dscene): maxc_cnt | maxc_next | dense_bad | zeros ([n] ints each, zeroed
+  // together), scene_l0 | scene_cmax ([n] floats each), 4 unused ints, dbg_counts[8].
+  static size_t dscene_bytes(int n) { return 4 * 6 * (size_t)n + 128; }
+  static void carve_dscene(void* p, int n, sb::TcArgs& tc) {
+    using A = sb::TcArgs;
+    int* A::* const ints[] = {&A::maxc_cnt, &A::maxc_next, &A::dense_bad, &A::zeros};
+    for (int i = 0; i < 4; ++i) tc.*ints[i] = static_cast<int*>(p) + (size_t)i * n;
+    tc.scene_l0 = reinterpret_cast<float*>(tc.maxc_cnt + 4 * (size_t)n);
+    tc.scene_cmax = tc.scene_l0 + n;
+    tc.dbg_counts = reinterpret_cast<int*>(tc.scene_cmax + n) + 4;
+  }
 };
 
 // Reads back what the oldest frame in flight left for the host: per scene {live tracks, arena blocks, newly expired} and
@@ -694,7 +1327,7 @@ int sb200_tracker::absorb_oldest(bool block) {
   } else {
     const int* h_fo = q.h_out.as<int>();            // [n][3] live tracks, arena blocks, newly expired
     const int* h_status = h_fo + 3 * (size_t)n;
-    const sb::FrameDyn* dyn = reinterpret_cast<const sb::FrameDyn*>(reinterpret_cast<const char*>(q.h_out.p) + dyn_offset(n));
+    const FrameBack& back = *q.back();
     for (int s = 0; s < n; ++s) {
       const int slot = q.slots[s];
       if (h_status[s] && !async_rc) {
@@ -711,15 +1344,14 @@ int sb200_tracker::absorb_oldest(bool block) {
       wasted_count += h_fo[3 * s + 2];
     }
     if (fhist_on) {   // the history pool's counters {free, handed out} as the frame's sweep left them
-      const int* hp = reinterpret_cast<const int*>(reinterpret_cast<const char*>(dyn) + sizeof(sb::FrameDyn) + 2 * sizeof(int));
-      hpool_free = hp[0];
-      hpool_top = hp[1];
+      hpool_free = back.hpool[0];
+      hpool_top = back.hpool[1];
     }
-    acc_units_mn += dyn->units_mn;
-    acc_units_rows += dyn->units_rows;
+    acc_units_mn += back.dyn.units_mn;
+    acc_units_rows += back.dyn.units_rows;
     acc_frames += 1;
     {
-      const int dense_scenes = *reinterpret_cast<const int*>(reinterpret_cast<const char*>(dyn) + sizeof(sb::FrameDyn));
+      const int dense_scenes = back.dense_scenes;
       if (q.mode != 0) acc_dense_scenes += (unsigned long long)dense_scenes;   // mode 0 IS the exact kernel: not a fallback
       last_dense_scenes = dense_scenes;
       // most scenes of a screened frame overflowed their survivor lists: the threshold cuts (almost) nothing, so the
@@ -728,8 +1360,8 @@ int sb200_tracker::absorb_oldest(bool block) {
       if (q.mode == 1 && !q.fp8 && n >= 1 && dense_scenes * 4 > n) adapt_dense = true;
       if (q.mode == 2 && n >= 1 && dense_scenes * 4 > n) adapt_dense = false;
       if (q.mode == 1) {
-        const int* sc = reinterpret_cast<const int*>(reinterpret_cast<const char*>(dyn) + sizeof(sb::FrameDyn) + 16);
-        const unsigned long long kept = (unsigned int)sc[0], cut = (unsigned int)sc[1], ovf = (unsigned int)sc[2];
+        const unsigned long long kept = (unsigned int)back.screen[0], cut = (unsigned int)back.screen[1],
+                                 ovf = (unsigned int)back.screen[2];
         acc_screen[q.fp8 ? 0 : 1] += 1;
         acc_screen[2] += kept;
         acc_screen[3] += cut;
@@ -755,12 +1387,8 @@ int sb200_tracker::absorb_oldest(bool block) {
               q.mode, last_dense_scenes, n, stage_ms[0], stage_ms[1], stage_ms[2], stage_ms[3], stage_ms[4], kernel_ms[0], kernel_ms[1]);
     cudaGetLastError();   // an event that was never recorded in this frame leaves cudaErrorInvalidResourceHandle behind
   }
-  for (int s = 0; s < n; ++s) pending_add[q.slots[s]] -= q.m[s];
-  inflight_live_ub -= q.live_ub;
-  if (fhist_on) hpool_pend -= q.total;
-  q.active = false;
+  unbook(q);
   pend_head = (pend_head + 1) % kDepth;
-  pend_count -= 1;
   return 0;
 }
 
@@ -781,64 +1409,19 @@ int sb200_tracker::drain(const char* why) {
   return 0;
 }
 
-#define ENS(b, ...) ens(b, __VA_ARGS__, #b)
+// enqueues one request as a frame, in the stages above (DESIGN.md §3a)
 int sb200_tracker::predict(int32_t n_scenes, const uint64_t* scene_ids, const int32_t* det_offsets, const float* boxes,
                            const float* features, const uint8_t* has_feature, const float* quality,
                            const int64_t* custom_ids, const float* own_area, const sb200_predict_out* out,
                            bool device_io, bool wait) {
   CU(cudaSetDevice(device));
   static const bool trace = getenv("SB200_TRACE") != nullptr;
-  auto tnow = [] { return std::chrono::steady_clock::now(); };
-  auto t_begin = tnow();
-  auto since = [&](std::chrono::steady_clock::time_point a) { return std::chrono::duration<double, std::milli>(tnow() - a).count(); };
-  if (n_scenes < 0) return fail(SB200_ERR_INVALID, "n_scenes must be >= 0");
-  if (n_scenes > 0 && (!scene_ids || !det_offsets)) return fail(SB200_ERR_INVALID, "scene_ids / det_offsets are NULL");
-  const int total = n_scenes > 0 ? det_offsets[n_scenes] : 0;
-  if (n_scenes > 0 && det_offsets[0] != 0) return fail(SB200_ERR_INVALID, "det_offsets[0] must be 0");
-  for (int s = 0; s < n_scenes; ++s)
-    if (det_offsets[s + 1] < det_offsets[s]) return fail(SB200_ERR_INVALID, "det_offsets must be non-decreasing");
-  if (total > 0 && !boxes) return fail(SB200_ERR_INVALID, "boxes is NULL");
-  if (!P.is_visual) { features = nullptr; has_feature = nullptr; quality = nullptr; own_area = nullptr; }
-  int rc = 0;
-  // frames that have completed since the last call hand over their results; an error of an earlier asynchronous frame
-  // is reported now
-  poll();
-  if (async_rc) { if ((rc = drain("error of an earlier frame"))) return rc; }
-  // same scene list as the previous request (the steady state of a batch tracker): validated slots are reused
-  const bool same_req = (int)last_req_scenes.size() == n_scenes && n_scenes > 0 &&
-                        memcmp(last_req_scenes.data(), scene_ids, sizeof(uint64_t) * (size_t)n_scenes) == 0;
-  if (!same_req && n_scenes > 0) {
-    std::unordered_map<uint64_t, int> seen;
-    for (int s = 0; s < n_scenes; ++s)
-      if (!seen.emplace(scene_ids[s], s).second) return fail(SB200_ERR_INVALID, "scene %llu appears twice in one request", (unsigned long long)scene_ids[s]);
-  }
-  // Everything that can refuse the request is checked BEFORE any tracker state changes (epochs, the auto-waste counter):
-  // the on-chip assignment solver holds a scene's rows and columns in shared memory.
-  {
-    int max_m0 = 0, max_n0 = 0;
-    for (int s = 0; s < n_scenes; ++s) {
-      const int m = det_offsets[s + 1] - det_offsets[s];
-      int slot = -1;
-      if (same_req) slot = last_req_slots[s];
-      else { auto it = slot_of.find(scene_ids[s]); if (it != slot_of.end()) slot = it->second; }
-      const int nub = slot >= 0 ? n_tracks[slot] + pending_add[slot] : 0;
-      max_m0 = std::max(max_m0, m);
-      max_n0 = std::max(max_n0, nub);
-    }
-    const int cap0 = P.is_visual ? kDenseVoteCap : 0;
-    if (sb::voting_smem_need(max_m0, max_n0, cap0) > sb::kVotingSmemLimit) {
-      if (pend_count > 0) {   // the bound counts every detection in flight as a new track: get the exact counts first
-        if ((rc = drain("assignment solver bound"))) return rc;
-        max_n0 = 0;
-        for (int s = 0; s < n_scenes; ++s) {
-          auto it = slot_of.find(scene_ids[s]);
-          if (it != slot_of.end()) max_n0 = std::max(max_n0, n_tracks[it->second]);
-        }
-      }
-      if (sb::voting_smem_need(max_m0, max_n0, cap0) > sb::kVotingSmemLimit)
-        return fail(SB200_ERR_CAPACITY, "scene too large for the on-chip assignment solver (m=%d, n=%d)", max_m0, max_n0);
-    }
-  }
+  const auto t_begin = std::chrono::steady_clock::now();
+  auto since = [&] { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_begin).count(); };
+  Request rq{n_scenes, 0, scene_ids, det_offsets, in_ptrs(boxes, features, has_feature, quality, custom_ids, own_area),
+             out ? *out : sb200_predict_out{}, device_io};
+  int rc = check_request(rq);
+  if (rc) return rc;
   // auto-waste tick (src/trackers/sort/simple_api.rs:115-120): a collection point of the reference, host and device meet
   if (auto_waste_counter == 0) {
     if ((rc = drain("auto-waste tick"))) return rc;
@@ -847,7 +1430,7 @@ int sb200_tracker::predict(int32_t n_scenes, const uint64_t* scene_ids, const in
   } else auto_waste_counter -= 1;
   if (n_scenes == 0) return wait ? drain() : 0;
 
-  if (!same_req) {
+  if (!rq.same_req) {
     last_req_slots.resize(n_scenes);
     for (int s = 0; s < n_scenes; ++s) last_req_slots[s] = slot_for(scene_ids[s], true);
     last_req_scenes.assign(scene_ids, scene_ids + n_scenes);
@@ -857,618 +1440,32 @@ int sb200_tracker::predict(int32_t n_scenes, const uint64_t* scene_ids, const in
     absorb_oldest(true);
   }   // back-pressure: at most kDepth frames in flight
 
-  // ---- upper bounds of everything the device will size exactly (tracks per scene with frames still in flight)
-  const int K = P.max_obs;
-  std::vector<int> n_ub(n_scenes), nb_ub(n_scenes), m_of(n_scenes);
-  int max_m = 0, max_n = 0, max_nb = 0, need_tracks = 0;
-  long long live_ub = 0, pos_total = 0, vis_total = 0, col_total = 0, posl_total = 0, visl_total = 0, work = 0;
-  auto bounds = [&]() {
-    max_m = max_n = max_nb = need_tracks = 0;
-    live_ub = pos_total = vis_total = col_total = work = 0;
-    for (int s = 0; s < n_scenes; ++s) {
-      const int slot = last_req_slots[s];
-      const int m = det_offsets[s + 1] - det_offsets[s];
-      m_of[s] = m;
-      n_ub[s] = n_tracks[slot] + pending_add[slot];
-      nb_ub[s] = P.is_visual ? arena_top[slot] + pending_add[slot] : 0;
-      live_ub += n_ub[s];
-      pos_total += (long long)m * n_ub[s];
-      if (P.is_visual) vis_total += (long long)m * n_ub[s] * K;
-      col_total += ((long long)nb_ub[s] * K + 127) / 128 * 128;
-      work += (long long)m * n_ub[s] * K;
-      max_m = std::max(max_m, m);
-      max_n = std::max(max_n, n_ub[s]);
-      max_nb = std::max(max_nb, nb_ub[s]);
-      need_tracks = std::max(need_tracks, n_ub[s] + m);
-    }
-  };
-  bounds();
-  {
-    // Capacity has to hold the UPPER BOUNDS: with frames in flight every queued detection counts as a possible new track.
-    // So the store is sized for the pipeline once -- the caller's hint (or what this frame needs) plus the detections of
-    // kDepth frames -- and later frames neither wait for the device nor reallocate.
-    const int pipe_room = kDepth * std::max(max_m, opts.max_dets_per_scene_hint);
-    int hint_s = std::max((int)scene_of_slot.size(), opts.max_scenes_hint);
-    if (hint_s > scene_cap || need_tracks > track_cap) {
-      // the store has to grow: meet the device first (the exact counts are the ones to grow from)
-      if ((rc = drain("track store bound"))) return rc;
-      bounds();
-      // grow generously (a regrow copies the whole feature arena: tens of milliseconds): what is needed now plus the
-      // pipeline's room, and at least half again as much as before
-      const int want_t = std::max(need_tracks, opts.max_tracks_per_scene_hint) + pipe_room;
-      if (hint_s > scene_cap || need_tracks > track_cap)
-        if ((rc = ensure_store(hint_s, std::max(want_t, track_cap + track_cap / 2)))) return rc;
-    }
-    // room for every live track of the frames in flight and of this one in the wasted buffer: the end-of-frame sweep
-    // appends without a host check
-    if (wasted_count + inflight_live_ub + live_ub + 1 > wb.cap) {
-      // the bound that failed is the pipeline's (frames in flight + this one): grow for twice that, or the next frame meets
-      // the same bound again -- after the wait the exact counts alone would fit and nothing would grow
-      const long long pipe_need = inflight_live_ub + live_ub;
-      if ((rc = drain("wasted buffer bound"))) return rc;
-      bounds();
-      // a full ring: kDepth frames in flight plus this one, each bounded by the live tracks plus every detection queued before it
-      const long long dets = std::max<long long>(total, (long long)std::max(opts.max_scenes_hint, n_scenes) * opts.max_dets_per_scene_hint);
-      const long long ring_need = (long long)(kDepth + 1) * (live_ub + (long long)kDepth * dets);
-      // and the records already waiting for collection doubled: a caller that collects rarely pays for few regrows
-      // and several times that while it is cheap (<= ~2 GB of records): a regrow drains the ring and reallocates
-      const long long rec_bytes = 72 + (hist_len > 1 ? 48ll * hist_len : 0);
-      const long long base_need = std::max<long long>(ring_need, 2 * pipe_need);
-      const long long mult = std::max<long long>(1, std::min<long long>(8, (2ll << 30) / std::max<long long>(1, base_need * rec_bytes)));
-      if ((rc = ensure_wasted(2 * wasted_count + mult * base_need + 1))) return rc;
-    }
-    // Feature-history pool.  New tracks take free blocks first, so the blocks handed out after this frame are at most
-    //   top + max(0, detections queued since - free)      (top, free: as of the last absorbed frame or collection).
-    // When that bound exceeds the pool, meet the device (the counts become exact) and grow, if needed, to
-    //   top + max(0, f * detections of this frame - free),   f = the frames the bound covered (in flight + this one),
-    // and at least half again as much as before.  So the pool is at most 1.5 x (live + uncollected wasted tracks + the
-    // detections of the frames actually queued together, less the free blocks): a caller that waits for every frame (the
-    // Python API) has f = 1, and only a caller that really queues f frames gets room for f frames of new tracks.
-    if (fhist_on && total > 0 && hpool_top + std::max<long long>(0, hpool_pend + total - hpool_free) > hpool_cap) {
-      const long long frames = pend_count + 1;
-      if ((rc = drain("feature history pool bound"))) return rc;   // hpool_top / hpool_free are exact from here on
-      const long long want = hpool_top + std::max<long long>(0, frames * total - hpool_free);
-      if (want > hpool_cap && (rc = ensure_hpool(std::max<long long>(want, hpool_cap + hpool_cap / 2)))) return rc;
-    }
-    if (!b_idc.p) {
-      if ((rc = b_idc.ensure(8))) return rc;
-      CU(cudaMemsetAsync(b_idc.p, 0, 8, stream));
-    }
-  }
-  // ---- this frame's slot in the ring
+  FramePlan pl;
+  if ((rc = reserve_state(rq, pl))) return rc;
   Pending& q = pend[(pend_head + pend_count) % kDepth];
-  if (!q.done) {
-    CU(cudaEventCreateWithFlags(&q.done, cudaEventDisableTiming));
-    for (auto& e : q.ev) CU(cudaEventCreate(&e));
-    for (auto& e : q.ev_k) CU(cudaEventCreate(&e));
-    for (auto& e : q.ev_pos) CU(cudaEventCreate(&e));
-  }
-  if ((rc = q.h_req.ensure(sizeof(sb::SceneReq) * (size_t)n_scenes)) ||
-      (rc = q.h_out.ensure(dyn_offset(n_scenes) + sizeof(sb::FrameDyn) + 32)))
-    return rc;
-  // visual cost path of this frame: tensor-core screen + exact refinement for large frames with a selective threshold, the
-  // dense tensor-core weight sums for thresholds that cut nothing, the exact SIMT kernel otherwise (small frames, and as the
-  // device-side fallback of single scenes)
-  bool want_tc = false, want_dense = false, want_fp8 = false;
-  if (P.is_visual && features != nullptr && total > 0) {
-    const bool selective = P.visual_kind == SB200_VIS_EUCLIDEAN ? (P.visual_threshold < 1e18f) : (P.visual_threshold > -1.0f);
-    const bool big = P.d8 >= 64 && work * P.d8 >= (1ll << 28);
-    const bool dense_ok = P.n_constraints == 0;
-    want_tc = selective && big;
-    want_dense = big && dense_ok && (!selective || adapt_dense);
-    if (want_dense) want_tc = false;
-    if (const char* e = getenv("SB200_VIS_KERNEL")) {
-      if (!strcmp(e, "simt")) { want_tc = false; want_dense = false; }
-      else if (!strcmp(e, "tc")) { want_tc = work > 0; want_dense = false; }
-      else if (!strcmp(e, "dense")) { want_dense = work > 0 && dense_ok; want_tc = work > 0 && !want_dense; }
-      else if (!strcmp(e, "tc8") || !strcmp(e, "tc16")) { want_tc = work > 0; want_dense = false; }
-    }
-    // screen precision (d8 <= 512): e4m3 unless a recent e4m3 frame showed its slack to be too wide; SB200_VIS_KERNEL=tc8 /
-    // tc16 force one
-    const char* ek = getenv("SB200_VIS_KERNEL");
-    const bool can8 = want_tc && P.d8 <= sb::kFp8MaxD8 && ts.feat_fp8 != nullptr;
-    if (ek && !strcmp(ek, "tc8")) want_fp8 = can8;
-    else if (ek && !strcmp(ek, "tc16")) want_fp8 = false;
-    else {
-      want_fp8 = can8 && fp8_hold == 0;
-      if (can8 && fp8_hold > 0) fp8_hold -= 1;
-    }
-  }
-  const int vote_cap = want_dense ? kDenseVoteCap : sb::kVoteVisCap;
-  sb::Params Pf = P;
-  Pf.vote_vis_cap = vote_cap;
-  sb::SceneReq* hreq = q.h_req.as<sb::SceneReq>();
-  for (int s = 0; s < n_scenes; ++s) {
-    sb::SceneReq& r = hreq[s];
-    r.slot = last_req_slots[s];
-    r.m = m_of[s];
-    r.det_base = det_offsets[s];
-    r.epoch = epoch[r.slot] + 1;   // EpochDb::next_epoch, src/trackers/epoch_db.rs:35-49 (committed below)
-    r.scene_id = scene_ids[s];
-    r.pos_lbase = (int)posl_total;
-    r.pos_lcap = (int)std::min<long long>((long long)r.m * 32, (long long)sb::kVotePosCap * 2);
-    posl_total += r.pos_lcap;
-    r.vis_lbase = (int)visl_total;
-    r.vis_lcap = P.is_visual ? (int)std::min<long long>((long long)r.m * 64, (long long)vote_cap * 4) : 0;
-    visl_total += r.vis_lcap;
-  }
-  // ---- frame buffers (sized once from the capacity hints when given, so steady-state frames never reallocate)
-  const long long hint_dets = (long long)std::max(opts.max_scenes_hint, n_scenes) * opts.max_dets_per_scene_hint;
-  const size_t T = (size_t)std::max<long long>(std::max(total, 1), hint_dets);
-  const int hint_tracks = opts.max_tracks_per_scene_hint > 0 ? track_cap : 0;   // the store's rows per scene: hint + pipeline room
-  const long long hint_cols = (long long)std::max(opts.max_scenes_hint, n_scenes) * (((long long)hint_tracks * K + 127) / 128 * 128);
-  const long long pos_ub = pos_total;
-  {
-    const long long hint_pos = hint_dets * hint_tracks;
-    pos_total = std::max(pos_total, hint_pos);
-    if (P.is_visual) vis_total = std::max(vis_total, hint_pos * K);
-  }
-  // candidate-side buffers: the set of this frame (the other one may still be read by the frame in front of it)
-  const int cset = (int)(frame_seq & 1);
-  CandBufs& cb = cand[cset];
-  if ((rc = ENS(cb.box, T * 24)) || (rc = ENS(cb.radius, T * 4)) || (rc = ENS(cb.conf, T * 4)) ||
-      (rc = ENS(f_winner, T * 4)) || (rc = ENS(f_cvt, T)) || (rc = ENS(f_scenes, sizeof(sb::SceneDesc) * n_scenes)) ||
-      (rc = ENS(f_newcount, 4 * (size_t)n_scenes)) || (rc = ENS(f_dyn, sizeof(sb::FrameDyn))) ||
-      (rc = ENS(f_apprank, T * 8)) || (rc = ENS(f_appmeta, 16 * (size_t)n_scenes)) ||
-      (rc = ENS(f_pos, std::max<size_t>(4, (size_t)pos_total * 4))))
-    return rc;
-  if (P.positional_kind == SB200_POS_IOU && (rc = ENS(cb.vert, T * 64))) return rc;
-  if (P.is_visual) {
-    if (fhist_on && (rc = ENS(f_histdst, T * 4))) return rc;
-    if ((rc = ENS(cb.flags, T)) || (rc = ENS(cb.norm2, T * 4)) || (rc = ENS(f_featdst, T * 4)) ||
-        (rc = ENS(f_vis, std::max<size_t>(4, (size_t)vis_total * 4))) || (rc = ENS(f_scene_max, 4 * (size_t)n_scenes)))
-      return rc;
-  }
-  sb::TcArgs tc;
-  memset(&tc, 0, sizeof(tc));
-  tc.num_sms = num_sms;
-  int mstep = 0, cstep = 256;
-  const long long visl_alloc = std::max(visl_total, hint_dets * 64);
-  if (want_tc || want_dense) {
-    tc.use_tc = true;
-    tc.dense = want_dense;
-    mstep = 256;   // a cluster covers two 128-row candidate tiles
-    // dense: column tiles end at block boundaries, a track's observations stay together
-    cstep = want_dense ? (256 / K) * K : sb::vis_screen_ucols(P.d8, num_sms, n_scenes, m_of.data(), nb_ub.data(), K);
-    tc.cstep = cstep;
-    long long tiles_ub = 0, slabs_ub = 0, ws_ub = 0, blk_ub = 0;
-    for (int s = 0; s < n_scenes; ++s) {
-      const long long ct = ((long long)nb_ub[s] * K + cstep - 1) / cstep;
-      tiles_ub += (long long)((m_of[s] + mstep - 1) / mstep) * ct;
-      slabs_ub += ct;
-      ws_ub += ct * (cstep / K) * ((m_of[s] + 127) / 128 * 128);   // blocks padded to whole column tiles
-      blk_ub += ct * (cstep / K);
-    }
-    tc.n_tiles = (int)tiles_ub;   // upper bound: the list and its length are built on the device
-    // the list is sized from the hints like the other frame buffers (the bound grows with the frames in flight: a list
-    // sized for this frame alone would be outgrown, and wait for the device, again and again)
-    long long tiles_alloc = tiles_ub;
-    {
-      const long long hs = std::max(opts.max_scenes_hint, n_scenes), hd = std::max(opts.max_dets_per_scene_hint, max_m);
-      const long long ht = std::max(hint_tracks, max_nb);
-      tiles_alloc = std::max(tiles_alloc, hs * ((hd + mstep - 1) / mstep) * ((ht * K + cstep - 1) / cstep + 1));
-      if (f_tiles.bytes > 0 && sizeof(sb::TcTile) * (size_t)tiles_alloc > f_tiles.bytes) tiles_alloc += tiles_alloc / 2;
-    }
-    // both operand copies of the candidates whenever the e4m3 screen can run: a switch between the precisions must not
-    // allocate (and synchronise) in the middle of a stream of frames
-    const bool alloc8 = !want_dense && P.d8 <= sb::kFp8MaxD8 && ts.feat_fp8 != nullptr;
-    if (alloc8 && ((rc = ENS(cb.fp8, T * sb::fp8_pitch(P.d8))) || (rc = ENS(cb.scale, T * 4)) || (rc = ENS(b_bf16log, kBf16LogCap * 4))))
-      return rc;
-    if ((rc = ENS(cb.bf16, T * P.d8 * 2)) || (rc = ENS(f_tiles, sizeof(sb::TcTile) * (size_t)std::max<long long>(1, tiles_alloc))) ||
-        (rc = ENS(f_rowmeta, sizeof(sb::VisRowMeta) * (T + 256))))
-      return rc;
-    tc.rowmeta = f_rowmeta.as<sb::VisRowMeta>();
-    tc.max_rows = max_nb * K;
-    tc.d_tiles = f_tiles.as<sb::TcTile>();
-    tc.d_n_tiles = &f_dyn.as<sb::FrameDyn>()->n_tiles;
-    tc.a_rows = total;
-    tc.b_rows = (long long)scene_cap * track_cap * K;
-    if (!want_dense) {
-      if ((rc = ENS(f_colmeta, sizeof(sb::VisColMeta) * (size_t)(std::max(col_total, hint_cols) + 256))) ||
-          (rc = ENS(f_colb, 4 * (size_t)(std::max(col_total, hint_cols) + 256))) ||
-          (rc = ENS(f_colvalid, (size_t)(std::max(col_total, hint_cols) + 256) / 8 + 16)) ||
-          (rc = ENS(f_colgeo, sizeof(sb::VisColGeo) * (size_t)std::max<long long>(1, P.n_constraints > 0 ? std::max(col_total, hint_cols) : 1))))
-        return rc;
-      tc.colmeta = f_colmeta.as<sb::VisColMeta>();
-      tc.colgeo = f_colgeo.as<sb::VisColGeo>();
-      tc.colb = f_colb.as<float>();
-      tc.colvalid = f_colvalid.as<unsigned int>();
-      tc.total_cols = (int)col_total;
-      if (alloc8 && P.visual_kind != SB200_VIS_COSINE) {
-        if ((rc = ENS(f_colsb, 4 * (size_t)(std::max(col_total, hint_cols) + 256)))) return rc;
-        if (want_fp8) tc.colsb = f_colsb.as<float>();
-      }
-      tc.fp8 = want_fp8;
-    } else {
-      // sized from the hints like the other frame buffers, so steady-state frames never reallocate
-      const long long hs = std::max(opts.max_scenes_hint, n_scenes), ht = hint_tracks;
-      const long long hd = std::max(opts.max_dets_per_scene_hint, 0);
-      ws_ub = std::max(ws_ub, hs * (ht + 256) * ((hd + 127) / 128 * 128));
-      blk_ub = std::max(blk_ub, hs * (ht + 256));
-      slabs_ub = std::max(slabs_ub, hs * ((ht * K + cstep - 1) / cstep + 1));
-      if ((rc = ENS(f_drowb, 4 * 5 * T)) || (rc = ENS(f_dcolb, 4 * (size_t)std::max<long long>(1, blk_ub))) ||
-          (rc = ENS(f_slabk, 4 * 256 * (size_t)std::max<long long>(1, slabs_ub))))
-        return rc;
-      if ((rc = ENS(f_ws, 4 * (size_t)std::max<long long>(1, ws_ub))) || (rc = ENS(f_tmeta, sizeof(sb::DenseTrackMeta) * (size_t)std::max<long long>(1, blk_ub))) ||
-          (rc = ENS(f_rowinfo, 8 * (size_t)std::max<long long>(1, blk_ub * K))) || (rc = ENS(f_slabc, 4 * 256 * (size_t)std::max<long long>(1, slabs_ub))) ||
-          (rc = ENS(f_slabm, 4 * 256 * (size_t)std::max<long long>(1, slabs_ub))) || (rc = ENS(f_slabmask, 2 * 32 * (size_t)std::max<long long>(1, slabs_ub))) ||
-          (rc = ENS(f_dscene, 4 * 6 * (size_t)n_scenes + 128)) || (rc = ENS(f_maxc, sizeof(sb::VisPair) * (size_t)std::max<long long>(1, visl_alloc))) ||
-          (rc = ENS(f_maxcval, 4 * (size_t)std::max<long long>(1, visl_alloc))))
-        return rc;
-      tc.max_blocks = max_nb;
-      tc.n_slabs_ub = (int)slabs_ub;
-      tc.ws = f_ws.p;
-      tc.d_rowb = f_drowb.as<unsigned int>();
-      tc.d_colb = f_dcolb.as<unsigned int>();
-      tc.blk_ub = blk_ub;
-      tc.slab_ktf = f_slabk.as<float>();
-      tc.tmeta = f_tmeta.as<sb::DenseTrackMeta>();
-      tc.rowinfo = f_rowinfo.as<int2>();
-      tc.slab_colc = f_slabc.as<float>();
-      tc.slab_cmax = f_slabm.as<float>();
-      tc.slab_vmask = f_slabmask.as<unsigned int>();
-      tc.slab_bmask = tc.slab_vmask + (size_t)slabs_ub * 8;
-      // per-scene scalars: maxc_cnt | maxc_next | dense_bad | zeros (ints, zeroed together), then l0 | cmax (floats)
-      tc.maxc_cnt = f_dscene.as<int>();
-      tc.maxc_next = tc.maxc_cnt + n_scenes;
-      tc.dense_bad = tc.maxc_cnt + 2 * n_scenes;
-      tc.zeros = tc.maxc_cnt + 3 * n_scenes;
-      tc.scene_l0 = reinterpret_cast<float*>(tc.maxc_cnt + 4 * n_scenes);
-      tc.scene_cmax = tc.scene_l0 + n_scenes;
-      tc.dbg_counts = reinterpret_cast<int*>(tc.scene_cmax + n_scenes) + 4;
-      tc.maxc = f_maxc.as<sb::VisPair>();
-      tc.maxc_val = f_maxcval.as<float>();
-    }
-  }
-  sb::Frame f;
-  memset(&f, 0, sizeof(f));
-  f.total = total;
-  f.pos_total = pos_ub;
-  f.dyn = f_dyn.as<sb::FrameDyn>();
-  f.id_counter = b_idc.as<unsigned long long>();
-  f.id_add = P.is_batch ? (long long)total : -1;
-  f.dense_bad = tc.dense ? tc.dense_bad : nullptr;
-  // dense positional matrices for every scene only on request (SB200_FULL_COSTS: parity of sb200_last_costs)
-  f.pos_dense_all = getenv("SB200_FULL_COSTS") != nullptr;
-  f.feat_type = feat_type;
-  bool prefetched = false;
-  Staging* sin = nullptr;
-  // inputs
-  if (device_io) {
-    f.in_boxes = boxes; f.in_feat = features; f.in_hasf = has_feature; f.in_quality = quality;
-    f.in_custom = reinterpret_cast<const long long*>(custom_ids); f.in_own = own_area;
-  } else {
-    // device staging: a set already filled by sb200_prefetch_inputs() for exactly these host buffers (all six columns)
-    // is used as is; otherwise the H2D copies are issued below
-    const void* key[6] = {boxes, features, features ? has_feature : nullptr, quality, custom_ids, own_area};
-    int use = -1;
-    for (int k = 0; k < 2; ++k)
-      if (stg[k].pending && stg[k].total == total && stg[k].type == feat_type && memcmp(stg[k].key, key, sizeof(key)) == 0)
-        use = k;
-    if (use >= 0) {
-      prefetched = true;
-      stg[use].pending = false;
-      CU(cudaStreamWaitEvent(stream, stg[use].ev, 0));
-    } else {
-      use = stg[0].pending ? 1 : (stg[1].pending ? 0 : 1 - stg_last);
-      stg[use].pending = false;
-    }
-    stg_last = use;
-    Staging& S = stg[use];
-    sin = &S;
-    if (prefetched && (S.boxes.bytes < T * 24 || (features && S.feat.bytes < T * (size_t)P.feature_dim * feat_bytes()))) {
-      // the filled set is smaller than this frame's sizing rule (hints changed?): re-copy instead of reallocating
-      prefetched = false;
-    }
-    if ((rc = ENS(S.boxes, T * 24))) return rc;
-    f.in_boxes = S.boxes.as<float>();
-    if (features && total > 0) {
-      if ((rc = ENS(S.feat, T * (size_t)P.feature_dim * feat_bytes()))) return rc;
-      f.in_feat = S.feat.p;
-      if (has_feature) {
-        if ((rc = ENS(S.hasf, T))) return rc;
-        f.in_hasf = S.hasf.as<unsigned char>();
-      }
-    }
-    if (quality && total > 0) { if ((rc = ENS(S.quality, T * 4))) return rc; f.in_quality = S.quality.as<float>(); }
-    if (custom_ids && total > 0) { if ((rc = ENS(S.custom, T * 8))) return rc; f.in_custom = S.custom.as<long long>(); }
-    if (own_area && total > 0) { if ((rc = ENS(S.own, T * 4))) return rc; f.in_own = S.own.as<float>(); }
-  }
-  f.c_box = cb.box.as<float>(); f.c_radius = cb.radius.as<float>(); f.c_conf = cb.conf.as<float>();
-  f.c_vert = cb.vert.as<double>(); f.c_flags = cb.flags.as<unsigned char>(); f.c_norm2 = cb.norm2.as<float>();
-  f.winner = f_winner.as<int>(); f.c_vt = f_cvt.as<unsigned char>(); f.pos = f_pos.as<float>(); f.vis = f_vis.as<float>();
-  f.scenes = f_scenes.as<sb::SceneDesc>(); f.new_count = f_newcount.as<int>();
-  f.new_count_all = f.new_count;
-  f.feat_dst = P.is_visual ? f_featdst.as<int>() : nullptr;
-  f.hist_dst = fhist_on ? f_histdst.as<int>() : nullptr;
-  f.app_rank = f_apprank.as<int2>(); f.app_meta = f_appmeta.as<int4>();
-  if ((rc = ENS(f_frameout, sizeof(int) * 3 * (size_t)n_scenes))) return rc;
-  f.frame_out = f_frameout.as<int>();
-  f.c_bf16 = tc.use_tc && !tc.fp8 ? cb.bf16.p : nullptr; f.scene_max = f_scene_max.as<unsigned int>();
-  f.c_fp8 = tc.fp8 ? cb.fp8.as<unsigned char>() : nullptr;
-  f.c_scale = tc.fp8 ? cb.scale.as<float>() : nullptr;
-  // sparse entry lists + per-scene counters (pos_cnt | vis_cnt | scene_mode | vis_mode | refine_next | dense_cnt | status),
-  // zeroed every frame by frame_setup_kernel
-  const size_t n_counters = 6 * (size_t)n_scenes + 4;
-  if ((rc = ENS(f_poslist, sizeof(sb::PosEntry) * (size_t)std::max<long long>(1, std::max(posl_total, hint_dets * 32)))) ||
-      (rc = ENS(f_counters, sizeof(int) * n_counters)))
-    return rc;
-  if (P.is_visual && ((rc = ENS(f_pairs, sizeof(sb::VisPair) * (size_t)std::max<long long>(1, visl_alloc))) ||
-                      (rc = ENS(f_visval, sizeof(float) * (size_t)std::max<long long>(1, visl_alloc)))))
-    return rc;
-  f.pos_list = f_poslist.as<sb::PosEntry>();
-  f.pos_cnt = f_counters.as<int>();
-  f.vis_cnt = f.pos_cnt + n_scenes;
-  f.scene_mode = f.pos_cnt + 2 * n_scenes;
-  f.vis_mode = f.pos_cnt + 3 * n_scenes;
-  f.refine_next = f.pos_cnt + 4 * n_scenes;
-  f.status = f.pos_cnt + 5 * n_scenes;
-  f.dense_cnt = f.pos_cnt + 6 * n_scenes;
-  f.screen_cnt = tc.use_tc && !tc.dense ? f.dense_cnt + 1 : nullptr;   // the 3 ints after it: zeroed with the counters
-  f.vis_pairs = f_pairs.as<sb::VisPair>();
-  f.vis_val = f_visval.as<float>();
-  // outputs
-  sb200_predict_out o{};
-  if (out) o = *out;
-  if (device_io) {
-    f.o_ids = reinterpret_cast<unsigned long long*>(o.ids); f.o_epochs = o.epochs; f.o_lengths = o.lengths;
-    f.o_vt = o.voting_types; f.o_pred = o.predicted_boxes; f.o_obs = o.observed_boxes;
-  } else {
-    if (o.ids) { if ((rc = ENS(o_ids, T * 8))) return rc; f.o_ids = o_ids.as<unsigned long long>(); }
-    if (o.epochs) { if ((rc = ENS(o_epochs, T * 4))) return rc; f.o_epochs = o_epochs.as<unsigned int>(); }
-    if (o.lengths) { if ((rc = ENS(o_lengths, T * 4))) return rc; f.o_lengths = o_lengths.as<unsigned int>(); }
-    if (o.voting_types) { if ((rc = ENS(o_vt, T))) return rc; f.o_vt = o_vt.as<unsigned char>(); }
-    if (o.predicted_boxes) { if ((rc = ENS(o_pred, T * 24))) return rc; f.o_pred = o_pred.as<float>(); }
-    if (o.observed_boxes) { if ((rc = ENS(o_obs, T * 24))) return rc; f.o_obs = o_obs.as<float>(); }
-  }
-  // Visual trackers on the tensor-core path evaluate the positional metric lazily: VisualVoting only consults it for
-  // candidates the visual BestFit pass left undecided, against tracks that pass did not claim, so the order is
-  // screen -> refine -> BestFit pre-pass (masks) -> culled scan of what is still open -> full voting.
-  // SB200_FULL_COSTS=1 (every pair is evaluated, sb200_last_costs is complete) keeps the plain order.
-  const bool fork = P.is_visual && tc.use_tc && tc.n_tiles > 0 && !f.pos_dense_all;
-  if (fork) {
-    if ((rc = ENS(cb.decided, T)) || (rc = ENS(f_excl, (size_t)scene_cap * track_cap + 16)) || (rc = ENS(f_prewin, T * 4))) return rc;
-    f.decided = cb.decided.as<unsigned char>();
-    f.excl = f_excl.as<unsigned char>();
-    f.pre_winner = f_prewin.as<int>();
-  }
-  const bool derive_own = P.is_visual && P.use_own_area && f.in_own == nullptr && total > 0;
-  if (derive_own && ((rc = ENS(f_own, T * 4)) || (rc = ENS(f_ownovf, 16 + T * sizeof(int2))))) return rc;
-
-  // ======================================================================== nothing below can fail for capacity reasons:
-  // the request is committed (epochs, ring slot, bounds of the frames in flight)
-  for (int s = 0; s < n_scenes; ++s) epoch[last_req_slots[s]] += 1;
-  if (features != nullptr && total > 0) seen_features = true;
-  frame_seq += 1;
-  q.active = true;
-  q.n_scenes = n_scenes;
-  q.total = total;
-  q.slots.assign(last_req_slots.begin(), last_req_slots.end());
-  q.m = m_of;
-  q.live_ub = live_ub;
-  q.tc_timed = false;
-  q.pos_forked = false;
-  q.mode = tc.dense ? 2 : (tc.use_tc ? 1 : 0);
-  q.fp8 = tc.use_tc && !tc.dense && tc.fp8;
-  for (int s = 0; s < n_scenes; ++s) pending_add[last_req_slots[s]] += m_of[s];
-  inflight_live_ub += live_ub;
-  if (fhist_on) hpool_pend += total;
-  pend_count += 1;
-  last_n_scenes = n_scenes;
-  // a CUDA failure while the frame is being enqueued takes it out of the ring again (the context is lost anyway)
-  struct Rollback {
-    sb200_tracker* t; Pending* q; bool armed;
-    ~Rollback() {
-      if (!armed) return;
-      for (int s = 0; s < q->n_scenes; ++s) t->pending_add[q->slots[s]] -= q->m[s];
-      t->inflight_live_ub -= q->live_ub;
-      if (t->fhist_on) t->hpool_pend -= q->total;
-      q->active = false;
-      t->pend_count -= 1;
-    }
-  } rollback{this, &q, true};
-
-  const double ms_setup = since(t_begin);
-  if (has_user_stream) {   // everything the caller's stream holds now comes first
-    if (!ev_user_in) { CU(cudaEventCreateWithFlags(&ev_user_in, cudaEventDisableTiming)); CU(cudaEventCreateWithFlags(&ev_user_out, cudaEventDisableTiming)); }
-    CU(cudaEventRecord(ev_user_in, user_stream));
-    CU(cudaStreamWaitEvent(stream, ev_user_in, 0));
-  }
-  if (!device_io && !prefetched && total > 0) {
-    const size_t n = (size_t)total;
-    CU(cudaMemcpyAsync(sin->boxes.p, boxes, n * 24, cudaMemcpyHostToDevice, stream));
-    if (f.in_feat) {
-      CU(cudaMemcpyAsync(sin->feat.p, features, n * (size_t)P.feature_dim * feat_bytes(), cudaMemcpyHostToDevice, stream));
-      if (f.in_hasf) CU(cudaMemcpyAsync(sin->hasf.p, has_feature, n, cudaMemcpyHostToDevice, stream));
-    }
-    if (f.in_quality) CU(cudaMemcpyAsync(sin->quality.p, quality, n * 4, cudaMemcpyHostToDevice, stream));
-    if (f.in_custom) CU(cudaMemcpyAsync(sin->custom.p, custom_ids, n * 8, cudaMemcpyHostToDevice, stream));
-    if (f.in_own) CU(cudaMemcpyAsync(sin->own.p, own_area, n * 4, cudaMemcpyHostToDevice, stream));
-  }
-  // scene descriptors, tile list, frame scalars; list counters and status words zeroed
-  if (!side_stream) {
-    int lo = 0, hi = 0;
-    CU(cudaDeviceGetStreamPriorityRange(&lo, &hi));
-    CU(cudaStreamCreateWithPriority(&side_stream, cudaStreamNonBlocking, hi));
-    for (auto& e : ev_fork) CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-    CU(cudaEventCreateWithFlags(&ev_join, cudaEventDisableTiming));
-  }
-  // The frame's tables come from one small CTA: with nothing else to wait for (no own-area derivation, which reads them) it
-  // runs beside the candidate preparation, on the side stream, and the main stream joins before the first kernel that reads them.
-  if (!prep_stream) {
-    int lo = 0, hi = 0;
-    CU(cudaDeviceGetStreamPriorityRange(&lo, &hi));
-    CU(cudaStreamCreateWithPriority(&prep_stream, cudaStreamNonBlocking, lo));
-    CU(cudaEventCreateWithFlags(&ev_prep_done, cudaEventDisableTiming));
-    CU(cudaEventCreateWithFlags(&ev_inputs, cudaEventDisableTiming));
-  }
-  if (q.fp8 && f.in_feat) {
-    f.skip_bf16 = true;
-    if (!bf16_stale_all && bf16_log_n + total <= kBf16LogCap) {
-      f.bf16_log = b_bf16log.as<int>() + bf16_log_n;
-      bf16_log_n += total;
-    } else {
-      bf16_stale_all = true;
-    }
-  } else if (tc.use_tc && !tc.fp8) {   // the BF16 screen or the dense path reads the BF16 rows
-    if ((rc = regen_bf16())) return rc;
-  }
-  const bool prep_ahead = !derive_own && total > 0;
-  // (the tables go to the side stream: on the work stream they would move the next frame's preparation squarely under the
-  // screen kernel)
-  const bool side_setup = !derive_own && total > 0;
-  cudaStream_t s_setup = stream;
-  if (side_setup) {
-    CU(cudaEventRecord(ev_fork[0], stream));
-    CU(cudaStreamWaitEvent(side_stream, ev_fork[0], 0));
-    s_setup = side_stream;
-  }
-  sb::launch_frame_setup(P, ts, f, reinterpret_cast<const sb::SceneReq*>(q.h_req.dp), n_scenes, b_ntracks.as<int>(), mstep,
-                         cstep, tc.dense, f_tiles.as<sb::TcTile>(), f_dyn.as<sb::FrameDyn>(), f_counters.as<int>(), (int)n_counters, s_setup);
-  tc.max_init_done = 1;   // frame_setup resets scene_max
-  if (side_setup && Pf.is_visual && tc.use_tc && !tc.dense && tc.n_tiles > 0 && max_m > 0 && max_n > 0 && f.in_feat) {
-    // the screen's column metadata reads the tables and the store only: it follows the setup on the side stream
-    sb::launch_vis_colmeta(Pf, ts, f, n_scenes, max_n, tc, side_stream);
-    tc.colmeta_done = 1;
-  }
-  if (side_setup) CU(cudaEventRecord(ev_join, side_stream));
-  CU(cudaEventRecord(q.ev[0], stream));
-  if (derive_own) {
-    // visual_sort/simple_api.rs:110-127: with an own-area threshold and no shares supplied by the caller, the shares come
-    // from the scene's observation boxes (exclusively_owned_areas_normalized_shares)
-    sb::launch_own_area(f, n_scenes, max_m, f.in_boxes, f_own.as<float>(), f_ownovf.as<int>(),
-                        reinterpret_cast<int2*>(f_ownovf.as<char>() + 16), stream);
-    f.in_own = f_own.as<float>();
-  }
-  // Candidate preparation needs the request only (boxes, features): it runs on its own stream as soon as the inputs are there
-  // and the frame that read this set of candidate buffers (two frames back) has ended -- in the steady state under the
-  // tensor-core kernel of the frame in front.  (With derived own-area shares it needs the frame tables: main stream.)
-  if (prep_ahead) {
-    if (has_user_stream) CU(cudaStreamWaitEvent(prep_stream, ev_user_in, 0));
-    if (!device_io) {   // staged inputs: the prefetch copy, or the copies issued above on the work stream
-      if (prefetched) CU(cudaStreamWaitEvent(prep_stream, sin->ev, 0));
-      else { CU(cudaEventRecord(ev_inputs, stream)); CU(cudaStreamWaitEvent(prep_stream, ev_inputs, 0)); }
-    }
-    if (set_busy[cset]) CU(cudaStreamWaitEvent(prep_stream, ev_set_free[cset], 0));
-    // ... and not before the frame in front has left its cost kernels: the preparation is HBM traffic that would slow that
-    // frame's tensor-core screen.  Waiting keeps the tensor-core kernel undisturbed and the step time reproducible.
-    if (cost_done_valid) CU(cudaStreamWaitEvent(prep_stream, ev_cost_done, 0));
-    sb::launch_prep(Pf, f, n_scenes, max_m, prep_stream);
-    CU(cudaEventRecord(ev_prep_done, prep_stream));
-    CU(cudaStreamWaitEvent(stream, ev_prep_done, 0));
-  } else {
-    sb::launch_prep(Pf, f, n_scenes, max_m, stream);
-  }
-  if (side_setup) CU(cudaStreamWaitEvent(stream, ev_join, 0));
-  CU(cudaEventRecord(q.ev[1], stream));
-  sb::TcArgs tcc = tc;
-  if (tc.use_tc && tc.n_tiles > 0) { tcc.ev_screen0 = q.ev_k[0]; tcc.ev_screen1 = q.ev_k[1]; tcc.ev_refine1 = q.ev_k[2]; q.tc_timed = true; }
-  if (!fork) {
-    sb::launch_pos_cost(Pf, ts, f, n_scenes, max_m, max_n, stream);
-    CU(cudaEventRecord(q.ev[2], stream));
-    int vr0 = sb::launch_vis_cost(Pf, ts, f, n_scenes, max_m, max_n, tcc, stream);
-    if (vr0 != 0) return fail(SB200_ERR_CUDA, "visual cost launch failed (%d)", vr0);
-    // scenes whose entry list overflowed vote on the dense matrix: it is filled and scanned for them alone, now
-    if (!f.pos_dense_all) sb::launch_pos_scan_lazy(Pf, ts, f, n_scenes, max_m, max_n, /*pass=*/1, stream);
-  } else {
-    CU(cudaEventRecord(q.ev[2], stream));
-    {
-      int vr0 = sb::launch_vis_cost_a(Pf, ts, f, n_scenes, max_m, max_n, tcc, stream);   // metadata, screen, vis_mode, refinement
-      if (vr0 != 0) return fail(SB200_ERR_CUDA, "visual cost launch failed (%d)", vr0);
-      vr0 = sb::launch_vote_masks(Pf, ts, f, n_scenes, max_m, max_n, stream);            // who is still open positionally
-      if (vr0 != 0) return fail(SB200_ERR_CUDA, "voting launch failed: %s", cudaGetErrorString((cudaError_t)vr0));
-    }
-    CU(cudaEventRecord(q.ev_pos[0], stream));
-    sb::launch_pos_scan_lazy(Pf, ts, f, n_scenes, max_m, max_n, /*pass=*/0, stream);
-    CU(cudaEventRecord(q.ev_pos[1], stream));
-    int vr1 = sb::launch_vis_cost_b(Pf, ts, f, n_scenes, max_m, max_n, tcc, stream);     // final scene mode, dense fallbacks
-    if (vr1 != 0) return fail(SB200_ERR_CUDA, "visual cost launch failed (%d)", vr1);
-    sb::launch_pos_scan_lazy(Pf, ts, f, n_scenes, max_m, max_n, /*pass=*/1, stream);     // scenes that fell back to dense voting
-    q.pos_forked = true;
-  }
-  CU(cudaEventRecord(q.ev[3], stream));
-  if (!ev_cost_done) CU(cudaEventCreateWithFlags(&ev_cost_done, cudaEventDisableTiming));
-  CU(cudaEventRecord(ev_cost_done, stream));
-  cost_done_valid = true;
-  int vr = sb::launch_voting(Pf, ts, f, n_scenes, max_m, max_n, stream);
-  if (vr != 0) return fail(SB200_ERR_CUDA, "voting launch failed: %s", cudaGetErrorString((cudaError_t)vr));
-  CU(cudaEventRecord(q.ev[4], stream));
-  sb::launch_apply(Pf, ts, f, n_scenes, max_m, 0ull, b_ntracks.as<int>(), stream);
-  // The sweep (latency-bound, one CTA per scene) and the feature store (HBM-bound) touch disjoint arrays -- a track's feature
-  // block is not moved by the compaction -- so the sweep runs on the side stream beside the store; the frame ends at the join.
-  const bool side_sweep = Pf.is_visual && f.in_feat && total > 0;
-  if (side_sweep) {
-    CU(cudaEventRecord(ev_fork[1], stream));
-    CU(cudaStreamWaitEvent(side_stream, ev_fork[1], 0));
-    sb::launch_frame_sweep(Pf, ts, f, n_scenes, b_ntracks.as<int>(), wb, side_stream);
-    CU(cudaEventRecord(ev_join, side_stream));
-    sb::launch_feat_store(Pf, ts, f, stream);
-    CU(cudaStreamWaitEvent(stream, ev_join, 0));
-  } else {
-    sb::launch_feat_store(Pf, ts, f, stream);
-    sb::launch_frame_sweep(Pf, ts, f, n_scenes, b_ntracks.as<int>(), wb, stream);
-  }
-  CU(cudaEventRecord(q.ev[5], stream));
-  CU(cudaGetLastError());
-
-  // results back
-  if (!device_io && total > 0) {
-    if (o.ids) CU(cudaMemcpyAsync(o.ids, f.o_ids, (size_t)total * 8, cudaMemcpyDeviceToHost, stream));
-    if (o.epochs) CU(cudaMemcpyAsync(o.epochs, f.o_epochs, (size_t)total * 4, cudaMemcpyDeviceToHost, stream));
-    if (o.lengths) CU(cudaMemcpyAsync(o.lengths, f.o_lengths, (size_t)total * 4, cudaMemcpyDeviceToHost, stream));
-    if (o.voting_types) CU(cudaMemcpyAsync(o.voting_types, f.o_vt, (size_t)total, cudaMemcpyDeviceToHost, stream));
-    if (o.predicted_boxes) CU(cudaMemcpyAsync(o.predicted_boxes, f.o_pred, (size_t)total * 24, cudaMemcpyDeviceToHost, stream));
-    if (o.observed_boxes) CU(cudaMemcpyAsync(o.observed_boxes, f.o_obs, (size_t)total * 24, cudaMemcpyDeviceToHost, stream));
-  }
-  {
-    char* ho = reinterpret_cast<char*>(q.h_out.p);
-    CU(cudaMemcpyAsync(ho, f.frame_out, 12 * (size_t)n_scenes, cudaMemcpyDeviceToHost, stream));
-    CU(cudaMemcpyAsync(ho + 12 * (size_t)n_scenes, f.status, 4 * (size_t)n_scenes, cudaMemcpyDeviceToHost, stream));
-    CU(cudaMemcpyAsync(ho + dyn_offset(n_scenes), f_dyn.p, sizeof(sb::FrameDyn), cudaMemcpyDeviceToHost, stream));
-    CU(cudaMemcpyAsync(ho + dyn_offset(n_scenes) + sizeof(sb::FrameDyn), f.dense_cnt, 4, cudaMemcpyDeviceToHost, stream));
-    if (fhist_on)
-      CU(cudaMemcpyAsync(ho + dyn_offset(n_scenes) + sizeof(sb::FrameDyn) + 8, ts.hpool, 8, cudaMemcpyDeviceToHost, stream));
-    // the screen's survivors, the part of them the exact test cut, the scenes whose list overflowed (zeros on other paths)
-    CU(cudaMemcpyAsync(ho + dyn_offset(n_scenes) + sizeof(sb::FrameDyn) + 16, f.dense_cnt + 1, 12, cudaMemcpyDeviceToHost, stream));
-  }
-  static const bool trace_dense = trace && atoi(getenv("SB200_TRACE")) >= 2;   // synchronises: level 2 only
-  if (trace_dense && tc.dense && tc.n_tiles > 0) {
-    int hc[8] = {0};
-    int vc = 0;
-    CU(cudaMemcpyAsync(hc, tc.dbg_counts, sizeof(hc), cudaMemcpyDeviceToHost, stream));
-    CU(cudaStreamSynchronize(stream));
-    std::vector<int> vcnt((size_t)n_scenes);
-    CU(cudaMemcpy(vcnt.data(), f.vis_cnt, 4 * (size_t)n_scenes, cudaMemcpyDeviceToHost));
-    long long tot = 0; int mx = 0;
-    for (int v : vcnt) { tot += v; mx = std::max(mx, v); }
-    (void)vc;
-    fprintf(stderr, "[sb200] dense frame: fallback reasons threshold %d, max-list overflow %d, no maximum %d; max candidates %d; pairs to refine %lld (largest scene %d)\n",
-            hc[0], hc[1], hc[2], hc[3], tot, mx);
-  }
-  CU(cudaEventRecord(q.done, stream));
-  if (!ev_set_free[cset]) CU(cudaEventCreateWithFlags(&ev_set_free[cset], cudaEventDisableTiming));
-  CU(cudaEventRecord(ev_set_free[cset], stream));   // this frame's candidate buffers may be rewritten after this point
-  set_busy[cset] = true;
-  if (has_user_stream && join_per_call) {   // the caller's stream continues after the frame
-    CU(cudaEventRecord(ev_user_out, stream));
-    CU(cudaStreamWaitEvent(user_stream, ev_user_out, 0));
-  }
+  if ((rc = plan_frame(rq, q, pl))) return rc;
+  sb::Frame f{};   // bind_frame sets what the frame uses, the rest stays zero
+  sb::TcArgs tc{};
+  if ((rc = bind_frame(rq, pl, f, tc))) return rc;
+  // ==================================================== nothing below can fail for capacity reasons: the request is committed
+  Rollback rollback = commit(rq, pl, q);
+  const double ms_setup = since();
+  if ((rc = enqueue(rq, pl, q, f, tc))) return rc;
   rollback.armed = false;
-  if (sin) { CU(cudaEventRecord(sin->ev_read, stream)); sin->read_pending = true; }
-  const double ms_launch = since(t_begin);
+  if (pl.sin) { CU(cudaEventRecord(pl.sin->ev_read, stream)); pl.sin->read_pending = true; }
+  const double ms_launch = since();
   if (wait) rc = drain();
-  host_ms_total += since(t_begin);
+  host_ms_total += since();
   host_calls += 1;
-  if (trace && prefetched && sin && wait) {
+  if (trace && pl.prefetched && wait) {
     float cms = 0.0f;
-    if (cudaEventElapsedTime(&cms, sin->ev0, sin->ev) == cudaSuccess)
+    if (cudaEventElapsedTime(&cms, pl.sin->ev0, pl.sin->ev) == cudaSuccess)
       fprintf(stderr, "[sb200] prefetch copy of this frame took %.3f ms on the copy stream\n", cms);
   }
-  if (trace) fprintf(stderr, "[sb200] predict: setup %.3f ms, launched at %.3f ms, returned at %.3f ms (total dets %d, %d in flight)\n", ms_setup, ms_launch, since(t_begin), total, pend_count);
+  if (trace) fprintf(stderr, "[sb200] predict: setup %.3f ms, launched at %.3f ms, returned at %.3f ms (total dets %d, %d in flight)\n", ms_setup, ms_launch, since(), rq.total, pend_count);
   return rc;
 }
 
-#undef ENS
 // =============================================================================================== C ABI
 extern "C" {
 
@@ -1530,6 +1527,19 @@ int sb200_tracker_create(const sb200_options* opts, sb200_tracker** out) {
     if (e == cudaSuccess) e = cudaEventCreateWithFlags(&g.ev_read, cudaEventDisableTiming);
     if (e != cudaSuccess) { delete t; return fail(SB200_ERR_CUDA, "cudaEventCreate failed: %s", cudaGetErrorString(e)); }
   }
+  // the internal streams, and the events of the frame ring and of the fork / join points
+  e = cudaStreamCreateWithPriority(&t->side_stream, cudaStreamNonBlocking, prio_hi);
+  if (e == cudaSuccess) e = cudaStreamCreateWithPriority(&t->prep_stream, cudaStreamNonBlocking, prio_lo);
+  for (cudaEvent_t* p : {&t->ev_fork[0], &t->ev_fork[1], &t->ev_join, &t->ev_prep_done, &t->ev_inputs, &t->ev_cost_done,
+                         &t->ev_set_free[0], &t->ev_set_free[1]})
+    if (e == cudaSuccess) e = cudaEventCreateWithFlags(p, cudaEventDisableTiming);
+  for (auto& q : t->pend) {
+    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&q.done, cudaEventDisableTiming);
+    for (auto& x : q.ev) if (e == cudaSuccess) e = cudaEventCreate(&x);
+    for (auto& x : q.ev_k) if (e == cudaSuccess) e = cudaEventCreate(&x);
+    for (auto& x : q.ev_pos) if (e == cudaSuccess) e = cudaEventCreate(&x);
+  }
+  if (e != cudaSuccess) { delete t; return fail(SB200_ERR_CUDA, "stream / event creation failed: %s", cudaGetErrorString(e)); }
   if (opts->max_scenes_hint > 0 || opts->max_tracks_per_scene_hint > 0) {
     // + room for the tracks the frames in flight may add (see predict())
     rc = t->ensure_store(std::max(1, opts->max_scenes_hint),
@@ -1616,7 +1626,7 @@ int sb200_set_feature_dim(sb200_tracker* t, int32_t feature_dim) {
     if ((rc = c.buf->ensure(rows * c.w))) return rc;
     c.point(*t, c.buf->p);
   }
-  for (auto& g : t->stg) g.feat.release();
+  for (auto& g : t->stg) g.col[sb200_tracker::kFeat].release();   // the staged features: their row width changed
   return 0;
 }
 
@@ -1704,39 +1714,30 @@ int sb200_prefetch_inputs(sb200_tracker* t, int32_t total, const float* boxes, c
   if (!t || total < 0 || (total > 0 && !boxes)) return fail(SB200_ERR_INVALID, "bad arguments");
   CU(cudaSetDevice(t->device));
   if (total == 0) return 0;
-  if (!t->P.is_visual) { features = nullptr; has_feature = nullptr; quality = nullptr; own_area = nullptr; }
   if (!t->copy_stream) CU(cudaStreamCreateWithFlags(&t->copy_stream, cudaStreamNonBlocking));
   // a free set: not holding an unconsumed prefetch; with nothing pending, the one the last predict did not read
   if (t->stg[0].pending && t->stg[1].pending)
     return fail(SB200_ERR_INVALID, "two prefetched requests are already waiting for their predict call");
   const int k = t->stg[0].pending ? 1 : (t->stg[1].pending ? 0 : 1 - t->stg_last);
   sb200_tracker::Staging& S = t->stg[k];
-  // capacity exactly as predict() sizes it (hints included), so the predict call never reallocates a filled set
-  const size_t T = (size_t)std::max<long long>(total, (long long)t->opts.max_scenes_hint * t->opts.max_dets_per_scene_hint);
-  const size_t n = (size_t)total;
+  const sb200_tracker::InPtrs in = t->in_ptrs(boxes, features, has_feature, quality, custom_ids, own_area);
+  const auto ic = t->in_cols();
+  // rows as predict() sizes them (the scene count is not known yet), so the predict call never reallocates a filled set
+  const size_t T = t->frame_rows(total, 0);
   int rc = 0;
   cudaStream_t cs = t->copy_stream;
-  if (features == nullptr) has_feature = nullptr;
   // the set's previous reader (a frame that may still be in flight) finishes first; a reallocation meets the device
-  const size_t fbytes = t->feat_bytes();
-  if (S.boxes.bytes < T * 24 || (features && S.feat.bytes < T * (size_t)t->P.feature_dim * fbytes) || (has_feature && S.hasf.bytes < T) ||
-      (quality && S.quality.bytes < T * 4) || (custom_ids && S.custom.bytes < T * 8) || (own_area && S.own.bytes < T * 4)) {
-    if ((rc = t->drain())) return rc;
-  }
+  bool grows = false;
+  for (int c = 0; c < sb200_tracker::kInCols; ++c) grows |= in[c] && S.col[c].bytes < T * ic[c].w;
+  if (grows && (rc = t->drain())) return rc;
   if (S.read_pending) { CU(cudaStreamWaitEvent(cs, S.ev_read, 0)); S.read_pending = false; }
-  if ((rc = S.boxes.ensure(T * 24))) return rc;
+  for (int c = 0; c < sb200_tracker::kInCols; ++c)
+    if (in[c] && (rc = S.col[c].ensure(T * ic[c].w))) return rc;
   CU(cudaEventRecord(S.ev0, cs));
-  CU(cudaMemcpyAsync(S.boxes.p, boxes, n * 24, cudaMemcpyHostToDevice, cs));
-  if (features) {
-    if ((rc = S.feat.ensure(T * (size_t)t->P.feature_dim * fbytes))) return rc;
-    CU(cudaMemcpyAsync(S.feat.p, features, n * (size_t)t->P.feature_dim * fbytes, cudaMemcpyHostToDevice, cs));
-    if (has_feature) { if ((rc = S.hasf.ensure(T))) return rc; CU(cudaMemcpyAsync(S.hasf.p, has_feature, n, cudaMemcpyHostToDevice, cs)); }
-  }
-  if (quality) { if ((rc = S.quality.ensure(T * 4))) return rc; CU(cudaMemcpyAsync(S.quality.p, quality, n * 4, cudaMemcpyHostToDevice, cs)); }
-  if (custom_ids) { if ((rc = S.custom.ensure(T * 8))) return rc; CU(cudaMemcpyAsync(S.custom.p, custom_ids, n * 8, cudaMemcpyHostToDevice, cs)); }
-  if (own_area) { if ((rc = S.own.ensure(T * 4))) return rc; CU(cudaMemcpyAsync(S.own.p, own_area, n * 4, cudaMemcpyHostToDevice, cs)); }
+  for (int c = 0; c < sb200_tracker::kInCols; ++c)
+    if (in[c]) CU(cudaMemcpyAsync(S.col[c].p, in[c], (size_t)total * ic[c].w, cudaMemcpyHostToDevice, cs));
   CU(cudaEventRecord(S.ev, cs));
-  S.key[0] = boxes; S.key[1] = features; S.key[2] = has_feature; S.key[3] = quality; S.key[4] = custom_ids; S.key[5] = own_area;
+  S.key = in;
   S.total = total; S.type = t->feat_type; S.pending = true;
   return 0;
 }
@@ -2020,9 +2021,10 @@ int64_t sb200_last_costs(sb200_tracker* t, uint64_t scene_id, int64_t cap, float
     // the dense matrix exists for scenes in dense voting mode and in SB200_FULL_COSTS runs; elsewhere the entry list is
     // the matrix (None wherever no entry is listed)
     int h[2] = {0, 0};   // pos_cnt, scene_mode
-    const int ns = t->last_n_scenes;
-    CU(cudaMemcpyAsync(&h[0], t->f_counters.as<int>() + si, 4, cudaMemcpyDeviceToHost, t->stream));
-    CU(cudaMemcpyAsync(&h[1], t->f_counters.as<int>() + 2 * (size_t)ns + si, 4, cudaMemcpyDeviceToHost, t->stream));
+    sb::Frame ctr{};
+    sb200_tracker::carve_counters(t->f_counters.as<int>(), t->last_n_scenes, ctr);
+    CU(cudaMemcpyAsync(&h[0], ctr.pos_cnt + si, 4, cudaMemcpyDeviceToHost, t->stream));
+    CU(cudaMemcpyAsync(&h[1], ctr.scene_mode + si, 4, cudaMemcpyDeviceToHost, t->stream));
     CU(cudaStreamSynchronize(t->stream));
     const bool dense_exists = h[1] != 0 || getenv("SB200_FULL_COSTS") != nullptr;
     if (dense_exists) {

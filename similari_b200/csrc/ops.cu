@@ -247,18 +247,15 @@ int sb200_visual_cost_matrix(int32_t visual_kind, float threshold, const float* 
   fill_u8_kernel<<<(n + 255) / 256, 256, 0, sc.st>>>(ts.feat_cnt, 1, n);
   sb::launch_prep(p, f, 1, m, sc.st);
   fill_u8_kernel<<<(m + 255) / 256, 256, 0, sc.st>>>(f.c_flags, 3, m);
-  // same kernel selection rule as the tracker (engine.cu): tensor-core screen + exact refinement for large
-  // contractions with a selective threshold; SB200_VIS_KERNEL=simt|tc|tc16|tc8 overrides.  The operator has no frames to
-  // learn the e4m3 screen's selectivity from: it screens on BF16 unless tc8 asks for e4m3 operands (d8 <= 512).
+  // the tracker's path rule (sb_engine.cuh), except that the operator has no dense path, and no frames to learn the e4m3
+  // screen's selectivity from: it screens on BF16 unless SB200_VIS_KERNEL=tc8 asks for e4m3 operands (d8 <= 512)
   sb::TcArgs tc;
   memset(&tc, 0, sizeof(tc));
-  const bool selective = visual_kind == SB200_VIS_EUCLIDEAN ? (threshold < 1e18f) : (threshold > -1.0f);
-  tc.use_tc = selective && p.d8 >= 64 && (long long)m * n * p.d8 >= (1ll << 28);
-  if (const char* ev = getenv("SB200_VIS_KERNEL")) {
-    if (!strcmp(ev, "simt")) tc.use_tc = false;
-    else if (!strcmp(ev, "tc") || !strcmp(ev, "tc16")) tc.use_tc = true;
-    else if (!strcmp(ev, "tc8")) { tc.use_tc = true; tc.fp8 = p.d8 <= sb::kFp8MaxD8; }
-  }
+  const sb::VisKernel vk = sb::vis_kernel_env();
+  tc.use_tc = vk == sb::kVisTc || vk == sb::kVisTc8 || vk == sb::kVisTc16 ||
+              (vk != sb::kVisSimt && sb::vis_selective(visual_kind == SB200_VIS_EUCLIDEAN, threshold) &&
+               sb::vis_tc_worth(p.d8, (long long)m * n));
+  tc.fp8 = vk == sb::kVisTc8 && p.d8 <= sb::kFp8MaxD8;
   f.scene_max = sc.alloc<unsigned int>(1);
   cudaDeviceGetAttribute(&tc.num_sms, cudaDevAttrMultiProcessorCount, device);
   {
@@ -370,12 +367,12 @@ static int run_voting(bool visual, float threshold, int min_votes, const float* 
     f.scene_mode = f.pos_cnt + 2;
     f.vis_mode = f.pos_cnt + 3;
   }
-  // one scene, list slices sized as the tracker sizes them (engine.cu, predict)
+  // one scene, list slices sized as the tracker sizes them
   sb::SceneDesc sd;
   memset(&sd, 0, sizeof(sd));
   sd.m = m; sd.n = n; sd.epoch = 1;
-  sd.pos_lcap = (int)std::min<long long>((long long)m * 32, (long long)sb::kVotePosCap * 2);
-  sd.vis_lcap = visual ? (int)std::min<long long>((long long)m * 64, (long long)sb::kVoteVisCap * 4) : 0;
+  sd.pos_lcap = sb::pos_lcap(m);
+  sd.vis_lcap = visual ? sb::vis_lcap(m, sb::kVoteVisCap) : 0;
   f.scenes = sc.upload(&sd, 1);
   f.pos_list = sc.alloc<sb::PosEntry>(sd.pos_lcap);
   if (visual) {

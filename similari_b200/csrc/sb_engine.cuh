@@ -17,6 +17,9 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <cstdlib>
+#include <cstring>
+
 #include "sb_math.cuh"
 
 namespace sb {
@@ -189,6 +192,35 @@ struct VisPair { int g, row, scene, outcol; };  // screen survivor: detection, f
 struct PosEntry { unsigned short m, n; float v; };  // one valid (candidate, track, cost) positional entry
 constexpr int kVotePosCap = 3072;   // sparse entries per scene the voting kernel keeps in shared memory
 constexpr int kVoteVisCap = 4096;   // power of two: the BestFit bitonic sort pads the list up to the next power of two
+
+// Host side: the slices of a scene of m detections in the sparse entry lists (SceneDesc::pos_lcap / vis_lcap);
+// vote_cap is the voting kernel's visual capacity (Params::vote_vis_cap).
+inline int pos_lcap(int m) {
+  const long long c = (long long)m * 32;
+  return (int)(c < 2ll * kVotePosCap ? c : 2ll * kVotePosCap);
+}
+inline int vis_lcap(int m, int vote_cap) {
+  const long long c = (long long)m * 64;
+  return (int)(c < 4ll * vote_cap ? c : 4ll * vote_cap);
+}
+// Visual cost path, shared by the tracker and the operators.  The tensor-core screen and its exact refinement pay off for
+// a selective threshold (one that can cut pairs) on rows of d8 >= 64 when the frame's dot products (`work`, pairs of
+// candidate and stored feature row) reach 2^28 multiply-adds; smaller frames take the exact SIMT kernel.
+inline bool vis_selective(bool euclidean, float threshold) { return euclidean ? threshold < 1e18f : threshold > -1.0f; }
+inline bool vis_tc_worth(int d8, long long work) { return d8 >= 64 && work * d8 >= (1ll << 28); }
+// SB200_VIS_KERNEL=simt|tc|tc8|tc16|dense forces a path (tc8 / tc16: the screen on e4m3 / BF16 operands); any other
+// value, or none, leaves the choice to the rule.  Read on every call: tests switch it between calls.
+enum VisKernel { kVisRule, kVisSimt, kVisTc, kVisTc8, kVisTc16, kVisDense };
+inline VisKernel vis_kernel_env() {
+  const char* e = getenv("SB200_VIS_KERNEL");
+  if (!e) return kVisRule;
+  if (!strcmp(e, "simt")) return kVisSimt;
+  if (!strcmp(e, "tc")) return kVisTc;
+  if (!strcmp(e, "tc8")) return kVisTc8;
+  if (!strcmp(e, "tc16")) return kVisTc16;
+  if (!strcmp(e, "dense")) return kVisDense;
+  return kVisRule;
+}
 
 struct TrackStore {
   int track_cap;
