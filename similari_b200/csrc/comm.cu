@@ -17,10 +17,11 @@
 #include <string>
 
 #include "../../include/similari_b200.h"
-
-extern "C" void sb200__set_error(const char* msg);   // engine.cu
+#include "sb_host.cuh"
 
 namespace {
+
+using sb::fail;
 
 typedef struct ncclComm* ncclComm_t;
 typedef struct { char internal[128]; } ncclUniqueId;
@@ -65,11 +66,6 @@ Nccl* nccl() {
   return &n;
 }
 
-int cfail(int code, const std::string& msg) {
-  sb200__set_error(msg.c_str());
-  return code;
-}
-
 }  // namespace
 
 struct sb200_comm {
@@ -80,15 +76,15 @@ struct sb200_comm {
 #define NC(x)                                                                                            \
   do {                                                                                                   \
     int r_ = (x);                                                                                        \
-    if (r_ != 0) return cfail(SB200_ERR_CUDA, std::string(#x " failed: ") + nccl()->GetErrorString(r_)); \
+    if (r_ != 0) return fail(SB200_ERR_CUDA, "%s failed: %s", #x, nccl()->GetErrorString(r_));            \
   } while (0)
 
 extern "C" {
 
 int sb200_comm_unique_id(void* out128) {
-  if (!out128) return cfail(SB200_ERR_INVALID, "out128 is NULL");
+  if (!out128) return fail(SB200_ERR_INVALID, "out128 is NULL");
   Nccl* n = nccl();
-  if (!n->h) return cfail(SB200_ERR_CUDA, n->err);
+  if (!n->h) return fail(SB200_ERR_CUDA, "%s", n->err.c_str());
   ncclUniqueId id;
   NC(n->GetUniqueId(&id));
   memcpy(out128, &id, 128);
@@ -96,17 +92,17 @@ int sb200_comm_unique_id(void* out128) {
 }
 
 int sb200_comm_create(int32_t rank, int32_t world, const void* id128, int32_t device, sb200_comm** out) {
-  if (!id128 || !out || world < 1 || rank < 0 || rank >= world) return cfail(SB200_ERR_INVALID, "bad arguments");
+  if (!id128 || !out || world < 1 || rank < 0 || rank >= world) return fail(SB200_ERR_INVALID, "bad arguments");
   *out = nullptr;
   Nccl* n = nccl();
-  if (!n->h) return cfail(SB200_ERR_CUDA, n->err);
-  if (cudaSetDevice(device) != cudaSuccess) return cfail(SB200_ERR_CUDA, "cudaSetDevice failed");
+  if (!n->h) return fail(SB200_ERR_CUDA, "%s", n->err.c_str());
+  if (cudaSetDevice(device) != cudaSuccess) return fail(SB200_ERR_CUDA, "cudaSetDevice failed");
   ncclUniqueId id;
   memcpy(&id, id128, 128);
   sb200_comm* c = new sb200_comm();
   c->rank = rank; c->world = world; c->device = device;
   int r = n->CommInitRank(&c->comm, world, id, rank);
-  if (r != 0) { delete c; return cfail(SB200_ERR_CUDA, std::string("ncclCommInitRank failed: ") + n->GetErrorString(r)); }
+  if (r != 0) { delete c; return fail(SB200_ERR_CUDA, "ncclCommInitRank failed: %s", n->GetErrorString(r)); }
   *out = c;
   return 0;
 }
@@ -122,7 +118,7 @@ void sb200_comm_destroy(sb200_comm* c) {
 static int exchange(sb200_comm* c, int root, const int32_t* det_range, int ncols, const size_t* row_bytes,
                     void* const* root_cols, void* const* my_cols, bool scatter, cudaStream_t st) {
   Nccl* n = nccl();
-  if (cudaSetDevice(c->device) != cudaSuccess) return cfail(SB200_ERR_CUDA, "cudaSetDevice failed");
+  if (cudaSetDevice(c->device) != cudaSuccess) return fail(SB200_ERR_CUDA, "cudaSetDevice failed");
   const int me = c->rank;
   const size_t my_rows = (size_t)(det_range[me + 1] - det_range[me]);
   NC(n->GroupStart());
@@ -130,7 +126,7 @@ static int exchange(sb200_comm* c, int root, const int32_t* det_range, int ncols
     if (!my_cols[k]) continue;
     const size_t rb = row_bytes[k];
     if (me == root) {
-      if (!root_cols[k]) { n->GroupEnd(); return cfail(SB200_ERR_INVALID, "root column is NULL"); }
+      if (!root_cols[k]) { n->GroupEnd(); return fail(SB200_ERR_INVALID, "root column is NULL"); }
       char* all = reinterpret_cast<char*>(root_cols[k]);
       for (int r = 0; r < c->world; ++r) {
         const size_t rows = (size_t)(det_range[r + 1] - det_range[r]);
@@ -158,7 +154,7 @@ int sb200_shard_scatter(sb200_comm* c, int32_t root, const int32_t* det_range, i
                         const float* all_features, const uint8_t* all_has_feature, const float* all_quality,
                         const int64_t* all_custom_ids, float* my_boxes, float* my_features, uint8_t* my_has_feature,
                         float* my_quality, int64_t* my_custom_ids, void* cuda_stream) {
-  if (!c || !det_range || root < 0 || root >= c->world || !my_boxes) return cfail(SB200_ERR_INVALID, "bad arguments");
+  if (!c || !det_range || root < 0 || root >= c->world || !my_boxes) return fail(SB200_ERR_INVALID, "bad arguments");
   const size_t rb[5] = {24, (size_t)feature_dim * 4, 1, 4, 8};
   void* rootc[5] = {(void*)all_boxes, (void*)all_features, (void*)all_has_feature, (void*)all_quality, (void*)all_custom_ids};
   void* myc[5] = {my_boxes, my_features, my_has_feature, my_quality, my_custom_ids};
@@ -167,8 +163,8 @@ int sb200_shard_scatter(sb200_comm* c, int32_t root, const int32_t* det_range, i
 
 int sb200_shard_gather(sb200_comm* c, int32_t root, const int32_t* det_range, const sb200_predict_out* mine,
                        const sb200_predict_out* all, void* cuda_stream) {
-  if (!c || !det_range || root < 0 || root >= c->world || !mine) return cfail(SB200_ERR_INVALID, "bad arguments");
-  if (c->rank == root && !all) return cfail(SB200_ERR_INVALID, "the root needs the `all` columns");
+  if (!c || !det_range || root < 0 || root >= c->world || !mine) return fail(SB200_ERR_INVALID, "bad arguments");
+  if (c->rank == root && !all) return fail(SB200_ERR_INVALID, "the root needs the `all` columns");
   const size_t rb[6] = {8, 4, 4, 1, 24, 24};
   sb200_predict_out none{};
   const sb200_predict_out& a = all ? *all : none;

@@ -9,7 +9,6 @@
 #include <cmath>
 #include <cstddef>
 #include <cstdlib>
-#include <cstdarg>
 #include <cstdio>
 #include <cstring>
 #include <map>
@@ -21,6 +20,7 @@
 
 #include "../../include/similari_b200.h"
 #include "sb_engine.cuh"
+#include "sb_host.cuh"
 
 #include <atomic>
 
@@ -30,94 +30,11 @@ void note_launch(int n) { g_launches.fetch_add((unsigned long long)n, std::memor
 unsigned long long launch_count() { return g_launches.load(std::memory_order_relaxed); }
 }  // namespace sb
 
+using sb::DBuf;
+using sb::HBuf;
+using sb::fail;
+
 namespace {
-
-thread_local std::string g_err;
-
-int fail(int code, const char* fmt, ...) {
-  char buf[512];
-  va_list ap;
-  va_start(ap, fmt);
-  vsnprintf(buf, sizeof(buf), fmt, ap);
-  va_end(ap);
-  g_err = buf;
-  return code;
-}
-
-#define CU(x)                                                                                  \
-  do {                                                                                         \
-    cudaError_t e_ = (x);                                                                      \
-    if (e_ != cudaSuccess)                                                                     \
-      return fail(SB200_ERR_CUDA, "%s failed: %s (%s:%d)", #x, cudaGetErrorString(e_), __FILE__, __LINE__); \
-  } while (0)
-
-// grow-only device buffer; it owns its memory (move-only, freed by the destructor)
-struct DBuf {
-  void* p = nullptr;
-  size_t bytes = 0;
-  DBuf() = default;
-  DBuf(const DBuf&) = delete;
-  DBuf& operator=(const DBuf&) = delete;
-  DBuf(DBuf&& o) noexcept : p(o.p), bytes(o.bytes) { o.p = nullptr; o.bytes = 0; }
-  DBuf& operator=(DBuf&& o) noexcept {
-    if (this != &o) { release(); p = o.p; bytes = o.bytes; o.p = nullptr; o.bytes = 0; }
-    return *this;
-  }
-  ~DBuf() { release(); }
-  int ensure(size_t need) {
-    if (need <= bytes) return 0;
-    size_t nb = std::max(need, bytes + bytes / 2);
-    void* np = nullptr;
-    cudaError_t e = cudaMalloc(&np, nb);
-    if (e != cudaSuccess) return fail(SB200_ERR_CUDA, "cudaMalloc(%zu) failed: %s", nb, cudaGetErrorString(e));
-    if (p) cudaFree(p);
-    p = np;
-    bytes = nb;
-    return 0;
-  }
-  void release() {
-    if (p) cudaFree(p);
-    p = nullptr;
-    bytes = 0;
-  }
-  template <typename T> T* as() const { return reinterpret_cast<T*>(p); }
-};
-
-struct HBuf {  // grow-only pinned host buffer, mapped into the device address space (dp); owns its memory like DBuf
-  void* p = nullptr;
-  void* dp = nullptr;   // device-side alias: kernels can read the buffer over PCIe without a copy-engine transfer
-  size_t bytes = 0;
-  HBuf() = default;
-  HBuf(const HBuf&) = delete;
-  HBuf& operator=(const HBuf&) = delete;
-  HBuf(HBuf&& o) noexcept : p(o.p), dp(o.dp), bytes(o.bytes) { o.p = o.dp = nullptr; o.bytes = 0; }
-  HBuf& operator=(HBuf&& o) noexcept {
-    if (this != &o) { release(); p = o.p; dp = o.dp; bytes = o.bytes; o.p = o.dp = nullptr; o.bytes = 0; }
-    return *this;
-  }
-  ~HBuf() { release(); }
-  int ensure(size_t need) {
-    if (need <= bytes) return 0;
-    HBuf nb;   // freed on failure
-    const size_t n = std::max(need, bytes + bytes / 2);
-    void* np = nullptr;
-    cudaError_t e = cudaHostAlloc(&np, n, cudaHostAllocMapped);
-    if (e != cudaSuccess) return fail(SB200_ERR_CUDA, "cudaHostAlloc(%zu) failed: %s", n, cudaGetErrorString(e));
-    nb.p = np;
-    e = cudaHostGetDevicePointer(&nb.dp, nb.p, 0);
-    if (e != cudaSuccess) return fail(SB200_ERR_CUDA, "cudaHostGetDevicePointer failed: %s", cudaGetErrorString(e));
-    nb.bytes = n;
-    *this = std::move(nb);
-    return 0;
-  }
-  void release() {
-    if (p) cudaFreeHost(p);
-    p = nullptr;
-    dp = nullptr;
-    bytes = 0;
-  }
-  template <typename T> T* as() const { return reinterpret_cast<T*>(p); }
-};
 
 // A column of the tracker's device state (sb200_tracker::store_table, slot_table, wasted_table, pool_table): the buffer
 // that owns it, the TrackStore / WastedBuf pointer the kernels read it through, and its row width.  `rows` says what a
@@ -207,7 +124,6 @@ struct sb200_tracker {
   // frame -- the stream-order contract, without the library's kernels sitting in the caller's stream (so the library is free
   // to start the next frame's candidate preparation under the current frame, see prep_stream).
   cudaStream_t stream = nullptr;
-  bool own_stream = true;
   cudaStream_t user_stream = nullptr;   // valid when has_user_stream (0 is the legacy default stream)
   bool has_user_stream = false;
   bool join_per_call = true;   // the caller's stream waits for every call's frame (else: sb200_stream_join)
@@ -390,7 +306,7 @@ struct sb200_tracker {
     for (cudaEvent_t e : {ev_user_in, ev_user_out, ev_prep_done, ev_set_free[0], ev_set_free[1], ev_inputs, ev_join_req, ev_cost_done}) if (e) cudaEventDestroy(e);
     for (auto& e : ev_fork) if (e) cudaEventDestroy(e);
     if (ev_join) cudaEventDestroy(ev_join);
-    if (own_stream && stream) cudaStreamDestroy(stream);
+    if (stream) cudaStreamDestroy(stream);
   }
 
   template <auto F> static void in_ts(sb200_tracker& t, void* p) { t.ts.*F = static_cast<std::remove_reference_t<decltype(t.ts.*F)>>(p); }
@@ -1069,12 +985,12 @@ struct sb200_tracker {
     f.c_fp8 = tc.fp8 ? cb.fp8.as<unsigned char>() : nullptr;
     f.c_scale = tc.fp8 ? cb.scale.as<float>() : nullptr;
     if ((rc = ENS(f_poslist, sizeof(sb::PosEntry) * (size_t)std::max<long long>(1, std::max(pl.posl_total, hint_dets(n_scenes) * 32)), f.pos_list)) ||
-        (rc = ENS(f_counters, sizeof(int) * counter_ints(n_scenes))))
+        (rc = ENS(f_counters, sizeof(int) * sb::counter_ints(n_scenes))))
       return rc;
     if (P.is_visual && ((rc = ENS(f_pairs, sizeof(sb::VisPair) * (size_t)std::max<long long>(1, visl_alloc), f.vis_pairs)) ||
                         (rc = ENS(f_visval, sizeof(float) * (size_t)std::max<long long>(1, visl_alloc), f.vis_val))))
       return rc;
-    carve_counters(f_counters.as<int>(), n_scenes, f);
+    sb::carve_counters(f_counters.as<int>(), n_scenes, f);
     if (!tc.use_tc || tc.dense) f.screen_cnt = nullptr;   // only the screen counts its survivors
     // outputs: the caller's device columns, or staged and copied back by enqueue()
     const std::array<OutCol, kOutCols> oc = out_cols(rq.out);
@@ -1128,7 +1044,6 @@ struct sb200_tracker {
     sb::Params Pf = P;
     Pf.vote_vis_cap = pl.vote_cap;
     if (has_user_stream) {   // everything the caller's stream holds now comes first
-      if (!ev_user_in) { CU(cudaEventCreateWithFlags(&ev_user_in, cudaEventDisableTiming)); CU(cudaEventCreateWithFlags(&ev_user_out, cudaEventDisableTiming)); }
       CU(cudaEventRecord(ev_user_in, user_stream));
       CU(cudaStreamWaitEvent(stream, ev_user_in, 0));
     }
@@ -1161,7 +1076,7 @@ struct sb200_tracker {
     }
     sb::launch_frame_setup(P, ts, f, reinterpret_cast<const sb::SceneReq*>(q.h_req.dp), n_scenes, b_ntracks.as<int>(), pl.mstep,
                            pl.cstep, tc.dense, f_tiles.as<sb::TcTile>(), f_dyn.as<sb::FrameDyn>(), f_counters.as<int>(),
-                           (int)counter_ints(n_scenes), s_setup);
+                           (int)sb::counter_ints(n_scenes), s_setup);
     tc.max_init_done = 1;   // frame_setup resets scene_max
     if (side_setup && Pf.is_visual && tc.use_tc && !tc.dense && tc.n_tiles > 0 && max_m > 0 && max_n > 0 && f.in_feat) {
       // the screen's column metadata reads the tables and the store only: it follows the setup on the side stream
@@ -1254,7 +1169,7 @@ struct sb200_tracker {
     }
     FrameBack* back = q.back();
     sb::Frame cnt{};   // the counters, screen_cnt included on every path (zeros where nothing counts)
-    carve_counters(f_counters.as<int>(), n_scenes, cnt);
+    sb::carve_counters(f_counters.as<int>(), n_scenes, cnt);
     CU(cudaMemcpyAsync(q.h_out.p, f.frame_out, 12 * (size_t)n_scenes, cudaMemcpyDeviceToHost, stream));
     CU(cudaMemcpyAsync(q.h_out.as<char>() + 12 * (size_t)n_scenes, cnt.status, 4 * (size_t)n_scenes, cudaMemcpyDeviceToHost, stream));
     CU(cudaMemcpyAsync(&back->dyn, f_dyn.p, sizeof(back->dyn), cudaMemcpyDeviceToHost, stream));
@@ -1283,15 +1198,6 @@ struct sb200_tracker {
     return 0;
   }
 
-  // The per-scene counters of a frame (f_counters), zeroed together by frame_setup_kernel: pos_cnt | vis_cnt | scene_mode |
-  // vis_mode | refine_next | status, [n] ints each, then dense_cnt and screen_cnt[3].
-  static size_t counter_ints(int n) { return 6 * (size_t)n + 4; }
-  static void carve_counters(int* c, int n, sb::Frame& f) {
-    using F = sb::Frame;
-    int* F::* const rows[] = {&F::pos_cnt, &F::vis_cnt, &F::scene_mode, &F::vis_mode, &F::refine_next, &F::status, &F::dense_cnt};
-    for (int i = 0; i < 7; ++i) f.*rows[i] = c + (size_t)i * n;
-    f.screen_cnt = f.dense_cnt + 1;
-  }
   // The per-scene block of the dense path (f_dscene): maxc_cnt | maxc_next | dense_bad | zeros ([n] ints each, zeroed
   // together), scene_l0 | scene_cmax ([n] floats each), 4 unused ints, dbg_counts[8].
   static size_t dscene_bytes(int n) { return 4 * 6 * (size_t)n + 128; }
@@ -1469,14 +1375,9 @@ int sb200_tracker::predict(int32_t n_scenes, const uint64_t* scene_ids, const in
 // =============================================================================================== C ABI
 extern "C" {
 
-const char* sb200_last_error(void) { return g_err.c_str(); }
-void sb200__set_error(const char* msg) { g_err = msg ? msg : ""; }  // used by ops.cu / nms
+const char* sb200_last_error(void) { return sb::g_err.c_str(); }
 
-int sb200_device_count(void) {
-  int n = 0;
-  if (cudaGetDeviceCount(&n) != cudaSuccess) { cudaGetLastError(); return 0; }
-  return n;
-}
+int sb200_device_count(void) { return sb::device_count(); }
 
 void sb200_options_default(sb200_options* o) {
   if (!o) return;
@@ -1499,11 +1400,10 @@ void sb200_options_default(sb200_options* o) {
 int sb200_tracker_create(const sb200_options* opts, sb200_tracker** out) {
   if (!opts || !out) return fail(SB200_ERR_INVALID, "opts / out is NULL");
   *out = nullptr;
-  int ndev = sb200_device_count();
-  if (ndev <= 0) return fail(SB200_ERR_CUDA, "no CUDA device available (this library has no CPU execution path)");
-  if (opts->device < 0 || opts->device >= ndev) return fail(SB200_ERR_INVALID, "device %d out of range (%d devices)", opts->device, ndev);
+  int rc = sb::check_device(opts->device);
+  if (rc) return rc;
   sb::Params P;
-  int rc = make_params(*opts, &P);
+  rc = make_params(*opts, &P);
   if (rc) return rc;
   CU(cudaSetDevice(opts->device));
   sb200_tracker* t = new sb200_tracker();
@@ -1527,11 +1427,11 @@ int sb200_tracker_create(const sb200_options* opts, sb200_tracker** out) {
     if (e == cudaSuccess) e = cudaEventCreateWithFlags(&g.ev_read, cudaEventDisableTiming);
     if (e != cudaSuccess) { delete t; return fail(SB200_ERR_CUDA, "cudaEventCreate failed: %s", cudaGetErrorString(e)); }
   }
-  // the internal streams, and the events of the frame ring and of the fork / join points
+  // the internal streams, and the events of the frame ring, of the fork / join points and of the caller-stream joins
   e = cudaStreamCreateWithPriority(&t->side_stream, cudaStreamNonBlocking, prio_hi);
   if (e == cudaSuccess) e = cudaStreamCreateWithPriority(&t->prep_stream, cudaStreamNonBlocking, prio_lo);
   for (cudaEvent_t* p : {&t->ev_fork[0], &t->ev_fork[1], &t->ev_join, &t->ev_prep_done, &t->ev_inputs, &t->ev_cost_done,
-                         &t->ev_set_free[0], &t->ev_set_free[1]})
+                         &t->ev_set_free[0], &t->ev_set_free[1], &t->ev_user_in, &t->ev_user_out})
     if (e == cudaSuccess) e = cudaEventCreateWithFlags(p, cudaEventDisableTiming);
   for (auto& q : t->pend) {
     if (e == cudaSuccess) e = cudaEventCreateWithFlags(&q.done, cudaEventDisableTiming);
@@ -2022,7 +1922,7 @@ int64_t sb200_last_costs(sb200_tracker* t, uint64_t scene_id, int64_t cap, float
     // the matrix (None wherever no entry is listed)
     int h[2] = {0, 0};   // pos_cnt, scene_mode
     sb::Frame ctr{};
-    sb200_tracker::carve_counters(t->f_counters.as<int>(), t->last_n_scenes, ctr);
+    sb::carve_counters(t->f_counters.as<int>(), t->last_n_scenes, ctr);
     CU(cudaMemcpyAsync(&h[0], ctr.pos_cnt + si, 4, cudaMemcpyDeviceToHost, t->stream));
     CU(cudaMemcpyAsync(&h[1], ctr.scene_mode + si, 4, cudaMemcpyDeviceToHost, t->stream));
     CU(cudaStreamSynchronize(t->stream));
@@ -2406,10 +2306,6 @@ int save_blob(sb200_tracker* t, uint32_t type, const std::vector<int>& slots, vo
 // blob that the caller's stream is still writing (a receive) or reading (a send) is complete before the blob calls touch it.
 int join_caller(sb200_tracker* t) {
   if (!t->has_user_stream) return 0;
-  if (!t->ev_user_in) {
-    CU(cudaEventCreateWithFlags(&t->ev_user_in, cudaEventDisableTiming));
-    CU(cudaEventCreateWithFlags(&t->ev_user_out, cudaEventDisableTiming));
-  }
   CU(cudaEventRecord(t->ev_user_in, t->user_stream));
   CU(cudaStreamWaitEvent(t->stream, t->ev_user_in, 0));
   return 0;
@@ -2516,10 +2412,10 @@ extern "C" {
 
 int sb200_tracker_save(sb200_tracker* t, void* dst, size_t cap, size_t* bytes) {
   if (!t || !bytes) return fail(SB200_ERR_INVALID, "tracker / bytes is NULL");
-  if (sb200_device_count() <= 0) return fail(SB200_ERR_CUDA, "no CUDA device available");
-  CU(cudaSetDevice(t->device));
-  int rc = t->drain();
+  int rc = sb::check_device(0);   // any device at all, before `t` is read
   if (rc) return rc;
+  CU(cudaSetDevice(t->device));
+  if ((rc = t->drain())) return rc;
   if ((rc = join_caller(t))) return rc;   // the caller's pending work on the destination comes first
   std::vector<int> slots(t->scene_of_slot.size());
   for (size_t i = 0; i < slots.size(); ++i) slots[i] = (int)i;
@@ -2529,13 +2425,12 @@ int sb200_tracker_save(sb200_tracker* t, void* dst, size_t cap, size_t* bytes) {
 int sb200_tracker_load(const void* src, size_t bytes, int32_t device, sb200_tracker** out) {
   if (!src || !out) return fail(SB200_ERR_INVALID, "src / out is NULL");
   *out = nullptr;
-  const int ndev = sb200_device_count();
-  if (ndev <= 0) return fail(SB200_ERR_CUDA, "no CUDA device available (this library has no CPU execution path)");
-  if (device < 0 || device >= ndev) return fail(SB200_ERR_INVALID, "device %d out of range (%d devices)", device, ndev);
+  int rc = sb::check_device(device);
+  if (rc) return rc;
   BlobHeader h;
   std::vector<BlobScene> table;
   // no tracker (and no caller stream) yet: a device blob must be complete when the call is made
-  int rc = parse_blob(src, bytes, kBlobTracker, nullptr, &h, &table);
+  rc = parse_blob(src, bytes, kBlobTracker, nullptr, &h, &table);
   if (rc) return rc;
   // created without the capacity hints, then sized to the source's store exactly (a save of the loaded tracker is the
   // same blob), then the hints restored for the growth of later frames
@@ -2603,10 +2498,10 @@ int sb200_tracker_load(const void* src, size_t bytes, int32_t device, sb200_trac
 int sb200_scenes_export(sb200_tracker* t, int32_t n_scenes, const uint64_t* scene_ids, int32_t remove, void* dst,
                         size_t cap, size_t* bytes) {
   if (!t || !bytes || n_scenes < 1 || !scene_ids) return fail(SB200_ERR_INVALID, "bad arguments");
-  if (sb200_device_count() <= 0) return fail(SB200_ERR_CUDA, "no CUDA device available");
-  CU(cudaSetDevice(t->device));
-  int rc = t->drain();
+  int rc = sb::check_device(0);   // any device at all, before `t` is read
   if (rc) return rc;
+  CU(cudaSetDevice(t->device));
+  if ((rc = t->drain())) return rc;
   std::vector<int> slots((size_t)n_scenes);
   std::unordered_map<uint64_t, int> seen;
   for (int i = 0; i < n_scenes; ++i) {
@@ -2634,10 +2529,10 @@ int sb200_scenes_export(sb200_tracker* t, int32_t n_scenes, const uint64_t* scen
 
 int sb200_scenes_import(sb200_tracker* t, const void* src, size_t bytes) {
   if (!t || !src) return fail(SB200_ERR_INVALID, "tracker / src is NULL");
-  if (sb200_device_count() <= 0) return fail(SB200_ERR_CUDA, "no CUDA device available");
-  CU(cudaSetDevice(t->device));
-  int rc = t->drain();
+  int rc = sb::check_device(0);   // any device at all, before `t` is read
   if (rc) return rc;
+  CU(cudaSetDevice(t->device));
+  if ((rc = t->drain())) return rc;
   BlobHeader h;
   std::vector<BlobScene> table;
   if ((rc = join_caller(t))) return rc;   // a blob the caller's stream is still writing is complete from here on
@@ -2701,7 +2596,7 @@ int sb200_tracker_options(sb200_tracker* t, sb200_options* out, int32_t* feature
 
 void* sb200_host_alloc(size_t bytes) {
   void* p = nullptr;
-  if (cudaMallocHost(&p, bytes) != cudaSuccess) { cudaGetLastError(); g_err = "cudaMallocHost failed"; return nullptr; }
+  if (cudaMallocHost(&p, bytes) != cudaSuccess) { cudaGetLastError(); fail(SB200_ERR_CUDA, "cudaMallocHost failed"); return nullptr; }
   return p;
 }
 void sb200_host_free(void* p) { if (p) cudaFreeHost(p); }

@@ -7,75 +7,18 @@
 #include <algorithm>
 #include <cmath>
 #include <cstring>
-#include <string>
 #include <unordered_map>
 #include <unordered_set>
 #include <vector>
 
 #include "../../include/similari_b200.h"
 #include "sb_fstore.cuh"
-
-extern "C" void sb200__set_error(const char* msg);  // engine.cu
+#include "sb_host.cuh"
 
 namespace {
 
-int fs_fail(int code, const std::string& msg) {
-  sb200__set_error(msg.c_str());
-  return code;
-}
-
-#define FS_CU(x)                                                                          \
-  do {                                                                                    \
-    cudaError_t e_ = (x);                                                                 \
-    if (e_ != cudaSuccess) return fs_fail(SB200_ERR_CUDA, std::string(#x " failed: ") + cudaGetErrorString(e_)); \
-  } while (0)
-
-// device memory owned by the handle (move-only)
-struct Dev {
-  void* p = nullptr;
-  size_t bytes = 0;
-  Dev() = default;
-  Dev(const Dev&) = delete;
-  Dev& operator=(const Dev&) = delete;
-  Dev(Dev&& o) noexcept : p(o.p), bytes(o.bytes) { o.p = nullptr; o.bytes = 0; }
-  Dev& operator=(Dev&& o) noexcept {
-    if (this != &o) { if (p) cudaFree(p); p = o.p; bytes = o.bytes; o.p = nullptr; o.bytes = 0; }
-    return *this;
-  }
-  ~Dev() { if (p) cudaFree(p); }
-  // grow-only scratch: contents are not kept
-  int ensure(size_t need) {
-    if (need <= bytes) return 0;
-    const size_t nb = std::max(need, bytes + bytes / 2);
-    void* np = nullptr;
-    FS_CU(cudaMalloc(&np, nb));
-    if (p) cudaFree(p);
-    p = np;
-    bytes = nb;
-    return 0;
-  }
-  template <typename T> T* as() const { return reinterpret_cast<T*>(p); }
-};
-
-// pinned host staging buffer (grow-only, contents not kept)
-struct Pinned {
-  void* p = nullptr;
-  size_t bytes = 0;
-  Pinned() = default;
-  Pinned(const Pinned&) = delete;
-  Pinned& operator=(const Pinned&) = delete;
-  ~Pinned() { if (p) cudaFreeHost(p); }
-  int ensure(size_t need) {
-    if (need <= bytes) return 0;
-    const size_t nb = std::max(need, bytes + bytes / 2);
-    void* np = nullptr;
-    FS_CU(cudaHostAlloc(&np, nb, cudaHostAllocDefault));
-    if (p) cudaFreeHost(p);
-    p = np;
-    bytes = nb;
-    return 0;
-  }
-};
+using sb::DBuf;
+using sb::fail;
 
 size_t align16(size_t v) { return (v + 15) & ~size_t(15); }
 
@@ -114,12 +57,12 @@ struct sb200_fstore {
   float stage_ms[3] = {0, 0, 0};
   // store columns
   size_t cap = 0;
-  Dev feat, cnt, start, ids, run;
+  DBuf feat, cnt, start, ids, run;
   std::vector<uint64_t> hid;                 // ids in store order
   std::unordered_map<uint64_t, int> hpos;    // id -> store position
   // per-call buffers
-  Dev dreq, dres, plan, qnorm, snorm, dist, gpos, gout;
-  Pinned hreq, hres;
+  DBuf dreq, dres, plan, qnorm, snorm, dist, gpos, gout;
+  sb::PinnedBuf<cudaHostAllocDefault> hreq, hres;   // staging, contents not kept
 
   ~sb200_fstore() {
     if (st) cudaStreamSynchronize(st);
@@ -141,14 +84,14 @@ struct sb200_fstore {
   }
 
   // fresh columns for `n` tracks; the caller copies what it keeps
-  int alloc_columns(size_t n, Dev* f, Dev* c, Dev* s, Dev* i, Dev* r) {
+  int alloc_columns(size_t n, DBuf* f, DBuf* c, DBuf* s, DBuf* i, DBuf* r) {
     n = std::max<size_t>(n, 1);
     if (int rc = f->ensure(n * o.max_observations * d8 * 4)) return rc;
     if (int rc = c->ensure(n * 4)) return rc;
     if (int rc = s->ensure(n * 4)) return rc;
     if (int rc = i->ensure(n * 8)) return rc;
     if (int rc = r->ensure(n * 4)) return rc;
-    FS_CU(cudaMemsetAsync(r->p, 0, n * 4, st));
+    CU(cudaMemsetAsync(r->p, 0, n * 4, st));
     return 0;
   }
 
@@ -156,23 +99,23 @@ struct sb200_fstore {
   int reserve(size_t need) {
     if (need <= cap) return 0;
     const size_t nc = std::max(need, cap + cap / 2);
-    Dev f, c, s, i, r;
+    DBuf f, c, s, i, r;
     if (int rc = alloc_columns(nc, &f, &c, &s, &i, &r)) return rc;
     const size_t live = hid.size();
     if (live) {
-      FS_CU(cudaMemcpyAsync(f.p, feat.p, live * o.max_observations * d8 * 4, cudaMemcpyDeviceToDevice, st));
-      FS_CU(cudaMemcpyAsync(c.p, cnt.p, live * 4, cudaMemcpyDeviceToDevice, st));
-      FS_CU(cudaMemcpyAsync(s.p, start.p, live * 4, cudaMemcpyDeviceToDevice, st));
-      FS_CU(cudaMemcpyAsync(i.p, ids.p, live * 8, cudaMemcpyDeviceToDevice, st));
+      CU(cudaMemcpyAsync(f.p, feat.p, live * o.max_observations * d8 * 4, cudaMemcpyDeviceToDevice, st));
+      CU(cudaMemcpyAsync(c.p, cnt.p, live * 4, cudaMemcpyDeviceToDevice, st));
+      CU(cudaMemcpyAsync(s.p, start.p, live * 4, cudaMemcpyDeviceToDevice, st));
+      CU(cudaMemcpyAsync(i.p, ids.p, live * 8, cudaMemcpyDeviceToDevice, st));
     }
-    FS_CU(cudaStreamSynchronize(st));   // the old columns are freed below
+    CU(cudaStreamSynchronize(st));   // the old columns are freed below
     feat = std::move(f); cnt = std::move(c); start = std::move(s); ids = std::move(i); run = std::move(r);
     cap = nc;
     return 0;
   }
 
   int begin() {
-    FS_CU(cudaSetDevice(o.device));
+    CU(cudaSetDevice(o.device));
     stage_ms[0] = stage_ms[1] = stage_ms[2] = 0.0f;
     return 0;
   }
@@ -223,37 +166,36 @@ struct sb200_fstore {
   // checks of a search / associate request; fills the newest-K row ranges
   int check_queries(int Q, const uint64_t* qids, const int32_t* offs, const float* feats, bool assoc,
                     std::vector<int>* qoff, std::vector<const float*>* src) {
-    if (Q < 0) return fs_fail(SB200_ERR_INVALID, "n_queries < 0");
+    if (Q < 0) return fail(SB200_ERR_INVALID, "n_queries < 0");
     if (Q == 0) return 0;
-    if (!qids || !offs) return fs_fail(SB200_ERR_INVALID, "query_ids / obs_offsets is NULL");
-    if (offs[0] != 0) return fs_fail(SB200_ERR_INVALID, "obs_offsets[0] != 0");
+    if (!qids || !offs) return fail(SB200_ERR_INVALID, "query_ids / obs_offsets is NULL");
+    if (offs[0] != 0) return fail(SB200_ERR_INVALID, "obs_offsets[0] != 0");
     std::unordered_set<uint64_t> seen;
     seen.reserve((size_t)Q * 2);
     qoff->assign(1, 0);
     const int K = o.max_observations;
     for (int q = 0; q < Q; ++q) {
       const int n = offs[q + 1] - offs[q];
-      if (n <= 0) return fs_fail(SB200_ERR_INVALID, "query " + std::to_string(q) + " has no observations");
+      if (n <= 0) return fail(SB200_ERR_INVALID, "query %d has no observations", q);
       if (!seen.insert(qids[q]).second)
-        return fs_fail(SB200_ERR_INVALID, "query id " + std::to_string(qids[q]) + " appears twice in the call");
+        return fail(SB200_ERR_INVALID, "query id %llu appears twice in the call", (unsigned long long)qids[q]);
       if (assoc && hpos.count(qids[q]))
-        return fs_fail(SB200_ERR_INVALID, "query id " + std::to_string(qids[q]) + " is already stored");
+        return fail(SB200_ERR_INVALID, "query id %llu is already stored", (unsigned long long)qids[q]);
       for (int k = std::max(0, n - K); k < n; ++k) src->push_back(feats + (size_t)(offs[q] + k) * o.feature_dim);
       qoff->push_back((int)src->size());
     }
-    if (!feats) return fs_fail(SB200_ERR_INVALID, "features is NULL");
+    if (!feats) return fail(SB200_ERR_INVALID, "features is NULL");
     const long long pairs = (long long)src->size() * (long long)hid.size() * K;
     if (pairs > sb::kFsMaxPairs)
-      return fs_fail(SB200_ERR_CAPACITY, "the call needs " + std::to_string(pairs) +
-                                             " observation pairs; one call holds at most 2^30");
+      return fail(SB200_ERR_CAPACITY, "the call needs %lld observation pairs; one call holds at most 2^30", pairs);
     return 0;
   }
 
   int finish_timing(bool dist_ran, bool topn_ran, bool apply_ran) {
     float ms = 0.0f;
-    if (dist_ran) { FS_CU(cudaEventElapsedTime(&ms, ev[0], ev[1])); stage_ms[0] = ms; }
-    if (topn_ran) { FS_CU(cudaEventElapsedTime(&ms, ev[1], ev[2])); stage_ms[1] = ms; }
-    if (apply_ran) { FS_CU(cudaEventElapsedTime(&ms, ev[2], ev[3])); stage_ms[2] = ms; }
+    if (dist_ran) { CU(cudaEventElapsedTime(&ms, ev[0], ev[1])); stage_ms[0] = ms; }
+    if (topn_ran) { CU(cudaEventElapsedTime(&ms, ev[1], ev[2])); stage_ms[1] = ms; }
+    if (apply_ran) { CU(cudaEventElapsedTime(&ms, ev[2], ev[3])); stage_ms[2] = ms; }
     return 0;
   }
 
@@ -264,7 +206,7 @@ struct sb200_fstore {
     std::vector<const float*> src;
     if (int rc = check_queries(Q, qids, offs, feats, assoc, &qoff, &src)) return rc;
     if (Q > 0 && (!counts || !winners || !weights || (assoc && (!track_ids || !merged))))
-      return fs_fail(SB200_ERR_INVALID, "an output is NULL");
+      return fail(SB200_ERR_INVALID, "an output is NULL");
     if (int rc = begin()) return rc;
     if (Q == 0) return 0;
     const int R = (int)src.size(), topn = o.topn, K = o.max_observations;
@@ -286,17 +228,17 @@ struct sb200_fstore {
     stage(L, Q, qids, qoff, src, std::vector<int>(Q, -1));
     const sb::FsStore s = view();
     const sb::FsCall c = call_view(L, Q, R, &RL);
-    FS_CU(cudaMemcpyAsync(dreq.p, hreq.p, L.total, cudaMemcpyHostToDevice, st));
-    FS_CU(cudaEventRecord(ev[0], st));
+    CU(cudaMemcpyAsync(dreq.p, hreq.p, L.total, cudaMemcpyHostToDevice, st));
+    CU(cudaEventRecord(ev[0], st));
     sb::fs_launch_dist(o.metric, o.distance_filter, s, c, st);
-    FS_CU(cudaEventRecord(ev[1], st));
+    CU(cudaEventRecord(ev[1], st));
     sb::fs_launch_topn(o.max_distance, o.min_votes, topn, assoc, s, c, st);
-    FS_CU(cudaEventRecord(ev[2], st));
+    CU(cudaEventRecord(ev[2], st));
     if (assoc) sb::fs_launch_apply(s, c, st);
-    FS_CU(cudaEventRecord(ev[3], st));
-    FS_CU(cudaMemcpyAsync(hres.p, dres.p, RL.total, cudaMemcpyDeviceToHost, st));
-    FS_CU(cudaStreamSynchronize(st));
-    FS_CU(cudaGetLastError());
+    CU(cudaEventRecord(ev[3], st));
+    CU(cudaMemcpyAsync(hres.p, dres.p, RL.total, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    CU(cudaGetLastError());
     if (int rc = finish_timing(S > 0, true, assoc)) return rc;
     const char* h = static_cast<const char*>(hres.p);
     const double* w = reinterpret_cast<const double*>(h + RL.w);
@@ -325,8 +267,8 @@ struct sb200_fstore {
   }
 
   int add(int n, const uint64_t* idv, const float* feats) {
-    if (n < 0) return fs_fail(SB200_ERR_INVALID, "n < 0");
-    if (n > 0 && (!idv || !feats)) return fs_fail(SB200_ERR_INVALID, "ids / features is NULL");
+    if (n < 0) return fail(SB200_ERR_INVALID, "n < 0");
+    if (n > 0 && (!idv || !feats)) return fail(SB200_ERR_INVALID, "ids / features is NULL");
     if (int rc = begin()) return rc;
     if (n == 0) return 0;
     // destination of every observation: a stored track, or a new one placed at the first appearance of its id
@@ -356,12 +298,12 @@ struct sb200_fstore {
     stage(L, n, idv, qoff, src, dest);
     const sb::FsStore s = view();
     const sb::FsCall c = call_view(L, n, n, nullptr);
-    FS_CU(cudaMemcpyAsync(dreq.p, hreq.p, L.total, cudaMemcpyHostToDevice, st));
-    FS_CU(cudaEventRecord(ev[2], st));
+    CU(cudaMemcpyAsync(dreq.p, hreq.p, L.total, cudaMemcpyHostToDevice, st));
+    CU(cudaEventRecord(ev[2], st));
     sb::fs_launch_apply(s, c, st);
-    FS_CU(cudaEventRecord(ev[3], st));
-    FS_CU(cudaStreamSynchronize(st));
-    FS_CU(cudaGetLastError());
+    CU(cudaEventRecord(ev[3], st));
+    CU(cudaStreamSynchronize(st));
+    CU(cudaGetLastError());
     if (int rc = finish_timing(false, false, true)) return rc;
     for (uint64_t id : fresh) {
       hpos[id] = (int)hid.size();
@@ -371,8 +313,8 @@ struct sb200_fstore {
   }
 
   int64_t fetch(int n, const uint64_t* idv, int remove, int32_t* counts, float* feats) {
-    if (n < 0) return fs_fail(SB200_ERR_INVALID, "n < 0");
-    if (n > 0 && (!idv || !counts || !feats)) return fs_fail(SB200_ERR_INVALID, "ids / counts / features is NULL");
+    if (n < 0) return fail(SB200_ERR_INVALID, "n < 0");
+    if (n > 0 && (!idv || !counts || !feats)) return fail(SB200_ERR_INVALID, "ids / counts / features is NULL");
     if (int rc = begin()) return rc;
     if (n == 0) return 0;
     const int K = o.max_observations, D = o.feature_dim;
@@ -390,14 +332,14 @@ struct sb200_fstore {
     if (int rc = gpos.ensure((size_t)n * 4)) return rc;
     if (int rc = gout.ensure(align16(out_bytes) + (size_t)n * 4)) return rc;
     if (int rc = hres.ensure(align16(out_bytes) + (size_t)n * 4)) return rc;
-    FS_CU(cudaMemcpyAsync(gpos.p, pos.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(gpos.p, pos.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
     const sb::FsStore s = view();
     float* dout = gout.as<float>();
     int* dcnt = reinterpret_cast<int*>(gout.as<char>() + align16(out_bytes));
     sb::fs_launch_gather(s, gpos.as<int>(), n, dout, dcnt, st);
-    FS_CU(cudaMemcpyAsync(hres.p, gout.p, align16(out_bytes) + (size_t)n * 4, cudaMemcpyDeviceToHost, st));
-    FS_CU(cudaStreamSynchronize(st));
-    FS_CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(hres.p, gout.p, align16(out_bytes) + (size_t)n * 4, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    CU(cudaGetLastError());
     const float* h = static_cast<const float*>(hres.p);
     const int* hc = reinterpret_cast<const int*>(static_cast<const char*>(hres.p) + align16(out_bytes));
     for (int i = 0; i < n; ++i) {
@@ -410,15 +352,15 @@ struct sb200_fstore {
       from.reserve(hid.size());
       for (size_t p = 0; p < hid.size(); ++p)
         if (!gone[p]) from.push_back((int)p);
-      Dev f, c, st_, i, r;
+      DBuf f, c, st_, i, r;
       if (int rc = alloc_columns(cap, &f, &c, &st_, &i, &r)) return rc;
       if (int rc = gpos.ensure(std::max<size_t>(from.size(), 1) * 4)) return rc;
-      FS_CU(cudaMemcpyAsync(gpos.p, from.data(), from.size() * 4, cudaMemcpyHostToDevice, st));
+      CU(cudaMemcpyAsync(gpos.p, from.data(), from.size() * 4, cudaMemcpyHostToDevice, st));
       sb::FsStore d = s;
       d.feat = f.as<float>(); d.cnt = c.as<int>(); d.start = st_.as<int>(); d.ids = i.as<unsigned long long>();
       sb::fs_launch_compact(s, d, gpos.as<int>(), (int)from.size(), st);
-      FS_CU(cudaStreamSynchronize(st));
-      FS_CU(cudaGetLastError());
+      CU(cudaStreamSynchronize(st));
+      CU(cudaGetLastError());
       feat = std::move(f); cnt = std::move(c); start = std::move(st_); ids = std::move(i); run = std::move(r);
       std::vector<uint64_t> kept;
       kept.reserve(from.size());
@@ -433,34 +375,26 @@ struct sb200_fstore {
 
 // a call without a handle: SB200_ERR_CUDA when there is no device to have made one, else SB200_ERR_INVALID
 int no_handle() {
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) {
-    cudaGetLastError();
-    return fs_fail(SB200_ERR_CUDA, "no CUDA device available (this library has no CPU execution path)");
-  }
-  return fs_fail(SB200_ERR_INVALID, "NULL handle");
+  if (int rc = sb::check_device(0)) return rc;
+  return fail(SB200_ERR_INVALID, "NULL handle");
 }
 
 extern "C" {
 
 int sb200_fstore_create(const sb200_fstore_options* opts, sb200_fstore** out) {
-  if (!opts || !out) return fs_fail(SB200_ERR_INVALID, "opts / out is NULL");
+  if (!opts || !out) return fail(SB200_ERR_INVALID, "opts / out is NULL");
   *out = nullptr;
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) {
-    cudaGetLastError();
-    return fs_fail(SB200_ERR_CUDA, "no CUDA device available (this library has no CPU execution path)");
-  }
+  if (int rc = sb::check_device(0)) return rc;   // no device at all; the index is checked after the options
   const sb200_fstore_options& o = *opts;
-  if (o.metric != SB200_VIS_EUCLIDEAN && o.metric != SB200_VIS_COSINE) return fs_fail(SB200_ERR_INVALID, "unknown metric");
+  if (o.metric != SB200_VIS_EUCLIDEAN && o.metric != SB200_VIS_COSINE) return fail(SB200_ERR_INVALID, "unknown metric");
   if (o.max_observations < 1 || o.max_observations > SB200_FSTORE_MAX_OBS)
-    return fs_fail(SB200_ERR_INVALID, "max_observations must lie in 1..64");
+    return fail(SB200_ERR_INVALID, "max_observations must lie in 1..64");
   if (o.feature_dim < 1 || o.feature_dim > SB200_FSTORE_MAX_DIM)
-    return fs_fail(SB200_ERR_INVALID, "feature_dim must lie in 1..8192");
-  if (o.topn < 1 || o.topn > SB200_FSTORE_MAX_TOPN) return fs_fail(SB200_ERR_INVALID, "topn must lie in 1..64");
-  if (o.min_votes < 0) return fs_fail(SB200_ERR_INVALID, "min_votes < 0");
-  if (o.device < 0 || o.device >= ndev) return fs_fail(SB200_ERR_INVALID, "device out of range");
-  FS_CU(cudaSetDevice(o.device));
+    return fail(SB200_ERR_INVALID, "feature_dim must lie in 1..8192");
+  if (o.topn < 1 || o.topn > SB200_FSTORE_MAX_TOPN) return fail(SB200_ERR_INVALID, "topn must lie in 1..64");
+  if (o.min_votes < 0) return fail(SB200_ERR_INVALID, "min_votes < 0");
+  if (int rc = sb::check_device(o.device)) return rc;
+  CU(cudaSetDevice(o.device));
   sb200_fstore* s = new sb200_fstore();
   s->o = o;
   s->d8 = (o.feature_dim + 7) / 8 * 8;
@@ -468,7 +402,7 @@ int sb200_fstore_create(const sb200_fstore_options* opts, sb200_fstore** out) {
   for (int i = 0; i < 4 && e == cudaSuccess; ++i) e = cudaEventCreate(&s->ev[i]);
   if (e != cudaSuccess) {
     delete s;
-    return fs_fail(SB200_ERR_CUDA, std::string("stream / event creation failed: ") + cudaGetErrorString(e));
+    return fail(SB200_ERR_CUDA, "stream / event creation failed: %s", cudaGetErrorString(e));
   }
   *out = s;
   return 0;
@@ -511,7 +445,7 @@ int64_t sb200_fstore_size(sb200_fstore* s) {
 
 int64_t sb200_fstore_ids(sb200_fstore* s, int64_t cap, uint64_t* ids) {
   if (!s) return no_handle();
-  if (cap < 0 || (cap > 0 && !ids)) return fs_fail(SB200_ERR_INVALID, "bad cap / ids");
+  if (cap < 0 || (cap > 0 && !ids)) return fail(SB200_ERR_INVALID, "bad cap / ids");
   const int64_t n = (int64_t)s->hid.size();
   std::copy(s->hid.begin(), s->hid.begin() + std::min(n, cap), ids);
   return n;
@@ -519,7 +453,7 @@ int64_t sb200_fstore_ids(sb200_fstore* s, int64_t cap, uint64_t* ids) {
 
 int sb200_fstore_last_stage_ms(sb200_fstore* s, float* out3) {
   if (!s) return no_handle();
-  if (!out3) return fs_fail(SB200_ERR_INVALID, "out3 is NULL");
+  if (!out3) return fail(SB200_ERR_INVALID, "out3 is NULL");
   std::copy(s->stage_ms, s->stage_ms + 3, out3);
   return 0;
 }

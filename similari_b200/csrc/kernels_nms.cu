@@ -24,13 +24,11 @@
 #include <functional>
 #include <memory>
 #include <mutex>
-#include <string>
 #include <vector>
 
 #include "../../include/similari_b200.h"
 #include "sb_engine.cuh"
-
-extern "C" void sb200__set_error(const char* msg);
+#include "sb_host.cuh"
 
 namespace sb {
 namespace {
@@ -361,31 +359,20 @@ int nms_enqueue(int n_sets, const int* offsets, const float* boxes, const float*
   return (int)e;
 }
 
-int nms_fail(int code, const std::string& m) {
-  sb200__set_error(m.c_str());
-  return code;
-}
-
 // Checks shared by both batch entries, in the order of sb200_nms; nothing is read but `offsets`.
 int nms_check(int n_sets, const int* offsets, const float* boxes, const int* keep_idx, const int* keep_counts, int device) {
-  if (n_sets < 0 || !offsets) return nms_fail(SB200_ERR_INVALID, "nms_batch: n_sets < 0 or offsets is NULL");
-  if (offsets[0] != 0) return nms_fail(SB200_ERR_INVALID, "nms_batch: offsets[0] != 0");
+  if (n_sets < 0 || !offsets) return fail(SB200_ERR_INVALID, "nms_batch: n_sets < 0 or offsets is NULL");
+  if (offsets[0] != 0) return fail(SB200_ERR_INVALID, "nms_batch: offsets[0] != 0");
   for (int s = 0; s < n_sets; ++s)
     if (offsets[s + 1] < offsets[s])
-      return nms_fail(SB200_ERR_INVALID, "nms_batch: offsets decrease at set " + std::to_string(s));
+      return fail(SB200_ERR_INVALID, "nms_batch: offsets decrease at set %d", s);
   if ((n_sets > 0 && !keep_counts) || (offsets[n_sets] > 0 && (!boxes || !keep_idx)))
-    return nms_fail(SB200_ERR_INVALID, "nms_batch: bad arguments");
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) {
-    cudaGetLastError();
-    return nms_fail(SB200_ERR_CUDA, "no CUDA device available (this library has no CPU execution path)");
-  }
-  if (device < 0 || device >= ndev) return nms_fail(SB200_ERR_INVALID, "device out of range");
+    return fail(SB200_ERR_INVALID, "nms_batch: bad arguments");
+  if (int rc = check_device(device)) return rc;
   for (int s = 0; s < n_sets; ++s) {
     const int n = offsets[s + 1] - offsets[s];
     if ((size_t)((n + 63) / 64) * 8 > kSweepBitmapBytes)
-      return nms_fail(SB200_ERR_CAPACITY, "nms: set " + std::to_string(s) + " has " + std::to_string(n) +
-                                              " boxes, too many for the on-chip sweep");
+      return fail(SB200_ERR_CAPACITY, "nms: set %d has %d boxes, too many for the on-chip sweep", s, n);
   }
   return 0;
 }
@@ -399,7 +386,7 @@ extern "C" int sb200_nms_batch_device(int32_t n_sets, const int32_t* offsets, co
                                       void* cuda_stream) {
   int rc = sb::nms_check(n_sets, offsets, boxes, keep_idx, keep_counts, device);
   if (rc) return rc;
-  if (cudaSetDevice(device) != cudaSuccess) return sb::nms_fail(SB200_ERR_CUDA, "cudaSetDevice failed");
+  CU(cudaSetDevice(device));
   cudaStream_t st = (cudaStream_t)cuda_stream;
   cudaError_t e = cudaSuccess;
   if (offsets[n_sets] == 0) {
@@ -409,7 +396,7 @@ extern "C" int sb200_nms_batch_device(int32_t n_sets, const int32_t* offsets, co
     e = (cudaError_t)sb::nms_enqueue(n_sets, offsets, boxes, scores, nms_threshold, sthr, keep_idx, keep_counts,
                                      keep_mask, device, st);
   }
-  if (e != cudaSuccess) return sb::nms_fail(SB200_ERR_CUDA, std::string("nms: CUDA error: ") + cudaGetErrorString(e));
+  if (e != cudaSuccess) return sb::fail(SB200_ERR_CUDA, "nms: CUDA error: %s", cudaGetErrorString(e));
   return 0;
 }
 
@@ -423,10 +410,9 @@ extern "C" int64_t sb200_nms_batch(int32_t n_sets, const int32_t* offsets, const
     if (n_sets > 0) memset(keep_counts, 0, 4 * (size_t)n_sets);
     return 0;
   }
-  if (cudaSetDevice(device) != cudaSuccess) return sb::nms_fail(SB200_ERR_CUDA, "cudaSetDevice failed");
+  CU(cudaSetDevice(device));
   cudaStream_t st;
-  if (cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking) != cudaSuccess)
-    return sb::nms_fail(SB200_ERR_CUDA, "cudaStreamCreate failed");
+  CU(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
   // device copies: boxes, scores, keep_idx, keep_counts, keep_mask
   const size_t o_sc = sb::align256(24 * total), o_idx = o_sc + sb::align256(4 * total);
   const size_t o_cnt = o_idx + sb::align256(4 * total), o_km = o_cnt + sb::align256(4 * (size_t)n_sets);
@@ -451,7 +437,7 @@ extern "C" int64_t sb200_nms_batch(int32_t n_sets, const int32_t* offsets, const
   cudaError_t es = cudaStreamSynchronize(st);
   if (e == cudaSuccess) e = es;
   cudaStreamDestroy(st);
-  if (e != cudaSuccess) return sb::nms_fail(SB200_ERR_CUDA, std::string("nms: CUDA error: ") + cudaGetErrorString(e));
+  if (e != cudaSuccess) return sb::fail(SB200_ERR_CUDA, "nms: CUDA error: %s", cudaGetErrorString(e));
   int64_t kept = 0;
   for (int s = 0; s < n_sets; ++s) kept += keep_counts[s];
   return kept;
@@ -459,7 +445,7 @@ extern "C" int64_t sb200_nms_batch(int32_t n_sets, const int32_t* offsets, const
 
 extern "C" int64_t sb200_nms(const float* boxes, const float* scores, int32_t n, float nms_threshold, float score_threshold,
                              int32_t has_score_threshold, int32_t* out_idx, int32_t device) {
-  if (n < 0 || (n > 0 && (!boxes || !out_idx))) return sb::nms_fail(SB200_ERR_INVALID, "bad arguments");
+  if (n < 0 || (n > 0 && (!boxes || !out_idx))) return sb::fail(SB200_ERR_INVALID, "bad arguments");
   const int32_t offsets[2] = {0, n};
   std::vector<int32_t> idx(std::max(n, 1));
   int32_t count = 0;

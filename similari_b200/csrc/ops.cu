@@ -11,53 +11,56 @@
 
 #include "../../include/similari_b200.h"
 #include "sb_engine.cuh"
-
-extern "C" void sb200__set_error(const char* msg);  // engine.cu
+#include "sb_host.cuh"
 
 namespace {
 
+using sb::DBuf;
+using sb::fail;
+
+// The device memory and stream of one operator call.  The first allocation, upload or memset that fails sets the last
+// error and `rc`, and the ones after it are skipped: an operator checks `rc` once, before its first launch.
 struct Scratch {
-  std::vector<void*> ptrs;
+  std::vector<DBuf> bufs;
   cudaStream_t st = nullptr;
+  int rc = 0;
   ~Scratch() {
-    for (void* p : ptrs) cudaFree(p);
+    bufs.clear();
     if (st) cudaStreamDestroy(st);
+  }
+  void check(cudaError_t e, const char* what) {
+    if (e == cudaSuccess || rc) return;
+    cudaGetLastError();
+    rc = fail(SB200_ERR_CUDA, "%s failed: %s", what, cudaGetErrorString(e));
   }
   template <typename T>
   T* alloc(size_t n, bool zero = false) {
-    void* p = nullptr;
-    if (cudaMalloc(&p, std::max<size_t>(1, n) * sizeof(T)) != cudaSuccess) return nullptr;
-    ptrs.push_back(p);
-    if (zero) cudaMemsetAsync(p, 0, std::max<size_t>(1, n) * sizeof(T), st);
-    return reinterpret_cast<T*>(p);
+    if (rc) return nullptr;
+    const size_t bytes = std::max<size_t>(1, n) * sizeof(T);
+    DBuf b;
+    if ((rc = b.ensure(bytes))) return nullptr;
+    if (zero) check(cudaMemsetAsync(b.p, 0, bytes, st), "cudaMemsetAsync");
+    bufs.push_back(std::move(b));
+    return bufs.back().as<T>();
   }
   template <typename T>
   T* upload(const T* h, size_t n) {
     T* d = alloc<T>(n);
-    if (d && n) cudaMemcpyAsync(d, h, n * sizeof(T), cudaMemcpyHostToDevice, st);
+    if (d && n) check(cudaMemcpyAsync(d, h, n * sizeof(T), cudaMemcpyHostToDevice, st), "cudaMemcpyAsync");
     return d;
   }
 };
 
-int ops_fail(int code, const std::string& msg) {
-  sb200__set_error(msg.c_str());
-  return code;
-}
 int begin(Scratch& sc, int device) {
-  int n = 0;
-  if (cudaGetDeviceCount(&n) != cudaSuccess || n <= 0) {
-    cudaGetLastError();
-    return ops_fail(SB200_ERR_CUDA, "no CUDA device available (this library has no CPU execution path)");
-  }
-  if (device < 0 || device >= n) return ops_fail(SB200_ERR_INVALID, "device out of range");
-  if (cudaSetDevice(device) != cudaSuccess) return ops_fail(SB200_ERR_CUDA, "cudaSetDevice failed");
-  if (cudaStreamCreateWithFlags(&sc.st, cudaStreamNonBlocking) != cudaSuccess) return ops_fail(SB200_ERR_CUDA, "cudaStreamCreate failed");
+  if (int rc = sb::check_device(device)) return rc;
+  CU(cudaSetDevice(device));
+  CU(cudaStreamCreateWithFlags(&sc.st, cudaStreamNonBlocking));
   return 0;
 }
 int finish(Scratch& sc) {
   cudaError_t e = cudaStreamSynchronize(sc.st);
   if (e == cudaSuccess) e = cudaGetLastError();
-  if (e != cudaSuccess) return ops_fail(SB200_ERR_CUDA, std::string("CUDA error: ") + cudaGetErrorString(e));
+  if (e != cudaSuccess) return fail(SB200_ERR_CUDA, "CUDA error: %s", cudaGetErrorString(e));
   return 0;
 }
 
@@ -131,9 +134,9 @@ int sb200_sort_cost_matrix(int32_t positional_kind, float iou_threshold, float m
                            float vel_weight, const float* cand_boxes, int32_t m, const float* track_boxes,
                            const float* track_states30, int32_t n, float* out_mn, int32_t device) {
   if (m < 0 || n < 0 || (m > 0 && !cand_boxes) || (n > 0 && !track_boxes) || (m > 0 && n > 0 && !out_mn))
-    return ops_fail(SB200_ERR_INVALID, "bad arguments");
+    return fail(SB200_ERR_INVALID, "bad arguments");
   if (positional_kind == SB200_POS_MAHA && n > 0 && !track_states30)
-    return ops_fail(SB200_ERR_INVALID, "track_states30 is required for the Mahalanobis metric");
+    return fail(SB200_ERR_INVALID, "track_states30 is required for the Mahalanobis metric");
   Scratch sc;
   int rc = begin(sc, device);
   if (rc) return rc;
@@ -164,15 +167,15 @@ int sb200_sort_cost_matrix(int32_t positional_kind, float iou_threshold, float m
   f.pos = sc.alloc<float>((size_t)m * n);
   f.pos_total = (long long)m * n;
   f.pos_dense_all = true;               // the operator returns the dense matrix
-  f.pos_cnt = sc.alloc<int>(4, true);   // sparse list disabled here (capacity 0): only the dense matrix is returned
-  f.pos_list = sc.alloc<sb::PosEntry>(1);
+  int* counters = sc.alloc<int>(sb::counter_ints(1), true);
+  f.pos_list = sc.alloc<sb::PosEntry>(1);   // sparse list disabled here (capacity 0): only the dense matrix is returned
   sb::SceneDesc d;
   memset(&d, 0, sizeof(d));
   d.m = m; d.n = n; d.epoch = 1;
   f.scenes = sc.upload(&d, 1);
-  if (!ts.pred || !ts.radius || !ts.epoch || !ts.vert || !ts.kst || !f.in_boxes || !f.c_box || !f.c_radius ||
-      !f.c_conf || !f.c_vert || !f.pos || !f.scenes)
-    return ops_fail(SB200_ERR_CUDA, "cudaMalloc failed");
+  if (sc.rc) return sc.rc;
+  sb::carve_counters(counters, 1, f);
+  f.screen_cnt = nullptr;   // the operators count nothing
   track_geom_kernel<<<(n + 127) / 128, 128, 0, sc.st>>>(positional_kind == SB200_POS_IOU, ts.pred, n, ts.radius, ts.vert, ts.epoch);
   sb::launch_prep(p, f, 1, m, sc.st);
   sb::launch_pos_cost(p, ts, f, 1, m, n, sc.st);
@@ -183,7 +186,7 @@ int sb200_sort_cost_matrix(int32_t positional_kind, float iou_threshold, float m
 int sb200_visual_cost_matrix(int32_t visual_kind, float threshold, const float* cand_features, int32_t m,
                              const float* track_features, int32_t n, int32_t d, float* out_mn, int32_t device) {
   if (m < 0 || n < 0 || d <= 0 || (m > 0 && !cand_features) || (n > 0 && !track_features) || (m > 0 && n > 0 && !out_mn))
-    return ops_fail(SB200_ERR_INVALID, "bad arguments");
+    return fail(SB200_ERR_INVALID, "bad arguments");
   Scratch sc;
   int rc = begin(sc, device);
   if (rc) return rc;
@@ -231,22 +234,7 @@ int sb200_visual_cost_matrix(int32_t visual_kind, float threshold, const float* 
   f.c_flags = sc.alloc<unsigned char>(m);
   f.c_norm2 = sc.alloc<float>(m, true);
   f.vis = sc.alloc<float>((size_t)m * n);
-  sb::SceneDesc sd;
-  memset(&sd, 0, sizeof(sd));
-  sd.m = m; sd.n = n; sd.nb = n; sd.epoch = 1;   // stateless operator: one observation per track, block == track
-  f.scenes = sc.upload(&sd, 1);
-  if (!ft.in_feat || !ft.in_boxes || !ft.c_box || !ft.c_radius || !ft.c_conf || !ft.c_flags || !ft.c_norm2 || !ts.pred ||
-      !ts.radius || !ts.epoch || !ts.feat || !ts.obs_phys || !ts.obs_hasf || !ts.obs_n || !ts.feat_cnt || !f.in_feat ||
-      !f.in_boxes || !f.c_box || !f.c_radius || !f.c_conf || !f.c_flags || !f.c_norm2 || !f.vis || !f.scenes)
-    return ops_fail(SB200_ERR_CUDA, "cudaMalloc failed");
-  sb::launch_prep(p, ft, 1, n, sc.st);
   ts.fnorm2 = ft.c_norm2;
-  cudaMemcpy2DAsync(ts.feat, (size_t)p.d8 * 4, ft.in_feat, (size_t)d * 4, (size_t)d * 4, n, cudaMemcpyDeviceToDevice, sc.st);
-  fill_u8_kernel<<<(n + 255) / 256, 256, 0, sc.st>>>(ts.obs_hasf, 1, n);
-  fill_u8_kernel<<<(n + 255) / 256, 256, 0, sc.st>>>(ts.obs_n, 1, n);
-  fill_u8_kernel<<<(n + 255) / 256, 256, 0, sc.st>>>(ts.feat_cnt, 1, n);
-  sb::launch_prep(p, f, 1, m, sc.st);
-  fill_u8_kernel<<<(m + 255) / 256, 256, 0, sc.st>>>(f.c_flags, 3, m);
   // the tracker's path rule (sb_engine.cuh), except that the operator has no dense path, and no frames to learn the e4m3
   // screen's selectivity from: it screens on BF16 unless SB200_VIS_KERNEL=tc8 asks for e4m3 operands (d8 <= 512)
   sb::TcArgs tc;
@@ -256,24 +244,24 @@ int sb200_visual_cost_matrix(int32_t visual_kind, float threshold, const float* 
               (vk != sb::kVisSimt && sb::vis_selective(visual_kind == SB200_VIS_EUCLIDEAN, threshold) &&
                sb::vis_tc_worth(p.d8, (long long)m * n));
   tc.fp8 = vk == sb::kVisTc8 && p.d8 <= sb::kFp8MaxD8;
-  f.scene_max = sc.alloc<unsigned int>(1);
   cudaDeviceGetAttribute(&tc.num_sms, cudaDevAttrMultiProcessorCount, device);
-  {
-    int lcap = std::max(4096, m * 64);
-    if (const char* ev = getenv("SB200_VIS_PAIR_CAP")) lcap = std::max(1, atoi(ev));
-    sd.vis_lbase = 0; sd.vis_lcap = lcap; sd.pos_lbase = 0; sd.pos_lcap = 0;
-    cudaMemcpyAsync(f.scenes, &sd, sizeof(sd), cudaMemcpyHostToDevice, sc.st);
-    f.vis_pairs = sc.alloc<sb::VisPair>((size_t)lcap);
-    f.vis_val = sc.alloc<float>((size_t)lcap);
-    f.pos_cnt = sc.alloc<int>(8, true);
-    f.vis_cnt = f.pos_cnt + 1;
-    f.scene_mode = f.pos_cnt + 2;
-    f.vis_mode = f.pos_cnt + 3;
-    f.refine_next = f.pos_cnt + 4;
-    f.dense_cnt = f.pos_cnt + 5;
-    f.pos_list = sc.alloc<sb::PosEntry>(1);
-    if (!f.vis_pairs || !f.vis_val || !f.pos_cnt || !f.pos_list) return ops_fail(SB200_ERR_CUDA, "cudaMalloc failed");
-  }
+  int lcap = std::max(4096, m * 64);
+  if (const char* ev = getenv("SB200_VIS_PAIR_CAP")) lcap = std::max(1, atoi(ev));
+  sb::SceneDesc sd;
+  memset(&sd, 0, sizeof(sd));
+  sd.m = m; sd.n = n; sd.nb = n; sd.epoch = 1;   // stateless operator: one observation per track, block == track
+  sd.vis_lcap = lcap;
+  f.scenes = sc.upload(&sd, 1);
+  f.scene_max = sc.alloc<unsigned int>(1);
+  f.vis_pairs = sc.alloc<sb::VisPair>((size_t)lcap);
+  f.vis_val = sc.alloc<float>((size_t)lcap);
+  int* counters = sc.alloc<int>(sb::counter_ints(1), true);
+  f.pos_list = sc.alloc<sb::PosEntry>(1);
+  // the candidates' operand rows join the frame after its launch_prep: the operator converts them with launch_to_* below,
+  // and cand_norm_kernel would write them as well if it saw them
+  unsigned char* c_fp8 = nullptr;
+  float* c_scale = nullptr;
+  unsigned short* c_bf16 = nullptr;
   if (tc.use_tc) {
     std::vector<sb::TcTile> tiles;
     tc.cstep = sb::vis_screen_ucols(p.d8, tc.num_sms, 1, &m, &n, 1);
@@ -285,14 +273,13 @@ int sb200_visual_cost_matrix(int32_t visual_kind, float threshold, const float* 
     tc.b_rows = n;
     if (tc.fp8) {
       const int p8 = sb::fp8_pitch(p.d8);
-      f.c_fp8 = sc.alloc<unsigned char>((size_t)m * p8);
-      f.c_scale = sc.alloc<float>(m);
+      c_fp8 = sc.alloc<unsigned char>((size_t)m * p8);
+      c_scale = sc.alloc<float>(m);
       ts.feat_fp8 = sc.alloc<unsigned char>((size_t)n * p8);
       ts.fscale = sc.alloc<float>(n);
       tc.colsb = sc.alloc<float>(n + 256);
-      if (!f.c_fp8 || !f.c_scale || !ts.feat_fp8 || !ts.fscale || !tc.colsb) return ops_fail(SB200_ERR_CUDA, "cudaMalloc failed");
     } else {
-      f.c_bf16 = sc.alloc<unsigned short>((size_t)m * p.d8);
+      c_bf16 = sc.alloc<unsigned short>((size_t)m * p.d8);
       ts.feat_bf16 = sc.alloc<unsigned short>((size_t)n * p.d8);
     }
     tc.colmeta = sc.alloc<sb::VisColMeta>(n + 256);   // the screen kernel bulk-copies whole 256-column slabs
@@ -301,8 +288,21 @@ int sb200_visual_cost_matrix(int32_t visual_kind, float threshold, const float* 
     tc.colvalid = sc.alloc<unsigned int>((n + 256) / 32 + 4);
     tc.rowmeta = sc.alloc<sb::VisRowMeta>(m + 256);
     tc.total_cols = n;
-    if (!tc.d_tiles || (!tc.fp8 && (!f.c_bf16 || !ts.feat_bf16)) || !tc.colmeta || !tc.colgeo || !tc.rowmeta || !tc.colb || !tc.colvalid)
-      return ops_fail(SB200_ERR_CUDA, "cudaMalloc failed");
+  }
+  if (sc.rc) return sc.rc;
+  sb::carve_counters(counters, 1, f);
+  f.screen_cnt = nullptr;   // the operators count nothing
+  sb::launch_prep(p, ft, 1, n, sc.st);
+  cudaMemcpy2DAsync(ts.feat, (size_t)p.d8 * 4, ft.in_feat, (size_t)d * 4, (size_t)d * 4, n, cudaMemcpyDeviceToDevice, sc.st);
+  fill_u8_kernel<<<(n + 255) / 256, 256, 0, sc.st>>>(ts.obs_hasf, 1, n);
+  fill_u8_kernel<<<(n + 255) / 256, 256, 0, sc.st>>>(ts.obs_n, 1, n);
+  fill_u8_kernel<<<(n + 255) / 256, 256, 0, sc.st>>>(ts.feat_cnt, 1, n);
+  sb::launch_prep(p, f, 1, m, sc.st);
+  fill_u8_kernel<<<(m + 255) / 256, 256, 0, sc.st>>>(f.c_flags, 3, m);
+  f.c_fp8 = c_fp8;
+  f.c_scale = c_scale;
+  f.c_bf16 = c_bf16;
+  if (tc.use_tc) {
     // (the tracker fuses these into cand_norm_kernel and feat_store_kernel)
     if (tc.fp8) {
       sb::launch_to_fp8(static_cast<const float*>(ft.in_feat), d, d, p.d8, n, ts.feat_fp8, ts.fscale, sc.st);
@@ -312,18 +312,17 @@ int sb200_visual_cost_matrix(int32_t visual_kind, float threshold, const float* 
       sb::launch_to_bf16(static_cast<const float*>(f.in_feat), d, d, p.d8, m, f.c_bf16, sc.st);
     }
   }
-  ts.fnorm2 = ft.c_norm2;
   int vr = sb::launch_vis_cost(p, ts, f, 1, m, n, tc, sc.st);
   if (vr == 0 && tc.use_tc) sb::launch_vis_densify(p, f, 1, sc.st);
-  if (vr != 0) return ops_fail(SB200_ERR_CUDA, "visual cost launch failed");
+  if (vr != 0) return fail(SB200_ERR_CUDA, "visual cost launch failed");
   cudaMemcpyAsync(out_mn, f.vis, (size_t)m * n * 4, cudaMemcpyDeviceToHost, sc.st);
   return finish(sc);
 }
 
 static int run_voting(bool visual, float threshold, int min_votes, const float* pos_mn, const float* vis_mnk, int m, int n,
                       int k, int32_t* winner, uint8_t* voting_type, int device) {
-  if (m < 0 || n < 0 || (m > 0 && !winner) || (m > 0 && n > 0 && !pos_mn)) return ops_fail(SB200_ERR_INVALID, "bad arguments");
-  if (visual && (k < 1 || k > sb::kMaxObs || (m > 0 && n > 0 && !vis_mnk))) return ops_fail(SB200_ERR_INVALID, "bad arguments");
+  if (m < 0 || n < 0 || (m > 0 && !winner) || (m > 0 && n > 0 && !pos_mn)) return fail(SB200_ERR_INVALID, "bad arguments");
+  if (visual && (k < 1 || k > sb::kMaxObs || (m > 0 && n > 0 && !vis_mnk))) return fail(SB200_ERR_INVALID, "bad arguments");
   // Which voting kernel runs: by default the tracker's rule (the sparse kernel on the entry lists unless a list exceeds
   // its capacity); SB200_VOTE_KERNEL=dense|sparse|prepass forces one, so that a test can hand each kernel the matrix of
   // its choosing.  A forced kernel the rule would not allow is an error, never a silent switch to the other one.
@@ -332,9 +331,9 @@ static int run_voting(bool visual, float threshold, int min_votes, const float* 
     if (!strcmp(ev, "dense")) want = kDense;
     else if (!strcmp(ev, "sparse")) want = kSparse;
     else if (!strcmp(ev, "prepass")) want = kPrepass;
-    else if (*ev) return ops_fail(SB200_ERR_INVALID, "SB200_VOTE_KERNEL must be dense, sparse or prepass");
+    else if (*ev) return fail(SB200_ERR_INVALID, "SB200_VOTE_KERNEL must be dense, sparse or prepass");
   }
-  if (want == kPrepass && !visual) return ops_fail(SB200_ERR_INVALID, "SB200_VOTE_KERNEL=prepass applies to visual voting only");
+  if (want == kPrepass && !visual) return fail(SB200_ERR_INVALID, "SB200_VOTE_KERNEL=prepass applies to visual voting only");
   Scratch sc;
   int rc = begin(sc, device);
   if (rc) return rc;
@@ -357,16 +356,12 @@ static int run_voting(bool visual, float threshold, int min_votes, const float* 
   f.winner = sc.alloc<int>(m);
   f.c_vt = sc.alloc<unsigned char>(m);
   f.new_count = sc.alloc<int>(1);
-  {
-    // scene mode 1 until the rule below runs: the scene-maximum reduction skips sparse scenes (the tracker's refinement
-    // reduces their maximum), and the operator has no refinement
-    int hm[4] = {0, 0, 1, 1};
-    f.pos_cnt = sc.upload(hm, 4);
-    if (!f.pos_cnt) return ops_fail(SB200_ERR_CUDA, "cudaMalloc failed");
-    f.vis_cnt = f.pos_cnt + 1;
-    f.scene_mode = f.pos_cnt + 2;
-    f.vis_mode = f.pos_cnt + 3;
-  }
+  // the counters, zero but for scene mode 1 until the rule below runs: the scene-maximum reduction skips sparse scenes
+  // (the tracker's refinement reduces their maximum), and the operator has no refinement
+  std::vector<int> counters(sb::counter_ints(1), 0);
+  sb::carve_counters(counters.data(), 1, f);
+  *f.scene_mode = *f.vis_mode = 1;
+  int* d_counters = sc.upload(counters.data(), counters.size());
   // one scene, list slices sized as the tracker sizes them
   sb::SceneDesc sd;
   memset(&sd, 0, sizeof(sd));
@@ -378,15 +373,20 @@ static int run_voting(bool visual, float threshold, int min_votes, const float* 
   if (visual) {
     f.vis_pairs = sc.alloc<sb::VisPair>(sd.vis_lcap);
     f.vis_val = sc.alloc<float>(sd.vis_lcap);
+    f.scene_max = sc.alloc<unsigned int>(1);
   }
-  if (!f.pos || (visual && (!f.vis || !f.vis_pairs || !f.vis_val)) || !f.winner || !f.c_vt || !f.new_count || !f.scenes ||
-      !f.pos_list)
-    return ops_fail(SB200_ERR_CUDA, "cudaMalloc failed");
+  if (want == kPrepass) {
+    f.decided = sc.alloc<unsigned char>(m);
+    f.excl = sc.alloc<unsigned char>(n);
+    f.pre_winner = sc.alloc<int>(m);
+  }
+  if (sc.rc) return sc.rc;
+  sb::carve_counters(d_counters, 1, f);
+  f.screen_cnt = nullptr;   // the operators count nothing
+  f.dense_cnt = nullptr;    // ... and voting has no dense visual kernel that the count would let leave early
   vote_list_kernel<<<1, kListThreads, 0, sc.st>>>(f.pos, m, n, sd.pos_lcap, f.pos_list, nullptr, nullptr, f.pos_cnt);
   if (visual) vote_list_kernel<<<1, kListThreads, 0, sc.st>>>(f.vis, m, n * k, sd.vis_lcap, nullptr, f.vis_pairs, f.vis_val, f.vis_cnt);
   if (visual) {
-    f.scene_max = sc.alloc<unsigned int>(1);
-    if (!f.scene_max) return ops_fail(SB200_ERR_CUDA, "cudaMalloc failed");
     sb::launch_scene_max(p, f, 1, /*init_only=*/true, sc.st);
     if (n > 0) sb::launch_scene_max(p, f, 1, /*init_only=*/false, sc.st);
   }
@@ -400,21 +400,17 @@ static int run_voting(bool visual, float threshold, int min_votes, const float* 
     cudaMemcpyAsync(&mode, f.scene_mode, sizeof(int), cudaMemcpyDeviceToHost, sc.st);
     if ((rc = finish(sc))) return rc;
     if (mode != 0)
-      return ops_fail(SB200_ERR_CAPACITY, "SB200_VOTE_KERNEL: the entry lists exceed the sparse voting kernel's capacity");
+      return fail(SB200_ERR_CAPACITY, "SB200_VOTE_KERNEL: the entry lists exceed the sparse voting kernel's capacity");
   }
   if (want == kPrepass) {
     // the tracker's lazy positional stage: BestFit pre-pass, then the full pass reuses its decisions
-    f.decided = sc.alloc<unsigned char>(m);
-    f.excl = sc.alloc<unsigned char>(n);
-    f.pre_winner = sc.alloc<int>(m);
-    if (!f.decided || !f.excl || !f.pre_winner) return ops_fail(SB200_ERR_CUDA, "cudaMalloc failed");
     int vr = sb::launch_vote_masks(p, ts, f, 1, m, n, sc.st);
-    if (vr == -3) return ops_fail(SB200_ERR_CAPACITY, "scene too large for the on-chip assignment solver");
-    if (vr != 0) return ops_fail(SB200_ERR_CUDA, std::string("voting launch failed: ") + cudaGetErrorString((cudaError_t)vr));
+    if (vr == -3) return fail(SB200_ERR_CAPACITY, "scene too large for the on-chip assignment solver");
+    if (vr != 0) return fail(SB200_ERR_CUDA, "voting launch failed: %s", cudaGetErrorString((cudaError_t)vr));
   }
   int vr = sb::launch_voting(p, ts, f, 1, m, n, sc.st);
-  if (vr == -3) return ops_fail(SB200_ERR_CAPACITY, "scene too large for the on-chip assignment solver");
-  if (vr != 0) return ops_fail(SB200_ERR_CUDA, std::string("voting launch failed: ") + cudaGetErrorString((cudaError_t)vr));
+  if (vr == -3) return fail(SB200_ERR_CAPACITY, "scene too large for the on-chip assignment solver");
+  if (vr != 0) return fail(SB200_ERR_CUDA, "voting launch failed: %s", cudaGetErrorString((cudaError_t)vr));
   cudaMemcpyAsync(winner, f.winner, (size_t)m * 4, cudaMemcpyDeviceToHost, sc.st);
   if (voting_type) cudaMemcpyAsync(voting_type, f.c_vt, (size_t)m, cudaMemcpyDeviceToHost, sc.st);
   return finish(sc);
@@ -430,7 +426,7 @@ int sb200_visual_voting(float positional_threshold, int32_t min_votes, const flo
 }
 
 int sb200_own_area_shares(const float* boxes, int32_t n, float* out, int32_t device) {
-  if (n < 0 || (n > 0 && (!boxes || !out))) return ops_fail(SB200_ERR_INVALID, "bad arguments");
+  if (n < 0 || (n > 0 && (!boxes || !out))) return fail(SB200_ERR_INVALID, "bad arguments");
   Scratch sc;
   int rc = begin(sc, device);
   if (rc) return rc;
@@ -447,19 +443,19 @@ int sb200_own_area_shares(const float* boxes, int32_t n, float* out, int32_t dev
   float* d_out = sc.alloc<float>(n);
   int* d_ovf_cnt = sc.alloc<int>(1);
   int2* d_ovf = sc.alloc<int2>(n);
-  if (!f.scenes || !f.status || !d_boxes || !d_out || !d_ovf_cnt || !d_ovf) return ops_fail(SB200_ERR_CUDA, "cudaMalloc failed");
+  if (sc.rc) return sc.rc;
   sb::launch_own_area(f, 1, n, d_boxes, d_out, d_ovf_cnt, d_ovf, sc.st);
   int status = 0;
   cudaMemcpyAsync(out, d_out, (size_t)n * 4, cudaMemcpyDeviceToHost, sc.st);
   cudaMemcpyAsync(&status, f.status, sizeof(int), cudaMemcpyDeviceToHost, sc.st);
   rc = finish(sc);
   if (rc) return rc;
-  if (status & 2) return ops_fail(SB200_ERR_CAPACITY, "more than 2800 boxes overlap one box (own-area shares)");
+  if (status & 2) return fail(SB200_ERR_CAPACITY, "more than 2800 boxes overlap one box (own-area shares)");
   return 0;
 }
 
 static int kalman_op(int op, float pw, float vw, const float* in30, const float* boxes, int n, float* out30, int device) {
-  if (n < 0 || (n > 0 && !out30) || (op != 0 && n > 0 && !in30) || (op != 1 && n > 0 && !boxes)) return ops_fail(SB200_ERR_INVALID, "bad arguments");
+  if (n < 0 || (n > 0 && !out30) || (op != 0 && n > 0 && !in30) || (op != 1 && n > 0 && !boxes)) return fail(SB200_ERR_INVALID, "bad arguments");
   Scratch sc;
   int rc = begin(sc, device);
   if (rc) return rc;
@@ -467,7 +463,7 @@ static int kalman_op(int op, float pw, float vw, const float* in30, const float*
   float* din = in30 ? sc.upload(in30, (size_t)n * 30) : nullptr;
   float* db = boxes ? sc.upload(boxes, (size_t)n * 6) : nullptr;
   float* dout = sc.alloc<float>((size_t)n * 30);
-  if ((in30 && !din) || (boxes && !db) || !dout) return ops_fail(SB200_ERR_CUDA, "cudaMalloc failed");
+  if (sc.rc) return sc.rc;
   sb::launch_kalman_ops(op, pw, vw, din, db, n, dout, sc.st);
   cudaMemcpyAsync(out30, dout, (size_t)n * 120, cudaMemcpyDeviceToHost, sc.st);
   return finish(sc);
@@ -486,7 +482,7 @@ int sb200_kalman_update(float pw, float vw, const float* in30, const float* boxe
 int sb200_kalman_distance(float pw, float vw, const float* states30, const float* boxes, int32_t n, float* out,
                           int32_t device) {
   (void)vw;   // the distance reads only the position weight (project, :104-120)
-  if (n < 0 || (n > 0 && (!states30 || !boxes || !out))) return ops_fail(SB200_ERR_INVALID, "bad arguments");
+  if (n < 0 || (n > 0 && (!states30 || !boxes || !out))) return fail(SB200_ERR_INVALID, "bad arguments");
   Scratch sc;
   int rc = begin(sc, device);
   if (rc) return rc;
@@ -494,7 +490,7 @@ int sb200_kalman_distance(float pw, float vw, const float* states30, const float
   float* din = sc.upload(states30, (size_t)n * 30);
   float* db = sc.upload(boxes, (size_t)n * 6);
   float* dout = sc.alloc<float>(n);
-  if (!din || !db || !dout) return ops_fail(SB200_ERR_CUDA, "cudaMalloc failed");
+  if (sc.rc) return sc.rc;
   sb::launch_kalman_distance(pw, din, db, n, dout, sc.st);
   cudaMemcpyAsync(out, dout, (size_t)n * 4, cudaMemcpyDeviceToHost, sc.st);
   return finish(sc);
@@ -505,7 +501,7 @@ static int point_kalman_op(int op, float pw, float vw, const float* in12, const 
                            int device) {
   const bool need_in = op != 0, need_pts = op != 1;
   if (n < 0 || (n > 0 && (!out || (need_in && !in12) || (need_pts && !points))))
-    return ops_fail(SB200_ERR_INVALID, "bad arguments");
+    return fail(SB200_ERR_INVALID, "bad arguments");
   Scratch sc;
   int rc = begin(sc, device);
   if (rc) return rc;
@@ -514,7 +510,7 @@ static int point_kalman_op(int op, float pw, float vw, const float* in12, const 
   float* din = need_in ? sc.upload(in12, (size_t)n * 12) : nullptr;
   float* dp = need_pts ? sc.upload(points, (size_t)n * 2) : nullptr;
   float* dout = sc.alloc<float>(out_floats);
-  if ((need_in && !din) || (need_pts && !dp) || !dout) return ops_fail(SB200_ERR_CUDA, "cudaMalloc failed");
+  if (sc.rc) return sc.rc;
   sb::launch_point_kalman(op, pw, vw, din, dp, n, dout, sc.st);
   cudaMemcpyAsync(out, dout, out_floats * 4, cudaMemcpyDeviceToHost, sc.st);
   return finish(sc);
@@ -540,14 +536,14 @@ int sb200_point_kalman_distance(float pw, float vw, const float* states12, const
 
 // Universal2DBox::get_vertices, src/utils/bbox.rs:169-171,287-330
 int sb200_box_vertices(const float* boxes, int32_t n, double* out8, int32_t device) {
-  if (n < 0 || (n > 0 && (!boxes || !out8))) return ops_fail(SB200_ERR_INVALID, "bad arguments");
+  if (n < 0 || (n > 0 && (!boxes || !out8))) return fail(SB200_ERR_INVALID, "bad arguments");
   Scratch sc;
   int rc = begin(sc, device);
   if (rc) return rc;
   if (n == 0) return 0;
   float* db = sc.upload(boxes, (size_t)n * 6);
   double* dv = sc.alloc<double>((size_t)n * 8);
-  if (!db || !dv) return ops_fail(SB200_ERR_CUDA, "cudaMalloc failed");
+  if (sc.rc) return sc.rc;
   sb::launch_box_vertices(db, n, dv, sc.st);
   cudaMemcpyAsync(out8, dv, (size_t)n * 64, cudaMemcpyDeviceToHost, sc.st);
   return finish(sc);
@@ -557,7 +553,7 @@ int sb200_box_vertices(const float* boxes, int32_t n, double* out8, int32_t devi
 int sb200_clip_polygons(const float* subjects, const float* clippings, int32_t n, double* out_vertices,
                         int32_t* out_counts, double* out_areas, int32_t device) {
   if (n < 0 || (n > 0 && (!subjects || !clippings || !out_vertices || !out_counts || !out_areas)))
-    return ops_fail(SB200_ERR_INVALID, "bad arguments");
+    return fail(SB200_ERR_INVALID, "bad arguments");
   Scratch sc;
   int rc = begin(sc, device);
   if (rc) return rc;
@@ -569,26 +565,26 @@ int sb200_clip_polygons(const float* subjects, const float* clippings, int32_t n
   int* dn = sc.alloc<int>(n);
   double* da = sc.alloc<double>(n);
   int* dst = sc.alloc<int>(1, true);
-  if (!ds || !dc || !dv || !dn || !da || !dst) return ops_fail(SB200_ERR_CUDA, "cudaMalloc failed");
+  if (sc.rc) return sc.rc;
   sb::launch_clip_polygons(ds, dc, n, dv, dn, da, dst, sc.st);
   int status = 0;
   cudaMemcpyAsync(&status, dst, sizeof(int), cudaMemcpyDeviceToHost, sc.st);
   rc = finish(sc);
   if (rc) return rc;
-  if (status & 1) return ops_fail(SB200_ERR_CAPACITY, "a clipped polygon would have more than 16 vertices");
+  if (status & 1) return fail(SB200_ERR_CAPACITY, "a clipped polygon would have more than 16 vertices");
   // outputs are written only when every pair fits
   cudaMemcpy(out_vertices, dv, nv * sizeof(double), cudaMemcpyDeviceToHost);
   cudaMemcpy(out_counts, dn, (size_t)n * 4, cudaMemcpyDeviceToHost);
   cudaMemcpy(out_areas, da, (size_t)n * 8, cudaMemcpyDeviceToHost);
   cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return ops_fail(SB200_ERR_CUDA, std::string("CUDA error: ") + cudaGetErrorString(e));
+  if (e != cudaSuccess) return fail(SB200_ERR_CUDA, "CUDA error: %s", cudaGetErrorString(e));
   return 0;
 }
 
 // intersection_area_py (src/utils/clipping/clipping_py.rs:41-46) of every (a[i], b[j]) pair
 int sb200_intersection_areas(const float* a, int32_t m, const float* b, int32_t n, double* out_mn, int32_t device) {
   if (m < 0 || n < 0 || (m > 0 && !a) || (n > 0 && !b) || (m > 0 && n > 0 && !out_mn))
-    return ops_fail(SB200_ERR_INVALID, "bad arguments");
+    return fail(SB200_ERR_INVALID, "bad arguments");
   Scratch sc;
   int rc = begin(sc, device);
   if (rc) return rc;
@@ -599,7 +595,7 @@ int sb200_intersection_areas(const float* a, int32_t m, const float* b, int32_t 
   double* vb = sc.alloc<double>((size_t)n * 8);
   double* dout = sc.alloc<double>((size_t)m * n);
   int* dst = sc.alloc<int>(1, true);
-  if (!da || !db || !va || !vb || !dout || !dst) return ops_fail(SB200_ERR_CUDA, "cudaMalloc failed");
+  if (sc.rc) return sc.rc;
   sb::launch_box_vertices(da, m, va, sc.st);
   sb::launch_box_vertices(db, n, vb, sc.st);
   sb::launch_intersection_areas(va, m, vb, n, dout, dst, sc.st);
@@ -607,9 +603,9 @@ int sb200_intersection_areas(const float* a, int32_t m, const float* b, int32_t 
   cudaMemcpyAsync(&status, dst, sizeof(int), cudaMemcpyDeviceToHost, sc.st);
   rc = finish(sc);
   if (rc) return rc;
-  if (status & 1) return ops_fail(SB200_ERR_CAPACITY, "a clipped polygon would have more than 16 vertices");
+  if (status & 1) return fail(SB200_ERR_CAPACITY, "a clipped polygon would have more than 16 vertices");
   cudaError_t e = cudaMemcpy(out_mn, dout, (size_t)m * n * sizeof(double), cudaMemcpyDeviceToHost);
-  if (e != cudaSuccess) return ops_fail(SB200_ERR_CUDA, std::string("CUDA error: ") + cudaGetErrorString(e));
+  if (e != cudaSuccess) return fail(SB200_ERR_CUDA, "CUDA error: %s", cudaGetErrorString(e));
   return 0;
 }
 

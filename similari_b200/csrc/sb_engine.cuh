@@ -395,6 +395,16 @@ struct Frame {  // per-request transient device buffers (a request may be proces
   float* o_obs;
 };
 
+// The per-scene counters of a frame, zeroed together (the tracker: by frame_setup_kernel): pos_cnt | vis_cnt | scene_mode |
+// vis_mode | refine_next | status, [n] ints each, then dense_cnt and screen_cnt[3].
+inline size_t counter_ints(int n) { return 6 * (size_t)n + 4; }
+inline void carve_counters(int* c, int n, Frame& f) {
+  using F = Frame;
+  int* F::* const rows[] = {&F::pos_cnt, &F::vis_cnt, &F::scene_mode, &F::vis_mode, &F::refine_next, &F::status, &F::dense_cnt};
+  for (int i = 0; i < 7; ++i) f.*rows[i] = c + (size_t)i * n;
+  f.screen_cnt = f.dense_cnt + 1;
+}
+
 struct TcTile { int scene, m0, c0, pad; };  // pad: column-tile index inside the scene (dense kernel: its metadata slab)  // one 128 x 256 output tile of the tensor-core visual cost kernel
 // per-frame metadata of one physical feature row (track n, physical slot p) of a scene, built once per frame
 struct VisColMeta {

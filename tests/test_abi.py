@@ -3,6 +3,8 @@ declares, struct layouts match, and compute entry points fail loudly (no CPU fal
 import ctypes as C
 import os
 import re
+import shutil
+import subprocess
 
 import numpy as np
 import pytest
@@ -27,6 +29,20 @@ def test_exports_every_declared_symbol(L):
     assert declared == set(_lib.EXPORTS), declared ^ set(_lib.EXPORTS)
     for name in declared:
         assert getattr(L, name) is not None
+
+
+def test_exports_only_declared_symbols(L):
+    """The library's dynamic sb200_* symbols are exactly the header's declarations: nothing undeclared leaks out."""
+    nm = shutil.which("nm")
+    if nm is None:
+        pytest.skip("nm is not installed")
+    from similari_b200 import _build
+
+    out = subprocess.run([nm, "-D", "--defined-only", _build.LIB], check=True, capture_output=True, text=True).stdout
+    exported = {line.split()[-1] for line in out.splitlines() if line.split() and line.split()[-1].startswith("sb200_")}
+    hdr = open(os.path.join(ROOT, "include", "similari_b200.h")).read()
+    declared = set(re.findall(r"\b(sb200_[a-z0-9_]+)\s*\(", hdr))
+    assert exported == declared, exported ^ declared
 
 
 def test_options_struct_layout_matches_oracle_mirror(L, oracle):
