@@ -233,7 +233,9 @@ __global__ void __launch_bounds__(TN * TY) pos_cost_kernel(Params p, TrackStore 
 // sorts the scene's track centres by x in shared memory; each thread then walks one candidate's x-window, runs the
 // cheap gates on shared-memory copies (x, y, r, epoch) and only touches the heavy per-track record (Kalman state /
 // f64 vertices) for the handful of survivors.  The dense matrix is pre-filled with None by pos_fill_none_kernel.
-// The window is padded by 1e-5 relative so that float rounding in too_far can never keep a culled pair.
+// The window is padded by 1e-5 relative so that float rounding in too_far can never keep a culled pair.  A scene with
+// a non-finite track x or radius, and a candidate with a non-finite x or radius, skip the window: every pair of them
+// goes through the gates, which decide it as the reference does (NaN distances are never too far).
 constexpr int PS_THREADS = 512;
 constexpr int PS_MAXN = 4096;   // tracks per scene the culled kernel sorts in shared memory (else dense kernel)
 
@@ -401,9 +403,10 @@ __global__ void __launch_bounds__(PS_THREADS, 2) pos_scan_kernel(Params p, Track
     if (n < N) {
       const float x = ts.pred[(tbase + n) * 6];
       const float r = ts.radius[tbase + n];
-      if (!(x == x) || !(r == r)) s_bad = 1;
-      // a track the visual pass claimed sorts behind every window but in front of the padding (so that [0, N) holds
-      // exactly the N tracks)
+      // a non-finite x or radius makes the window bounds meaningless (inf - inf): every candidate scans [0, N) in full
+      if (!isfinite(x) || !isfinite(r)) s_bad = 1;
+      // a track the visual pass claimed sorts behind every window; the sort key puts the padding behind every track,
+      // whatever its x (pos_sort_key), so that [0, N) holds exactly the N tracks
       kx[n] = (excl && excl[n]) ? 3.0e38f : x; kidx[n] = n;
       rmax = fmaxf(rmax, r);
     } else { kx[n] = 3.402823466e+38f; kidx[n] = -1; }
@@ -421,8 +424,7 @@ __global__ void __launch_bounds__(PS_THREADS, 2) pos_scan_kernel(Params p, Track
         const int ixj = i ^ j;
         if (ixj > i) {
           const float a = kx[i], b = kx[ixj];
-          const bool up = (i & k2) == 0;
-          if ((a > b) == up) {
+          if (pos_sort_swap(a, kidx[i], b, kidx[ixj], (i & k2) == 0)) {
             kx[i] = b; kx[ixj] = a;
             const int t = kidx[i]; kidx[i] = kidx[ixj]; kidx[ixj] = t;
           }
@@ -456,7 +458,7 @@ __global__ void __launch_bounds__(PS_THREADS, 2) pos_scan_kernel(Params p, Track
       const float cx = cb[0], cy = cb[1];
       const float cr = f.c_radius[g];
       int lo = 0, hi = N;
-      if (!bad && cx == cx && cr == cr) {
+      if (!bad && isfinite(cx) && isfinite(cr)) {   // else the full scan: the gates below decide every pair
         const float R = (cr + rmax) * (1.0f + 1e-5f) + 1e-30f;
         const float xlo = cx - R, xhi = cx + R;
         int a = 0, b = N;
@@ -467,7 +469,7 @@ __global__ void __launch_bounds__(PS_THREADS, 2) pos_scan_kernel(Params p, Track
         hi = a;
       }
       for (int i = lo; i < hi; ++i) {
-        if (excl && excl[kidx[i]]) continue;   // (only reachable on the unsorted NaN path; sorted windows never hold them)
+        if (excl && excl[kidx[i]]) continue;   // (only reachable on the full scan; sorted windows never hold them)
         const float tx = kx[i], ty = sy[i], tr = sr[i];
         if (!compat_ok(p, sc.epoch, sep[i], cx, cy, cr, tx, ty, tr) || too_far(cx, cy, cr, tx, ty, tr)) continue;
         const int slot = atomicAdd(&s_qn, 1);

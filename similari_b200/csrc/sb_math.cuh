@@ -11,6 +11,7 @@
 #pragma once
 #include <math.h>
 #include <stdint.h>
+#include <string.h>
 
 #ifndef __CUDACC__
 #ifndef __host__
@@ -66,6 +67,22 @@ SB_HD bool too_far(float xl, float yl, float rl, float xr, float yr, float rr) {
   float x = xl - xr;
   float y = yl - yr;
   return x * x + y * y > max_distance * max_distance;
+}
+// Sort key of the culled positional scan (pos_scan_kernel): a total order on (x, track index) with the padding
+// (idx < 0) after every track.  x in IEEE order (-0 before +0), every NaN after +inf, ties by index.  The float
+// compare `a > b` is not an order once a key is NaN (the network then moves padding into [0, N) and tracks out of it).
+SB_HD uint64_t pos_sort_key(float x, int idx) {
+  if (idx < 0) return ~0ull;
+  uint32_t u;
+  memcpy(&u, &x, 4);
+  u = (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+  if (is_nan(x)) u = 0xffffffffu;
+  return ((uint64_t)u << 32) | (uint32_t)idx;
+}
+// One compare-exchange of the bitonic network on (x, idx) entries: true when entries i and i ^ j swap, `up` the
+// direction of the i-th block of the current merge size.
+SB_HD bool pos_sort_swap(float xi, int ii, float xj, int ij, bool up) {
+  return (pos_sort_key(xi, ii) > pos_sort_key(xj, ij)) == up;
 }
 // Universal2DBox::dist_in_2r, src/utils/bbox.rs:464-474
 SB_HD float dist_in_2r(float xl, float yl, float rl, float xr, float yr, float rr) {
@@ -303,6 +320,9 @@ SB_HD float maha_distance(const float* mean5, const float* l5, float xc, float y
   const float y2 = (angle0 - mean5[2]) / l5[2];
   const float y3 = (aspect - mean5[3]) / l5[3];
   const float y4 = (height - mean5[4]) / l5[4];
+  // The reference's forward substitution adds (-y_i) * L_ri (L_ri == 0) to every later row, so an infinite y0..y3 (a
+  // finite box whose whitened residual overflows f32) makes its distance NaN -- None -- not +inf (cost 0).
+  if (isinf(y0) || isinf(y1) || isinf(y2) || isinf(y3)) return nanf("");
   float s = y0 * y0;
   s = s + y1 * y1;
   s = s + y2 * y2;

@@ -36,6 +36,26 @@ double shim_overlap_bound(const double* a8, const double* b8) { return sb::rect_
 int shim_iou_bound_fails(const float* l, const float* r, float conf, float thr) {
   return sb::iou_bound_fails(l[4], l[3], r[4], r[3], conf, thr) ? 1 : 0;
 }
+// pos_scan_kernel's sort of the track centres, run serially: the same padding to Np (a power of two) and the same
+// (k2, j) network.  Within one (k2, j) step the exchanges touch disjoint pairs, so the serial order gives the kernel's
+// result exactly.  kx, kidx: Np entries out.
+void shim_pos_sort(const float* x, int n, float* kx, int* kidx) {
+  int np = 1;
+  while (np < n) np <<= 1;
+  for (int i = 0; i < np; ++i) {
+    kx[i] = i < n ? x[i] : 3.402823466e+38f;
+    kidx[i] = i < n ? i : -1;
+  }
+  for (int k2 = 2; k2 <= np; k2 <<= 1)
+    for (int j = k2 >> 1; j > 0; j >>= 1)
+      for (int i = 0; i < np; ++i) {
+        const int ixj = i ^ j;
+        if (ixj > i && sb::pos_sort_swap(kx[i], kidx[i], kx[ixj], kidx[ixj], (i & k2) == 0)) {
+          const float a = kx[i]; kx[i] = kx[ixj]; kx[ixj] = a;
+          const int t = kidx[i]; kidx[i] = kidx[ixj]; kidx[ixj] = t;
+        }
+      }
+}
 }
 // sincos_cr (sb_sincos.cuh) and the C library's sin / cos over an array of f32 angles
 extern "C" void shim_sincos(const float* angles, long long n, double* s, double* c) {
