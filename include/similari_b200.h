@@ -475,6 +475,83 @@ int64_t sb200_fstore_ids(sb200_fstore* s, int64_t cap, uint64_t* ids);
 /* Device times (ms) of the last search / associate / add call: distances, TopN, apply (0 for a stage that did not run). */
 int sb200_fstore_last_stage_ms(sb200_fstore* s, float* out3);
 
+/* Element type (SB200_FEATURE_F32 | _F16 | _BF16) of the `features` argument of every later sb200_fstore_add / _search /
+ * _associate call and of their _device forms.  The column stays [rows][feature_dim] row-major; with F16 or BF16 the
+ * `const float* features` parameter carries a pointer to 2-byte elements.  Widening either type to f32 is exact, so
+ * every output and every stored row is bit for bit what the same call returns for the widened f32 request.  The stored
+ * rows stay f32 and sb200_fstore_fetch keeps returning f32.  A new store reads F32; a loaded store reads the type its
+ * blob was saved under.  SB200_ERR_INVALID for an unknown type.  No counterpart in the reference (its features are f32). */
+int sb200_fstore_set_feature_type(sb200_fstore* s, int32_t type);
+/* The options the store was created (or loaded) with, `device` included, and the element type now set.  Either output may
+ * be NULL.  What a caller that loads a blob needs to size the outputs of the other calls.  No counterpart in the
+ * reference. */
+int sb200_fstore_get_options(sb200_fstore* s, sb200_fstore_options* out, int32_t* feature_type);
+
+/* sb200_fstore_add / _search / _associate with `d_features` a DEVICE pointer on the store's device, in the element type
+ * set by sb200_fstore_set_feature_type: the column an embedding network has just written.  ids, query_ids, obs_offsets
+ * and every output stay HOST pointers, and every rejection is still decided on the host before anything is launched or
+ * changed; a `d_features` that is not device memory on the store's device is SB200_ERR_INVALID.  The request rows are
+ * read from the caller's column by a kernel: the features cross PCIe in neither direction.
+ * Stream order: the call's work waits, by an event, for what `cuda_stream` (a cudaStream_t; NULL: the legacy default
+ * stream) holds when the call is made, so a column that stream is still writing is complete before it is read.  The
+ * call returns after its results are on the host, so nothing enqueued after it can race the column.  There are no
+ * asynchronous forms: associate needs its results on the host to extend the id -> position map before the next call.
+ * Results are those of the host-pointer call on the same values.  They stand for the same reference functions as the
+ * host-pointer forms (TrackStore::add, foreign_track_distances + TopNVoting::winners, the loop of
+ * benches/feature_tracker.rs); device residency has no counterpart in the reference. */
+int sb200_fstore_add_device(sb200_fstore* s, int32_t n, const uint64_t* ids, const void* d_features, void* cuda_stream);
+int sb200_fstore_search_device(sb200_fstore* s, int32_t n_queries, const uint64_t* query_ids,
+                               const int32_t* obs_offsets, const void* d_features, int32_t* counts, uint64_t* winners,
+                               double* weights, void* cuda_stream);
+int sb200_fstore_associate_device(sb200_fstore* s, int32_t n_queries, const uint64_t* query_ids,
+                                  const int32_t* obs_offsets, const void* d_features, int32_t* counts,
+                                  uint64_t* winners, double* weights, uint64_t* track_ids, uint8_t* merged,
+                                  void* cuda_stream);
+
+/* ---- the store blob ----
+ * The whole store as one relocatable block of bytes: this header, then four sections at 256-byte aligned offsets, gaps
+ * zeroed, in this order: ids[live] (u64), cnt[live] (i32 observations held), start[live] (i32 ring slot of the oldest
+ * observation), feat[live][max_observations][d8] (f32 rows as stored; observation j of a track sits in ring slot
+ * (start + j) % max_observations).  Ring slots a track has never filled are written as zeros, so two stores that hold
+ * the same tracks in the same ring state give byte-equal blobs.  The magic differs from the tracker blob's: each loader
+ * refuses the other's blob. */
+#define SB200_FSTORE_BLOB_MAGIC 0x53464253u /* "SBFS" */
+#define SB200_FSTORE_BLOB_VERSION 1u
+#define SB200_FSTORE_BLOB_ALIGN 256u
+#define SB200_FSTORE_BLOB_SECTIONS 4
+typedef struct {
+  uint32_t magic;
+  uint32_t version;
+  uint64_t total_bytes;
+  int32_t metric; /* the fields of sb200_fstore_options, `device` excepted */
+  float distance_filter;
+  int32_t max_observations;
+  int32_t feature_dim;
+  int32_t topn;
+  float max_distance;
+  int32_t min_votes;
+  int32_t d8;           /* feature_dim rounded up to a multiple of 8: the stored row length */
+  int32_t feature_type; /* the element type set when the blob was written */
+  int32_t reserved;     /* 0 */
+  int64_t live;         /* stored tracks */
+  uint64_t sec_off[SB200_FSTORE_BLOB_SECTIONS];
+  uint64_t sec_bytes[SB200_FSTORE_BLOB_SECTIONS];
+} sb200_fstore_blob_header;
+/* Writes the blob to `buf` (`cap` bytes; host memory, or device memory on any device) and its size to *bytes.
+ * buf == NULL: reports the size and writes nothing.  SB200_ERR_CAPACITY when cap is too small: nothing is written and
+ * *bytes is still set.  Rows are copied, not re-derived; the store is not changed.  Timers and the stream are not part
+ * of the state.  No counterpart in the reference (its store is not serialisable). */
+int sb200_fstore_save(sb200_fstore* s, void* buf, uint64_t cap, uint64_t* bytes);
+/* A new store on `device` from a blob (host or device memory).  Exact continuation: fed the same calls, the loaded
+ * store returns what the saved one returns (counts, winner ids, f64 weights, track_ids, merged, fetched rows, id order,
+ * size).  A damaged blob is refused with SB200_ERR_INVALID before a store exists, sb200_last_error naming the field:
+ * magic, version, truncation, section bounds / order / 256-byte alignment / sizes, options outside the caps of
+ * sb200_fstore_create, d8 != round_up(feature_dim, 8), an id twice, and (by one kernel over the blob, before any row is
+ * copied) a cnt outside [1, max_observations] or a start outside [0, max_observations).  A flipped feature value is not
+ * detected: the blob carries no checksum.  A failed load leaves no handle and no device memory behind.  No counterpart
+ * in the reference. */
+int sb200_fstore_load(const void* buf, uint64_t bytes, int32_t device, sb200_fstore** out);
+
 /* Pinned host memory for callers that want the predict H2D/D2H copies to run at full PCIe speed. */
 void* sb200_host_alloc(size_t bytes);
 void sb200_host_free(void* p);

@@ -87,6 +87,32 @@ class FstoreOptions(C.Structure):
     ]
 
 
+FSTORE_BLOB_MAGIC, FSTORE_BLOB_VERSION, FSTORE_BLOB_ALIGN, FSTORE_BLOB_SECTIONS = 0x53464253, 1, 256, 4
+
+
+class FstoreBlobHeader(C.Structure):
+    """sb200_fstore_blob_header: the first bytes of a blob of sb200_fstore_save."""
+
+    _fields_ = [
+        ("magic", C.c_uint32),
+        ("version", C.c_uint32),
+        ("total_bytes", C.c_uint64),
+        ("metric", C.c_int32),
+        ("distance_filter", C.c_float),
+        ("max_observations", C.c_int32),
+        ("feature_dim", C.c_int32),
+        ("topn", C.c_int32),
+        ("max_distance", C.c_float),
+        ("min_votes", C.c_int32),
+        ("d8", C.c_int32),
+        ("feature_type", C.c_int32),
+        ("reserved", C.c_int32),
+        ("live", C.c_int64),
+        ("sec_off", C.c_uint64 * FSTORE_BLOB_SECTIONS),
+        ("sec_bytes", C.c_uint64 * FSTORE_BLOB_SECTIONS),
+    ]
+
+
 _lib = None
 
 # every symbol include/similari_b200.h declares (checked by tests/test_abi.py without a GPU)
@@ -106,7 +132,9 @@ EXPORTS = [
     "sb200_feature_history_pool", "sb200_tracker_save", "sb200_tracker_load", "sb200_scenes_export",
     "sb200_scenes_import", "sb200_tracker_options", "sb200_set_feature_type", "sb200_fstore_create",
     "sb200_fstore_destroy", "sb200_fstore_add", "sb200_fstore_search", "sb200_fstore_associate", "sb200_fstore_fetch",
-    "sb200_fstore_size", "sb200_fstore_ids", "sb200_fstore_last_stage_ms",
+    "sb200_fstore_size", "sb200_fstore_ids", "sb200_fstore_last_stage_ms", "sb200_fstore_set_feature_type",
+    "sb200_fstore_get_options", "sb200_fstore_add_device", "sb200_fstore_search_device",
+    "sb200_fstore_associate_device", "sb200_fstore_save", "sb200_fstore_load",
 ]
 
 
@@ -197,6 +225,13 @@ def lib():
         "sb200_fstore_size": (i64, [vp]),
         "sb200_fstore_ids": (i64, [vp, i64, vp]),
         "sb200_fstore_last_stage_ms": (C.c_int, [vp, vp]),
+        "sb200_fstore_set_feature_type": (C.c_int, [vp, i32]),
+        "sb200_fstore_get_options": (C.c_int, [vp, C.POINTER(FstoreOptions), C.POINTER(i32)]),
+        "sb200_fstore_add_device": (C.c_int, [vp, i32, vp, vp, vp]),
+        "sb200_fstore_search_device": (C.c_int, [vp, i32, vp, vp, vp, vp, vp, vp, vp]),
+        "sb200_fstore_associate_device": (C.c_int, [vp, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
+        "sb200_fstore_save": (C.c_int, [vp, vp, u64, C.POINTER(u64)]),
+        "sb200_fstore_load": (C.c_int, [vp, u64, i32, C.POINTER(vp)]),
         "sb200_host_alloc": (vp, [C.c_size_t]),
         "sb200_host_free": (None, [vp]),
     }

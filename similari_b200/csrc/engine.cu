@@ -19,6 +19,7 @@
 #include <vector>
 
 #include "../../include/similari_b200.h"
+#include "sb_blob.cuh"
 #include "sb_engine.cuh"
 #include "sb_host.cuh"
 
@@ -406,7 +407,10 @@ struct sb200_tracker {
   // plus one, where allocating all first would hold two whole stores at once.
   int grow(const std::vector<Col>& cols, size_t groups, size_t rows, size_t old_groups, size_t old_rows) {
     for (const Col& c : cols) {
-      const int rc = regrow(*c.buf, c.w, groups, rows, old_groups, old_rows, c.zero);
+      // Rows and row tails that no kernel has written yet travel in the state blob (the squared norms of a block's unused
+      // rows, the history rings of a short wasted record): every column a blob carries starts zeroed, so that trackers in
+      // the same state give the same blob whatever the allocation held before.
+      const int rc = regrow(*c.buf, c.w, groups, rows, old_groups, old_rows, c.zero || c.blob != kBlobNo);
       if (rc) return rc;
       if (c.point) c.point(*this, c.buf->p);
     }
@@ -2039,60 +2043,8 @@ uint64_t lay_out(BlobHeader& h, const std::vector<uint64_t>& sec) {
   return off;
 }
 
-// where a blob lives: -1 host memory, else the ordinal of the device that holds it
-int blob_device(const void* p) {
-  cudaPointerAttributes a;
-  if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return -1; }
-  return (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) ? a.device : -1;
-}
-
-// host <-> device copy of a blob through two pinned staging buffers (the copy of one chunk overlaps the host copy of the
-// other); memory that is pinned already is copied in one piece
-int host_copy(cudaStream_t st, void* host, void* dev, size_t n, bool to_host) {
-  cudaPointerAttributes a;
-  const bool pinned = cudaPointerGetAttributes(&a, host) == cudaSuccess && a.type == cudaMemoryTypeHost;
-  cudaGetLastError();
-  if (pinned || n <= (1u << 20)) {
-    CU(to_host ? cudaMemcpyAsync(host, dev, n, cudaMemcpyDeviceToHost, st) : cudaMemcpyAsync(dev, host, n, cudaMemcpyHostToDevice, st));
-    CU(cudaStreamSynchronize(st));
-    return 0;
-  }
-  constexpr size_t kStage = 32u << 20;
-  struct Stage {
-    void* p[2] = {nullptr, nullptr};
-    cudaEvent_t ev[2] = {nullptr, nullptr};
-    ~Stage() { for (int i = 0; i < 2; ++i) { if (p[i]) cudaFreeHost(p[i]); if (ev[i]) cudaEventDestroy(ev[i]); } }
-  } sg;
-  for (int i = 0; i < 2; ++i) {
-    CU(cudaHostAlloc(&sg.p[i], kStage, cudaHostAllocDefault));
-    CU(cudaEventCreateWithFlags(&sg.ev[i], cudaEventDisableTiming));
-  }
-  char* h = static_cast<char*>(host);
-  char* d = static_cast<char*>(dev);
-  const size_t nch = (n + kStage - 1) / kStage;
-  auto len = [&](size_t i) { return std::min(kStage, n - i * kStage); };
-  if (to_host) {
-    CU(cudaMemcpyAsync(sg.p[0], d, len(0), cudaMemcpyDeviceToHost, st));
-    CU(cudaEventRecord(sg.ev[0], st));
-    for (size_t i = 0; i < nch; ++i) {
-      if (i + 1 < nch) {
-        CU(cudaMemcpyAsync(sg.p[(i + 1) & 1], d + (i + 1) * kStage, len(i + 1), cudaMemcpyDeviceToHost, st));
-        CU(cudaEventRecord(sg.ev[(i + 1) & 1], st));
-      }
-      CU(cudaEventSynchronize(sg.ev[i & 1]));
-      memcpy(h + i * kStage, sg.p[i & 1], len(i));
-    }
-  } else {
-    for (size_t i = 0; i < nch; ++i) {
-      if (i >= 2) CU(cudaEventSynchronize(sg.ev[i & 1]));   // the copy out of this buffer two chunks ago has finished
-      memcpy(sg.p[i & 1], h + i * kStage, len(i));
-      CU(cudaMemcpyAsync(d + i * kStage, sg.p[i & 1], len(i), cudaMemcpyHostToDevice, st));
-      CU(cudaEventRecord(sg.ev[i & 1], st));
-    }
-  }
-  CU(cudaStreamSynchronize(st));
-  return 0;
-}
+using sb::blob_device;
+using sb::host_copy;
 
 struct SlotRows { int slot, n, blk, fre; };
 
@@ -2129,21 +2081,7 @@ int move_store(sb200_tracker* t, int dir, uint32_t type, const BlobHeader& h, ch
     }
   }
   const cudaStream_t st = t->stream;
-  if (!segs.empty()) {
-    std::vector<long long> cpre(segs.size() + 1, 0);
-    for (size_t i = 0; i < segs.size(); ++i)
-      cpre[i + 1] = cpre[i] + (long long)((segs[i].bytes + sb::kXferChunk - 1) / sb::kXferChunk);
-    DBuf d_tab;
-    const size_t sb_ = segs.size() * sizeof(sb::XferSeg);
-    int rc = d_tab.ensure(sb_ + cpre.size() * sizeof(long long));
-    if (rc) return rc;
-    CU(cudaMemcpyAsync(d_tab.p, segs.data(), sb_, cudaMemcpyHostToDevice, st));
-    CU(cudaMemcpyAsync(d_tab.as<char>() + sb_, cpre.data(), cpre.size() * sizeof(long long), cudaMemcpyHostToDevice, st));
-    const int e = sb::launch_xfer_copy(d_tab.as<sb::XferSeg>(), reinterpret_cast<const long long*>(d_tab.as<char>() + sb_),
-                                       (int)segs.size(), cpre.back(), t->num_sms, st);
-    if (e) return fail(SB200_ERR_CUDA, "state copy launch failed: %s", cudaGetErrorString((cudaError_t)e));
-    CU(cudaStreamSynchronize(st));
-  }
+  if (int rc = sb::copy_segments(segs, t->num_sms, st)) return rc;
   if (type == kBlobScenes && t->fhist_on && h.live_total > 0) {
     std::vector<int> tab(2 * rows.size() + 1, 0);   // slots | prefix of the live tracks
     for (size_t i = 0; i < rows.size(); ++i) { tab[i] = rows[i].slot; tab[rows.size() + i + 1] = tab[rows.size() + i] + rows[i].n; }

@@ -2,9 +2,13 @@
 // sequence of a call (distances -> TopN -> apply, kernels_fstore.cu) and the host copy of the store's id order.
 // A call stages its request in one pinned buffer, uploads it once, runs its kernels back to back on the handle's stream
 // and downloads its results once.  Everything a call can reject is checked before anything is launched or changed.
+// The request rows reach the device in one of two ways: an f32 host column is staged row by row in the pinned buffer; a
+// 2-byte host column (uploaded raw) and a device column (read in place) go through fs_stage_kernel.  The store blob
+// (sb200_fstore_save / _load) shares the trackers' copy machinery (sb_blob.cuh).
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <climits>
 #include <cmath>
 #include <cstring>
 #include <unordered_map>
@@ -12,6 +16,7 @@
 #include <vector>
 
 #include "../../include/similari_b200.h"
+#include "sb_blob.cuh"
 #include "sb_fstore.cuh"
 #include "sb_host.cuh"
 
@@ -24,8 +29,9 @@ size_t align16(size_t v) { return (v + 15) & ~size_t(15); }
 
 // byte offsets of one request in the staging buffer (the device copy has the same layout)
 struct ReqLayout {
-  size_t rows, qid, qoff, row_q, dest, maxkey, total;
-  ReqLayout(int Q, int R, int d8) {
+  size_t rows, qid, qoff, row_q, dest, maxkey, row_src, total;
+  // with_src: the request carries the row-index table of fs_stage_kernel instead of host-staged rows
+  ReqLayout(int Q, int R, int d8, bool with_src) {
     size_t o = 0;
     rows = o; o = align16(o + (size_t)R * d8 * 4);
     qid = o; o = align16(o + (size_t)Q * 8);
@@ -33,6 +39,8 @@ struct ReqLayout {
     row_q = o; o = align16(o + (size_t)R * 4);
     dest = o; o = align16(o + (size_t)Q * 4);
     maxkey = o; o = align16(o + 4);
+    row_src = o;
+    if (with_src) o = align16(o + (size_t)R * 4);
     total = o;
   }
 };
@@ -47,13 +55,39 @@ struct ResLayout {
   }
 };
 
+// the feature column of a call: a host pointer, or a device pointer with the caller's stream
+struct Column {
+  const void* p;
+  bool on_device;
+  cudaStream_t caller;
+};
+
+using BlobHeader = sb200_fstore_blob_header;
+constexpr uint64_t kSecAlign = SB200_FSTORE_BLOB_ALIGN;
+enum { kSecIds, kSecCnt, kSecStart, kSecFeat };
+uint64_t sec_align(uint64_t v) { return (v + kSecAlign - 1) / kSecAlign * kSecAlign; }
+
+int check_options(const sb200_fstore_options& o) {
+  if (o.metric != SB200_VIS_EUCLIDEAN && o.metric != SB200_VIS_COSINE) return fail(SB200_ERR_INVALID, "unknown metric");
+  if (o.max_observations < 1 || o.max_observations > SB200_FSTORE_MAX_OBS)
+    return fail(SB200_ERR_INVALID, "max_observations must lie in 1..64");
+  if (o.feature_dim < 1 || o.feature_dim > SB200_FSTORE_MAX_DIM)
+    return fail(SB200_ERR_INVALID, "feature_dim must lie in 1..8192");
+  if (o.topn < 1 || o.topn > SB200_FSTORE_MAX_TOPN) return fail(SB200_ERR_INVALID, "topn must lie in 1..64");
+  if (o.min_votes < 0) return fail(SB200_ERR_INVALID, "min_votes < 0");
+  return 0;
+}
+
 }  // namespace
 
 struct sb200_fstore {
   sb200_fstore_options o{};
   int d8 = 8;
+  int ftype = SB200_FEATURE_F32;   // element type of the calls' feature columns
+  int num_sms = 1;
   cudaStream_t st = nullptr;
   cudaEvent_t ev[4] = {};
+  cudaEvent_t ev_in = nullptr;     // what the caller's stream held when a device-column call was made
   float stage_ms[3] = {0, 0, 0};
   // store columns
   size_t cap = 0;
@@ -61,12 +95,13 @@ struct sb200_fstore {
   std::vector<uint64_t> hid;                 // ids in store order
   std::unordered_map<uint64_t, int> hpos;    // id -> store position
   // per-call buffers
-  DBuf dreq, dres, plan, qnorm, snorm, dist, gpos, gout;
-  sb::PinnedBuf<cudaHostAllocDefault> hreq, hres;   // staging, contents not kept
+  DBuf dreq, dres, plan, qnorm, snorm, dist, gpos, gout, dcol;
+  sb::PinnedBuf<cudaHostAllocDefault> hreq, hres, hcol;   // staging, contents not kept
 
   ~sb200_fstore() {
     if (st) cudaStreamSynchronize(st);
     for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e);
+    if (ev_in) cudaEventDestroy(ev_in);
     if (st) cudaStreamDestroy(st);
   }
 
@@ -120,23 +155,61 @@ struct sb200_fstore {
     return 0;
   }
 
-  // stages rows [R][d8] (zero-padded) + ids + offsets + row -> item + dest + the initial max_dist into hreq
-  void stage(const ReqLayout& L, int Q, const uint64_t* qids, const std::vector<int>& qoff,
-             const std::vector<const float*>& src, const std::vector<int>& dest) {
-    char* h = static_cast<char*>(hreq.p);
-    const int D = o.feature_dim, R = (int)src.size();
-    float* rows = reinterpret_cast<float*>(h + L.rows);
-    for (int r = 0; r < R; ++r) {
-      memcpy(rows + (size_t)r * d8, src[r], (size_t)D * 4);
-      for (int k = D; k < d8; ++k) rows[(size_t)r * d8 + k] = 0.0f;
+  size_t elem() const { return ftype == SB200_FEATURE_F32 ? 4 : 2; }
+
+  // a device column must be device memory on the store's device
+  int check_column(const Column& col) const {
+    if (!col.on_device || !col.p) return 0;
+    if (sb::blob_device(col.p) != o.device)
+      return fail(SB200_ERR_INVALID, "d_features is not device memory on device %d", o.device);
+    return 0;
+  }
+
+  // Puts the request on the device: rows [R][d8] (zero-padded), ids, offsets, row -> item, dest and the initial max_dist.
+  // row_src[r] is the row of the caller's column behind request row r; col_rows the rows of a host column to upload.
+  int upload(const ReqLayout& L, int Q, const uint64_t* qids, const std::vector<int>& qoff, const std::vector<int>& row_src,
+             const std::vector<int>& dest, const Column& col, size_t col_rows) {
+    const bool host_f32 = !col.on_device && ftype == SB200_FEATURE_F32;
+    const size_t base = host_f32 ? 0 : L.qid;   // the rows of the other paths are written on the device
+    const int D = o.feature_dim, R = (int)row_src.size();
+    if (int rc = hreq.ensure(L.total - base)) return rc;
+    if (int rc = dreq.ensure(L.total)) return rc;
+    auto at = [&](size_t off) { return static_cast<char*>(hreq.p) + (off - base); };   // off: an offset of L >= base
+    if (host_f32) {
+      const float* feats = static_cast<const float*>(col.p);
+      float* rows = reinterpret_cast<float*>(at(L.rows));
+      for (int r = 0; r < R; ++r) {
+        memcpy(rows + (size_t)r * d8, feats + (size_t)row_src[r] * D, (size_t)D * 4);
+        for (int k = D; k < d8; ++k) rows[(size_t)r * d8 + k] = 0.0f;
+      }
+    } else {
+      memcpy(at(L.row_src), row_src.data(), (size_t)R * 4);
     }
-    memcpy(h + L.qid, qids, (size_t)Q * 8);
-    memcpy(h + L.qoff, qoff.data(), (size_t)(Q + 1) * 4);
-    int* row_q = reinterpret_cast<int*>(h + L.row_q);
+    memcpy(at(L.qid), qids, (size_t)Q * 8);
+    memcpy(at(L.qoff), qoff.data(), (size_t)(Q + 1) * 4);
+    int* row_q = reinterpret_cast<int*>(at(L.row_q));
     for (int q = 0; q < Q; ++q)
       for (int r = qoff[q]; r < qoff[q + 1]; ++r) row_q[r] = q;
-    memcpy(h + L.dest, dest.data(), (size_t)Q * 4);
-    *reinterpret_cast<int*>(h + L.maxkey) = sb::fs_key(-1.0f);   // max_dist starts at -1.0 (topn.rs:78)
+    memcpy(at(L.dest), dest.data(), (size_t)Q * 4);
+    *reinterpret_cast<int*>(at(L.maxkey)) = sb::fs_key(-1.0f);   // max_dist starts at -1.0 (topn.rs:78)
+    const void* dev_col = col.p;
+    if (!host_f32 && !col.on_device) {   // the raw 2-byte rows: half the bytes of the widened request
+      const size_t bytes = col_rows * D * elem();
+      if (int rc = hcol.ensure(bytes)) return rc;
+      if (int rc = dcol.ensure(bytes)) return rc;
+      memcpy(hcol.p, col.p, bytes);
+      CU(cudaMemcpyAsync(dcol.p, hcol.p, bytes, cudaMemcpyHostToDevice, st));
+      dev_col = dcol.p;
+    }
+    if (col.on_device) {   // the column is complete once the caller's stream has reached this point
+      CU(cudaEventRecord(ev_in, col.caller));
+      CU(cudaStreamWaitEvent(st, ev_in, 0));
+    }
+    CU(cudaMemcpyAsync(dreq.as<char>() + base, hreq.p, L.total - base, cudaMemcpyHostToDevice, st));
+    if (!host_f32)
+      sb::fs_launch_stage(ftype, dev_col, reinterpret_cast<const int*>(dreq.as<char>() + L.row_src), R, D, d8,
+                          reinterpret_cast<float*>(dreq.as<char>() + L.rows), st);
+    return 0;
   }
 
   sb::FsCall call_view(const ReqLayout& L, int Q, int R, const ResLayout* RL) {
@@ -163,16 +236,15 @@ struct sb200_fstore {
     return c;
   }
 
-  // checks of a search / associate request; fills the newest-K row ranges
-  int check_queries(int Q, const uint64_t* qids, const int32_t* offs, const float* feats, bool assoc,
-                    std::vector<int>* qoff, std::vector<const float*>* src) {
+  // checks of a search / associate request; fills the newest-K row table
+  int check_queries(int Q, const uint64_t* qids, const int32_t* offs, const Column& col, bool assoc,
+                    std::vector<int>* qoff, std::vector<int>* row_src) {
     if (Q < 0) return fail(SB200_ERR_INVALID, "n_queries < 0");
     if (Q == 0) return 0;
     if (!qids || !offs) return fail(SB200_ERR_INVALID, "query_ids / obs_offsets is NULL");
     if (offs[0] != 0) return fail(SB200_ERR_INVALID, "obs_offsets[0] != 0");
     std::unordered_set<uint64_t> seen;
     seen.reserve((size_t)Q * 2);
-    qoff->assign(1, 0);
     const int K = o.max_observations;
     for (int q = 0; q < Q; ++q) {
       const int n = offs[q + 1] - offs[q];
@@ -181,11 +253,11 @@ struct sb200_fstore {
         return fail(SB200_ERR_INVALID, "query id %llu appears twice in the call", (unsigned long long)qids[q]);
       if (assoc && hpos.count(qids[q]))
         return fail(SB200_ERR_INVALID, "query id %llu is already stored", (unsigned long long)qids[q]);
-      for (int k = std::max(0, n - K); k < n; ++k) src->push_back(feats + (size_t)(offs[q] + k) * o.feature_dim);
-      qoff->push_back((int)src->size());
     }
-    if (!feats) return fail(SB200_ERR_INVALID, "features is NULL");
-    const long long pairs = (long long)src->size() * (long long)hid.size() * K;
+    if (!col.p) return fail(SB200_ERR_INVALID, "features is NULL");
+    if (int rc = check_column(col)) return rc;
+    sb::fs_row_table(Q, offs, K, row_src, qoff);
+    const long long pairs = (long long)row_src->size() * (long long)hid.size() * K;
     if (pairs > sb::kFsMaxPairs)
       return fail(SB200_ERR_CAPACITY, "the call needs %lld observation pairs; one call holds at most 2^30", pairs);
     return 0;
@@ -200,22 +272,19 @@ struct sb200_fstore {
   }
 
   // search (assoc == false) or associate
-  int run_queries(int Q, const uint64_t* qids, const int32_t* offs, const float* feats, int32_t* counts,
+  int run_queries(int Q, const uint64_t* qids, const int32_t* offs, const Column& col, int32_t* counts,
                   uint64_t* winners, double* weights, uint64_t* track_ids, uint8_t* merged, bool assoc) {
-    std::vector<int> qoff;
-    std::vector<const float*> src;
-    if (int rc = check_queries(Q, qids, offs, feats, assoc, &qoff, &src)) return rc;
+    std::vector<int> qoff, src;
+    if (int rc = check_queries(Q, qids, offs, col, assoc, &qoff, &src)) return rc;
     if (Q > 0 && (!counts || !winners || !weights || (assoc && (!track_ids || !merged))))
       return fail(SB200_ERR_INVALID, "an output is NULL");
     if (int rc = begin()) return rc;
     if (Q == 0) return 0;
     const int R = (int)src.size(), topn = o.topn, K = o.max_observations;
     const long long live = (long long)hid.size(), S = live * K;
-    const ReqLayout L(Q, R, d8);
+    const ReqLayout L(Q, R, d8, col.on_device || ftype != SB200_FEATURE_F32);
     const ResLayout RL(Q, topn);
-    if (int rc = hreq.ensure(L.total)) return rc;
     if (int rc = hres.ensure(RL.total)) return rc;
-    if (int rc = dreq.ensure(L.total)) return rc;
     if (int rc = dres.ensure(RL.total)) return rc;
     if (int rc = plan.ensure((size_t)Q * 16)) return rc;
     if (o.metric == SB200_VIS_COSINE) {
@@ -225,10 +294,9 @@ struct sb200_fstore {
     if (int rc = dist.ensure((size_t)std::max<long long>((long long)R * S, 1) * 4)) return rc;
     if (assoc)
       if (int rc = reserve(hid.size() + (size_t)Q)) return rc;
-    stage(L, Q, qids, qoff, src, std::vector<int>(Q, -1));
+    if (int rc = upload(L, Q, qids, qoff, src, std::vector<int>(Q, -1), col, (size_t)offs[Q])) return rc;
     const sb::FsStore s = view();
     const sb::FsCall c = call_view(L, Q, R, &RL);
-    CU(cudaMemcpyAsync(dreq.p, hreq.p, L.total, cudaMemcpyHostToDevice, st));
     CU(cudaEventRecord(ev[0], st));
     sb::fs_launch_dist(o.metric, o.distance_filter, s, c, st);
     CU(cudaEventRecord(ev[1], st));
@@ -266,9 +334,10 @@ struct sb200_fstore {
     return 0;
   }
 
-  int add(int n, const uint64_t* idv, const float* feats) {
+  int add(int n, const uint64_t* idv, const Column& col) {
     if (n < 0) return fail(SB200_ERR_INVALID, "n < 0");
-    if (n > 0 && (!idv || !feats)) return fail(SB200_ERR_INVALID, "ids / features is NULL");
+    if (n > 0 && (!idv || !col.p)) return fail(SB200_ERR_INVALID, "ids / features is NULL");
+    if (int rc = check_column(col)) return rc;
     if (int rc = begin()) return rc;
     if (n == 0) return 0;
     // destination of every observation: a stored track, or a new one placed at the first appearance of its id
@@ -286,19 +355,15 @@ struct sb200_fstore {
       }
       dest[i] = jt->second;
     }
-    std::vector<int> qoff(n + 1);
-    std::vector<const float*> src(n);
+    std::vector<int> qoff(n + 1), src(n);
     for (int i = 0; i <= n; ++i) qoff[i] = i;
-    for (int i = 0; i < n; ++i) src[i] = feats + (size_t)i * o.feature_dim;
-    const ReqLayout L(n, n, d8);
-    if (int rc = hreq.ensure(L.total)) return rc;
-    if (int rc = dreq.ensure(L.total)) return rc;
+    for (int i = 0; i < n; ++i) src[i] = i;
+    const ReqLayout L(n, n, d8, col.on_device || ftype != SB200_FEATURE_F32);
     if (int rc = plan.ensure((size_t)n * 16)) return rc;
     if (int rc = reserve(hid.size() + fresh.size())) return rc;
-    stage(L, n, idv, qoff, src, dest);
+    if (int rc = upload(L, n, idv, qoff, src, dest, col, (size_t)n)) return rc;
     const sb::FsStore s = view();
     const sb::FsCall c = call_view(L, n, n, nullptr);
-    CU(cudaMemcpyAsync(dreq.p, hreq.p, L.total, cudaMemcpyHostToDevice, st));
     CU(cudaEventRecord(ev[2], st));
     sb::fs_launch_apply(s, c, st);
     CU(cudaEventRecord(ev[3], st));
@@ -371,6 +436,114 @@ struct sb200_fstore {
     }
     return found;
   }
+
+  // ---- the store blob (layout: include/similari_b200.h)
+  uint64_t lay_out(BlobHeader* h) const {
+    const uint64_t live = hid.size();
+    const uint64_t sec[SB200_FSTORE_BLOB_SECTIONS] = {live * 8, live * 4, live * 4,
+                                                      live * o.max_observations * d8 * 4};
+    uint64_t off = sec_align(sizeof(BlobHeader));
+    for (int i = 0; i < SB200_FSTORE_BLOB_SECTIONS; ++i) {
+      h->sec_off[i] = off;
+      h->sec_bytes[i] = sec[i];
+      off += sec_align(sec[i]);
+    }
+    return off;
+  }
+
+  // the kernels that read or write a blob's sections use 16-byte accesses; any other device blob goes through a copy
+  static bool in_place_ok(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+
+  // the four columns and their sections of a blob on this device: dir 0 packs, dir 1 unpacks
+  int move_columns(int dir, const BlobHeader& h, char* dblob) {
+    char* col[SB200_FSTORE_BLOB_SECTIONS] = {ids.as<char>(), cnt.as<char>(), start.as<char>(), feat.as<char>()};
+    std::vector<sb::XferSeg> segs;
+    for (int i = 0; i < SB200_FSTORE_BLOB_SECTIONS; ++i) {
+      if (h.sec_bytes[i] == 0) continue;
+      char* sec = dblob + h.sec_off[i];
+      if (dir == 0) segs.push_back({col[i], sec, h.sec_bytes[i]});
+      else segs.push_back({sec, col[i], h.sec_bytes[i]});
+    }
+    return sb::copy_segments(segs, num_sms, st);
+  }
+
+  int save(void* dst, uint64_t cap_bytes, uint64_t* bytes) {
+    BlobHeader h;
+    memset(&h, 0, sizeof(h));
+    h.magic = SB200_FSTORE_BLOB_MAGIC; h.version = SB200_FSTORE_BLOB_VERSION;
+    h.metric = o.metric; h.distance_filter = o.distance_filter; h.max_observations = o.max_observations;
+    h.feature_dim = o.feature_dim; h.topn = o.topn; h.max_distance = o.max_distance; h.min_votes = o.min_votes;
+    h.d8 = d8; h.feature_type = ftype; h.live = (int64_t)hid.size();
+    const uint64_t total = h.total_bytes = lay_out(&h);
+    *bytes = total;
+    if (!dst) return 0;
+    if (cap_bytes < total) return fail(SB200_ERR_CAPACITY, "the blob needs %llu bytes", (unsigned long long)total);
+    CU(cudaSetDevice(o.device));
+    const int where = sb::blob_device(dst);
+    const bool in_place = where == o.device && in_place_ok(dst);
+    DBuf tmp;
+    char* dblob = static_cast<char*>(dst);
+    if (!in_place) {
+      if (int rc = tmp.ensure(total)) return rc;
+      dblob = tmp.as<char>();
+    }
+    CU(cudaMemcpyAsync(dblob, &h, sizeof(h), cudaMemcpyHostToDevice, st));
+    uint64_t end = sizeof(h);   // the gaps after the header and every section are zero (equal states give equal blobs)
+    for (int i = 0; i <= SB200_FSTORE_BLOB_SECTIONS; ++i) {
+      const uint64_t next = i < SB200_FSTORE_BLOB_SECTIONS ? h.sec_off[i] : total;
+      if (next > end) CU(cudaMemsetAsync(dblob + end, 0, next - end, st));
+      if (i < SB200_FSTORE_BLOB_SECTIONS) end = h.sec_off[i] + h.sec_bytes[i];
+    }
+    if (int rc = move_columns(0, h, dblob)) return rc;
+    sb::fs_launch_blob_scrub(reinterpret_cast<float*>(dblob + h.sec_off[kSecFeat]), cnt.as<int>(), start.as<int>(),
+                             (int)h.live, o.max_observations, d8, st);
+    CU(cudaStreamSynchronize(st));
+    CU(cudaGetLastError());
+    if (in_place) return 0;
+    if (where >= 0) {
+      CU(cudaMemcpyPeerAsync(dst, where, dblob, o.device, total, st));
+      CU(cudaStreamSynchronize(st));
+      return 0;
+    }
+    return sb::host_copy(st, dst, dblob, total, true);
+  }
+
+  // fills a store fresh from sb200_fstore_create with the checked blob `h` at `src`
+  int load(const BlobHeader& h, const void* src, std::vector<uint64_t>&& blob_ids) {
+    if (int rc = begin()) return rc;
+    const int live = (int)h.live, K = o.max_observations;
+    ftype = h.feature_type;
+    if (live == 0) return 0;
+    if (int rc = reserve((size_t)live)) return rc;
+    const int where = sb::blob_device(src);
+    DBuf tmp;
+    char* dblob = const_cast<char*>(static_cast<const char*>(src));
+    if (where != o.device || !in_place_ok(src)) {
+      if (int rc = tmp.ensure(h.total_bytes)) return rc;
+      dblob = tmp.as<char>();
+      if (where >= 0) {
+        CU(cudaMemcpyPeerAsync(dblob, o.device, src, where, h.total_bytes, st));
+        CU(cudaStreamSynchronize(st));
+      } else if (int rc = sb::host_copy(st, const_cast<void*>(src), dblob, h.total_bytes, false)) {
+        return rc;
+      }
+    }
+    // counts and ring starts index the rows in every later kernel: checked before anything is copied into the store
+    int bad[2] = {0, 0};
+    if (int rc = gpos.ensure(sizeof(bad))) return rc;
+    CU(cudaMemsetAsync(gpos.p, 0, sizeof(bad), st));
+    sb::fs_launch_blob_check(reinterpret_cast<const int*>(dblob + h.sec_off[kSecCnt]),
+                             reinterpret_cast<const int*>(dblob + h.sec_off[kSecStart]), live, K, gpos.as<int>(), st);
+    CU(cudaMemcpyAsync(bad, gpos.p, sizeof(bad), cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    CU(cudaGetLastError());
+    if (bad[0]) return fail(SB200_ERR_INVALID, "the blob holds %d cnt entries outside 1..%d", bad[0], K);
+    if (bad[1]) return fail(SB200_ERR_INVALID, "the blob holds %d start entries outside 0..%d", bad[1], K - 1);
+    if (int rc = move_columns(1, h, dblob)) return rc;
+    hid = std::move(blob_ids);
+    for (size_t p = 0; p < hid.size(); ++p) hpos[hid[p]] = (int)p;
+    return 0;
+  }
 };
 
 // a call without a handle: SB200_ERR_CUDA when there is no device to have made one, else SB200_ERR_INVALID
@@ -386,13 +559,7 @@ int sb200_fstore_create(const sb200_fstore_options* opts, sb200_fstore** out) {
   *out = nullptr;
   if (int rc = sb::check_device(0)) return rc;   // no device at all; the index is checked after the options
   const sb200_fstore_options& o = *opts;
-  if (o.metric != SB200_VIS_EUCLIDEAN && o.metric != SB200_VIS_COSINE) return fail(SB200_ERR_INVALID, "unknown metric");
-  if (o.max_observations < 1 || o.max_observations > SB200_FSTORE_MAX_OBS)
-    return fail(SB200_ERR_INVALID, "max_observations must lie in 1..64");
-  if (o.feature_dim < 1 || o.feature_dim > SB200_FSTORE_MAX_DIM)
-    return fail(SB200_ERR_INVALID, "feature_dim must lie in 1..8192");
-  if (o.topn < 1 || o.topn > SB200_FSTORE_MAX_TOPN) return fail(SB200_ERR_INVALID, "topn must lie in 1..64");
-  if (o.min_votes < 0) return fail(SB200_ERR_INVALID, "min_votes < 0");
+  if (int rc = check_options(o)) return rc;
   if (int rc = sb::check_device(o.device)) return rc;
   CU(cudaSetDevice(o.device));
   sb200_fstore* s = new sb200_fstore();
@@ -400,6 +567,8 @@ int sb200_fstore_create(const sb200_fstore_options* opts, sb200_fstore** out) {
   s->d8 = (o.feature_dim + 7) / 8 * 8;
   cudaError_t e = cudaStreamCreateWithFlags(&s->st, cudaStreamNonBlocking);
   for (int i = 0; i < 4 && e == cudaSuccess; ++i) e = cudaEventCreate(&s->ev[i]);
+  if (e == cudaSuccess) e = cudaEventCreateWithFlags(&s->ev_in, cudaEventDisableTiming);
+  if (e == cudaSuccess) e = cudaDeviceGetAttribute(&s->num_sms, cudaDevAttrMultiProcessorCount, o.device);
   if (e != cudaSuccess) {
     delete s;
     return fail(SB200_ERR_CUDA, "stream / event creation failed: %s", cudaGetErrorString(e));
@@ -416,20 +585,22 @@ void sb200_fstore_destroy(sb200_fstore* s) {
 
 int sb200_fstore_add(sb200_fstore* s, int32_t n, const uint64_t* ids, const float* features) {
   if (!s) return no_handle();
-  return s->add(n, ids, features);
+  return s->add(n, ids, {features, false, nullptr});
 }
 
 int sb200_fstore_search(sb200_fstore* s, int32_t n_queries, const uint64_t* query_ids, const int32_t* obs_offsets,
                         const float* features, int32_t* counts, uint64_t* winners, double* weights) {
   if (!s) return no_handle();
-  return s->run_queries(n_queries, query_ids, obs_offsets, features, counts, winners, weights, nullptr, nullptr, false);
+  return s->run_queries(n_queries, query_ids, obs_offsets, {features, false, nullptr}, counts, winners, weights, nullptr,
+                        nullptr, false);
 }
 
 int sb200_fstore_associate(sb200_fstore* s, int32_t n_queries, const uint64_t* query_ids, const int32_t* obs_offsets,
                            const float* features, int32_t* counts, uint64_t* winners, double* weights,
                            uint64_t* track_ids, uint8_t* merged) {
   if (!s) return no_handle();
-  return s->run_queries(n_queries, query_ids, obs_offsets, features, counts, winners, weights, track_ids, merged, true);
+  return s->run_queries(n_queries, query_ids, obs_offsets, {features, false, nullptr}, counts, winners, weights, track_ids,
+                        merged, true);
 }
 
 int64_t sb200_fstore_fetch(sb200_fstore* s, int32_t n, const uint64_t* ids, int32_t remove, int32_t* counts,
@@ -455,6 +626,102 @@ int sb200_fstore_last_stage_ms(sb200_fstore* s, float* out3) {
   if (!s) return no_handle();
   if (!out3) return fail(SB200_ERR_INVALID, "out3 is NULL");
   std::copy(s->stage_ms, s->stage_ms + 3, out3);
+  return 0;
+}
+
+int sb200_fstore_set_feature_type(sb200_fstore* s, int32_t type) {
+  if (!s) return no_handle();
+  if (type != SB200_FEATURE_F32 && type != SB200_FEATURE_F16 && type != SB200_FEATURE_BF16)
+    return fail(SB200_ERR_INVALID, "unknown feature type %d", type);
+  s->ftype = type;
+  return 0;
+}
+
+int sb200_fstore_get_options(sb200_fstore* s, sb200_fstore_options* out, int32_t* feature_type) {
+  if (!s) return no_handle();
+  if (out) *out = s->o;
+  if (feature_type) *feature_type = s->ftype;
+  return 0;
+}
+
+int sb200_fstore_add_device(sb200_fstore* s, int32_t n, const uint64_t* ids, const void* d_features, void* cuda_stream) {
+  if (!s) return no_handle();
+  return s->add(n, ids, {d_features, true, static_cast<cudaStream_t>(cuda_stream)});
+}
+
+int sb200_fstore_search_device(sb200_fstore* s, int32_t n_queries, const uint64_t* query_ids,
+                               const int32_t* obs_offsets, const void* d_features, int32_t* counts, uint64_t* winners,
+                               double* weights, void* cuda_stream) {
+  if (!s) return no_handle();
+  return s->run_queries(n_queries, query_ids, obs_offsets, {d_features, true, static_cast<cudaStream_t>(cuda_stream)},
+                        counts, winners, weights, nullptr, nullptr, false);
+}
+
+int sb200_fstore_associate_device(sb200_fstore* s, int32_t n_queries, const uint64_t* query_ids,
+                                  const int32_t* obs_offsets, const void* d_features, int32_t* counts,
+                                  uint64_t* winners, double* weights, uint64_t* track_ids, uint8_t* merged,
+                                  void* cuda_stream) {
+  if (!s) return no_handle();
+  return s->run_queries(n_queries, query_ids, obs_offsets, {d_features, true, static_cast<cudaStream_t>(cuda_stream)},
+                        counts, winners, weights, track_ids, merged, true);
+}
+
+int sb200_fstore_save(sb200_fstore* s, void* buf, uint64_t cap, uint64_t* bytes) {
+  if (!s) return no_handle();
+  if (!bytes) return fail(SB200_ERR_INVALID, "bytes is NULL");
+  return s->save(buf, cap, bytes);
+}
+
+int sb200_fstore_load(const void* buf, uint64_t bytes, int32_t device, sb200_fstore** out) {
+  if (!buf || !out) return fail(SB200_ERR_INVALID, "buf / out is NULL");
+  *out = nullptr;
+  if (int rc = sb::check_device(device)) return rc;
+  CU(cudaSetDevice(device));
+  // no store (and no caller stream) yet: a device blob must be complete when the call is made
+  if (bytes < sizeof(BlobHeader)) return fail(SB200_ERR_INVALID, "the blob is truncated (%llu bytes)", (unsigned long long)bytes);
+  BlobHeader h;
+  CU(cudaMemcpy(&h, buf, sizeof(h), cudaMemcpyDefault));
+  if (h.magic != SB200_FSTORE_BLOB_MAGIC) return fail(SB200_ERR_INVALID, "not a feature store blob (bad magic)");
+  if (h.version != SB200_FSTORE_BLOB_VERSION)
+    return fail(SB200_ERR_INVALID, "feature store blob version %u (this library reads %u)", h.version, SB200_FSTORE_BLOB_VERSION);
+  if (h.total_bytes > bytes)
+    return fail(SB200_ERR_INVALID, "the blob is truncated (%llu of total_bytes %llu)", (unsigned long long)bytes,
+                (unsigned long long)h.total_bytes);
+  sb200_fstore_options o = {h.metric, h.distance_filter, h.max_observations, h.feature_dim, h.topn, h.max_distance,
+                            h.min_votes, device};
+  if (int rc = check_options(o)) return rc;
+  if (h.d8 != (h.feature_dim + 7) / 8 * 8) return fail(SB200_ERR_INVALID, "d8 is not feature_dim rounded up to 8");
+  if (h.feature_type != SB200_FEATURE_F32 && h.feature_type != SB200_FEATURE_F16 && h.feature_type != SB200_FEATURE_BF16)
+    return fail(SB200_ERR_INVALID, "unknown feature_type %d", h.feature_type);
+  // live * K indexes the distance matrix's columns as an int
+  if (h.live < 0 || h.live > INT32_MAX / h.max_observations) return fail(SB200_ERR_INVALID, "live count out of range");
+  const uint64_t live = (uint64_t)h.live;
+  const uint64_t want[SB200_FSTORE_BLOB_SECTIONS] = {live * 8, live * 4, live * 4,
+                                                     live * h.max_observations * h.d8 * 4};
+  static const char* const kName[SB200_FSTORE_BLOB_SECTIONS] = {"ids", "cnt", "start", "feat"};
+  uint64_t end = sizeof(BlobHeader);
+  for (int i = 0; i < SB200_FSTORE_BLOB_SECTIONS; ++i) {
+    if (h.sec_off[i] % kSecAlign != 0) return fail(SB200_ERR_INVALID, "section %s is not 256-byte aligned", kName[i]);
+    if (h.sec_off[i] < end || h.sec_off[i] > h.total_bytes || h.sec_bytes[i] > h.total_bytes - h.sec_off[i])
+      return fail(SB200_ERR_INVALID, "section %s lies outside the blob or overlaps the one before", kName[i]);
+    if (h.sec_bytes[i] != want[i])
+      return fail(SB200_ERR_INVALID, "section %s holds %llu bytes, %llu expected", kName[i],
+                  (unsigned long long)h.sec_bytes[i], (unsigned long long)want[i]);
+    end = h.sec_off[i] + h.sec_bytes[i];
+  }
+  std::vector<uint64_t> blob_ids(live);
+  if (live) CU(cudaMemcpy(blob_ids.data(), static_cast<const char*>(buf) + h.sec_off[kSecIds], live * 8, cudaMemcpyDefault));
+  std::unordered_set<uint64_t> seen;
+  seen.reserve(live * 2);
+  for (uint64_t id : blob_ids)
+    if (!seen.insert(id).second) return fail(SB200_ERR_INVALID, "id %llu appears twice in the blob", (unsigned long long)id);
+  sb200_fstore* s = nullptr;
+  if (int rc = sb200_fstore_create(&o, &s)) return rc;
+  if (int rc = s->load(h, buf, std::move(blob_ids))) {
+    sb200_fstore_destroy(s);   // the handle owns every buffer made so far
+    return rc;
+  }
+  *out = s;
   return 0;
 }
 

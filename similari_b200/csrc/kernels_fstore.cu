@@ -1,4 +1,5 @@
-// kernels_fstore.cu -- the feature track store's call: distances, TopN voting, merge / append.
+// kernels_fstore.cu -- the feature track store's call: distances, TopN voting, merge / append; the request rows built
+// from a typed or device-resident feature column (fs_stage_kernel); the index check and slot scrub of the store blob.
 //
 // Replaces, for feature-only tracks (benches/feature_tracker.rs),
 //   TrackStore::foreign_track_distances -> Track::distances -> euclidean / cosine (src/track/store.rs:199-250,
@@ -344,6 +345,64 @@ __global__ void fs_compact_kernel(FsStore src, FsStore dst, const int* from) {
   }
 }
 
+// ------------------------------------------------------------------------------------------------ request rows
+// Builds FsCall::rows from a feature column that is on the device already (the caller's, or the uploaded raw rows of a
+// 2-byte host column): one thread per 8-lane block of a request row.  Widening is exact and done from the bits (sb_engine.cuh),
+// so every later stage sees the values of the widened f32 request.  With `vec` (D % 8 == 0 and a 16-byte aligned base) a
+// block of a 2-byte column is one 16-byte load, as in cand_norm_kernel; otherwise elements are read one by one and the
+// last block is zero-padded from D to d8.
+__device__ __forceinline__ void fs_load8(const float* p, float* x) {
+  const float4 a = *reinterpret_cast<const float4*>(p), b = *reinterpret_cast<const float4*>(p + 4);
+  x[0] = a.x; x[1] = a.y; x[2] = a.z; x[3] = a.w; x[4] = b.x; x[5] = b.y; x[6] = b.z; x[7] = b.w;
+}
+template <typename T>
+__device__ __forceinline__ void fs_load8(const T* p, float* x) {
+  feat_widen8(*reinterpret_cast<const uint4*>(p), p, x);
+}
+
+template <typename T>
+__global__ void __launch_bounds__(256) fs_stage_kernel(const T* __restrict__ col, const int* __restrict__ row_src, int R,
+                                                       int D, int d8, int vec, float* __restrict__ rows) {
+  const int nblk = d8 / 8;
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (long long)R * nblk) return;
+  const int r = (int)(i / nblk), k0 = (int)(i - (long long)r * nblk) * 8;
+  const T* src = col + (size_t)row_src[r] * D + k0;
+  float x[8];
+  if (vec) {
+    fs_load8(src, x);
+  } else {
+#pragma unroll
+    for (int l = 0; l < 8; ++l) x[l] = k0 + l < D ? feat_elem(src, l) : 0.0f;
+  }
+  float4* dst = reinterpret_cast<float4*>(rows + (size_t)r * d8 + k0);
+  dst[0] = make_float4(x[0], x[1], x[2], x[3]);
+  dst[1] = make_float4(x[4], x[5], x[6], x[7]);
+}
+
+// ------------------------------------------------------------------------------------------------ store blob
+__global__ void fs_blob_check_kernel(const int* __restrict__ cnt, const int* __restrict__ start, int n, int K, int* bad) {
+  int bc = 0, bs = 0;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    bc += (cnt[i] < 1 || cnt[i] > K);
+    bs += (start[i] < 0 || start[i] >= K);
+  }
+  if (bc) atomicAdd(bad, bc);
+  if (bs) atomicAdd(bad + 1, bs);
+}
+
+// one warp per track; a track whose ring is full has nothing to zero
+__global__ void fs_blob_scrub_kernel(float* feat, const int* __restrict__ cnt, const int* __restrict__ start, int n, int K,
+                                     int d8) {
+  const int t = (int)(((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
+  if (t >= n) return;
+  const int c = cnt[t], s0 = start[t], w4 = d8 / 4;
+  for (int j = c; j < K; ++j) {
+    float4* d = reinterpret_cast<float4*>(feat + ((size_t)t * K + (s0 + j) % K) * d8);
+    for (int e = lane; e < w4; e += 32) d[e] = make_float4(0.f, 0.f, 0.f, 0.f);
+  }
+}
+
 }  // namespace
 
 void fs_launch_dist(int metric, float filter, const FsStore& s, const FsCall& c, cudaStream_t st) {
@@ -384,6 +443,30 @@ void fs_launch_gather(const FsStore& s, const int* pos, int n, float* out, int* 
 void fs_launch_compact(const FsStore& src, const FsStore& dst, const int* from, int n, cudaStream_t st) {
   if (n == 0) return;
   fs_compact_kernel<<<n, 128, 0, st>>>(src, dst, from);
+  note_launch();
+}
+
+void fs_launch_stage(int type, const void* col, const int* row_src, int R, int D, int d8, float* rows, cudaStream_t st) {
+  if (R == 0) return;
+  const int vec = D % 8 == 0 && (reinterpret_cast<uintptr_t>(col) & 15) == 0;
+  const long long threads = (long long)R * (d8 / 8);
+  feat_dispatch(type, [&](auto tag) {
+    using T = decltype(tag);
+    fs_stage_kernel<T><<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(static_cast<const T*>(col), row_src, R, D, d8, vec,
+                                                                         rows);
+  });
+  note_launch();
+}
+
+void fs_launch_blob_check(const int* cnt, const int* start, int n, int K, int* bad, cudaStream_t st) {
+  if (n == 0) return;
+  fs_blob_check_kernel<<<std::min((n + 255) / 256, 1024), 256, 0, st>>>(cnt, start, n, K, bad);
+  note_launch();
+}
+
+void fs_launch_blob_scrub(float* feat, const int* cnt, const int* start, int n, int K, int d8, cudaStream_t st) {
+  if (n == 0) return;
+  fs_blob_scrub_kernel<<<(unsigned)(((long long)n * 32 + 255) / 256), 256, 0, st>>>(feat, cnt, start, n, K, d8);
   note_launch();
 }
 

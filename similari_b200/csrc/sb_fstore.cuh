@@ -7,6 +7,9 @@
 #include <stdint.h>
 #include <string.h>
 
+#include <algorithm>
+#include <vector>
+
 namespace sb {
 
 constexpr int kFsMaxTopn = 64;
@@ -51,6 +54,21 @@ __host__ __device__ __forceinline__ int fs_key(float f) {
   return b >= 0 ? b : (b ^ 0x7fffffff);
 }
 
+// The rows of the caller's feature column that take part in a search / associate call: the newest K of each query, query
+// by query, oldest first (a track built by TrackBuilder keeps its newest K, src/track/builder.rs:168-179).  row_src[r] is
+// the column row behind request row r, qoff[q] .. qoff[q + 1] the request rows of query q.  offs is the caller's CSR
+// (offs[0] == 0, every query with at least one row: checked by the caller).
+inline void fs_row_table(int Q, const int32_t* offs, int K, std::vector<int>* row_src, std::vector<int>* qoff) {
+  row_src->clear();
+  qoff->assign(1, 0);
+  for (int q = 0; q < Q; ++q) {
+    for (int r = std::max(offs[q], offs[q + 1] - K); r < offs[q + 1]; ++r) row_src->push_back(r);
+    qoff->push_back((int)row_src->size());
+  }
+}
+
+// rows[r][0 .. d8) = column row row_src[r] widened to f32 and zero-padded from D; `type` is the column's SB200_FEATURE_*
+void fs_launch_stage(int type, const void* col, const int* row_src, int R, int D, int d8, float* rows, cudaStream_t st);
 void fs_launch_dist(int metric, float filter, const FsStore& s, const FsCall& c, cudaStream_t st);
 void fs_launch_topn(float max_distance, int min_votes, int topn, bool want_dest, const FsStore& s, const FsCall& c,
                     cudaStream_t st);
@@ -59,5 +77,9 @@ void fs_launch_apply(const FsStore& s, const FsCall& c, cudaStream_t st);
 void fs_launch_gather(const FsStore& s, const int* pos, int n, float* out, int* out_cnt, cudaStream_t st);
 // dst[i] = src[from[i]] for the i < n kept tracks (stable compaction into fresh columns)
 void fs_launch_compact(const FsStore& src, const FsStore& dst, const int* from, int n, cudaStream_t st);
+// store blob, before any row is copied: bad[0] counts the cnt[i] outside [1, K], bad[1] the start[i] outside [0, K)
+void fs_launch_blob_check(const int* cnt, const int* start, int n, int K, int* bad, cudaStream_t st);
+// store blob, after its rows are copied: zeroes, in feat[n][K][d8], the ring slots that hold no observation
+void fs_launch_blob_scrub(float* feat, const int* cnt, const int* start, int n, int K, int d8, cudaStream_t st);
 
 }  // namespace sb

@@ -390,9 +390,9 @@ class Tracker:
 _ERR_CAPACITY = -3
 
 
-def _host_blob(call):
+def _host_blob(call, size_t=C.c_size_t):
     """Size query, then the blob into a uint8 array."""
-    n = C.c_size_t(0)
+    n = size_t(0)
     rc = call(None, 0, C.byref(n))
     if rc != _ERR_CAPACITY:
         check(rc)
@@ -401,8 +401,8 @@ def _host_blob(call):
     return out[: n.value]
 
 
-def _device_blob(call, d_ptr, cap):
-    n = C.c_size_t(0)
+def _device_blob(call, d_ptr, cap, size_t=C.c_size_t):
+    n = size_t(0)
     if not d_ptr:
         rc = call(None, 0, C.byref(n))
         if rc != _ERR_CAPACITY:
@@ -660,7 +660,13 @@ class FeatureStore:
     """Device-resident feature track store: the reference's TrackStore for feature-only tracks (one feature class, no
     track attributes) with TopNVoting(topn, max_distance, min_votes) on top (sb200_fstore_*).  Each track keeps its
     newest `max_observations` observations.  Queries are given in CSR form: ids[q] with the feature rows
-    features[offsets[q]:offsets[q + 1]], oldest first.  numpy in, numpy out."""
+    features[offsets[q]:offsets[q + 1]], oldest first.  numpy in, numpy out.
+
+    Features: a float16 array is sent as it is; any other dtype is widened to float32.  After set_feature_type("bf16")
+    (or "f16") a 2-byte array (e.g. the uint16 bits of bfloat16 values) is sent as it is, with that element type.  The
+    *_device calls take the raw address of a column on the store's device, in the type set by set_feature_type, and a
+    cudaStream_t (0: the legacy default stream) whose pending work the call waits for.  Results never depend on the
+    type or on where the column lives: they are those of the widened float32 request."""
 
     def __init__(self, metric="euclidean", distance_filter=100.0, max_observations=3, feature_dim=256, topn=1,
                  max_distance=100.0, min_votes=1, device=0):
@@ -673,6 +679,7 @@ class FeatureStore:
         check(self._L.sb200_fstore_create(C.byref(o), C.byref(h)))
         self._h = h
         self.K, self.D, self.topn = int(max_observations), int(feature_dim), int(topn)
+        self._explicit_type = None
 
     def close(self):
         if getattr(self, "_h", None):
@@ -685,20 +692,60 @@ class FeatureStore:
         except Exception:
             pass
 
+    def set_feature_type(self, feature_type):
+        """sb200_fstore_set_feature_type: "f32", "f16" or "bf16".  With a 2-byte type, host arrays of 2-byte elements are
+        sent as they are; with "f32" (the default) the host calls pick float16 arrays up by their dtype."""
+        if feature_type not in FEATURE_TYPES:
+            raise ValueError(f"feature_type must be one of {sorted(FEATURE_TYPES)}")
+        check(self._L.sb200_fstore_set_feature_type(self._h, FEATURE_TYPES[feature_type]))
+        self._explicit_type = None if feature_type == "f32" else feature_type
+
+    def feature_type(self):
+        """The element type now set in the library."""
+        t = C.c_int32(0)
+        check(self._L.sb200_fstore_get_options(self._h, None, C.byref(t)))
+        return {v: k for k, v in FEATURE_TYPES.items()}[t.value]
+
+    def _use_declared_type(self):
+        """Device columns and blobs go by the type set_feature_type declared, not by the dtype of the last host array."""
+        check(self._L.sb200_fstore_set_feature_type(self._h, FEATURE_TYPES[self._explicit_type or "f32"]))
+
+    def _column(self, features):
+        """The host column as the library will read it, with the library's element type set to match."""
+        if self._explicit_type is not None:
+            return _raw16(features, self._explicit_type).reshape(-1, self.D)
+        if isinstance(features, np.ndarray) and features.dtype == np.float16:
+            check(self._L.sb200_fstore_set_feature_type(self._h, _lib.FEATURE_F16))
+            return np.ascontiguousarray(features).reshape(-1, self.D)
+        check(self._L.sb200_fstore_set_feature_type(self._h, _lib.FEATURE_F32))
+        return _f32(features).reshape(-1, self.D)
+
     def add(self, ids, features):
         """TrackStore::add for each (ids[i], features[i]) in order."""
         ids = np.ascontiguousarray(ids, dtype=np.uint64)
-        f = _f32(features).reshape(len(ids), self.D)
+        f = self._column(features)
+        if len(f) != len(ids):
+            raise ValueError("features needs one row per id")
         check(self._L.sb200_fstore_add(self._h, len(ids), ptr(ids), ptr(f)))
+
+    def add_device(self, ids, d_features, stream=0):
+        """sb200_fstore_add_device: `d_features` is the raw device address of [len(ids)][feature_dim] elements of the
+        type set by set_feature_type (e.g. the data_ptr() of a torch CUDA tensor)."""
+        ids = np.ascontiguousarray(ids, dtype=np.uint64)
+        self._use_declared_type()
+        check(self._L.sb200_fstore_add_device(self._h, len(ids), ptr(ids), C.c_void_p(d_features or None),
+                                              C.c_void_p(stream or None)))
 
     def _queries(self, ids, offsets, features):
         ids = np.ascontiguousarray(ids, dtype=np.uint64)
         offs = np.ascontiguousarray(offsets, dtype=np.int32)
         if len(offs) != len(ids) + 1:
             raise ValueError("offsets must have len(ids) + 1 entries")
-        f = _f32(features).reshape(-1, self.D)
-        if len(ids) and int(offs[-1]) > len(f):
-            raise ValueError("offsets[-1] exceeds the feature rows")
+        f = None
+        if features is not None:   # None: a device column, which the caller sized
+            f = self._column(features)
+            if len(ids) and int(offs[-1]) > len(f):
+                raise ValueError("offsets[-1] exceeds the feature rows")
         q = len(ids)
         out = {"counts": np.zeros(q, np.int32), "winners": np.zeros((q, self.topn), np.uint64),
                "weights": np.zeros((q, self.topn), np.float64)}
@@ -720,6 +767,27 @@ class FeatureStore:
         check(self._L.sb200_fstore_associate(self._h, len(ids), ptr(ids), ptr(offs), ptr(f), ptr(out["counts"]),
                                              ptr(out["winners"]), ptr(out["weights"]), ptr(out["track_ids"]),
                                              ptr(out["merged"])))
+        return out
+
+    def search_device(self, ids, offsets, d_features, stream=0):
+        """sb200_fstore_search_device: search with the feature rows at the raw device address `d_features`."""
+        ids, offs, _, out = self._queries(ids, offsets, None)
+        self._use_declared_type()
+        check(self._L.sb200_fstore_search_device(self._h, len(ids), ptr(ids), ptr(offs), C.c_void_p(d_features or None),
+                                                 ptr(out["counts"]), ptr(out["winners"]), ptr(out["weights"]),
+                                                 C.c_void_p(stream or None)))
+        return out
+
+    def associate_device(self, ids, offsets, d_features, stream=0):
+        """sb200_fstore_associate_device: associate with the feature rows at the raw device address `d_features`."""
+        ids, offs, _, out = self._queries(ids, offsets, None)
+        self._use_declared_type()
+        out["track_ids"] = np.zeros(len(ids), np.uint64)
+        out["merged"] = np.zeros(len(ids), np.uint8)
+        check(self._L.sb200_fstore_associate_device(self._h, len(ids), ptr(ids), ptr(offs),
+                                                    C.c_void_p(d_features or None), ptr(out["counts"]),
+                                                    ptr(out["winners"]), ptr(out["weights"]), ptr(out["track_ids"]),
+                                                    ptr(out["merged"]), C.c_void_p(stream or None)))
         return out
 
     def fetch(self, ids, remove=False):
@@ -746,3 +814,33 @@ class FeatureStore:
         out = np.zeros(3, np.float32)
         check(self._L.sb200_fstore_last_stage_ms(self._h, ptr(out)))
         return out
+
+    # ---- the store blob
+    def save(self):
+        """sb200_fstore_save into host memory: the whole store as a uint8 array."""
+        self._use_declared_type()
+        return _host_blob(lambda p, cap, n: self._L.sb200_fstore_save(self._h, p, cap, n), C.c_uint64)
+
+    def save_device(self, d_ptr, cap):
+        """sb200_fstore_save into device memory (any device) at raw address `d_ptr` of `cap` bytes; returns the bytes
+        written.  d_ptr == 0 returns the size the blob needs and writes nothing."""
+        self._use_declared_type()
+        return _device_blob(lambda p, c, n: self._L.sb200_fstore_save(self._h, p, c, n), d_ptr, cap, C.c_uint64)
+
+    @classmethod
+    def load(cls, blob_or_ptr, nbytes=None, device=0):
+        """sb200_fstore_load: a new store on `device` from a blob of save() (a uint8 array / bytes) or at a raw device
+        address `blob_or_ptr` of `nbytes` bytes.  The options, and the feature type set, are the blob's."""
+        p, n, keep = _blob_src(blob_or_ptr, nbytes)
+        L = lib()
+        h = C.c_void_p()
+        check(L.sb200_fstore_load(p, n, int(device), C.byref(h)))
+        del keep
+        self = cls.__new__(cls)
+        self._L, self._h = L, h
+        o, t = _lib.FstoreOptions(), C.c_int32(0)
+        check(L.sb200_fstore_get_options(h, C.byref(o), C.byref(t)))
+        self.K, self.D, self.topn = int(o.max_observations), int(o.feature_dim), int(o.topn)
+        name = {v: k for k, v in FEATURE_TYPES.items()}[t.value]
+        self._explicit_type = None if name == "f32" else name
+        return self

@@ -1,0 +1,118 @@
+"""CPU checks of the feature store's I/O additions (typed and device-resident feature columns, the store blob): the new
+entry points are declared and exported, the blob header that Python mirrors is the one the C header declares, a load
+without a GPU fails loudly, and the host-side row table behind fs_stage_kernel (the newest K rows of each query) matches a
+numpy restatement."""
+import ctypes as C
+import os
+import re
+import subprocess
+
+import numpy as np
+import pytest
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+HEADER = os.path.join(ROOT, "include", "similari_b200.h")
+NEW = ["sb200_fstore_set_feature_type", "sb200_fstore_add_device", "sb200_fstore_search_device",
+       "sb200_fstore_associate_device", "sb200_fstore_save", "sb200_fstore_load"]
+CTYPES = {"uint32_t": C.c_uint32, "uint64_t": C.c_uint64, "int32_t": C.c_int32, "int64_t": C.c_int64, "float": C.c_float}
+
+
+@pytest.fixture(scope="module")
+def L():
+    from similari_b200 import _build, _lib
+
+    _build.build()
+    return _lib.lib()
+
+
+def test_new_symbols_are_declared_and_exported(L):
+    from similari_b200 import _lib
+
+    hdr = open(HEADER).read()
+    for name in NEW + ["sb200_fstore_get_options"]:
+        assert re.search(r"\b%s\s*\(" % name, hdr), name
+        assert name in _lib.EXPORTS
+        assert getattr(L, name).argtypes is not None
+
+
+def test_blob_header_mirror_matches_the_c_header():
+    from similari_b200 import _lib
+
+    hdr = open(HEADER).read()
+    defs = dict(re.findall(r"#define (SB200_FSTORE_BLOB_[A-Z]+) (\w+)", hdr))
+    val = lambda k: int(defs["SB200_FSTORE_BLOB_" + k].rstrip("u"), 0)  # noqa: E731
+    assert (val("MAGIC"), val("VERSION"), val("ALIGN"), val("SECTIONS")) == \
+        (_lib.FSTORE_BLOB_MAGIC, _lib.FSTORE_BLOB_VERSION, _lib.FSTORE_BLOB_ALIGN, _lib.FSTORE_BLOB_SECTIONS)
+    assert _lib.FSTORE_BLOB_MAGIC.to_bytes(4, "little") == b"SBFS"
+    body = re.search(r"typedef struct \{([^}]*)\} sb200_fstore_blob_header;", hdr).group(1)
+    body = re.sub(r"/\*.*?\*/", "", body, flags=re.S)
+    declared = []
+    for typ, name, dim in re.findall(r"(\w+)\s+(\w+)(?:\[(\w+)\])?;", body):
+        declared.append((name, CTYPES[typ] * val(dim.replace("SB200_FSTORE_BLOB_", "")) if dim else CTYPES[typ]))
+    mirror = [(n, t) for n, t in _lib.FstoreBlobHeader._fields_]
+    assert [n for n, _ in declared] == [n for n, _ in mirror]
+    for (n, a), (_, b) in zip(declared, mirror):
+        assert C.sizeof(a) == C.sizeof(b) and a._type_ == b._type_, n
+    assert C.sizeof(_lib.FstoreBlobHeader) == 128 <= _lib.FSTORE_BLOB_ALIGN
+    # every options field but the device travels in the blob
+    opts = [n for n, _ in _lib.FstoreOptions._fields_ if n != "device"]
+    assert [n for n, _ in mirror][3:3 + len(opts)] == opts
+
+
+def test_entry_points_fail_without_a_gpu(L):
+    from similari_b200 import _lib
+    import similari_b200.engine as eng
+
+    if L.sb200_device_count() > 0:
+        pytest.skip("a GPU is present; the loud-failure path is for CPU-only machines")
+    ids = np.zeros(1, np.uint64)
+    offs = np.array([0, 1], np.int32)
+    cnt = np.zeros(1, np.int32)
+    w = np.zeros(1, np.float64)
+    m = np.zeros(1, np.uint8)
+    n = C.c_uint64(0)
+    p = _lib.ptr
+    assert L.sb200_fstore_set_feature_type(None, 1) == -2
+    assert L.sb200_fstore_get_options(None, None, None) == -2
+    assert L.sb200_fstore_add_device(None, 1, p(ids), None, None) == -2
+    assert L.sb200_fstore_search_device(None, 1, p(ids), p(offs), None, p(cnt), p(ids), p(w), None) == -2
+    assert L.sb200_fstore_associate_device(None, 1, p(ids), p(offs), None, p(cnt), p(ids), p(w), p(ids), p(m), None) == -2
+    assert L.sb200_fstore_save(None, None, 0, C.byref(n)) == -2
+    blob = np.zeros(1024, np.uint8)
+    h = C.c_void_p()
+    assert L.sb200_fstore_load(p(blob), len(blob), 0, C.byref(h)) == -2 and h.value is None
+    assert b"no CUDA device" in L.sb200_last_error()
+    with pytest.raises(_lib.Sb200Error, match="-2"):
+        eng.FeatureStore.load(blob)
+
+
+@pytest.fixture(scope="module")
+def rows_shim(tmp_path_factory):
+    from similari_b200 import _build
+
+    so = str(tmp_path_factory.mktemp("fstore_shim") / "libfstore_rows.so")
+    inc = os.path.join(os.path.dirname(os.path.dirname(os.path.realpath(_build.nvcc()))), "include")
+    subprocess.check_call(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-I", inc,
+                           os.path.join(ROOT, "tests", "host_shim", "fstore_rows_shim.cpp"), "-o", so])
+    lib = C.CDLL(so)
+    lib.shim_fs_row_table.restype = C.c_int
+    lib.shim_fs_row_table.argtypes = [C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
+    return lib
+
+
+@pytest.mark.parametrize("K", [1, 3, 5, 64])
+def test_row_table_takes_the_newest_k_rows_of_each_query(rows_shim, K):
+    rng = np.random.default_rng(K)
+    for Q in (1, 2, 17, 300):
+        lens = rng.integers(1, 2 * K + 3, Q)
+        lens[0] = K   # exactly K, one more and one fewer are all present
+        if Q > 2:
+            lens[1], lens[2] = K + 1, max(1, K - 1)
+        offs = np.concatenate([[0], np.cumsum(lens)]).astype(np.int32)
+        row_src = np.full(int(offs[-1]), -1, np.int32)
+        qoff = np.full(Q + 1, -1, np.int32)
+        R = rows_shim.shim_fs_row_table(Q, offs.ctypes.data, K, row_src.ctypes.data, qoff.ctypes.data)
+        want = [np.arange(offs[q], offs[q + 1])[-K:] for q in range(Q)]
+        assert R == sum(len(x) for x in want)
+        assert np.array_equal(row_src[:R], np.concatenate(want))
+        assert np.array_equal(qoff, np.concatenate([[0], np.cumsum([len(x) for x in want])]))
