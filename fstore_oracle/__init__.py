@@ -3,7 +3,7 @@
 ctypes binding of ``fstore_oracle/libfstore_oracle.so`` (built from ``feature_store.cpp`` by ``build()``), which calls
 the distance code of ``oracle/liboracle.so``.  It restates the reference's TrackStore for feature-only tracks and
 TopNVoting::winners, and defines the orders the reference leaves to its shards and HashMaps (see feature_store.cpp).
-Only ``tests/``, ``__graft_entry__`` and ``tools/feature_store_bench.py`` import it; ``similari_b200`` never does.
+Only ``tests/``, ``__graft_entry__`` and the store benchmarks under ``tools/`` import it; ``similari_b200`` never does.
 """
 from __future__ import annotations
 
@@ -53,6 +53,8 @@ def lib():
             "ofs_size": (i64, [vp]),
             "ofs_ids": (i64, [vp, i64, vp]),
             "ofs_topn_voting": (C.c_int, [f32, i32, i32, i32, vp, vp, vp, vp, vp, vp]),
+            "ofs_search_owned": (C.c_int, [vp, i32, vp, i32, vp, vp, vp, i32]),
+            "ofs_merge_owned": (C.c_int, [vp, i32, vp, vp, i32]),
         }
         for name, (res, args) in sig.items():
             fn = getattr(L, name)
@@ -128,6 +130,27 @@ class FeatureStore:
         if rc:
             raise ValueError("invalid associate request")
         return out
+
+    def search_owned(self, ids, each=False):
+        """owned_track_distances + TopNVoting::winners for stored tracks; each=True: once per id."""
+        ids = np.ascontiguousarray(ids, dtype=np.uint64)
+        q = len(ids)
+        out = {"counts": np.zeros(q, np.int32), "winners": np.zeros((q, self.topn), np.uint64),
+               "weights": np.zeros((q, self.topn), np.float64)}
+        rc = self._L.ofs_search_owned(self._h, q, _p(ids), int(bool(each)), _p(out["counts"]), _p(out["winners"]),
+                                      _p(out["weights"]), self.threads)
+        if rc:
+            raise ValueError("invalid owned search request")
+        return out
+
+    def merge_owned(self, dest_ids, src_ids, remove=True):
+        """merge_owned for each pair (dest_ids[i], src_ids[i]) in order."""
+        d = np.ascontiguousarray(dest_ids, dtype=np.uint64)
+        s = np.ascontiguousarray(src_ids, dtype=np.uint64)
+        if len(d) != len(s):
+            raise ValueError("dest_ids and src_ids must have the same length")
+        if self._L.ofs_merge_owned(self._h, len(d), _p(d), _p(s), int(bool(remove))):
+            raise ValueError("invalid merge request")
 
     def fetch(self, ids, remove=False):
         ids = np.ascontiguousarray(ids, dtype=np.uint64)

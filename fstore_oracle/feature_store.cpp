@@ -279,6 +279,76 @@ int64_t ofs_fetch(ofs_store* s, int n, const uint64_t* ids, int remove, int32_t*
   return found;
 }
 
+// owned_track_distances (src/track/store.rs:471-486) + TopNVoting::winners, written literally: fetch_tracks the queried
+// set out of the store, search the remainder with the fetched tracks as queries, put the tracks back (at their store
+// positions: the order rule that replaces the reference's HashMap).  each != 0: once per id, in order.  An id that is not
+// stored gets count 0; an id twice is rejected (-1).
+int ofs_search_owned(ofs_store* s, int n, const uint64_t* ids, int each, int32_t* counts, uint64_t* winners,
+                     double* weights, int threads) {
+  if (n < 0) return -1;
+  std::unordered_set<uint64_t> seen;
+  for (int q = 0; q < n; ++q)
+    if (!seen.insert(ids[q]).second) return -1;
+  auto owned = [&](int a, int b) {   // one owned_track_distances(ids[a .. b)) call
+    const std::vector<Track> saved = s->tracks;
+    std::vector<Track> qs;
+    for (int q = a; q < b; ++q) {   // fetch_tracks
+      auto it = std::find_if(s->tracks.begin(), s->tracks.end(), [&](const Track& t) { return t.id == ids[q]; });
+      if (it == s->tracks.end()) continue;
+      qs.push_back(*it);
+      s->tracks.erase(it);
+    }
+    s->reindex();
+    const auto r = s->search(qs, threads);
+    s->tracks = saved;   // add_track of every fetched track
+    s->reindex();
+    for (int q = a; q < b; ++q) {
+      std::vector<Elt> none;
+      const std::vector<Elt>* res = &none;
+      for (size_t i = 0; i < qs.size(); ++i)
+        if (qs[i].id == ids[q]) res = &r[i];
+      counts[q] = (int32_t)res->size();
+      for (int e = 0; e < s->topn; ++e) {
+        const bool ok = e < (int)res->size();
+        winners[(size_t)q * s->topn + e] = ok ? (*res)[e].winner : 0;
+        weights[(size_t)q * s->topn + e] = ok ? (*res)[e].weight : 0.0;
+      }
+    }
+  };
+  if (each) {
+    for (int q = 0; q < n; ++q) owned(q, q + 1);
+  } else if (n > 0) {
+    owned(0, n);
+  }
+  return 0;
+}
+
+// merge_owned(dest, src, None, remove_src, false) (src/track/store.rs:584-611) for each pair in order: fetch src, extend
+// dest by its observations and keep the newest K (Track::merge + optimize), then put src back at its position or drop
+// it.  Rejected (-1) before anything changes: dest == src, a dest or src that is not stored, and with remove_src a pair
+// naming a track an earlier pair removed.
+int ofs_merge_owned(ofs_store* s, int n, const uint64_t* dest, const uint64_t* src, int remove_src) {
+  if (n < 0) return -1;
+  std::unordered_set<uint64_t> removed;
+  for (int i = 0; i < n; ++i) {
+    if (dest[i] == src[i] || !s->pos.count(dest[i]) || !s->pos.count(src[i])) return -1;
+    if (removed.count(dest[i]) || removed.count(src[i])) return -1;
+    if (remove_src) removed.insert(src[i]);
+  }
+  for (int i = 0; i < n; ++i) {
+    const size_t at = s->pos.at(src[i]);
+    const Track t = s->tracks[at];   // fetch_tracks([src])
+    s->tracks.erase(s->tracks.begin() + (std::ptrdiff_t)at);
+    s->reindex();
+    auto& o = s->tracks[s->pos.at(dest[i])].obs;   // merge_external -> Track::merge
+    o.insert(o.end(), t.obs.begin(), t.obs.end());
+    s->keep_newest(o);
+    if (!remove_src) s->tracks.insert(s->tracks.begin() + (std::ptrdiff_t)at, t);   // add_track
+    s->reindex();
+  }
+  return 0;
+}
+
 int64_t ofs_size(ofs_store* s) { return (int64_t)s->tracks.size(); }
 
 int64_t ofs_ids(ofs_store* s, int64_t cap, uint64_t* ids) {

@@ -472,7 +472,8 @@ int64_t sb200_fstore_fetch(sb200_fstore* s, int32_t n, const uint64_t* ids, int3
 int64_t sb200_fstore_size(sb200_fstore* s);
 /* Ids of the stored tracks in store order; writes min(cap, size) and returns the size. */
 int64_t sb200_fstore_ids(sb200_fstore* s, int64_t cap, uint64_t* ids);
-/* Device times (ms) of the last search / associate / add call: distances, TopN, apply (0 for a stage that did not run). */
+/* Device times (ms) of the last search / associate / add / search_owned / merge_owned call: distances, TopN, apply (0 for
+ * a stage that did not run).  search_owned counts its on-device row staging as distances and sums its chunks. */
 int sb200_fstore_last_stage_ms(sb200_fstore* s, float* out3);
 
 /* Element type (SB200_FEATURE_F32 | _F16 | _BF16) of the `features` argument of every later sb200_fstore_add / _search /
@@ -507,6 +508,35 @@ int sb200_fstore_associate_device(sb200_fstore* s, int32_t n_queries, const uint
                                   const int32_t* obs_offsets, const void* d_features, int32_t* counts,
                                   uint64_t* winners, double* weights, uint64_t* track_ids, uint8_t* merged,
                                   void* cuda_stream);
+
+/* TrackStore::owned_track_distances (src/track/store.rs:471-486) + TopNVoting::winners: the queries are STORED tracks,
+ * each with its stored observations, oldest first, as its observation list.  Outputs as for sb200_fstore_search.  The
+ * store is not changed and the feature type does not matter (the rows are the stored f32 rows).
+ *   each == 0: one owned_track_distances(ids) call.  As the reference fetches every queried track first, no query is
+ *     scored against another queried track: the candidates are the store minus the queried set.  max_dist is taken over
+ *     every kept entry of the call.  The 2^30-pair bound of sb200_fstore_search applies to the whole call.
+ *   each == 1: what owned_track_distances([id]) + winners gives when called once per id, in order, on the unchanged
+ *     store: each query excludes only itself and has its own max_dist.  The library splits the call into chunks within
+ *     the pair bound, so a whole store can be searched against itself in one call (deduplication of a gallery); only a
+ *     single query whose rows x (stored tracks x max_observations) exceed 2^30 is SB200_ERR_CAPACITY.
+ * An id that is not stored gets count 0 (fetch_tracks skips it).  SB200_ERR_INVALID for an id twice in the call or
+ * `each` outside {0, 1}.  Every stored track keeps its store position (the reference's fetch_tracks + add_track moves it
+ * within a HashMap, which has no order); ties go to the lower store position, as for search. */
+int sb200_fstore_search_owned(sb200_fstore* s, int32_t n, const uint64_t* ids, int32_t each, int32_t* counts,
+                              uint64_t* winners, double* weights);
+/* TrackStore::merge_owned(dest, src, None, remove_src, false) (src/track/store.rs:584-611) for each pair (dest_ids[i],
+ * src_ids[i]) in order, each pair seeing the state the earlier ones left: dest's observations are extended by src's
+ * current ones and the newest K kept (Track::merge, src/track.rs:522-588, with the bench's optimize).  Chains (A<-B then
+ * C<-A: C receives A's rows after A absorbed B) and stars (many sources into one destination) are allowed.  remove_src
+ * takes every source out of the store, a stable compaction as sb200_fstore_fetch with remove.  After the call the store
+ * (its blob, byte for byte) is that of the sequential emulation fetch([src]), add([dest] * n, rows), then fetch([src],
+ * remove) when remove_src.  SB200_ERR_INVALID, before anything changes, for dest == src (the reference's TrackNotFound:
+ * it fetched src first), a dest or src that is not stored, and, with remove_src, a pair that names a track an earlier
+ * pair removed; the reference would apply the pairs in front and then return the error, the same deviation as
+ * sb200_fstore_associate's.  `classes` and `merge_history` have no counterpart: there is one feature class and no
+ * history.  sb200_fstore_last_stage_ms reports the row moves as the apply stage. */
+int sb200_fstore_merge_owned(sb200_fstore* s, int32_t n, const uint64_t* dest_ids, const uint64_t* src_ids,
+                             int32_t remove_src);
 
 /* ---- the store blob ----
  * The whole store as one relocatable block of bytes: this header, then four sections at 256-byte aligned offsets, gaps

@@ -134,7 +134,8 @@ EXPORTS = [
     "sb200_fstore_destroy", "sb200_fstore_add", "sb200_fstore_search", "sb200_fstore_associate", "sb200_fstore_fetch",
     "sb200_fstore_size", "sb200_fstore_ids", "sb200_fstore_last_stage_ms", "sb200_fstore_set_feature_type",
     "sb200_fstore_get_options", "sb200_fstore_add_device", "sb200_fstore_search_device",
-    "sb200_fstore_associate_device", "sb200_fstore_save", "sb200_fstore_load",
+    "sb200_fstore_associate_device", "sb200_fstore_save", "sb200_fstore_load", "sb200_fstore_search_owned",
+    "sb200_fstore_merge_owned",
 ]
 
 
@@ -232,6 +233,8 @@ def lib():
         "sb200_fstore_associate_device": (C.c_int, [vp, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
         "sb200_fstore_save": (C.c_int, [vp, vp, u64, C.POINTER(u64)]),
         "sb200_fstore_load": (C.c_int, [vp, u64, i32, C.POINTER(vp)]),
+        "sb200_fstore_search_owned": (C.c_int, [vp, i32, vp, i32, vp, vp, vp]),
+        "sb200_fstore_merge_owned": (C.c_int, [vp, i32, vp, vp, i32]),
         "sb200_host_alloc": (vp, [C.c_size_t]),
         "sb200_host_free": (None, [vp]),
     }

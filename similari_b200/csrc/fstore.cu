@@ -4,7 +4,9 @@
 // and downloads its results once.  Everything a call can reject is checked before anything is launched or changed.
 // The request rows reach the device in one of two ways: an f32 host column is staged row by row in the pinned buffer; a
 // 2-byte host column (uploaded raw) and a device column (read in place) go through fs_stage_kernel.  The store blob
-// (sb200_fstore_save / _load) shares the trackers' copy machinery (sb_blob.cuh).
+// (sb200_fstore_save / _load) shares the trackers' copy machinery (sb_blob.cuh).  The owned calls (search_owned,
+// merge_owned) take stored tracks: their rows never leave the device, and the host reads back only the counts and ring
+// starts of the tracks they touch.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -29,18 +31,25 @@ size_t align16(size_t v) { return (v + 15) & ~size_t(15); }
 
 // byte offsets of one request in the staging buffer (the device copy has the same layout)
 struct ReqLayout {
-  size_t rows, qid, qoff, row_q, dest, maxkey, row_src, total;
-  // with_src: the request carries the row-index table of fs_stage_kernel instead of host-staged rows
-  ReqLayout(int Q, int R, int d8, bool with_src) {
+  size_t rows, qid, qoff, row_q, dest, maxkey, row_src, qpos, excl, total;
+  // with_src: the request carries the row-index table of fs_stage_kernel instead of host-staged rows.  An owned search
+  // (owned_live >= 0) carries nkey max_dist keys (one per query in the each mode), the store position of each query and
+  // an exclusion byte per stored track (owned_live of them; 0 in the each mode).
+  ReqLayout(int Q, int R, int d8, bool with_src, int nkey = 1, long long owned_live = -1) {
     size_t o = 0;
     rows = o; o = align16(o + (size_t)R * d8 * 4);
     qid = o; o = align16(o + (size_t)Q * 8);
     qoff = o; o = align16(o + (size_t)(Q + 1) * 4);
     row_q = o; o = align16(o + (size_t)R * 4);
     dest = o; o = align16(o + (size_t)Q * 4);
-    maxkey = o; o = align16(o + 4);
+    maxkey = o; o = align16(o + (size_t)nkey * 4);
     row_src = o;
     if (with_src) o = align16(o + (size_t)R * 4);
+    qpos = excl = o;
+    if (owned_live >= 0) {
+      o = align16(o + (size_t)Q * 4);
+      excl = o; o = align16(o + (size_t)owned_live);
+    }
     total = o;
   }
 };
@@ -412,29 +421,254 @@ struct sb200_fstore {
       for (int b = 0; b < K; ++b)
         memcpy(feats + ((size_t)i * K + b) * D, h + ((size_t)i * K + b) * d8, (size_t)D * 4);
     }
-    if (remove && found) {
-      std::vector<int> from;
-      from.reserve(hid.size());
-      for (size_t p = 0; p < hid.size(); ++p)
-        if (!gone[p]) from.push_back((int)p);
-      DBuf f, c, st_, i, r;
-      if (int rc = alloc_columns(cap, &f, &c, &st_, &i, &r)) return rc;
-      if (int rc = gpos.ensure(std::max<size_t>(from.size(), 1) * 4)) return rc;
-      CU(cudaMemcpyAsync(gpos.p, from.data(), from.size() * 4, cudaMemcpyHostToDevice, st));
-      sb::FsStore d = s;
-      d.feat = f.as<float>(); d.cnt = c.as<int>(); d.start = st_.as<int>(); d.ids = i.as<unsigned long long>();
-      sb::fs_launch_compact(s, d, gpos.as<int>(), (int)from.size(), st);
-      CU(cudaStreamSynchronize(st));
-      CU(cudaGetLastError());
-      feat = std::move(f); cnt = std::move(c); start = std::move(st_); ids = std::move(i); run = std::move(r);
-      std::vector<uint64_t> kept;
-      kept.reserve(from.size());
-      for (int p : from) kept.push_back(hid[p]);
-      hid.swap(kept);
-      hpos.clear();
-      for (size_t p = 0; p < hid.size(); ++p) hpos[hid[p]] = (int)p;
-    }
+    if (remove && found)
+      if (int rc = remove_marked(gone)) return rc;
     return found;
+  }
+
+  // takes the tracks with gone[p] out of the store: a stable compaction into fresh columns
+  int remove_marked(const std::vector<char>& gone) {
+    std::vector<int> from;
+    from.reserve(hid.size());
+    for (size_t p = 0; p < hid.size(); ++p)
+      if (!gone[p]) from.push_back((int)p);
+    DBuf f, c, st_, i, r;
+    if (int rc = alloc_columns(cap, &f, &c, &st_, &i, &r)) return rc;
+    if (int rc = gpos.ensure(std::max<size_t>(from.size(), 1) * 4)) return rc;
+    CU(cudaMemcpyAsync(gpos.p, from.data(), from.size() * 4, cudaMemcpyHostToDevice, st));
+    const sb::FsStore s = view();
+    sb::FsStore d = s;
+    d.feat = f.as<float>(); d.cnt = c.as<int>(); d.start = st_.as<int>(); d.ids = i.as<unsigned long long>();
+    sb::fs_launch_compact(s, d, gpos.as<int>(), (int)from.size(), st);
+    CU(cudaStreamSynchronize(st));
+    CU(cudaGetLastError());
+    feat = std::move(f); cnt = std::move(c); start = std::move(st_); ids = std::move(i); run = std::move(r);
+    std::vector<uint64_t> kept;
+    kept.reserve(from.size());
+    for (int p : from) kept.push_back(hid[p]);
+    hid.swap(kept);
+    hpos.clear();
+    for (size_t p = 0; p < hid.size(); ++p) hpos[hid[p]] = (int)p;
+    return 0;
+  }
+
+  // ---- owned calls: the queries / pairs are stored tracks
+  // ring state of the stored tracks at pos[]: ring[2 i] = cnt, ring[2 i + 1] = start.  The host keeps neither, so an
+  // owned call reads those of the tracks it touches back once, before it checks what depends on them.  Changes nothing.
+  int peek(const std::vector<int>& pos, std::vector<int>* ring) {
+    const size_t n = pos.size();
+    ring->assign(n * 2, 0);
+    if (n == 0) return 0;
+    if (int rc = gpos.ensure(n * 4)) return rc;
+    if (int rc = gout.ensure(n * 8)) return rc;
+    CU(cudaMemcpyAsync(gpos.p, pos.data(), n * 4, cudaMemcpyHostToDevice, st));
+    sb::fs_launch_peek(view(), gpos.as<int>(), (int)n, gout.as<int>(), st);
+    CU(cudaMemcpyAsync(ring->data(), gout.p, n * 8, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    CU(cudaGetLastError());
+    return 0;
+  }
+
+  // owned_track_distances + TopNVoting::winners.  each == 0: one group, whose members are not candidates of each other
+  // and share one max_dist; each == 1: every query on its own (excluding only itself, its own max_dist), in chunks that
+  // respect the pair bound.
+  int search_owned(int n, const uint64_t* qids, int each, int32_t* counts, uint64_t* winners, double* weights) {
+    if (n < 0) return fail(SB200_ERR_INVALID, "n < 0");
+    if (each != 0 && each != 1) return fail(SB200_ERR_INVALID, "each must be 0 or 1");
+    if (n > 0 && (!qids || !counts || !winners || !weights)) return fail(SB200_ERR_INVALID, "ids or an output is NULL");
+    std::unordered_set<uint64_t> seen;
+    seen.reserve((size_t)n * 2);
+    for (int q = 0; q < n; ++q)
+      if (!seen.insert(qids[q]).second)
+        return fail(SB200_ERR_INVALID, "id %llu appears twice in the call", (unsigned long long)qids[q]);
+    if (int rc = begin()) return rc;
+    if (n == 0) return 0;
+    const int topn = o.topn, K = o.max_observations;
+    const long long live = (long long)hid.size(), S = live * K;
+    std::vector<int> qpos(n, -1), found;
+    for (int q = 0; q < n; ++q) {
+      auto it = hpos.find(qids[q]);
+      if (it != hpos.end()) { qpos[q] = it->second; found.push_back(it->second); }
+    }
+    std::vector<int> ring;
+    if (int rc = peek(found, &ring)) return rc;
+    std::vector<int> qcnt(n, 0);   // rows of each query: its stored observations (0 when it is not stored)
+    for (int q = 0, f = 0; q < n; ++q)
+      if (qpos[q] >= 0) qcnt[q] = ring[2 * f++];
+    // chunks [chunk[i], chunk[i + 1]) of queries, each within the pair bound of one distance matrix
+    std::vector<int> chunk(1, 0);
+    long long rows = 0;
+    for (int q = 0; q < n; ++q) {
+      if ((long long)qcnt[q] * S > sb::kFsMaxPairs)
+        return fail(SB200_ERR_CAPACITY, "query %d needs %lld observation pairs; one query holds at most 2^30", q,
+                    (long long)qcnt[q] * S);
+      if (each && (rows + qcnt[q]) * S > sb::kFsMaxPairs) { chunk.push_back(q); rows = 0; }
+      rows += qcnt[q];
+    }
+    chunk.push_back(n);
+    if (!each && rows * S > sb::kFsMaxPairs)
+      return fail(SB200_ERR_CAPACITY, "the call needs %lld observation pairs; one call holds at most 2^30", rows * S);
+    std::fill(counts, counts + n, 0);
+    std::fill(winners, winners + (size_t)n * topn, 0);
+    std::fill(weights, weights + (size_t)n * topn, 0.0);
+    if (found.empty()) return 0;
+    std::vector<unsigned char> excl;
+    if (!each) {
+      excl.assign((size_t)live, 0);
+      for (int p : found) excl[p] = 1;
+    }
+    for (size_t i = 0; i + 1 < chunk.size(); ++i)
+      if (int rc = owned_chunk(chunk[i], chunk[i + 1], qids, qpos, qcnt, excl, each, counts, winners, weights))
+        return rc;
+    return 0;
+  }
+
+  // queries [a, b) of an owned search: request rows staged on the device, distances, TopN, results into the outputs
+  int owned_chunk(int a, int b, const uint64_t* qids, const std::vector<int>& qpos, const std::vector<int>& qcnt,
+                  const std::vector<unsigned char>& excl, int each, int32_t* counts, uint64_t* winners,
+                  double* weights) {
+    const int Q = b - a, topn = o.topn, K = o.max_observations;
+    const long long live = (long long)hid.size(), S = live * K;
+    std::vector<int> qoff(Q + 1, 0);
+    for (int q = 0; q < Q; ++q) qoff[q + 1] = qoff[q] + qcnt[a + q];
+    const int R = qoff[Q];
+    if (R == 0) return 0;
+    const int nkey = each ? Q : 1;
+    const ReqLayout L(Q, R, d8, false, nkey, (long long)excl.size());
+    const ResLayout RL(Q, topn);
+    if (int rc = hreq.ensure(L.total - L.qid)) return rc;
+    if (int rc = dreq.ensure(L.total)) return rc;
+    if (int rc = hres.ensure(RL.total)) return rc;
+    if (int rc = dres.ensure(RL.total)) return rc;
+    if (o.metric == SB200_VIS_COSINE) {
+      if (int rc = qnorm.ensure((size_t)R * 4)) return rc;
+      if (int rc = snorm.ensure((size_t)S * 4)) return rc;
+    }
+    if (int rc = dist.ensure((size_t)R * S * 4)) return rc;
+    auto at = [&](size_t off) { return static_cast<char*>(hreq.p) + (off - L.qid); };   // rows are written on the device
+    memcpy(at(L.qid), qids + a, (size_t)Q * 8);
+    memcpy(at(L.qoff), qoff.data(), (size_t)(Q + 1) * 4);
+    int* row_q = reinterpret_cast<int*>(at(L.row_q));
+    for (int q = 0; q < Q; ++q)
+      for (int r = qoff[q]; r < qoff[q + 1]; ++r) row_q[r] = q;
+    std::fill_n(reinterpret_cast<int*>(at(L.dest)), Q, -1);
+    std::fill_n(reinterpret_cast<int*>(at(L.maxkey)), nkey, sb::fs_key(-1.0f));   // max_dist starts at -1.0 (topn.rs:78)
+    int* qp = reinterpret_cast<int*>(at(L.qpos));
+    for (int q = 0; q < Q; ++q) qp[q] = std::max(qpos[a + q], 0);   // a query that is not stored has no rows
+    if (!excl.empty()) memcpy(at(L.excl), excl.data(), excl.size());
+    CU(cudaMemcpyAsync(dreq.as<char>() + L.qid, hreq.p, L.total - L.qid, cudaMemcpyHostToDevice, st));
+    const sb::FsStore s = view();
+    const sb::FsCall c = call_view(L, Q, R, &RL);
+    const int mode = each ? sb::kFsOwnedEach : sb::kFsOwnedGroup;
+    CU(cudaEventRecord(ev[0], st));
+    sb::fs_launch_owned_stage(s, c, reinterpret_cast<const int*>(dreq.as<char>() + L.qpos),
+                              reinterpret_cast<float*>(dreq.as<char>() + L.rows), st);
+    sb::fs_launch_dist(o.metric, o.distance_filter, s, c, st, mode,
+                       reinterpret_cast<const unsigned char*>(dreq.as<char>() + L.excl));
+    CU(cudaEventRecord(ev[1], st));
+    sb::fs_launch_topn(o.max_distance, o.min_votes, topn, false, s, c, st, mode);
+    CU(cudaEventRecord(ev[2], st));
+    CU(cudaMemcpyAsync(hres.p, dres.p, RL.total, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    CU(cudaGetLastError());
+    float ms = 0.0f;
+    CU(cudaEventElapsedTime(&ms, ev[0], ev[1]));
+    stage_ms[0] += ms;
+    CU(cudaEventElapsedTime(&ms, ev[1], ev[2]));
+    stage_ms[1] += ms;
+    const char* h = static_cast<const char*>(hres.p);
+    const double* w = reinterpret_cast<const double*>(h + RL.w);
+    const int* cn = reinterpret_cast<const int*>(h + RL.cnt);
+    const int* ps = reinterpret_cast<const int*>(h + RL.pos);
+    for (int q = 0; q < Q; ++q) {
+      counts[a + q] = cn[q];
+      for (int e = 0; e < cn[q]; ++e) {
+        winners[(size_t)(a + q) * topn + e] = hid[ps[(size_t)q * topn + e]];
+        weights[(size_t)(a + q) * topn + e] = w[(size_t)q * topn + e];
+      }
+    }
+    return 0;
+  }
+
+  // merge_owned for the pairs in order, each seeing the state the earlier ones left.  The final ring of every touched
+  // destination is planned on the host as references to pre-call slots (the slots the sequential fetch + add emulation
+  // leaves filled, with its ring starts); the rows that move are gathered into scratch and then scattered, so a chain
+  // never reads a row already overwritten.
+  int merge_owned(int n, const uint64_t* dids, const uint64_t* sids, int remove) {
+    if (n < 0) return fail(SB200_ERR_INVALID, "n < 0");
+    if (n > 0 && (!dids || !sids)) return fail(SB200_ERR_INVALID, "dest_ids / src_ids is NULL");
+    std::vector<int> dp(n), sp(n);
+    std::vector<char> gone(hid.size(), 0);
+    for (int i = 0; i < n; ++i) {
+      auto d = hpos.find(dids[i]), s = hpos.find(sids[i]);
+      if (d == hpos.end()) return fail(SB200_ERR_INVALID, "pair %d: dest %llu is not stored", i, (unsigned long long)dids[i]);
+      if (s == hpos.end()) return fail(SB200_ERR_INVALID, "pair %d: src %llu is not stored", i, (unsigned long long)sids[i]);
+      if (d->second == s->second)
+        return fail(SB200_ERR_INVALID, "pair %d: dest and src are the same track %llu", i, (unsigned long long)dids[i]);
+      if (gone[d->second] || gone[s->second])
+        return fail(SB200_ERR_INVALID, "pair %d names a track an earlier pair removed", i);
+      dp[i] = d->second;
+      sp[i] = s->second;
+      if (remove) gone[s->second] = 1;
+    }
+    if (int rc = begin()) return rc;
+    if (n == 0) return 0;
+    const int K = o.max_observations;
+    std::unordered_map<int, int> idx;   // store position -> touched track
+    std::vector<int> touched;
+    for (int i = 0; i < n; ++i)
+      for (int p : {dp[i], sp[i]})
+        if (idx.emplace(p, (int)touched.size()).second) touched.push_back(p);
+    std::vector<int> ring;
+    if (int rc = peek(touched, &ring)) return rc;
+    // per touched track: its rows oldest first as stored row indices (position * K + slot) of the pre-call store, and
+    // how many rows its ring has taken since the call began (old ones included): virtual row v sits in slot (s0 + v) % K
+    struct Plan { std::vector<int> rows; long long taken; bool dirty; };
+    std::vector<Plan> pl(touched.size());
+    for (size_t t = 0; t < touched.size(); ++t) {
+      const int p = touched[t], c0 = ring[2 * t], s0 = ring[2 * t + 1];
+      for (int j = 0; j < c0; ++j) pl[t].rows.push_back(p * K + (s0 + j) % K);
+      pl[t].taken = c0;
+      pl[t].dirty = false;
+    }
+    for (int i = 0; i < n; ++i) {
+      Plan& d = pl[idx[dp[i]]];
+      const Plan& s = pl[idx[sp[i]]];
+      d.rows.insert(d.rows.end(), s.rows.begin(), s.rows.end());
+      d.taken += (long long)s.rows.size();
+      if ((int)d.rows.size() > K) d.rows.erase(d.rows.begin(), d.rows.end() - K);   // keep the newest K
+      d.dirty = true;
+    }
+    std::vector<int> mv_src, mv_dst, hdr;
+    for (size_t t = 0; t < touched.size(); ++t) {
+      const int p = touched[t];
+      if (!pl[t].dirty || gone[p]) continue;
+      const int c1 = (int)pl[t].rows.size();
+      const int s1 = (int)((ring[2 * t + 1] + std::max<long long>(0, pl[t].taken - K)) % K);
+      hdr.insert(hdr.end(), {p, c1, s1});
+      for (int j = 0; j < c1; ++j) {
+        const int dst = p * K + (s1 + j) % K;
+        if (pl[t].rows[j] != dst) { mv_src.push_back(pl[t].rows[j]); mv_dst.push_back(dst); }
+      }
+    }
+    const int nm = (int)mv_src.size(), nh = (int)hdr.size() / 3;
+    std::vector<int> tab;
+    tab.reserve(2 * (size_t)nm + hdr.size());
+    tab.insert(tab.end(), mv_src.begin(), mv_src.end());
+    tab.insert(tab.end(), mv_dst.begin(), mv_dst.end());
+    tab.insert(tab.end(), hdr.begin(), hdr.end());
+    if (int rc = gpos.ensure(std::max<size_t>(tab.size(), 1) * 4)) return rc;
+    if (int rc = gout.ensure(std::max<size_t>((size_t)nm * d8 * 4, 16))) return rc;
+    CU(cudaMemcpyAsync(gpos.p, tab.data(), tab.size() * 4, cudaMemcpyHostToDevice, st));
+    const int* dtab = gpos.as<int>();
+    CU(cudaEventRecord(ev[2], st));
+    sb::fs_launch_move_rows(view(), dtab, dtab + nm, nm, dtab + 2 * nm, nh, gout.as<float>(), st);
+    CU(cudaEventRecord(ev[3], st));
+    CU(cudaStreamSynchronize(st));
+    CU(cudaGetLastError());
+    if (int rc = finish_timing(false, false, true)) return rc;
+    if (remove) return remove_marked(gone);
+    return 0;
   }
 
   // ---- the store blob (layout: include/similari_b200.h)
@@ -664,6 +898,18 @@ int sb200_fstore_associate_device(sb200_fstore* s, int32_t n_queries, const uint
   if (!s) return no_handle();
   return s->run_queries(n_queries, query_ids, obs_offsets, {d_features, true, static_cast<cudaStream_t>(cuda_stream)},
                         counts, winners, weights, track_ids, merged, true);
+}
+
+int sb200_fstore_search_owned(sb200_fstore* s, int32_t n, const uint64_t* ids, int32_t each, int32_t* counts,
+                              uint64_t* winners, double* weights) {
+  if (!s) return no_handle();
+  return s->search_owned(n, ids, each, counts, winners, weights);
+}
+
+int sb200_fstore_merge_owned(sb200_fstore* s, int32_t n, const uint64_t* dest_ids, const uint64_t* src_ids,
+                             int32_t remove_src) {
+  if (!s) return no_handle();
+  return s->merge_owned(n, dest_ids, src_ids, remove_src);
 }
 
 int sb200_fstore_save(sb200_fstore* s, void* buf, uint64_t cap, uint64_t* bytes) {

@@ -6,6 +6,8 @@
 //   src/track.rs:604-652, src/distance.rs:9-47) + postprocess_distances (d < distance_filter)
 //   TopNVoting::winners (src/track/voting/topn.rs:74-138)
 //   TrackStore::merge_external / add_track / add (src/track/store.rs:265-277, 510-580, 625-691)
+//   TrackStore::owned_track_distances / merge_owned (src/track/store.rs:471-486, 584-611): the owned stage, the
+//   distance / TopN instances of the owned modes and the two-launch row move
 // Every value that reaches the voting stage is the oracle's f32 bit for bit: --fmad=false, 8-lane blocks reduced by
 // reduce_add8 and accumulated one after another, then sqrt (euclidean) or the quotient by sqrt(|a|^2 |b|^2) (cosine).
 #include <climits>
@@ -57,8 +59,11 @@ constexpr int kDT = 64;
 constexpr int kDC = 4;
 constexpr int kDP = kDC * 8 + 4;
 
-template <int METRIC>
-__global__ void __launch_bounds__(256) fs_dist_kernel(FsStore s, FsCall c, float filter, int tiles_s) {
+// MODE (kFsForeign / kFsOwnedGroup / kFsOwnedEach) changes the epilogue only: the group mode drops every entry of a
+// queried track (excl), the each mode folds max_dist per query (per row across its 16 threads, then one atomicMax per row).
+template <int METRIC, int MODE>
+__global__ void __launch_bounds__(256) fs_dist_kernel(FsStore s, FsCall c, float filter, int tiles_s,
+                                                      const unsigned char* __restrict__ excl) {
   __shared__ __align__(16) float sa[kDT][kDP];
   __shared__ __align__(16) float sbm[kDT][kDP];
   __shared__ int s_max[8];
@@ -121,13 +126,15 @@ __global__ void __launch_bounds__(256) fs_dist_kernel(FsStore s, FsCall c, float
 
   // epilogue: the metric, postprocess_distances (d < filter), the same-id skip and empty ring slots -> NaN
   int kmax = INT_MIN;
+  int rmax[4] = {INT_MIN, INT_MIN, INT_MIN, INT_MIN};   // kFsOwnedEach: per row
   const float nan = __int_as_float(0x7fc00000);
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
     const int col = c0 + tx + 16 * j;
     if (col >= S) continue;
     const int t = col / s.K, slot = col - t * s.K;
-    const bool filled = ((slot - s.start[t] + s.K) % s.K) < s.cnt[t];
+    bool filled = ((slot - s.start[t] + s.K) % s.K) < s.cnt[t];
+    if (MODE == kFsOwnedGroup) filled = filled && !excl[t];
     const unsigned long long tid_ = s.ids[t];
     const float sn = METRIC == 1 ? c.snorm[col] : 0.0f;
 #pragma unroll
@@ -139,8 +146,24 @@ __global__ void __launch_bounds__(256) fs_dist_kernel(FsStore s, FsCall c, float
       else d = 1.0f - acc[i][j] / sqrtf(c.qnorm[row] * sn);
       const bool keep = filled && c.qid[c.row_q[row]] != tid_ && d < filter;
       c.dist[(size_t)row * S + col] = keep ? d : nan;
-      if (keep) kmax = max(kmax, fs_key(d));
+      if (MODE == kFsOwnedEach) {
+        if (keep) rmax[i] = max(rmax[i], fs_key(d));
+      } else {
+        if (keep) kmax = max(kmax, fs_key(d));
+      }
     }
+  }
+  if constexpr (MODE == kFsOwnedEach) {
+    // a row's 16 threads (tx) are one half of a warp
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      int m = rmax[i];
+#pragma unroll
+      for (int off = 8; off > 0; off >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, off));
+      const int row = r0 + ty + 16 * i;
+      if (tx == 0 && row < c.R && m != INT_MIN) atomicMax(c.maxkey + c.row_q[row], m);
+    }
+    return;
   }
   kmax = __reduce_max_sync(0xffffffffu, kmax);
   if ((tid & 31) == 0) s_max[tid >> 5] = kmax;
@@ -163,13 +186,15 @@ __device__ __forceinline__ bool fs_better(double wa, int pa, double wb, int pb) 
   return wa > wb || (wa == wb && pa < pb);
 }
 
+// PERQ: max_dist is the query's own (maxkey[q], kFsOwnedEach), else the call's (maxkey[0])
+template <int PERQ>
 __global__ void __launch_bounds__(kTopnThreads) fs_topn_kernel(FsStore s, FsCall c, float max_distance, int min_votes,
                                                                 int topn, int want_dest) {
   __shared__ double l_w[kFsMaxTopn], n_w[kFsMaxTopn], b_w[kTopnThreads];
   __shared__ int l_p[kFsMaxTopn], n_p[kFsMaxTopn], b_p[kTopnThreads];
   __shared__ int s_nb;
   const int q = blockIdx.x, tid = threadIdx.x;
-  const float maxd = fs_unkey(*c.maxkey);
+  const float maxd = fs_unkey(PERQ ? c.maxkey[q] : *c.maxkey);
   const unsigned long long qid = c.qid[q];
   const int a0 = c.qoff[q], na = c.qoff[q + 1] - a0;
   const int K = s.K;
@@ -345,6 +370,51 @@ __global__ void fs_compact_kernel(FsStore src, FsStore dst, const int* from) {
   }
 }
 
+// ------------------------------------------------------------------------------------------------ owned calls
+// search_owned: one thread per float4 of a request row; row r is observation r - qoff[q] (oldest first) of the
+// stored track at qpos[q], q = row_q[r].  No staging goes through the host.
+__global__ void __launch_bounds__(256) fs_owned_stage_kernel(FsStore s, FsCall c, const int* __restrict__ qpos,
+                                                             float* __restrict__ rows) {
+  const int w4 = s.d8 / 4;
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (long long)c.R * w4) return;
+  const int r = (int)(i / w4), e = (int)(i - (long long)r * w4);
+  const int q = c.row_q[r], p = qpos[q];
+  const int slot = (s.start[p] + (r - c.qoff[q])) % s.K;
+  reinterpret_cast<float4*>(rows + (size_t)r * s.d8)[e] =
+      reinterpret_cast<const float4*>(s.feat + ((size_t)p * s.K + slot) * s.d8)[e];
+}
+
+__global__ void fs_peek_kernel(FsStore s, const int* __restrict__ pos, int n, int* __restrict__ out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  out[2 * i] = s.cnt[pos[i]];
+  out[2 * i + 1] = s.start[pos[i]];
+}
+
+// merge_owned in two launches whatever the chain structure: every moving row is read from its pre-call slot into
+// scratch first, then written to its final slot, so no row is read after it has been overwritten.  One CTA per row.
+__global__ void fs_move_gather_kernel(FsStore s, const int* __restrict__ src, float* __restrict__ scratch) {
+  const int m = blockIdx.x, w4 = s.d8 / 4;
+  const float4* a = reinterpret_cast<const float4*>(s.feat + (size_t)src[m] * s.d8);
+  float4* b = reinterpret_cast<float4*>(scratch + (size_t)m * s.d8);
+  for (int e = threadIdx.x; e < w4; e += blockDim.x) b[e] = a[e];
+}
+
+__global__ void fs_move_scatter_kernel(FsStore s, const int* __restrict__ dst, int n_moves, const int* __restrict__ hdr,
+                                       int n_hdr, const float* __restrict__ scratch) {
+  const int m = blockIdx.x, w4 = s.d8 / 4;
+  if (m < n_moves) {
+    const float4* a = reinterpret_cast<const float4*>(scratch + (size_t)m * s.d8);
+    float4* b = reinterpret_cast<float4*>(s.feat + (size_t)dst[m] * s.d8);
+    for (int e = threadIdx.x; e < w4; e += blockDim.x) b[e] = a[e];
+  }
+  if (m < n_hdr && threadIdx.x == 0) {
+    s.cnt[hdr[3 * m]] = hdr[3 * m + 1];
+    s.start[hdr[3 * m]] = hdr[3 * m + 2];
+  }
+}
+
 // ------------------------------------------------------------------------------------------------ request rows
 // Builds FsCall::rows from a feature column that is on the device already (the caller's, or the uploaded raw rows of a
 // 2-byte host column): one thread per 8-lane block of a request row.  Widening is exact and done from the bits (sb_engine.cuh),
@@ -405,7 +475,15 @@ __global__ void fs_blob_scrub_kernel(float* feat, const int* __restrict__ cnt, c
 
 }  // namespace
 
-void fs_launch_dist(int metric, float filter, const FsStore& s, const FsCall& c, cudaStream_t st) {
+template <int MODE>
+void fs_dist_grid(int metric, float filter, const FsStore& s, const FsCall& c, int tiles_s, unsigned grid,
+                  const unsigned char* excl, cudaStream_t st) {
+  if (metric == 0) fs_dist_kernel<0, MODE><<<grid, 256, 0, st>>>(s, c, filter, tiles_s, excl);
+  else fs_dist_kernel<1, MODE><<<grid, 256, 0, st>>>(s, c, filter, tiles_s, excl);
+}
+
+void fs_launch_dist(int metric, float filter, const FsStore& s, const FsCall& c, cudaStream_t st, int mode,
+                    const unsigned char* excl) {
   const long long S = (long long)s.live * s.K;
   if (c.R == 0 || S == 0) return;
   if (metric == 1) {
@@ -415,16 +493,45 @@ void fs_launch_dist(int metric, float filter, const FsStore& s, const FsCall& c,
   }
   const int tiles_s = (int)((S + kDT - 1) / kDT), tiles_r = (c.R + kDT - 1) / kDT;
   const unsigned grid = (unsigned)((long long)tiles_s * tiles_r);
-  if (metric == 0) fs_dist_kernel<0><<<grid, 256, 0, st>>>(s, c, filter, tiles_s);
-  else fs_dist_kernel<1><<<grid, 256, 0, st>>>(s, c, filter, tiles_s);
+  if (mode == kFsOwnedGroup) fs_dist_grid<kFsOwnedGroup>(metric, filter, s, c, tiles_s, grid, excl, st);
+  else if (mode == kFsOwnedEach) fs_dist_grid<kFsOwnedEach>(metric, filter, s, c, tiles_s, grid, excl, st);
+  else fs_dist_grid<kFsForeign>(metric, filter, s, c, tiles_s, grid, excl, st);
   note_launch();
 }
 
 void fs_launch_topn(float max_distance, int min_votes, int topn, bool want_dest, const FsStore& s, const FsCall& c,
-                    cudaStream_t st) {
+                    cudaStream_t st, int mode) {
   if (c.Q == 0) return;
-  fs_topn_kernel<<<c.Q, kTopnThreads, 0, st>>>(s, c, max_distance, min_votes, topn, want_dest ? 1 : 0);
+  if (mode == kFsOwnedEach)
+    fs_topn_kernel<1><<<c.Q, kTopnThreads, 0, st>>>(s, c, max_distance, min_votes, topn, want_dest ? 1 : 0);
+  else
+    fs_topn_kernel<0><<<c.Q, kTopnThreads, 0, st>>>(s, c, max_distance, min_votes, topn, want_dest ? 1 : 0);
   note_launch();
+}
+
+void fs_launch_owned_stage(const FsStore& s, const FsCall& c, const int* qpos, float* rows, cudaStream_t st) {
+  if (c.R == 0) return;
+  const long long threads = (long long)c.R * (s.d8 / 4);
+  fs_owned_stage_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(s, c, qpos, rows);
+  note_launch();
+}
+
+void fs_launch_peek(const FsStore& s, const int* pos, int n, int* out, cudaStream_t st) {
+  if (n == 0) return;
+  fs_peek_kernel<<<(n + 255) / 256, 256, 0, st>>>(s, pos, n, out);
+  note_launch();
+}
+
+void fs_launch_move_rows(const FsStore& s, const int* src, const int* dst, int n_moves, const int* hdr, int n_hdr,
+                         float* scratch, cudaStream_t st) {
+  if (n_moves > 0) {
+    fs_move_gather_kernel<<<n_moves, 128, 0, st>>>(s, src, scratch);
+    note_launch();
+  }
+  if (std::max(n_moves, n_hdr) > 0) {
+    fs_move_scatter_kernel<<<std::max(n_moves, n_hdr), 128, 0, st>>>(s, dst, n_moves, hdr, n_hdr, scratch);
+    note_launch();
+  }
 }
 
 void fs_launch_apply(const FsStore& s, const FsCall& c, cudaStream_t st) {

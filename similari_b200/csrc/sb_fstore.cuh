@@ -47,6 +47,11 @@ struct FsCall {
   int Q, R;
 };
 
+// How an owned search (sb200_fstore_search_owned) differs from a search of foreign queries, as template parameters of
+// the distance and TopN kernels: kFsForeign is the search / associate path; kFsOwnedGroup drops the entries of the
+// tracks marked in excl[live] (the queried ones); kFsOwnedEach folds max_dist per query into maxkey[Q].
+enum { kFsForeign = 0, kFsOwnedGroup = 1, kFsOwnedEach = 2 };
+
 // order-preserving map of an f32 onto an int (negative values included); NaN never reaches it
 __host__ __device__ __forceinline__ int fs_key(float f) {
   int b;
@@ -69,9 +74,19 @@ inline void fs_row_table(int Q, const int32_t* offs, int K, std::vector<int>* ro
 
 // rows[r][0 .. d8) = column row row_src[r] widened to f32 and zero-padded from D; `type` is the column's SB200_FEATURE_*
 void fs_launch_stage(int type, const void* col, const int* row_src, int R, int D, int d8, float* rows, cudaStream_t st);
-void fs_launch_dist(int metric, float filter, const FsStore& s, const FsCall& c, cudaStream_t st);
+// rows[r][0 .. d8) = observation r - qoff[q] (oldest first) of the stored track at qpos[q], q = row_q[r]
+void fs_launch_owned_stage(const FsStore& s, const FsCall& c, const int* qpos, float* rows, cudaStream_t st);
+// mode: kFsForeign, kFsOwnedGroup (excl[live] marks the queried tracks) or kFsOwnedEach
+void fs_launch_dist(int metric, float filter, const FsStore& s, const FsCall& c, cudaStream_t st, int mode = kFsForeign,
+                    const unsigned char* excl = nullptr);
 void fs_launch_topn(float max_distance, int min_votes, int topn, bool want_dest, const FsStore& s, const FsCall& c,
-                    cudaStream_t st);
+                    cudaStream_t st, int mode = kFsForeign);
+// out[2 i] = cnt[pos[i]], out[2 i + 1] = start[pos[i]]: the ring state of the tracks an owned call touches
+void fs_launch_peek(const FsStore& s, const int* pos, int n, int* out, cudaStream_t st);
+// merge_owned: scratch[m] = stored row src[m], then stored row dst[m] = scratch[m] (rows index feat as [cap * K][d8]),
+// and cnt / start of the tracks hdr[3 j] set to hdr[3 j + 1] / hdr[3 j + 2]
+void fs_launch_move_rows(const FsStore& s, const int* src, const int* dst, int n_moves, const int* hdr, int n_hdr,
+                         float* scratch, cudaStream_t st);
 void fs_launch_apply(const FsStore& s, const FsCall& c, cudaStream_t st);
 // out[i][b][.] = observation b (oldest first) of the track at pos[i] (-1: none), out_cnt[i] its count (0 for -1)
 void fs_launch_gather(const FsStore& s, const int* pos, int n, float* out, int* out_cnt, cudaStream_t st);

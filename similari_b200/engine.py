@@ -790,6 +790,28 @@ class FeatureStore:
                                                     ptr(out["merged"]), C.c_void_p(stream or None)))
         return out
 
+    def search_owned(self, ids, each=False):
+        """sb200_fstore_search_owned: owned_track_distances + TopNVoting::winners with stored tracks as the queries, on
+        the device.  each=False: one group, whose members are not candidates of each other and share max_dist;
+        each=True: every id on its own (excluding only itself), as one call per id; a whole store may be passed.
+        Returns the search dict; an id that is not stored gets count 0."""
+        ids = np.ascontiguousarray(ids, dtype=np.uint64)
+        q = len(ids)
+        out = {"counts": np.zeros(q, np.int32), "winners": np.zeros((q, self.topn), np.uint64),
+               "weights": np.zeros((q, self.topn), np.float64)}
+        check(self._L.sb200_fstore_search_owned(self._h, q, ptr(ids), int(bool(each)), ptr(out["counts"]),
+                                                ptr(out["winners"]), ptr(out["weights"])))
+        return out
+
+    def merge_owned(self, dest_ids, src_ids, remove=True):
+        """sb200_fstore_merge_owned: for each pair in order, extend dest_ids[i] by the observations of src_ids[i] and
+        keep the newest max_observations; remove=True then takes every source out of the store."""
+        d = np.ascontiguousarray(dest_ids, dtype=np.uint64)
+        s = np.ascontiguousarray(src_ids, dtype=np.uint64)
+        if len(d) != len(s):
+            raise ValueError("dest_ids and src_ids must have the same length")
+        check(self._L.sb200_fstore_merge_owned(self._h, len(d), ptr(d), ptr(s), int(bool(remove))))
+
     def fetch(self, ids, remove=False):
         """(counts[n], features[n][max_observations][feature_dim]) of the tracks `ids`, oldest observation first (count 0:
         not stored); remove=True takes them out of the store (fetch_tracks)."""
