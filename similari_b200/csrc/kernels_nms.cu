@@ -283,31 +283,69 @@ cudaError_t stage_upload(int device, void* dst, size_t bytes, const std::functio
 
 size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
 
-// Enqueues the three launches for every set on st.  offsets (validated, total > 0) is a host array; every other pointer
-// is a device pointer.  No host synchronisation beyond the staging ring's bound.  Returns a cudaError_t.
-int nms_enqueue(int n_sets, const int* offsets, const float* boxes, const float* scores, float nms_thr, float score_thr,
-                int* keep_idx, int* keep_counts, unsigned char* keep_mask, int device, cudaStream_t st) {
-  const size_t total = (size_t)offsets[n_sets];
+// The device workspace of one call, from the set sizes alone: [sets | n_valid | tiles] (uploaded in one copy), then
+// order, sx, sy, sr, sarea, vert and every set's mask slab of n x ceil(n / 64) words.
+struct NmsWorkspace {
+  size_t total = 0;                 // boxes in the request
   int max_n = 0, max_words = 0;
-  size_t mask_words = 0, n_tiles = 0;
+  int big_set = 0;                  // the set with the largest mask slab
+  size_t n_tiles = 0, mask_words = 0;
+  size_t o_nvalid = 0, o_tiles = 0, up_bytes = 0, o_order = 0, o_f32 = 0, o_vert = 0, o_mask = 0, bytes = 0;
+};
+
+NmsWorkspace nms_workspace(int n_sets, const int* offsets) {
+  NmsWorkspace w;
+  w.total = (size_t)offsets[n_sets];
+  size_t big = 0;
   for (int s = 0; s < n_sets; ++s) {
-    const int n = offsets[s + 1] - offsets[s], w = (n + 63) / 64;
-    max_n = std::max(max_n, n);
-    max_words = std::max(max_words, w);
-    mask_words += (size_t)n * w;
-    n_tiles += (size_t)w * (w + 1) / 2;
+    const int n = offsets[s + 1] - offsets[s], nw = (n + 63) / 64;
+    w.max_n = std::max(w.max_n, n);
+    w.max_words = std::max(w.max_words, nw);
+    const size_t slab = (size_t)n * nw;
+    if (slab > big) { big = slab; w.big_set = s; }
+    w.mask_words += slab;
+    w.n_tiles += (size_t)nw * (nw + 1) / 2;
   }
-  // workspace: [sets | n_valid | tiles] (uploaded in one copy), then order, sx, sy, sr, sarea, vert, mask
-  const size_t o_nvalid = align256(sizeof(NmsSet) * n_sets);
-  const size_t o_tiles = o_nvalid + align256(sizeof(int) * n_sets);
-  const size_t up_bytes = o_tiles + sizeof(NmsTile) * n_tiles;
-  const size_t o_order = align256(up_bytes);
-  const size_t o_f32 = o_order + align256(4 * total);  // sx, sy, sr, sarea
-  const size_t o_vert = o_f32 + 4 * align256(4 * total);
-  const size_t o_mask = o_vert + align256(64 * total);
-  const size_t bytes = o_mask + 8 * mask_words;
+  w.o_nvalid = align256(sizeof(NmsSet) * n_sets);
+  w.o_tiles = w.o_nvalid + align256(sizeof(int) * n_sets);
+  w.up_bytes = w.o_tiles + sizeof(NmsTile) * w.n_tiles;
+  w.o_order = align256(w.up_bytes);
+  w.o_f32 = w.o_order + align256(4 * w.total);  // sx, sy, sr, sarea
+  w.o_vert = w.o_f32 + 4 * align256(4 * w.total);
+  w.o_mask = w.o_vert + align256(64 * w.total);
+  w.bytes = w.o_mask + 8 * w.mask_words;
+  return w;
+}
+
+// Total memory of the device, read once per device.  A fixed property, so whether a call is refused does not depend on
+// what other processes hold at the time.
+int device_total_memory(int device, size_t* bytes) {
+  static std::mutex mu;
+  static std::vector<size_t> total;
+  std::lock_guard<std::mutex> g(mu);
+  if ((int)total.size() <= device) total.resize(device + 1, 0);
+  if (!total[device]) {
+    cudaDeviceProp p;
+    cudaError_t e = cudaGetDeviceProperties(&p, device);
+    if (e != cudaSuccess) return fail(SB200_ERR_CUDA, "cudaGetDeviceProperties failed: %s", cudaGetErrorString(e));
+    total[device] = p.totalGlobalMem;
+  }
+  *bytes = total[device];
+  return 0;
+}
+
+// Enqueues the three launches for every set on st.  offsets (validated, total > 0) is a host array and lay its
+// workspace; every other pointer is a device pointer.  No host synchronisation beyond the staging ring's bound.
+// Returns a cudaError_t.
+int nms_enqueue(int n_sets, const int* offsets, const NmsWorkspace& lay, const float* boxes, const float* scores,
+                float nms_thr, float score_thr, int* keep_idx, int* keep_counts, unsigned char* keep_mask, int device,
+                cudaStream_t st) {
+  const size_t total = lay.total, n_tiles = lay.n_tiles, up_bytes = lay.up_bytes;
+  const size_t o_nvalid = lay.o_nvalid, o_tiles = lay.o_tiles, o_order = lay.o_order, o_f32 = lay.o_f32;
+  const size_t o_vert = lay.o_vert, o_mask = lay.o_mask;
+  const int max_n = lay.max_n, max_words = lay.max_words;
   unsigned char* ws = nullptr;
-  cudaError_t e = ws_alloc((void**)&ws, bytes, device, st);
+  cudaError_t e = ws_alloc((void**)&ws, lay.bytes, device, st);
   if (e != cudaSuccess) return (int)e;
 
   e = stage_upload(device, ws, up_bytes, [&](unsigned char* up) {
@@ -359,8 +397,10 @@ int nms_enqueue(int n_sets, const int* offsets, const float* boxes, const float*
   return (int)e;
 }
 
-// Checks shared by both batch entries, in the order of sb200_nms; nothing is read but `offsets`.
-int nms_check(int n_sets, const int* offsets, const float* boxes, const int* keep_idx, const int* keep_counts, int device) {
+// Checks shared by both batch entries, in the order of sb200_nms; nothing is read but `offsets`.  On success *lay is the
+// call's workspace.
+int nms_check(int n_sets, const int* offsets, const float* boxes, const int* keep_idx, const int* keep_counts, int device,
+              NmsWorkspace* lay) {
   if (n_sets < 0 || !offsets) return fail(SB200_ERR_INVALID, "nms_batch: n_sets < 0 or offsets is NULL");
   if (offsets[0] != 0) return fail(SB200_ERR_INVALID, "nms_batch: offsets[0] != 0");
   for (int s = 0; s < n_sets; ++s)
@@ -374,6 +414,15 @@ int nms_check(int n_sets, const int* offsets, const float* boxes, const int* kee
     if ((size_t)((n + 63) / 64) * 8 > kSweepBitmapBytes)
       return fail(SB200_ERR_CAPACITY, "nms: set %d has %d boxes, too many for the on-chip sweep", s, n);
   }
+  // the mask slabs grow as n^2 / 8 bytes: a set the bitmap admits can still need more memory than the device has
+  *lay = nms_workspace(n_sets, offsets);
+  size_t mem = 0;
+  if (int rc = device_total_memory(device, &mem)) return rc;
+  if (lay->bytes > mem) {
+    const int s = lay->big_set, n = offsets[s + 1] - offsets[s];
+    return fail(SB200_ERR_CAPACITY, "nms: set %d has %d boxes; the call's workspace (%zu bytes, %zu of them the mask of "
+                "that set) exceeds the device's %zu bytes", s, n, lay->bytes, (size_t)n * ((n + 63) / 64) * 8, mem);
+  }
   return 0;
 }
 
@@ -384,7 +433,8 @@ extern "C" int sb200_nms_batch_device(int32_t n_sets, const int32_t* offsets, co
                                       float nms_threshold, float score_threshold, int32_t has_score_threshold,
                                       int32_t* keep_idx, int32_t* keep_counts, uint8_t* keep_mask, int32_t device,
                                       void* cuda_stream) {
-  int rc = sb::nms_check(n_sets, offsets, boxes, keep_idx, keep_counts, device);
+  sb::NmsWorkspace lay;
+  int rc = sb::nms_check(n_sets, offsets, boxes, keep_idx, keep_counts, device, &lay);
   if (rc) return rc;
   CU(cudaSetDevice(device));
   cudaStream_t st = (cudaStream_t)cuda_stream;
@@ -393,7 +443,7 @@ extern "C" int sb200_nms_batch_device(int32_t n_sets, const int32_t* offsets, co
     if (n_sets > 0) e = cudaMemsetAsync(keep_counts, 0, 4 * (size_t)n_sets, st);
   } else {
     const float sthr = has_score_threshold ? score_threshold : -3.402823466e+38f;  // f32::MIN
-    e = (cudaError_t)sb::nms_enqueue(n_sets, offsets, boxes, scores, nms_threshold, sthr, keep_idx, keep_counts,
+    e = (cudaError_t)sb::nms_enqueue(n_sets, offsets, lay, boxes, scores, nms_threshold, sthr, keep_idx, keep_counts,
                                      keep_mask, device, st);
   }
   if (e != cudaSuccess) return sb::fail(SB200_ERR_CUDA, "nms: CUDA error: %s", cudaGetErrorString(e));
@@ -403,7 +453,8 @@ extern "C" int sb200_nms_batch_device(int32_t n_sets, const int32_t* offsets, co
 extern "C" int64_t sb200_nms_batch(int32_t n_sets, const int32_t* offsets, const float* boxes, const float* scores,
                                    float nms_threshold, float score_threshold, int32_t has_score_threshold,
                                    int32_t* keep_idx, int32_t* keep_counts, uint8_t* keep_mask, int32_t device) {
-  int rc = sb::nms_check(n_sets, offsets, boxes, keep_idx, keep_counts, device);
+  sb::NmsWorkspace lay;
+  int rc = sb::nms_check(n_sets, offsets, boxes, keep_idx, keep_counts, device, &lay);
   if (rc) return rc;
   const size_t total = (size_t)offsets[n_sets];
   if (total == 0) {
@@ -428,7 +479,7 @@ extern "C" int64_t sb200_nms_batch(int32_t n_sets, const int32_t* offsets, const
     if (e == cudaSuccess && ds) e = cudaMemcpyAsync(ds, scores, 4 * total, cudaMemcpyHostToDevice, st);
     const float sthr = has_score_threshold ? score_threshold : -3.402823466e+38f;  // f32::MIN
     if (e == cudaSuccess)
-      e = (cudaError_t)sb::nms_enqueue(n_sets, offsets, db, ds, nms_threshold, sthr, didx, dcnt, dkm, device, st);
+      e = (cudaError_t)sb::nms_enqueue(n_sets, offsets, lay, db, ds, nms_threshold, sthr, didx, dcnt, dkm, device, st);
     if (e == cudaSuccess) e = cudaMemcpyAsync(keep_idx, didx, 4 * total, cudaMemcpyDeviceToHost, st);
     if (e == cudaSuccess) e = cudaMemcpyAsync(keep_counts, dcnt, 4 * (size_t)n_sets, cudaMemcpyDeviceToHost, st);
     if (e == cudaSuccess && dkm) e = cudaMemcpyAsync(keep_mask, dkm, total, cudaMemcpyDeviceToHost, st);

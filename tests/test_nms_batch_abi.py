@@ -60,6 +60,18 @@ def test_missing_pointers_are_invalid(L, entry):
     assert _call(L, entry, 1, None, boxes, idx, counts) == -1
     # an empty request needs no box or index buffer
     empty = np.array([0, 0], np.int32)
+    if entry == "sb200_nms_batch_device" and L.sb200_device_count() > 0:
+        # the device entry writes its counts on the device: give it device memory
+        import torch
+
+        from similari_b200._lib import ptr
+
+        d_counts = torch.full((1,), 7, dtype=torch.int32, device="cuda")
+        torch.cuda.synchronize()
+        rc = L.sb200_nms_batch_device(1, ptr(empty), None, None, 0.5, 0.0, 0, None, d_counts.data_ptr(), None, 0, None)
+        torch.cuda.synchronize()
+        assert rc == 0 and int(d_counts[0]) == 0
+        return
     rc = _call(L, entry, 1, empty, None, None, counts)
     assert rc in (0, -2) and (rc == 0) == (L.sb200_device_count() > 0)
 
