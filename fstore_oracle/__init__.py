@@ -68,6 +68,30 @@ def _p(a):
     return a.ctypes.data_as(C.c_void_p) if a is not None else None
 
 
+def round_rows(x, storage):
+    """What a store of storage type `storage` ("f32", "f16", "bf16") holds for the f32 values `x`, widened back to f32:
+    each value rounded once to the type, to nearest with ties to even, overflow to +-inf, subnormals kept; NaN stays NaN
+    (its payload is not modelled).  Written from the formats' definitions, without numpy's or torch's casts, so that the
+    tests can check it against both."""
+    x = np.ascontiguousarray(x, dtype=np.float32)
+    if storage == "f32":
+        return x.copy()
+    nan = np.isnan(x)
+    if storage == "bf16":
+        u = x.view(np.uint32).astype(np.uint64)
+        r = ((u + 0x7FFF + ((u >> 16) & 1)) & 0xFFFF0000).astype(np.uint32).view(np.float32)
+        return np.where(nan, np.float32(np.nan), r)
+    if storage != "f16":
+        raise ValueError(f"unknown storage type {storage!r}")
+    with np.errstate(invalid="ignore", over="ignore"):
+        a = np.abs(x.astype(np.float64))   # exact
+        _, ex = np.frexp(np.where(np.isfinite(a) & (a > 0), a, 1.0))   # a = m * 2^ex, m in [0.5, 1)
+        ulp = np.ldexp(1.0, np.maximum(ex - 1, -14) - 10)              # binary16: 11 significant bits, emin = -14
+        r = np.rint(a / ulp) * ulp                                     # a / ulp is exact; rint ties to even
+        r = np.where(np.isinf(a) | (r > 65504.0), np.inf, r)
+        return np.where(nan, np.float32(np.nan), np.copysign(r, x).astype(np.float32))
+
+
 def topn_voting(topn, max_distance, min_votes, ents):
     """TopNVoting::winners.  ents: list of (from, to, distance or None).  Returns {query: [(winner, weight), ...]}."""
     fr = np.array([e[0] for e in ents], dtype=np.uint64)

@@ -480,13 +480,26 @@ int sb200_fstore_last_stage_ms(sb200_fstore* s, float* out3);
  * _associate call and of their _device forms.  The column stays [rows][feature_dim] row-major; with F16 or BF16 the
  * `const float* features` parameter carries a pointer to 2-byte elements.  Widening either type to f32 is exact, so
  * every output and every stored row is bit for bit what the same call returns for the widened f32 request.  The stored
- * rows stay f32 and sb200_fstore_fetch keeps returning f32.  A new store reads F32; a loaded store reads the type its
+ * rows are in the store's storage type (sb200_fstore_set_storage_type), which does not depend on this one: every
+ * combination works, and sb200_fstore_fetch keeps returning f32.  A new store reads F32; a loaded store reads the type its
  * blob was saved under.  SB200_ERR_INVALID for an unknown type.  No counterpart in the reference (its features are f32). */
 int sb200_fstore_set_feature_type(sb200_fstore* s, int32_t type);
 /* The options the store was created (or loaded) with, `device` included, and the element type now set.  Either output may
  * be NULL.  What a caller that loads a blob needs to size the outputs of the other calls.  No counterpart in the
  * reference. */
 int sb200_fstore_get_options(sb200_fstore* s, sb200_fstore_options* out, int32_t* feature_type);
+/* Storage type of the stored rows: SB200_FEATURE_F32 (the default), _F16 or _BF16.  A 2-byte store halves the device
+ * memory of the rows, their growth peak and the blob.  A row is stored by rounding its widened f32 value to the storage
+ * type once (__float2half_rn / __float2bfloat16_rn: to nearest, ties to even, overflow to +-inf, subnormals kept; a NaN
+ * stays some NaN, its payload unspecified).  Queries are never rounded: search and associate compare the request's f32
+ * rows with the stored rows widened to f32, the owned calls widened stored rows with widened stored rows, and
+ * sb200_fstore_fetch returns the stored values widened to f32.  So a 2-byte store fed a column of its own type returns,
+ * bit for bit, what an f32 store fed the same column returns; in general its results are those of an f32 store that
+ * holds the rounded rows.  Allowed while the store holds no tracks (also after sb200_fstore_fetch with remove emptied
+ * it); reallocates nothing.  SB200_ERR_INVALID, changing nothing, for an unknown type or a store that holds tracks.  A
+ * loaded store has the type its blob was saved under.  No counterpart in the reference (its features are f32). */
+int sb200_fstore_set_storage_type(sb200_fstore* s, int32_t type);
+int sb200_fstore_get_storage_type(sb200_fstore* s, int32_t* out);
 
 /* sb200_fstore_add / _search / _associate with `d_features` a DEVICE pointer on the store's device, in the element type
  * set by sb200_fstore_set_feature_type: the column an embedding network has just written.  ids, query_ids, obs_offsets
@@ -511,7 +524,8 @@ int sb200_fstore_associate_device(sb200_fstore* s, int32_t n_queries, const uint
 
 /* TrackStore::owned_track_distances (src/track/store.rs:471-486) + TopNVoting::winners: the queries are STORED tracks,
  * each with its stored observations, oldest first, as its observation list.  Outputs as for sb200_fstore_search.  The
- * store is not changed and the feature type does not matter (the rows are the stored f32 rows).
+ * store is not changed and the feature type does not matter (the rows are the stored rows, widened to f32 from the
+ * storage type).
  *   each == 0: one owned_track_distances(ids) call.  As the reference fetches every queried track first, no query is
  *     scored against another queried track: the candidates are the store minus the queried set.  max_dist is taken over
  *     every kept entry of the call.  The 2^30-pair bound of sb200_fstore_search applies to the whole call.
@@ -541,10 +555,14 @@ int sb200_fstore_merge_owned(sb200_fstore* s, int32_t n, const uint64_t* dest_id
 /* ---- the store blob ----
  * The whole store as one relocatable block of bytes: this header, then four sections at 256-byte aligned offsets, gaps
  * zeroed, in this order: ids[live] (u64), cnt[live] (i32 observations held), start[live] (i32 ring slot of the oldest
- * observation), feat[live][max_observations][d8] (f32 rows as stored; observation j of a track sits in ring slot
- * (start + j) % max_observations).  Ring slots a track has never filled are written as zeros, so two stores that hold
- * the same tracks in the same ring state give byte-equal blobs.  The magic differs from the tracker blob's: each loader
- * refuses the other's blob. */
+ * observation), feat[live][max_observations][d8] (rows as stored, in the storage type: 4 or 2 bytes per element;
+ * observation j of a track sits in ring slot (start + j) % max_observations).  Ring slots a track has never filled are
+ * written as zeros, so two stores that hold the same tracks in the same ring state give byte-equal blobs.  The magic
+ * differs from the tracker blob's: each loader refuses the other's blob.
+ * storage_type was a reserved 0 before 2-byte stores existed, which is SB200_FEATURE_F32: older blobs load unchanged, and
+ * an f32 store's blob is what it was.  A library from before 2-byte stores refuses a non-empty 2-byte store's blob by
+ * its feat section size (half of what an f32 store needs), so it cannot misread one; an empty 2-byte store's blob has
+ * a 0-byte feat section, and such a library loads it as an empty f32 store. */
 #define SB200_FSTORE_BLOB_MAGIC 0x53464253u /* "SBFS" */
 #define SB200_FSTORE_BLOB_VERSION 1u
 #define SB200_FSTORE_BLOB_ALIGN 256u
@@ -562,7 +580,7 @@ typedef struct {
   int32_t min_votes;
   int32_t d8;           /* feature_dim rounded up to a multiple of 8: the stored row length */
   int32_t feature_type; /* the element type set when the blob was written */
-  int32_t reserved;     /* 0 */
+  int32_t storage_type; /* the element type of the stored rows and of the feat section */
   int64_t live;         /* stored tracks */
   uint64_t sec_off[SB200_FSTORE_BLOB_SECTIONS];
   uint64_t sec_bytes[SB200_FSTORE_BLOB_SECTIONS];
@@ -576,7 +594,8 @@ int sb200_fstore_save(sb200_fstore* s, void* buf, uint64_t cap, uint64_t* bytes)
  * store returns what the saved one returns (counts, winner ids, f64 weights, track_ids, merged, fetched rows, id order,
  * size).  A damaged blob is refused with SB200_ERR_INVALID before a store exists, sb200_last_error naming the field:
  * magic, version, truncation, section bounds / order / 256-byte alignment / sizes, options outside the caps of
- * sb200_fstore_create, d8 != round_up(feature_dim, 8), an id twice, and (by one kernel over the blob, before any row is
+ * sb200_fstore_create, d8 != round_up(feature_dim, 8), an unknown feature_type or storage_type (checked before the
+ * section sizes, which depend on it), an id twice, and (by one kernel over the blob, before any row is
  * copied) a cnt outside [1, max_observations] or a start outside [0, max_observations).  A flipped feature value is not
  * detected: the blob carries no checksum.  A failed load leaves no handle and no device memory behind.  No counterpart
  * in the reference. */

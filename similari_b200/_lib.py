@@ -106,7 +106,7 @@ class FstoreBlobHeader(C.Structure):
         ("min_votes", C.c_int32),
         ("d8", C.c_int32),
         ("feature_type", C.c_int32),
-        ("reserved", C.c_int32),
+        ("storage_type", C.c_int32),
         ("live", C.c_int64),
         ("sec_off", C.c_uint64 * FSTORE_BLOB_SECTIONS),
         ("sec_bytes", C.c_uint64 * FSTORE_BLOB_SECTIONS),
@@ -135,7 +135,7 @@ EXPORTS = [
     "sb200_fstore_size", "sb200_fstore_ids", "sb200_fstore_last_stage_ms", "sb200_fstore_set_feature_type",
     "sb200_fstore_get_options", "sb200_fstore_add_device", "sb200_fstore_search_device",
     "sb200_fstore_associate_device", "sb200_fstore_save", "sb200_fstore_load", "sb200_fstore_search_owned",
-    "sb200_fstore_merge_owned",
+    "sb200_fstore_merge_owned", "sb200_fstore_set_storage_type", "sb200_fstore_get_storage_type",
 ]
 
 
@@ -235,6 +235,8 @@ def lib():
         "sb200_fstore_load": (C.c_int, [vp, u64, i32, C.POINTER(vp)]),
         "sb200_fstore_search_owned": (C.c_int, [vp, i32, vp, i32, vp, vp, vp]),
         "sb200_fstore_merge_owned": (C.c_int, [vp, i32, vp, vp, i32]),
+        "sb200_fstore_set_storage_type": (C.c_int, [vp, i32]),
+        "sb200_fstore_get_storage_type": (C.c_int, [vp, C.POINTER(i32)]),
         "sb200_host_alloc": (vp, [C.c_size_t]),
         "sb200_host_free": (None, [vp]),
     }

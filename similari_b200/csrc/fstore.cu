@@ -6,7 +6,8 @@
 // 2-byte host column (uploaded raw) and a device column (read in place) go through fs_stage_kernel.  The store blob
 // (sb200_fstore_save / _load) shares the trackers' copy machinery (sb_blob.cuh).  The owned calls (search_owned,
 // merge_owned) take stored tracks: their rows never leave the device, and the host reads back only the counts and ring
-// starts of the tracks they touch.
+// starts of the tracks they touch.  The stored rows are f32, binary16 or bfloat16 (stype, sb200_fstore_set_storage_type);
+// row_bytes() is the size of one stored row, and nothing else on the host depends on the storage type.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -76,6 +77,9 @@ constexpr uint64_t kSecAlign = SB200_FSTORE_BLOB_ALIGN;
 enum { kSecIds, kSecCnt, kSecStart, kSecFeat };
 uint64_t sec_align(uint64_t v) { return (v + kSecAlign - 1) / kSecAlign * kSecAlign; }
 
+bool known_type(int t) { return t == SB200_FEATURE_F32 || t == SB200_FEATURE_F16 || t == SB200_FEATURE_BF16; }
+size_t type_bytes(int t) { return t == SB200_FEATURE_F32 ? 4 : 2; }
+
 int check_options(const sb200_fstore_options& o) {
   if (o.metric != SB200_VIS_EUCLIDEAN && o.metric != SB200_VIS_COSINE) return fail(SB200_ERR_INVALID, "unknown metric");
   if (o.max_observations < 1 || o.max_observations > SB200_FSTORE_MAX_OBS)
@@ -93,6 +97,7 @@ struct sb200_fstore {
   sb200_fstore_options o{};
   int d8 = 8;
   int ftype = SB200_FEATURE_F32;   // element type of the calls' feature columns
+  int stype = SB200_FEATURE_F32;   // element type of the stored rows
   int num_sms = 1;
   cudaStream_t st = nullptr;
   cudaEvent_t ev[4] = {};
@@ -116,7 +121,7 @@ struct sb200_fstore {
 
   sb::FsStore view() const {
     sb::FsStore s;
-    s.feat = feat.as<float>();
+    s.feat = feat.p;
     s.cnt = cnt.as<int>();
     s.start = start.as<int>();
     s.ids = ids.as<unsigned long long>();
@@ -124,13 +129,17 @@ struct sb200_fstore {
     s.K = o.max_observations;
     s.d8 = d8;
     s.live = (int)hid.size();
+    s.stype = stype;
     return s;
   }
+
+  // bytes of one stored row (observation)
+  size_t row_bytes() const { return (size_t)d8 * type_bytes(stype); }
 
   // fresh columns for `n` tracks; the caller copies what it keeps
   int alloc_columns(size_t n, DBuf* f, DBuf* c, DBuf* s, DBuf* i, DBuf* r) {
     n = std::max<size_t>(n, 1);
-    if (int rc = f->ensure(n * o.max_observations * d8 * 4)) return rc;
+    if (int rc = f->ensure(n * o.max_observations * row_bytes())) return rc;
     if (int rc = c->ensure(n * 4)) return rc;
     if (int rc = s->ensure(n * 4)) return rc;
     if (int rc = i->ensure(n * 8)) return rc;
@@ -147,7 +156,7 @@ struct sb200_fstore {
     if (int rc = alloc_columns(nc, &f, &c, &s, &i, &r)) return rc;
     const size_t live = hid.size();
     if (live) {
-      CU(cudaMemcpyAsync(f.p, feat.p, live * o.max_observations * d8 * 4, cudaMemcpyDeviceToDevice, st));
+      CU(cudaMemcpyAsync(f.p, feat.p, live * o.max_observations * row_bytes(), cudaMemcpyDeviceToDevice, st));
       CU(cudaMemcpyAsync(c.p, cnt.p, live * 4, cudaMemcpyDeviceToDevice, st));
       CU(cudaMemcpyAsync(s.p, start.p, live * 4, cudaMemcpyDeviceToDevice, st));
       CU(cudaMemcpyAsync(i.p, ids.p, live * 8, cudaMemcpyDeviceToDevice, st));
@@ -438,7 +447,7 @@ struct sb200_fstore {
     CU(cudaMemcpyAsync(gpos.p, from.data(), from.size() * 4, cudaMemcpyHostToDevice, st));
     const sb::FsStore s = view();
     sb::FsStore d = s;
-    d.feat = f.as<float>(); d.cnt = c.as<int>(); d.start = st_.as<int>(); d.ids = i.as<unsigned long long>();
+    d.feat = f.p; d.cnt = c.as<int>(); d.start = st_.as<int>(); d.ids = i.as<unsigned long long>();
     sb::fs_launch_compact(s, d, gpos.as<int>(), (int)from.size(), st);
     CU(cudaStreamSynchronize(st));
     CU(cudaGetLastError());
@@ -658,11 +667,11 @@ struct sb200_fstore {
     tab.insert(tab.end(), mv_dst.begin(), mv_dst.end());
     tab.insert(tab.end(), hdr.begin(), hdr.end());
     if (int rc = gpos.ensure(std::max<size_t>(tab.size(), 1) * 4)) return rc;
-    if (int rc = gout.ensure(std::max<size_t>((size_t)nm * d8 * 4, 16))) return rc;
+    if (int rc = gout.ensure(std::max<size_t>((size_t)nm * row_bytes(), 16))) return rc;
     CU(cudaMemcpyAsync(gpos.p, tab.data(), tab.size() * 4, cudaMemcpyHostToDevice, st));
     const int* dtab = gpos.as<int>();
     CU(cudaEventRecord(ev[2], st));
-    sb::fs_launch_move_rows(view(), dtab, dtab + nm, nm, dtab + 2 * nm, nh, gout.as<float>(), st);
+    sb::fs_launch_move_rows(view(), dtab, dtab + nm, nm, dtab + 2 * nm, nh, gout.p, st);
     CU(cudaEventRecord(ev[3], st));
     CU(cudaStreamSynchronize(st));
     CU(cudaGetLastError());
@@ -675,7 +684,7 @@ struct sb200_fstore {
   uint64_t lay_out(BlobHeader* h) const {
     const uint64_t live = hid.size();
     const uint64_t sec[SB200_FSTORE_BLOB_SECTIONS] = {live * 8, live * 4, live * 4,
-                                                      live * o.max_observations * d8 * 4};
+                                                      live * o.max_observations * row_bytes()};
     uint64_t off = sec_align(sizeof(BlobHeader));
     for (int i = 0; i < SB200_FSTORE_BLOB_SECTIONS; ++i) {
       h->sec_off[i] = off;
@@ -707,7 +716,7 @@ struct sb200_fstore {
     h.magic = SB200_FSTORE_BLOB_MAGIC; h.version = SB200_FSTORE_BLOB_VERSION;
     h.metric = o.metric; h.distance_filter = o.distance_filter; h.max_observations = o.max_observations;
     h.feature_dim = o.feature_dim; h.topn = o.topn; h.max_distance = o.max_distance; h.min_votes = o.min_votes;
-    h.d8 = d8; h.feature_type = ftype; h.live = (int64_t)hid.size();
+    h.d8 = d8; h.feature_type = ftype; h.storage_type = stype; h.live = (int64_t)hid.size();
     const uint64_t total = h.total_bytes = lay_out(&h);
     *bytes = total;
     if (!dst) return 0;
@@ -729,8 +738,8 @@ struct sb200_fstore {
       if (i < SB200_FSTORE_BLOB_SECTIONS) end = h.sec_off[i] + h.sec_bytes[i];
     }
     if (int rc = move_columns(0, h, dblob)) return rc;
-    sb::fs_launch_blob_scrub(reinterpret_cast<float*>(dblob + h.sec_off[kSecFeat]), cnt.as<int>(), start.as<int>(),
-                             (int)h.live, o.max_observations, d8, st);
+    sb::fs_launch_blob_scrub(stype, dblob + h.sec_off[kSecFeat], cnt.as<int>(), start.as<int>(), (int)h.live,
+                             o.max_observations, d8, st);
     CU(cudaStreamSynchronize(st));
     CU(cudaGetLastError());
     if (in_place) return 0;
@@ -747,6 +756,7 @@ struct sb200_fstore {
     if (int rc = begin()) return rc;
     const int live = (int)h.live, K = o.max_observations;
     ftype = h.feature_type;
+    stype = h.storage_type;
     if (live == 0) return 0;
     if (int rc = reserve((size_t)live)) return rc;
     const int where = sb::blob_device(src);
@@ -865,9 +875,27 @@ int sb200_fstore_last_stage_ms(sb200_fstore* s, float* out3) {
 
 int sb200_fstore_set_feature_type(sb200_fstore* s, int32_t type) {
   if (!s) return no_handle();
-  if (type != SB200_FEATURE_F32 && type != SB200_FEATURE_F16 && type != SB200_FEATURE_BF16)
-    return fail(SB200_ERR_INVALID, "unknown feature type %d", type);
+  if (!known_type(type)) return fail(SB200_ERR_INVALID, "unknown feature type %d", type);
   s->ftype = type;
+  return 0;
+}
+
+int sb200_fstore_set_storage_type(sb200_fstore* s, int32_t type) {
+  if (!s) return no_handle();
+  if (!known_type(type)) return fail(SB200_ERR_INVALID, "unknown storage type %d", type);
+  if (!s->hid.empty())
+    return fail(SB200_ERR_INVALID, "the storage type is fixed while the store holds tracks (%zu)", s->hid.size());
+  s->stype = type;
+  // no track is stored, so nothing moves: the capacity is what the allocated columns hold in rows of the new type, and
+  // the next reserve allocates when it needs more
+  if (s->cap) s->cap = std::min(s->cap, s->feat.bytes / ((size_t)s->o.max_observations * s->row_bytes()));
+  return 0;
+}
+
+int sb200_fstore_get_storage_type(sb200_fstore* s, int32_t* out) {
+  if (!s) return no_handle();
+  if (!out) return fail(SB200_ERR_INVALID, "out is NULL");
+  *out = s->stype;
   return 0;
 }
 
@@ -937,13 +965,14 @@ int sb200_fstore_load(const void* buf, uint64_t bytes, int32_t device, sb200_fst
                             h.min_votes, device};
   if (int rc = check_options(o)) return rc;
   if (h.d8 != (h.feature_dim + 7) / 8 * 8) return fail(SB200_ERR_INVALID, "d8 is not feature_dim rounded up to 8");
-  if (h.feature_type != SB200_FEATURE_F32 && h.feature_type != SB200_FEATURE_F16 && h.feature_type != SB200_FEATURE_BF16)
-    return fail(SB200_ERR_INVALID, "unknown feature_type %d", h.feature_type);
+  if (!known_type(h.feature_type)) return fail(SB200_ERR_INVALID, "unknown feature_type %d", h.feature_type);
+  // before the section sizes, which depend on it
+  if (!known_type(h.storage_type)) return fail(SB200_ERR_INVALID, "unknown storage_type %d", h.storage_type);
   // live * K indexes the distance matrix's columns as an int
   if (h.live < 0 || h.live > INT32_MAX / h.max_observations) return fail(SB200_ERR_INVALID, "live count out of range");
   const uint64_t live = (uint64_t)h.live;
   const uint64_t want[SB200_FSTORE_BLOB_SECTIONS] = {live * 8, live * 4, live * 4,
-                                                     live * h.max_observations * h.d8 * 4};
+                                                     live * h.max_observations * h.d8 * type_bytes(h.storage_type)};
   static const char* const kName[SB200_FSTORE_BLOB_SECTIONS] = {"ids", "cnt", "start", "feat"};
   uint64_t end = sizeof(BlobHeader);
   for (int i = 0; i < SB200_FSTORE_BLOB_SECTIONS; ++i) {

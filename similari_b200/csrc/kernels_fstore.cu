@@ -1,5 +1,9 @@
 // kernels_fstore.cu -- the feature track store's call: distances, TopN voting, merge / append; the request rows built
 // from a typed or device-resident feature column (fs_stage_kernel); the index check and slot scrub of the store blob.
+// Every kernel that touches stored rows is a template over their element type Elem (float, __half or __nv_bfloat16,
+// FsStore::stype); its launcher picks the instance.  A 2-byte stored element is widened to f32 from its bits where it is
+// loaded, which is exact, so every stage after the load sees f32 values; fs_apply_kernel rounds a request row once when
+// it stores it.  The f32 instances are the kernels of the f32-only store.
 //
 // Replaces, for feature-only tracks (benches/feature_tracker.rs),
 //   TrackStore::foreign_track_distances -> Track::distances -> euclidean / cosine (src/track/store.rs:199-250,
@@ -21,29 +25,73 @@ namespace {
 
 __device__ __forceinline__ float fs_unkey(int k) { return __int_as_float(k >= 0 ? k : (k ^ 0x7fffffff)); }
 
+// ------------------------------------------------------------------------------------------------ stored elements
+// 16 bytes hold kPer16<Elem> stored elements, so a stored row is d8 / kPer16<Elem> 16-byte vectors (d8 is a multiple of
+// 8, and a 2-byte row of d8 elements keeps 16-byte alignment).
+template <typename Elem>
+constexpr int kPer16 = 16 / (int)sizeof(Elem);
+
+// 8 elements at p (16-byte aligned) as f32: two float4 loads, or one 16-byte load of a 2-byte type widened from its bits
+__device__ __forceinline__ void fs_load8(const float* p, float* x) {
+  const float4 a = *reinterpret_cast<const float4*>(p), b = *reinterpret_cast<const float4*>(p + 4);
+  x[0] = a.x; x[1] = a.y; x[2] = a.z; x[3] = a.w; x[4] = b.x; x[5] = b.y; x[6] = b.z; x[7] = b.w;
+}
+template <typename T>
+__device__ __forceinline__ void fs_load8(const T* p, float* x) {
+  feat_widen8(*reinterpret_cast<const uint4*>(p), p, x);
+}
+
+// The rounding of a stored row: each f32 element once to the storage type, to nearest with ties to even, overflow to
+// +-inf, subnormals kept (cvt.rn), two elements per 32-bit word, the lower index in the low half.  A NaN stays a NaN.
+__device__ __forceinline__ unsigned int fs_round2(float a, float b, const __half*) {
+  return (unsigned int)__half_as_ushort(__float2half_rn(a)) | ((unsigned int)__half_as_ushort(__float2half_rn(b)) << 16);
+}
+__device__ __forceinline__ unsigned int fs_round2(float a, float b, const __nv_bfloat16*) {
+  return (unsigned int)__bfloat16_as_ushort(__float2bfloat16_rn(a)) |
+         ((unsigned int)__bfloat16_as_ushort(__float2bfloat16_rn(b)) << 16);
+}
+template <typename T>
+__device__ __forceinline__ uint4 fs_round8(const float4& a, const float4& b) {
+  const T* tag = nullptr;
+  return make_uint4(fs_round2(a.x, a.y, tag), fs_round2(a.z, a.w, tag), fs_round2(b.x, b.y, tag), fs_round2(b.z, b.w, tag));
+}
+
 // ------------------------------------------------------------------------------------------------ squared norms
 // One warp per row (query rows first, then every stored slot): per 8-lane block reduce_add, blocks accumulated in
 // order (src/distance.rs:36-44).  Lane l takes blocks l, l + 32, ...; lane 0 adds the block sums in block order.
-__global__ void fs_norm_kernel(FsStore s, FsCall c) {
-  const long long w = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int lane = threadIdx.x & 31;
-  const long long S = (long long)s.live * s.K;
-  if (w >= c.R + S) return;
-  const float* row = w < c.R ? c.rows + (size_t)w * s.d8 : s.feat + (size_t)(w - c.R) * s.d8;
-  const int nblk = s.d8 / 8;
+// A stored row of a 2-byte type is widened as it is loaded.
+template <typename T>
+__device__ __forceinline__ float fs_norm_acc(const T* row, int nblk, int lane) {
   float acc = 0.0f;
   for (int base = 0; base < nblk; base += 32) {
     const int blk = base + lane;
     float bs = 0.0f;
     if (blk < nblk) {
-      const float4 x0 = *reinterpret_cast<const float4*>(row + blk * 8);
-      const float4 x1 = *reinterpret_cast<const float4*>(row + blk * 8 + 4);
-      float t[8] = {x0.x * x0.x, x0.y * x0.y, x0.z * x0.z, x0.w * x0.w, x1.x * x1.x, x1.y * x1.y, x1.z * x1.z, x1.w * x1.w};
+      float x[8];
+      fs_load8(row + blk * 8, x);
+      float t[8] = {x[0] * x[0], x[1] * x[1], x[2] * x[2], x[3] * x[3], x[4] * x[4], x[5] * x[5], x[6] * x[6], x[7] * x[7]};
       bs = reduce_add8(t);
     }
     const int cntb = min(32, nblk - base);
     for (int j = 0; j < cntb; ++j) acc = acc + __shfl_sync(0xffffffffu, bs, j);
   }
+  return acc;
+}
+
+template <typename Elem>
+__global__ void fs_norm_kernel(FsStore s, FsCall c) {
+  const long long w = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  const long long S = (long long)s.live * s.K;
+  if (w >= c.R + S) return;
+  const Elem* feat = static_cast<const Elem*>(s.feat);
+  const int nblk = s.d8 / 8;
+  float acc;
+  if constexpr (sizeof(Elem) == 4)   // one row pointer for both kinds of row
+    acc = fs_norm_acc(w < c.R ? c.rows + (size_t)w * s.d8 : feat + (size_t)(w - c.R) * s.d8, nblk, lane);
+  else   // w is the same across the warp
+    acc = w < c.R ? fs_norm_acc(c.rows + (size_t)w * s.d8, nblk, lane)
+                  : fs_norm_acc(feat + (size_t)(w - c.R) * s.d8, nblk, lane);
   if (lane == 0) {
     if (w < c.R) c.qnorm[w] = acc;
     else c.snorm[w - c.R] = acc;
@@ -61,7 +109,10 @@ constexpr int kDP = kDC * 8 + 4;
 
 // MODE (kFsForeign / kFsOwnedGroup / kFsOwnedEach) changes the epilogue only: the group mode drops every entry of a
 // queried track (excl), the each mode folds max_dist per query (per row across its 16 threads, then one atomicMax per row).
-template <int METRIC, int MODE>
+// Elem changes the staging of the stored (B) rows only: a 2-byte row block of 8 elements is one 16-byte load, widened
+// into the same f32 tile, so 64 rows x kDC blocks are one load per thread; everything after the tile is the same.
+static_assert(kDT * kDC == 256, "one 16-byte load of stored 2-byte elements per thread and stage");
+template <typename Elem, int METRIC, int MODE>
 __global__ void __launch_bounds__(256) fs_dist_kernel(FsStore s, FsCall c, float filter, int tiles_s,
                                                       const unsigned char* __restrict__ excl) {
   __shared__ __align__(16) float sa[kDT][kDP];
@@ -71,6 +122,7 @@ __global__ void __launch_bounds__(256) fs_dist_kernel(FsStore s, FsCall c, float
   const int S = s.live * s.K;
   const int r0 = (int)(blockIdx.x / tiles_s) * kDT, c0 = (int)(blockIdx.x % tiles_s) * kDT;
   const int nblk = s.d8 / 8;
+  const Elem* feat = static_cast<const Elem*>(s.feat);
   float acc[4][4];
 #pragma unroll
   for (int i = 0; i < 4; ++i)
@@ -78,16 +130,32 @@ __global__ void __launch_bounds__(256) fs_dist_kernel(FsStore s, FsCall c, float
     for (int j = 0; j < 4; ++j) acc[i][j] = 0.0f;
 
   for (int b0 = 0; b0 < nblk; b0 += kDC) {
+    if constexpr (sizeof(Elem) == 4) {
 #pragma unroll
-    for (int k = tid; k < kDT * kDC * 2; k += 256) {
-      const int row = k / (kDC * 2), q4 = k % (kDC * 2), blk = b0 + q4 / 2;
-      float4 va = make_float4(0.f, 0.f, 0.f, 0.f), vb = va;
-      if (blk < nblk) {
-        if (r0 + row < c.R) va = *reinterpret_cast<const float4*>(c.rows + (size_t)(r0 + row) * s.d8 + q4 * 4 + b0 * 8);
-        if (c0 + row < S) vb = *reinterpret_cast<const float4*>(s.feat + (size_t)(c0 + row) * s.d8 + q4 * 4 + b0 * 8);
+      for (int k = tid; k < kDT * kDC * 2; k += 256) {
+        const int row = k / (kDC * 2), q4 = k % (kDC * 2), blk = b0 + q4 / 2;
+        float4 va = make_float4(0.f, 0.f, 0.f, 0.f), vb = va;
+        if (blk < nblk) {
+          if (r0 + row < c.R) va = *reinterpret_cast<const float4*>(c.rows + (size_t)(r0 + row) * s.d8 + q4 * 4 + b0 * 8);
+          if (c0 + row < S) vb = *reinterpret_cast<const float4*>(feat + (size_t)(c0 + row) * s.d8 + q4 * 4 + b0 * 8);
+        }
+        *reinterpret_cast<float4*>(&sa[row][q4 * 4]) = va;
+        *reinterpret_cast<float4*>(&sbm[row][q4 * 4]) = vb;
       }
-      *reinterpret_cast<float4*>(&sa[row][q4 * 4]) = va;
-      *reinterpret_cast<float4*>(&sbm[row][q4 * 4]) = vb;
+    } else {
+#pragma unroll
+      for (int k = tid; k < kDT * kDC * 2; k += 256) {
+        const int row = k / (kDC * 2), q4 = k % (kDC * 2), blk = b0 + q4 / 2;
+        float4 va = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (blk < nblk && r0 + row < c.R)
+          va = *reinterpret_cast<const float4*>(c.rows + (size_t)(r0 + row) * s.d8 + q4 * 4 + b0 * 8);
+        *reinterpret_cast<float4*>(&sa[row][q4 * 4]) = va;
+      }
+      const int row = tid / kDC, q8 = tid % kDC, blk = b0 + q8;
+      float x[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+      if (blk < nblk && c0 + row < S) fs_load8(feat + (size_t)(c0 + row) * s.d8 + blk * 8, x);
+      *reinterpret_cast<float4*>(&sbm[row][q8 * 8]) = make_float4(x[0], x[1], x[2], x[3]);
+      *reinterpret_cast<float4*>(&sbm[row][q8 * 8 + 4]) = make_float4(x[4], x[5], x[6], x[7]);
     }
     __syncthreads();
     const int nb = min(kDC, nblk - b0);
@@ -326,7 +394,9 @@ __global__ void __launch_bounds__(kOrderThreads) fs_order_kernel(FsStore s, FsCa
   }
 }
 
-// One CTA per item: writes the item's surviving rows into their ring slots.
+// One CTA per item: writes the item's surviving rows into their ring slots.  A 2-byte store rounds each f32 element
+// once (fs_round8): one thread per 8-element block, one 16-byte store.
+template <typename Elem>
 __global__ void fs_apply_kernel(FsStore s, FsCall c) {
   const int q = blockIdx.x;
   const int4 pl = c.plan[q];
@@ -336,12 +406,19 @@ __global__ void fs_apply_kernel(FsStore s, FsCall c) {
     if (ci < pl.z - K) continue;
     const int slot = (pl.w + ci) % K;
     const float4* src = reinterpret_cast<const float4*>(c.rows + (size_t)(a0 + k) * s.d8);
-    float4* dst = reinterpret_cast<float4*>(s.feat + ((size_t)pl.x * K + slot) * s.d8);
-    for (int e = threadIdx.x; e < w4; e += blockDim.x) dst[e] = src[e];
+    if constexpr (sizeof(Elem) == 4) {
+      float4* dst = reinterpret_cast<float4*>(static_cast<float*>(s.feat) + ((size_t)pl.x * K + slot) * s.d8);
+      for (int e = threadIdx.x; e < w4; e += blockDim.x) dst[e] = src[e];
+    } else {
+      uint4* dst = reinterpret_cast<uint4*>(static_cast<Elem*>(s.feat) + ((size_t)pl.x * K + slot) * s.d8);
+      for (int e = threadIdx.x; e < w4 / 2; e += blockDim.x) dst[e] = fs_round8<Elem>(src[2 * e], src[2 * e + 1]);
+    }
   }
 }
 
 // ------------------------------------------------------------------------------------------------ fetch / remove
+// out is f32 whatever the storage type: a 2-byte row is widened, one 8-element block per thread
+template <typename Elem>
 __global__ void fs_gather_kernel(FsStore s, const int* pos, float* out, int* out_cnt) {
   const int i = blockIdx.x, p = pos[i], K = s.K, w4 = s.d8 / 4;
   const int n = p >= 0 ? s.cnt[p] : 0;
@@ -349,19 +426,31 @@ __global__ void fs_gather_kernel(FsStore s, const int* pos, float* out, int* out
   for (int b = 0; b < K; ++b) {
     float4* dst = reinterpret_cast<float4*>(out + ((size_t)i * K + b) * s.d8);
     if (b < n) {
-      const float4* src = reinterpret_cast<const float4*>(s.feat + ((size_t)p * K + (s.start[p] + b) % K) * s.d8);
-      for (int e = threadIdx.x; e < w4; e += blockDim.x) dst[e] = src[e];
+      const Elem* row = static_cast<const Elem*>(s.feat) + ((size_t)p * K + (s.start[p] + b) % K) * s.d8;
+      if constexpr (sizeof(Elem) == 4) {
+        const float4* src = reinterpret_cast<const float4*>(row);
+        for (int e = threadIdx.x; e < w4; e += blockDim.x) dst[e] = src[e];
+      } else {
+        for (int e = threadIdx.x; e < w4 / 2; e += blockDim.x) {
+          float x[8];
+          fs_load8(row + 8 * e, x);
+          dst[2 * e] = make_float4(x[0], x[1], x[2], x[3]);
+          dst[2 * e + 1] = make_float4(x[4], x[5], x[6], x[7]);
+        }
+      }
     } else {
       for (int e = threadIdx.x; e < w4; e += blockDim.x) dst[e] = make_float4(0.f, 0.f, 0.f, 0.f);
     }
   }
 }
 
+// The row movers below copy rows as 16-byte vectors (float4 whatever the element type): d8 / kPer16<Elem> per row.
+template <typename Elem>
 __global__ void fs_compact_kernel(FsStore src, FsStore dst, const int* from) {
   const int i = blockIdx.x, p = from[i];
-  const size_t w4 = (size_t)src.K * src.d8 / 4;
-  const float4* a = reinterpret_cast<const float4*>(src.feat + (size_t)p * src.K * src.d8);
-  float4* b = reinterpret_cast<float4*>(dst.feat + (size_t)i * src.K * src.d8);
+  const size_t w4 = (size_t)src.K * src.d8 / kPer16<Elem>;
+  const float4* a = reinterpret_cast<const float4*>(static_cast<const Elem*>(src.feat) + (size_t)p * src.K * src.d8);
+  float4* b = reinterpret_cast<float4*>(static_cast<Elem*>(dst.feat) + (size_t)i * src.K * src.d8);
   for (size_t e = threadIdx.x; e < w4; e += blockDim.x) b[e] = a[e];
   if (threadIdx.x == 0) {
     dst.cnt[i] = src.cnt[p];
@@ -371,18 +460,29 @@ __global__ void fs_compact_kernel(FsStore src, FsStore dst, const int* from) {
 }
 
 // ------------------------------------------------------------------------------------------------ owned calls
-// search_owned: one thread per float4 of a request row; row r is observation r - qoff[q] (oldest first) of the
-// stored track at qpos[q], q = row_q[r].  No staging goes through the host.
+// search_owned: one thread per 16-byte vector of a stored row (a float4, or 8 elements of a 2-byte type, widened); row r
+// is observation r - qoff[q] (oldest first) of the stored track at qpos[q], q = row_q[r].  No staging goes through the
+// host.
+template <typename Elem>
 __global__ void __launch_bounds__(256) fs_owned_stage_kernel(FsStore s, FsCall c, const int* __restrict__ qpos,
                                                              float* __restrict__ rows) {
-  const int w4 = s.d8 / 4;
+  const int w4 = s.d8 / kPer16<Elem>;
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (long long)c.R * w4) return;
   const int r = (int)(i / w4), e = (int)(i - (long long)r * w4);
   const int q = c.row_q[r], p = qpos[q];
   const int slot = (s.start[p] + (r - c.qoff[q])) % s.K;
-  reinterpret_cast<float4*>(rows + (size_t)r * s.d8)[e] =
-      reinterpret_cast<const float4*>(s.feat + ((size_t)p * s.K + slot) * s.d8)[e];
+  const Elem* feat = static_cast<const Elem*>(s.feat);
+  if constexpr (sizeof(Elem) == 4) {
+    reinterpret_cast<float4*>(rows + (size_t)r * s.d8)[e] =
+        reinterpret_cast<const float4*>(feat + ((size_t)p * s.K + slot) * s.d8)[e];
+  } else {
+    float x[8];
+    fs_load8(feat + ((size_t)p * s.K + slot) * s.d8 + 8 * e, x);
+    float4* dst = reinterpret_cast<float4*>(rows + (size_t)r * s.d8) + 2 * e;
+    dst[0] = make_float4(x[0], x[1], x[2], x[3]);
+    dst[1] = make_float4(x[4], x[5], x[6], x[7]);
+  }
 }
 
 __global__ void fs_peek_kernel(FsStore s, const int* __restrict__ pos, int n, int* __restrict__ out) {
@@ -394,19 +494,22 @@ __global__ void fs_peek_kernel(FsStore s, const int* __restrict__ pos, int n, in
 
 // merge_owned in two launches whatever the chain structure: every moving row is read from its pre-call slot into
 // scratch first, then written to its final slot, so no row is read after it has been overwritten.  One CTA per row.
-__global__ void fs_move_gather_kernel(FsStore s, const int* __restrict__ src, float* __restrict__ scratch) {
-  const int m = blockIdx.x, w4 = s.d8 / 4;
-  const float4* a = reinterpret_cast<const float4*>(s.feat + (size_t)src[m] * s.d8);
+// Scratch rows are in the storage type: rows move, they are never converted.
+template <typename Elem>
+__global__ void fs_move_gather_kernel(FsStore s, const int* __restrict__ src, Elem* __restrict__ scratch) {
+  const int m = blockIdx.x, w4 = s.d8 / kPer16<Elem>;
+  const float4* a = reinterpret_cast<const float4*>(static_cast<const Elem*>(s.feat) + (size_t)src[m] * s.d8);
   float4* b = reinterpret_cast<float4*>(scratch + (size_t)m * s.d8);
   for (int e = threadIdx.x; e < w4; e += blockDim.x) b[e] = a[e];
 }
 
+template <typename Elem>
 __global__ void fs_move_scatter_kernel(FsStore s, const int* __restrict__ dst, int n_moves, const int* __restrict__ hdr,
-                                       int n_hdr, const float* __restrict__ scratch) {
-  const int m = blockIdx.x, w4 = s.d8 / 4;
+                                       int n_hdr, const Elem* __restrict__ scratch) {
+  const int m = blockIdx.x, w4 = s.d8 / kPer16<Elem>;
   if (m < n_moves) {
     const float4* a = reinterpret_cast<const float4*>(scratch + (size_t)m * s.d8);
-    float4* b = reinterpret_cast<float4*>(s.feat + (size_t)dst[m] * s.d8);
+    float4* b = reinterpret_cast<float4*>(static_cast<Elem*>(s.feat) + (size_t)dst[m] * s.d8);
     for (int e = threadIdx.x; e < w4; e += blockDim.x) b[e] = a[e];
   }
   if (m < n_hdr && threadIdx.x == 0) {
@@ -421,15 +524,6 @@ __global__ void fs_move_scatter_kernel(FsStore s, const int* __restrict__ dst, i
 // so every later stage sees the values of the widened f32 request.  With `vec` (D % 8 == 0 and a 16-byte aligned base) a
 // block of a 2-byte column is one 16-byte load, as in cand_norm_kernel; otherwise elements are read one by one and the
 // last block is zero-padded from D to d8.
-__device__ __forceinline__ void fs_load8(const float* p, float* x) {
-  const float4 a = *reinterpret_cast<const float4*>(p), b = *reinterpret_cast<const float4*>(p + 4);
-  x[0] = a.x; x[1] = a.y; x[2] = a.z; x[3] = a.w; x[4] = b.x; x[5] = b.y; x[6] = b.z; x[7] = b.w;
-}
-template <typename T>
-__device__ __forceinline__ void fs_load8(const T* p, float* x) {
-  feat_widen8(*reinterpret_cast<const uint4*>(p), p, x);
-}
-
 template <typename T>
 __global__ void __launch_bounds__(256) fs_stage_kernel(const T* __restrict__ col, const int* __restrict__ row_src, int R,
                                                        int D, int d8, int vec, float* __restrict__ rows) {
@@ -462,11 +556,12 @@ __global__ void fs_blob_check_kernel(const int* __restrict__ cnt, const int* __r
 }
 
 // one warp per track; a track whose ring is full has nothing to zero
-__global__ void fs_blob_scrub_kernel(float* feat, const int* __restrict__ cnt, const int* __restrict__ start, int n, int K,
+template <typename Elem>
+__global__ void fs_blob_scrub_kernel(Elem* feat, const int* __restrict__ cnt, const int* __restrict__ start, int n, int K,
                                      int d8) {
   const int t = (int)(((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
   if (t >= n) return;
-  const int c = cnt[t], s0 = start[t], w4 = d8 / 4;
+  const int c = cnt[t], s0 = start[t], w4 = d8 / kPer16<Elem>;
   for (int j = c; j < K; ++j) {
     float4* d = reinterpret_cast<float4*>(feat + ((size_t)t * K + (s0 + j) % K) * d8);
     for (int e = lane; e < w4; e += 32) d[e] = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -475,27 +570,30 @@ __global__ void fs_blob_scrub_kernel(float* feat, const int* __restrict__ cnt, c
 
 }  // namespace
 
-template <int MODE>
+template <typename Elem, int MODE>
 void fs_dist_grid(int metric, float filter, const FsStore& s, const FsCall& c, int tiles_s, unsigned grid,
                   const unsigned char* excl, cudaStream_t st) {
-  if (metric == 0) fs_dist_kernel<0, MODE><<<grid, 256, 0, st>>>(s, c, filter, tiles_s, excl);
-  else fs_dist_kernel<1, MODE><<<grid, 256, 0, st>>>(s, c, filter, tiles_s, excl);
+  if (metric == 0) fs_dist_kernel<Elem, 0, MODE><<<grid, 256, 0, st>>>(s, c, filter, tiles_s, excl);
+  else fs_dist_kernel<Elem, 1, MODE><<<grid, 256, 0, st>>>(s, c, filter, tiles_s, excl);
 }
 
 void fs_launch_dist(int metric, float filter, const FsStore& s, const FsCall& c, cudaStream_t st, int mode,
                     const unsigned char* excl) {
   const long long S = (long long)s.live * s.K;
   if (c.R == 0 || S == 0) return;
-  if (metric == 1) {
-    const long long warps = c.R + S;
-    fs_norm_kernel<<<(unsigned)((warps * 32 + 255) / 256), 256, 0, st>>>(s, c);
-    note_launch();
-  }
   const int tiles_s = (int)((S + kDT - 1) / kDT), tiles_r = (c.R + kDT - 1) / kDT;
   const unsigned grid = (unsigned)((long long)tiles_s * tiles_r);
-  if (mode == kFsOwnedGroup) fs_dist_grid<kFsOwnedGroup>(metric, filter, s, c, tiles_s, grid, excl, st);
-  else if (mode == kFsOwnedEach) fs_dist_grid<kFsOwnedEach>(metric, filter, s, c, tiles_s, grid, excl, st);
-  else fs_dist_grid<kFsForeign>(metric, filter, s, c, tiles_s, grid, excl, st);
+  feat_dispatch(s.stype, [&](auto tag) {
+    using Elem = decltype(tag);
+    if (metric == 1) {
+      const long long warps = c.R + S;
+      fs_norm_kernel<Elem><<<(unsigned)((warps * 32 + 255) / 256), 256, 0, st>>>(s, c);
+      note_launch();
+    }
+    if (mode == kFsOwnedGroup) fs_dist_grid<Elem, kFsOwnedGroup>(metric, filter, s, c, tiles_s, grid, excl, st);
+    else if (mode == kFsOwnedEach) fs_dist_grid<Elem, kFsOwnedEach>(metric, filter, s, c, tiles_s, grid, excl, st);
+    else fs_dist_grid<Elem, kFsForeign>(metric, filter, s, c, tiles_s, grid, excl, st);
+  });
   note_launch();
 }
 
@@ -511,8 +609,11 @@ void fs_launch_topn(float max_distance, int min_votes, int topn, bool want_dest,
 
 void fs_launch_owned_stage(const FsStore& s, const FsCall& c, const int* qpos, float* rows, cudaStream_t st) {
   if (c.R == 0) return;
-  const long long threads = (long long)c.R * (s.d8 / 4);
-  fs_owned_stage_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(s, c, qpos, rows);
+  feat_dispatch(s.stype, [&](auto tag) {
+    using Elem = decltype(tag);
+    const long long threads = (long long)c.R * (s.d8 / kPer16<Elem>);
+    fs_owned_stage_kernel<Elem><<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(s, c, qpos, rows);
+  });
   note_launch();
 }
 
@@ -523,33 +624,37 @@ void fs_launch_peek(const FsStore& s, const int* pos, int n, int* out, cudaStrea
 }
 
 void fs_launch_move_rows(const FsStore& s, const int* src, const int* dst, int n_moves, const int* hdr, int n_hdr,
-                         float* scratch, cudaStream_t st) {
-  if (n_moves > 0) {
-    fs_move_gather_kernel<<<n_moves, 128, 0, st>>>(s, src, scratch);
-    note_launch();
-  }
-  if (std::max(n_moves, n_hdr) > 0) {
-    fs_move_scatter_kernel<<<std::max(n_moves, n_hdr), 128, 0, st>>>(s, dst, n_moves, hdr, n_hdr, scratch);
-    note_launch();
-  }
+                         void* scratch, cudaStream_t st) {
+  feat_dispatch(s.stype, [&](auto tag) {
+    using Elem = decltype(tag);
+    if (n_moves > 0) {
+      fs_move_gather_kernel<Elem><<<n_moves, 128, 0, st>>>(s, src, static_cast<Elem*>(scratch));
+      note_launch();
+    }
+    if (std::max(n_moves, n_hdr) > 0) {
+      fs_move_scatter_kernel<Elem><<<std::max(n_moves, n_hdr), 128, 0, st>>>(s, dst, n_moves, hdr, n_hdr,
+                                                                             static_cast<const Elem*>(scratch));
+      note_launch();
+    }
+  });
 }
 
 void fs_launch_apply(const FsStore& s, const FsCall& c, cudaStream_t st) {
   if (c.Q == 0) return;
   fs_order_kernel<<<1, kOrderThreads, 0, st>>>(s, c);
-  fs_apply_kernel<<<c.Q, 128, 0, st>>>(s, c);
+  feat_dispatch(s.stype, [&](auto tag) { fs_apply_kernel<decltype(tag)><<<c.Q, 128, 0, st>>>(s, c); });
   note_launch(2);
 }
 
 void fs_launch_gather(const FsStore& s, const int* pos, int n, float* out, int* out_cnt, cudaStream_t st) {
   if (n == 0) return;
-  fs_gather_kernel<<<n, 128, 0, st>>>(s, pos, out, out_cnt);
+  feat_dispatch(s.stype, [&](auto tag) { fs_gather_kernel<decltype(tag)><<<n, 128, 0, st>>>(s, pos, out, out_cnt); });
   note_launch();
 }
 
 void fs_launch_compact(const FsStore& src, const FsStore& dst, const int* from, int n, cudaStream_t st) {
   if (n == 0) return;
-  fs_compact_kernel<<<n, 128, 0, st>>>(src, dst, from);
+  feat_dispatch(src.stype, [&](auto tag) { fs_compact_kernel<decltype(tag)><<<n, 128, 0, st>>>(src, dst, from); });
   note_launch();
 }
 
@@ -571,9 +676,13 @@ void fs_launch_blob_check(const int* cnt, const int* start, int n, int K, int* b
   note_launch();
 }
 
-void fs_launch_blob_scrub(float* feat, const int* cnt, const int* start, int n, int K, int d8, cudaStream_t st) {
+void fs_launch_blob_scrub(int stype, void* feat, const int* cnt, const int* start, int n, int K, int d8, cudaStream_t st) {
   if (n == 0) return;
-  fs_blob_scrub_kernel<<<(unsigned)(((long long)n * 32 + 255) / 256), 256, 0, st>>>(feat, cnt, start, n, K, d8);
+  feat_dispatch(stype, [&](auto tag) {
+    using Elem = decltype(tag);
+    fs_blob_scrub_kernel<Elem><<<(unsigned)(((long long)n * 32 + 255) / 256), 256, 0, st>>>(static_cast<Elem*>(feat), cnt,
+                                                                                           start, n, K, d8);
+  });
   note_launch();
 }
 

@@ -19,14 +19,18 @@ constexpr long long kFsMaxPairs = 1LL << 30;   // observation pairs of one call'
 
 // The store's device columns, in store order (insertion order; removal is a stable compaction).  Observation j (oldest
 // first) of track t lives in ring slot (start[t] + j) % K of feat[t][.][.]; rows are zero-padded from D to d8 as
-// Feature::from_vec pads (src/track/utils.rs:45-71).
+// Feature::from_vec pads (src/track/utils.rs:45-71).  Rows are stored as f32, binary16 or bfloat16 (stype, an
+// SB200_FEATURE_*); every kernel that touches them is instantiated per storage type, picked by its launcher, and widens a
+// stored element to f32 where it loads it.  stype sits in what was the struct's tail padding, so the layout the existing
+// f32 kernels read is unchanged.
 struct FsStore {
-  float* feat;                // [cap][K][d8]
+  void* feat;                 // [cap][K][d8] elements of stype
   int* cnt;                   // [cap] observations held (1..K)
   int* start;                 // [cap] ring slot of the oldest observation
   unsigned long long* ids;    // [cap]
   int* run;                   // [cap] scratch of the apply stage; zero between calls
   int K, d8, live;
+  int stype;                  // storage type of feat (SB200_FEATURE_*); host side only
 };
 
 // One request on the device.  Items are the queries of search / associate, or the single observations of add.
@@ -83,18 +87,21 @@ void fs_launch_topn(float max_distance, int min_votes, int topn, bool want_dest,
                     cudaStream_t st, int mode = kFsForeign);
 // out[2 i] = cnt[pos[i]], out[2 i + 1] = start[pos[i]]: the ring state of the tracks an owned call touches
 void fs_launch_peek(const FsStore& s, const int* pos, int n, int* out, cudaStream_t st);
-// merge_owned: scratch[m] = stored row src[m], then stored row dst[m] = scratch[m] (rows index feat as [cap * K][d8]),
-// and cnt / start of the tracks hdr[3 j] set to hdr[3 j + 1] / hdr[3 j + 2]
+// merge_owned: scratch[m] = stored row src[m], then stored row dst[m] = scratch[m] (rows index feat as [cap * K][d8];
+// scratch rows are in the storage type), and cnt / start of the tracks hdr[3 j] set to hdr[3 j + 1] / hdr[3 j + 2]
 void fs_launch_move_rows(const FsStore& s, const int* src, const int* dst, int n_moves, const int* hdr, int n_hdr,
-                         float* scratch, cudaStream_t st);
+                         void* scratch, cudaStream_t st);
+// merge / append; the f32 request rows are rounded to the storage type here (round to nearest even), and nowhere else
 void fs_launch_apply(const FsStore& s, const FsCall& c, cudaStream_t st);
-// out[i][b][.] = observation b (oldest first) of the track at pos[i] (-1: none), out_cnt[i] its count (0 for -1)
+// out[i][b][.] = observation b (oldest first) of the track at pos[i] (-1: none), widened to f32, out_cnt[i] its count (0
+// for -1)
 void fs_launch_gather(const FsStore& s, const int* pos, int n, float* out, int* out_cnt, cudaStream_t st);
 // dst[i] = src[from[i]] for the i < n kept tracks (stable compaction into fresh columns)
 void fs_launch_compact(const FsStore& src, const FsStore& dst, const int* from, int n, cudaStream_t st);
 // store blob, before any row is copied: bad[0] counts the cnt[i] outside [1, K], bad[1] the start[i] outside [0, K)
 void fs_launch_blob_check(const int* cnt, const int* start, int n, int K, int* bad, cudaStream_t st);
-// store blob, after its rows are copied: zeroes, in feat[n][K][d8], the ring slots that hold no observation
-void fs_launch_blob_scrub(float* feat, const int* cnt, const int* start, int n, int K, int d8, cudaStream_t st);
+// store blob, after its rows are copied: zeroes, in feat[n][K][d8] (elements of stype), the ring slots that hold no
+// observation
+void fs_launch_blob_scrub(int stype, void* feat, const int* cnt, const int* start, int n, int K, int d8, cudaStream_t st);
 
 }  // namespace sb

@@ -666,12 +666,19 @@ class FeatureStore:
     (or "f16") a 2-byte array (e.g. the uint16 bits of bfloat16 values) is sent as it is, with that element type.  The
     *_device calls take the raw address of a column on the store's device, in the type set by set_feature_type, and a
     cudaStream_t (0: the legacy default stream) whose pending work the call waits for.  Results never depend on the
-    type or on where the column lives: they are those of the widened float32 request."""
+    type or on where the column lives: they are those of the widened float32 request.
+
+    Storage: `storage` ("f32", "f16" or "bf16") is the element type of the stored rows (sb200_fstore_set_storage_type).
+    A 2-byte store takes half the device memory and half the blob; each row is rounded to it once, when it is stored,
+    and queries are never rounded.  Fed features of its own type, a 2-byte store returns exactly what an f32 store
+    returns; fetch() returns the stored values as float32."""
 
     def __init__(self, metric="euclidean", distance_filter=100.0, max_observations=3, feature_dim=256, topn=1,
-                 max_distance=100.0, min_votes=1, device=0):
+                 max_distance=100.0, min_votes=1, device=0, storage="f32"):
         if metric not in METRICS:
             raise ValueError(f"metric must be one of {sorted(METRICS)}")
+        if storage not in FEATURE_TYPES:
+            raise ValueError(f"storage must be one of {sorted(FEATURE_TYPES)}")
         self._L = lib()
         o = _lib.FstoreOptions(METRICS[metric], distance_filter, max_observations, feature_dim, topn, max_distance,
                                min_votes, device)
@@ -680,6 +687,7 @@ class FeatureStore:
         self._h = h
         self.K, self.D, self.topn = int(max_observations), int(feature_dim), int(topn)
         self._explicit_type = None
+        check(self._L.sb200_fstore_set_storage_type(h, FEATURE_TYPES[storage]))
 
     def close(self):
         if getattr(self, "_h", None):
@@ -704,6 +712,12 @@ class FeatureStore:
         """The element type now set in the library."""
         t = C.c_int32(0)
         check(self._L.sb200_fstore_get_options(self._h, None, C.byref(t)))
+        return {v: k for k, v in FEATURE_TYPES.items()}[t.value]
+
+    def storage_type(self):
+        """The element type of the stored rows: "f32", "f16" or "bf16" (a loaded store has its blob's)."""
+        t = C.c_int32(0)
+        check(self._L.sb200_fstore_get_storage_type(self._h, C.byref(t)))
         return {v: k for k, v in FEATURE_TYPES.items()}[t.value]
 
     def _use_declared_type(self):
