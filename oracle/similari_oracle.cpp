@@ -183,7 +183,8 @@ bool iou(const Box& l, const Box& r, float* out) {
 // parameter interval, so each edge needs an interval union only.  Coincident outlines (exact zeros): a segment on an
 // edge line of another box is inside it iff both run the same way (between two covering boxes: only the lower index
 // covers), and never counts as inside box_i itself.  Pinned by the reference's own test (bbox_own_areas.rs:50-79:
-// 75 / 50 / 75) and cross-checked against inclusion-exclusion and Monte-Carlo in tests/test_own_area_cpu.py;
+// 75 / 50 / 75) and cross-checked against inclusion-exclusion (tests/test_own_area_cpu.py) and an exact slab / cell
+// reference (tests/test_own_area_exact_cpu.py);
 // parity with geo's floating-point pipeline beyond that is unpinned (expected agreement ~1e-12 relative).
 namespace own {
 bool inside_interval(const P2& p, const P2& d, const P2 q[4], double s, bool on_edge_same_dir_inside, double* t0, double* t1) {
@@ -228,6 +229,16 @@ bool apart(const P2 a[4], const P2 b[4]) {
   }
   return false;
 }
+// a box of zero area: its edges come in coincident pairs of opposite direction, which the coincident-edge rules above do
+// not cancel on another box's edge line
+bool zero_area(const P2 q[4]) {
+  double a = 0.0;
+  for (int v = 1; v < 3; ++v) {
+    const double ux = q[v].x - q[0].x, uy = q[v].y - q[0].y, wx = q[v + 1].x - q[0].x, wy = q[v + 1].y - q[0].y;
+    a += ux * wy - uy * wx;
+  }
+  return a == 0.0;
+}
 }  // namespace own
 
 std::vector<float> own_area_shares(const std::vector<Box>& boxes) {
@@ -241,6 +252,7 @@ std::vector<float> own_area_shares(const std::vector<Box>& boxes) {
     for (int j = 0; j < n; ++j) {
       if (j == i || too_far(boxes[i], boxes[j])) continue;          // bbox_own_areas.rs:10-15
       if (own::apart(quad[i].data(), quad[j].data())) continue;      // disjoint: the difference removes nothing
+      if (own::zero_area(quad[j].data())) continue;                   // aspect or height 0: covers nothing
       qs.push_back(quad[j].data());
     }
     std::vector<P2> ring(quad[i].begin(), quad[i].end());

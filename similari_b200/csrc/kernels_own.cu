@@ -3,8 +3,8 @@
 // Replaces exclusively_owned_areas + exclusively_owned_areas_normalized_shares
 // (src/utils/clipping/bbox_own_areas.rs:8-46) as the visual trackers call them when an own-area threshold is set
 // (src/trackers/visual_sort/simple_api.rs:110-127, visual_sort/batch_api.rs:236-249).  Arithmetic: sb_own_area.cuh.
-// Step 1: the lanes scan the scene's boxes 32 at a time; a box that is not too_far and not certainly disjoint (separating
-// axis pre-gate) is appended, in index order, to the warp's list in shared memory.  Step 2: the 4 * (k + 1) edges of box_i
+// Step 1: the lanes scan the scene's boxes 32 at a time; a box that is not too_far, not certainly disjoint (separating
+// axis pre-gate) and not of zero area (own_can_cover) is appended, in index order, to the warp's list in shared memory.  Step 2: the 4 * (k + 1) edges of box_i
 // and of the k listed boxes are spread over the lanes; each lane integrates its edges' parts that border the difference
 // region; a shuffle tree adds the lanes.  Cost: O(m) cheap gates + O(k^2) half-plane tests per detection.
 #include "sb_engine.cuh"
@@ -39,7 +39,7 @@ __global__ void __launch_bounds__(OW_WARPS * 32) own_area_kernel(Frame f, const 
       const float* bj = boxes + (size_t)(sc.det_base + j) * 6;
       if (!too_far(bx, by, ri, bj[0], bj[1], box_radius(bj[3], bj[4]))) {   // bbox_own_areas.rs:12-14
         box_vertices(bj[0], bj[1], bj[2], bj[3], bj[4], vj);
-        keep = rect_overlap_bound(vi, vj) != 0.0;                           // certainly disjoint boxes remove nothing
+        keep = own_can_cover(vi, vj);
       }
     }
     const unsigned int mask = __ballot_sync(0xffffffffu, keep);
@@ -103,7 +103,7 @@ __global__ void __launch_bounds__(OB_T) own_area_big_kernel(Frame f, const float
         const float* bj = boxes + (size_t)(sc.det_base + j) * 6;
         if (!too_far(bx, by, ri, bj[0], bj[1], box_radius(bj[3], bj[4]))) {
           box_vertices(bj[0], bj[1], bj[2], bj[3], bj[4], vj);
-          keep = rect_overlap_bound(vi, vj) != 0.0;
+          keep = own_can_cover(vi, vj);
         }
       }
       const unsigned int mask = __ballot_sync(0xffffffffu, keep);

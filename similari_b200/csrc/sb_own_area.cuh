@@ -19,7 +19,7 @@
 // "Inside box_i" (for the edges of the covering boxes) is open: a covering box's edge on box_i's outline never borders D.
 //
 // `__host__ __device__` like sb_math.cuh: the CPU suite checks these functions (tests/host_shim) against the oracle and
-// against independent inclusion-exclusion / Monte-Carlo evaluations without a GPU.
+// against an exact reference that does not use this formulation (tests/own_area_exact.py) without a GPU.
 #pragma once
 #include "sb_math.cuh"
 
@@ -38,6 +38,14 @@ SB_HD double quad_area_signed(const double* q) {
     pax = qx; pay = qy;
   }
   return tmp / 2.0;
+}
+
+// Whether box j (vertices vj) can take area from box i (vi) and so joins box i's list.  Certainly disjoint boxes remove
+// nothing (separating-axis gate; it also drops boxes with a NaN vertex).  Nor do boxes of zero area (aspect or height
+// 0): their edges come in coincident pairs of opposite direction, which the tie rules for coincident edges do not
+// cancel where the pair lies on another box's edge line.
+SB_HD bool own_can_cover(const double* vi, const double* vj) {
+  return quad_area_signed(vj) != 0.0 && rect_overlap_bound(vi, vj) != 0.0;
 }
 
 // Parameter interval [t0, t1] of the segment P + t d (t in [0, 1]) inside the convex quadrilateral q whose vertices run
@@ -178,7 +186,7 @@ SB_HD float own_area_share_seq(const float* boxes, int n, int i) {
     if (too_far(bi[0], bi[1], ri, bj[0], bj[1], box_radius(bj[3], bj[4]))) continue;   // bbox_own_areas.rs:12-14
     double vj[8];
     box_vertices(bj[0], bj[1], bj[2], bj[3], bj[4], vj);
-    if (rect_overlap_bound(quads, vj) == 0.0) continue;   // certainly disjoint: removes nothing
+    if (!own_can_cover(quads, vj)) continue;
     if (k >= kOwnMaxNb) return -1.0f;
     ++k;
     for (int q = 0; q < 8; ++q) quads[k * 8 + q] = vj[q];

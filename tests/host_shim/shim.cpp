@@ -2,6 +2,7 @@
 // compare it bit-for-bit with the oracle before any GPU time is spent.  TEST INFRASTRUCTURE: the product never
 // loads this library and has no CPU execution path.
 #include <string.h>
+#include <vector>
 #include "../../similari_b200/csrc/sb_math.cuh"
 #include "../../similari_b200/csrc/sb_own_area.cuh"
 extern "C" {
@@ -31,6 +32,31 @@ float shim_maha(float pw, const float* st, const float* b) {
 long long shim_weight(float v) { return sb::weight_i64(v); }
 void shim_own_area_shares(const float* boxes, int n, float* out) {
   for (int i = 0; i < n; ++i) out[i] = sb::own_area_share_seq(boxes, n, i);
+}
+// own_area_big_kernel's arithmetic for box i, run serially: the same gather in index order as own_area_share_seq, without
+// its kOwnMaxNb cap (the kernel's cap is kOwnBigNb: -1 above it), and own_edge_term_big summed in edge order.
+float shim_own_area_share_big(const float* boxes, int n, int i) {
+  const float* bi = boxes + (size_t)i * 6;
+  std::vector<double> quads(8);
+  sb::box_vertices(bi[0], bi[1], bi[2], bi[3], bi[4], quads.data());
+  const double s = sb::quad_area_signed(quads.data()) < 0.0 ? -1.0 : 1.0;
+  const float ri = sb::box_radius(bi[3], bi[4]);
+  int k = 0;
+  for (int j = 0; j < n; ++j) {
+    if (j == i) continue;
+    const float* bj = boxes + (size_t)j * 6;
+    if (sb::too_far(bi[0], bi[1], ri, bj[0], bj[1], sb::box_radius(bj[3], bj[4]))) continue;
+    double vj[8];
+    sb::box_vertices(bj[0], bj[1], bj[2], bj[3], bj[4], vj);
+    if (!sb::own_can_cover(quads.data(), vj)) continue;
+    if (k >= sb::kOwnBigNb) return -1.0f;
+    ++k;
+    quads.insert(quads.end(), vj, vj + 8);
+  }
+  double sum = 0.0;
+  for (int js = 0; js <= k; ++js)
+    for (int e = 0; e < 4; ++e) sum += sb::own_edge_term_big(quads.data(), k, js, e, s);
+  return sb::own_share(s * sum / 2.0, bi[3], bi[4]);
 }
 double shim_overlap_bound(const double* a8, const double* b8) { return sb::rect_overlap_bound(a8, b8); }
 int shim_iou_bound_fails(const float* l, const float* r, float conf, float thr) {
