@@ -552,6 +552,40 @@ int sb200_fstore_search_owned(sb200_fstore* s, int32_t n, const uint64_t* ids, i
 int sb200_fstore_merge_owned(sb200_fstore* s, int32_t n, const uint64_t* dest_ids, const uint64_t* src_ids,
                              int32_t remove_src);
 
+/* The TrackStore side of examples/track_merging.rs for the visual trackers: a collection of tracker `t`'s wasted records
+ * whose feature histories go into store `s` without leaving the device.
+ * Records: collects up to `cap` wasted records exactly as sb200_wasted_history(t, cap, ..., history_cap, ...) does (the
+ * same collection point with its auto-waste step, the same records in the same order, the same outputs); any of those
+ * output pointers may be NULL.  history_cap bounds only the box histories.
+ * Query of record i: the present features of its whole kept history (its newest min(length, history_length)
+ * observations), oldest first; feature_counts[i] is their number and queried[i] is 1 when it is > 0.  The queried
+ * records are associated with the store as ONE sb200_fstore_associate call would associate them, with query id
+ * ids[i] + id_offset (mod 2^64) and those rows as the f32 request (so max_dist is taken over every kept entry of the
+ * call; the store keeps the newest max_observations rows of each query).  The store outputs are indexed by record:
+ * counts[n], winners[n][topn], weights[n][topn], track_ids[n], merged[n], each meaning what it means for
+ * sb200_fstore_associate; a record that is not queried gets 0 in every one of them.  Every output may be NULL.
+ * Exactness: outputs, the store (its blob) and the tracker (its blob) afterwards are, bit for bit, those of
+ * sb200_wasted_visual(t, cap, ..., history_cap) followed by sb200_fstore_associate on the present rows of the queried
+ * records, for every storage type, feature type and feature column type.
+ * Refusals, SB200_ERR_INVALID unless noted, sb200_last_error naming the cause.  Before anything happens: a NULL handle,
+ * cap < 0 or history_cap < 0, a tracker that is not visual or whose feature history is off, tracker and store on
+ * different devices, a feature_dim that differs (checked once the tracker's dimension is fixed: a tracker that has never
+ * seen a feature holds no present rows).  After the auto-waste step, before any record leaves the wasted buffer and
+ * before the store changes: a query id that is already stored; a call whose distance matrix needs more than 2^30
+ * observation pairs (SB200_ERR_CAPACITY: the call is not split, as that would change max_dist; lower `cap`).  After a
+ * refusal the records are all still in the wasted buffer and the store is unchanged; the auto-waste step, which any
+ * collection point runs, is the only effect.
+ * The call is synchronous and both handles are single-threaded.  The records' history blocks go back to the tracker's
+ * pool only after the store's work on them is complete, so a frame enqueued after the call may reuse them.  An empty
+ * buffer, or records without a present feature, launch no store kernel and leave the store unchanged.  Returns the
+ * records collected (>= 0) or a negative status.  No counterpart in the reference's Python API. */
+int64_t sb200_fstore_associate_wasted(sb200_fstore* s, sb200_tracker* t, int64_t cap, uint64_t id_offset, uint64_t* ids,
+                                      uint64_t* scene_ids, uint32_t* epochs, uint32_t* lengths, float* predicted_boxes,
+                                      float* observed_boxes, int32_t history_cap, float* predicted_history,
+                                      float* observed_history, int32_t* history_counts, int32_t* feature_counts,
+                                      uint8_t* queried, int32_t* counts, uint64_t* winners, double* weights,
+                                      uint64_t* track_ids, uint8_t* merged);
+
 /* ---- the store blob ----
  * The whole store as one relocatable block of bytes: this header, then four sections at 256-byte aligned offsets, gaps
  * zeroed, in this order: ids[live] (u64), cnt[live] (i32 observations held), start[live] (i32 ring slot of the oldest

@@ -136,6 +136,7 @@ EXPORTS = [
     "sb200_fstore_get_options", "sb200_fstore_add_device", "sb200_fstore_search_device",
     "sb200_fstore_associate_device", "sb200_fstore_save", "sb200_fstore_load", "sb200_fstore_search_owned",
     "sb200_fstore_merge_owned", "sb200_fstore_set_storage_type", "sb200_fstore_get_storage_type",
+    "sb200_fstore_associate_wasted",
 ]
 
 
@@ -237,6 +238,8 @@ def lib():
         "sb200_fstore_merge_owned": (C.c_int, [vp, i32, vp, vp, i32]),
         "sb200_fstore_set_storage_type": (C.c_int, [vp, i32]),
         "sb200_fstore_get_storage_type": (C.c_int, [vp, C.POINTER(i32)]),
+        "sb200_fstore_associate_wasted": (i64, [vp, vp, i64, u64, vp, vp, vp, vp, vp, vp, i32, vp, vp, vp, vp, vp, vp, vp,
+                                                vp, vp, vp]),
         "sb200_host_alloc": (vp, [C.c_size_t]),
         "sb200_host_free": (None, [vp]),
     }

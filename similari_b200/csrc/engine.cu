@@ -22,6 +22,7 @@
 #include "sb_blob.cuh"
 #include "sb_engine.cuh"
 #include "sb_host.cuh"
+#include "sb_wstore.cuh"
 
 #include <atomic>
 
@@ -1738,6 +1739,47 @@ int64_t sb200_wasted(sb200_tracker* t, int64_t cap, uint64_t* ids, uint64_t* sce
   return n;
 }
 
+// the first n records of the wasted buffer and their box histories into `o`, as sb200_wasted_history returns them
+static int read_wasted(sb200_tracker* t, int64_t n, const sb::WastedOut& o) {
+  cudaStream_t st = t->stream;
+  const int32_t history_cap = o.history_cap;
+  std::vector<uint32_t> hlen((size_t)n);
+  if (o.ids) CU(cudaMemcpyAsync(o.ids, t->wb.id, 8 * n, cudaMemcpyDeviceToHost, st));
+  if (o.scene_ids) CU(cudaMemcpyAsync(o.scene_ids, t->wb.scene, 8 * n, cudaMemcpyDeviceToHost, st));
+  if (o.epochs) CU(cudaMemcpyAsync(o.epochs, t->wb.epoch, 4 * n, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(hlen.data(), t->wb.length, 4 * n, cudaMemcpyDeviceToHost, st));
+  std::vector<float> lastp((size_t)n * 6), lasto((size_t)n * 6);
+  CU(cudaMemcpyAsync(lastp.data(), t->wb.pred, 24 * n, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(lasto.data(), t->wb.obs, 24 * n, cudaMemcpyDeviceToHost, st));
+  const int H = t->hist_len;
+  std::vector<float> hp, ho;
+  if (H > 1 && history_cap > 0) {
+    hp.resize((size_t)n * H * 6); ho.resize((size_t)n * H * 6);
+    CU(cudaMemcpyAsync(hp.data(), t->wb.hist_pred, sizeof(float) * hp.size(), cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(ho.data(), t->wb.hist_obs, sizeof(float) * ho.size(), cudaMemcpyDeviceToHost, st));
+  }
+  CU(cudaStreamSynchronize(st));
+  if (o.lengths) memcpy(o.lengths, hlen.data(), 4 * (size_t)n);
+  if (o.predicted_boxes) memcpy(o.predicted_boxes, lastp.data(), 24 * (size_t)n);
+  if (o.observed_boxes) memcpy(o.observed_boxes, lasto.data(), 24 * (size_t)n);
+  // rings -> chronological order (oldest first), at most history_cap boxes per track
+  for (int64_t i = 0; i < n; ++i) {
+    const uint32_t len = hlen[(size_t)i];
+    int cnt = (int)std::min<uint32_t>(len, (uint32_t)H);
+    cnt = std::min(cnt, (int)history_cap);
+    if (o.history_counts) o.history_counts[i] = history_cap > 0 ? cnt : 0;
+    for (int c = 0; c < cnt; ++c) {
+      const uint32_t j = len - (uint32_t)cnt + (uint32_t)c;   // observation number
+      const float* sp; const float* so;
+      if (H > 1) { sp = &hp[((size_t)i * H + j % H) * 6]; so = &ho[((size_t)i * H + j % H) * 6]; }
+      else { sp = &lastp[(size_t)i * 6]; so = &lasto[(size_t)i * 6]; }
+      if (o.predicted_history) memcpy(o.predicted_history + ((size_t)i * history_cap + c) * 6, sp, 24);
+      if (o.observed_history) memcpy(o.observed_history + ((size_t)i * history_cap + c) * 6, so, 24);
+    }
+  }
+  return 0;
+}
+
 // sb200_wasted_history, and sb200_wasted_visual when `features` / `feature_present` are given
 static int64_t wasted_records(sb200_tracker* t, int64_t cap, uint64_t* ids, uint64_t* scene_ids, uint32_t* epochs,
                               uint32_t* lengths, float* predicted_boxes, float* observed_boxes, int32_t history_cap,
@@ -1754,40 +1796,9 @@ static int64_t wasted_records(sb200_tracker* t, int64_t cap, uint64_t* ids, uint
   const int64_t n = std::min<int64_t>(cap, t->wasted_count);
   if (n == 0) return 0;
   cudaStream_t st = t->stream;
-  std::vector<uint32_t> hlen((size_t)n);
-  if (ids) CU(cudaMemcpyAsync(ids, t->wb.id, 8 * n, cudaMemcpyDeviceToHost, st));
-  if (scene_ids) CU(cudaMemcpyAsync(scene_ids, t->wb.scene, 8 * n, cudaMemcpyDeviceToHost, st));
-  if (epochs) CU(cudaMemcpyAsync(epochs, t->wb.epoch, 4 * n, cudaMemcpyDeviceToHost, st));
-  CU(cudaMemcpyAsync(hlen.data(), t->wb.length, 4 * n, cudaMemcpyDeviceToHost, st));
-  std::vector<float> lastp((size_t)n * 6), lasto((size_t)n * 6);
-  CU(cudaMemcpyAsync(lastp.data(), t->wb.pred, 24 * n, cudaMemcpyDeviceToHost, st));
-  CU(cudaMemcpyAsync(lasto.data(), t->wb.obs, 24 * n, cudaMemcpyDeviceToHost, st));
-  const int H = t->hist_len;
-  std::vector<float> hp, ho;
-  if (H > 1 && history_cap > 0) {
-    hp.resize((size_t)n * H * 6); ho.resize((size_t)n * H * 6);
-    CU(cudaMemcpyAsync(hp.data(), t->wb.hist_pred, sizeof(float) * hp.size(), cudaMemcpyDeviceToHost, st));
-    CU(cudaMemcpyAsync(ho.data(), t->wb.hist_obs, sizeof(float) * ho.size(), cudaMemcpyDeviceToHost, st));
-  }
-  CU(cudaStreamSynchronize(st));
-  if (lengths) memcpy(lengths, hlen.data(), 4 * (size_t)n);
-  if (predicted_boxes) memcpy(predicted_boxes, lastp.data(), 24 * (size_t)n);
-  if (observed_boxes) memcpy(observed_boxes, lasto.data(), 24 * (size_t)n);
-  // rings -> chronological order (oldest first), at most history_cap boxes per track
-  for (int64_t i = 0; i < n; ++i) {
-    const uint32_t len = hlen[(size_t)i];
-    int cnt = (int)std::min<uint32_t>(len, (uint32_t)H);
-    cnt = std::min(cnt, (int)history_cap);
-    if (history_counts) history_counts[i] = history_cap > 0 ? cnt : 0;
-    for (int c = 0; c < cnt; ++c) {
-      const uint32_t j = len - (uint32_t)cnt + (uint32_t)c;   // observation number
-      const float* sp; const float* so;
-      if (H > 1) { sp = &hp[((size_t)i * H + j % H) * 6]; so = &ho[((size_t)i * H + j % H) * 6]; }
-      else { sp = &lastp[(size_t)i * 6]; so = &lasto[(size_t)i * 6]; }
-      if (predicted_history) memcpy(predicted_history + ((size_t)i * history_cap + c) * 6, sp, 24);
-      if (observed_history) memcpy(observed_history + ((size_t)i * history_cap + c) * 6, so, 24);
-    }
-  }
+  if ((rc = read_wasted(t, n, {ids, scene_ids, epochs, lengths, predicted_boxes, observed_boxes, history_cap,
+                               predicted_history, observed_history, history_counts})))
+    return rc;
   if (want_feat && history_cap > 0) {
     // the records' rings are gathered on the device in the same order, a chunk of records at a time, and copied back once
     const size_t rec_bytes = (size_t)history_cap * t->P.d8 * 4;
@@ -2540,3 +2551,32 @@ void* sb200_host_alloc(size_t bytes) {
 void sb200_host_free(void* p) { if (p) cudaFreeHost(p); }
 
 }  // extern "C"
+
+// =============================================================================================== sb200_fstore_associate_wasted
+// The tracker's side of that call (sb_wstore.cuh); wasted_store.cu holds the call itself.
+namespace sb {
+
+TrackerFeatureInfo tracker_feature_info(sb200_tracker* t) {
+  return {t->device, t->P.is_visual, t->fhist_on, t->P.feature_dim, t->seen_features};
+}
+
+int64_t tracker_collect_wasted(sb200_tracker* t, int64_t cap, const WastedOut& out, std::vector<uint64_t>* ids,
+                               WastedFeatures* feat) {
+  CU(cudaSetDevice(t->device));
+  { int rc_ = t->drain(); if (rc_) return rc_; }
+  int rc = t->run_waste();  // wasted() starts with auto_waste (tracker_api.rs:90-91)
+  if (rc) return rc;
+  const int64_t n = std::min<int64_t>(cap, t->wasted_count);
+  if (n == 0) return 0;
+  ids->resize((size_t)n);
+  WastedOut o = out;
+  o.ids = ids->data();
+  if ((rc = read_wasted(t, n, o))) return rc;
+  if (out.ids) memcpy(out.ids, ids->data(), 8 * (size_t)n);
+  *feat = {t->wb.hblk, t->wb.length, t->ts.hrows, t->ts.hpresent, t->hist_len, t->P.d8, t->stream};
+  return n;
+}
+
+int tracker_drop_wasted(sb200_tracker* t, int64_t n) { return t->drop_wasted_front(n); }
+
+}  // namespace sb

@@ -22,6 +22,7 @@
 #include "sb_blob.cuh"
 #include "sb_fstore.cuh"
 #include "sb_host.cuh"
+#include "sb_wstore.cuh"
 
 namespace {
 
@@ -185,9 +186,11 @@ struct sb200_fstore {
 
   // Puts the request on the device: rows [R][d8] (zero-padded), ids, offsets, row -> item, dest and the initial max_dist.
   // row_src[r] is the row of the caller's column behind request row r; col_rows the rows of a host column to upload.
+  // With `rsrc` there is no column: rsrc writes the rows on the device (row_src gives only their number).
   int upload(const ReqLayout& L, int Q, const uint64_t* qids, const std::vector<int>& qoff, const std::vector<int>& row_src,
-             const std::vector<int>& dest, const Column& col, size_t col_rows) {
-    const bool host_f32 = !col.on_device && ftype == SB200_FEATURE_F32;
+             const std::vector<int>& dest, const Column& col, size_t col_rows, const sb::FsRowSource* rsrc = nullptr) {
+    const bool host_f32 = !rsrc && !col.on_device && ftype == SB200_FEATURE_F32;
+    const bool staged = !rsrc && !host_f32;     // rows built by fs_stage_kernel from the column
     const size_t base = host_f32 ? 0 : L.qid;   // the rows of the other paths are written on the device
     const int D = o.feature_dim, R = (int)row_src.size();
     if (int rc = hreq.ensure(L.total - base)) return rc;
@@ -200,7 +203,7 @@ struct sb200_fstore {
         memcpy(rows + (size_t)r * d8, feats + (size_t)row_src[r] * D, (size_t)D * 4);
         for (int k = D; k < d8; ++k) rows[(size_t)r * d8 + k] = 0.0f;
       }
-    } else {
+    } else if (staged) {
       memcpy(at(L.row_src), row_src.data(), (size_t)R * 4);
     }
     memcpy(at(L.qid), qids, (size_t)Q * 8);
@@ -211,7 +214,7 @@ struct sb200_fstore {
     memcpy(at(L.dest), dest.data(), (size_t)Q * 4);
     *reinterpret_cast<int*>(at(L.maxkey)) = sb::fs_key(-1.0f);   // max_dist starts at -1.0 (topn.rs:78)
     const void* dev_col = col.p;
-    if (!host_f32 && !col.on_device) {   // the raw 2-byte rows: half the bytes of the widened request
+    if (staged && !col.on_device) {   // the raw 2-byte rows: half the bytes of the widened request
       const size_t bytes = col_rows * D * elem();
       if (int rc = hcol.ensure(bytes)) return rc;
       if (int rc = dcol.ensure(bytes)) return rc;
@@ -219,14 +222,18 @@ struct sb200_fstore {
       CU(cudaMemcpyAsync(dcol.p, hcol.p, bytes, cudaMemcpyHostToDevice, st));
       dev_col = dcol.p;
     }
-    if (col.on_device) {   // the column is complete once the caller's stream has reached this point
+    if (staged && col.on_device) {   // the column is complete once the caller's stream has reached this point
       CU(cudaEventRecord(ev_in, col.caller));
       CU(cudaStreamWaitEvent(st, ev_in, 0));
     }
     CU(cudaMemcpyAsync(dreq.as<char>() + base, hreq.p, L.total - base, cudaMemcpyHostToDevice, st));
-    if (!host_f32)
-      sb::fs_launch_stage(ftype, dev_col, reinterpret_cast<const int*>(dreq.as<char>() + L.row_src), R, D, d8,
-                          reinterpret_cast<float*>(dreq.as<char>() + L.rows), st);
+    char* d = dreq.as<char>();
+    if (staged)
+      sb::fs_launch_stage(ftype, dev_col, reinterpret_cast<const int*>(d + L.row_src), R, D, d8,
+                          reinterpret_cast<float*>(d + L.rows), st);
+    if (rsrc)
+      return rsrc->fill(rsrc->ctx, reinterpret_cast<float*>(d + L.rows), reinterpret_cast<const int*>(d + L.qoff),
+                        reinterpret_cast<const int*>(d + L.row_q), R, st);
     return 0;
   }
 
@@ -263,7 +270,6 @@ struct sb200_fstore {
     if (offs[0] != 0) return fail(SB200_ERR_INVALID, "obs_offsets[0] != 0");
     std::unordered_set<uint64_t> seen;
     seen.reserve((size_t)Q * 2);
-    const int K = o.max_observations;
     for (int q = 0; q < Q; ++q) {
       const int n = offs[q + 1] - offs[q];
       if (n <= 0) return fail(SB200_ERR_INVALID, "query %d has no observations", q);
@@ -274,6 +280,12 @@ struct sb200_fstore {
     }
     if (!col.p) return fail(SB200_ERR_INVALID, "features is NULL");
     if (int rc = check_column(col)) return rc;
+    return plan_rows(Q, offs, qoff, row_src);
+  }
+
+  // the newest-K row table of a request, within the pair bound of one distance matrix
+  int plan_rows(int Q, const int32_t* offs, std::vector<int>* qoff, std::vector<int>* row_src) const {
+    const int K = o.max_observations;
     sb::fs_row_table(Q, offs, K, row_src, qoff);
     const long long pairs = (long long)row_src->size() * (long long)hid.size() * K;
     if (pairs > sb::kFsMaxPairs)
@@ -298,9 +310,36 @@ struct sb200_fstore {
       return fail(SB200_ERR_INVALID, "an output is NULL");
     if (int rc = begin()) return rc;
     if (Q == 0) return 0;
+    return launch_queries(Q, qids, qoff, src, col, (size_t)offs[Q], nullptr, counts, winners, weights, track_ids, merged,
+                          assoc);
+  }
+
+  // associate whose request rows `rsrc` writes on the device (sb200_fstore_associate_wasted); offs as for associate
+  int associate_rows(int Q, const uint64_t* qids, const int32_t* offs, const sb::FsRowSource& rsrc, int32_t* counts,
+                     uint64_t* winners, double* weights, uint64_t* track_ids, uint8_t* merged) {
+    std::unordered_set<uint64_t> seen;
+    seen.reserve((size_t)Q * 2);
+    for (int q = 0; q < Q; ++q) {
+      if (!seen.insert(qids[q]).second)
+        return fail(SB200_ERR_INVALID, "query id %llu appears twice in the call", (unsigned long long)qids[q]);
+      if (hpos.count(qids[q]))
+        return fail(SB200_ERR_INVALID, "query id %llu is already stored", (unsigned long long)qids[q]);
+    }
+    std::vector<int> qoff, src;
+    if (int rc = plan_rows(Q, offs, &qoff, &src)) return rc;
+    if (int rc = begin()) return rc;
+    if (Q == 0) return 0;
+    return launch_queries(Q, qids, qoff, src, Column{nullptr, false, nullptr}, 0, &rsrc, counts, winners, weights,
+                          track_ids, merged, true);
+  }
+
+  // the device part of search / associate, after every check: upload, distances, TopN, apply, results
+  int launch_queries(int Q, const uint64_t* qids, const std::vector<int>& qoff, const std::vector<int>& src,
+                     const Column& col, size_t col_rows, const sb::FsRowSource* rsrc, int32_t* counts,
+                     uint64_t* winners, double* weights, uint64_t* track_ids, uint8_t* merged, bool assoc) {
     const int R = (int)src.size(), topn = o.topn, K = o.max_observations;
     const long long live = (long long)hid.size(), S = live * K;
-    const ReqLayout L(Q, R, d8, col.on_device || ftype != SB200_FEATURE_F32);
+    const ReqLayout L(Q, R, d8, !rsrc && (col.on_device || ftype != SB200_FEATURE_F32));
     const ResLayout RL(Q, topn);
     if (int rc = hres.ensure(RL.total)) return rc;
     if (int rc = dres.ensure(RL.total)) return rc;
@@ -312,7 +351,7 @@ struct sb200_fstore {
     if (int rc = dist.ensure((size_t)std::max<long long>((long long)R * S, 1) * 4)) return rc;
     if (assoc)
       if (int rc = reserve(hid.size() + (size_t)Q)) return rc;
-    if (int rc = upload(L, Q, qids, qoff, src, std::vector<int>(Q, -1), col, (size_t)offs[Q])) return rc;
+    if (int rc = upload(L, Q, qids, qoff, src, std::vector<int>(Q, -1), col, col_rows, rsrc)) return rc;
     const sb::FsStore s = view();
     const sb::FsCall c = call_view(L, Q, R, &RL);
     CU(cudaEventRecord(ev[0], st));
@@ -1001,3 +1040,20 @@ int sb200_fstore_load(const void* buf, uint64_t bytes, int32_t device, sb200_fst
 }
 
 }  // extern "C"
+
+// =============================================================================================== sb200_fstore_associate_wasted
+// The store's side of that call (sb_wstore.cuh); wasted_store.cu holds the call itself.
+namespace sb {
+
+void fstore_info(sb200_fstore* s, int* device, int* feature_dim, int* topn) {
+  *device = s->o.device;
+  *feature_dim = s->o.feature_dim;
+  *topn = s->o.topn;
+}
+
+int fstore_associate_rows(sb200_fstore* s, int Q, const uint64_t* qids, const int32_t* offs, const FsRowSource& src,
+                          int32_t* counts, uint64_t* winners, double* weights, uint64_t* track_ids, uint8_t* merged) {
+  return s->associate_rows(Q, qids, offs, src, counts, winners, weights, track_ids, merged);
+}
+
+}  // namespace sb

@@ -826,6 +826,50 @@ class FeatureStore:
             raise ValueError("dest_ids and src_ids must have the same length")
         check(self._L.sb200_fstore_merge_owned(self._h, len(d), ptr(d), ptr(s), int(bool(remove))))
 
+    def associate_wasted(self, tracker, cap=None, id_offset=0, history_cap=None):
+        """sb200_fstore_associate_wasted: collects up to `cap` wasted records of the visual `tracker` (None: every record,
+        in one call) as tracker.wasted_history(cap, history_cap) does, and associates each record's present history
+        features (oldest first) with this store under the id ids[i] + id_offset, as one associate() call would; the
+        features never leave the device.  Returns the wasted_history() dict plus, per record, feature_counts,
+        queried (bool) and the associate outputs counts / winners / weights / track_ids / merged (0 where not
+        queried).  The tracker needs its feature history on (set_feature_history)."""
+        if not isinstance(tracker, Tracker):
+            raise TypeError("tracker must be an engine.Tracker")
+        id_offset = int(id_offset)
+        if not 0 <= id_offset < 1 << 64:
+            raise ValueError("id_offset must lie in [0, 2^64)")
+        H = int(history_cap if history_cap is not None else max(1, min(64, tracker.opts.history_length or 64)))
+        if H < 0:
+            raise ValueError("history_cap must be >= 0")
+        if cap is None:
+            cap = self._wasted_pending(tracker)
+        cap = int(cap)
+        if cap < 0:
+            raise ValueError("cap must be >= 0")
+        n_out, t = max(1, cap), self.topn
+        ids, sc = np.zeros(n_out, np.uint64), np.zeros(n_out, np.uint64)
+        ep, ln = np.zeros(n_out, np.uint32), np.zeros(n_out, np.uint32)
+        pr, ob = np.zeros((n_out, 6), np.float32), np.zeros((n_out, 6), np.float32)
+        hp, ho = np.zeros((n_out, max(1, H), 6), np.float32), np.zeros((n_out, max(1, H), 6), np.float32)
+        hc, fc, qd = np.zeros(n_out, np.int32), np.zeros(n_out, np.int32), np.zeros(n_out, np.uint8)
+        cn, wn, wt = np.zeros(n_out, np.int32), np.zeros((n_out, t), np.uint64), np.zeros((n_out, t), np.float64)
+        ti, mg = np.zeros(n_out, np.uint64), np.zeros(n_out, np.uint8)
+        n = check(self._L.sb200_fstore_associate_wasted(
+            self._h, tracker._h, cap, id_offset, ptr(ids), ptr(sc), ptr(ep), ptr(ln), ptr(pr), ptr(ob), H, ptr(hp),
+            ptr(ho), ptr(hc), ptr(fc), ptr(qd), ptr(cn), ptr(wn), ptr(wt), ptr(ti), ptr(mg)))
+        return {"ids": ids[:n], "scene_ids": sc[:n], "epochs": ep[:n], "lengths": ln[:n], "predicted": pr[:n],
+                "observed": ob[:n], "predicted_history": [hp[i, : hc[i]].copy() for i in range(n)],
+                "observed_history": [ho[i, : hc[i]].copy() for i in range(n)], "feature_counts": fc[:n],
+                "queried": qd[:n].astype(bool), "counts": cn[:n], "winners": wn[:n], "weights": wt[:n],
+                "track_ids": ti[:n], "merged": mg[:n]}
+
+    @staticmethod
+    def _wasted_pending(tracker):
+        """An upper bound of the records the next collection of `tracker` can return: every live track and every
+        uncollected wasted record holds one block of the feature-history pool."""
+        pool = tracker.feature_history_pool()
+        return pool["handed_out"] - pool["free"]
+
     def fetch(self, ids, remove=False):
         """(counts[n], features[n][max_observations][feature_dim]) of the tracks `ids`, oldest observation first (count 0:
         not stored); remove=True takes them out of the store (fetch_tracks)."""
