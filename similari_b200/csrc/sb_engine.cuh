@@ -54,9 +54,12 @@ inline float screen_rel_err(int d) {
 //      is at most 2^-10 (1 + u) (sum|a_i| + sum|b_i|) + d 2^-20 <= 2^-10 (1 + u) sqrt(d) (||a|| + ||b||) + d 2^-20; both
 //      scaled norms are >= max|x| >= 224, so relative to ||a|| ||b|| it is <= 2 (1 + u) sqrt(d) 2^-10 / 224 + d 2^-20 / 224^2.
 //   3. Accumulation.  Products of e4m3 values are exact in fp32.  The FP8 tensor cores of the H100 are publicly reported to
-//      keep only about 14 bits when they add a k32 group of products to the accumulator.  Model (NOT measured here, wide
-//      margin): every k32 step aligns its 32 products and the accumulator to the largest of them and truncates each to
-//      13 significant bits, then rounds the sum.  Each of those 34 operations errs by less than 2^-12 of the step's largest
+//      keep only about 14 bits when they add a k32 group of products to the accumulator.  Model (one bit narrower than
+//      the hardware): every k32 step aligns its 32 products and the accumulator to the largest of them and truncates each
+//      to 13 significant bits, then rounds the sum.  tests/gpu_probe/fp8_wgmma_probe.cu measures it on an H100 (80 GB): an
+//      accumulator of 2^16 keeps a next-step product of 8 and drops one of 4 (14 bits), and on the constructions of
+//      tests/screen_fp8_constructions.py the error stays below 10.6 * 2^-12 of the largest step term per k32 step.  Each of
+//      those 34 operations errs by less than 2^-12 of the step's largest
 //      term, which is at most sum|a~_i b~_i| <= (1 + u)^2 ||a|| ||b|| (plus the floor, covered by the 1.01 below), so
 //      ceil(d / 32) steps add at most ceil(d / 32) * 34 * 2^-12 * (1 + u)^2 * 1.01.
 // At d = 512 the sum is 0.129 + 0.0003 + 0.150 = 0.280: on unit-norm features the Euclidean screen keeps d <= 0.7 pairs

@@ -214,8 +214,10 @@ VIS_KW = dict(positional_kind=1, iou_threshold=0.3, max_idle_epochs=5, visual_mi
 def test_tracker_screen_keeps_pairs_on_the_threshold(eng, oracle, vis, monkeypatch):
     """The tracker's BF16 rows come from cand_norm_kernel and feat_store, not from the operator's conversion.  Each of four
     scenes holds a track whose three observations are b and, one frame later, a detection a far from it: the threshold is
-    the oracle's value for (a, b), so only a visual match keeps the track's id."""
-    monkeypatch.setenv("SB200_VIS_KERNEL", "tc")
+    the oracle's value for (a, b), so only a visual match keeps the track's id.  The tracker screens D = 512 on e4m3 by
+    default; tc16 keeps every frame on the BF16 screen this pair is built for (test_gpu_screen_fp8_bounds.py covers the
+    e4m3 rows)."""
+    monkeypatch.setenv("SB200_VIS_KERNEL", "tc16")
     d, n = 512, 130
     seed, kind = TRACKER_PAIRS[vis]
     a, b = screen_pair(seed, d, 1.0, kind)
@@ -240,6 +242,8 @@ def test_tracker_screen_keeps_pairs_on_the_threshold(eng, oracle, vis, monkeypat
     g = _drive(eng, oracle, dict(kind=3, visual_kind=vis, visual_threshold=thr, feature_dim=d, visual_max_observations=3,
                                  visual_min_votes=1, **VIS_KW), frames)
     assert g.work_counters()["tc_frames"] >= 3
+    sc = g.screen_counters()
+    assert sc["bf16_frames"] >= 3 and sc["fp8_frames"] == 0, sc
 
 
 # ------------------------------------------------------------------------------------ degenerate features, dense selection
