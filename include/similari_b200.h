@@ -273,7 +273,8 @@ int sb200_last_kernel_ms(sb200_tracker* t, float* out2);
 
 /* ---- state blob: save / restore a tracker, move scenes between trackers and GPUs (no reference counterpart: the
  * reference's state lives in host memory).  One versioned binary format; DESIGN.md section 3b describes it.
- * `dst` / `src` may be host memory or device memory on any device.  Every entry first waits for the frames in flight
+ * `dst` / `src` may be host memory or device memory on any device, at any address: a device blob that is not 16-byte
+ * aligned, or not on the tracker's device, goes through a device copy.  Every entry first waits for the frames in flight
  * (an error of an asynchronous frame is returned there).  Size query: with dst == NULL or cap too small, save and export
  * write nothing, set *bytes to the size they need and return SB200_ERR_CAPACITY.  A rejected call changes nothing.
  * Stream order of a device blob: save, export and import are ordered after what the stream named with
@@ -592,7 +593,9 @@ int64_t sb200_fstore_associate_wasted(sb200_fstore* s, sb200_tracker* t, int64_t
  * observation), feat[live][max_observations][d8] (rows as stored, in the storage type: 4 or 2 bytes per element;
  * observation j of a track sits in ring slot (start + j) % max_observations).  Ring slots a track has never filled are
  * written as zeros, so two stores that hold the same tracks in the same ring state give byte-equal blobs.  The magic
- * differs from the tracker blob's: each loader refuses the other's blob.
+ * differs from the tracker blob's: each loader refuses the other's blob.  A blob may sit in host memory or in device
+ * memory on any device, at any address: a device blob that is not 16-byte aligned, or not on the store's device, goes
+ * through a device copy.
  * storage_type was a reserved 0 before 2-byte stores existed, which is SB200_FEATURE_F32: older blobs load unchanged, and
  * an f32 store's blob is what it was.  A library from before 2-byte stores refuses a non-empty 2-byte store's blob by
  * its feat section size (half of what an f32 store needs), so it cannot misread one; an empty 2-byte store's blob has

@@ -1997,7 +1997,6 @@ constexpr uint32_t kBlobMagic = 0x42534253u;   // "SBSB"
 constexpr uint32_t kBlobVersion = 1;
 constexpr uint32_t kBlobTracker = 1, kBlobScenes = 2;
 constexpr int kMaxSections = 48;
-constexpr uint64_t kSecAlign = 256;
 
 struct BlobHeader {
   uint32_t magic, version, type, n_sections;
@@ -2042,21 +2041,6 @@ int64_t tracker_rows(const BlobHeader& h, int rows) {
   return rows == kRowWasted ? h.wasted_count : (rows == kRowHistTop ? h.hpool_top : h.hpool_free);
 }
 
-// header sections from their sizes; returns the blob's total size
-uint64_t lay_out(BlobHeader& h, const std::vector<uint64_t>& sec) {
-  uint64_t off = (sizeof(BlobHeader) + kSecAlign - 1) / kSecAlign * kSecAlign;
-  h.n_sections = (uint32_t)sec.size();
-  for (size_t i = 0; i < sec.size(); ++i) {
-    h.sec_off[i] = off;
-    h.sec_bytes[i] = sec[i];
-    off += (sec[i] + kSecAlign - 1) / kSecAlign * kSecAlign;
-  }
-  return off;
-}
-
-using sb::blob_device;
-using sb::host_copy;
-
 struct SlotRows { int slot, n, blk, fre; };
 
 // Pack (dir 0: store -> blob) or unpack (dir 1: blob -> store) of the store columns of `rows` (one per scene, in blob
@@ -2066,11 +2050,6 @@ int move_store(sb200_tracker* t, int dir, uint32_t type, const BlobHeader& h, ch
                int hist_base) {
   const size_t tc = (size_t)t->track_cap;
   std::vector<sb::XferSeg> segs;
-  auto add = [&](char* store, char* blob, uint64_t bytes) {
-    if (bytes == 0) return;
-    if (dir == 0) segs.push_back({store, blob, bytes});
-    else segs.push_back({blob, store, bytes});
-  };
   const std::vector<Col> cols = blob_cols(t, type);
   size_t hist_sec = 0;   // scene blob: the history rows, then the present bytes, of the live tracks (launch_xfer_hist)
   for (size_t c = 0; c < cols.size(); ++c) {
@@ -2081,13 +2060,14 @@ int move_store(sb200_tracker* t, int dir, uint32_t type, const BlobHeader& h, ch
       continue;
     }
     if (col.rows >= kRowWasted) {
-      add(col.buf->as<char>(), sec, (uint64_t)tracker_rows(h, col.rows) * col.w);
+      sb::add_segment(segs, dir, col.buf->as<char>(), sec, (uint64_t)tracker_rows(h, col.rows) * col.w);
       continue;
     }
     int64_t pre = 0;
     for (const SlotRows& r : rows) {
       const int64_t cnt = col.rows == kRowTrack ? r.n : (col.rows == kRowBlock ? r.blk : r.fre);
-      add(col.buf->as<char>() + (size_t)r.slot * tc * col.w, sec + (uint64_t)pre * col.w, (uint64_t)cnt * col.w);
+      sb::add_segment(segs, dir, col.buf->as<char>() + (size_t)r.slot * tc * col.w, sec + (uint64_t)pre * col.w,
+                      (uint64_t)cnt * col.w);
       pre += cnt;
     }
   }
@@ -2218,37 +2198,19 @@ int save_blob(sb200_tracker* t, uint32_t type, const std::vector<int>& slots, vo
   int rc = 0;
   h.id_counter = read_id_counter(t, &rc);
   if (rc) return rc;
-  const uint64_t total = lay_out(h, section_bytes(t, type, h.n_scenes, h.live_total, h.blk_total, h.free_total,
-                                                  h.wasted_count, h.hpool_top, h.hpool_free));
-  h.total_bytes = total;
-  *bytes = (size_t)total;
-  if (!dst || cap < total) return fail(SB200_ERR_CAPACITY, "the blob needs %llu bytes", (unsigned long long)total);
-  const int where = blob_device(dst);
-  DBuf tmp;
-  char* dblob = static_cast<char*>(dst);
-  if (where != t->device) {
-    if ((rc = tmp.ensure(total))) return rc;
-    dblob = tmp.as<char>();
-  }
-  CU(cudaMemcpyAsync(dblob, &h, sizeof(h), cudaMemcpyHostToDevice, t->stream));
-  {   // the alignment gaps after the header and every section are zero (equal states give equal blobs)
-    uint64_t end = sizeof(h);
-    for (uint32_t i = 0; i <= h.n_sections; ++i) {
-      const uint64_t next = i < h.n_sections ? h.sec_off[i] : total;
-      if (next > end) CU(cudaMemsetAsync(dblob + end, 0, next - end, t->stream));
-      if (i < h.n_sections) end = h.sec_off[i] + h.sec_bytes[i];
-    }
-  }
-  if (!table.empty())
-    CU(cudaMemcpyAsync(dblob + h.sec_off[0], table.data(), table.size() * sizeof(BlobScene), cudaMemcpyHostToDevice, t->stream));
-  if ((rc = move_store(t, 0, type, h, dblob, rows, 0))) return rc;
-  if (where == t->device) return 0;
-  if (where >= 0) {
-    CU(cudaMemcpyPeerAsync(dst, where, dblob, t->device, total, t->stream));
-    CU(cudaStreamSynchronize(t->stream));
-    return 0;
-  }
-  return host_copy(t->stream, dst, dblob, total, true);
+  const std::vector<uint64_t> sec = section_bytes(t, type, h.n_scenes, h.live_total, h.blk_total, h.free_total,
+                                                  h.wasted_count, h.hpool_top, h.hpool_free);
+  h.n_sections = (uint32_t)sec.size();
+  sb::lay_out(h, sec.data(), h.n_sections);
+  *bytes = (size_t)h.total_bytes;
+  if (!dst || cap < h.total_bytes)
+    return fail(SB200_ERR_CAPACITY, "the blob needs %llu bytes", (unsigned long long)h.total_bytes);
+  return sb::write_blob(dst, t->device, t->stream, h, h.n_sections, [&](char* p) {
+    if (!table.empty())
+      CU(cudaMemcpyAsync(p + h.sec_off[0], table.data(), table.size() * sizeof(BlobScene), cudaMemcpyHostToDevice,
+                         t->stream));
+    return move_store(t, 0, type, h, p, rows, 0);
+  });
 }
 
 // Orders the tracker's work after what the caller's stream (sb200_tracker_set_stream) holds now, as predict does: a device
@@ -2294,14 +2256,7 @@ int parse_blob(const void* src, size_t bytes, uint32_t want_type, cudaStream_t s
                                                            : "a scene blob: use sb200_scenes_import");
   if (h->total_bytes > bytes) return fail(SB200_ERR_INVALID, "the blob is truncated (%zu of %llu bytes)", bytes, (unsigned long long)h->total_bytes);
   if (h->n_sections < 1 || h->n_sections > (uint32_t)kMaxSections) return fail(SB200_ERR_INVALID, "bad section count");
-  // sections in order, aligned as the writer lays them out (the kernels read them with 16-byte accesses), disjoint
-  uint64_t end = sizeof(BlobHeader);
-  for (uint32_t i = 0; i < h->n_sections; ++i) {
-    if (h->sec_off[i] < end || h->sec_off[i] > h->total_bytes || h->sec_bytes[i] > h->total_bytes - h->sec_off[i])
-      return fail(SB200_ERR_INVALID, "section %u lies outside the blob or overlaps the one before", i);
-    if (h->sec_off[i] % kSecAlign != 0) return fail(SB200_ERR_INVALID, "section %u is not aligned", i);
-    end = h->sec_off[i] + h->sec_bytes[i];
-  }
+  if (int rc = sb::check_section_table(*h, h->n_sections)) return rc;
   if (h->n_scenes < 0 || h->live_total < 0 || h->blk_total < 0 || h->free_total < 0 || h->wasted_count < 0 ||
       h->revealed < 0 || h->revealed > h->wasted_count || h->hpool_top < 0 || h->hpool_free < 0 || h->hpool_free > h->hpool_top ||
       h->hpool_cap < 0 || (h->hpool_cap > 0 && h->hpool_cap < h->hpool_top) ||
@@ -2336,22 +2291,6 @@ int check_sections(sb200_tracker* t, const BlobHeader& h) {
   for (size_t i = 0; i < sec.size(); ++i)
     if (sec[i] != h.sec_bytes[i]) return fail(SB200_ERR_INVALID, "section %zu holds %llu bytes, %llu expected", i,
                                               (unsigned long long)h.sec_bytes[i], (unsigned long long)sec[i]);
-  return 0;
-}
-
-// the blob on the tracker's device: `src` itself, or a copy in `tmp`
-int blob_on_device(sb200_tracker* t, const void* src, size_t bytes, DBuf& tmp, const char** out) {
-  const int where = blob_device(src);
-  if (where == t->device) { *out = static_cast<const char*>(src); return 0; }
-  int rc = tmp.ensure(bytes);
-  if (rc) return rc;
-  if (where >= 0) {
-    CU(cudaMemcpyPeerAsync(tmp.p, t->device, src, where, bytes, t->stream));
-    CU(cudaStreamSynchronize(t->stream));
-  } else if ((rc = host_copy(t->stream, const_cast<void*>(src), tmp.p, bytes, false))) {
-    return rc;
-  }
-  *out = tmp.as<const char>();
   return 0;
 }
 
@@ -2405,7 +2344,7 @@ int sb200_tracker_load(const void* src, size_t bytes, int32_t device, sb200_trac
   if ((rc = t->b_idc.ensure(8))) return rc;
   const char* dblob = nullptr;
   DBuf tmp;
-  if ((rc = blob_on_device(t, src, (size_t)h.total_bytes, tmp, &dblob))) return rc;
+  if ((rc = sb::blob_on_device(src, h.total_bytes, t->device, t->stream, tmp, &dblob))) return rc;
   if ((rc = check_indices(t, h.type, h, dblob, table))) return rc;
   std::vector<SlotRows> rows(table.size());
   std::vector<sb::XferSlot> st(table.size());
@@ -2512,7 +2451,7 @@ int sb200_scenes_import(sb200_tracker* t, const void* src, size_t bytes) {
     return rc;
   const char* dblob = nullptr;
   DBuf tmp;
-  if ((rc = blob_on_device(t, src, (size_t)h.total_bytes, tmp, &dblob))) return rc;
+  if ((rc = sb::blob_on_device(src, h.total_bytes, t->device, t->stream, tmp, &dblob))) return rc;
   if ((rc = check_indices(t, h.type, h, dblob, table))) return rc;
   std::vector<SlotRows> rows(table.size());
   std::vector<sb::XferSlot> st(table.size());

@@ -4,10 +4,11 @@
 // and downloads its results once.  Everything a call can reject is checked before anything is launched or changed.
 // The request rows reach the device in one of two ways: an f32 host column is staged row by row in the pinned buffer; a
 // 2-byte host column (uploaded raw) and a device column (read in place) go through fs_stage_kernel.  The store blob
-// (sb200_fstore_save / _load) shares the trackers' copy machinery (sb_blob.cuh).  The owned calls (search_owned,
-// merge_owned) take stored tracks: their rows never leave the device, and the host reads back only the counts and ring
-// starts of the tracks they touch.  The stored rows are f32, binary16 or bfloat16 (stype, sb200_fstore_set_storage_type);
-// row_bytes() is the size of one stored row, and nothing else on the host depends on the storage type.
+// (sb200_fstore_save / _load) shares the trackers' section layout, placement and copy machinery (sb_blob.cuh).  The
+// owned calls (search_owned, merge_owned) take stored tracks: their rows never leave the device, and the host reads back
+// only the counts and ring starts of the tracks they touch.  The stored rows are f32, binary16 or bfloat16 (stype,
+// sb200_fstore_set_storage_type); row_bytes() is the size of one stored row, and nothing else on the host depends on the
+// storage type.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -74,9 +75,7 @@ struct Column {
 };
 
 using BlobHeader = sb200_fstore_blob_header;
-constexpr uint64_t kSecAlign = SB200_FSTORE_BLOB_ALIGN;
 enum { kSecIds, kSecCnt, kSecStart, kSecFeat };
-uint64_t sec_align(uint64_t v) { return (v + kSecAlign - 1) / kSecAlign * kSecAlign; }
 
 bool known_type(int t) { return t == SB200_FEATURE_F32 || t == SB200_FEATURE_F16 || t == SB200_FEATURE_BF16; }
 size_t type_bytes(int t) { return t == SB200_FEATURE_F32 ? 4 : 2; }
@@ -720,32 +719,12 @@ struct sb200_fstore {
   }
 
   // ---- the store blob (layout: include/similari_b200.h)
-  uint64_t lay_out(BlobHeader* h) const {
-    const uint64_t live = hid.size();
-    const uint64_t sec[SB200_FSTORE_BLOB_SECTIONS] = {live * 8, live * 4, live * 4,
-                                                      live * o.max_observations * row_bytes()};
-    uint64_t off = sec_align(sizeof(BlobHeader));
-    for (int i = 0; i < SB200_FSTORE_BLOB_SECTIONS; ++i) {
-      h->sec_off[i] = off;
-      h->sec_bytes[i] = sec[i];
-      off += sec_align(sec[i]);
-    }
-    return off;
-  }
-
-  // the kernels that read or write a blob's sections use 16-byte accesses; any other device blob goes through a copy
-  static bool in_place_ok(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
-
   // the four columns and their sections of a blob on this device: dir 0 packs, dir 1 unpacks
   int move_columns(int dir, const BlobHeader& h, char* dblob) {
     char* col[SB200_FSTORE_BLOB_SECTIONS] = {ids.as<char>(), cnt.as<char>(), start.as<char>(), feat.as<char>()};
     std::vector<sb::XferSeg> segs;
-    for (int i = 0; i < SB200_FSTORE_BLOB_SECTIONS; ++i) {
-      if (h.sec_bytes[i] == 0) continue;
-      char* sec = dblob + h.sec_off[i];
-      if (dir == 0) segs.push_back({col[i], sec, h.sec_bytes[i]});
-      else segs.push_back({sec, col[i], h.sec_bytes[i]});
-    }
+    for (int i = 0; i < SB200_FSTORE_BLOB_SECTIONS; ++i)
+      sb::add_segment(segs, dir, col[i], dblob + h.sec_off[i], h.sec_bytes[i]);
     return sb::copy_segments(segs, num_sms, st);
   }
 
@@ -756,38 +735,23 @@ struct sb200_fstore {
     h.metric = o.metric; h.distance_filter = o.distance_filter; h.max_observations = o.max_observations;
     h.feature_dim = o.feature_dim; h.topn = o.topn; h.max_distance = o.max_distance; h.min_votes = o.min_votes;
     h.d8 = d8; h.feature_type = ftype; h.storage_type = stype; h.live = (int64_t)hid.size();
-    const uint64_t total = h.total_bytes = lay_out(&h);
-    *bytes = total;
+    const uint64_t live = hid.size();
+    const uint64_t sec[SB200_FSTORE_BLOB_SECTIONS] = {live * 8, live * 4, live * 4,
+                                                      live * o.max_observations * row_bytes()};
+    sb::lay_out(h, sec, SB200_FSTORE_BLOB_SECTIONS);
+    *bytes = h.total_bytes;
     if (!dst) return 0;
-    if (cap_bytes < total) return fail(SB200_ERR_CAPACITY, "the blob needs %llu bytes", (unsigned long long)total);
+    if (cap_bytes < h.total_bytes)
+      return fail(SB200_ERR_CAPACITY, "the blob needs %llu bytes", (unsigned long long)h.total_bytes);
     CU(cudaSetDevice(o.device));
-    const int where = sb::blob_device(dst);
-    const bool in_place = where == o.device && in_place_ok(dst);
-    DBuf tmp;
-    char* dblob = static_cast<char*>(dst);
-    if (!in_place) {
-      if (int rc = tmp.ensure(total)) return rc;
-      dblob = tmp.as<char>();
-    }
-    CU(cudaMemcpyAsync(dblob, &h, sizeof(h), cudaMemcpyHostToDevice, st));
-    uint64_t end = sizeof(h);   // the gaps after the header and every section are zero (equal states give equal blobs)
-    for (int i = 0; i <= SB200_FSTORE_BLOB_SECTIONS; ++i) {
-      const uint64_t next = i < SB200_FSTORE_BLOB_SECTIONS ? h.sec_off[i] : total;
-      if (next > end) CU(cudaMemsetAsync(dblob + end, 0, next - end, st));
-      if (i < SB200_FSTORE_BLOB_SECTIONS) end = h.sec_off[i] + h.sec_bytes[i];
-    }
-    if (int rc = move_columns(0, h, dblob)) return rc;
-    sb::fs_launch_blob_scrub(stype, dblob + h.sec_off[kSecFeat], cnt.as<int>(), start.as<int>(), (int)h.live,
-                             o.max_observations, d8, st);
-    CU(cudaStreamSynchronize(st));
-    CU(cudaGetLastError());
-    if (in_place) return 0;
-    if (where >= 0) {
-      CU(cudaMemcpyPeerAsync(dst, where, dblob, o.device, total, st));
+    return sb::write_blob(dst, o.device, st, h, SB200_FSTORE_BLOB_SECTIONS, [&](char* p) {
+      if (int rc = move_columns(0, h, p)) return rc;
+      sb::fs_launch_blob_scrub(stype, p + h.sec_off[kSecFeat], cnt.as<int>(), start.as<int>(), (int)h.live,
+                               o.max_observations, d8, st);
       CU(cudaStreamSynchronize(st));
+      CU(cudaGetLastError());
       return 0;
-    }
-    return sb::host_copy(st, dst, dblob, total, true);
+    });
   }
 
   // fills a store fresh from sb200_fstore_create with the checked blob `h` at `src`
@@ -798,19 +762,9 @@ struct sb200_fstore {
     stype = h.storage_type;
     if (live == 0) return 0;
     if (int rc = reserve((size_t)live)) return rc;
-    const int where = sb::blob_device(src);
     DBuf tmp;
-    char* dblob = const_cast<char*>(static_cast<const char*>(src));
-    if (where != o.device || !in_place_ok(src)) {
-      if (int rc = tmp.ensure(h.total_bytes)) return rc;
-      dblob = tmp.as<char>();
-      if (where >= 0) {
-        CU(cudaMemcpyPeerAsync(dblob, o.device, src, where, h.total_bytes, st));
-        CU(cudaStreamSynchronize(st));
-      } else if (int rc = sb::host_copy(st, const_cast<void*>(src), dblob, h.total_bytes, false)) {
-        return rc;
-      }
-    }
+    const char* dblob = nullptr;
+    if (int rc = sb::blob_on_device(src, h.total_bytes, o.device, st, tmp, &dblob)) return rc;
     // counts and ring starts index the rows in every later kernel: checked before anything is copied into the store
     int bad[2] = {0, 0};
     if (int rc = gpos.ensure(sizeof(bad))) return rc;
@@ -822,7 +776,7 @@ struct sb200_fstore {
     CU(cudaGetLastError());
     if (bad[0]) return fail(SB200_ERR_INVALID, "the blob holds %d cnt entries outside 1..%d", bad[0], K);
     if (bad[1]) return fail(SB200_ERR_INVALID, "the blob holds %d start entries outside 0..%d", bad[1], K - 1);
-    if (int rc = move_columns(1, h, dblob)) return rc;
+    if (int rc = move_columns(1, h, const_cast<char*>(dblob))) return rc;
     hid = std::move(blob_ids);
     for (size_t p = 0; p < hid.size(); ++p) hpos[hid[p]] = (int)p;
     return 0;
@@ -1013,16 +967,11 @@ int sb200_fstore_load(const void* buf, uint64_t bytes, int32_t device, sb200_fst
   const uint64_t want[SB200_FSTORE_BLOB_SECTIONS] = {live * 8, live * 4, live * 4,
                                                      live * h.max_observations * h.d8 * type_bytes(h.storage_type)};
   static const char* const kName[SB200_FSTORE_BLOB_SECTIONS] = {"ids", "cnt", "start", "feat"};
-  uint64_t end = sizeof(BlobHeader);
-  for (int i = 0; i < SB200_FSTORE_BLOB_SECTIONS; ++i) {
-    if (h.sec_off[i] % kSecAlign != 0) return fail(SB200_ERR_INVALID, "section %s is not 256-byte aligned", kName[i]);
-    if (h.sec_off[i] < end || h.sec_off[i] > h.total_bytes || h.sec_bytes[i] > h.total_bytes - h.sec_off[i])
-      return fail(SB200_ERR_INVALID, "section %s lies outside the blob or overlaps the one before", kName[i]);
+  if (int rc = sb::check_section_table(h, SB200_FSTORE_BLOB_SECTIONS, kName)) return rc;
+  for (int i = 0; i < SB200_FSTORE_BLOB_SECTIONS; ++i)
     if (h.sec_bytes[i] != want[i])
       return fail(SB200_ERR_INVALID, "section %s holds %llu bytes, %llu expected", kName[i],
                   (unsigned long long)h.sec_bytes[i], (unsigned long long)want[i]);
-    end = h.sec_off[i] + h.sec_bytes[i];
-  }
   std::vector<uint64_t> blob_ids(live);
   if (live) CU(cudaMemcpy(blob_ids.data(), static_cast<const char*>(buf) + h.sec_off[kSecIds], live * 8, cudaMemcpyDefault));
   std::unordered_set<uint64_t> seen;
