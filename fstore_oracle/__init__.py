@@ -21,6 +21,8 @@ _LIB_PATH = os.path.join(_HERE, "libfstore_oracle.so")
 _ORACLE_DIR = os.path.dirname(os.path.abspath(oracle.__file__))
 
 EUCLIDEAN, COSINE = 0, 1
+# track attribute rules (feature_store.cpp): None = no attributes
+GATES = {None: 0, "same_source": 1, "any_source": 2}
 
 
 def build(force: bool = False) -> str:
@@ -55,6 +57,11 @@ def lib():
             "ofs_topn_voting": (C.c_int, [f32, i32, i32, i32, vp, vp, vp, vp, vp, vp]),
             "ofs_search_owned": (C.c_int, [vp, i32, vp, i32, vp, vp, vp, i32]),
             "ofs_merge_owned": (C.c_int, [vp, i32, vp, vp, i32]),
+            "ofs_set_gate": (C.c_int, [vp, i32]),
+            "ofs_add_attr": (C.c_int, [vp, i32, vp, vp, vp, vp, vp]),
+            "ofs_search_attr": (C.c_int, [vp, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, i32]),
+            "ofs_associate_attr": (C.c_int, [vp, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i32]),
+            "ofs_fetch_attr": (i64, [vp, i32, vp, vp, vp, vp]),
         }
         for name, (res, args) in sig.items():
             fn = getattr(L, name)
@@ -110,22 +117,46 @@ class FeatureStore:
     """The oracle's feature track store; same calls and results as similari_b200.engine.FeatureStore."""
 
     def __init__(self, metric=EUCLIDEAN, distance_filter=100.0, max_observations=3, feature_dim=256, topn=1,
-                 max_distance=100.0, min_votes=1, threads=1):
+                 max_distance=100.0, min_votes=1, threads=1, gate=None):
         self._L = lib()
         self.K, self.D, self.topn, self.threads = int(max_observations), int(feature_dim), int(topn), int(threads)
         self._h = self._L.ofs_create(metric, distance_filter, self.K, self.D, self.topn, max_distance, min_votes)
         if not self._h:
             raise ValueError("invalid feature store options")
+        if gate not in GATES:
+            raise ValueError(f"gate must be one of {list(GATES)}")
+        self.gate = gate
+        if self._L.ofs_set_gate(self._h, GATES[gate]):
+            raise ValueError("invalid gate")
+
+    def _attrs(self, n, sources, t_start, t_end):
+        """The three attribute columns of a call: required on a gated store, refused on an ungated one."""
+        given = [a is not None for a in (sources, t_start, t_end)]
+        if self.gate is None:
+            if any(given):
+                raise ValueError("sources / t_start / t_end need a gated store")
+            return None
+        if not all(given):
+            raise ValueError("a gated store needs sources, t_start and t_end")
+        a = (np.ascontiguousarray(sources, dtype=np.uint64), np.ascontiguousarray(t_start, dtype=np.int64),
+             np.ascontiguousarray(t_end, dtype=np.int64))
+        if any(len(x) != n for x in a):
+            raise ValueError("sources / t_start / t_end need one entry per row")
+        return a
 
     def __del__(self):
         if getattr(self, "_h", None):
             self._L.ofs_destroy(self._h)
             self._h = None
 
-    def add(self, ids, features):
+    def add(self, ids, features, sources=None, t_start=None, t_end=None):
         ids = np.ascontiguousarray(ids, dtype=np.uint64)
         f = np.ascontiguousarray(features, dtype=np.float32).reshape(len(ids), self.D)
-        self._L.ofs_add(self._h, len(ids), _p(ids), _p(f))
+        a = self._attrs(len(ids), sources, t_start, t_end)
+        if a is None:
+            self._L.ofs_add(self._h, len(ids), _p(ids), _p(f))
+        elif self._L.ofs_add_attr(self._h, len(ids), _p(ids), *map(_p, a), _p(f)):
+            raise ValueError("invalid add request")
 
     def _queries(self, ids, offsets, features):
         ids = np.ascontiguousarray(ids, dtype=np.uint64)
@@ -136,21 +167,30 @@ class FeatureStore:
                "weights": np.zeros((q, self.topn), np.float64)}
         return ids, offs, f, out
 
-    def search(self, ids, offsets, features):
+    def search(self, ids, offsets, features, sources=None, t_start=None, t_end=None):
         ids, offs, f, out = self._queries(ids, offsets, features)
-        rc = self._L.ofs_search(self._h, len(ids), _p(ids), _p(offs), _p(f), _p(out["counts"]), _p(out["winners"]),
-                                _p(out["weights"]), self.threads)
+        a = self._attrs(len(ids), sources, t_start, t_end)
+        if a is None:
+            rc = self._L.ofs_search(self._h, len(ids), _p(ids), _p(offs), _p(f), _p(out["counts"]),
+                                    _p(out["winners"]), _p(out["weights"]), self.threads)
+        else:
+            rc = self._L.ofs_search_attr(self._h, len(ids), _p(ids), _p(offs), *map(_p, a), _p(f), _p(out["counts"]),
+                                         _p(out["winners"]), _p(out["weights"]), self.threads)
         if rc:
             raise ValueError("invalid search request")
         return out
 
-    def associate(self, ids, offsets, features):
+    def associate(self, ids, offsets, features, sources=None, t_start=None, t_end=None):
         ids, offs, f, out = self._queries(ids, offsets, features)
+        a = self._attrs(len(ids), sources, t_start, t_end)
         out["track_ids"] = np.zeros(len(ids), np.uint64)
         out["merged"] = np.zeros(len(ids), np.uint8)
-        rc = self._L.ofs_associate(self._h, len(ids), _p(ids), _p(offs), _p(f), _p(out["counts"]),
-                                   _p(out["winners"]), _p(out["weights"]), _p(out["track_ids"]), _p(out["merged"]),
-                                   self.threads)
+        res = [_p(out[k]) for k in ("counts", "winners", "weights", "track_ids", "merged")]
+        if a is None:
+            rc = self._L.ofs_associate(self._h, len(ids), _p(ids), _p(offs), _p(f), *res, self.threads)
+        else:
+            rc = self._L.ofs_associate_attr(self._h, len(ids), _p(ids), _p(offs), *map(_p, a), _p(f), *res,
+                                            self.threads)
         if rc:
             raise ValueError("invalid associate request")
         return out
@@ -182,6 +222,14 @@ class FeatureStore:
         feats = np.zeros((len(ids), self.K, self.D), np.float32)
         self._L.ofs_fetch(self._h, len(ids), _p(ids), int(bool(remove)), _p(counts), _p(feats))
         return counts, feats
+
+    def attributes(self, ids):
+        """(sources, t_start, t_end) of the tracks `ids` (0 where an id is not stored) of a gated store."""
+        ids = np.ascontiguousarray(ids, dtype=np.uint64)
+        src, t0, t1 = np.zeros(len(ids), np.uint64), np.zeros(len(ids), np.int64), np.zeros(len(ids), np.int64)
+        if self._L.ofs_fetch_attr(self._h, len(ids), _p(ids), _p(src), _p(t0), _p(t1)) < 0:
+            raise ValueError("attributes() needs a gated store")
+        return src, t0, t1
 
     def size(self):
         return int(self._L.ofs_size(self._h))

@@ -10,6 +10,13 @@
 //   - TopN ties (equal weights) go to the group that appeared first, i.e. the lower store position.
 // It is the parity reference of tests/test_gpu_feature_store.py and the timed CPU baseline of
 // tools/feature_store_bench.py; the product never links it.
+// Track attributes (gate != 0): each track carries the CamTrackingAttributes of examples/track_merging.rs:218-245, a
+// source (camera) id and a [t_start, t_end] window.  compatible = the windows are disjoint (touching counts as disjoint)
+// and, under gate 1, the sources are equal; merge = the hull of the windows.  An incompatible (query, track) pair gives no
+// entries (Track::distances' error, src/track.rs:604-652).  Associate merges a query into its first winner only if it is
+// compatible with the winner's window as extended by the queries merged into it earlier in the call, else the query
+// becomes a new track; merge_owned refuses a call with an incompatible pair (checked in pair order) before anything
+// changes.
 #include <algorithm>
 #include <cmath>
 #include <cstdint>
@@ -95,6 +102,8 @@ void parallel_for(int n, int threads, const std::function<void(int, int)>& fn) {
 struct Track {
   uint64_t id;
   std::vector<std::vector<float>> obs;   // zero-padded to d8, oldest first
+  uint64_t src = 0;                      // attributes of a gated store
+  int64_t t0 = 0, t1 = 0;
 };
 
 }  // namespace
@@ -102,8 +111,20 @@ struct Track {
 struct ofs_store {
   int metric, K, D, d8, topn, min_votes;
   float filter, max_distance;
+  int gate = 0;   // 0: no attributes; 1: windows disjoint and sources equal; 2: windows disjoint
   std::vector<Track> tracks;
   std::unordered_map<uint64_t, size_t> pos;
+
+  // CamTrackingAttributes::compatible (examples/track_merging.rs:222-225); always true without a gate
+  bool compatible(const Track& a, const Track& b) const {
+    if (!gate) return true;
+    return (a.t0 >= b.t1 || a.t1 <= b.t0) && (gate == 2 || a.src == b.src);
+  }
+  // CamTrackingAttributes::merge: the hull of the windows (the destination keeps its source)
+  static void hull(Track& d, const Track& s) {
+    d.t0 = std::min(d.t0, s.t0);
+    d.t1 = std::max(d.t1, s.t1);
+  }
 
   std::vector<float> pad(const float* v) const {
     std::vector<float> out((size_t)d8, 0.0f);
@@ -124,10 +145,13 @@ struct ofs_store {
   }
 
   // TrackBuilder: each observation through add_observation (and optimize), so only the newest K remain
-  std::vector<Track> build_queries(int Q, const uint64_t* ids, const int32_t* offs, const float* feats) const {
+  std::vector<Track> build_queries(int Q, const uint64_t* ids, const int32_t* offs, const float* feats,
+                                   const uint64_t* src = nullptr, const int64_t* t0 = nullptr,
+                                   const int64_t* t1 = nullptr) const {
     std::vector<Track> qs((size_t)Q);
     for (int q = 0; q < Q; ++q) {
       qs[q].id = ids[q];
+      if (src) { qs[q].src = src[q]; qs[q].t0 = t0[q]; qs[q].t1 = t1[q]; }
       for (int r = offs[q]; r < offs[q + 1]; ++r) {
         qs[q].obs.push_back(pad(feats + (size_t)r * D));
         keep_newest(qs[q].obs);
@@ -156,6 +180,7 @@ struct ofs_store {
       for (int q = b; q < e; ++q)
         for (const Track& t : tracks) {
           if (t.id == qs[q].id) continue;   // src/track/store.rs:206
+          if (!compatible(qs[q], t)) continue;   // Track::distances returns IncompatibleAttributes
           for (const auto& a : qs[q].obs)
             for (const auto& o : t.obs) {
               const float d = metric_of(a.data(), o.data());
@@ -210,6 +235,7 @@ void ofs_destroy(ofs_store* s) { delete s; }
 
 // TrackStore::add, src/track/store.rs:530-568, in call order
 int ofs_add(ofs_store* s, int n, const uint64_t* ids, const float* feats) {
+  if (s->gate) return -1;
   for (int i = 0; i < n; ++i) {
     auto it = s->pos.find(ids[i]);
     if (it == s->pos.end()) {
@@ -226,26 +252,30 @@ int ofs_add(ofs_store* s, int n, const uint64_t* ids, const float* feats) {
 
 int ofs_search(ofs_store* s, int Q, const uint64_t* ids, const int32_t* offs, const float* feats, int32_t* counts,
                uint64_t* winners, double* weights, int threads) {
-  if (s->check(Q, ids, offs, false)) return -1;
+  if (s->gate || s->check(Q, ids, offs, false)) return -1;
   if (Q == 0) return 0;
   s->write(s->search(s->build_queries(Q, ids, offs, feats), threads), counts, winners, weights);
   return 0;
 }
 
 // one iteration of benches/feature_tracker.rs: search, then merge_external into results[0].winner_track or add_track
-int ofs_associate(ofs_store* s, int Q, const uint64_t* ids, const int32_t* offs, const float* feats, int32_t* counts,
-                  uint64_t* winners, double* weights, uint64_t* track_ids, uint8_t* merged, int threads) {
+static int associate(ofs_store* s, int Q, const uint64_t* ids, const int32_t* offs, const float* feats,
+                     const uint64_t* src, const int64_t* t0, const int64_t* t1, int32_t* counts, uint64_t* winners,
+                     double* weights, uint64_t* track_ids, uint8_t* merged, int threads) {
   if (s->check(Q, ids, offs, true)) return -1;
   if (Q == 0) return 0;
-  auto qs = s->build_queries(Q, ids, offs, feats);
+  auto qs = s->build_queries(Q, ids, offs, feats, src, t0, t1);
   const auto r = s->search(qs, threads);
   s->write(r, counts, winners, weights);
   for (int q = 0; q < Q; ++q) {
-    if (!r[q].empty()) {
+    // with a gate, the window of the first winner as the queries merged into it earlier in this call extended it
+    if (!r[q].empty() && s->compatible(qs[q], s->tracks[s->pos.at(r[q][0].winner)])) {
       // Track::merge (src/track.rs:522-600): extend, then optimize keeps the newest K
-      auto& dst = s->tracks[s->pos.at(r[q][0].winner)].obs;
+      Track& dt = s->tracks[s->pos.at(r[q][0].winner)];
+      auto& dst = dt.obs;
       dst.insert(dst.end(), qs[q].obs.begin(), qs[q].obs.end());
       s->keep_newest(dst);
+      if (s->gate) ofs_store::hull(dt, qs[q]);
       track_ids[q] = r[q][0].winner;
       merged[q] = 1;
     } else {
@@ -256,6 +286,13 @@ int ofs_associate(ofs_store* s, int Q, const uint64_t* ids, const int32_t* offs,
     }
   }
   return 0;
+}
+
+int ofs_associate(ofs_store* s, int Q, const uint64_t* ids, const int32_t* offs, const float* feats, int32_t* counts,
+                  uint64_t* winners, double* weights, uint64_t* track_ids, uint8_t* merged, int threads) {
+  if (s->gate) return -1;
+  return associate(s, Q, ids, offs, feats, nullptr, nullptr, nullptr, counts, winners, weights, track_ids, merged,
+                   threads);
 }
 
 // fetch_tracks (src/track/store.rs:388-401) when remove != 0, else a read-only lookup; features [n][K][D]
@@ -335,18 +372,98 @@ int ofs_merge_owned(ofs_store* s, int n, const uint64_t* dest, const uint64_t* s
     if (removed.count(dest[i]) || removed.count(src[i])) return -1;
     if (remove_src) removed.insert(src[i]);
   }
+  const std::vector<Track> saved = s->tracks;   // a pair found incompatible refuses the whole call
   for (int i = 0; i < n; ++i) {
     const size_t at = s->pos.at(src[i]);
     const Track t = s->tracks[at];   // fetch_tracks([src])
     s->tracks.erase(s->tracks.begin() + (std::ptrdiff_t)at);
     s->reindex();
-    auto& o = s->tracks[s->pos.at(dest[i])].obs;   // merge_external -> Track::merge
+    Track& dt = s->tracks[s->pos.at(dest[i])];   // merge_external -> Track::merge
+    if (!s->compatible(dt, t)) {
+      s->tracks = saved;
+      s->reindex();
+      return -1;
+    }
+    if (s->gate) ofs_store::hull(dt, t);
+    auto& o = dt.obs;
     o.insert(o.end(), t.obs.begin(), t.obs.end());
     s->keep_newest(o);
     if (!remove_src) s->tracks.insert(s->tracks.begin() + (std::ptrdiff_t)at, t);   // add_track
     s->reindex();
   }
   return 0;
+}
+
+// ---- track attributes (gate != 0)
+// The rule may change only while the store holds no tracks.
+int ofs_set_gate(ofs_store* s, int rule) {
+  if (rule < 0 || rule > 2 || !s->tracks.empty()) return -1;
+  s->gate = rule;
+  return 0;
+}
+
+static bool bad_windows(int n, const int64_t* t0, const int64_t* t1) {
+  for (int i = 0; i < n; ++i)
+    if (t0[i] > t1[i]) return true;
+  return false;
+}
+
+// TrackStore::add with attributes: an unknown id creates a track with the row's triple, a known id takes the hull of
+// the windows; a source that differs from the track's is refused (the reference's WrongCamID) before anything changes.
+int ofs_add_attr(ofs_store* s, int n, const uint64_t* ids, const uint64_t* src, const int64_t* t0, const int64_t* t1,
+                 const float* feats) {
+  if (!s->gate || n < 0 || bad_windows(n, t0, t1)) return -1;
+  std::unordered_map<uint64_t, uint64_t> source;
+  for (const Track& t : s->tracks) source[t.id] = t.src;
+  for (int i = 0; i < n; ++i) {
+    auto it = source.emplace(ids[i], src[i]).first;
+    if (it->second != src[i]) return -1;
+  }
+  for (int i = 0; i < n; ++i) {
+    auto it = s->pos.find(ids[i]);
+    if (it == s->pos.end()) {
+      s->pos[ids[i]] = s->tracks.size();
+      s->tracks.push_back({ids[i], {s->pad(feats + (size_t)i * s->D)}, src[i], t0[i], t1[i]});
+    } else {
+      Track& t = s->tracks[it->second];
+      t.obs.push_back(s->pad(feats + (size_t)i * s->D));
+      s->keep_newest(t.obs);
+      t.t0 = std::min(t.t0, t0[i]);
+      t.t1 = std::max(t.t1, t1[i]);
+    }
+  }
+  return 0;
+}
+
+int ofs_search_attr(ofs_store* s, int Q, const uint64_t* ids, const int32_t* offs, const uint64_t* src, const int64_t* t0,
+                    const int64_t* t1, const float* feats, int32_t* counts, uint64_t* winners, double* weights,
+                    int threads) {
+  if (!s->gate || s->check(Q, ids, offs, false) || bad_windows(Q, t0, t1)) return -1;
+  if (Q == 0) return 0;
+  s->write(s->search(s->build_queries(Q, ids, offs, feats, src, t0, t1), threads), counts, winners, weights);
+  return 0;
+}
+
+int ofs_associate_attr(ofs_store* s, int Q, const uint64_t* ids, const int32_t* offs, const uint64_t* src,
+                       const int64_t* t0, const int64_t* t1, const float* feats, int32_t* counts, uint64_t* winners,
+                       double* weights, uint64_t* track_ids, uint8_t* merged, int threads) {
+  if (!s->gate || bad_windows(Q, t0, t1)) return -1;
+  return associate(s, Q, ids, offs, feats, src, t0, t1, counts, winners, weights, track_ids, merged, threads);
+}
+
+// the triples of the tracks `ids` (0 for an id that is not stored); returns how many were found
+int64_t ofs_fetch_attr(ofs_store* s, int n, const uint64_t* ids, uint64_t* src, int64_t* t0, int64_t* t1) {
+  if (!s->gate) return -1;
+  int64_t found = 0;
+  for (int i = 0; i < n; ++i) {
+    auto it = s->pos.find(ids[i]);
+    const bool ok = it != s->pos.end();
+    src[i] = ok ? s->tracks[it->second].src : 0;
+    t0[i] = ok ? s->tracks[it->second].t0 : 0;
+    t1[i] = ok ? s->tracks[it->second].t1 : 0;
+    found += ok;
+  }
+  return found;
 }
 
 int64_t ofs_size(ofs_store* s) { return (int64_t)s->tracks.size(); }

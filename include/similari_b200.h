@@ -409,8 +409,9 @@ int sb200_shard_gather(sb200_comm* c, int32_t root, const int32_t* det_range, co
                        const sb200_predict_out* all, void* cuda_stream);
 
 /* ---- feature track store: TrackStore (src/track/store.rs) for feature-only tracks, with TopNVoting on top ----
- * The tracks of benches/feature_tracker.rs: one feature class, no track attributes (compatible is always true, baked is
- * always Ready), every observation carries a feature.  Each track keeps its newest max_observations (K) observations in
+ * The tracks of benches/feature_tracker.rs: one feature class, baked is always Ready, every observation carries a
+ * feature.  Without a gate (the default) there are no track attributes and compatible is always true; a gated store
+ * (sb200_fstore_set_gate, below) keeps the attributes of examples/track_merging.rs.  Each track keeps its newest max_observations (K) observations in
  * their original order (the bench's optimize: reverse / truncate(K) / reverse).  The store lives on the device.
  *
  * Order rules (the reference's shard / HashMap order is replaced by these, which the oracle defines):
@@ -587,6 +588,65 @@ int64_t sb200_fstore_associate_wasted(sb200_fstore* s, sb200_tracker* t, int64_t
                                       uint8_t* queried, int32_t* counts, uint64_t* winners, double* weights,
                                       uint64_t* track_ids, uint8_t* merged);
 
+/* ---- track attributes: a time window and a source per track, and the reference's `compatible` as a gate ----
+ * The CamTrackingAttributes of examples/track_merging.rs:218-245: each track of a GATED store carries a source (camera)
+ * id and a window [t_start, t_end] (i64, in the caller's unit; t_start <= t_end).  The rule:
+ *   SB200_FSTORE_GATE_NONE (0, the default): no attributes; every call behaves as it always has.
+ *   SB200_FSTORE_GATE_SAME_SOURCE (1): compatible(a, b) = (a.t_start >= b.t_end || a.t_end <= b.t_start) &&
+ *     a.source == b.source, the example's `compatible` exactly: the windows are disjoint, touching windows count as
+ *     disjoint.  Two tracks seen at the same time by the same camera are different objects.
+ *   SB200_FSTORE_GATE_ANY_SOURCE (2): the windows are disjoint, whatever the sources (cross-camera galleries).
+ * merge (CamTrackingAttributes::merge) gives the destination the hull of the two windows; it keeps its source.
+ * Semantics on a gated store:
+ *   search: an incompatible (query, stored track) pair gives no entries: it does not vote and does not raise max_dist,
+ *     the error path of Track::distances (src/track.rs:604-652).  So weights may differ from an ungated search's, as in
+ *     the reference.
+ *   add: an unknown id creates a track with the row's triple; a known id takes the hull of the windows; a source that
+ *     differs from the track's (or from an earlier row's of the same new id) is SB200_ERR_INVALID (WrongCamID).
+ *   associate: queries in order; a query is merged into its first winner only if it is compatible with that track's
+ *     window as extended by the queries merged into it earlier in the same call; otherwise it becomes a new track with
+ *     its own triple.  A merged destination takes the hull.  The reference's merge_external instead returns
+ *     IncompatibleAttributes at that point, after merging the queries in front of it (Track::merge,
+ *     src/track.rs:522-530): a documented deviation.  It keeps two coexisting queries that win one track apart.
+ *   search_owned: each query is gated against every candidate it is scored with, by their stored attributes.
+ *   merge_owned: each pair is checked, in order, against the windows the earlier pairs left; an incompatible pair
+ *     refuses the whole call (SB200_ERR_INVALID) before anything changes.  A destination takes the hull.
+ *   fetch with remove: the attributes leave with their tracks.
+ * Refusals, SB200_ERR_INVALID with sb200_last_error naming the cause, decided before anything changes: the plain add /
+ * search / associate (and their _device forms) on a gated store; an _attr call on an ungated store; t_start > t_end;
+ * sb200_fstore_associate_wasted on a gated store (the tracker keeps no birth epoch, so a wasted record has no exact
+ * window).  The host keeps no copy of the attributes: a call reads back those of the tracks it touches only. */
+#define SB200_FSTORE_GATE_NONE 0
+#define SB200_FSTORE_GATE_SAME_SOURCE 1
+#define SB200_FSTORE_GATE_ANY_SOURCE 2
+/* Sets the rule.  Allowed while the store holds no tracks (also after sb200_fstore_fetch with remove emptied it), as
+ * sb200_fstore_set_storage_type.  SB200_ERR_INVALID, changing nothing, for an unknown rule or a store that holds tracks.
+ * A loaded store has its blob's rule. */
+int sb200_fstore_set_gate(sb200_fstore* s, int32_t rule);
+int sb200_fstore_get_gate(sb200_fstore* s, int32_t* out);
+/* One triple per row (add) or per query (search / associate): host arrays. */
+typedef struct {
+  const uint64_t* source;
+  const int64_t* t_start;
+  const int64_t* t_end;
+} sb200_fstore_attrs;
+/* sb200_fstore_add / _search / _associate of a gated store.  Exactly one of `features` (host) and `d_features` (device,
+ * with `cuda_stream` as for the _device forms) is non-NULL; either is in the type set by sb200_fstore_set_feature_type.
+ * Outputs as for the calls without attributes. */
+int sb200_fstore_add_attr(sb200_fstore* s, int32_t n, const uint64_t* ids, const sb200_fstore_attrs* attrs,
+                          const float* features, const void* d_features, void* cuda_stream);
+int sb200_fstore_search_attr(sb200_fstore* s, int32_t n_queries, const uint64_t* query_ids, const int32_t* obs_offsets,
+                             const sb200_fstore_attrs* attrs, const float* features, const void* d_features,
+                             int32_t* counts, uint64_t* winners, double* weights, void* cuda_stream);
+int sb200_fstore_associate_attr(sb200_fstore* s, int32_t n_queries, const uint64_t* query_ids,
+                                const int32_t* obs_offsets, const sb200_fstore_attrs* attrs, const float* features,
+                                const void* d_features, int32_t* counts, uint64_t* winners, double* weights,
+                                uint64_t* track_ids, uint8_t* merged, void* cuda_stream);
+/* The triples of the tracks `ids` of a gated store (0 in every column for an id that is not stored).  Returns how many of
+ * the ids were found, or a negative status. */
+int64_t sb200_fstore_fetch_attr(sb200_fstore* s, int32_t n, const uint64_t* ids, uint64_t* source, int64_t* t_start,
+                                int64_t* t_end);
+
 /* ---- the store blob ----
  * The whole store as one relocatable block of bytes: this header, then four sections at 256-byte aligned offsets, gaps
  * zeroed, in this order: ids[live] (u64), cnt[live] (i32 observations held), start[live] (i32 ring slot of the oldest
@@ -622,6 +682,32 @@ typedef struct {
   uint64_t sec_off[SB200_FSTORE_BLOB_SECTIONS];
   uint64_t sec_bytes[SB200_FSTORE_BLOB_SECTIONS];
 } sb200_fstore_blob_header;
+/* The blob of a gated store: version 2, this header (the version-1 fields through `live`, then the rule), then seven
+ * sections laid out as version 1's: ids, cnt, start, feat, then source[live] (u64), t_start[live] and t_end[live] (i64).
+ * An ungated store writes version 1, byte for byte as before, and a version-1 blob loads as an ungated store.  A library
+ * from before gated stores refuses a version-2 blob by its version check. */
+#define SB200_FSTORE_BLOB_VERSION_GATED 2u
+#define SB200_FSTORE_BLOB_SECTIONS_V2 7
+typedef struct {
+  uint32_t magic;
+  uint32_t version; /* SB200_FSTORE_BLOB_VERSION_GATED */
+  uint64_t total_bytes;
+  int32_t metric;
+  float distance_filter;
+  int32_t max_observations;
+  int32_t feature_dim;
+  int32_t topn;
+  float max_distance;
+  int32_t min_votes;
+  int32_t d8;
+  int32_t feature_type;
+  int32_t storage_type;
+  int64_t live;
+  int32_t gate;      /* SB200_FSTORE_GATE_SAME_SOURCE or _ANY_SOURCE */
+  int32_t reserved;  /* 0 */
+  uint64_t sec_off[SB200_FSTORE_BLOB_SECTIONS_V2];
+  uint64_t sec_bytes[SB200_FSTORE_BLOB_SECTIONS_V2];
+} sb200_fstore_blob_header_v2;
 /* Writes the blob to `buf` (`cap` bytes; host memory, or device memory on any device) and its size to *bytes.
  * buf == NULL: reports the size and writes nothing.  SB200_ERR_CAPACITY when cap is too small: nothing is written and
  * *bytes is still set.  Rows are copied, not re-derived; the store is not changed.  Timers and the stream are not part
@@ -633,7 +719,8 @@ int sb200_fstore_save(sb200_fstore* s, void* buf, uint64_t cap, uint64_t* bytes)
  * magic, version, truncation, section bounds / order / 256-byte alignment / sizes, options outside the caps of
  * sb200_fstore_create, d8 != round_up(feature_dim, 8), an unknown feature_type or storage_type (checked before the
  * section sizes, which depend on it), an id twice, and (by one kernel over the blob, before any row is
- * copied) a cnt outside [1, max_observations] or a start outside [0, max_observations).  A flipped feature value is not
+ * copied) a cnt outside [1, max_observations] or a start outside [0, max_observations); in a version-2 blob also an
+ * unknown gate rule and (by kernel) a stored window with t_start > t_end.  A flipped feature value is not
  * detected: the blob carries no checksum.  A failed load leaves no handle and no device memory behind.  No counterpart
  * in the reference. */
 int sb200_fstore_load(const void* buf, uint64_t bytes, int32_t device, sb200_fstore** out);

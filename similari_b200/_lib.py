@@ -113,6 +113,28 @@ class FstoreBlobHeader(C.Structure):
     ]
 
 
+FSTORE_BLOB_VERSION_GATED, FSTORE_BLOB_SECTIONS_V2 = 2, 7
+# track attribute rules of the feature store (sb200_fstore_set_gate)
+FSTORE_GATE_NONE, FSTORE_GATE_SAME_SOURCE, FSTORE_GATE_ANY_SOURCE = 0, 1, 2
+
+
+class FstoreBlobHeaderV2(C.Structure):
+    """sb200_fstore_blob_header_v2: the first bytes of the blob of a gated store."""
+
+    _fields_ = FstoreBlobHeader._fields_[:-2] + [
+        ("gate", C.c_int32),
+        ("reserved", C.c_int32),
+        ("sec_off", C.c_uint64 * FSTORE_BLOB_SECTIONS_V2),
+        ("sec_bytes", C.c_uint64 * FSTORE_BLOB_SECTIONS_V2),
+    ]
+
+
+class FstoreAttrs(C.Structure):
+    """sb200_fstore_attrs: host columns of one source and one [t_start, t_end] window per row."""
+
+    _fields_ = [("source", C.c_void_p), ("t_start", C.c_void_p), ("t_end", C.c_void_p)]
+
+
 _lib = None
 
 # every symbol include/similari_b200.h declares (checked by tests/test_abi.py without a GPU)
@@ -136,7 +158,8 @@ EXPORTS = [
     "sb200_fstore_get_options", "sb200_fstore_add_device", "sb200_fstore_search_device",
     "sb200_fstore_associate_device", "sb200_fstore_save", "sb200_fstore_load", "sb200_fstore_search_owned",
     "sb200_fstore_merge_owned", "sb200_fstore_set_storage_type", "sb200_fstore_get_storage_type",
-    "sb200_fstore_associate_wasted",
+    "sb200_fstore_associate_wasted", "sb200_fstore_set_gate", "sb200_fstore_get_gate", "sb200_fstore_add_attr",
+    "sb200_fstore_search_attr", "sb200_fstore_associate_attr", "sb200_fstore_fetch_attr",
 ]
 
 
@@ -237,6 +260,13 @@ def lib():
         "sb200_fstore_search_owned": (C.c_int, [vp, i32, vp, i32, vp, vp, vp]),
         "sb200_fstore_merge_owned": (C.c_int, [vp, i32, vp, vp, i32]),
         "sb200_fstore_set_storage_type": (C.c_int, [vp, i32]),
+        "sb200_fstore_set_gate": (C.c_int, [vp, i32]),
+        "sb200_fstore_get_gate": (C.c_int, [vp, C.POINTER(i32)]),
+        "sb200_fstore_add_attr": (C.c_int, [vp, i32, vp, C.POINTER(FstoreAttrs), vp, vp, vp]),
+        "sb200_fstore_search_attr": (C.c_int, [vp, i32, vp, vp, C.POINTER(FstoreAttrs), vp, vp, vp, vp, vp, vp]),
+        "sb200_fstore_associate_attr": (C.c_int, [vp, i32, vp, vp, C.POINTER(FstoreAttrs), vp, vp, vp, vp, vp, vp, vp,
+                                                  vp]),
+        "sb200_fstore_fetch_attr": (i64, [vp, i32, vp, vp, vp, vp]),
         "sb200_fstore_get_storage_type": (C.c_int, [vp, C.POINTER(i32)]),
         "sb200_fstore_associate_wasted": (i64, [vp, vp, i64, u64, vp, vp, vp, vp, vp, vp, i32, vp, vp, vp, vp, vp, vp, vp,
                                                 vp, vp, vp]),

@@ -8,12 +8,14 @@
 // owned calls (search_owned, merge_owned) take stored tracks: their rows never leave the device, and the host reads back
 // only the counts and ring starts of the tracks they touch.  The stored rows are f32, binary16 or bfloat16 (stype,
 // sb200_fstore_set_storage_type); row_bytes() is the size of one stored row, and nothing else on the host depends on the
-// storage type.
+// storage type.  A gated store (sb200_fstore_set_gate) also keeps a source and a window per track in three device
+// columns of its own; a call reads back the triples of the tracks it touches, and an ungated store allocates none.
 #include <cuda_runtime.h>
 
 #include <algorithm>
 #include <climits>
 #include <cmath>
+#include <cstddef>
 #include <cstring>
 #include <unordered_map>
 #include <unordered_set>
@@ -75,7 +77,16 @@ struct Column {
 };
 
 using BlobHeader = sb200_fstore_blob_header;
-enum { kSecIds, kSecCnt, kSecStart, kSecFeat };
+using BlobHeaderV2 = sb200_fstore_blob_header_v2;
+enum { kSecIds, kSecCnt, kSecStart, kSecFeat, kSecSrc, kSecT0, kSecT1 };
+static_assert(offsetof(BlobHeaderV2, live) == offsetof(BlobHeader, live), "version 2 repeats version 1's fields");
+
+// a gated call's triples on the host: n entries of each column
+struct Triples {
+  std::vector<uint64_t> src;
+  std::vector<int64_t> t0, t1;
+  explicit Triples(size_t n = 0) : src(n), t0(n), t1(n) {}
+};
 
 bool known_type(int t) { return t == SB200_FEATURE_F32 || t == SB200_FEATURE_F16 || t == SB200_FEATURE_BF16; }
 size_t type_bytes(int t) { return t == SB200_FEATURE_F32 ? 4 : 2; }
@@ -106,6 +117,9 @@ struct sb200_fstore {
   // store columns
   size_t cap = 0;
   DBuf feat, cnt, start, ids, run;
+  int gate = SB200_FSTORE_GATE_NONE;
+  DBuf asrc, at0, at1;                       // gated store: [cap] source, t_start, t_end
+  DBuf qattr;                                // a gated call's triples, [n] of each column
   std::vector<uint64_t> hid;                 // ids in store order
   std::unordered_map<uint64_t, int> hpos;    // id -> store position
   // per-call buffers
@@ -148,22 +162,130 @@ struct sb200_fstore {
     return 0;
   }
 
+  // fresh, zero-filled attribute columns for `n` tracks (none for an ungated store); the caller copies what it keeps
+  int alloc_attrs(size_t n, DBuf* a, DBuf* b, DBuf* c) {
+    if (!gate) return 0;
+    n = std::max<size_t>(n, 1);
+    for (DBuf* x : {a, b, c}) {
+      if (int rc = x->ensure(n * 8)) return rc;
+      CU(cudaMemsetAsync(x->p, 0, n * 8, st));
+    }
+    return 0;
+  }
+
+  sb::FsAttrCols attr_cols() const {
+    return {asrc.as<unsigned long long>(), at0.as<long long>(), at1.as<long long>()};
+  }
+
   // capacity for `need` tracks: grows by at least 1.5x, keeping the live tracks
   int reserve(size_t need) {
     if (need <= cap) return 0;
     const size_t nc = std::max(need, cap + cap / 2);
-    DBuf f, c, s, i, r;
+    DBuf f, c, s, i, r, a0, a1, a2;
     if (int rc = alloc_columns(nc, &f, &c, &s, &i, &r)) return rc;
+    if (int rc = alloc_attrs(nc, &a0, &a1, &a2)) return rc;
     const size_t live = hid.size();
     if (live) {
       CU(cudaMemcpyAsync(f.p, feat.p, live * o.max_observations * row_bytes(), cudaMemcpyDeviceToDevice, st));
       CU(cudaMemcpyAsync(c.p, cnt.p, live * 4, cudaMemcpyDeviceToDevice, st));
       CU(cudaMemcpyAsync(s.p, start.p, live * 4, cudaMemcpyDeviceToDevice, st));
       CU(cudaMemcpyAsync(i.p, ids.p, live * 8, cudaMemcpyDeviceToDevice, st));
+      if (gate) {
+        CU(cudaMemcpyAsync(a0.p, asrc.p, live * 8, cudaMemcpyDeviceToDevice, st));
+        CU(cudaMemcpyAsync(a1.p, at0.p, live * 8, cudaMemcpyDeviceToDevice, st));
+        CU(cudaMemcpyAsync(a2.p, at1.p, live * 8, cudaMemcpyDeviceToDevice, st));
+      }
     }
     CU(cudaStreamSynchronize(st));   // the old columns are freed below
     feat = std::move(f); cnt = std::move(c); start = std::move(s); ids = std::move(i); run = std::move(r);
+    asrc = std::move(a0); at0 = std::move(a1); at1 = std::move(a2);
     cap = nc;
+    return 0;
+  }
+
+  // ---- track attributes (gated store)
+  int refuse_gated() const {
+    if (gate) return fail(SB200_ERR_INVALID, "the store is gated (rule %d): use the _attr calls, with a source and a window per row", gate);
+    return 0;
+  }
+
+  // checks of the triples of an _attr call with n rows / queries
+  int check_attrs(int n, const sb200_fstore_attrs* a) const {
+    if (!gate) return fail(SB200_ERR_INVALID, "the store has no gate (sb200_fstore_set_gate): the _attr calls need one");
+    if (n <= 0) return 0;
+    if (!a || !a->source || !a->t_start || !a->t_end) return fail(SB200_ERR_INVALID, "attrs or one of its columns is NULL");
+    for (int i = 0; i < n; ++i)
+      if (a->t_start[i] > a->t_end[i])
+        return fail(SB200_ERR_INVALID, "row %d: t_start %lld > t_end %lld", i, (long long)a->t_start[i],
+                    (long long)a->t_end[i]);
+    return 0;
+  }
+
+  // the device triples of a call (n of each column, in qattr) as the gated kernels read them
+  sb::FsGate gate_view(int n) const {
+    const unsigned long long* q = qattr.as<unsigned long long>();
+    return {attr_cols(), q, reinterpret_cast<const long long*>(q + n), reinterpret_cast<const long long*>(q + 2 * (size_t)n),
+            gate};
+  }
+  sb::FsAttrCols qattr_cols(int n) const {
+    unsigned long long* q = qattr.as<unsigned long long>();
+    return {q, reinterpret_cast<long long*>(q + n), reinterpret_cast<long long*>(q + 2 * (size_t)n)};
+  }
+
+  // uploads n triples into qattr
+  int upload_triples(int n, const uint64_t* src, const int64_t* t0, const int64_t* t1) {
+    if (int rc = qattr.ensure(std::max(n, 1) * 24)) return rc;
+    if (n == 0) return 0;
+    char* d = qattr.as<char>();
+    CU(cudaMemcpyAsync(d, src, (size_t)n * 8, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(d + (size_t)n * 8, t0, (size_t)n * 8, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(d + (size_t)n * 16, t1, (size_t)n * 8, cudaMemcpyHostToDevice, st));
+    return 0;
+  }
+
+  // the stored triples at pos[] (-1: zeros), read back; changes nothing
+  int peek_attrs(const std::vector<int>& pos, Triples* out) {
+    const int n = (int)pos.size();
+    *out = Triples(pos.size());
+    if (n == 0) return 0;
+    if (int rc = gpos.ensure((size_t)n * 4)) return rc;
+    if (int rc = gout.ensure((size_t)n * 24)) return rc;
+    CU(cudaMemcpyAsync(gpos.p, pos.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
+    unsigned long long* g = gout.as<unsigned long long>();
+    sb::fs_launch_attr_gather(attr_cols(), gpos.as<int>(), n,
+                              {g, reinterpret_cast<long long*>(g + n), reinterpret_cast<long long*>(g + 2 * (size_t)n)}, st);
+    CU(cudaMemcpyAsync(out->src.data(), g, (size_t)n * 8, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(out->t0.data(), g + n, (size_t)n * 8, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(out->t1.data(), g + 2 * (size_t)n, (size_t)n * 8, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    CU(cudaGetLastError());
+    return 0;
+  }
+
+  // writes the triples `v` to the stored positions pos[]
+  int write_attrs(const std::vector<int>& pos, const Triples& v) {
+    const int n = (int)pos.size();
+    if (n == 0) return 0;
+    if (int rc = gpos.ensure((size_t)n * 4)) return rc;
+    if (int rc = upload_triples(n, v.src.data(), v.t0.data(), v.t1.data())) return rc;
+    CU(cudaMemcpyAsync(gpos.p, pos.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
+    sb::fs_launch_attr_scatter(attr_cols(), gpos.as<int>(), n, qattr_cols(n), st);
+    CU(cudaStreamSynchronize(st));
+    CU(cudaGetLastError());
+    return 0;
+  }
+
+  int set_gate(int rule) {
+    if (rule != SB200_FSTORE_GATE_NONE && rule != SB200_FSTORE_GATE_SAME_SOURCE && rule != SB200_FSTORE_GATE_ANY_SOURCE)
+      return fail(SB200_ERR_INVALID, "unknown gate rule %d", rule);
+    if (!hid.empty()) return fail(SB200_ERR_INVALID, "the gate is fixed while the store holds tracks (%zu)", hid.size());
+    CU(cudaSetDevice(o.device));
+    gate = rule;
+    DBuf a0, a1, a2;   // no track is stored: the columns start empty, sized to the capacity
+    if (cap)
+      if (int rc = alloc_attrs(cap, &a0, &a1, &a2)) return rc;
+    CU(cudaStreamSynchronize(st));
+    asrc = std::move(a0); at0 = std::move(a1); at1 = std::move(a2);
     return 0;
   }
 
@@ -301,8 +423,10 @@ struct sb200_fstore {
   }
 
   // search (assoc == false) or associate
+  // attrs: the queries' triples of a gated store's call (checked by the caller), else nullptr
   int run_queries(int Q, const uint64_t* qids, const int32_t* offs, const Column& col, int32_t* counts,
-                  uint64_t* winners, double* weights, uint64_t* track_ids, uint8_t* merged, bool assoc) {
+                  uint64_t* winners, double* weights, uint64_t* track_ids, uint8_t* merged, bool assoc,
+                  const sb200_fstore_attrs* attrs = nullptr) {
     std::vector<int> qoff, src;
     if (int rc = check_queries(Q, qids, offs, col, assoc, &qoff, &src)) return rc;
     if (Q > 0 && (!counts || !winners || !weights || (assoc && (!track_ids || !merged))))
@@ -310,7 +434,7 @@ struct sb200_fstore {
     if (int rc = begin()) return rc;
     if (Q == 0) return 0;
     return launch_queries(Q, qids, qoff, src, col, (size_t)offs[Q], nullptr, counts, winners, weights, track_ids, merged,
-                          assoc);
+                          assoc, attrs);
   }
 
   // associate whose request rows `rsrc` writes on the device (sb200_fstore_associate_wasted); offs as for associate
@@ -335,7 +459,8 @@ struct sb200_fstore {
   // the device part of search / associate, after every check: upload, distances, TopN, apply, results
   int launch_queries(int Q, const uint64_t* qids, const std::vector<int>& qoff, const std::vector<int>& src,
                      const Column& col, size_t col_rows, const sb::FsRowSource* rsrc, int32_t* counts,
-                     uint64_t* winners, double* weights, uint64_t* track_ids, uint8_t* merged, bool assoc) {
+                     uint64_t* winners, double* weights, uint64_t* track_ids, uint8_t* merged, bool assoc,
+                     const sb200_fstore_attrs* attrs = nullptr) {
     const int R = (int)src.size(), topn = o.topn, K = o.max_observations;
     const long long live = (long long)hid.size(), S = live * K;
     const ReqLayout L(Q, R, d8, !rsrc && (col.on_device || ftype != SB200_FEATURE_F32));
@@ -351,16 +476,26 @@ struct sb200_fstore {
     if (assoc)
       if (int rc = reserve(hid.size() + (size_t)Q)) return rc;
     if (int rc = upload(L, Q, qids, qoff, src, std::vector<int>(Q, -1), col, col_rows, rsrc)) return rc;
+    if (attrs)
+      if (int rc = upload_triples(Q, attrs->source, attrs->t_start, attrs->t_end)) return rc;
+    const sb::FsGate g = gate_view(Q);
     const sb::FsStore s = view();
     const sb::FsCall c = call_view(L, Q, R, &RL);
     CU(cudaEventRecord(ev[0], st));
-    sb::fs_launch_dist(o.metric, o.distance_filter, s, c, st);
+    sb::fs_launch_dist(o.metric, o.distance_filter, s, c, st, sb::kFsForeign, nullptr, attrs ? &g : nullptr);
     CU(cudaEventRecord(ev[1], st));
     sb::fs_launch_topn(o.max_distance, o.min_votes, topn, assoc, s, c, st);
     CU(cudaEventRecord(ev[2], st));
+    if (assoc && attrs) sb::fs_launch_gate_resolve(c, g, st);
     if (assoc) sb::fs_launch_apply(s, c, st);
+    if (assoc && attrs) sb::fs_launch_attr_new(s.live, c, g, st);
     CU(cudaEventRecord(ev[3], st));
     CU(cudaMemcpyAsync(hres.p, dres.p, RL.total, cudaMemcpyDeviceToHost, st));
+    std::vector<int> where;   // gated associate: the position each query ended up at (>= live: a new track)
+    if (assoc && attrs) {
+      where.resize(Q);
+      CU(cudaMemcpyAsync(where.data(), c.dest, (size_t)Q * 4, cudaMemcpyDeviceToHost, st));
+    }
     CU(cudaStreamSynchronize(st));
     CU(cudaGetLastError());
     if (int rc = finish_timing(S > 0, true, assoc)) return rc;
@@ -379,7 +514,8 @@ struct sb200_fstore {
     if (assoc) {
       for (int q = 0; q < Q; ++q) {
         merged[q] = cn[q] > 0 ? 1 : 0;
-        track_ids[q] = cn[q] > 0 ? winners[(size_t)q * topn] : qids[q];
+        if (attrs) merged[q] = where[q] < live ? 1 : 0;   // a first winner the gate refused leaves a new track
+        track_ids[q] = merged[q] ? winners[(size_t)q * topn] : qids[q];
       }
       for (int q = 0; q < Q; ++q)
         if (!merged[q]) {
@@ -390,7 +526,8 @@ struct sb200_fstore {
     return 0;
   }
 
-  int add(int n, const uint64_t* idv, const Column& col) {
+  // attrs: the rows' triples of a gated store's call (checked by the caller), else nullptr
+  int add(int n, const uint64_t* idv, const Column& col, const sb200_fstore_attrs* attrs = nullptr) {
     if (n < 0) return fail(SB200_ERR_INVALID, "n < 0");
     if (n > 0 && (!idv || !col.p)) return fail(SB200_ERR_INVALID, "ids / features is NULL");
     if (int rc = check_column(col)) return rc;
@@ -411,6 +548,11 @@ struct sb200_fstore {
       }
       dest[i] = jt->second;
     }
+    // gated: the final triple of every touched track, planned from the stored ones before anything changes
+    std::vector<int> tpos;
+    Triples fin;
+    if (attrs)
+      if (int rc = plan_add_attrs(n, idv, dest, live, *attrs, &tpos, &fin)) return rc;
     std::vector<int> qoff(n + 1), src(n);
     for (int i = 0; i <= n; ++i) qoff[i] = i;
     for (int i = 0; i < n; ++i) src[i] = i;
@@ -430,7 +572,62 @@ struct sb200_fstore {
       hpos[id] = (int)hid.size();
       hid.push_back(id);
     }
+    return write_attrs(tpos, fin);
+  }
+
+  // add's attributes: a new track takes its first row's triple, a track takes the hull of its rows' windows, and a row
+  // whose source differs from its track's is refused.  tpos = the touched positions, fin their final triples.
+  int plan_add_attrs(int n, const uint64_t* idv, const std::vector<int>& dest, int live, const sb200_fstore_attrs& a,
+                     std::vector<int>* tpos, Triples* fin) {
+    std::unordered_map<int, int> at;   // position -> index into tpos
+    std::vector<int> known;
+    for (int i = 0; i < n; ++i)
+      if (at.emplace(dest[i], (int)tpos->size()).second) {
+        tpos->push_back(dest[i]);
+        if (dest[i] < live) known.push_back(dest[i]);
+      }
+    Triples old;
+    if (int rc = peek_attrs(known, &old)) return rc;
+    *fin = Triples(tpos->size());
+    std::vector<char> set(tpos->size(), 0);
+    for (size_t k = 0; k < known.size(); ++k) {
+      const int j = at[known[k]];
+      fin->src[j] = old.src[k]; fin->t0[j] = old.t0[k]; fin->t1[j] = old.t1[k];
+      set[j] = 1;
+    }
+    for (int i = 0; i < n; ++i) {
+      const int j = at[dest[i]];
+      if (!set[j]) {
+        fin->src[j] = a.source[i]; fin->t0[j] = a.t_start[i]; fin->t1[j] = a.t_end[i];
+        set[j] = 1;
+        continue;
+      }
+      if (fin->src[j] != a.source[i])
+        return fail(SB200_ERR_INVALID, "row %d: source %llu differs from track %llu's source %llu", i,
+                    (unsigned long long)a.source[i], (unsigned long long)idv[i], (unsigned long long)fin->src[j]);
+      fin->t0[j] = std::min<int64_t>(fin->t0[j], a.t_start[i]);
+      fin->t1[j] = std::max<int64_t>(fin->t1[j], a.t_end[i]);
+    }
     return 0;
+  }
+
+  int64_t fetch_attr(int n, const uint64_t* idv, uint64_t* src, int64_t* t0, int64_t* t1) {
+    if (!gate) return fail(SB200_ERR_INVALID, "the store has no gate (sb200_fstore_set_gate): it keeps no attributes");
+    if (n < 0) return fail(SB200_ERR_INVALID, "n < 0");
+    if (n > 0 && (!idv || !src || !t0 || !t1)) return fail(SB200_ERR_INVALID, "ids or an output is NULL");
+    if (int rc = begin()) return rc;
+    std::vector<int> pos(n, -1);
+    int64_t found = 0;
+    for (int i = 0; i < n; ++i) {
+      auto it = hpos.find(idv[i]);
+      if (it != hpos.end()) { pos[i] = it->second; ++found; }
+    }
+    Triples v;
+    if (int rc = peek_attrs(pos, &v)) return rc;
+    std::copy(v.src.begin(), v.src.end(), src);
+    std::copy(v.t0.begin(), v.t0.end(), t0);
+    std::copy(v.t1.begin(), v.t1.end(), t1);
+    return found;
   }
 
   int64_t fetch(int n, const uint64_t* idv, int remove, int32_t* counts, float* feats) {
@@ -479,17 +676,22 @@ struct sb200_fstore {
     from.reserve(hid.size());
     for (size_t p = 0; p < hid.size(); ++p)
       if (!gone[p]) from.push_back((int)p);
-    DBuf f, c, st_, i, r;
+    DBuf f, c, st_, i, r, a0, a1, a2;
     if (int rc = alloc_columns(cap, &f, &c, &st_, &i, &r)) return rc;
+    if (int rc = alloc_attrs(cap, &a0, &a1, &a2)) return rc;
     if (int rc = gpos.ensure(std::max<size_t>(from.size(), 1) * 4)) return rc;
     CU(cudaMemcpyAsync(gpos.p, from.data(), from.size() * 4, cudaMemcpyHostToDevice, st));
     const sb::FsStore s = view();
     sb::FsStore d = s;
     d.feat = f.p; d.cnt = c.as<int>(); d.start = st_.as<int>(); d.ids = i.as<unsigned long long>();
     sb::fs_launch_compact(s, d, gpos.as<int>(), (int)from.size(), st);
+    if (gate)
+      sb::fs_launch_attr_gather(attr_cols(), gpos.as<int>(), (int)from.size(),
+                                {a0.as<unsigned long long>(), a1.as<long long>(), a2.as<long long>()}, st);
     CU(cudaStreamSynchronize(st));
     CU(cudaGetLastError());
     feat = std::move(f); cnt = std::move(c); start = std::move(st_); ids = std::move(i); run = std::move(r);
+    asrc = std::move(a0); at0 = std::move(a1); at1 = std::move(a2);
     std::vector<uint64_t> kept;
     kept.reserve(from.size());
     for (int p : from) kept.push_back(hid[p]);
@@ -607,11 +809,15 @@ struct sb200_fstore {
     const sb::FsStore s = view();
     const sb::FsCall c = call_view(L, Q, R, &RL);
     const int mode = each ? sb::kFsOwnedEach : sb::kFsOwnedGroup;
+    const int* dqpos = reinterpret_cast<const int*>(dreq.as<char>() + L.qpos);
+    if (gate)   // the queries' triples are their stored ones
+      if (int rc = qattr.ensure((size_t)Q * 24)) return rc;
+    const sb::FsGate g = gate_view(Q);
     CU(cudaEventRecord(ev[0], st));
-    sb::fs_launch_owned_stage(s, c, reinterpret_cast<const int*>(dreq.as<char>() + L.qpos),
-                              reinterpret_cast<float*>(dreq.as<char>() + L.rows), st);
+    if (gate) sb::fs_launch_attr_gather(attr_cols(), dqpos, Q, qattr_cols(Q), st);
+    sb::fs_launch_owned_stage(s, c, dqpos, reinterpret_cast<float*>(dreq.as<char>() + L.rows), st);
     sb::fs_launch_dist(o.metric, o.distance_filter, s, c, st, mode,
-                       reinterpret_cast<const unsigned char*>(dreq.as<char>() + L.excl));
+                       reinterpret_cast<const unsigned char*>(dreq.as<char>() + L.excl), gate ? &g : nullptr);
     CU(cudaEventRecord(ev[1], st));
     sb::fs_launch_topn(o.max_distance, o.min_votes, topn, false, s, c, st, mode);
     CU(cudaEventRecord(ev[2], st));
@@ -668,6 +874,10 @@ struct sb200_fstore {
         if (idx.emplace(p, (int)touched.size()).second) touched.push_back(p);
     std::vector<int> ring;
     if (int rc = peek(touched, &ring)) return rc;
+    std::vector<int> wpos;   // gated: the destinations whose windows change, and their final triples
+    Triples win;
+    if (gate)
+      if (int rc = plan_merge_attrs(n, dp, sp, idx, touched, &wpos, &win)) return rc;
     // per touched track: its rows oldest first as stored row indices (position * K + slot) of the pre-call store, and
     // how many rows its ring has taken since the call began (old ones included): virtual row v sits in slot (s0 + v) % K
     struct Plan { std::vector<int> rows; long long taken; bool dirty; };
@@ -714,38 +924,84 @@ struct sb200_fstore {
     CU(cudaStreamSynchronize(st));
     CU(cudaGetLastError());
     if (int rc = finish_timing(false, false, true)) return rc;
+    if (int rc = write_attrs(wpos, win)) return rc;
     if (remove) return remove_marked(gone);
     return 0;
   }
 
+  // merge_owned's attributes: each pair, in order, must be compatible with the windows the earlier pairs left (else the
+  // call is refused); a destination takes the hull
+  int plan_merge_attrs(int n, const std::vector<int>& dp, const std::vector<int>& sp,
+                       std::unordered_map<int, int>& idx, const std::vector<int>& touched, std::vector<int>* wpos,
+                       Triples* win) {
+    Triples cur;
+    if (int rc = peek_attrs(touched, &cur)) return rc;
+    std::vector<char> dirty(touched.size(), 0);
+    for (int i = 0; i < n; ++i) {
+      const int d = idx[dp[i]], s = idx[sp[i]];
+      if (!sb::fs_compatible(gate, cur.src[d], cur.t0[d], cur.t1[d], cur.src[s], cur.t0[s], cur.t1[s]))
+        return fail(SB200_ERR_INVALID,
+                    "pair %d: src %llu (source %llu, [%lld, %lld]) is not compatible with dest %llu (source %llu, "
+                    "[%lld, %lld])", i, (unsigned long long)hid[sp[i]], (unsigned long long)cur.src[s],
+                    (long long)cur.t0[s], (long long)cur.t1[s], (unsigned long long)hid[dp[i]],
+                    (unsigned long long)cur.src[d], (long long)cur.t0[d], (long long)cur.t1[d]);
+      cur.t0[d] = std::min(cur.t0[d], cur.t0[s]);
+      cur.t1[d] = std::max(cur.t1[d], cur.t1[s]);
+      dirty[d] = 1;
+    }
+    for (size_t t = 0; t < touched.size(); ++t)
+      if (dirty[t]) {
+        wpos->push_back(touched[t]);
+        win->src.push_back(cur.src[t]); win->t0.push_back(cur.t0[t]); win->t1.push_back(cur.t1[t]);
+      }
+    return 0;
+  }
+
   // ---- the store blob (layout: include/similari_b200.h)
-  // the four columns and their sections of a blob on this device: dir 0 packs, dir 1 unpacks
-  int move_columns(int dir, const BlobHeader& h, char* dblob) {
-    char* col[SB200_FSTORE_BLOB_SECTIONS] = {ids.as<char>(), cnt.as<char>(), start.as<char>(), feat.as<char>()};
+  // the columns and their `n` sections (4, or 7 for a gated store) of a blob on this device: dir 0 packs, dir 1 unpacks
+  int move_columns(int dir, const uint64_t* sec_off, const uint64_t* sec_bytes, int n, char* dblob) {
+    char* col[SB200_FSTORE_BLOB_SECTIONS_V2] = {ids.as<char>(), cnt.as<char>(), start.as<char>(), feat.as<char>(),
+                                                asrc.as<char>(), at0.as<char>(), at1.as<char>()};
     std::vector<sb::XferSeg> segs;
-    for (int i = 0; i < SB200_FSTORE_BLOB_SECTIONS; ++i)
-      sb::add_segment(segs, dir, col[i], dblob + h.sec_off[i], h.sec_bytes[i]);
+    for (int i = 0; i < n; ++i) sb::add_segment(segs, dir, col[i], dblob + sec_off[i], sec_bytes[i]);
     return sb::copy_segments(segs, num_sms, st);
   }
 
-  int save(void* dst, uint64_t cap_bytes, uint64_t* bytes) {
-    BlobHeader h;
+  // the header fields both versions share
+  template <class H> void fill_header(H& h, uint32_t version) const {
     memset(&h, 0, sizeof(h));
-    h.magic = SB200_FSTORE_BLOB_MAGIC; h.version = SB200_FSTORE_BLOB_VERSION;
+    h.magic = SB200_FSTORE_BLOB_MAGIC; h.version = version;
     h.metric = o.metric; h.distance_filter = o.distance_filter; h.max_observations = o.max_observations;
     h.feature_dim = o.feature_dim; h.topn = o.topn; h.max_distance = o.max_distance; h.min_votes = o.min_votes;
     h.d8 = d8; h.feature_type = ftype; h.storage_type = stype; h.live = (int64_t)hid.size();
+  }
+
+  int save(void* dst, uint64_t cap_bytes, uint64_t* bytes) {
     const uint64_t live = hid.size();
-    const uint64_t sec[SB200_FSTORE_BLOB_SECTIONS] = {live * 8, live * 4, live * 4,
-                                                      live * o.max_observations * row_bytes()};
+    const uint64_t sec[SB200_FSTORE_BLOB_SECTIONS_V2] = {live * 8, live * 4, live * 4,
+                                                         live * o.max_observations * row_bytes(), live * 8, live * 8,
+                                                         live * 8};
+    if (gate) {   // version 2: the attribute sections follow feat
+      BlobHeaderV2 h;
+      fill_header(h, SB200_FSTORE_BLOB_VERSION_GATED);
+      h.gate = gate;
+      sb::lay_out(h, sec, SB200_FSTORE_BLOB_SECTIONS_V2);
+      return write_header_and_columns(dst, cap_bytes, bytes, h, SB200_FSTORE_BLOB_SECTIONS_V2);
+    }
+    BlobHeader h;
+    fill_header(h, SB200_FSTORE_BLOB_VERSION);
     sb::lay_out(h, sec, SB200_FSTORE_BLOB_SECTIONS);
+    return write_header_and_columns(dst, cap_bytes, bytes, h, SB200_FSTORE_BLOB_SECTIONS);
+  }
+
+  template <class H> int write_header_and_columns(void* dst, uint64_t cap_bytes, uint64_t* bytes, const H& h, int n) {
     *bytes = h.total_bytes;
     if (!dst) return 0;
     if (cap_bytes < h.total_bytes)
       return fail(SB200_ERR_CAPACITY, "the blob needs %llu bytes", (unsigned long long)h.total_bytes);
     CU(cudaSetDevice(o.device));
-    return sb::write_blob(dst, o.device, st, h, SB200_FSTORE_BLOB_SECTIONS, [&](char* p) {
-      if (int rc = move_columns(0, h, p)) return rc;
+    return sb::write_blob(dst, o.device, st, h, n, [&](char* p) {
+      if (int rc = move_columns(0, h.sec_off, h.sec_bytes, n, p)) return rc;
       sb::fs_launch_blob_scrub(stype, p + h.sec_off[kSecFeat], cnt.as<int>(), start.as<int>(), (int)h.live,
                                o.max_observations, d8, st);
       CU(cudaStreamSynchronize(st));
@@ -754,12 +1010,15 @@ struct sb200_fstore {
     });
   }
 
-  // fills a store fresh from sb200_fstore_create with the checked blob `h` at `src`
-  int load(const BlobHeader& h, const void* src, std::vector<uint64_t>&& blob_ids) {
+  // fills a store fresh from sb200_fstore_create with the checked blob `h` at `src`; a version-2 blob also carries the
+  // rule `rule` and its attribute sections (sec_off / sec_bytes: the blob's section table, 4 or 7 entries)
+  int load(const BlobHeader& h, int rule, const uint64_t* sec_off, const uint64_t* sec_bytes, const void* src,
+           std::vector<uint64_t>&& blob_ids) {
     if (int rc = begin()) return rc;
     const int live = (int)h.live, K = o.max_observations;
     ftype = h.feature_type;
     stype = h.storage_type;
+    if (int rc = set_gate(rule)) return rc;
     if (live == 0) return 0;
     if (int rc = reserve((size_t)live)) return rc;
     DBuf tmp;
@@ -767,16 +1026,24 @@ struct sb200_fstore {
     if (int rc = sb::blob_on_device(src, h.total_bytes, o.device, st, tmp, &dblob)) return rc;
     // counts and ring starts index the rows in every later kernel: checked before anything is copied into the store
     int bad[2] = {0, 0};
-    if (int rc = gpos.ensure(sizeof(bad))) return rc;
-    CU(cudaMemsetAsync(gpos.p, 0, sizeof(bad), st));
-    sb::fs_launch_blob_check(reinterpret_cast<const int*>(dblob + h.sec_off[kSecCnt]),
-                             reinterpret_cast<const int*>(dblob + h.sec_off[kSecStart]), live, K, gpos.as<int>(), st);
+    int bad_w = 0;
+    if (int rc = gpos.ensure(sizeof(bad) + sizeof(bad_w))) return rc;
+    CU(cudaMemsetAsync(gpos.p, 0, sizeof(bad) + sizeof(bad_w), st));
+    sb::fs_launch_blob_check(reinterpret_cast<const int*>(dblob + sec_off[kSecCnt]),
+                             reinterpret_cast<const int*>(dblob + sec_off[kSecStart]), live, K, gpos.as<int>(), st);
+    if (rule)
+      sb::fs_launch_attr_check(reinterpret_cast<const long long*>(dblob + sec_off[kSecT0]),
+                               reinterpret_cast<const long long*>(dblob + sec_off[kSecT1]), live, gpos.as<int>() + 2, st);
     CU(cudaMemcpyAsync(bad, gpos.p, sizeof(bad), cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(&bad_w, gpos.as<int>() + 2, sizeof(bad_w), cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
     CU(cudaGetLastError());
     if (bad[0]) return fail(SB200_ERR_INVALID, "the blob holds %d cnt entries outside 1..%d", bad[0], K);
     if (bad[1]) return fail(SB200_ERR_INVALID, "the blob holds %d start entries outside 0..%d", bad[1], K - 1);
-    if (int rc = move_columns(1, h, const_cast<char*>(dblob))) return rc;
+    if (bad_w) return fail(SB200_ERR_INVALID, "the blob holds %d windows with t_start > t_end", bad_w);
+    if (int rc = move_columns(1, sec_off, sec_bytes, rule ? SB200_FSTORE_BLOB_SECTIONS_V2 : SB200_FSTORE_BLOB_SECTIONS,
+                              const_cast<char*>(dblob)))
+      return rc;
     hid = std::move(blob_ids);
     for (size_t p = 0; p < hid.size(); ++p) hpos[hid[p]] = (int)p;
     return 0;
@@ -822,12 +1089,14 @@ void sb200_fstore_destroy(sb200_fstore* s) {
 
 int sb200_fstore_add(sb200_fstore* s, int32_t n, const uint64_t* ids, const float* features) {
   if (!s) return no_handle();
+  if (int rc = s->refuse_gated()) return rc;
   return s->add(n, ids, {features, false, nullptr});
 }
 
 int sb200_fstore_search(sb200_fstore* s, int32_t n_queries, const uint64_t* query_ids, const int32_t* obs_offsets,
                         const float* features, int32_t* counts, uint64_t* winners, double* weights) {
   if (!s) return no_handle();
+  if (int rc = s->refuse_gated()) return rc;
   return s->run_queries(n_queries, query_ids, obs_offsets, {features, false, nullptr}, counts, winners, weights, nullptr,
                         nullptr, false);
 }
@@ -836,6 +1105,7 @@ int sb200_fstore_associate(sb200_fstore* s, int32_t n_queries, const uint64_t* q
                            const float* features, int32_t* counts, uint64_t* winners, double* weights,
                            uint64_t* track_ids, uint8_t* merged) {
   if (!s) return no_handle();
+  if (int rc = s->refuse_gated()) return rc;
   return s->run_queries(n_queries, query_ids, obs_offsets, {features, false, nullptr}, counts, winners, weights, track_ids,
                         merged, true);
 }
@@ -901,6 +1171,7 @@ int sb200_fstore_get_options(sb200_fstore* s, sb200_fstore_options* out, int32_t
 
 int sb200_fstore_add_device(sb200_fstore* s, int32_t n, const uint64_t* ids, const void* d_features, void* cuda_stream) {
   if (!s) return no_handle();
+  if (int rc = s->refuse_gated()) return rc;
   return s->add(n, ids, {d_features, true, static_cast<cudaStream_t>(cuda_stream)});
 }
 
@@ -908,6 +1179,7 @@ int sb200_fstore_search_device(sb200_fstore* s, int32_t n_queries, const uint64_
                                const int32_t* obs_offsets, const void* d_features, int32_t* counts, uint64_t* winners,
                                double* weights, void* cuda_stream) {
   if (!s) return no_handle();
+  if (int rc = s->refuse_gated()) return rc;
   return s->run_queries(n_queries, query_ids, obs_offsets, {d_features, true, static_cast<cudaStream_t>(cuda_stream)},
                         counts, winners, weights, nullptr, nullptr, false);
 }
@@ -917,8 +1189,65 @@ int sb200_fstore_associate_device(sb200_fstore* s, int32_t n_queries, const uint
                                   uint64_t* winners, double* weights, uint64_t* track_ids, uint8_t* merged,
                                   void* cuda_stream) {
   if (!s) return no_handle();
+  if (int rc = s->refuse_gated()) return rc;
   return s->run_queries(n_queries, query_ids, obs_offsets, {d_features, true, static_cast<cudaStream_t>(cuda_stream)},
                         counts, winners, weights, track_ids, merged, true);
+}
+
+int sb200_fstore_set_gate(sb200_fstore* s, int32_t rule) {
+  if (!s) return no_handle();
+  return s->set_gate(rule);
+}
+
+int sb200_fstore_get_gate(sb200_fstore* s, int32_t* out) {
+  if (!s) return no_handle();
+  if (!out) return fail(SB200_ERR_INVALID, "out is NULL");
+  *out = s->gate;
+  return 0;
+}
+
+// the feature column of an _attr call: exactly one of a host and a device pointer
+static int attr_column(int n, const float* features, const void* d_features, void* cuda_stream, Column* col) {
+  if (n > 0 && (features == nullptr) == (d_features == nullptr))
+    return fail(SB200_ERR_INVALID, "exactly one of features and d_features must be non-NULL");
+  *col = d_features ? Column{d_features, true, static_cast<cudaStream_t>(cuda_stream)} : Column{features, false, nullptr};
+  return 0;
+}
+
+int sb200_fstore_add_attr(sb200_fstore* s, int32_t n, const uint64_t* ids, const sb200_fstore_attrs* attrs,
+                          const float* features, const void* d_features, void* cuda_stream) {
+  if (!s) return no_handle();
+  if (int rc = s->check_attrs(n, attrs)) return rc;
+  Column col;
+  if (int rc = attr_column(n, features, d_features, cuda_stream, &col)) return rc;
+  return s->add(n, ids, col, attrs);
+}
+
+int sb200_fstore_search_attr(sb200_fstore* s, int32_t n_queries, const uint64_t* query_ids, const int32_t* obs_offsets,
+                             const sb200_fstore_attrs* attrs, const float* features, const void* d_features,
+                             int32_t* counts, uint64_t* winners, double* weights, void* cuda_stream) {
+  if (!s) return no_handle();
+  if (int rc = s->check_attrs(n_queries, attrs)) return rc;
+  Column col;
+  if (int rc = attr_column(n_queries, features, d_features, cuda_stream, &col)) return rc;
+  return s->run_queries(n_queries, query_ids, obs_offsets, col, counts, winners, weights, nullptr, nullptr, false, attrs);
+}
+
+int sb200_fstore_associate_attr(sb200_fstore* s, int32_t n_queries, const uint64_t* query_ids,
+                                const int32_t* obs_offsets, const sb200_fstore_attrs* attrs, const float* features,
+                                const void* d_features, int32_t* counts, uint64_t* winners, double* weights,
+                                uint64_t* track_ids, uint8_t* merged, void* cuda_stream) {
+  if (!s) return no_handle();
+  if (int rc = s->check_attrs(n_queries, attrs)) return rc;
+  Column col;
+  if (int rc = attr_column(n_queries, features, d_features, cuda_stream, &col)) return rc;
+  return s->run_queries(n_queries, query_ids, obs_offsets, col, counts, winners, weights, track_ids, merged, true, attrs);
+}
+
+int64_t sb200_fstore_fetch_attr(sb200_fstore* s, int32_t n, const uint64_t* ids, uint64_t* source, int64_t* t_start,
+                                int64_t* t_end) {
+  if (!s) return no_handle();
+  return s->fetch_attr(n, ids, source, t_start, t_end);
 }
 
 int sb200_fstore_search_owned(sb200_fstore* s, int32_t n, const uint64_t* ids, int32_t each, int32_t* counts,
@@ -949,8 +1278,22 @@ int sb200_fstore_load(const void* buf, uint64_t bytes, int32_t device, sb200_fst
   BlobHeader h;
   CU(cudaMemcpy(&h, buf, sizeof(h), cudaMemcpyDefault));
   if (h.magic != SB200_FSTORE_BLOB_MAGIC) return fail(SB200_ERR_INVALID, "not a feature store blob (bad magic)");
-  if (h.version != SB200_FSTORE_BLOB_VERSION)
-    return fail(SB200_ERR_INVALID, "feature store blob version %u (this library reads %u)", h.version, SB200_FSTORE_BLOB_VERSION);
+  if (h.version != SB200_FSTORE_BLOB_VERSION && h.version != SB200_FSTORE_BLOB_VERSION_GATED)
+    return fail(SB200_ERR_INVALID, "feature store blob version %u (this library reads %u and %u)", h.version,
+                SB200_FSTORE_BLOB_VERSION, SB200_FSTORE_BLOB_VERSION_GATED);
+  // version 2 (a gated store): the same fields, the rule and a 7-section table
+  const bool v2 = h.version == SB200_FSTORE_BLOB_VERSION_GATED;
+  BlobHeaderV2 h2;
+  memset(&h2, 0, sizeof(h2));
+  if (v2) {
+    if (bytes < sizeof(h2)) return fail(SB200_ERR_INVALID, "the blob is truncated (%llu bytes)", (unsigned long long)bytes);
+    CU(cudaMemcpy(&h2, buf, sizeof(h2), cudaMemcpyDefault));
+    if (h2.gate != SB200_FSTORE_GATE_SAME_SOURCE && h2.gate != SB200_FSTORE_GATE_ANY_SOURCE)
+      return fail(SB200_ERR_INVALID, "a version-2 blob with unknown gate rule %d", h2.gate);
+  }
+  const int nsec = v2 ? SB200_FSTORE_BLOB_SECTIONS_V2 : SB200_FSTORE_BLOB_SECTIONS;
+  const uint64_t* sec_off = v2 ? h2.sec_off : h.sec_off;
+  const uint64_t* sec_bytes = v2 ? h2.sec_bytes : h.sec_bytes;
   if (h.total_bytes > bytes)
     return fail(SB200_ERR_INVALID, "the blob is truncated (%llu of total_bytes %llu)", (unsigned long long)bytes,
                 (unsigned long long)h.total_bytes);
@@ -964,23 +1307,25 @@ int sb200_fstore_load(const void* buf, uint64_t bytes, int32_t device, sb200_fst
   // live * K indexes the distance matrix's columns as an int
   if (h.live < 0 || h.live > INT32_MAX / h.max_observations) return fail(SB200_ERR_INVALID, "live count out of range");
   const uint64_t live = (uint64_t)h.live;
-  const uint64_t want[SB200_FSTORE_BLOB_SECTIONS] = {live * 8, live * 4, live * 4,
-                                                     live * h.max_observations * h.d8 * type_bytes(h.storage_type)};
-  static const char* const kName[SB200_FSTORE_BLOB_SECTIONS] = {"ids", "cnt", "start", "feat"};
-  if (int rc = sb::check_section_table(h, SB200_FSTORE_BLOB_SECTIONS, kName)) return rc;
-  for (int i = 0; i < SB200_FSTORE_BLOB_SECTIONS; ++i)
-    if (h.sec_bytes[i] != want[i])
+  const uint64_t want[SB200_FSTORE_BLOB_SECTIONS_V2] = {live * 8, live * 4, live * 4,
+                                                        live * h.max_observations * h.d8 * type_bytes(h.storage_type),
+                                                        live * 8, live * 8, live * 8};
+  static const char* const kName[SB200_FSTORE_BLOB_SECTIONS_V2] = {"ids", "cnt", "start", "feat", "source", "t_start",
+                                                                   "t_end"};
+  if (int rc = v2 ? sb::check_section_table(h2, nsec, kName) : sb::check_section_table(h, nsec, kName)) return rc;
+  for (int i = 0; i < nsec; ++i)
+    if (sec_bytes[i] != want[i])
       return fail(SB200_ERR_INVALID, "section %s holds %llu bytes, %llu expected", kName[i],
-                  (unsigned long long)h.sec_bytes[i], (unsigned long long)want[i]);
+                  (unsigned long long)sec_bytes[i], (unsigned long long)want[i]);
   std::vector<uint64_t> blob_ids(live);
-  if (live) CU(cudaMemcpy(blob_ids.data(), static_cast<const char*>(buf) + h.sec_off[kSecIds], live * 8, cudaMemcpyDefault));
+  if (live) CU(cudaMemcpy(blob_ids.data(), static_cast<const char*>(buf) + sec_off[kSecIds], live * 8, cudaMemcpyDefault));
   std::unordered_set<uint64_t> seen;
   seen.reserve(live * 2);
   for (uint64_t id : blob_ids)
     if (!seen.insert(id).second) return fail(SB200_ERR_INVALID, "id %llu appears twice in the blob", (unsigned long long)id);
   sb200_fstore* s = nullptr;
   if (int rc = sb200_fstore_create(&o, &s)) return rc;
-  if (int rc = s->load(h, buf, std::move(blob_ids))) {
+  if (int rc = s->load(h, v2 ? h2.gate : SB200_FSTORE_GATE_NONE, sec_off, sec_bytes, buf, std::move(blob_ids))) {
     sb200_fstore_destroy(s);   // the handle owns every buffer made so far
     return rc;
   }
@@ -999,6 +1344,8 @@ void fstore_info(sb200_fstore* s, int* device, int* feature_dim, int* topn) {
   *feature_dim = s->o.feature_dim;
   *topn = s->o.topn;
 }
+
+int fstore_gate(sb200_fstore* s) { return s->gate; }
 
 int fstore_associate_rows(sb200_fstore* s, int Q, const uint64_t* qids, const int32_t* offs, const FsRowSource& src,
                           int32_t* counts, uint64_t* winners, double* weights, uint64_t* track_ids, uint8_t* merged) {

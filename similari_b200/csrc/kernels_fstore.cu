@@ -12,6 +12,9 @@
 //   TrackStore::merge_external / add_track / add (src/track/store.rs:265-277, 510-580, 625-691)
 //   TrackStore::owned_track_distances / merge_owned (src/track/store.rs:471-486, 584-611): the owned stage, the
 //   distance / TopN instances of the owned modes and the two-launch row move
+//   Track::distances' attributes.compatible check and Track::merge's attributes.merge (src/track.rs:604-652, 522-530)
+//   with examples/track_merging.rs:218-245's CamTrackingAttributes, for a gated store: the gated distance instances,
+//   fs_gate_resolve_kernel and the attribute kernels
 // Every value that reaches the voting stage is the oracle's f32 bit for bit: --fmad=false, 8-lane blocks reduced by
 // reduce_add8 and accumulated one after another, then sqrt (euclidean) or the quotient by sqrt(|a|^2 |b|^2) (cosine).
 #include <climits>
@@ -107,14 +110,29 @@ constexpr int kDT = 64;
 constexpr int kDC = 4;
 constexpr int kDP = kDC * 8 + 4;
 
+// The gate of a gated store: the empty pack (every ungated instance) passes every pair; a gated instance takes one FsGate
+// after the existing parameters and drops the pairs that are not compatible, in the epilogue, as filtered entries.
+struct FsTriple {
+  unsigned long long src;
+  long long t0, t1;
+};
+__device__ __forceinline__ FsTriple fs_stored_triple(int) { return FsTriple{}; }
+__device__ __forceinline__ FsTriple fs_stored_triple(int t, const FsGate& g) {
+  return FsTriple{g.st.src[t], g.st.t0[t], g.st.t1[t]};
+}
+__device__ __forceinline__ bool fs_gate_pass(int, const FsTriple&) { return true; }
+__device__ __forceinline__ bool fs_gate_pass(int q, const FsTriple& b, const FsGate& g) {
+  return fs_compatible(g.rule, g.qsrc[q], g.qt0[q], g.qt1[q], b.src, b.t0, b.t1);
+}
+
 // MODE (kFsForeign / kFsOwnedGroup / kFsOwnedEach) changes the epilogue only: the group mode drops every entry of a
 // queried track (excl), the each mode folds max_dist per query (per row across its 16 threads, then one atomicMax per row).
 // Elem changes the staging of the stored (B) rows only: a 2-byte row block of 8 elements is one 16-byte load, widened
 // into the same f32 tile, so 64 rows x kDC blocks are one load per thread; everything after the tile is the same.
 static_assert(kDT * kDC == 256, "one 16-byte load of stored 2-byte elements per thread and stage");
-template <typename Elem, int METRIC, int MODE>
+template <typename Elem, int METRIC, int MODE, typename... Gate>
 __global__ void __launch_bounds__(256) fs_dist_kernel(FsStore s, FsCall c, float filter, int tiles_s,
-                                                      const unsigned char* __restrict__ excl) {
+                                                      const unsigned char* __restrict__ excl, Gate... gate) {
   __shared__ __align__(16) float sa[kDT][kDP];
   __shared__ __align__(16) float sbm[kDT][kDP];
   __shared__ int s_max[8];
@@ -205,6 +223,7 @@ __global__ void __launch_bounds__(256) fs_dist_kernel(FsStore s, FsCall c, float
     if (MODE == kFsOwnedGroup) filled = filled && !excl[t];
     const unsigned long long tid_ = s.ids[t];
     const float sn = METRIC == 1 ? c.snorm[col] : 0.0f;
+    const FsTriple tt = fs_stored_triple(t, gate...);   // once per stored track of the column
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       const int row = r0 + ty + 16 * i;
@@ -212,7 +231,7 @@ __global__ void __launch_bounds__(256) fs_dist_kernel(FsStore s, FsCall c, float
       float d;
       if (METRIC == 0) d = sqrtf(acc[i][j]);
       else d = 1.0f - acc[i][j] / sqrtf(c.qnorm[row] * sn);
-      const bool keep = filled && c.qid[c.row_q[row]] != tid_ && d < filter;
+      const bool keep = filled && c.qid[c.row_q[row]] != tid_ && d < filter && fs_gate_pass(c.row_q[row], tt, gate...);
       c.dist[(size_t)row * S + col] = keep ? d : nan;
       if (MODE == kFsOwnedEach) {
         if (keep) rmax[i] = max(rmax[i], fs_key(d));
@@ -394,6 +413,74 @@ __global__ void __launch_bounds__(kOrderThreads) fs_order_kernel(FsStore s, FsCa
   }
 }
 
+// ------------------------------------------------------------------------------------------------ gate (associate)
+// One CTA, queries in chunks of kOrderThreads.  In each chunk the first query of every destination walks the chunk's
+// queries with that destination in order, carrying the window in the stored columns from one chunk to the next.
+__global__ void __launch_bounds__(kOrderThreads) fs_gate_resolve_kernel(FsCall c, FsGate g) {
+  __shared__ int s_d[kOrderThreads];
+  const int tid = threadIdx.x;
+  for (int base = 0; base < c.Q; base += kOrderThreads) {
+    const int n = min(kOrderThreads, c.Q - base);
+    const int d = tid < n ? c.dest[base + tid] : -1;
+    s_d[tid] = d;
+    __syncthreads();
+    bool lead = d >= 0;
+    for (int j = 0; j < tid && lead; ++j) lead = s_d[j] != d;
+    if (lead) {
+      const unsigned long long src = g.st.src[d];
+      long long w0 = g.st.t0[d], w1 = g.st.t1[d];
+      for (int j = tid; j < n; ++j) {
+        if (s_d[j] != d) continue;
+        const int q = base + j;
+        const long long q0 = g.qt0[q], q1 = g.qt1[q];
+        if (fs_compatible(g.rule, g.qsrc[q], q0, q1, src, w0, w1)) {
+          w0 = min(w0, q0);
+          w1 = max(w1, q1);
+        } else {
+          c.dest[q] = -1;
+        }
+      }
+      g.st.t0[d] = w0;
+      g.st.t1[d] = w1;
+    }
+    __syncthreads();   // the windows and dest[] of this chunk precede the next chunk's reads
+  }
+}
+
+__global__ void fs_attr_new_kernel(int live, FsCall c, FsGate g) {
+  const int q = blockIdx.x * blockDim.x + threadIdx.x;
+  if (q >= c.Q) return;
+  const int p = c.dest[q];
+  if (p < live) return;
+  g.st.src[p] = g.qsrc[q];
+  g.st.t0[p] = g.qt0[q];
+  g.st.t1[p] = g.qt1[q];
+}
+
+__global__ void fs_attr_gather_kernel(FsAttrCols a, const int* __restrict__ pos, int n, FsAttrCols out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int p = pos[i];
+  out.src[i] = p >= 0 ? a.src[p] : 0ull;
+  out.t0[i] = p >= 0 ? a.t0[p] : 0ll;
+  out.t1[i] = p >= 0 ? a.t1[p] : 0ll;
+}
+
+__global__ void fs_attr_scatter_kernel(FsAttrCols a, const int* __restrict__ pos, int n, FsAttrCols in) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int p = pos[i];
+  a.src[p] = in.src[i];
+  a.t0[p] = in.t0[i];
+  a.t1[p] = in.t1[i];
+}
+
+__global__ void fs_attr_check_kernel(const long long* __restrict__ t0, const long long* __restrict__ t1, int n, int* bad) {
+  int b = 0;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) b += t0[i] > t1[i];
+  if (b) atomicAdd(bad, b);
+}
+
 // One CTA per item: writes the item's surviving rows into their ring slots.  A 2-byte store rounds each f32 element
 // once (fs_round8): one thread per 8-element block, one 16-byte store.
 template <typename Elem>
@@ -570,15 +657,23 @@ __global__ void fs_blob_scrub_kernel(Elem* feat, const int* __restrict__ cnt, co
 
 }  // namespace
 
-template <typename Elem, int MODE>
+template <typename Elem, int MODE, typename... Gate>
 void fs_dist_grid(int metric, float filter, const FsStore& s, const FsCall& c, int tiles_s, unsigned grid,
-                  const unsigned char* excl, cudaStream_t st) {
-  if (metric == 0) fs_dist_kernel<Elem, 0, MODE><<<grid, 256, 0, st>>>(s, c, filter, tiles_s, excl);
-  else fs_dist_kernel<Elem, 1, MODE><<<grid, 256, 0, st>>>(s, c, filter, tiles_s, excl);
+                  const unsigned char* excl, cudaStream_t st, Gate... gate) {
+  if (metric == 0) fs_dist_kernel<Elem, 0, MODE><<<grid, 256, 0, st>>>(s, c, filter, tiles_s, excl, gate...);
+  else fs_dist_kernel<Elem, 1, MODE><<<grid, 256, 0, st>>>(s, c, filter, tiles_s, excl, gate...);
+}
+
+template <typename Elem, typename... Gate>
+void fs_dist_mode(int mode, int metric, float filter, const FsStore& s, const FsCall& c, int tiles_s, unsigned grid,
+                  const unsigned char* excl, cudaStream_t st, Gate... gate) {
+  if (mode == kFsOwnedGroup) fs_dist_grid<Elem, kFsOwnedGroup>(metric, filter, s, c, tiles_s, grid, excl, st, gate...);
+  else if (mode == kFsOwnedEach) fs_dist_grid<Elem, kFsOwnedEach>(metric, filter, s, c, tiles_s, grid, excl, st, gate...);
+  else fs_dist_grid<Elem, kFsForeign>(metric, filter, s, c, tiles_s, grid, excl, st, gate...);
 }
 
 void fs_launch_dist(int metric, float filter, const FsStore& s, const FsCall& c, cudaStream_t st, int mode,
-                    const unsigned char* excl) {
+                    const unsigned char* excl, const FsGate* gate) {
   const long long S = (long long)s.live * s.K;
   if (c.R == 0 || S == 0) return;
   const int tiles_s = (int)((S + kDT - 1) / kDT), tiles_r = (c.R + kDT - 1) / kDT;
@@ -590,9 +685,8 @@ void fs_launch_dist(int metric, float filter, const FsStore& s, const FsCall& c,
       fs_norm_kernel<Elem><<<(unsigned)((warps * 32 + 255) / 256), 256, 0, st>>>(s, c);
       note_launch();
     }
-    if (mode == kFsOwnedGroup) fs_dist_grid<Elem, kFsOwnedGroup>(metric, filter, s, c, tiles_s, grid, excl, st);
-    else if (mode == kFsOwnedEach) fs_dist_grid<Elem, kFsOwnedEach>(metric, filter, s, c, tiles_s, grid, excl, st);
-    else fs_dist_grid<Elem, kFsForeign>(metric, filter, s, c, tiles_s, grid, excl, st);
+    if (gate) fs_dist_mode<Elem>(mode, metric, filter, s, c, tiles_s, grid, excl, st, *gate);
+    else fs_dist_mode<Elem>(mode, metric, filter, s, c, tiles_s, grid, excl, st);
   });
   note_launch();
 }
@@ -644,6 +738,36 @@ void fs_launch_apply(const FsStore& s, const FsCall& c, cudaStream_t st) {
   fs_order_kernel<<<1, kOrderThreads, 0, st>>>(s, c);
   feat_dispatch(s.stype, [&](auto tag) { fs_apply_kernel<decltype(tag)><<<c.Q, 128, 0, st>>>(s, c); });
   note_launch(2);
+}
+
+void fs_launch_gate_resolve(const FsCall& c, const FsGate& g, cudaStream_t st) {
+  if (c.Q == 0) return;
+  fs_gate_resolve_kernel<<<1, kOrderThreads, 0, st>>>(c, g);
+  note_launch();
+}
+
+void fs_launch_attr_new(int live, const FsCall& c, const FsGate& g, cudaStream_t st) {
+  if (c.Q == 0) return;
+  fs_attr_new_kernel<<<(c.Q + 255) / 256, 256, 0, st>>>(live, c, g);
+  note_launch();
+}
+
+void fs_launch_attr_gather(const FsAttrCols& a, const int* pos, int n, const FsAttrCols& out, cudaStream_t st) {
+  if (n == 0) return;
+  fs_attr_gather_kernel<<<(n + 255) / 256, 256, 0, st>>>(a, pos, n, out);
+  note_launch();
+}
+
+void fs_launch_attr_scatter(const FsAttrCols& a, const int* pos, int n, const FsAttrCols& in, cudaStream_t st) {
+  if (n == 0) return;
+  fs_attr_scatter_kernel<<<(n + 255) / 256, 256, 0, st>>>(a, pos, n, in);
+  note_launch();
+}
+
+void fs_launch_attr_check(const long long* t0, const long long* t1, int n, int* bad, cudaStream_t st) {
+  if (n == 0) return;
+  fs_attr_check_kernel<<<std::min((n + 255) / 256, 1024), 256, 0, st>>>(t0, t1, n, bad);
+  note_launch();
 }
 
 void fs_launch_gather(const FsStore& s, const int* pos, int n, float* out, int* out_cnt, cudaStream_t st) {

@@ -1,7 +1,7 @@
 // sb_fstore.cuh -- device side of the feature track store (csrc/kernels_fstore.cu), shared with its host side
-// (csrc/fstore.cu).  The store is the reference's TrackStore specialised to feature-only tracks: one feature class, no
-// track attributes, the newest `max_observations` (K) observations of each track (src/track/store.rs,
-// benches/feature_tracker.rs).
+// (csrc/fstore.cu).  The store is the reference's TrackStore specialised to feature-only tracks: one feature class, the
+// newest `max_observations` (K) observations of each track (src/track/store.rs, benches/feature_tracker.rs), and, in a
+// gated store only, the CamTrackingAttributes of examples/track_merging.rs as track attributes (FsAttrCols, FsGate).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -51,6 +51,31 @@ struct FsCall {
   int Q, R;
 };
 
+// Track attributes of a gated store (sb200_fstore_set_gate): per stored track a source id and a [t0, t1] window, in
+// columns of their own so that FsStore and FsCall keep their layout (CamTrackingAttributes, examples/track_merging.rs:
+// 218-245).  An ungated store has none, and its kernels never see these structs.
+struct FsAttrCols {
+  unsigned long long* src;   // [cap]
+  long long* t0;             // [cap]
+  long long* t1;             // [cap]
+};
+// What the gated instances read: the stored columns, one triple per query of the call ([Q], indexed through row_q for
+// a request row) and the rule (SB200_FSTORE_GATE_SAME_SOURCE or _ANY_SOURCE).
+struct FsGate {
+  FsAttrCols st;
+  const unsigned long long* qsrc;
+  const long long* qt0;
+  const long long* qt1;
+  int rule;
+};
+
+// CamTrackingAttributes::compatible (examples/track_merging.rs:222-225): the windows are disjoint, touching windows
+// counting as disjoint, and under SB200_FSTORE_GATE_SAME_SOURCE (1) the sources are equal.  Symmetric in a and b.
+__host__ __device__ __forceinline__ bool fs_compatible(int rule, unsigned long long as, long long a0, long long a1,
+                                                       unsigned long long bs, long long b0, long long b1) {
+  return (a0 >= b1 || a1 <= b0) && (rule != 1 || as == bs);
+}
+
 // How an owned search (sb200_fstore_search_owned) differs from a search of foreign queries, as template parameters of
 // the distance and TopN kernels: kFsForeign is the search / associate path; kFsOwnedGroup drops the entries of the
 // tracks marked in excl[live] (the queried ones); kFsOwnedEach folds max_dist per query into maxkey[Q].
@@ -81,8 +106,9 @@ void fs_launch_stage(int type, const void* col, const int* row_src, int R, int D
 // rows[r][0 .. d8) = observation r - qoff[q] (oldest first) of the stored track at qpos[q], q = row_q[r]
 void fs_launch_owned_stage(const FsStore& s, const FsCall& c, const int* qpos, float* rows, cudaStream_t st);
 // mode: kFsForeign, kFsOwnedGroup (excl[live] marks the queried tracks) or kFsOwnedEach
+// gate: a gated store's attributes; the pairs it finds incompatible are dropped like filtered ones (NaN)
 void fs_launch_dist(int metric, float filter, const FsStore& s, const FsCall& c, cudaStream_t st, int mode = kFsForeign,
-                    const unsigned char* excl = nullptr);
+                    const unsigned char* excl = nullptr, const FsGate* gate = nullptr);
 void fs_launch_topn(float max_distance, int min_votes, int topn, bool want_dest, const FsStore& s, const FsCall& c,
                     cudaStream_t st, int mode = kFsForeign);
 // out[2 i] = cnt[pos[i]], out[2 i + 1] = start[pos[i]]: the ring state of the tracks an owned call touches
@@ -98,6 +124,19 @@ void fs_launch_apply(const FsStore& s, const FsCall& c, cudaStream_t st);
 void fs_launch_gather(const FsStore& s, const int* pos, int n, float* out, int* out_cnt, cudaStream_t st);
 // dst[i] = src[from[i]] for the i < n kept tracks (stable compaction into fresh columns)
 void fs_launch_compact(const FsStore& src, const FsStore& dst, const int* from, int n, cudaStream_t st);
+// gated associate, between TopN and apply: in query order, a query stays with its first winner (dest[q]) only if it is
+// compatible with that track's window as extended by the queries kept with it before; else dest[q] = -1 (a new track).
+// The kept queries' hulls are written into the stored windows.
+void fs_launch_gate_resolve(const FsCall& c, const FsGate& g, cudaStream_t st);
+// gated associate, after apply: the triple of every query that became a new track (dest[q] >= live) into its position
+void fs_launch_attr_new(int live, const FsCall& c, const FsGate& g, cudaStream_t st);
+// out[i] = the triple at pos[i] (0 for pos[i] < 0): read-back of touched tracks, the triples of owned queries and the
+// compaction of fetch(remove) (out = fresh columns, pos = the kept positions)
+void fs_launch_attr_gather(const FsAttrCols& a, const int* pos, int n, const FsAttrCols& out, cudaStream_t st);
+// the triple at pos[i] = in[i]
+void fs_launch_attr_scatter(const FsAttrCols& a, const int* pos, int n, const FsAttrCols& in, cudaStream_t st);
+// store blob of a gated store, before anything is copied: bad[0] counts the windows with t0 > t1
+void fs_launch_attr_check(const long long* t0, const long long* t1, int n, int* bad, cudaStream_t st);
 // store blob, before any row is copied: bad[0] counts the cnt[i] outside [1, K], bad[1] the start[i] outside [0, K)
 void fs_launch_blob_check(const int* cnt, const int* start, int n, int K, int* bad, cudaStream_t st);
 // store blob, after its rows are copied: zeroes, in feat[n][K][d8] (elements of stype), the ring slots that hold no

@@ -105,6 +105,9 @@ int64_t sb200_fstore_associate_wasted(sb200_fstore* s, sb200_tracker* t, int64_t
                                       uint64_t* track_ids, uint8_t* merged) {
   if (!s || !t) return fail(SB200_ERR_INVALID, "store / tracker is NULL");
   if (cap < 0 || history_cap < 0) return fail(SB200_ERR_INVALID, "cap < 0 or history_cap < 0");
+  if (sb::fstore_gate(s))
+    return fail(SB200_ERR_INVALID, "associate_wasted needs an ungated store: a wasted record has no exact window (the "
+                                   "tracker keeps no birth epoch)");
   const sb::TrackerFeatureInfo ti = sb::tracker_feature_info(t);
   if (!ti.visual) return fail(SB200_ERR_INVALID, "the tracker is not a visual tracker");
   if (!ti.history) return fail(SB200_ERR_INVALID, "the tracker's feature history is off (sb200_set_feature_history)");

@@ -654,6 +654,9 @@ def nms_batch_device(offsets, d_boxes, d_scores, nms_threshold, score_threshold,
 
 
 METRICS = {"euclidean": _lib.VIS_EUCLIDEAN, "cosine": _lib.VIS_COSINE}
+# track attribute rules of the feature store (sb200_fstore_set_gate)
+GATES = {None: _lib.FSTORE_GATE_NONE, "same_source": _lib.FSTORE_GATE_SAME_SOURCE,
+         "any_source": _lib.FSTORE_GATE_ANY_SOURCE}
 
 
 class FeatureStore:
@@ -671,14 +674,22 @@ class FeatureStore:
     Storage: `storage` ("f32", "f16" or "bf16") is the element type of the stored rows (sb200_fstore_set_storage_type).
     A 2-byte store takes half the device memory and half the blob; each row is rounded to it once, when it is stored,
     and queries are never rounded.  Fed features of its own type, a 2-byte store returns exactly what an f32 store
-    returns; fetch() returns the stored values as float32."""
+    returns; fetch() returns the stored values as float32.
+
+    Gate: with gate="same_source" or "any_source" every track carries a source id and a [t_start, t_end] window (the
+    CamTrackingAttributes of the reference's examples/track_merging.rs), and a query and a track are compared, and
+    merged, only when their windows are disjoint (touching counts as disjoint) and, for "same_source", their sources are
+    equal.  add / search / associate and their _device forms then need sources=, t_start= and t_end= (one per row or
+    query); attributes(ids) returns the stored ones.  gate=None (the default) is the store without attributes."""
 
     def __init__(self, metric="euclidean", distance_filter=100.0, max_observations=3, feature_dim=256, topn=1,
-                 max_distance=100.0, min_votes=1, device=0, storage="f32"):
+                 max_distance=100.0, min_votes=1, device=0, storage="f32", gate=None):
         if metric not in METRICS:
             raise ValueError(f"metric must be one of {sorted(METRICS)}")
         if storage not in FEATURE_TYPES:
             raise ValueError(f"storage must be one of {sorted(FEATURE_TYPES)}")
+        if gate not in GATES:
+            raise ValueError(f"gate must be one of {list(GATES)}")
         self._L = lib()
         o = _lib.FstoreOptions(METRICS[metric], distance_filter, max_observations, feature_dim, topn, max_distance,
                                min_votes, device)
@@ -688,6 +699,24 @@ class FeatureStore:
         self.K, self.D, self.topn = int(max_observations), int(feature_dim), int(topn)
         self._explicit_type = None
         check(self._L.sb200_fstore_set_storage_type(h, FEATURE_TYPES[storage]))
+        check(self._L.sb200_fstore_set_gate(h, GATES[gate]))
+        self.gate = gate
+
+    def _attrs(self, n, sources, t_start, t_end):
+        """The sb200_fstore_attrs of a call (and the arrays it points into), or None for an ungated store.  The three
+        keywords are required on a gated store and refused on an ungated one."""
+        given = [a is not None for a in (sources, t_start, t_end)]
+        if self.gate is None:
+            if any(given):
+                raise ValueError("sources / t_start / t_end need a gated store (FeatureStore(gate=...))")
+            return None
+        if not all(given):
+            raise ValueError(f"a gated store (gate={self.gate!r}) needs sources, t_start and t_end")
+        cols = (np.ascontiguousarray(sources, dtype=np.uint64), np.ascontiguousarray(t_start, dtype=np.int64),
+                np.ascontiguousarray(t_end, dtype=np.int64))
+        if any(c.shape != (n,) for c in cols):
+            raise ValueError("sources / t_start / t_end need one entry per row (add) or query (search / associate)")
+        return _lib.FstoreAttrs(*(c.ctypes.data for c in cols)), cols
 
     def close(self):
         if getattr(self, "_h", None):
@@ -734,21 +763,31 @@ class FeatureStore:
         check(self._L.sb200_fstore_set_feature_type(self._h, _lib.FEATURE_F32))
         return _f32(features).reshape(-1, self.D)
 
-    def add(self, ids, features):
-        """TrackStore::add for each (ids[i], features[i]) in order."""
+    def add(self, ids, features, sources=None, t_start=None, t_end=None):
+        """TrackStore::add for each (ids[i], features[i]) in order (a gated store: with sources[i] and the window
+        [t_start[i], t_end[i]])."""
         ids = np.ascontiguousarray(ids, dtype=np.uint64)
+        a = self._attrs(len(ids), sources, t_start, t_end)
         f = self._column(features)
         if len(f) != len(ids):
             raise ValueError("features needs one row per id")
-        check(self._L.sb200_fstore_add(self._h, len(ids), ptr(ids), ptr(f)))
+        if a is None:
+            check(self._L.sb200_fstore_add(self._h, len(ids), ptr(ids), ptr(f)))
+        else:
+            check(self._L.sb200_fstore_add_attr(self._h, len(ids), ptr(ids), C.byref(a[0]), ptr(f), None, None))
 
-    def add_device(self, ids, d_features, stream=0):
+    def add_device(self, ids, d_features, stream=0, sources=None, t_start=None, t_end=None):
         """sb200_fstore_add_device: `d_features` is the raw device address of [len(ids)][feature_dim] elements of the
         type set by set_feature_type (e.g. the data_ptr() of a torch CUDA tensor)."""
         ids = np.ascontiguousarray(ids, dtype=np.uint64)
+        a = self._attrs(len(ids), sources, t_start, t_end)
         self._use_declared_type()
-        check(self._L.sb200_fstore_add_device(self._h, len(ids), ptr(ids), C.c_void_p(d_features or None),
-                                              C.c_void_p(stream or None)))
+        if a is None:
+            check(self._L.sb200_fstore_add_device(self._h, len(ids), ptr(ids), C.c_void_p(d_features or None),
+                                                  C.c_void_p(stream or None)))
+        else:
+            check(self._L.sb200_fstore_add_attr(self._h, len(ids), ptr(ids), C.byref(a[0]), None,
+                                                C.c_void_p(d_features or None), C.c_void_p(stream or None)))
 
     def _queries(self, ids, offsets, features):
         ids = np.ascontiguousarray(ids, dtype=np.uint64)
@@ -765,43 +804,64 @@ class FeatureStore:
                "weights": np.zeros((q, self.topn), np.float64)}
         return ids, offs, f, out
 
-    def search(self, ids, offsets, features):
-        """foreign_track_distances + TopNVoting::winners: counts[q], winners[q][topn] (track ids), weights[q][topn]."""
+    def search(self, ids, offsets, features, sources=None, t_start=None, t_end=None):
+        """foreign_track_distances + TopNVoting::winners: counts[q], winners[q][topn] (track ids), weights[q][topn].  A
+        gated store takes one source and window per query; incompatible pairs neither vote nor count toward max_dist."""
+        a = self._attrs(len(ids), sources, t_start, t_end)
         ids, offs, f, out = self._queries(ids, offsets, features)
-        check(self._L.sb200_fstore_search(self._h, len(ids), ptr(ids), ptr(offs), ptr(f), ptr(out["counts"]),
-                                          ptr(out["winners"]), ptr(out["weights"])))
+        res = [ptr(out[k]) for k in ("counts", "winners", "weights")]
+        if a is None:
+            check(self._L.sb200_fstore_search(self._h, len(ids), ptr(ids), ptr(offs), ptr(f), *res))
+        else:
+            check(self._L.sb200_fstore_search_attr(self._h, len(ids), ptr(ids), ptr(offs), C.byref(a[0]), ptr(f), None,
+                                                   *res, None))
         return out
 
-    def associate(self, ids, offsets, features):
+    def associate(self, ids, offsets, features, sources=None, t_start=None, t_end=None):
         """search, then merge each query with a result into its first winner and add the others as new tracks.  Adds
-        track_ids[q] (where the query ended up) and merged[q] to the search outputs."""
+        track_ids[q] (where the query ended up) and merged[q] to the search outputs.  A gated store merges a query only
+        if it is compatible with its first winner's window as the queries merged into it earlier in the call extended it;
+        otherwise the query becomes a new track."""
+        a = self._attrs(len(ids), sources, t_start, t_end)
         ids, offs, f, out = self._queries(ids, offsets, features)
         out["track_ids"] = np.zeros(len(ids), np.uint64)
         out["merged"] = np.zeros(len(ids), np.uint8)
-        check(self._L.sb200_fstore_associate(self._h, len(ids), ptr(ids), ptr(offs), ptr(f), ptr(out["counts"]),
-                                             ptr(out["winners"]), ptr(out["weights"]), ptr(out["track_ids"]),
-                                             ptr(out["merged"])))
+        res = [ptr(out[k]) for k in ("counts", "winners", "weights", "track_ids", "merged")]
+        if a is None:
+            check(self._L.sb200_fstore_associate(self._h, len(ids), ptr(ids), ptr(offs), ptr(f), *res))
+        else:
+            check(self._L.sb200_fstore_associate_attr(self._h, len(ids), ptr(ids), ptr(offs), C.byref(a[0]), ptr(f),
+                                                      None, *res, None))
         return out
 
-    def search_device(self, ids, offsets, d_features, stream=0):
+    def search_device(self, ids, offsets, d_features, stream=0, sources=None, t_start=None, t_end=None):
         """sb200_fstore_search_device: search with the feature rows at the raw device address `d_features`."""
+        a = self._attrs(len(ids), sources, t_start, t_end)
         ids, offs, _, out = self._queries(ids, offsets, None)
         self._use_declared_type()
-        check(self._L.sb200_fstore_search_device(self._h, len(ids), ptr(ids), ptr(offs), C.c_void_p(d_features or None),
-                                                 ptr(out["counts"]), ptr(out["winners"]), ptr(out["weights"]),
-                                                 C.c_void_p(stream or None)))
+        res = [ptr(out[k]) for k in ("counts", "winners", "weights")]
+        d, st = C.c_void_p(d_features or None), C.c_void_p(stream or None)
+        if a is None:
+            check(self._L.sb200_fstore_search_device(self._h, len(ids), ptr(ids), ptr(offs), d, *res, st))
+        else:
+            check(self._L.sb200_fstore_search_attr(self._h, len(ids), ptr(ids), ptr(offs), C.byref(a[0]), None, d, *res,
+                                                   st))
         return out
 
-    def associate_device(self, ids, offsets, d_features, stream=0):
+    def associate_device(self, ids, offsets, d_features, stream=0, sources=None, t_start=None, t_end=None):
         """sb200_fstore_associate_device: associate with the feature rows at the raw device address `d_features`."""
+        a = self._attrs(len(ids), sources, t_start, t_end)
         ids, offs, _, out = self._queries(ids, offsets, None)
         self._use_declared_type()
         out["track_ids"] = np.zeros(len(ids), np.uint64)
         out["merged"] = np.zeros(len(ids), np.uint8)
-        check(self._L.sb200_fstore_associate_device(self._h, len(ids), ptr(ids), ptr(offs),
-                                                    C.c_void_p(d_features or None), ptr(out["counts"]),
-                                                    ptr(out["winners"]), ptr(out["weights"]), ptr(out["track_ids"]),
-                                                    ptr(out["merged"]), C.c_void_p(stream or None)))
+        res = [ptr(out[k]) for k in ("counts", "winners", "weights", "track_ids", "merged")]
+        d, st = C.c_void_p(d_features or None), C.c_void_p(stream or None)
+        if a is None:
+            check(self._L.sb200_fstore_associate_device(self._h, len(ids), ptr(ids), ptr(offs), d, *res, st))
+        else:
+            check(self._L.sb200_fstore_associate_attr(self._h, len(ids), ptr(ids), ptr(offs), C.byref(a[0]), None, d,
+                                                      *res, st))
         return out
 
     def search_owned(self, ids, each=False):
@@ -879,6 +939,17 @@ class FeatureStore:
         check(self._L.sb200_fstore_fetch(self._h, len(ids), ptr(ids), int(bool(remove)), ptr(counts), ptr(feats)))
         return counts, feats
 
+    def attributes(self, ids):
+        """(sources, t_start, t_end) of the tracks `ids` of a gated store, each an array with one entry per id (0 where
+        an id is not stored)."""
+        if self.gate is None:
+            raise ValueError("attributes() needs a gated store (FeatureStore(gate=...))")
+        ids = np.ascontiguousarray(ids, dtype=np.uint64)
+        n = len(ids)
+        src, t0, t1 = np.zeros(n, np.uint64), np.zeros(n, np.int64), np.zeros(n, np.int64)
+        check(self._L.sb200_fstore_fetch_attr(self._h, n, ptr(ids), ptr(src), ptr(t0), ptr(t1)))
+        return src, t0, t1
+
     def size(self):
         return int(check(self._L.sb200_fstore_size(self._h)))
 
@@ -923,4 +994,7 @@ class FeatureStore:
         self.K, self.D, self.topn = int(o.max_observations), int(o.feature_dim), int(o.topn)
         name = {v: k for k, v in FEATURE_TYPES.items()}[t.value]
         self._explicit_type = None if name == "f32" else name
+        g = C.c_int32(0)
+        check(L.sb200_fstore_get_gate(h, C.byref(g)))
+        self.gate = {v: k for k, v in GATES.items()}[g.value]
         return self
