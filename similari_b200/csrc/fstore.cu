@@ -10,6 +10,7 @@
 // sb200_fstore_set_storage_type); row_bytes() is the size of one stored row, and nothing else on the host depends on the
 // storage type.  A gated store (sb200_fstore_set_gate) also keeps a source and a window per track in three device
 // columns of its own; a call reads back the triples of the tracks it touches, and an ungated store allocates none.
+// Allocation, growth, compaction, the gate switch and the blob sections all go by one table of columns (kCols).
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -58,6 +59,21 @@ struct ReqLayout {
     total = o;
   }
 };
+// Stages what every request carries at hq, the host address of offset L.qid: ids, offsets, row -> query, dest (nullptr:
+// -1 for every query) and nkey initial max_dist keys.
+void stage_request(const ReqLayout& L, char* hq, int Q, const uint64_t* qids, const int* qoff, const int* dest, int nkey) {
+  auto at = [&](size_t off) { return hq + (off - L.qid); };
+  memcpy(at(L.qid), qids, (size_t)Q * 8);
+  memcpy(at(L.qoff), qoff, (size_t)(Q + 1) * 4);
+  int* row_q = reinterpret_cast<int*>(at(L.row_q));
+  for (int q = 0; q < Q; ++q)
+    for (int r = qoff[q]; r < qoff[q + 1]; ++r) row_q[r] = q;
+  int* d = reinterpret_cast<int*>(at(L.dest));
+  if (dest) memcpy(d, dest, (size_t)Q * 4);
+  else std::fill_n(d, Q, -1);
+  std::fill_n(reinterpret_cast<int*>(at(L.maxkey)), nkey, sb::fs_key(-1.0f));   // max_dist starts at -1.0 (topn.rs:78)
+}
+
 struct ResLayout {
   size_t w, cnt, pos, total;
   ResLayout(int Q, int topn) {
@@ -114,11 +130,17 @@ struct sb200_fstore {
   cudaEvent_t ev[4] = {};
   cudaEvent_t ev_in = nullptr;     // what the caller's stream held when a device-column call was made
   float stage_ms[3] = {0, 0, 0};
-  // store columns
+  // store columns (kCols)
   size_t cap = 0;
   DBuf feat, cnt, start, ids, run;
   int gate = SB200_FSTORE_GATE_NONE;
   DBuf asrc, at0, at1;                       // gated store: [cap] source, t_start, t_end
+  // A store column: its buffer, bytes per track (0: K stored rows), whether only a gated store has it, whether allocation
+  // zero-fills it, and its blob section (kSec*) and name.  Without a section (-1) it is scratch, which growth and
+  // compaction start afresh.
+  struct Col { DBuf sb200_fstore::*buf; uint32_t w; bool gated, zero; int sec; const char* name; };
+  static constexpr int kNumCols = 8;
+  static const Col kCols[kNumCols];
   DBuf qattr;                                // a gated call's triples, [n] of each column
   std::vector<uint64_t> hid;                 // ids in store order
   std::unordered_map<uint64_t, int> hpos;    // id -> store position
@@ -148,29 +170,49 @@ struct sb200_fstore {
   }
 
   // bytes of one stored row (observation)
-  size_t row_bytes() const { return (size_t)d8 * type_bytes(stype); }
+  static size_t row_bytes(int d8, int stype) { return (size_t)d8 * type_bytes(stype); }
+  size_t row_bytes() const { return row_bytes(d8, stype); }
+  static size_t track_bytes(const Col& c, int K, size_t row_bytes) { return c.w ? c.w : K * row_bytes; }
+  size_t track_bytes(const Col& c) const { return track_bytes(c, o.max_observations, row_bytes()); }
+  static bool has(const Col& c, int gate) { return gate || !c.gated; }   // a store with rule `gate` has column c
+  // The blob sections of a store of `live` tracks (kSec* order): their bytes, which save writes and load expects, and
+  // (names != nullptr) their names.  Returns their number: 4, or 7 for a gated store.
+  static int sections(uint64_t live, int K, int d8, int stype, int gate, uint64_t* bytes, const char** names = nullptr) {
+    int n = 0;
+    for (const Col& c : kCols)
+      if (c.sec >= 0 && has(c, gate)) {
+        bytes[c.sec] = live * track_bytes(c, K, row_bytes(d8, stype));
+        if (names) names[c.sec] = c.name;
+        ++n;
+      }
+    return n;
+  }
 
-  // fresh columns for `n` tracks; the caller copies what it keeps
-  int alloc_columns(size_t n, DBuf* f, DBuf* c, DBuf* s, DBuf* i, DBuf* r) {
+  // fresh columns of this store for max(n, 1) tracks in nw[] (one per kCols entry; attrs_only: the gated ones alone),
+  // zero-filled where the table says so; the caller copies what it keeps
+  int alloc(size_t n, DBuf* nw, bool attrs_only = false) {
     n = std::max<size_t>(n, 1);
-    if (int rc = f->ensure(n * o.max_observations * row_bytes())) return rc;
-    if (int rc = c->ensure(n * 4)) return rc;
-    if (int rc = s->ensure(n * 4)) return rc;
-    if (int rc = i->ensure(n * 8)) return rc;
-    if (int rc = r->ensure(n * 4)) return rc;
-    CU(cudaMemsetAsync(r->p, 0, n * 4, st));
+    for (int k = 0; k < kNumCols; ++k) {
+      const Col& c = kCols[k];
+      if (!has(c, gate) || (attrs_only && !c.gated)) continue;
+      const size_t bytes = n * track_bytes(c);
+      if (int rc = nw[k].ensure(bytes)) return rc;
+      if (c.zero) CU(cudaMemsetAsync(nw[k].p, 0, bytes, st));
+    }
     return 0;
   }
 
-  // fresh, zero-filled attribute columns for `n` tracks (none for an ungated store); the caller copies what it keeps
-  int alloc_attrs(size_t n, DBuf* a, DBuf* b, DBuf* c) {
-    if (!gate) return 0;
-    n = std::max<size_t>(n, 1);
-    for (DBuf* x : {a, b, c}) {
-      if (int rc = x->ensure(n * 8)) return rc;
-      CU(cudaMemsetAsync(x->p, 0, n * 8, st));
-    }
-    return 0;
+  // exchanges the store's columns with nw[] (attrs_only: the gated ones alone)
+  void swap_columns(DBuf* nw, bool attrs_only = false) {
+    for (int k = 0; k < kNumCols; ++k)
+      if (!attrs_only || kCols[k].gated) std::swap(this->*kCols[k].buf, nw[k]);
+  }
+
+  // the tracks every column holds as allocated, at most cap (after a storage type change: in rows of the new type)
+  size_t held() const {
+    size_t n = cap;
+    for (const Col& c : kCols) if (has(c, gate)) n = std::min(n, (this->*c.buf).bytes / track_bytes(c));
+    return n;
   }
 
   sb::FsAttrCols attr_cols() const {
@@ -181,24 +223,14 @@ struct sb200_fstore {
   int reserve(size_t need) {
     if (need <= cap) return 0;
     const size_t nc = std::max(need, cap + cap / 2);
-    DBuf f, c, s, i, r, a0, a1, a2;
-    if (int rc = alloc_columns(nc, &f, &c, &s, &i, &r)) return rc;
-    if (int rc = alloc_attrs(nc, &a0, &a1, &a2)) return rc;
+    DBuf nw[kNumCols];
+    if (int rc = alloc(nc, nw)) return rc;
     const size_t live = hid.size();
-    if (live) {
-      CU(cudaMemcpyAsync(f.p, feat.p, live * o.max_observations * row_bytes(), cudaMemcpyDeviceToDevice, st));
-      CU(cudaMemcpyAsync(c.p, cnt.p, live * 4, cudaMemcpyDeviceToDevice, st));
-      CU(cudaMemcpyAsync(s.p, start.p, live * 4, cudaMemcpyDeviceToDevice, st));
-      CU(cudaMemcpyAsync(i.p, ids.p, live * 8, cudaMemcpyDeviceToDevice, st));
-      if (gate) {
-        CU(cudaMemcpyAsync(a0.p, asrc.p, live * 8, cudaMemcpyDeviceToDevice, st));
-        CU(cudaMemcpyAsync(a1.p, at0.p, live * 8, cudaMemcpyDeviceToDevice, st));
-        CU(cudaMemcpyAsync(a2.p, at1.p, live * 8, cudaMemcpyDeviceToDevice, st));
-      }
-    }
-    CU(cudaStreamSynchronize(st));   // the old columns are freed below
-    feat = std::move(f); cnt = std::move(c); start = std::move(s); ids = std::move(i); run = std::move(r);
-    asrc = std::move(a0); at0 = std::move(a1); at1 = std::move(a2);
+    for (int k = 0; k < kNumCols; ++k)   // the live tracks of the state columns
+      if (live && kCols[k].sec >= 0 && has(kCols[k], gate))
+        CU(cudaMemcpyAsync(nw[k].p, (this->*kCols[k].buf).p, live * track_bytes(kCols[k]), cudaMemcpyDeviceToDevice, st));
+    CU(cudaStreamSynchronize(st));   // the old columns are freed with nw
+    swap_columns(nw);
     cap = nc;
     return 0;
   }
@@ -227,8 +259,9 @@ struct sb200_fstore {
     return {attr_cols(), q, reinterpret_cast<const long long*>(q + n), reinterpret_cast<const long long*>(q + 2 * (size_t)n),
             gate};
   }
-  sb::FsAttrCols qattr_cols(int n) const {
-    unsigned long long* q = qattr.as<unsigned long long>();
+  // n triples in b, as the column of each field
+  static sb::FsAttrCols triples(const DBuf& b, int n) {
+    unsigned long long* q = b.as<unsigned long long>();
     return {q, reinterpret_cast<long long*>(q + n), reinterpret_cast<long long*>(q + 2 * (size_t)n)};
   }
 
@@ -251,14 +284,12 @@ struct sb200_fstore {
     if (int rc = gpos.ensure((size_t)n * 4)) return rc;
     if (int rc = gout.ensure((size_t)n * 24)) return rc;
     CU(cudaMemcpyAsync(gpos.p, pos.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
-    unsigned long long* g = gout.as<unsigned long long>();
-    sb::fs_launch_attr_gather(attr_cols(), gpos.as<int>(), n,
-                              {g, reinterpret_cast<long long*>(g + n), reinterpret_cast<long long*>(g + 2 * (size_t)n)}, st);
+    const unsigned long long* g = gout.as<unsigned long long>();
+    sb::fs_launch_attr_gather(attr_cols(), gpos.as<int>(), n, triples(gout, n), st);
     CU(cudaMemcpyAsync(out->src.data(), g, (size_t)n * 8, cudaMemcpyDeviceToHost, st));
     CU(cudaMemcpyAsync(out->t0.data(), g + n, (size_t)n * 8, cudaMemcpyDeviceToHost, st));
     CU(cudaMemcpyAsync(out->t1.data(), g + 2 * (size_t)n, (size_t)n * 8, cudaMemcpyDeviceToHost, st));
-    CU(cudaStreamSynchronize(st));
-    CU(cudaGetLastError());
+    if (int rc = finish()) return rc;
     return 0;
   }
 
@@ -269,9 +300,8 @@ struct sb200_fstore {
     if (int rc = gpos.ensure((size_t)n * 4)) return rc;
     if (int rc = upload_triples(n, v.src.data(), v.t0.data(), v.t1.data())) return rc;
     CU(cudaMemcpyAsync(gpos.p, pos.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
-    sb::fs_launch_attr_scatter(attr_cols(), gpos.as<int>(), n, qattr_cols(n), st);
-    CU(cudaStreamSynchronize(st));
-    CU(cudaGetLastError());
+    sb::fs_launch_attr_scatter(attr_cols(), gpos.as<int>(), n, triples(qattr, n), st);
+    if (int rc = finish()) return rc;
     return 0;
   }
 
@@ -281,11 +311,11 @@ struct sb200_fstore {
     if (!hid.empty()) return fail(SB200_ERR_INVALID, "the gate is fixed while the store holds tracks (%zu)", hid.size());
     CU(cudaSetDevice(o.device));
     gate = rule;
-    DBuf a0, a1, a2;   // no track is stored: the columns start empty, sized to the capacity
+    DBuf nw[kNumCols];   // no track is stored: the columns start empty, sized to the capacity
     if (cap)
-      if (int rc = alloc_attrs(cap, &a0, &a1, &a2)) return rc;
+      if (int rc = alloc(cap, nw, true)) return rc;
     CU(cudaStreamSynchronize(st));
-    asrc = std::move(a0); at0 = std::move(a1); at1 = std::move(a2);
+    swap_columns(nw, true);
     return 0;
   }
 
@@ -305,11 +335,12 @@ struct sb200_fstore {
     return 0;
   }
 
-  // Puts the request on the device: rows [R][d8] (zero-padded), ids, offsets, row -> item, dest and the initial max_dist.
+  // Puts the request on the device: rows [R][d8] (zero-padded), ids, offsets, row -> item, dest (nullptr: -1 for every
+  // item) and the initial max_dist.
   // row_src[r] is the row of the caller's column behind request row r; col_rows the rows of a host column to upload.
   // With `rsrc` there is no column: rsrc writes the rows on the device (row_src gives only their number).
   int upload(const ReqLayout& L, int Q, const uint64_t* qids, const std::vector<int>& qoff, const std::vector<int>& row_src,
-             const std::vector<int>& dest, const Column& col, size_t col_rows, const sb::FsRowSource* rsrc = nullptr) {
+             const int* dest, const Column& col, size_t col_rows, const sb::FsRowSource* rsrc = nullptr) {
     const bool host_f32 = !rsrc && !col.on_device && ftype == SB200_FEATURE_F32;
     const bool staged = !rsrc && !host_f32;     // rows built by fs_stage_kernel from the column
     const size_t base = host_f32 ? 0 : L.qid;   // the rows of the other paths are written on the device
@@ -327,13 +358,7 @@ struct sb200_fstore {
     } else if (staged) {
       memcpy(at(L.row_src), row_src.data(), (size_t)R * 4);
     }
-    memcpy(at(L.qid), qids, (size_t)Q * 8);
-    memcpy(at(L.qoff), qoff.data(), (size_t)(Q + 1) * 4);
-    int* row_q = reinterpret_cast<int*>(at(L.row_q));
-    for (int q = 0; q < Q; ++q)
-      for (int r = qoff[q]; r < qoff[q + 1]; ++r) row_q[r] = q;
-    memcpy(at(L.dest), dest.data(), (size_t)Q * 4);
-    *reinterpret_cast<int*>(at(L.maxkey)) = sb::fs_key(-1.0f);   // max_dist starts at -1.0 (topn.rs:78)
+    stage_request(L, at(L.qid), Q, qids, qoff.data(), dest, 1);
     const void* dev_col = col.p;
     if (staged && !col.on_device) {   // the raw 2-byte rows: half the bytes of the widened request
       const size_t bytes = col_rows * D * elem();
@@ -389,16 +414,7 @@ struct sb200_fstore {
     if (Q == 0) return 0;
     if (!qids || !offs) return fail(SB200_ERR_INVALID, "query_ids / obs_offsets is NULL");
     if (offs[0] != 0) return fail(SB200_ERR_INVALID, "obs_offsets[0] != 0");
-    std::unordered_set<uint64_t> seen;
-    seen.reserve((size_t)Q * 2);
-    for (int q = 0; q < Q; ++q) {
-      const int n = offs[q + 1] - offs[q];
-      if (n <= 0) return fail(SB200_ERR_INVALID, "query %d has no observations", q);
-      if (!seen.insert(qids[q]).second)
-        return fail(SB200_ERR_INVALID, "query id %llu appears twice in the call", (unsigned long long)qids[q]);
-      if (assoc && hpos.count(qids[q]))
-        return fail(SB200_ERR_INVALID, "query id %llu is already stored", (unsigned long long)qids[q]);
-    }
+    if (int rc = check_ids(Q, qids, "query id", assoc, offs)) return rc;
     if (!col.p) return fail(SB200_ERR_INVALID, "features is NULL");
     if (int rc = check_column(col)) return rc;
     return plan_rows(Q, offs, qoff, row_src);
@@ -414,12 +430,60 @@ struct sb200_fstore {
     return 0;
   }
 
-  int finish_timing(bool dist_ran, bool topn_ran, bool apply_ran) {
-    float ms = 0.0f;
-    if (dist_ran) { CU(cudaEventElapsedTime(&ms, ev[0], ev[1])); stage_ms[0] = ms; }
-    if (topn_ran) { CU(cudaEventElapsedTime(&ms, ev[1], ev[2])); stage_ms[1] = ms; }
-    if (apply_ran) { CU(cudaEventElapsedTime(&ms, ev[2], ev[3])); stage_ms[2] = ms; }
+  // Refuses the first of a call's n ids that appears twice in it (`what`: "query id" or "id") or, with `fresh`, that is
+  // already stored; with offs, the query of each id is first refused when it has no observations.
+  int check_ids(int n, const uint64_t* ids, const char* what, bool fresh, const int32_t* offs = nullptr) const {
+    std::unordered_set<uint64_t> seen;
+    seen.reserve((size_t)n * 2);
+    for (int q = 0; q < n; ++q) {
+      if (offs && offs[q + 1] - offs[q] <= 0) return fail(SB200_ERR_INVALID, "query %d has no observations", q);
+      if (!seen.insert(ids[q]).second)
+        return fail(SB200_ERR_INVALID, "%s %llu appears twice in the call", what, (unsigned long long)ids[q]);
+      if (fresh && hpos.count(ids[q]))
+        return fail(SB200_ERR_INVALID, "%s %llu is already stored", what, (unsigned long long)ids[q]);
+    }
     return 0;
+  }
+
+  // the per-call buffers of Q queries with R rows against S stored rows: results, plan, norms and distances
+  int size_call(const ResLayout& RL, int Q, int R, long long S) {
+    if (int rc = hres.ensure(RL.total)) return rc;
+    if (int rc = dres.ensure(RL.total)) return rc;
+    if (int rc = plan.ensure((size_t)Q * 16)) return rc;
+    if (o.metric == SB200_VIS_COSINE) {
+      if (int rc = qnorm.ensure((size_t)R * 4)) return rc;
+      if (int rc = snorm.ensure((size_t)std::max<long long>(S, 1) * 4)) return rc;
+    }
+    return dist.ensure((size_t)std::max<long long>((long long)R * S, 1) * 4);
+  }
+
+  // waits for the stream and reports a failed kernel; then adds the times of stages [first, last) to stage_ms (stage i
+  // runs from ev[i] to ev[i + 1])
+  int finish(int first = 0, int last = 0) {
+    CU(cudaStreamSynchronize(st));
+    CU(cudaGetLastError());
+    for (int i = first; i < last; ++i) {
+      float ms = 0.0f;
+      CU(cudaEventElapsedTime(&ms, ev[i], ev[i + 1]));
+      stage_ms[i] += ms;
+    }
+    return 0;
+  }
+
+  // the TopN results of Q queries (hres, layout RL) as counts[Q], winners[Q][topn] and weights[Q][topn], zero past a count
+  void read_results(const ResLayout& RL, int Q, int32_t* counts, uint64_t* winners, double* weights) const {
+    const char* h = static_cast<const char*>(hres.p);
+    const double* w = reinterpret_cast<const double*>(h + RL.w);
+    const int* cn = reinterpret_cast<const int*>(h + RL.cnt);
+    const int* ps = reinterpret_cast<const int*>(h + RL.pos);
+    for (int q = 0; q < Q; ++q) {
+      counts[q] = cn[q];
+      for (int e = 0; e < o.topn; ++e) {
+        const size_t i = (size_t)q * o.topn + e;
+        winners[i] = e < cn[q] ? hid[ps[i]] : 0;
+        weights[i] = e < cn[q] ? w[i] : 0.0;
+      }
+    }
   }
 
   // search (assoc == false) or associate
@@ -440,14 +504,7 @@ struct sb200_fstore {
   // associate whose request rows `rsrc` writes on the device (sb200_fstore_associate_wasted); offs as for associate
   int associate_rows(int Q, const uint64_t* qids, const int32_t* offs, const sb::FsRowSource& rsrc, int32_t* counts,
                      uint64_t* winners, double* weights, uint64_t* track_ids, uint8_t* merged) {
-    std::unordered_set<uint64_t> seen;
-    seen.reserve((size_t)Q * 2);
-    for (int q = 0; q < Q; ++q) {
-      if (!seen.insert(qids[q]).second)
-        return fail(SB200_ERR_INVALID, "query id %llu appears twice in the call", (unsigned long long)qids[q]);
-      if (hpos.count(qids[q]))
-        return fail(SB200_ERR_INVALID, "query id %llu is already stored", (unsigned long long)qids[q]);
-    }
+    if (int rc = check_ids(Q, qids, "query id", true)) return rc;
     std::vector<int> qoff, src;
     if (int rc = plan_rows(Q, offs, &qoff, &src)) return rc;
     if (int rc = begin()) return rc;
@@ -465,17 +522,10 @@ struct sb200_fstore {
     const long long live = (long long)hid.size(), S = live * K;
     const ReqLayout L(Q, R, d8, !rsrc && (col.on_device || ftype != SB200_FEATURE_F32));
     const ResLayout RL(Q, topn);
-    if (int rc = hres.ensure(RL.total)) return rc;
-    if (int rc = dres.ensure(RL.total)) return rc;
-    if (int rc = plan.ensure((size_t)Q * 16)) return rc;
-    if (o.metric == SB200_VIS_COSINE) {
-      if (int rc = qnorm.ensure((size_t)R * 4)) return rc;
-      if (int rc = snorm.ensure((size_t)std::max<long long>(S, 1) * 4)) return rc;
-    }
-    if (int rc = dist.ensure((size_t)std::max<long long>((long long)R * S, 1) * 4)) return rc;
+    if (int rc = size_call(RL, Q, R, S)) return rc;
     if (assoc)
       if (int rc = reserve(hid.size() + (size_t)Q)) return rc;
-    if (int rc = upload(L, Q, qids, qoff, src, std::vector<int>(Q, -1), col, col_rows, rsrc)) return rc;
+    if (int rc = upload(L, Q, qids, qoff, src, nullptr, col, col_rows, rsrc)) return rc;
     if (attrs)
       if (int rc = upload_triples(Q, attrs->source, attrs->t_start, attrs->t_end)) return rc;
     const sb::FsGate g = gate_view(Q);
@@ -496,25 +546,11 @@ struct sb200_fstore {
       where.resize(Q);
       CU(cudaMemcpyAsync(where.data(), c.dest, (size_t)Q * 4, cudaMemcpyDeviceToHost, st));
     }
-    CU(cudaStreamSynchronize(st));
-    CU(cudaGetLastError());
-    if (int rc = finish_timing(S > 0, true, assoc)) return rc;
-    const char* h = static_cast<const char*>(hres.p);
-    const double* w = reinterpret_cast<const double*>(h + RL.w);
-    const int* cn = reinterpret_cast<const int*>(h + RL.cnt);
-    const int* ps = reinterpret_cast<const int*>(h + RL.pos);
-    for (int q = 0; q < Q; ++q) {
-      counts[q] = cn[q];
-      for (int e = 0; e < topn; ++e) {
-        const bool ok = e < cn[q];
-        winners[(size_t)q * topn + e] = ok ? hid[ps[(size_t)q * topn + e]] : 0;
-        weights[(size_t)q * topn + e] = ok ? w[(size_t)q * topn + e] : 0.0;
-      }
-    }
+    if (int rc = finish(S > 0 ? 0 : 1, assoc ? 3 : 2)) return rc;   // no distance stage on an empty store
+    read_results(RL, Q, counts, winners, weights);
     if (assoc) {
       for (int q = 0; q < Q; ++q) {
-        merged[q] = cn[q] > 0 ? 1 : 0;
-        if (attrs) merged[q] = where[q] < live ? 1 : 0;   // a first winner the gate refused leaves a new track
+        merged[q] = attrs ? where[q] < live : counts[q] > 0;   // a first winner the gate refused leaves a new track
         track_ids[q] = merged[q] ? winners[(size_t)q * topn] : qids[q];
       }
       for (int q = 0; q < Q; ++q)
@@ -559,15 +595,13 @@ struct sb200_fstore {
     const ReqLayout L(n, n, d8, col.on_device || ftype != SB200_FEATURE_F32);
     if (int rc = plan.ensure((size_t)n * 16)) return rc;
     if (int rc = reserve(hid.size() + fresh.size())) return rc;
-    if (int rc = upload(L, n, idv, qoff, src, dest, col, (size_t)n)) return rc;
+    if (int rc = upload(L, n, idv, qoff, src, dest.data(), col, (size_t)n)) return rc;
     const sb::FsStore s = view();
     const sb::FsCall c = call_view(L, n, n, nullptr);
     CU(cudaEventRecord(ev[2], st));
     sb::fs_launch_apply(s, c, st);
     CU(cudaEventRecord(ev[3], st));
-    CU(cudaStreamSynchronize(st));
-    CU(cudaGetLastError());
-    if (int rc = finish_timing(false, false, true)) return rc;
+    if (int rc = finish(2, 3)) return rc;
     for (uint64_t id : fresh) {
       hpos[id] = (int)hid.size();
       hid.push_back(id);
@@ -656,8 +690,7 @@ struct sb200_fstore {
     int* dcnt = reinterpret_cast<int*>(gout.as<char>() + align16(out_bytes));
     sb::fs_launch_gather(s, gpos.as<int>(), n, dout, dcnt, st);
     CU(cudaMemcpyAsync(hres.p, gout.p, align16(out_bytes) + (size_t)n * 4, cudaMemcpyDeviceToHost, st));
-    CU(cudaStreamSynchronize(st));
-    CU(cudaGetLastError());
+    if (int rc = finish()) return rc;
     const float* h = static_cast<const float*>(hres.p);
     const int* hc = reinterpret_cast<const int*>(static_cast<const char*>(hres.p) + align16(out_bytes));
     for (int i = 0; i < n; ++i) {
@@ -676,22 +709,16 @@ struct sb200_fstore {
     from.reserve(hid.size());
     for (size_t p = 0; p < hid.size(); ++p)
       if (!gone[p]) from.push_back((int)p);
-    DBuf f, c, st_, i, r, a0, a1, a2;
-    if (int rc = alloc_columns(cap, &f, &c, &st_, &i, &r)) return rc;
-    if (int rc = alloc_attrs(cap, &a0, &a1, &a2)) return rc;
+    DBuf nw[kNumCols];
+    if (int rc = alloc(cap, nw)) return rc;
     if (int rc = gpos.ensure(std::max<size_t>(from.size(), 1) * 4)) return rc;
     CU(cudaMemcpyAsync(gpos.p, from.data(), from.size() * 4, cudaMemcpyHostToDevice, st));
     const sb::FsStore s = view();
-    sb::FsStore d = s;
-    d.feat = f.p; d.cnt = c.as<int>(); d.start = st_.as<int>(); d.ids = i.as<unsigned long long>();
-    sb::fs_launch_compact(s, d, gpos.as<int>(), (int)from.size(), st);
-    if (gate)
-      sb::fs_launch_attr_gather(attr_cols(), gpos.as<int>(), (int)from.size(),
-                                {a0.as<unsigned long long>(), a1.as<long long>(), a2.as<long long>()}, st);
-    CU(cudaStreamSynchronize(st));
-    CU(cudaGetLastError());
-    feat = std::move(f); cnt = std::move(c); start = std::move(st_); ids = std::move(i); run = std::move(r);
-    asrc = std::move(a0); at0 = std::move(a1); at1 = std::move(a2);
+    const sb::FsAttrCols sa = attr_cols();
+    swap_columns(nw);   // nw holds the old columns until the compaction below has read them
+    sb::fs_launch_compact(s, view(), gpos.as<int>(), (int)from.size(), st);
+    if (gate) sb::fs_launch_attr_gather(sa, gpos.as<int>(), (int)from.size(), attr_cols(), st);
+    if (int rc = finish()) return rc;
     std::vector<uint64_t> kept;
     kept.reserve(from.size());
     for (int p : from) kept.push_back(hid[p]);
@@ -713,8 +740,7 @@ struct sb200_fstore {
     CU(cudaMemcpyAsync(gpos.p, pos.data(), n * 4, cudaMemcpyHostToDevice, st));
     sb::fs_launch_peek(view(), gpos.as<int>(), (int)n, gout.as<int>(), st);
     CU(cudaMemcpyAsync(ring->data(), gout.p, n * 8, cudaMemcpyDeviceToHost, st));
-    CU(cudaStreamSynchronize(st));
-    CU(cudaGetLastError());
+    if (int rc = finish()) return rc;
     return 0;
   }
 
@@ -725,11 +751,7 @@ struct sb200_fstore {
     if (n < 0) return fail(SB200_ERR_INVALID, "n < 0");
     if (each != 0 && each != 1) return fail(SB200_ERR_INVALID, "each must be 0 or 1");
     if (n > 0 && (!qids || !counts || !winners || !weights)) return fail(SB200_ERR_INVALID, "ids or an output is NULL");
-    std::unordered_set<uint64_t> seen;
-    seen.reserve((size_t)n * 2);
-    for (int q = 0; q < n; ++q)
-      if (!seen.insert(qids[q]).second)
-        return fail(SB200_ERR_INVALID, "id %llu appears twice in the call", (unsigned long long)qids[q]);
+    if (int rc = check_ids(n, qids, "id", false)) return rc;
     if (int rc = begin()) return rc;
     if (n == 0) return 0;
     const int topn = o.topn, K = o.max_observations;
@@ -787,21 +809,9 @@ struct sb200_fstore {
     const ResLayout RL(Q, topn);
     if (int rc = hreq.ensure(L.total - L.qid)) return rc;
     if (int rc = dreq.ensure(L.total)) return rc;
-    if (int rc = hres.ensure(RL.total)) return rc;
-    if (int rc = dres.ensure(RL.total)) return rc;
-    if (o.metric == SB200_VIS_COSINE) {
-      if (int rc = qnorm.ensure((size_t)R * 4)) return rc;
-      if (int rc = snorm.ensure((size_t)S * 4)) return rc;
-    }
-    if (int rc = dist.ensure((size_t)R * S * 4)) return rc;
+    if (int rc = size_call(RL, Q, R, S)) return rc;
     auto at = [&](size_t off) { return static_cast<char*>(hreq.p) + (off - L.qid); };   // rows are written on the device
-    memcpy(at(L.qid), qids + a, (size_t)Q * 8);
-    memcpy(at(L.qoff), qoff.data(), (size_t)(Q + 1) * 4);
-    int* row_q = reinterpret_cast<int*>(at(L.row_q));
-    for (int q = 0; q < Q; ++q)
-      for (int r = qoff[q]; r < qoff[q + 1]; ++r) row_q[r] = q;
-    std::fill_n(reinterpret_cast<int*>(at(L.dest)), Q, -1);
-    std::fill_n(reinterpret_cast<int*>(at(L.maxkey)), nkey, sb::fs_key(-1.0f));   // max_dist starts at -1.0 (topn.rs:78)
+    stage_request(L, at(L.qid), Q, qids + a, qoff.data(), nullptr, nkey);
     int* qp = reinterpret_cast<int*>(at(L.qpos));
     for (int q = 0; q < Q; ++q) qp[q] = std::max(qpos[a + q], 0);   // a query that is not stored has no rows
     if (!excl.empty()) memcpy(at(L.excl), excl.data(), excl.size());
@@ -814,7 +824,7 @@ struct sb200_fstore {
       if (int rc = qattr.ensure((size_t)Q * 24)) return rc;
     const sb::FsGate g = gate_view(Q);
     CU(cudaEventRecord(ev[0], st));
-    if (gate) sb::fs_launch_attr_gather(attr_cols(), dqpos, Q, qattr_cols(Q), st);
+    if (gate) sb::fs_launch_attr_gather(attr_cols(), dqpos, Q, triples(qattr, Q), st);
     sb::fs_launch_owned_stage(s, c, dqpos, reinterpret_cast<float*>(dreq.as<char>() + L.rows), st);
     sb::fs_launch_dist(o.metric, o.distance_filter, s, c, st, mode,
                        reinterpret_cast<const unsigned char*>(dreq.as<char>() + L.excl), gate ? &g : nullptr);
@@ -822,24 +832,8 @@ struct sb200_fstore {
     sb::fs_launch_topn(o.max_distance, o.min_votes, topn, false, s, c, st, mode);
     CU(cudaEventRecord(ev[2], st));
     CU(cudaMemcpyAsync(hres.p, dres.p, RL.total, cudaMemcpyDeviceToHost, st));
-    CU(cudaStreamSynchronize(st));
-    CU(cudaGetLastError());
-    float ms = 0.0f;
-    CU(cudaEventElapsedTime(&ms, ev[0], ev[1]));
-    stage_ms[0] += ms;
-    CU(cudaEventElapsedTime(&ms, ev[1], ev[2]));
-    stage_ms[1] += ms;
-    const char* h = static_cast<const char*>(hres.p);
-    const double* w = reinterpret_cast<const double*>(h + RL.w);
-    const int* cn = reinterpret_cast<const int*>(h + RL.cnt);
-    const int* ps = reinterpret_cast<const int*>(h + RL.pos);
-    for (int q = 0; q < Q; ++q) {
-      counts[a + q] = cn[q];
-      for (int e = 0; e < cn[q]; ++e) {
-        winners[(size_t)(a + q) * topn + e] = hid[ps[(size_t)q * topn + e]];
-        weights[(size_t)(a + q) * topn + e] = w[(size_t)q * topn + e];
-      }
-    }
+    if (int rc = finish(0, 2)) return rc;   // summed over the chunks
+    read_results(RL, Q, counts + a, winners + (size_t)a * topn, weights + (size_t)a * topn);
     return 0;
   }
 
@@ -921,9 +915,7 @@ struct sb200_fstore {
     CU(cudaEventRecord(ev[2], st));
     sb::fs_launch_move_rows(view(), dtab, dtab + nm, nm, dtab + 2 * nm, nh, gout.p, st);
     CU(cudaEventRecord(ev[3], st));
-    CU(cudaStreamSynchronize(st));
-    CU(cudaGetLastError());
-    if (int rc = finish_timing(false, false, true)) return rc;
+    if (int rc = finish(2, 3)) return rc;
     if (int rc = write_attrs(wpos, win)) return rc;
     if (remove) return remove_marked(gone);
     return 0;
@@ -960,8 +952,9 @@ struct sb200_fstore {
   // ---- the store blob (layout: include/similari_b200.h)
   // the columns and their `n` sections (4, or 7 for a gated store) of a blob on this device: dir 0 packs, dir 1 unpacks
   int move_columns(int dir, const uint64_t* sec_off, const uint64_t* sec_bytes, int n, char* dblob) {
-    char* col[SB200_FSTORE_BLOB_SECTIONS_V2] = {ids.as<char>(), cnt.as<char>(), start.as<char>(), feat.as<char>(),
-                                                asrc.as<char>(), at0.as<char>(), at1.as<char>()};
+    char* col[SB200_FSTORE_BLOB_SECTIONS_V2] = {};
+    for (const Col& c : kCols)
+      if (c.sec >= 0) col[c.sec] = (this->*c.buf).as<char>();
     std::vector<sb::XferSeg> segs;
     for (int i = 0; i < n; ++i) sb::add_segment(segs, dir, col[i], dblob + sec_off[i], sec_bytes[i]);
     return sb::copy_segments(segs, num_sms, st);
@@ -977,21 +970,19 @@ struct sb200_fstore {
   }
 
   int save(void* dst, uint64_t cap_bytes, uint64_t* bytes) {
-    const uint64_t live = hid.size();
-    const uint64_t sec[SB200_FSTORE_BLOB_SECTIONS_V2] = {live * 8, live * 4, live * 4,
-                                                         live * o.max_observations * row_bytes(), live * 8, live * 8,
-                                                         live * 8};
+    uint64_t sec[SB200_FSTORE_BLOB_SECTIONS_V2];
+    const int n = sections(hid.size(), o.max_observations, d8, stype, gate, sec);
     if (gate) {   // version 2: the attribute sections follow feat
       BlobHeaderV2 h;
       fill_header(h, SB200_FSTORE_BLOB_VERSION_GATED);
       h.gate = gate;
-      sb::lay_out(h, sec, SB200_FSTORE_BLOB_SECTIONS_V2);
-      return write_header_and_columns(dst, cap_bytes, bytes, h, SB200_FSTORE_BLOB_SECTIONS_V2);
+      sb::lay_out(h, sec, n);
+      return write_header_and_columns(dst, cap_bytes, bytes, h, n);
     }
     BlobHeader h;
     fill_header(h, SB200_FSTORE_BLOB_VERSION);
-    sb::lay_out(h, sec, SB200_FSTORE_BLOB_SECTIONS);
-    return write_header_and_columns(dst, cap_bytes, bytes, h, SB200_FSTORE_BLOB_SECTIONS);
+    sb::lay_out(h, sec, n);
+    return write_header_and_columns(dst, cap_bytes, bytes, h, n);
   }
 
   template <class H> int write_header_and_columns(void* dst, uint64_t cap_bytes, uint64_t* bytes, const H& h, int n) {
@@ -1002,11 +993,9 @@ struct sb200_fstore {
     CU(cudaSetDevice(o.device));
     return sb::write_blob(dst, o.device, st, h, n, [&](char* p) {
       if (int rc = move_columns(0, h.sec_off, h.sec_bytes, n, p)) return rc;
-      sb::fs_launch_blob_scrub(stype, p + h.sec_off[kSecFeat], cnt.as<int>(), start.as<int>(), (int)h.live,
-                               o.max_observations, d8, st);
-      CU(cudaStreamSynchronize(st));
-      CU(cudaGetLastError());
-      return 0;
+      const sb::FsStore s = view();
+      sb::fs_launch_blob_scrub(stype, p + h.sec_off[kSecFeat], s.cnt, s.start, (int)h.live, o.max_observations, d8, st);
+      return finish();
     });
   }
 
@@ -1036,8 +1025,7 @@ struct sb200_fstore {
                                reinterpret_cast<const long long*>(dblob + sec_off[kSecT1]), live, gpos.as<int>() + 2, st);
     CU(cudaMemcpyAsync(bad, gpos.p, sizeof(bad), cudaMemcpyDeviceToHost, st));
     CU(cudaMemcpyAsync(&bad_w, gpos.as<int>() + 2, sizeof(bad_w), cudaMemcpyDeviceToHost, st));
-    CU(cudaStreamSynchronize(st));
-    CU(cudaGetLastError());
+    if (int rc = finish()) return rc;
     if (bad[0]) return fail(SB200_ERR_INVALID, "the blob holds %d cnt entries outside 1..%d", bad[0], K);
     if (bad[1]) return fail(SB200_ERR_INVALID, "the blob holds %d start entries outside 0..%d", bad[1], K - 1);
     if (bad_w) return fail(SB200_ERR_INVALID, "the blob holds %d windows with t_start > t_end", bad_w);
@@ -1048,6 +1036,17 @@ struct sb200_fstore {
     for (size_t p = 0; p < hid.size(); ++p) hpos[hid[p]] = (int)p;
     return 0;
   }
+};
+
+const sb200_fstore::Col sb200_fstore::kCols[kNumCols] = {
+    {&sb200_fstore::feat, 0, false, false, kSecFeat, "feat"},
+    {&sb200_fstore::cnt, 4, false, false, kSecCnt, "cnt"},
+    {&sb200_fstore::start, 4, false, false, kSecStart, "start"},
+    {&sb200_fstore::ids, 8, false, false, kSecIds, "ids"},
+    {&sb200_fstore::run, 4, false, true, -1, nullptr},
+    {&sb200_fstore::asrc, 8, true, true, kSecSrc, "source"},
+    {&sb200_fstore::at0, 8, true, true, kSecT0, "t_start"},
+    {&sb200_fstore::at1, 8, true, true, kSecT1, "t_end"},
 };
 
 // a call without a handle: SB200_ERR_CUDA when there is no device to have made one, else SB200_ERR_INVALID
@@ -1151,7 +1150,7 @@ int sb200_fstore_set_storage_type(sb200_fstore* s, int32_t type) {
   s->stype = type;
   // no track is stored, so nothing moves: the capacity is what the allocated columns hold in rows of the new type, and
   // the next reserve allocates when it needs more
-  if (s->cap) s->cap = std::min(s->cap, s->feat.bytes / ((size_t)s->o.max_observations * s->row_bytes()));
+  s->cap = s->held();
   return 0;
 }
 
@@ -1291,7 +1290,6 @@ int sb200_fstore_load(const void* buf, uint64_t bytes, int32_t device, sb200_fst
     if (h2.gate != SB200_FSTORE_GATE_SAME_SOURCE && h2.gate != SB200_FSTORE_GATE_ANY_SOURCE)
       return fail(SB200_ERR_INVALID, "a version-2 blob with unknown gate rule %d", h2.gate);
   }
-  const int nsec = v2 ? SB200_FSTORE_BLOB_SECTIONS_V2 : SB200_FSTORE_BLOB_SECTIONS;
   const uint64_t* sec_off = v2 ? h2.sec_off : h.sec_off;
   const uint64_t* sec_bytes = v2 ? h2.sec_bytes : h.sec_bytes;
   if (h.total_bytes > bytes)
@@ -1307,15 +1305,13 @@ int sb200_fstore_load(const void* buf, uint64_t bytes, int32_t device, sb200_fst
   // live * K indexes the distance matrix's columns as an int
   if (h.live < 0 || h.live > INT32_MAX / h.max_observations) return fail(SB200_ERR_INVALID, "live count out of range");
   const uint64_t live = (uint64_t)h.live;
-  const uint64_t want[SB200_FSTORE_BLOB_SECTIONS_V2] = {live * 8, live * 4, live * 4,
-                                                        live * h.max_observations * h.d8 * type_bytes(h.storage_type),
-                                                        live * 8, live * 8, live * 8};
-  static const char* const kName[SB200_FSTORE_BLOB_SECTIONS_V2] = {"ids", "cnt", "start", "feat", "source", "t_start",
-                                                                   "t_end"};
-  if (int rc = v2 ? sb::check_section_table(h2, nsec, kName) : sb::check_section_table(h, nsec, kName)) return rc;
+  uint64_t want[SB200_FSTORE_BLOB_SECTIONS_V2];
+  const char* name[SB200_FSTORE_BLOB_SECTIONS_V2];
+  const int nsec = sb200_fstore::sections(live, h.max_observations, h.d8, h.storage_type, v2 ? h2.gate : 0, want, name);
+  if (int rc = v2 ? sb::check_section_table(h2, nsec, name) : sb::check_section_table(h, nsec, name)) return rc;
   for (int i = 0; i < nsec; ++i)
     if (sec_bytes[i] != want[i])
-      return fail(SB200_ERR_INVALID, "section %s holds %llu bytes, %llu expected", kName[i],
+      return fail(SB200_ERR_INVALID, "section %s holds %llu bytes, %llu expected", name[i],
                   (unsigned long long)sec_bytes[i], (unsigned long long)want[i]);
   std::vector<uint64_t> blob_ids(live);
   if (live) CU(cudaMemcpy(blob_ids.data(), static_cast<const char*>(buf) + sec_off[kSecIds], live * 8, cudaMemcpyDefault));

@@ -771,10 +771,7 @@ class FeatureStore:
         f = self._column(features)
         if len(f) != len(ids):
             raise ValueError("features needs one row per id")
-        if a is None:
-            check(self._L.sb200_fstore_add(self._h, len(ids), ptr(ids), ptr(f)))
-        else:
-            check(self._L.sb200_fstore_add_attr(self._h, len(ids), ptr(ids), C.byref(a[0]), ptr(f), None, None))
+        self._call("add", a, (len(ids), ptr(ids)), f)
 
     def add_device(self, ids, d_features, stream=0, sources=None, t_start=None, t_end=None):
         """sb200_fstore_add_device: `d_features` is the raw device address of [len(ids)][feature_dim] elements of the
@@ -782,14 +779,25 @@ class FeatureStore:
         ids = np.ascontiguousarray(ids, dtype=np.uint64)
         a = self._attrs(len(ids), sources, t_start, t_end)
         self._use_declared_type()
-        if a is None:
-            check(self._L.sb200_fstore_add_device(self._h, len(ids), ptr(ids), C.c_void_p(d_features or None),
-                                                  C.c_void_p(stream or None)))
-        else:
-            check(self._L.sb200_fstore_add_attr(self._h, len(ids), ptr(ids), C.byref(a[0]), None,
-                                                C.c_void_p(d_features or None), C.c_void_p(stream or None)))
+        self._call("add", a, (len(ids), ptr(ids)), None, d_features, stream)
 
-    def _queries(self, ids, offsets, features):
+    def _call(self, op, a, lead, f, d_features=None, stream=0, out=None):
+        """sb200_fstore_{op} with the host column f, or sb200_fstore_{op}_device with the device column d_features and
+        the caller's stream (f is None); on a gated store (a from _attrs) sb200_fstore_{op}_attr, which takes either.
+        lead: the arguments before the attributes and features; out: the output arrays, in the call's order."""
+        res = [ptr(v) for v in out.values()] if out else []
+        if f is None:
+            col, st = (None, C.c_void_p(d_features or None)), C.c_void_p(stream or None)
+        else:
+            col, st = (ptr(f), None), None
+        if a is not None:
+            check(getattr(self._L, f"sb200_fstore_{op}_attr")(self._h, *lead, C.byref(a[0]), *col, *res, st))
+        elif f is None:
+            check(getattr(self._L, f"sb200_fstore_{op}_device")(self._h, *lead, col[1], *res, st))
+        else:
+            check(getattr(self._L, f"sb200_fstore_{op}")(self._h, *lead, col[0], *res))
+
+    def _queries(self, ids, offsets, features, assoc=False):
         ids = np.ascontiguousarray(ids, dtype=np.uint64)
         offs = np.ascontiguousarray(offsets, dtype=np.int32)
         if len(offs) != len(ids) + 1:
@@ -802,6 +810,9 @@ class FeatureStore:
         q = len(ids)
         out = {"counts": np.zeros(q, np.int32), "winners": np.zeros((q, self.topn), np.uint64),
                "weights": np.zeros((q, self.topn), np.float64)}
+        if assoc:
+            out["track_ids"] = np.zeros(q, np.uint64)
+            out["merged"] = np.zeros(q, np.uint8)
         return ids, offs, f, out
 
     def search(self, ids, offsets, features, sources=None, t_start=None, t_end=None):
@@ -809,12 +820,7 @@ class FeatureStore:
         gated store takes one source and window per query; incompatible pairs neither vote nor count toward max_dist."""
         a = self._attrs(len(ids), sources, t_start, t_end)
         ids, offs, f, out = self._queries(ids, offsets, features)
-        res = [ptr(out[k]) for k in ("counts", "winners", "weights")]
-        if a is None:
-            check(self._L.sb200_fstore_search(self._h, len(ids), ptr(ids), ptr(offs), ptr(f), *res))
-        else:
-            check(self._L.sb200_fstore_search_attr(self._h, len(ids), ptr(ids), ptr(offs), C.byref(a[0]), ptr(f), None,
-                                                   *res, None))
+        self._call("search", a, (len(ids), ptr(ids), ptr(offs)), f, out=out)
         return out
 
     def associate(self, ids, offsets, features, sources=None, t_start=None, t_end=None):
@@ -823,15 +829,8 @@ class FeatureStore:
         if it is compatible with its first winner's window as the queries merged into it earlier in the call extended it;
         otherwise the query becomes a new track."""
         a = self._attrs(len(ids), sources, t_start, t_end)
-        ids, offs, f, out = self._queries(ids, offsets, features)
-        out["track_ids"] = np.zeros(len(ids), np.uint64)
-        out["merged"] = np.zeros(len(ids), np.uint8)
-        res = [ptr(out[k]) for k in ("counts", "winners", "weights", "track_ids", "merged")]
-        if a is None:
-            check(self._L.sb200_fstore_associate(self._h, len(ids), ptr(ids), ptr(offs), ptr(f), *res))
-        else:
-            check(self._L.sb200_fstore_associate_attr(self._h, len(ids), ptr(ids), ptr(offs), C.byref(a[0]), ptr(f),
-                                                      None, *res, None))
+        ids, offs, f, out = self._queries(ids, offsets, features, assoc=True)
+        self._call("associate", a, (len(ids), ptr(ids), ptr(offs)), f, out=out)
         return out
 
     def search_device(self, ids, offsets, d_features, stream=0, sources=None, t_start=None, t_end=None):
@@ -839,29 +838,15 @@ class FeatureStore:
         a = self._attrs(len(ids), sources, t_start, t_end)
         ids, offs, _, out = self._queries(ids, offsets, None)
         self._use_declared_type()
-        res = [ptr(out[k]) for k in ("counts", "winners", "weights")]
-        d, st = C.c_void_p(d_features or None), C.c_void_p(stream or None)
-        if a is None:
-            check(self._L.sb200_fstore_search_device(self._h, len(ids), ptr(ids), ptr(offs), d, *res, st))
-        else:
-            check(self._L.sb200_fstore_search_attr(self._h, len(ids), ptr(ids), ptr(offs), C.byref(a[0]), None, d, *res,
-                                                   st))
+        self._call("search", a, (len(ids), ptr(ids), ptr(offs)), None, d_features, stream, out)
         return out
 
     def associate_device(self, ids, offsets, d_features, stream=0, sources=None, t_start=None, t_end=None):
         """sb200_fstore_associate_device: associate with the feature rows at the raw device address `d_features`."""
         a = self._attrs(len(ids), sources, t_start, t_end)
-        ids, offs, _, out = self._queries(ids, offsets, None)
+        ids, offs, _, out = self._queries(ids, offsets, None, assoc=True)
         self._use_declared_type()
-        out["track_ids"] = np.zeros(len(ids), np.uint64)
-        out["merged"] = np.zeros(len(ids), np.uint8)
-        res = [ptr(out[k]) for k in ("counts", "winners", "weights", "track_ids", "merged")]
-        d, st = C.c_void_p(d_features or None), C.c_void_p(stream or None)
-        if a is None:
-            check(self._L.sb200_fstore_associate_device(self._h, len(ids), ptr(ids), ptr(offs), d, *res, st))
-        else:
-            check(self._L.sb200_fstore_associate_attr(self._h, len(ids), ptr(ids), ptr(offs), C.byref(a[0]), None, d,
-                                                      *res, st))
+        self._call("associate", a, (len(ids), ptr(ids), ptr(offs)), None, d_features, stream, out)
         return out
 
     def search_owned(self, ids, each=False):
