@@ -162,6 +162,8 @@ def lib():
             "orc_tracker_idle_tracks": (C.c_int, [C.c_void_p, C.c_uint64, C.c_int, u64p, u32p, u32p, f32p, f32p]),
             "orc_tracker_clear_wasted": (None, [C.c_void_p]),
             "orc_tracker_scene_tracks": (C.c_int, [C.c_void_p, C.c_uint64, C.c_int, u64p, f32p, f32p, i32p]),
+            "orc_tracker_scene_observations": (C.c_int, [C.c_void_p, C.c_uint64, C.c_int, C.c_int, C.c_int, i32p, u8p,
+                                                         f32p, f32p, f32p]),
             "orc_tracker_last_costs": (C.c_int, [C.c_void_p, C.c_uint64, C.c_int, f32p, i32p, i32p]),
         }
         for name, (res, args) in sig.items():
@@ -439,6 +441,22 @@ class Tracker:
         n = self._L.orc_tracker_scene_tracks(self._h, scene_id, cap, _p(ids, C.c_uint64), _p(bx, C.c_float),
                                              _p(st, C.c_float), _p(fc, C.c_int32))
         return {"ids": ids[:n], "boxes": bx[:n], "states": st[:n], "feat_counts": fc[:n]}
+
+    def scene_observations(self, scene_id=0):
+        """Track::obs of every track of the scene, in store order: n_obs [n], and per observation [n, K] has_feat,
+        quality, the feature zero-padded to d8 ([n, K, d8]) and its squared norm.  Entries past n_obs are zero."""
+        K = max(1, int(self.opts.visual_max_observations))
+        d8 = (int(self.opts.feature_dim) + 7) // 8 * 8
+        cap = max(1, self.active_tracks())
+        n_obs = np.zeros(cap, dtype=np.int32)
+        hf = np.zeros((cap, K), dtype=np.uint8)
+        q = np.zeros((cap, K), dtype=np.float32)
+        feats = np.zeros((cap, K, d8), dtype=np.float32)
+        n2 = np.zeros((cap, K), dtype=np.float32)
+        n = self._L.orc_tracker_scene_observations(self._h, scene_id, cap, K, d8, _p(n_obs, C.c_int32),
+                                                   _p(hf, C.c_uint8), _p(q, C.c_float), _p(feats, C.c_float),
+                                                   _p(n2, C.c_float))
+        return {"n_obs": n_obs[:n], "has_feat": hf[:n], "quality": q[:n], "feats": feats[:n], "norm2": n2[:n]}
 
     def last_costs(self, scene_id=0, cap=1 << 22):
         out = np.zeros(cap, dtype=np.float32)

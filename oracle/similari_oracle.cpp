@@ -578,6 +578,18 @@ inline bool use_avx2() {
 inline bool use_avx2() { return false; }
 #endif
 
+// squared norm of one padded feature, the f1 / f2 accumulation of cosine (src/distance.rs:36-44): per-block reduce_add
+// of the lane squares, blocks added in order (the same operations on both paths)
+float norm2_p(const float* a, int blocks) {
+  float acc = 0.0f;
+  for (int i = 0; i < blocks; ++i) {
+    float blk[8];
+    for (int l = 0; l < 8; ++l) blk[l] = a[i * 8 + l] * a[i * 8 + l];
+    acc = acc + reduce_add8(blk);
+  }
+  return acc;
+}
+
 // euclidean, src/distance.rs:9-19
 float euclidean_p(const float* a, const float* b, int blocks) {
 #ifdef ORC_HAVE_AVX2_PATH
@@ -1398,6 +1410,31 @@ int orc_tracker_scene_tracks(orc_tracker* t, uint64_t scene_id, int cap, uint64_
     if (boxes6) store_box(tr.last_pred, boxes6 + (size_t)k * 6);
     if (states110) store_state(tr.st, states110 + (size_t)k * 110);
     if (feat_counts) feat_counts[k] = (int32_t)tr.feat_count;
+    ++k;
+  }
+  return k;
+}
+int orc_tracker_scene_observations(orc_tracker* t, uint64_t scene_id, int cap, int K, int d8, int32_t* n_obs,
+                                   uint8_t* has_feat, float* quality, float* feats, float* norm2) {
+  auto it = t->store.find(scene_id);
+  if (it == t->store.end()) return 0;
+  const int blocks = d8 / 8;
+  int k = 0;
+  for (auto& tr : it->second) {
+    if (k >= cap) break;
+    const int n = (int)std::min(tr.obs.size(), (size_t)K);
+    n_obs[k] = n;
+    for (int j = 0; j < K; ++j) {
+      const size_t e = (size_t)k * K + j;
+      const Obs* o = j < n ? &tr.obs[j] : nullptr;
+      const bool f = o && o->has_feat;
+      has_feat[e] = f ? 1 : 0;
+      quality[e] = o ? o->quality : 0.0f;
+      float* row = feats + e * d8;
+      std::memset(row, 0, sizeof(float) * (size_t)d8);
+      if (f) std::memcpy(row, o->feat.data(), sizeof(float) * std::min((size_t)d8, o->feat.size()));
+      norm2[e] = f ? norm2_p(row, blocks) : 0.0f;
+    }
     ++k;
   }
   return k;

@@ -150,6 +150,11 @@ void orc_tracker_clear_wasted(orc_tracker* t);
 /* debugging / parity: dump dense per-scene store (track order == store order) */
 int orc_tracker_scene_tracks(orc_tracker* t, uint64_t scene_id, int cap, uint64_t* ids, float* boxes6,
                              float* states110, int32_t* feat_counts);
+/* each track's logical observation list Track::obs (store order): n_obs[cap]; per observation [cap][K]: has_feat,
+ * quality, the feature zero-padded to d8 (zeros when absent) and its squared norm in the order cosine accumulates it
+ * (distance.rs:36-44); entries past n_obs are zero.  Returns the number of tracks written. */
+int orc_tracker_scene_observations(orc_tracker* t, uint64_t scene_id, int cap, int K, int d8, int32_t* n_obs,
+                                   uint8_t* has_feat, float* quality, float* feats, float* norm2);
 /* last frame's per-scene dense cost matrices (positional M x N, NaN none) for parity tests */
 int orc_tracker_last_costs(orc_tracker* t, uint64_t scene_id, int cap, float* out, int32_t* m, int32_t* n);
 
