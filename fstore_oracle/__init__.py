@@ -23,6 +23,8 @@ _ORACLE_DIR = os.path.dirname(os.path.abspath(oracle.__file__))
 EUCLIDEAN, COSINE = 0, 1
 # track attribute rules (feature_store.cpp): None = no attributes
 GATES = {None: 0, "same_source": 1, "any_source": 2}
+# retention rules (feature_store.cpp): the newest K, or the best by quality with a capacity growing with the merges
+RETENTIONS = {"newest": 0, "quality": 1}
 
 
 def build(force: bool = False) -> str:
@@ -62,6 +64,12 @@ def lib():
             "ofs_search_attr": (C.c_int, [vp, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, i32]),
             "ofs_associate_attr": (C.c_int, [vp, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i32]),
             "ofs_fetch_attr": (i64, [vp, i32, vp, vp, vp, vp]),
+            "ofs_set_retention": (C.c_int, [vp, i32, i32, f32]),
+            "ofs_add_quality": (C.c_int, [vp, i32, vp, vp, vp, vp, vp, vp]),
+            "ofs_search_quality": (C.c_int, [vp, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i32]),
+            "ofs_associate_quality": (C.c_int, [vp, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i32]),
+            "ofs_fetch_quality": (i64, [vp, i32, vp, i32, vp, vp, vp]),
+            "ofs_merge_history": (i64, [vp, i32, vp, vp, i64, vp]),
         }
         for name, (res, args) in sig.items():
             fn = getattr(L, name)
@@ -117,7 +125,8 @@ class FeatureStore:
     """The oracle's feature track store; same calls and results as similari_b200.engine.FeatureStore."""
 
     def __init__(self, metric=EUCLIDEAN, distance_filter=100.0, max_observations=3, feature_dim=256, topn=1,
-                 max_distance=100.0, min_votes=1, threads=1, gate=None):
+                 max_distance=100.0, min_votes=1, threads=1, gate=None, retention="newest", initial_capacity=4,
+                 merge_extension=1.5):
         self._L = lib()
         self.K, self.D, self.topn, self.threads = int(max_observations), int(feature_dim), int(topn), int(threads)
         self._h = self._L.ofs_create(metric, distance_filter, self.K, self.D, self.topn, max_distance, min_votes)
@@ -128,6 +137,28 @@ class FeatureStore:
         self.gate = gate
         if self._L.ofs_set_gate(self._h, GATES[gate]):
             raise ValueError("invalid gate")
+        if retention not in RETENTIONS:
+            raise ValueError(f"retention must be one of {list(RETENTIONS)}")
+        if self._L.ofs_set_retention(self._h, RETENTIONS[retention], int(initial_capacity), float(merge_extension)):
+            raise ValueError("invalid retention parameters")
+        self._retention = (retention, int(initial_capacity), float(merge_extension))
+
+    def retention(self):
+        """(rule, initial_capacity, merge_extension)."""
+        return self._retention
+
+    def _quality(self, n, quality):
+        """The quality column of a call: required on a quality store, refused on a newest one."""
+        if self._retention[0] == "newest":
+            if quality is not None:
+                raise ValueError("quality= needs a quality store")
+            return None
+        if quality is None:
+            raise ValueError("a quality store needs quality=")
+        q = np.ascontiguousarray(quality, dtype=np.float32)
+        if q.shape != (n,):
+            raise ValueError("quality needs one value per row")
+        return q
 
     def _attrs(self, n, sources, t_start, t_end):
         """The three attribute columns of a call: required on a gated store, refused on an ungated one."""
@@ -149,11 +180,15 @@ class FeatureStore:
             self._L.ofs_destroy(self._h)
             self._h = None
 
-    def add(self, ids, features, sources=None, t_start=None, t_end=None):
+    def add(self, ids, features, sources=None, t_start=None, t_end=None, quality=None):
         ids = np.ascontiguousarray(ids, dtype=np.uint64)
         f = np.ascontiguousarray(features, dtype=np.float32).reshape(len(ids), self.D)
         a = self._attrs(len(ids), sources, t_start, t_end)
-        if a is None:
+        q = self._quality(len(ids), quality)
+        if q is not None:
+            if self._L.ofs_add_quality(self._h, len(ids), _p(ids), _p(q), *(map(_p, a) if a else (None,) * 3), _p(f)):
+                raise ValueError("invalid add request")
+        elif a is None:
             self._L.ofs_add(self._h, len(ids), _p(ids), _p(f))
         elif self._L.ofs_add_attr(self._h, len(ids), _p(ids), *map(_p, a), _p(f)):
             raise ValueError("invalid add request")
@@ -167,10 +202,15 @@ class FeatureStore:
                "weights": np.zeros((q, self.topn), np.float64)}
         return ids, offs, f, out
 
-    def search(self, ids, offsets, features, sources=None, t_start=None, t_end=None):
+    def search(self, ids, offsets, features, sources=None, t_start=None, t_end=None, quality=None):
         ids, offs, f, out = self._queries(ids, offsets, features)
         a = self._attrs(len(ids), sources, t_start, t_end)
-        if a is None:
+        q = self._quality(len(f), quality)
+        if q is not None:
+            rc = self._L.ofs_search_quality(self._h, len(ids), _p(ids), _p(offs), _p(q),
+                                            *(map(_p, a) if a else (None,) * 3), _p(f), _p(out["counts"]),
+                                            _p(out["winners"]), _p(out["weights"]), self.threads)
+        elif a is None:
             rc = self._L.ofs_search(self._h, len(ids), _p(ids), _p(offs), _p(f), _p(out["counts"]),
                                     _p(out["winners"]), _p(out["weights"]), self.threads)
         else:
@@ -180,13 +220,17 @@ class FeatureStore:
             raise ValueError("invalid search request")
         return out
 
-    def associate(self, ids, offsets, features, sources=None, t_start=None, t_end=None):
+    def associate(self, ids, offsets, features, sources=None, t_start=None, t_end=None, quality=None):
         ids, offs, f, out = self._queries(ids, offsets, features)
         a = self._attrs(len(ids), sources, t_start, t_end)
+        q = self._quality(len(f), quality)
         out["track_ids"] = np.zeros(len(ids), np.uint64)
         out["merged"] = np.zeros(len(ids), np.uint8)
         res = [_p(out[k]) for k in ("counts", "winners", "weights", "track_ids", "merged")]
-        if a is None:
+        if q is not None:
+            rc = self._L.ofs_associate_quality(self._h, len(ids), _p(ids), _p(offs), _p(q),
+                                               *(map(_p, a) if a else (None,) * 3), _p(f), *res, self.threads)
+        elif a is None:
             rc = self._L.ofs_associate(self._h, len(ids), _p(ids), _p(offs), _p(f), *res, self.threads)
         else:
             rc = self._L.ofs_associate_attr(self._h, len(ids), _p(ids), _p(offs), *map(_p, a), _p(f), *res,
@@ -222,6 +266,28 @@ class FeatureStore:
         feats = np.zeros((len(ids), self.K, self.D), np.float32)
         self._L.ofs_fetch(self._h, len(ids), _p(ids), int(bool(remove)), _p(counts), _p(feats))
         return counts, feats
+
+    def fetch_quality(self, ids, remove=False):
+        """(counts, features, qualities[n][K]) of a quality store, rows in the track's order (best first)."""
+        ids = np.ascontiguousarray(ids, dtype=np.uint64)
+        counts = np.zeros(len(ids), np.int32)
+        feats = np.zeros((len(ids), self.K, self.D), np.float32)
+        qual = np.zeros((len(ids), self.K), np.float32)
+        if self._L.ofs_fetch_quality(self._h, len(ids), _p(ids), int(bool(remove)), _p(counts), _p(feats), _p(qual)) < 0:
+            raise ValueError("fetch_quality() needs a quality store")
+        return counts, feats, qual
+
+    def merge_history(self, ids):
+        """The merge history of each of the tracks `ids` (an empty array where an id is not stored)."""
+        ids = np.ascontiguousarray(ids, dtype=np.uint64)
+        lens = np.zeros(len(ids), np.int32)
+        total = self._L.ofs_merge_history(self._h, len(ids), _p(ids), _p(lens), 0, None)
+        if total < 0:
+            raise ValueError("merge_history() needs a quality store")
+        out = np.zeros(max(1, total), np.uint64)
+        self._L.ofs_merge_history(self._h, len(ids), _p(ids), _p(lens), total, _p(out))
+        offs = np.concatenate([[0], np.cumsum(lens)])
+        return [out[offs[i]: offs[i + 1]].copy() for i in range(len(ids))]
 
     def attributes(self, ids):
         """(sources, t_start, t_end) of the tracks `ids` (0 where an id is not stored) of a gated store."""

@@ -17,6 +17,12 @@
 // compatible with the winner's window as extended by the queries merged into it earlier in the call, else the query
 // becomes a new track; merge_owned refuses a call with an incompatible pair (checked in pair order) before anything
 // changes.
+// Retention (retention != 0): the rule of examples/track_merging.rs's `optimize` (:279-297) instead of the bench's newest
+// K.  Each observation carries an f32 quality and each track a merge history (Track::get_merge_history), [id] when it is
+// created, to which every merge appends the source's whole history (Track::merge with merge_history = true,
+// src/track.rs:522-588).  After an observation is appended or a merge concatenates dest ++ src, the list is stably sorted
+// by quality, descending, and truncated to c(h) = min(K, (u64)((float)initial_capacity * powf(merge_extension, (float)h)))
+// with h the track's history length (:257-265).  Queries are fresh tracks (h = 1) built the same way.
 #include <algorithm>
 #include <cmath>
 #include <cstdint>
@@ -101,9 +107,11 @@ void parallel_for(int n, int threads, const std::function<void(int, int)>& fn) {
 
 struct Track {
   uint64_t id;
-  std::vector<std::vector<float>> obs;   // zero-padded to d8, oldest first
+  std::vector<std::vector<float>> obs;   // zero-padded to d8, oldest first (a quality store: the track's order)
   uint64_t src = 0;                      // attributes of a gated store
   int64_t t0 = 0, t1 = 0;
+  std::vector<float> q;                  // a quality store: the quality of each observation
+  std::vector<uint64_t> hist;            // a quality store: the merge history
 };
 
 }  // namespace
@@ -112,6 +120,8 @@ struct ofs_store {
   int metric, K, D, d8, topn, min_votes;
   float filter, max_distance;
   int gate = 0;   // 0: no attributes; 1: windows disjoint and sources equal; 2: windows disjoint
+  int retention = 0;   // 0: newest K; 1: best by quality, capacity growing with the merge history
+  std::vector<int> cap_tab;   // retention 1: c(h) for h = 0 .. the first h with c(h) == K (or h = 0 alone when constant)
   std::vector<Track> tracks;
   std::unordered_map<uint64_t, size_t> pos;
 
@@ -135,6 +145,41 @@ struct ofs_store {
   void keep_newest(std::vector<std::vector<float>>& o) const {
     if ((int)o.size() > K) o.erase(o.begin(), o.end() - K);
   }
+  // retention 1: c(h), from the table the first h with c(h) == K ends (a constant capacity has one entry)
+  int capacity(size_t h) const { return cap_tab[std::min(h, cap_tab.size() - 1)]; }
+  // retention 1: optimize, the stable sort by quality, descending (-0.0 == +0.0), then the truncation to c(h)
+  void keep_best(Track& t) const {
+    std::vector<size_t> ix(t.obs.size());
+    for (size_t i = 0; i < ix.size(); ++i) ix[i] = i;
+    std::stable_sort(ix.begin(), ix.end(), [&](size_t a, size_t b) { return t.q[a] > t.q[b]; });
+    ix.resize(std::min(ix.size(), (size_t)capacity(t.hist.size())));
+    std::vector<std::vector<float>> obs;
+    std::vector<float> q;
+    for (size_t i : ix) { obs.push_back(std::move(t.obs[i])); q.push_back(t.q[i]); }
+    t.obs.swap(obs);
+    t.q.swap(q);
+  }
+  // Track::merge: dest ++ src, and a quality store's history and optimize
+  void merge_into(Track& d, const Track& src) const {
+    d.obs.insert(d.obs.end(), src.obs.begin(), src.obs.end());
+    if (!retention) { keep_newest(d.obs); return; }
+    d.q.insert(d.q.end(), src.q.begin(), src.q.end());
+    d.hist.insert(d.hist.end(), src.hist.begin(), src.hist.end());
+    keep_best(d);
+  }
+  // add_observation + optimize of one row
+  void append(Track& t, const float* feat, float quality) const {
+    t.obs.push_back(pad(feat));
+    if (!retention) { keep_newest(t.obs); return; }
+    t.q.push_back(quality);
+    keep_best(t);
+  }
+  Track fresh(uint64_t id) const {
+    Track t;
+    t.id = id;
+    if (retention) t.hist.push_back(id);
+    return t;
+  }
   float metric_of(const float* a, const float* b) const {
     if (metric == 0) return orc_euclidean_blocks(a, b, d8 / 8);
     return 1.0f - orc_cosine_blocks(a, b, d8 / 8);
@@ -144,18 +189,16 @@ struct ofs_store {
     for (size_t i = 0; i < tracks.size(); ++i) pos[tracks[i].id] = i;
   }
 
-  // TrackBuilder: each observation through add_observation (and optimize), so only the newest K remain
+  // TrackBuilder: each observation through add_observation (and optimize), so only the newest K remain (a quality
+  // store: the best c(1), with the qualities `qual`, one per row)
   std::vector<Track> build_queries(int Q, const uint64_t* ids, const int32_t* offs, const float* feats,
                                    const uint64_t* src = nullptr, const int64_t* t0 = nullptr,
-                                   const int64_t* t1 = nullptr) const {
+                                   const int64_t* t1 = nullptr, const float* qual = nullptr) const {
     std::vector<Track> qs((size_t)Q);
     for (int q = 0; q < Q; ++q) {
-      qs[q].id = ids[q];
+      qs[q] = fresh(ids[q]);
       if (src) { qs[q].src = src[q]; qs[q].t0 = t0[q]; qs[q].t1 = t1[q]; }
-      for (int r = offs[q]; r < offs[q + 1]; ++r) {
-        qs[q].obs.push_back(pad(feats + (size_t)r * D));
-        keep_newest(qs[q].obs);
-      }
+      for (int r = offs[q]; r < offs[q + 1]; ++r) append(qs[q], feats + (size_t)r * D, qual ? qual[r] : 0.0f);
     }
     return qs;
   }
@@ -235,12 +278,14 @@ void ofs_destroy(ofs_store* s) { delete s; }
 
 // TrackStore::add, src/track/store.rs:530-568, in call order
 int ofs_add(ofs_store* s, int n, const uint64_t* ids, const float* feats) {
-  if (s->gate) return -1;
+  if (s->gate || s->retention) return -1;
   for (int i = 0; i < n; ++i) {
     auto it = s->pos.find(ids[i]);
     if (it == s->pos.end()) {
       s->pos[ids[i]] = s->tracks.size();
-      s->tracks.push_back({ids[i], {s->pad(feats + (size_t)i * s->D)}});
+      Track t = s->fresh(ids[i]);
+      t.obs.push_back(s->pad(feats + (size_t)i * s->D));
+      s->tracks.push_back(std::move(t));
     } else {
       auto& o = s->tracks[it->second].obs;
       o.push_back(s->pad(feats + (size_t)i * s->D));
@@ -252,7 +297,7 @@ int ofs_add(ofs_store* s, int n, const uint64_t* ids, const float* feats) {
 
 int ofs_search(ofs_store* s, int Q, const uint64_t* ids, const int32_t* offs, const float* feats, int32_t* counts,
                uint64_t* winners, double* weights, int threads) {
-  if (s->gate || s->check(Q, ids, offs, false)) return -1;
+  if (s->gate || s->retention || s->check(Q, ids, offs, false)) return -1;
   if (Q == 0) return 0;
   s->write(s->search(s->build_queries(Q, ids, offs, feats), threads), counts, winners, weights);
   return 0;
@@ -261,10 +306,10 @@ int ofs_search(ofs_store* s, int Q, const uint64_t* ids, const int32_t* offs, co
 // one iteration of benches/feature_tracker.rs: search, then merge_external into results[0].winner_track or add_track
 static int associate(ofs_store* s, int Q, const uint64_t* ids, const int32_t* offs, const float* feats,
                      const uint64_t* src, const int64_t* t0, const int64_t* t1, int32_t* counts, uint64_t* winners,
-                     double* weights, uint64_t* track_ids, uint8_t* merged, int threads) {
+                     double* weights, uint64_t* track_ids, uint8_t* merged, int threads, const float* qual = nullptr) {
   if (s->check(Q, ids, offs, true)) return -1;
   if (Q == 0) return 0;
-  auto qs = s->build_queries(Q, ids, offs, feats, src, t0, t1);
+  auto qs = s->build_queries(Q, ids, offs, feats, src, t0, t1, qual);
   const auto r = s->search(qs, threads);
   s->write(r, counts, winners, weights);
   for (int q = 0; q < Q; ++q) {
@@ -272,9 +317,7 @@ static int associate(ofs_store* s, int Q, const uint64_t* ids, const int32_t* of
     if (!r[q].empty() && s->compatible(qs[q], s->tracks[s->pos.at(r[q][0].winner)])) {
       // Track::merge (src/track.rs:522-600): extend, then optimize keeps the newest K
       Track& dt = s->tracks[s->pos.at(r[q][0].winner)];
-      auto& dst = dt.obs;
-      dst.insert(dst.end(), qs[q].obs.begin(), qs[q].obs.end());
-      s->keep_newest(dst);
+      s->merge_into(dt, qs[q]);
       if (s->gate) ofs_store::hull(dt, qs[q]);
       track_ids[q] = r[q][0].winner;
       merged[q] = 1;
@@ -290,7 +333,7 @@ static int associate(ofs_store* s, int Q, const uint64_t* ids, const int32_t* of
 
 int ofs_associate(ofs_store* s, int Q, const uint64_t* ids, const int32_t* offs, const float* feats, int32_t* counts,
                   uint64_t* winners, double* weights, uint64_t* track_ids, uint8_t* merged, int threads) {
-  if (s->gate) return -1;
+  if (s->gate || s->retention) return -1;
   return associate(s, Q, ids, offs, feats, nullptr, nullptr, nullptr, counts, winners, weights, track_ids, merged,
                    threads);
 }
@@ -361,8 +404,8 @@ int ofs_search_owned(ofs_store* s, int n, const uint64_t* ids, int each, int32_t
 }
 
 // merge_owned(dest, src, None, remove_src, false) (src/track/store.rs:584-611) for each pair in order: fetch src, extend
-// dest by its observations and keep the newest K (Track::merge + optimize), then put src back at its position or drop
-// it.  Rejected (-1) before anything changes: dest == src, a dest or src that is not stored, and with remove_src a pair
+// dest by its observations and keep the newest K (Track::merge + optimize; a quality store: merge_history = true and the
+// best c(h)), then put src back at its position or drop it.  Rejected (-1) before anything changes: dest == src, a dest or src that is not stored, and with remove_src a pair
 // naming a track an earlier pair removed.
 int ofs_merge_owned(ofs_store* s, int n, const uint64_t* dest, const uint64_t* src, int remove_src) {
   if (n < 0) return -1;
@@ -385,9 +428,7 @@ int ofs_merge_owned(ofs_store* s, int n, const uint64_t* dest, const uint64_t* s
       return -1;
     }
     if (s->gate) ofs_store::hull(dt, t);
-    auto& o = dt.obs;
-    o.insert(o.end(), t.obs.begin(), t.obs.end());
-    s->keep_newest(o);
+    s->merge_into(dt, t);
     if (!remove_src) s->tracks.insert(s->tracks.begin() + (std::ptrdiff_t)at, t);   // add_track
     s->reindex();
   }
@@ -412,7 +453,7 @@ static bool bad_windows(int n, const int64_t* t0, const int64_t* t1) {
 // the windows; a source that differs from the track's is refused (the reference's WrongCamID) before anything changes.
 int ofs_add_attr(ofs_store* s, int n, const uint64_t* ids, const uint64_t* src, const int64_t* t0, const int64_t* t1,
                  const float* feats) {
-  if (!s->gate || n < 0 || bad_windows(n, t0, t1)) return -1;
+  if (!s->gate || s->retention || n < 0 || bad_windows(n, t0, t1)) return -1;
   std::unordered_map<uint64_t, uint64_t> source;
   for (const Track& t : s->tracks) source[t.id] = t.src;
   for (int i = 0; i < n; ++i) {
@@ -423,7 +464,10 @@ int ofs_add_attr(ofs_store* s, int n, const uint64_t* ids, const uint64_t* src, 
     auto it = s->pos.find(ids[i]);
     if (it == s->pos.end()) {
       s->pos[ids[i]] = s->tracks.size();
-      s->tracks.push_back({ids[i], {s->pad(feats + (size_t)i * s->D)}, src[i], t0[i], t1[i]});
+      Track t = s->fresh(ids[i]);
+      t.obs.push_back(s->pad(feats + (size_t)i * s->D));
+      t.src = src[i]; t.t0 = t0[i]; t.t1 = t1[i];
+      s->tracks.push_back(std::move(t));
     } else {
       Track& t = s->tracks[it->second];
       t.obs.push_back(s->pad(feats + (size_t)i * s->D));
@@ -438,7 +482,7 @@ int ofs_add_attr(ofs_store* s, int n, const uint64_t* ids, const uint64_t* src, 
 int ofs_search_attr(ofs_store* s, int Q, const uint64_t* ids, const int32_t* offs, const uint64_t* src, const int64_t* t0,
                     const int64_t* t1, const float* feats, int32_t* counts, uint64_t* winners, double* weights,
                     int threads) {
-  if (!s->gate || s->check(Q, ids, offs, false) || bad_windows(Q, t0, t1)) return -1;
+  if (!s->gate || s->retention || s->check(Q, ids, offs, false) || bad_windows(Q, t0, t1)) return -1;
   if (Q == 0) return 0;
   s->write(s->search(s->build_queries(Q, ids, offs, feats, src, t0, t1), threads), counts, winners, weights);
   return 0;
@@ -447,7 +491,7 @@ int ofs_search_attr(ofs_store* s, int Q, const uint64_t* ids, const int32_t* off
 int ofs_associate_attr(ofs_store* s, int Q, const uint64_t* ids, const int32_t* offs, const uint64_t* src,
                        const int64_t* t0, const int64_t* t1, const float* feats, int32_t* counts, uint64_t* winners,
                        double* weights, uint64_t* track_ids, uint8_t* merged, int threads) {
-  if (!s->gate || bad_windows(Q, t0, t1)) return -1;
+  if (!s->gate || s->retention || bad_windows(Q, t0, t1)) return -1;
   return associate(s, Q, ids, offs, feats, src, t0, t1, counts, winners, weights, track_ids, merged, threads);
 }
 
@@ -464,6 +508,124 @@ int64_t ofs_fetch_attr(ofs_store* s, int n, const uint64_t* ids, uint64_t* src, 
     found += ok;
   }
   return found;
+}
+
+// ---- retention by quality (retention != 0)
+// Sets the rule and its parameters while the store holds no tracks.  Refused (-1): an unknown rule, initial_capacity < 1,
+// a merge_extension that is not finite or is below 1, and parameters whose capacity has not reached K by h = 65536
+// unless merge_extension == 1.
+int ofs_set_retention(ofs_store* s, int rule, int initial_capacity, float merge_extension) {
+  if ((rule != 0 && rule != 1) || !s->tracks.empty()) return -1;
+  if (rule == 0) {
+    s->retention = 0;
+    s->cap_tab.clear();
+    return 0;
+  }
+  if (initial_capacity < 1 || !std::isfinite(merge_extension) || merge_extension < 1.0f) return -1;
+  auto c = [&](int h) {   // f32 arithmetic, then Rust's saturating `as u64`, then min(K, .)
+    const float v = (float)initial_capacity * powf(merge_extension, (float)h);
+    return v >= (float)s->K ? s->K : (int)(uint64_t)v;
+  };
+  std::vector<int> tab{c(0)};
+  while (tab.back() < s->K && merge_extension != 1.0f) {
+    if (tab.size() > 65536) return -1;
+    tab.push_back(c((int)tab.size()));
+  }
+  s->retention = 1;
+  s->cap_tab = tab;
+  return 0;
+}
+
+static bool bad_quality(int n, const float* q) {
+  for (int i = 0; i < n; ++i)
+    if (std::isnan(q[i])) return true;
+  return false;
+}
+
+// TrackStore::add of a quality store: an unknown id creates a track with history [id]; each row is appended and the
+// track optimized at its capacity.  src == nullptr: an ungated store.
+int ofs_add_quality(ofs_store* s, int n, const uint64_t* ids, const float* qual, const uint64_t* src, const int64_t* t0,
+                    const int64_t* t1, const float* feats) {
+  if (!s->retention || (s->gate != 0) != (src != nullptr) || n < 0 || bad_quality(n, qual)) return -1;
+  if (src) {
+    if (bad_windows(n, t0, t1)) return -1;
+    std::unordered_map<uint64_t, uint64_t> source;
+    for (const Track& t : s->tracks) source[t.id] = t.src;
+    for (int i = 0; i < n; ++i)
+      if (source.emplace(ids[i], src[i]).first->second != src[i]) return -1;
+  }
+  for (int i = 0; i < n; ++i) {
+    auto it = s->pos.find(ids[i]);
+    if (it == s->pos.end()) {
+      Track t = s->fresh(ids[i]);
+      if (src) { t.src = src[i]; t.t0 = t0[i]; t.t1 = t1[i]; }
+      s->pos[ids[i]] = s->tracks.size();
+      s->tracks.push_back(std::move(t));
+      it = s->pos.find(ids[i]);
+      s->tracks[it->second].obs.push_back(s->pad(feats + (size_t)i * s->D));
+      s->tracks[it->second].q.push_back(qual[i]);
+    } else {
+      Track& t = s->tracks[it->second];
+      s->append(t, feats + (size_t)i * s->D, qual[i]);
+      if (src) { t.t0 = std::min(t.t0, t0[i]); t.t1 = std::max(t.t1, t1[i]); }
+    }
+  }
+  return 0;
+}
+
+int ofs_search_quality(ofs_store* s, int Q, const uint64_t* ids, const int32_t* offs, const float* qual,
+                       const uint64_t* src, const int64_t* t0, const int64_t* t1, const float* feats, int32_t* counts,
+                       uint64_t* winners, double* weights, int threads) {
+  if (!s->retention || (s->gate != 0) != (src != nullptr) || s->check(Q, ids, offs, false)) return -1;
+  if (Q == 0) return 0;
+  if (bad_quality(offs[Q], qual) || (src && bad_windows(Q, t0, t1))) return -1;
+  s->write(s->search(s->build_queries(Q, ids, offs, feats, src, t0, t1, qual), threads), counts, winners, weights);
+  return 0;
+}
+
+int ofs_associate_quality(ofs_store* s, int Q, const uint64_t* ids, const int32_t* offs, const float* qual,
+                          const uint64_t* src, const int64_t* t0, const int64_t* t1, const float* feats,
+                          int32_t* counts, uint64_t* winners, double* weights, uint64_t* track_ids, uint8_t* merged,
+                          int threads) {
+  if (!s->retention || (s->gate != 0) != (src != nullptr) || s->check(Q, ids, offs, true)) return -1;
+  if (Q == 0) return 0;
+  if (bad_quality(offs[Q], qual) || (src && bad_windows(Q, t0, t1))) return -1;
+  return associate(s, Q, ids, offs, feats, src, t0, t1, counts, winners, weights, track_ids, merged, threads, qual);
+}
+
+// ofs_fetch plus the qualities [n][K] of the rows returned (0 past a count: an id that is not stored, or that an
+// earlier entry of the same call removed, returns none)
+int64_t ofs_fetch_quality(ofs_store* s, int n, const uint64_t* ids, int remove, int32_t* counts, float* feats,
+                          float* qual) {
+  if (!s->retention) return -1;
+  std::memset(qual, 0, sizeof(float) * (size_t)n * s->K);
+  std::unordered_set<uint64_t> gone;
+  for (int i = 0; i < n; ++i) {
+    auto it = s->pos.find(ids[i]);
+    if (it == s->pos.end() || gone.count(ids[i])) continue;
+    const Track& t = s->tracks[it->second];
+    std::copy(t.q.begin(), t.q.end(), qual + (size_t)i * s->K);
+    if (remove) gone.insert(ids[i]);
+  }
+  return ofs_fetch(s, n, ids, remove, counts, feats);
+}
+
+// Track::get_merge_history of the tracks `ids` in CSR form: lengths[i] (0: not stored), the histories concatenated into
+// out (at most cap entries written); returns the total length
+int64_t ofs_merge_history(ofs_store* s, int n, const uint64_t* ids, int32_t* lengths, int64_t cap, uint64_t* out) {
+  if (!s->retention) return -1;
+  int64_t total = 0;
+  for (int i = 0; i < n; ++i) {
+    auto it = s->pos.find(ids[i]);
+    lengths[i] = 0;
+    if (it == s->pos.end()) continue;
+    for (uint64_t h : s->tracks[it->second].hist) {
+      if (total < cap) out[total] = h;
+      ++total;
+    }
+    lengths[i] = (int32_t)s->tracks[it->second].hist.size();
+  }
+  return total;
 }
 
 int64_t ofs_size(ofs_store* s) { return (int64_t)s->tracks.size(); }

@@ -549,8 +549,9 @@ int sb200_fstore_search_owned(sb200_fstore* s, int32_t n, const uint64_t* ids, i
  * remove) when remove_src.  SB200_ERR_INVALID, before anything changes, for dest == src (the reference's TrackNotFound:
  * it fetched src first), a dest or src that is not stored, and, with remove_src, a pair that names a track an earlier
  * pair removed; the reference would apply the pairs in front and then return the error, the same deviation as
- * sb200_fstore_associate's.  `classes` and `merge_history` have no counterpart: there is one feature class and no
- * history.  sb200_fstore_last_stage_ms reports the row moves as the apply stage. */
+ * sb200_fstore_associate's.  `classes` has no counterpart: there is one feature class; a newest store keeps no merge
+ * history, a quality store (sb200_fstore_set_retention) merges with merge_history = true and its rule.
+ * sb200_fstore_last_stage_ms reports the row moves as the apply stage. */
 int sb200_fstore_merge_owned(sb200_fstore* s, int32_t n, const uint64_t* dest_ids, const uint64_t* src_ids,
                              int32_t remove_src);
 
@@ -647,6 +648,68 @@ int sb200_fstore_associate_attr(sb200_fstore* s, int32_t n_queries, const uint64
 int64_t sb200_fstore_fetch_attr(sb200_fstore* s, int32_t n, const uint64_t* ids, uint64_t* source, int64_t* t_start,
                                 int64_t* t_end);
 
+/* ---- retention by quality: each track keeps its best observations, and its capacity grows with its merges ----
+ * The store semantics of examples/track_merging.rs (its `optimize`, :279-297, with the defaults of :257-265) in place of
+ * the newest K of benches/feature_tracker.rs:
+ *   SB200_FSTORE_KEEP_NEWEST (0, the default): every track keeps its newest K observations; every call behaves as it
+ *     always has, and the store saves as version 1 or 2.
+ *   SB200_FSTORE_KEEP_BEST_QUALITY (1): every observation carries an f32 quality (the example's observation attribute,
+ *     e.g. VisualSortObservation.feature_quality) and every track a merge history (Track::get_merge_history): [id] when
+ *     the track is created (add of an unknown id, a query that becomes a new track), to which every merge appends the
+ *     source's whole history (Track::merge with merge_history = true, src/track.rs:522-588): associate merging a query
+ *     into its winner, and each merge_owned pair.  A source left in the store keeps its history.  A track of history
+ *     length h holds at most
+ *       c(h) = min(K, (u64)((float)initial_capacity * powf(merge_extension, (float)h)))
+ *     observations, f32 arithmetic and a truncating cast as Rust's `as u64`; the host tabulates c(h) with the C
+ *     library's powf (which Rust's f32::powf calls on Linux) up to the first h with c(h) == K, and the device never
+ *     evaluates powf.  After a row is appended (add) or a merge concatenates dest ++ src, the track's list is stably
+ *     sorted by quality, descending (equal qualities keep their order: dest's rows first, then src's; -0.0 == +0.0), and
+ *     truncated to c(h) at the destination's new h.  Merges of one call are applied in order, each at its own c(h): a
+ *     row dropped by an earlier merge does not come back.  A query of search / associate is a fresh track (h = 1): its
+ *     best c(1) rows in quality order (ties to the earlier row) take part, and entries are enumerated in that order, so
+ *     the f64 weights follow it.  Stored tracks are searched in their order, best first.
+ * Calls on a quality store: sb200_fstore_add_quality, _search_quality and _associate_quality (the plain, _device and
+ * _attr forms are refused; the _quality forms are refused on a newest store); search_owned and merge_owned as always,
+ * with the rule above for merge_owned; sb200_fstore_fetch returns each track's rows in its order, best first, and
+ * sb200_fstore_fetch_quality their qualities too.  A gated quality store decides every associate destination as a gated
+ * store does, then applies the quality merge.  sb200_fstore_associate_wasted on a quality store is refused, changing
+ * nothing (the tracker's feature history keeps no quality).
+ * Refusals, SB200_ERR_INVALID with sb200_last_error naming the cause, decided on the host before anything changes: a NaN
+ * quality (the reference panics on it, partial_cmp().unwrap()); in sb200_fstore_set_retention an unknown rule, a store
+ * that holds tracks, initial_capacity < 1, a merge_extension that is not finite or is below 1, and parameters whose
+ * capacity has not reached K by h = 65536 unless merge_extension == 1 (a constant capacity) -- values the reference
+ * would accept. */
+#define SB200_FSTORE_KEEP_NEWEST 0
+#define SB200_FSTORE_KEEP_BEST_QUALITY 1
+/* Sets the rule and its parameters (the example's defaults are 4 and 1.5; ignored for SB200_FSTORE_KEEP_NEWEST).
+ * Allowed while the store holds no tracks, as sb200_fstore_set_gate.  A loaded store has its blob's. */
+int sb200_fstore_set_retention(sb200_fstore* s, int32_t rule, int32_t initial_capacity, float merge_extension);
+/* Any output may be NULL. */
+int sb200_fstore_get_retention(sb200_fstore* s, int32_t* rule, int32_t* initial_capacity, float* merge_extension);
+/* sb200_fstore_add / _search / _associate of a quality store.  quality: host memory, one value per row of the feature
+ * column (n for add, obs_offsets[n_queries] for search / associate).  attrs: a gated store's triples, NULL on an ungated
+ * store.  Exactly one of `features` (host) and `d_features` (device, with `cuda_stream` as for the _device forms) is
+ * non-NULL; either is in the type set by sb200_fstore_set_feature_type.  Outputs as for the calls without quality. */
+int sb200_fstore_add_quality(sb200_fstore* s, int32_t n, const uint64_t* ids, const float* quality,
+                             const sb200_fstore_attrs* attrs, const float* features, const void* d_features,
+                             void* cuda_stream);
+int sb200_fstore_search_quality(sb200_fstore* s, int32_t n_queries, const uint64_t* query_ids,
+                                const int32_t* obs_offsets, const float* quality, const sb200_fstore_attrs* attrs,
+                                const float* features, const void* d_features, int32_t* counts, uint64_t* winners,
+                                double* weights, void* cuda_stream);
+int sb200_fstore_associate_quality(sb200_fstore* s, int32_t n_queries, const uint64_t* query_ids,
+                                   const int32_t* obs_offsets, const float* quality, const sb200_fstore_attrs* attrs,
+                                   const float* features, const void* d_features, int32_t* counts, uint64_t* winners,
+                                   double* weights, uint64_t* track_ids, uint8_t* merged, void* cuda_stream);
+/* sb200_fstore_fetch of a quality store, plus quality[n][K]: the quality of each returned row (0 past counts[i]). */
+int64_t sb200_fstore_fetch_quality(sb200_fstore* s, int32_t n, const uint64_t* ids, int32_t remove, int32_t* counts,
+                                   float* features, float* quality);
+/* The merge histories of the tracks `ids` of a quality store in CSR form: lengths[i] (0: not stored), and the histories
+ * concatenated, in order, into out (at most `cap` entries written; out may be NULL when cap == 0).  Returns their total
+ * length, or a negative status. */
+int64_t sb200_fstore_merge_history(sb200_fstore* s, int32_t n, const uint64_t* ids, int32_t* lengths, int64_t cap,
+                                   uint64_t* out);
+
 /* ---- the store blob ----
  * The whole store as one relocatable block of bytes: this header, then four sections at 256-byte aligned offsets, gaps
  * zeroed, in this order: ids[live] (u64), cnt[live] (i32 observations held), start[live] (i32 ring slot of the oldest
@@ -708,6 +771,39 @@ typedef struct {
   uint64_t sec_off[SB200_FSTORE_BLOB_SECTIONS_V2];
   uint64_t sec_bytes[SB200_FSTORE_BLOB_SECTIONS_V2];
 } sb200_fstore_blob_header_v2;
+/* The blob of a quality store: version 3, this header (the version-2 fields, the retention rule and its parameters),
+ * then ten sections laid out as version 1's: ids, cnt, start, feat, source, t_start, t_end (0 bytes each on an ungated
+ * store), quality[live][max_observations] (f32, slot by slot as feat, 0 in a slot that holds no observation),
+ * history_length[live] (i32, >= 1) and history[sum of history_length] (u64, the histories concatenated in store order,
+ * each starting with its track's id).  A newest store writes version 1 or 2 as before.  Load also refuses an unknown
+ * rule or bad parameters, a history length of 0, a history whose first id is not its track's id, a history section
+ * whose size is not the sum of the lengths, and every state the rule cannot produce: a ring start other than 0, a count
+ * above c(history length), and (by kernel) a NaN quality in a filled slot or a list out of quality order.  Empty slots
+ * of feat and quality are written as zeros, so two stores holding the same lists and histories give byte-equal blobs. */
+#define SB200_FSTORE_BLOB_VERSION_QUALITY 3u
+#define SB200_FSTORE_BLOB_SECTIONS_V3 10
+typedef struct {
+  uint32_t magic;
+  uint32_t version; /* SB200_FSTORE_BLOB_VERSION_QUALITY */
+  uint64_t total_bytes;
+  int32_t metric;
+  float distance_filter;
+  int32_t max_observations;
+  int32_t feature_dim;
+  int32_t topn;
+  float max_distance;
+  int32_t min_votes;
+  int32_t d8;
+  int32_t feature_type;
+  int32_t storage_type;
+  int64_t live;
+  int32_t gate;             /* SB200_FSTORE_GATE_* (NONE allowed) */
+  int32_t retention;        /* SB200_FSTORE_KEEP_BEST_QUALITY */
+  int32_t initial_capacity;
+  float merge_extension;
+  uint64_t sec_off[SB200_FSTORE_BLOB_SECTIONS_V3];
+  uint64_t sec_bytes[SB200_FSTORE_BLOB_SECTIONS_V3];
+} sb200_fstore_blob_header_v3;
 /* Writes the blob to `buf` (`cap` bytes; host memory, or device memory on any device) and its size to *bytes.
  * buf == NULL: reports the size and writes nothing.  SB200_ERR_CAPACITY when cap is too small: nothing is written and
  * *bytes is still set.  Rows are copied, not re-derived; the store is not changed.  Timers and the stream are not part

@@ -129,6 +129,24 @@ class FstoreBlobHeaderV2(C.Structure):
     ]
 
 
+FSTORE_BLOB_VERSION_QUALITY, FSTORE_BLOB_SECTIONS_V3 = 3, 10
+# retention rules of the feature store (sb200_fstore_set_retention)
+FSTORE_KEEP_NEWEST, FSTORE_KEEP_BEST_QUALITY = 0, 1
+
+
+class FstoreBlobHeaderV3(C.Structure):
+    """sb200_fstore_blob_header_v3: the first bytes of the blob of a quality store."""
+
+    _fields_ = FstoreBlobHeader._fields_[:-2] + [
+        ("gate", C.c_int32),
+        ("retention", C.c_int32),
+        ("initial_capacity", C.c_int32),
+        ("merge_extension", C.c_float),
+        ("sec_off", C.c_uint64 * FSTORE_BLOB_SECTIONS_V3),
+        ("sec_bytes", C.c_uint64 * FSTORE_BLOB_SECTIONS_V3),
+    ]
+
+
 class FstoreAttrs(C.Structure):
     """sb200_fstore_attrs: host columns of one source and one [t_start, t_end] window per row."""
 
@@ -160,6 +178,9 @@ EXPORTS = [
     "sb200_fstore_merge_owned", "sb200_fstore_set_storage_type", "sb200_fstore_get_storage_type",
     "sb200_fstore_associate_wasted", "sb200_fstore_set_gate", "sb200_fstore_get_gate", "sb200_fstore_add_attr",
     "sb200_fstore_search_attr", "sb200_fstore_associate_attr", "sb200_fstore_fetch_attr",
+    "sb200_fstore_set_retention", "sb200_fstore_get_retention", "sb200_fstore_add_quality",
+    "sb200_fstore_search_quality", "sb200_fstore_associate_quality", "sb200_fstore_fetch_quality",
+    "sb200_fstore_merge_history",
 ]
 
 
@@ -267,6 +288,14 @@ def lib():
         "sb200_fstore_associate_attr": (C.c_int, [vp, i32, vp, vp, C.POINTER(FstoreAttrs), vp, vp, vp, vp, vp, vp, vp,
                                                   vp]),
         "sb200_fstore_fetch_attr": (i64, [vp, i32, vp, vp, vp, vp]),
+        "sb200_fstore_set_retention": (C.c_int, [vp, i32, i32, C.c_float]),
+        "sb200_fstore_get_retention": (C.c_int, [vp, C.POINTER(i32), C.POINTER(i32), C.POINTER(C.c_float)]),
+        "sb200_fstore_add_quality": (C.c_int, [vp, i32, vp, vp, C.POINTER(FstoreAttrs), vp, vp, vp]),
+        "sb200_fstore_search_quality": (C.c_int, [vp, i32, vp, vp, vp, C.POINTER(FstoreAttrs), vp, vp, vp, vp, vp, vp]),
+        "sb200_fstore_associate_quality": (C.c_int, [vp, i32, vp, vp, vp, C.POINTER(FstoreAttrs), vp, vp, vp, vp, vp,
+                                                     vp, vp, vp]),
+        "sb200_fstore_fetch_quality": (i64, [vp, i32, vp, i32, vp, vp, vp]),
+        "sb200_fstore_merge_history": (i64, [vp, i32, vp, vp, i64, vp]),
         "sb200_fstore_get_storage_type": (C.c_int, [vp, C.POINTER(i32)]),
         "sb200_fstore_associate_wasted": (i64, [vp, vp, i64, u64, vp, vp, vp, vp, vp, vp, i32, vp, vp, vp, vp, vp, vp, vp,
                                                 vp, vp, vp]),

@@ -11,6 +11,11 @@
 // storage type.  A gated store (sb200_fstore_set_gate) also keeps a source and a window per track in three device
 // columns of its own; a call reads back the triples of the tracks it touches, and an ungated store allocates none.
 // Allocation, growth, compaction, the gate switch and the blob sections all go by one table of columns (kCols).
+// A quality store (sb200_fstore_set_retention) keeps each track's rows in the track's order (best first) from ring slot
+// 0, so the search, fetch and owned kernels walk it unchanged, plus a quality per slot (qual) and a history length per
+// track (hlen) on the device and the merge histories on the host (hist, beside hid, updated from each call's
+// read-back).  Associate and add plan and apply their merges on the device (fs_launch_qmerge), with one read-back as on
+// a newest store; merge_owned plans on the host from the qualities of the tracks it touches, as it plans rings.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -18,6 +23,7 @@
 #include <cmath>
 #include <cstddef>
 #include <cstring>
+#include <numeric>
 #include <unordered_map>
 #include <unordered_set>
 #include <vector>
@@ -94,8 +100,13 @@ struct Column {
 
 using BlobHeader = sb200_fstore_blob_header;
 using BlobHeaderV2 = sb200_fstore_blob_header_v2;
-enum { kSecIds, kSecCnt, kSecStart, kSecFeat, kSecSrc, kSecT0, kSecT1 };
+using BlobHeaderV3 = sb200_fstore_blob_header_v3;
+enum { kSecIds, kSecCnt, kSecStart, kSecFeat, kSecSrc, kSecT0, kSecT1, kSecQual, kSecHlen, kSecHist };
 static_assert(offsetof(BlobHeaderV2, live) == offsetof(BlobHeader, live), "version 2 repeats version 1's fields");
+static_assert(offsetof(BlobHeaderV3, gate) == offsetof(BlobHeaderV2, gate), "version 3 repeats version 2's fields");
+static_assert(kSecHist + 1 == SB200_FSTORE_BLOB_SECTIONS_V3, "the version-3 section table");
+// the store kinds that have a column (sb200_fstore::Col::need)
+enum { kNeedAll, kNeedGate, kNeedQuality };
 
 // a gated call's triples on the host: n entries of each column
 struct Triples {
@@ -106,6 +117,33 @@ struct Triples {
 
 bool known_type(int t) { return t == SB200_FEATURE_F32 || t == SB200_FEATURE_F16 || t == SB200_FEATURE_BF16; }
 size_t type_bytes(int t) { return t == SB200_FEATURE_F32 ? 4 : 2; }
+
+// c(h) = min(K, (u64)((float)init * powf(ext, (float)h))) for h = 0 .. the first h with c(h) == K (h = 0 alone for a
+// constant capacity, ext == 1), as examples/track_merging.rs:257-265 computes it: f32 arithmetic with the C library's
+// powf (what Rust's f32::powf calls), then the truncating cast of `as u64`.  Refuses what the store does not take.
+int capacity_table(int K, int init, float ext, std::vector<int>* tab) {
+  if (init < 1) return fail(SB200_ERR_INVALID, "initial_capacity %d < 1", init);
+  if (!std::isfinite(ext) || ext < 1.0f) return fail(SB200_ERR_INVALID, "merge_extension %g is not finite or is below 1", ext);
+  auto c = [&](int h) {
+    const float v = (float)init * powf(ext, (float)h);
+    return v >= (float)K ? K : (int)(uint64_t)v;
+  };
+  tab->assign(1, c(0));
+  while (tab->back() < K && ext != 1.0f) {
+    if (tab->size() > 65536)
+      return fail(SB200_ERR_INVALID, "initial_capacity %d and merge_extension %g do not reach max_observations %d by a "
+                  "merge history of 65536", init, ext, K);
+    tab->push_back(c((int)tab->size()));
+  }
+  return 0;
+}
+
+// the first NaN of n qualities, or -1
+int first_nan(int n, const float* q) {
+  for (int i = 0; i < n; ++i)
+    if (std::isnan(q[i])) return i;
+  return -1;
+}
 
 int check_options(const sb200_fstore_options& o) {
   if (o.metric != SB200_VIS_EUCLIDEAN && o.metric != SB200_VIS_COSINE) return fail(SB200_ERR_INVALID, "unknown metric");
@@ -135,11 +173,19 @@ struct sb200_fstore {
   DBuf feat, cnt, start, ids, run;
   int gate = SB200_FSTORE_GATE_NONE;
   DBuf asrc, at0, at1;                       // gated store: [cap] source, t_start, t_end
-  // A store column: its buffer, bytes per track (0: K stored rows), whether only a gated store has it, whether allocation
-  // zero-fills it, and its blob section (kSec*) and name.  Without a section (-1) it is scratch, which growth and
-  // compaction start afresh.
-  struct Col { DBuf sb200_fstore::*buf; uint32_t w; bool gated, zero; int sec; const char* name; };
-  static constexpr int kNumCols = 8;
+  int keep = SB200_FSTORE_KEEP_NEWEST;       // retention rule, and its parameters for a quality store
+  int init_cap = 4;
+  float ext = 1.5f;
+  std::vector<int> cap_tab;                  // quality store: c(h) (capacity_table), and its device copy
+  DBuf dcap;
+  DBuf qual, hlen;                           // quality store: [cap][K] quality of the row in each slot, [cap] history length
+  DBuf dqr;                                  // quality store: the request rows' qualities of a call
+  std::vector<std::vector<uint64_t>> hist;   // quality store: merge history of each track, in store order
+  // A store column: its buffer, bytes per track (0: K stored rows) or per slot (per_obs), the kind of store that has it
+  // (kNeed*), whether allocation zero-fills it, and its blob section (kSec*) and name.  Without a section (-1) it is
+  // scratch, which growth and compaction start afresh.
+  struct Col { DBuf sb200_fstore::*buf; uint32_t w; bool per_obs; int need; bool zero; int sec; const char* name; };
+  static constexpr int kNumCols = 10;
   static const Col kCols[kNumCols];
   DBuf qattr;                                // a gated call's triples, [n] of each column
   std::vector<uint64_t> hid;                 // ids in store order
@@ -172,29 +218,42 @@ struct sb200_fstore {
   // bytes of one stored row (observation)
   static size_t row_bytes(int d8, int stype) { return (size_t)d8 * type_bytes(stype); }
   size_t row_bytes() const { return row_bytes(d8, stype); }
-  static size_t track_bytes(const Col& c, int K, size_t row_bytes) { return c.w ? c.w : K * row_bytes; }
+  static size_t track_bytes(const Col& c, int K, size_t row_bytes) {
+    return c.w ? (c.per_obs ? (size_t)K * c.w : c.w) : K * row_bytes;
+  }
   size_t track_bytes(const Col& c) const { return track_bytes(c, o.max_observations, row_bytes()); }
-  static bool has(const Col& c, int gate) { return gate || !c.gated; }   // a store with rule `gate` has column c
+  // a store with rule `gate` and retention `keep` has column c
+  static bool has(const Col& c, int gate, int keep) {
+    return c.need == kNeedAll || (c.need == kNeedGate && gate) || (c.need == kNeedQuality && keep);
+  }
+  bool has(const Col& c) const { return has(c, gate, keep); }
   // The blob sections of a store of `live` tracks (kSec* order): their bytes, which save writes and load expects, and
-  // (names != nullptr) their names.  Returns their number: 4, or 7 for a gated store.
-  static int sections(uint64_t live, int K, int d8, int stype, int gate, uint64_t* bytes, const char** names = nullptr) {
+  // (names != nullptr) their names.  Returns their number: 4, or 7 for a gated store; a quality store (version 3) has
+  // all 10, the attribute ones empty when it is ungated, and hist_total history entries.
+  static int sections(uint64_t live, int K, int d8, int stype, int gate, int keep, uint64_t hist_total, uint64_t* bytes,
+                      const char** names = nullptr) {
     int n = 0;
     for (const Col& c : kCols)
-      if (c.sec >= 0 && has(c, gate)) {
-        bytes[c.sec] = live * track_bytes(c, K, row_bytes(d8, stype));
+      if (c.sec >= 0 && (has(c, gate, keep) || (keep && c.need == kNeedGate))) {
+        bytes[c.sec] = has(c, gate, keep) ? live * track_bytes(c, K, row_bytes(d8, stype)) : 0;
         if (names) names[c.sec] = c.name;
         ++n;
       }
+    if (keep) {
+      bytes[kSecHist] = hist_total * 8;
+      if (names) names[kSecHist] = "history";
+      ++n;
+    }
     return n;
   }
 
-  // fresh columns of this store for max(n, 1) tracks in nw[] (one per kCols entry; attrs_only: the gated ones alone),
-  // zero-filled where the table says so; the caller copies what it keeps
-  int alloc(size_t n, DBuf* nw, bool attrs_only = false) {
+  // fresh columns of this store for max(n, 1) tracks in nw[] (one per kCols entry; only != kNeedAll: the columns of
+  // that kind of store alone), zero-filled where the table says so; the caller copies what it keeps
+  int alloc(size_t n, DBuf* nw, int only = kNeedAll) {
     n = std::max<size_t>(n, 1);
     for (int k = 0; k < kNumCols; ++k) {
       const Col& c = kCols[k];
-      if (!has(c, gate) || (attrs_only && !c.gated)) continue;
+      if (!has(c) || (only != kNeedAll && c.need != only)) continue;
       const size_t bytes = n * track_bytes(c);
       if (int rc = nw[k].ensure(bytes)) return rc;
       if (c.zero) CU(cudaMemsetAsync(nw[k].p, 0, bytes, st));
@@ -202,16 +261,16 @@ struct sb200_fstore {
     return 0;
   }
 
-  // exchanges the store's columns with nw[] (attrs_only: the gated ones alone)
-  void swap_columns(DBuf* nw, bool attrs_only = false) {
+  // exchanges the store's columns with nw[] (only != kNeedAll: the columns of that kind of store alone)
+  void swap_columns(DBuf* nw, int only = kNeedAll) {
     for (int k = 0; k < kNumCols; ++k)
-      if (!attrs_only || kCols[k].gated) std::swap(this->*kCols[k].buf, nw[k]);
+      if (only == kNeedAll || kCols[k].need == only) std::swap(this->*kCols[k].buf, nw[k]);
   }
 
   // the tracks every column holds as allocated, at most cap (after a storage type change: in rows of the new type)
   size_t held() const {
     size_t n = cap;
-    for (const Col& c : kCols) if (has(c, gate)) n = std::min(n, (this->*c.buf).bytes / track_bytes(c));
+    for (const Col& c : kCols) if (has(c)) n = std::min(n, (this->*c.buf).bytes / track_bytes(c));
     return n;
   }
 
@@ -227,7 +286,7 @@ struct sb200_fstore {
     if (int rc = alloc(nc, nw)) return rc;
     const size_t live = hid.size();
     for (int k = 0; k < kNumCols; ++k)   // the live tracks of the state columns
-      if (live && kCols[k].sec >= 0 && has(kCols[k], gate))
+      if (live && kCols[k].sec >= 0 && has(kCols[k]))
         CU(cudaMemcpyAsync(nw[k].p, (this->*kCols[k].buf).p, live * track_bytes(kCols[k]), cudaMemcpyDeviceToDevice, st));
     CU(cudaStreamSynchronize(st));   // the old columns are freed with nw
     swap_columns(nw);
@@ -313,10 +372,172 @@ struct sb200_fstore {
     gate = rule;
     DBuf nw[kNumCols];   // no track is stored: the columns start empty, sized to the capacity
     if (cap)
-      if (int rc = alloc(cap, nw, true)) return rc;
+      if (int rc = alloc(cap, nw, kNeedGate)) return rc;
     CU(cudaStreamSynchronize(st));
-    swap_columns(nw, true);
+    swap_columns(nw, kNeedGate);
     return 0;
+  }
+
+  // ---- retention by quality
+  int set_retention(int rule, int init, float ex) {
+    if (rule != SB200_FSTORE_KEEP_NEWEST && rule != SB200_FSTORE_KEEP_BEST_QUALITY)
+      return fail(SB200_ERR_INVALID, "unknown retention rule %d", rule);
+    if (!hid.empty()) return fail(SB200_ERR_INVALID, "the retention is fixed while the store holds tracks (%zu)", hid.size());
+    std::vector<int> tab;
+    if (rule == SB200_FSTORE_KEEP_BEST_QUALITY)
+      if (int rc = capacity_table(o.max_observations, init, ex, &tab)) return rc;
+    CU(cudaSetDevice(o.device));
+    if (!tab.empty()) {
+      if (int rc = dcap.ensure(tab.size() * 4)) return rc;
+      CU(cudaMemcpy(dcap.p, tab.data(), tab.size() * 4, cudaMemcpyHostToDevice));
+    }
+    keep = rule;
+    if (rule == SB200_FSTORE_KEEP_BEST_QUALITY) { init_cap = init; ext = ex; }
+    cap_tab.swap(tab);
+    DBuf nw[kNumCols];   // as set_gate: the quality column starts empty, sized to the capacity
+    if (cap)
+      if (int rc = alloc(cap, nw, kNeedQuality)) return rc;
+    CU(cudaStreamSynchronize(st));
+    swap_columns(nw, kNeedQuality);
+    return 0;
+  }
+
+  int refuse_quality() const {
+    if (keep) return fail(SB200_ERR_INVALID, "the store keeps its best observations by quality: use the _quality calls");
+    return 0;
+  }
+
+  // checks of a _quality call with n rows: a quality store, a quality per row and none NaN, attrs as the gate needs them
+  int check_quality(int n, const float* q, const sb200_fstore_attrs* attrs) const {
+    if (!keep) return fail(SB200_ERR_INVALID, "the store keeps its newest observations: the _quality calls need "
+                                              "sb200_fstore_set_retention(SB200_FSTORE_KEEP_BEST_QUALITY)");
+    if (!gate && attrs) return fail(SB200_ERR_INVALID, "attrs must be NULL on an ungated store");
+    if (n > 0 && !q) return fail(SB200_ERR_INVALID, "quality is NULL");
+    const int bad = n > 0 ? first_nan(n, q) : -1;
+    if (bad >= 0) return fail(SB200_ERR_INVALID, "row %d: the quality is NaN", bad);
+    return 0;
+  }
+
+  int capacity(size_t h) const { return cap_tab[std::min(h, cap_tab.size() - 1)]; }
+
+  // A track's list while a call is planned: ref[j] is its observation j, a pre-call stored row (position * K + slot,
+  // >= 0) or request row r (-(r + 1)), q[j] its quality; h its merge history; dirty once the call changes it.
+  struct QTrack {
+    int pos;
+    std::vector<int> ref;
+    std::vector<float> q;
+    std::vector<uint64_t> h;
+    bool dirty;
+  };
+
+  // optimize (examples/track_merging.rs:279-297): the stable sort by quality, descending, then the truncation to c(h)
+  void keep_best(QTrack& t) const {
+    std::vector<int> ix(t.ref.size());
+    std::iota(ix.begin(), ix.end(), 0);
+    std::stable_sort(ix.begin(), ix.end(), [&](int a, int b) { return t.q[a] > t.q[b]; });
+    ix.resize(std::min(ix.size(), (size_t)capacity(t.h.size())));
+    std::vector<int> ref;
+    std::vector<float> q;
+    for (int i : ix) { ref.push_back(t.ref[i]); q.push_back(t.q[i]); }
+    t.ref.swap(ref);
+    t.q.swap(q);
+  }
+  // Track::merge with merge_history = true (src/track.rs:522-588): dest ++ src, then optimize at dest's new capacity
+  void merge_into(QTrack& d, const QTrack& src) const {
+    d.ref.insert(d.ref.end(), src.ref.begin(), src.ref.end());
+    d.q.insert(d.q.end(), src.q.begin(), src.q.end());
+    d.h.insert(d.h.end(), src.h.begin(), src.h.end());
+    keep_best(d);
+    d.dirty = true;
+  }
+
+  // the lists of the stored tracks at pos[] as they are: their rows, qualities and histories.  Changes nothing.
+  int peek_tracks(const std::vector<int>& pos, std::vector<QTrack>* out) {
+    const size_t n = pos.size();
+    const int K = o.max_observations;
+    out->clear();
+    if (n == 0) return 0;
+    if (int rc = gpos.ensure(n * 4)) return rc;
+    if (int rc = gout.ensure(n * (2 + (size_t)K) * 4)) return rc;
+    CU(cudaMemcpyAsync(gpos.p, pos.data(), n * 4, cudaMemcpyHostToDevice, st));
+    sb::fs_launch_qpeek(view(), qual.as<float>(), gpos.as<int>(), (int)n, gout.as<int>(), gout.as<float>() + 2 * n, st);
+    std::vector<int> ring(2 * n);
+    std::vector<float> qv(n * K);
+    CU(cudaMemcpyAsync(ring.data(), gout.p, n * 8, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(qv.data(), gout.as<float>() + 2 * n, n * K * 4, cudaMemcpyDeviceToHost, st));
+    if (int rc = finish()) return rc;
+    for (size_t i = 0; i < n; ++i) {
+      QTrack t{pos[i], {}, {}, hist[pos[i]], false};
+      for (int j = 0; j < ring[2 * i]; ++j) {
+        t.ref.push_back(pos[i] * K + (ring[2 * i + 1] + j) % K);
+        t.q.push_back(qv[i * K + j]);
+      }
+      out->push_back(std::move(t));
+    }
+    return 0;
+  }
+
+  // merge_owned: writes the planned lists of the dirty tracks of t[] (every ref a stored row): observation j of a track
+  // at position p goes to slot j, by the two-launch move (every row read from its pre-call slot before any is written),
+  // then each track's K qualities (0 past its count) and its history length
+  int apply_tracks(const std::vector<QTrack>& t) {
+    const int K = o.max_observations;
+    std::vector<int> mv_src, mv_dst, hdr, qpos, hl;
+    std::vector<float> qv;
+    for (const QTrack& tr : t) {
+      if (!tr.dirty) continue;
+      const int c1 = (int)tr.ref.size();
+      hdr.insert(hdr.end(), {tr.pos, c1, 0});
+      for (int j = 0; j < c1; ++j) {
+        const int dst = tr.pos * K + j;
+        if (tr.ref[j] != dst) { mv_src.push_back(tr.ref[j]); mv_dst.push_back(dst); }
+      }
+      qpos.push_back(tr.pos);
+      hl.push_back((int)tr.h.size());
+      for (int j = 0; j < K; ++j) qv.push_back(j < c1 ? tr.q[j] : 0.0f);
+    }
+    const int nm = (int)mv_src.size(), nh = (int)hdr.size() / 3, nq = (int)qpos.size();
+    std::vector<int> tab;
+    tab.reserve(2 * (size_t)nm + hdr.size() + qpos.size() + hl.size() + qv.size());
+    for (const std::vector<int>* v : {&mv_src, &mv_dst, &hdr, &qpos, &hl}) tab.insert(tab.end(), v->begin(), v->end());
+    const size_t qoff = tab.size();
+    tab.resize(qoff + qv.size());
+    if (!qv.empty()) memcpy(tab.data() + qoff, qv.data(), qv.size() * 4);
+    if (int rc = gpos.ensure(std::max<size_t>(tab.size(), 1) * 4)) return rc;
+    if (int rc = gout.ensure(std::max<size_t>((size_t)nm * row_bytes(), 16))) return rc;
+    CU(cudaMemcpyAsync(gpos.p, tab.data(), tab.size() * 4, cudaMemcpyHostToDevice, st));
+    const int* dtab = gpos.as<int>();
+    const int* dq = dtab + 2 * nm + 3 * nh;
+    CU(cudaEventRecord(ev[2], st));
+    sb::fs_launch_move_rows(view(), dtab, dtab + nm, nm, dtab + 2 * nm, nh, gout.p, st);
+    sb::fs_launch_qual_set(qual.as<float>(), hlen.as<int>(), dq, reinterpret_cast<const float*>(dtab + qoff), dq + nq, nq,
+                           K, st);
+    CU(cudaEventRecord(ev[3], st));
+    return finish(2, 3);
+  }
+
+  // The device view of a quality store's associate (assoc) or add, with rq[R] the request rows' qualities uploaded
+  int qcall(const std::vector<float>& rq, bool assoc, sb::FsQCall* qc) {
+    if (int rc = dqr.ensure(std::max<size_t>(rq.size(), 1) * 4)) return rc;
+    if (!rq.empty()) CU(cudaMemcpyAsync(dqr.p, rq.data(), rq.size() * 4, cudaMemcpyHostToDevice, st));
+    *qc = {qual.as<float>(), hlen.as<int>(), dcap.as<int>(), (int)cap_tab.size(), dqr.as<float>(), assoc ? 1 : 0};
+    return 0;
+  }
+
+  // The best c(1) rows of each query in quality order, ties to the earlier row (a query is a fresh track, h = 1):
+  // row_src / qoff as fs_row_table makes them
+  void quality_row_table(int Q, const int32_t* offs, const float* q, std::vector<int>* row_src,
+                         std::vector<int>* qoff) const {
+    row_src->clear();
+    qoff->assign(1, 0);
+    for (int i = 0; i < Q; ++i) {
+      std::vector<int> ix(offs[i + 1] - offs[i]);
+      std::iota(ix.begin(), ix.end(), offs[i]);
+      std::stable_sort(ix.begin(), ix.end(), [&](int a, int b) { return q[a] > q[b]; });
+      ix.resize(std::min(ix.size(), (size_t)capacity(1)));
+      row_src->insert(row_src->end(), ix.begin(), ix.end());
+      qoff->push_back((int)row_src->size());
+    }
   }
 
   int begin() {
@@ -408,8 +629,9 @@ struct sb200_fstore {
   }
 
   // checks of a search / associate request; fills the newest-K row table
+  // (quality: a quality store's qualities, one per row of the column, checked here; the row table is then its own)
   int check_queries(int Q, const uint64_t* qids, const int32_t* offs, const Column& col, bool assoc,
-                    std::vector<int>* qoff, std::vector<int>* row_src) {
+                    std::vector<int>* qoff, std::vector<int>* row_src, const float* quality = nullptr) {
     if (Q < 0) return fail(SB200_ERR_INVALID, "n_queries < 0");
     if (Q == 0) return 0;
     if (!qids || !offs) return fail(SB200_ERR_INVALID, "query_ids / obs_offsets is NULL");
@@ -417,13 +639,20 @@ struct sb200_fstore {
     if (int rc = check_ids(Q, qids, "query id", assoc, offs)) return rc;
     if (!col.p) return fail(SB200_ERR_INVALID, "features is NULL");
     if (int rc = check_column(col)) return rc;
-    return plan_rows(Q, offs, qoff, row_src);
+    if (keep) {
+      if (!quality) return fail(SB200_ERR_INVALID, "quality is NULL");
+      const int bad = first_nan(offs[Q], quality);
+      if (bad >= 0) return fail(SB200_ERR_INVALID, "row %d: the quality is NaN", bad);
+    }
+    return plan_rows(Q, offs, qoff, row_src, quality);
   }
 
-  // the newest-K row table of a request, within the pair bound of one distance matrix
-  int plan_rows(int Q, const int32_t* offs, std::vector<int>* qoff, std::vector<int>* row_src) const {
+  // the newest-K row table of a request (with quality: quality_row_table), within the pair bound of one distance matrix
+  int plan_rows(int Q, const int32_t* offs, std::vector<int>* qoff, std::vector<int>* row_src,
+                const float* quality = nullptr) const {
     const int K = o.max_observations;
-    sb::fs_row_table(Q, offs, K, row_src, qoff);
+    if (quality) quality_row_table(Q, offs, quality, row_src, qoff);
+    else sb::fs_row_table(Q, offs, K, row_src, qoff);
     const long long pairs = (long long)row_src->size() * (long long)hid.size() * K;
     if (pairs > sb::kFsMaxPairs)
       return fail(SB200_ERR_CAPACITY, "the call needs %lld observation pairs; one call holds at most 2^30", pairs);
@@ -488,17 +717,18 @@ struct sb200_fstore {
 
   // search (assoc == false) or associate
   // attrs: the queries' triples of a gated store's call (checked by the caller), else nullptr
+  // quality: a quality store's qualities, one per row of the column
   int run_queries(int Q, const uint64_t* qids, const int32_t* offs, const Column& col, int32_t* counts,
                   uint64_t* winners, double* weights, uint64_t* track_ids, uint8_t* merged, bool assoc,
-                  const sb200_fstore_attrs* attrs = nullptr) {
+                  const sb200_fstore_attrs* attrs = nullptr, const float* quality = nullptr) {
     std::vector<int> qoff, src;
-    if (int rc = check_queries(Q, qids, offs, col, assoc, &qoff, &src)) return rc;
+    if (int rc = check_queries(Q, qids, offs, col, assoc, &qoff, &src, quality)) return rc;
     if (Q > 0 && (!counts || !winners || !weights || (assoc && (!track_ids || !merged))))
       return fail(SB200_ERR_INVALID, "an output is NULL");
     if (int rc = begin()) return rc;
     if (Q == 0) return 0;
     return launch_queries(Q, qids, qoff, src, col, (size_t)offs[Q], nullptr, counts, winners, weights, track_ids, merged,
-                          assoc, attrs);
+                          assoc, attrs, quality);
   }
 
   // associate whose request rows `rsrc` writes on the device (sb200_fstore_associate_wasted); offs as for associate
@@ -517,8 +747,9 @@ struct sb200_fstore {
   int launch_queries(int Q, const uint64_t* qids, const std::vector<int>& qoff, const std::vector<int>& src,
                      const Column& col, size_t col_rows, const sb::FsRowSource* rsrc, int32_t* counts,
                      uint64_t* winners, double* weights, uint64_t* track_ids, uint8_t* merged, bool assoc,
-                     const sb200_fstore_attrs* attrs = nullptr) {
+                     const sb200_fstore_attrs* attrs = nullptr, const float* quality = nullptr) {
     const int R = (int)src.size(), topn = o.topn, K = o.max_observations;
+    const bool qa = assoc && keep;   // a quality store's merges are planned and applied by fs_launch_qmerge
     const long long live = (long long)hid.size(), S = live * K;
     const ReqLayout L(Q, R, d8, !rsrc && (col.on_device || ftype != SB200_FEATURE_F32));
     const ResLayout RL(Q, topn);
@@ -528,6 +759,12 @@ struct sb200_fstore {
     if (int rc = upload(L, Q, qids, qoff, src, nullptr, col, col_rows, rsrc)) return rc;
     if (attrs)
       if (int rc = upload_triples(Q, attrs->source, attrs->t_start, attrs->t_end)) return rc;
+    sb::FsQCall qc{};
+    if (qa) {
+      std::vector<float> rq(R);
+      for (int r = 0; r < R; ++r) rq[r] = quality[src[r]];
+      if (int rc = qcall(rq, true, &qc)) return rc;
+    }
     const sb::FsGate g = gate_view(Q);
     const sb::FsStore s = view();
     const sb::FsCall c = call_view(L, Q, R, &RL);
@@ -537,12 +774,14 @@ struct sb200_fstore {
     sb::fs_launch_topn(o.max_distance, o.min_votes, topn, assoc, s, c, st);
     CU(cudaEventRecord(ev[2], st));
     if (assoc && attrs) sb::fs_launch_gate_resolve(c, g, st);
-    if (assoc) sb::fs_launch_apply(s, c, st);
+    if (qa) sb::fs_launch_qmerge(s, c, qc, st);
+    else if (assoc) sb::fs_launch_apply(s, c, st);
     if (assoc && attrs) sb::fs_launch_attr_new(s.live, c, g, st);
     CU(cudaEventRecord(ev[3], st));
     CU(cudaMemcpyAsync(hres.p, dres.p, RL.total, cudaMemcpyDeviceToHost, st));
-    std::vector<int> where;   // gated associate: the position each query ended up at (>= live: a new track)
-    if (assoc && attrs) {
+    // gated or quality associate: the position each query ended up at (>= live: a new track)
+    std::vector<int> where;
+    if (assoc && (attrs || qa)) {
       where.resize(Q);
       CU(cudaMemcpyAsync(where.data(), c.dest, (size_t)Q * 4, cudaMemcpyDeviceToHost, st));
     }
@@ -550,20 +789,25 @@ struct sb200_fstore {
     read_results(RL, Q, counts, winners, weights);
     if (assoc) {
       for (int q = 0; q < Q; ++q) {
-        merged[q] = attrs ? where[q] < live : counts[q] > 0;   // a first winner the gate refused leaves a new track
+        // a first winner the gate refused leaves a new track
+        merged[q] = attrs || qa ? where[q] < live : counts[q] > 0;
         track_ids[q] = merged[q] ? winners[(size_t)q * topn] : qids[q];
+        if (qa && merged[q]) hist[where[q]].push_back(qids[q]);   // Track::merge with merge_history = true
       }
       for (int q = 0; q < Q; ++q)
         if (!merged[q]) {
           hpos[qids[q]] = (int)hid.size();
           hid.push_back(qids[q]);
+          if (qa) hist.push_back({qids[q]});
         }
     }
     return 0;
   }
 
-  // attrs: the rows' triples of a gated store's call (checked by the caller), else nullptr
-  int add(int n, const uint64_t* idv, const Column& col, const sb200_fstore_attrs* attrs = nullptr) {
+  // attrs: the rows' triples of a gated store's call (checked by the caller), else nullptr; quality: a quality store's
+  // qualities, one per row (checked by the caller)
+  int add(int n, const uint64_t* idv, const Column& col, const sb200_fstore_attrs* attrs = nullptr,
+          const float* quality = nullptr) {
     if (n < 0) return fail(SB200_ERR_INVALID, "n < 0");
     if (n > 0 && (!idv || !col.p)) return fail(SB200_ERR_INVALID, "ids / features is NULL");
     if (int rc = check_column(col)) return rc;
@@ -596,15 +840,20 @@ struct sb200_fstore {
     if (int rc = plan.ensure((size_t)n * 16)) return rc;
     if (int rc = reserve(hid.size() + fresh.size())) return rc;
     if (int rc = upload(L, n, idv, qoff, src, dest.data(), col, (size_t)n)) return rc;
+    sb::FsQCall qc{};
+    if (keep)   // each row appended to its track in order, and the track optimized at its capacity
+      if (int rc = qcall(std::vector<float>(quality, quality + n), false, &qc)) return rc;
     const sb::FsStore s = view();
     const sb::FsCall c = call_view(L, n, n, nullptr);
     CU(cudaEventRecord(ev[2], st));
-    sb::fs_launch_apply(s, c, st);
+    if (keep) sb::fs_launch_qmerge(s, c, qc, st);
+    else sb::fs_launch_apply(s, c, st);
     CU(cudaEventRecord(ev[3], st));
     if (int rc = finish(2, 3)) return rc;
     for (uint64_t id : fresh) {
       hpos[id] = (int)hid.size();
       hid.push_back(id);
+      if (keep) hist.push_back({id});
     }
     return write_attrs(tpos, fin);
   }
@@ -664,9 +913,11 @@ struct sb200_fstore {
     return found;
   }
 
-  int64_t fetch(int n, const uint64_t* idv, int remove, int32_t* counts, float* feats) {
+  // qout: a quality store's qualities [n][K] of the rows returned (fetch_quality), else nullptr
+  int64_t fetch(int n, const uint64_t* idv, int remove, int32_t* counts, float* feats, float* qout = nullptr) {
     if (n < 0) return fail(SB200_ERR_INVALID, "n < 0");
     if (n > 0 && (!idv || !counts || !feats)) return fail(SB200_ERR_INVALID, "ids / counts / features is NULL");
+    if (qout && !keep) return fail(SB200_ERR_INVALID, "the store keeps no qualities (it keeps its newest observations)");
     if (int rc = begin()) return rc;
     if (n == 0) return 0;
     const int K = o.max_observations, D = o.feature_dim;
@@ -679,6 +930,15 @@ struct sb200_fstore {
       pos[i] = it->second;
       ++found;
       if (remove) gone[it->second] = 1;
+    }
+    if (qout) {
+      std::vector<int> fpos;
+      for (int p : pos) if (p >= 0) fpos.push_back(p);
+      std::vector<QTrack> tl;
+      if (int rc = peek_tracks(fpos, &tl)) return rc;
+      std::fill(qout, qout + (size_t)n * K, 0.0f);
+      for (int i = 0, f = 0; i < n; ++i)
+        if (pos[i] >= 0) std::copy(tl[f].q.begin(), tl[f].q.end(), qout + (size_t)i * K), ++f;
     }
     const size_t out_bytes = (size_t)n * K * d8 * 4;
     if (int rc = gpos.ensure((size_t)n * 4)) return rc;
@@ -715,14 +975,26 @@ struct sb200_fstore {
     CU(cudaMemcpyAsync(gpos.p, from.data(), from.size() * 4, cudaMemcpyHostToDevice, st));
     const sb::FsStore s = view();
     const sb::FsAttrCols sa = attr_cols();
+    const void* sq = qual.p;
+    const void* sh = hlen.p;
     swap_columns(nw);   // nw holds the old columns until the compaction below has read them
     sb::fs_launch_compact(s, view(), gpos.as<int>(), (int)from.size(), st);
     if (gate) sb::fs_launch_attr_gather(sa, gpos.as<int>(), (int)from.size(), attr_cols(), st);
+    if (keep) {
+      sb::fs_launch_words_compact(sq, qual.p, gpos.as<int>(), (int)from.size(), o.max_observations, st);
+      sb::fs_launch_words_compact(sh, hlen.p, gpos.as<int>(), (int)from.size(), 1, st);
+    }
     if (int rc = finish()) return rc;
     std::vector<uint64_t> kept;
     kept.reserve(from.size());
     for (int p : from) kept.push_back(hid[p]);
     hid.swap(kept);
+    if (keep) {
+      std::vector<std::vector<uint64_t>> kh;
+      kh.reserve(from.size());
+      for (int p : from) kh.push_back(std::move(hist[p]));
+      hist.swap(kh);
+    }
     hpos.clear();
     for (size_t p = 0; p < hid.size(); ++p) hpos[hid[p]] = (int)p;
     return 0;
@@ -866,12 +1138,25 @@ struct sb200_fstore {
     for (int i = 0; i < n; ++i)
       for (int p : {dp[i], sp[i]})
         if (idx.emplace(p, (int)touched.size()).second) touched.push_back(p);
-    std::vector<int> ring;
-    if (int rc = peek(touched, &ring)) return rc;
     std::vector<int> wpos;   // gated: the destinations whose windows change, and their final triples
     Triples win;
     if (gate)
       if (int rc = plan_merge_attrs(n, dp, sp, idx, touched, &wpos, &win)) return rc;
+    if (keep) {   // each pair's merge optimized at its destination's capacity, planned from the peeked lists
+      std::vector<QTrack> tl;
+      if (int rc = peek_tracks(touched, &tl)) return rc;
+      for (int i = 0; i < n; ++i) merge_into(tl[idx[dp[i]]], tl[idx[sp[i]]]);
+      for (QTrack& t : tl)
+        if (gone[t.pos]) t.dirty = false;
+      if (int rc = apply_tracks(tl)) return rc;
+      for (const QTrack& t : tl)
+        if (t.dirty) hist[t.pos] = t.h;
+      if (int rc = write_attrs(wpos, win)) return rc;
+      if (remove) return remove_marked(gone);
+      return 0;
+    }
+    std::vector<int> ring;
+    if (int rc = peek(touched, &ring)) return rc;
     // per touched track: its rows oldest first as stored row indices (position * K + slot) of the pre-call store, and
     // how many rows its ring has taken since the call began (old ones included): virtual row v sits in slot (s0 + v) % K
     struct Plan { std::vector<int> rows; long long taken; bool dirty; };
@@ -950,13 +1235,15 @@ struct sb200_fstore {
   }
 
   // ---- the store blob (layout: include/similari_b200.h)
-  // the columns and their `n` sections (4, or 7 for a gated store) of a blob on this device: dir 0 packs, dir 1 unpacks
+  // the columns and their `n` sections (4, 7 for a gated store, 10 for a quality store: the histories, which have no
+  // device column, are left to the caller) of a blob on this device: dir 0 packs, dir 1 unpacks
   int move_columns(int dir, const uint64_t* sec_off, const uint64_t* sec_bytes, int n, char* dblob) {
-    char* col[SB200_FSTORE_BLOB_SECTIONS_V2] = {};
+    char* col[SB200_FSTORE_BLOB_SECTIONS_V3] = {};
     for (const Col& c : kCols)
       if (c.sec >= 0) col[c.sec] = (this->*c.buf).as<char>();
     std::vector<sb::XferSeg> segs;
-    for (int i = 0; i < n; ++i) sb::add_segment(segs, dir, col[i], dblob + sec_off[i], sec_bytes[i]);
+    for (int i = 0; i < n; ++i)
+      if (col[i]) sb::add_segment(segs, dir, col[i], dblob + sec_off[i], sec_bytes[i]);
     return sb::copy_segments(segs, num_sms, st);
   }
 
@@ -970,8 +1257,21 @@ struct sb200_fstore {
   }
 
   int save(void* dst, uint64_t cap_bytes, uint64_t* bytes) {
-    uint64_t sec[SB200_FSTORE_BLOB_SECTIONS_V2];
-    const int n = sections(hid.size(), o.max_observations, d8, stype, gate, sec);
+    uint64_t sec[SB200_FSTORE_BLOB_SECTIONS_V3];
+    if (keep) {   // version 3: the quality, history length and history sections follow the attribute ones
+      std::vector<uint64_t> hc;
+      for (const std::vector<uint64_t>& h : hist) hc.insert(hc.end(), h.begin(), h.end());
+      const int n = sections(hid.size(), o.max_observations, d8, stype, gate, keep, hc.size(), sec);
+      BlobHeaderV3 h;
+      fill_header(h, SB200_FSTORE_BLOB_VERSION_QUALITY);
+      h.gate = gate;
+      h.retention = keep;
+      h.initial_capacity = init_cap;
+      h.merge_extension = ext;
+      sb::lay_out(h, sec, n);
+      return write_header_and_columns(dst, cap_bytes, bytes, h, n, &hc);
+    }
+    const int n = sections(hid.size(), o.max_observations, d8, stype, gate, keep, 0, sec);
     if (gate) {   // version 2: the attribute sections follow feat
       BlobHeaderV2 h;
       fill_header(h, SB200_FSTORE_BLOB_VERSION_GATED);
@@ -985,7 +1285,9 @@ struct sb200_fstore {
     return write_header_and_columns(dst, cap_bytes, bytes, h, n);
   }
 
-  template <class H> int write_header_and_columns(void* dst, uint64_t cap_bytes, uint64_t* bytes, const H& h, int n) {
+  // hc: a quality store's concatenated histories, written into their section
+  template <class H> int write_header_and_columns(void* dst, uint64_t cap_bytes, uint64_t* bytes, const H& h, int n,
+                                                  const std::vector<uint64_t>* hc = nullptr) {
     *bytes = h.total_bytes;
     if (!dst) return 0;
     if (cap_bytes < h.total_bytes)
@@ -995,19 +1297,26 @@ struct sb200_fstore {
       if (int rc = move_columns(0, h.sec_off, h.sec_bytes, n, p)) return rc;
       const sb::FsStore s = view();
       sb::fs_launch_blob_scrub(stype, p + h.sec_off[kSecFeat], s.cnt, s.start, (int)h.live, o.max_observations, d8, st);
+      if (hc) {
+        sb::fs_launch_qual_scrub(reinterpret_cast<float*>(p + h.sec_off[kSecQual]), s.cnt, s.start, (int)h.live,
+                                 o.max_observations, st);
+        if (!hc->empty()) CU(cudaMemcpyAsync(p + h.sec_off[kSecHist], hc->data(), hc->size() * 8, cudaMemcpyHostToDevice, st));
+      }
       return finish();
     });
   }
 
-  // fills a store fresh from sb200_fstore_create with the checked blob `h` at `src`; a version-2 blob also carries the
-  // rule `rule` and its attribute sections (sec_off / sec_bytes: the blob's section table, 4 or 7 entries)
-  int load(const BlobHeader& h, int rule, const uint64_t* sec_off, const uint64_t* sec_bytes, const void* src,
-           std::vector<uint64_t>&& blob_ids) {
+  // fills a store fresh from sb200_fstore_create with the checked blob `h` at `src`; a version-2 or -3 blob also
+  // carries the rule `rule` and its attribute sections, a version-3 blob the retention `kr` (its parameters init / ex),
+  // the quality section and the histories `hists` (sec_off / sec_bytes: the blob's section table, nsec entries)
+  int load(const BlobHeader& h, int rule, int kr, int init, float ex, const uint64_t* sec_off, const uint64_t* sec_bytes,
+           int nsec, const void* src, std::vector<uint64_t>&& blob_ids, std::vector<std::vector<uint64_t>>&& hists) {
     if (int rc = begin()) return rc;
     const int live = (int)h.live, K = o.max_observations;
     ftype = h.feature_type;
     stype = h.storage_type;
     if (int rc = set_gate(rule)) return rc;
+    if (int rc = set_retention(kr, init, ex)) return rc;
     if (live == 0) return 0;
     if (int rc = reserve((size_t)live)) return rc;
     DBuf tmp;
@@ -1015,38 +1324,48 @@ struct sb200_fstore {
     if (int rc = sb::blob_on_device(src, h.total_bytes, o.device, st, tmp, &dblob)) return rc;
     // counts and ring starts index the rows in every later kernel: checked before anything is copied into the store
     int bad[2] = {0, 0};
-    int bad_w = 0;
-    if (int rc = gpos.ensure(sizeof(bad) + sizeof(bad_w))) return rc;
-    CU(cudaMemsetAsync(gpos.p, 0, sizeof(bad) + sizeof(bad_w), st));
+    int bad_w = 0, bad_q[2] = {0, 0};
+    if (int rc = gpos.ensure(sizeof(bad) + sizeof(bad_w) + sizeof(bad_q))) return rc;
+    CU(cudaMemsetAsync(gpos.p, 0, sizeof(bad) + sizeof(bad_w) + sizeof(bad_q), st));
     sb::fs_launch_blob_check(reinterpret_cast<const int*>(dblob + sec_off[kSecCnt]),
                              reinterpret_cast<const int*>(dblob + sec_off[kSecStart]), live, K, gpos.as<int>(), st);
     if (rule)
       sb::fs_launch_attr_check(reinterpret_cast<const long long*>(dblob + sec_off[kSecT0]),
                                reinterpret_cast<const long long*>(dblob + sec_off[kSecT1]), live, gpos.as<int>() + 2, st);
     CU(cudaMemcpyAsync(bad, gpos.p, sizeof(bad), cudaMemcpyDeviceToHost, st));
+    if (kr)
+      sb::fs_launch_qual_check(reinterpret_cast<const float*>(dblob + sec_off[kSecQual]),
+                               reinterpret_cast<const int*>(dblob + sec_off[kSecCnt]),
+                               reinterpret_cast<const int*>(dblob + sec_off[kSecStart]), live, K, gpos.as<int>() + 3, st);
     CU(cudaMemcpyAsync(&bad_w, gpos.as<int>() + 2, sizeof(bad_w), cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(bad_q, gpos.as<int>() + 3, sizeof(bad_q), cudaMemcpyDeviceToHost, st));
     if (int rc = finish()) return rc;
     if (bad[0]) return fail(SB200_ERR_INVALID, "the blob holds %d cnt entries outside 1..%d", bad[0], K);
     if (bad[1]) return fail(SB200_ERR_INVALID, "the blob holds %d start entries outside 0..%d", bad[1], K - 1);
     if (bad_w) return fail(SB200_ERR_INVALID, "the blob holds %d windows with t_start > t_end", bad_w);
-    if (int rc = move_columns(1, sec_off, sec_bytes, rule ? SB200_FSTORE_BLOB_SECTIONS_V2 : SB200_FSTORE_BLOB_SECTIONS,
-                              const_cast<char*>(dblob)))
-      return rc;
+    if (bad_q[0]) return fail(SB200_ERR_INVALID, "the blob holds %d NaN qualities in filled slots", bad_q[0]);
+    if (bad_q[1])
+      return fail(SB200_ERR_INVALID, "the blob holds %d observations out of the quality order (above the one before)",
+                  bad_q[1]);
+    if (int rc = move_columns(1, sec_off, sec_bytes, nsec, const_cast<char*>(dblob))) return rc;
     hid = std::move(blob_ids);
+    hist = std::move(hists);
     for (size_t p = 0; p < hid.size(); ++p) hpos[hid[p]] = (int)p;
     return 0;
   }
 };
 
 const sb200_fstore::Col sb200_fstore::kCols[kNumCols] = {
-    {&sb200_fstore::feat, 0, false, false, kSecFeat, "feat"},
-    {&sb200_fstore::cnt, 4, false, false, kSecCnt, "cnt"},
-    {&sb200_fstore::start, 4, false, false, kSecStart, "start"},
-    {&sb200_fstore::ids, 8, false, false, kSecIds, "ids"},
-    {&sb200_fstore::run, 4, false, true, -1, nullptr},
-    {&sb200_fstore::asrc, 8, true, true, kSecSrc, "source"},
-    {&sb200_fstore::at0, 8, true, true, kSecT0, "t_start"},
-    {&sb200_fstore::at1, 8, true, true, kSecT1, "t_end"},
+    {&sb200_fstore::feat, 0, false, kNeedAll, false, kSecFeat, "feat"},
+    {&sb200_fstore::cnt, 4, false, kNeedAll, false, kSecCnt, "cnt"},
+    {&sb200_fstore::start, 4, false, kNeedAll, false, kSecStart, "start"},
+    {&sb200_fstore::ids, 8, false, kNeedAll, false, kSecIds, "ids"},
+    {&sb200_fstore::run, 4, false, kNeedAll, true, -1, nullptr},
+    {&sb200_fstore::asrc, 8, false, kNeedGate, true, kSecSrc, "source"},
+    {&sb200_fstore::at0, 8, false, kNeedGate, true, kSecT0, "t_start"},
+    {&sb200_fstore::at1, 8, false, kNeedGate, true, kSecT1, "t_end"},
+    {&sb200_fstore::qual, 4, true, kNeedQuality, true, kSecQual, "quality"},
+    {&sb200_fstore::hlen, 4, false, kNeedQuality, true, kSecHlen, "history_length"},
 };
 
 // a call without a handle: SB200_ERR_CUDA when there is no device to have made one, else SB200_ERR_INVALID
@@ -1089,6 +1408,7 @@ void sb200_fstore_destroy(sb200_fstore* s) {
 int sb200_fstore_add(sb200_fstore* s, int32_t n, const uint64_t* ids, const float* features) {
   if (!s) return no_handle();
   if (int rc = s->refuse_gated()) return rc;
+  if (int rc = s->refuse_quality()) return rc;
   return s->add(n, ids, {features, false, nullptr});
 }
 
@@ -1096,6 +1416,7 @@ int sb200_fstore_search(sb200_fstore* s, int32_t n_queries, const uint64_t* quer
                         const float* features, int32_t* counts, uint64_t* winners, double* weights) {
   if (!s) return no_handle();
   if (int rc = s->refuse_gated()) return rc;
+  if (int rc = s->refuse_quality()) return rc;
   return s->run_queries(n_queries, query_ids, obs_offsets, {features, false, nullptr}, counts, winners, weights, nullptr,
                         nullptr, false);
 }
@@ -1105,6 +1426,7 @@ int sb200_fstore_associate(sb200_fstore* s, int32_t n_queries, const uint64_t* q
                            uint64_t* track_ids, uint8_t* merged) {
   if (!s) return no_handle();
   if (int rc = s->refuse_gated()) return rc;
+  if (int rc = s->refuse_quality()) return rc;
   return s->run_queries(n_queries, query_ids, obs_offsets, {features, false, nullptr}, counts, winners, weights, track_ids,
                         merged, true);
 }
@@ -1171,6 +1493,7 @@ int sb200_fstore_get_options(sb200_fstore* s, sb200_fstore_options* out, int32_t
 int sb200_fstore_add_device(sb200_fstore* s, int32_t n, const uint64_t* ids, const void* d_features, void* cuda_stream) {
   if (!s) return no_handle();
   if (int rc = s->refuse_gated()) return rc;
+  if (int rc = s->refuse_quality()) return rc;
   return s->add(n, ids, {d_features, true, static_cast<cudaStream_t>(cuda_stream)});
 }
 
@@ -1179,6 +1502,7 @@ int sb200_fstore_search_device(sb200_fstore* s, int32_t n_queries, const uint64_
                                double* weights, void* cuda_stream) {
   if (!s) return no_handle();
   if (int rc = s->refuse_gated()) return rc;
+  if (int rc = s->refuse_quality()) return rc;
   return s->run_queries(n_queries, query_ids, obs_offsets, {d_features, true, static_cast<cudaStream_t>(cuda_stream)},
                         counts, winners, weights, nullptr, nullptr, false);
 }
@@ -1189,6 +1513,7 @@ int sb200_fstore_associate_device(sb200_fstore* s, int32_t n_queries, const uint
                                   void* cuda_stream) {
   if (!s) return no_handle();
   if (int rc = s->refuse_gated()) return rc;
+  if (int rc = s->refuse_quality()) return rc;
   return s->run_queries(n_queries, query_ids, obs_offsets, {d_features, true, static_cast<cudaStream_t>(cuda_stream)},
                         counts, winners, weights, track_ids, merged, true);
 }
@@ -1216,6 +1541,7 @@ static int attr_column(int n, const float* features, const void* d_features, voi
 int sb200_fstore_add_attr(sb200_fstore* s, int32_t n, const uint64_t* ids, const sb200_fstore_attrs* attrs,
                           const float* features, const void* d_features, void* cuda_stream) {
   if (!s) return no_handle();
+  if (int rc = s->refuse_quality()) return rc;
   if (int rc = s->check_attrs(n, attrs)) return rc;
   Column col;
   if (int rc = attr_column(n, features, d_features, cuda_stream, &col)) return rc;
@@ -1226,6 +1552,7 @@ int sb200_fstore_search_attr(sb200_fstore* s, int32_t n_queries, const uint64_t*
                              const sb200_fstore_attrs* attrs, const float* features, const void* d_features,
                              int32_t* counts, uint64_t* winners, double* weights, void* cuda_stream) {
   if (!s) return no_handle();
+  if (int rc = s->refuse_quality()) return rc;
   if (int rc = s->check_attrs(n_queries, attrs)) return rc;
   Column col;
   if (int rc = attr_column(n_queries, features, d_features, cuda_stream, &col)) return rc;
@@ -1237,6 +1564,7 @@ int sb200_fstore_associate_attr(sb200_fstore* s, int32_t n_queries, const uint64
                                 const void* d_features, int32_t* counts, uint64_t* winners, double* weights,
                                 uint64_t* track_ids, uint8_t* merged, void* cuda_stream) {
   if (!s) return no_handle();
+  if (int rc = s->refuse_quality()) return rc;
   if (int rc = s->check_attrs(n_queries, attrs)) return rc;
   Column col;
   if (int rc = attr_column(n_queries, features, d_features, cuda_stream, &col)) return rc;
@@ -1247,6 +1575,89 @@ int64_t sb200_fstore_fetch_attr(sb200_fstore* s, int32_t n, const uint64_t* ids,
                                 int64_t* t_end) {
   if (!s) return no_handle();
   return s->fetch_attr(n, ids, source, t_start, t_end);
+}
+
+int sb200_fstore_set_retention(sb200_fstore* s, int32_t rule, int32_t initial_capacity, float merge_extension) {
+  if (!s) return no_handle();
+  return s->set_retention(rule, initial_capacity, merge_extension);
+}
+
+int sb200_fstore_get_retention(sb200_fstore* s, int32_t* rule, int32_t* initial_capacity, float* merge_extension) {
+  if (!s) return no_handle();
+  if (rule) *rule = s->keep;
+  if (initial_capacity) *initial_capacity = s->init_cap;
+  if (merge_extension) *merge_extension = s->ext;
+  return 0;
+}
+
+int sb200_fstore_add_quality(sb200_fstore* s, int32_t n, const uint64_t* ids, const float* quality,
+                             const sb200_fstore_attrs* attrs, const float* features, const void* d_features,
+                             void* cuda_stream) {
+  if (!s) return no_handle();
+  if (n < 0) return fail(SB200_ERR_INVALID, "n < 0");
+  if (int rc = s->check_quality(n, quality, attrs)) return rc;
+  if (s->gate)
+    if (int rc = s->check_attrs(n, attrs)) return rc;
+  Column col;
+  if (int rc = attr_column(n, features, d_features, cuda_stream, &col)) return rc;
+  return s->add(n, ids, col, s->gate ? attrs : nullptr, quality);
+}
+
+int sb200_fstore_search_quality(sb200_fstore* s, int32_t n_queries, const uint64_t* query_ids,
+                                const int32_t* obs_offsets, const float* quality, const sb200_fstore_attrs* attrs,
+                                const float* features, const void* d_features, int32_t* counts, uint64_t* winners,
+                                double* weights, void* cuda_stream) {
+  if (!s) return no_handle();
+  if (int rc = s->check_quality(0, quality, attrs)) return rc;   // the rows' qualities: once the offsets are checked
+  if (s->gate)
+    if (int rc = s->check_attrs(n_queries, attrs)) return rc;
+  Column col;
+  if (int rc = attr_column(n_queries, features, d_features, cuda_stream, &col)) return rc;
+  return s->run_queries(n_queries, query_ids, obs_offsets, col, counts, winners, weights, nullptr, nullptr, false,
+                        s->gate ? attrs : nullptr, quality);
+}
+
+int sb200_fstore_associate_quality(sb200_fstore* s, int32_t n_queries, const uint64_t* query_ids,
+                                   const int32_t* obs_offsets, const float* quality, const sb200_fstore_attrs* attrs,
+                                   const float* features, const void* d_features, int32_t* counts, uint64_t* winners,
+                                   double* weights, uint64_t* track_ids, uint8_t* merged, void* cuda_stream) {
+  if (!s) return no_handle();
+  if (int rc = s->check_quality(0, quality, attrs)) return rc;
+  if (s->gate)
+    if (int rc = s->check_attrs(n_queries, attrs)) return rc;
+  Column col;
+  if (int rc = attr_column(n_queries, features, d_features, cuda_stream, &col)) return rc;
+  return s->run_queries(n_queries, query_ids, obs_offsets, col, counts, winners, weights, track_ids, merged, true,
+                        s->gate ? attrs : nullptr, quality);
+}
+
+int64_t sb200_fstore_fetch_quality(sb200_fstore* s, int32_t n, const uint64_t* ids, int32_t remove, int32_t* counts,
+                                   float* features, float* quality) {
+  if (!s) return no_handle();
+  if (n > 0 && !quality) return fail(SB200_ERR_INVALID, "quality is NULL");
+  if (!s->keep) return fail(SB200_ERR_INVALID, "the store keeps no qualities (it keeps its newest observations)");
+  return s->fetch(n, ids, remove, counts, features, quality);
+}
+
+int64_t sb200_fstore_merge_history(sb200_fstore* s, int32_t n, const uint64_t* ids, int32_t* lengths, int64_t cap,
+                                   uint64_t* out) {
+  if (!s) return no_handle();
+  if (!s->keep) return fail(SB200_ERR_INVALID, "the store keeps no merge histories (it keeps its newest observations)");
+  if (n < 0 || cap < 0) return fail(SB200_ERR_INVALID, "n < 0 or cap < 0");
+  if ((n > 0 && (!ids || !lengths)) || (cap > 0 && !out)) return fail(SB200_ERR_INVALID, "ids / lengths / out is NULL");
+  int64_t total = 0;
+  for (int i = 0; i < n; ++i) {
+    auto it = s->hpos.find(ids[i]);
+    lengths[i] = 0;
+    if (it == s->hpos.end()) continue;
+    const std::vector<uint64_t>& h = s->hist[it->second];
+    for (uint64_t v : h) {
+      if (total < cap) out[total] = v;
+      ++total;
+    }
+    lengths[i] = (int32_t)h.size();
+  }
+  return total;
 }
 
 int sb200_fstore_search_owned(sb200_fstore* s, int32_t n, const uint64_t* ids, int32_t each, int32_t* counts,
@@ -1277,9 +1688,10 @@ int sb200_fstore_load(const void* buf, uint64_t bytes, int32_t device, sb200_fst
   BlobHeader h;
   CU(cudaMemcpy(&h, buf, sizeof(h), cudaMemcpyDefault));
   if (h.magic != SB200_FSTORE_BLOB_MAGIC) return fail(SB200_ERR_INVALID, "not a feature store blob (bad magic)");
-  if (h.version != SB200_FSTORE_BLOB_VERSION && h.version != SB200_FSTORE_BLOB_VERSION_GATED)
-    return fail(SB200_ERR_INVALID, "feature store blob version %u (this library reads %u and %u)", h.version,
-                SB200_FSTORE_BLOB_VERSION, SB200_FSTORE_BLOB_VERSION_GATED);
+  if (h.version != SB200_FSTORE_BLOB_VERSION && h.version != SB200_FSTORE_BLOB_VERSION_GATED &&
+      h.version != SB200_FSTORE_BLOB_VERSION_QUALITY)
+    return fail(SB200_ERR_INVALID, "feature store blob version %u (this library reads %u, %u and %u)", h.version,
+                SB200_FSTORE_BLOB_VERSION, SB200_FSTORE_BLOB_VERSION_GATED, SB200_FSTORE_BLOB_VERSION_QUALITY);
   // version 2 (a gated store): the same fields, the rule and a 7-section table
   const bool v2 = h.version == SB200_FSTORE_BLOB_VERSION_GATED;
   BlobHeaderV2 h2;
@@ -1290,8 +1702,23 @@ int sb200_fstore_load(const void* buf, uint64_t bytes, int32_t device, sb200_fst
     if (h2.gate != SB200_FSTORE_GATE_SAME_SOURCE && h2.gate != SB200_FSTORE_GATE_ANY_SOURCE)
       return fail(SB200_ERR_INVALID, "a version-2 blob with unknown gate rule %d", h2.gate);
   }
-  const uint64_t* sec_off = v2 ? h2.sec_off : h.sec_off;
-  const uint64_t* sec_bytes = v2 ? h2.sec_bytes : h.sec_bytes;
+  // version 3 (a quality store): version 2's fields, the retention and its parameters, and a 10-section table
+  const bool v3 = h.version == SB200_FSTORE_BLOB_VERSION_QUALITY;
+  BlobHeaderV3 h3;
+  memset(&h3, 0, sizeof(h3));
+  if (v3) {
+    if (bytes < sizeof(h3)) return fail(SB200_ERR_INVALID, "the blob is truncated (%llu bytes)", (unsigned long long)bytes);
+    CU(cudaMemcpy(&h3, buf, sizeof(h3), cudaMemcpyDefault));
+    if (h3.gate != SB200_FSTORE_GATE_NONE && h3.gate != SB200_FSTORE_GATE_SAME_SOURCE &&
+        h3.gate != SB200_FSTORE_GATE_ANY_SOURCE)
+      return fail(SB200_ERR_INVALID, "a version-3 blob with unknown gate rule %d", h3.gate);
+    if (h3.retention != SB200_FSTORE_KEEP_BEST_QUALITY)
+      return fail(SB200_ERR_INVALID, "a version-3 blob with unknown retention rule %d", h3.retention);
+  }
+  const uint64_t* sec_off = v3 ? h3.sec_off : v2 ? h2.sec_off : h.sec_off;
+  const uint64_t* sec_bytes = v3 ? h3.sec_bytes : v2 ? h2.sec_bytes : h.sec_bytes;
+  const int gate = v3 ? h3.gate : v2 ? h2.gate : SB200_FSTORE_GATE_NONE;
+  const int keep = v3 ? h3.retention : SB200_FSTORE_KEEP_NEWEST;
   if (h.total_bytes > bytes)
     return fail(SB200_ERR_INVALID, "the blob is truncated (%llu of total_bytes %llu)", (unsigned long long)bytes,
                 (unsigned long long)h.total_bytes);
@@ -1304,13 +1731,19 @@ int sb200_fstore_load(const void* buf, uint64_t bytes, int32_t device, sb200_fst
   if (!known_type(h.storage_type)) return fail(SB200_ERR_INVALID, "unknown storage_type %d", h.storage_type);
   // live * K indexes the distance matrix's columns as an int
   if (h.live < 0 || h.live > INT32_MAX / h.max_observations) return fail(SB200_ERR_INVALID, "live count out of range");
+  std::vector<int> tab;   // version 3: c(h)
+  if (v3)
+    if (int rc = capacity_table(h.max_observations, h3.initial_capacity, h3.merge_extension, &tab)) return rc;
   const uint64_t live = (uint64_t)h.live;
-  uint64_t want[SB200_FSTORE_BLOB_SECTIONS_V2];
-  const char* name[SB200_FSTORE_BLOB_SECTIONS_V2];
-  const int nsec = sb200_fstore::sections(live, h.max_observations, h.d8, h.storage_type, v2 ? h2.gate : 0, want, name);
-  if (int rc = v2 ? sb::check_section_table(h2, nsec, name) : sb::check_section_table(h, nsec, name)) return rc;
+  uint64_t want[SB200_FSTORE_BLOB_SECTIONS_V3];
+  const char* name[SB200_FSTORE_BLOB_SECTIONS_V3];
+  const int nsec = sb200_fstore::sections(live, h.max_observations, h.d8, h.storage_type, gate, keep, 0, want, name);
+  if (int rc = v3   ? sb::check_section_table(h3, nsec, name)
+               : v2 ? sb::check_section_table(h2, nsec, name)
+                    : sb::check_section_table(h, nsec, name))
+    return rc;
   for (int i = 0; i < nsec; ++i)
-    if (sec_bytes[i] != want[i])
+    if (i != kSecHist && sec_bytes[i] != want[i])   // the history's size is checked against its lengths below
       return fail(SB200_ERR_INVALID, "section %s holds %llu bytes, %llu expected", name[i],
                   (unsigned long long)sec_bytes[i], (unsigned long long)want[i]);
   std::vector<uint64_t> blob_ids(live);
@@ -1319,9 +1752,48 @@ int sb200_fstore_load(const void* buf, uint64_t bytes, int32_t device, sb200_fst
   seen.reserve(live * 2);
   for (uint64_t id : blob_ids)
     if (!seen.insert(id).second) return fail(SB200_ERR_INVALID, "id %llu appears twice in the blob", (unsigned long long)id);
+  std::vector<std::vector<uint64_t>> hists;   // version 3: every history non-empty and led by its track's id
+  if (v3) {
+    std::vector<int32_t> hl(live);
+    if (live) CU(cudaMemcpy(hl.data(), static_cast<const char*>(buf) + sec_off[kSecHlen], live * 4, cudaMemcpyDefault));
+    uint64_t total = 0;
+    for (uint64_t t = 0; t < live; ++t) {
+      if (hl[t] < 1)
+        return fail(SB200_ERR_INVALID, "track %llu has a merge history of length %d", (unsigned long long)blob_ids[t], hl[t]);
+      total += (uint64_t)hl[t];
+    }
+    if (sec_bytes[kSecHist] != total * 8)
+      return fail(SB200_ERR_INVALID, "section history holds %llu bytes, %llu expected (the sum of the history lengths)",
+                  (unsigned long long)sec_bytes[kSecHist], (unsigned long long)(total * 8));
+    // a state the rule produces: every list from ring slot 0, and no longer than its capacity
+    std::vector<int32_t> cn(live), sn(live);
+    if (live) {
+      CU(cudaMemcpy(cn.data(), static_cast<const char*>(buf) + sec_off[kSecCnt], live * 4, cudaMemcpyDefault));
+      CU(cudaMemcpy(sn.data(), static_cast<const char*>(buf) + sec_off[kSecStart], live * 4, cudaMemcpyDefault));
+    }
+    for (uint64_t t = 0; t < live; ++t) {
+      if (sn[t] != 0)
+        return fail(SB200_ERR_INVALID, "track %llu has ring start %d; a quality store's lists start at slot 0",
+                    (unsigned long long)blob_ids[t], sn[t]);
+      const int c = tab[std::min<size_t>((size_t)hl[t], tab.size() - 1)];
+      if (cn[t] > c)
+        return fail(SB200_ERR_INVALID, "track %llu holds %d observations, above its capacity %d at history length %d",
+                    (unsigned long long)blob_ids[t], cn[t], c, hl[t]);
+    }
+    std::vector<uint64_t> hc(total);
+    if (total) CU(cudaMemcpy(hc.data(), static_cast<const char*>(buf) + sec_off[kSecHist], total * 8, cudaMemcpyDefault));
+    hists.resize(live);
+    for (uint64_t t = 0, at = 0; t < live; at += (uint64_t)hl[t], ++t) {
+      hists[t].assign(hc.begin() + at, hc.begin() + at + hl[t]);
+      if (hists[t][0] != blob_ids[t])
+        return fail(SB200_ERR_INVALID, "the merge history of track %llu starts with %llu, not with its id",
+                    (unsigned long long)blob_ids[t], (unsigned long long)hists[t][0]);
+    }
+  }
   sb200_fstore* s = nullptr;
   if (int rc = sb200_fstore_create(&o, &s)) return rc;
-  if (int rc = s->load(h, v2 ? h2.gate : SB200_FSTORE_GATE_NONE, sec_off, sec_bytes, buf, std::move(blob_ids))) {
+  if (int rc = s->load(h, gate, keep, h3.initial_capacity, h3.merge_extension, sec_off, sec_bytes, nsec, buf,
+                       std::move(blob_ids), std::move(hists))) {
     sb200_fstore_destroy(s);   // the handle owns every buffer made so far
     return rc;
   }
@@ -1342,6 +1814,8 @@ void fstore_info(sb200_fstore* s, int* device, int* feature_dim, int* topn) {
 }
 
 int fstore_gate(sb200_fstore* s) { return s->gate; }
+
+int fstore_retention(sb200_fstore* s) { return s->keep; }
 
 int fstore_associate_rows(sb200_fstore* s, int Q, const uint64_t* qids, const int32_t* offs, const FsRowSource& src,
                           int32_t* counts, uint64_t* winners, double* weights, uint64_t* track_ids, uint8_t* merged) {

@@ -655,6 +655,193 @@ __global__ void fs_blob_scrub_kernel(Elem* feat, const int* __restrict__ cnt, co
   }
 }
 
+// ------------------------------------------------------------------------------------------------ quality store
+// A quality store (sb200_fstore_set_retention) keeps each track's observations in the track's order (best first) in ring
+// slots 0, 1, ... (its ring start is always 0), so every kernel above walks it in that order unchanged.  qual[cap][K]
+// holds the quality of the row in each slot (0 in a slot that holds none) and hlen[cap] each track's history length.
+// Associate and add plan and apply on the device (fs_qorder_kernel, then fs_qmerge_kernel); merge_owned plans on the
+// host: stored rows move with the two row move kernels above, request rows are written by fs_put_rows_kernel, and
+// fs_qual_set_kernel rewrites the qualities and history lengths of every touched track.
+
+// Associate / add on a quality store, after TopN (and the gate): one CTA, items in chunks of kOrderThreads.  Item q with
+// dest[q] == -1 becomes a new track after the stored ones and the earlier new ones (fs_order_kernel's rule); dest[q] is
+// set to its position p, and run[p] (zero between calls) to the largest Q - q, marking p's first item as its leader.
+__global__ void __launch_bounds__(kOrderThreads) fs_qorder_kernel(FsStore s, FsCall c) {
+  __shared__ int s_warp[kOrderThreads / 32];
+  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+  int new_base = 0;
+  for (int base = 0; base < c.Q; base += kOrderThreads) {
+    const int q = base + tid;
+    const bool in = q < c.Q;
+    const int d = in ? c.dest[q] : 0;
+    const bool isnew = in && d < 0;
+    const unsigned int bal = __ballot_sync(0xffffffffu, isnew);
+    if (lane == 0) s_warp[wid] = __popc(bal);
+    __syncthreads();
+    int woff = 0, chunk_new = 0;
+    for (int w = 0; w < kOrderThreads / 32; ++w) {
+      woff += w < wid ? s_warp[w] : 0;
+      chunk_new += s_warp[w];
+    }
+    const int p = isnew ? s.live + new_base + woff + __popc(bal & ((1u << lane) - 1u)) : d;
+    if (in) {
+      c.dest[q] = p;
+      atomicMax(s.run + p, c.Q - q);
+    }
+    __syncthreads();   // s_warp is rewritten by the next chunk
+    new_base += chunk_new;
+  }
+}
+
+// One CTA per item; the leader of each destination p (run[p] == Q - q) plans and applies p's whole call.  Thread 0 walks
+// p's items in order (found 128 at a time by the block): associate adds each query's history (length 1) and merges its
+// rows; add appends its row (a new track starts with history length 1).  Each step is the stable merge of two lists
+// sorted by quality, descending (the stored list, and a query's rows from the row table, are sorted; equal qualities
+// keep the stored rows first), truncated to c(h) at the new h (cap_tab), so a row an earlier step dropped never comes
+// back.  The surviving stored rows are a prefix of the old list and only move later, so they are moved in place, last
+// first; request rows are then rounded into their slots as fs_apply_kernel rounds them.  Every thread handles the same
+// 16-byte vectors of every row, so no row is read after another thread has overwritten it.
+template <typename Elem>
+__global__ void __launch_bounds__(128) fs_qmerge_kernel(FsStore s, FsCall c, FsQCall qc) {
+  __shared__ int s_src[kFsMaxObs], t_src[kFsMaxObs];   // >= 0: old slot; < 0: request row -(r + 1)
+  __shared__ float s_q[kFsMaxObs], t_q[kFsMaxObs];
+  __shared__ unsigned int s_hit[4];
+  __shared__ int s_n, s_h;
+  const int q = blockIdx.x, tid = threadIdx.x, K = s.K;
+  const int p = c.dest[q];
+  if (s.run[p] != c.Q - q) return;   // not p's first item (uniform across the CTA)
+  const bool old = p < s.live;
+  const int n0 = old ? s.cnt[p] : 0;
+  for (int j = tid; j < n0; j += blockDim.x) {
+    s_src[j] = j;
+    s_q[j] = qc.qual[(size_t)p * K + j];
+  }
+  if (tid == 0) {
+    s_n = n0;
+    s_h = old ? qc.hlen[p] : 0;
+  }
+  __syncthreads();
+  for (int base = q; base < c.Q; base += blockDim.x) {
+    const bool hit = base + tid < c.Q && c.dest[base + tid] == p;
+    const unsigned int b = __ballot_sync(0xffffffffu, hit);
+    if ((tid & 31) == 0) s_hit[tid >> 5] = b;
+    __syncthreads();
+    if (tid == 0) {
+      int n = s_n, h = s_h;
+      for (int w = 0; w < 4; ++w)
+        for (unsigned int m = s_hit[w]; m; m &= m - 1) {
+          const int qi = base + 32 * w + __ffs(m) - 1;
+          if (qc.assoc) ++h;
+          else if (h == 0) h = 1;
+          const int cap = qc.cap_tab[min(h, qc.ntab - 1)];
+          const int r0 = c.qoff[qi], r1 = c.qoff[qi + 1];
+          int a = 0, r = r0, k = 0;
+          while (k < cap && (a < n || r < r1)) {
+            if (r == r1 || (a < n && !(qc.rq[r] > s_q[a]))) { t_src[k] = s_src[a]; t_q[k] = s_q[a]; ++a; }
+            else { t_src[k] = -(r + 1); t_q[k] = qc.rq[r]; ++r; }
+            ++k;
+          }
+          for (int j = 0; j < k; ++j) { s_src[j] = t_src[j]; s_q[j] = t_q[j]; }
+          n = k;
+        }
+      s_n = n;
+      s_h = h;
+    }
+    __syncthreads();
+  }
+  const int n = s_n, w16 = s.d8 / kPer16<Elem>;
+  Elem* feat = static_cast<Elem*>(s.feat);
+  for (int i = n - 1; i >= 0; --i) {   // stored rows, in place: slot s_src[i] <= i
+    const int j = s_src[i];
+    if (j < 0 || j == i) continue;
+    const float4* a = reinterpret_cast<const float4*>(feat + ((size_t)p * K + j) * s.d8);
+    float4* d = reinterpret_cast<float4*>(feat + ((size_t)p * K + i) * s.d8);
+    for (int e = tid; e < w16; e += blockDim.x) d[e] = a[e];
+  }
+  for (int i = 0; i < n; ++i) {   // request rows
+    if (s_src[i] >= 0) continue;
+    const float4* src = reinterpret_cast<const float4*>(c.rows + (size_t)(-s_src[i] - 1) * s.d8);
+    if constexpr (sizeof(Elem) == 4) {
+      float4* d = reinterpret_cast<float4*>(feat + ((size_t)p * K + i) * s.d8);
+      for (int e = tid; e < w16; e += blockDim.x) d[e] = src[e];
+    } else {
+      uint4* d = reinterpret_cast<uint4*>(feat + ((size_t)p * K + i) * s.d8);
+      for (int e = tid; e < w16; e += blockDim.x) d[e] = fs_round8<Elem>(src[2 * e], src[2 * e + 1]);
+    }
+  }
+  for (int i = tid; i < n; i += blockDim.x) qc.qual[(size_t)p * K + i] = s_q[i];
+  if (tid == 0) {
+    s.cnt[p] = n;
+    s.start[p] = 0;
+    qc.hlen[p] = s_h;
+    if (!old) s.ids[p] = c.qid[q];
+    s.run[p] = 0;
+  }
+}
+
+// out[2 i] = cnt, out[2 i + 1] = start of the track at pos[i]; oq[i][j] = the quality of its observation j (0 past cnt)
+__global__ void fs_qpeek_kernel(FsStore s, const float* __restrict__ qual, const int* __restrict__ pos, int n,
+                                int* __restrict__ out, float* __restrict__ oq) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int p = pos[i], c = s.cnt[p], st = s.start[p], K = s.K;
+  out[2 * i] = c;
+  out[2 * i + 1] = st;
+  for (int j = 0; j < K; ++j) oq[(size_t)i * K + j] = j < c ? qual[(size_t)p * K + (st + j) % K] : 0.0f;
+}
+
+// qual[pos[i]][j] = vals[i][j], j < K; hlen[pos[i]] = hl[i]
+__global__ void fs_qual_set_kernel(float* __restrict__ qual, int* __restrict__ hlen, const int* __restrict__ pos,
+                                   const float* __restrict__ vals, const int* __restrict__ hl, int n, int K) {
+  const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= (long long)n * K) return;
+  const int i = (int)(e / K), j = (int)(e - (long long)i * K);
+  qual[(size_t)pos[i] * K + j] = vals[e];
+  if (j == 0) hlen[pos[i]] = hl[i];
+}
+
+// dst[i][.] = src[from[i]][.], w 32-bit words per track: the qualities and history lengths of fs_compact_kernel's kept
+// tracks
+__global__ void fs_words_compact_kernel(const unsigned int* __restrict__ src, unsigned int* __restrict__ dst,
+                                        const int* __restrict__ from, int n, int w) {
+  const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= (long long)n * w) return;
+  const int i = (int)(e / w), j = (int)(e - (long long)i * w);
+  dst[e] = src[(size_t)from[i] * w + j];
+}
+
+// ring slot j of a track with ring start st holds observation (j - st) mod K; filled when that is < c.  Safe for any
+// st and c (a blob's, not yet checked).
+__device__ __forceinline__ bool fs_slot_filled(int j, int st, int c, int K) {
+  return (((j - st) % K) + K) % K < c;
+}
+
+// store blob: bad[0] counts the NaN qualities in filled slots, bad[1] the observations whose quality is above the one
+// before (a list out of the quality order)
+__global__ void fs_qual_check_kernel(const float* __restrict__ qual, const int* __restrict__ cnt,
+                                     const int* __restrict__ start, int n, int K, int* bad) {
+  int b = 0, o = 0;
+  for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < (long long)n * K;
+       e += (long long)gridDim.x * blockDim.x) {
+    const int t = (int)(e / K), j = (int)(e - (long long)t * K);
+    const int st = start[t], i = (((j - st) % K) + K) % K;   // observation index of slot j
+    if (i >= cnt[t]) continue;
+    b += isnan(qual[e]);
+    if (i > 0) o += qual[e] > qual[(size_t)t * K + (((st + i - 1) % K) + K) % K];
+  }
+  if (b) atomicAdd(bad, b);
+  if (o) atomicAdd(bad + 1, o);
+}
+
+// store blob, after its sections are copied: zeroes the qualities of the slots that hold no observation
+__global__ void fs_qual_scrub_kernel(float* __restrict__ qual, const int* __restrict__ cnt, const int* __restrict__ start,
+                                     int n, int K) {
+  const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= (long long)n * K) return;
+  const int t = (int)(e / K), j = (int)(e - (long long)t * K);
+  if (!fs_slot_filled(j, start[t], cnt[t], K)) qual[e] = 0.0f;
+}
+
 }  // namespace
 
 template <typename Elem, int MODE, typename... Gate>
@@ -807,6 +994,50 @@ void fs_launch_blob_scrub(int stype, void* feat, const int* cnt, const int* star
     fs_blob_scrub_kernel<Elem><<<(unsigned)(((long long)n * 32 + 255) / 256), 256, 0, st>>>(static_cast<Elem*>(feat), cnt,
                                                                                            start, n, K, d8);
   });
+  note_launch();
+}
+
+namespace {
+unsigned fs_blocks(long long threads) { return (unsigned)((threads + 255) / 256); }
+}  // namespace
+
+void fs_launch_qpeek(const FsStore& s, const float* qual, const int* pos, int n, int* out, float* oq, cudaStream_t st) {
+  if (n == 0) return;
+  fs_qpeek_kernel<<<fs_blocks(n), 256, 0, st>>>(s, qual, pos, n, out, oq);
+  note_launch();
+}
+
+void fs_launch_qual_set(float* qual, int* hlen, const int* pos, const float* vals, const int* hl, int n, int K,
+                        cudaStream_t st) {
+  if (n == 0) return;
+  fs_qual_set_kernel<<<fs_blocks((long long)n * K), 256, 0, st>>>(qual, hlen, pos, vals, hl, n, K);
+  note_launch();
+}
+
+void fs_launch_words_compact(const void* src, void* dst, const int* from, int n, int w, cudaStream_t st) {
+  if (n == 0) return;
+  fs_words_compact_kernel<<<fs_blocks((long long)n * w), 256, 0, st>>>(static_cast<const unsigned int*>(src),
+                                                                       static_cast<unsigned int*>(dst), from, n, w);
+  note_launch();
+}
+
+void fs_launch_qmerge(const FsStore& s, const FsCall& c, const FsQCall& qc, cudaStream_t st) {
+  if (c.Q == 0) return;
+  fs_qorder_kernel<<<1, kOrderThreads, 0, st>>>(s, c);
+  feat_dispatch(s.stype, [&](auto tag) { fs_qmerge_kernel<decltype(tag)><<<c.Q, 128, 0, st>>>(s, c, qc); });
+  note_launch(2);
+}
+
+void fs_launch_qual_check(const float* qual, const int* cnt, const int* start, int n, int K, int* bad, cudaStream_t st) {
+  if (n == 0) return;
+  fs_qual_check_kernel<<<(unsigned)std::min<long long>(fs_blocks((long long)n * K), 1024), 256, 0, st>>>(qual, cnt, start,
+                                                                                                          n, K, bad);
+  note_launch();
+}
+
+void fs_launch_qual_scrub(float* qual, const int* cnt, const int* start, int n, int K, cudaStream_t st) {
+  if (n == 0) return;
+  fs_qual_scrub_kernel<<<fs_blocks((long long)n * K), 256, 0, st>>>(qual, cnt, start, n, K);
   note_launch();
 }
 

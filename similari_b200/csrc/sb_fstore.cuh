@@ -1,7 +1,9 @@
 // sb_fstore.cuh -- device side of the feature track store (csrc/kernels_fstore.cu), shared with its host side
 // (csrc/fstore.cu).  The store is the reference's TrackStore specialised to feature-only tracks: one feature class, the
 // newest `max_observations` (K) observations of each track (src/track/store.rs, benches/feature_tracker.rs), and, in a
-// gated store only, the CamTrackingAttributes of examples/track_merging.rs as track attributes (FsAttrCols, FsGate).
+// gated store only, the CamTrackingAttributes of examples/track_merging.rs as track attributes (FsAttrCols, FsGate).  A
+// quality store keeps each track's best observations instead, in its order from the ring start, with a quality per
+// slot (examples/track_merging.rs:279-297, sb200_fstore_set_retention; the fs_launch_q* calls below).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -142,5 +144,36 @@ void fs_launch_blob_check(const int* cnt, const int* start, int n, int K, int* b
 // store blob, after its rows are copied: zeroes, in feat[n][K][d8] (elements of stype), the ring slots that hold no
 // observation
 void fs_launch_blob_scrub(int stype, void* feat, const int* cnt, const int* start, int n, int K, int d8, cudaStream_t st);
+
+// ---- a quality store (sb200_fstore_set_retention): observations kept in the track's order in ring slots 0, 1, ... (the
+// ring start is always 0), qual[cap][K] the quality of the row in each slot (0 where a slot holds none) and hlen[cap]
+// each track's merge history length.
+// What associate and add on a quality store read besides FsStore and FsCall (a struct of its own, so that FsStore and
+// FsCall keep their layout): the quality and history-length columns, c(h) for h < ntab (c(h) = cap_tab[ntab - 1]
+// beyond), the request rows' qualities [R], and whether the call merges queries (associate: each adds a history of
+// length 1) or appends rows (add).
+struct FsQCall {
+  float* qual;
+  int* hlen;
+  const int* cap_tab;
+  int ntab;
+  const float* rq;
+  int assoc;
+};
+// associate / add: new positions for dest[q] == -1, then each destination's merges and appends in item order, each
+// truncated at its own capacity, and the rows, qualities, counts, history lengths and new ids written
+void fs_launch_qmerge(const FsStore& s, const FsCall& c, const FsQCall& qc, cudaStream_t st);
+// out[2 i] = cnt, out[2 i + 1] = start of the track at pos[i]; oq[i][j] = the quality of its observation j (0 past cnt)
+void fs_launch_qpeek(const FsStore& s, const float* qual, const int* pos, int n, int* out, float* oq, cudaStream_t st);
+// qual[pos[i]][0 .. K) = vals[i][0 .. K), hlen[pos[i]] = hl[i]
+void fs_launch_qual_set(float* qual, int* hlen, const int* pos, const float* vals, const int* hl, int n, int K,
+                        cudaStream_t st);
+// dst[i][.] = src[from[i]][.], i < n, w 32-bit words per track: the qualities and history lengths of a compaction
+void fs_launch_words_compact(const void* src, void* dst, const int* from, int n, int w, cudaStream_t st);
+// store blob, before anything is copied: bad[0] counts the NaN qualities in filled slots, bad[1] the observations whose
+// quality is above the one before
+void fs_launch_qual_check(const float* qual, const int* cnt, const int* start, int n, int K, int* bad, cudaStream_t st);
+// store blob, after its sections are copied: zeroes the qualities of the slots that hold no observation
+void fs_launch_qual_scrub(float* qual, const int* cnt, const int* start, int n, int K, cudaStream_t st);
 
 }  // namespace sb

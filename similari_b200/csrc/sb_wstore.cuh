@@ -60,6 +60,8 @@ int tracker_drop_wasted(sb200_tracker* t, int64_t n);
 void fstore_info(sb200_fstore* s, int* device, int* feature_dim, int* topn);
 // the store's gate rule (SB200_FSTORE_GATE_*); a gated store refuses associate_wasted
 int fstore_gate(sb200_fstore* s);
+// the store's retention rule (SB200_FSTORE_KEEP_*); a quality store refuses associate_wasted
+int fstore_retention(sb200_fstore* s);
 
 // Writes the request rows of a store call on the store's stream `st`: rows[R][d8] f32 (zero-padded from feature_dim),
 // request row r holding observation r - qoff[q] of the rows query q = row_q[r] keeps (its newest max_observations,

@@ -108,6 +108,9 @@ int64_t sb200_fstore_associate_wasted(sb200_fstore* s, sb200_tracker* t, int64_t
   if (sb::fstore_gate(s))
     return fail(SB200_ERR_INVALID, "associate_wasted needs an ungated store: a wasted record has no exact window (the "
                                    "tracker keeps no birth epoch)");
+  if (sb::fstore_retention(s))
+    return fail(SB200_ERR_INVALID, "associate_wasted needs a store that keeps its newest observations: the tracker's "
+                                   "feature history keeps no quality");
   const sb::TrackerFeatureInfo ti = sb::tracker_feature_info(t);
   if (!ti.visual) return fail(SB200_ERR_INVALID, "the tracker is not a visual tracker");
   if (!ti.history) return fail(SB200_ERR_INVALID, "the tracker's feature history is off (sb200_set_feature_history)");

@@ -657,6 +657,8 @@ METRICS = {"euclidean": _lib.VIS_EUCLIDEAN, "cosine": _lib.VIS_COSINE}
 # track attribute rules of the feature store (sb200_fstore_set_gate)
 GATES = {None: _lib.FSTORE_GATE_NONE, "same_source": _lib.FSTORE_GATE_SAME_SOURCE,
          "any_source": _lib.FSTORE_GATE_ANY_SOURCE}
+# retention rules of the feature store (sb200_fstore_set_retention)
+RETENTIONS = {"newest": _lib.FSTORE_KEEP_NEWEST, "quality": _lib.FSTORE_KEEP_BEST_QUALITY}
 
 
 class FeatureStore:
@@ -680,16 +682,26 @@ class FeatureStore:
     CamTrackingAttributes of the reference's examples/track_merging.rs), and a query and a track are compared, and
     merged, only when their windows are disjoint (touching counts as disjoint) and, for "same_source", their sources are
     equal.  add / search / associate and their _device forms then need sources=, t_start= and t_end= (one per row or
-    query); attributes(ids) returns the stored ones.  gate=None (the default) is the store without attributes."""
+    query); attributes(ids) returns the stored ones.  gate=None (the default) is the store without attributes.
+
+    Retention: retention="quality" keeps each track's best observations by quality, as the reference's
+    examples/track_merging.rs does, instead of its newest ones: every row carries an f32 quality (quality=, one per row,
+    required on such a store and refused on a newest one), every track a merge history (merge_history(ids)), and a track
+    of history length h holds at most min(max_observations, int(initial_capacity * merge_extension ** h)) rows, best
+    first; fetch_quality(ids) returns them with their qualities.  A query takes part with its best
+    int(initial_capacity * merge_extension) rows.  associate_wasted is refused on such a store."""
 
     def __init__(self, metric="euclidean", distance_filter=100.0, max_observations=3, feature_dim=256, topn=1,
-                 max_distance=100.0, min_votes=1, device=0, storage="f32", gate=None):
+                 max_distance=100.0, min_votes=1, device=0, storage="f32", gate=None, retention="newest",
+                 initial_capacity=4, merge_extension=1.5):
         if metric not in METRICS:
             raise ValueError(f"metric must be one of {sorted(METRICS)}")
         if storage not in FEATURE_TYPES:
             raise ValueError(f"storage must be one of {sorted(FEATURE_TYPES)}")
         if gate not in GATES:
             raise ValueError(f"gate must be one of {list(GATES)}")
+        if retention not in RETENTIONS:
+            raise ValueError(f"retention must be one of {list(RETENTIONS)}")
         self._L = lib()
         o = _lib.FstoreOptions(METRICS[metric], distance_filter, max_observations, feature_dim, topn, max_distance,
                                min_votes, device)
@@ -701,6 +713,29 @@ class FeatureStore:
         check(self._L.sb200_fstore_set_storage_type(h, FEATURE_TYPES[storage]))
         check(self._L.sb200_fstore_set_gate(h, GATES[gate]))
         self.gate = gate
+        check(self._L.sb200_fstore_set_retention(h, RETENTIONS[retention], int(initial_capacity),
+                                                 float(merge_extension)))
+        self._keep = retention
+
+    def retention(self):
+        """(rule, initial_capacity, merge_extension): rule "newest" or "quality"."""
+        r, i, e = C.c_int32(0), C.c_int32(0), C.c_float(0.0)
+        check(self._L.sb200_fstore_get_retention(self._h, C.byref(r), C.byref(i), C.byref(e)))
+        return {v: k for k, v in RETENTIONS.items()}[r.value], int(i.value), float(e.value)
+
+    def _quality(self, n, quality):
+        """The quality column of a call (n values), or None for a newest store: required on a quality store and
+        refused on a newest one, as the gate keywords are."""
+        if self._keep == "newest":
+            if quality is not None:
+                raise ValueError("quality= needs a quality store (FeatureStore(retention='quality'))")
+            return None
+        if quality is None:
+            raise ValueError("a quality store needs quality=, one value per feature row")
+        q = np.ascontiguousarray(quality, dtype=np.float32)
+        if q.shape != (n,):
+            raise ValueError("quality needs one value per feature row")
+        return q
 
     def _attrs(self, n, sources, t_start, t_end):
         """The sb200_fstore_attrs of a call (and the arrays it points into), or None for an ungated store.  The three
@@ -763,34 +798,40 @@ class FeatureStore:
         check(self._L.sb200_fstore_set_feature_type(self._h, _lib.FEATURE_F32))
         return _f32(features).reshape(-1, self.D)
 
-    def add(self, ids, features, sources=None, t_start=None, t_end=None):
+    def add(self, ids, features, sources=None, t_start=None, t_end=None, quality=None):
         """TrackStore::add for each (ids[i], features[i]) in order (a gated store: with sources[i] and the window
-        [t_start[i], t_end[i]])."""
+        [t_start[i], t_end[i]]; a quality store: with quality[i])."""
         ids = np.ascontiguousarray(ids, dtype=np.uint64)
         a = self._attrs(len(ids), sources, t_start, t_end)
+        q = self._quality(len(ids), quality)
         f = self._column(features)
         if len(f) != len(ids):
             raise ValueError("features needs one row per id")
-        self._call("add", a, (len(ids), ptr(ids)), f)
+        self._call("add", a, (len(ids), ptr(ids)), f, q=q)
 
-    def add_device(self, ids, d_features, stream=0, sources=None, t_start=None, t_end=None):
+    def add_device(self, ids, d_features, stream=0, sources=None, t_start=None, t_end=None, quality=None):
         """sb200_fstore_add_device: `d_features` is the raw device address of [len(ids)][feature_dim] elements of the
         type set by set_feature_type (e.g. the data_ptr() of a torch CUDA tensor)."""
         ids = np.ascontiguousarray(ids, dtype=np.uint64)
         a = self._attrs(len(ids), sources, t_start, t_end)
+        q = self._quality(len(ids), quality)
         self._use_declared_type()
-        self._call("add", a, (len(ids), ptr(ids)), None, d_features, stream)
+        self._call("add", a, (len(ids), ptr(ids)), None, d_features, stream, q=q)
 
-    def _call(self, op, a, lead, f, d_features=None, stream=0, out=None):
+    def _call(self, op, a, lead, f, d_features=None, stream=0, out=None, q=None):
         """sb200_fstore_{op} with the host column f, or sb200_fstore_{op}_device with the device column d_features and
-        the caller's stream (f is None); on a gated store (a from _attrs) sb200_fstore_{op}_attr, which takes either.
+        the caller's stream (f is None); on a gated store (a from _attrs) sb200_fstore_{op}_attr, which takes either;
+        on a quality store (q: the qualities) sb200_fstore_{op}_quality, which takes either and a's attributes or NULL.
         lead: the arguments before the attributes and features; out: the output arrays, in the call's order."""
         res = [ptr(v) for v in out.values()] if out else []
         if f is None:
             col, st = (None, C.c_void_p(d_features or None)), C.c_void_p(stream or None)
         else:
             col, st = (ptr(f), None), None
-        if a is not None:
+        if q is not None:
+            attrs = C.byref(a[0]) if a is not None else None
+            check(getattr(self._L, f"sb200_fstore_{op}_quality")(self._h, *lead, ptr(q), attrs, *col, *res, st))
+        elif a is not None:
             check(getattr(self._L, f"sb200_fstore_{op}_attr")(self._h, *lead, C.byref(a[0]), *col, *res, st))
         elif f is None:
             check(getattr(self._L, f"sb200_fstore_{op}_device")(self._h, *lead, col[1], *res, st))
@@ -815,38 +856,44 @@ class FeatureStore:
             out["merged"] = np.zeros(q, np.uint8)
         return ids, offs, f, out
 
-    def search(self, ids, offsets, features, sources=None, t_start=None, t_end=None):
+    def search(self, ids, offsets, features, sources=None, t_start=None, t_end=None, quality=None):
         """foreign_track_distances + TopNVoting::winners: counts[q], winners[q][topn] (track ids), weights[q][topn].  A
-        gated store takes one source and window per query; incompatible pairs neither vote nor count toward max_dist."""
+        gated store takes one source and window per query; incompatible pairs neither vote nor count toward max_dist.
+        A quality store takes one quality per feature row."""
         a = self._attrs(len(ids), sources, t_start, t_end)
         ids, offs, f, out = self._queries(ids, offsets, features)
-        self._call("search", a, (len(ids), ptr(ids), ptr(offs)), f, out=out)
+        q = self._quality(int(offs[-1]) if len(ids) else 0, quality)
+        self._call("search", a, (len(ids), ptr(ids), ptr(offs)), f, out=out, q=q)
         return out
 
-    def associate(self, ids, offsets, features, sources=None, t_start=None, t_end=None):
+    def associate(self, ids, offsets, features, sources=None, t_start=None, t_end=None, quality=None):
         """search, then merge each query with a result into its first winner and add the others as new tracks.  Adds
         track_ids[q] (where the query ended up) and merged[q] to the search outputs.  A gated store merges a query only
         if it is compatible with its first winner's window as the queries merged into it earlier in the call extended it;
         otherwise the query becomes a new track."""
         a = self._attrs(len(ids), sources, t_start, t_end)
         ids, offs, f, out = self._queries(ids, offsets, features, assoc=True)
-        self._call("associate", a, (len(ids), ptr(ids), ptr(offs)), f, out=out)
+        q = self._quality(int(offs[-1]) if len(ids) else 0, quality)
+        self._call("associate", a, (len(ids), ptr(ids), ptr(offs)), f, out=out, q=q)
         return out
 
-    def search_device(self, ids, offsets, d_features, stream=0, sources=None, t_start=None, t_end=None):
+    def search_device(self, ids, offsets, d_features, stream=0, sources=None, t_start=None, t_end=None, quality=None):
         """sb200_fstore_search_device: search with the feature rows at the raw device address `d_features`."""
         a = self._attrs(len(ids), sources, t_start, t_end)
         ids, offs, _, out = self._queries(ids, offsets, None)
+        q = self._quality(int(offs[-1]) if len(ids) else 0, quality)
         self._use_declared_type()
-        self._call("search", a, (len(ids), ptr(ids), ptr(offs)), None, d_features, stream, out)
+        self._call("search", a, (len(ids), ptr(ids), ptr(offs)), None, d_features, stream, out, q=q)
         return out
 
-    def associate_device(self, ids, offsets, d_features, stream=0, sources=None, t_start=None, t_end=None):
+    def associate_device(self, ids, offsets, d_features, stream=0, sources=None, t_start=None, t_end=None,
+                         quality=None):
         """sb200_fstore_associate_device: associate with the feature rows at the raw device address `d_features`."""
         a = self._attrs(len(ids), sources, t_start, t_end)
         ids, offs, _, out = self._queries(ids, offsets, None, assoc=True)
+        q = self._quality(int(offs[-1]) if len(ids) else 0, quality)
         self._use_declared_type()
-        self._call("associate", a, (len(ids), ptr(ids), ptr(offs)), None, d_features, stream, out)
+        self._call("associate", a, (len(ids), ptr(ids), ptr(offs)), None, d_features, stream, out, q=q)
         return out
 
     def search_owned(self, ids, each=False):
@@ -924,6 +971,28 @@ class FeatureStore:
         check(self._L.sb200_fstore_fetch(self._h, len(ids), ptr(ids), int(bool(remove)), ptr(counts), ptr(feats)))
         return counts, feats
 
+    def fetch_quality(self, ids, remove=False):
+        """(counts, features, qualities) of a quality store: fetch() plus qualities[n][max_observations], the quality of
+        each returned row (0 past a count); rows in the track's order, best first."""
+        ids = np.ascontiguousarray(ids, dtype=np.uint64)
+        counts = np.zeros(len(ids), np.int32)
+        feats = np.zeros((len(ids), self.K, self.D), np.float32)
+        qual = np.zeros((len(ids), self.K), np.float32)
+        check(self._L.sb200_fstore_fetch_quality(self._h, len(ids), ptr(ids), int(bool(remove)), ptr(counts), ptr(feats),
+                                                 ptr(qual)))
+        return counts, feats, qual
+
+    def merge_history(self, ids):
+        """Track::get_merge_history of each of the tracks `ids` of a quality store: a uint64 array per id, starting with
+        the track's own id (empty where an id is not stored)."""
+        ids = np.ascontiguousarray(ids, dtype=np.uint64)
+        lens = np.zeros(max(1, len(ids)), np.int32)
+        total = int(check(self._L.sb200_fstore_merge_history(self._h, len(ids), ptr(ids), ptr(lens), 0, None)))
+        out = np.zeros(max(1, total), np.uint64)
+        check(self._L.sb200_fstore_merge_history(self._h, len(ids), ptr(ids), ptr(lens), total, ptr(out)))
+        offs = np.concatenate([[0], np.cumsum(lens[:len(ids)])])
+        return [out[offs[i]: offs[i + 1]].copy() for i in range(len(ids))]
+
     def attributes(self, ids):
         """(sources, t_start, t_end) of the tracks `ids` of a gated store, each an array with one entry per id (0 where
         an id is not stored)."""
@@ -982,4 +1051,5 @@ class FeatureStore:
         g = C.c_int32(0)
         check(L.sb200_fstore_get_gate(h, C.byref(g)))
         self.gate = {v: k for k, v in GATES.items()}[g.value]
+        self._keep = self.retention()[0]
         return self
