@@ -70,6 +70,8 @@ def lib():
             "ofs_associate_quality": (C.c_int, [vp, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i32]),
             "ofs_fetch_quality": (i64, [vp, i32, vp, i32, vp, vp, vp]),
             "ofs_merge_history": (i64, [vp, i32, vp, vp, i64, vp]),
+            "ofs_find_baked": (i64, [vp, i64, i64, i64, vp]),
+            "ofs_associate_store": (C.c_int, [vp, vp, i32, vp, i32, vp, vp, vp, vp, vp, i32]),
         }
         for name, (res, args) in sig.items():
             fn = getattr(L, name)
@@ -296,6 +298,29 @@ class FeatureStore:
         if self._L.ofs_fetch_attr(self._h, len(ids), _p(ids), _p(src), _p(t0), _p(t1)) < 0:
             raise ValueError("attributes() needs a gated store")
         return src, t0, t1
+
+    def find_baked(self, now, baked_period=0):
+        """The ids (store order) of the tracks of a gated store with now > t_end + baked_period, exactly."""
+        n = self.size()
+        out = np.zeros(max(1, n), np.uint64)
+        total = self._L.ofs_find_baked(self._h, int(now), int(baked_period), n, _p(out))
+        if total < 0:
+            raise ValueError("find_baked() needs a gated store")
+        return out[:total]
+
+    def associate_store(self, src, ids, remove=True):
+        """fetch_tracks(ids) of the oracle store `src`, then one associate of this store with those tracks as its
+        queries (each merged into its winner with its list and history, or added whole); remove=True takes them out of
+        `src`.  Returns the associate dict."""
+        ids = np.ascontiguousarray(ids, dtype=np.uint64)
+        q = len(ids)
+        out = {"counts": np.zeros(q, np.int32), "winners": np.zeros((q, self.topn), np.uint64),
+               "weights": np.zeros((q, self.topn), np.float64), "track_ids": np.zeros(q, np.uint64),
+               "merged": np.zeros(q, np.uint8)}
+        if self._L.ofs_associate_store(self._h, src._h, q, _p(ids), int(bool(remove)),
+                                       *(_p(v) for v in out.values()), self.threads):
+            raise ValueError("invalid associate_store request")
+        return out
 
     def size(self):
         return int(self._L.ofs_size(self._h))

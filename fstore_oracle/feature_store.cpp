@@ -22,7 +22,8 @@
 // created, to which every merge appends the source's whole history (Track::merge with merge_history = true,
 // src/track.rs:522-588).  After an observation is appended or a merge concatenates dest ++ src, the list is stably sorted
 // by quality, descending, and truncated to c(h) = min(K, (u64)((float)initial_capacity * powf(merge_extension, (float)h)))
-// with h the track's history length (:257-265).  Queries are fresh tracks (h = 1) built the same way.
+// with h the track's history length (:257-265).  Queries are fresh tracks (h = 1) built the same way, or, in
+// ofs_associate_store, stored tracks of another store, which bring their lists and histories whole.
 #include <algorithm>
 #include <cmath>
 #include <cstdint>
@@ -121,6 +122,8 @@ struct ofs_store {
   float filter, max_distance;
   int gate = 0;   // 0: no attributes; 1: windows disjoint and sources equal; 2: windows disjoint
   int retention = 0;   // 0: newest K; 1: best by quality, capacity growing with the merge history
+  int init_cap = 0;           // retention 1: its parameters
+  float ext = 0.0f;
   std::vector<int> cap_tab;   // retention 1: c(h) for h = 0 .. the first h with c(h) == K (or h = 0 alone when constant)
   std::vector<Track> tracks;
   std::unordered_map<uint64_t, size_t> pos;
@@ -304,12 +307,10 @@ int ofs_search(ofs_store* s, int Q, const uint64_t* ids, const int32_t* offs, co
 }
 
 // one iteration of benches/feature_tracker.rs: search, then merge_external into results[0].winner_track or add_track
-static int associate(ofs_store* s, int Q, const uint64_t* ids, const int32_t* offs, const float* feats,
-                     const uint64_t* src, const int64_t* t0, const int64_t* t1, int32_t* counts, uint64_t* winners,
-                     double* weights, uint64_t* track_ids, uint8_t* merged, int threads, const float* qual = nullptr) {
-  if (s->check(Q, ids, offs, true)) return -1;
-  if (Q == 0) return 0;
-  auto qs = s->build_queries(Q, ids, offs, feats, src, t0, t1, qual);
+// (the queries qs: fresh tracks built from a request, or stored tracks of another store, ofs_associate_store)
+static void associate_tracks(ofs_store* s, const std::vector<Track>& qs, int32_t* counts, uint64_t* winners,
+                             double* weights, uint64_t* track_ids, uint8_t* merged, int threads) {
+  const int Q = (int)qs.size();
   const auto r = s->search(qs, threads);
   s->write(r, counts, winners, weights);
   for (int q = 0; q < Q; ++q) {
@@ -328,6 +329,15 @@ static int associate(ofs_store* s, int Q, const uint64_t* ids, const int32_t* of
       merged[q] = 0;
     }
   }
+}
+
+static int associate(ofs_store* s, int Q, const uint64_t* ids, const int32_t* offs, const float* feats,
+                     const uint64_t* src, const int64_t* t0, const int64_t* t1, int32_t* counts, uint64_t* winners,
+                     double* weights, uint64_t* track_ids, uint8_t* merged, int threads, const float* qual = nullptr) {
+  if (s->check(Q, ids, offs, true)) return -1;
+  if (Q == 0) return 0;
+  associate_tracks(s, s->build_queries(Q, ids, offs, feats, src, t0, t1, qual), counts, winners, weights, track_ids,
+                   merged, threads);
   return 0;
 }
 
@@ -532,6 +542,8 @@ int ofs_set_retention(ofs_store* s, int rule, int initial_capacity, float merge_
     tab.push_back(c((int)tab.size()));
   }
   s->retention = 1;
+  s->init_cap = initial_capacity;
+  s->ext = merge_extension;
   s->cap_tab = tab;
   return 0;
 }
@@ -626,6 +638,48 @@ int64_t ofs_merge_history(ofs_store* s, int n, const uint64_t* ids, int32_t* len
     lengths[i] = (int32_t)s->tracks[it->second].hist.size();
   }
   return total;
+}
+
+// ---- store to store (examples/track_merging.rs:371-481)
+// TrackStore::find_usable with `baked` (:240-247): the ids of the tracks with now > t_end + baked_period, in store order,
+// compared in 128-bit integers as the reference compares in u128.  The first min(cap, total) are written; returns the
+// total, or -1 for an ungated store or cap < 0.
+int64_t ofs_find_baked(ofs_store* s, int64_t now, int64_t baked_period, int64_t cap, uint64_t* ids) {
+  if (!s->gate || cap < 0) return -1;
+  int64_t total = 0;
+  for (const Track& t : s->tracks)
+    if ((__int128)now > (__int128)t.t1 + (__int128)baked_period) {
+      if (total < cap) ids[total] = t.id;
+      ++total;
+    }
+  return total;
+}
+
+// fetch_tracks(ids) of src, each track whole (its list, qualities, triple and merge history), then one associate of dst
+// with those tracks as its queries in the order of ids: merge_external(winner, &track, .., true) merges the lists and
+// appends the history (h + h_q), add_track keeps the track whole; then, with remove, the tracks leave src (a stable
+// compaction).  Refused (-1) before either store changes: dst == src, a different feature_dim, max_observations, gate,
+// retention or retention parameters, n < 0, remove not 0 / 1, an id twice, not stored in src, or stored in dst.
+int ofs_associate_store(ofs_store* d, ofs_store* s, int n, const uint64_t* ids, int remove, int32_t* counts,
+                        uint64_t* winners, double* weights, uint64_t* track_ids, uint8_t* merged, int threads) {
+  if (d == s || d->D != s->D || d->K != s->K || d->gate != s->gate || d->retention != s->retention) return -1;
+  if (d->retention && (d->init_cap != s->init_cap || d->ext != s->ext)) return -1;
+  if (n < 0 || (remove != 0 && remove != 1)) return -1;
+  std::unordered_set<uint64_t> seen;
+  for (int i = 0; i < n; ++i)
+    if (!seen.insert(ids[i]).second || !s->pos.count(ids[i]) || d->pos.count(ids[i])) return -1;
+  if (n == 0) return 0;
+  std::vector<Track> qs;
+  for (int i = 0; i < n; ++i) qs.push_back(s->tracks[s->pos.at(ids[i])]);
+  associate_tracks(d, qs, counts, winners, weights, track_ids, merged, threads);
+  if (remove) {
+    std::vector<Track> kept;
+    for (Track& t : s->tracks)
+      if (!seen.count(t.id)) kept.push_back(std::move(t));
+    s->tracks.swap(kept);
+    s->reindex();
+  }
+  return 0;
 }
 
 int64_t ofs_size(ofs_store* s) { return (int64_t)s->tracks.size(); }

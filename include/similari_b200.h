@@ -710,6 +710,41 @@ int64_t sb200_fstore_fetch_quality(sb200_fstore* s, int32_t n, const uint64_t* i
 int64_t sb200_fstore_merge_history(sb200_fstore* s, int32_t n, const uint64_t* ids, int32_t* lengths, int64_t cap,
                                    uint64_t* out);
 
+/* ---- store to store: the main loop of the reference's examples/track_merging.rs (:371-481) ----
+ * A collecting store gathers each tracklet's observations; the tracks that are baked move into a merge store (the
+ * gallery), each merged into its winner or added whole.  Both calls run on the device: no stored row, window or quality
+ * crosses PCIe. */
+/* TrackStore::find_usable (src/track/store.rs:348-374) with the example's `baked` (:240-247) on a gated store: the ids of
+ * the tracks with now > t_end + baked_period, compared exactly for every int64 value (the reference compares in u128),
+ * in store order.  The first min(cap, total) are written to ids (NULL allowed when cap == 0); returns the total, or a
+ * negative status.  One kernel selects on the device; only the count and the selected positions are read back.
+ * Deviation: the reference keeps baked_period per track (the example resets it with BakedPeriodUpdate(0) when it
+ * promotes a track); here it is an argument of the call, so the store keeps no extra state and its blob is unchanged.
+ * There are no Wasted or Err statuses.  SB200_ERR_INVALID, changing nothing: an ungated store (it keeps no windows),
+ * cap < 0, ids == NULL with cap > 0. */
+int64_t sb200_fstore_find_baked(sb200_fstore* s, int64_t now, int64_t baked_period, int64_t cap, uint64_t* ids);
+/* fetch_tracks(ids) of `src`, then one sb200_fstore_associate of `dst` with those tracks as its queries, in the order of
+ * ids, each merged into its winner with merge_external(winner, &track, .., true) or added with add_track
+ * (examples/track_merging.rs:371-481, Track::merge src/track.rs:522-588).  A query's id is its src id, its rows its kept
+ * rows in its own order (a newest store: oldest first; a quality store: best first, with their qualities), widened
+ * exactly from src's storage type and rounded to dst's at apply time as any f32 request.  A gated query carries its
+ * src source and window, and the gate decides the merges as in sb200_fstore_associate_attr.  On quality stores a query
+ * brings its history length h_q and its history: a merge sets h += h_q, merges the two quality lists stably (dst rows
+ * first on ties), truncates at c(h) and appends the query's history to the destination's; a new track keeps src's list,
+ * h_q and history whole.  Outputs as sb200_fstore_associate.  remove = 1 then takes the queried tracks out of src (a
+ * stable compaction, as sb200_fstore_fetch with remove); remove = 0 leaves src unchanged.  The call is synchronous: it
+ * reads src's columns on dst's stream once src's stream is idle, and compacts src after dst's work is complete.  On
+ * newest stores both stores end exactly as after src.fetch(ids, remove) (+ sb200_fstore_fetch_attr on a gated store)
+ * then dst.associate of the fetched rows.  dst and src must be distinct handles on one device with equal feature_dim,
+ * max_observations, gate rule, retention rule and retention parameters; storage types, metric, topn and thresholds may
+ * differ (they belong to dst's voting).  SB200_ERR_INVALID, before either store changes: a NULL handle, dst == src,
+ * a mismatch above, n < 0, remove not 0 or 1, an id given twice, an id not stored in src, an id already stored in dst
+ * (the reference's DuplicateTrackId).  SB200_ERR_CAPACITY: more than 2^30 observation pairs (the call is not split,
+ * which would change max_dist).  n == 0 changes nothing.  sb200_fstore_last_stage_ms(dst) reports the call's stages. */
+int sb200_fstore_associate_store(sb200_fstore* dst, sb200_fstore* src, int32_t n, const uint64_t* ids, int32_t remove,
+                                 int32_t* counts, uint64_t* winners, double* weights, uint64_t* track_ids,
+                                 uint8_t* merged);
+
 /* ---- the store blob ----
  * The whole store as one relocatable block of bytes: this header, then four sections at 256-byte aligned offsets, gaps
  * zeroed, in this order: ids[live] (u64), cnt[live] (i32 observations held), start[live] (i32 ring slot of the oldest

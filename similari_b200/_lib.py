@@ -180,7 +180,7 @@ EXPORTS = [
     "sb200_fstore_search_attr", "sb200_fstore_associate_attr", "sb200_fstore_fetch_attr",
     "sb200_fstore_set_retention", "sb200_fstore_get_retention", "sb200_fstore_add_quality",
     "sb200_fstore_search_quality", "sb200_fstore_associate_quality", "sb200_fstore_fetch_quality",
-    "sb200_fstore_merge_history",
+    "sb200_fstore_merge_history", "sb200_fstore_find_baked", "sb200_fstore_associate_store",
 ]
 
 
@@ -296,6 +296,8 @@ def lib():
                                                      vp, vp, vp]),
         "sb200_fstore_fetch_quality": (i64, [vp, i32, vp, i32, vp, vp, vp]),
         "sb200_fstore_merge_history": (i64, [vp, i32, vp, vp, i64, vp]),
+        "sb200_fstore_find_baked": (i64, [vp, i64, i64, i64, vp]),
+        "sb200_fstore_associate_store": (C.c_int, [vp, vp, i32, vp, i32, vp, vp, vp, vp, vp]),
         "sb200_fstore_get_storage_type": (C.c_int, [vp, C.POINTER(i32)]),
         "sb200_fstore_associate_wasted": (i64, [vp, vp, i64, u64, vp, vp, vp, vp, vp, vp, i32, vp, vp, vp, vp, vp, vp, vp,
                                                 vp, vp, vp]),

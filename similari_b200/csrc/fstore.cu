@@ -16,6 +16,10 @@
 // track (hlen) on the device and the merge histories on the host (hist, beside hid, updated from each call's
 // read-back).  Associate and add plan and apply their merges on the device (fs_launch_qmerge), with one read-back as on
 // a newest store; merge_owned plans on the host from the qualities of the tracks it touches, as it plans rings.
+// associate_store takes stored tracks of another store as the queries of one associate call: its row source
+// (StoreRows) stages their rows, triples, qualities and history lengths from the source store's columns on the
+// destination's stream, so the rows never leave the device; find_baked selects tracks by their t_end on the device and
+// reads back only the selected positions.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -108,6 +112,14 @@ static_assert(kSecHist + 1 == SB200_FSTORE_BLOB_SECTIONS_V3, "the version-3 sect
 // the store kinds that have a column (sb200_fstore::Col::need)
 enum { kNeedAll, kNeedGate, kNeedQuality };
 
+// The queries of associate_store, which its row source puts on the device besides the rows: their triples in qattr (a
+// gated store) and their rows' qualities in dqr (a quality store).  hq[Q]: their history lengths on the device, and
+// hist[q] their merge histories (a quality store; else nullptr).
+struct TrackQueries {
+  const int* hq;
+  const std::vector<std::vector<uint64_t>>* hist;
+};
+
 // a gated call's triples on the host: n entries of each column
 struct Triples {
   std::vector<uint64_t> src;
@@ -188,6 +200,7 @@ struct sb200_fstore {
   static constexpr int kNumCols = 10;
   static const Col kCols[kNumCols];
   DBuf qattr;                                // a gated call's triples, [n] of each column
+  DBuf sq;                                   // associate_store: the queried src positions [n], history lengths [n]
   std::vector<uint64_t> hid;                 // ids in store order
   std::unordered_map<uint64_t, int> hpos;    // id -> store position
   // per-call buffers
@@ -731,25 +744,29 @@ struct sb200_fstore {
                           assoc, attrs, quality);
   }
 
-  // associate whose request rows `rsrc` writes on the device (sb200_fstore_associate_wasted); offs as for associate
+  // associate whose request rows `rsrc` writes on the device (sb200_fstore_associate_wasted, and associate_store with
+  // its queries `tq`); offs as for associate
   int associate_rows(int Q, const uint64_t* qids, const int32_t* offs, const sb::FsRowSource& rsrc, int32_t* counts,
-                     uint64_t* winners, double* weights, uint64_t* track_ids, uint8_t* merged) {
+                     uint64_t* winners, double* weights, uint64_t* track_ids, uint8_t* merged,
+                     const TrackQueries* tq = nullptr) {
     if (int rc = check_ids(Q, qids, "query id", true)) return rc;
     std::vector<int> qoff, src;
     if (int rc = plan_rows(Q, offs, &qoff, &src)) return rc;
     if (int rc = begin()) return rc;
     if (Q == 0) return 0;
     return launch_queries(Q, qids, qoff, src, Column{nullptr, false, nullptr}, 0, &rsrc, counts, winners, weights,
-                          track_ids, merged, true);
+                          track_ids, merged, true, nullptr, nullptr, tq);
   }
 
   // the device part of search / associate, after every check: upload, distances, TopN, apply, results
   int launch_queries(int Q, const uint64_t* qids, const std::vector<int>& qoff, const std::vector<int>& src,
                      const Column& col, size_t col_rows, const sb::FsRowSource* rsrc, int32_t* counts,
                      uint64_t* winners, double* weights, uint64_t* track_ids, uint8_t* merged, bool assoc,
-                     const sb200_fstore_attrs* attrs = nullptr, const float* quality = nullptr) {
+                     const sb200_fstore_attrs* attrs = nullptr, const float* quality = nullptr,
+                     const TrackQueries* tq = nullptr) {
     const int R = (int)src.size(), topn = o.topn, K = o.max_observations;
     const bool qa = assoc && keep;   // a quality store's merges are planned and applied by fs_launch_qmerge
+    const bool gated = attrs || (tq && gate);   // the queries' triples are in qattr
     const long long live = (long long)hid.size(), S = live * K;
     const ReqLayout L(Q, R, d8, !rsrc && (col.on_device || ftype != SB200_FEATURE_F32));
     const ResLayout RL(Q, topn);
@@ -760,7 +777,9 @@ struct sb200_fstore {
     if (attrs)
       if (int rc = upload_triples(Q, attrs->source, attrs->t_start, attrs->t_end)) return rc;
     sb::FsQCall qc{};
-    if (qa) {
+    if (qa && tq) {   // the row source wrote the rows' qualities
+      qc = {qual.as<float>(), hlen.as<int>(), dcap.as<int>(), (int)cap_tab.size(), dqr.as<float>(), 1};
+    } else if (qa) {
       std::vector<float> rq(R);
       for (int r = 0; r < R; ++r) rq[r] = quality[src[r]];
       if (int rc = qcall(rq, true, &qc)) return rc;
@@ -769,36 +788,41 @@ struct sb200_fstore {
     const sb::FsStore s = view();
     const sb::FsCall c = call_view(L, Q, R, &RL);
     CU(cudaEventRecord(ev[0], st));
-    sb::fs_launch_dist(o.metric, o.distance_filter, s, c, st, sb::kFsForeign, nullptr, attrs ? &g : nullptr);
+    sb::fs_launch_dist(o.metric, o.distance_filter, s, c, st, sb::kFsForeign, nullptr, gated ? &g : nullptr);
     CU(cudaEventRecord(ev[1], st));
     sb::fs_launch_topn(o.max_distance, o.min_votes, topn, assoc, s, c, st);
     CU(cudaEventRecord(ev[2], st));
-    if (assoc && attrs) sb::fs_launch_gate_resolve(c, g, st);
-    if (qa) sb::fs_launch_qmerge(s, c, qc, st);
+    if (assoc && gated) sb::fs_launch_gate_resolve(c, g, st);
+    if (qa) sb::fs_launch_qmerge(s, c, qc, st, tq ? tq->hq : nullptr);
     else if (assoc) sb::fs_launch_apply(s, c, st);
-    if (assoc && attrs) sb::fs_launch_attr_new(s.live, c, g, st);
+    if (assoc && gated) sb::fs_launch_attr_new(s.live, c, g, st);
     CU(cudaEventRecord(ev[3], st));
     CU(cudaMemcpyAsync(hres.p, dres.p, RL.total, cudaMemcpyDeviceToHost, st));
     // gated or quality associate: the position each query ended up at (>= live: a new track)
     std::vector<int> where;
-    if (assoc && (attrs || qa)) {
+    if (assoc && (gated || qa)) {
       where.resize(Q);
       CU(cudaMemcpyAsync(where.data(), c.dest, (size_t)Q * 4, cudaMemcpyDeviceToHost, st));
     }
     if (int rc = finish(S > 0 ? 0 : 1, assoc ? 3 : 2)) return rc;   // no distance stage on an empty store
     read_results(RL, Q, counts, winners, weights);
     if (assoc) {
+      // Track::merge with merge_history = true appends the query's history: [id], or a stored track's whole one
+      auto qhist = [&](int q) { return tq ? (*tq->hist)[q] : std::vector<uint64_t>{qids[q]}; };
       for (int q = 0; q < Q; ++q) {
         // a first winner the gate refused leaves a new track
-        merged[q] = attrs || qa ? where[q] < live : counts[q] > 0;
+        merged[q] = gated || qa ? where[q] < live : counts[q] > 0;
         track_ids[q] = merged[q] ? winners[(size_t)q * topn] : qids[q];
-        if (qa && merged[q]) hist[where[q]].push_back(qids[q]);   // Track::merge with merge_history = true
+        if (qa && merged[q]) {
+          const std::vector<uint64_t> h = qhist(q);
+          hist[where[q]].insert(hist[where[q]].end(), h.begin(), h.end());
+        }
       }
       for (int q = 0; q < Q; ++q)
         if (!merged[q]) {
           hpos[qids[q]] = (int)hid.size();
           hid.push_back(qids[q]);
-          if (qa) hist.push_back({qids[q]});
+          if (qa) hist.push_back(qhist(q));
         }
     }
     return 0;
@@ -911,6 +935,112 @@ struct sb200_fstore {
     std::copy(v.t0.begin(), v.t0.end(), t0);
     std::copy(v.t1.begin(), v.t1.end(), t1);
     return found;
+  }
+
+  // ---- store to store (examples/track_merging.rs:371-481)
+  // TrackStore::find_usable with `baked` (now > t_end + period): the baked ids in store order, the first min(cap, total)
+  // into ids; returns the total.  Only the count and the selected positions come back.
+  int64_t find_baked(int64_t now, int64_t period, int64_t cap_ids, uint64_t* idv) {
+    if (!gate) return fail(SB200_ERR_INVALID, "the store has no gate (sb200_fstore_set_gate): it keeps no windows");
+    if (cap_ids < 0 || (cap_ids > 0 && !idv)) return fail(SB200_ERR_INVALID, "cap < 0, or ids is NULL with cap > 0");
+    if (int rc = begin()) return rc;
+    const int n = (int)hid.size();
+    if (n == 0) return 0;
+    if (int rc = gout.ensure(((size_t)n + 1) * 4)) return rc;
+    sb::fs_launch_baked(at1.as<long long>(), n, (long long)now, (long long)period, gout.as<int>(), st);
+    int total = 0;
+    CU(cudaMemcpyAsync(&total, gout.p, 4, cudaMemcpyDeviceToHost, st));
+    if (int rc = finish()) return rc;
+    const int m = (int)std::min<int64_t>(cap_ids, total);
+    if (m > 0) {
+      std::vector<int> pos(m);
+      CU(cudaMemcpyAsync(pos.data(), gout.as<int>() + 1, (size_t)m * 4, cudaMemcpyDeviceToHost, st));
+      if (int rc = finish()) return rc;
+      for (int i = 0; i < m; ++i) idv[i] = hid[pos[i]];
+    }
+    return total;
+  }
+
+  // associate_store's row source: the queried tracks of `src` (positions qpos[Q] on the device) staged on this store's
+  // stream into the call's rows, and into the tables TrackQueries names
+  struct StoreRows {
+    sb200_fstore* src;
+    const int* qpos;
+    int Q;
+    sb::FsAttrCols qattr;   // gated: the queries' triples
+    float* rq;              // quality store: the rows' qualities
+    int* hq;                // quality store: the queries' history lengths
+  };
+  static int stage_store_rows(void* ctx, float* rows, const int* qoff, const int* row_q, int R, cudaStream_t st) {
+    const StoreRows& x = *static_cast<const StoreRows*>(ctx);
+    const sb200_fstore& src = *x.src;
+    sb::FsCall c{};
+    c.qoff = qoff;
+    c.row_q = row_q;
+    c.Q = x.Q;
+    c.R = R;
+    const sb::FsStore s = src.view();   // each row widened exactly from src's storage type
+    sb::fs_launch_owned_stage(s, c, x.qpos, rows, st);
+    if (src.gate) sb::fs_launch_attr_gather(src.attr_cols(), x.qpos, x.Q, x.qattr, st);
+    if (src.keep) {
+      sb::fs_launch_qual_stage(s, c, src.qual.as<float>(), x.qpos, x.rq, st);
+      sb::fs_launch_words_compact(src.hlen.p, x.hq, x.qpos, x.Q, 1, st);
+    }
+    CU(cudaGetLastError());
+    return 0;
+  }
+
+  // fetch_tracks(ids) from src, then one associate call of this store with those tracks as its queries (merge_external
+  // with merge_history = true, or add_track), then, with remove, the tracks taken out of src
+  int associate_store(sb200_fstore* src, int n, const uint64_t* idv, int remove, int32_t* counts, uint64_t* winners,
+                      double* weights, uint64_t* track_ids, uint8_t* merged) {
+    if (src == this) return fail(SB200_ERR_INVALID, "dst and src are the same store (merge_owned merges within one)");
+    const sb200_fstore_options& so = src->o;
+    if (so.device != o.device) return fail(SB200_ERR_INVALID, "src is on device %d, dst on device %d", so.device, o.device);
+    if (so.feature_dim != o.feature_dim || so.max_observations != o.max_observations)
+      return fail(SB200_ERR_INVALID, "feature_dim / max_observations differ: %d / %d in src, %d / %d in dst",
+                  so.feature_dim, so.max_observations, o.feature_dim, o.max_observations);
+    if (src->gate != gate) return fail(SB200_ERR_INVALID, "gate rules differ: %d in src, %d in dst", src->gate, gate);
+    if (src->keep != keep || (keep && (src->init_cap != init_cap || src->ext != ext)))
+      return fail(SB200_ERR_INVALID, "retention rules or their parameters differ between src and dst");
+    if (n < 0) return fail(SB200_ERR_INVALID, "n < 0");
+    if (remove != 0 && remove != 1) return fail(SB200_ERR_INVALID, "remove must be 0 or 1");
+    if (n > 0 && (!idv || !counts || !winners || !weights || !track_ids || !merged))
+      return fail(SB200_ERR_INVALID, "ids or an output is NULL");
+    if (int rc = check_ids(n, idv, "id", true)) return rc;
+    std::vector<int> pos(n);
+    for (int i = 0; i < n; ++i) {
+      auto it = src->hpos.find(idv[i]);
+      if (it == src->hpos.end())
+        return fail(SB200_ERR_INVALID, "id %llu is not stored in src", (unsigned long long)idv[i]);
+      pos[i] = it->second;
+    }
+    if (int rc = begin()) return rc;
+    if (n == 0) return 0;
+    // src's stream is idle once peek returns, so every column this call reads from src is complete
+    std::vector<int> ring;
+    if (int rc = src->peek(pos, &ring)) return rc;
+    std::vector<int32_t> offs(n + 1, 0);
+    for (int i = 0; i < n; ++i) offs[i + 1] = offs[i] + ring[2 * i];
+    std::vector<std::vector<uint64_t>> qhist;
+    if (keep)
+      for (int p : pos) qhist.push_back(src->hist[p]);
+    if (int rc = sq.ensure((size_t)n * 8)) return rc;
+    if (gate)
+      if (int rc = qattr.ensure((size_t)n * 24)) return rc;
+    if (keep)
+      if (int rc = dqr.ensure((size_t)offs[n] * 4)) return rc;
+    CU(cudaMemcpyAsync(sq.p, pos.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
+    StoreRows ctx{src, sq.as<int>(), n, triples(qattr, n), dqr.as<float>(), sq.as<int>() + n};
+    const TrackQueries tq{keep ? sq.as<int>() + n : nullptr, keep ? &qhist : nullptr};
+    // returns once this store's stream has finished, so src's rows are read no more
+    if (int rc = associate_rows(n, idv, offs.data(), {stage_store_rows, &ctx}, counts, winners, weights, track_ids,
+                                merged, &tq))
+      return rc;
+    if (!remove) return 0;
+    std::vector<char> gone(src->hid.size(), 0);
+    for (int p : pos) gone[p] = 1;
+    return src->remove_marked(gone);
   }
 
   // qout: a quality store's qualities [n][K] of the rows returned (fetch_quality), else nullptr
@@ -1658,6 +1788,18 @@ int64_t sb200_fstore_merge_history(sb200_fstore* s, int32_t n, const uint64_t* i
     lengths[i] = (int32_t)h.size();
   }
   return total;
+}
+
+int64_t sb200_fstore_find_baked(sb200_fstore* s, int64_t now, int64_t baked_period, int64_t cap, uint64_t* ids) {
+  if (!s) return no_handle();
+  return s->find_baked(now, baked_period, cap, ids);
+}
+
+int sb200_fstore_associate_store(sb200_fstore* dst, sb200_fstore* src, int32_t n, const uint64_t* ids, int32_t remove,
+                                 int32_t* counts, uint64_t* winners, double* weights, uint64_t* track_ids,
+                                 uint8_t* merged) {
+  if (!dst || !src) return no_handle();
+  return dst->associate_store(src, n, ids, remove, counts, winners, weights, track_ids, merged);
 }
 
 int sb200_fstore_search_owned(sb200_fstore* s, int32_t n, const uint64_t* ids, int32_t each, int32_t* counts,

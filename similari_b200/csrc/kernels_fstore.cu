@@ -15,6 +15,9 @@
 //   Track::distances' attributes.compatible check and Track::merge's attributes.merge (src/track.rs:604-652, 522-530)
 //   with examples/track_merging.rs:218-245's CamTrackingAttributes, for a gated store: the gated distance instances,
 //   fs_gate_resolve_kernel and the attribute kernels
+//   TrackStore::find_usable (src/track/store.rs:348-374) with examples/track_merging.rs:240-247's `baked`, for a gated
+//   store: fs_baked_kernel; and that example's fetch_tracks + merge_external(.., true) / add_track from one store into
+//   another: the owned stage reading the source store, fs_qual_stage_kernel and the hq instances of fs_qmerge_kernel
 // Every value that reaches the voting stage is the oracle's f32 bit for bit: --fmad=false, 8-lane blocks reduced by
 // reduce_add8 and accumulated one after another, then sqrt (euclidean) or the quotient by sqrt(|a|^2 |b|^2) (cosine).
 #include <climits>
@@ -701,8 +704,18 @@ __global__ void __launch_bounds__(kOrderThreads) fs_qorder_kernel(FsStore s, FsC
 // back.  The surviving stored rows are a prefix of the old list and only move later, so they are moved in place, last
 // first; request rows are then rounded into their slots as fs_apply_kernel rounds them.  Every thread handles the same
 // 16-byte vectors of every row, so no row is read after another thread has overwritten it.
-template <typename Elem>
-__global__ void __launch_bounds__(128) fs_qmerge_kernel(FsStore s, FsCall c, FsQCall qc) {
+// The history length after item qi: associate adds a query of history 1 and add starts a new track at 1 (the empty
+// pack, every existing instance); associate_store adds the queried stored track's whole history, hq[qi] (Track::merge
+// with merge_history = true, src/track.rs:555-560).
+__device__ __forceinline__ int fs_qhist(int h, int, const FsQCall& qc) {
+  if (qc.assoc) ++h;
+  else if (h == 0) h = 1;
+  return h;
+}
+__device__ __forceinline__ int fs_qhist(int h, int qi, const FsQCall&, const int* hq) { return h + hq[qi]; }
+
+template <typename Elem, typename... HQ>
+__global__ void __launch_bounds__(128) fs_qmerge_kernel(FsStore s, FsCall c, FsQCall qc, HQ... hq) {
   __shared__ int s_src[kFsMaxObs], t_src[kFsMaxObs];   // >= 0: old slot; < 0: request row -(r + 1)
   __shared__ float s_q[kFsMaxObs], t_q[kFsMaxObs];
   __shared__ unsigned int s_hit[4];
@@ -731,8 +744,7 @@ __global__ void __launch_bounds__(128) fs_qmerge_kernel(FsStore s, FsCall c, FsQ
       for (int w = 0; w < 4; ++w)
         for (unsigned int m = s_hit[w]; m; m &= m - 1) {
           const int qi = base + 32 * w + __ffs(m) - 1;
-          if (qc.assoc) ++h;
-          else if (h == 0) h = 1;
+          h = fs_qhist(h, qi, qc, hq...);
           const int cap = qc.cap_tab[min(h, qc.ntab - 1)];
           const int r0 = c.qoff[qi], r1 = c.qoff[qi + 1];
           int a = 0, r = r0, k = 0;
@@ -776,6 +788,46 @@ __global__ void __launch_bounds__(128) fs_qmerge_kernel(FsStore s, FsCall c, FsQ
     qc.hlen[p] = s_h;
     if (!old) s.ids[p] = c.qid[q];
     s.run[p] = 0;
+  }
+}
+
+// associate_store on a quality store: the quality of each request row, read where fs_owned_stage_kernel reads its row
+__global__ void fs_qual_stage_kernel(FsStore s, FsCall c, const float* __restrict__ qual, const int* __restrict__ qpos,
+                                     float* __restrict__ rq) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= c.R) return;
+  const int q = c.row_q[r], p = qpos[q];
+  rq[r] = qual[(size_t)p * s.K + (s.start[p] + (r - c.qoff[q])) % s.K];
+}
+
+// ------------------------------------------------------------------------------------------------ find_baked
+// One CTA of kOrderThreads: warp w scans the contiguous strip [w L, (w + 1) L) of the n tracks, 32 coalesced windows
+// at a time.  A first pass counts each strip's baked tracks, the strips' counts are prefix-summed, and a second pass
+// writes each baked position at its warp's offset plus its rank in the ballot, so the positions come out in store order.
+__global__ void __launch_bounds__(kOrderThreads) fs_baked_kernel(const long long* __restrict__ t_end, int n, long long now,
+                                                                 long long period, int* __restrict__ out) {
+  constexpr int kWarps = kOrderThreads / 32;
+  __shared__ int s_cnt[kWarps];
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  const int L = (n + kOrderThreads - 1) / kOrderThreads * 32;
+  const int b = (int)min((long long)n, (long long)wid * L), e = min(n, b + L);
+  int cnt = 0;
+  for (int i = b + lane; i < e; i += 32) cnt += fs_baked(now, t_end[i], period) ? 1 : 0;
+  cnt = __reduce_add_sync(0xffffffffu, cnt);
+  if (lane == 0) s_cnt[wid] = cnt;
+  __syncthreads();
+  int at = 0, total = 0;
+  for (int w = 0; w < kWarps; ++w) {
+    at += w < wid ? s_cnt[w] : 0;
+    total += s_cnt[w];
+  }
+  if (threadIdx.x == 0) out[0] = total;
+  for (int base = b; base < e; base += 32) {
+    const int i = base + lane;
+    const bool baked = i < e && fs_baked(now, t_end[i], period);
+    const unsigned int bal = __ballot_sync(0xffffffffu, baked);
+    if (baked) out[1 + at + __popc(bal & ((1u << lane) - 1u))] = i;
+    at += __popc(bal);
   }
 }
 
@@ -1021,11 +1073,26 @@ void fs_launch_words_compact(const void* src, void* dst, const int* from, int n,
   note_launch();
 }
 
-void fs_launch_qmerge(const FsStore& s, const FsCall& c, const FsQCall& qc, cudaStream_t st) {
+void fs_launch_qmerge(const FsStore& s, const FsCall& c, const FsQCall& qc, cudaStream_t st, const int* hq) {
   if (c.Q == 0) return;
   fs_qorder_kernel<<<1, kOrderThreads, 0, st>>>(s, c);
-  feat_dispatch(s.stype, [&](auto tag) { fs_qmerge_kernel<decltype(tag)><<<c.Q, 128, 0, st>>>(s, c, qc); });
+  feat_dispatch(s.stype, [&](auto tag) {
+    if (hq) fs_qmerge_kernel<decltype(tag)><<<c.Q, 128, 0, st>>>(s, c, qc, hq);
+    else fs_qmerge_kernel<decltype(tag)><<<c.Q, 128, 0, st>>>(s, c, qc);
+  });
   note_launch(2);
+}
+
+void fs_launch_qual_stage(const FsStore& s, const FsCall& c, const float* qual, const int* qpos, float* rq,
+                          cudaStream_t st) {
+  if (c.R == 0) return;
+  fs_qual_stage_kernel<<<fs_blocks(c.R), 256, 0, st>>>(s, c, qual, qpos, rq);
+  note_launch();
+}
+
+void fs_launch_baked(const long long* t_end, int n, long long now, long long period, int* out, cudaStream_t st) {
+  fs_baked_kernel<<<1, kOrderThreads, 0, st>>>(t_end, n, now, period, out);
+  note_launch();
 }
 
 void fs_launch_qual_check(const float* qual, const int* cnt, const int* start, int n, int K, int* bad, cudaStream_t st) {

@@ -10,6 +10,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <climits>
 #include <vector>
 
 namespace sb {
@@ -76,6 +77,13 @@ struct FsGate {
 __host__ __device__ __forceinline__ bool fs_compatible(int rule, unsigned long long as, long long a0, long long a1,
                                                        unsigned long long bs, long long b0, long long b1) {
   return (a0 >= b1 || a1 <= b0) && (rule != 1 || as == bs);
+}
+
+// The reference's `baked` (examples/track_merging.rs:240-247, compared in u128): now > t_end + period, exact for every
+// int64 value.  The sum leaves the int64 range only where its sign alone decides the answer.
+__host__ __device__ __forceinline__ bool fs_baked(long long now, long long t_end, long long period) {
+  if (period >= 0) return t_end <= LLONG_MAX - period && now > t_end + period;
+  return t_end < LLONG_MIN - period || now > t_end + period;
 }
 
 // How an owned search (sb200_fstore_search_owned) differs from a search of foreign queries, as template parameters of
@@ -161,8 +169,16 @@ struct FsQCall {
   int assoc;
 };
 // associate / add: new positions for dest[q] == -1, then each destination's merges and appends in item order, each
-// truncated at its own capacity, and the rows, qualities, counts, history lengths and new ids written
-void fs_launch_qmerge(const FsStore& s, const FsCall& c, const FsQCall& qc, cudaStream_t st);
+// truncated at its own capacity, and the rows, qualities, counts, history lengths and new ids written.  hq: the history
+// length of each query (associate_store, whose queries are stored tracks of another store), else every query adds 1.
+void fs_launch_qmerge(const FsStore& s, const FsCall& c, const FsQCall& qc, cudaStream_t st, const int* hq = nullptr);
+// associate_store on a quality store: rq[r] = the quality of the stored observation fs_launch_owned_stage copies into
+// request row r (of the track at qpos[row_q[r]] of the store s, with its qualities qual)
+void fs_launch_qual_stage(const FsStore& s, const FsCall& c, const float* qual, const int* qpos, float* rq,
+                          cudaStream_t st);
+// find_baked: out[0] = the number of the n tracks with fs_baked(now, t_end[i], period), out[1 ..] their positions in
+// store order
+void fs_launch_baked(const long long* t_end, int n, long long now, long long period, int* out, cudaStream_t st);
 // out[2 i] = cnt, out[2 i + 1] = start of the track at pos[i]; oq[i][j] = the quality of its observation j (0 past cnt)
 void fs_launch_qpeek(const FsStore& s, const float* qual, const int* pos, int n, int* out, float* oq, cudaStream_t st);
 // qual[pos[i]][0 .. K) = vals[i][0 .. K), hlen[pos[i]] = hl[i]

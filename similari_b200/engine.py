@@ -955,6 +955,34 @@ class FeatureStore:
                 "queried": qd[:n].astype(bool), "counts": cn[:n], "winners": wn[:n], "weights": wt[:n],
                 "track_ids": ti[:n], "merged": mg[:n]}
 
+    def find_baked(self, now, baked_period=0):
+        """sb200_fstore_find_baked: TrackStore::find_usable with the `baked` rule of the reference's
+        examples/track_merging.rs on a gated store: the ids (uint64 array, store order) of the tracks with
+        now > t_end + baked_period, compared exactly for every int64 now / baked_period.  Selected on the device."""
+        now, period = int(now), int(baked_period)
+        if not all(-(1 << 63) <= v < 1 << 63 for v in (now, period)):
+            raise ValueError("now and baked_period must fit in int64")
+        n = self.size()
+        out = np.zeros(max(1, n), np.uint64)
+        total = int(check(self._L.sb200_fstore_find_baked(self._h, now, period, n, ptr(out))))
+        return out[:min(total, n)]
+
+    def associate_store(self, src, ids, remove=True):
+        """sb200_fstore_associate_store: fetch_tracks(ids) from the FeatureStore `src`, then associate them with this
+        store as one associate() call whose queries are those tracks (their kept rows, qualities, windows and merge
+        histories), each merged into its winner or added whole; remove=True then takes them out of `src`.  The rows
+        never leave the device.  Returns the associate dict."""
+        if not isinstance(src, FeatureStore):
+            raise TypeError("src must be an engine.FeatureStore")
+        ids = np.ascontiguousarray(ids, dtype=np.uint64)
+        q = len(ids)
+        out = {"counts": np.zeros(q, np.int32), "winners": np.zeros((q, self.topn), np.uint64),
+               "weights": np.zeros((q, self.topn), np.float64), "track_ids": np.zeros(q, np.uint64),
+               "merged": np.zeros(q, np.uint8)}
+        check(self._L.sb200_fstore_associate_store(self._h, src._h, q, ptr(ids), int(bool(remove)),
+                                                   *(ptr(v) for v in out.values())))
+        return out
+
     @staticmethod
     def _wasted_pending(tracker):
         """An upper bound of the records the next collection of `tracker` can return: every live track and every
