@@ -72,6 +72,9 @@ def lib():
             "ofs_merge_history": (i64, [vp, i32, vp, vp, i64, vp]),
             "ofs_find_baked": (i64, [vp, i64, i64, i64, vp]),
             "ofs_associate_store": (C.c_int, [vp, vp, i32, vp, i32, vp, vp, vp, vp, vp, i32]),
+            "ofs_set_classes": (C.c_int, [vp, i32, vp, vp]),
+            "ofs_use_class": (C.c_int, [vp, C.c_uint64]),
+            "ofs_class_counts": (i64, [vp, i32, vp, vp]),
         }
         for name, (res, args) in sig.items():
             fn = getattr(L, name)
@@ -128,7 +131,7 @@ class FeatureStore:
 
     def __init__(self, metric=EUCLIDEAN, distance_filter=100.0, max_observations=3, feature_dim=256, topn=1,
                  max_distance=100.0, min_votes=1, threads=1, gate=None, retention="newest", initial_capacity=4,
-                 merge_extension=1.5):
+                 merge_extension=1.5, classes=None):
         self._L = lib()
         self.K, self.D, self.topn, self.threads = int(max_observations), int(feature_dim), int(topn), int(threads)
         self._h = self._L.ofs_create(metric, distance_filter, self.K, self.D, self.topn, max_distance, min_votes)
@@ -144,6 +147,29 @@ class FeatureStore:
         if self._L.ofs_set_retention(self._h, RETENTIONS[retention], int(initial_capacity), float(merge_extension)):
             raise ValueError("invalid retention parameters")
         self._retention = (retention, int(initial_capacity), float(merge_extension))
+        self._classes = {0: self.D} if classes is None else {int(k): int(v) for k, v in dict(classes).items()}
+        cid = np.array(list(self._classes), np.uint64)
+        dims = np.array(list(self._classes.values()), np.int32)
+        if self._L.ofs_set_classes(self._h, len(cid), _p(cid), _p(dims)):
+            raise ValueError("invalid classes")
+        self._use(None)
+
+    def _use(self, feature_class):
+        """Selects the class of the next call (None: the first declared one)."""
+        c = next(iter(self._classes)) if feature_class is None else int(feature_class)
+        if c not in self._classes or self._L.ofs_use_class(self._h, c):
+            raise ValueError(f"feature_class {c} is not declared")
+        self.D = self._classes[c]
+
+    def classes(self):
+        return dict(self._classes)
+
+    def class_counts(self, ids):
+        """counts[n][len(classes())]: each track's rows per class, declared order (0 where not stored)."""
+        ids = np.ascontiguousarray(ids, dtype=np.uint64)
+        out = np.zeros((len(ids), len(self._classes)), np.int32)
+        self._L.ofs_class_counts(self._h, len(ids), _p(ids), _p(out))
+        return out
 
     def retention(self):
         """(rule, initial_capacity, merge_extension)."""
@@ -182,7 +208,8 @@ class FeatureStore:
             self._L.ofs_destroy(self._h)
             self._h = None
 
-    def add(self, ids, features, sources=None, t_start=None, t_end=None, quality=None):
+    def add(self, ids, features, sources=None, t_start=None, t_end=None, quality=None, feature_class=None):
+        self._use(feature_class)
         ids = np.ascontiguousarray(ids, dtype=np.uint64)
         f = np.ascontiguousarray(features, dtype=np.float32).reshape(len(ids), self.D)
         a = self._attrs(len(ids), sources, t_start, t_end)
@@ -204,7 +231,8 @@ class FeatureStore:
                "weights": np.zeros((q, self.topn), np.float64)}
         return ids, offs, f, out
 
-    def search(self, ids, offsets, features, sources=None, t_start=None, t_end=None, quality=None):
+    def search(self, ids, offsets, features, sources=None, t_start=None, t_end=None, quality=None, feature_class=None):
+        self._use(feature_class)
         ids, offs, f, out = self._queries(ids, offsets, features)
         a = self._attrs(len(ids), sources, t_start, t_end)
         q = self._quality(len(f), quality)
@@ -222,7 +250,8 @@ class FeatureStore:
             raise ValueError("invalid search request")
         return out
 
-    def associate(self, ids, offsets, features, sources=None, t_start=None, t_end=None, quality=None):
+    def associate(self, ids, offsets, features, sources=None, t_start=None, t_end=None, quality=None, feature_class=None):
+        self._use(feature_class)
         ids, offs, f, out = self._queries(ids, offsets, features)
         a = self._attrs(len(ids), sources, t_start, t_end)
         q = self._quality(len(f), quality)
@@ -241,8 +270,9 @@ class FeatureStore:
             raise ValueError("invalid associate request")
         return out
 
-    def search_owned(self, ids, each=False):
+    def search_owned(self, ids, each=False, feature_class=None):
         """owned_track_distances + TopNVoting::winners for stored tracks; each=True: once per id."""
+        self._use(feature_class)
         ids = np.ascontiguousarray(ids, dtype=np.uint64)
         q = len(ids)
         out = {"counts": np.zeros(q, np.int32), "winners": np.zeros((q, self.topn), np.uint64),
@@ -262,15 +292,17 @@ class FeatureStore:
         if self._L.ofs_merge_owned(self._h, len(d), _p(d), _p(s), int(bool(remove))):
             raise ValueError("invalid merge request")
 
-    def fetch(self, ids, remove=False):
+    def fetch(self, ids, remove=False, feature_class=None):
+        self._use(feature_class)
         ids = np.ascontiguousarray(ids, dtype=np.uint64)
         counts = np.zeros(len(ids), np.int32)
         feats = np.zeros((len(ids), self.K, self.D), np.float32)
         self._L.ofs_fetch(self._h, len(ids), _p(ids), int(bool(remove)), _p(counts), _p(feats))
         return counts, feats
 
-    def fetch_quality(self, ids, remove=False):
+    def fetch_quality(self, ids, remove=False, feature_class=None):
         """(counts, features, qualities[n][K]) of a quality store, rows in the track's order (best first)."""
+        self._use(feature_class)
         ids = np.ascontiguousarray(ids, dtype=np.uint64)
         counts = np.zeros(len(ids), np.int32)
         feats = np.zeros((len(ids), self.K, self.D), np.float32)
@@ -308,10 +340,12 @@ class FeatureStore:
             raise ValueError("find_baked() needs a gated store")
         return out[:total]
 
-    def associate_store(self, src, ids, remove=True):
+    def associate_store(self, src, ids, remove=True, feature_class=None):
         """fetch_tracks(ids) of the oracle store `src`, then one associate of this store with those tracks as its
         queries (each merged into its winner with its list and history, or added whole); remove=True takes them out of
         `src`.  Returns the associate dict."""
+        self._use(feature_class)
+        src._use(feature_class)
         ids = np.ascontiguousarray(ids, dtype=np.uint64)
         q = len(ids)
         out = {"counts": np.zeros(q, np.int32), "winners": np.zeros((q, self.topn), np.uint64),

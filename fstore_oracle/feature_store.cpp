@@ -24,7 +24,13 @@
 // by quality, descending, and truncated to c(h) = min(K, (u64)((float)initial_capacity * powf(merge_extension, (float)h)))
 // with h the track's history length (:257-265).  Queries are fresh tracks (h = 1) built the same way, or, in
 // ofs_associate_store, stored tracks of another store, which bring their lists and histories whole.
+// Feature classes (ofs_set_classes): each track keeps its rows by class (Track::observations, a class -> rows map).  The
+// rows of the selected class (ofs_use_class) are the track's obs / q, the others wait in its `cls` map; every call that
+// takes rows works on the selected class, and a track without rows of it gives no entries (Track::distances'
+// ObservationForClassNotFound).  A merge (Track::merge with classes = None) walks the classes the source holds in
+// ascending id; on a quality store each class step appends the source's history before it optimizes that class.
 #include <algorithm>
+#include <map>
 #include <cmath>
 #include <cstdint>
 #include <cstring>
@@ -106,8 +112,14 @@ void parallel_for(int n, int threads, const std::function<void(int, int)>& fn) {
   for (auto& x : th) x.join();
 }
 
+struct Rows {
+  std::vector<std::vector<float>> obs;
+  std::vector<float> q;
+};
+
 struct Track {
   uint64_t id;
+  std::map<uint64_t, Rows> cls;          // the rows of the classes other than the selected one
   std::vector<std::vector<float>> obs;   // zero-padded to d8, oldest first (a quality store: the track's order)
   uint64_t src = 0;                      // attributes of a gated store
   int64_t t0 = 0, t1 = 0;
@@ -127,6 +139,15 @@ struct ofs_store {
   std::vector<int> cap_tab;   // retention 1: c(h) for h = 0 .. the first h with c(h) == K (or h = 0 alone when constant)
   std::vector<Track> tracks;
   std::unordered_map<uint64_t, size_t> pos;
+  std::vector<std::pair<uint64_t, int>> classes{{0, 0}};   // declared (id, dim); {0, feature_dim} by default
+  uint64_t cur = 0;                                         // the selected class
+
+  // the rows of class k of track t (the selected class's are t.obs / t.q)
+  std::pair<std::vector<std::vector<float>>*, std::vector<float>*> rows(Track& t, uint64_t k) const {
+    if (k == cur) return {&t.obs, &t.q};
+    Rows& r = t.cls[k];
+    return {&r.obs, &r.q};
+  }
 
   // CamTrackingAttributes::compatible (examples/track_merging.rs:222-225); always true without a gate
   bool compatible(const Track& a, const Track& b) const {
@@ -151,24 +172,39 @@ struct ofs_store {
   // retention 1: c(h), from the table the first h with c(h) == K ends (a constant capacity has one entry)
   int capacity(size_t h) const { return cap_tab[std::min(h, cap_tab.size() - 1)]; }
   // retention 1: optimize, the stable sort by quality, descending (-0.0 == +0.0), then the truncation to c(h)
-  void keep_best(Track& t) const {
-    std::vector<size_t> ix(t.obs.size());
+  void keep_best(std::vector<std::vector<float>>& to, std::vector<float>& tq, size_t h) const {
+    std::vector<size_t> ix(to.size());
     for (size_t i = 0; i < ix.size(); ++i) ix[i] = i;
-    std::stable_sort(ix.begin(), ix.end(), [&](size_t a, size_t b) { return t.q[a] > t.q[b]; });
-    ix.resize(std::min(ix.size(), (size_t)capacity(t.hist.size())));
+    std::stable_sort(ix.begin(), ix.end(), [&](size_t a, size_t b) { return tq[a] > tq[b]; });
+    ix.resize(std::min(ix.size(), (size_t)capacity(h)));
     std::vector<std::vector<float>> obs;
     std::vector<float> q;
-    for (size_t i : ix) { obs.push_back(std::move(t.obs[i])); q.push_back(t.q[i]); }
-    t.obs.swap(obs);
-    t.q.swap(q);
+    for (size_t i : ix) { obs.push_back(std::move(to[i])); q.push_back(tq[i]); }
+    to.swap(obs);
+    tq.swap(q);
   }
-  // Track::merge: dest ++ src, and a quality store's history and optimize
-  void merge_into(Track& d, const Track& src) const {
-    d.obs.insert(d.obs.end(), src.obs.begin(), src.obs.end());
-    if (!retention) { keep_newest(d.obs); return; }
-    d.q.insert(d.q.end(), src.q.begin(), src.q.end());
-    d.hist.insert(d.hist.end(), src.hist.begin(), src.hist.end());
-    keep_best(d);
+  void keep_best(Track& t) const { keep_best(t.obs, t.q, t.hist.size()); }
+  // Track::merge with classes = None: for each class src holds, in ascending id, dest's rows ++ src's, then (a quality
+  // store) the history dest ++ src and optimize of that class at the new capacity; a newest store keeps the newest K
+  void merge_into(Track& d, const Track& src_track) const {
+    Track src = src_track;
+    std::vector<uint64_t> ids;
+    for (const auto& c : classes) ids.push_back(c.first);
+    std::sort(ids.begin(), ids.end());
+    for (uint64_t k : ids) {
+      auto so = rows(src, k);
+      if (so.first->empty()) continue;
+      auto dr = rows(d, k);
+      dr.first->insert(dr.first->end(), so.first->begin(), so.first->end());
+      if (!retention) { keep_newest(*dr.first); continue; }
+      dr.second->insert(dr.second->end(), so.second->begin(), so.second->end());
+      d.hist.insert(d.hist.end(), src.hist.begin(), src.hist.end());
+      keep_best(*dr.first, *dr.second, d.hist.size());
+    }
+  }
+  // rows of every declared class of t, in declared order
+  void class_counts(Track& t, int32_t* out) const {
+    for (size_t k = 0; k < classes.size(); ++k) out[k] = (int32_t)rows(t, classes[k].first).first->size();
   }
   // add_observation + optimize of one row
   void append(Track& t, const float* feat, float quality) const {
@@ -262,6 +298,64 @@ struct ofs_store {
 
 extern "C" {
 
+// The classes (n ids, each with its dim) of an empty store; the first is selected.  -1 for a bad n, a repeated id, a
+// dim out of 1..8192 or a store that holds tracks.
+int ofs_set_classes(ofs_store* s, int n, const uint64_t* ids, const int32_t* dims) {
+  if (n < 1 || n > 16 || !s->tracks.empty()) return -1;
+  for (int i = 0; i < n; ++i) {
+    if (dims[i] < 1 || dims[i] > 8192) return -1;
+    for (int j = 0; j < i; ++j)
+      if (ids[j] == ids[i]) return -1;
+  }
+  s->classes.clear();
+  for (int i = 0; i < n; ++i) s->classes.push_back({ids[i], dims[i]});
+  s->cur = ids[0];
+  s->D = dims[0];
+  s->d8 = (dims[0] + 7) / 8 * 8;
+  return 0;
+}
+
+// selects class `id` for the calls that take rows; -1 for an id the store does not declare
+int ofs_use_class(ofs_store* s, uint64_t id) {
+  int dim = 0;
+  for (const auto& c : s->classes)
+    if (c.first == id) dim = c.second;
+  if (!dim) return -1;
+  if (id == s->cur) return 0;
+  for (Track& t : s->tracks) {
+    Rows& old = t.cls[s->cur];
+    old.obs.swap(t.obs);
+    old.q.swap(t.q);
+    if (old.obs.empty()) t.cls.erase(s->cur);
+    auto it = t.cls.find(id);
+    t.obs.clear();
+    t.q.clear();
+    if (it != t.cls.end()) {
+      t.obs.swap(it->second.obs);
+      t.q.swap(it->second.q);
+      t.cls.erase(it);
+    }
+  }
+  s->cur = id;
+  s->D = dim;
+  s->d8 = (dim + 7) / 8 * 8;
+  return 0;
+}
+
+// counts[i][k]: the rows of track ids[i] in declared class k (0 when not stored); returns the ids found
+int64_t ofs_class_counts(ofs_store* s, int n, const uint64_t* ids, int32_t* counts) {
+  int64_t found = 0;
+  const size_t nc = s->classes.size();
+  for (int i = 0; i < n; ++i) {
+    auto it = s->pos.find(ids[i]);
+    std::fill(counts + (size_t)i * nc, counts + (size_t)(i + 1) * nc, 0);
+    if (it == s->pos.end()) continue;
+    s->class_counts(s->tracks[it->second], counts + (size_t)i * nc);
+    ++found;
+  }
+  return found;
+}
+
 ofs_store* ofs_create(int metric, float distance_filter, int max_observations, int feature_dim, int topn,
                       float max_distance, int min_votes) {
   if ((metric != 0 && metric != 1) || max_observations < 1 || feature_dim < 1 || topn < 1) return nullptr;
@@ -271,6 +365,7 @@ ofs_store* ofs_create(int metric, float distance_filter, int max_observations, i
   s->K = max_observations;
   s->D = feature_dim;
   s->d8 = (feature_dim + 7) / 8 * 8;
+  s->classes = {{0, feature_dim}};
   s->topn = topn;
   s->max_distance = max_distance;
   s->min_votes = min_votes;
@@ -662,7 +757,10 @@ int64_t ofs_find_baked(ofs_store* s, int64_t now, int64_t baked_period, int64_t 
 // retention or retention parameters, n < 0, remove not 0 / 1, an id twice, not stored in src, or stored in dst.
 int ofs_associate_store(ofs_store* d, ofs_store* s, int n, const uint64_t* ids, int remove, int32_t* counts,
                         uint64_t* winners, double* weights, uint64_t* track_ids, uint8_t* merged, int threads) {
-  if (d == s || d->D != s->D || d->K != s->K || d->gate != s->gate || d->retention != s->retention) return -1;
+  auto sorted = [](std::vector<std::pair<uint64_t, int>> c) { std::sort(c.begin(), c.end()); return c; };
+  if (d == s || sorted(d->classes) != sorted(s->classes) || d->cur != s->cur || d->K != s->K || d->gate != s->gate ||
+      d->retention != s->retention)
+    return -1;
   if (d->retention && (d->init_cap != s->init_cap || d->ext != s->ext)) return -1;
   if (n < 0 || (remove != 0 && remove != 1)) return -1;
   std::unordered_set<uint64_t> seen;

@@ -549,11 +549,51 @@ int sb200_fstore_search_owned(sb200_fstore* s, int32_t n, const uint64_t* ids, i
  * remove) when remove_src.  SB200_ERR_INVALID, before anything changes, for dest == src (the reference's TrackNotFound:
  * it fetched src first), a dest or src that is not stored, and, with remove_src, a pair that names a track an earlier
  * pair removed; the reference would apply the pairs in front and then return the error, the same deviation as
- * sb200_fstore_associate's.  `classes` has no counterpart: there is one feature class; a newest store keeps no merge
- * history, a quality store (sb200_fstore_set_retention) merges with merge_history = true and its rule.
+ * sb200_fstore_associate's.  `classes` is the reference's None: every feature class the source holds, walked in
+ * ascending class id (the reference walks a HashMap; this order is the store's own, as the store order and the TopN tie
+ * order are).  A newest store keeps no merge history; a quality store (sb200_fstore_set_retention) merges with
+ * merge_history = true and its rule, each class step appending the source's history before it truncates that class's
+ * list, so a source holding m classes appends its history m times and class step j truncates at
+ * c(h_dest + j * h_src).  On a gated store the windows' hull is taken once per pair.
  * sb200_fstore_last_stage_ms reports the row moves as the apply stage. */
 int sb200_fstore_merge_owned(sb200_fstore* s, int32_t n, const uint64_t* dest_ids, const uint64_t* src_ids,
                              int32_t remove_src);
+
+/* Feature classes (the reference's `feature_class` of TrackStore::add, foreign_track_distances, owned_track_distances
+ * and Track::get_feature_classes, src/track/store.rs, src/track.rs).  A store declares its n classes (1..16, distinct
+ * ids, each with its own feature_dim in 1..8192) once, while it holds no tracks; a new store has one class, id 0, of the
+ * options' feature_dim.  max_observations, the storage type, the gate and the retention rule are store-wide.  Capacity
+ * is shared: every class holds cap * max_observations rows of its own dim, also for tracks without rows in it, so a
+ * class costs its rows' device memory whether few or all tracks hold it.  SB200_ERR_INVALID for a bad n, a repeated
+ * id, a dim out of range or a store that holds tracks. */
+#define SB200_FSTORE_MAX_CLASSES 16
+int sb200_fstore_set_classes(sb200_fstore* s, int32_t n, const uint64_t* class_ids, const int32_t* feature_dims);
+/* The declared classes in declared order: the first min(cap, n) ids and dims; returns n. */
+int32_t sb200_fstore_get_classes(sb200_fstore* s, int32_t cap, uint64_t* class_ids, int32_t* feature_dims);
+/* Selects the class of every later call that takes or returns rows: add, search and associate in every form, fetch,
+ * fetch_quality, search_owned, associate_wasted and associate_store.  Handle state, like sb200_fstore_set_feature_type:
+ * a new or loaded store selects its first declared class.  The row length of those calls' feature columns is the
+ * selected class's dim, and sb200_fstore_get_options reports it as feature_dim.  Per call on class c:
+ *   - add: an unknown id creates a track whose other classes are empty; a known id appends to class c under the
+ *     store's rule (a quality store: at the track's c(h); the history does not change).
+ *   - search / associate: a stored track without class-c rows gives no entries (the reference's
+ *     ObservationForClassNotFound): it does not vote and does not raise max_dist.  A merged query extends its winner's
+ *     class c alone (a quality store extends the history once); a query that becomes a new track holds class c alone.
+ *   - search_owned: a queried track without class-c rows gets count 0.
+ *   - fetch / fetch_quality: class c's rows; counts[i] can be 0 for a stored track, and the return value still counts
+ *     the stored ids.  With remove the whole track leaves, every class with it: read the other classes' rows first.
+ *   - associate_wasted: refused unless class c's dim is the tracker's feature dim.
+ *   - associate_store: the queries are src's class-c rows; a queried track without them has no results and is added
+ *     whole.  A merged query then moves every class it holds into its winner, in ascending class id, each class step
+ *     on a quality store appending the query's history as merge_owned's does; a new track keeps every class.  Both
+ *     stores must declare the same class ids with the same dims.
+ * merge_owned moves every class (see there); find_baked, the attributes, merge histories, ids and size do not depend on
+ * the class.  SB200_ERR_INVALID for an id the store does not declare. */
+int sb200_fstore_use_class(sb200_fstore* s, uint64_t class_id);
+/* counts[i][k] (n rows of get_classes' n entries, declared order): the rows of track ids[i] in class k, 0 in every
+ * class for an id that is not stored; the reference's get_feature_classes with their lengths.  One gather kernel.
+ * Returns the number of ids found. */
+int64_t sb200_fstore_class_counts(sb200_fstore* s, int32_t n, const uint64_t* ids, int32_t* counts);
 
 /* The TrackStore side of examples/track_merging.rs for the visual trackers: a collection of tracker `t`'s wasted records
  * whose feature histories go into store `s` without leaving the device.
@@ -839,6 +879,45 @@ typedef struct {
   uint64_t sec_off[SB200_FSTORE_BLOB_SECTIONS_V3];
   uint64_t sec_bytes[SB200_FSTORE_BLOB_SECTIONS_V3];
 } sb200_fstore_blob_header_v3;
+/* The blob of a store of several feature classes, or of one class whose id is not 0: version 4, this header (the
+ * version-3 fields, with gate and retention NONE allowed, then n_classes; feature_dim and d8 are the first declared
+ * class's), then 8 + 4 * n_classes sections laid out as version 1's:
+ *   shared: ids, source, t_start, t_end (0 bytes each on an ungated store), history_length, history (0 bytes each on a
+ *   newest store);
+ *   the class table: class_ids[n_classes] (u64), class_dims[n_classes] (i32), in declared order;
+ *   per class, in declared order: cnt[live], start[live], feat[live][max_observations][d8 of the class] and
+ *   quality[live][max_observations] (0 bytes on a newest store).
+ * A store of the single class 0 (every store that never declared other classes) writes version 1, 2 or 3 byte for byte
+ * as before, and those blobs load as one class of id 0.  Load also refuses a version-4 blob with n_classes outside
+ * 1..16, a class id twice or a dim outside 1..8192, and, by kernel, a cnt outside [0, max_observations], a start
+ * outside [0, max_observations) or a track without a row in any class; a quality store's checks of version 3 hold per
+ * class. */
+#define SB200_FSTORE_BLOB_VERSION_CLASSES 4u
+#define SB200_FSTORE_BLOB_SECTIONS_V4 (8 + 4 * SB200_FSTORE_MAX_CLASSES)
+typedef struct {
+  uint32_t magic;
+  uint32_t version; /* SB200_FSTORE_BLOB_VERSION_CLASSES */
+  uint64_t total_bytes;
+  int32_t metric;
+  float distance_filter;
+  int32_t max_observations;
+  int32_t feature_dim;
+  int32_t topn;
+  float max_distance;
+  int32_t min_votes;
+  int32_t d8;
+  int32_t feature_type;
+  int32_t storage_type;
+  int64_t live;
+  int32_t gate;             /* SB200_FSTORE_GATE_* */
+  int32_t retention;        /* SB200_FSTORE_KEEP_* */
+  int32_t initial_capacity;
+  float merge_extension;
+  int32_t n_classes;
+  int32_t reserved;         /* 0 */
+  uint64_t sec_off[SB200_FSTORE_BLOB_SECTIONS_V4];
+  uint64_t sec_bytes[SB200_FSTORE_BLOB_SECTIONS_V4];
+} sb200_fstore_blob_header_v4;
 /* Writes the blob to `buf` (`cap` bytes; host memory, or device memory on any device) and its size to *bytes.
  * buf == NULL: reports the size and writes nothing.  SB200_ERR_CAPACITY when cap is too small: nothing is written and
  * *bytes is still set.  Rows are copied, not re-derived; the store is not changed.  Timers and the stream are not part

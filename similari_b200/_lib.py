@@ -181,6 +181,7 @@ EXPORTS = [
     "sb200_fstore_set_retention", "sb200_fstore_get_retention", "sb200_fstore_add_quality",
     "sb200_fstore_search_quality", "sb200_fstore_associate_quality", "sb200_fstore_fetch_quality",
     "sb200_fstore_merge_history", "sb200_fstore_find_baked", "sb200_fstore_associate_store",
+    "sb200_fstore_set_classes", "sb200_fstore_get_classes", "sb200_fstore_use_class", "sb200_fstore_class_counts",
 ]
 
 
@@ -298,6 +299,10 @@ def lib():
         "sb200_fstore_merge_history": (i64, [vp, i32, vp, vp, i64, vp]),
         "sb200_fstore_find_baked": (i64, [vp, i64, i64, i64, vp]),
         "sb200_fstore_associate_store": (C.c_int, [vp, vp, i32, vp, i32, vp, vp, vp, vp, vp]),
+        "sb200_fstore_set_classes": (C.c_int, [vp, i32, vp, vp]),
+        "sb200_fstore_get_classes": (i32, [vp, i32, vp, vp]),
+        "sb200_fstore_use_class": (C.c_int, [vp, u64]),
+        "sb200_fstore_class_counts": (i64, [vp, i32, vp, vp]),
         "sb200_fstore_get_storage_type": (C.c_int, [vp, C.POINTER(i32)]),
         "sb200_fstore_associate_wasted": (i64, [vp, vp, i64, u64, vp, vp, vp, vp, vp, vp, i32, vp, vp, vp, vp, vp, vp, vp,
                                                 vp, vp, vp]),

@@ -532,16 +532,18 @@ class _VisualBase(_TrackerBase):
                                       w["features"][i], w["feature_present"][i])
                 for i in range(len(w["ids"]))]
 
-    def wasted_to_store(self, store: engine.FeatureStore, id_offset=0) -> List[Tuple[WastedSortTrack, Optional[int]]]:
+    def wasted_to_store(self, store: engine.FeatureStore, id_offset=0,
+                        feature_class=None) -> List[Tuple[WastedSortTrack, Optional[int]]]:
         """Collects the wasted tracks as wasted() does and associates each one's observed features (the present ones,
         oldest first) with the feature track `store` under the id track.id + id_offset, as one
         FeatureStore.associate call would, without the features leaving the device (the TrackStore side of the
         reference's examples/track_merging.rs).  Returns [(track, where it went in the store)], the store track id
-        being None for a track without a feature; the box histories are those wasted() reports.  An extension with no
-        PyO3 counterpart in the reference."""
+        being None for a track without a feature; the box histories are those wasted() reports.  feature_class: the
+        store's class the features go to (None: its first declared class).  An extension with no PyO3 counterpart in the
+        reference."""
         if self._t is None:
             return []
-        w = store.associate_wasted(self._t, id_offset=id_offset)
+        w = store.associate_wasted(self._t, id_offset=id_offset, feature_class=feature_class)
         return [(WastedSortTrack(w["ids"][i], w["epochs"][i], Universal2DBox._from_row(w["predicted"][i]),
                                  Universal2DBox._from_row(w["observed"][i]), w["scene_ids"][i], w["lengths"][i],
                                  [Universal2DBox._from_row(r) for r in w["predicted_history"][i]],

@@ -109,8 +109,35 @@ enum { kSecIds, kSecCnt, kSecStart, kSecFeat, kSecSrc, kSecT0, kSecT1, kSecQual,
 static_assert(offsetof(BlobHeaderV2, live) == offsetof(BlobHeader, live), "version 2 repeats version 1's fields");
 static_assert(offsetof(BlobHeaderV3, gate) == offsetof(BlobHeaderV2, gate), "version 3 repeats version 2's fields");
 static_assert(kSecHist + 1 == SB200_FSTORE_BLOB_SECTIONS_V3, "the version-3 section table");
+using BlobHeaderV4 = sb200_fstore_blob_header_v4;
+static_assert(offsetof(BlobHeaderV4, merge_extension) == offsetof(BlobHeaderV3, merge_extension),
+              "version 4 repeats version 3's fields");
+static_assert(SB200_FSTORE_MAX_CLASSES == sb::kFsMaxClasses, "the class bound of the kernels");
+// version 4: the shared sections, the class table, then kV4PerClass sections per class from kV4Class
+enum { kV4Ids, kV4Src, kV4T0, kV4T1, kV4Hlen, kV4Hist, kV4ClassIds, kV4ClassDims, kV4Class };
+enum { kV4Cnt, kV4Start, kV4Feat, kV4Qual, kV4PerClass };
+constexpr const char* kV4Names[kV4Class + kV4PerClass] = {"ids", "source", "t_start", "t_end", "history_length", "history",
+                                                          "class_ids", "class_dims", "cnt", "start", "feat", "quality"};
+// The version-4 sections of a store of `live` tracks with the n class dims `dims`: their bytes (which save writes and
+// load expects, the history's from hist_total) and names; returns their number.
+int sections_v4(uint64_t live, int K, int stype, int gate, int keep, int n, const int32_t* dims, uint64_t hist_total,
+                uint64_t* bytes, const char** names) {
+  const uint64_t g = gate ? live * 8 : 0;
+  const uint64_t sh[kV4Class] = {live * 8, g, g, g, keep ? live * 4 : 0, keep ? hist_total * 8 : 0, (uint64_t)n * 8,
+                                 (uint64_t)n * 4};
+  for (int i = 0; i < kV4Class; ++i) { bytes[i] = sh[i]; names[i] = kV4Names[i]; }
+  for (int k = 0; k < n; ++k) {
+    const uint64_t d8 = (uint64_t)(dims[k] + 7) / 8 * 8, at = kV4Class + (uint64_t)kV4PerClass * k;
+    const uint64_t pc[kV4PerClass] = {live * 4, live * 4, live * K * d8 * (stype == SB200_FEATURE_F32 ? 4 : 2),
+                                      keep ? live * K * 4 : 0};
+    for (int j = 0; j < kV4PerClass; ++j) { bytes[at + j] = pc[j]; names[at + j] = kV4Names[kV4Class + j]; }
+  }
+  return kV4Class + kV4PerClass * n;
+}
 // the store kinds that have a column (sb200_fstore::Col::need)
 enum { kNeedAll, kNeedGate, kNeedQuality };
+// which columns a step of alloc / swap_columns handles: every one, the shared ones, or the selected class's
+enum { kPartAll, kPartShared, kPartClass };
 
 // The queries of associate_store, which its row source puts on the device besides the rows: their triples in qattr (a
 // gated store) and their rows' qualities in dqr (a quality store).  hq[Q]: their history lengths on the device, and
@@ -196,11 +223,22 @@ struct sb200_fstore {
   // A store column: its buffer, bytes per track (0: K stored rows) or per slot (per_obs), the kind of store that has it
   // (kNeed*), whether allocation zero-fills it, and its blob section (kSec*) and name.  Without a section (-1) it is
   // scratch, which growth and compaction start afresh.
-  struct Col { DBuf sb200_fstore::*buf; uint32_t w; bool per_obs; int need; bool zero; int sec; const char* name; };
+  // Per-class columns (per_class) exist once per declared feature class; the selected class's sit in the members above
+  // and the others' in cls (select).
+  struct Col {
+    DBuf sb200_fstore::*buf; uint32_t w; bool per_obs; int need; bool zero; int sec; const char* name; bool per_class;
+  };
   static constexpr int kNumCols = 10;
   static const Col kCols[kNumCols];
+  // Feature classes (sb200_fstore_set_classes), in declared order.  Capacity is shared, so every class holds its feat
+  // [cap][K][d8_c], cnt, start and (quality store) qual columns; cls[sel]'s buffers are empty while it is selected, its
+  // columns being the members feat, cnt, start and qual, and d8 / o.feature_dim being its own.
+  struct ClassCols { uint64_t id; int dim, d8; DBuf feat, cnt, start, qual; };
+  std::vector<ClassCols> cls;
+  int sel = 0;
   DBuf qattr;                                // a gated call's triples, [n] of each column
   DBuf sq;                                   // associate_store: the queried src positions [n], history lengths [n]
+  DBuf dinc;                                 // associate_store, quality store of classes: history increments [n]
   std::vector<uint64_t> hid;                 // ids in store order
   std::unordered_map<uint64_t, int> hpos;    // id -> store position
   // per-call buffers
@@ -260,13 +298,18 @@ struct sb200_fstore {
     return n;
   }
 
+  static bool in_part(const Col& c, int part) {
+    return part == kPartAll || (part == kPartClass) == c.per_class;
+  }
+
   // fresh columns of this store for max(n, 1) tracks in nw[] (one per kCols entry; only != kNeedAll: the columns of
-  // that kind of store alone), zero-filled where the table says so; the caller copies what it keeps
-  int alloc(size_t n, DBuf* nw, int only = kNeedAll) {
+  // that kind of store alone; part: kPartShared / kPartClass, the shared ones or the selected class's alone),
+  // zero-filled where the table says so; the caller copies what it keeps
+  int alloc(size_t n, DBuf* nw, int only = kNeedAll, int part = kPartAll) {
     n = std::max<size_t>(n, 1);
     for (int k = 0; k < kNumCols; ++k) {
       const Col& c = kCols[k];
-      if (!has(c) || (only != kNeedAll && c.need != only)) continue;
+      if (!has(c) || (only != kNeedAll && c.need != only) || !in_part(c, part)) continue;
       const size_t bytes = n * track_bytes(c);
       if (int rc = nw[k].ensure(bytes)) return rc;
       if (c.zero) CU(cudaMemsetAsync(nw[k].p, 0, bytes, st));
@@ -274,16 +317,136 @@ struct sb200_fstore {
     return 0;
   }
 
-  // exchanges the store's columns with nw[] (only != kNeedAll: the columns of that kind of store alone)
-  void swap_columns(DBuf* nw, int only = kNeedAll) {
+  // exchanges the store's columns with nw[] (only, part: as for alloc)
+  void swap_columns(DBuf* nw, int only = kNeedAll, int part = kPartAll) {
     for (int k = 0; k < kNumCols; ++k)
-      if (only == kNeedAll || kCols[k].need == only) std::swap(this->*kCols[k].buf, nw[k]);
+      if ((only == kNeedAll || kCols[k].need == only) && in_part(kCols[k], part)) std::swap(this->*kCols[k].buf, nw[k]);
+  }
+
+  // ---- feature classes
+  // exchanges the per-class members with class k's parked buffers
+  void swap_class(int k) {
+    ClassCols& c = cls[k];
+    std::swap(feat, c.feat);
+    std::swap(cnt, c.cnt);
+    std::swap(start, c.start);
+    std::swap(qual, c.qual);
+  }
+  // makes class k the one whose columns the members (and view()) are
+  void select(int k) {
+    if (k == sel) return;
+    swap_class(sel);
+    swap_class(k);
+    sel = k;
+    d8 = cls[k].d8;
+    o.feature_dim = cls[k].dim;
+  }
+  // runs f(k) with each class k selected in turn, in `order` (default: declared order), then selects the class
+  // selected before; stops at the first nonzero return
+  template <class F> int each_class(F f, const std::vector<int>* order = nullptr) {
+    const int s0 = sel;
+    int rc = 0;
+    for (int i = 0; i < (int)cls.size() && !rc; ++i) {
+      const int k = order ? (*order)[i] : i;
+      select(k);
+      rc = f(k);
+    }
+    select(s0);
+    return rc;
+  }
+  // the class indices in ascending class id: the order in which a merge walks a source's classes
+  std::vector<int> ascending_classes() const {
+    std::vector<int> ix(cls.size());
+    std::iota(ix.begin(), ix.end(), 0);
+    std::sort(ix.begin(), ix.end(), [&](int a, int b) { return cls[a].id < cls[b].id; });
+    return ix;
+  }
+  int class_index(uint64_t id) const {
+    for (size_t k = 0; k < cls.size(); ++k)
+      if (cls[k].id == id) return (int)k;
+    return -1;
+  }
+  // the store holds one class, id 0: the blob is a version 1 to 3 one
+  bool plain_classes() const { return cls.size() == 1 && cls[0].id == 0; }
+
+  int set_classes(int n, const uint64_t* idv, const int32_t* dims) {
+    if (n < 1 || n > SB200_FSTORE_MAX_CLASSES) return fail(SB200_ERR_INVALID, "n must lie in 1..%d", SB200_FSTORE_MAX_CLASSES);
+    if (!idv || !dims) return fail(SB200_ERR_INVALID, "class_ids / feature_dims is NULL");
+    for (int i = 0; i < n; ++i) {
+      if (dims[i] < 1 || dims[i] > SB200_FSTORE_MAX_DIM)
+        return fail(SB200_ERR_INVALID, "class %llu: feature_dim %d outside 1..%d", (unsigned long long)idv[i], dims[i],
+                    SB200_FSTORE_MAX_DIM);
+      for (int j = 0; j < i; ++j)
+        if (idv[j] == idv[i]) return fail(SB200_ERR_INVALID, "class id %llu appears twice", (unsigned long long)idv[i]);
+    }
+    if (!hid.empty()) return fail(SB200_ERR_INVALID, "the classes are fixed while the store holds tracks (%zu)", hid.size());
+    CU(cudaSetDevice(o.device));
+    CU(cudaStreamSynchronize(st));
+    // no track is stored: every class starts without columns, and the next reserve allocates all columns afresh
+    swap_class(sel);
+    std::vector<ClassCols> nc(n);
+    for (int i = 0; i < n; ++i) {
+      nc[i].id = idv[i];
+      nc[i].dim = dims[i];
+      nc[i].d8 = (dims[i] + 7) / 8 * 8;
+    }
+    cls.swap(nc);
+    sel = 0;
+    swap_class(0);
+    d8 = cls[0].d8;
+    o.feature_dim = cls[0].dim;
+    cap = 0;
+    return 0;
+  }
+
+  int use_class(uint64_t id) {
+    const int k = class_index(id);
+    if (k < 0) return fail(SB200_ERR_INVALID, "the store declares no class %llu", (unsigned long long)id);
+    select(k);
+    return 0;
+  }
+
+  // every class's cnt and start columns, in declared order, as the class kernels read them
+  sb::FsClassCols class_cols() {
+    sb::FsClassCols cc{};
+    cc.n = (int)cls.size();
+    each_class([&](int k) {
+      cc.cnt[k] = cnt.as<int>();
+      cc.start[k] = start.as<int>();
+      return 0;
+    });
+    return cc;
+  }
+
+  // counts[i][k]: the rows of track ids[i] in class k (0 for an id that is not stored); returns the ids found
+  int64_t class_counts(int n, const uint64_t* idv, int32_t* counts) {
+    if (n < 0) return fail(SB200_ERR_INVALID, "n < 0");
+    if (n > 0 && (!idv || !counts)) return fail(SB200_ERR_INVALID, "ids / counts is NULL");
+    if (int rc = begin()) return rc;
+    if (n == 0) return 0;
+    std::vector<int> pos(n, -1);
+    int64_t found = 0;
+    for (int i = 0; i < n; ++i) {
+      auto it = hpos.find(idv[i]);
+      if (it != hpos.end()) { pos[i] = it->second; ++found; }
+    }
+    const size_t out = (size_t)n * cls.size();
+    if (int rc = gpos.ensure((size_t)n * 4)) return rc;
+    if (int rc = gout.ensure(out * 4)) return rc;
+    CU(cudaMemcpyAsync(gpos.p, pos.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
+    sb::fs_launch_class_counts(class_cols(), gpos.as<int>(), n, gout.as<int>(), st);
+    CU(cudaMemcpyAsync(counts, gout.p, out * 4, cudaMemcpyDeviceToHost, st));
+    if (int rc = finish()) return rc;
+    return found;
   }
 
   // the tracks every column holds as allocated, at most cap (after a storage type change: in rows of the new type)
-  size_t held() const {
+  size_t held() {
     size_t n = cap;
-    for (const Col& c : kCols) if (has(c)) n = std::min(n, (this->*c.buf).bytes / track_bytes(c));
+    each_class([&](int) {
+      for (const Col& c : kCols) if (has(c)) n = std::min(n, (this->*c.buf).bytes / track_bytes(c));
+      return 0;
+    });
     return n;
   }
 
@@ -295,15 +458,21 @@ struct sb200_fstore {
   int reserve(size_t need) {
     if (need <= cap) return 0;
     const size_t nc = std::max(need, cap + cap / 2);
+    if (int rc = each_class([&](int) { return grow(nc, kPartClass); })) return rc;
+    if (int rc = grow(nc, kPartShared)) return rc;
+    cap = nc;
+    return 0;
+  }
+  // reserve's step for the columns of `part`
+  int grow(size_t nc, int part) {
     DBuf nw[kNumCols];
-    if (int rc = alloc(nc, nw)) return rc;
+    if (int rc = alloc(nc, nw, kNeedAll, part)) return rc;
     const size_t live = hid.size();
     for (int k = 0; k < kNumCols; ++k)   // the live tracks of the state columns
-      if (live && kCols[k].sec >= 0 && has(kCols[k]))
+      if (live && kCols[k].sec >= 0 && has(kCols[k]) && in_part(kCols[k], part))
         CU(cudaMemcpyAsync(nw[k].p, (this->*kCols[k].buf).p, live * track_bytes(kCols[k]), cudaMemcpyDeviceToDevice, st));
     CU(cudaStreamSynchronize(st));   // the old columns are freed with nw
-    swap_columns(nw);
-    cap = nc;
+    swap_columns(nw, kNeedAll, part);
     return 0;
   }
 
@@ -407,12 +576,17 @@ struct sb200_fstore {
     keep = rule;
     if (rule == SB200_FSTORE_KEEP_BEST_QUALITY) { init_cap = init; ext = ex; }
     cap_tab.swap(tab);
-    DBuf nw[kNumCols];   // as set_gate: the quality column starts empty, sized to the capacity
-    if (cap)
-      if (int rc = alloc(cap, nw, kNeedQuality)) return rc;
-    CU(cudaStreamSynchronize(st));
-    swap_columns(nw, kNeedQuality);
-    return 0;
+    // as set_gate: the quality columns start empty, sized to the capacity
+    auto fresh = [&](int part) {
+      DBuf nw[kNumCols];
+      if (cap)
+        if (int rc = alloc(cap, nw, kNeedQuality, part)) return rc;
+      CU(cudaStreamSynchronize(st));
+      swap_columns(nw, kNeedQuality, part);
+      return 0;
+    };
+    if (int rc = each_class([&](int) { return fresh(kPartClass); })) return rc;
+    return fresh(kPartShared);
   }
 
   int refuse_quality() const {
@@ -748,14 +922,14 @@ struct sb200_fstore {
   // its queries `tq`); offs as for associate
   int associate_rows(int Q, const uint64_t* qids, const int32_t* offs, const sb::FsRowSource& rsrc, int32_t* counts,
                      uint64_t* winners, double* weights, uint64_t* track_ids, uint8_t* merged,
-                     const TrackQueries* tq = nullptr) {
+                     const TrackQueries* tq = nullptr, std::vector<int>* decided = nullptr) {
     if (int rc = check_ids(Q, qids, "query id", true)) return rc;
     std::vector<int> qoff, src;
     if (int rc = plan_rows(Q, offs, &qoff, &src)) return rc;
     if (int rc = begin()) return rc;
     if (Q == 0) return 0;
     return launch_queries(Q, qids, qoff, src, Column{nullptr, false, nullptr}, 0, &rsrc, counts, winners, weights,
-                          track_ids, merged, true, nullptr, nullptr, tq);
+                          track_ids, merged, true, nullptr, nullptr, tq, decided);
   }
 
   // the device part of search / associate, after every check: upload, distances, TopN, apply, results
@@ -763,7 +937,7 @@ struct sb200_fstore {
                      const Column& col, size_t col_rows, const sb::FsRowSource* rsrc, int32_t* counts,
                      uint64_t* winners, double* weights, uint64_t* track_ids, uint8_t* merged, bool assoc,
                      const sb200_fstore_attrs* attrs = nullptr, const float* quality = nullptr,
-                     const TrackQueries* tq = nullptr) {
+                     const TrackQueries* tq = nullptr, std::vector<int>* decided = nullptr) {
     const int R = (int)src.size(), topn = o.topn, K = o.max_observations;
     const bool qa = assoc && keep;   // a quality store's merges are planned and applied by fs_launch_qmerge
     const bool gated = attrs || (tq && gate);   // the queries' triples are in qattr
@@ -793,6 +967,14 @@ struct sb200_fstore {
     sb::fs_launch_topn(o.max_distance, o.min_votes, topn, assoc, s, c, st);
     CU(cudaEventRecord(ev[2], st));
     if (assoc && gated) sb::fs_launch_gate_resolve(c, g, st);
+    if (decided) {   // associate_store of several classes on a quality store: the caller applies every class
+      decided->resize(Q);
+      CU(cudaMemcpyAsync(hres.p, dres.p, RL.total, cudaMemcpyDeviceToHost, st));
+      CU(cudaMemcpyAsync(decided->data(), c.dest, (size_t)Q * 4, cudaMemcpyDeviceToHost, st));
+      if (int rc = finish(S > 0 ? 0 : 1, 2)) return rc;
+      read_results(RL, Q, counts, winners, weights);
+      return 0;
+    }
     if (qa) sb::fs_launch_qmerge(s, c, qc, st, tq ? tq->hq : nullptr);
     else if (assoc) sb::fs_launch_apply(s, c, st);
     if (assoc && gated) sb::fs_launch_attr_new(s.live, c, g, st);
@@ -997,9 +1179,15 @@ struct sb200_fstore {
     if (src == this) return fail(SB200_ERR_INVALID, "dst and src are the same store (merge_owned merges within one)");
     const sb200_fstore_options& so = src->o;
     if (so.device != o.device) return fail(SB200_ERR_INVALID, "src is on device %d, dst on device %d", so.device, o.device);
-    if (so.feature_dim != o.feature_dim || so.max_observations != o.max_observations)
-      return fail(SB200_ERR_INVALID, "feature_dim / max_observations differ: %d / %d in src, %d / %d in dst",
-                  so.feature_dim, so.max_observations, o.feature_dim, o.max_observations);
+    if (so.max_observations != o.max_observations)
+      return fail(SB200_ERR_INVALID, "max_observations differ: %d in src, %d in dst", so.max_observations,
+                  o.max_observations);
+    bool same = src->cls.size() == cls.size();
+    for (size_t k = 0; same && k < cls.size(); ++k) {
+      const int j = src->class_index(cls[k].id);
+      same = j >= 0 && src->cls[j].dim == cls[k].dim;
+    }
+    if (!same) return fail(SB200_ERR_INVALID, "feature classes or feature_dim differ between src and dst");
     if (src->gate != gate) return fail(SB200_ERR_INVALID, "gate rules differ: %d in src, %d in dst", src->gate, gate);
     if (src->keep != keep || (keep && (src->init_cap != init_cap || src->ext != ext)))
       return fail(SB200_ERR_INVALID, "retention rules or their parameters differ between src and dst");
@@ -1017,6 +1205,17 @@ struct sb200_fstore {
     }
     if (int rc = begin()) return rc;
     if (n == 0) return 0;
+    // the queries are src's rows of the class this store has selected
+    const int src_sel = src->sel;
+    src->select(src->class_index(cls[sel].id));
+    const int rc = associate_tracks(src, n, idv, pos, remove, counts, winners, weights, track_ids, merged);
+    src->select(src_sel);
+    return rc;
+  }
+
+  // associate_store once every check has passed, with src's class selected as this store's
+  int associate_tracks(sb200_fstore* src, int n, const uint64_t* idv, const std::vector<int>& pos, int remove,
+                       int32_t* counts, uint64_t* winners, double* weights, uint64_t* track_ids, uint8_t* merged) {
     // src's stream is idle once peek returns, so every column this call reads from src is complete
     std::vector<int> ring;
     if (int rc = src->peek(pos, &ring)) return rc;
@@ -1033,14 +1232,146 @@ struct sb200_fstore {
     CU(cudaMemcpyAsync(sq.p, pos.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
     StoreRows ctx{src, sq.as<int>(), n, triples(qattr, n), dqr.as<float>(), sq.as<int>() + n};
     const TrackQueries tq{keep ? sq.as<int>() + n : nullptr, keep ? &qhist : nullptr};
+    // a quality store of several classes decides the destinations here and applies every class below
+    const bool qpasses = keep && cls.size() > 1;
+    std::vector<int> dec;
     // returns once this store's stream has finished, so src's rows are read no more
     if (int rc = associate_rows(n, idv, offs.data(), {stage_store_rows, &ctx}, counts, winners, weights, track_ids,
-                                merged, &tq))
+                                merged, &tq, qpasses ? &dec : nullptr))
       return rc;
+    if (qpasses) {
+      if (int rc = qmerge_classes(src, ctx, n, idv, pos, qhist, dec, winners, track_ids, merged)) return rc;
+    } else if (cls.size() > 1) {   // where each query went, and then its rows of the other classes
+      std::vector<int> dpos(n);
+      for (int q = 0; q < n; ++q) dpos[q] = hpos.at(merged[q] ? track_ids[q] : idv[q]);
+      const int s0 = sel, src_sel = src->sel;
+      const std::vector<int> asc = ascending_classes();
+      const int rc = each_class([&](int k) {
+        if (k == s0) return 0;
+        src->select(src->class_index(cls[k].id));
+        return append_class_rows(src, ctx, n, idv, pos, dpos);
+      }, &asc);
+      src->select(src_sel);
+      if (rc) return rc;
+    }
     if (!remove) return 0;
     std::vector<char> gone(src->hid.size(), 0);
     for (int p : pos) gone[p] = 1;
     return src->remove_marked(gone);
+  }
+
+  // associate_store on a quality store of several classes, once TopN and the gate have decided each query's
+  // destination (dec[q]: a stored position, or -1 for a new track).  Track::merge walks the classes a query holds in
+  // ascending id, each step appending the query's history h(q) before it optimizes that class; so one fs_qmerge_kernel
+  // pass per class, in ascending id, over every query (a query without rows of the class truncates at a capacity no
+  // smaller than its list's, which changes nothing), whose history increments make each item of a destination reach
+  //   h0 + S(q) + le(q) h(q),   S(q) = the sum of |C(j)| h(j) over the destination's earlier items j,
+  // le(q) = the classes q holds up to this pass's id, |C(j)| all the classes j holds.  A pass starts from the
+  // history length the previous one left (h0 in the first); a new track is the query whole, h(q) in every pass.
+  int qmerge_classes(sb200_fstore* src, const StoreRows& ctx0, int n, const uint64_t* idv, const std::vector<int>& pos,
+                     const std::vector<std::vector<uint64_t>>& qhist, const std::vector<int>& dec,
+                     const uint64_t* winners, uint64_t* track_ids, uint8_t* merged) {
+    const int live = (int)hid.size(), nc = (int)cls.size(), src_sel = src->sel;
+    std::vector<std::vector<int>> qcnt(nc);   // rows of each query in each class
+    for (int k = 0; k < nc; ++k) {
+      std::vector<int> ring;
+      src->select(src->class_index(cls[k].id));
+      if (int rc = src->peek(pos, &ring)) { src->select(src_sel); return rc; }
+      for (int q = 0; q < n; ++q) qcnt[k].push_back(ring[2 * q]);
+    }
+    src->select(src_sel);
+    std::vector<int> dpos(n), held(n, 0), prev(n, -1), last_of(n, -1);
+    std::vector<long long> S(n, 0), h(n);
+    std::unordered_map<int, int> last;
+    std::unordered_map<int, long long> acc;
+    for (int q = 0, fresh = 0; q < n; ++q) {
+      for (int k = 0; k < nc; ++k) held[q] += qcnt[k][q] > 0;
+      h[q] = (long long)qhist[q].size();
+      dpos[q] = dec[q] >= 0 ? dec[q] : live + fresh++;
+      if (dec[q] < 0) continue;
+      auto it = last.find(dpos[q]);
+      prev[q] = it == last.end() ? -1 : it->second;
+      last[dpos[q]] = q;
+      S[q] = acc[dpos[q]];
+      acc[dpos[q]] += held[q] * h[q];
+    }
+    for (int q = 0; q < n; ++q)
+      if (dec[q] >= 0) last_of[q] = last[dpos[q]];
+    std::vector<long long> le(n, 0), r(n, 0), r_prev;
+    std::vector<int> inc(n);
+    for (int k : ascending_classes()) {
+      std::vector<int> qoff(n + 1, 0);
+      for (int q = 0; q < n; ++q) qoff[q + 1] = qoff[q] + qcnt[k][q];
+      const int R = qoff[n];
+      if (R == 0) continue;   // no query holds the class
+      for (int q = 0; q < n; ++q) {
+        le[q] += qcnt[k][q] > 0;
+        r[q] = S[q] + le[q] * h[q];
+      }
+      for (int q = 0; q < n; ++q) {
+        long long from = 0;   // the relative history length the kernel holds before item q
+        if (prev[q] >= 0) from = r[prev[q]];
+        else if (!r_prev.empty() && dec[q] >= 0) from = r_prev[last_of[q]];
+        inc[q] = (int)(dec[q] >= 0 ? r[q] - from : h[q]);
+      }
+      r_prev = r;
+      src->select(src->class_index(cls[k].id));
+      const int s0 = sel;
+      select(k);
+      int rc = dqr.ensure((size_t)R * 4);
+      if (!rc) rc = dinc.ensure((size_t)n * 4);
+      if (!rc) {
+        StoreRows ctx = ctx0;
+        ctx.rq = dqr.as<float>();
+        const sb::FsRowSource rs{stage_store_rows, &ctx};
+        const ReqLayout L(n, R, d8, false);
+        rc = upload(L, n, idv, qoff, std::vector<int>(R), dpos.data(), Column{nullptr, false, nullptr}, 0, &rs);
+        if (!rc && cudaMemcpyAsync(dinc.p, inc.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st) != cudaSuccess)
+          rc = fail(SB200_ERR_CUDA, "history increment upload failed");
+        if (!rc) {
+          const sb::FsCall c = call_view(L, n, R, nullptr);
+          const sb::FsQCall qc{qual.as<float>(), hlen.as<int>(), dcap.as<int>(), (int)cap_tab.size(), dqr.as<float>(), 1};
+          sb::fs_launch_qmerge(view(), c, qc, st, dinc.as<int>());
+          if (gate) sb::fs_launch_attr_new(live, c, gate_view(n), st);
+          rc = finish();
+        }
+      }
+      select(s0);
+      src->select(src_sel);
+      if (rc) return rc;
+    }
+    for (int q = 0; q < n; ++q) {
+      merged[q] = dec[q] >= 0;
+      track_ids[q] = merged[q] ? winners[(size_t)q * o.topn] : idv[q];
+      for (int c = 0; merged[q] && c < held[q]; ++c)   // one history step per class the query holds
+        hist[dpos[q]].insert(hist[dpos[q]].end(), qhist[q].begin(), qhist[q].end());
+    }
+    for (int q = 0; q < n; ++q)
+      if (!merged[q]) {
+        hpos[idv[q]] = (int)hid.size();
+        hid.push_back(idv[q]);
+        hist.push_back(qhist[q]);
+      }
+    return 0;
+  }
+
+  // associate_store on a newest store of several classes: the selected class's rows of the queried src tracks (at
+  // src positions pos, staged by ctx) appended to the tracks they went to (dpos), as an add appends rows
+  int append_class_rows(sb200_fstore* src, const StoreRows& ctx, int n, const uint64_t* idv, const std::vector<int>& pos,
+                        const std::vector<int>& dpos) {
+    std::vector<int> ring;
+    if (int rc = src->peek(pos, &ring)) return rc;
+    std::vector<int> qoff(n + 1, 0);
+    for (int i = 0; i < n; ++i) qoff[i + 1] = qoff[i] + ring[2 * i];
+    const int R = qoff[n];
+    if (R == 0) return 0;
+    const std::vector<int> rows(R);   // only their number: the row source writes them
+    const ReqLayout L(n, R, d8, false);
+    if (int rc = plan.ensure((size_t)n * 16)) return rc;
+    const sb::FsRowSource rs{stage_store_rows, const_cast<StoreRows*>(&ctx)};
+    if (int rc = upload(L, n, idv, qoff, rows, dpos.data(), Column{nullptr, false, nullptr}, 0, &rs)) return rc;
+    sb::fs_launch_apply(view(), call_view(L, n, R, nullptr), st);
+    return finish();
   }
 
   // qout: a quality store's qualities [n][K] of the rows returned (fetch_quality), else nullptr
@@ -1099,22 +1430,29 @@ struct sb200_fstore {
     from.reserve(hid.size());
     for (size_t p = 0; p < hid.size(); ++p)
       if (!gone[p]) from.push_back((int)p);
-    DBuf nw[kNumCols];
-    if (int rc = alloc(cap, nw)) return rc;
+    DBuf nws[kNumCols];
+    if (int rc = alloc(cap, nws, kNeedAll, kPartShared)) return rc;
     if (int rc = gpos.ensure(std::max<size_t>(from.size(), 1) * 4)) return rc;
     CU(cudaMemcpyAsync(gpos.p, from.data(), from.size() * 4, cudaMemcpyHostToDevice, st));
-    const sb::FsStore s = view();
+    const unsigned long long* old_ids = ids.as<unsigned long long>();
     const sb::FsAttrCols sa = attr_cols();
-    const void* sq = qual.p;
     const void* sh = hlen.p;
-    swap_columns(nw);   // nw holds the old columns until the compaction below has read them
-    sb::fs_launch_compact(s, view(), gpos.as<int>(), (int)from.size(), st);
+    swap_columns(nws, kNeedAll, kPartShared);   // nws holds the old columns until the compaction below has read them
     if (gate) sb::fs_launch_attr_gather(sa, gpos.as<int>(), (int)from.size(), attr_cols(), st);
-    if (keep) {
-      sb::fs_launch_words_compact(sq, qual.p, gpos.as<int>(), (int)from.size(), o.max_observations, st);
-      sb::fs_launch_words_compact(sh, hlen.p, gpos.as<int>(), (int)from.size(), 1, st);
-    }
-    if (int rc = finish()) return rc;
+    if (keep) sb::fs_launch_words_compact(sh, hlen.p, gpos.as<int>(), (int)from.size(), 1, st);
+    // each class's columns, the fresh ones zero past the kept tracks; every class writes the same ids
+    if (int rc = each_class([&](int) {
+          DBuf nw[kNumCols];
+          if (int rc = alloc(cap, nw, kNeedAll, kPartClass)) return rc;
+          sb::FsStore s = view();
+          s.ids = const_cast<unsigned long long*>(old_ids);
+          const void* sq = qual.p;
+          swap_columns(nw, kNeedAll, kPartClass);
+          sb::fs_launch_compact(s, view(), gpos.as<int>(), (int)from.size(), st);
+          if (keep) sb::fs_launch_words_compact(sq, qual.p, gpos.as<int>(), (int)from.size(), o.max_observations, st);
+          return finish();
+        }))
+      return rc;
     std::vector<uint64_t> kept;
     kept.reserve(from.size());
     for (int p : from) kept.push_back(hid[p]);
@@ -1273,18 +1611,48 @@ struct sb200_fstore {
     if (gate)
       if (int rc = plan_merge_attrs(n, dp, sp, idx, touched, &wpos, &win)) return rc;
     if (keep) {   // each pair's merge optimized at its destination's capacity, planned from the peeked lists
-      std::vector<QTrack> tl;
-      if (int rc = peek_tracks(touched, &tl)) return rc;
-      for (int i = 0; i < n; ++i) merge_into(tl[idx[dp[i]]], tl[idx[sp[i]]]);
-      for (QTrack& t : tl)
-        if (gone[t.pos]) t.dirty = false;
-      if (int rc = apply_tracks(tl)) return rc;
-      for (const QTrack& t : tl)
-        if (t.dirty) hist[t.pos] = t.h;
+      // Track::merge walks the classes the source holds (ascending id here), and each class step appends the source's
+      // history to the destination's before it optimizes that class's list at the new capacity
+      const std::vector<int> asc = ascending_classes();
+      std::vector<std::vector<QTrack>> tl(cls.size());
+      if (int rc = each_class([&](int k) { return peek_tracks(touched, &tl[k]); })) return rc;
+      std::vector<std::vector<uint64_t>> h(touched.size());
+      for (size_t t = 0; t < touched.size(); ++t) h[t] = hist[touched[t]];
+      for (int i = 0; i < n; ++i) {
+        const int d = idx[dp[i]], sr = idx[sp[i]];
+        for (int k : asc) {
+          if (tl[k][sr].ref.empty()) continue;   // a class the source does not hold
+          tl[k][d].h = h[d];
+          tl[k][sr].h = h[sr];
+          merge_into(tl[k][d], tl[k][sr]);
+          h[d] = tl[k][d].h;
+        }
+      }
+      std::vector<char> dirty(touched.size(), 0);
+      for (std::vector<QTrack>& v : tl)
+        for (size_t t = 0; t < touched.size(); ++t) {
+          v[t].h = h[t];   // every class writes the track's final history length
+          if (gone[v[t].pos]) v[t].dirty = false;
+          dirty[t] |= v[t].dirty;
+        }
+      if (int rc = each_class([&](int k) { return apply_tracks(tl[k]); })) return rc;
+      for (size_t t = 0; t < touched.size(); ++t)
+        if (dirty[t]) hist[touched[t]] = h[t];
       if (int rc = write_attrs(wpos, win)) return rc;
       if (remove) return remove_marked(gone);
       return 0;
     }
+    // a newest store: each class's rings planned and moved on their own
+    if (int rc = each_class([&](int) { return merge_rings(n, dp, sp, idx, touched, gone); })) return rc;
+    if (int rc = write_attrs(wpos, win)) return rc;
+    if (remove) return remove_marked(gone);
+    return 0;
+  }
+
+  // merge_owned on a newest store, for the selected class
+  int merge_rings(int n, const std::vector<int>& dp, const std::vector<int>& sp, std::unordered_map<int, int>& idx,
+                  const std::vector<int>& touched, const std::vector<char>& gone) {
+    const int K = o.max_observations;
     std::vector<int> ring;
     if (int rc = peek(touched, &ring)) return rc;
     // per touched track: its rows oldest first as stored row indices (position * K + slot) of the pre-call store, and
@@ -1330,10 +1698,7 @@ struct sb200_fstore {
     CU(cudaEventRecord(ev[2], st));
     sb::fs_launch_move_rows(view(), dtab, dtab + nm, nm, dtab + 2 * nm, nh, gout.p, st);
     CU(cudaEventRecord(ev[3], st));
-    if (int rc = finish(2, 3)) return rc;
-    if (int rc = write_attrs(wpos, win)) return rc;
-    if (remove) return remove_marked(gone);
-    return 0;
+    return finish(2, 3);
   }
 
   // merge_owned's attributes: each pair, in order, must be compatible with the windows the earlier pairs left (else the
@@ -1387,6 +1752,7 @@ struct sb200_fstore {
   }
 
   int save(void* dst, uint64_t cap_bytes, uint64_t* bytes) {
+    if (!plain_classes()) return save_classes(dst, cap_bytes, bytes);
     uint64_t sec[SB200_FSTORE_BLOB_SECTIONS_V3];
     if (keep) {   // version 3: the quality, history length and history sections follow the attribute ones
       std::vector<uint64_t> hc;
@@ -1413,6 +1779,122 @@ struct sb200_fstore {
     fill_header(h, SB200_FSTORE_BLOB_VERSION);
     sb::lay_out(h, sec, n);
     return write_header_and_columns(dst, cap_bytes, bytes, h, n);
+  }
+
+  // version 4 (a store of other classes than the single class 0)
+  int save_classes(void* dst, uint64_t cap_bytes, uint64_t* bytes) {
+    std::vector<uint64_t> hc;
+    for (const std::vector<uint64_t>& h : hist) hc.insert(hc.end(), h.begin(), h.end());
+    const int nc = (int)cls.size(), K = o.max_observations, live = (int)hid.size();
+    std::vector<uint64_t> cid(nc);
+    std::vector<int32_t> cdim(nc);
+    for (int k = 0; k < nc; ++k) { cid[k] = cls[k].id; cdim[k] = cls[k].dim; }
+    uint64_t sec[SB200_FSTORE_BLOB_SECTIONS_V4];
+    const char* names[SB200_FSTORE_BLOB_SECTIONS_V4];
+    const int n = sections_v4(live, K, stype, gate, keep, nc, cdim.data(), hc.size(), sec, names);
+    BlobHeaderV4 h;
+    fill_header(h, SB200_FSTORE_BLOB_VERSION_CLASSES);
+    h.feature_dim = cls[0].dim;   // not the selected class's: the blob does not depend on the selection
+    h.d8 = cls[0].d8;
+    h.gate = gate;
+    h.retention = keep;
+    h.initial_capacity = init_cap;
+    h.merge_extension = ext;
+    h.n_classes = nc;
+    sb::lay_out(h, sec, n);
+    *bytes = h.total_bytes;
+    if (!dst) return 0;
+    if (cap_bytes < h.total_bytes)
+      return fail(SB200_ERR_CAPACITY, "the blob needs %llu bytes", (unsigned long long)h.total_bytes);
+    CU(cudaSetDevice(o.device));
+    return sb::write_blob(dst, o.device, st, h, n, [&](char* p) {
+      if (int rc = move_classes(0, h.sec_off, p)) return rc;
+      each_class([&](int k) {
+        const uint64_t at = kV4Class + (uint64_t)kV4PerClass * k;
+        sb::fs_launch_blob_scrub(stype, p + h.sec_off[at + kV4Feat], cnt.as<int>(), start.as<int>(), live, K, d8, st);
+        if (keep) sb::fs_launch_qual_scrub(reinterpret_cast<float*>(p + h.sec_off[at + kV4Qual]), cnt.as<int>(),
+                                           start.as<int>(), live, K, st);
+        return 0;
+      });
+      CU(cudaMemcpyAsync(p + h.sec_off[kV4ClassIds], cid.data(), nc * 8, cudaMemcpyHostToDevice, st));
+      CU(cudaMemcpyAsync(p + h.sec_off[kV4ClassDims], cdim.data(), nc * 4, cudaMemcpyHostToDevice, st));
+      if (!hc.empty()) CU(cudaMemcpyAsync(p + h.sec_off[kV4Hist], hc.data(), hc.size() * 8, cudaMemcpyHostToDevice, st));
+      return finish();
+    });
+  }
+
+  // the device columns and the version-4 sections at sec_off of a blob at dblob on this device (dir 0 packs, dir 1
+  // unpacks), for the live tracks
+  int move_classes(int dir, const uint64_t* sec_off, char* dblob) {
+    const uint64_t live = hid.size();
+    const int K = o.max_observations;
+    std::vector<sb::XferSeg> segs;
+    auto add = [&](const DBuf& b, int sec, uint64_t n) {
+      if (n) sb::add_segment(segs, dir, const_cast<char*>(b.as<char>()), dblob + sec_off[sec], n);
+    };
+    add(ids, kV4Ids, live * 8);
+    if (gate) { add(asrc, kV4Src, live * 8); add(at0, kV4T0, live * 8); add(at1, kV4T1, live * 8); }
+    if (keep) add(hlen, kV4Hlen, live * 4);
+    for (int k = 0; k < (int)cls.size(); ++k) {
+      const ClassCols& c = cls[k];
+      const bool me = k == sel;   // the selected class's columns are the members
+      const int at = kV4Class + kV4PerClass * k;
+      add(me ? cnt : c.cnt, at + kV4Cnt, live * 4);
+      add(me ? start : c.start, at + kV4Start, live * 4);
+      add(me ? feat : c.feat, at + kV4Feat, live * K * row_bytes(c.d8, stype));
+      if (keep) add(me ? qual : c.qual, at + kV4Qual, live * K * 4);
+    }
+    return sb::copy_segments(segs, num_sms, st);
+  }
+
+  // fills a store fresh from sb200_fstore_create, whose classes are the blob's, with the version-4 blob `h` at `src`
+  // (checked on the host); refuses what its kernels find
+  int load_classes(const BlobHeaderV4& h, const void* src, std::vector<uint64_t>&& blob_ids,
+                   std::vector<std::vector<uint64_t>>&& hists) {
+    if (int rc = begin()) return rc;
+    const int live = (int)h.live, K = o.max_observations, nc = (int)cls.size();
+    ftype = h.feature_type;
+    stype = h.storage_type;
+    if (int rc = set_gate(h.gate)) return rc;
+    if (int rc = set_retention(h.retention, h.initial_capacity, h.merge_extension)) return rc;
+    if (live == 0) return 0;
+    if (int rc = reserve((size_t)live)) return rc;
+    DBuf tmp;
+    const char* dblob = nullptr;
+    if (int rc = sb::blob_on_device(src, h.total_bytes, o.device, st, tmp, &dblob)) return rc;
+    sb::FsClassCols cc{};
+    cc.n = nc;
+    for (int k = 0; k < nc; ++k) {
+      const int at = kV4Class + kV4PerClass * k;
+      cc.cnt[k] = reinterpret_cast<const int*>(dblob + h.sec_off[at + kV4Cnt]);
+      cc.start[k] = reinterpret_cast<const int*>(dblob + h.sec_off[at + kV4Start]);
+    }
+    int bad[6] = {0, 0, 0, 0, 0, 0};   // class check, windows, quality
+    if (int rc = gpos.ensure(sizeof(bad))) return rc;
+    CU(cudaMemsetAsync(gpos.p, 0, sizeof(bad), st));
+    sb::fs_launch_class_check(cc, live, K, gpos.as<int>(), st);
+    if (h.gate)
+      sb::fs_launch_attr_check(reinterpret_cast<const long long*>(dblob + h.sec_off[kV4T0]),
+                               reinterpret_cast<const long long*>(dblob + h.sec_off[kV4T1]), live, gpos.as<int>() + 3, st);
+    if (h.retention)
+      for (int k = 0; k < nc; ++k)
+        sb::fs_launch_qual_check(reinterpret_cast<const float*>(dblob + h.sec_off[kV4Class + kV4PerClass * k + kV4Qual]),
+                                 cc.cnt[k], cc.start[k], live, K, gpos.as<int>() + 4, st);
+    CU(cudaMemcpyAsync(bad, gpos.p, sizeof(bad), cudaMemcpyDeviceToHost, st));
+    if (int rc = finish()) return rc;
+    if (bad[0]) return fail(SB200_ERR_INVALID, "the blob holds %d cnt entries outside 0..%d", bad[0], K);
+    if (bad[1]) return fail(SB200_ERR_INVALID, "the blob holds %d start entries outside 0..%d", bad[1], K - 1);
+    if (bad[2]) return fail(SB200_ERR_INVALID, "the blob holds %d tracks without a row in any class", bad[2]);
+    if (bad[3]) return fail(SB200_ERR_INVALID, "the blob holds %d windows with t_start > t_end", bad[3]);
+    if (bad[4]) return fail(SB200_ERR_INVALID, "the blob holds %d NaN qualities in filled slots", bad[4]);
+    if (bad[5])
+      return fail(SB200_ERR_INVALID, "the blob holds %d observations out of the quality order (above the one before)",
+                  bad[5]);
+    hid = std::move(blob_ids);
+    if (int rc = move_classes(1, h.sec_off, const_cast<char*>(dblob))) return rc;
+    hist = std::move(hists);
+    for (size_t p = 0; p < hid.size(); ++p) hpos[hid[p]] = (int)p;
+    return 0;
   }
 
   // hc: a quality store's concatenated histories, written into their section
@@ -1486,22 +1968,136 @@ struct sb200_fstore {
 };
 
 const sb200_fstore::Col sb200_fstore::kCols[kNumCols] = {
-    {&sb200_fstore::feat, 0, false, kNeedAll, false, kSecFeat, "feat"},
-    {&sb200_fstore::cnt, 4, false, kNeedAll, false, kSecCnt, "cnt"},
-    {&sb200_fstore::start, 4, false, kNeedAll, false, kSecStart, "start"},
-    {&sb200_fstore::ids, 8, false, kNeedAll, false, kSecIds, "ids"},
-    {&sb200_fstore::run, 4, false, kNeedAll, true, -1, nullptr},
-    {&sb200_fstore::asrc, 8, false, kNeedGate, true, kSecSrc, "source"},
-    {&sb200_fstore::at0, 8, false, kNeedGate, true, kSecT0, "t_start"},
-    {&sb200_fstore::at1, 8, false, kNeedGate, true, kSecT1, "t_end"},
-    {&sb200_fstore::qual, 4, true, kNeedQuality, true, kSecQual, "quality"},
-    {&sb200_fstore::hlen, 4, false, kNeedQuality, true, kSecHlen, "history_length"},
+    {&sb200_fstore::feat, 0, false, kNeedAll, false, kSecFeat, "feat", true},
+    {&sb200_fstore::cnt, 4, false, kNeedAll, true, kSecCnt, "cnt", true},
+    {&sb200_fstore::start, 4, false, kNeedAll, true, kSecStart, "start", true},
+    {&sb200_fstore::ids, 8, false, kNeedAll, false, kSecIds, "ids", false},
+    {&sb200_fstore::run, 4, false, kNeedAll, true, -1, nullptr, false},
+    {&sb200_fstore::asrc, 8, false, kNeedGate, true, kSecSrc, "source", false},
+    {&sb200_fstore::at0, 8, false, kNeedGate, true, kSecT0, "t_start", false},
+    {&sb200_fstore::at1, 8, false, kNeedGate, true, kSecT1, "t_end", false},
+    {&sb200_fstore::qual, 4, true, kNeedQuality, true, kSecQual, "quality", true},
+    {&sb200_fstore::hlen, 4, false, kNeedQuality, true, kSecHlen, "history_length", false},
 };
 
 // a call without a handle: SB200_ERR_CUDA when there is no device to have made one, else SB200_ERR_INVALID
 int no_handle() {
   if (int rc = sb::check_device(0)) return rc;
   return fail(SB200_ERR_INVALID, "NULL handle");
+}
+
+extern "C" int sb200_fstore_create(const sb200_fstore_options* opts, sb200_fstore** out);
+
+// sb200_fstore_load of a version-4 blob (its magic and version read): every check the host can make from the header,
+// the class table, the ids, the histories and (quality store) the counts, then the store, whose kernels check the rest
+static int load_classes(const void* buf, uint64_t bytes, int32_t device, sb200_fstore** out) {
+  BlobHeaderV4 h;
+  if (bytes < sizeof(h)) return fail(SB200_ERR_INVALID, "the blob is truncated (%llu bytes)", (unsigned long long)bytes);
+  CU(cudaMemcpy(&h, buf, sizeof(h), cudaMemcpyDefault));
+  if (h.gate != SB200_FSTORE_GATE_NONE && h.gate != SB200_FSTORE_GATE_SAME_SOURCE && h.gate != SB200_FSTORE_GATE_ANY_SOURCE)
+    return fail(SB200_ERR_INVALID, "a version-4 blob with unknown gate rule %d", h.gate);
+  if (h.retention != SB200_FSTORE_KEEP_NEWEST && h.retention != SB200_FSTORE_KEEP_BEST_QUALITY)
+    return fail(SB200_ERR_INVALID, "a version-4 blob with unknown retention rule %d", h.retention);
+  const int nc = h.n_classes;
+  if (nc < 1 || nc > SB200_FSTORE_MAX_CLASSES)
+    return fail(SB200_ERR_INVALID, "n_classes %d outside 1..%d", nc, SB200_FSTORE_MAX_CLASSES);
+  if (h.total_bytes > bytes)
+    return fail(SB200_ERR_INVALID, "the blob is truncated (%llu of total_bytes %llu)", (unsigned long long)bytes,
+                (unsigned long long)h.total_bytes);
+  sb200_fstore_options o = {h.metric, h.distance_filter, h.max_observations, h.feature_dim, h.topn, h.max_distance,
+                            h.min_votes, device};
+  if (int rc = check_options(o)) return rc;
+  if (h.d8 != (h.feature_dim + 7) / 8 * 8) return fail(SB200_ERR_INVALID, "d8 is not feature_dim rounded up to 8");
+  if (!known_type(h.feature_type)) return fail(SB200_ERR_INVALID, "unknown feature_type %d", h.feature_type);
+  if (!known_type(h.storage_type)) return fail(SB200_ERR_INVALID, "unknown storage_type %d", h.storage_type);
+  if (h.live < 0 || h.live > INT32_MAX / h.max_observations) return fail(SB200_ERR_INVALID, "live count out of range");
+  const int K = h.max_observations;
+  const uint64_t live = (uint64_t)h.live;
+  std::vector<int> tab;
+  if (h.retention)
+    if (int rc = capacity_table(K, h.initial_capacity, h.merge_extension, &tab)) return rc;
+  // the section table up to the class table, then the class table, then every section's size
+  const char* name[SB200_FSTORE_BLOB_SECTIONS_V4];
+  uint64_t want[SB200_FSTORE_BLOB_SECTIONS_V4];
+  const int32_t one_dim = 1;
+  const int nsec = sections_v4(live, K, h.storage_type, h.gate, h.retention, nc, std::vector<int32_t>(nc, one_dim).data(),
+                               0, want, name);
+  if (int rc = sb::check_section_table(h, nsec, name)) return rc;
+  if (h.sec_bytes[kV4ClassIds] != (uint64_t)nc * 8 || h.sec_bytes[kV4ClassDims] != (uint64_t)nc * 4)
+    return fail(SB200_ERR_INVALID, "the class table does not hold n_classes = %d entries", nc);
+  std::vector<uint64_t> cid(nc);
+  std::vector<int32_t> cdim(nc);
+  CU(cudaMemcpy(cid.data(), static_cast<const char*>(buf) + h.sec_off[kV4ClassIds], nc * 8, cudaMemcpyDefault));
+  CU(cudaMemcpy(cdim.data(), static_cast<const char*>(buf) + h.sec_off[kV4ClassDims], nc * 4, cudaMemcpyDefault));
+  for (int k = 0; k < nc; ++k) {
+    if (cdim[k] < 1 || cdim[k] > SB200_FSTORE_MAX_DIM)
+      return fail(SB200_ERR_INVALID, "class %llu: feature_dim %d outside 1..%d", (unsigned long long)cid[k], cdim[k],
+                  SB200_FSTORE_MAX_DIM);
+    for (int j = 0; j < k; ++j)
+      if (cid[j] == cid[k]) return fail(SB200_ERR_INVALID, "class id %llu appears twice", (unsigned long long)cid[k]);
+  }
+  if (cdim[0] != h.feature_dim) return fail(SB200_ERR_INVALID, "feature_dim is not the first class's dim");
+  sections_v4(live, K, h.storage_type, h.gate, h.retention, nc, cdim.data(), 0, want, name);
+  for (int i = 0; i < nsec; ++i)
+    if (i != kV4Hist && h.sec_bytes[i] != want[i])   // the history's size is checked against its lengths below
+      return fail(SB200_ERR_INVALID, "section %s holds %llu bytes, %llu expected", name[i],
+                  (unsigned long long)h.sec_bytes[i], (unsigned long long)want[i]);
+  auto at = [&](int sec) { return static_cast<const char*>(buf) + h.sec_off[sec]; };
+  std::vector<uint64_t> blob_ids(live);
+  if (live) CU(cudaMemcpy(blob_ids.data(), at(kV4Ids), live * 8, cudaMemcpyDefault));
+  std::unordered_set<uint64_t> seen;
+  seen.reserve(live * 2);
+  for (uint64_t id : blob_ids)
+    if (!seen.insert(id).second) return fail(SB200_ERR_INVALID, "id %llu appears twice in the blob", (unsigned long long)id);
+  std::vector<std::vector<uint64_t>> hists;
+  if (h.retention) {   // as version 3, with every class's list
+    std::vector<int32_t> hl(live);
+    if (live) CU(cudaMemcpy(hl.data(), at(kV4Hlen), live * 4, cudaMemcpyDefault));
+    uint64_t total = 0;
+    for (uint64_t t = 0; t < live; ++t) {
+      if (hl[t] < 1)
+        return fail(SB200_ERR_INVALID, "track %llu has a merge history of length %d", (unsigned long long)blob_ids[t], hl[t]);
+      total += (uint64_t)hl[t];
+    }
+    if (h.sec_bytes[kV4Hist] != total * 8)
+      return fail(SB200_ERR_INVALID, "section history holds %llu bytes, %llu expected (the sum of the history lengths)",
+                  (unsigned long long)h.sec_bytes[kV4Hist], (unsigned long long)(total * 8));
+    std::vector<int32_t> cn(live), sn(live);
+    for (int k = 0; k < nc && live; ++k) {
+      CU(cudaMemcpy(cn.data(), at(kV4Class + kV4PerClass * k + kV4Cnt), live * 4, cudaMemcpyDefault));
+      CU(cudaMemcpy(sn.data(), at(kV4Class + kV4PerClass * k + kV4Start), live * 4, cudaMemcpyDefault));
+      for (uint64_t t = 0; t < live; ++t) {
+        if (sn[t] != 0)
+          return fail(SB200_ERR_INVALID, "track %llu has ring start %d; a quality store's lists start at slot 0",
+                      (unsigned long long)blob_ids[t], sn[t]);
+        const int c = tab[std::min<size_t>((size_t)hl[t], tab.size() - 1)];
+        if (cn[t] > c)
+          return fail(SB200_ERR_INVALID, "track %llu holds %d observations, above its capacity %d at history length %d",
+                      (unsigned long long)blob_ids[t], cn[t], c, hl[t]);
+      }
+    }
+    std::vector<uint64_t> hc(total);
+    if (total) CU(cudaMemcpy(hc.data(), at(kV4Hist), total * 8, cudaMemcpyDefault));
+    hists.resize(live);
+    for (uint64_t t = 0, a = 0; t < live; a += (uint64_t)hl[t], ++t) {
+      hists[t].assign(hc.begin() + a, hc.begin() + a + hl[t]);
+      if (hists[t][0] != blob_ids[t])
+        return fail(SB200_ERR_INVALID, "the merge history of track %llu starts with %llu, not with its id",
+                    (unsigned long long)blob_ids[t], (unsigned long long)hists[t][0]);
+    }
+  } else if (h.sec_bytes[kV4Hist] != 0) {
+    return fail(SB200_ERR_INVALID, "a newest store's blob with a history section");
+  }
+  sb200_fstore* s = nullptr;
+  if (int rc = sb200_fstore_create(&o, &s)) return rc;
+  int rc = s->set_classes(nc, cid.data(), cdim.data());
+  if (!rc) rc = s->load_classes(h, buf, std::move(blob_ids), std::move(hists));
+  if (rc) {
+    sb200_fstore_destroy(s);   // the handle owns every buffer made so far
+    return rc;
+  }
+  *out = s;
+  return 0;
 }
 
 extern "C" {
@@ -1517,6 +2113,10 @@ int sb200_fstore_create(const sb200_fstore_options* opts, sb200_fstore** out) {
   sb200_fstore* s = new sb200_fstore();
   s->o = o;
   s->d8 = (o.feature_dim + 7) / 8 * 8;
+  s->cls.resize(1);
+  s->cls[0].id = 0;
+  s->cls[0].dim = o.feature_dim;
+  s->cls[0].d8 = s->d8;
   cudaError_t e = cudaStreamCreateWithFlags(&s->st, cudaStreamNonBlocking);
   for (int i = 0; i < 4 && e == cudaSuccess; ++i) e = cudaEventCreate(&s->ev[i]);
   if (e == cudaSuccess) e = cudaEventCreateWithFlags(&s->ev_in, cudaEventDisableTiming);
@@ -1814,6 +2414,31 @@ int sb200_fstore_merge_owned(sb200_fstore* s, int32_t n, const uint64_t* dest_id
   return s->merge_owned(n, dest_ids, src_ids, remove_src);
 }
 
+int sb200_fstore_set_classes(sb200_fstore* s, int32_t n, const uint64_t* class_ids, const int32_t* feature_dims) {
+  if (!s) return no_handle();
+  return s->set_classes(n, class_ids, feature_dims);
+}
+
+int32_t sb200_fstore_get_classes(sb200_fstore* s, int32_t cap, uint64_t* class_ids, int32_t* feature_dims) {
+  if (!s) return no_handle();
+  if (cap < 0 || (cap > 0 && (!class_ids || !feature_dims))) return fail(SB200_ERR_INVALID, "bad cap / outputs");
+  for (int k = 0; k < std::min(cap, (int32_t)s->cls.size()); ++k) {
+    class_ids[k] = s->cls[k].id;
+    feature_dims[k] = s->cls[k].dim;
+  }
+  return (int32_t)s->cls.size();
+}
+
+int sb200_fstore_use_class(sb200_fstore* s, uint64_t class_id) {
+  if (!s) return no_handle();
+  return s->use_class(class_id);
+}
+
+int64_t sb200_fstore_class_counts(sb200_fstore* s, int32_t n, const uint64_t* ids, int32_t* counts) {
+  if (!s) return no_handle();
+  return s->class_counts(n, ids, counts);
+}
+
 int sb200_fstore_save(sb200_fstore* s, void* buf, uint64_t cap, uint64_t* bytes) {
   if (!s) return no_handle();
   if (!bytes) return fail(SB200_ERR_INVALID, "bytes is NULL");
@@ -1830,10 +2455,11 @@ int sb200_fstore_load(const void* buf, uint64_t bytes, int32_t device, sb200_fst
   BlobHeader h;
   CU(cudaMemcpy(&h, buf, sizeof(h), cudaMemcpyDefault));
   if (h.magic != SB200_FSTORE_BLOB_MAGIC) return fail(SB200_ERR_INVALID, "not a feature store blob (bad magic)");
+  if (h.version == SB200_FSTORE_BLOB_VERSION_CLASSES) return load_classes(buf, bytes, device, out);
   if (h.version != SB200_FSTORE_BLOB_VERSION && h.version != SB200_FSTORE_BLOB_VERSION_GATED &&
       h.version != SB200_FSTORE_BLOB_VERSION_QUALITY)
-    return fail(SB200_ERR_INVALID, "feature store blob version %u (this library reads %u, %u and %u)", h.version,
-                SB200_FSTORE_BLOB_VERSION, SB200_FSTORE_BLOB_VERSION_GATED, SB200_FSTORE_BLOB_VERSION_QUALITY);
+    return fail(SB200_ERR_INVALID, "feature store blob version %u (this library reads %u to %u)", h.version,
+                SB200_FSTORE_BLOB_VERSION, SB200_FSTORE_BLOB_VERSION_CLASSES);
   // version 2 (a gated store): the same fields, the rule and a 7-section table
   const bool v2 = h.version == SB200_FSTORE_BLOB_VERSION_GATED;
   BlobHeaderV2 h2;

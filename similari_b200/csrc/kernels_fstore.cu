@@ -894,6 +894,31 @@ __global__ void fs_qual_scrub_kernel(float* __restrict__ qual, const int* __rest
   if (!fs_slot_filled(j, start[t], cnt[t], K)) qual[e] = 0.0f;
 }
 
+// ------------------------------------------------------------------------------------------------ feature classes
+__global__ void fs_class_counts_kernel(FsClassCols cc, const int* __restrict__ pos, int n, int* __restrict__ out) {
+  const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= (long long)n * cc.n) return;
+  const int i = (int)(e / cc.n), k = (int)(e - (long long)i * cc.n), p = pos[i];
+  out[e] = p >= 0 ? cc.cnt[k][p] : 0;
+}
+
+__global__ void fs_class_check_kernel(FsClassCols cc, int n, int K, int* bad) {
+  int bc = 0, bs = 0, be = 0;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    bool rows = false;
+    for (int k = 0; k < cc.n; ++k) {
+      const int c = cc.cnt[k][i], s0 = cc.start[k][i];
+      bc += (c < 0 || c > K);
+      bs += (s0 < 0 || s0 >= K);
+      rows |= c > 0;
+    }
+    be += !rows;
+  }
+  if (bc) atomicAdd(bad, bc);
+  if (bs) atomicAdd(bad + 1, bs);
+  if (be) atomicAdd(bad + 2, be);
+}
+
 }  // namespace
 
 template <typename Elem, int MODE, typename... Gate>
@@ -1092,6 +1117,18 @@ void fs_launch_qual_stage(const FsStore& s, const FsCall& c, const float* qual, 
 
 void fs_launch_baked(const long long* t_end, int n, long long now, long long period, int* out, cudaStream_t st) {
   fs_baked_kernel<<<1, kOrderThreads, 0, st>>>(t_end, n, now, period, out);
+  note_launch();
+}
+
+void fs_launch_class_counts(const FsClassCols& cc, const int* pos, int n, int* out, cudaStream_t st) {
+  if (n == 0) return;
+  fs_class_counts_kernel<<<fs_blocks((long long)n * cc.n), 256, 0, st>>>(cc, pos, n, out);
+  note_launch();
+}
+
+void fs_launch_class_check(const FsClassCols& cc, int n, int K, int* bad, cudaStream_t st) {
+  if (n == 0) return;
+  fs_class_check_kernel<<<std::min((n + 255) / 256, 1024), 256, 0, st>>>(cc, n, K, bad);
   note_launch();
 }
 

@@ -19,6 +19,7 @@ constexpr int kFsMaxTopn = 64;
 constexpr int kFsMaxObs = 64;
 constexpr int kFsMaxDim = 8192;
 constexpr long long kFsMaxPairs = 1LL << 30;   // observation pairs of one call's distance matrix (4 B each)
+constexpr int kFsMaxClasses = 16;   // SB200_FSTORE_MAX_CLASSES
 
 // The store's device columns, in store order (insertion order; removal is a stable compaction).  Observation j (oldest
 // first) of track t lives in ring slot (start[t] + j) % K of feat[t][.][.]; rows are zero-padded from D to d8 as
@@ -152,6 +153,20 @@ void fs_launch_blob_check(const int* cnt, const int* start, int n, int K, int* b
 // store blob, after its rows are copied: zeroes, in feat[n][K][d8] (elements of stype), the ring slots that hold no
 // observation
 void fs_launch_blob_scrub(int stype, void* feat, const int* cnt, const int* start, int n, int K, int d8, cudaStream_t st);
+
+// ---- feature classes (sb200_fstore_set_classes): each class has its own feat, cnt, start (and qual) columns, over the
+// shared ids, run and capacity, so every kernel above runs on one class's FsStore unchanged.  The cnt and start columns
+// of every class, in declared order:
+struct FsClassCols {
+  const int* cnt[kFsMaxClasses];
+  const int* start[kFsMaxClasses];
+  int n;
+};
+// out[i][k] = cnt of class k at pos[i] (0 for pos[i] < 0)
+void fs_launch_class_counts(const FsClassCols& cc, const int* pos, int n, int* out, cudaStream_t st);
+// store blob of version 4, before anything is copied (the columns: the blob's sections): bad[0] counts the cnt outside
+// [0, K], bad[1] the start outside [0, K), bad[2] the tracks without a row in any class
+void fs_launch_class_check(const FsClassCols& cc, int n, int K, int* bad, cudaStream_t st);
 
 // ---- a quality store (sb200_fstore_set_retention): observations kept in the track's order in ring slots 0, 1, ... (the
 // ring start is always 0), qual[cap][K] the quality of the row in each slot (0 where a slot holds none) and hlen[cap]

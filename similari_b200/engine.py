@@ -689,11 +689,19 @@ class FeatureStore:
     required on such a store and refused on a newest one), every track a merge history (merge_history(ids)), and a track
     of history length h holds at most min(max_observations, int(initial_capacity * merge_extension ** h)) rows, best
     first; fetch_quality(ids) returns them with their qualities.  A query takes part with its best
-    int(initial_capacity * merge_extension) rows.  associate_wasted is refused on such a store."""
+    int(initial_capacity * merge_extension) rows.  associate_wasted is refused on such a store.
+
+    Feature classes: classes={class_id: feature_dim, ...} declares several feature classes (the reference's
+    feature_class), each with its own dim; None is {0: feature_dim}.  add, search, associate, their _device forms,
+    search_owned, fetch, fetch_quality, associate_wasted and associate_store take feature_class= (None: the first
+    declared class) and work on that class's rows alone; a stored track without rows of the class takes no part in a
+    search of it.  merge_owned and associate_store move every class a track holds.  classes() and class_counts(ids)
+    report the classes and each track's rows in each.  A store of the single class 0 saves as before; any other
+    declaration saves as blob version 4, which carries the class table."""
 
     def __init__(self, metric="euclidean", distance_filter=100.0, max_observations=3, feature_dim=256, topn=1,
                  max_distance=100.0, min_votes=1, device=0, storage="f32", gate=None, retention="newest",
-                 initial_capacity=4, merge_extension=1.5):
+                 initial_capacity=4, merge_extension=1.5, classes=None):
         if metric not in METRICS:
             raise ValueError(f"metric must be one of {sorted(METRICS)}")
         if storage not in FEATURE_TYPES:
@@ -716,6 +724,38 @@ class FeatureStore:
         check(self._L.sb200_fstore_set_retention(h, RETENTIONS[retention], int(initial_capacity),
                                                  float(merge_extension)))
         self._keep = retention
+        if classes is not None:
+            cls = {int(k): int(v) for k, v in dict(classes).items()}
+            ids, dims = np.array(list(cls), np.uint64), np.array(list(cls.values()), np.int32)
+            check(self._L.sb200_fstore_set_classes(h, len(ids), ptr(ids), ptr(dims)))
+        self._read_classes()
+
+    def _read_classes(self):
+        n = int(check(self._L.sb200_fstore_get_classes(self._h, 0, None, None)))
+        ids, dims = np.zeros(n, np.uint64), np.zeros(n, np.int32)
+        check(self._L.sb200_fstore_get_classes(self._h, n, ptr(ids), ptr(dims)))
+        self._classes = {int(k): int(d) for k, d in zip(ids, dims)}
+        self._use(None)
+
+    def _use(self, feature_class):
+        """Selects the class of the next call (None: the first declared one); its dim becomes the row length D."""
+        c = next(iter(self._classes)) if feature_class is None else int(feature_class)
+        if c not in self._classes:
+            raise ValueError(f"feature_class {c} is not one of the store's classes {list(self._classes)}")
+        check(self._L.sb200_fstore_use_class(self._h, c))
+        self.D = self._classes[c]
+
+    def classes(self):
+        """The declared classes, {class_id: feature_dim}, in declared order."""
+        return dict(self._classes)
+
+    def class_counts(self, ids):
+        """counts[n][len(classes())]: each track's rows in each class, in declared order (0 where an id is not
+        stored); the reference's get_feature_classes with their lengths."""
+        ids = np.ascontiguousarray(ids, dtype=np.uint64)
+        out = np.zeros((len(ids), len(self._classes)), np.int32)
+        check(self._L.sb200_fstore_class_counts(self._h, len(ids), ptr(ids), ptr(out)))
+        return out
 
     def retention(self):
         """(rule, initial_capacity, merge_extension): rule "newest" or "quality"."""
@@ -798,9 +838,10 @@ class FeatureStore:
         check(self._L.sb200_fstore_set_feature_type(self._h, _lib.FEATURE_F32))
         return _f32(features).reshape(-1, self.D)
 
-    def add(self, ids, features, sources=None, t_start=None, t_end=None, quality=None):
+    def add(self, ids, features, sources=None, t_start=None, t_end=None, quality=None, feature_class=None):
         """TrackStore::add for each (ids[i], features[i]) in order (a gated store: with sources[i] and the window
-        [t_start[i], t_end[i]]; a quality store: with quality[i])."""
+        [t_start[i], t_end[i]]; a quality store: with quality[i]), into class feature_class."""
+        self._use(feature_class)
         ids = np.ascontiguousarray(ids, dtype=np.uint64)
         a = self._attrs(len(ids), sources, t_start, t_end)
         q = self._quality(len(ids), quality)
@@ -809,9 +850,11 @@ class FeatureStore:
             raise ValueError("features needs one row per id")
         self._call("add", a, (len(ids), ptr(ids)), f, q=q)
 
-    def add_device(self, ids, d_features, stream=0, sources=None, t_start=None, t_end=None, quality=None):
+    def add_device(self, ids, d_features, stream=0, sources=None, t_start=None, t_end=None, quality=None,
+                   feature_class=None):
         """sb200_fstore_add_device: `d_features` is the raw device address of [len(ids)][feature_dim] elements of the
         type set by set_feature_type (e.g. the data_ptr() of a torch CUDA tensor)."""
+        self._use(feature_class)
         ids = np.ascontiguousarray(ids, dtype=np.uint64)
         a = self._attrs(len(ids), sources, t_start, t_end)
         q = self._quality(len(ids), quality)
@@ -856,29 +899,36 @@ class FeatureStore:
             out["merged"] = np.zeros(q, np.uint8)
         return ids, offs, f, out
 
-    def search(self, ids, offsets, features, sources=None, t_start=None, t_end=None, quality=None):
+    def search(self, ids, offsets, features, sources=None, t_start=None, t_end=None, quality=None, feature_class=None):
         """foreign_track_distances + TopNVoting::winners: counts[q], winners[q][topn] (track ids), weights[q][topn].  A
         gated store takes one source and window per query; incompatible pairs neither vote nor count toward max_dist.
-        A quality store takes one quality per feature row."""
+        A quality store takes one quality per feature row.  feature_class: the class searched; a stored track without
+        rows of it gives no entries."""
+        self._use(feature_class)
         a = self._attrs(len(ids), sources, t_start, t_end)
         ids, offs, f, out = self._queries(ids, offsets, features)
         q = self._quality(int(offs[-1]) if len(ids) else 0, quality)
         self._call("search", a, (len(ids), ptr(ids), ptr(offs)), f, out=out, q=q)
         return out
 
-    def associate(self, ids, offsets, features, sources=None, t_start=None, t_end=None, quality=None):
+    def associate(self, ids, offsets, features, sources=None, t_start=None, t_end=None, quality=None,
+                  feature_class=None):
         """search, then merge each query with a result into its first winner and add the others as new tracks.  Adds
         track_ids[q] (where the query ended up) and merged[q] to the search outputs.  A gated store merges a query only
         if it is compatible with its first winner's window as the queries merged into it earlier in the call extended it;
-        otherwise the query becomes a new track."""
+        otherwise the query becomes a new track.  A merged query extends its winner's class feature_class; a new track
+        holds that class alone."""
+        self._use(feature_class)
         a = self._attrs(len(ids), sources, t_start, t_end)
         ids, offs, f, out = self._queries(ids, offsets, features, assoc=True)
         q = self._quality(int(offs[-1]) if len(ids) else 0, quality)
         self._call("associate", a, (len(ids), ptr(ids), ptr(offs)), f, out=out, q=q)
         return out
 
-    def search_device(self, ids, offsets, d_features, stream=0, sources=None, t_start=None, t_end=None, quality=None):
+    def search_device(self, ids, offsets, d_features, stream=0, sources=None, t_start=None, t_end=None, quality=None,
+                      feature_class=None):
         """sb200_fstore_search_device: search with the feature rows at the raw device address `d_features`."""
+        self._use(feature_class)
         a = self._attrs(len(ids), sources, t_start, t_end)
         ids, offs, _, out = self._queries(ids, offsets, None)
         q = self._quality(int(offs[-1]) if len(ids) else 0, quality)
@@ -887,8 +937,9 @@ class FeatureStore:
         return out
 
     def associate_device(self, ids, offsets, d_features, stream=0, sources=None, t_start=None, t_end=None,
-                         quality=None):
+                         quality=None, feature_class=None):
         """sb200_fstore_associate_device: associate with the feature rows at the raw device address `d_features`."""
+        self._use(feature_class)
         a = self._attrs(len(ids), sources, t_start, t_end)
         ids, offs, _, out = self._queries(ids, offsets, None, assoc=True)
         q = self._quality(int(offs[-1]) if len(ids) else 0, quality)
@@ -896,11 +947,12 @@ class FeatureStore:
         self._call("associate", a, (len(ids), ptr(ids), ptr(offs)), None, d_features, stream, out, q=q)
         return out
 
-    def search_owned(self, ids, each=False):
+    def search_owned(self, ids, each=False, feature_class=None):
         """sb200_fstore_search_owned: owned_track_distances + TopNVoting::winners with stored tracks as the queries, on
         the device.  each=False: one group, whose members are not candidates of each other and share max_dist;
         each=True: every id on its own (excluding only itself), as one call per id; a whole store may be passed.
-        Returns the search dict; an id that is not stored gets count 0."""
+        Returns the search dict; an id that is not stored, or without rows of feature_class, gets count 0."""
+        self._use(feature_class)
         ids = np.ascontiguousarray(ids, dtype=np.uint64)
         q = len(ids)
         out = {"counts": np.zeros(q, np.int32), "winners": np.zeros((q, self.topn), np.uint64),
@@ -911,20 +963,22 @@ class FeatureStore:
 
     def merge_owned(self, dest_ids, src_ids, remove=True):
         """sb200_fstore_merge_owned: for each pair in order, extend dest_ids[i] by the observations of src_ids[i] and
-        keep the newest max_observations; remove=True then takes every source out of the store."""
+        keep the newest max_observations; remove=True then takes every source out of the store.  Every class a source
+        holds is merged, in ascending class id."""
         d = np.ascontiguousarray(dest_ids, dtype=np.uint64)
         s = np.ascontiguousarray(src_ids, dtype=np.uint64)
         if len(d) != len(s):
             raise ValueError("dest_ids and src_ids must have the same length")
         check(self._L.sb200_fstore_merge_owned(self._h, len(d), ptr(d), ptr(s), int(bool(remove))))
 
-    def associate_wasted(self, tracker, cap=None, id_offset=0, history_cap=None):
+    def associate_wasted(self, tracker, cap=None, id_offset=0, history_cap=None, feature_class=None):
         """sb200_fstore_associate_wasted: collects up to `cap` wasted records of the visual `tracker` (None: every record,
         in one call) as tracker.wasted_history(cap, history_cap) does, and associates each record's present history
         features (oldest first) with this store under the id ids[i] + id_offset, as one associate() call would; the
         features never leave the device.  Returns the wasted_history() dict plus, per record, feature_counts,
         queried (bool) and the associate outputs counts / winners / weights / track_ids / merged (0 where not
-        queried).  The tracker needs its feature history on (set_feature_history)."""
+        queried).  The tracker needs its feature history on (set_feature_history), and feature_class a dim equal to
+        the tracker's."""
         if not isinstance(tracker, Tracker):
             raise TypeError("tracker must be an engine.Tracker")
         id_offset = int(id_offset)
@@ -946,6 +1000,7 @@ class FeatureStore:
         hc, fc, qd = np.zeros(n_out, np.int32), np.zeros(n_out, np.int32), np.zeros(n_out, np.uint8)
         cn, wn, wt = np.zeros(n_out, np.int32), np.zeros((n_out, t), np.uint64), np.zeros((n_out, t), np.float64)
         ti, mg = np.zeros(n_out, np.uint64), np.zeros(n_out, np.uint8)
+        self._use(feature_class)
         n = check(self._L.sb200_fstore_associate_wasted(
             self._h, tracker._h, cap, id_offset, ptr(ids), ptr(sc), ptr(ep), ptr(ln), ptr(pr), ptr(ob), H, ptr(hp),
             ptr(ho), ptr(hc), ptr(fc), ptr(qd), ptr(cn), ptr(wn), ptr(wt), ptr(ti), ptr(mg)))
@@ -967,13 +1022,15 @@ class FeatureStore:
         total = int(check(self._L.sb200_fstore_find_baked(self._h, now, period, n, ptr(out))))
         return out[:min(total, n)]
 
-    def associate_store(self, src, ids, remove=True):
+    def associate_store(self, src, ids, remove=True, feature_class=None):
         """sb200_fstore_associate_store: fetch_tracks(ids) from the FeatureStore `src`, then associate them with this
         store as one associate() call whose queries are those tracks (their kept rows, qualities, windows and merge
         histories), each merged into its winner or added whole; remove=True then takes them out of `src`.  The rows
-        never leave the device.  Returns the associate dict."""
+        never leave the device.  Returns the associate dict.  The search runs on feature_class; a merged track then
+        brings its other classes too, and a track without rows of feature_class is added whole."""
         if not isinstance(src, FeatureStore):
             raise TypeError("src must be an engine.FeatureStore")
+        self._use(feature_class)
         ids = np.ascontiguousarray(ids, dtype=np.uint64)
         q = len(ids)
         out = {"counts": np.zeros(q, np.int32), "winners": np.zeros((q, self.topn), np.uint64),
@@ -990,18 +1047,21 @@ class FeatureStore:
         pool = tracker.feature_history_pool()
         return pool["handed_out"] - pool["free"]
 
-    def fetch(self, ids, remove=False):
+    def fetch(self, ids, remove=False, feature_class=None):
         """(counts[n], features[n][max_observations][feature_dim]) of the tracks `ids`, oldest observation first (count 0:
-        not stored); remove=True takes them out of the store (fetch_tracks)."""
+        not stored, or no rows of feature_class); remove=True takes them out of the store (fetch_tracks), every class
+        with them."""
+        self._use(feature_class)
         ids = np.ascontiguousarray(ids, dtype=np.uint64)
         counts = np.zeros(len(ids), np.int32)
         feats = np.zeros((len(ids), self.K, self.D), np.float32)
         check(self._L.sb200_fstore_fetch(self._h, len(ids), ptr(ids), int(bool(remove)), ptr(counts), ptr(feats)))
         return counts, feats
 
-    def fetch_quality(self, ids, remove=False):
+    def fetch_quality(self, ids, remove=False, feature_class=None):
         """(counts, features, qualities) of a quality store: fetch() plus qualities[n][max_observations], the quality of
         each returned row (0 past a count); rows in the track's order, best first."""
+        self._use(feature_class)
         ids = np.ascontiguousarray(ids, dtype=np.uint64)
         counts = np.zeros(len(ids), np.int32)
         feats = np.zeros((len(ids), self.K, self.D), np.float32)
@@ -1080,4 +1140,5 @@ class FeatureStore:
         check(L.sb200_fstore_get_gate(h, C.byref(g)))
         self.gate = {v: k for k, v in GATES.items()}[g.value]
         self._keep = self.retention()[0]
+        self._read_classes()
         return self
