@@ -25,6 +25,8 @@ EUCLIDEAN, COSINE = 0, 1
 GATES = {None: 0, "same_source": 1, "any_source": 2}
 # retention rules (feature_store.cpp): the newest K, or the best by quality with a capacity growing with the merges
 RETENTIONS = {"newest": 0, "quality": 1}
+# voting rules (feature_store.cpp): TopNVoting or BestFitVoting
+VOTINGS = {"topn": 0, "best_fit": 1}
 
 
 def build(force: bool = False) -> str:
@@ -75,6 +77,8 @@ def lib():
             "ofs_set_classes": (C.c_int, [vp, i32, vp, vp]),
             "ofs_use_class": (C.c_int, [vp, C.c_uint64]),
             "ofs_class_counts": (i64, [vp, i32, vp, vp]),
+            "ofs_set_voting": (C.c_int, [vp, i32]),
+            "ofs_bestfit_voting": (C.c_int, [f32, i32, i32, i32, vp, vp, vp, vp, vp, vp]),
         }
         for name, (res, args) in sig.items():
             fn = getattr(L, name)
@@ -114,12 +118,23 @@ def round_rows(x, storage):
 
 def topn_voting(topn, max_distance, min_votes, ents):
     """TopNVoting::winners.  ents: list of (from, to, distance or None).  Returns {query: [(winner, weight), ...]}."""
+    return _voting(lib().ofs_topn_voting, topn, max_distance, min_votes, ents)
+
+
+def bestfit_voting(topn, max_distance, min_votes, ents):
+    """BestFitVoting::winners on TopN's groups: every element claims its track in the order weight descending, then
+    the group's first appearance; a loser's winner is its own query.  Each query's list is cut at topn after the claims.
+    ents and the result as for topn_voting."""
+    return _voting(lib().ofs_bestfit_voting, topn, max_distance, min_votes, ents)
+
+
+def _voting(fn, topn, max_distance, min_votes, ents):
     fr = np.array([e[0] for e in ents], dtype=np.uint64)
     to = np.array([e[1] for e in ents], dtype=np.uint64)
     fe = np.array([np.nan if e[2] is None else e[2] for e in ents], dtype=np.float32)
     cap = max(1, len(ents))
     q, w, wt = np.zeros(cap, np.uint64), np.zeros(cap, np.uint64), np.zeros(cap, np.float64)
-    n = lib().ofs_topn_voting(max_distance, min_votes, topn, len(ents), _p(fr), _p(to), _p(fe), _p(q), _p(w), _p(wt))
+    n = fn(max_distance, min_votes, topn, len(ents), _p(fr), _p(to), _p(fe), _p(q), _p(w), _p(wt))
     res = {}
     for i in range(n):
         res.setdefault(int(q[i]), []).append((int(w[i]), float(wt[i])))
@@ -131,7 +146,7 @@ class FeatureStore:
 
     def __init__(self, metric=EUCLIDEAN, distance_filter=100.0, max_observations=3, feature_dim=256, topn=1,
                  max_distance=100.0, min_votes=1, threads=1, gate=None, retention="newest", initial_capacity=4,
-                 merge_extension=1.5, classes=None):
+                 merge_extension=1.5, classes=None, voting="topn"):
         self._L = lib()
         self.K, self.D, self.topn, self.threads = int(max_observations), int(feature_dim), int(topn), int(threads)
         self._h = self._L.ofs_create(metric, distance_filter, self.K, self.D, self.topn, max_distance, min_votes)
@@ -153,6 +168,16 @@ class FeatureStore:
         if self._L.ofs_set_classes(self._h, len(cid), _p(cid), _p(dims)):
             raise ValueError("invalid classes")
         self._use(None)
+        self.set_voting(voting)
+
+    def set_voting(self, voting):
+        """"topn" or "best_fit": how every later search / associate / search_owned / associate_store votes."""
+        if voting not in VOTINGS or self._L.ofs_set_voting(self._h, VOTINGS[voting]):
+            raise ValueError(f"voting must be one of {list(VOTINGS)}")
+        self._voting = voting
+
+    def voting(self):
+        return self._voting
 
     def _use(self, feature_class):
         """Selects the class of the next call (None: the first declared one)."""

@@ -7,7 +7,9 @@
 //   - store order = insertion order; removal is a stable compaction;
 //   - entries are enumerated as (query, stored track in store order, query observation, track observation), oldest
 //     observations first; a group's f64 weight is summed in that order;
-//   - TopN ties (equal weights) go to the group that appeared first, i.e. the lower store position.
+//   - TopN ties (equal weights) go to the group that appeared first, i.e. the lower store position;
+//   - BestFit (ofs_set_voting) orders the call's elements by weight descending, then query (call order), then store
+//     position: the group's first appearance again.
 // It is the parity reference of tests/test_gpu_feature_store.py and the timed CPU baseline of
 // tools/feature_store_bench.py; the product never links it.
 // Track attributes (gate != 0): each track carries the CamTrackingAttributes of examples/track_merging.rs:218-245, a
@@ -58,10 +60,9 @@ struct PairHash {
   }
 };
 
-// TopNVoting::winners.  Returns, per query in order of first appearance, its at most `topn` elements, weight
-// descending, equal weights in order of the group's first appearance.
-std::vector<std::vector<Elt>> topn_voting(float max_distance, size_t min_votes, size_t topn, const std::vector<Ent>& ents,
-                                          std::vector<uint64_t>* queries) {
+// The groups of TopNVoting::winners and BestFitVoting::winners (topn.rs:78-117, best.rs:56-104 compute them alike): the
+// groups that reach min_votes, in order of first appearance, with their f64 weights
+std::vector<Elt> vote_groups(float max_distance, size_t min_votes, const std::vector<Ent>& ents) {
   float max_dist = -1.0f;
   std::vector<std::pair<std::pair<uint64_t, uint64_t>, std::vector<float>>> groups;
   std::unordered_map<std::pair<uint64_t, uint64_t>, size_t, PairHash> gidx;
@@ -78,23 +79,62 @@ std::vector<std::vector<Elt>> topn_voting(float max_distance, size_t min_votes, 
       groups[it->second].second.push_back(e.d);
     }
   }
-  std::vector<std::vector<Elt>> res;
-  std::unordered_map<uint64_t, size_t> qidx;
+  std::vector<Elt> out;
   for (auto& g : groups) {
     if (g.second.size() < min_votes) continue;
     double weight = 0.0;
     for (float d : g.second) weight += (double)(max_dist - d);
-    auto it = qidx.find(g.first.first);
-    if (it == qidx.end()) {
-      it = qidx.emplace(g.first.first, res.size()).first;
-      res.emplace_back();
-      queries->push_back(g.first.first);
-    }
-    res[it->second].push_back({g.first.first, g.first.second, weight});
+    out.push_back({g.first.first, g.first.second, weight});
   }
+  return out;
+}
+
+// the index of each element's query, queries numbered in order of first appearance (appended to *queries)
+std::vector<size_t> query_index(const std::vector<Elt>& el, std::vector<uint64_t>* queries) {
+  std::unordered_map<uint64_t, size_t> qidx;
+  std::vector<size_t> at;
+  for (const Elt& e : el) {
+    auto it = qidx.find(e.query);
+    if (it == qidx.end()) {
+      it = qidx.emplace(e.query, queries->size()).first;
+      queries->push_back(e.query);
+    }
+    at.push_back(it->second);
+  }
+  return at;
+}
+
+// TopNVoting::winners.  Returns, per query in order of first appearance, its at most `topn` elements, weight
+// descending, equal weights in order of the group's first appearance.
+std::vector<std::vector<Elt>> topn_voting(float max_distance, size_t min_votes, size_t topn, const std::vector<Ent>& ents,
+                                          std::vector<uint64_t>* queries) {
+  const std::vector<Elt> el = vote_groups(max_distance, min_votes, ents);
+  const std::vector<size_t> at = query_index(el, queries);
+  std::vector<std::vector<Elt>> res(queries->size());
+  for (size_t i = 0; i < el.size(); ++i) res[at[i]].push_back(el[i]);
   for (auto& r : res) {
     std::stable_sort(r.begin(), r.end(), [](const Elt& a, const Elt& b) { return a.weight > b.weight; });
     if (r.size() > topn) r.resize(topn);
+  }
+  return res;
+}
+
+// BestFitVoting::winners (best.rs:52-128) on TopN's groups: every element of the call, weight descending, equal weights
+// in order of the group's first appearance (in a store's enumeration: query, then store position), wins its track
+// unless an earlier element took it; the winner of one that does not is its own query (best.rs:112-120).  The claims
+// run over all elements; then, per query in order of first appearance, its first `topn` elements in that order.
+std::vector<std::vector<Elt>> bestfit_voting(float max_distance, size_t min_votes, size_t topn,
+                                             const std::vector<Ent>& ents, std::vector<uint64_t>* queries) {
+  std::vector<Elt> el = vote_groups(max_distance, min_votes, ents);
+  const std::vector<size_t> at = query_index(el, queries);
+  std::vector<size_t> ord(el.size());
+  for (size_t i = 0; i < ord.size(); ++i) ord[i] = i;
+  std::stable_sort(ord.begin(), ord.end(), [&](size_t a, size_t b) { return el[a].weight > el[b].weight; });
+  std::unordered_set<uint64_t> taken;
+  std::vector<std::vector<Elt>> res(queries->size());
+  for (size_t i : ord) {
+    if (!taken.insert(el[i].winner).second) el[i].winner = el[i].query;
+    if (res[at[i]].size() < topn) res[at[i]].push_back(el[i]);
   }
   return res;
 }
@@ -134,6 +174,7 @@ struct ofs_store {
   float filter, max_distance;
   int gate = 0;   // 0: no attributes; 1: windows disjoint and sources equal; 2: windows disjoint
   int retention = 0;   // 0: newest K; 1: best by quality, capacity growing with the merge history
+  int voting = 0;      // 0: TopNVoting; 1: BestFitVoting
   int init_cap = 0;           // retention 1: its parameters
   float ext = 0.0f;
   std::vector<int> cap_tab;   // retention 1: c(h) for h = 0 .. the first h with c(h) == K (or h = 0 alone when constant)
@@ -255,8 +296,8 @@ struct ofs_store {
     return 0;
   }
 
-  // foreign_track_distances + postprocess_distances (d < filter) + TopNVoting::winners
-  std::vector<std::vector<Elt>> search(const std::vector<Track>& qs, int threads) const {
+  // foreign_track_distances + postprocess_distances (d < filter) + the voting `rule` (-1: the store's)
+  std::vector<std::vector<Elt>> search(const std::vector<Track>& qs, int threads, int rule = -1) const {
     std::vector<std::vector<Ent>> per((size_t)qs.size());
     parallel_for((int)qs.size(), threads, [&](int b, int e) {
       for (int q = b; q < e; ++q)
@@ -273,7 +314,9 @@ struct ofs_store {
     std::vector<Ent> ents;
     for (auto& p : per) ents.insert(ents.end(), p.begin(), p.end());
     std::vector<uint64_t> order;
-    auto groups = topn_voting(max_distance, (size_t)std::max(min_votes, 0), (size_t)topn, ents, &order);
+    auto groups = (rule < 0 ? voting : rule) == 1
+                      ? bestfit_voting(max_distance, (size_t)std::max(min_votes, 0), (size_t)topn, ents, &order)
+                      : topn_voting(max_distance, (size_t)std::max(min_votes, 0), (size_t)topn, ents, &order);
     std::unordered_map<uint64_t, size_t> at;
     for (size_t i = 0; i < order.size(); ++i) at[order[i]] = i;
     std::vector<std::vector<Elt>> out(qs.size());
@@ -402,7 +445,9 @@ int ofs_search(ofs_store* s, int Q, const uint64_t* ids, const int32_t* offs, co
 }
 
 // one iteration of benches/feature_tracker.rs: search, then merge_external into results[0].winner_track or add_track
-// (the queries qs: fresh tracks built from a request, or stored tracks of another store, ofs_associate_store)
+// (the queries qs: fresh tracks built from a request, or stored tracks of another store, ofs_associate_store); a first
+// winner equal to the query's own id (BestFit: another query took the track) means add_track, as
+// examples/middleware_sort_tracker.rs:76-81 reads it
 static void associate_tracks(ofs_store* s, const std::vector<Track>& qs, int32_t* counts, uint64_t* winners,
                              double* weights, uint64_t* track_ids, uint8_t* merged, int threads) {
   const int Q = (int)qs.size();
@@ -410,7 +455,8 @@ static void associate_tracks(ofs_store* s, const std::vector<Track>& qs, int32_t
   s->write(r, counts, winners, weights);
   for (int q = 0; q < Q; ++q) {
     // with a gate, the window of the first winner as the queries merged into it earlier in this call extended it
-    if (!r[q].empty() && s->compatible(qs[q], s->tracks[s->pos.at(r[q][0].winner)])) {
+    if (!r[q].empty() && r[q][0].winner != qs[q].id &&
+        s->compatible(qs[q], s->tracks[s->pos.at(r[q][0].winner)])) {
       // Track::merge (src/track.rs:522-600): extend, then optimize keeps the newest K
       Track& dt = s->tracks[s->pos.at(r[q][0].winner)];
       s->merge_into(dt, qs[q]);
@@ -464,7 +510,7 @@ int64_t ofs_fetch(ofs_store* s, int n, const uint64_t* ids, int remove, int32_t*
   return found;
 }
 
-// owned_track_distances (src/track/store.rs:471-486) + TopNVoting::winners, written literally: fetch_tracks the queried
+// owned_track_distances (src/track/store.rs:471-486) + the store's voting, written literally: fetch_tracks the queried
 // set out of the store, search the remainder with the fetched tracks as queries, put the tracks back (at their store
 // positions: the order rule that replaces the reference's HashMap).  each != 0: once per id, in order.  An id that is not
 // stored gets count 0; an id twice is rejected (-1).
@@ -474,7 +520,7 @@ int ofs_search_owned(ofs_store* s, int n, const uint64_t* ids, int each, int32_t
   std::unordered_set<uint64_t> seen;
   for (int q = 0; q < n; ++q)
     if (!seen.insert(ids[q]).second) return -1;
-  auto owned = [&](int a, int b) {   // one owned_track_distances(ids[a .. b)) call
+  auto owned = [&](int a, int b, int rule) {   // one owned_track_distances(ids[a .. b)) call
     const std::vector<Track> saved = s->tracks;
     std::vector<Track> qs;
     for (int q = a; q < b; ++q) {   // fetch_tracks
@@ -484,7 +530,7 @@ int ofs_search_owned(ofs_store* s, int n, const uint64_t* ids, int each, int32_t
       s->tracks.erase(it);
     }
     s->reindex();
-    const auto r = s->search(qs, threads);
+    const auto r = s->search(qs, threads, rule);
     s->tracks = saved;   // add_track of every fetched track
     s->reindex();
     for (int q = a; q < b; ++q) {
@@ -500,10 +546,10 @@ int ofs_search_owned(ofs_store* s, int n, const uint64_t* ids, int each, int32_t
       }
     }
   };
-  if (each) {
-    for (int q = 0; q < n; ++q) owned(q, q + 1);
+  if (each) {   // one voting call per query: BestFit has no other query to lose a track to, and is TopN
+    for (int q = 0; q < n; ++q) owned(q, q + 1, 0);
   } else if (n > 0) {
-    owned(0, n);
+    owned(0, n, -1);
   }
   return 0;
 }
@@ -780,6 +826,14 @@ int ofs_associate_store(ofs_store* d, ofs_store* s, int n, const uint64_t* ids, 
   return 0;
 }
 
+// ---- voting (0: TopNVoting, 1: BestFitVoting): how search, associate, search_owned and associate_store vote; it may
+// change at any time.  -1 for an unknown rule.
+int ofs_set_voting(ofs_store* s, int rule) {
+  if (rule != 0 && rule != 1) return -1;
+  s->voting = rule;
+  return 0;
+}
+
 int64_t ofs_size(ofs_store* s) { return (int64_t)s->tracks.size(); }
 
 int64_t ofs_ids(ofs_store* s, int64_t cap, uint64_t* ids) {
@@ -787,14 +841,8 @@ int64_t ofs_ids(ofs_store* s, int64_t cap, uint64_t* ids) {
   return (int64_t)s->tracks.size();
 }
 
-// TopNVoting::winners on an entry list (feat NaN == None).  Writes n results (query, winner, weight): queries in order
-// of first appearance, each query's results weight descending, equal weights in order of first appearance.
-int ofs_topn_voting(float max_distance, int min_votes, int topn, int n_ent, const uint64_t* from, const uint64_t* to,
-                    const float* feat, uint64_t* out_query, uint64_t* out_winner, double* out_weight) {
-  std::vector<Ent> ents((size_t)n_ent);
-  for (int i = 0; i < n_ent; ++i) ents[i] = {from[i], to[i], feat[i]};
-  std::vector<uint64_t> order;
-  const auto groups = topn_voting(max_distance, (size_t)std::max(min_votes, 0), (size_t)topn, ents, &order);
+static int write_voting(const std::vector<std::vector<Elt>>& groups, uint64_t* out_query, uint64_t* out_winner,
+                        double* out_weight) {
   int n = 0;
   for (const auto& g : groups)
     for (const Elt& e : g) {
@@ -804,6 +852,28 @@ int ofs_topn_voting(float max_distance, int min_votes, int topn, int n_ent, cons
       ++n;
     }
   return n;
+}
+
+// TopNVoting::winners on an entry list (feat NaN == None).  Writes n results (query, winner, weight): queries in order
+// of first appearance, each query's results weight descending, equal weights in order of first appearance.
+int ofs_topn_voting(float max_distance, int min_votes, int topn, int n_ent, const uint64_t* from, const uint64_t* to,
+                    const float* feat, uint64_t* out_query, uint64_t* out_winner, double* out_weight) {
+  std::vector<Ent> ents((size_t)n_ent);
+  for (int i = 0; i < n_ent; ++i) ents[i] = {from[i], to[i], feat[i]};
+  std::vector<uint64_t> order;
+  return write_voting(topn_voting(max_distance, (size_t)std::max(min_votes, 0), (size_t)topn, ents, &order), out_query,
+                      out_winner, out_weight);
+}
+
+// BestFitVoting::winners on an entry list, as bestfit_voting above (claims over every element, each query's list cut at
+// topn); results written as ofs_topn_voting writes them.
+int ofs_bestfit_voting(float max_distance, int min_votes, int topn, int n_ent, const uint64_t* from, const uint64_t* to,
+                       const float* feat, uint64_t* out_query, uint64_t* out_winner, double* out_weight) {
+  std::vector<Ent> ents((size_t)n_ent);
+  for (int i = 0; i < n_ent; ++i) ents[i] = {from[i], to[i], feat[i]};
+  std::vector<uint64_t> order;
+  return write_voting(bestfit_voting(max_distance, (size_t)std::max(min_votes, 0), (size_t)topn, ents, &order),
+                      out_query, out_winner, out_weight);
 }
 
 }  // extern "C"

@@ -475,7 +475,8 @@ int64_t sb200_fstore_size(sb200_fstore* s);
 /* Ids of the stored tracks in store order; writes min(cap, size) and returns the size. */
 int64_t sb200_fstore_ids(sb200_fstore* s, int64_t cap, uint64_t* ids);
 /* Device times (ms) of the last search / associate / add / search_owned / merge_owned call: distances, TopN, apply (0 for
- * a stage that did not run).  search_owned counts its on-device row staging as distances and sums its chunks. */
+ * a stage that did not run).  search_owned counts its on-device row staging as distances and sums its chunks.  Under
+ * BestFit voting (sb200_fstore_set_voting) the TopN stage includes the claim passes. */
 int sb200_fstore_last_stage_ms(sb200_fstore* s, float* out3);
 
 /* Element type (SB200_FEATURE_F32 | _F16 | _BF16) of the `features` argument of every later sb200_fstore_add / _search /
@@ -687,6 +688,38 @@ int sb200_fstore_associate_attr(sb200_fstore* s, int32_t n_queries, const uint64
  * the ids were found, or a negative status. */
 int64_t sb200_fstore_fetch_attr(sb200_fstore* s, int32_t n, const uint64_t* ids, uint64_t* source, int64_t* t_start,
                                 int64_t* t_end);
+
+/* ---- voting: TopNVoting or BestFitVoting on top of the store's distances ----
+ * The reference's TrackStore leaves the voting to its caller (foreign_track_distances -> any Voting::winners).  The
+ * store has the two built-in rules of src/track/voting:
+ *   SB200_FSTORE_VOTING_TOPN (0, the default): TopNVoting (topn.rs:74-138), each query ranked on its own, as every call
+ *     above describes.  Several queries of one associate call whose first winner is the same track are all merged
+ *     into it.
+ *   SB200_FSTORE_VOTING_BEST_FIT (1): BestFitVoting (best.rs:52-128), the rule of the reference's VisualVoting.  Groups,
+ *     votes, min_votes, max_distance, max_dist and the f64 weights are TopN's.  Every group of the call that reaches
+ *     min_votes is an element; elements are ordered by weight descending, then query (call order) ascending, then store
+ *     position ascending (the reference sorts stably over HashMap order, which leaves ties open; this order is the
+ *     store's own).  An element wins its track iff no earlier element names that track: the heaviest group naming a
+ *     track takes it, the lowest query on ties.  All groups claim, also those past a query's topn cut.
+ *     - search, search_owned (each == 0) and the search part of every associate: counts[q] and the weights are TopN's
+ *       (q's elements in order, at most topn); the winner of an element that does not win its track is the query's own
+ *       id (best.rs:112-120).
+ *     - associate in every form, associate_store and associate_wasted: a query is merged into its first element's track
+ *       iff that element wins it; otherwise it becomes a new track under its own id, as the reference's callers read a
+ *       winner equal to the query (examples/middleware_sort_tracker.rs:76-81).  So no two queries of one call merge into
+ *       one track, and merged[q] can be 0 with counts[q] > 0.  On a gated store every destination is exclusive and every
+ *       scored pair compatible, so the gate keeps each of them.
+ *     - search_owned with each == 1: one voting call per query, where BestFit gives TopN's results.
+ *   The claims cost two more passes over the call's distance matrix, which sb200_fstore_last_stage_ms counts in the
+ *   voting stage.  Quality stores, feature classes, storage, feature and column types and gates work unchanged.
+ * The rule is handle state, like the feature type: it decides how a call reads the store, not what the store holds, so
+ * it may be changed at any time and is not saved in the blob (every blob is what it was); a new or loaded store votes
+ * TopN.  sb200_fstore_associate_store votes with dst's rule.  No per-call argument. */
+#define SB200_FSTORE_VOTING_TOPN 0
+#define SB200_FSTORE_VOTING_BEST_FIT 1
+/* SB200_ERR_INVALID, changing nothing, for an unknown rule. */
+int sb200_fstore_set_voting(sb200_fstore* s, int32_t rule);
+int sb200_fstore_get_voting(sb200_fstore* s, int32_t* out);
 
 /* ---- retention by quality: each track keeps its best observations, and its capacity grows with its merges ----
  * The store semantics of examples/track_merging.rs (its `optimize`, :279-297, with the defaults of :257-265) in place of

@@ -132,6 +132,8 @@ class FstoreBlobHeaderV2(C.Structure):
 FSTORE_BLOB_VERSION_QUALITY, FSTORE_BLOB_SECTIONS_V3 = 3, 10
 # retention rules of the feature store (sb200_fstore_set_retention)
 FSTORE_KEEP_NEWEST, FSTORE_KEEP_BEST_QUALITY = 0, 1
+# voting rules of the feature store (sb200_fstore_set_voting)
+FSTORE_VOTING_TOPN, FSTORE_VOTING_BEST_FIT = 0, 1
 
 
 class FstoreBlobHeaderV3(C.Structure):
@@ -182,6 +184,7 @@ EXPORTS = [
     "sb200_fstore_search_quality", "sb200_fstore_associate_quality", "sb200_fstore_fetch_quality",
     "sb200_fstore_merge_history", "sb200_fstore_find_baked", "sb200_fstore_associate_store",
     "sb200_fstore_set_classes", "sb200_fstore_get_classes", "sb200_fstore_use_class", "sb200_fstore_class_counts",
+    "sb200_fstore_set_voting", "sb200_fstore_get_voting",
 ]
 
 
@@ -284,6 +287,8 @@ def lib():
         "sb200_fstore_set_storage_type": (C.c_int, [vp, i32]),
         "sb200_fstore_set_gate": (C.c_int, [vp, i32]),
         "sb200_fstore_get_gate": (C.c_int, [vp, C.POINTER(i32)]),
+        "sb200_fstore_set_voting": (C.c_int, [vp, i32]),
+        "sb200_fstore_get_voting": (C.c_int, [vp, C.POINTER(i32)]),
         "sb200_fstore_add_attr": (C.c_int, [vp, i32, vp, C.POINTER(FstoreAttrs), vp, vp, vp]),
         "sb200_fstore_search_attr": (C.c_int, [vp, i32, vp, vp, C.POINTER(FstoreAttrs), vp, vp, vp, vp, vp, vp]),
         "sb200_fstore_associate_attr": (C.c_int, [vp, i32, vp, vp, C.POINTER(FstoreAttrs), vp, vp, vp, vp, vp, vp, vp,

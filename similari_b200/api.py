@@ -536,7 +536,8 @@ class _VisualBase(_TrackerBase):
                         feature_class=None) -> List[Tuple[WastedSortTrack, Optional[int]]]:
         """Collects the wasted tracks as wasted() does and associates each one's observed features (the present ones,
         oldest first) with the feature track `store` under the id track.id + id_offset, as one
-        FeatureStore.associate call would, without the features leaving the device (the TrackStore side of the
+        FeatureStore.associate call would (under the store's voting rule: with "best_fit" no two tracks of one
+        collection merge into one stored track), without the features leaving the device (the TrackStore side of the
         reference's examples/track_merging.rs).  Returns [(track, where it went in the store)], the store track id
         being None for a track without a feature; the box histories are those wasted() reports.  feature_class: the
         store's class the features go to (None: its first declared class).  An extension with no PyO3 counterpart in the

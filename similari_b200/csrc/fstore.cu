@@ -211,6 +211,7 @@ struct sb200_fstore {
   size_t cap = 0;
   DBuf feat, cnt, start, ids, run;
   int gate = SB200_FSTORE_GATE_NONE;
+  int voting = SB200_FSTORE_VOTING_TOPN;     // how calls read the store; handle state, not saved in the blob
   DBuf asrc, at0, at1;                       // gated store: [cap] source, t_start, t_end
   int keep = SB200_FSTORE_KEEP_NEWEST;       // retention rule, and its parameters for a quality store
   int init_cap = 4;
@@ -243,6 +244,7 @@ struct sb200_fstore {
   std::unordered_map<uint64_t, int> hpos;    // id -> store position
   // per-call buffers
   DBuf dreq, dres, plan, qnorm, snorm, dist, gpos, gout, dcol;
+  DBuf claim;                                // BestFit voting: [live] u64 column maxima, then [live] i32 claimants
   sb::PinnedBuf<cudaHostAllocDefault> hreq, hres, hcol;   // staging, contents not kept
 
   ~sb200_fstore() {
@@ -886,8 +888,21 @@ struct sb200_fstore {
     return 0;
   }
 
-  // the TopN results of Q queries (hres, layout RL) as counts[Q], winners[Q][topn] and weights[Q][topn], zero past a count
-  void read_results(const ResLayout& RL, int Q, int32_t* counts, uint64_t* winners, double* weights) const {
+  // BestFit voting (sb200_fstore_set_voting), after TopN on the call c: the claims across its queries, rewriting the
+  // results and, with want_dest, the destinations; nothing under TopN
+  int claim_best_fit(const sb::FsStore& s, const sb::FsCall& c, bool want_dest) {
+    if (voting != SB200_FSTORE_VOTING_BEST_FIT) return 0;
+    if (int rc = claim.ensure((size_t)std::max(s.live, 1) * 12)) return rc;
+    unsigned long long* wmax = claim.as<unsigned long long>();
+    CU(sb::fs_launch_claim(o.max_distance, o.min_votes, o.topn, want_dest, s, c, wmax,
+                           reinterpret_cast<int*>(wmax + s.live), st));
+    return 0;
+  }
+
+  // the TopN results of Q queries (hres, layout RL) as counts[Q], winners[Q][topn] and weights[Q][topn], zero past a count;
+  // an element BestFit rewrote (position -2) names the query's own id, qids[q]
+  void read_results(const ResLayout& RL, int Q, const uint64_t* qids, int32_t* counts, uint64_t* winners,
+                    double* weights) const {
     const char* h = static_cast<const char*>(hres.p);
     const double* w = reinterpret_cast<const double*>(h + RL.w);
     const int* cn = reinterpret_cast<const int*>(h + RL.cnt);
@@ -896,7 +911,7 @@ struct sb200_fstore {
       counts[q] = cn[q];
       for (int e = 0; e < o.topn; ++e) {
         const size_t i = (size_t)q * o.topn + e;
-        winners[i] = e < cn[q] ? hid[ps[i]] : 0;
+        winners[i] = e < cn[q] ? (ps[i] == -2 ? qids[q] : hid[ps[i]]) : 0;
         weights[i] = e < cn[q] ? w[i] : 0.0;
       }
     }
@@ -965,14 +980,16 @@ struct sb200_fstore {
     sb::fs_launch_dist(o.metric, o.distance_filter, s, c, st, sb::kFsForeign, nullptr, gated ? &g : nullptr);
     CU(cudaEventRecord(ev[1], st));
     sb::fs_launch_topn(o.max_distance, o.min_votes, topn, assoc, s, c, st);
+    if (int rc = claim_best_fit(s, c, assoc)) return rc;
     CU(cudaEventRecord(ev[2], st));
+    // BestFit destinations are exclusive and every scored pair is compatible, so the gate keeps each of them
     if (assoc && gated) sb::fs_launch_gate_resolve(c, g, st);
     if (decided) {   // associate_store of several classes on a quality store: the caller applies every class
       decided->resize(Q);
       CU(cudaMemcpyAsync(hres.p, dres.p, RL.total, cudaMemcpyDeviceToHost, st));
       CU(cudaMemcpyAsync(decided->data(), c.dest, (size_t)Q * 4, cudaMemcpyDeviceToHost, st));
       if (int rc = finish(S > 0 ? 0 : 1, 2)) return rc;
-      read_results(RL, Q, counts, winners, weights);
+      read_results(RL, Q, qids, counts, winners, weights);
       return 0;
     }
     if (qa) sb::fs_launch_qmerge(s, c, qc, st, tq ? tq->hq : nullptr);
@@ -980,20 +997,21 @@ struct sb200_fstore {
     if (assoc && gated) sb::fs_launch_attr_new(s.live, c, g, st);
     CU(cudaEventRecord(ev[3], st));
     CU(cudaMemcpyAsync(hres.p, dres.p, RL.total, cudaMemcpyDeviceToHost, st));
-    // gated or quality associate: the position each query ended up at (>= live: a new track)
+    // gated, quality or BestFit associate: the position each query ended up at (>= live: a new track)
+    const bool best = voting == SB200_FSTORE_VOTING_BEST_FIT;
     std::vector<int> where;
-    if (assoc && (gated || qa)) {
+    if (assoc && (gated || qa || best)) {
       where.resize(Q);
       CU(cudaMemcpyAsync(where.data(), c.dest, (size_t)Q * 4, cudaMemcpyDeviceToHost, st));
     }
     if (int rc = finish(S > 0 ? 0 : 1, assoc ? 3 : 2)) return rc;   // no distance stage on an empty store
-    read_results(RL, Q, counts, winners, weights);
+    read_results(RL, Q, qids, counts, winners, weights);
     if (assoc) {
       // Track::merge with merge_history = true appends the query's history: [id], or a stored track's whole one
       auto qhist = [&](int q) { return tq ? (*tq->hist)[q] : std::vector<uint64_t>{qids[q]}; };
       for (int q = 0; q < Q; ++q) {
-        // a first winner the gate refused leaves a new track
-        merged[q] = gated || qa ? where[q] < live : counts[q] > 0;
+        // a first winner the gate refused, or another query claimed under BestFit, leaves a new track
+        merged[q] = gated || qa || best ? where[q] < live : counts[q] > 0;
         track_ids[q] = merged[q] ? winners[(size_t)q * topn] : qids[q];
         if (qa && merged[q]) {
           const std::vector<uint64_t> h = qhist(q);
@@ -1570,10 +1588,12 @@ struct sb200_fstore {
                        reinterpret_cast<const unsigned char*>(dreq.as<char>() + L.excl), gate ? &g : nullptr);
     CU(cudaEventRecord(ev[1], st));
     sb::fs_launch_topn(o.max_distance, o.min_votes, topn, false, s, c, st, mode);
+    if (!each)   // each == 1 is one voting call per query: no claim crosses queries, and BestFit is TopN
+      if (int rc = claim_best_fit(s, c, false)) return rc;
     CU(cudaEventRecord(ev[2], st));
     CU(cudaMemcpyAsync(hres.p, dres.p, RL.total, cudaMemcpyDeviceToHost, st));
     if (int rc = finish(0, 2)) return rc;   // summed over the chunks
-    read_results(RL, Q, counts + a, winners + (size_t)a * topn, weights + (size_t)a * topn);
+    read_results(RL, Q, qids + a, counts + a, winners + (size_t)a * topn, weights + (size_t)a * topn);
     return 0;
   }
 
@@ -2257,6 +2277,21 @@ int sb200_fstore_get_gate(sb200_fstore* s, int32_t* out) {
   if (!s) return no_handle();
   if (!out) return fail(SB200_ERR_INVALID, "out is NULL");
   *out = s->gate;
+  return 0;
+}
+
+int sb200_fstore_set_voting(sb200_fstore* s, int32_t rule) {
+  if (!s) return no_handle();
+  if (rule != SB200_FSTORE_VOTING_TOPN && rule != SB200_FSTORE_VOTING_BEST_FIT)
+    return fail(SB200_ERR_INVALID, "unknown voting rule %d", rule);
+  s->voting = rule;
+  return 0;
+}
+
+int sb200_fstore_get_voting(sb200_fstore* s, int32_t* out) {
+  if (!s) return no_handle();
+  if (!out) return fail(SB200_ERR_INVALID, "out is NULL");
+  *out = s->voting;
   return 0;
 }
 

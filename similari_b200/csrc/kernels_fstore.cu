@@ -276,6 +276,32 @@ __device__ __forceinline__ bool fs_better(double wa, int pa, double wb, int pb) 
   return wa > wb || (wa == wb && pa < pb);
 }
 
+// The votes of the group (query rows a0 .. a0 + na, stored track t) and, in *w, its weight: fs_topn_kernel's loop (kept
+// inline there, so that its instances keep their code), the same operations in the same order, so a group weighs the
+// same bits in TopN and in the BestFit claim passes.
+__device__ __forceinline__ int fs_group(const FsStore& s, const FsCall& c, int t, int a0, int na, float maxd,
+                                        float max_distance, double* w) {
+  const int K = s.K;
+  const size_t S = (size_t)s.live * K;
+  const int n = s.cnt[t], st = s.start[t];
+  int votes = 0;
+  double acc = 0.0;
+  for (int a = 0; a < na; ++a) {
+    const float* dr = c.dist + (size_t)(a0 + a) * S + (size_t)t * K;
+    int slot = st;
+    for (int b = 0; b < n; ++b) {
+      const float d = dr[slot];
+      if (d <= max_distance) {   // false for NaN: dropped entries
+        ++votes;
+        acc = acc + (double)(maxd - d);
+      }
+      slot = slot + 1 == K ? 0 : slot + 1;
+    }
+  }
+  *w = acc;
+  return votes;
+}
+
 // PERQ: max_dist is the query's own (maxkey[q], kFsOwnedEach), else the call's (maxkey[0])
 template <int PERQ>
 __global__ void __launch_bounds__(kTopnThreads) fs_topn_kernel(FsStore s, FsCall c, float max_distance, int min_votes,
@@ -348,6 +374,50 @@ __global__ void __launch_bounds__(kTopnThreads) fs_topn_kernel(FsStore s, FsCall
     c.out_cnt[q] = nl;
     if (want_dest) c.dest[q] = nl > 0 ? l_p[0] : -1;
   }
+}
+
+// ------------------------------------------------------------------------------------------------ BestFit claims
+// BestFitVoting::winners (src/track/voting/best.rs:52-128) over one call's groups, after TopN: a group (q, t) that
+// reaches min_votes wins track t iff it comes first, among all the groups of the call naming t, in the order weight
+// descending, then q ascending.  Every group counts, also those past a query's topn cut.  No sort is needed: a group wins
+// iff it holds the column maximum.  Each pass is laid out as TopN (one CTA per query, a thread per stored track) and
+// recomputes the weights with fs_group.  Weights are >= +0 (every kept d is <= max_dist), so their f64 bits order as
+// u64 and one atomicMax folds them.
+//   pass 0: wmax[t] = the largest weight of a group naming t (a stale read of wmax only skips an atomic that would
+//           not raise it);
+//   pass 1: qmin[t] = the lowest q whose group on t weighs wmax[t].
+__global__ void __launch_bounds__(kTopnThreads) fs_claim_kernel(FsStore s, FsCall c, float max_distance, int min_votes,
+                                                                 int pass, unsigned long long* __restrict__ wmax,
+                                                                 int* __restrict__ qmin) {
+  const int q = blockIdx.x;
+  const float maxd = fs_unkey(*c.maxkey);
+  const unsigned long long qid = c.qid[q];
+  const int a0 = c.qoff[q], na = c.qoff[q + 1] - a0;
+  const int need = max(1, min_votes);
+  for (int t = threadIdx.x; t < s.live; t += kTopnThreads) {
+    double w;
+    if (s.ids[t] == qid || fs_group(s, c, t, a0, na, maxd, max_distance, &w) < need) continue;
+    const unsigned long long b = (unsigned long long)__double_as_longlong(w);
+    if (pass == 0) {
+      if (b > wmax[t]) atomicMax(wmax + t, b);
+    } else if (b == wmax[t]) {
+      atomicMin(qmin + t, q);
+    }
+  }
+}
+
+// Element e of query q's TopN list keeps its track only if q claimed it; otherwise its position becomes -2, which the
+// host reports as the query's own id (best.rs:112-120).  dest[q] (want_dest) = the first element's track when q claimed
+// it, else -1.
+__global__ void fs_claim_final_kernel(FsCall c, int topn, int want_dest, const int* __restrict__ qmin) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (long long)c.Q * topn) return;
+  const int q = (int)(i / topn), e = (int)(i % topn);
+  if (e >= c.out_cnt[q]) return;
+  const int p = c.out_pos[i];
+  const bool won = qmin[p] == q;
+  if (!won) c.out_pos[i] = -2;
+  if (want_dest && e == 0) c.dest[q] = won ? p : -1;
 }
 
 // ------------------------------------------------------------------------------------------------ apply
@@ -963,6 +1033,20 @@ void fs_launch_topn(float max_distance, int min_votes, int topn, bool want_dest,
   else
     fs_topn_kernel<0><<<c.Q, kTopnThreads, 0, st>>>(s, c, max_distance, min_votes, topn, want_dest ? 1 : 0);
   note_launch();
+}
+
+cudaError_t fs_launch_claim(float max_distance, int min_votes, int topn, bool want_dest, const FsStore& s,
+                            const FsCall& c, unsigned long long* wmax, int* qmin, cudaStream_t st) {
+  if (c.Q == 0 || s.live == 0) return cudaSuccess;
+  cudaError_t e = cudaMemsetAsync(wmax, 0, (size_t)s.live * 8, st);
+  if (e == cudaSuccess) e = cudaMemsetAsync(qmin, 0x7f, (size_t)s.live * 4, st);   // above every query index
+  if (e != cudaSuccess) return e;
+  for (int pass = 0; pass < 2; ++pass)
+    fs_claim_kernel<<<c.Q, kTopnThreads, 0, st>>>(s, c, max_distance, min_votes, pass, wmax, qmin);
+  const long long n = (long long)c.Q * topn;
+  fs_claim_final_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(c, topn, want_dest ? 1 : 0, qmin);
+  note_launch(3);
+  return cudaSuccess;
 }
 
 void fs_launch_owned_stage(const FsStore& s, const FsCall& c, const int* qpos, float* rows, cudaStream_t st) {

@@ -122,6 +122,12 @@ void fs_launch_dist(int metric, float filter, const FsStore& s, const FsCall& c,
                     const unsigned char* excl = nullptr, const FsGate* gate = nullptr);
 void fs_launch_topn(float max_distance, int min_votes, int topn, bool want_dest, const FsStore& s, const FsCall& c,
                     cudaStream_t st, int mode = kFsForeign);
+// BestFit voting, after fs_launch_topn on the same call (the call's max_dist in maxkey[0]): every group of the call claims
+// its track, the heaviest group, lower query on ties, winning it; a reported element whose track another query claimed
+// gets position -2 (the host reports the query's id), and with want_dest dest[q] = the first element's track if q
+// claimed it, else -1.  wmax / qmin: [live] scratch, initialised here.  Returns the error of that initialisation.
+cudaError_t fs_launch_claim(float max_distance, int min_votes, int topn, bool want_dest, const FsStore& s,
+                            const FsCall& c, unsigned long long* wmax, int* qmin, cudaStream_t st);
 // out[2 i] = cnt[pos[i]], out[2 i + 1] = start[pos[i]]: the ring state of the tracks an owned call touches
 void fs_launch_peek(const FsStore& s, const int* pos, int n, int* out, cudaStream_t st);
 // merge_owned: scratch[m] = stored row src[m], then stored row dst[m] = scratch[m] (rows index feat as [cap * K][d8];

@@ -659,12 +659,14 @@ GATES = {None: _lib.FSTORE_GATE_NONE, "same_source": _lib.FSTORE_GATE_SAME_SOURC
          "any_source": _lib.FSTORE_GATE_ANY_SOURCE}
 # retention rules of the feature store (sb200_fstore_set_retention)
 RETENTIONS = {"newest": _lib.FSTORE_KEEP_NEWEST, "quality": _lib.FSTORE_KEEP_BEST_QUALITY}
+# voting rules of the feature store (sb200_fstore_set_voting)
+VOTINGS = {"topn": _lib.FSTORE_VOTING_TOPN, "best_fit": _lib.FSTORE_VOTING_BEST_FIT}
 
 
 class FeatureStore:
     """Device-resident feature track store: the reference's TrackStore for feature-only tracks (one feature class, no
-    track attributes) with TopNVoting(topn, max_distance, min_votes) on top (sb200_fstore_*).  Each track keeps its
-    newest `max_observations` observations.  Queries are given in CSR form: ids[q] with the feature rows
+    track attributes) with TopNVoting(topn, max_distance, min_votes) (or BestFitVoting, voting=) on top
+    (sb200_fstore_*).  Each track keeps its newest `max_observations` observations.  Queries are given in CSR form: ids[q] with the feature rows
     features[offsets[q]:offsets[q + 1]], oldest first.  numpy in, numpy out.
 
     Features: a float16 array is sent as it is; any other dtype is widened to float32.  After set_feature_type("bf16")
@@ -697,11 +699,18 @@ class FeatureStore:
     declared class) and work on that class's rows alone; a stored track without rows of the class takes no part in a
     search of it.  merge_owned and associate_store move every class a track holds.  classes() and class_counts(ids)
     report the classes and each track's rows in each.  A store of the single class 0 saves as before; any other
-    declaration saves as blob version 4, which carries the class table."""
+    declaration saves as blob version 4, which carries the class table.
+
+    Voting: voting="topn" (the default) ranks each query on its own, so several queries of one associate call can merge
+    into the same track.  voting="best_fit" is the reference's BestFitVoting (the rule of its VisualVoting): over all the
+    queries of a call, each stored track goes to the query whose group weighs most for it (the lower query index on
+    ties), a reported winner that another query took is replaced by the query's own id, and associate merges a query
+    only into a track it took, else adds it as a new track.  search_owned(each=True) is unchanged by it.  set_voting()
+    changes the rule at any time; it is not saved in the blob, and load() takes voting= (default "topn")."""
 
     def __init__(self, metric="euclidean", distance_filter=100.0, max_observations=3, feature_dim=256, topn=1,
                  max_distance=100.0, min_votes=1, device=0, storage="f32", gate=None, retention="newest",
-                 initial_capacity=4, merge_extension=1.5, classes=None):
+                 initial_capacity=4, merge_extension=1.5, classes=None, voting="topn"):
         if metric not in METRICS:
             raise ValueError(f"metric must be one of {sorted(METRICS)}")
         if storage not in FEATURE_TYPES:
@@ -729,6 +738,20 @@ class FeatureStore:
             ids, dims = np.array(list(cls), np.uint64), np.array(list(cls.values()), np.int32)
             check(self._L.sb200_fstore_set_classes(h, len(ids), ptr(ids), ptr(dims)))
         self._read_classes()
+        self.set_voting(voting)
+
+    def set_voting(self, voting):
+        """sb200_fstore_set_voting: "topn" or "best_fit", the rule of every later search, associate (every form,
+        associate_wasted and associate_store included) and search_owned."""
+        if voting not in VOTINGS:
+            raise ValueError(f"voting must be one of {list(VOTINGS)}")
+        check(self._L.sb200_fstore_set_voting(self._h, VOTINGS[voting]))
+
+    def voting(self):
+        """The voting rule, "topn" or "best_fit"."""
+        v = C.c_int32(0)
+        check(self._L.sb200_fstore_get_voting(self._h, C.byref(v)))
+        return {k: n for n, k in VOTINGS.items()}[v.value]
 
     def _read_classes(self):
         n = int(check(self._L.sb200_fstore_get_classes(self._h, 0, None, None)))
@@ -1103,7 +1126,7 @@ class FeatureStore:
         return out[:n]
 
     def last_stage_ms(self):
-        """Device times (ms) of the last call: distances, TopN, apply."""
+        """Device times (ms) of the last call: distances, voting (TopN, plus the claims under BestFit), apply."""
         out = np.zeros(3, np.float32)
         check(self._L.sb200_fstore_last_stage_ms(self._h, ptr(out)))
         return out
@@ -1121,9 +1144,12 @@ class FeatureStore:
         return _device_blob(lambda p, c, n: self._L.sb200_fstore_save(self._h, p, c, n), d_ptr, cap, C.c_uint64)
 
     @classmethod
-    def load(cls, blob_or_ptr, nbytes=None, device=0):
+    def load(cls, blob_or_ptr, nbytes=None, device=0, voting="topn"):
         """sb200_fstore_load: a new store on `device` from a blob of save() (a uint8 array / bytes) or at a raw device
-        address `blob_or_ptr` of `nbytes` bytes.  The options, and the feature type set, are the blob's."""
+        address `blob_or_ptr` of `nbytes` bytes.  The options, and the feature type set, are the blob's; the voting rule,
+        which the blob does not hold, is `voting`."""
+        if voting not in VOTINGS:
+            raise ValueError(f"voting must be one of {list(VOTINGS)}")
         p, n, keep = _blob_src(blob_or_ptr, nbytes)
         L = lib()
         h = C.c_void_p()
@@ -1141,4 +1167,5 @@ class FeatureStore:
         self.gate = {v: k for k, v in GATES.items()}[g.value]
         self._keep = self.retention()[0]
         self._read_classes()
+        self.set_voting(voting)
         return self
