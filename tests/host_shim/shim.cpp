@@ -87,6 +87,9 @@ void shim_pos_sort(const float* x, int n, float* kx, int* kidx) {
 extern "C" void shim_sincos(const float* angles, long long n, double* s, double* c) {
   for (long long i = 0; i < n; ++i) sb::sc::sincos_cr((double)angles[i], &s[i], &c[i]);
 }
+extern "C" void shim_sincos_f64(const double* x, long long n, double* s, double* c) {
+  for (long long i = 0; i < n; ++i) sb::sc::sincos_cr(x[i], &s[i], &c[i]);
+}
 extern "C" void shim_libm_sincos(const float* angles, long long n, double* s, double* c) {
   for (long long i = 0; i < n; ++i) { s[i] = sin((double)angles[i]); c[i] = cos((double)angles[i]); }
 }
