@@ -78,7 +78,8 @@ typedef struct {
   int32_t visual_kind;
   float visual_threshold;
   int32_t feature_dim;            /* D; 0 for Sort / BatchSort */
-  int32_t visual_max_observations;
+  int32_t visual_max_observations; /* observations kept per track, 1..32 (reference default 5, its examples 25); above
+                                    * 32 the tracker is refused with SB200_ERR_CAPACITY before anything is created */
   int32_t visual_min_votes;
   int32_t visual_minimal_track_length;
   float visual_minimal_area;
@@ -319,7 +320,7 @@ int sb200_visual_cost_matrix(int32_t visual_kind, float threshold, const float* 
                              const float* track_features, int32_t n, int32_t d, float* out_mn, int32_t device);
 /* SortVoting::winners on a dense cost matrix (NaN == None): winner[m] = track index or -1 (new track). */
 int sb200_sort_voting(float threshold, const float* cost_mn, int32_t m, int32_t n, int32_t* winner, int32_t device);
-/* VisualVoting::winners on dense matrices: pos[m][n], vis[m][n][k] (NaN == None). */
+/* VisualVoting::winners on dense matrices: pos[m][n], vis[m][n][k] (NaN == None), k = observations per track in 1..32. */
 int sb200_visual_voting(float positional_threshold, int32_t min_votes, const float* pos_mn, const float* vis_mnk,
                         int32_t m, int32_t n, int32_t k, int32_t* winner, uint8_t* voting_type, int32_t device);
 /* Kalman filter steps on packed states (src/utils/kalman/kalman_2d_box.rs:58-148), n states at once. */

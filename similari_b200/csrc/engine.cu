@@ -91,8 +91,8 @@ int make_params(const sb200_options& o, sb::Params* out) {
     if (o.visual_kind != SB200_VIS_EUCLIDEAN && o.visual_kind != SB200_VIS_COSINE)
       return fail(SB200_ERR_INVALID, "unknown visual metric %d", o.visual_kind);
     if (o.feature_dim <= 0) return fail(SB200_ERR_INVALID, "feature_dim must be > 0 for visual trackers");
-    if (o.visual_max_observations < 1 || o.visual_max_observations > sb::kMaxObs)
-      return fail(SB200_ERR_CAPACITY, "visual_max_observations must be in [1, %d]", sb::kMaxObs);
+    if (o.visual_max_observations < 1 || o.visual_max_observations > sb::kMaxObsWide)
+      return fail(SB200_ERR_CAPACITY, "visual_max_observations must be in [1, %d]", sb::kMaxObsWide);
     p.visual_threshold = o.visual_threshold;
     p.feature_dim = o.feature_dim;
     p.d8 = (o.feature_dim + 7) / 8 * 8;

@@ -438,6 +438,78 @@ __global__ void vis_dense_meta_kernel(Params p, TrackStore ts, Frame f, int max_
   if ((threadIdx.x & 31) == 0 && cmax > 0.0f) atomicMax(reinterpret_cast<int*>(scene_cmax) + s, __float_as_int(cmax));
 }
 
+// K > kMaxObs: one warp per arena block, lane k reading logical observation k and lane ph writing physical row ph, the
+// two joined through the warp's shared-memory row (rowinfo and colc of every physical slot).  Same records as above.
+constexpr int DMW_WARPS = 4;
+__global__ void __launch_bounds__(DMW_WARPS * 32)
+vis_dense_meta_wide_kernel(Params p, TrackStore ts, Frame f, int max_blocks, int cstep, DenseTrackMeta* tmeta, int2* rowinfo,
+                           float* slab_colc, float* slab_cmax, float* slab_ktf, unsigned int* slab_vmask,
+                           unsigned int* slab_bmask, float* scene_cmax, int* dense_bad) {
+  __shared__ int2 s_ri[DMW_WARPS][32];
+  __shared__ float s_colc[DMW_WARPS][32];
+  const int s = blockIdx.y;
+  const SceneDesc sc = f.scenes[s];
+  const int K = p.max_obs;
+  const int wi = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int b = blockIdx.x * DMW_WARPS + wi;
+  if (!(b < sc.nb && b < max_blocks)) return;   // warp-uniform
+  const unsigned int all = 0xffffffffu;
+  const size_t sbase = (size_t)sc.slot * ts.track_cap;
+  const int n = ts.blk_owner ? ts.blk_owner[sbase + b] : b;
+  s_ri[wi][lane] = make_int2(-1, -1);
+  s_colc[wi][lane] = 0.0f;
+  __syncwarp();
+  bool use = false;   // lane's logical observation holds a feature of a valid track
+  float nb2 = 0.0f;
+  if (n >= 0) {
+    const size_t ti = sbase + n;
+    const int on = ts.obs_n[ti];
+    const unsigned int tep = ts.epoch[ti];
+    const unsigned int delta = sc.epoch > tep ? sc.epoch - tep : tep - sc.epoch;
+    const bool valid = (ts.feat_cnt[ti] >= p.min_track_length) && ((unsigned int)p.max_idle_epochs >= delta);
+    const int k = lane;
+    if (k < K && k < on && ts.obs_hasf[ti * K + k]) {
+      const int ph = ts.obs_phys[ti * K + k];
+      const size_t frow = (sbase + b) * K + ph;
+      int fr = -1;
+      if (valid) {
+        fr = (int)frow;
+        nb2 = ts.fnorm2[frow];
+        if (!dense_norm_ok(p, nb2)) dense_bad[s] = 1;
+        s_colc[wi][ph] = p.visual_kind == 1 ? rsqrtf(nb2) : nb2;
+        use = true;
+      }
+      s_ri[wi][ph] = make_int2(n * K + k, fr);
+    }
+  }
+  float cmax = use ? nb2 : 0.0f;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) cmax = fmaxf(cmax, __shfl_xor_sync(all, cmax, o));
+  const int kt = __popc(__ballot_sync(all, use));
+  __syncwarp();
+  if (lane == 0) {
+    DenseTrackMeta tm;
+    tm.n = n; tm.kt = n >= 0 ? kt : 0; tm.cmax = n >= 0 ? cmax : 0.0f; tm.pad = 0;
+    tmeta[sc.blk_off + b] = tm;
+    if (cmax > 0.0f) atomicMax(reinterpret_cast<int*>(scene_cmax) + s, __float_as_int(cmax));
+  }
+  const int need_votes = p.min_votes > 1 ? p.min_votes : 1;
+  const float ktf = (n >= 0 && kt >= need_votes) ? (float)kt : 0.0f;
+  const int ph = lane;
+  if (ph < K) {
+    const int2 ri = s_ri[wi][ph];
+    const int prow = b * K + ph;
+    rowinfo[(size_t)sc.blk_off * K + prow] = ri;
+    const int j = prow / cstep, cc = prow - j * cstep;
+    const size_t slab = (size_t)sc.slab_off + j;
+    slab_colc[slab * TC_BN + cc] = s_colc[wi][ph];
+    slab_cmax[slab * TC_BN + cc] = cmax;
+    slab_ktf[slab * TC_BN + cc] = ktf;
+    if (ri.y >= 0) atomicOr(&slab_vmask[slab * (TC_BN / 32) + (cc >> 5)], 1u << (cc & 31));
+    if (ph == K - 1) atomicOr(&slab_bmask[slab * (TC_BN / 32) + (cc >> 5)], 1u << (cc & 31));
+  }
+}
+
 __global__ void vis_dense_rowmeta_kernel(Params p, Frame f, VisRowMeta* rowmeta) {
   int g = blockIdx.x * blockDim.x + threadIdx.x;
   if (g >= f.total) return;
@@ -522,6 +594,8 @@ __global__ void __launch_bounds__(256) vis_dense_sample_kernel(Params p, TrackSt
 // One CTA per scene.  Pass A: best lower bound of every row (candidate) and column (block) of the weight matrix; pass B:
 // every group whose upper bound reaches one of the two is emitted to the scene's pair list with all its valid observations.
 constexpr int SEL_T = 512;
+// WIDE (K > kMaxObs): an emitted group reads its block's rowinfo twice (count, then list) instead of keeping it per thread.
+template <bool WIDE>
 __global__ void __launch_bounds__(SEL_T) vis_dense_select_kernel(Params p, Frame f, const __half2* ws, const DenseTrackMeta* tmeta,
                                                                  const int2* rowinfo, const int* maxc_cnt, const int* max_nan,
                                                                  int* dense_bad, int* dbg_counts, const unsigned int* rowb,
@@ -622,17 +696,20 @@ __global__ void __launch_bounds__(SEL_T) vis_dense_select_kernel(Params p, Frame
               // the group may hold a row or column maximum: all its valid observations go to the exact pass
               const int g = sc.det_base + m;
               int cnt = 0;
-              int2 ri[kMaxObs];
+              int2 ri[WIDE ? 1 : kMaxObs];
               for (int ph = 0; ph < K; ++ph) {
-                ri[ph] = rowinfo[(size_t)sc.blk_off * K + (size_t)b * K + ph];
-                cnt += ri[ph].y >= 0;
+                const int r = WIDE ? 0 : ph;
+                ri[r] = rowinfo[(size_t)sc.blk_off * K + (size_t)b * K + ph];
+                cnt += ri[r].y >= 0;
               }
               int pos = atomicAdd(&f.vis_cnt[s], cnt);
               for (int ph = 0; ph < K; ++ph) {
-                if (ri[ph].y < 0) continue;
+                const int r = WIDE ? 0 : ph;
+                if (WIDE) ri[r] = rowinfo[(size_t)sc.blk_off * K + (size_t)b * K + ph];
+                if (ri[r].y < 0) continue;
                 if (pos < sc.vis_lcap) {
                   VisPair vp;
-                  vp.g = g; vp.row = ri[ph].y; vp.scene = s; vp.outcol = ri[ph].x;
+                  vp.g = g; vp.row = ri[r].y; vp.scene = s; vp.outcol = ri[r].x;
                   f.vis_pairs[sc.vis_lbase + pos] = vp;
                 }
                 ++pos;
@@ -672,7 +749,14 @@ int launch_vis_dense(const Params& p, const TrackStore& ts, const Frame& f, int 
     cudaMemsetAsync(tc.d_rowb, 0, (size_t)f.total * kDenseKClasses * 4, st);
     cudaMemsetAsync(tc.d_colb, 0, (size_t)tc.blk_ub * 4, st);
   }
-  if (tc.max_blocks > 0) {
+  const bool wide = p.max_obs > kMaxObs;
+  if (tc.max_blocks > 0 && wide) {
+    dim3 grid((tc.max_blocks + DMW_WARPS - 1) / DMW_WARPS, n_scenes);
+    vis_dense_meta_wide_kernel<<<grid, DMW_WARPS * 32, 0, st>>>(p, ts, f, tc.max_blocks, tc.cstep, tc.tmeta, tc.rowinfo,
+                                                              tc.slab_colc, tc.slab_cmax, tc.slab_ktf, tc.slab_vmask,
+                                                              tc.slab_bmask, tc.scene_cmax, tc.dense_bad);
+    note_launch();
+  } else if (tc.max_blocks > 0) {
     dim3 grid((tc.max_blocks + 127) / 128, n_scenes);
     vis_dense_meta_kernel<<<grid, 128, 0, st>>>(p, ts, f, tc.max_blocks, tc.cstep, tc.tmeta, tc.rowinfo, tc.slab_colc, tc.slab_cmax,
                                                 tc.slab_ktf, tc.slab_vmask, tc.slab_bmask, tc.scene_cmax,
@@ -735,10 +819,10 @@ int launch_vis_dense(const Params& p, const TrackStore& ts, const Frame& f, int 
   }
   {
     const size_t smem = (size_t)std::max(1, tc.max_blocks) * 6 + 64;
-    if (smem > 48 * 1024) cudaFuncSetAttribute(vis_dense_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    vis_dense_select_kernel<<<n_scenes, SEL_T, smem, st>>>(p, f, reinterpret_cast<const __half2*>(tc.ws), tc.tmeta, tc.rowinfo,
-                                                           tc.maxc_cnt, tc.dense_bad, tc.dense_bad, tc.dbg_counts, tc.d_rowb,
-                                                           tc.d_colb, fused ? 1 : 0);
+    const auto kernel = wide ? vis_dense_select_kernel<true> : vis_dense_select_kernel<false>;
+    if (smem > 48 * 1024) cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    kernel<<<n_scenes, SEL_T, smem, st>>>(p, f, reinterpret_cast<const __half2*>(tc.ws), tc.tmeta, tc.rowinfo, tc.maxc_cnt,
+                                          tc.dense_bad, tc.dense_bad, tc.dbg_counts, tc.d_rowb, tc.d_colb, fused ? 1 : 0);
     note_launch();
   }
   return 0;

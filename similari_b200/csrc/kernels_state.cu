@@ -92,7 +92,10 @@ __global__ void __launch_bounds__(AT) apply_rank_kernel(Params p, TrackStore ts,
   }
 }
 
-// Phase 2 of apply: one thread per detection creates its track or merges into the track it won.
+// Phase 2 of apply: one thread per detection creates its track or merges into the track it won.  WIDE (K > kMaxObs):
+// a merge leaves the track's observation list, its feature count and the detection's feature row to apply_obs_wide_kernel,
+// which runs next, one warp per detection, instead of holding K-sized lists per thread.
+template <bool WIDE>
 __global__ void __launch_bounds__(256) apply_kernel(Params p, TrackStore ts, Frame f, unsigned long long id_base) {
   const int K = p.max_obs;
   {
@@ -177,7 +180,7 @@ __global__ void __launch_bounds__(256) apply_kernel(Params p, TrackStore ts, Fra
       int on = 0;
       unsigned char l_hasf[kMaxObs], l_phys[kMaxObs]; float l_q[kMaxObs];
       size_t blk = idx;
-      if (p.is_visual) {
+      if (!WIDE && p.is_visual) {
         on = ts.obs_n[idx];
         for (int k = 0; k < K; ++k) {   // slots at and beyond obs_n were never written
           const bool have = k < on;
@@ -198,50 +201,52 @@ __global__ void __launch_bounds__(256) apply_kernel(Params p, TrackStore ts, Fra
       if (p.is_visual) {
         o_vt = (signed char)f.c_vt[g];
         ts.vt[idx] = o_vt;
-        // is_merge && !feature_can_be_used(collect thresholds) => feature dropped (visual_sort/metric.rs:327-337)
-        bool keep = (flags & 1) != 0;
-        if (keep) {
-          bool ok = quality >= p.min_quality_collect;
-          if (p.use_own_area && f.in_own) ok = ok && (f.in_own[g] >= p.min_own_collect);
-          ok = ok && (box_area(cb.aspect, cb.height) >= p.min_area);
-          keep = ok;
-        }
-        // optimize_observations: retain featured, stable sort by quality desc, drop last when len >= max
-        unsigned char phys[kMaxObs]; float q[kMaxObs];
-        int cnt = 0;
-        unsigned int used = 0;
-        for (int k = 0; k < K; ++k) {
-          if (k < on && l_hasf[k]) {
-            phys[cnt] = l_phys[k]; q[cnt] = l_q[k];
-            ++cnt;
+        if (!WIDE) {   // WIDE: apply_obs_wide_kernel
+          // is_merge && !feature_can_be_used(collect thresholds) => feature dropped (visual_sort/metric.rs:327-337)
+          bool keep = (flags & 1) != 0;
+          if (keep) {
+            bool ok = quality >= p.min_quality_collect;
+            if (p.use_own_area && f.in_own) ok = ok && (f.in_own[g] >= p.min_own_collect);
+            ok = ok && (box_area(cb.aspect, cb.height) >= p.min_area);
+            keep = ok;
           }
+          // optimize_observations: retain featured, stable sort by quality desc, drop last when len >= max
+          unsigned char phys[kMaxObs]; float q[kMaxObs];
+          int cnt = 0;
+          unsigned int used = 0;
+          for (int k = 0; k < K; ++k) {
+            if (k < on && l_hasf[k]) {
+              phys[cnt] = l_phys[k]; q[cnt] = l_q[k];
+              ++cnt;
+            }
+          }
+          for (int a = 1; a < cnt; ++a) {  // stable insertion sort, descending quality
+            unsigned char pa = phys[a]; float qa = q[a];
+            int b = a - 1;
+            while (b >= 0 && q[b] < qa) { phys[b + 1] = phys[b]; q[b + 1] = q[b]; --b; }
+            phys[b + 1] = pa; q[b + 1] = qa;
+          }
+          if (cnt >= K && cnt > 0) --cnt;
+          for (int k = 0; k < cnt; ++k) used |= 1u << phys[k];
+          int freep = 0;
+          while (used & (1u << freep)) ++freep;
+          // push new, swap(0, last)
+          unsigned char hasf_l[kMaxObs];
+          for (int k = 0; k < cnt; ++k) hasf_l[k] = 1;
+          phys[cnt] = (unsigned char)freep; q[cnt] = quality; hasf_l[cnt] = keep ? 1 : 0;
+          ++cnt;
+          { unsigned char tp = phys[0]; phys[0] = phys[cnt - 1]; phys[cnt - 1] = tp;
+            float tq = q[0]; q[0] = q[cnt - 1]; q[cnt - 1] = tq;
+            unsigned char th = hasf_l[0]; hasf_l[0] = hasf_l[cnt - 1]; hasf_l[cnt - 1] = th; }
+          int fc = 0;
+          for (int k = 0; k < cnt; ++k) {
+            ts.obs_phys[idx * K + k] = phys[k]; ts.obs_q[idx * K + k] = q[k]; ts.obs_hasf[idx * K + k] = hasf_l[k];
+            fc += hasf_l[k];
+          }
+          ts.obs_n[idx] = (unsigned char)cnt;
+          ts.feat_cnt[idx] = (unsigned char)fc;
+          if (keep) fdst = (int)(blk * K + freep);
         }
-        for (int a = 1; a < cnt; ++a) {  // stable insertion sort, descending quality
-          unsigned char pa = phys[a]; float qa = q[a];
-          int b = a - 1;
-          while (b >= 0 && q[b] < qa) { phys[b + 1] = phys[b]; q[b + 1] = q[b]; --b; }
-          phys[b + 1] = pa; q[b + 1] = qa;
-        }
-        if (cnt >= K && cnt > 0) --cnt;
-        for (int k = 0; k < cnt; ++k) used |= 1u << phys[k];
-        int freep = 0;
-        while (used & (1u << freep)) ++freep;
-        // push new, swap(0, last)
-        unsigned char hasf_l[kMaxObs];
-        for (int k = 0; k < cnt; ++k) hasf_l[k] = 1;
-        phys[cnt] = (unsigned char)freep; q[cnt] = quality; hasf_l[cnt] = keep ? 1 : 0;
-        ++cnt;
-        { unsigned char tp = phys[0]; phys[0] = phys[cnt - 1]; phys[cnt - 1] = tp;
-          float tq = q[0]; q[0] = q[cnt - 1]; q[cnt - 1] = tq;
-          unsigned char th = hasf_l[0]; hasf_l[0] = hasf_l[cnt - 1]; hasf_l[cnt - 1] = th; }
-        int fc = 0;
-        for (int k = 0; k < cnt; ++k) {
-          ts.obs_phys[idx * K + k] = phys[k]; ts.obs_q[idx * K + k] = q[k]; ts.obs_hasf[idx * K + k] = hasf_l[k];
-          fc += hasf_l[k];
-        }
-        ts.obs_n[idx] = (unsigned char)cnt;
-        ts.feat_cnt[idx] = (unsigned char)fc;
-        if (keep) fdst = (int)(blk * K + freep);
       }
     }
     ts.epoch[idx] = sc.epoch;
@@ -266,7 +271,7 @@ __global__ void __launch_bounds__(256) apply_kernel(Params p, TrackStore ts, Fra
 #pragma unroll
       for (int i = 0; i < 4; ++i) v2[i] = make_double2(vx[2 * i], vx[2 * i + 1]);
     }
-    if (f.feat_dst) f.feat_dst[g] = fdst;
+    if (f.feat_dst && !(WIDE && !isnew)) f.feat_dst[g] = fdst;
     if (ts.hblk) {
       // feature history: every observation pushes its feature, or None, before the collect gate
       // (VisualMetric::optimize, visual_sort/metric.rs:319-324).  A new track takes the pool block of its frame-wide rank:
@@ -298,6 +303,78 @@ __global__ void __launch_bounds__(256) apply_kernel(Params p, TrackStore ts, Fra
     if (f.o_vt) f.o_vt[g] = p.is_visual ? (o_vt < 0 ? (unsigned char)1 : (unsigned char)o_vt) : (unsigned char)1;
     if (f.o_pred) write_box(f.o_pred + (size_t)g * 6, pred);
     if (f.o_obs) write_box(f.o_obs + (size_t)g * 6, isnew ? Box{f.in_boxes[(size_t)g * 6], f.in_boxes[(size_t)g * 6 + 1], f.in_boxes[(size_t)g * 6 + 2], f.in_boxes[(size_t)g * 6 + 3], f.in_boxes[(size_t)g * 6 + 4], f.in_boxes[(size_t)g * 6 + 5]} : cb);
+  }
+}
+
+// The observation list of a visual merge for K > kMaxObs (K <= 32): one warp per detection, lane k holding logical
+// observation k (physical slot, quality, feature flag).  Same steps as apply_kernel<false>, in the same order:
+// optimize_observations keeps the observations with a feature, insertion-sorts them by descending quality (one
+// insertion per step; the ballot finds where the shifting stops, exactly as the sequential loop does, NaN qualities
+// included), drops the last when K are kept, then pushes the new observation into the lowest free physical slot and swaps
+// it to the front.  A 32-bit mask holds every physical slot, which bounds K at 32.
+__global__ void __launch_bounds__(256) apply_obs_wide_kernel(Params p, TrackStore ts, Frame f) {
+  const int w = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
+  if (w >= f.total) return;
+  const int g = f.det0 + w;
+  const int win = f.winner[g];
+  if (win < 0) return;   // a new track: apply_kernel wrote its single observation
+  const int K = p.max_obs;
+  const unsigned int all = 0xffffffffu;
+  const SceneDesc& sc = f.scenes[f.app_rank[g].x];
+  const size_t idx = (size_t)sc.slot * ts.track_cap + win;
+  const unsigned char flags = f.c_flags[g];
+  const float quality = f.in_quality ? f.in_quality[g] : 1.0f;
+  bool keep = (flags & 1) != 0;   // the collect gate of apply_kernel
+  if (keep) {
+    const float* cbp = f.c_box + (size_t)g * 6;
+    bool ok = quality >= p.min_quality_collect;
+    if (p.use_own_area && f.in_own) ok = ok && (f.in_own[g] >= p.min_own_collect);
+    ok = ok && (box_area(cbp[3], cbp[4]) >= p.min_area);
+    keep = ok;
+  }
+  const int on = ts.obs_n[idx];
+  const bool have = lane < on && lane < K;   // slots at and beyond obs_n were never written
+  const bool retain = have && ts.obs_hasf[idx * K + lane];
+  const int ph0 = retain ? ts.obs_phys[idx * K + lane] : 0;
+  const float q0 = retain ? ts.obs_q[idx * K + lane] : 0.0f;
+  // retain featured, in logical order: lane j takes the j-th retained observation
+  const unsigned int rmask = __ballot_sync(all, retain);
+  int cnt = __popc(rmask);
+  int src = 0;   // lowest bit s with popc(rmask & bits 0..s) == lane + 1 (binary search; 31 when lane >= cnt)
+  for (int b = 16; b > 0; b >>= 1)
+    if (__popc(rmask & ((2u << (src + b - 1)) - 1u)) < lane + 1) src += b;
+  int ph = __shfl_sync(all, ph0, src);
+  float q = __shfl_sync(all, q0, src);
+  for (int a = 1; a < cnt; ++a) {   // stable insertion sort, descending quality
+    const float qa = __shfl_sync(all, q, a);
+    const int pa = __shfl_sync(all, ph, a);
+    // the sequential loop shifts while q[b] < qa, from b = a - 1 down: it stops below the highest b < a without that
+    const unsigned int stop = __ballot_sync(all, lane < a && !(q < qa));
+    const int pos = stop ? 32 - __clz((int)stop) : 0;
+    const float qu = __shfl_up_sync(all, q, 1);
+    const int pu = __shfl_up_sync(all, ph, 1);
+    if (lane > pos && lane <= a) { q = qu; ph = pu; }
+    if (lane == pos) { q = qa; ph = pa; }
+  }
+  if (cnt >= K && cnt > 0) --cnt;
+  const unsigned int used = __reduce_or_sync(all, lane < cnt ? 1u << ph : 0u);
+  const int freep = __ffs((int)~used) - 1;   // cnt < K <= 32: a slot is free
+  // push new, swap(0, last)
+  unsigned char hasf = lane < cnt ? 1 : 0;
+  if (lane == cnt) { ph = freep; q = quality; hasf = keep ? 1 : 0; }
+  ++cnt;
+  const int from = lane == 0 ? cnt - 1 : (lane == cnt - 1 ? 0 : lane);
+  ph = __shfl_sync(all, ph, from);
+  q = __shfl_sync(all, q, from);
+  hasf = (unsigned char)__shfl_sync(all, (int)hasf, from);
+  if (lane < cnt) {
+    ts.obs_phys[idx * K + lane] = (unsigned char)ph; ts.obs_q[idx * K + lane] = q; ts.obs_hasf[idx * K + lane] = hasf;
+  }
+  const int fc = __popc(__ballot_sync(all, lane < cnt && hasf));
+  if (lane == 0) {
+    ts.obs_n[idx] = (unsigned char)cnt;
+    ts.feat_cnt[idx] = (unsigned char)fc;
+    if (f.feat_dst) f.feat_dst[g] = keep ? (int)(feat_block(ts, sc.slot, idx) * K + freep) : -1;
   }
 }
 
@@ -520,8 +597,14 @@ void launch_apply(const Params& p, const TrackStore& ts, const Frame& f, int n_s
   apply_rank_kernel<<<n_scenes, AT, 0, st>>>(p, ts, f, n_scenes, d_n_tracks);
   note_launch();
   if (f.total > 0) {
-    apply_kernel<<<(f.total + 255) / 256, 256, 0, st>>>(p, ts, f, id_base);
-    note_launch();
+    if (p.max_obs > kMaxObs) {
+      apply_kernel<true><<<(f.total + 255) / 256, 256, 0, st>>>(p, ts, f, id_base);
+      apply_obs_wide_kernel<<<(unsigned)(((long long)f.total * 32 + 255) / 256), 256, 0, st>>>(p, ts, f);
+      note_launch(2);
+    } else {
+      apply_kernel<false><<<(f.total + 255) / 256, 256, 0, st>>>(p, ts, f, id_base);
+      note_launch();
+    }
   }
 }
 
@@ -574,6 +657,8 @@ __device__ __forceinline__ void compact_rows(T* arr, size_t base, int width, con
   }
 }
 
+// WIDE (K > kMaxObs): the observation columns move as K-wide rows through compact_rows instead of per-thread lists.
+template <bool WIDE>
 __global__ void __launch_bounds__(WT) waste_kernel(Params p, TrackStore ts, const unsigned int* cur_epoch,
                                                    const unsigned long long* scene_ids, int* n_tracks, WastedBuf wb,
                                                    const SceneDesc* scenes, int* frame_out, unsigned long long* id_counter,
@@ -694,7 +779,7 @@ __global__ void __launch_bounds__(WT) waste_kernel(Params p, TrackStore ts, cons
           v_on = ts.obs_n[t]; v_fc = ts.feat_cnt[t];
           if (arena) v_fb = ts.fblk[t];
           if (ts.hblk) v_hb = ts.hblk[t];
-          for (int k = 0; k < K; ++k) {   // slots at and beyond obs_n were never written
+          for (int k = 0; k < (WIDE ? 0 : K); ++k) {   // slots at and beyond obs_n were never written
             const bool have = k < (int)v_on;
             v_ph[k] = have ? ts.obs_phys[t * K + k] : (unsigned char)0; v_hf[k] = have ? ts.obs_hasf[t * K + k] : (unsigned char)0;
             v_q[k] = have ? ts.obs_q[t * K + k] : 0.0f;
@@ -710,7 +795,7 @@ __global__ void __launch_bounds__(WT) waste_kernel(Params p, TrackStore ts, cons
         ts.obs_n[t] = v_on; ts.feat_cnt[t] = v_fc;
         if (arena) ts.fblk[t] = v_fb;
         if (ts.hblk) ts.hblk[t] = v_hb;
-        for (int k = 0; k < K; ++k) { ts.obs_phys[t * K + k] = v_ph[k]; ts.obs_hasf[t * K + k] = v_hf[k]; ts.obs_q[t * K + k] = v_q[k]; }
+        for (int k = 0; k < (WIDE ? 0 : K); ++k) { ts.obs_phys[t * K + k] = v_ph[k]; ts.obs_hasf[t * K + k] = v_hf[k]; ts.obs_q[t * K + k] = v_q[k]; }
       }
     }
     __syncthreads();
@@ -719,6 +804,11 @@ __global__ void __launch_bounds__(WT) waste_kernel(Params p, TrackStore ts, cons
   compact_rows(ts.obs, base, 6, s_dst, first, n);
   compact_rows(ts.kst, base, ts.kst_stride, s_dst, first, n);
   if (p.positional_kind == 1) compact_rows(ts.vert, base, 8, s_dst, first, n);
+  if (WIDE && p.is_visual) {
+    compact_rows(ts.obs_phys, base, K, s_dst, first, n);
+    compact_rows(ts.obs_hasf, base, K, s_dst, first, n);
+    compact_rows(ts.obs_q, base, K, s_dst, first, n);
+  }
   if (ts.hist_len > 1) {
     compact_rows(ts.hist_pred, base, ts.hist_len * 6, s_dst, first, n);
     compact_rows(ts.hist_obs, base, ts.hist_len * 6, s_dst, first, n);
@@ -736,9 +826,10 @@ static void launch_waste_kernel(const Params& p, const TrackStore& ts, int n_cta
                                 const SceneDesc* scenes, int* frame_out, unsigned long long* id_counter, long long id_add,
                                 const int* new_count, cudaStream_t st) {
   const size_t smem = (size_t)std::max(1, ts.track_cap) * sizeof(int);   // s_dst for the largest possible scene
-  if (smem > 48 * 1024) cudaFuncSetAttribute(waste_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  waste_kernel<<<n_ctas, WT, smem, st>>>(p, ts, d_cur_epoch, d_scene_ids, d_n_tracks, wb, scenes, frame_out, id_counter,
-                                         id_add, new_count, n_ctas);
+  const auto kernel = p.max_obs > kMaxObs ? waste_kernel<true> : waste_kernel<false>;
+  if (smem > 48 * 1024) cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  kernel<<<n_ctas, WT, smem, st>>>(p, ts, d_cur_epoch, d_scene_ids, d_n_tracks, wb, scenes, frame_out, id_counter, id_add,
+                                   new_count, n_ctas);
   note_launch();
 }
 

@@ -322,7 +322,7 @@ int sb200_visual_cost_matrix(int32_t visual_kind, float threshold, const float* 
 static int run_voting(bool visual, float threshold, int min_votes, const float* pos_mn, const float* vis_mnk, int m, int n,
                       int k, int32_t* winner, uint8_t* voting_type, int device) {
   if (m < 0 || n < 0 || (m > 0 && !winner) || (m > 0 && n > 0 && !pos_mn)) return fail(SB200_ERR_INVALID, "bad arguments");
-  if (visual && (k < 1 || k > sb::kMaxObs || (m > 0 && n > 0 && !vis_mnk))) return fail(SB200_ERR_INVALID, "bad arguments");
+  if (visual && (k < 1 || k > sb::kMaxObsWide || (m > 0 && n > 0 && !vis_mnk))) return fail(SB200_ERR_INVALID, "bad arguments");
   // Which voting kernel runs: by default the tracker's rule (the sparse kernel on the entry lists unless a list exceeds
   // its capacity); SB200_VOTE_KERNEL=dense|sparse|prepass forces one, so that a test can hand each kernel the matrix of
   // its choosing.  A forced kernel the rule would not allow is an error, never a silent switch to the other one.

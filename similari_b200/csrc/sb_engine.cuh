@@ -26,7 +26,8 @@ namespace sb {
 
 constexpr int kMaxConstraints = 8;
 constexpr int kNumSms = 132;  // H100 SXM: grid sizes of the launches that do not query the device
-constexpr int kMaxObs = 8;  // visual_max_observations supported on device (reference default 5)
+constexpr int kMaxObs = 8;  // visual_max_observations the per-thread kernels keep in registers (reference default 5)
+constexpr int kMaxObsWide = 32;  // visual_max_observations supported on device: above kMaxObs, one warp lane per observation
 constexpr int kStateStride = 32;   // floats per Kalman state row in the tracker's store (kStateFloats padded to 128 bytes)
 constexpr int kMaxHist = 64;  // box history kept per track on the device (history_length above it, or 0 = unlimited, is capped)
 
