@@ -249,6 +249,18 @@ int64_t sb200_idle_tracks(sb200_tracker* t, uint64_t scene_id, int64_t cap, uint
 /* Debug / parity: dense dump of one scene's store in store order.  states: [n][30] = mean[10] + 5 x (Pxx,Pxv,Pvx,Pvv). */
 int64_t sb200_scene_tracks(sb200_tracker* t, uint64_t scene_id, int64_t cap, uint64_t* ids, float* boxes,
                            float* states30, int32_t* feature_counts);
+/* Track::obs of every live track of scene `scene_id`, in store order (the tracks sb200_scene_tracks lists): ids[i],
+ * n_obs[i], and per logical observation j < K = visual_max_observations: has_feature[i][K], quality[i][K] and
+ * features[i][K][feature_dim] (f32; zeros where the observation has no feature and past n_obs[i]; quality is the
+ * observation's, with or without a feature, and 0 past n_obs[i]).  The logical order is the one the reference's optimize
+ * leaves (visual_sort/metric.rs:129-154, 297-374): the older featured observations sorted by descending quality, the last
+ * one dropped at K, the newest pushed and swapped to the front.  One gather kernel writes the rows in that order from the
+ * tracker's f32 arena into a staging buffer, and one copy brings it down.  Any output may be NULL.
+ * Drains completed frames like every query; no auto-waste step; changes nothing.  Returns the number of tracks written
+ * (at most cap; 0 for a scene the tracker does not hold), or a negative status.  SB200_ERR_INVALID for a NULL tracker,
+ * a tracker that is not visual, cap < 0. */
+int64_t sb200_scene_observations(sb200_tracker* t, uint64_t scene_id, int64_t cap, uint64_t* ids, int32_t* n_obs,
+                                 uint8_t* has_feature, float* quality, float* features);
 /* Debug / parity: last frame's positional cost matrix of a scene ([m][n] f32, NaN == None), n = the scene's live tracks
  * in store order.  Visual trackers on the tensor-core path evaluate the positional metric lazily -- only for candidates
  * the visual BestFit pass left undecided against tracks it did not claim, the pairs VisualVoting::winners
@@ -818,6 +830,40 @@ int64_t sb200_fstore_find_baked(sb200_fstore* s, int64_t now, int64_t baked_peri
 int sb200_fstore_associate_store(sb200_fstore* dst, sb200_fstore* src, int32_t n, const uint64_t* ids, int32_t remove,
                                  int32_t* counts, uint64_t* winners, double* weights, uint64_t* track_ids,
                                  uint8_t* merged);
+
+/* Re-identification: the live tracks of visual tracker `t` as the queries of ONE search of store `s`; no feature row
+ * crosses PCIe.  Pair i names live track track_ids[i] of scene scene_ids[i], as sb200_scene_observations lists it.
+ * found[i] is 0 when the tracker holds no such live track (tracks expire between frames, also early into the wasted
+ * buffer): not an error.  The query of a found track is all p of its present observations in Track::obs order (see
+ * sb200_scene_observations), under the id track_ids[i] + id_offset (mod 2^64); feature_counts[i] = p, queried[i] = 1
+ * when p > 0.  The store then applies its own query rule, the reference's composition of a track built from Track::obs
+ * in order: a newest store keeps the last max_observations rows, a quality store the best c(1) rows by quality.
+ * Because optimize swaps the newest observation to the front, Track::obs is the newest observation, then the other
+ * featured ones by descending quality except the best one, which the swap moved to the end: a newest store whose
+ * max_observations is below p drops the NEWEST observation first.
+ * The queried pairs, in pair order, form one search (max_dist over the whole call) with the store's voting rule and its
+ * selected class (sb200_fstore_use_class).  On a quality store every row carries its observation's quality (the
+ * _search_quality form); a gated store takes the caller's (source, t_start, t_end) per pair in `attrs` (the _search_attr
+ * form), an ungated one takes attrs == NULL.  Outputs per pair, 0 where not queried: counts[n], winners[n][topn],
+ * weights[n][topn] as sb200_fstore_search gives them; any output may be NULL.
+ * Exactness: every output equals, bit for bit, sb200_scene_observations, then each found track's present rows in order
+ * (with their qualities on a quality store) as the f32 request of sb200_fstore_search (or its _quality / _attr form),
+ * for every metric, storage type, voting rule, retention rule, gate and class.
+ * Read-only: both blobs are unchanged and no auto-waste step runs; later frames are those of a tracker that never made
+ * the call.
+ * Refusals, SB200_ERR_INVALID with sb200_last_error naming the cause, before anything changes: a NULL handle, n < 0, a
+ * tracker that is not visual, tracker and store on different devices, the selected class's dim differing from the
+ * tracker's feature_dim (once the tracker's dimension is fixed), a (scene, id) pair given twice (or two queried pairs
+ * with one query id), attrs missing on a gated store or given on an ungated one (or a t_start > t_end), a NaN quality on
+ * a quality store.  SB200_ERR_CAPACITY: more than 2^30 observation pairs (the call is not split, which would change
+ * max_dist).  The call is synchronous: it drains the tracker, reads the arena on the store's stream once the tracker's
+ * stream is idle, and returns once the store's stream has finished, so a frame enqueued after it never races its reads.
+ * n == 0 and calls with no queried pair launch no store kernel.  sb200_fstore_last_stage_ms(s) reports the call's
+ * stages.  Returns 0 or a negative status.  No counterpart in the reference's Python API. */
+int sb200_fstore_search_tracks(sb200_fstore* s, sb200_tracker* t, int32_t n, const uint64_t* scene_ids,
+                               const uint64_t* track_ids, uint64_t id_offset, const sb200_fstore_attrs* attrs,
+                               uint8_t* found, int32_t* feature_counts, uint8_t* queried,
+                               int32_t* counts, uint64_t* winners, double* weights);
 
 /* ---- the store blob ----
  * The whole store as one relocatable block of bytes: this header, then four sections at 256-byte aligned offsets, gaps

@@ -10,7 +10,7 @@ import subprocess
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libsimilari_b200.so")
-SOURCES = ["engine.cu", "ops.cu", "kernels_cost.cu", "kernels_feat_tc.cu", "kernels_feat_dense.cu", "kernels_assign.cu", "kernels_state.cu", "kernels_nms.cu", "kernels_own.cu", "kernels_geom.cu", "kernels_xfer.cu", "comm.cu", "kernels_fstore.cu", "fstore.cu", "wasted_store.cu"]
+SOURCES = ["engine.cu", "ops.cu", "kernels_cost.cu", "kernels_feat_tc.cu", "kernels_feat_dense.cu", "kernels_assign.cu", "kernels_state.cu", "kernels_nms.cu", "kernels_own.cu", "kernels_geom.cu", "kernels_xfer.cu", "comm.cu", "kernels_fstore.cu", "fstore.cu", "wasted_store.cu", "live_store.cu"]
 HEADERS = ["sb_engine.cuh", "sb_math.cuh", "sb_own_area.cuh", "sb_tc.cuh", "sb_sincos.cuh", "sb_sincos_table.inc", "sb_fstore.cuh", "sb_host.cuh", "sb_blob.cuh", "sb_wstore.cuh", os.path.join("..", "..", "include", "similari_b200.h")]
 
 # --fmad=false: the reference (Rust) never contracts a*b+c; parity of the i64 weights depends on it.

@@ -184,7 +184,7 @@ EXPORTS = [
     "sb200_fstore_search_quality", "sb200_fstore_associate_quality", "sb200_fstore_fetch_quality",
     "sb200_fstore_merge_history", "sb200_fstore_find_baked", "sb200_fstore_associate_store",
     "sb200_fstore_set_classes", "sb200_fstore_get_classes", "sb200_fstore_use_class", "sb200_fstore_class_counts",
-    "sb200_fstore_set_voting", "sb200_fstore_get_voting",
+    "sb200_fstore_set_voting", "sb200_fstore_get_voting", "sb200_scene_observations", "sb200_fstore_search_tracks",
 ]
 
 
@@ -311,6 +311,9 @@ def lib():
         "sb200_fstore_get_storage_type": (C.c_int, [vp, C.POINTER(i32)]),
         "sb200_fstore_associate_wasted": (i64, [vp, vp, i64, u64, vp, vp, vp, vp, vp, vp, i32, vp, vp, vp, vp, vp, vp, vp,
                                                 vp, vp, vp]),
+        "sb200_scene_observations": (i64, [vp, u64, i64, vp, vp, vp, vp, vp]),
+        "sb200_fstore_search_tracks": (C.c_int, [vp, vp, i32, vp, vp, u64, C.POINTER(FstoreAttrs), vp, vp, vp, vp, vp,
+                                                 vp]),
         "sb200_host_alloc": (vp, [C.c_size_t]),
         "sb200_host_free": (None, [vp]),
     }

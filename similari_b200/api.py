@@ -552,6 +552,22 @@ class _VisualBase(_TrackerBase):
                  int(w["track_ids"][i]) if w["queried"][i] else None)
                 for i in range(len(w["ids"]))]
 
+    def search_store(self, store: engine.FeatureStore, tracks: List[SortTrack], id_offset=0, sources=None, t_start=None,
+                     t_end=None, feature_class=None) -> List[Tuple[SortTrack, Optional[List[Tuple[int, float]]]]]:
+        """Re-identification: looks the live `tracks` (the SortTracks a predict returned, by scene_id and id) up in the
+        feature track `store` with one FeatureStore.search_tracks call, their observed features read where the tracker
+        keeps them.  Returns [(track, [(store track id, weight), ...])], the list being None for a track that is no
+        longer live or holds no feature.  A gated store takes sources / t_start / t_end, one per track.  An extension
+        with no PyO3 counterpart in the reference."""
+        tracks = list(tracks)
+        if self._t is None:
+            return [(tr, None) for tr in tracks]
+        r = store.search_tracks(self._t, [tr.scene_id for tr in tracks], [tr.id for tr in tracks], id_offset=id_offset,
+                                sources=sources, t_start=t_start, t_end=t_end, feature_class=feature_class)
+        return [(tr, [(int(r["winners"][i, e]), float(r["weights"][i, e])) for e in range(int(r["counts"][i]))]
+                 if r["queried"][i] else None)
+                for i, tr in enumerate(tracks)]
+
 
 class VisualSort(_VisualBase):
     """src/trackers/visual_sort/simple_api.rs `PyVisualSort`."""

@@ -2518,4 +2518,19 @@ int64_t tracker_collect_wasted(sb200_tracker* t, int64_t cap, const WastedOut& o
 
 int tracker_drop_wasted(sb200_tracker* t, int64_t n) { return t->drop_wasted_front(n); }
 
+// The tracker's side of sb200_scene_observations and sb200_fstore_search_tracks (live_store.cu).
+int tracker_live(sb200_tracker* t, int n, const uint64_t* scene_ids, LiveTracks* lt, std::vector<LiveScene>* scenes) {
+  CU(cudaSetDevice(t->device));
+  { int rc_ = t->drain(); if (rc_) return rc_; }
+  const TrackStore& ts = t->ts;
+  *lt = {ts.id, ts.fblk, ts.obs_phys, ts.obs_hasf, ts.obs_n, ts.obs_q, ts.feat, t->track_cap, t->P.max_obs, t->P.d8,
+         t->P.feature_dim, t->stream};
+  scenes->resize((size_t)n);
+  for (int i = 0; i < n; ++i) {
+    const int slot = t->slot_for(scene_ids[i], false);
+    (*scenes)[(size_t)i] = slot < 0 ? LiveScene{-1, 0} : LiveScene{(long long)slot * t->track_cap, t->n_tracks[slot]};
+  }
+  return 0;
+}
+
 }  // namespace sb

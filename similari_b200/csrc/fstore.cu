@@ -947,6 +947,22 @@ struct sb200_fstore {
                           track_ids, merged, true, nullptr, nullptr, tq, decided);
   }
 
+  // search whose request rows `rsrc` writes on the device (sb200_fstore_search_tracks); quality / attrs as run_queries
+  // takes them, the triples checked by the caller; *row_table receives the row table before rsrc runs
+  int search_rows(int Q, const uint64_t* qids, const int32_t* offs, const float* quality, const sb200_fstore_attrs* attrs,
+                  const sb::FsRowSource& rsrc, std::vector<int>* row_table, int32_t* counts, uint64_t* winners,
+                  double* weights) {
+    if (int rc = check_ids(Q, qids, "query id", false, offs)) return rc;
+    const int bad = keep && Q > 0 ? first_nan(offs[Q], quality) : -1;
+    if (bad >= 0) return fail(SB200_ERR_INVALID, "row %d: the quality is NaN", bad);
+    std::vector<int> qoff;
+    if (int rc = plan_rows(Q, offs, &qoff, row_table, keep ? quality : nullptr)) return rc;
+    if (int rc = begin()) return rc;
+    if (Q == 0) return 0;
+    return launch_queries(Q, qids, qoff, *row_table, Column{nullptr, false, nullptr}, 0, &rsrc, counts, winners, weights,
+                          nullptr, nullptr, false, attrs, quality);
+  }
+
   // the device part of search / associate, after every check: upload, distances, TopN, apply, results
   int launch_queries(int Q, const uint64_t* qids, const std::vector<int>& qoff, const std::vector<int>& src,
                      const Column& col, size_t col_rows, const sb::FsRowSource* rsrc, int32_t* counts,
@@ -2623,6 +2639,14 @@ int fstore_retention(sb200_fstore* s) { return s->keep; }
 int fstore_associate_rows(sb200_fstore* s, int Q, const uint64_t* qids, const int32_t* offs, const FsRowSource& src,
                           int32_t* counts, uint64_t* winners, double* weights, uint64_t* track_ids, uint8_t* merged) {
   return s->associate_rows(Q, qids, offs, src, counts, winners, weights, track_ids, merged);
+}
+
+int fstore_check_attrs(sb200_fstore* s, int n, const sb200_fstore_attrs* attrs) { return s->check_attrs(n, attrs); }
+
+int fstore_search_rows(sb200_fstore* s, int Q, const uint64_t* qids, const int32_t* offs, const float* quality,
+                       const sb200_fstore_attrs* attrs, const FsRowSource& src, std::vector<int>* row_table,
+                       int32_t* counts, uint64_t* winners, double* weights) {
+  return s->search_rows(Q, qids, offs, quality, attrs, src, row_table, counts, winners, weights);
 }
 
 }  // namespace sb

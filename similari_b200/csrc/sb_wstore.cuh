@@ -1,6 +1,6 @@
-// sb_wstore.cuh -- the internal interfaces behind sb200_fstore_associate_wasted (wasted_store.cu): what that call needs of
-// a visual tracker (engine.cu) and of a feature track store (fstore.cu).  Host code; each handle stays opaque outside
-// its own file.
+// sb_wstore.cuh -- the internal interfaces behind sb200_fstore_associate_wasted (wasted_store.cu) and the live-track calls
+// (live_store.cu): what those calls need of a visual tracker (engine.cu) and of a feature track store (fstore.cu).  Host
+// code; each handle stays opaque outside its own file.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -56,6 +56,30 @@ int64_t tracker_collect_wasted(sb200_tracker* t, int64_t cap, const WastedOut& o
 // pool.  The caller has finished every read of those blocks.
 int tracker_drop_wasted(sb200_tracker* t, int64_t n);
 
+// Where a visual tracker keeps Track::obs of its live tracks (sb200_scene_observations, sb200_fstore_search_tracks,
+// live_store.cu): the TrackStore columns.  The live tracks of a scene are the store indices [base, base + n_tracks) of
+// its slot (base = slot * track_cap); logical observation j < obs_n[idx] of track idx has the present byte
+// obs_hasf[idx * K + j], the quality obs_q[idx * K + j] and the f32 row (base + fblk[idx]) * K + obs_phys[idx * K + j]
+// of feat ([.][d8], zero-padded from feature_dim).  `st` is the tracker's work stream, idle when tracker_live returns.
+struct LiveTracks {
+  const unsigned long long* id;
+  const int* fblk;
+  const unsigned char* obs_phys;
+  const unsigned char* obs_hasf;
+  const unsigned char* obs_n;
+  const float* obs_q;
+  const float* feat;
+  int track_cap, K, d8, feature_dim;
+  cudaStream_t st;
+};
+struct LiveScene {
+  long long base;   // -1: the tracker holds no such scene
+  int n_tracks;
+};
+// A query point of a visual tracker (a drain; no auto-waste step, nothing changes): the columns, and the slot of each of
+// the n scene ids.  Valid until the next call that enqueues a frame or changes the tracker.
+int tracker_live(sb200_tracker* t, int n, const uint64_t* scene_ids, LiveTracks* lt, std::vector<LiveScene>* scenes);
+
 // ---- store side (fstore.cu)
 void fstore_info(sb200_fstore* s, int* device, int* feature_dim, int* topn);
 // the store's gate rule (SB200_FSTORE_GATE_*); a gated store refuses associate_wasted
@@ -64,8 +88,9 @@ int fstore_gate(sb200_fstore* s);
 int fstore_retention(sb200_fstore* s);
 
 // Writes the request rows of a store call on the store's stream `st`: rows[R][d8] f32 (zero-padded from feature_dim),
-// request row r holding observation r - qoff[q] of the rows query q = row_q[r] keeps (its newest max_observations,
-// oldest first).  qoff / row_q / rows are device pointers of the call.  Returns 0 or a negative status.
+// request row r holding observation r - qoff[q] of the rows query q = row_q[r] keeps (associate: its newest
+// max_observations, oldest first; fstore_search_rows: the rows its row table names).  qoff / row_q / rows are device
+// pointers of the call.  Returns 0 or a negative status.
 struct FsRowSource {
   int (*fill)(void* ctx, float* rows, const int* qoff, const int* row_q, int R, cudaStream_t st);
   void* ctx;
@@ -75,5 +100,16 @@ struct FsRowSource {
 // Checks (ids, pair bound), outputs and store changes as there; every rejection comes before the store changes.
 int fstore_associate_rows(sb200_fstore* s, int Q, const uint64_t* qids, const int32_t* offs, const FsRowSource& src,
                           int32_t* counts, uint64_t* winners, double* weights, uint64_t* track_ids, uint8_t* merged);
+
+// The checks of sb200_fstore_search_attr's triples for n queries (a gated store; columns present; t_start <= t_end).
+int fstore_check_attrs(sb200_fstore* s, int n, const sb200_fstore_attrs* attrs);
+
+// sb200_fstore_search of Q queries, query q with offs[q + 1] - offs[q] >= 1 rows written on the device by `src`; on a
+// quality store sb200_fstore_search_quality with quality[offs[Q]] the rows' qualities (a NaN is refused here), on a gated
+// store the _attr form with `attrs` (checked by the caller).  The store's query rule picks the request rows: request row
+// r is row (*row_table)[r] of the call, set before src.fill runs.  Checks (ids, pair bound) and outputs as there.
+int fstore_search_rows(sb200_fstore* s, int Q, const uint64_t* qids, const int32_t* offs, const float* quality,
+                       const sb200_fstore_attrs* attrs, const FsRowSource& src, std::vector<int>* row_table,
+                       int32_t* counts, uint64_t* winners, double* weights);
 
 }  // namespace sb

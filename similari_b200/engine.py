@@ -322,6 +322,21 @@ class Tracker:
         n = check(self._L.sb200_scene_tracks(self._h, scene_id, cap, ptr(ids), ptr(bx), ptr(st), ptr(fc)))
         return {"ids": ids[:n], "boxes": bx[:n], "states": st[:n], "feat_counts": fc[:n]}
 
+    def scene_observations(self, scene_id=0):
+        """sb200_scene_observations: Track::obs of every live track of the scene, in store order (the tracks
+        scene_tracks lists), gathered on the device from the tracker's arena: ids [n], n_obs [n], and per logical
+        observation has_feat [n, K], quality [n, K] and feats [n, K, feature_dim] (float32; zeros where the observation has
+        no feature and past n_obs).  K = visual_max_observations.  An unknown scene gives n = 0."""
+        K = max(1, int(self.opts.visual_max_observations))
+        D = int(self.opts.feature_dim)
+        cap = int(self.scene_track_counts([scene_id])[0])
+        ids, n_obs = np.zeros(max(1, cap), np.uint64), np.zeros(max(1, cap), np.int32)
+        hf, q = np.zeros((max(1, cap), K), np.uint8), np.zeros((max(1, cap), K), np.float32)
+        feats = np.zeros((max(1, cap), K, D), np.float32)
+        n = int(check(self._L.sb200_scene_observations(self._h, int(scene_id), cap, ptr(ids), ptr(n_obs), ptr(hf), ptr(q),
+                                                        ptr(feats))))
+        return {"ids": ids[:n], "n_obs": n_obs[:n], "has_feat": hf[:n], "quality": q[:n], "feats": feats[:n]}
+
     def last_costs(self, scene_id=0, cap=1 << 22):
         out = np.zeros(cap, np.float32)
         m, n = C.c_int32(0), C.c_int32(0)
@@ -1032,6 +1047,35 @@ class FeatureStore:
                 "observed_history": [ho[i, : hc[i]].copy() for i in range(n)], "feature_counts": fc[:n],
                 "queried": qd[:n].astype(bool), "counts": cn[:n], "winners": wn[:n], "weights": wt[:n],
                 "track_ids": ti[:n], "merged": mg[:n]}
+
+    def search_tracks(self, tracker, scene_ids, track_ids, id_offset=0, sources=None, t_start=None, t_end=None,
+                      feature_class=None):
+        """sb200_fstore_search_tracks: the live tracks (scene_ids[i], track_ids[i]) of the visual `tracker` as the
+        queries of one search of this store, their present observations (Track::obs order, as
+        tracker.scene_observations gives them) read on the device under the id track_ids[i] + id_offset.  The store's
+        query rule picks the rows (a newest store keeps the last max_observations, which drops the newest observation
+        first; a quality store the best ones, with the qualities the tracker keeps).  A gated store takes one source
+        and window per pair.  Returns per pair found (bool: the track is live), feature_counts, queried (bool) and the
+        search outputs counts / winners / weights (0 where not queried).  Changes neither the tracker nor the store."""
+        if not isinstance(tracker, Tracker):
+            raise TypeError("tracker must be an engine.Tracker")
+        id_offset = int(id_offset)
+        if not 0 <= id_offset < 1 << 64:
+            raise ValueError("id_offset must lie in [0, 2^64)")
+        sc = np.ascontiguousarray(scene_ids, dtype=np.uint64)
+        ti = np.ascontiguousarray(track_ids, dtype=np.uint64)
+        if sc.shape != ti.shape or sc.ndim != 1:
+            raise ValueError("scene_ids and track_ids must be 1-d and of the same length")
+        n, t = len(ti), self.topn
+        a = self._attrs(n, sources, t_start, t_end)
+        self._use(feature_class)
+        fd, fc, qd = np.zeros(max(1, n), np.uint8), np.zeros(max(1, n), np.int32), np.zeros(max(1, n), np.uint8)
+        cn, wn, wt = np.zeros(max(1, n), np.int32), np.zeros((max(1, n), t), np.uint64), np.zeros((max(1, n), t), np.float64)
+        check(self._L.sb200_fstore_search_tracks(
+            self._h, tracker._h, n, ptr(sc), ptr(ti), id_offset, C.byref(a[0]) if a is not None else None, ptr(fd), ptr(fc), ptr(qd),
+            ptr(cn), ptr(wn), ptr(wt)))
+        return {"found": fd[:n].astype(bool), "feature_counts": fc[:n], "queried": qd[:n].astype(bool), "counts": cn[:n],
+                "winners": wn[:n], "weights": wt[:n]}
 
     def find_baked(self, now, baked_period=0):
         """sb200_fstore_find_baked: TrackStore::find_usable with the `baked` rule of the reference's
