@@ -98,6 +98,8 @@ int make_params(const sb200_options& o, sb::Params* out) {
     p.d8 = (o.feature_dim + 7) / 8 * 8;
     p.vis_rel_err = sb::screen_rel_err(o.feature_dim);
     p.vis_rel_err8 = sb::screen_rel_err_fp8(o.feature_dim);
+    p.vis_dense_f32 = sb::dense_f32_err(o.feature_dim);
+    p.vis_sample_margin = sb::dense_sample_margin(o.feature_dim);
     p.max_obs = o.visual_max_observations;
     p.min_votes = o.visual_min_votes;
     p.min_track_length = o.visual_minimal_track_length;
@@ -814,7 +816,8 @@ struct sb200_tracker {
       const sb::VisKernel vk = sb::vis_kernel_env();
       const bool selective = sb::vis_selective(P.visual_kind == SB200_VIS_EUCLIDEAN, P.visual_threshold);
       const bool big = sb::vis_tc_worth(P.d8, pl.work);
-      const bool dense_ok = P.n_constraints == 0;
+      // features wider than kDenseMaxD have no proven dense bound (dense_f32_err is infinite): never the dense path
+      const bool dense_ok = P.n_constraints == 0 && std::isfinite(P.vis_dense_f32) && std::isfinite(P.vis_sample_margin);
       pl.want_dense = big && dense_ok && (!selective || adapt_dense);
       pl.want_tc = selective && big && !pl.want_dense;
       if (vk == sb::kVisSimt) { pl.want_tc = false; pl.want_dense = false; }
@@ -1525,6 +1528,8 @@ int sb200_set_feature_dim(sb200_tracker* t, int32_t feature_dim) {
   t->P.d8 = (feature_dim + 7) / 8 * 8;
   t->P.vis_rel_err = sb::screen_rel_err(feature_dim);
   t->P.vis_rel_err8 = sb::screen_rel_err_fp8(feature_dim);
+  t->P.vis_dense_f32 = sb::dense_f32_err(feature_dim);
+  t->P.vis_sample_margin = sb::dense_sample_margin(feature_dim);
   t->opts.feature_dim = feature_dim;
   for (const auto& [c, rows] : d8_cols()) {
     if (rows == 0) continue;

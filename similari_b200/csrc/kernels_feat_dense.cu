@@ -44,10 +44,10 @@
 namespace sb {
 
 // error of x~ = |a|^2 + |b|^2 - 2 dot~ against the reference's f32 squared distance, relative to (|a|^2 + |b|^2):
-// 2 E |a||b| <= E (|a|^2 + |b|^2) for the BF16 dot product (E = p.vis_rel_err, screen_rel_err), plus 2e-4 for the f32
-// roundings of the norms, of x~ itself and of the reference's own 512-term summation.  Cosine: |cos~ - cos| <= E + 2e-4
-// absolute.
-__device__ __forceinline__ float dense_err(const Params& p) { return p.vis_rel_err + 2e-4f; }
+// 2 E |a||b| <= E (|a|^2 + |b|^2) for the BF16 dot product (E = p.vis_rel_err, screen_rel_err), plus F = p.vis_dense_f32
+// (dense_f32_err, growing with the width) for the f32 roundings of the norms, of x~ itself and of the reference's own
+// summation.  Cosine: |cos~ - cos| <= E + F absolute.
+__device__ __forceinline__ float dense_err(const Params& p) { return p.vis_rel_err + p.vis_dense_f32; }
 
 // The bounds above hold for finite operands whose squared norms stay below FLT_MAX / 4 (then neither |a|^2 + |b|^2 nor
 // 2 dot~ overflows) and, under cosine, are not zero.  A scene with any other feature (a NaN or infinite component, a zero
@@ -523,8 +523,10 @@ __global__ void vis_dense_rowmeta_kernel(Params p, Frame f, VisRowMeta* rowmeta)
 }
 
 // Sampled lower bound of the scene's maximal distance (in the weight-sum kernel's domain: squared distance, or 1 - cos):
-// up to 64 candidates x 64 valid feature rows, plain f32 dot products.  Any real element bounds the maximum from below, so
-// whatever the sample is, the candidates the weight-sum kernel keeps (x~ >= l0 - bound) contain the true maximum.
+// up to 32 candidates x 32 valid feature rows, plain f32 dot products less the margin p.vis_sample_margin
+// (dense_sample_margin, growing with the width), which keeps each sampled value below the reference's value of its pair.
+// Any real element bounds the maximum from below, so whatever the sample is, the candidates the weight-sum kernel keeps
+// (x~ >= l0 - bound) contain the true maximum.  (Widths without a proven bound never reach this path: engine.cu.)
 // T: element type of the request's feature column (widened on load).
 constexpr int DSAMP = 32;
 template <class T>
@@ -578,8 +580,8 @@ __global__ void __launch_bounds__(256) vis_dense_sample_kernel(Params p, TrackSt
     for (int o = 16; o > 0; o >>= 1) dot += __shfl_xor_sync(0xffffffffu, dot, o);
     const float na = f.c_norm2[g], nb2 = ts.fnorm2[fr];
     float v;
-    if (p.visual_kind == 1) v = 1.0f - dot * rsqrtf(na) * rsqrtf(nb2) - 1e-4f;
-    else v = (na + nb2 - 2.0f * dot) - 1e-4f * (na + nb2);
+    if (p.visual_kind == 1) v = 1.0f - dot * rsqrtf(na) * rsqrtf(nb2) - p.vis_sample_margin;
+    else v = (na + nb2 - 2.0f * dot) - p.vis_sample_margin * (na + nb2);
     best = fmaxf(best, v);
   }
   if (lane == 0) s_w[wid] = best;

@@ -199,6 +199,8 @@ int sb200_visual_cost_matrix(int32_t visual_kind, float threshold, const float* 
   p.d8 = (d + 7) / 8 * 8;
   p.vis_rel_err = sb::screen_rel_err(d);
   p.vis_rel_err8 = sb::screen_rel_err_fp8(d);
+  p.vis_dense_f32 = sb::dense_f32_err(d);
+  p.vis_sample_margin = sb::dense_sample_margin(d);
   p.max_obs = 1;
   p.min_track_length = 0;
   // track side: norms through the candidate-norm kernel on a scratch frame

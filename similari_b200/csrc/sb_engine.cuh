@@ -74,6 +74,51 @@ inline float screen_rel_err_fp8(int d) {
   return (float)((rnd + sub + acc) * (1.0 + 0x1p-20));   // rounded up past the f32 conversion
 }
 
+// The f32 part of the dense path's error bound (kernels_feat_dense.cu dense_err), as a function of the width d.  The dense
+// path compares x~ = |a|^2 + |b|^2 - 2 dot~ (f32 norms of cand_norm_kernel, BF16 tensor-core dot) with the reference's f32
+// squared distance acc = sum over 8-lane blocks of reduce_add8((a - b)^2), blocks added in order (src/distance.rs), relative
+// to N = |a|^2 + |b|^2; under cosine it compares 1 - dot~ rsqrt(|a|^2) rsqrt(|b|^2) with 1 - divided / sqrt(f1 f2)
+// absolutely.  The BF16 operands and the tensor-core accumulation are screen_rel_err's; this is everything else.  With
+// u = 2^-24, g(k) = k u / (1 - k u) and n8 = ceil(d / 8) blocks, a term that passes k roundings errs by at most g(k) of its
+// magnitude (Higham, Accuracy and Stability of Numerical Algorithms, 2nd ed., Lemma 3.1):
+//   1. Norms.  A square is rounded once, the block tree adds three roundings, the blocks are added in order (n8 - 1): each
+//      term of |a|^2 passes n8 + 3 roundings, |na - |a|^2| <= g(n8 + 3) |a|^2, and the two norms together g(n8 + 3) N.
+//   2. The reference.  a - b, its square (twice the first rounding) and the same n8 + 2 additions: n8 + 5 roundings of
+//      terms that sum to |a - b|^2 <= 2 N, so |acc - |a - b|^2| <= 2 g(n8 + 5) N.  Cosine: divided errs by g(n8 + 3)
+//      sum|a_i b_i| <= g(n8 + 3) |a||b|, its norms f1, f2 by g(n8 + 3) each, and so do the kernel's norms: 3 g(n8 + 3).
+//   3. Forming x~ (a sum and an fma on values <= 2.1 N) and the bound (f32 products of the f32 norms, themselves low by up
+//      to g(n8 + 3)): 8 u N.  Cosine: two rsqrtf (2 ulp = 4 u each), two products, the subtraction from 1 and the
+//      reference's product, square root and division: 15 u.
+// Both metrics stay below g(3 n8 + 24) <= (3 n8 + 24) u (1 + 2^-8) for d <= kDenseMaxD = 2^16 (k u <= 2^-9 there).  The
+// factor 1 + 2^-5 leaves room for the share of the BF16 term the kernel under-counts because it scales E by the f32
+// norms: E g(n8 + 6) N, with E = screen_rel_err(d) <= 2^-6 + 2^-16 up to kDenseMaxD, is below 0.03 (3 n8 + 24) u N.
+// That is 1.3e-5 at d = 512 and 1.9e-4 at d = 8192; the path has always budgeted 2e-4, which the function keeps as a
+// floor, so it changes the bound only above d ~ 8900.  Wider than kDenseMaxD no bound is proven here: +inf keeps the
+// tracker off the dense path (engine.cu).
+constexpr int kDenseMaxD = 1 << 16;
+inline float dense_f32_err(int d) {
+  if (d > kDenseMaxD) return __builtin_inff();
+  const double n8 = (double)((d + 7) / 8);
+  const double e = (3.0 * n8 + 24.0) * 0x1p-24 * (1.0 + 0x1p-5);
+  return e <= 2e-4 ? 2e-4f : (float)(e * (1.0 + 0x1p-20));   // rounded up past the f32 conversion
+}
+
+// Margin of the dense path's sampled lower bound of the scene's maximal distance (vis_dense_sample_kernel): a sampled
+// pair's distance, computed with a lane-strided f32 FMA dot product, minus margin * N (Euclidean) or margin (cosine) must
+// not exceed the reference's value for that pair, or the max-candidate list could miss the true maximum.  The sampled
+// value uses the same f32 norms as above (1.: g(n8 + 3) N) against the same reference (2.: 2 g(n8 + 5) N), and its dot
+// product: every lane adds ceil(d / 32) products by fma (one rounding each), five butterfly additions join the lanes, so
+// |dot_s - dot| <= g(ceil(d / 32) + 5) sum|a_i b_i| and 2 |dot_s - dot| <= g(ceil(d / 32) + 5) N.  Forming the sample and
+// subtracting the margin: 8 u N.  Cosine: dot_s, divided and both pairs of norms (g(ceil(d / 32) + 5) + 3 g(n8 + 3)), the
+// rsqrtf and the reference's quotient as above, 17 u.  So (3 n8 + ceil(d / 32) + 32) u (1 + 2^-5), about 13 d / 32 u:
+// 1.5e-5 at d = 512, 1.04e-4 at d = 4096, 2.1e-4 at d = 8192.  The path has always subtracted 1e-4, kept as the floor.
+inline float dense_sample_margin(int d) {
+  if (d > kDenseMaxD) return __builtin_inff();
+  const double n8 = (double)((d + 7) / 8), n32 = (double)((d + 31) / 32);
+  const double e = (3.0 * n8 + n32 + 32.0) * 0x1p-24 * (1.0 + 0x1p-5);
+  return e <= 1e-4 ? 1e-4f : (float)(e * (1.0 + 0x1p-20));
+}
+
 // Rows whose squared norm lies outside [2^-60, 2^60] (zero, tiny, huge, inf or NaN features) keep every pair in the e4m3
 // screen: the exact pass decides.  Inside that range max|x| lies in [2^-35, 2^30], the scale 2^k_r is a normal float and
 // the folded screen constants neither overflow nor lose bits to subnormals.
@@ -142,6 +187,8 @@ struct Params {  // immutable per tracker, passed by value to kernels
   float visual_threshold;
   float vis_rel_err;  // screen_rel_err(feature_dim): the BF16 slack of the tensor-core visual kernels
   float vis_rel_err8; // screen_rel_err_fp8(feature_dim): the slack of the e4m3 screen
+  float vis_dense_f32;      // dense_f32_err(feature_dim): the f32 part of the dense path's bound
+  float vis_sample_margin;  // dense_sample_margin(feature_dim): margin of the dense path's sampled maximal distance
   int feature_dim, d8, max_obs, min_votes, min_track_length;
   int vote_vis_cap;   // visual entries per scene the sparse voting kernel keeps in shared memory (0: kVoteVisCap)
   float min_area, min_quality_use, min_quality_collect, min_own_use, min_own_collect;
