@@ -58,22 +58,24 @@ __device__ __forceinline__ float dec_f32(unsigned int u) {
 }
 
 // per-scene maximum over all valid visual entries ("max_dist" of best.rs:58,72-74), init -1.0
-__global__ void vis_max_kernel(Params p, Frame f, unsigned int* scene_max) {
-  if (f.scene_mode[blockIdx.y] == 0) return;  // sparse scenes: the refine kernel already reduced their maximum
-  const SceneDesc sc = f.scenes[blockIdx.y];
-  const long long cnt = (long long)sc.m * sc.n * p.max_obs;
-  const float* v = f.vis + sc.vis_off;
-  float mx = -1.0f;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < cnt; i += (long long)gridDim.x * blockDim.x) {
-    float e = v[i];
-    if (!is_nan(e) && mx < e) mx = e;
-  }
+__global__ void vis_max_kernel(Params p, Frame f, unsigned int* scene_max, int n_scenes) {
+  for (int s = blockIdx.y; s < n_scenes; s += gridDim.y) {
+    if (f.scene_mode[s] == 0) continue;  // sparse scenes: the refine kernel already reduced their maximum
+    const SceneDesc sc = f.scenes[s];
+    const long long cnt = (long long)sc.m * sc.n * p.max_obs;
+    const float* v = f.vis + sc.vis_off;
+    float mx = -1.0f;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < cnt; i += (long long)gridDim.x * blockDim.x) {
+      float e = v[i];
+      if (!is_nan(e) && mx < e) mx = e;
+    }
 #pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    float t = __shfl_xor_sync(0xffffffffu, mx, o);
-    if (mx < t) mx = t;
+    for (int o = 16; o > 0; o >>= 1) {
+      float t = __shfl_xor_sync(0xffffffffu, mx, o);
+      if (mx < t) mx = t;
+    }
+    if ((threadIdx.x & 31) == 0) atomicMax(scene_max + s, enc_f32(mx));
   }
-  if ((threadIdx.x & 31) == 0) atomicMax(scene_max + blockIdx.y, enc_f32(mx));
 }
 __global__ void vis_max_init_kernel(unsigned int* scene_max, int n) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1029,8 +1031,8 @@ void launch_scene_max(const Params& p, const Frame& f, int n_scenes, bool init_o
   if (init_only) {
     vis_max_init_kernel<<<(n_scenes + 255) / 256, 256, 0, st>>>(f.scene_max, n_scenes);
   } else {
-    dim3 grid(32, n_scenes);
-    vis_max_kernel<<<grid, 256, 0, st>>>(p, f, f.scene_max);
+    dim3 grid(32, scene_grid(n_scenes));
+    vis_max_kernel<<<grid, 256, 0, st>>>(p, f, f.scene_max, n_scenes);
   }
   note_launch();
 }

@@ -140,90 +140,94 @@ struct CandTile {
 };
 
 template <int POS>
-__global__ void __launch_bounds__(TN * TY) pos_cost_kernel(Params p, TrackStore ts, Frame f) {
-  const SceneDesc sc = f.scenes[blockIdx.z];
-  const int n0 = blockIdx.x * TN, m0 = blockIdx.y * TM;
-  if (n0 >= sc.n || m0 >= sc.m) return;
+__global__ void __launch_bounds__(TN * TY) pos_cost_kernel(Params p, TrackStore ts, Frame f, int n_scenes) {
   __shared__ CandTile ct;
-  const int tid = threadIdx.y * TN + threadIdx.x;
-  // stage candidates
-  for (int i = tid; i < TM; i += TN * TY) {
-    int m = m0 + i;
-    if (m < sc.m) {
-      int g = sc.det_base + m;
-      const float* cb = f.c_box + (size_t)g * 6;
-      ct.xc[i] = cb[0]; ct.yc[i] = cb[1]; ct.ang0[i] = angle_or0(cb[2]); ct.asp[i] = cb[3]; ct.h[i] = cb[4];
-      ct.r[i] = f.c_radius[g]; ct.conf[i] = f.c_conf[g];
+  for (int s = blockIdx.z; s < n_scenes; s += gridDim.z) {
+    const SceneDesc sc = f.scenes[s];
+    const int n0 = blockIdx.x * TN, m0 = blockIdx.y * TM;
+    if (n0 >= sc.n || m0 >= sc.m) continue;   // CTA-uniform
+    const int tid = threadIdx.y * TN + threadIdx.x;
+    // stage candidates
+    for (int i = tid; i < TM; i += TN * TY) {
+      int m = m0 + i;
+      if (m < sc.m) {
+        int g = sc.det_base + m;
+        const float* cb = f.c_box + (size_t)g * 6;
+        ct.xc[i] = cb[0]; ct.yc[i] = cb[1]; ct.ang0[i] = angle_or0(cb[2]); ct.asp[i] = cb[3]; ct.h[i] = cb[4];
+        ct.r[i] = f.c_radius[g]; ct.conf[i] = f.c_conf[g];
+      }
     }
-  }
-  if (POS == 1) {
-    for (int i = tid; i < TM * 8; i += TN * TY) {
-      int m = m0 + i / 8;
-      if (m < sc.m) ct.vert[i / 8][i % 8] = f.c_vert[(size_t)(sc.det_base + m) * 8 + (i % 8)];
+    if (POS == 1) {
+      for (int i = tid; i < TM * 8; i += TN * TY) {
+        int m = m0 + i / 8;
+        if (m < sc.m) ct.vert[i / 8][i % 8] = f.c_vert[(size_t)(sc.det_base + m) * 8 + (i % 8)];
+      }
     }
-  }
-  __syncthreads();
-  const int n = n0 + threadIdx.x;
-  if (n >= sc.n) return;
-  const size_t ti = (size_t)sc.slot * ts.track_cap + n;
-  const float* tb = ts.pred + ti * 6;
-  const float txc = tb[0], tyc = tb[1], tasp = tb[3], th = tb[4];
-  const float tr = ts.radius[ti];
-  const unsigned int tep = ts.epoch[ti];
-  float mean5[5], l5[5];
-  double tv[8];
-  if (POS == 0) {
-    const float* st = ts.kst + ti * ts.kst_stride;
-    const float hh = st[4];
-#pragma unroll
-    for (int i = 0; i < 5; ++i) {
-      mean5[i] = st[i];
-      l5[i] = sqrtf(kalman_proj_var(p.pos_weight, hh, st[10 + 4 * i], i));
-    }
-  } else {
-#pragma unroll
-    for (int i = 0; i < 8; ++i) tv[i] = ts.vert[ti * 8 + i];
-  }
-  float* out = f.pos + sc.pos_off;
-  const float qnan = nanf("");
-#pragma unroll 1
-  for (int i = threadIdx.y; i < TM; i += TY) {
-    int m = m0 + i;
-    if (m >= sc.m) break;
-    float v = qnan;
-    const float cx = ct.xc[i], cy = ct.yc[i], cr = ct.r[i];
-    if (compat_ok(p, sc.epoch, tep, cx, cy, cr, txc, tyc, tr) && !too_far(cx, cy, cr, txc, tyc, tr)) {
+    __syncthreads();
+    const int n = n0 + threadIdx.x;
+    if (n < sc.n) {
+      const size_t ti = (size_t)sc.slot * ts.track_cap + n;
+      const float* tb = ts.pred + ti * 6;
+      const float txc = tb[0], tyc = tb[1], tasp = tb[3], th = tb[4];
+      const float tr = ts.radius[ti];
+      const unsigned int tep = ts.epoch[ti];
+      float mean5[5], l5[5];
+      double tv[8];
       if (POS == 0) {
-        float d = maha_distance(mean5, l5, cx, cy, ct.ang0[i], ct.asp[i], ct.h[i]);
-        v = maha_cost(d) / ct.conf[i];
+        const float* st = ts.kst + ti * ts.kst_stride;
+        const float hh = st[4];
+#pragma unroll
+        for (int i = 0; i < 5; ++i) {
+          mean5[i] = st[i];
+          l5[i] = sqrtf(kalman_proj_var(p.pos_weight, hh, st[10 + 4 * i], i));
+        }
       } else {
-        double a = clip_area(ct.vert[i], tv);
-        float iou = iou_from_area(a, ct.h[i], ct.asp[i], th, tasp);
-        if (!is_nan(iou)) {
-          iou = iou * ct.conf[i];
-          v = iou >= p.iou_threshold ? iou : qnan;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) tv[i] = ts.vert[ti * 8 + i];
+      }
+      float* out = f.pos + sc.pos_off;
+      const float qnan = nanf("");
+#pragma unroll 1
+      for (int i = threadIdx.y; i < TM; i += TY) {
+        int m = m0 + i;
+        if (m >= sc.m) break;
+        float v = qnan;
+        const float cx = ct.xc[i], cy = ct.yc[i], cr = ct.r[i];
+        if (compat_ok(p, sc.epoch, tep, cx, cy, cr, txc, tyc, tr) && !too_far(cx, cy, cr, txc, tyc, tr)) {
+          if (POS == 0) {
+            float d = maha_distance(mean5, l5, cx, cy, ct.ang0[i], ct.asp[i], ct.h[i]);
+            v = maha_cost(d) / ct.conf[i];
+          } else {
+            double a = clip_area(ct.vert[i], tv);
+            float iou = iou_from_area(a, ct.h[i], ct.asp[i], th, tasp);
+            if (!is_nan(iou)) {
+              iou = iou * ct.conf[i];
+              v = iou >= p.iou_threshold ? iou : qnan;
+            }
+          }
+        }
+        out[(size_t)m * sc.n + n] = v;
+        // sparse view for the voting stage: valid entries are rare (gated by 2R and the threshold), append them
+        const bool valid = !is_nan(v);
+        const unsigned am = __activemask();
+        const unsigned bal = __ballot_sync(am, valid);
+        if (bal) {
+          const int lane = threadIdx.x & 31;
+          const int leader = __ffs(bal) - 1;
+          int base = 0;
+          if (lane == leader) base = atomicAdd(&f.pos_cnt[s], __popc(bal));
+          base = __shfl_sync(am, base, leader);
+          if (valid) {
+            const int slot = base + __popc(bal & ((1u << lane) - 1));
+            if (slot < sc.pos_lcap) {
+              PosEntry e; e.m = (unsigned short)m; e.n = (unsigned short)n; e.v = v;
+              f.pos_list[sc.pos_lbase + slot] = e;
+            }
+          }
         }
       }
     }
-    out[(size_t)m * sc.n + n] = v;
-    // sparse view for the voting stage: valid entries are rare (gated by 2R and the threshold), append them
-    const bool valid = !is_nan(v);
-    const unsigned am = __activemask();
-    const unsigned bal = __ballot_sync(am, valid);
-    if (bal) {
-      const int lane = threadIdx.x & 31;
-      const int leader = __ffs(bal) - 1;
-      int base = 0;
-      if (lane == leader) base = atomicAdd(&f.pos_cnt[blockIdx.z], __popc(bal));
-      base = __shfl_sync(am, base, leader);
-      if (valid) {
-        const int slot = base + __popc(bal & ((1u << lane) - 1));
-        if (slot < sc.pos_lcap) {
-          PosEntry e; e.m = (unsigned short)m; e.n = (unsigned short)n; e.v = v;
-          f.pos_list[sc.pos_lbase + slot] = e;
-        }
-      }
-    }
+    __syncthreads();   // every thread is done with ct before the next scene restages it
   }
 }
 
@@ -500,10 +504,10 @@ static void pos_scan_impl(const Params& p, const TrackStore& ts, const Frame& f,
   if (pos_use_dense(max_n)) {
     if (lazy_pass == 1) return;   // the dense kernel has already written every element
     // very large scenes: dense tiled kernel
-    dim3 grid((max_n + TN - 1) / TN, (max_m + TM - 1) / TM, n_scenes);
+    dim3 grid((max_n + TN - 1) / TN, (max_m + TM - 1) / TM, scene_grid(n_scenes));
     dim3 block(TN, TY);
-    if (p.positional_kind == 0) pos_cost_kernel<0><<<grid, block, 0, st>>>(p, ts, f);
-    else pos_cost_kernel<1><<<grid, block, 0, st>>>(p, ts, f);
+    if (p.positional_kind == 0) pos_cost_kernel<0><<<grid, block, 0, st>>>(p, ts, f, n_scenes);
+    else pos_cost_kernel<1><<<grid, block, 0, st>>>(p, ts, f, n_scenes);
     note_launch();
     return;
   }

@@ -381,61 +381,62 @@ vis_wsum_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
 __global__ void vis_dense_meta_kernel(Params p, TrackStore ts, Frame f, int max_blocks, int cstep, DenseTrackMeta* tmeta,
                                       int2* rowinfo, float* slab_colc, float* slab_cmax, float* slab_ktf,
                                       unsigned int* slab_vmask, unsigned int* slab_bmask, float* scene_cmax,
-                                      int* dense_bad) {
-  const int s = blockIdx.y;
-  const SceneDesc sc = f.scenes[s];
-  const int K = p.max_obs;
-  const int b = blockIdx.x * blockDim.x + threadIdx.x;
-  float cmax = 0.0f;
-  if (b < sc.nb && b < max_blocks) {
-    const size_t sbase = (size_t)sc.slot * ts.track_cap;
-    const int n = ts.blk_owner ? ts.blk_owner[sbase + b] : b;
-    DenseTrackMeta tm;
-    tm.n = n; tm.kt = 0; tm.cmax = 0.0f; tm.pad = 0;
-    int outcol[kMaxObs], frow_of[kMaxObs];
-    float colc[kMaxObs];
-    for (int ph = 0; ph < K; ++ph) { outcol[ph] = -1; frow_of[ph] = -1; colc[ph] = 0.0f; }
-    if (n >= 0) {
-      const size_t ti = sbase + n;
-      const int on = ts.obs_n[ti];
-      const unsigned int tep = ts.epoch[ti];
-      const unsigned int delta = sc.epoch > tep ? sc.epoch - tep : tep - sc.epoch;
-      const bool valid = (ts.feat_cnt[ti] >= p.min_track_length) && ((unsigned int)p.max_idle_epochs >= delta);
-      for (int k = 0; k < K; ++k) {
-        if (k < on && ts.obs_hasf[ti * K + k]) {
-          const int ph = ts.obs_phys[ti * K + k];
-          const size_t frow = (sbase + b) * K + ph;
-          outcol[ph] = n * K + k;
-          if (valid) {
-            frow_of[ph] = (int)frow;
-            const float nb2 = ts.fnorm2[frow];
-            if (!dense_norm_ok(p, nb2)) dense_bad[s] = 1;
-            colc[ph] = p.visual_kind == 1 ? rsqrtf(nb2) : nb2;
-            cmax = fmaxf(cmax, nb2);
-            tm.kt += 1;
+                                      int* dense_bad, int n_scenes) {
+  for (int s = blockIdx.y; s < n_scenes; s += gridDim.y) {
+    const SceneDesc sc = f.scenes[s];
+    const int K = p.max_obs;
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    float cmax = 0.0f;
+    if (b < sc.nb && b < max_blocks) {
+      const size_t sbase = (size_t)sc.slot * ts.track_cap;
+      const int n = ts.blk_owner ? ts.blk_owner[sbase + b] : b;
+      DenseTrackMeta tm;
+      tm.n = n; tm.kt = 0; tm.cmax = 0.0f; tm.pad = 0;
+      int outcol[kMaxObs], frow_of[kMaxObs];
+      float colc[kMaxObs];
+      for (int ph = 0; ph < K; ++ph) { outcol[ph] = -1; frow_of[ph] = -1; colc[ph] = 0.0f; }
+      if (n >= 0) {
+        const size_t ti = sbase + n;
+        const int on = ts.obs_n[ti];
+        const unsigned int tep = ts.epoch[ti];
+        const unsigned int delta = sc.epoch > tep ? sc.epoch - tep : tep - sc.epoch;
+        const bool valid = (ts.feat_cnt[ti] >= p.min_track_length) && ((unsigned int)p.max_idle_epochs >= delta);
+        for (int k = 0; k < K; ++k) {
+          if (k < on && ts.obs_hasf[ti * K + k]) {
+            const int ph = ts.obs_phys[ti * K + k];
+            const size_t frow = (sbase + b) * K + ph;
+            outcol[ph] = n * K + k;
+            if (valid) {
+              frow_of[ph] = (int)frow;
+              const float nb2 = ts.fnorm2[frow];
+              if (!dense_norm_ok(p, nb2)) dense_bad[s] = 1;
+              colc[ph] = p.visual_kind == 1 ? rsqrtf(nb2) : nb2;
+              cmax = fmaxf(cmax, nb2);
+              tm.kt += 1;
+            }
           }
         }
+        tm.cmax = cmax;
       }
-      tm.cmax = cmax;
+      tmeta[sc.blk_off + b] = tm;
+      const int need_votes = p.min_votes > 1 ? p.min_votes : 1;
+      const float ktf = (tm.n >= 0 && tm.kt >= need_votes) ? (float)tm.kt : 0.0f;
+      for (int ph = 0; ph < K; ++ph) {
+        const int prow = b * K + ph;
+        rowinfo[(size_t)sc.blk_off * K + prow] = make_int2(outcol[ph], frow_of[ph]);
+        const int j = prow / cstep, cc = prow - j * cstep;
+        const size_t slab = (size_t)sc.slab_off + j;
+        slab_colc[slab * TC_BN + cc] = colc[ph];
+        slab_cmax[slab * TC_BN + cc] = cmax;
+        slab_ktf[slab * TC_BN + cc] = ktf;
+        if (frow_of[ph] >= 0) atomicOr(&slab_vmask[slab * (TC_BN / 32) + (cc >> 5)], 1u << (cc & 31));
+        if (ph == K - 1) atomicOr(&slab_bmask[slab * (TC_BN / 32) + (cc >> 5)], 1u << (cc & 31));
+      }
     }
-    tmeta[sc.blk_off + b] = tm;
-    const int need_votes = p.min_votes > 1 ? p.min_votes : 1;
-    const float ktf = (tm.n >= 0 && tm.kt >= need_votes) ? (float)tm.kt : 0.0f;
-    for (int ph = 0; ph < K; ++ph) {
-      const int prow = b * K + ph;
-      rowinfo[(size_t)sc.blk_off * K + prow] = make_int2(outcol[ph], frow_of[ph]);
-      const int j = prow / cstep, cc = prow - j * cstep;
-      const size_t slab = (size_t)sc.slab_off + j;
-      slab_colc[slab * TC_BN + cc] = colc[ph];
-      slab_cmax[slab * TC_BN + cc] = cmax;
-      slab_ktf[slab * TC_BN + cc] = ktf;
-      if (frow_of[ph] >= 0) atomicOr(&slab_vmask[slab * (TC_BN / 32) + (cc >> 5)], 1u << (cc & 31));
-      if (ph == K - 1) atomicOr(&slab_bmask[slab * (TC_BN / 32) + (cc >> 5)], 1u << (cc & 31));
-    }
-  }
 #pragma unroll
-  for (int o = 16; o > 0; o >>= 1) cmax = fmaxf(cmax, __shfl_xor_sync(0xffffffffu, cmax, o));
-  if ((threadIdx.x & 31) == 0 && cmax > 0.0f) atomicMax(reinterpret_cast<int*>(scene_cmax) + s, __float_as_int(cmax));
+    for (int o = 16; o > 0; o >>= 1) cmax = fmaxf(cmax, __shfl_xor_sync(0xffffffffu, cmax, o));
+    if ((threadIdx.x & 31) == 0 && cmax > 0.0f) atomicMax(reinterpret_cast<int*>(scene_cmax) + s, __float_as_int(cmax));
+  }
 }
 
 // K > kMaxObs: one warp per arena block, lane k reading logical observation k and lane ph writing physical row ph, the
@@ -444,69 +445,70 @@ constexpr int DMW_WARPS = 4;
 __global__ void __launch_bounds__(DMW_WARPS * 32)
 vis_dense_meta_wide_kernel(Params p, TrackStore ts, Frame f, int max_blocks, int cstep, DenseTrackMeta* tmeta, int2* rowinfo,
                            float* slab_colc, float* slab_cmax, float* slab_ktf, unsigned int* slab_vmask,
-                           unsigned int* slab_bmask, float* scene_cmax, int* dense_bad) {
+                           unsigned int* slab_bmask, float* scene_cmax, int* dense_bad, int n_scenes) {
   __shared__ int2 s_ri[DMW_WARPS][32];
   __shared__ float s_colc[DMW_WARPS][32];
-  const int s = blockIdx.y;
-  const SceneDesc sc = f.scenes[s];
-  const int K = p.max_obs;
-  const int wi = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int b = blockIdx.x * DMW_WARPS + wi;
-  if (!(b < sc.nb && b < max_blocks)) return;   // warp-uniform
-  const unsigned int all = 0xffffffffu;
-  const size_t sbase = (size_t)sc.slot * ts.track_cap;
-  const int n = ts.blk_owner ? ts.blk_owner[sbase + b] : b;
-  s_ri[wi][lane] = make_int2(-1, -1);
-  s_colc[wi][lane] = 0.0f;
-  __syncwarp();
-  bool use = false;   // lane's logical observation holds a feature of a valid track
-  float nb2 = 0.0f;
-  if (n >= 0) {
-    const size_t ti = sbase + n;
-    const int on = ts.obs_n[ti];
-    const unsigned int tep = ts.epoch[ti];
-    const unsigned int delta = sc.epoch > tep ? sc.epoch - tep : tep - sc.epoch;
-    const bool valid = (ts.feat_cnt[ti] >= p.min_track_length) && ((unsigned int)p.max_idle_epochs >= delta);
-    const int k = lane;
-    if (k < K && k < on && ts.obs_hasf[ti * K + k]) {
-      const int ph = ts.obs_phys[ti * K + k];
-      const size_t frow = (sbase + b) * K + ph;
-      int fr = -1;
-      if (valid) {
-        fr = (int)frow;
-        nb2 = ts.fnorm2[frow];
-        if (!dense_norm_ok(p, nb2)) dense_bad[s] = 1;
-        s_colc[wi][ph] = p.visual_kind == 1 ? rsqrtf(nb2) : nb2;
-        use = true;
+  for (int s = blockIdx.y; s < n_scenes; s += gridDim.y) {
+    const SceneDesc sc = f.scenes[s];
+    const int K = p.max_obs;
+    const int wi = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int b = blockIdx.x * DMW_WARPS + wi;
+    if (!(b < sc.nb && b < max_blocks)) continue;   // warp-uniform
+    const unsigned int all = 0xffffffffu;
+    const size_t sbase = (size_t)sc.slot * ts.track_cap;
+    const int n = ts.blk_owner ? ts.blk_owner[sbase + b] : b;
+    s_ri[wi][lane] = make_int2(-1, -1);
+    s_colc[wi][lane] = 0.0f;
+    __syncwarp();
+    bool use = false;   // lane's logical observation holds a feature of a valid track
+    float nb2 = 0.0f;
+    if (n >= 0) {
+      const size_t ti = sbase + n;
+      const int on = ts.obs_n[ti];
+      const unsigned int tep = ts.epoch[ti];
+      const unsigned int delta = sc.epoch > tep ? sc.epoch - tep : tep - sc.epoch;
+      const bool valid = (ts.feat_cnt[ti] >= p.min_track_length) && ((unsigned int)p.max_idle_epochs >= delta);
+      const int k = lane;
+      if (k < K && k < on && ts.obs_hasf[ti * K + k]) {
+        const int ph = ts.obs_phys[ti * K + k];
+        const size_t frow = (sbase + b) * K + ph;
+        int fr = -1;
+        if (valid) {
+          fr = (int)frow;
+          nb2 = ts.fnorm2[frow];
+          if (!dense_norm_ok(p, nb2)) dense_bad[s] = 1;
+          s_colc[wi][ph] = p.visual_kind == 1 ? rsqrtf(nb2) : nb2;
+          use = true;
+        }
+        s_ri[wi][ph] = make_int2(n * K + k, fr);
       }
-      s_ri[wi][ph] = make_int2(n * K + k, fr);
     }
-  }
-  float cmax = use ? nb2 : 0.0f;
+    float cmax = use ? nb2 : 0.0f;
 #pragma unroll
-  for (int o = 16; o > 0; o >>= 1) cmax = fmaxf(cmax, __shfl_xor_sync(all, cmax, o));
-  const int kt = __popc(__ballot_sync(all, use));
-  __syncwarp();
-  if (lane == 0) {
-    DenseTrackMeta tm;
-    tm.n = n; tm.kt = n >= 0 ? kt : 0; tm.cmax = n >= 0 ? cmax : 0.0f; tm.pad = 0;
-    tmeta[sc.blk_off + b] = tm;
-    if (cmax > 0.0f) atomicMax(reinterpret_cast<int*>(scene_cmax) + s, __float_as_int(cmax));
-  }
-  const int need_votes = p.min_votes > 1 ? p.min_votes : 1;
-  const float ktf = (n >= 0 && kt >= need_votes) ? (float)kt : 0.0f;
-  const int ph = lane;
-  if (ph < K) {
-    const int2 ri = s_ri[wi][ph];
-    const int prow = b * K + ph;
-    rowinfo[(size_t)sc.blk_off * K + prow] = ri;
-    const int j = prow / cstep, cc = prow - j * cstep;
-    const size_t slab = (size_t)sc.slab_off + j;
-    slab_colc[slab * TC_BN + cc] = s_colc[wi][ph];
-    slab_cmax[slab * TC_BN + cc] = cmax;
-    slab_ktf[slab * TC_BN + cc] = ktf;
-    if (ri.y >= 0) atomicOr(&slab_vmask[slab * (TC_BN / 32) + (cc >> 5)], 1u << (cc & 31));
-    if (ph == K - 1) atomicOr(&slab_bmask[slab * (TC_BN / 32) + (cc >> 5)], 1u << (cc & 31));
+    for (int o = 16; o > 0; o >>= 1) cmax = fmaxf(cmax, __shfl_xor_sync(all, cmax, o));
+    const int kt = __popc(__ballot_sync(all, use));
+    __syncwarp();
+    if (lane == 0) {
+      DenseTrackMeta tm;
+      tm.n = n; tm.kt = n >= 0 ? kt : 0; tm.cmax = n >= 0 ? cmax : 0.0f; tm.pad = 0;
+      tmeta[sc.blk_off + b] = tm;
+      if (cmax > 0.0f) atomicMax(reinterpret_cast<int*>(scene_cmax) + s, __float_as_int(cmax));
+    }
+    const int need_votes = p.min_votes > 1 ? p.min_votes : 1;
+    const float ktf = (n >= 0 && kt >= need_votes) ? (float)kt : 0.0f;
+    const int ph = lane;
+    if (ph < K) {
+      const int2 ri = s_ri[wi][ph];
+      const int prow = b * K + ph;
+      rowinfo[(size_t)sc.blk_off * K + prow] = ri;
+      const int j = prow / cstep, cc = prow - j * cstep;
+      const size_t slab = (size_t)sc.slab_off + j;
+      slab_colc[slab * TC_BN + cc] = s_colc[wi][ph];
+      slab_cmax[slab * TC_BN + cc] = cmax;
+      slab_ktf[slab * TC_BN + cc] = ktf;
+      if (ri.y >= 0) atomicOr(&slab_vmask[slab * (TC_BN / 32) + (cc >> 5)], 1u << (cc & 31));
+      if (ph == K - 1) atomicOr(&slab_bmask[slab * (TC_BN / 32) + (cc >> 5)], 1u << (cc & 31));
+    }
   }
 }
 
@@ -753,16 +755,16 @@ int launch_vis_dense(const Params& p, const TrackStore& ts, const Frame& f, int 
   }
   const bool wide = p.max_obs > kMaxObs;
   if (tc.max_blocks > 0 && wide) {
-    dim3 grid((tc.max_blocks + DMW_WARPS - 1) / DMW_WARPS, n_scenes);
+    dim3 grid((tc.max_blocks + DMW_WARPS - 1) / DMW_WARPS, scene_grid(n_scenes));
     vis_dense_meta_wide_kernel<<<grid, DMW_WARPS * 32, 0, st>>>(p, ts, f, tc.max_blocks, tc.cstep, tc.tmeta, tc.rowinfo,
                                                               tc.slab_colc, tc.slab_cmax, tc.slab_ktf, tc.slab_vmask,
-                                                              tc.slab_bmask, tc.scene_cmax, tc.dense_bad);
+                                                              tc.slab_bmask, tc.scene_cmax, tc.dense_bad, n_scenes);
     note_launch();
   } else if (tc.max_blocks > 0) {
-    dim3 grid((tc.max_blocks + 127) / 128, n_scenes);
+    dim3 grid((tc.max_blocks + 127) / 128, scene_grid(n_scenes));
     vis_dense_meta_kernel<<<grid, 128, 0, st>>>(p, ts, f, tc.max_blocks, tc.cstep, tc.tmeta, tc.rowinfo, tc.slab_colc, tc.slab_cmax,
                                                 tc.slab_ktf, tc.slab_vmask, tc.slab_bmask, tc.scene_cmax,
-                                                tc.dense_bad);
+                                                tc.dense_bad, n_scenes);
     note_launch();
   }
   vis_dense_rowmeta_kernel<<<(f.total + 255) / 256, 256, 0, st>>>(p, f, tc.rowmeta);

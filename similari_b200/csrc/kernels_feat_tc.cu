@@ -615,127 +615,132 @@ __device__ __forceinline__ float refine_block_sum(const float* av, const float* 
 
 // T: element type of the request's feature column
 template <bool COSINE, bool TAIL, class T>
-__global__ void __launch_bounds__(RF_WARPS * 32, 8) vis_refine_kernel(Params p, TrackStore ts, Frame f, int* nan_flag) {
+__global__ void __launch_bounds__(RF_WARPS * 32, 8) vis_refine_kernel(Params p, TrackStore ts, Frame f, int* nan_flag,
+                                                                      int n_scenes) {
   __shared__ float s_bs[RF_WARPS][RF_CLAIM][RF_PITCH];
   __shared__ int s_cnt[2];
-  const int scene = blockIdx.y;
-  if (f.vis_mode[scene] != 0) {   // survivor list overflowed: this scene is computed densely
-    if (f.screen_cnt && blockIdx.x == 0 && threadIdx.x == 0) atomicAdd(f.screen_cnt + 2, 1);
-    return;
-  }
-  const SceneDesc sc = f.scenes[scene];
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  if (f.screen_cnt) {
-    if (threadIdx.x < 2) s_cnt[threadIdx.x] = 0;
-    __syncthreads();
-  }
-  int n_ref = 0, n_cut = 0;   // survivors this lane refined, and how many of them the exact test cut
-  const int n_pairs = min(f.vis_cnt[scene], sc.vis_lcap);
-  const int nblk = p.d8 / 8;
-  const int D = p.feature_dim;
-  float (*bs)[RF_PITCH] = s_bs[w];
-  float vmax = nanf("");
-  // warps claim RF_CLAIM survivors at a time from the scene's counter: however many survive, the scene's warps finish together
-  for (;;) {
-    int i0 = 0;
-    if (lane == 0) i0 = atomicAdd(f.refine_next + scene, RF_CLAIM);
-    i0 = __shfl_sync(0xffffffffu, i0, 0);
-    if (i0 >= n_pairs) break;
-    const int npair = min(RF_CLAIM, n_pairs - i0);
-    VisPair mine;
-    mine.g = 0; mine.row = 0; mine.scene = 0; mine.outcol = 0;
-    if (lane < npair) mine = f.vis_pairs[sc.vis_lbase + i0 + lane];
-    float acc = 0.0f;
-    for (int seg0 = 0; seg0 < nblk; seg0 += RF_SEG) {
-      const int segn = min(RF_SEG, nblk - seg0);
-      // A candidate's survivors sit next to each other in the list (the observations of its track are adjacent columns
-      // of one screen tile; the dense path emits whole groups): its row is loaded once and reused while the candidate
-      // stays the same -- a third of the L2 -> SM traffic of this kernel.
-      int g_prev = -1;
-      float av[RF_SEG / 32][8];
+  for (int scene = blockIdx.y; scene < n_scenes; scene += gridDim.y) {
+    if (f.vis_mode[scene] != 0) {   // survivor list overflowed: this scene is computed densely
+      if (f.screen_cnt && blockIdx.x == 0 && threadIdx.x == 0) atomicAdd(f.screen_cnt + 2, 1);
+      continue;
+    }
+    const SceneDesc sc = f.scenes[scene];
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    if (f.screen_cnt) {
+      if (threadIdx.x < 2) s_cnt[threadIdx.x] = 0;
+      __syncthreads();
+    }
+    int n_ref = 0, n_cut = 0;   // survivors this lane refined, and how many of them the exact test cut
+    const int n_pairs = min(f.vis_cnt[scene], sc.vis_lcap);
+    const int nblk = p.d8 / 8;
+    const int D = p.feature_dim;
+    float (*bs)[RF_PITCH] = s_bs[w];
+    float vmax = nanf("");
+    // warps claim RF_CLAIM survivors at a time from the scene's counter: however many survive, the scene's warps finish together
+    for (;;) {
+      int i0 = 0;
+      if (lane == 0) i0 = atomicAdd(f.refine_next + scene, RF_CLAIM);
+      i0 = __shfl_sync(0xffffffffu, i0, 0);
+      if (i0 >= n_pairs) break;
+      const int npair = min(RF_CLAIM, n_pairs - i0);
+      VisPair mine;
+      mine.g = 0; mine.row = 0; mine.scene = 0; mine.outcol = 0;
+      if (lane < npair) mine = f.vis_pairs[sc.vis_lbase + i0 + lane];
+      float acc = 0.0f;
+      for (int seg0 = 0; seg0 < nblk; seg0 += RF_SEG) {
+        const int segn = min(RF_SEG, nblk - seg0);
+        // A candidate's survivors sit next to each other in the list (the observations of its track are adjacent columns
+        // of one screen tile; the dense path emits whole groups): its row is loaded once and reused while the candidate
+        // stays the same -- a third of the L2 -> SM traffic of this kernel.
+        int g_prev = -1;
+        float av[RF_SEG / 32][8];
 #pragma unroll 4
-      for (int pp = 0; pp < npair; ++pp) {
-        const int g = __shfl_sync(0xffffffffu, mine.g, pp);
-        const int row = __shfl_sync(0xffffffffu, mine.row, pp);
-        const float* b = ts.feat + (size_t)row * p.d8;
-        if (g != g_prev) {   // warp-uniform
-          const T* a = static_cast<const T*>(f.in_feat) + (size_t)g * D;
+        for (int pp = 0; pp < npair; ++pp) {
+          const int g = __shfl_sync(0xffffffffu, mine.g, pp);
+          const int row = __shfl_sync(0xffffffffu, mine.row, pp);
+          const float* b = ts.feat + (size_t)row * p.d8;
+          if (g != g_prev) {   // warp-uniform
+            const T* a = static_cast<const T*>(f.in_feat) + (size_t)g * D;
 #pragma unroll
-          for (int h = 0; h < RF_SEG / 32; ++h)
-            if (h * 32 + lane < segn) refine_load_a<TAIL>(a, seg0 + h * 32 + lane, D, av[h]);
-          g_prev = g;
+            for (int h = 0; h < RF_SEG / 32; ++h)
+              if (h * 32 + lane < segn) refine_load_a<TAIL>(a, seg0 + h * 32 + lane, D, av[h]);
+            g_prev = g;
+          }
+#pragma unroll
+          for (int h = 0; h < RF_SEG / 32; ++h) {
+            const int j = h * 32 + lane;
+            if (j < segn) bs[pp][j] = refine_block_sum<COSINE>(av[h], b, seg0 + j);
+          }
         }
-#pragma unroll
-        for (int h = 0; h < RF_SEG / 32; ++h) {
-          const int j = h * 32 + lane;
-          if (j < segn) bs[pp][j] = refine_block_sum<COSINE>(av[h], b, seg0 + j);
+        __syncwarp();
+        if (lane < npair)
+          for (int j = 0; j < segn; ++j) acc = acc + bs[lane][j];
+        __syncwarp();
+      }
+      if (lane < npair) {
+        float v = nanf("");
+        if (COSINE) {
+          const float d = acc / sqrtf(f.c_norm2[mine.g] * ts.fnorm2[mine.row]);
+          if (d >= p.visual_threshold) v = 1.0f - d;       // is_ok + distance_to_weight
+        } else {
+          const float d = sqrtf(acc);
+          if (d <= p.visual_threshold) v = d;
         }
+        f.vis_val[sc.vis_lbase + i0 + lane] = v;
+        n_ref += 1;
+        n_cut += is_nan(v) ? 1 : 0;
+        if (!is_nan(v) && !(v <= vmax)) vmax = v;   // best.rs "max_dist": maximum over the entries that exist
+        if (nan_flag && is_nan(v)) nan_flag[scene] = 1;   // dense path: an entry the threshold cuts voids its precondition
       }
-      __syncwarp();
-      if (lane < npair)
-        for (int j = 0; j < segn; ++j) acc = acc + bs[lane][j];
-      __syncwarp();
     }
-    if (lane < npair) {
-      float v = nanf("");
-      if (COSINE) {
-        const float d = acc / sqrtf(f.c_norm2[mine.g] * ts.fnorm2[mine.row]);
-        if (d >= p.visual_threshold) v = 1.0f - d;       // is_ok + distance_to_weight
-      } else {
-        const float d = sqrtf(acc);
-        if (d <= p.visual_threshold) v = d;
-      }
-      f.vis_val[sc.vis_lbase + i0 + lane] = v;
-      n_ref += 1;
-      n_cut += is_nan(v) ? 1 : 0;
-      if (!is_nan(v) && !(v <= vmax)) vmax = v;   // best.rs "max_dist": maximum over the entries that exist
-      if (nan_flag && is_nan(v)) nan_flag[scene] = 1;   // dense path: an entry the threshold cuts voids its precondition
+    // one atomic per warp
+    unsigned int u = 0u;
+    if (!is_nan(vmax)) {
+      u = __float_as_uint(vmax);
+      u = (u & 0x80000000u) ? ~u : (u | 0x80000000u);
     }
-  }
-  // one atomic per warp
-  unsigned int u = 0u;
-  if (!is_nan(vmax)) {
-    u = __float_as_uint(vmax);
-    u = (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-  }
 #pragma unroll
-  for (int o = 16; o > 0; o >>= 1) u = max(u, __shfl_xor_sync(0xffffffffu, u, o));
-  if (lane == 0 && u != 0u) atomicMax(f.scene_max + scene, u);
-  if (f.screen_cnt) {   // the screen's selectivity: one shared atomic per warp, one global atomic per CTA
-    n_ref = __reduce_add_sync(0xffffffffu, n_ref);
-    n_cut = __reduce_add_sync(0xffffffffu, n_cut);
-    if (lane == 0 && n_ref) { atomicAdd(&s_cnt[0], n_ref); atomicAdd(&s_cnt[1], n_cut); }
-    __syncthreads();
-    if (threadIdx.x == 0 && s_cnt[0]) { atomicAdd(f.screen_cnt, s_cnt[0]); if (s_cnt[1]) atomicAdd(f.screen_cnt + 1, s_cnt[1]); }
+    for (int o = 16; o > 0; o >>= 1) u = max(u, __shfl_xor_sync(0xffffffffu, u, o));
+    if (lane == 0 && u != 0u) atomicMax(f.scene_max + scene, u);
+    if (f.screen_cnt) {   // the screen's selectivity: one shared atomic per warp, one global atomic per CTA
+      n_ref = __reduce_add_sync(0xffffffffu, n_ref);
+      n_cut = __reduce_add_sync(0xffffffffu, n_cut);
+      if (lane == 0 && n_ref) { atomicAdd(&s_cnt[0], n_ref); atomicAdd(&s_cnt[1], n_cut); }
+      __syncthreads();
+      if (threadIdx.x == 0 && s_cnt[0]) { atomicAdd(f.screen_cnt, s_cnt[0]); if (s_cnt[1]) atomicAdd(f.screen_cnt + 1, s_cnt[1]); }
+      __syncthreads();   // thread 0 has read s_cnt before the next scene zeroes it
+    }
   }
 }
 
 // dense view of the sparse scenes' visual entries (operators / debugging): None everywhere, then the refined survivors
-__global__ void vis_fill_none_kernel(Params p, Frame f) {
-  const int scene = blockIdx.y;
-  if (f.scene_mode[scene] != 0) return;
-  const SceneDesc sc = f.scenes[scene];
-  const long long cnt = (long long)sc.m * sc.n * p.max_obs;
-  float* out = f.vis + sc.vis_off;
-  const float qnan = nanf("");
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < cnt; i += (long long)gridDim.x * blockDim.x) out[i] = qnan;
+__global__ void vis_fill_none_kernel(Params p, Frame f, int n_scenes) {
+  for (int scene = blockIdx.y; scene < n_scenes; scene += gridDim.y) {
+    if (f.scene_mode[scene] != 0) continue;
+    const SceneDesc sc = f.scenes[scene];
+    const long long cnt = (long long)sc.m * sc.n * p.max_obs;
+    float* out = f.vis + sc.vis_off;
+    const float qnan = nanf("");
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < cnt; i += (long long)gridDim.x * blockDim.x) out[i] = qnan;
+  }
 }
-__global__ void vis_scatter_kernel(Params p, Frame f) {
-  const int scene = blockIdx.y;
-  if (f.scene_mode[scene] != 0) return;
-  const SceneDesc sc = f.scenes[scene];
-  const int n_pairs = min(f.vis_cnt[scene], sc.vis_lcap);
-  float* out = f.vis + sc.vis_off;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n_pairs; i += gridDim.x * blockDim.x) {
-    const VisPair vp = f.vis_pairs[sc.vis_lbase + i];
-    out[(size_t)(vp.g - sc.det_base) * (sc.n * p.max_obs) + vp.outcol] = f.vis_val[sc.vis_lbase + i];
+__global__ void vis_scatter_kernel(Params p, Frame f, int n_scenes) {
+  for (int scene = blockIdx.y; scene < n_scenes; scene += gridDim.y) {
+    if (f.scene_mode[scene] != 0) continue;
+    const SceneDesc sc = f.scenes[scene];
+    const int n_pairs = min(f.vis_cnt[scene], sc.vis_lcap);
+    float* out = f.vis + sc.vis_off;
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n_pairs; i += gridDim.x * blockDim.x) {
+      const VisPair vp = f.vis_pairs[sc.vis_lbase + i];
+      out[(size_t)(vp.g - sc.det_base) * (sc.n * p.max_obs) + vp.outcol] = f.vis_val[sc.vis_lbase + i];
+    }
   }
 }
 void launch_vis_densify(const Params& p, const Frame& f, int n_scenes, cudaStream_t st) {
   if (n_scenes == 0) return;
-  dim3 grid(64, n_scenes);
-  vis_fill_none_kernel<<<grid, 256, 0, st>>>(p, f);
-  vis_scatter_kernel<<<grid, 256, 0, st>>>(p, f);
+  dim3 grid(64, scene_grid(n_scenes));
+  vis_fill_none_kernel<<<grid, 256, 0, st>>>(p, f, n_scenes);
+  vis_scatter_kernel<<<grid, 256, 0, st>>>(p, f, n_scenes);
   note_launch(2);
 }
 
@@ -808,70 +813,71 @@ static bool screen_fp8(const Params& p, const TcArgs& tc) { return tc.fp8 && !tc
 // fp8_norm_ok), and the scale itself in colsb.
 __global__ void vis_meta_kernel(Params p, TrackStore ts, Frame f, int n_scenes, int max_rows, VisColMeta* colmeta,
                                 VisColGeo* colgeo, float* colb, float* colsb, unsigned int* colvalid, bool fp8) {
-  const int s = blockIdx.y;
-  const SceneDesc sc = f.scenes[s];
-  const int K = p.max_obs;
-  const int prow = blockIdx.x * blockDim.x + threadIdx.x;
-  const bool in = prow < sc.nb * K && prow < max_rows;
-  VisColMeta cm;
-  cm.colb = 0.0f; cm.colc = 0.0f; cm.outcol = -1; cm.row = -1;
-  float csb = 1.0f;
-  if (in) {
-    const int b = prow / K, ph = prow - b * K;
-    const size_t sbase = (size_t)sc.slot * ts.track_cap;
-    const int n = ts.blk_owner ? ts.blk_owner[sbase + b] : b;
-    const size_t ti = sbase + (n >= 0 ? n : 0);
-    const size_t frow = (sbase + b) * K + ph;   // feature row of this column
-    unsigned int tep = 0u;
-    if (n >= 0) {
-      const int on = ts.obs_n[ti];
-      // logical <-> physical observation bookkeeping of this track
-      int k_of = -1, live_mask = 0;
-      for (int k = 0; k < K; ++k) {
-        if (k < on && ts.obs_hasf[ti * K + k]) {
-          int pp = ts.obs_phys[ti * K + k];
-          live_mask |= 1 << pp;
-          if (pp == ph) k_of = k;
-        }
-      }
-      tep = ts.epoch[ti];
-      if (k_of >= 0) {
-        const unsigned int delta = sc.epoch > tep ? sc.epoch - tep : tep - sc.epoch;
-        cm.outcol = n * K + k_of;
-        const bool valid = (ts.feat_cnt[ti] >= p.min_track_length) && ((unsigned int)p.max_idle_epochs >= delta);
-        const float nb = ts.fnorm2[frow];
-        const float E = fp8 ? p.vis_rel_err8 : p.vis_rel_err;
-        cm.colb = p.visual_kind == 1 ? sqrtf(nb) : 0.5f * nb * (1.0f - 1e-5f - E);
-        if (fp8) {
-          if (fp8_norm_ok(nb)) { csb = ts.fscale[frow]; cm.colb *= csb; }
-          else cm.colb = nanf("");
-        }
-        cm.row = valid ? (int)frow : -1;
-      } else {
-        // dead physical slot -> owns the dead_rank-th logical column without a feature (written as None)
-        int dead_rank = 0;
-        for (int pp = 0; pp < ph; ++pp) dead_rank += ((live_mask >> pp) & 1) ? 0 : 1;
-        int seen = 0;
+  for (int s = blockIdx.y; s < n_scenes; s += gridDim.y) {
+    const SceneDesc sc = f.scenes[s];
+    const int K = p.max_obs;
+    const int prow = blockIdx.x * blockDim.x + threadIdx.x;
+    const bool in = prow < sc.nb * K && prow < max_rows;
+    VisColMeta cm;
+    cm.colb = 0.0f; cm.colc = 0.0f; cm.outcol = -1; cm.row = -1;
+    float csb = 1.0f;
+    if (in) {
+      const int b = prow / K, ph = prow - b * K;
+      const size_t sbase = (size_t)sc.slot * ts.track_cap;
+      const int n = ts.blk_owner ? ts.blk_owner[sbase + b] : b;
+      const size_t ti = sbase + (n >= 0 ? n : 0);
+      const size_t frow = (sbase + b) * K + ph;   // feature row of this column
+      unsigned int tep = 0u;
+      if (n >= 0) {
+        const int on = ts.obs_n[ti];
+        // logical <-> physical observation bookkeeping of this track
+        int k_of = -1, live_mask = 0;
         for (int k = 0; k < K; ++k) {
-          bool lv = k < on && ts.obs_hasf[ti * K + k];
-          if (!lv) { if (seen == dead_rank) { cm.outcol = n * K + k; break; } ++seen; }
+          if (k < on && ts.obs_hasf[ti * K + k]) {
+            int pp = ts.obs_phys[ti * K + k];
+            live_mask |= 1 << pp;
+            if (pp == ph) k_of = k;
+          }
+        }
+        tep = ts.epoch[ti];
+        if (k_of >= 0) {
+          const unsigned int delta = sc.epoch > tep ? sc.epoch - tep : tep - sc.epoch;
+          cm.outcol = n * K + k_of;
+          const bool valid = (ts.feat_cnt[ti] >= p.min_track_length) && ((unsigned int)p.max_idle_epochs >= delta);
+          const float nb = ts.fnorm2[frow];
+          const float E = fp8 ? p.vis_rel_err8 : p.vis_rel_err;
+          cm.colb = p.visual_kind == 1 ? sqrtf(nb) : 0.5f * nb * (1.0f - 1e-5f - E);
+          if (fp8) {
+            if (fp8_norm_ok(nb)) { csb = ts.fscale[frow]; cm.colb *= csb; }
+            else cm.colb = nanf("");
+          }
+          cm.row = valid ? (int)frow : -1;
+        } else {
+          // dead physical slot -> owns the dead_rank-th logical column without a feature (written as None)
+          int dead_rank = 0;
+          for (int pp = 0; pp < ph; ++pp) dead_rank += ((live_mask >> pp) & 1) ? 0 : 1;
+          int seen = 0;
+          for (int k = 0; k < K; ++k) {
+            bool lv = k < on && ts.obs_hasf[ti * K + k];
+            if (!lv) { if (seen == dead_rank) { cm.outcol = n * K + k; break; } ++seen; }
+          }
         }
       }
+      colmeta[sc.col_off + prow] = cm;
+      colb[sc.col_off + prow] = cm.colb;
+      if (fp8 && p.visual_kind != 1) colsb[sc.col_off + prow] = csb;
+      if (p.n_constraints > 0) {
+        VisColGeo cg;
+        cg.tx = 0.0f; cg.ty = 0.0f; cg.tr = 0.0f; cg.tep = tep;
+        if (n >= 0) { const float* tb = ts.pred + ti * 6; cg.tx = tb[0]; cg.ty = tb[1]; cg.tr = ts.radius[ti]; }
+        colgeo[sc.col_off + prow] = cg;
+      }
     }
-    colmeta[sc.col_off + prow] = cm;
-    colb[sc.col_off + prow] = cm.colb;
-    if (fp8 && p.visual_kind != 1) colsb[sc.col_off + prow] = csb;
-    if (p.n_constraints > 0) {
-      VisColGeo cg;
-      cg.tx = 0.0f; cg.ty = 0.0f; cg.tr = 0.0f; cg.tep = tep;
-      if (n >= 0) { const float* tb = ts.pred + ti * 6; cg.tx = tb[0]; cg.ty = tb[1]; cg.tr = ts.radius[ti]; }
-      colgeo[sc.col_off + prow] = cg;
-    }
+    // col_off is a multiple of 128, so the 32 columns of a warp are exactly one word of the validity mask
+    const unsigned int vb = __ballot_sync(0xffffffffu, cm.row >= 0);
+    if ((threadIdx.x & 31) == 0 && vb != 0) colvalid[(sc.col_off + prow) >> 5] = vb;
+    else if ((threadIdx.x & 31) == 0 && in) colvalid[(sc.col_off + prow) >> 5] = 0u;
   }
-  // col_off is a multiple of 128, so the 32 columns of a warp are exactly one word of the validity mask
-  const unsigned int vb = __ballot_sync(0xffffffffu, cm.row >= 0);
-  if ((threadIdx.x & 31) == 0 && vb != 0) colvalid[(sc.col_off + prow) >> 5] = vb;
-  else if ((threadIdx.x & 31) == 0 && in) colvalid[(sc.col_off + prow) >> 5] = 0u;
 }
 
 // fp8: cosine rowk carries the row's 2^k, Euclidean rowi = 2^-k; NaN rowk (every pair kept) outside fp8_norm_ok
@@ -900,18 +906,18 @@ __global__ void vis_rowmeta_kernel(Params p, Frame f, VisRowMeta* rowmeta, bool 
 // exact refinement of the scene pair lists (f.vis_pairs / vis_cnt / refine_next / vis_val; scenes with vis_mode != 0 skipped)
 int launch_vis_refine(const Params& p, const TrackStore& ts, const Frame& f, int n_scenes, int* nan_flag, cudaStream_t st) {
   if (n_scenes == 0) return 0;
-  dim3 grid(16, n_scenes);   // 64 warps x RF_CLAIM survivors per scene in flight; more survivors are claimed in further rounds
+  dim3 grid(16, scene_grid(n_scenes));   // 64 warps x RF_CLAIM survivors per scene in flight; more survivors are claimed in further rounds
   // the vector path needs 16-byte aligned input rows (a caller-owned device pointer on the device-io path); rows of d8
   // elements are 16-byte multiples for every element type
   const bool tail = p.feature_dim != p.d8 || (reinterpret_cast<uintptr_t>(f.in_feat) & 15) != 0;
   feat_dispatch(f.feat_type, [&](auto t) {
     using T = decltype(t);
     if (p.visual_kind == 1) {
-      if (tail) vis_refine_kernel<true, true, T><<<grid, RF_WARPS * 32, 0, st>>>(p, ts, f, nan_flag);
-      else vis_refine_kernel<true, false, T><<<grid, RF_WARPS * 32, 0, st>>>(p, ts, f, nan_flag);
+      if (tail) vis_refine_kernel<true, true, T><<<grid, RF_WARPS * 32, 0, st>>>(p, ts, f, nan_flag, n_scenes);
+      else vis_refine_kernel<true, false, T><<<grid, RF_WARPS * 32, 0, st>>>(p, ts, f, nan_flag, n_scenes);
     } else {
-      if (tail) vis_refine_kernel<false, true, T><<<grid, RF_WARPS * 32, 0, st>>>(p, ts, f, nan_flag);
-      else vis_refine_kernel<false, false, T><<<grid, RF_WARPS * 32, 0, st>>>(p, ts, f, nan_flag);
+      if (tail) vis_refine_kernel<false, true, T><<<grid, RF_WARPS * 32, 0, st>>>(p, ts, f, nan_flag, n_scenes);
+      else vis_refine_kernel<false, false, T><<<grid, RF_WARPS * 32, 0, st>>>(p, ts, f, nan_flag, n_scenes);
     }
   });
   note_launch();
@@ -922,7 +928,7 @@ void launch_vis_colmeta(const Params& p, const TrackStore& ts, const Frame& f, i
                         cudaStream_t st) {
   const int max_rows = tc.max_rows > 0 ? tc.max_rows : max_n * p.max_obs;
   if (tc.n_tiles == 0 || max_rows <= 0) return;
-  dim3 grid((max_rows + 255) / 256, n_scenes);
+  dim3 grid((max_rows + 255) / 256, scene_grid(n_scenes));
   vis_meta_kernel<<<grid, 256, 0, st>>>(p, ts, f, n_scenes, max_rows, tc.colmeta, tc.colgeo, tc.colb, tc.colsb, tc.colvalid,
                                         screen_fp8(p, tc));
   note_launch();

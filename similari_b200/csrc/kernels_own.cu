@@ -14,58 +14,61 @@ namespace sb {
 
 constexpr int OW_WARPS = 4;
 
-__global__ void __launch_bounds__(OW_WARPS * 32) own_area_kernel(Frame f, const float* __restrict__ boxes, float* __restrict__ out, int* ovf_cnt, int2* ovf) {
+__global__ void __launch_bounds__(OW_WARPS * 32) own_area_kernel(Frame f, const float* __restrict__ boxes, float* __restrict__ out, int* ovf_cnt, int2* ovf,
+                                                                 int n_scenes) {
   __shared__ double s_quads[OW_WARPS][(kOwnMaxNb + 1) * 8];
-  const int scene = blockIdx.y;
-  const SceneDesc sc = f.scenes[scene];
-  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int m = blockIdx.x * OW_WARPS + w;
-  if (m >= sc.m) return;   // warp-uniform
-  double* quads = s_quads[w];
-  const int g = sc.det_base + m;
-  const float* bi = boxes + (size_t)g * 6;
-  const float bx = bi[0], by = bi[1], basp = bi[3], bh = bi[4];
-  double vi[8];
-  box_vertices(bx, by, bi[2], basp, bh, vi);   // every lane: the same eight values
-  if (lane < 8) quads[lane] = vi[lane];
-  const double s = quad_area_signed(vi) < 0.0 ? -1.0 : 1.0;
-  const float ri = box_radius(basp, bh);
-  int k = 0;
-  for (int j0 = 0; j0 < sc.m; j0 += 32) {
-    const int j = j0 + lane;
-    bool keep = false;
-    double vj[8];
-    if (j < sc.m && j != m) {
-      const float* bj = boxes + (size_t)(sc.det_base + j) * 6;
-      if (!too_far(bx, by, ri, bj[0], bj[1], box_radius(bj[3], bj[4]))) {   // bbox_own_areas.rs:12-14
-        box_vertices(bj[0], bj[1], bj[2], bj[3], bj[4], vj);
-        keep = own_can_cover(vi, vj);
+  for (int scene = blockIdx.y; scene < n_scenes; scene += gridDim.y) {
+    const SceneDesc sc = f.scenes[scene];
+    const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int m = blockIdx.x * OW_WARPS + w;
+    if (m >= sc.m) continue;   // warp-uniform
+    double* quads = s_quads[w];
+    const int g = sc.det_base + m;
+    const float* bi = boxes + (size_t)g * 6;
+    const float bx = bi[0], by = bi[1], basp = bi[3], bh = bi[4];
+    double vi[8];
+    box_vertices(bx, by, bi[2], basp, bh, vi);   // every lane: the same eight values
+    __syncwarp();   // the warp has read its previous scene's list
+    if (lane < 8) quads[lane] = vi[lane];
+    const double s = quad_area_signed(vi) < 0.0 ? -1.0 : 1.0;
+    const float ri = box_radius(basp, bh);
+    int k = 0;
+    for (int j0 = 0; j0 < sc.m; j0 += 32) {
+      const int j = j0 + lane;
+      bool keep = false;
+      double vj[8];
+      if (j < sc.m && j != m) {
+        const float* bj = boxes + (size_t)(sc.det_base + j) * 6;
+        if (!too_far(bx, by, ri, bj[0], bj[1], box_radius(bj[3], bj[4]))) {   // bbox_own_areas.rs:12-14
+          box_vertices(bj[0], bj[1], bj[2], bj[3], bj[4], vj);
+          keep = own_can_cover(vi, vj);
+        }
       }
-    }
-    const unsigned int mask = __ballot_sync(0xffffffffu, keep);
-    if (keep) {
-      const int slot = k + __popc(mask & ((1u << lane) - 1u));
-      if (slot < kOwnMaxNb) {
+      const unsigned int mask = __ballot_sync(0xffffffffu, keep);
+      if (keep) {
+        const int slot = k + __popc(mask & ((1u << lane) - 1u));
+        if (slot < kOwnMaxNb) {
 #pragma unroll
-        for (int q = 0; q < 8; ++q) quads[(slot + 1) * 8 + q] = vj[q];
+          for (int q = 0; q < 8; ++q) quads[(slot + 1) * 8 + q] = vj[q];
+        }
       }
+      k += __popc(mask);
     }
-    k += __popc(mask);
-  }
-  __syncwarp();
-  if (k > kOwnMaxNb) {   // more overlapping boxes than the warp's list holds: the CTA-per-detection second pass takes it
-    if (lane == 0) {
-      const int slot = atomicAdd(ovf_cnt, 1);
-      ovf[slot] = make_int2(scene, m);
-      out[g] = 1.0f;
+    __syncwarp();
+    if (k > kOwnMaxNb) {   // more overlapping boxes than the warp's list holds: the CTA-per-detection second pass takes it
+      if (lane == 0) {
+        const int slot = atomicAdd(ovf_cnt, 1);
+        ovf[slot] = make_int2(scene, m);
+        out[g] = 1.0f;
+      }
+      continue;
     }
-    return;
-  }
-  double sum = 0.0;
-  for (int q = lane; q < 4 * (k + 1); q += 32) sum += own_edge_term(quads, k, q >> 2, q & 3, s);
+    double sum = 0.0;
+    for (int q = lane; q < 4 * (k + 1); q += 32) sum += own_edge_term(quads, k, q >> 2, q & 3, s);
 #pragma unroll
-  for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-  if (lane == 0) out[g] = own_share(s * sum / 2.0, basp, bh);
+    for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+    if (lane == 0) out[g] = own_share(s * sum / 2.0, basp, bh);
+  }
 }
 
 // Second pass: one CTA per detection that more than kOwnMaxNb boxes overlap (dense crowds).  The overlapping boxes are
@@ -147,8 +150,8 @@ void launch_own_area(const Frame& f, int n_scenes, int max_m, const float* d_box
                      int2* d_ovf, cudaStream_t st) {
   if (n_scenes == 0 || max_m == 0) return;
   cudaMemsetAsync(d_ovf_cnt, 0, sizeof(int), st);
-  dim3 grid((max_m + OW_WARPS - 1) / OW_WARPS, n_scenes);
-  own_area_kernel<<<grid, OW_WARPS * 32, 0, st>>>(f, d_boxes, d_out, d_ovf_cnt, d_ovf);
+  dim3 grid((max_m + OW_WARPS - 1) / OW_WARPS, scene_grid(n_scenes));
+  own_area_kernel<<<grid, OW_WARPS * 32, 0, st>>>(f, d_boxes, d_out, d_ovf_cnt, d_ovf, n_scenes);
   const size_t smem = (size_t)(kOwnBigNb + 1) * 8 * sizeof(double);
   cudaFuncSetAttribute(own_area_big_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   own_area_big_kernel<<<kNumSms, OB_T, smem, st>>>(f, d_boxes, d_out, d_ovf_cnt, d_ovf);

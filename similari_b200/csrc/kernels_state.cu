@@ -553,7 +553,7 @@ __global__ void bf16_regen_kernel(TrackStore ts, int d8, int K, const int* __res
 void launch_bf16_regen(const TrackStore& ts, int d8, int K, const int* rows, long long n, int n_slots, cudaStream_t st) {
   if (rows ? n <= 0 : n_slots <= 0) return;
   const long long warps = rows ? n : (long long)ts.track_cap * K;   // per slot: an upper bound of its arena rows
-  const dim3 grid((unsigned)std::min<long long>((warps + 7) / 8, 2048), rows ? 1u : (unsigned)std::min(n_slots, 65535));
+  const dim3 grid((unsigned)std::min<long long>((warps + 7) / 8, 2048), rows ? 1u : scene_grid(n_slots));
   bf16_regen_kernel<<<grid, 256, 0, st>>>(ts, d8, K, rows, n, n_slots);
   note_launch();
 }

@@ -26,6 +26,10 @@ namespace sb {
 
 constexpr int kMaxConstraints = 8;
 constexpr int kNumSms = 132;  // H100 SXM: grid sizes of the launches that do not query the device
+// gridDim.y and gridDim.z stop at 65,535, and a request's scene count has no bound: a launch with one scene per y (or z)
+// index takes at most this many and its kernel strides over the scenes
+constexpr int kMaxGridYZ = 65535;
+inline unsigned int scene_grid(int n_scenes) { return (unsigned int)(n_scenes < kMaxGridYZ ? n_scenes : kMaxGridYZ); }
 constexpr int kMaxObs = 8;  // visual_max_observations the per-thread kernels keep in registers (reference default 5)
 constexpr int kMaxObsWide = 32;  // visual_max_observations supported on device: above kMaxObs, one warp lane per observation
 constexpr int kStateStride = 32;   // floats per Kalman state row in the tracker's store (kStateFloats padded to 128 bytes)
