@@ -4,7 +4,9 @@
 // and downloads its results once.  Everything a call can reject is checked before anything is launched or changed.
 // The request rows reach the device in one of two ways: an f32 host column is staged row by row in the pinned buffer; a
 // 2-byte host column (uploaded raw) and a device column (read in place) go through fs_stage_kernel.  The store blob
-// (sb200_fstore_save / _load) shares the trackers' section layout, placement and copy machinery (sb_blob.cuh).  The
+// (sb200_fstore_save / _load) shares the trackers' section layout, placement and copy machinery (sb_blob.cuh); all four
+// of its versions go through one section plan (sb::fs_blob_sections), one writer (save) and one loader (load_blob, then
+// the member load, whose device check is fs_class_check_kernel for every version).  The
 // owned calls (search_owned, merge_owned) take stored tracks: their rows never leave the device, and the host reads back
 // only the counts and ring starts of the tracks they touch.  The stored rows are f32, binary16 or bfloat16 (stype,
 // sb200_fstore_set_storage_type); row_bytes() is the size of one stored row, and nothing else on the host depends on the
@@ -105,35 +107,47 @@ struct Column {
 using BlobHeader = sb200_fstore_blob_header;
 using BlobHeaderV2 = sb200_fstore_blob_header_v2;
 using BlobHeaderV3 = sb200_fstore_blob_header_v3;
-enum { kSecIds, kSecCnt, kSecStart, kSecFeat, kSecSrc, kSecT0, kSecT1, kSecQual, kSecHlen, kSecHist };
+using BlobHeaderV4 = sb200_fstore_blob_header_v4;
 static_assert(offsetof(BlobHeaderV2, live) == offsetof(BlobHeader, live), "version 2 repeats version 1's fields");
 static_assert(offsetof(BlobHeaderV3, gate) == offsetof(BlobHeaderV2, gate), "version 3 repeats version 2's fields");
-static_assert(kSecHist + 1 == SB200_FSTORE_BLOB_SECTIONS_V3, "the version-3 section table");
-using BlobHeaderV4 = sb200_fstore_blob_header_v4;
 static_assert(offsetof(BlobHeaderV4, merge_extension) == offsetof(BlobHeaderV3, merge_extension),
               "version 4 repeats version 3's fields");
 static_assert(SB200_FSTORE_MAX_CLASSES == sb::kFsMaxClasses, "the class bound of the kernels");
-// version 4: the shared sections, the class table, then kV4PerClass sections per class from kV4Class
-enum { kV4Ids, kV4Src, kV4T0, kV4T1, kV4Hlen, kV4Hist, kV4ClassIds, kV4ClassDims, kV4Class };
-enum { kV4Cnt, kV4Start, kV4Feat, kV4Qual, kV4PerClass };
-constexpr const char* kV4Names[kV4Class + kV4PerClass] = {"ids", "source", "t_start", "t_end", "history_length", "history",
-                                                          "class_ids", "class_dims", "cnt", "start", "feat", "quality"};
-// The version-4 sections of a store of `live` tracks with the n class dims `dims`: their bytes (which save writes and
-// load expects, the history's from hist_total) and names; returns their number.
-int sections_v4(uint64_t live, int K, int stype, int gate, int keep, int n, const int32_t* dims, uint64_t hist_total,
-                uint64_t* bytes, const char** names) {
-  const uint64_t g = gate ? live * 8 : 0;
-  const uint64_t sh[kV4Class] = {live * 8, g, g, g, keep ? live * 4 : 0, keep ? hist_total * 8 : 0, (uint64_t)n * 8,
-                                 (uint64_t)n * 4};
-  for (int i = 0; i < kV4Class; ++i) { bytes[i] = sh[i]; names[i] = kV4Names[i]; }
-  for (int k = 0; k < n; ++k) {
-    const uint64_t d8 = (uint64_t)(dims[k] + 7) / 8 * 8, at = kV4Class + (uint64_t)kV4PerClass * k;
-    const uint64_t pc[kV4PerClass] = {live * 4, live * 4, live * K * d8 * (stype == SB200_FEATURE_F32 ? 4 : 2),
-                                      keep ? live * K * 4 : 0};
-    for (int j = 0; j < kV4PerClass; ++j) { bytes[at + j] = pc[j]; names[at + j] = kV4Names[kV4Class + j]; }
+
+// The header of each blob version; `version` (1 to 4) names the blob's, and visit(f) calls f on it.
+struct BlobHeaders {
+  uint32_t version;
+  BlobHeader v1;
+  BlobHeaderV2 v2;
+  BlobHeaderV3 v3;
+  BlobHeaderV4 v4;
+  template <class F> auto visit(F&& f) {
+    switch (version) {
+      case 1: return f(v1);
+      case 2: return f(v2);
+      case 3: return f(v3);
+    }
+    return f(v4);
   }
-  return kV4Class + kV4PerClass * n;
-}
+};
+
+// What load reads from a blob's header besides the fields every version shares: a version-1 blob is an ungated newest
+// store, a version-2 blob a gated newest one, and versions 1 to 3 hold one class
+struct BlobView {
+  uint32_t version;
+  int gate = SB200_FSTORE_GATE_NONE, keep = SB200_FSTORE_KEEP_NEWEST, init_cap = 0;
+  float ext = 0.0f;
+  int n_classes = 1;
+  const uint64_t* sec_off = nullptr;
+  const uint64_t* sec_bytes = nullptr;
+};
+// the gate and retention rules a blob of each version may carry (bit r: rule r), by version
+constexpr unsigned kBlobGates[5] = {0, 1u << SB200_FSTORE_GATE_NONE,
+                                    1u << SB200_FSTORE_GATE_SAME_SOURCE | 1u << SB200_FSTORE_GATE_ANY_SOURCE, 7u, 7u};
+constexpr unsigned kBlobKeeps[5] = {0, 1u << SB200_FSTORE_KEEP_NEWEST, 1u << SB200_FSTORE_KEEP_NEWEST,
+                                    1u << SB200_FSTORE_KEEP_BEST_QUALITY, 3u};
+bool allowed(unsigned rules, int r) { return r >= 0 && r < 32 && (rules >> r & 1u); }
+
 // the store kinds that have a column (sb200_fstore::Col::need)
 enum { kNeedAll, kNeedGate, kNeedQuality };
 // which columns a step of alloc / swap_columns handles: every one, the shared ones, or the selected class's
@@ -222,12 +236,12 @@ struct sb200_fstore {
   DBuf dqr;                                  // quality store: the request rows' qualities of a call
   std::vector<std::vector<uint64_t>> hist;   // quality store: merge history of each track, in store order
   // A store column: its buffer, bytes per track (0: K stored rows) or per slot (per_obs), the kind of store that has it
-  // (kNeed*), whether allocation zero-fills it, and its blob section (kSec*) and name.  Without a section (-1) it is
-  // scratch, which growth and compaction start afresh.
+  // (kNeed*), whether allocation zero-fills it, and what its blob sections hold (sb::kFsSec*).  Without a section (-1)
+  // it is scratch, which growth and compaction start afresh.
   // Per-class columns (per_class) exist once per declared feature class; the selected class's sit in the members above
   // and the others' in cls (select).
   struct Col {
-    DBuf sb200_fstore::*buf; uint32_t w; bool per_obs; int need; bool zero; int sec; const char* name; bool per_class;
+    DBuf sb200_fstore::*buf; uint32_t w; bool per_obs; int need; bool zero; int sec; bool per_class;
   };
   static constexpr int kNumCols = 10;
   static const Col kCols[kNumCols];
@@ -269,37 +283,15 @@ struct sb200_fstore {
   }
 
   // bytes of one stored row (observation)
-  static size_t row_bytes(int d8, int stype) { return (size_t)d8 * type_bytes(stype); }
-  size_t row_bytes() const { return row_bytes(d8, stype); }
-  static size_t track_bytes(const Col& c, int K, size_t row_bytes) {
-    return c.w ? (c.per_obs ? (size_t)K * c.w : c.w) : K * row_bytes;
+  size_t row_bytes() const { return (size_t)d8 * type_bytes(stype); }
+  size_t track_bytes(const Col& c) const {
+    const size_t K = o.max_observations;
+    return c.w ? (c.per_obs ? K * c.w : c.w) : K * row_bytes();
   }
-  size_t track_bytes(const Col& c) const { return track_bytes(c, o.max_observations, row_bytes()); }
-  // a store with rule `gate` and retention `keep` has column c
-  static bool has(const Col& c, int gate, int keep) {
+  // the store (its gate rule and retention) has column c
+  bool has(const Col& c) const {
     return c.need == kNeedAll || (c.need == kNeedGate && gate) || (c.need == kNeedQuality && keep);
   }
-  bool has(const Col& c) const { return has(c, gate, keep); }
-  // The blob sections of a store of `live` tracks (kSec* order): their bytes, which save writes and load expects, and
-  // (names != nullptr) their names.  Returns their number: 4, or 7 for a gated store; a quality store (version 3) has
-  // all 10, the attribute ones empty when it is ungated, and hist_total history entries.
-  static int sections(uint64_t live, int K, int d8, int stype, int gate, int keep, uint64_t hist_total, uint64_t* bytes,
-                      const char** names = nullptr) {
-    int n = 0;
-    for (const Col& c : kCols)
-      if (c.sec >= 0 && (has(c, gate, keep) || (keep && c.need == kNeedGate))) {
-        bytes[c.sec] = has(c, gate, keep) ? live * track_bytes(c, K, row_bytes(d8, stype)) : 0;
-        if (names) names[c.sec] = c.name;
-        ++n;
-      }
-    if (keep) {
-      bytes[kSecHist] = hist_total * 8;
-      if (names) names[kSecHist] = "history";
-      ++n;
-    }
-    return n;
-  }
-
   static bool in_part(const Col& c, int part) {
     return part == kPartAll || (part == kPartClass) == c.per_class;
   }
@@ -1765,160 +1757,120 @@ struct sb200_fstore {
     return 0;
   }
 
-  // ---- the store blob (layout: include/similari_b200.h)
-  // the columns and their `n` sections (4, 7 for a gated store, 10 for a quality store: the histories, which have no
-  // device column, are left to the caller) of a blob on this device: dir 0 packs, dir 1 unpacks
-  int move_columns(int dir, const uint64_t* sec_off, const uint64_t* sec_bytes, int n, char* dblob) {
-    char* col[SB200_FSTORE_BLOB_SECTIONS_V3] = {};
-    for (const Col& c : kCols)
-      if (c.sec >= 0) col[c.sec] = (this->*c.buf).as<char>();
+  // ---- the store blob (layouts: include/similari_b200.h)
+  // the device columns and the sections of `plan` at sec_off of a blob at dblob on this device: dir 0 packs, dir 1
+  // unpacks.  Each class's columns are the members while it is selected; the class table and the histories, which have
+  // no device column, are left to the caller.
+  int move(int dir, const std::vector<sb::FsSection>& plan, const uint64_t* sec_off, char* dblob) {
     std::vector<sb::XferSeg> segs;
-    for (int i = 0; i < n; ++i)
-      if (col[i]) sb::add_segment(segs, dir, col[i], dblob + sec_off[i], sec_bytes[i]);
+    each_class([&](int k) {
+      for (size_t i = 0; i < plan.size(); ++i)
+        for (const Col& c : kCols)
+          if (c.sec == plan[i].role && (c.per_class ? plan[i].cls == k : k == 0))
+            sb::add_segment(segs, dir, (this->*c.buf).as<char>(), dblob + sec_off[i], plan[i].bytes);
+      return 0;
+    });
     return sb::copy_segments(segs, num_sms, st);
   }
 
-  // the header fields both versions share
-  template <class H> void fill_header(H& h, uint32_t version) const {
-    memset(&h, 0, sizeof(h));
-    h.magic = SB200_FSTORE_BLOB_MAGIC; h.version = version;
-    h.metric = o.metric; h.distance_filter = o.distance_filter; h.max_observations = o.max_observations;
-    h.feature_dim = o.feature_dim; h.topn = o.topn; h.max_distance = o.max_distance; h.min_votes = o.min_votes;
-    h.d8 = d8; h.feature_type = ftype; h.storage_type = stype; h.live = (int64_t)hid.size();
-  }
-
   int save(void* dst, uint64_t cap_bytes, uint64_t* bytes) {
-    if (!plain_classes()) return save_classes(dst, cap_bytes, bytes);
-    uint64_t sec[SB200_FSTORE_BLOB_SECTIONS_V3];
-    if (keep) {   // version 3: the quality, history length and history sections follow the attribute ones
-      std::vector<uint64_t> hc;
-      for (const std::vector<uint64_t>& h : hist) hc.insert(hc.end(), h.begin(), h.end());
-      const int n = sections(hid.size(), o.max_observations, d8, stype, gate, keep, hc.size(), sec);
-      BlobHeaderV3 h;
-      fill_header(h, SB200_FSTORE_BLOB_VERSION_QUALITY);
+    // a store of the single class 0 writes the version it wrote before classes existed
+    const uint32_t version = !plain_classes() ? 4 : keep ? 3 : gate ? 2 : 1;
+    const int nc = (int)cls.size(), K = o.max_observations, live = (int)hid.size();
+    std::vector<uint64_t> hc, cid(nc);
+    std::vector<int32_t> cdim(nc);
+    for (const std::vector<uint64_t>& h : hist) hc.insert(hc.end(), h.begin(), h.end());
+    for (int k = 0; k < nc; ++k) { cid[k] = cls[k].id; cdim[k] = cls[k].dim; }
+    const std::vector<sb::FsSection> plan =
+        sb::fs_blob_sections((int)version, live, K, stype, gate, keep, nc, cdim.data(), hc.size());
+    std::vector<uint64_t> sec;
+    for (const sb::FsSection& e : plan) sec.push_back(e.bytes);
+    BlobHeaders hs{version};
+    const uint64_t total = hs.visit([&](auto& h) {
+      memset(&h, 0, sizeof(h));
+      h.magic = SB200_FSTORE_BLOB_MAGIC; h.version = version;
+      h.metric = o.metric; h.distance_filter = o.distance_filter; h.max_observations = K; h.topn = o.topn;
+      h.max_distance = o.max_distance; h.min_votes = o.min_votes; h.feature_type = ftype; h.storage_type = stype;
+      h.feature_dim = cls[0].dim;   // not the selected class's: the blob does not depend on the selection
+      h.d8 = cls[0].d8;
+      h.live = live;
+      sb::lay_out(h, sec.data(), (uint32_t)sec.size());
+      return h.total_bytes;
+    });
+    auto rules = [&](auto& h) {
       h.gate = gate;
       h.retention = keep;
       h.initial_capacity = init_cap;
       h.merge_extension = ext;
-      sb::lay_out(h, sec, n);
-      return write_header_and_columns(dst, cap_bytes, bytes, h, n, &hc);
-    }
-    const int n = sections(hid.size(), o.max_observations, d8, stype, gate, keep, 0, sec);
-    if (gate) {   // version 2: the attribute sections follow feat
-      BlobHeaderV2 h;
-      fill_header(h, SB200_FSTORE_BLOB_VERSION_GATED);
-      h.gate = gate;
-      sb::lay_out(h, sec, n);
-      return write_header_and_columns(dst, cap_bytes, bytes, h, n);
-    }
-    BlobHeader h;
-    fill_header(h, SB200_FSTORE_BLOB_VERSION);
-    sb::lay_out(h, sec, n);
-    return write_header_and_columns(dst, cap_bytes, bytes, h, n);
-  }
-
-  // version 4 (a store of other classes than the single class 0)
-  int save_classes(void* dst, uint64_t cap_bytes, uint64_t* bytes) {
-    std::vector<uint64_t> hc;
-    for (const std::vector<uint64_t>& h : hist) hc.insert(hc.end(), h.begin(), h.end());
-    const int nc = (int)cls.size(), K = o.max_observations, live = (int)hid.size();
-    std::vector<uint64_t> cid(nc);
-    std::vector<int32_t> cdim(nc);
-    for (int k = 0; k < nc; ++k) { cid[k] = cls[k].id; cdim[k] = cls[k].dim; }
-    uint64_t sec[SB200_FSTORE_BLOB_SECTIONS_V4];
-    const char* names[SB200_FSTORE_BLOB_SECTIONS_V4];
-    const int n = sections_v4(live, K, stype, gate, keep, nc, cdim.data(), hc.size(), sec, names);
-    BlobHeaderV4 h;
-    fill_header(h, SB200_FSTORE_BLOB_VERSION_CLASSES);
-    h.feature_dim = cls[0].dim;   // not the selected class's: the blob does not depend on the selection
-    h.d8 = cls[0].d8;
-    h.gate = gate;
-    h.retention = keep;
-    h.initial_capacity = init_cap;
-    h.merge_extension = ext;
-    h.n_classes = nc;
-    sb::lay_out(h, sec, n);
-    *bytes = h.total_bytes;
+    };
+    if (version == 2) hs.v2.gate = gate;
+    if (version == 3) rules(hs.v3);
+    if (version == 4) { rules(hs.v4); hs.v4.n_classes = nc; }
+    *bytes = total;
     if (!dst) return 0;
-    if (cap_bytes < h.total_bytes)
-      return fail(SB200_ERR_CAPACITY, "the blob needs %llu bytes", (unsigned long long)h.total_bytes);
+    if (cap_bytes < total) return fail(SB200_ERR_CAPACITY, "the blob needs %llu bytes", (unsigned long long)total);
     CU(cudaSetDevice(o.device));
-    return sb::write_blob(dst, o.device, st, h, n, [&](char* p) {
-      if (int rc = move_classes(0, h.sec_off, p)) return rc;
-      each_class([&](int k) {
-        const uint64_t at = kV4Class + (uint64_t)kV4PerClass * k;
-        sb::fs_launch_blob_scrub(stype, p + h.sec_off[at + kV4Feat], cnt.as<int>(), start.as<int>(), live, K, d8, st);
-        if (keep) sb::fs_launch_qual_scrub(reinterpret_cast<float*>(p + h.sec_off[at + kV4Qual]), cnt.as<int>(),
-                                           start.as<int>(), live, K, st);
-        return 0;
+    return hs.visit([&](const auto& h) {
+      return sb::write_blob(dst, o.device, st, h, (uint32_t)plan.size(), [&](char* p) {
+        auto at = [&](int role, int k = 0) { return p + h.sec_off[sb::fs_blob_section(plan, role, k)]; };
+        if (int rc = move(0, plan, h.sec_off, p)) return rc;
+        each_class([&](int k) {
+          sb::fs_launch_blob_scrub(stype, at(sb::kFsSecFeat, k), cnt.as<int>(), start.as<int>(), live, K, d8, st);
+          if (keep)
+            sb::fs_launch_qual_scrub(reinterpret_cast<float*>(at(sb::kFsSecQuality, k)), cnt.as<int>(), start.as<int>(),
+                                     live, K, st);
+          return 0;
+        });
+        if (version == 4) {
+          CU(cudaMemcpyAsync(at(sb::kFsSecClassIds), cid.data(), nc * 8, cudaMemcpyHostToDevice, st));
+          CU(cudaMemcpyAsync(at(sb::kFsSecClassDims), cdim.data(), nc * 4, cudaMemcpyHostToDevice, st));
+        }
+        if (!hc.empty()) CU(cudaMemcpyAsync(at(sb::kFsSecHistory), hc.data(), hc.size() * 8, cudaMemcpyHostToDevice, st));
+        return finish();
       });
-      CU(cudaMemcpyAsync(p + h.sec_off[kV4ClassIds], cid.data(), nc * 8, cudaMemcpyHostToDevice, st));
-      CU(cudaMemcpyAsync(p + h.sec_off[kV4ClassDims], cdim.data(), nc * 4, cudaMemcpyHostToDevice, st));
-      if (!hc.empty()) CU(cudaMemcpyAsync(p + h.sec_off[kV4Hist], hc.data(), hc.size() * 8, cudaMemcpyHostToDevice, st));
-      return finish();
     });
   }
 
-  // the device columns and the version-4 sections at sec_off of a blob at dblob on this device (dir 0 packs, dir 1
-  // unpacks), for the live tracks
-  int move_classes(int dir, const uint64_t* sec_off, char* dblob) {
-    const uint64_t live = hid.size();
-    const int K = o.max_observations;
-    std::vector<sb::XferSeg> segs;
-    auto add = [&](const DBuf& b, int sec, uint64_t n) {
-      if (n) sb::add_segment(segs, dir, const_cast<char*>(b.as<char>()), dblob + sec_off[sec], n);
-    };
-    add(ids, kV4Ids, live * 8);
-    if (gate) { add(asrc, kV4Src, live * 8); add(at0, kV4T0, live * 8); add(at1, kV4T1, live * 8); }
-    if (keep) add(hlen, kV4Hlen, live * 4);
-    for (int k = 0; k < (int)cls.size(); ++k) {
-      const ClassCols& c = cls[k];
-      const bool me = k == sel;   // the selected class's columns are the members
-      const int at = kV4Class + kV4PerClass * k;
-      add(me ? cnt : c.cnt, at + kV4Cnt, live * 4);
-      add(me ? start : c.start, at + kV4Start, live * 4);
-      add(me ? feat : c.feat, at + kV4Feat, live * K * row_bytes(c.d8, stype));
-      if (keep) add(me ? qual : c.qual, at + kV4Qual, live * K * 4);
-    }
-    return sb::copy_segments(segs, num_sms, st);
-  }
-
-  // fills a store fresh from sb200_fstore_create, whose classes are the blob's, with the version-4 blob `h` at `src`
-  // (checked on the host); refuses what its kernels find
-  int load_classes(const BlobHeaderV4& h, const void* src, std::vector<uint64_t>&& blob_ids,
-                   std::vector<std::vector<uint64_t>>&& hists) {
+  // fills a store fresh from sb200_fstore_create, whose classes are the blob's, with the blob `h` / `v` at `src`, laid
+  // out as `plan` (its host checks passed); refuses what its kernels find
+  int load(const BlobHeader& h, const BlobView& v, const std::vector<sb::FsSection>& plan, const void* src,
+           std::vector<uint64_t>&& blob_ids, std::vector<std::vector<uint64_t>>&& hists) {
     if (int rc = begin()) return rc;
     const int live = (int)h.live, K = o.max_observations, nc = (int)cls.size();
     ftype = h.feature_type;
     stype = h.storage_type;
-    if (int rc = set_gate(h.gate)) return rc;
-    if (int rc = set_retention(h.retention, h.initial_capacity, h.merge_extension)) return rc;
+    if (int rc = set_gate(v.gate)) return rc;
+    if (int rc = set_retention(v.keep, v.init_cap, v.ext)) return rc;
     if (live == 0) return 0;
     if (int rc = reserve((size_t)live)) return rc;
     DBuf tmp;
     const char* dblob = nullptr;
     if (int rc = sb::blob_on_device(src, h.total_bytes, o.device, st, tmp, &dblob)) return rc;
+    auto at = [&](int role, int k = 0) { return dblob + v.sec_off[sb::fs_blob_section(plan, role, k)]; };
+    // counts and ring starts index the rows in every later kernel: checked before anything is copied into the store
     sb::FsClassCols cc{};
     cc.n = nc;
     for (int k = 0; k < nc; ++k) {
-      const int at = kV4Class + kV4PerClass * k;
-      cc.cnt[k] = reinterpret_cast<const int*>(dblob + h.sec_off[at + kV4Cnt]);
-      cc.start[k] = reinterpret_cast<const int*>(dblob + h.sec_off[at + kV4Start]);
+      cc.cnt[k] = reinterpret_cast<const int*>(at(sb::kFsSecCnt, k));
+      cc.start[k] = reinterpret_cast<const int*>(at(sb::kFsSecStart, k));
     }
     int bad[6] = {0, 0, 0, 0, 0, 0};   // class check, windows, quality
     if (int rc = gpos.ensure(sizeof(bad))) return rc;
     CU(cudaMemsetAsync(gpos.p, 0, sizeof(bad), st));
     sb::fs_launch_class_check(cc, live, K, gpos.as<int>(), st);
-    if (h.gate)
-      sb::fs_launch_attr_check(reinterpret_cast<const long long*>(dblob + h.sec_off[kV4T0]),
-                               reinterpret_cast<const long long*>(dblob + h.sec_off[kV4T1]), live, gpos.as<int>() + 3, st);
-    if (h.retention)
+    if (v.gate)
+      sb::fs_launch_attr_check(reinterpret_cast<const long long*>(at(sb::kFsSecTStart)),
+                               reinterpret_cast<const long long*>(at(sb::kFsSecTEnd)), live, gpos.as<int>() + 3, st);
+    if (v.keep)
       for (int k = 0; k < nc; ++k)
-        sb::fs_launch_qual_check(reinterpret_cast<const float*>(dblob + h.sec_off[kV4Class + kV4PerClass * k + kV4Qual]),
-                                 cc.cnt[k], cc.start[k], live, K, gpos.as<int>() + 4, st);
+        sb::fs_launch_qual_check(reinterpret_cast<const float*>(at(sb::kFsSecQuality, k)), cc.cnt[k], cc.start[k], live,
+                                 K, gpos.as<int>() + 4, st);
     CU(cudaMemcpyAsync(bad, gpos.p, sizeof(bad), cudaMemcpyDeviceToHost, st));
     if (int rc = finish()) return rc;
-    if (bad[0]) return fail(SB200_ERR_INVALID, "the blob holds %d cnt entries outside 0..%d", bad[0], K);
+    // versions 1 to 3 hold every track in their one class: a track without rows is a cnt outside their 1..K
+    const int lo = v.version < 4 ? 1 : 0;
+    if (lo) { bad[0] += bad[2]; bad[2] = 0; }
+    if (bad[0]) return fail(SB200_ERR_INVALID, "the blob holds %d cnt entries outside %d..%d", bad[0], lo, K);
     if (bad[1]) return fail(SB200_ERR_INVALID, "the blob holds %d start entries outside 0..%d", bad[1], K - 1);
     if (bad[2]) return fail(SB200_ERR_INVALID, "the blob holds %d tracks without a row in any class", bad[2]);
     if (bad[3]) return fail(SB200_ERR_INVALID, "the blob holds %d windows with t_start > t_end", bad[3]);
@@ -1927,76 +1879,7 @@ struct sb200_fstore {
       return fail(SB200_ERR_INVALID, "the blob holds %d observations out of the quality order (above the one before)",
                   bad[5]);
     hid = std::move(blob_ids);
-    if (int rc = move_classes(1, h.sec_off, const_cast<char*>(dblob))) return rc;
-    hist = std::move(hists);
-    for (size_t p = 0; p < hid.size(); ++p) hpos[hid[p]] = (int)p;
-    return 0;
-  }
-
-  // hc: a quality store's concatenated histories, written into their section
-  template <class H> int write_header_and_columns(void* dst, uint64_t cap_bytes, uint64_t* bytes, const H& h, int n,
-                                                  const std::vector<uint64_t>* hc = nullptr) {
-    *bytes = h.total_bytes;
-    if (!dst) return 0;
-    if (cap_bytes < h.total_bytes)
-      return fail(SB200_ERR_CAPACITY, "the blob needs %llu bytes", (unsigned long long)h.total_bytes);
-    CU(cudaSetDevice(o.device));
-    return sb::write_blob(dst, o.device, st, h, n, [&](char* p) {
-      if (int rc = move_columns(0, h.sec_off, h.sec_bytes, n, p)) return rc;
-      const sb::FsStore s = view();
-      sb::fs_launch_blob_scrub(stype, p + h.sec_off[kSecFeat], s.cnt, s.start, (int)h.live, o.max_observations, d8, st);
-      if (hc) {
-        sb::fs_launch_qual_scrub(reinterpret_cast<float*>(p + h.sec_off[kSecQual]), s.cnt, s.start, (int)h.live,
-                                 o.max_observations, st);
-        if (!hc->empty()) CU(cudaMemcpyAsync(p + h.sec_off[kSecHist], hc->data(), hc->size() * 8, cudaMemcpyHostToDevice, st));
-      }
-      return finish();
-    });
-  }
-
-  // fills a store fresh from sb200_fstore_create with the checked blob `h` at `src`; a version-2 or -3 blob also
-  // carries the rule `rule` and its attribute sections, a version-3 blob the retention `kr` (its parameters init / ex),
-  // the quality section and the histories `hists` (sec_off / sec_bytes: the blob's section table, nsec entries)
-  int load(const BlobHeader& h, int rule, int kr, int init, float ex, const uint64_t* sec_off, const uint64_t* sec_bytes,
-           int nsec, const void* src, std::vector<uint64_t>&& blob_ids, std::vector<std::vector<uint64_t>>&& hists) {
-    if (int rc = begin()) return rc;
-    const int live = (int)h.live, K = o.max_observations;
-    ftype = h.feature_type;
-    stype = h.storage_type;
-    if (int rc = set_gate(rule)) return rc;
-    if (int rc = set_retention(kr, init, ex)) return rc;
-    if (live == 0) return 0;
-    if (int rc = reserve((size_t)live)) return rc;
-    DBuf tmp;
-    const char* dblob = nullptr;
-    if (int rc = sb::blob_on_device(src, h.total_bytes, o.device, st, tmp, &dblob)) return rc;
-    // counts and ring starts index the rows in every later kernel: checked before anything is copied into the store
-    int bad[2] = {0, 0};
-    int bad_w = 0, bad_q[2] = {0, 0};
-    if (int rc = gpos.ensure(sizeof(bad) + sizeof(bad_w) + sizeof(bad_q))) return rc;
-    CU(cudaMemsetAsync(gpos.p, 0, sizeof(bad) + sizeof(bad_w) + sizeof(bad_q), st));
-    sb::fs_launch_blob_check(reinterpret_cast<const int*>(dblob + sec_off[kSecCnt]),
-                             reinterpret_cast<const int*>(dblob + sec_off[kSecStart]), live, K, gpos.as<int>(), st);
-    if (rule)
-      sb::fs_launch_attr_check(reinterpret_cast<const long long*>(dblob + sec_off[kSecT0]),
-                               reinterpret_cast<const long long*>(dblob + sec_off[kSecT1]), live, gpos.as<int>() + 2, st);
-    CU(cudaMemcpyAsync(bad, gpos.p, sizeof(bad), cudaMemcpyDeviceToHost, st));
-    if (kr)
-      sb::fs_launch_qual_check(reinterpret_cast<const float*>(dblob + sec_off[kSecQual]),
-                               reinterpret_cast<const int*>(dblob + sec_off[kSecCnt]),
-                               reinterpret_cast<const int*>(dblob + sec_off[kSecStart]), live, K, gpos.as<int>() + 3, st);
-    CU(cudaMemcpyAsync(&bad_w, gpos.as<int>() + 2, sizeof(bad_w), cudaMemcpyDeviceToHost, st));
-    CU(cudaMemcpyAsync(bad_q, gpos.as<int>() + 3, sizeof(bad_q), cudaMemcpyDeviceToHost, st));
-    if (int rc = finish()) return rc;
-    if (bad[0]) return fail(SB200_ERR_INVALID, "the blob holds %d cnt entries outside 1..%d", bad[0], K);
-    if (bad[1]) return fail(SB200_ERR_INVALID, "the blob holds %d start entries outside 0..%d", bad[1], K - 1);
-    if (bad_w) return fail(SB200_ERR_INVALID, "the blob holds %d windows with t_start > t_end", bad_w);
-    if (bad_q[0]) return fail(SB200_ERR_INVALID, "the blob holds %d NaN qualities in filled slots", bad_q[0]);
-    if (bad_q[1])
-      return fail(SB200_ERR_INVALID, "the blob holds %d observations out of the quality order (above the one before)",
-                  bad_q[1]);
-    if (int rc = move_columns(1, sec_off, sec_bytes, nsec, const_cast<char*>(dblob))) return rc;
-    hid = std::move(blob_ids);
+    if (int rc = move(1, plan, v.sec_off, const_cast<char*>(dblob))) return rc;
     hist = std::move(hists);
     for (size_t p = 0; p < hid.size(); ++p) hpos[hid[p]] = (int)p;
     return 0;
@@ -2004,16 +1887,16 @@ struct sb200_fstore {
 };
 
 const sb200_fstore::Col sb200_fstore::kCols[kNumCols] = {
-    {&sb200_fstore::feat, 0, false, kNeedAll, false, kSecFeat, "feat", true},
-    {&sb200_fstore::cnt, 4, false, kNeedAll, true, kSecCnt, "cnt", true},
-    {&sb200_fstore::start, 4, false, kNeedAll, true, kSecStart, "start", true},
-    {&sb200_fstore::ids, 8, false, kNeedAll, false, kSecIds, "ids", false},
-    {&sb200_fstore::run, 4, false, kNeedAll, true, -1, nullptr, false},
-    {&sb200_fstore::asrc, 8, false, kNeedGate, true, kSecSrc, "source", false},
-    {&sb200_fstore::at0, 8, false, kNeedGate, true, kSecT0, "t_start", false},
-    {&sb200_fstore::at1, 8, false, kNeedGate, true, kSecT1, "t_end", false},
-    {&sb200_fstore::qual, 4, true, kNeedQuality, true, kSecQual, "quality", true},
-    {&sb200_fstore::hlen, 4, false, kNeedQuality, true, kSecHlen, "history_length", false},
+    {&sb200_fstore::feat, 0, false, kNeedAll, false, sb::kFsSecFeat, true},
+    {&sb200_fstore::cnt, 4, false, kNeedAll, true, sb::kFsSecCnt, true},
+    {&sb200_fstore::start, 4, false, kNeedAll, true, sb::kFsSecStart, true},
+    {&sb200_fstore::ids, 8, false, kNeedAll, false, sb::kFsSecIds, false},
+    {&sb200_fstore::run, 4, false, kNeedAll, true, -1, false},
+    {&sb200_fstore::asrc, 8, false, kNeedGate, true, sb::kFsSecSource, false},
+    {&sb200_fstore::at0, 8, false, kNeedGate, true, sb::kFsSecTStart, false},
+    {&sb200_fstore::at1, 8, false, kNeedGate, true, sb::kFsSecTEnd, false},
+    {&sb200_fstore::qual, 4, true, kNeedQuality, true, sb::kFsSecQuality, true},
+    {&sb200_fstore::hlen, 4, false, kNeedQuality, true, sb::kFsSecHistLen, false},
 };
 
 // a call without a handle: SB200_ERR_CUDA when there is no device to have made one, else SB200_ERR_INVALID
@@ -2024,17 +1907,46 @@ int no_handle() {
 
 extern "C" int sb200_fstore_create(const sb200_fstore_options* opts, sb200_fstore** out);
 
-// sb200_fstore_load of a version-4 blob (its magic and version read): every check the host can make from the header,
-// the class table, the ids, the histories and (quality store) the counts, then the store, whose kernels check the rest
-static int load_classes(const void* buf, uint64_t bytes, int32_t device, sb200_fstore** out) {
-  BlobHeaderV4 h;
-  if (bytes < sizeof(h)) return fail(SB200_ERR_INVALID, "the blob is truncated (%llu bytes)", (unsigned long long)bytes);
-  CU(cudaMemcpy(&h, buf, sizeof(h), cudaMemcpyDefault));
-  if (h.gate != SB200_FSTORE_GATE_NONE && h.gate != SB200_FSTORE_GATE_SAME_SOURCE && h.gate != SB200_FSTORE_GATE_ANY_SOURCE)
-    return fail(SB200_ERR_INVALID, "a version-4 blob with unknown gate rule %d", h.gate);
-  if (h.retention != SB200_FSTORE_KEEP_NEWEST && h.retention != SB200_FSTORE_KEEP_BEST_QUALITY)
-    return fail(SB200_ERR_INVALID, "a version-4 blob with unknown retention rule %d", h.retention);
-  const int nc = h.n_classes;
+// sb200_fstore_load on `device`: every check the host can make from the header, the class table, the ids, the
+// histories and (quality store) the counts and ring starts, then the store, whose kernels check the rest
+static int load_blob(const void* buf, uint64_t bytes, int32_t device, sb200_fstore** out) {
+  // no store (and no caller stream) yet: a device blob must be complete when the call is made
+  auto truncated = [&] { return fail(SB200_ERR_INVALID, "the blob is truncated (%llu bytes)", (unsigned long long)bytes); };
+  BlobHeaders hs;
+  const BlobHeader& h = hs.v1;   // the fields every version shares
+  if (bytes < sizeof(h)) return truncated();
+  CU(cudaMemcpy(&hs.v1, buf, sizeof(h), cudaMemcpyDefault));
+  if (h.magic != SB200_FSTORE_BLOB_MAGIC) return fail(SB200_ERR_INVALID, "not a feature store blob (bad magic)");
+  if (h.version < SB200_FSTORE_BLOB_VERSION || h.version > SB200_FSTORE_BLOB_VERSION_CLASSES)
+    return fail(SB200_ERR_INVALID, "feature store blob version %u (this library reads %u to %u)", h.version,
+                SB200_FSTORE_BLOB_VERSION, SB200_FSTORE_BLOB_VERSION_CLASSES);
+  hs.version = h.version;
+  BlobView v;
+  v.version = h.version;
+  if (int rc = hs.visit([&](auto& x) {
+        if (static_cast<const void*>(&x) != &h) {   // a version-1 header is read already
+          if (bytes < sizeof(x)) return truncated();
+          CU(cudaMemcpy(&x, buf, sizeof(x), cudaMemcpyDefault));
+        }
+        v.sec_off = x.sec_off;
+        v.sec_bytes = x.sec_bytes;
+        return 0;
+      }))
+    return rc;
+  auto rules = [&](const auto& x) {
+    v.gate = x.gate;
+    v.keep = x.retention;
+    v.init_cap = x.initial_capacity;
+    v.ext = x.merge_extension;
+  };
+  if (v.version == 2) v.gate = hs.v2.gate;
+  if (v.version == 3) rules(hs.v3);
+  if (v.version == 4) { rules(hs.v4); v.n_classes = hs.v4.n_classes; }
+  if (!allowed(kBlobGates[v.version], v.gate))
+    return fail(SB200_ERR_INVALID, "a version-%u blob with unknown gate rule %d", v.version, v.gate);
+  if (!allowed(kBlobKeeps[v.version], v.keep))
+    return fail(SB200_ERR_INVALID, "a version-%u blob with unknown retention rule %d", v.version, v.keep);
+  const int nc = v.n_classes;
   if (nc < 1 || nc > SB200_FSTORE_MAX_CLASSES)
     return fail(SB200_ERR_INVALID, "n_classes %d outside 1..%d", nc, SB200_FSTORE_MAX_CLASSES);
   if (h.total_bytes > bytes)
@@ -2045,63 +1957,72 @@ static int load_classes(const void* buf, uint64_t bytes, int32_t device, sb200_f
   if (int rc = check_options(o)) return rc;
   if (h.d8 != (h.feature_dim + 7) / 8 * 8) return fail(SB200_ERR_INVALID, "d8 is not feature_dim rounded up to 8");
   if (!known_type(h.feature_type)) return fail(SB200_ERR_INVALID, "unknown feature_type %d", h.feature_type);
+  // before the section sizes, which depend on it
   if (!known_type(h.storage_type)) return fail(SB200_ERR_INVALID, "unknown storage_type %d", h.storage_type);
+  // live * K indexes the distance matrix's columns as an int
   if (h.live < 0 || h.live > INT32_MAX / h.max_observations) return fail(SB200_ERR_INVALID, "live count out of range");
   const int K = h.max_observations;
   const uint64_t live = (uint64_t)h.live;
-  std::vector<int> tab;
-  if (h.retention)
-    if (int rc = capacity_table(K, h.initial_capacity, h.merge_extension, &tab)) return rc;
-  // the section table up to the class table, then the class table, then every section's size
-  const char* name[SB200_FSTORE_BLOB_SECTIONS_V4];
-  uint64_t want[SB200_FSTORE_BLOB_SECTIONS_V4];
-  const int32_t one_dim = 1;
-  const int nsec = sections_v4(live, K, h.storage_type, h.gate, h.retention, nc, std::vector<int32_t>(nc, one_dim).data(),
-                               0, want, name);
-  if (int rc = sb::check_section_table(h, nsec, name)) return rc;
-  if (h.sec_bytes[kV4ClassIds] != (uint64_t)nc * 8 || h.sec_bytes[kV4ClassDims] != (uint64_t)nc * 4)
-    return fail(SB200_ERR_INVALID, "the class table does not hold n_classes = %d entries", nc);
-  std::vector<uint64_t> cid(nc);
-  std::vector<int32_t> cdim(nc);
-  CU(cudaMemcpy(cid.data(), static_cast<const char*>(buf) + h.sec_off[kV4ClassIds], nc * 8, cudaMemcpyDefault));
-  CU(cudaMemcpy(cdim.data(), static_cast<const char*>(buf) + h.sec_off[kV4ClassDims], nc * 4, cudaMemcpyDefault));
-  for (int k = 0; k < nc; ++k) {
-    if (cdim[k] < 1 || cdim[k] > SB200_FSTORE_MAX_DIM)
-      return fail(SB200_ERR_INVALID, "class %llu: feature_dim %d outside 1..%d", (unsigned long long)cid[k], cdim[k],
-                  SB200_FSTORE_MAX_DIM);
-    for (int j = 0; j < k; ++j)
-      if (cid[j] == cid[k]) return fail(SB200_ERR_INVALID, "class id %llu appears twice", (unsigned long long)cid[k]);
+  std::vector<int> tab;   // quality store: c(h)
+  if (v.keep)
+    if (int rc = capacity_table(K, v.init_cap, v.ext, &tab)) return rc;
+  // the section table (a version-4 blob's class dims are not read yet: only the names and the number count), then the
+  // class table, then every section's size
+  std::vector<uint64_t> cid(nc, 0);
+  std::vector<int32_t> cdim(nc, h.feature_dim);
+  std::vector<sb::FsSection> plan =
+      sb::fs_blob_sections((int)v.version, live, K, h.storage_type, v.gate, v.keep, nc, cdim.data(), 0);
+  std::vector<const char*> name;
+  for (const sb::FsSection& e : plan) name.push_back(e.name);
+  if (int rc = hs.visit([&](const auto& x) { return sb::check_section_table(x, (uint32_t)plan.size(), name.data()); }))
+    return rc;
+  auto at = [&](int role, int k = 0) {
+    return static_cast<const char*>(buf) + v.sec_off[sb::fs_blob_section(plan, role, k)];
+  };
+  auto sec_bytes = [&](int role, int k = 0) { return v.sec_bytes[sb::fs_blob_section(plan, role, k)]; };
+  if (v.version == SB200_FSTORE_BLOB_VERSION_CLASSES) {
+    if (sec_bytes(sb::kFsSecClassIds) != (uint64_t)nc * 8 || sec_bytes(sb::kFsSecClassDims) != (uint64_t)nc * 4)
+      return fail(SB200_ERR_INVALID, "the class table does not hold n_classes = %d entries", nc);
+    CU(cudaMemcpy(cid.data(), at(sb::kFsSecClassIds), nc * 8, cudaMemcpyDefault));
+    CU(cudaMemcpy(cdim.data(), at(sb::kFsSecClassDims), nc * 4, cudaMemcpyDefault));
+    for (int k = 0; k < nc; ++k) {
+      if (cdim[k] < 1 || cdim[k] > SB200_FSTORE_MAX_DIM)
+        return fail(SB200_ERR_INVALID, "class %llu: feature_dim %d outside 1..%d", (unsigned long long)cid[k], cdim[k],
+                    SB200_FSTORE_MAX_DIM);
+      for (int j = 0; j < k; ++j)
+        if (cid[j] == cid[k]) return fail(SB200_ERR_INVALID, "class id %llu appears twice", (unsigned long long)cid[k]);
+    }
+    if (cdim[0] != h.feature_dim) return fail(SB200_ERR_INVALID, "feature_dim is not the first class's dim");
+    plan = sb::fs_blob_sections((int)v.version, live, K, h.storage_type, v.gate, v.keep, nc, cdim.data(), 0);
   }
-  if (cdim[0] != h.feature_dim) return fail(SB200_ERR_INVALID, "feature_dim is not the first class's dim");
-  sections_v4(live, K, h.storage_type, h.gate, h.retention, nc, cdim.data(), 0, want, name);
-  for (int i = 0; i < nsec; ++i)
-    if (i != kV4Hist && h.sec_bytes[i] != want[i])   // the history's size is checked against its lengths below
-      return fail(SB200_ERR_INVALID, "section %s holds %llu bytes, %llu expected", name[i],
-                  (unsigned long long)h.sec_bytes[i], (unsigned long long)want[i]);
-  auto at = [&](int sec) { return static_cast<const char*>(buf) + h.sec_off[sec]; };
+  for (size_t i = 0; i < plan.size(); ++i)
+    if (plan[i].role != sb::kFsSecHistory && v.sec_bytes[i] != plan[i].bytes)   // the history's: against its lengths
+      return fail(SB200_ERR_INVALID, "section %s holds %llu bytes, %llu expected", plan[i].name,
+                  (unsigned long long)v.sec_bytes[i], (unsigned long long)plan[i].bytes);
   std::vector<uint64_t> blob_ids(live);
-  if (live) CU(cudaMemcpy(blob_ids.data(), at(kV4Ids), live * 8, cudaMemcpyDefault));
+  if (live) CU(cudaMemcpy(blob_ids.data(), at(sb::kFsSecIds), live * 8, cudaMemcpyDefault));
   std::unordered_set<uint64_t> seen;
   seen.reserve(live * 2);
   for (uint64_t id : blob_ids)
     if (!seen.insert(id).second) return fail(SB200_ERR_INVALID, "id %llu appears twice in the blob", (unsigned long long)id);
-  std::vector<std::vector<uint64_t>> hists;
-  if (h.retention) {   // as version 3, with every class's list
+  std::vector<std::vector<uint64_t>> hists;   // quality store: every history non-empty and led by its track's id
+  if (v.keep) {
     std::vector<int32_t> hl(live);
-    if (live) CU(cudaMemcpy(hl.data(), at(kV4Hlen), live * 4, cudaMemcpyDefault));
+    if (live) CU(cudaMemcpy(hl.data(), at(sb::kFsSecHistLen), live * 4, cudaMemcpyDefault));
     uint64_t total = 0;
     for (uint64_t t = 0; t < live; ++t) {
       if (hl[t] < 1)
         return fail(SB200_ERR_INVALID, "track %llu has a merge history of length %d", (unsigned long long)blob_ids[t], hl[t]);
       total += (uint64_t)hl[t];
     }
-    if (h.sec_bytes[kV4Hist] != total * 8)
+    if (sec_bytes(sb::kFsSecHistory) != total * 8)
       return fail(SB200_ERR_INVALID, "section history holds %llu bytes, %llu expected (the sum of the history lengths)",
-                  (unsigned long long)h.sec_bytes[kV4Hist], (unsigned long long)(total * 8));
+                  (unsigned long long)sec_bytes(sb::kFsSecHistory), (unsigned long long)(total * 8));
+    // a state the rule produces: every list of every class from ring slot 0, and no longer than its capacity
     std::vector<int32_t> cn(live), sn(live);
     for (int k = 0; k < nc && live; ++k) {
-      CU(cudaMemcpy(cn.data(), at(kV4Class + kV4PerClass * k + kV4Cnt), live * 4, cudaMemcpyDefault));
-      CU(cudaMemcpy(sn.data(), at(kV4Class + kV4PerClass * k + kV4Start), live * 4, cudaMemcpyDefault));
+      CU(cudaMemcpy(cn.data(), at(sb::kFsSecCnt, k), live * 4, cudaMemcpyDefault));
+      CU(cudaMemcpy(sn.data(), at(sb::kFsSecStart, k), live * 4, cudaMemcpyDefault));
       for (uint64_t t = 0; t < live; ++t) {
         if (sn[t] != 0)
           return fail(SB200_ERR_INVALID, "track %llu has ring start %d; a quality store's lists start at slot 0",
@@ -2113,7 +2034,7 @@ static int load_classes(const void* buf, uint64_t bytes, int32_t device, sb200_f
       }
     }
     std::vector<uint64_t> hc(total);
-    if (total) CU(cudaMemcpy(hc.data(), at(kV4Hist), total * 8, cudaMemcpyDefault));
+    if (total) CU(cudaMemcpy(hc.data(), at(sb::kFsSecHistory), total * 8, cudaMemcpyDefault));
     hists.resize(live);
     for (uint64_t t = 0, a = 0; t < live; a += (uint64_t)hl[t], ++t) {
       hists[t].assign(hc.begin() + a, hc.begin() + a + hl[t]);
@@ -2121,13 +2042,14 @@ static int load_classes(const void* buf, uint64_t bytes, int32_t device, sb200_f
         return fail(SB200_ERR_INVALID, "the merge history of track %llu starts with %llu, not with its id",
                     (unsigned long long)blob_ids[t], (unsigned long long)hists[t][0]);
     }
-  } else if (h.sec_bytes[kV4Hist] != 0) {
+  } else if (v.version == SB200_FSTORE_BLOB_VERSION_CLASSES && sec_bytes(sb::kFsSecHistory) != 0) {
     return fail(SB200_ERR_INVALID, "a newest store's blob with a history section");
   }
   sb200_fstore* s = nullptr;
   if (int rc = sb200_fstore_create(&o, &s)) return rc;
-  int rc = s->set_classes(nc, cid.data(), cdim.data());
-  if (!rc) rc = s->load_classes(h, buf, std::move(blob_ids), std::move(hists));
+  // the fresh store holds the single class 0 of feature_dim, which versions 1 to 3 declare
+  int rc = v.version == SB200_FSTORE_BLOB_VERSION_CLASSES ? s->set_classes(nc, cid.data(), cdim.data()) : 0;
+  if (!rc) rc = s->load(h, v, plan, buf, std::move(blob_ids), std::move(hists));
   if (rc) {
     sb200_fstore_destroy(s);   // the handle owns every buffer made so far
     return rc;
@@ -2501,123 +2423,7 @@ int sb200_fstore_load(const void* buf, uint64_t bytes, int32_t device, sb200_fst
   *out = nullptr;
   if (int rc = sb::check_device(device)) return rc;
   CU(cudaSetDevice(device));
-  // no store (and no caller stream) yet: a device blob must be complete when the call is made
-  if (bytes < sizeof(BlobHeader)) return fail(SB200_ERR_INVALID, "the blob is truncated (%llu bytes)", (unsigned long long)bytes);
-  BlobHeader h;
-  CU(cudaMemcpy(&h, buf, sizeof(h), cudaMemcpyDefault));
-  if (h.magic != SB200_FSTORE_BLOB_MAGIC) return fail(SB200_ERR_INVALID, "not a feature store blob (bad magic)");
-  if (h.version == SB200_FSTORE_BLOB_VERSION_CLASSES) return load_classes(buf, bytes, device, out);
-  if (h.version != SB200_FSTORE_BLOB_VERSION && h.version != SB200_FSTORE_BLOB_VERSION_GATED &&
-      h.version != SB200_FSTORE_BLOB_VERSION_QUALITY)
-    return fail(SB200_ERR_INVALID, "feature store blob version %u (this library reads %u to %u)", h.version,
-                SB200_FSTORE_BLOB_VERSION, SB200_FSTORE_BLOB_VERSION_CLASSES);
-  // version 2 (a gated store): the same fields, the rule and a 7-section table
-  const bool v2 = h.version == SB200_FSTORE_BLOB_VERSION_GATED;
-  BlobHeaderV2 h2;
-  memset(&h2, 0, sizeof(h2));
-  if (v2) {
-    if (bytes < sizeof(h2)) return fail(SB200_ERR_INVALID, "the blob is truncated (%llu bytes)", (unsigned long long)bytes);
-    CU(cudaMemcpy(&h2, buf, sizeof(h2), cudaMemcpyDefault));
-    if (h2.gate != SB200_FSTORE_GATE_SAME_SOURCE && h2.gate != SB200_FSTORE_GATE_ANY_SOURCE)
-      return fail(SB200_ERR_INVALID, "a version-2 blob with unknown gate rule %d", h2.gate);
-  }
-  // version 3 (a quality store): version 2's fields, the retention and its parameters, and a 10-section table
-  const bool v3 = h.version == SB200_FSTORE_BLOB_VERSION_QUALITY;
-  BlobHeaderV3 h3;
-  memset(&h3, 0, sizeof(h3));
-  if (v3) {
-    if (bytes < sizeof(h3)) return fail(SB200_ERR_INVALID, "the blob is truncated (%llu bytes)", (unsigned long long)bytes);
-    CU(cudaMemcpy(&h3, buf, sizeof(h3), cudaMemcpyDefault));
-    if (h3.gate != SB200_FSTORE_GATE_NONE && h3.gate != SB200_FSTORE_GATE_SAME_SOURCE &&
-        h3.gate != SB200_FSTORE_GATE_ANY_SOURCE)
-      return fail(SB200_ERR_INVALID, "a version-3 blob with unknown gate rule %d", h3.gate);
-    if (h3.retention != SB200_FSTORE_KEEP_BEST_QUALITY)
-      return fail(SB200_ERR_INVALID, "a version-3 blob with unknown retention rule %d", h3.retention);
-  }
-  const uint64_t* sec_off = v3 ? h3.sec_off : v2 ? h2.sec_off : h.sec_off;
-  const uint64_t* sec_bytes = v3 ? h3.sec_bytes : v2 ? h2.sec_bytes : h.sec_bytes;
-  const int gate = v3 ? h3.gate : v2 ? h2.gate : SB200_FSTORE_GATE_NONE;
-  const int keep = v3 ? h3.retention : SB200_FSTORE_KEEP_NEWEST;
-  if (h.total_bytes > bytes)
-    return fail(SB200_ERR_INVALID, "the blob is truncated (%llu of total_bytes %llu)", (unsigned long long)bytes,
-                (unsigned long long)h.total_bytes);
-  sb200_fstore_options o = {h.metric, h.distance_filter, h.max_observations, h.feature_dim, h.topn, h.max_distance,
-                            h.min_votes, device};
-  if (int rc = check_options(o)) return rc;
-  if (h.d8 != (h.feature_dim + 7) / 8 * 8) return fail(SB200_ERR_INVALID, "d8 is not feature_dim rounded up to 8");
-  if (!known_type(h.feature_type)) return fail(SB200_ERR_INVALID, "unknown feature_type %d", h.feature_type);
-  // before the section sizes, which depend on it
-  if (!known_type(h.storage_type)) return fail(SB200_ERR_INVALID, "unknown storage_type %d", h.storage_type);
-  // live * K indexes the distance matrix's columns as an int
-  if (h.live < 0 || h.live > INT32_MAX / h.max_observations) return fail(SB200_ERR_INVALID, "live count out of range");
-  std::vector<int> tab;   // version 3: c(h)
-  if (v3)
-    if (int rc = capacity_table(h.max_observations, h3.initial_capacity, h3.merge_extension, &tab)) return rc;
-  const uint64_t live = (uint64_t)h.live;
-  uint64_t want[SB200_FSTORE_BLOB_SECTIONS_V3];
-  const char* name[SB200_FSTORE_BLOB_SECTIONS_V3];
-  const int nsec = sb200_fstore::sections(live, h.max_observations, h.d8, h.storage_type, gate, keep, 0, want, name);
-  if (int rc = v3   ? sb::check_section_table(h3, nsec, name)
-               : v2 ? sb::check_section_table(h2, nsec, name)
-                    : sb::check_section_table(h, nsec, name))
-    return rc;
-  for (int i = 0; i < nsec; ++i)
-    if (i != kSecHist && sec_bytes[i] != want[i])   // the history's size is checked against its lengths below
-      return fail(SB200_ERR_INVALID, "section %s holds %llu bytes, %llu expected", name[i],
-                  (unsigned long long)sec_bytes[i], (unsigned long long)want[i]);
-  std::vector<uint64_t> blob_ids(live);
-  if (live) CU(cudaMemcpy(blob_ids.data(), static_cast<const char*>(buf) + sec_off[kSecIds], live * 8, cudaMemcpyDefault));
-  std::unordered_set<uint64_t> seen;
-  seen.reserve(live * 2);
-  for (uint64_t id : blob_ids)
-    if (!seen.insert(id).second) return fail(SB200_ERR_INVALID, "id %llu appears twice in the blob", (unsigned long long)id);
-  std::vector<std::vector<uint64_t>> hists;   // version 3: every history non-empty and led by its track's id
-  if (v3) {
-    std::vector<int32_t> hl(live);
-    if (live) CU(cudaMemcpy(hl.data(), static_cast<const char*>(buf) + sec_off[kSecHlen], live * 4, cudaMemcpyDefault));
-    uint64_t total = 0;
-    for (uint64_t t = 0; t < live; ++t) {
-      if (hl[t] < 1)
-        return fail(SB200_ERR_INVALID, "track %llu has a merge history of length %d", (unsigned long long)blob_ids[t], hl[t]);
-      total += (uint64_t)hl[t];
-    }
-    if (sec_bytes[kSecHist] != total * 8)
-      return fail(SB200_ERR_INVALID, "section history holds %llu bytes, %llu expected (the sum of the history lengths)",
-                  (unsigned long long)sec_bytes[kSecHist], (unsigned long long)(total * 8));
-    // a state the rule produces: every list from ring slot 0, and no longer than its capacity
-    std::vector<int32_t> cn(live), sn(live);
-    if (live) {
-      CU(cudaMemcpy(cn.data(), static_cast<const char*>(buf) + sec_off[kSecCnt], live * 4, cudaMemcpyDefault));
-      CU(cudaMemcpy(sn.data(), static_cast<const char*>(buf) + sec_off[kSecStart], live * 4, cudaMemcpyDefault));
-    }
-    for (uint64_t t = 0; t < live; ++t) {
-      if (sn[t] != 0)
-        return fail(SB200_ERR_INVALID, "track %llu has ring start %d; a quality store's lists start at slot 0",
-                    (unsigned long long)blob_ids[t], sn[t]);
-      const int c = tab[std::min<size_t>((size_t)hl[t], tab.size() - 1)];
-      if (cn[t] > c)
-        return fail(SB200_ERR_INVALID, "track %llu holds %d observations, above its capacity %d at history length %d",
-                    (unsigned long long)blob_ids[t], cn[t], c, hl[t]);
-    }
-    std::vector<uint64_t> hc(total);
-    if (total) CU(cudaMemcpy(hc.data(), static_cast<const char*>(buf) + sec_off[kSecHist], total * 8, cudaMemcpyDefault));
-    hists.resize(live);
-    for (uint64_t t = 0, at = 0; t < live; at += (uint64_t)hl[t], ++t) {
-      hists[t].assign(hc.begin() + at, hc.begin() + at + hl[t]);
-      if (hists[t][0] != blob_ids[t])
-        return fail(SB200_ERR_INVALID, "the merge history of track %llu starts with %llu, not with its id",
-                    (unsigned long long)blob_ids[t], (unsigned long long)hists[t][0]);
-    }
-  }
-  sb200_fstore* s = nullptr;
-  if (int rc = sb200_fstore_create(&o, &s)) return rc;
-  if (int rc = s->load(h, gate, keep, h3.initial_capacity, h3.merge_extension, sec_off, sec_bytes, nsec, buf,
-                       std::move(blob_ids), std::move(hists))) {
-    sb200_fstore_destroy(s);   // the handle owns every buffer made so far
-    return rc;
-  }
-  *out = s;
-  return 0;
+  return load_blob(buf, bytes, device, out);
 }
 
 }  // extern "C"

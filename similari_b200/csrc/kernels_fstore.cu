@@ -1,5 +1,6 @@
 // kernels_fstore.cu -- the feature track store's call: distances, TopN voting, merge / append; the request rows built
-// from a typed or device-resident feature column (fs_stage_kernel); the index check and slot scrub of the store blob.
+// from a typed or device-resident feature column (fs_stage_kernel); the slot scrub of the store blob, whose index check
+// is fs_class_check_kernel for every blob version.
 // Every kernel that touches stored rows is a template over their element type Elem (float, __half or __nv_bfloat16,
 // FsStore::stype); its launcher picks the instance.  A 2-byte stored element is widened to f32 from its bits where it is
 // loaded, which is exact, so every stage after the load sees f32 values; fs_apply_kernel rounds a request row once when
@@ -705,16 +706,6 @@ __global__ void __launch_bounds__(256) fs_stage_kernel(const T* __restrict__ col
 }
 
 // ------------------------------------------------------------------------------------------------ store blob
-__global__ void fs_blob_check_kernel(const int* __restrict__ cnt, const int* __restrict__ start, int n, int K, int* bad) {
-  int bc = 0, bs = 0;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    bc += (cnt[i] < 1 || cnt[i] > K);
-    bs += (start[i] < 0 || start[i] >= K);
-  }
-  if (bc) atomicAdd(bad, bc);
-  if (bs) atomicAdd(bad + 1, bs);
-}
-
 // one warp per track; a track whose ring is full has nothing to zero
 template <typename Elem>
 __global__ void fs_blob_scrub_kernel(Elem* feat, const int* __restrict__ cnt, const int* __restrict__ start, int n, int K,
@@ -1139,12 +1130,6 @@ void fs_launch_stage(int type, const void* col, const int* row_src, int R, int D
     fs_stage_kernel<T><<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(static_cast<const T*>(col), row_src, R, D, d8, vec,
                                                                          rows);
   });
-  note_launch();
-}
-
-void fs_launch_blob_check(const int* cnt, const int* start, int n, int K, int* bad, cudaStream_t st) {
-  if (n == 0) return;
-  fs_blob_check_kernel<<<std::min((n + 255) / 256, 1024), 256, 0, st>>>(cnt, start, n, K, bad);
   note_launch();
 }
 

@@ -13,6 +13,8 @@
 #include <climits>
 #include <vector>
 
+#include "../../include/similari_b200.h"
+
 namespace sb {
 
 constexpr int kFsMaxTopn = 64;
@@ -154,8 +156,6 @@ void fs_launch_attr_gather(const FsAttrCols& a, const int* pos, int n, const FsA
 void fs_launch_attr_scatter(const FsAttrCols& a, const int* pos, int n, const FsAttrCols& in, cudaStream_t st);
 // store blob of a gated store, before anything is copied: bad[0] counts the windows with t0 > t1
 void fs_launch_attr_check(const long long* t0, const long long* t1, int n, int* bad, cudaStream_t st);
-// store blob, before any row is copied: bad[0] counts the cnt[i] outside [1, K], bad[1] the start[i] outside [0, K)
-void fs_launch_blob_check(const int* cnt, const int* start, int n, int K, int* bad, cudaStream_t st);
 // store blob, after its rows are copied: zeroes, in feat[n][K][d8] (elements of stype), the ring slots that hold no
 // observation
 void fs_launch_blob_scrub(int stype, void* feat, const int* cnt, const int* start, int n, int K, int d8, cudaStream_t st);
@@ -170,8 +170,8 @@ struct FsClassCols {
 };
 // out[i][k] = cnt of class k at pos[i] (0 for pos[i] < 0)
 void fs_launch_class_counts(const FsClassCols& cc, const int* pos, int n, int* out, cudaStream_t st);
-// store blob of version 4, before anything is copied (the columns: the blob's sections): bad[0] counts the cnt outside
-// [0, K], bad[1] the start outside [0, K), bad[2] the tracks without a row in any class
+// store blob of any version, before anything is copied (the columns: the blob's sections): bad[0] counts the cnt outside
+// [0, K], bad[1] the start outside [0, K), bad[2] the tracks without a row in any class (of one class: the cnt of 0)
 void fs_launch_class_check(const FsClassCols& cc, int n, int K, int* bad, cudaStream_t st);
 
 // ---- a quality store (sb200_fstore_set_retention): observations kept in the track's order in ring slots 0, 1, ... (the
@@ -212,5 +212,64 @@ void fs_launch_words_compact(const void* src, void* dst, const int* from, int n,
 void fs_launch_qual_check(const float* qual, const int* cnt, const int* start, int n, int K, int* bad, cudaStream_t st);
 // store blob, after its sections are copied: zeroes the qualities of the slots that hold no observation
 void fs_launch_qual_scrub(float* qual, const int* cnt, const int* start, int n, int K, cudaStream_t st);
+
+// ---- the store blob's sections (layouts: include/similari_b200.h).  What a section holds:
+enum {
+  kFsSecIds, kFsSecSource, kFsSecTStart, kFsSecTEnd, kFsSecHistLen, kFsSecHistory, kFsSecClassIds, kFsSecClassDims,
+  kFsSecCnt, kFsSecStart, kFsSecFeat, kFsSecQuality
+};
+struct FsSection {
+  const char* name;
+  uint64_t bytes;
+  int role;   // kFsSec*
+  int cls;    // the class index of a per-class section (cnt, start, feat, quality), else 0
+};
+
+// The sections of a blob of `version` (1 to 4), in blob order, for a store of `live` tracks of K observations stored as
+// `stype`, with gate rule `gate`, retention rule `keep`, n classes of dims[] and hist_total merge history entries.
+// Versions 1 to 3 are one class's; a version-2 blob is gated, and a version-3 one keeps by quality.  Host code only.
+inline std::vector<FsSection> fs_blob_sections(int version, uint64_t live, int K, int stype, int gate, int keep, int n,
+                                               const int32_t* dims, uint64_t hist_total) {
+  static const char* const kNames[] = {"ids",        "source",     "t_start", "t_end", "history_length", "history",
+                                       "class_ids",  "class_dims", "cnt",     "start", "feat",           "quality"};
+  std::vector<FsSection> out;
+  auto add = [&](int role, uint64_t bytes, int k = 0) { out.push_back({kNames[role], bytes, role, k}); };
+  const uint64_t g = gate ? live * 8 : 0, hl = keep ? live * 4 : 0, h = keep ? hist_total * 8 : 0;
+  const uint64_t q = keep ? live * K * 4 : 0, elem = stype == SB200_FEATURE_F32 ? 4 : 2;
+  auto feat = [&](int k) { return live * K * ((uint64_t)(dims[k] + 7) / 8 * 8) * elem; };
+  auto attrs = [&] { add(kFsSecSource, g); add(kFsSecTStart, g); add(kFsSecTEnd, g); };
+  add(kFsSecIds, live * 8);
+  if (version < 4) {
+    add(kFsSecCnt, live * 4);
+    add(kFsSecStart, live * 4);
+    add(kFsSecFeat, feat(0));
+    if (version >= 2) attrs();
+    if (version == 3) {
+      add(kFsSecQuality, q);
+      add(kFsSecHistLen, hl);
+      add(kFsSecHistory, h);
+    }
+    return out;
+  }
+  attrs();
+  add(kFsSecHistLen, hl);
+  add(kFsSecHistory, h);
+  add(kFsSecClassIds, (uint64_t)n * 8);
+  add(kFsSecClassDims, (uint64_t)n * 4);
+  for (int k = 0; k < n; ++k) {
+    add(kFsSecCnt, live * 4, k);
+    add(kFsSecStart, live * 4, k);
+    add(kFsSecFeat, feat(k), k);
+    add(kFsSecQuality, q, k);
+  }
+  return out;
+}
+
+// the index in `plan` of the section of `role` (and class k), or -1
+inline int fs_blob_section(const std::vector<FsSection>& plan, int role, int k = 0) {
+  for (size_t i = 0; i < plan.size(); ++i)
+    if (plan[i].role == role && plan[i].cls == k) return (int)i;
+  return -1;
+}
 
 }  // namespace sb

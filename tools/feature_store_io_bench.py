@@ -159,7 +159,7 @@ def blob_profile(st, info):
     kernels = {}
     for e in prof.events():
         if e.device_type == torch.autograd.DeviceType.CUDA and "kernel" in e.name:
-            name = next((k for k in ("xfer_copy_kernel", "fs_blob_scrub_kernel", "fs_blob_check_kernel") if k in e.name),
+            name = next((k for k in ("xfer_copy_kernel", "fs_blob_scrub_kernel", "fs_class_check_kernel") if k in e.name),
                         e.name)
             kernels.setdefault(name, []).append(e.device_time if hasattr(e, "device_time") else e.cuda_time)
     copy_us = [v for k, v in kernels.items() if "xfer_copy_kernel" in k]
