@@ -340,6 +340,13 @@ def ptr(a):
     return a.ctypes.data_as(C.c_void_p)
 
 
+def check_int32(v, what):
+    """Raises OverflowError unless v fits an int32 argument or field: ctypes would store it modulo 2^32 without a word."""
+    if not -(2**31) <= int(v) < 2**31:
+        raise OverflowError(f"{what} {int(v)} is outside int32")
+    return int(v)
+
+
 def default_options(**kw) -> Options:
     o = Options()
     lib().sb200_options_default(C.byref(o))
@@ -349,11 +356,13 @@ def default_options(**kw) -> Options:
             raise Sb200Error(f"at most {MAX_CONSTRAINTS} spatio-temporal constraints")
         o.n_constraints = len(constraints)
         for i, (e, d) in enumerate(constraints):
-            o.constraint_epochs[i] = int(e)
+            o.constraint_epochs[i] = check_int32(e, "constraint epoch")
             o.constraint_max_dist[i] = float(d)
     for k, v in kw.items():
         if not hasattr(o, k):
             raise AttributeError(k)
+        if dict(Options._fields_)[k] is C.c_int32:
+            v = check_int32(v, k)
         setattr(o, k, v)
     return o
 

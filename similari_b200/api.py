@@ -132,6 +132,15 @@ class VisualSortMetricType:
         return VisualSortMetricType(_lib.VIS_COSINE, threshold)
 
 
+def _sorted_unique(constraints):
+    """Stable sort by epoch, then the first entry of every epoch (spatio_temporal_constraints.rs:36-46)."""
+    out = []
+    for c in sorted(constraints, key=lambda c: c[0]):
+        if not out or out[-1][0] != c[0]:
+            out.append(c)
+    return out
+
+
 class SpatioTemporalConstraints:
     """src/trackers/spatio_temporal_constraints.rs `PySpatioTemporalConstraints`."""
 
@@ -139,15 +148,19 @@ class SpatioTemporalConstraints:
         self.constraints: List[Tuple[int, float]] = []
 
     def add_constraints(self, constraints):
+        new = []
         for d, m in constraints:
+            if int(d) < 0:   # the reference's epochs are usize
+                raise OverflowError(f"constraint epoch {int(d)} is negative")
             assert m > 0.0, "The distance is expected to be a positive float"
-            self.constraints.append((int(d), float(m)))
-        self.constraints.sort(key=lambda c: c[0])  # stable; dedup keeps the first
-        out = []
-        for c in self.constraints:
-            if not out or out[-1][0] != c[0]:
-                out.append(c)
-        self.constraints = out
+            new.append((int(d), float(m)))
+        self.constraints = _sorted_unique(self.constraints + new)
+
+    def _tracker_constraints(self):
+        """The list a tracker's int32 options take.  max_idle_epochs is an int32, so no epoch delta a tracker compares
+        exceeds 2^31 - 1, and for every such delta an epoch above 2^31 - 1 decides as 2^31 - 1 does: epochs are
+        saturated there, and of the entries that then share 2^31 - 1 the first -- the one validate() reaches -- is kept."""
+        return _sorted_unique([(min(d, 2**31 - 1), m) for d, m in self.constraints])
 
     def validate(self, epoch_delta, dist):
         assert dist >= 0.0, "The distance is expected to be a positive float"
@@ -283,7 +296,7 @@ def _sort_options(kind, bbox_history, max_idle_epochs, method, min_confidence, c
     return default_options(kind=kind, positional_kind=method.kind, iou_threshold=method.threshold,
                            min_confidence=min_confidence, max_idle_epochs=int(max_idle_epochs),
                            history_length=int(bbox_history), kalman_position_weight=pw, kalman_velocity_weight=vw,
-                           constraints=constraints.constraints if constraints else None)
+                           constraints=constraints._tracker_constraints() if constraints else None)
 
 
 class Sort(_TrackerBase):
@@ -397,7 +410,7 @@ class VisualSortOptions:
         self._kw["visual_kind"], self._kw["visual_threshold"] = metric.kind, metric.threshold
 
     def spatio_temporal_constraints(self, constraints: SpatioTemporalConstraints):
-        self._constraints = constraints.constraints
+        self._constraints = constraints._tracker_constraints()
 
     def positional_metric(self, metric: PositionalMetricType):
         self._kw["positional_kind"], self._kw["iou_threshold"] = metric.kind, metric.threshold

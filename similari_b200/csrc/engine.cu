@@ -79,6 +79,8 @@ int make_params(const sb200_options& o, sb::Params* out) {
   for (int i = 0; i < o.n_constraints; ++i) {
     if (!(o.constraint_max_dist[i] > 0.0f))
       return fail(SB200_ERR_INVALID, "The distance is expected to be a positive float");
+    // the reference's epochs are usize; compat_ok compares them as unsigned
+    if (o.constraint_epochs[i] < 0) return fail(SB200_ERR_INVALID, "constraint epochs must be >= 0");
     c.emplace_back(o.constraint_epochs[i], o.constraint_max_dist[i]);
   }
   std::stable_sort(c.begin(), c.end(), [](const std::pair<int, float>& a, const std::pair<int, float>& b) { return a.first < b.first; });
@@ -699,6 +701,12 @@ struct sb200_tracker {
       std::unordered_map<uint64_t, int> seen;
       for (int s = 0; s < n_scenes; ++s)
         if (!seen.emplace(scene_ids[s], s).second) return fail(SB200_ERR_INVALID, "scene %llu appears twice in one request", (unsigned long long)scene_ids[s]);
+    }
+    // the host epochs already count the frames in flight
+    for (int s = 0; s < n_scenes; ++s) {
+      const int slot = rq.same_req ? last_req_slots[s] : slot_for(scene_ids[s], false);
+      if (slot >= 0 && epoch[slot] == UINT32_MAX)
+        return fail(SB200_ERR_INVALID, "scene %llu is at the last epoch %u", (unsigned long long)scene_ids[s], UINT32_MAX);
     }
     // the on-chip assignment solver holds a scene's rows and columns in shared memory
     int max_m0 = 0, max_n0 = 0;
@@ -1664,6 +1672,10 @@ int sb200_skip_epochs(sb200_tracker* t, uint64_t scene_id, int32_t n) {
   if (!t || n < 0) return fail(SB200_ERR_INVALID, "bad arguments");
   CU(cudaSetDevice(t->device));
   { int rc_ = t->drain(); if (rc_) return rc_; }
+  const int old = t->slot_for(scene_id, false);   // a new scene is at epoch 0: n < 2^31 always fits
+  if (old >= 0 && (uint64_t)t->epoch[old] + (uint64_t)n > UINT32_MAX)
+    return fail(SB200_ERR_INVALID, "scene %llu: epoch %u + %d is past the last epoch %u", (unsigned long long)scene_id,
+                t->epoch[old], n, UINT32_MAX);
   int slot = t->slot_for(scene_id, true);
   int rc = t->ensure_store((int)t->scene_of_slot.size(), std::max(t->track_cap, 64));
   if (rc) return rc;

@@ -18,7 +18,9 @@ namespace sb {
 // --------------------------------------------------------------------------------------------------------
 // prep: one thread per detection. Candidate track construction (sort/simple_api.rs:125-145): the Kalman
 // initiate->predict->update of a fresh state leaves the box unchanged except angle == 0.0 -> None
-// (src/utils/kalman.rs:82-86); confidence is preserved (kalman_prediction.rs:28-29).
+// (src/utils/kalman.rs:82-86); confidence is preserved (kalman_prediction.rs:28-29).  A NaN or infinite centre, aspect,
+// height or angle (a NaN angle is None) makes every component of that state NaN (0 * NaN in the update), so the
+// candidate's box is NaN but for its confidence: its gate distances, its IoU and its feature's area test see NaN.
 __global__ void prep_kernel(Params p, Frame f) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= f.total) return;
@@ -27,6 +29,8 @@ __global__ void prep_kernel(Params p, Frame f) {
   const float* b = f.in_boxes + (size_t)i * 6;
   float xc = b[0], yc = b[1], ang = b[2], asp = b[3], h = b[4], conf = b[5];
   if (ang == 0.0f) ang = nanf("");
+  if (!isfinite(xc) || !isfinite(yc) || !isfinite(asp) || !isfinite(h) || isinf(ang))
+    xc = yc = ang = asp = h = nanf("");
   float* cb = f.c_box + (size_t)i * 6;
   cb[0] = xc; cb[1] = yc; cb[2] = ang; cb[3] = asp; cb[4] = h; cb[5] = conf;
   f.c_radius[i] = box_radius(asp, h);

@@ -702,7 +702,9 @@ __global__ void __launch_bounds__(WT) waste_kernel(Params p, TrackStore ts, cons
   int seen = 0;   // expired tracks in the chunks before (uniform)
   for (int j0 = 0; j0 < n; j0 += WT) {
     const int j = j0 + tid;
-    const int w = (j < n && ts.epoch[base + j] + (unsigned int)p.max_idle_epochs < cur) ? 1 : 0;
+    // cur - ep > max_idle: the reference's ep + max_idle < cur in usize, which ep + max_idle in u32 can wrap past
+    const unsigned int ep = j < n ? ts.epoch[base + j] : cur;
+    const int w = (cur > ep && cur - ep > (unsigned int)p.max_idle_epochs) ? 1 : 0;
     int x = w;
 #pragma unroll
     for (int o = 1; o < 32; o <<= 1) {

@@ -10,7 +10,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from ._lib import Options, PredictOut, check, default_options, lib, ptr
+from ._lib import Options, PredictOut, check, check_int32, default_options, lib, ptr
 
 F32MAX = float(np.finfo(np.float32).max)
 
@@ -209,6 +209,7 @@ class Tracker:
                                                  vp(d_own_area), C.byref(po)))
 
     def skip_epochs(self, n, scene_id=0):
+        check_int32(n, "skip_epochs count")   # ctypes would pass it on modulo 2^32
         check(self._L.sb200_skip_epochs(self._h, scene_id, n))
 
     def current_epoch(self, scene_id=0):

@@ -30,6 +30,10 @@ float shim_maha(float pw, const float* st, const float* b) {
   return sb::maha_distance(st, l5, b[0], b[1], sb::angle_or0(b[2]), b[3], b[4]);
 }
 long long shim_weight(float v) { return sb::weight_i64(v); }
+float shim_box_radius(float aspect, float height) { return sb::box_radius(aspect, height); }
+float shim_dist_in_2r(float xl, float yl, float rl, float xr, float yr, float rr) {
+  return sb::dist_in_2r(xl, yl, rl, xr, yr, rr);
+}
 void shim_own_area_shares(const float* boxes, int n, float* out) {
   for (int i = 0; i < n; ++i) out[i] = sb::own_area_share_seq(boxes, n, i);
 }
