@@ -10,6 +10,10 @@ import numpy as np
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+HEADER = os.path.join(ROOT, "include", "similari_b200.h")
+# the header's return and scalar parameter types, as ctypes binds them
+CTYPES = {"void": None, "int": C.c_int, "int32_t": C.c_int32, "int64_t": C.c_int64, "uint64_t": C.c_uint64,
+          "float": C.c_float, "size_t": C.c_size_t, "void*": C.c_void_p, "const char*": C.c_char_p}
 
 
 @pytest.fixture(scope="module")
@@ -23,12 +27,33 @@ def L():
 def test_exports_every_declared_symbol(L):
     from similari_b200 import _lib
 
-    hdr = open(os.path.join(ROOT, "include", "similari_b200.h")).read()
+    hdr = open(HEADER).read()
     declared = set(re.findall(r"\b(sb200_[a-z0-9_]+)\s*\(", hdr))
     assert declared, "no declarations parsed"
     assert declared == set(_lib.EXPORTS), declared ^ set(_lib.EXPORTS)
     for name in declared:
         assert getattr(L, name) is not None
+    for name in _lib.EXPORTS:
+        assert getattr(L, name).argtypes is not None, name
+
+
+def test_bindings_match_the_declarations(L):
+    """Each declared function is bound with the header's return type and one argtype per parameter: the scalar's own
+    type, or a pointer type for a pointer."""
+    hdr = re.sub(r"/\*.*?\*/|//[^\n]*", "", open(HEADER).read(), flags=re.S)
+    decls = re.findall(r"(\w[\w ]*\**)\s*\b(sb200_[a-z0-9_]+)\s*\(([^)]*)\)\s*;", hdr)
+    assert len(decls) == len(set(n for _, n, _ in decls)) > 100
+    for ret, name, params in decls:
+        fn = getattr(L, name)
+        assert fn.restype is CTYPES[" ".join(ret.split())], (name, ret, fn.restype)
+        params = [] if params.strip() in ("", "void") else [" ".join(p.split()) for p in params.split(",")]
+        assert len(fn.argtypes) == len(params), name
+        for p, t in zip(params, fn.argtypes):
+            typ = re.sub(r"\s*\b\w+$", "", p) if re.search(r"[\s*]\w+$", p) else p
+            if typ.endswith("*"):
+                assert t in (C.c_void_p, C.c_char_p) or issubclass(t, C._Pointer), (name, p, t)
+            else:
+                assert t is CTYPES[typ], (name, p, t)
 
 
 def test_exports_only_declared_symbols(L):
@@ -81,6 +106,64 @@ def test_no_cpu_fallback(L):
         import similari_b200.engine as eng
 
         eng.Tracker(o)
+
+
+def test_store_entry_points_fail_without_a_gpu(L):
+    """Without a CUDA device every feature-store entry point fails loudly with SB200_ERR_CUDA, and the Python store
+    refuses to be created or loaded."""
+    from similari_b200 import _lib
+    import similari_b200.engine as eng
+
+    if L.sb200_device_count() > 0:
+        pytest.skip("a GPU is present; the loud-failure path is for CPU-only machines")
+    p = _lib.ptr
+    o = _lib.FstoreOptions(0, 100.0, 3, 256, 1, 100.0, 1, 0)
+    h = C.c_void_p()
+    assert L.sb200_fstore_create(C.byref(o), C.byref(h)) == -2 and h.value is None
+    ids = np.zeros(1, np.uint64)
+    offs = np.array([0, 1], np.int32)
+    f = np.zeros((1, 256), np.float32)
+    cnt = np.zeros(1, np.int32)
+    w = np.zeros(1, np.float64)
+    m = np.zeros(1, np.uint8)
+    t = np.zeros(1, np.int64)
+    assert L.sb200_fstore_add(None, 1, p(ids), p(f)) == -2
+    assert L.sb200_fstore_search(None, 1, p(ids), p(offs), p(f), p(cnt), p(ids), p(w)) == -2
+    assert L.sb200_fstore_associate(None, 1, p(ids), p(offs), p(f), p(cnt), p(ids), p(w), p(ids), p(m)) == -2
+    assert L.sb200_fstore_fetch(None, 1, p(ids), 0, p(cnt), p(f)) == -2
+    assert L.sb200_fstore_size(None) == -2
+    assert L.sb200_fstore_ids(None, 1, p(ids)) == -2
+    assert L.sb200_fstore_last_stage_ms(None, p(f)) == -2
+    L.sb200_fstore_destroy(None)
+    assert L.sb200_fstore_set_feature_type(None, 1) == -2
+    assert L.sb200_fstore_get_options(None, None, None) == -2
+    assert L.sb200_fstore_add_device(None, 1, p(ids), None, None) == -2
+    assert L.sb200_fstore_search_device(None, 1, p(ids), p(offs), None, p(cnt), p(ids), p(w), None) == -2
+    assert L.sb200_fstore_associate_device(None, 1, p(ids), p(offs), None, p(cnt), p(ids), p(w), p(ids), p(m),
+                                           None) == -2
+    n = C.c_uint64(0)
+    assert L.sb200_fstore_save(None, None, 0, C.byref(n)) == -2
+    blob = np.zeros(1024, np.uint8)
+    assert L.sb200_fstore_load(p(blob), len(blob), 0, C.byref(h)) == -2 and h.value is None
+    assert b"no CUDA device" in L.sb200_last_error()
+    assert L.sb200_fstore_search_owned(None, 1, p(ids), 0, p(cnt), p(ids), p(w)) == -2
+    assert L.sb200_fstore_merge_owned(None, 1, p(ids), p(ids), 1) == -2
+    assert b"no CUDA device" in L.sb200_last_error()
+    st = C.c_int32(5)
+    assert L.sb200_fstore_set_storage_type(None, 1) == -2
+    assert L.sb200_fstore_get_storage_type(None, C.byref(st)) == -2 and st.value == 5
+    assert b"no CUDA device" in L.sb200_last_error()
+    assert L.sb200_fstore_set_gate(None, 1) == -2
+    assert L.sb200_fstore_fetch_attr(None, 1, p(ids), p(ids), p(t), p(t)) == -2
+    assert b"no CUDA device" in L.sb200_last_error()
+    with pytest.raises(_lib.Sb200Error):
+        eng.FeatureStore()
+    with pytest.raises(_lib.Sb200Error, match="-2"):
+        eng.FeatureStore.load(blob)
+    with pytest.raises(_lib.Sb200Error, match="-2"):
+        eng.FeatureStore(storage="f16")
+    with pytest.raises(ValueError, match="storage"):
+        eng.FeatureStore(storage="f8")
 
 
 def test_invalid_arguments_are_reported(L):

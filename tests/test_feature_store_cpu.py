@@ -1,8 +1,6 @@
 """CPU checks of the feature track store: the oracle's TopN voting against the known answers of
 src/track/voting/topn.rs, the oracle's store semantics on hand-built cases (keep-newest-K, same-id skip, the strict
-distance filter, max_dist across the queries of a call, min_votes, the tie order), and the C ABI without a GPU."""
-import ctypes as C
-
+distance filter, max_dist across the queries of a call, min_votes, the tie order)."""
 import numpy as np
 import pytest
 
@@ -142,34 +140,3 @@ def test_rejected_requests():
     with pytest.raises(ValueError):
         s.associate(*_q([1], [[1.0]]))
     assert list(s.ids()) == [1]
-
-
-def test_entry_points_fail_without_a_gpu():
-    from similari_b200 import _build, _lib
-
-    _build.build()
-    L = _lib.lib()
-    if L.sb200_device_count() > 0:
-        pytest.skip("a GPU is present; the loud-failure path is for CPU-only machines")
-    o = _lib.FstoreOptions(0, 100.0, 3, 256, 1, 100.0, 1, 0)
-    h = C.c_void_p()
-    assert L.sb200_fstore_create(C.byref(o), C.byref(h)) == -2 and h.value is None
-    ids = np.zeros(1, np.uint64)
-    offs = np.array([0, 1], np.int32)
-    f = np.zeros((1, 256), np.float32)
-    cnt = np.zeros(1, np.int32)
-    w = np.zeros(1, np.float64)
-    m = np.zeros(1, np.uint8)
-    p = _lib.ptr
-    assert L.sb200_fstore_add(None, 1, p(ids), p(f)) == -2
-    assert L.sb200_fstore_search(None, 1, p(ids), p(offs), p(f), p(cnt), p(ids), p(w)) == -2
-    assert L.sb200_fstore_associate(None, 1, p(ids), p(offs), p(f), p(cnt), p(ids), p(w), p(ids), p(m)) == -2
-    assert L.sb200_fstore_fetch(None, 1, p(ids), 0, p(cnt), p(f)) == -2
-    assert L.sb200_fstore_size(None) == -2
-    assert L.sb200_fstore_ids(None, 1, p(ids)) == -2
-    assert L.sb200_fstore_last_stage_ms(None, p(f)) == -2
-    L.sb200_fstore_destroy(None)
-    import similari_b200.engine as eng
-
-    with pytest.raises(_lib.Sb200Error):
-        eng.FeatureStore()

@@ -4,16 +4,12 @@ The query rule of search_tracks on the oracles alone: an oracle tracker is fed a
 feature-less detections, a merge below the collect threshold), its scene_observations give Track::obs, and each track's
 present rows in that order go to an fstore_oracle search.  A store keeps the last max_observations rows of a query, so
 with the store's K below the tracker's present count the NEWEST observation is the one dropped (optimize swaps it to
-the front); one case pins that by hand.  The entry points are declared, exported and typed, and refuse NULL handles
-without touching a device."""
+the front); one case pins that by hand.  The entry points refuse NULL handles without touching a device."""
 import ctypes as C
-import os
-import re
 
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 D = 12
 Q_COLLECT = 0.4
 # (quality, has_feature) of detection 0 (the new track) and of every merge after it
@@ -136,18 +132,6 @@ def test_featureless_tracks_are_not_queried(oracle):
     obs = o.scene_observations(0)
     assert obs["n_obs"].tolist() == [1] and not obs["has_feat"].any()
     assert len(_present(obs, 0)[0]) == 0
-
-
-def test_declared_exported_and_typed(L):
-    from similari_b200 import _lib
-
-    hdr = open(os.path.join(ROOT, "include", "similari_b200.h")).read()
-    assert re.search(r"\bint64_t sb200_scene_observations\(sb200_tracker\* t, uint64_t scene_id, int64_t cap", hdr)
-    assert re.search(r"\bint sb200_fstore_search_tracks\(sb200_fstore\* s, sb200_tracker\* t, int32_t n", hdr)
-    for name, res, nargs in (("sb200_scene_observations", C.c_int64, 8), ("sb200_fstore_search_tracks", C.c_int, 13)):
-        assert name in _lib.EXPORTS
-        fn = getattr(L, name)
-        assert fn.restype is res and len(fn.argtypes) == nargs
 
 
 def test_null_handles_without_a_device(L):

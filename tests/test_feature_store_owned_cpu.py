@@ -1,18 +1,11 @@
 """CPU checks of the feature store's owned calls (search_owned, merge_owned): the oracle on hand-built 1-d stores with
-weights worked out by hand, the oracle's owned calls against compositions of its existing calls, and the C ABI without a
-GPU."""
-import ctypes as C
-import os
-import re
-
+weights worked out by hand, and the oracle's owned calls against compositions of its existing calls."""
 import numpy as np
 import pytest
 
 import fstore_oracle as fo
+from fstore_checks import same_results
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-HEADER = os.path.join(ROOT, "include", "similari_b200.h")
-NEW = ["sb200_fstore_search_owned", "sb200_fstore_merge_owned"]
 
 
 def _store(**kw):
@@ -143,12 +136,6 @@ def _random_store(seed, metric, **kw):
     return make, rng
 
 
-def _same(a, b):
-    for k in ("counts", "winners"):
-        assert np.array_equal(a[k], b[k]), k
-    assert np.array_equal(a["weights"].view(np.uint64), b["weights"].view(np.uint64))
-
-
 @pytest.mark.parametrize("metric", [fo.EUCLIDEAN, fo.COSINE])
 def test_each_equals_one_search_of_the_fetched_rows_per_id(metric):
     make, rng = _random_store(1 + metric, metric)
@@ -162,7 +149,7 @@ def test_each_equals_one_search_of_the_fetched_rows_per_id(metric):
             assert r["counts"][i] == 0
             continue
         one = s.search([qid], np.array([0, cnt[0]], np.int32), f[0, :cnt[0]])
-        _same({k: v[i:i + 1] for k, v in r.items()}, one)
+        same_results({k: v[i:i + 1] for k, v in r.items()}, one)
 
 
 @pytest.mark.parametrize("metric", [fo.EUCLIDEAN, fo.COSINE])
@@ -175,7 +162,7 @@ def test_group_equals_a_search_on_a_copy_without_the_queried_ids(metric):
     cnt, f = copy.fetch(q, remove=True)
     offs = np.concatenate([[0], np.cumsum(cnt)]).astype(np.int32)
     rows = np.concatenate([f[i, :cnt[i]] for i in range(len(q))])
-    _same(r, copy.search(q, offs, rows))
+    same_results(r, copy.search(q, offs, rows))
     assert np.array_equal(s.ids(), make().ids())   # the owned search leaves the store as it was
 
 
@@ -203,35 +190,3 @@ def test_merge_equals_fetch_and_add():
         cs, fs = s.fetch(s.ids())
         ce, fe = e.fetch(e.ids())
         assert np.array_equal(cs, ce) and np.array_equal(fs.view(np.uint32), fe.view(np.uint32))
-
-
-@pytest.fixture(scope="module")
-def L():
-    from similari_b200 import _build, _lib
-
-    _build.build()
-    return _lib.lib()
-
-
-def test_new_symbols_are_declared_and_exported(L):
-    from similari_b200 import _lib
-
-    hdr = open(HEADER).read()
-    for name in NEW:
-        assert re.search(r"\b%s\s*\(" % name, hdr), name
-        assert name in _lib.EXPORTS
-        assert getattr(L, name).argtypes is not None
-
-
-def test_entry_points_fail_without_a_gpu(L):
-    from similari_b200 import _lib
-
-    if L.sb200_device_count() > 0:
-        pytest.skip("a GPU is present; the loud-failure path is for CPU-only machines")
-    ids = np.zeros(1, np.uint64)
-    cnt = np.zeros(1, np.int32)
-    w = np.zeros(1, np.float64)
-    p = _lib.ptr
-    assert L.sb200_fstore_search_owned(None, 1, p(ids), 0, p(cnt), p(ids), p(w)) == -2
-    assert L.sb200_fstore_merge_owned(None, 1, p(ids), p(ids), 1) == -2
-    assert b"no CUDA device" in L.sb200_last_error()

@@ -1,40 +1,12 @@
-"""CPU checks of the feature store's storage type (sb200_fstore_set_storage_type / _get_storage_type): the two entry
-points are declared, exported and typed, the blob header mirror carries storage_type, both fail loudly without a GPU, and
-the numpy rounding model the GPU tests compare stored rows with (fstore_oracle.round_rows) equals numpy's float16 and
-torch's bfloat16 conversions bit for bit."""
+"""CPU checks of the feature store's storage type (sb200_fstore_set_storage_type / _get_storage_type): the blob header
+mirror carries storage_type, and the numpy rounding model the GPU tests compare stored rows with
+(fstore_oracle.round_rows) equals numpy's float16 and torch's bfloat16 conversions bit for bit."""
 import ctypes as C
-import os
-import re
 
 import numpy as np
 import pytest
 
 import fstore_oracle as fo
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-HEADER = os.path.join(ROOT, "include", "similari_b200.h")
-NEW = ["sb200_fstore_set_storage_type", "sb200_fstore_get_storage_type"]
-
-
-@pytest.fixture(scope="module")
-def L():
-    from similari_b200 import _build, _lib
-
-    _build.build()
-    return _lib.lib()
-
-
-def test_new_symbols_are_declared_exported_and_typed(L):
-    from similari_b200 import _lib
-
-    hdr = open(HEADER).read()
-    for name in NEW:
-        assert re.search(r"\bint %s\(sb200_fstore\* s, int32_t" % name, hdr), name
-        assert name in _lib.EXPORTS
-        fn = getattr(L, name)
-        assert fn.argtypes is not None and fn.restype is C.c_int
-    assert L.sb200_fstore_set_storage_type.argtypes == [C.c_void_p, C.c_int32]
-    assert L.sb200_fstore_get_storage_type.argtypes[1]._type_ is C.c_int32
 
 
 def test_blob_header_carries_the_storage_type():
@@ -46,22 +18,6 @@ def test_blob_header_carries_the_storage_type():
     assert _lib.FstoreBlobHeader.storage_type.offset == 52 and C.sizeof(_lib.FstoreBlobHeader) == 128
     assert _lib.FSTORE_BLOB_VERSION == 1   # an f32 store's blob is what it was; 0 there is SB200_FEATURE_F32
     assert _lib.FEATURE_F32 == 0
-
-
-def test_entry_points_fail_without_a_gpu(L):
-    import similari_b200.engine as eng
-    from similari_b200 import _lib
-
-    if L.sb200_device_count() > 0:
-        pytest.skip("a GPU is present; the loud-failure path is for CPU-only machines")
-    t = C.c_int32(5)
-    assert L.sb200_fstore_set_storage_type(None, 1) == -2
-    assert L.sb200_fstore_get_storage_type(None, C.byref(t)) == -2 and t.value == 5
-    assert b"no CUDA device" in L.sb200_last_error()
-    with pytest.raises(_lib.Sb200Error, match="-2"):
-        eng.FeatureStore(storage="f16")
-    with pytest.raises(ValueError, match="storage"):
-        eng.FeatureStore(storage="f8")
 
 
 # ------------------------------------------------------------------------------------------------ the rounding model

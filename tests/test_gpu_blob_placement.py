@@ -8,6 +8,7 @@ import numpy as np
 import pytest
 
 import test_gpu_feature_store_storage as fss
+from fstore_checks import same_results
 import test_gpu_state_transfer as tst
 from test_gpu_state_transfer import eng  # noqa: F401  (the module's fixture)
 
@@ -92,4 +93,4 @@ def test_store_blob_at_any_offset(off, storage):
     for st in steps:   # fresh ids: the script's query ids must not be stored yet
         if st[0] in ("search", "associate"):
             st[1][:] += 5000
-    fss._same(fss._run(dev, steps, raw), fss._run(host, steps, raw))
+    same_results(fss._run(dev, steps, raw), fss._run(host, steps, raw))

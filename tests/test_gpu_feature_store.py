@@ -3,40 +3,12 @@ winner ids, f64 weights, merged flags and the stored observations after every ca
 import numpy as np
 import pytest
 
-import fstore_oracle as fo
+from fstore_checks import same_results, same_store, store_pair
 from similari_b200.workload import FeatGen
 
 pytestmark = pytest.mark.gpu
-
-METRICS = {"euclidean": fo.EUCLIDEAN, "cosine": fo.COSINE}
-
-
-def _pair(metric="euclidean", **kw):
-    import similari_b200.engine as eng
-
-    opts = dict(distance_filter=100.0, max_observations=3, feature_dim=256, topn=1, max_distance=100.0, min_votes=1)
-    opts.update(kw)
-    return eng.FeatureStore(metric=metric, **opts), fo.FeatureStore(metric=METRICS[metric], **opts)
-
-
-def _same_results(rg, ro):
-    for k in ro:
-        a, b = rg[k], ro[k]
-        assert a.dtype == b.dtype and a.shape == b.shape, k
-        if a.dtype == np.float64:
-            assert np.array_equal(a.view(np.uint64), b.view(np.uint64)), (k, a, b)
-        else:
-            assert np.array_equal(a, b), (k, a, b)
-
-
-def _same_store(g, o):
-    ids = o.ids()
-    assert np.array_equal(g.ids(), ids)
-    assert g.size() == o.size() == len(ids)
-    cg, fg = g.fetch(ids)
-    co, fo_ = o.fetch(ids)
-    assert np.array_equal(cg, co)
-    assert np.array_equal(fg.view(np.uint32), fo_.view(np.uint32))
+# the options of benches/feature_tracker.rs (engine.FeatureStore's defaults)
+BENCH = dict(distance_filter=100.0, feature_dim=256, topn=1, max_distance=100.0)
 
 
 def _queries(rows_per_query, dim):
@@ -51,15 +23,15 @@ def _queries(rows_per_query, dim):
 def test_feature_tracker_loop(metric, objects):
     """benches/feature_tracker.rs: every iteration one new single-observation track per object, associated with TopN(1,
     100.0, 1) under d < 100.0, K = 3, D = 256."""
-    g, o = _pair(metric)
+    g, o = store_pair(metric, **BENCH)
     gens = [FeatGen(1000.0 * i, 256, 0.1, seed=1000 + i) for i in range(objects)]
     iteration = 0
     for _ in range(20):
         ids = np.arange(iteration + 1, iteration + 1 + objects, dtype=np.uint64)
         iteration += objects
         offs, feats = _queries([[gen.next()] for gen in gens], 256)
-        _same_results(g.associate(ids, offs, feats), o.associate(ids, offs, feats))
-        _same_store(g, o)
+        same_results(g.associate(ids, offs, feats), o.associate(ids, offs, feats))
+        same_store(g, o)
     assert g.size() >= objects
     assert np.all(g.last_stage_ms() >= 0)
 
@@ -68,14 +40,14 @@ def test_feature_tracker_loop(metric, objects):
 def test_track_search_shape(metric):
     """benches/track_search.rs's shape: a 30-observation query against 100 tracks of 30 observations."""
     rng = np.random.default_rng(7)
-    g, o = _pair(metric, max_observations=30, feature_dim=128, topn=5, distance_filter=1e9, max_distance=1e9)
+    g, o = store_pair(metric, max_observations=30, feature_dim=128, topn=5)
     ids = np.repeat(np.arange(1, 101, dtype=np.uint64), 30)
     feats = rng.standard_normal((3000, 128)).astype(np.float32)
     g.add(ids, feats)
     o.add(ids, feats)
-    _same_store(g, o)
+    same_store(g, o)
     offs, q = _queries([rng.standard_normal((30, 128))], 128)
-    _same_results(g.search(np.array([1000], np.uint64), offs, q), o.search(np.array([1000], np.uint64), offs, q))
+    same_results(g.search(np.array([1000], np.uint64), offs, q), o.search(np.array([1000], np.uint64), offs, q))
 
 
 @pytest.mark.parametrize("metric", ["euclidean", "cosine"])
@@ -84,20 +56,20 @@ def test_track_search_shape(metric):
 def test_dims_and_topn(metric, dim, topn):
     """D a multiple of 8, not one, and wide; topn 1, 5 and more than the store holds (40 tracks)."""
     rng = np.random.default_rng(dim * 100 + topn)
-    g, o = _pair(metric, feature_dim=dim, topn=topn, max_observations=4, distance_filter=1e9, max_distance=1e9)
+    g, o = store_pair(metric, feature_dim=dim, topn=topn, max_observations=4)
     for step in range(3):
         n = 40
         ids = rng.integers(1, 41, n).astype(np.uint64)
         f = rng.standard_normal((n, dim)).astype(np.float32)
         g.add(ids, f)
         o.add(ids, f)
-        _same_store(g, o)
+        same_store(g, o)
         qid = np.arange(100, 108, dtype=np.uint64)
         offs, q = _queries([rng.standard_normal((k % 6 + 1, dim)) for k in range(8)], dim)
-        _same_results(g.search(qid, offs, q), o.search(qid, offs, q))
+        same_results(g.search(qid, offs, q), o.search(qid, offs, q))
         qid = qid + 1000 * (step + 1)
-        _same_results(g.associate(qid, offs, q), o.associate(qid, offs, q))
-        _same_store(g, o)
+        same_results(g.associate(qid, offs, q), o.associate(qid, offs, q))
+        same_store(g, o)
 
 
 @pytest.mark.parametrize("metric", ["euclidean", "cosine"])
@@ -115,43 +87,43 @@ def test_min_votes_and_exact_thresholds(metric):
     ds = sorted(dist(queries[0], t) for t in tracks)
     for min_votes in (2, 3):
         for md, flt in ((ds[20], ds[40]), (ds[5], ds[20])):
-            g, o = _pair(metric, feature_dim=dim, max_observations=3, topn=8, min_votes=min_votes, max_distance=md,
-                         distance_filter=flt)
+            g, o = store_pair(metric, feature_dim=dim, max_observations=3, topn=8, min_votes=min_votes, max_distance=md,
+                              distance_filter=flt)
             g.add(ids, tracks)
             o.add(ids, tracks)
             offs, q = _queries([queries[:2], queries[2:]], dim)
             qid = np.array([500, 501], np.uint64)
             ro = o.search(qid, offs, q)
-            _same_results(g.search(qid, offs, q), ro)
-            _same_results(g.associate(qid, offs, q), o.associate(qid, offs, q))
-            _same_store(g, o)
+            same_results(g.search(qid, offs, q), ro)
+            same_results(g.associate(qid, offs, q), o.associate(qid, offs, q))
+            same_store(g, o)
 
 
 @pytest.mark.parametrize("metric", ["euclidean", "cosine"])
 def test_ties_empty_store_and_remove_then_add(metric):
     rng = np.random.default_rng(3)
     dim = 16
-    g, o = _pair(metric, feature_dim=dim, topn=6, distance_filter=1e9, max_distance=1e9)
+    g, o = store_pair(metric, feature_dim=dim, topn=6)
     offs, q = _queries([rng.standard_normal((2, dim))], dim)
-    _same_results(g.search(np.array([9], np.uint64), offs, q), o.search(np.array([9], np.uint64), offs, q))
+    same_results(g.search(np.array([9], np.uint64), offs, q), o.search(np.array([9], np.uint64), offs, q))
     base = rng.standard_normal((1, dim)).astype(np.float32)
     dup = np.repeat(base, 5, axis=0)   # five identical tracks: equal weights, store order decides
     ids = np.array([30, 10, 50, 20, 40], np.uint64)
     for s in (g, o):
         s.add(ids, dup)
-    _same_results(g.search(np.array([9], np.uint64), offs, q), o.search(np.array([9], np.uint64), offs, q))
+    same_results(g.search(np.array([9], np.uint64), offs, q), o.search(np.array([9], np.uint64), offs, q))
     r = g.search(np.array([9], np.uint64), offs, q)
     assert r["winners"][0, :5].tolist() == [30, 10, 50, 20, 40]
     for s in (g, o):
         s.fetch(np.array([10, 77, 10], np.uint64), remove=True)
         s.add(np.array([10, 60], np.uint64), dup[:2])
-    _same_store(g, o)
-    _same_results(g.search(np.array([9], np.uint64), offs, q), o.search(np.array([9], np.uint64), offs, q))
+    same_store(g, o)
+    same_results(g.search(np.array([9], np.uint64), offs, q), o.search(np.array([9], np.uint64), offs, q))
     cg = g.fetch(np.array([10, 77, 10], np.uint64))
     co = o.fetch(np.array([10, 77, 10], np.uint64))
     assert np.array_equal(cg[0], co[0]) and np.array_equal(cg[1], co[1])
-    _same_results(g.associate(np.array([9], np.uint64), offs, q), o.associate(np.array([9], np.uint64), offs, q))
-    _same_store(g, o)
+    same_results(g.associate(np.array([9], np.uint64), offs, q), o.associate(np.array([9], np.uint64), offs, q))
+    same_store(g, o)
 
 
 @pytest.mark.parametrize("metric", ["euclidean", "cosine"])
@@ -165,7 +137,7 @@ def test_degenerate_features(metric):
     t[3, 0] = np.inf
     t[4] = 1e30
     t[5] = 1e-30
-    g, o = _pair(metric, feature_dim=dim, topn=8, distance_filter=50.0, max_distance=20.0)
+    g, o = store_pair(metric, feature_dim=dim, topn=8, distance_filter=50.0, max_distance=20.0)
     ids = np.arange(1, 9, dtype=np.uint64)
     g.add(ids, t)
     o.add(ids, t)
@@ -175,22 +147,22 @@ def test_degenerate_features(metric):
     q[3, 7] = -np.inf
     offs, qf = _queries([q[:2], q[2:4], q[4:]], dim)
     qid = np.array([100, 101, 102], np.uint64)
-    _same_results(g.search(qid, offs, qf), o.search(qid, offs, qf))
-    _same_results(g.associate(qid, offs, qf), o.associate(qid, offs, qf))
-    _same_store(g, o)
+    same_results(g.search(qid, offs, qf), o.search(qid, offs, qf))
+    same_results(g.associate(qid, offs, qf), o.associate(qid, offs, qf))
+    same_store(g, o)
 
 
 def test_growth_across_calls():
     rng = np.random.default_rng(9)
-    g, o = _pair("euclidean", feature_dim=32, max_observations=2, topn=3, distance_filter=9.0, max_distance=4.0)
+    g, o = store_pair("euclidean", feature_dim=32, max_observations=2, topn=3, distance_filter=9.0, max_distance=4.0)
     nid = 1
     for step in range(12):
         n = 50 * (step + 1)
         ids = np.arange(nid, nid + n, dtype=np.uint64)
         nid += n
         offs, q = _queries([rng.standard_normal((1 + i % 3, 32)) for i in range(n)], 32)
-        _same_results(g.associate(ids, offs, q), o.associate(ids, offs, q))
-        _same_store(g, o)
+        same_results(g.associate(ids, offs, q), o.associate(ids, offs, q))
+        same_store(g, o)
     assert g.size() > 2000
 
 
@@ -199,7 +171,7 @@ def test_rejected_calls_change_nothing():
     import similari_b200.engine as eng
 
     rng = np.random.default_rng(1)
-    g, o = _pair("euclidean", feature_dim=8, max_observations=64, topn=2)
+    g, o = store_pair("euclidean", **BENCH | dict(feature_dim=8, max_observations=64, topn=2))
     ids = np.arange(1, 16385, dtype=np.uint64)
     f = rng.standard_normal((len(ids), 8)).astype(np.float32)
     g.add(ids, f)
@@ -232,7 +204,7 @@ def test_rejected_calls_change_nothing():
         with pytest.raises(Sb200Error, match="-3"):
             call(np.arange(100000, 101025, dtype=np.uint64), offs, big)
         unchanged()
-    _same_store(g, o)
+    same_store(g, o)
     for kw in (dict(topn=65), dict(max_observations=65), dict(feature_dim=8193), dict(topn=0)):
         opts = dict(feature_dim=8)
         opts.update(kw)

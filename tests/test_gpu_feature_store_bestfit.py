@@ -11,12 +11,16 @@ import numpy as np
 import pytest
 
 import fstore_oracle as fo
+from fstore_checks import gpu_store, same_results, same_store, store_pair
 
 pytestmark = pytest.mark.gpu
 
 F32 = np.float32
 TYPES = ("f32", "f16", "bf16")
 GATES = (None, "same_source", "any_source")
+# thresholds per metric that take the near tracks in and leave the unrelated ones out
+OPTS = {"euclidean": dict(max_observations=4, feature_dim=24, topn=3, distance_filter=8.0, max_distance=5.0),
+        "cosine": dict(max_observations=4, feature_dim=24, topn=3, distance_filter=1.2, max_distance=0.5)}
 
 
 @pytest.fixture(scope="module")
@@ -27,50 +31,6 @@ def eng():
     if lib().sb200_device_count() <= 0:
         pytest.fail("no CUDA device: the gpu-marked tests must run on an H100")
     return e
-
-
-def _opts(metric, **kw):
-    euc = metric == "euclidean"
-    o = dict(distance_filter=8.0 if euc else 1.2, max_observations=4, feature_dim=24, topn=3,
-             max_distance=5.0 if euc else 0.5, min_votes=1)
-    o.update(kw)
-    return o
-
-
-def _pair(eng, metric="euclidean", storage="f32", gate=None, retention="newest", **kw):
-    o = _opts(metric, **kw)
-    g = eng.FeatureStore(metric=metric, storage=storage, gate=gate, retention=retention, voting="best_fit", **o)
-    r = fo.FeatureStore(metric=fo.EUCLIDEAN if metric == "euclidean" else fo.COSINE, gate=gate, retention=retention,
-                        voting="best_fit", **{k: v for k, v in o.items()})
-    return g, r
-
-
-def _same(a, b):
-    assert a.keys() == b.keys()
-    for k in a:
-        x, y = np.asarray(a[k]), np.asarray(b[k])
-        if x.dtype == np.float64:
-            x, y = x.view(np.uint64), y.view(np.uint64)
-        assert np.array_equal(x, y), (k, x, y)
-
-
-def _same_state(g, r, quality, gate, classes=(None,)):
-    ids = r.ids()
-    assert np.array_equal(g.ids(), ids)
-    for c in classes:
-        if quality:
-            gc, gf, gq = g.fetch_quality(ids, feature_class=c)
-            rc, rf, rq = r.fetch_quality(ids, feature_class=c)
-            assert np.array_equal(gq.view(np.uint32), rq.view(np.uint32))
-        else:
-            (gc, gf), (rc, rf) = g.fetch(ids, feature_class=c), r.fetch(ids, feature_class=c)
-        assert np.array_equal(gc, rc)
-        assert np.array_equal(gf.view(np.uint32), rf.view(np.uint32))
-    if quality:
-        assert all(np.array_equal(a, b) for a, b in zip(g.merge_history(ids), r.merge_history(ids)))
-    if gate:
-        for a, b in zip(g.attributes(ids), r.attributes(ids)):
-            assert np.array_equal(a, b)
 
 
 def _distinct_merges(out):
@@ -131,37 +91,37 @@ class World:
 def test_every_call_matches_the_oracle(eng, storage, metric, gate, retention):
     seed = TYPES.index(storage) * 100 + GATES.index(gate) * 10 + (metric == "cosine") * 2 + (retention == "quality")
     w = World(seed, 24, storage, gate, retention)
-    g, r = _pair(eng, metric, storage, gate, retention, min_votes=1 + seed % 2)
+    g, r = store_pair(metric, storage, gate, retention, "best_fit", min_votes=1 + seed % 2, **OPTS[metric])
     w.fill([g, r], 1, 40, 0)
     merged = new_with_results = 0
     for k in range(3):
         ids, offs, rows, kw = w.queries(1000 + 100 * k, 60, 10_000 * (k + 1))
-        _same(g.search(ids, offs, rows, **kw), r.search(ids, offs, rows, **kw))
+        same_results(g.search(ids, offs, rows, **kw), r.search(ids, offs, rows, **kw))
         a = g.associate(ids, offs, rows, **kw)
-        _same(a, r.associate(ids, offs, rows, **kw))
+        same_results(a, r.associate(ids, offs, rows, **kw))
         _distinct_merges(a)
         merged += int(a["merged"].sum())
         new_with_results += int(((a["counts"] > 0) & (a["merged"] == 0)).sum())
-        _same_state(g, r, w.quality, gate)
+        same_store(g, r)
     assert merged > 0 and new_with_results > 0
     owned = g.ids()[::3]
-    _same(g.search_owned(owned), r.search_owned(owned))
+    same_results(g.search_owned(owned), r.search_owned(owned))
     each = g.search_owned(owned, each=True)
-    _same(each, r.search_owned(owned, each=True))
+    same_results(each, r.search_owned(owned, each=True))
     g.set_voting("topn")
-    _same(each, g.search_owned(owned, each=True))
+    same_results(each, g.search_owned(owned, each=True))
     g.set_voting("best_fit")
     # associate_store from a source store of the same configuration, with dst's BestFit rule
-    gs, rs = _pair(eng, metric, storage, gate, retention, min_votes=1 + seed % 2)
+    gs, rs = store_pair(metric, storage, gate, retention, "best_fit", min_votes=1 + seed % 2, **OPTS[metric])
     gs.set_voting("topn")
     rs.set_voting("topn")
     w.fill([gs, rs], 5000, 30, 100_000)
     moved = gs.ids()[::2]
     a = g.associate_store(gs, moved, remove=True)
-    _same(a, r.associate_store(rs, moved, remove=True))
+    same_results(a, r.associate_store(rs, moved, remove=True))
     _distinct_merges(a)
-    _same_state(g, r, w.quality, gate)
-    _same_state(gs, rs, w.quality, gate)
+    same_store(g, r)
+    same_store(gs, rs)
     blob = g.save()
     g.set_voting("topn")
     assert np.array_equal(g.save(), blob)
@@ -175,7 +135,7 @@ def test_column_types_and_device_columns(eng, ftype):
     import torch
 
     w = World(31, 40, "f16", None, "newest")
-    g, r = _pair(eng, "euclidean", "bf16", feature_dim=40)
+    g, r = store_pair("euclidean", "bf16", voting="best_fit", **OPTS["euclidean"] | dict(feature_dim=40))
     w.centres = fo.round_rows(fo.round_rows(w.centres, "f16"), "bf16")
     w.storage = "bf16"
     w.fill([g, r], 1, 50, 0)
@@ -192,17 +152,16 @@ def test_column_types_and_device_columns(eng, ftype):
             col = rows.astype(np.float16) if ftype == "f16" else (rows.view(np.uint32) >> 16).astype(np.uint16)
             a = g.associate(ids, offs, col)
             g.set_feature_type("f32")
-        _same(a, r.associate(ids, offs, rows))
+        same_results(a, r.associate(ids, offs, rows))
         _distinct_merges(a)
-    _same_state(g, r, False, None)
+    same_store(g, r)
 
 
 @pytest.mark.parametrize("retention", ["newest", "quality"])
 def test_two_classes(eng, retention):
     classes = {7: 16, 2: 24}
-    o = _opts("euclidean", feature_dim=16)
-    g = eng.FeatureStore(classes=classes, retention=retention, voting="best_fit", **o)
-    r = fo.FeatureStore(classes=classes, retention=retention, voting="best_fit", **o)
+    g, r = store_pair(retention=retention, voting="best_fit", classes=classes,
+                      **OPTS["euclidean"] | dict(feature_dim=16))
     rng = np.random.default_rng(5)
     q = retention == "quality"
     cen = {c: rng.standard_normal((6, d)).astype(F32) * 2 for c, d in classes.items()}
@@ -220,10 +179,9 @@ def test_two_classes(eng, retention):
         rows = cen[c][np.repeat(rng.integers(0, 2, n), 2)] + 0.4 * rng.standard_normal((2 * n, d)).astype(F32)
         kw = dict(quality=rng.integers(0, 4, 2 * n).astype(F32)) if q else {}
         a = g.associate(ids, offs, rows, feature_class=c, **kw)
-        _same(a, r.associate(ids, offs, rows, feature_class=c, **kw))
+        same_results(a, r.associate(ids, offs, rows, feature_class=c, **kw))
         _distinct_merges(a)
-    _same_state(g, r, q, None, classes=tuple(classes))
-    assert np.array_equal(g.class_counts(r.ids()), r.class_counts(r.ids()))
+    same_store(g, r)
 
 
 @pytest.mark.parametrize("metric", ["euclidean", "cosine"])
@@ -231,8 +189,7 @@ def test_thousands_of_queries_on_a_handful_of_tracks(eng, metric):
     """4,000 queries of one or two rows on 6 tracks; many queries repeat the same rows, so their groups tie exactly
     and the lower query index must win."""
     rng = np.random.default_rng(9)
-    g, r = _pair(eng, metric, "f32", None, "newest", max_observations=2, feature_dim=32, topn=4,
-                 distance_filter=1e9, max_distance=1e9)
+    g, r = store_pair(metric, voting="best_fit", max_observations=2, feature_dim=32, topn=4)
     base = rng.standard_normal((6, 32)).astype(F32)
     ids = np.repeat(np.arange(1, 7, dtype=np.uint64), 2)
     rows = base[ids - 1] + 0.2 * rng.standard_normal((12, 32)).astype(F32)
@@ -245,23 +202,23 @@ def test_thousands_of_queries_on_a_handful_of_tracks(eng, metric):
     q = pool[rng.integers(0, 40, int(offs[-1]))]
     qid = np.arange(10_000, 10_000 + n, dtype=np.uint64)
     a = g.associate(qid, offs, q)
-    _same(a, r.associate(qid, offs, q))
+    same_results(a, r.associate(qid, offs, q))
     assert 0 < a["merged"].sum() <= 6
     _distinct_merges(a)
     ws = a["weights"][:, 0][a["counts"] > 0]
     assert len(np.unique(ws)) < len(ws)   # exact ties took part
-    _same_state(g, r, False, None)
+    same_store(g, r)
     s = g.search(qid[:3000], offs[:3001], q[: offs[3000]])
-    _same(s, r.search(qid[:3000], offs[:3001], q[: offs[3000]]))
-    _same(g.search_owned(g.ids()[:5]), r.search_owned(r.ids()[:5]))
+    same_results(s, r.search(qid[:3000], offs[:3001], q[: offs[3000]]))
+    same_results(g.search_owned(g.ids()[:5]), r.search_owned(r.ids()[:5]))
 
 
 def test_switching_the_rule_between_calls(eng):
     """One store switches rules between calls, the oracle with it; a TopN call after switching back leaves it byte for
     byte as an untouched TopN twin that made the same calls under TopN."""
     w = World(77, 24, "f32", None, "newest")
-    g, r = _pair(eng)
-    twin = eng.FeatureStore(metric="euclidean", **_opts("euclidean"))
+    g, r = store_pair(voting="best_fit", **OPTS["euclidean"])
+    twin = gpu_store(**OPTS["euclidean"])
     w.fill([g, r, twin], 1, 40, 0)
     rules = ["best_fit", "topn", "best_fit", "best_fit", "topn"]
     for k, rule in enumerate(rules):
@@ -269,18 +226,18 @@ def test_switching_the_rule_between_calls(eng):
         r.set_voting(rule)
         ids, offs, rows, _ = w.queries(1000 + 100 * k, 50, 0)
         if rule == "best_fit":
-            _same(g.search(ids, offs, rows), r.search(ids, offs, rows))
-            _same(g.search_owned(g.ids()[:9]), r.search_owned(r.ids()[:9]))
+            same_results(g.search(ids, offs, rows), r.search(ids, offs, rows))
+            same_results(g.search_owned(g.ids()[:9]), r.search_owned(r.ids()[:9]))
             continue   # searches change nothing, so the twin stays in step
         a = g.associate(ids, offs, rows)
-        _same(a, r.associate(ids, offs, rows))
-        _same(a, twin.associate(ids, offs, rows))
+        same_results(a, r.associate(ids, offs, rows))
+        same_results(a, twin.associate(ids, offs, rows))
         assert np.array_equal(g.save(), twin.save())
     g.set_voting("best_fit")
     r.set_voting("best_fit")
     ids, offs, rows, _ = w.queries(9000, 50, 0)
-    _same(g.associate(ids, offs, rows), r.associate(ids, offs, rows))
-    _same_state(g, r, False, None)
+    same_results(g.associate(ids, offs, rows), r.associate(ids, offs, rows))
+    same_store(g, r)
     from similari_b200._lib import lib
 
     before = g.voting()

@@ -8,28 +8,12 @@ blobs included; and every refusal against an unchanged store."""
 import numpy as np
 import pytest
 
+from fstore_checks import gpu_store, same_results, same_store, store_pair
+
 pytestmark = pytest.mark.gpu
 
 METRICS = ("euclidean", "cosine")
 TYPES = ("f32", "f16", "bf16")
-
-
-def _store(classes=None, **kw):
-    import similari_b200.engine as eng
-
-    o = dict(distance_filter=1e9, max_observations=3, feature_dim=16, topn=4, max_distance=1e9, min_votes=1)
-    o.update(kw)
-    return eng.FeatureStore(classes=classes, **o)
-
-
-def _bits(a):
-    return a.view(np.uint64) if a.dtype == np.float64 else a
-
-
-def _same(ra, rb):
-    assert ra.keys() == rb.keys()
-    for k in ra:
-        assert np.array_equal(_bits(ra[k]), _bits(rb[k])), (k, ra[k], rb[k])
 
 
 def _rows(s, ids, c, quality=False):
@@ -67,8 +51,8 @@ def _fill(s, singles, rng, n, classes, K, storage_round=None):
 def test_class_search_is_a_single_class_search(metric, storage):
     rng = np.random.default_rng(7)
     classes = {3: 16, 1: 24}
-    s = _store(classes, metric=metric, storage=storage)
-    singles = {c: _store(None, metric=metric, storage=storage, feature_dim=d) for c, d in classes.items()}
+    s = gpu_store(metric, storage, classes=classes)
+    singles = {c: gpu_store(metric=metric, storage=storage, feature_dim=d) for c, d in classes.items()}
     _fill(s, singles, rng, 40, classes, 3)
     assert s.classes() == classes
     ids = np.arange(1, 41, dtype=np.uint64)
@@ -83,10 +67,10 @@ def test_class_search_is_a_single_class_search(metric, storage):
     for c, d in classes.items():
         q = rng.standard_normal((9, d)).astype(np.float32)
         qid, off = np.arange(500, 504, dtype=np.uint64), np.array([0, 2, 5, 6, 9], np.int32)
-        _same(s.search(qid, off, q, feature_class=c), singles[c].search(qid, off, q))
-        _same(s.search_owned(ids[:6], feature_class=c), singles[c].search_owned(ids[:6]))
-        _same(s.search_owned(ids[:6], each=True, feature_class=c), singles[c].search_owned(ids[:6], each=True))
-        _same(s.associate(qid, off, q, feature_class=c), singles[c].associate(qid, off, q))
+        same_results(s.search(qid, off, q, feature_class=c), singles[c].search(qid, off, q))
+        same_results(s.search_owned(ids[:6], feature_class=c), singles[c].search_owned(ids[:6]))
+        same_results(s.search_owned(ids[:6], each=True, feature_class=c), singles[c].search_owned(ids[:6], each=True))
+        same_results(s.associate(qid, off, q, feature_class=c), singles[c].associate(qid, off, q))
         n = len(singles[c].ids())
         got = _rows(s, singles[c].ids(), c)
         want = _rows(singles[c], singles[c].ids(), None)
@@ -96,7 +80,7 @@ def test_class_search_is_a_single_class_search(metric, storage):
 
 
 def test_new_track_holds_the_queried_class_alone():
-    s = _store({0: 8, 9: 16})
+    s = gpu_store(classes={0: 8, 9: 16})
     s.add([1], np.ones((1, 16), np.float32), feature_class=9)
     out = s.associate([2], [0, 1], np.full((1, 8), 5, np.float32), feature_class=0)
     assert out["merged"][0] == 0
@@ -120,7 +104,7 @@ def test_merge_owned_moves_every_class(gate, storage):
     rng = np.random.default_rng(11)
     classes = {4: 8, 2: 16}
     K = 3
-    s = _store(classes, storage=storage, gate=gate, max_observations=K)
+    s = gpu_store(classes=classes, storage=storage, gate=gate, max_observations=K)
     kw = {}
     ids = np.arange(1, 13, dtype=np.uint64)
     for c, d in classes.items():
@@ -158,7 +142,8 @@ def test_quality_merge_owned_steps_each_class():
     """init 1, extension 2: c(h) = min(K, 2^h), exact.  A source holding two classes appends its history twice; the
     lower class id is truncated at c(h + 1), the higher at c(h + 2)."""
     K = 8
-    s = _store({7: 8, 2: 8}, max_observations=K, retention="quality", initial_capacity=1, merge_extension=2.0)
+    s = gpu_store(classes={7: 8, 2: 8}, max_observations=K, retention="quality", initial_capacity=1,
+                  merge_extension=2.0)
     rng = np.random.default_rng(3)
     f = rng.standard_normal((20, 8)).astype(np.float32)
     q = rng.permutation(20).astype(np.float32)
@@ -185,8 +170,8 @@ def test_associate_store_brings_every_class(gate):
     classes = {0: 8, 1: 16}
     K = 4
     kw = dict(max_observations=K, gate=gate)
-    dst, src = _store(classes, **kw), _store(classes, **kw)
-    single_d, single_s = _store(None, feature_dim=8, **kw), _store(None, feature_dim=8, **kw)
+    dst, src = gpu_store(classes=classes, **kw), gpu_store(classes=classes, **kw)
+    single_d, single_s = gpu_store(feature_dim=8, **kw), gpu_store(feature_dim=8, **kw)
 
     def add(stores, ids, c, t):
         f = rng.standard_normal((len(ids), classes[c])).astype(np.float32)
@@ -203,8 +188,7 @@ def test_associate_store_brings_every_class(gate):
     bs = {c: _rows(src, q, c) for c in classes}
     out = dst.associate_store(src, q, remove=True, feature_class=0)
     ref = single_d.associate_store(single_s, q[:3], remove=True)
-    for k in ref:
-        assert np.array_equal(_bits(out[k][:3]), _bits(ref[k])), k
+    same_results({k: v[:3] for k, v in out.items()}, ref)
     assert out["counts"][3] == 0 and out["merged"][3] == 0 and out["track_ids"][3] == 16
     assert src.ids().tolist() == [13, 14]
     cur = {c: {d: r[0] for d, r in bd[c].items()} for c in classes}
@@ -221,13 +205,13 @@ def test_associate_store_brings_every_class(gate):
 
 def test_default_class_declared_is_the_default():
     rng = np.random.default_rng(1)
-    a, b = _store(None, retention="quality"), _store({0: 16}, retention="quality")
+    a, b = gpu_store(retention="quality"), gpu_store(classes={0: 16}, retention="quality")
     ids = np.repeat(np.arange(1, 9, dtype=np.uint64), 3)
     f, q = rng.standard_normal((len(ids), 16)).astype(np.float32), rng.random(len(ids)).astype(np.float32)
     for s in (a, b):
         s.add(ids, f, quality=q)
     qq = rng.standard_normal((4, 16)).astype(np.float32)
-    _same(a.associate([20, 21], [0, 2, 4], qq, quality=np.ones(4, np.float32)),
+    same_results(a.associate([20, 21], [0, 2, 4], qq, quality=np.ones(4, np.float32)),
           b.associate([20, 21], [0, 2, 4], qq, quality=np.ones(4, np.float32)))
     a.merge_owned([1], [2])
     b.merge_owned([1], [2])
@@ -245,8 +229,8 @@ def test_large_gallery_class_search():
     rng = np.random.default_rng(9)
     K, n = 12, 20000
     classes = {0: 128, 1: 512}
-    s = _store(classes, max_observations=K, topn=5, storage="f16")
-    singles = {c: _store(None, max_observations=K, topn=5, feature_dim=d, storage="f16") for c, d in classes.items()}
+    s = gpu_store(classes=classes, max_observations=K, topn=5, storage="f16")
+    singles = {c: gpu_store(max_observations=K, topn=5, feature_dim=d, storage="f16") for c, d in classes.items()}
     ids = np.repeat(np.arange(1, n + 1, dtype=np.uint64), 2)
     for c, d in classes.items():
         f = rng.standard_normal((len(ids), d)).astype(np.float16)
@@ -255,7 +239,7 @@ def test_large_gallery_class_search():
     for c, d in classes.items():
         q = rng.standard_normal((64, d)).astype(np.float16)
         off = np.arange(0, 65, 2, dtype=np.int32)
-        _same(s.search(np.arange(10**6, 10**6 + 32, dtype=np.uint64), off, q, feature_class=c),
+        same_results(s.search(np.arange(10**6, 10**6 + 32, dtype=np.uint64), off, q, feature_class=c),
               singles[c].search(np.arange(10**6, 10**6 + 32, dtype=np.uint64), off, q))
 
 
@@ -264,16 +248,10 @@ def _state(s):
     return ids, s.class_counts(ids), {c: s.fetch(ids, feature_class=c) for c in s.classes()}
 
 
-def _same_state(a, b):
-    assert np.array_equal(a[0], b[0]) and np.array_equal(a[1], b[1])
-    for c in a[2]:
-        assert np.array_equal(a[2][c][0], b[2][c][0]) and np.array_equal(a[2][c][1], b[2][c][1])
-
-
 def test_refusals_leave_the_store_unchanged():
     from similari_b200._lib import Sb200Error
 
-    s = _store({0: 8, 1: 16})
+    s = gpu_store(classes={0: 8, 1: 16})
     s.add([1, 2], np.ones((2, 8), np.float32), feature_class=0)
     s.add([2], np.ones((1, 16), np.float32), feature_class=1)
     before = _state(s)
@@ -284,53 +262,23 @@ def test_refusals_leave_the_store_unchanged():
 
     for n, i, d in ((1, [5], [8]), (0, [0], [8])):
         assert L.sb200_fstore_set_classes(h, n, ptr(np.array(i, np.uint64)), ptr(np.array(d, np.int32))) != 0
-    e = _store()
+    e = gpu_store()
     for n, i, d in ((0, ids16, dims16), (17, ids16, dims16), (2, np.array([3, 3], np.uint64), dims16),
                     (1, ids16, np.array([0], np.int32)), (1, ids16, np.array([8193], np.int32))):
         assert L.sb200_fstore_set_classes(e._h, n, ptr(i), ptr(d)) != 0
     e._read_classes()
-    assert e.classes() == {0: 16} and e.save().tobytes() == _store().save().tobytes()
+    assert e.classes() == {0: 16} and e.save().tobytes() == gpu_store().save().tobytes()
     assert L.sb200_fstore_use_class(h, 5) != 0
     with pytest.raises(ValueError):
         s.search([9], [0, 1], np.ones((1, 8), np.float32), feature_class=5)
-    other = _store({0: 8, 1: 24})
+    other = gpu_store(classes={0: 8, 1: 24})
     other.add([7], np.ones((1, 8), np.float32))
     with pytest.raises(Sb200Error):
         s.associate_store(other, [7])
-    _same_state(before, _state(s))
+    same_results(_state(s), before)
 
 
 # ---- against the CPU oracle (fstore_oracle), bit for bit
-def _pair(classes, storage="f32", metric="euclidean", **kw):
-    import fstore_oracle as fo
-
-    o = dict(distance_filter=1e9, max_observations=4, feature_dim=16, topn=3, max_distance=1e9, min_votes=1)
-    o.update(kw)
-    g = _store(classes, storage=storage, metric=metric, **o)
-    m = fo.FeatureStore(metric={"euclidean": fo.EUCLIDEAN, "cosine": fo.COSINE}[metric], classes=classes, **o)
-    return g, m
-
-
-def _same_state_oracle(g, m, quality):
-    ids = m.ids()
-    assert np.array_equal(g.ids(), ids)
-    assert np.array_equal(g.class_counts(np.append(ids, 12345)), m.class_counts(np.append(ids, 12345)))
-    for c in m.classes():
-        if quality:
-            a, b = g.fetch_quality(ids, feature_class=c), m.fetch_quality(ids, feature_class=c)
-        else:
-            a, b = g.fetch(ids, feature_class=c), m.fetch(ids, feature_class=c)
-        for x, y in zip(a, b):
-            assert np.array_equal(x.view(np.uint32) if x.dtype == np.float32 else x,
-                                  y.view(np.uint32) if y.dtype == np.float32 else y), c
-    if quality:
-        for x, y in zip(g.merge_history(ids), m.merge_history(ids)):
-            assert np.array_equal(x, y)
-    if g.gate:
-        for x, y in zip(g.attributes(ids), m.attributes(ids)):
-            assert np.array_equal(x, y)
-
-
 @pytest.mark.parametrize("device_cols", [False, True])
 @pytest.mark.parametrize("gate,retention", [(None, "newest"), ("same_source", "newest"), (None, "quality"),
                                             ("any_source", "quality")])
@@ -344,8 +292,8 @@ def test_mixed_sequence_matches_the_oracle(storage, metric, gate, retention, dev
 
     classes = {6: 16, 2: 24}
     qual = retention == "quality"
-    kw = dict(gate=gate, retention=retention, initial_capacity=2, merge_extension=1.5)
-    g, m = _pair(classes, storage, metric, **kw)
+    kw = dict(gate=gate, retention=retention, initial_capacity=2, merge_extension=1.5, max_observations=4, topn=3)
+    g, m = store_pair(metric, storage, classes=classes, **kw)
     rng = np.random.default_rng(21)
 
     def rows(n, d):
@@ -364,7 +312,7 @@ def test_mixed_sequence_matches_the_oracle(storage, metric, gate, retention, dev
         ra = getattr(g, call)(*args, **k)
         rb = getattr(m, call)(*args, **k)
         if ra is not None:
-            _same(ra, rb)
+            same_results(ra, rb)
         return ra
 
     for c, d in classes.items():
@@ -385,7 +333,7 @@ def test_mixed_sequence_matches_the_oracle(storage, metric, gate, retention, dev
 
         t = torch.from_numpy(f).cuda()
         torch.cuda.synchronize()
-        _same(g.associate_device(qid, off, t.data_ptr(), feature_class=2, **a),
+        same_results(g.associate_device(qid, off, t.data_ptr(), feature_class=2, **a),
               m.associate(qid, off, f, feature_class=2, **a))
     else:
         both("associate", qid, off, f, feature_class=2, **a)
@@ -393,13 +341,13 @@ def test_mixed_sequence_matches_the_oracle(storage, metric, gate, retention, dev
     if qual:
         a["quality"] = rng.permutation(len(f)).astype(np.float32)
     both("search", qid, off, f, feature_class=6, **a)
-    _same_state_oracle(g, m, qual)
+    same_store(g, m)
 
     blob = g.save()
     g = eng.FeatureStore.load(blob)
     assert g.classes() == classes
     assert np.array_equal(g.save(), blob)
-    _same_state_oracle(g, m, qual)
+    same_store(g, m)
 
     pairs_d, pairs_s = [], []   # pairs the gate allows, given the windows the associate left
     src_, t0, t1 = (dict(zip(m.ids().tolist(), v.tolist())) for v in m.attributes(m.ids())) if gate else ({}, {}, {})
@@ -415,9 +363,9 @@ def test_mixed_sequence_matches_the_oracle(storage, metric, gate, retention, dev
     both("merge_owned", pairs_d, pairs_s, remove=True)
     both("search_owned", m.ids()[:5], feature_class=6)
     both("search_owned", m.ids()[:5], each=True, feature_class=2)
-    _same_state_oracle(g, m, qual)
+    same_store(g, m)
 
-    gs, ms = _pair(classes, storage, metric, **kw)
+    gs, ms = store_pair(metric, storage, classes=classes, **kw)
     for c, d in classes.items():
         tr = np.array([t for t in range(300, 310) if (t + c) % 3 != 0], np.uint64)
         ids = np.repeat(tr, 2)
@@ -426,9 +374,9 @@ def test_mixed_sequence_matches_the_oracle(storage, metric, gate, retention, dev
         gs.add(ids, f, feature_class=c, **e)
         ms.add(ids, f, feature_class=c, **e)
     q = np.arange(300, 310, dtype=np.uint64)
-    _same(g.associate_store(gs, q, feature_class=6), m.associate_store(ms, q, feature_class=6))
-    _same_state_oracle(g, m, qual)
-    _same_state_oracle(gs, ms, qual)
+    same_results(g.associate_store(gs, q, feature_class=6), m.associate_store(ms, q, feature_class=6))
+    same_store(g, m)
+    same_store(gs, ms)
     blob = g.save()
     assert np.array_equal(eng.FeatureStore.load(blob).save(), blob)
 
@@ -438,8 +386,8 @@ def test_quality_associate_store_steps_each_class():
     c(4) = 10 -> K = 8): the first brings classes 2 and 9 (steps at h = 2, 3), the second class 9 alone (h = 4)."""
     classes = {9: 8, 2: 8}
     kw = dict(retention="quality", initial_capacity=2, merge_extension=1.5, max_observations=8, topn=1)
-    g, m = _pair(classes, **kw)
-    gs, ms = _pair(classes, **kw)
+    g, m = store_pair(classes=classes, **kw)
+    gs, ms = store_pair(classes=classes, **kw)
     f = np.zeros((3, 8), np.float32)
     for s in (g, m):
         s.add([1, 1, 1], f, quality=[3, 2, 1], feature_class=2)
@@ -448,8 +396,8 @@ def test_quality_associate_store_steps_each_class():
         s.add([5, 5, 5], f, quality=[9, 8, 7], feature_class=2)
         s.add([5, 5, 5], f, quality=[90, 80, 70], feature_class=9)
         s.add([6, 6, 6], f, quality=[60, 50, 40], feature_class=9)
-    _same(g.associate_store(gs, [5, 6], feature_class=9), m.associate_store(ms, [5, 6], feature_class=9))
-    _same_state_oracle(g, m, True)
+    same_results(g.associate_store(gs, [5, 6], feature_class=9), m.associate_store(ms, [5, 6], feature_class=9))
+    same_store(g, m)
     assert [h.tolist() for h in g.merge_history([1])] == [[1, 5, 5, 6]]
     assert g.class_counts([1]).tolist() == [[8, 4]]
 
@@ -458,7 +406,7 @@ def test_version_4_blob_refusals():
     import similari_b200.engine as eng
     from similari_b200._lib import Sb200Error
 
-    g = _store({0: 8, 3: 16})
+    g = gpu_store(classes={0: 8, 3: 16})
     g.add([1, 2], np.ones((2, 8), np.float32))
     g.add([2], np.ones((1, 16), np.float32), feature_class=3)
     blob = g.save()

@@ -7,24 +7,13 @@ import numpy as np
 import pytest
 
 import fstore_oracle as fo
+from fstore_checks import gpu_store, same_results, same_store, store_options, store_pair
 
 pytestmark = pytest.mark.gpu
 
 K, DIM = 3, 20   # d8 = 24: every stored row has a zero tail
-OPTS = dict(distance_filter=1e9, max_observations=K, feature_dim=DIM, topn=3, max_distance=1e9, min_votes=1)
+OPTS = dict(max_observations=K, feature_dim=DIM, topn=3)
 NEXT_TYPE = {"f32": "f16", "f16": "bf16", "bf16": "f32"}
-
-
-def _same_store(g, o):
-    ids = o.ids()
-    assert np.array_equal(g.ids(), ids)
-    cg, fg = g.fetch(ids)
-    co, fo_ = o.fetch(ids)
-    assert np.array_equal(cg, co)
-    assert np.array_equal(fg.view(np.uint32), fo_.view(np.uint32))
-    if o.gate is not None:
-        for x, y in zip(g.attributes(ids), o.attributes(ids)):
-            assert np.array_equal(x, y)
 
 
 def _rows(rng, track_ids, storage, gated):
@@ -44,13 +33,6 @@ def _add(stores, call):
         s.add(ids, f, **at)
 
 
-def _remove(g, o, ids):
-    cg, fg = g.fetch(ids, remove=True)
-    co, fo_ = o.fetch(ids, remove=True)
-    assert np.array_equal(cg, co)
-    assert np.array_equal(fg.view(np.uint32), fo_.view(np.uint32))
-
-
 @pytest.mark.parametrize("start_gated", [False, True])
 @pytest.mark.parametrize("storage", ["f32", "f16", "bf16"])
 def test_columns_survive_growth_compaction_and_a_gate_switch(storage, start_gated):
@@ -59,23 +41,23 @@ def test_columns_survive_growth_compaction_and_a_gate_switch(storage, start_gate
 
     rng = np.random.default_rng(zlib.crc32(f"columns {storage} {start_gated}".encode()))
     gate = "same_source" if start_gated else None
-    g = eng.FeatureStore(storage=storage, gate=gate, **OPTS)
-    o = fo.FeatureStore(gate=gate, **OPTS)
+    g, o = store_pair(storage=storage, gate=gate, **OPTS)
     # growth: eight adds of ten new tracks each (and rows for tracks already stored), through several reserves
     for step in range(8):
         new = np.arange(10 * step + 1, 10 * step + 11, dtype=np.uint64)
         old = rng.choice(np.arange(1, 10 * step + 1, dtype=np.uint64), min(5, 10 * step), replace=False)
         _add((g, o), _rows(rng, np.concatenate([new, old]), storage, start_gated))
-        _same_store(g, o)
+        same_store(g, o)
     # compaction: a scattered third of the tracks leaves, then the store grows again
-    _remove(g, o, o.ids()[rng.permutation(o.size())[: o.size() // 3]])
-    _same_store(g, o)
+    gone = o.ids()[rng.permutation(o.size())[: o.size() // 3]]
+    same_results(g.fetch(gone, remove=True), o.fetch(gone, remove=True))
+    same_store(g, o)
     for step in range(8, 12):
         _add((g, o), _rows(rng, np.arange(10 * step + 1, 10 * step + 11, dtype=np.uint64), storage, start_gated))
-        _same_store(g, o)
+        same_store(g, o)
     most = o.size()
     # emptied, the store keeps its capacity; the gate and the storage type change there
-    _remove(g, o, o.ids())
+    same_results(g.fetch(o.ids(), remove=True), o.fetch(o.ids(), remove=True))
     assert g.size() == 0
     gate = None if start_gated else "same_source"
     storage = NEXT_TYPE[storage]
@@ -83,15 +65,15 @@ def test_columns_survive_growth_compaction_and_a_gate_switch(storage, start_gate
     check(g._L.sb200_fstore_set_storage_type(g._h, eng.FEATURE_TYPES[storage]))
     g.gate = gate
     assert g.storage_type() == storage
-    o = fo.FeatureStore(gate=gate, **OPTS)
-    _same_store(g, o)
+    o = fo.FeatureStore(gate=gate, **store_options(**OPTS))
+    same_store(g, o)
     # refill past the old capacity (below 1.5x the most tracks ever stored)
-    twin = eng.FeatureStore(storage=storage, gate=gate, **OPTS)
+    twin = gpu_store(storage=storage, gate=gate, **OPTS)
     first = 1000
     while o.size() < 2 * most:
         call = _rows(rng, np.arange(first, first + 25, dtype=np.uint64), storage, gate is not None)
         _add((g, o, twin), call)
-        _same_store(g, o)
+        same_store(g, o)
         first += 25
     blob = g.save()
     assert np.array_equal(blob, twin.save())
@@ -105,9 +87,7 @@ def test_columns_survive_growth_compaction_and_a_gate_switch(storage, start_gate
     if gate is not None:
         t0 = rng.integers(2000, 3000, len(ids)).astype(np.int64)
         at = dict(sources=(1 + ids % 3).astype(np.uint64), t_start=t0, t_end=t0 + 5)
-    ra, rb = g.associate(ids, offs, f, **at), loaded.associate(ids, offs, f, **at)
-    for k in ra:
-        assert np.array_equal(ra[k].view(np.uint8), rb[k].view(np.uint8)), k
+    same_results(g.associate(ids, offs, f, **at), loaded.associate(ids, offs, f, **at))
     gone = g.ids()[::4]
     for s in (g, loaded):
         s.fetch(gone, remove=True)

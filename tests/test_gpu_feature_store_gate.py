@@ -2,52 +2,15 @@
 owned calls and the attribute columns bit for bit against the CPU oracle, every refusal leaving the store's blob as it
 was, and the version-2 blob: round trip, byte-equal twins, load refusals; an ungated store's blob stays version 1."""
 import ctypes as C
-import os
 import zlib
 
 import numpy as np
 import pytest
 
 import fstore_oracle as fo
+from fstore_checks import gpu_store, refused_blob, same_results, same_store, store_pair
 
 pytestmark = pytest.mark.gpu
-
-METRICS = {"euclidean": fo.EUCLIDEAN, "cosine": fo.COSINE}
-THREADS = max(1, min(16, os.cpu_count() or 1))
-
-
-def _opts(**kw):
-    o = dict(distance_filter=1e9, max_observations=3, feature_dim=16, topn=5, max_distance=1e9, min_votes=1)
-    o.update(kw)
-    return o
-
-
-def _pair(metric="euclidean", gate="same_source", storage="f32", **kw):
-    import similari_b200.engine as eng
-
-    return (eng.FeatureStore(metric=metric, storage=storage, gate=gate, **_opts(**kw)),
-            fo.FeatureStore(metric=METRICS[metric], gate=gate, threads=THREADS, **_opts(**kw)))
-
-
-def _same(a, b, what=""):
-    for k in b:
-        x, y = a[k], b[k]
-        assert x.dtype == y.dtype and x.shape == y.shape, (what, k)
-        if x.dtype == np.float64:
-            assert np.array_equal(x.view(np.uint64), y.view(np.uint64)), (what, k, x, y)
-        else:
-            assert np.array_equal(x, y), (what, k, x, y)
-
-
-def _same_store(g, o):
-    ids = o.ids()
-    assert np.array_equal(g.ids(), ids)
-    cg, fg = g.fetch(ids)
-    co, fo_ = o.fetch(ids)
-    assert np.array_equal(cg, co)
-    assert np.array_equal(fg.view(np.uint32), fo_.view(np.uint32))
-    for x, y in zip(g.attributes(ids), o.attributes(ids)):
-        assert np.array_equal(x, y)
 
 
 def _windows(rng, n, span=400, length=40, sources=2):
@@ -94,7 +57,7 @@ def test_search_and_associate_match_the_oracle(storage, metric, gate):
 
     rng = np.random.default_rng(zlib.crc32(f"{storage} {metric} {gate}".encode()))
     dim, K = 24, 3
-    g, o = _pair(metric, gate, storage, max_observations=K, feature_dim=dim, topn=4, min_votes=1)
+    g, o = store_pair(metric, storage, gate, max_observations=K, feature_dim=dim, topn=4, min_votes=1)
     _fill((g, o), rng, 60, dim, storage, K)
     refused = 0   # queries whose first winner the gate refused in associate
     for it in range(4):
@@ -107,15 +70,15 @@ def test_search_and_associate_match_the_oracle(storage, metric, gate):
             torch.cuda.synchronize()
         else:
             rg = g.search(ids, offs, f, **at)
-        _same(rg, o.search(ids, offs, f, **at), "search")
+        same_results(rg, o.search(ids, offs, f, **at), "search")
         if on_device:
             rg = g.associate_device(ids, offs, d.data_ptr(), **at)
         else:
             rg = g.associate(ids, offs, f, **at)
         ro = o.associate(ids, offs, f, **at)
-        _same(rg, ro, "associate")
+        same_results(rg, ro, "associate")
         refused += int(((ro["counts"] > 0) & (ro["merged"] == 0)).sum())
-        _same_store(g, o)
+        same_store(g, o)
     assert refused > 0
     # the device column path of add
     ids = np.array([1, 2, 5000], np.uint64)
@@ -125,7 +88,7 @@ def test_search_and_associate_match_the_oracle(storage, metric, gate):
     g.add_device(ids, _device(f).data_ptr(), **at)
     torch.cuda.synchronize()
     o.add(ids, f, **at)
-    _same_store(g, o)
+    same_store(g, o)
 
 
 @pytest.mark.parametrize("metric", ["euclidean", "cosine"])
@@ -133,7 +96,7 @@ def test_gallery_scale(metric):
     """20,000 tracks x K = 3 x 512-d with random windows: a search and an associate of 64 queries."""
     rng = np.random.default_rng(11)
     dim, K, n = 512, 3, 20_000
-    g, o = _pair(metric, "same_source", max_observations=K, feature_dim=dim, topn=5, min_votes=1)
+    g, o = store_pair(metric, gate="same_source", max_observations=K, feature_dim=dim, topn=5, min_votes=1)
     ids = np.repeat(np.arange(1, n + 1, dtype=np.uint64), K)
     f = rng.standard_normal((len(ids), dim)).astype(np.float32)
     w = _windows(rng, n, span=100_000, length=2_000, sources=4)
@@ -142,11 +105,10 @@ def test_gallery_scale(metric):
         s.add(ids, f, **at)
     q, offs, qf = _queries(rng, 64, dim, "f32", 10 ** 6)
     qa = _windows(rng, 64, span=100_000, length=2_000, sources=4)
-    _same(g.search(q, offs, qf, **qa), o.search(q, offs, qf, **qa), "search")
-    _same(g.associate(q, offs, qf, **qa), o.associate(q, offs, qf, **qa), "associate")
+    same_results(g.search(q, offs, qf, **qa), o.search(q, offs, qf, **qa), "search")
+    same_results(g.associate(q, offs, qf, **qa), o.associate(q, offs, qf, **qa), "associate")
     sel = np.concatenate([o.ids()[:100], o.ids()[-64:]])
-    for x, y in zip(g.attributes(sel), o.attributes(sel)):
-        assert np.array_equal(x, y)
+    same_results(g.attributes(sel), o.attributes(sel))
 
 
 @pytest.mark.parametrize("metric", ["euclidean", "cosine"])
@@ -154,13 +116,13 @@ def test_gallery_scale(metric):
 def test_owned_calls_match_the_oracle(metric, gate):
     rng = np.random.default_rng(5)
     dim, K = 16, 3
-    g, o = _pair(metric, gate, max_observations=K, feature_dim=dim, topn=5)
+    g, o = store_pair(metric, gate=gate, max_observations=K, feature_dim=dim, topn=5)
     _fill((g, o), rng, 50, dim, "f32", K)
     ids = o.ids()
     q = np.concatenate([ids[rng.permutation(len(ids))[:12]], [777777]]).astype(np.uint64)
     for each in (False, True):
-        _same(g.search_owned(q, each=each), o.search_owned(q, each=each), f"owned each={each}")
-    _same(g.search_owned(ids, each=True), o.search_owned(ids, each=True), "owned whole store")
+        same_results(g.search_owned(q, each=each), o.search_owned(q, each=each), f"owned each={each}")
+    same_results(g.search_owned(ids, each=True), o.search_owned(ids, each=True), "owned whole store")
     # merge_owned: random pairs, applied when the oracle accepts them, refused by both when it does not
     accepted = refused = 0
     for _ in range(30):
@@ -180,12 +142,12 @@ def test_owned_calls_match_the_oracle(metric, gate):
                 g.merge_owned([d], [s], remove=remove)
             assert np.array_equal(g.save(), blob)
             refused += 1
-        _same_store(g, o)
+        same_store(g, o)
     assert accepted and refused
 
 
 def test_fetch_attr_after_merges_and_removals():
-    g, o = _pair(max_observations=2, feature_dim=8)
+    g, o = store_pair(gate="same_source", max_observations=2, feature_dim=8, topn=5)
     rng = np.random.default_rng(2)
     f = rng.standard_normal((6, 8)).astype(np.float32)
     at = dict(sources=np.array([1, 1, 1, 2, 1, 1], np.uint64), t_start=np.array([0, 10, 20, 0, 40, 50], np.int64),
@@ -195,7 +157,7 @@ def test_fetch_attr_after_merges_and_removals():
         s.add(ids, f, **at)
         s.merge_owned([1, 1], [2, 3], remove=True)
         s.fetch([5], remove=True)
-    _same_store(g, o)
+    same_store(g, o)
     src, t0, t1 = g.attributes([1, 2, 3, 4, 5, 6])
     assert src.tolist() == [1, 0, 0, 2, 0, 1]
     assert t0.tolist() == [0, 0, 0, 0, 0, 50] and t1.tolist() == [25, 0, 0, 100, 0, 55]
@@ -212,7 +174,7 @@ def test_refusals_leave_the_store_unchanged():
 
     L = _lib.lib()
     p = _lib.ptr
-    g, _ = _pair(max_observations=2, feature_dim=8)
+    g = gpu_store(gate="same_source", max_observations=2, feature_dim=8, topn=5)
     f = np.ones((3, 8), np.float32)
     g.add([1, 2, 3], f, sources=[1, 1, 2], t_start=[0, 10, 0], t_end=[5, 15, 5])
     blob = g.save()
@@ -257,7 +219,7 @@ def test_refusals_leave_the_store_unchanged():
     assert "window" in L.sb200_last_error().decode()
     assert np.array_equal(g.save(), blob)
     # the _attr calls on an ungated store
-    u = eng.FeatureStore(**_opts(feature_dim=8))
+    u = gpu_store(feature_dim=8, topn=5)
     t0g, t1g = np.array([0], np.int64), np.array([1], np.int64)
     a = _lib.FstoreAttrs(src.ctypes.data, t0g.ctypes.data, t1g.ctypes.data)
     rc, msg = _rc(L, L.sb200_fstore_add_attr, u._h, 1, p(ids), C.byref(a), p(f), None, None)
@@ -275,8 +237,8 @@ def test_gated_blob_round_trips_and_twins_are_byte_equal():
 
     rng = np.random.default_rng(8)
     for storage in ("f32", "bf16"):
-        g1, o = _pair(storage=storage, gate="any_source", max_observations=3, feature_dim=20)
-        g2, _ = _pair(storage=storage, gate="any_source", max_observations=3, feature_dim=20)
+        g1, o = store_pair(storage=storage, gate="any_source", max_observations=3, feature_dim=20, topn=5)
+        g2 = gpu_store(storage=storage, gate="any_source", max_observations=3, feature_dim=20, topn=5)
         _fill((g1, g2, o), rng, 30, 20, storage, 3)
         for src in range(2, 30):   # the first track whose window track 1 can absorb
             try:
@@ -295,18 +257,18 @@ def test_gated_blob_round_trips_and_twins_are_byte_equal():
         c = eng.FeatureStore.load(b1)
         assert c.gate == "any_source"
         assert np.array_equal(c.save(), b1)
-        _same_store(c, o)
+        same_store(c, o)
         q, offs, qf = _queries(rng, 10, 20, storage, 5000)
         at = _windows(rng, 10)
-        _same(c.associate(q, offs, qf, **at), o.associate(q, offs, qf, **at))
-        _same_store(c, o)
+        same_results(c.associate(q, offs, qf, **at), o.associate(q, offs, qf, **at))
+        same_store(c, o)
 
 
 def test_an_ungated_store_still_writes_version_1():
     import similari_b200.engine as eng
     from similari_b200 import _lib
 
-    s = eng.FeatureStore(**_opts(feature_dim=8))
+    s = gpu_store(feature_dim=8, topn=5)
     s.add([1, 2], np.ones((2, 8), np.float32))
     b = s.save()
     h = _lib.FstoreBlobHeader.from_buffer_copy(b[:128].tobytes())
@@ -316,22 +278,11 @@ def test_an_ungated_store_still_writes_version_1():
     assert c.gate is None and np.array_equal(c.save(), b)
 
 
-def _refused(blob, field):
-    from similari_b200 import _lib
-
-    L = _lib.lib()
-    h = C.c_void_p()
-    blob = np.ascontiguousarray(blob)
-    assert L.sb200_fstore_load(_lib.ptr(blob), len(blob), 0, C.byref(h)) == -1
-    assert h.value is None
-    assert field in L.sb200_last_error().decode(), L.sb200_last_error()
-
-
 def test_damaged_version_2_blobs_are_refused():
     import similari_b200.engine as eng
     from similari_b200 import _lib
 
-    g, _ = _pair(feature_dim=8)
+    g = gpu_store(gate="same_source", feature_dim=8, topn=5)
     g.add([1, 2, 3], np.ones((3, 8), np.float32), sources=[1, 1, 1], t_start=[0, 10, 20], t_end=[5, 15, 25])
     blob = g.save()
     hdr = _lib.FstoreBlobHeaderV2.from_buffer_copy(blob[:C.sizeof(_lib.FstoreBlobHeaderV2)].tobytes())
@@ -344,11 +295,11 @@ def test_damaged_version_2_blobs_are_refused():
     def column(b, sec):
         return b[hdr.sec_off[sec]: hdr.sec_off[sec] + hdr.sec_bytes[sec]].view(np.int64)
 
-    _refused(damaged(lambda b, h: setattr(h, "gate", 0)), "gate")
-    _refused(damaged(lambda b, h: setattr(h, "gate", 3)), "gate")
-    _refused(damaged(lambda b, h: column(b, 5).__setitem__(1, 16)), "t_start > t_end")
-    _refused(damaged(lambda b, h: column(b, 6).__setitem__(2, -1)), "t_start > t_end")
-    _refused(damaged(lambda b, h: h.sec_bytes.__setitem__(6, h.sec_bytes[6] - 8)), "t_end holds")
-    _refused(damaged(lambda b, h: h.sec_off.__setitem__(4, h.sec_off[4] + 8)), "source is not 256-byte aligned")
-    _refused(blob[:150], "truncated")
+    refused_blob(damaged(lambda b, h: setattr(h, "gate", 0)), "gate")
+    refused_blob(damaged(lambda b, h: setattr(h, "gate", 3)), "gate")
+    refused_blob(damaged(lambda b, h: column(b, 5).__setitem__(1, 16)), "t_start > t_end")
+    refused_blob(damaged(lambda b, h: column(b, 6).__setitem__(2, -1)), "t_start > t_end")
+    refused_blob(damaged(lambda b, h: h.sec_bytes.__setitem__(6, h.sec_bytes[6] - 8)), "t_end holds")
+    refused_blob(damaged(lambda b, h: h.sec_off.__setitem__(4, h.sec_off[4] + 8)), "source is not 256-byte aligned")
+    refused_blob(blob[:150], "truncated")
     assert np.array_equal(eng.FeatureStore.load(blob).save(), blob)

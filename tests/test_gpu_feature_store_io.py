@@ -8,23 +8,16 @@ import numpy as np
 import pytest
 
 import fstore_oracle as fo
+from fstore_checks import METRICS, gpu_store, refused_blob, same_results, store_options
 
 pytestmark = pytest.mark.gpu
 
-METRICS = {"euclidean": fo.EUCLIDEAN, "cosine": fo.COSINE}
 TORCH_TYPES = {"f32": "float32", "f16": "float16", "bf16": "bfloat16"}
 
 
-def _opts(dim, K, **kw):
-    o = dict(distance_filter=1e9, max_observations=K, feature_dim=dim, topn=4, max_distance=1e9, min_votes=1)
-    o.update(kw)
-    return o
-
-
 def _store(metric, dim, K, t="f32", **kw):
-    import similari_b200.engine as eng
-
-    s = eng.FeatureStore(metric=metric, **_opts(dim, K, **kw))
+    """A store whose host calls send columns of type t."""
+    s = gpu_store(metric, max_observations=K, feature_dim=dim, **kw)
     s.set_feature_type(t)
     return s
 
@@ -103,18 +96,6 @@ def _run(store, steps, rows, feed=None):
     return outs
 
 
-def _bits(a):
-    a = np.ascontiguousarray(a)
-    return a.view({4: np.uint32, 8: np.uint64}.get(a.dtype.itemsize, a.dtype)) if a.dtype.kind == "f" else a
-
-
-def _same(a, b):
-    assert len(a) == len(b)
-    for i, (x, y) in enumerate(zip(a, b)):
-        assert x.dtype == y.dtype and x.shape == y.shape, i
-        assert np.array_equal(_bits(x), _bits(y)), (i, x, y)
-
-
 # ------------------------------------------------------------------------------------------------ element types
 @pytest.mark.parametrize("metric", ["euclidean", "cosine"])
 @pytest.mark.parametrize("dim", [8, 100, 256, 513])
@@ -124,10 +105,10 @@ def test_typed_columns_equal_the_widened_request(metric, dim, K):
     for t in ("f16", "bf16"):
         raw, wide = _pool(64, dim, t, seed=7 * dim + K)
         typed, plain = _store(metric, dim, K, t), _store(metric, dim, K)
-        oracle = fo.FeatureStore(metric=METRICS[metric], **_opts(dim, K))
+        oracle = fo.FeatureStore(metric=METRICS[metric], **store_options(max_observations=K, feature_dim=dim))
         want = _run(plain, steps, wide)
-        _same(_run(typed, steps, raw), want)
-        _same(_run(oracle, steps, wide), want)
+        same_results(_run(typed, steps, raw), want)
+        same_results(_run(oracle, steps, wide), want)
         assert typed.feature_type() == t and plain.feature_type() == "f32"
 
 
@@ -142,7 +123,7 @@ def test_float16_arrays_are_sent_as_they_are():
     assert a.feature_type() == "f32"
     b.add(ids, wide[:20])
     b.add(ids, wide[20:])
-    _same(_flat(a.fetch(ids)), _flat(b.fetch(ids)))
+    same_results(_flat(a.fetch(ids)), _flat(b.fetch(ids)))
     with pytest.raises(ValueError):
         _store("euclidean", 24, 3, "bf16").add(ids, wide[:20])   # a declared 2-byte type takes 2-byte elements only
 
@@ -189,8 +170,8 @@ def test_device_columns_equal_the_host_request(metric, t, dim, shift):
     raw, wide = _pool(64, dim, t, seed=dim + shift)
     dev, host, plain = _store(metric, dim, K, t), _store(metric, dim, K, t), _store(metric, dim, K)
     want = _run(plain, steps, wide)
-    _same(_run(host, steps, raw), want)
-    _same(_run(dev, steps, raw, feed=_device_feed(dev, t, dim, shift)), want)
+    same_results(_run(host, steps, raw), want)
+    same_results(_run(dev, steps, raw, feed=_device_feed(dev, t, dim, shift)), want)
 
 
 def test_device_calls_on_the_default_stream_and_empty_store():
@@ -202,9 +183,9 @@ def test_device_calls_on_the_default_stream_and_empty_store():
     col = torch.from_numpy(raw).cuda()   # written on the legacy default stream, which stream == 0 names
     ids = np.arange(50, 58, dtype=np.uint64)
     offs = np.arange(0, 9, dtype=np.int32) * 4
-    _same(_flat(dev.associate_device(ids, offs, col.data_ptr())), _flat(plain.associate(ids, offs, wide)))
-    _same(_flat(dev.search_device(ids + 100, offs, col.data_ptr())), _flat(plain.search(ids + 100, offs, wide)))
-    _same([dev.ids()] + _flat(dev.fetch(dev.ids())), [plain.ids()] + _flat(plain.fetch(plain.ids())))
+    same_results(_flat(dev.associate_device(ids, offs, col.data_ptr())), _flat(plain.associate(ids, offs, wide)))
+    same_results(_flat(dev.search_device(ids + 100, offs, col.data_ptr())), _flat(plain.search(ids + 100, offs, wide)))
+    same_results([dev.ids()] + _flat(dev.fetch(dev.ids())), [plain.ids()] + _flat(plain.fetch(plain.ids())))
 
 
 def test_a_host_pointer_is_not_a_device_column():
@@ -224,7 +205,7 @@ def test_a_host_pointer_is_not_a_device_column():
                      lambda p: s.associate_device(ids, offs, p)):
             with pytest.raises(Sb200Error, match="-1.*d_features"):
                 call(host.ctypes.data)
-            _same([s.ids()] + _flat(s.fetch(s.ids())), before)
+            same_results([s.ids()] + _flat(s.fetch(s.ids())), before)
 
 
 # ------------------------------------------------------------------------------------------------ the store blob
@@ -268,7 +249,7 @@ def test_save_load_continues_exactly(metric, t):
     state = [s.ids()] + _flat(s.fetch(s.ids()))
     for c in copies:
         assert (c.K, c.D, c.topn, c.feature_type()) == (K, dim, 4, t)
-        _same([c.ids()] + _flat(c.fetch(c.ids())), state)
+        same_results([c.ids()] + _flat(c.fetch(c.ids())), state)
         assert np.array_equal(c.save(), blob)
     steps = _script(dim, K, 64, seed=23)
     for st in steps:   # fresh ids: the script's query ids must not be stored yet
@@ -276,7 +257,7 @@ def test_save_load_continues_exactly(metric, t):
             st[1][:] += 5000
     want = _run(s, steps, raw)
     for c in copies:
-        _same(_run(c, steps, raw), want)
+        same_results(_run(c, steps, raw), want)
 
 
 def test_equal_states_give_equal_blobs():
@@ -292,7 +273,7 @@ def test_equal_states_give_equal_blobs():
     b.add(np.array([1, 1, 7, 7, 7, 1], np.uint64), raw[[21, 22, 25, 26, 27, 23]])
     b.fetch(np.array([7], np.uint64), remove=True)                            # compaction into fresh columns
     b.add(np.array([2], np.uint64), raw[[24]])
-    _same([a.ids()] + _flat(a.fetch(a.ids())), [b.ids()] + _flat(b.fetch(b.ids())))
+    same_results([a.ids()] + _flat(a.fetch(a.ids())), [b.ids()] + _flat(b.fetch(b.ids())))
     blob = a.save()
     assert np.array_equal(blob, b.save())
     # the unfilled slots of track 2 are zeros in the blob
@@ -317,19 +298,7 @@ def test_empty_store_round_trips():
     ids = np.arange(1, 9, dtype=np.uint64)
     for x in (s, c):
         x.add(ids, raw[:8])
-    _same(_flat(c.fetch(ids)), _flat(s.fetch(ids)))
-
-
-def _refused(blob, field):
-    """sb200_fstore_load refuses `blob` with SB200_ERR_INVALID, names `field`, and hands back no handle."""
-    from similari_b200 import _lib
-
-    L = _lib.lib()
-    h = C.c_void_p()
-    blob = np.ascontiguousarray(blob)
-    assert L.sb200_fstore_load(_lib.ptr(blob), len(blob), 0, C.byref(h)) == -1
-    assert h.value is None
-    assert field in L.sb200_last_error().decode(), L.sb200_last_error()
+    same_results(_flat(c.fetch(ids)), _flat(s.fetch(ids)))
 
 
 def test_damaged_blobs_are_refused():
@@ -350,27 +319,27 @@ def test_damaged_blobs_are_refused():
     def column(b, sec, dtype):
         return b[hdr.sec_off[sec]: hdr.sec_off[sec] + hdr.sec_bytes[sec]].view(dtype)
 
-    _refused(blob[:-1], "truncated")
-    _refused(blob[:100], "truncated")
-    _refused(damaged(lambda b, h: setattr(h, "version", 2)), "version")
-    _refused(damaged(lambda b, h: setattr(h, "magic", 0x42534253)), "magic")
-    _refused(damaged(lambda b, h: column(b, 1, np.int32).__setitem__(live // 2, 0)), "cnt")
-    _refused(damaged(lambda b, h: column(b, 1, np.int32).__setitem__(0, K + 1)), "cnt")
-    _refused(damaged(lambda b, h: column(b, 2, np.int32).__setitem__(live - 1, K)), "start")
-    _refused(damaged(lambda b, h: column(b, 2, np.int32).__setitem__(0, -1)), "start")
-    _refused(damaged(lambda b, h: column(b, 0, np.uint64).__setitem__(1, column(b, 0, np.uint64)[0])), "twice")
-    _refused(damaged(lambda b, h: h.sec_off.__setitem__(1, h.sec_off[1] + 8)), "cnt is not 256-byte aligned")
-    _refused(damaged(lambda b, h: h.sec_off.__setitem__(2, h.sec_off[1])), "start lies outside")
-    _refused(damaged(lambda b, h: h.sec_bytes.__setitem__(3, h.sec_bytes[3] - 4)), "feat holds")
-    _refused(damaged(lambda b, h: setattr(h, "max_observations", 65)), "max_observations")
-    _refused(damaged(lambda b, h: setattr(h, "topn", 0)), "topn")
-    _refused(damaged(lambda b, h: setattr(h, "feature_dim", 8193)), "feature_dim")
-    _refused(damaged(lambda b, h: setattr(h, "metric", 2)), "metric")
-    _refused(damaged(lambda b, h: setattr(h, "d8", h.d8 + 8)), "d8")
-    _refused(damaged(lambda b, h: setattr(h, "feature_type", 3)), "feature_type")
+    refused_blob(blob[:-1], "truncated")
+    refused_blob(blob[:100], "truncated")
+    refused_blob(damaged(lambda b, h: setattr(h, "version", 2)), "version")
+    refused_blob(damaged(lambda b, h: setattr(h, "magic", 0x42534253)), "magic")
+    refused_blob(damaged(lambda b, h: column(b, 1, np.int32).__setitem__(live // 2, 0)), "cnt")
+    refused_blob(damaged(lambda b, h: column(b, 1, np.int32).__setitem__(0, K + 1)), "cnt")
+    refused_blob(damaged(lambda b, h: column(b, 2, np.int32).__setitem__(live - 1, K)), "start")
+    refused_blob(damaged(lambda b, h: column(b, 2, np.int32).__setitem__(0, -1)), "start")
+    refused_blob(damaged(lambda b, h: column(b, 0, np.uint64).__setitem__(1, column(b, 0, np.uint64)[0])), "twice")
+    refused_blob(damaged(lambda b, h: h.sec_off.__setitem__(1, h.sec_off[1] + 8)), "cnt is not 256-byte aligned")
+    refused_blob(damaged(lambda b, h: h.sec_off.__setitem__(2, h.sec_off[1])), "start lies outside")
+    refused_blob(damaged(lambda b, h: h.sec_bytes.__setitem__(3, h.sec_bytes[3] - 4)), "feat holds")
+    refused_blob(damaged(lambda b, h: setattr(h, "max_observations", 65)), "max_observations")
+    refused_blob(damaged(lambda b, h: setattr(h, "topn", 0)), "topn")
+    refused_blob(damaged(lambda b, h: setattr(h, "feature_dim", 8193)), "feature_dim")
+    refused_blob(damaged(lambda b, h: setattr(h, "metric", 2)), "metric")
+    refused_blob(damaged(lambda b, h: setattr(h, "d8", h.d8 + 8)), "d8")
+    refused_blob(damaged(lambda b, h: setattr(h, "feature_type", 3)), "feature_type")
     # a tracker blob is not a store blob, and the other way round
     tracker = eng.Tracker(_lib.default_options())
-    _refused(tracker.save(), "magic")
+    refused_blob(tracker.save(), "magic")
     with pytest.raises(_lib.Sb200Error, match="-1"):
         eng.Tracker.load(blob)
     # the undamaged blob still loads, and the store that wrote it is as it was

@@ -13,6 +13,8 @@ import dataclasses
 import numpy as np
 import pytest
 
+from fstore_checks import same_results, store_pair
+
 pytestmark = pytest.mark.gpu
 
 F32 = np.float32
@@ -81,18 +83,6 @@ class Driver:
         return f
 
 
-def _bits(a):
-    a = np.ascontiguousarray(a)
-    return a.view(np.uint64) if a.dtype == np.float64 else a.view(np.uint32) if a.dtype == F32 else a
-
-
-def _same(a, b):
-    assert a.keys() == b.keys(), (a.keys(), b.keys())
-    for k in a:
-        assert a[k].shape == b[k].shape, k
-        assert np.array_equal(_bits(a[k]), _bits(b[k])), k
-
-
 # ---------------------------------------------------------------------------------------------------------- read-back
 def _oracle_live(o, sid, max_idle):
     """Positions of the oracle's tracks the device still holds (it sweeps expired tracks at the end of their frame, the
@@ -112,7 +102,7 @@ def _check_against_oracle(g, o, scene_ids, dim, where):
         assert a["ids"].tolist() == g.scene_tracks(sid)["ids"].tolist(), (where, sid)
         want = {"ids": a["ids"], "n_obs": ob["n_obs"][live], "has_feat": ob["has_feat"][live],
                 "quality": ob["quality"][live], "feats": np.ascontiguousarray(ob["feats"][live][:, :, :dim])}
-        _same(a, want)
+        same_results(a, want)
 
 
 CASES = [(1, "f32"), (3, "f32"), (5, "f16"), (8, "bf16"), (25, "f32"), (32, "bf16")]
@@ -274,7 +264,7 @@ def test_search_tracks_equals_the_host_composition(eng, case):
     a = s.search_tracks(t, sc, ti, id_offset=off, feature_class=fclass, **(attrs or {}))
     assert np.array_equal(t.save(), tb) and np.array_equal(s.save(), sb)
     b = _compose(t, s, sc, ti, off, fclass, attrs)
-    _same(a, b)
+    same_results(a, b)
     n_gone = min(len(gone), 6)
     assert a["found"].sum() == len(ti) - n_gone - 2   # every live track; no expired, unknown or unknown-scene pair
     assert (a["counts"] > 0).sum() > 0, "no query found a stored track: the case checks nothing"
@@ -307,14 +297,10 @@ def test_next_frames_equal_a_twin_that_never_searched(eng):
 
 def test_matches_the_oracles_directly(eng, oracle):
     """The oracle tracker fed the same frames, its scene_observations' present rows through fstore_oracle's search."""
-    import fstore_oracle as fo
-
     K, dim = 5, 24
     g = _tracker(eng, K, dim)
     o = oracle.Tracker(oracle.make_options(**_kw(K, dim)))
-    s = _store(eng, dim, K=3, topn=3)
-    so = fo.FeatureStore(metric=fo.EUCLIDEAN, distance_filter=1.0, max_observations=3, feature_dim=dim, topn=3,
-                         max_distance=1.0, min_votes=1)
+    s, so = store_pair(distance_filter=1.0, max_observations=3, feature_dim=dim, topn=3, max_distance=1.0)
     d = Driver(2, 40, dim, 0x0AC1E)
     for _ in range(6):
         f = d.frame([g], [o])
@@ -346,9 +332,7 @@ def test_matches_the_oracles_directly(eng, oracle):
             qi.append(i)
     assert np.flatnonzero(a["queried"]).tolist() == qi
     r = so.search(ti[qi], offs, np.concatenate(qrows))
-    assert np.array_equal(a["counts"][qi], r["counts"])
-    assert np.array_equal(a["winners"][qi], r["winners"])
-    assert np.array_equal(a["weights"][qi].view(np.uint64), r["weights"].view(np.uint64))
+    same_results({k: a[k][qi] for k in r}, r)
     assert r["counts"].sum() > 0
 
 

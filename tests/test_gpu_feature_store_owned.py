@@ -4,43 +4,9 @@ against the fetch + add emulation, and the chunked each-mode search against smal
 import numpy as np
 import pytest
 
-import fstore_oracle as fo
+from fstore_checks import gpu_store, same_results, same_store, store_pair
 
 pytestmark = pytest.mark.gpu
-
-METRICS = {"euclidean": fo.EUCLIDEAN, "cosine": fo.COSINE}
-
-
-def _opts(**kw):
-    o = dict(distance_filter=1e9, max_observations=3, feature_dim=16, topn=5, max_distance=1e9, min_votes=1)
-    o.update(kw)
-    return o
-
-
-def _pair(metric="euclidean", **kw):
-    import similari_b200.engine as eng
-
-    return eng.FeatureStore(metric=metric, **_opts(**kw)), fo.FeatureStore(metric=METRICS[metric], **_opts(**kw))
-
-
-def _same_results(rg, ro):
-    for k in ro:
-        a, b = rg[k], ro[k]
-        assert a.dtype == b.dtype and a.shape == b.shape, k
-        if a.dtype == np.float64:
-            assert np.array_equal(a.view(np.uint64), b.view(np.uint64)), (k, a, b)
-        else:
-            assert np.array_equal(a, b), (k, a, b)
-
-
-def _same_store(g, o):
-    ids = o.ids()
-    assert np.array_equal(g.ids(), ids)
-    assert g.size() == o.size() == len(ids)
-    cg, fg = g.fetch(ids)
-    co, fo_ = o.fetch(ids)
-    assert np.array_equal(cg, co)
-    assert np.array_equal(fg.view(np.uint32), fo_.view(np.uint32))
 
 
 def _fill(stores, rng, n_tracks, dim, K, dup=0):
@@ -66,14 +32,14 @@ def _fill(stores, rng, n_tracks, dim, K, dup=0):
 def test_search_owned_matches_the_oracle(metric, K, dim):
     rng = np.random.default_rng(K * 1000 + dim)
     for topn, min_votes in ((1, 1), (5, 2)):
-        g, o = _pair(metric, max_observations=K, feature_dim=dim, topn=topn, min_votes=min_votes)
+        g, o = store_pair(metric, max_observations=K, feature_dim=dim, topn=topn, min_votes=min_votes)
         _fill((g, o), rng, 40, dim, K, dup=2)
         ids = o.ids()
         q = np.concatenate([ids[rng.permutation(len(ids))[:9]], [777777]]).astype(np.uint64)
         for each in (False, True):
-            _same_results(g.search_owned(q, each=each), o.search_owned(q, each=each))
-        _same_results(g.search_owned(ids, each=True), o.search_owned(ids, each=True))
-        _same_store(g, o)
+            same_results(g.search_owned(q, each=each), o.search_owned(q, each=each))
+        same_results(g.search_owned(ids, each=True), o.search_owned(ids, each=True))
+        same_store(g, o)
         assert np.all(g.last_stage_ms()[:2] >= 0)
 
 
@@ -82,12 +48,12 @@ def test_exact_thresholds_and_ties(metric):
     """max_distance and distance_filter placed on distances the oracle computes; duplicate rows tie on weight and go to
     the lower position."""
     rng = np.random.default_rng(17)
-    g0, o0 = _pair(metric, feature_dim=24)
+    g0, o0 = store_pair(metric, feature_dim=24, topn=5)
     _fill((g0, o0), rng, 30, 24, 3, dup=3)
     tie = o0.search_owned([5], each=True)
     same = [x for x in tie["winners"][0, :tie["counts"][0]].tolist() if x in (1, 31, 32, 33)]
     assert same == sorted(same)   # track 1 and its copies tie; the lower store position comes first
-    _same_results(g0.search_owned([5], each=True), tie)
+    same_results(g0.search_owned([5], each=True), tie)
     # distances from track 5's rows to every other stored row, as the oracle computes them
     import oracle
     cnt, f = o0.fetch([5])
@@ -97,27 +63,27 @@ def test_exact_thresholds_and_ties(metric):
     ds = sorted(dist(f[0, i], fs[t, j]) for i in range(cnt[0]) for t in range(len(cs)) for j in range(cs[t])
                 if o0.ids()[t] != 5)
     for md, flt in ((ds[10], ds[30]), (ds[3], ds[10])):
-        g, o = _pair(metric, feature_dim=24, max_distance=md, distance_filter=flt, min_votes=2, topn=8)
+        g, o = store_pair(metric, feature_dim=24, max_distance=md, distance_filter=flt, min_votes=2, topn=8)
         _fill((g, o), np.random.default_rng(17), 30, 24, 3, dup=3)
         for each in (False, True):
             q = np.array([5, 1, 31], np.uint64)
-            _same_results(g.search_owned(q, each=each), o.search_owned(q, each=each))
+            same_results(g.search_owned(q, each=each), o.search_owned(q, each=each))
 
 
 def test_search_owned_edges():
-    g, o = _pair()
+    g, o = store_pair(topn=5)
     for each in (False, True):
-        _same_results(g.search_owned([], each=each), o.search_owned([], each=each))
-        _same_results(g.search_owned([4, 5], each=each), o.search_owned([4, 5], each=each))   # empty store
+        same_results(g.search_owned([], each=each), o.search_owned([], each=each))
+        same_results(g.search_owned([4, 5], each=each), o.search_owned([4, 5], each=each))   # empty store
     rng = np.random.default_rng(2)
     _fill((g, o), rng, 12, 16, 3)
     g.set_feature_type("f16")   # the rows are the stored f32 rows whatever the type
     for each in (False, True):
-        _same_results(g.search_owned(o.ids(), each=each), o.search_owned(o.ids(), each=each))
+        same_results(g.search_owned(o.ids(), each=each), o.search_owned(o.ids(), each=each))
     import similari_b200._lib as L
     with pytest.raises(L.Sb200Error):
         g.search_owned([1, 1])
-    _same_store(g, o)
+    same_store(g, o)
 
 
 def _blob(s):
@@ -161,42 +127,41 @@ def test_merge_owned_matches_the_oracle_and_the_emulation(metric, K, remove):
     import similari_b200.engine as eng
 
     rng = np.random.default_rng(K * 10 + remove)
-    g, o = _pair(metric, max_observations=K, feature_dim=40)
-    e = eng.FeatureStore(metric=metric, **_opts(max_observations=K, feature_dim=40))
+    g, o = store_pair(metric, max_observations=K, feature_dim=40, topn=5)
+    e = gpu_store(metric, max_observations=K, feature_dim=40, topn=5)
     _fill((g, o, e), rng, 60, 40, K)
     for step in range(3):
         dest, src = _pairs(rng, o.ids(), 25, remove)
         g.merge_owned(dest, src, remove=remove)
         o.merge_owned(dest, src, remove=remove)
         _emulate(e, dest, src, remove)
-        _same_store(g, o)
+        same_store(g, o)
         assert _blob(g) == _blob(e)
         assert g.last_stage_ms()[2] >= 0
         q = o.ids()[: 6]
         for each in (False, True):
-            _same_results(g.search_owned(q, each=each), o.search_owned(q, each=each))
+            same_results(g.search_owned(q, each=each), o.search_owned(q, each=each))
         qid = np.arange(5000 + 10 * step, 5003 + 10 * step, dtype=np.uint64)
         offs = np.array([0, 1, 3, 4], np.int32)
         f = rng.standard_normal((4, 40)).astype(np.float32)
-        _same_results(g.search(qid, offs, f), o.search(qid, offs, f))
-        _same_results(g.associate(qid, offs, f), o.associate(qid, offs, f))
+        same_results(g.search(qid, offs, f), o.search(qid, offs, f))
+        same_results(g.associate(qid, offs, f), o.associate(qid, offs, f))
         e.associate(qid, offs, f)
-        _same_store(g, o)
+        same_store(g, o)
     h = eng.FeatureStore.load(g.save())
     dest, src = _pairs(rng, o.ids(), 10, remove)
     for s in (g, h, o):
         s.merge_owned(dest, src, remove=remove)
-    _same_store(h, o)
+    same_store(h, o)
     assert _blob(h) == _blob(g)
 
 
 def test_star_of_many_sources_and_refusals():
     import similari_b200._lib as L
-    import similari_b200.engine as eng
 
     rng = np.random.default_rng(5)
-    g, o = _pair(max_observations=4, feature_dim=8)
-    e = eng.FeatureStore(**_opts(max_observations=4, feature_dim=8))
+    g, o = store_pair(max_observations=4, feature_dim=8, topn=5)
+    e = gpu_store(max_observations=4, feature_dim=8, topn=5)
     _fill((g, o, e), rng, 1200, 8, 4)
     src = [int(x) for x in o.ids()[1:1001]]
     dest = [int(o.ids()[0])] * len(src)
@@ -214,29 +179,25 @@ def test_star_of_many_sources_and_refusals():
     for s in (g, o):
         s.merge_owned(dest, src, remove=True)
     _emulate(e, dest, src, True)
-    _same_store(g, o)
+    same_store(g, o)
     assert _blob(g) == _blob(e)
 
 
 def test_each_mode_chunks_a_whole_store():
     """40,000 single-observation 8-d tracks, all queried: 40,000 x 40,000 pairs need two chunks of 2^30."""
-    import similari_b200.engine as eng
-
     rng = np.random.default_rng(40)
     n = 40000
-    g = eng.FeatureStore(**_opts(max_observations=1, feature_dim=8, topn=3))
-    o = fo.FeatureStore(metric=fo.EUCLIDEAN, **_opts(max_observations=1, feature_dim=8, topn=3))
+    g, o = store_pair(max_observations=1, feature_dim=8, topn=3)
     ids = np.arange(1, n + 1, dtype=np.uint64)
     f = rng.standard_normal((n, 8)).astype(np.float32)
     g.add(ids, f)
     o.add(ids, f)
     whole = g.search_owned(ids, each=True)
     parts = [g.search_owned(ids[a:a + 9000], each=True) for a in range(0, n, 9000)]
-    for k in whole:
-        assert np.array_equal(whole[k].view(np.uint8), np.concatenate([p[k] for p in parts]).view(np.uint8)), k
+    same_results(whole, {k: np.concatenate([p[k] for p in parts]) for k in whole})
     sample = rng.choice(n, 6, replace=False)
     ro = o.search_owned(ids[sample], each=True)
-    _same_results({k: v[sample] for k, v in whole.items()}, ro)
+    same_results({k: v[sample] for k, v in whole.items()}, ro)
     import similari_b200._lib as L
     with pytest.raises(L.Sb200Error, match="-3|2\\^30"):
         g.search_owned(ids, each=False)

@@ -5,63 +5,20 @@ for byte, for every pair of storage types, both metrics, gated and ungated, remo
 held to the CPU oracle bit for bit.  Also: a seeded collect / find_baked / promote pipeline with a save and load of both
 stores in the middle, find_baked against Python integers, a gallery-scale case and every refusal."""
 import itertools
-import os
 import zlib
 
 import numpy as np
 import pytest
 
 import fstore_oracle as fo
+from fstore_checks import gpu_store, same_results, same_store, store_pair
 
 pytestmark = pytest.mark.gpu
 
-METRICS = {"euclidean": fo.EUCLIDEAN, "cosine": fo.COSINE}
 TYPES = ("f32", "f16", "bf16")
-THREADS = max(1, min(16, os.cpu_count() or 1))
 I64_MIN, I64_MAX = -(1 << 63), (1 << 63) - 1
 ERR_INVALID, ERR_CAPACITY = -1, -3
-
-
-def _opts(**kw):
-    o = dict(distance_filter=1e9, max_observations=4, feature_dim=20, topn=2, max_distance=3.0, min_votes=1)
-    o.update(kw)
-    return o
-
-
-def _gpu(storage="f32", metric="euclidean", gate=None, retention="newest", **kw):
-    import similari_b200.engine as eng
-
-    return eng.FeatureStore(metric=metric, storage=storage, gate=gate, retention=retention, **_opts(**kw))
-
-
-def _oracle(metric="euclidean", gate=None, retention="newest", **kw):
-    return fo.FeatureStore(metric=METRICS[metric], gate=gate, retention=retention, threads=THREADS, **_opts(**kw))
-
-
-def _same(a, b, what=""):
-    assert a.keys() == b.keys(), what
-    for k in b:
-        x, y = a[k], b[k]
-        assert x.dtype == y.dtype and x.shape == y.shape, (what, k)
-        if x.dtype == np.float64:
-            assert np.array_equal(x.view(np.uint64), y.view(np.uint64)), (what, k, x, y)
-        else:
-            assert np.array_equal(x, y), (what, k, x, y)
-
-
-def _same_quality_store(g, o, what=""):
-    ids = o.ids()
-    assert np.array_equal(g.ids(), ids), what
-    cg, fg, qg = g.fetch_quality(ids)
-    co, fo_, qo = o.fetch_quality(ids)
-    assert np.array_equal(cg, co), what
-    assert np.array_equal(fg.view(np.uint32), fo_.view(np.uint32)), what
-    assert np.array_equal(qg.view(np.uint32), qo.view(np.uint32)), what
-    for x, y in zip(g.merge_history(ids), o.merge_history(ids)):
-        assert np.array_equal(x, y), what
-    if o.gate is not None:
-        for x, y in zip(g.attributes(ids), o.attributes(ids)):
-            assert np.array_equal(x, y), what
+OPTS = dict(max_observations=4, feature_dim=20, topn=2, max_distance=3.0)
 
 
 def _exact(x):
@@ -116,8 +73,8 @@ def test_newest_stores_match_the_host_composition(metric, gate):
             rng = np.random.default_rng(zlib.crc32(repr((metric, gate, st_d, st_s, remove)).encode()))
             K, dim = 4, 20
             md = 3.0 if metric == "euclidean" else 0.5   # near pairs within, unrelated ones beyond
-            da, db = _gpu(st_d, metric, gate, max_distance=md), _gpu(st_d, metric, gate, max_distance=md)
-            sa, sb = _gpu(st_s, metric, gate, topn=3), _gpu(st_s, metric, gate, topn=3)
+            da, db = (gpu_store(metric, st_d, gate=gate, **OPTS | dict(max_distance=md)) for _ in range(2))
+            sa, sb = (gpu_store(metric, st_s, gate=gate, **OPTS | dict(topn=3)) for _ in range(2))
             centers = rng.standard_normal((30, dim))
             _fill([da, db], rng, np.arange(1, 31, dtype=np.uint64), K, dim, centers, gate)
             near = centers[rng.integers(0, 30, 40)] + 0.02
@@ -128,7 +85,7 @@ def test_newest_stores_match_the_host_composition(metric, gate):
                 what = (metric, gate, st_d, st_s, remove, rnd)
                 ra = da.associate_store(sa, ids, remove=bool(remove))
                 rb = _compose(db, sb, ids, bool(remove))
-                _same(ra, rb, what)
+                same_results(ra, rb, what)
                 merged, new = merged + int(ra["merged"].sum()), new + int((ra["merged"] == 0).sum())
                 assert np.array_equal(da.save(), db.save()), what
                 assert np.array_equal(sa.save(), sb.save()), what
@@ -138,8 +95,8 @@ def test_newest_stores_match_the_host_composition(metric, gate):
 
 def _quality_pair(metric, gate, st_d, st_s, rng, K=12, dim=24):
     kw = dict(max_observations=K, feature_dim=dim, topn=3, max_distance=4.0)
-    dg, do = _gpu(st_d, metric, gate, "quality", **kw), _oracle(metric, gate, "quality", **kw)
-    sg, so = _gpu(st_s, metric, gate, "quality", **kw), _oracle(metric, gate, "quality", **kw)
+    dg, do = store_pair(metric, st_d, gate, "quality", **kw)
+    sg, so = store_pair(metric, st_s, gate, "quality", **kw)
     centers = rng.standard_normal((24, dim))
     _fill([dg, do], rng, np.arange(1, 25, dtype=np.uint64), K, dim, centers, gate, quality=True)
     near = rng.integers(0, 24, 60)
@@ -165,16 +122,16 @@ def _quality_pair(metric, gate, st_d, st_s, rng, K=12, dim=24):
 def test_quality_stores_match_the_oracle(types, metric, gate):
     rng = np.random.default_rng(zlib.crc32(repr((types, metric, gate)).encode()))
     dg, do, sg, so = _quality_pair(metric, gate, *types, rng)
-    _same_quality_store(dg, do, "dst before")
-    _same_quality_store(sg, so, "src before")
+    same_store(dg, do)
+    same_store(sg, so)
     for rnd in range(4):
         ids = rng.permutation(np.setdiff1d(so.ids(), do.ids()))[: int(rng.integers(1, 16))]
         remove = rnd != 1
         rg = dg.associate_store(sg, ids, remove=remove)
         ro = do.associate_store(so, ids, remove=remove)
-        _same(rg, ro, (types, metric, gate, rnd))
-        _same_quality_store(dg, do, ("dst", rnd))
-        _same_quality_store(sg, so, ("src", rnd))
+        same_results(rg, ro, (types, metric, gate, rnd))
+        same_store(dg, do)
+        same_store(sg, so)
     assert np.any([len(h) > 2 for h in dg.merge_history(dg.ids())])
 
 
@@ -188,10 +145,8 @@ def test_pipeline_with_a_save_and_load_in_the_middle(retention):
     K, dim, period = 12, 32, 3
     kw = dict(max_observations=K, feature_dim=dim, topn=1, max_distance=2.5, min_votes=2)
     q = retention == "quality"
-    col_g = _gpu("f16", "euclidean", "same_source", retention, **kw)
-    gal_g = _gpu("bf16", "euclidean", "same_source", retention, **kw)
-    col_o = _oracle("euclidean", "same_source", retention, **kw)
-    gal_o = _oracle("euclidean", "same_source", retention, **kw)
+    col_g, col_o = store_pair("euclidean", "f16", "same_source", retention, **kw)
+    gal_g, gal_o = store_pair("euclidean", "bf16", "same_source", retention, **kw)
     people = rng.standard_normal((20, dim)).astype(np.float32)
     active, next_id, promoted = {}, 1, 0
     for frame in range(60):
@@ -213,19 +168,12 @@ def test_pipeline_with_a_save_and_load_in_the_middle(retention):
         assert np.array_equal(col_g.find_baked(frame, period), baked), frame
         rg = gal_g.associate_store(col_g, baked)
         ro = gal_o.associate_store(col_o, baked)
-        _same(rg, ro, frame)
+        same_results(rg, ro, frame)
         promoted += len(baked)
         assert np.array_equal(col_g.ids(), col_o.ids()) and np.array_equal(gal_g.ids(), gal_o.ids())
         if frame % 10 == 9:
-            if q:
-                _same_quality_store(gal_g, gal_o, frame)
-                _same_quality_store(col_g, col_o, frame)
-            else:
-                for g, o in ((gal_g, gal_o), (col_g, col_o)):
-                    (cg, fg), (co, fo_) = g.fetch(o.ids()), o.fetch(o.ids())
-                    assert np.array_equal(cg, co) and np.array_equal(fg.view(np.uint32), fo_.view(np.uint32)), frame
-                    for x, y in zip(g.attributes(o.ids()), o.attributes(o.ids())):
-                        assert np.array_equal(x, y), frame
+            same_store(gal_g, gal_o)
+            same_store(col_g, col_o)
     assert promoted > 40 and gal_o.size() < promoted   # tracklets were merged into identities
 
 
@@ -238,7 +186,7 @@ def test_find_baked_matches_python_integers():
     ends = rng.integers(-10**6, 10**6, n).astype(np.int64)
     ends[: len(extremes)] = extremes
     ends[rng.random(n) < 0.05] = rng.choice(extremes, 1)[0]
-    g = _gpu(gate="any_source", max_observations=1, feature_dim=8)
+    g = gpu_store(gate="any_source", **OPTS | dict(max_observations=1, feature_dim=8))
     ids = rng.permutation(np.arange(1, n + 1, dtype=np.uint64) * 7)
     g.add(ids, np.zeros((n, 8), np.float32), sources=np.ones(n, np.uint64), t_start=np.full(n, I64_MIN, np.int64),
           t_end=ends)
@@ -275,7 +223,7 @@ def test_gallery_scale():
     rng = np.random.default_rng(7)
     K, dim, n = 12, 512, 20000
     kw = dict(max_observations=K, feature_dim=dim, topn=4, max_distance=12.0, min_votes=1)
-    g = _gpu("bf16", "euclidean", "same_source", **kw)
+    g = gpu_store("euclidean", "bf16", gate="same_source", **OPTS | kw)
     centers = rng.standard_normal((n, dim)).astype(np.float32)
     for a in range(0, n, 2000):
         ids = np.repeat(np.arange(a + 1, a + 2001, dtype=np.uint64), K)
@@ -284,15 +232,14 @@ def test_gallery_scale():
         g.add(ids, rows, sources=ids % 3 + 1, t_start=t, t_end=t + 5)
     blob = g.save()
     twin = eng.FeatureStore.load(blob)
-    src_a = _gpu("f32", "euclidean", "same_source", **kw)
-    src_b = _gpu("f32", "euclidean", "same_source", **kw)
+    src_a, src_b = (gpu_store(gate="same_source", **OPTS | kw) for _ in range(2))
     pick = rng.integers(0, n, 256)
     _fill([src_a, src_b], rng, np.arange(10**6, 10**6 + 256, dtype=np.uint64), K, dim, centers[pick], "same_source",
           t_base=10**6)
     ids = src_a.ids()
     ra = g.associate_store(src_a, ids)
     rb = _compose(twin, src_b, ids, True)
-    _same(ra, rb, "gallery")
+    same_results(ra, rb, "gallery")
     assert ra["merged"].sum() > 40 and (ra["merged"] == 0).sum() > 40   # the source gate leaves about 1 in 3
     assert np.array_equal(g.save(), twin.save())
     assert src_a.size() == 0 and np.array_equal(src_a.save(), src_b.save())
@@ -303,8 +250,8 @@ def test_refusals_leave_both_stores_unchanged():
 
     L, p = _lib.lib(), _lib.ptr
     kw = dict(max_observations=4, feature_dim=8)
-    dst = _gpu(gate="same_source", retention="quality", **kw)
-    src = _gpu(gate="same_source", retention="quality", storage="bf16", **kw)
+    dst = gpu_store(gate="same_source", retention="quality", **OPTS | kw)
+    src = gpu_store(storage="bf16", gate="same_source", retention="quality", **OPTS | kw)
     f = np.ones((3, 8), np.float32)
     dst.add([1], f[:1], sources=[1], t_start=[0], t_end=[1], quality=[1])
     src.add([7, 8], f[:2], sources=[1, 1], t_start=[5, 5], t_end=[6, 6], quality=[1, 1])
@@ -323,15 +270,16 @@ def test_refusals_leave_both_stores_unchanged():
     refused(dst._h, None, [7], "NULL")
     refused(None, src._h, [7], "NULL")
     refused(dst._h, dst._h, [1], "same store")
-    for other, word in [(_gpu(gate="same_source", retention="quality", max_observations=4, feature_dim=16),
+    for other, word in [(dict(gate="same_source", retention="quality", max_observations=4, feature_dim=16),
                          "feature_dim"),
-                        (_gpu(gate="same_source", retention="quality", max_observations=6, feature_dim=8),
+                        (dict(gate="same_source", retention="quality", max_observations=6, feature_dim=8),
                          "max_observations"),
-                        (_gpu(gate="any_source", retention="quality", **kw), "gate"),
-                        (_gpu(retention="quality", **kw), "gate"),
-                        (_gpu(gate="same_source", **kw), "retention"),
-                        (_gpu(gate="same_source", retention="quality", initial_capacity=3, **kw), "retention"),
-                        (_gpu(gate="same_source", retention="quality", merge_extension=2.0, **kw), "retention")]:
+                        (dict(gate="any_source", retention="quality", **kw), "gate"),
+                        (dict(retention="quality", **kw), "gate"),
+                        (dict(gate="same_source", **kw), "retention"),
+                        (dict(gate="same_source", retention="quality", initial_capacity=3, **kw), "retention"),
+                        (dict(gate="same_source", retention="quality", merge_extension=2.0, **kw), "retention")]:
+        other = gpu_store(**OPTS | other)
         refused(dst._h, other._h, [], word)
     refused(dst._h, src._h, [7], "n < 0", n=-1)
     refused(dst._h, src._h, [7], "remove", remove=2)
@@ -340,8 +288,7 @@ def test_refusals_leave_both_stores_unchanged():
     refused(dst._h, src._h, [8, 1], "already stored")
     refused(dst._h, src._h, [7], "NULL", outs=[o[0], None, o[2], o[3], o[4]])
     # the pair bound: 65 x 64 queried rows against 4096 x 64 stored slots is just above 2^30 pairs
-    big_d = _gpu(max_observations=64, feature_dim=8)
-    big_s = _gpu(max_observations=64, feature_dim=8)
+    big_d, big_s = (gpu_store(**OPTS | dict(max_observations=64, feature_dim=8)) for _ in range(2))
     big_d.add(np.repeat(np.arange(1, 4097, dtype=np.uint64), 64), np.zeros((4096 * 64, 8), np.float32))
     big_s.add(np.repeat(np.arange(10**6, 10**6 + 65, dtype=np.uint64), 64), np.zeros((65 * 64, 8), np.float32))
     bd, bs = big_d.save(), big_s.save()
@@ -351,7 +298,7 @@ def test_refusals_leave_both_stores_unchanged():
     assert rc == ERR_CAPACITY and "2^30" in L.sb200_last_error().decode()
     assert np.array_equal(big_d.save(), bd) and np.array_equal(big_s.save(), bs)
     # find_baked
-    u = _gpu(**kw)
+    u = gpu_store(**OPTS | kw)
     assert L.sb200_fstore_find_baked(u._h, 0, 0, 0, None) < 0 and "gate" in L.sb200_last_error().decode()
     assert L.sb200_fstore_find_baked(dst._h, 0, 0, -1, None) < 0
     assert L.sb200_fstore_find_baked(dst._h, 0, 0, 1, None) < 0

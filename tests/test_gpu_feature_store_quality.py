@@ -4,56 +4,17 @@ every storage type, both metrics, gated and ungated, with a save and load in the
 merge_owned chains and stars; a gallery-scale case; the version-3 blob (byte-equal twins, refusals); and every refusal
 leaving the store (and, for associate_wasted, the tracker) as it was."""
 import ctypes as C
-import os
 import zlib
 
 import numpy as np
 import pytest
 
 import fstore_oracle as fo
+from fstore_checks import gpu_store, refused_blob, same_results, same_store, store_pair
 
 pytestmark = pytest.mark.gpu
 
-METRICS = {"euclidean": fo.EUCLIDEAN, "cosine": fo.COSINE}
-THREADS = max(1, min(16, os.cpu_count() or 1))
-
-
-def _opts(**kw):
-    o = dict(distance_filter=1e9, max_observations=12, feature_dim=16, topn=4, max_distance=1e9, min_votes=1)
-    o.update(kw)
-    return o
-
-
-def _pair(metric="euclidean", gate=None, storage="f32", **kw):
-    import similari_b200.engine as eng
-
-    return (eng.FeatureStore(metric=metric, storage=storage, gate=gate, retention="quality", **_opts(**kw)),
-            fo.FeatureStore(metric=METRICS[metric], gate=gate, threads=THREADS, retention="quality", **_opts(**kw)))
-
-
-def _same(a, b, what=""):
-    for k in b:
-        x, y = a[k], b[k]
-        assert x.dtype == y.dtype and x.shape == y.shape, (what, k)
-        if x.dtype == np.float64:
-            assert np.array_equal(x.view(np.uint64), y.view(np.uint64)), (what, k, x, y)
-        else:
-            assert np.array_equal(x, y), (what, k, x, y)
-
-
-def _same_store(g, o):
-    ids = o.ids()
-    assert np.array_equal(g.ids(), ids)
-    cg, fg, qg = g.fetch_quality(ids)
-    co, fo_, qo = o.fetch_quality(ids)
-    assert np.array_equal(cg, co)
-    assert np.array_equal(fg.view(np.uint32), fo_.view(np.uint32))
-    assert np.array_equal(qg.view(np.uint32), qo.view(np.uint32))
-    for x, y in zip(g.merge_history(ids), o.merge_history(ids)):
-        assert np.array_equal(x, y)
-    if o.gate is not None:
-        for x, y in zip(g.attributes(ids), o.attributes(ids)):
-            assert np.array_equal(x, y)
+QUALITY = dict(retention="quality", max_observations=12)
 
 
 def _feats(rng, n, dim, storage):
@@ -121,12 +82,12 @@ def _step(rng, g, o, it, dim, storage, gate, next_id):
             rg = getattr(g, op + "_device")(qid, offs, d.data_ptr(), quality=q, **at)
         else:
             rg = getattr(g, op)(qid, offs, f, quality=q, **at)
-        _same(rg, ro, op)
+        same_results(rg, ro, op)
         return next_id + Q
     if kind == 4:   # owned search, both modes
         sel = rng.choice(ids, min(len(ids), int(rng.integers(1, 6))), replace=False).astype(np.uint64)
         each = bool(rng.integers(0, 2))
-        _same(g.search_owned(sel, each=each), o.search_owned(sel, each=each), "search_owned")
+        same_results(g.search_owned(sel, each=each), o.search_owned(sel, each=each), "search_owned")
         return next_id
     if kind == 5:   # merge_owned: a chain or a star, with or without removal
         k = int(rng.integers(2, min(6, len(ids)) + 1))
@@ -148,9 +109,7 @@ def _step(rng, g, o, it, dim, storage, gate, next_id):
         return next_id
     sel = rng.choice(ids, min(len(ids), 3), replace=False).astype(np.uint64)   # fetch, sometimes removing
     remove = bool(rng.integers(0, 4) == 0)
-    for x, y in zip(g.fetch_quality(sel, remove=remove), o.fetch_quality(sel, remove=remove)):
-        assert np.array_equal(x.view(np.uint32) if x.dtype == np.float32 else x,
-                              y.view(np.uint32) if y.dtype == np.float32 else y)
+    same_results(g.fetch_quality(sel, remove=remove), o.fetch_quality(sel, remove=remove))
     return next_id
 
 
@@ -162,44 +121,44 @@ def test_mixed_sequences_match_the_oracle(storage, metric, gate):
 
     rng = np.random.default_rng(zlib.crc32(f"quality {storage} {metric} {gate}".encode()))
     dim = 24
-    g, o = _pair(metric, gate, storage, feature_dim=dim)
+    g, o = store_pair(metric, storage, gate, **QUALITY, feature_dim=dim)
     next_id = 1
     for it in range(240):
         next_id = _step(rng, g, o, it, dim, storage, gate, next_id)
         if it % 40 == 39:
-            _same_store(g, o)
+            same_store(g, o)
         if it == 120:   # save and load in the middle: the loaded store continues identically
             blob = g.save()
             g = eng.FeatureStore.load(blob)
             assert g.retention() == ("quality", 4, 1.5) and g.gate == gate and g.storage_type() == storage
             assert np.array_equal(g.save(), blob)
-    _same_store(g, o)
+    same_store(g, o)
     assert max(len(h) for h in o.merge_history(o.ids())) > 2   # merges happened
 
 
 @pytest.mark.parametrize("remove", [False, True])
 def test_merge_chains_and_stars(remove):
     rng = np.random.default_rng(3 + remove)
-    g, o = _pair(storage="bf16", max_observations=9, initial_capacity=2, merge_extension=2.0)
+    g, o = store_pair(storage="bf16", retention="quality", max_observations=9, initial_capacity=2, merge_extension=2.0)
     n = 12
     aid = np.repeat(np.arange(1, n + 1, dtype=np.uint64), 7)
     f, q = _feats(rng, len(aid), 16, "bf16"), _quality(rng, len(aid))
     for s in (g, o):
         s.add(aid, f, quality=q)
-    _same_store(g, o)
+    same_store(g, o)
     chain = (np.array([2, 3, 4, 5], np.uint64), np.array([1, 2, 3, 4], np.uint64))   # 2 <- 1, 3 <- 2, ...
     star = (np.array([6, 6, 6], np.uint64), np.array([7, 8, 9], np.uint64))
     for d, s in (chain, star):
         for x in (g, o):
             x.merge_owned(d, s, remove=remove)
-        _same_store(g, o)
+        same_store(g, o)
     assert o.merge_history([5])[0].tolist() == [5, 4, 3, 2, 1]
 
 
 def test_gallery_scale():
     rng = np.random.default_rng(20000)
     dim, n = 512, 20000
-    g, o = _pair("cosine", storage="f16", feature_dim=dim, topn=5)
+    g, o = store_pair("cosine", "f16", **QUALITY, feature_dim=dim, topn=5)
     aid = np.repeat(np.arange(1, n + 1, dtype=np.uint64), 8)
     rng.shuffle(aid)
     f, q = _feats(rng, len(aid), dim, "f16"), _quality(rng, len(aid))
@@ -210,18 +169,15 @@ def test_gallery_scale():
     offs = np.concatenate([[0], np.cumsum(lens)]).astype(np.int32)
     qid = np.arange(10 ** 6, 10 ** 6 + Q, dtype=np.uint64)
     qf, qq = _feats(rng, int(offs[-1]), dim, "f16"), _quality(rng, int(offs[-1]))
-    _same(g.associate(qid, offs, qf, quality=qq), o.associate(qid, offs, qf, quality=qq), "associate")
+    same_results(g.associate(qid, offs, qf, quality=qq), o.associate(qid, offs, qf, quality=qq), "associate")
     sel = o.ids()[::997]
-    _same(g.search_owned(sel), o.search_owned(sel), "search_owned")
+    same_results(g.search_owned(sel), o.search_owned(sel), "search_owned")
     g.merge_owned(sel[1:], sel[:-1])
     o.merge_owned(sel[1:], sel[:-1])
     assert np.array_equal(g.ids(), o.ids())
     some = np.concatenate([sel[-1:], qid, o.ids()[::1009]])   # the merged track, the queries' tracks and a sample
-    for x, y in zip(g.fetch_quality(some), o.fetch_quality(some)):
-        assert np.array_equal(x.view(np.uint32) if x.dtype == np.float32 else x,
-                              y.view(np.uint32) if y.dtype == np.float32 else y)
-    for x, y in zip(g.merge_history(some), o.merge_history(some)):
-        assert np.array_equal(x, y)
+    same_results(g.fetch_quality(some), o.fetch_quality(some))
+    same_results(g.merge_history(some), o.merge_history(some))
 
 
 def _rc(L, fn, *args):
@@ -234,7 +190,7 @@ def test_refusals_leave_the_store_unchanged():
 
     L = _lib.lib()
     p = _lib.ptr
-    g, _ = _pair(feature_dim=8)
+    g = gpu_store(**QUALITY, feature_dim=8)
     f = np.ones((3, 8), np.float32)
     g.add([1, 2, 1], f, quality=[1, 2, 3])
     blob = g.save()
@@ -274,7 +230,7 @@ def test_refusals_leave_the_store_unchanged():
     assert "quality" in L.sb200_last_error().decode()
     assert np.array_equal(g.save(), blob) and np.array_equal(t.save(), tb)
     # the _quality calls on a newest store, and bad parameters on an empty one
-    u = eng.FeatureStore(**_opts(feature_dim=8))
+    u = gpu_store(max_observations=12, feature_dim=8)
     q1 = np.ones(1, np.float32)
     rc, msg = _rc(L, L.sb200_fstore_add_quality, u._h, 1, p(ids), p(q1), None, p(f), None, None)
     assert rc == -1 and "newest" in msg
@@ -293,8 +249,8 @@ def test_quality_blob_twins_are_byte_equal_and_newest_blobs_unchanged():
 
     rng = np.random.default_rng(31)
     for gate in (None, "any_source"):
-        g1, o = _pair(gate=gate, storage="f16", feature_dim=20)
-        g2, _ = _pair(gate=gate, storage="f16", feature_dim=20)
+        g1, o = store_pair(storage="f16", gate=gate, **QUALITY, feature_dim=20)
+        g2 = gpu_store(storage="f16", gate=gate, **QUALITY, feature_dim=20)
         aid = np.repeat(np.arange(1, 21, dtype=np.uint64), 5)
         f, q = _feats(rng, len(aid), 20, "f16"), _quality(rng, len(aid))
         t0 = (aid.astype(np.int64) * 10)
@@ -310,29 +266,18 @@ def test_quality_blob_twins_are_byte_equal_and_newest_blobs_unchanged():
         assert (h.sec_bytes[4] == 0) == (gate is None)
         c = eng.FeatureStore.load(b1)
         assert np.array_equal(c.save(), b1)
-        _same_store(c, o)
-    n = eng.FeatureStore(**_opts(feature_dim=8))
+        same_store(c, o)
+    n = gpu_store(max_observations=12, feature_dim=8)
     n.add([1, 2], np.ones((2, 8), np.float32))
     hn = _lib.FstoreBlobHeader.from_buffer_copy(n.save()[:128].tobytes())
     assert hn.version == 1
-
-
-def _refused(blob, field):
-    from similari_b200 import _lib
-
-    L = _lib.lib()
-    h = C.c_void_p()
-    blob = np.ascontiguousarray(blob)
-    assert L.sb200_fstore_load(_lib.ptr(blob), len(blob), 0, C.byref(h)) == -1
-    assert h.value is None
-    assert field in L.sb200_last_error().decode(), L.sb200_last_error()
 
 
 def test_damaged_version_3_blobs_are_refused():
     import similari_b200.engine as eng
     from similari_b200 import _lib
 
-    g, _ = _pair(feature_dim=8, max_observations=4)
+    g = gpu_store(retention="quality", feature_dim=8, max_observations=4)
     g.add([1, 2, 3, 1], np.ones((4, 8), np.float32), quality=[1, 2, 3, 4])
     g.merge_owned([1], [2], remove=False)
     blob = g.save()
@@ -347,18 +292,18 @@ def test_damaged_version_3_blobs_are_refused():
     def column(b, sec, dtype):
         return b[hdr.sec_off[sec]: hdr.sec_off[sec] + hdr.sec_bytes[sec]].view(dtype)
 
-    _refused(damaged(lambda b, h: setattr(h, "retention", 2)), "retention")
-    _refused(damaged(lambda b, h: setattr(h, "initial_capacity", 0)), "initial_capacity")
-    _refused(damaged(lambda b, h: setattr(h, "merge_extension", float("nan"))), "merge_extension")
-    _refused(damaged(lambda b, h: column(b, 7, np.float32).__setitem__(4, np.nan)), "NaN")   # track 2's first slot
-    _refused(damaged(lambda b, h: column(b, 8, np.int32).__setitem__(2, 0)), "length 0")
-    _refused(damaged(lambda b, h: column(b, 9, np.uint64).__setitem__(2, 7)), "not with its id")
-    _refused(damaged(lambda b, h: column(b, 8, np.int32).__setitem__(0, 3)), "history holds")
-    _refused(damaged(lambda b, h: h.sec_bytes.__setitem__(7, h.sec_bytes[7] - 4)), "quality holds")
+    refused_blob(damaged(lambda b, h: setattr(h, "retention", 2)), "retention")
+    refused_blob(damaged(lambda b, h: setattr(h, "initial_capacity", 0)), "initial_capacity")
+    refused_blob(damaged(lambda b, h: setattr(h, "merge_extension", float("nan"))), "merge_extension")
+    refused_blob(damaged(lambda b, h: column(b, 7, np.float32).__setitem__(4, np.nan)), "NaN")   # track 2's first slot
+    refused_blob(damaged(lambda b, h: column(b, 8, np.int32).__setitem__(2, 0)), "length 0")
+    refused_blob(damaged(lambda b, h: column(b, 9, np.uint64).__setitem__(2, 7)), "not with its id")
+    refused_blob(damaged(lambda b, h: column(b, 8, np.int32).__setitem__(0, 3)), "history holds")
+    refused_blob(damaged(lambda b, h: h.sec_bytes.__setitem__(7, h.sec_bytes[7] - 4)), "quality holds")
     # states the rule cannot produce: a list out of quality order, a ring start other than 0, a count above c(h)
-    _refused(damaged(lambda b, h: column(b, 7, np.float32).__setitem__(1, 5.0)), "quality order")
-    _refused(damaged(lambda b, h: column(b, 2, np.int32).__setitem__(1, 1)), "ring start")
-    _refused(damaged(lambda b, h: setattr(h, "initial_capacity", 1)), "above its capacity")   # c(2) = 2 < 3 rows
+    refused_blob(damaged(lambda b, h: column(b, 7, np.float32).__setitem__(1, 5.0)), "quality order")
+    refused_blob(damaged(lambda b, h: column(b, 2, np.int32).__setitem__(1, 1)), "ring start")
+    refused_blob(damaged(lambda b, h: setattr(h, "initial_capacity", 1)), "above its capacity")   # c(2) = 2 < 3 rows
     c = eng.FeatureStore.load(damaged(lambda b, h: column(b, 7, np.float32).__setitem__(7, np.nan)))   # empty slot
     assert np.array_equal(c.save(), blob)
 
@@ -371,8 +316,8 @@ def test_twins_reached_by_different_routes_save_byte_equal_blobs():
 
     rng = np.random.default_rng(12)
     for storage in ("f32", "bf16"):
-        ga, o = _pair(storage=storage, feature_dim=20)
-        gb, _ = _pair(storage=storage, feature_dim=20)
+        ga, o = store_pair(storage=storage, **QUALITY, feature_dim=20)
+        gb = gpu_store(storage=storage, **QUALITY, feature_dim=20)
         x, y, z = (_feats(rng, 6, 20, storage) for _ in range(3))
         one, two = np.ones(6, np.uint64), np.full(6, 2, np.uint64)
         ga.add(one, x, quality=np.full(6, 0.25, np.float32))   # displaced, row by row, by the six better rows of y
@@ -383,8 +328,8 @@ def test_twins_reached_by_different_routes_save_byte_equal_blobs():
         for s in (o,):
             s.add(one, y, quality=np.ones(6, np.float32))
             s.add(two, z, quality=np.arange(6, dtype=np.float32))
-        _same_store(ga, o)
-        _same_store(gb, o)
+        same_store(ga, o)
+        same_store(gb, o)
         blob = gb.save()
         assert np.array_equal(ga.save(), blob)
         V3 = _lib.FstoreBlobHeaderV3
@@ -399,17 +344,16 @@ def test_twins_reached_by_different_routes_save_byte_equal_blobs():
         q = _quality(rng, 9)
         for s in (ga, gb, gc, o):
             s.add(np.array([1] * 4 + [2] * 5, np.uint64), _feats(np.random.default_rng(1), 9, 20, storage), quality=q)
-        _same_store(gc, o)
+        same_store(gc, o)
         assert np.array_equal(ga.save(), gb.save()) and np.array_equal(gb.save(), gc.save())
 
 
 def test_fetch_with_remove_and_a_repeated_id():
-    g, o = _pair(feature_dim=8)
+    g, o = store_pair(**QUALITY, feature_dim=8)
     f = _feats(np.random.default_rng(4), 3, 8, "f32")
     for s in (g, o):
         s.add([1, 1, 2], f, quality=[0.5, 0.75, 1.0])
     rg, ro = g.fetch_quality([1, 1, 2, 3], remove=True), o.fetch_quality([1, 1, 2, 3], remove=True)
-    for x, y in zip(rg, ro):
-        assert np.array_equal(x, y)
+    same_results(rg, ro)
     assert rg[0].tolist() == [2, 0, 1, 0] and not rg[2][1].any()
     assert g.size() == o.size() == 0

@@ -5,29 +5,20 @@ comparison is for equality, weights as f64 bits:
 - fed any other column, it holds the rows rounded once (fstore_oracle.round_rows), searches like an f32 store that holds
   the rounded rows and is queried with the unrounded ones, and associates like that search followed by add(round(rows));
 - its blob carries storage_type and a feat section of half the size, and continues exactly after a load."""
-import ctypes as C
-
 import numpy as np
 import pytest
 
 import fstore_oracle as fo
+from fstore_checks import METRICS, bits, gpu_store, refused_blob, same_results, store_options
 
 pytestmark = pytest.mark.gpu
 
-METRICS = {"euclidean": fo.EUCLIDEAN, "cosine": fo.COSINE}
 CODES = {"f32": 0, "f16": 1, "bf16": 2}
 
 
-def _opts(dim, K, **kw):
-    o = dict(distance_filter=1e9, max_observations=K, feature_dim=dim, topn=4, max_distance=1e9, min_votes=1)
-    o.update(kw)
-    return o
-
-
 def _store(metric, dim, K, column="f32", storage="f32", **kw):
-    import similari_b200.engine as eng
-
-    s = eng.FeatureStore(metric=metric, storage=storage, **_opts(dim, K, **kw))
+    """A store of the storage type whose host calls send columns of type `column`."""
+    s = gpu_store(metric, storage, max_observations=K, feature_dim=dim, **kw)
     s.set_feature_type(column)
     assert s.storage_type() == storage
     return s
@@ -58,18 +49,6 @@ def _pool(n, dim, t, seed, edges=True):
         for i, v in enumerate([0x0000, 0x8000, 0x0001, 0x807F, 0x7F7F, 0x3380, 0x477F, 0x4780]):
             bits[i, ::2] = v
     return bits, (bits.astype(np.uint32) << 16).view(np.float32)
-
-
-def _bits(a):
-    a = np.ascontiguousarray(a)
-    return a.view({4: np.uint32, 8: np.uint64}.get(a.dtype.itemsize, a.dtype)) if a.dtype.kind == "f" else a
-
-
-def _same(a, b):
-    assert len(a) == len(b)
-    for i, (x, y) in enumerate(zip(a, b)):
-        assert x.dtype == y.dtype and x.shape == y.shape, i
-        assert np.array_equal(_bits(x), _bits(y)), (i, x, y)
 
 
 def _flat(out):
@@ -167,11 +146,11 @@ def test_own_type_feed_equals_an_f32_store(storage, metric, K, dim):
     steps = _script(K, 96)
     raw, wide = _pool(96, dim, storage, seed=dim * 10 + K)
     want = _run(_store(metric, dim, K, storage, "f32"), steps, raw)
-    _same(_run(_store(metric, dim, K, storage, storage), steps, raw), want)
-    _same(_run(_store(metric, dim, K, storage, storage), steps, raw, device=True), want)
+    same_results(_run(_store(metric, dim, K, storage, storage), steps, raw), want)
+    same_results(_run(_store(metric, dim, K, storage, storage), steps, raw, device=True), want)
     if K == 3 and dim != 512:   # the f32 store itself against the oracle, on the widened rows
-        oracle = fo.FeatureStore(metric=METRICS[metric], **_opts(dim, K))
-        _same(_run(oracle, steps, wide), want)
+        oracle = fo.FeatureStore(metric=METRICS[metric], **store_options(max_observations=K, feature_dim=dim))
+        same_results(_run(oracle, steps, wide), want)
 
 
 # ------------------------------------------------------------------------------------------------ rounding feed
@@ -181,7 +160,7 @@ def _fetched_equal_model(store, ids, want):
         got, exp = feats[i, :c], want[i][:c]
         nan = np.isnan(exp)
         assert np.array_equal(np.isnan(got), nan)
-        assert np.array_equal(_bits(got[~nan]), _bits(exp[~nan]))
+        assert np.array_equal(bits(got[~nan]), bits(exp[~nan]))
 
 
 @pytest.mark.parametrize("storage,column", [("f16", "f32"), ("f16", "bf16"), ("bf16", "f32"), ("bf16", "f16")])
@@ -203,7 +182,7 @@ def test_rounding_feed(storage, column, metric):
     # search: queries are never rounded
     qids = np.arange(100, 106, dtype=np.uint64)
     offs = np.array([0, 1, 3, 6, 10, 14, 16], np.int32)
-    _same(_flat(half.search(qids, offs, raw[48:64])), _flat(ref.search(qids, offs, wide[48:64])))
+    same_results(_flat(half.search(qids, offs, raw[48:64])), _flat(ref.search(qids, offs, wide[48:64])))
     # associate = search with the unrounded rows, then add(dest, round(rows)) query by query (the newest K rows)
     aids = np.arange(200, 206, dtype=np.uint64)
     aoffs = np.array([0, 2, 3, 7, 9, 12, 16], np.int32)
@@ -216,12 +195,12 @@ def test_rounding_feed(storage, column, metric):
         ref.add(np.full(aoffs[q + 1] - lo, dest, np.uint64), fo.round_rows(a_wide[lo:aoffs[q + 1]], storage))
     want = dict(s, merged=(s["counts"] > 0).astype(np.uint8),
                 track_ids=np.where(s["counts"] > 0, s["winners"][:, 0], aids).astype(np.uint64))
-    _same(_flat(got), _flat(want))
+    same_results(_flat(got), _flat(want))
     assert np.array_equal(half.ids(), ref.ids())
     rc, rf = ref.fetch(ref.ids())
     _fetched_equal_model(half, ref.ids(), [rf[i] for i in range(len(rc))])
     # owned calls compare widened stored rows
-    _same(_flat(half.search_owned(half.ids(), each=True)), _flat(ref.search_owned(ref.ids(), each=True)))
+    same_results(_flat(half.search_owned(half.ids(), each=True)), _flat(ref.search_owned(ref.ids(), each=True)))
 
 
 # ------------------------------------------------------------------------------------------------ blob
@@ -271,7 +250,7 @@ def test_blob_of_a_half_store(storage, metric):
     copies = [eng.FeatureStore.load(blob), eng.FeatureStore.load(dblob.data_ptr(), n)]
     for c in copies:
         assert c.storage_type() == storage and c.feature_type() == storage
-        _same(_state(c), _state(s))
+        same_results(_state(c), _state(s))
         assert np.array_equal(c.save(), blob)
     steps = _script(K, 96)
     for st in steps:   # fresh ids: the script's query ids must not be stored yet
@@ -279,7 +258,7 @@ def test_blob_of_a_half_store(storage, metric):
             st[1][:] += 5000
     want = _run(s, steps, raw)
     for c in copies:
-        _same(_run(c, steps, raw), want)
+        same_results(_run(c, steps, raw), want)
 
 
 def test_blob_storage_type_is_checked():
@@ -287,28 +266,19 @@ def test_blob_storage_type_is_checked():
 
     s, _ = _worn("f16", "f16")
     f, _ = _worn("f32", "f16")
-    L = _lib.lib()
-
-    def refused(blob, field):
-        h = C.c_void_p()
-        blob = np.ascontiguousarray(blob)
-        assert L.sb200_fstore_load(_lib.ptr(blob), len(blob), 0, C.byref(h)) == -1
-        assert h.value is None
-        assert field in L.sb200_last_error().decode(), L.sb200_last_error()
-
     for blob in (s.save(), f.save()):
         b = blob.copy()
         _lib.FstoreBlobHeader.from_buffer(b).storage_type = 7
-        refused(b, "storage_type")
+        refused_blob(b, "storage_type")
         b = blob.copy()
         _lib.FstoreBlobHeader.from_buffer(b).storage_type = -1
-        refused(b, "storage_type")
+        refused_blob(b, "storage_type")
     b = f.save().copy()
     _lib.FstoreBlobHeader.from_buffer(b).storage_type = 1   # an f32 blob relabelled: its feat section is twice too big
-    refused(b, "feat holds")
+    refused_blob(b, "feat holds")
     b = s.save().copy()
     _lib.FstoreBlobHeader.from_buffer(b).storage_type = 0
-    refused(b, "feat holds")
+    refused_blob(b, "feat holds")
 
 
 def test_empty_half_store_blob():
@@ -340,7 +310,7 @@ def test_setter_refusals_and_reuse_after_removal():
         assert L.sb200_fstore_set_storage_type(s._h, t) == -1
         assert ("holds tracks" if t != 7 else "unknown") in L.sb200_last_error().decode()
     assert s.storage_type() == "f16"
-    _same(_state(s), before)
+    same_results(_state(s), before)
     assert np.array_equal(s.save(), blob)
     # emptied by fetch(remove): allowed again, also to a wider type than the columns were allocated for
     s.fetch(s.ids(), remove=True)
@@ -352,7 +322,7 @@ def test_setter_refusals_and_reuse_after_removal():
     for x in (s, fresh):
         x.add(ids[:100], raw[100:200])
         x.add(ids[100:], raw[200:400])   # grows past the old columns
-    _same(_state(s), _state(fresh))
+    same_results(_state(s), _state(fresh))
     assert np.array_equal(s.save(), fresh.save())
 
 
@@ -374,5 +344,5 @@ def test_gallery_search_is_identical_at_100k_tracks():
     qid = np.arange(10**9, 10**9 + Q, dtype=np.uint64)
     offs = np.arange(Q + 1, dtype=np.int32)
     a, b = (_flat(s.search(qid, offs, q)) for s in stores.values())
-    _same(a, b)
+    same_results(a, b)
     assert a[0].min() == 5

@@ -13,6 +13,8 @@ import dataclasses
 import numpy as np
 import pytest
 
+from fstore_checks import same_results, same_store, store_pair
+
 pytestmark = pytest.mark.gpu
 
 F32 = np.float32
@@ -150,23 +152,8 @@ def _compose(eng, t, s, cap, H, id_offset=0, history_cap=None):
     return res
 
 
-def _same(a, b):
-    assert a.keys() == b.keys()
-    for k in a:
-        x, y = a[k], b[k]
-        if isinstance(x, list):
-            assert len(x) == len(y), k
-            for u, v in zip(x, y):
-                assert np.array_equal(np.asarray(u).view(np.uint32), np.asarray(v).view(np.uint32)), k
-        elif x.dtype == np.float64 or y.dtype == np.float64:
-            assert np.array_equal(x.view(np.uint64), y.view(np.uint64)), k
-        elif x.dtype == F32:
-            assert np.array_equal(x.view(np.uint32), y.view(np.uint32)), k
-        else:
-            assert np.array_equal(x, y), (k, x, y)
-
-
 def _same_state(ta, tb, sa, sb):
+    same_store(sa, sb)
     assert np.array_equal(sa.save(), sb.save())
     assert np.array_equal(ta.save(), tb.save())
 
@@ -177,7 +164,7 @@ def _collect(eng, ta, tb, sa, sb, H, cap=None, id_offset=0, history_cap=None):
         tb = eng.Tracker.load(ta.save())
     a = sa.associate_wasted(ta, cap=cap, id_offset=id_offset, history_cap=history_cap)
     b = _compose(eng, tb, sb, len(a["ids"]) if cap is None else cap, H, id_offset, history_cap)
-    _same(a, b)
+    same_results(a, b)
     _same_state(ta, tb, sa, sb)
     return a
 
@@ -320,13 +307,9 @@ def test_freed_blocks_reused_by_the_next_frame(eng):
 
 def test_matches_the_oracle_directly(eng):
     """The composed rows through fstore_oracle's ofs_associate: winners and f64 weights match the call exactly."""
-    import fstore_oracle as fo
-
     dim, H = 32, 10
     t = _tracker(eng, 3, H, dim)
-    s = _store(eng, dim, K=3, topn=3)
-    o = fo.FeatureStore(metric=fo.EUCLIDEAN, distance_filter=1.0, max_observations=3, feature_dim=dim, topn=3,
-                        max_distance=1.0, min_votes=1)
+    s, o = store_pair(distance_filter=1.0, max_observations=3, feature_dim=dim, topn=3, max_distance=1.0)
     d = Driver(2, 40, dim, 0x5EED0500, gaps=True)
     merged = 0
     for fr in range(16):
@@ -345,10 +328,8 @@ def test_matches_the_oracle_directly(eng):
             if not qi:
                 continue
             r = o.associate(w["ids"][qi], offs, np.concatenate(rows))
-            assert np.array_equal(a["counts"][qi], r["counts"])
-            assert np.array_equal(a["winners"][qi], r["winners"])
-            assert np.array_equal(a["weights"][qi].view(np.uint64), r["weights"].view(np.uint64))
-            assert np.array_equal(a["merged"][qi], r["merged"])
+            same_results({k: a[k][qi] for k in ("counts", "winners", "weights", "merged")},
+                         {k: r[k] for k in ("counts", "winners", "weights", "merged")})
             merged += int(r["merged"].sum())
     assert merged > 0
 
@@ -380,9 +361,7 @@ def _nothing_moved(eng, ta, tb, s, blob, H=5):
     assert np.array_equal(s.save(), blob)
     a, b = _wasted_visual(eng, ta, 1 << 14, H), _wasted_visual(eng, tb, 1 << 14, H)
     assert len(a["ids"]) > 0
-    for k in a:
-        x, y = a[k], b[k]
-        assert np.array_equal(x.view(np.uint32) if x.dtype == F32 else x, y.view(np.uint32) if y.dtype == F32 else y), k
+    same_results(a, b)
 
 
 def test_refusals_before_anything_happens(eng):
