@@ -277,7 +277,7 @@ struct sb200_tracker {
   int stg_last = 1;   // staging set used by the most recent predict
   struct CandBufs { DBuf box, radius, conf, vert, flags, norm2, bf16, decided, fp8, scale; } cand[2];   // candidate side, two sets
   DBuf f_winner, f_cvt, f_pos, f_vis, f_scenes, f_newcount,
-      f_status, f_featdst, f_apprank, f_appmeta, f_frameout, f_excl, f_prewin, f_own, f_ownovf, f_dyn, f_ws, f_tmeta, f_rowinfo, f_slabc, f_slabm, f_slabmask,
+      f_status, f_featdst, f_approw, f_appmeta, f_frameout, f_excl, f_prewin, f_own, f_ownovf, f_dyn, f_ws, f_tmeta, f_rowinfo, f_slabc, f_slabm, f_slabmask,
       f_dscene, f_maxc, f_maxcval, f_drowb, f_dcolb, f_slabk, f_scene_max, f_tiles, f_pairs, f_colmeta, f_colgeo, f_colb, f_colvalid, f_rowmeta, f_poslist, f_counters, f_visval, f_colsb;
   int num_sms = 132;
   DBuf o_col[kOutCols];
@@ -878,7 +878,7 @@ struct sb200_tracker {
     if ((rc = ENS(cb.box, T * 24, f.c_box)) || (rc = ENS(cb.radius, T * 4, f.c_radius)) || (rc = ENS(cb.conf, T * 4, f.c_conf)) ||
         (rc = ENS(f_winner, T * 4, f.winner)) || (rc = ENS(f_cvt, T, f.c_vt)) ||
         (rc = ENS(f_scenes, sizeof(sb::SceneDesc) * n_scenes, f.scenes)) || (rc = ENS(f_newcount, 4 * (size_t)n_scenes, f.new_count)) ||
-        (rc = ENS(f_dyn, sizeof(sb::FrameDyn), f.dyn)) || (rc = ENS(f_apprank, T * 8, f.app_rank)) ||
+        (rc = ENS(f_dyn, sizeof(sb::FrameDyn), f.dyn)) || (rc = ENS(f_approw, 4 * (size_t)n_scenes * track_cap, f.app_row)) ||
         (rc = ENS(f_appmeta, 16 * (size_t)n_scenes, f.app_meta)) || (rc = ENS(f_pos, std::max<size_t>(4, (size_t)pl.pos_total * 4), f.pos)))
       return rc;
     if (P.positional_kind == SB200_POS_IOU && (rc = ENS(cb.vert, T * 64, f.c_vert))) return rc;
@@ -1160,7 +1160,7 @@ struct sb200_tracker {
     int vr = sb::launch_voting(Pf, ts, f, n_scenes, max_m, max_n, stream);
     if (vr != 0) return fail(SB200_ERR_CUDA, "voting launch failed: %s", cudaGetErrorString((cudaError_t)vr));
     CU(cudaEventRecord(q.ev[4], stream));
-    sb::launch_apply(Pf, ts, f, n_scenes, max_m, 0ull, b_ntracks.as<int>(), stream);
+    sb::launch_apply(Pf, ts, f, n_scenes, max_n + max_m, 0ull, b_ntracks.as<int>(), stream);
     // The sweep (latency-bound, one CTA per scene) and the feature store (HBM-bound) touch disjoint arrays -- a track's feature
     // block is not moved by the compaction -- so the sweep runs on the side stream beside the store; the frame ends at the join.
     const bool side_sweep = Pf.is_visual && f.in_feat && total > 0;

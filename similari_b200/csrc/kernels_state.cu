@@ -28,7 +28,8 @@ __device__ __forceinline__ void write_box_row(float* dst, const Box& b) {
 }
 
 // Phase 1 of apply (one CTA per scene): rank of every new-track candidate among the scene's new candidates (candidate
-// order), the scene of every detection, and the scene's counters.  The per-detection work is phase 2, one thread each.
+// order), the scene's counters, and the inverse map of the frame: for every store row j of the scene, the detection that
+// updates it (app_row, -1: no detection).  Phase 2 runs by store row, so that consecutive lanes write consecutive rows.
 __global__ void __launch_bounds__(AT) apply_rank_kernel(Params p, TrackStore ts, Frame f, int n_scenes, int* n_tracks) {
   __shared__ int s_warp[AT / 32];
   __shared__ int s_carry;
@@ -52,6 +53,9 @@ __global__ void __launch_bounds__(AT) apply_rank_kernel(Params p, TrackStore ts,
       s_newbefore = t;
     }
   }
+  // the stored rows nobody matches stay -1; rows [n, n + added) are all taken by the new tracks below
+  int* row_det = f.app_row + (size_t)sidx * ts.track_cap;
+  for (int j = tid; j < sc.n; j += AT) row_det[j] = -1;
   if (tid == 0) { s_carry = 0; if (!need_before) s_newbefore = 0; }
   __syncthreads();
   const int* winner = f.winner + sc.det_base;
@@ -75,15 +79,24 @@ __global__ void __launch_bounds__(AT) apply_rank_kernel(Params p, TrackStore ts,
     __syncthreads();
     if (tid == AT - 1) s_carry = carry + woff + x;
     __syncthreads();
-    if (active) f.app_rank[sc.det_base + m] = make_int2(sidx, rank);
+    if (active) {
+      const int g = sc.det_base + m;
+      if (!isnew) row_det[win] = g;
+      else if (sc.n + rank < ts.track_cap) row_det[sc.n + rank] = g;
+      else {   // store overflow: the frame fails; nothing of this detection may be stored later
+        atomicOr(&f.status[sidx], 1);
+        if (f.feat_dst) f.feat_dst[g] = -1;
+        if (f.hist_dst) f.hist_dst[g] = -1;
+      }
+    }
   }
   __syncthreads();
   if (tid == 0) {
     // feature arena of this scene (visual trackers): new tracks take blocks from the free list first, then fresh ones
     const int nfree0 = ts.fblk ? ts.n_free[sc.slot] : 0;
     const int top0 = ts.fblk ? ts.arena_top[sc.slot] : 0;
-    f.app_meta[sidx] = make_int4(s_newbefore, nfree0, top0, 0);
     const int added = min(sc.n + s_carry, ts.track_cap) - sc.n;
+    f.app_meta[sidx] = make_int4(s_newbefore, nfree0, top0, sc.n + added);
     n_tracks[sc.slot] = sc.n + added;
     if (ts.fblk) {
       ts.n_free[sc.slot] = nfree0 - min(nfree0, added);
@@ -92,289 +105,368 @@ __global__ void __launch_bounds__(AT) apply_rank_kernel(Params p, TrackStore ts,
   }
 }
 
-// Phase 2 of apply: one thread per detection creates its track or merges into the track it won.  WIDE (K > kMaxObs):
-// a merge leaves the track's observation list, its feature count and the detection's feature row to apply_obs_wide_kernel,
-// which runs next, one warp per detection, instead of holding K-sized lists per thread.
+// K <= kMaxObs: the observation list of a visual merge, unrolled to kMaxObs entries with only static indices, so that every
+// list stays in registers.  optimize_observations (visual_sort/metric.rs:297-374): retain the observations with a feature,
+// stable insertion sort by descending quality (the swaps make the same comparisons as the sequential shifts, NaN included),
+// drop the last when K are kept, push the new observation into the lowest free physical slot and swap it to the front.
+// Returns the physical slot of the new observation.
+struct ObsList {   // a track's stored list as loaded, entries k < K (those at and beyond n were never written)
+  int n;
+  unsigned long long hasf, phys;   // byte k: entry k (packed: the whole list fits the registers of the apply)
+  float q[kMaxObs];
+};
+// loaded without waiting for the count, so that the loads go out with the track's other loads
+__device__ __forceinline__ ObsList load_obs_list(const TrackStore& ts, size_t idx, int K) {
+  ObsList l;
+  l.n = ts.obs_n[idx];
+  l.hasf = l.phys = 0;
+#pragma unroll
+  for (int k = 0; k < kMaxObs; ++k) {
+    if (k < K) {
+      l.hasf |= (unsigned long long)ts.obs_hasf[idx * K + k] << (8 * k);
+      l.phys |= (unsigned long long)ts.obs_phys[idx * K + k] << (8 * k);
+    }
+    l.q[k] = k < K ? ts.obs_q[idx * K + k] : 0.0f;
+  }
+  return l;
+}
+__device__ __forceinline__ int merge_obs_list(const TrackStore& ts, size_t idx, int K, const ObsList& l, float quality,
+                                              bool keep) {
+  unsigned char phys[kMaxObs], hasf[kMaxObs];
+  float q[kMaxObs];
+  int cnt = 0;
+#pragma unroll
+  for (int k = 0; k < kMaxObs; ++k) {
+    const bool have = k < K && k < l.n;
+    const unsigned char lh = have ? (unsigned char)(l.hasf >> (8 * k)) : (unsigned char)0;
+    const unsigned char lp = (unsigned char)(l.phys >> (8 * k));
+    const float lq = l.q[k];
+    phys[k] = 0; q[k] = 0.0f; hasf[k] = 0;
+#pragma unroll
+    for (int c = 0; c <= k; ++c)
+      if (lh && c == cnt) { phys[c] = lp; q[c] = lq; }
+    cnt += lh ? 1 : 0;
+  }
+#pragma unroll
+  for (int a = 1; a < kMaxObs; ++a) {
+    bool shift = a < cnt;
+#pragma unroll
+    for (int b = a - 1; b >= 0; --b) {
+      shift = shift && q[b] < q[b + 1];
+      if (shift) {
+        const unsigned char tp = phys[b]; phys[b] = phys[b + 1]; phys[b + 1] = tp;
+        const float tq = q[b]; q[b] = q[b + 1]; q[b + 1] = tq;
+      }
+    }
+  }
+  if (cnt >= K && cnt > 0) --cnt;
+  unsigned int used = 0;
+#pragma unroll
+  for (int k = 0; k < kMaxObs; ++k)
+    if (k < cnt) { used |= 1u << phys[k]; hasf[k] = 1; }
+  const int freep = __ffs((int)~used) - 1;   // cnt < K <= kMaxObs: a slot is free
+  // push new, swap(0, last)
+#pragma unroll
+  for (int c = 0; c < kMaxObs; ++c)
+    if (c == cnt) { phys[c] = (unsigned char)freep; q[c] = quality; hasf[c] = keep ? 1 : 0; }
+  ++cnt;
+  unsigned char pl = 0, hl = 0;
+  float ql = 0.0f;
+#pragma unroll
+  for (int c = 0; c < kMaxObs; ++c)
+    if (c == cnt - 1) { pl = phys[c]; ql = q[c]; hl = hasf[c]; }
+#pragma unroll
+  for (int c = 1; c < kMaxObs; ++c)
+    if (c == cnt - 1) { phys[c] = phys[0]; q[c] = q[0]; hasf[c] = hasf[0]; }
+  phys[0] = pl; q[0] = ql; hasf[0] = hl;
+  int fc = 0;
+#pragma unroll
+  for (int k = 0; k < kMaxObs; ++k)
+    if (k < cnt) {
+      ts.obs_phys[idx * K + k] = phys[k]; ts.obs_q[idx * K + k] = q[k]; ts.obs_hasf[idx * K + k] = hasf[k];
+      fc += hasf[k];
+    }
+  ts.obs_n[idx] = (unsigned char)cnt;
+  ts.feat_cnt[idx] = (unsigned char)fc;
+  return freep;
+}
+
+// Phase 2 of apply, by store row: grid (row tiles, scenes), thread j of a scene creates or merges store row j from the
+// detection app_row names, and leaves at once when it names none.  Consecutive lanes hold consecutive rows, so the narrow
+// columns are written in whole sectors; the detection side is a gather inside the scene's candidate range.  The 128-byte
+// Kalman rows and the 64-byte vertex rows go through a per-warp tile of shared memory, so that each load or store instruction
+// moves whole rows (float4 chunk c of the warp's row r at r * 8 + (c ^ (r & 7)): no bank conflicts either way).
+// WIDE (K > kMaxObs): a merge leaves the track's observation list, its feature count and the detection's feature row to
+// apply_obs_wide_kernel, which runs next, one warp per row, instead of holding K-sized lists per thread.
+constexpr int APT = 128;   // threads of the row-indexed apply: ~10 CTAs for a scene of ~1,200 rows
+
 template <bool WIDE>
-__global__ void __launch_bounds__(256) apply_kernel(Params p, TrackStore ts, Frame f, unsigned long long id_base) {
+__global__ void __launch_bounds__(APT, 4) apply_kernel(Params p, TrackStore ts, Frame f, int n_scenes,
+                                                    unsigned long long id_base) {
+  __shared__ float4 s_tile[APT / 32][32 * 8];
+  __shared__ double2 s_vtile[APT / 32][32 * 4];
   const int K = p.max_obs;
-  {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= f.total) return;
-    const int g = f.det0 + i;
-    const int2 sr = f.app_rank[g];
-    const int sidx = sr.x, rank = sr.y;
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  float4* tile = s_tile[wid];
+  double2* vtile = s_vtile[wid];
+  if (f.id_counter) id_base = *f.id_counter;   // stream-ordered predict: the counter lives on the device
+  for (int sidx = blockIdx.y; sidx < n_scenes; sidx += gridDim.y) {
     const SceneDesc& sc = f.scenes[sidx];
     const int4 meta = f.app_meta[sidx];
-    const int s_newbefore = meta.x, nfree0 = meta.y, top0 = meta.z;
+    const int s_newbefore = meta.x, nfree0 = meta.y, top0 = meta.z, rows = meta.w;
     const size_t sbase = (size_t)sc.slot * ts.track_cap;
-    const int win = f.winner[g];
-    const int isnew = win < 0 ? 1 : 0;
-
-    const float* cbp = f.c_box + (size_t)g * 6;
-    const Box cb{cbp[0], cbp[1], cbp[2], cbp[3], cbp[4], cbp[5]};
-    const long long custom = f.in_custom ? f.in_custom[g] : (-9223372036854775807LL - 1);
-    const unsigned char flags = p.is_visual ? f.c_flags[g] : 0;
-    const float quality = (p.is_visual && f.in_quality) ? f.in_quality[g] : 1.0f;
-    unsigned long long tid64;
-    if (f.id_counter) id_base = *f.id_counter;   // stream-ordered predict: the counter lives on the device
-    if (p.is_batch) tid64 = id_base + (unsigned long long)g + 1ull;  // one id per candidate (batch_api.rs:102-106)
-    else tid64 = id_base + (unsigned long long)(s_newbefore + rank) + 1ull;
-    size_t idx;
-    float st[kStateFloats], st2[kStateFloats];
-    Box pred;
-    int fdst = -1;
-    unsigned long long o_id = 0; unsigned int o_len = 0; signed char o_vt = -1;   // SortTrack columns of this detection
-    if (isnew) {
-      const int j = sc.n + rank;
-      if (j >= ts.track_cap) {   // store overflow: the frame fails; nothing of this detection may be stored later
-        atomicOr(&f.status[sidx], 1);
-        if (f.feat_dst) f.feat_dst[g] = -1;
-        if (f.hist_dst) f.hist_dst[g] = -1;
-        return;
+    const int* row_det = f.app_row + (size_t)sidx * ts.track_cap;
+    for (int w0 = blockIdx.x * APT + wid * 32; w0 < rows; w0 += gridDim.x * APT) {   // warp-uniform
+      const int j = w0 + lane;
+      const int g = j < rows ? row_det[j] : -1;
+      const bool valid = g >= 0, isnew = j >= sc.n;
+      const unsigned int vmask = __ballot_sync(0xffffffffu, valid);
+      if (vmask == 0) continue;
+      const unsigned int mmask = __ballot_sync(0xffffffffu, valid && !isnew);
+      const size_t idx = sbase + j;
+      float4* k4 = reinterpret_cast<float4*>(ts.kst) + (sbase + w0) * (kStateStride / 4);
+      // the Kalman rows of the warp's merges, whole rows per load
+#pragma unroll
+      for (int it = 0; it < 8; ++it) {
+        const int r = it * 4 + (lane >> 3), c = lane & 7;
+        if ((mmask >> r) & 1u) tile[r * 8 + (c ^ (r & 7))] = k4[r * 8 + c];
       }
-      idx = (size_t)sc.slot * ts.track_cap + j;
-      const float* rb = f.in_boxes + (size_t)g * 6;
-      const Box raw{rb[0], rb[1], rb[2], rb[3], rb[4], rb[5]};
-      kalman_initiate(p.pos_weight, p.vel_weight, raw, st);
-      kalman_predict(p.pos_weight, p.vel_weight, st, st2);
-      kalman_update(p.pos_weight, st2, raw, st);
-      pred = state_box(st, raw.conf);
-      ts.id[idx] = tid64;
-      ts.length[idx] = 1;
-      ts.vt[idx] = -1;
-      o_id = tid64; o_len = 1; o_vt = -1;
-      write_box_row(ts.obs + idx * 6, raw);
-      if (p.is_visual) {
-        ts.obs_n[idx] = 1;
-        ts.obs_phys[idx * K] = 0;
-        ts.obs_hasf[idx * K] = flags & 1;
-        ts.obs_q[idx * K] = quality;
-        ts.feat_cnt[idx] = flags & 1;
-        size_t blk = idx;
-        if (ts.fblk) {
-          const int b = rank < nfree0 ? ts.blk_free[sbase + (nfree0 - 1 - rank)] : top0 + (rank - nfree0);
-          ts.fblk[idx] = b;
-          ts.blk_owner[sbase + b] = j;
-          blk = sbase + b;
-        }
-        if (flags & 1) fdst = (int)(blk * K);
-      }
-    } else {
-      idx = (size_t)sc.slot * ts.track_cap + win;
-      // every load of the merge first (one round trip to memory), then the arithmetic, then the stores
-#pragma unroll
-      if (ts.kst_stride == kStateStride) {   // 128-byte rows: eight 16-byte loads
-        const float4* r4 = reinterpret_cast<const float4*>(ts.kst + idx * kStateStride);
-        float4 v[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) v[i] = r4[i];
-#pragma unroll
-        for (int i = 0; i < kStateFloats; ++i) st2[i] = reinterpret_cast<const float*>(v)[i];
-      } else {
-#pragma unroll
-        for (int i = 0; i < kStateFloats; ++i) st2[i] = ts.kst[idx * ts.kst_stride + i];
-      }
-      const unsigned int len0 = ts.length[idx];
-      o_id = ts.id[idx];
-      int on = 0;
-      unsigned char l_hasf[kMaxObs], l_phys[kMaxObs]; float l_q[kMaxObs];
-      size_t blk = idx;
-      if (!WIDE && p.is_visual) {
-        on = ts.obs_n[idx];
-        for (int k = 0; k < K; ++k) {   // slots at and beyond obs_n were never written
-          const bool have = k < on;
-          l_hasf[k] = have ? ts.obs_hasf[idx * K + k] : (unsigned char)0;
-          l_phys[k] = have ? ts.obs_phys[idx * K + k] : (unsigned char)0;
-          l_q[k] = have ? ts.obs_q[idx * K + k] : 0.0f;
-        }
-        blk = feat_block(ts, sc.slot, idx);
-      }
-      kalman_predict(p.pos_weight, p.vel_weight, st2, st);
-      kalman_update(p.pos_weight, st, cb, st2);
-#pragma unroll
-      for (int i = 0; i < kStateFloats; ++i) st[i] = st2[i];
-      pred = state_box(st, cb.conf);
-      o_len = len0 + 1;
-      ts.length[idx] = o_len;
-      write_box_row(ts.obs + idx * 6, cb);
-      if (p.is_visual) {
-        o_vt = (signed char)f.c_vt[g];
-        ts.vt[idx] = o_vt;
-        if (!WIDE) {   // WIDE: apply_obs_wide_kernel
-          // is_merge && !feature_can_be_used(collect thresholds) => feature dropped (visual_sort/metric.rs:327-337)
-          bool keep = (flags & 1) != 0;
-          if (keep) {
-            bool ok = quality >= p.min_quality_collect;
-            if (p.use_own_area && f.in_own) ok = ok && (f.in_own[g] >= p.min_own_collect);
-            ok = ok && (box_area(cb.aspect, cb.height) >= p.min_area);
-            keep = ok;
+      __syncwarp();
+      if (valid) {
+        const float* cbp = f.c_box + (size_t)g * 6;
+        const Box cb{cbp[0], cbp[1], cbp[2], cbp[3], cbp[4], cbp[5]};
+        const long long custom = f.in_custom ? f.in_custom[g] : (-9223372036854775807LL - 1);
+        const unsigned char flags = p.is_visual ? f.c_flags[g] : 0;
+        const float quality = (p.is_visual && f.in_quality) ? f.in_quality[g] : 1.0f;
+        const int rank = j - sc.n;
+        unsigned long long tid64;
+        if (p.is_batch) tid64 = id_base + (unsigned long long)g + 1ull;  // one id per candidate (batch_api.rs:102-106)
+        else tid64 = id_base + (unsigned long long)(s_newbefore + rank) + 1ull;
+        // every load of the row first (one round trip to memory), then the arithmetic, then the stores
+        unsigned int len0 = 0; unsigned long long id0 = 0; int blk_b = 0, hb = 0;
+        ObsList ol;
+        if (!isnew) {
+          len0 = ts.length[idx];
+          id0 = ts.id[idx];
+          if (!WIDE && p.is_visual) {
+            ol = load_obs_list(ts, idx, K);
+            if (ts.fblk) blk_b = ts.fblk[idx];
           }
-          // optimize_observations: retain featured, stable sort by quality desc, drop last when len >= max
-          unsigned char phys[kMaxObs]; float q[kMaxObs];
-          int cnt = 0;
-          unsigned int used = 0;
-          for (int k = 0; k < K; ++k) {
-            if (k < on && l_hasf[k]) {
-              phys[cnt] = l_phys[k]; q[cnt] = l_q[k];
-              ++cnt;
+          if (ts.hblk) hb = ts.hblk[idx];
+        } else {
+          if (ts.fblk) blk_b = rank < nfree0 ? ts.blk_free[sbase + (nfree0 - 1 - rank)] : top0 + (rank - nfree0);
+          if (ts.hblk) {
+            // a new track takes the history-pool block of its frame-wide rank: the free list first, then fresh blocks
+            const int r = s_newbefore + rank, hn0 = ts.hpool[0];
+            hb = r < hn0 ? ts.hfree[hn0 - 1 - r] : ts.hpool[1] + (r - hn0);
+          }
+        }
+        float st[kStateFloats], st2[kStateFloats];
+        Box pred;
+        // this lane's new Kalman row (zero-padded to 128 bytes) and vertex row into the warp's tiles, as soon as they are
+        // known: the state is dead before the observation list is merged
+        auto stage = [&](const Box& pr) {
+#pragma unroll
+          for (int c = 0; c < 8; ++c) {
+            float e[4];
+#pragma unroll
+            for (int i = 0; i < 4; ++i) e[i] = 4 * c + i < kStateFloats ? st[4 * c + i] : 0.0f;
+            tile[lane * 8 + (c ^ (lane & 7))] = make_float4(e[0], e[1], e[2], e[3]);
+          }
+          if (p.positional_kind == 1) {   // double2 chunk c of row r at r * 4 + (c ^ ((r >> 1) & 3))
+            double vx[8];
+            box_vertices(pr.xc, pr.yc, pr.angle, pr.aspect, pr.height, vx);
+#pragma unroll
+            for (int c = 0; c < 4; ++c) vtile[lane * 4 + (c ^ ((lane >> 1) & 3))] = make_double2(vx[2 * c], vx[2 * c + 1]);
+          }
+        };
+        int fdst = -1;
+        unsigned long long o_id = 0; unsigned int o_len = 0; signed char o_vt = -1;   // SortTrack columns of this detection
+        if (isnew) {
+          const float* rb = f.in_boxes + (size_t)g * 6;
+          const Box raw{rb[0], rb[1], rb[2], rb[3], rb[4], rb[5]};
+          kalman_initiate(p.pos_weight, p.vel_weight, raw, st);
+          kalman_predict(p.pos_weight, p.vel_weight, st, st2);
+          kalman_update(p.pos_weight, st2, raw, st);
+          pred = state_box(st, raw.conf);
+          stage(pred);
+          ts.id[idx] = tid64;
+          ts.length[idx] = 1;
+          ts.vt[idx] = -1;
+          o_id = tid64; o_len = 1; o_vt = -1;
+          write_box_row(ts.obs + idx * 6, raw);
+          if (p.is_visual) {
+            ts.obs_n[idx] = 1;
+            ts.obs_phys[idx * K] = 0;
+            ts.obs_hasf[idx * K] = flags & 1;
+            ts.obs_q[idx * K] = quality;
+            ts.feat_cnt[idx] = flags & 1;
+            size_t blk = idx;
+            if (ts.fblk) {
+              ts.fblk[idx] = blk_b;
+              ts.blk_owner[sbase + blk_b] = j;
+              blk = sbase + blk_b;
+            }
+            if (flags & 1) fdst = (int)(blk * K);
+          }
+        } else {
+#pragma unroll
+          for (int c = 0; c < 8; ++c) {
+            const float4 v = tile[lane * 8 + (c ^ (lane & 7))];
+            const float e[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+            for (int i = 0; i < 4; ++i)
+              if (4 * c + i < kStateFloats) st2[4 * c + i] = e[i];
+          }
+          o_id = id0;
+          kalman_predict(p.pos_weight, p.vel_weight, st2, st);
+          kalman_update(p.pos_weight, st, cb, st2);
+#pragma unroll
+          for (int i = 0; i < kStateFloats; ++i) st[i] = st2[i];
+          pred = state_box(st, cb.conf);
+          stage(pred);
+          o_len = len0 + 1;
+          ts.length[idx] = o_len;
+          write_box_row(ts.obs + idx * 6, cb);
+          if (p.is_visual) {
+            o_vt = (signed char)f.c_vt[g];
+            ts.vt[idx] = o_vt;
+            if (!WIDE) {   // WIDE: apply_obs_wide_kernel
+              // is_merge && !feature_can_be_used(collect thresholds) => feature dropped (visual_sort/metric.rs:327-337)
+              bool keep = (flags & 1) != 0;
+              if (keep) {
+                bool ok = quality >= p.min_quality_collect;
+                if (p.use_own_area && f.in_own) ok = ok && (f.in_own[g] >= p.min_own_collect);
+                ok = ok && (box_area(cb.aspect, cb.height) >= p.min_area);
+                keep = ok;
+              }
+              const size_t blk = ts.fblk ? sbase + blk_b : idx;   // feat_block
+              const int freep = merge_obs_list(ts, idx, K, ol, quality, keep);
+              if (keep) fdst = (int)(blk * K + freep);
             }
           }
-          for (int a = 1; a < cnt; ++a) {  // stable insertion sort, descending quality
-            unsigned char pa = phys[a]; float qa = q[a];
-            int b = a - 1;
-            while (b >= 0 && q[b] < qa) { phys[b + 1] = phys[b]; q[b + 1] = q[b]; --b; }
-            phys[b + 1] = pa; q[b + 1] = qa;
-          }
-          if (cnt >= K && cnt > 0) --cnt;
-          for (int k = 0; k < cnt; ++k) used |= 1u << phys[k];
-          int freep = 0;
-          while (used & (1u << freep)) ++freep;
-          // push new, swap(0, last)
-          unsigned char hasf_l[kMaxObs];
-          for (int k = 0; k < cnt; ++k) hasf_l[k] = 1;
-          phys[cnt] = (unsigned char)freep; q[cnt] = quality; hasf_l[cnt] = keep ? 1 : 0;
-          ++cnt;
-          { unsigned char tp = phys[0]; phys[0] = phys[cnt - 1]; phys[cnt - 1] = tp;
-            float tq = q[0]; q[0] = q[cnt - 1]; q[cnt - 1] = tq;
-            unsigned char th = hasf_l[0]; hasf_l[0] = hasf_l[cnt - 1]; hasf_l[cnt - 1] = th; }
-          int fc = 0;
-          for (int k = 0; k < cnt; ++k) {
-            ts.obs_phys[idx * K + k] = phys[k]; ts.obs_q[idx * K + k] = q[k]; ts.obs_hasf[idx * K + k] = hasf_l[k];
-            fc += hasf_l[k];
-          }
-          ts.obs_n[idx] = (unsigned char)cnt;
-          ts.feat_cnt[idx] = (unsigned char)fc;
-          if (keep) fdst = (int)(blk * K + freep);
+        }
+        ts.epoch[idx] = sc.epoch;
+        ts.custom[idx] = custom;
+        write_box_row(ts.pred + idx * 6, pred);
+        ts.radius[idx] = box_radius(pred.aspect, pred.height);
+        if (f.feat_dst && !(WIDE && !isnew)) f.feat_dst[g] = fdst;
+        if (ts.hblk) {
+          // feature history: every observation pushes its feature, or None, before the collect gate
+          // (VisualMetric::optimize, visual_sort/metric.rs:319-324).  The sweep at the end of the frame advances hpool by
+          // the count of new tracks.
+          if (isnew) ts.hblk[idx] = hb;
+          const size_t hrow = (size_t)hb * ts.fhist_len + (o_len - 1u) % (unsigned int)ts.fhist_len;
+          ts.hpresent[hrow] = flags & 1;
+          f.hist_dst[g] = (flags & 1) ? (int)hrow : -1;
+        }
+        const float* rb2 = f.in_boxes + (size_t)g * 6;
+        const Box obs = isnew ? Box{rb2[0], rb2[1], rb2[2], rb2[3], rb2[4], rb2[5]} : cb;
+        if (ts.hist_len > 1) {   // update_history: observation number o_len - 1 goes to ring slot (o_len - 1) % hist_len
+          const size_t hslot = (idx * ts.hist_len + (size_t)((o_len - 1u) % (unsigned int)ts.hist_len)) * 6;
+          write_box_row(ts.hist_pred + hslot, pred);
+          write_box_row(ts.hist_obs + hslot, obs);
+        }
+        // SortTrack (src/trackers/sort.rs:286-311)
+        if (f.o_ids) f.o_ids[g] = o_id;
+        if (f.o_epochs) f.o_epochs[g] = sc.epoch;
+        if (f.o_lengths) f.o_lengths[g] = o_len;
+        if (f.o_vt) f.o_vt[g] = p.is_visual ? (o_vt < 0 ? (unsigned char)1 : (unsigned char)o_vt) : (unsigned char)1;
+        if (f.o_pred) write_box(f.o_pred + (size_t)g * 6, pred);
+        if (f.o_obs) write_box(f.o_obs + (size_t)g * 6, obs);
+      }
+      // the new Kalman and vertex rows, whole rows per store
+      __syncwarp();
+#pragma unroll
+      for (int it = 0; it < 8; ++it) {
+        const int r = it * 4 + (lane >> 3), c = lane & 7;
+        if ((vmask >> r) & 1u) k4[r * 8 + c] = tile[r * 8 + (c ^ (r & 7))];
+      }
+      if (p.positional_kind == 1) {
+        double2* v2 = reinterpret_cast<double2*>(ts.vert) + (sbase + w0) * 4;
+#pragma unroll
+        for (int it = 0; it < 4; ++it) {
+          const int r = it * 8 + (lane >> 2), c = lane & 3;
+          if ((vmask >> r) & 1u) v2[r * 4 + c] = vtile[r * 4 + (c ^ ((r >> 1) & 3))];
         }
       }
+      __syncwarp();   // the next round refills the tiles
     }
-    ts.epoch[idx] = sc.epoch;
-    ts.custom[idx] = custom;
-    if (ts.kst_stride == kStateStride) {
-      float4 v[8];
-#pragma unroll
-      for (int i = 0; i < 32; ++i) reinterpret_cast<float*>(v)[i] = i < kStateFloats ? st[i] : 0.0f;
-      float4* r4 = reinterpret_cast<float4*>(ts.kst + idx * kStateStride);
-#pragma unroll
-      for (int i = 0; i < 8; ++i) r4[i] = v[i];
-    } else {
-#pragma unroll
-      for (int i = 0; i < kStateFloats; ++i) ts.kst[idx * ts.kst_stride + i] = st[i];
-    }
-    write_box_row(ts.pred + idx * 6, pred);
-    ts.radius[idx] = box_radius(pred.aspect, pred.height);
-    if (p.positional_kind == 1) {
-      double vx[8];
-      box_vertices(pred.xc, pred.yc, pred.angle, pred.aspect, pred.height, vx);
-      double2* v2 = reinterpret_cast<double2*>(ts.vert + idx * 8);
-#pragma unroll
-      for (int i = 0; i < 4; ++i) v2[i] = make_double2(vx[2 * i], vx[2 * i + 1]);
-    }
-    if (f.feat_dst && !(WIDE && !isnew)) f.feat_dst[g] = fdst;
-    if (ts.hblk) {
-      // feature history: every observation pushes its feature, or None, before the collect gate
-      // (VisualMetric::optimize, visual_sort/metric.rs:319-324).  A new track takes the pool block of its frame-wide rank:
-      // the free list first, then fresh blocks.  The sweep at the end of the frame advances hpool by the same count.
-      int hb;
-      if (isnew) {
-        const int r = s_newbefore + rank, hn0 = ts.hpool[0];
-        hb = r < hn0 ? ts.hfree[hn0 - 1 - r] : ts.hpool[1] + (r - hn0);
-        ts.hblk[idx] = hb;
-      } else {
-        hb = ts.hblk[idx];
-      }
-      const size_t hrow = (size_t)hb * ts.fhist_len + (o_len - 1u) % (unsigned int)ts.fhist_len;
-      ts.hpresent[hrow] = flags & 1;
-      f.hist_dst[g] = (flags & 1) ? (int)hrow : -1;
-    }
-    if (ts.hist_len > 1) {   // update_history: observation number o_len - 1 goes to ring slot (o_len - 1) % hist_len
-      const size_t hslot = (idx * ts.hist_len + (size_t)((o_len - 1u) % (unsigned int)ts.hist_len)) * 6;
-      write_box_row(ts.hist_pred + hslot, pred);
-      if (isnew) {
-        const float* rb2 = f.in_boxes + (size_t)g * 6;
-        write_box_row(ts.hist_obs + hslot, Box{rb2[0], rb2[1], rb2[2], rb2[3], rb2[4], rb2[5]});
-      } else write_box_row(ts.hist_obs + hslot, cb);
-    }
-    // SortTrack (src/trackers/sort.rs:286-311)
-    if (f.o_ids) f.o_ids[g] = o_id;
-    if (f.o_epochs) f.o_epochs[g] = sc.epoch;
-    if (f.o_lengths) f.o_lengths[g] = o_len;
-    if (f.o_vt) f.o_vt[g] = p.is_visual ? (o_vt < 0 ? (unsigned char)1 : (unsigned char)o_vt) : (unsigned char)1;
-    if (f.o_pred) write_box(f.o_pred + (size_t)g * 6, pred);
-    if (f.o_obs) write_box(f.o_obs + (size_t)g * 6, isnew ? Box{f.in_boxes[(size_t)g * 6], f.in_boxes[(size_t)g * 6 + 1], f.in_boxes[(size_t)g * 6 + 2], f.in_boxes[(size_t)g * 6 + 3], f.in_boxes[(size_t)g * 6 + 4], f.in_boxes[(size_t)g * 6 + 5]} : cb);
   }
 }
 
-// The observation list of a visual merge for K > kMaxObs (K <= 32): one warp per detection, lane k holding logical
-// observation k (physical slot, quality, feature flag).  Same steps as apply_kernel<false>, in the same order:
+// The observation list of a visual merge for K > kMaxObs (K <= 32): one warp per stored row, lane k holding logical
+// observation k (physical slot, quality, feature flag).  Same steps as merge_obs_list, in the same order:
 // optimize_observations keeps the observations with a feature, insertion-sorts them by descending quality (one
 // insertion per step; the ballot finds where the shifting stops, exactly as the sequential loop does, NaN qualities
 // included), drops the last when K are kept, then pushes the new observation into the lowest free physical slot and swaps
-// it to the front.  A 32-bit mask holds every physical slot, which bounds K at 32.
-__global__ void __launch_bounds__(256) apply_obs_wide_kernel(Params p, TrackStore ts, Frame f) {
-  const int w = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
-  if (w >= f.total) return;
-  const int g = f.det0 + w;
-  const int win = f.winner[g];
-  if (win < 0) return;   // a new track: apply_kernel wrote its single observation
+// it to the front.  A 32-bit mask holds every physical slot, which bounds K at 32.  Rows below the scene's n are merges.
+__global__ void __launch_bounds__(256) apply_obs_wide_kernel(Params p, TrackStore ts, Frame f, int n_scenes) {
+  const int lane = threadIdx.x & 31, wpb = blockDim.x >> 5;
   const int K = p.max_obs;
   const unsigned int all = 0xffffffffu;
-  const SceneDesc& sc = f.scenes[f.app_rank[g].x];
-  const size_t idx = (size_t)sc.slot * ts.track_cap + win;
-  const unsigned char flags = f.c_flags[g];
-  const float quality = f.in_quality ? f.in_quality[g] : 1.0f;
-  bool keep = (flags & 1) != 0;   // the collect gate of apply_kernel
-  if (keep) {
-    const float* cbp = f.c_box + (size_t)g * 6;
-    bool ok = quality >= p.min_quality_collect;
-    if (p.use_own_area && f.in_own) ok = ok && (f.in_own[g] >= p.min_own_collect);
-    ok = ok && (box_area(cbp[3], cbp[4]) >= p.min_area);
-    keep = ok;
-  }
-  const int on = ts.obs_n[idx];
-  const bool have = lane < on && lane < K;   // slots at and beyond obs_n were never written
-  const bool retain = have && ts.obs_hasf[idx * K + lane];
-  const int ph0 = retain ? ts.obs_phys[idx * K + lane] : 0;
-  const float q0 = retain ? ts.obs_q[idx * K + lane] : 0.0f;
-  // retain featured, in logical order: lane j takes the j-th retained observation
-  const unsigned int rmask = __ballot_sync(all, retain);
-  int cnt = __popc(rmask);
-  int src = 0;   // lowest bit s with popc(rmask & bits 0..s) == lane + 1 (binary search; 31 when lane >= cnt)
-  for (int b = 16; b > 0; b >>= 1)
-    if (__popc(rmask & ((2u << (src + b - 1)) - 1u)) < lane + 1) src += b;
-  int ph = __shfl_sync(all, ph0, src);
-  float q = __shfl_sync(all, q0, src);
-  for (int a = 1; a < cnt; ++a) {   // stable insertion sort, descending quality
-    const float qa = __shfl_sync(all, q, a);
-    const int pa = __shfl_sync(all, ph, a);
-    // the sequential loop shifts while q[b] < qa, from b = a - 1 down: it stops below the highest b < a without that
-    const unsigned int stop = __ballot_sync(all, lane < a && !(q < qa));
-    const int pos = stop ? 32 - __clz((int)stop) : 0;
-    const float qu = __shfl_up_sync(all, q, 1);
-    const int pu = __shfl_up_sync(all, ph, 1);
-    if (lane > pos && lane <= a) { q = qu; ph = pu; }
-    if (lane == pos) { q = qa; ph = pa; }
-  }
-  if (cnt >= K && cnt > 0) --cnt;
-  const unsigned int used = __reduce_or_sync(all, lane < cnt ? 1u << ph : 0u);
-  const int freep = __ffs((int)~used) - 1;   // cnt < K <= 32: a slot is free
-  // push new, swap(0, last)
-  unsigned char hasf = lane < cnt ? 1 : 0;
-  if (lane == cnt) { ph = freep; q = quality; hasf = keep ? 1 : 0; }
-  ++cnt;
-  const int from = lane == 0 ? cnt - 1 : (lane == cnt - 1 ? 0 : lane);
-  ph = __shfl_sync(all, ph, from);
-  q = __shfl_sync(all, q, from);
-  hasf = (unsigned char)__shfl_sync(all, (int)hasf, from);
-  if (lane < cnt) {
-    ts.obs_phys[idx * K + lane] = (unsigned char)ph; ts.obs_q[idx * K + lane] = q; ts.obs_hasf[idx * K + lane] = hasf;
-  }
-  const int fc = __popc(__ballot_sync(all, lane < cnt && hasf));
-  if (lane == 0) {
-    ts.obs_n[idx] = (unsigned char)cnt;
-    ts.feat_cnt[idx] = (unsigned char)fc;
-    if (f.feat_dst) f.feat_dst[g] = keep ? (int)(feat_block(ts, sc.slot, idx) * K + freep) : -1;
+  for (int sidx = blockIdx.y; sidx < n_scenes; sidx += gridDim.y) {
+    const int slot = f.scenes[sidx].slot, n = f.scenes[sidx].n;
+    const int* row_det = f.app_row + (size_t)sidx * ts.track_cap;
+    for (int j = blockIdx.x * wpb + (int)(threadIdx.x >> 5); j < n; j += gridDim.x * wpb) {
+      const int g = row_det[j];
+      if (g < 0) continue;
+      const size_t idx = (size_t)slot * ts.track_cap + j;
+      const unsigned char flags = f.c_flags[g];
+      const float quality = f.in_quality ? f.in_quality[g] : 1.0f;
+      bool keep = (flags & 1) != 0;   // the collect gate of apply_kernel
+      if (keep) {
+        const float* cbp = f.c_box + (size_t)g * 6;
+        bool ok = quality >= p.min_quality_collect;
+        if (p.use_own_area && f.in_own) ok = ok && (f.in_own[g] >= p.min_own_collect);
+        ok = ok && (box_area(cbp[3], cbp[4]) >= p.min_area);
+        keep = ok;
+      }
+      const int on = ts.obs_n[idx];
+      const bool have = lane < on && lane < K;   // slots at and beyond obs_n were never written
+      const bool retain = have && ts.obs_hasf[idx * K + lane];
+      const int ph0 = retain ? ts.obs_phys[idx * K + lane] : 0;
+      const float q0 = retain ? ts.obs_q[idx * K + lane] : 0.0f;
+      // retain featured, in logical order: lane j takes the j-th retained observation
+      const unsigned int rmask = __ballot_sync(all, retain);
+      int cnt = __popc(rmask);
+      int src = 0;   // lowest bit s with popc(rmask & bits 0..s) == lane + 1 (binary search; 31 when lane >= cnt)
+      for (int b = 16; b > 0; b >>= 1)
+        if (__popc(rmask & ((2u << (src + b - 1)) - 1u)) < lane + 1) src += b;
+      int ph = __shfl_sync(all, ph0, src);
+      float q = __shfl_sync(all, q0, src);
+      for (int a = 1; a < cnt; ++a) {   // stable insertion sort, descending quality
+        const float qa = __shfl_sync(all, q, a);
+        const int pa = __shfl_sync(all, ph, a);
+        // the sequential loop shifts while q[b] < qa, from b = a - 1 down: it stops below the highest b < a without that
+        const unsigned int stop = __ballot_sync(all, lane < a && !(q < qa));
+        const int pos = stop ? 32 - __clz((int)stop) : 0;
+        const float qu = __shfl_up_sync(all, q, 1);
+        const int pu = __shfl_up_sync(all, ph, 1);
+        if (lane > pos && lane <= a) { q = qu; ph = pu; }
+        if (lane == pos) { q = qa; ph = pa; }
+      }
+      if (cnt >= K && cnt > 0) --cnt;
+      const unsigned int used = __reduce_or_sync(all, lane < cnt ? 1u << ph : 0u);
+      const int freep = __ffs((int)~used) - 1;   // cnt < K <= 32: a slot is free
+      // push new, swap(0, last)
+      unsigned char hasf = lane < cnt ? 1 : 0;
+      if (lane == cnt) { ph = freep; q = quality; hasf = keep ? 1 : 0; }
+      ++cnt;
+      const int from = lane == 0 ? cnt - 1 : (lane == cnt - 1 ? 0 : lane);
+      ph = __shfl_sync(all, ph, from);
+      q = __shfl_sync(all, q, from);
+      hasf = (unsigned char)__shfl_sync(all, (int)hasf, from);
+      if (lane < cnt) {
+        ts.obs_phys[idx * K + lane] = (unsigned char)ph; ts.obs_q[idx * K + lane] = q; ts.obs_hasf[idx * K + lane] = hasf;
+      }
+      const int fc = __popc(__ballot_sync(all, lane < cnt && hasf));
+      if (lane == 0) {
+        ts.obs_n[idx] = (unsigned char)cnt;
+        ts.feat_cnt[idx] = (unsigned char)fc;
+        if (f.feat_dst) f.feat_dst[g] = keep ? (int)(feat_block(ts, slot, idx) * K + freep) : -1;
+      }
+    }
   }
 }
 
@@ -590,19 +682,21 @@ void launch_hist_gather(const TrackStore& ts, int d8, const int* blk, const unsi
   note_launch();
 }
 
-void launch_apply(const Params& p, const TrackStore& ts, const Frame& f, int n_scenes, int max_m,
+void launch_apply(const Params& p, const TrackStore& ts, const Frame& f, int n_scenes, int max_rows,
                   unsigned long long id_base, int* d_n_tracks, cudaStream_t st) {
-  (void)max_m;
   if (n_scenes == 0) return;
   apply_rank_kernel<<<n_scenes, AT, 0, st>>>(p, ts, f, n_scenes, d_n_tracks);
   note_launch();
   if (f.total > 0) {
+    // max_rows bounds every scene's rows (stored tracks + detections); the kernels stride past it all the same
+    const int rows = std::max(1, std::min(max_rows, ts.track_cap));
+    const dim3 grid((unsigned)((rows + APT - 1) / APT), scene_grid(n_scenes));
     if (p.max_obs > kMaxObs) {
-      apply_kernel<true><<<(f.total + 255) / 256, 256, 0, st>>>(p, ts, f, id_base);
-      apply_obs_wide_kernel<<<(unsigned)(((long long)f.total * 32 + 255) / 256), 256, 0, st>>>(p, ts, f);
+      apply_kernel<true><<<grid, APT, 0, st>>>(p, ts, f, n_scenes, id_base);
+      apply_obs_wide_kernel<<<dim3((unsigned)((rows + 7) / 8), scene_grid(n_scenes)), 256, 0, st>>>(p, ts, f, n_scenes);
       note_launch(2);
     } else {
-      apply_kernel<false><<<(f.total + 255) / 256, 256, 0, st>>>(p, ts, f, id_base);
+      apply_kernel<false><<<grid, APT, 0, st>>>(p, ts, f, n_scenes, id_base);
       note_launch();
     }
   }

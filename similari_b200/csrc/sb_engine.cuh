@@ -418,8 +418,9 @@ struct Frame {  // per-request transient device buffers (a request may be proces
   int* bf16_log;           // [total] with skip_bf16: feat_dst again, this frame's part of the tracker's dirty-row log
                            // (null: the log is full, every arena row gets converted)
   int* hist_dst;           // [total] destination history row (block*fhist_len + ring slot) or -1 (null: history off)
-  int2* app_rank;          // [total] apply phase 1: (scene of the detection, rank among the scene's new tracks)
-  int4* app_meta;          // [scenes] apply phase 1: (new tracks of earlier scenes, free blocks, arena top) before the frame
+  int* app_row;            // [scenes][track_cap] apply phase 1: the detection that updates store row j of the scene, or -1
+  int4* app_meta;          // [scenes] apply phase 1: (new tracks of earlier scenes, free blocks, arena top) before the frame,
+                           // and the scene's store rows after it
   int* frame_out;          // [n_scenes][3] written by the end-of-frame sweep: live tracks, arena blocks, newly expired
   const FrameDyn* dyn;     // device-built frame scalars (null in the stateless operators: host values are used)
   unsigned long long* id_counter;   // device copy of the tracker's id counter (null: the id_base argument is used)
@@ -598,7 +599,8 @@ constexpr size_t kVotingSmemLimit = 220 * 1024;
 // returns cudaError from configuration (dynamic smem), 0 on success
 int launch_voting(const Params& p, const TrackStore& ts, const Frame& f, int n_scenes, int max_m, int max_n,
                   cudaStream_t st);
-void launch_apply(const Params& p, const TrackStore& ts, const Frame& f, int n_scenes, int max_m,
+// max_rows: an upper bound of every scene's stored tracks plus detections
+void launch_apply(const Params& p, const TrackStore& ts, const Frame& f, int n_scenes, int max_rows,
                   unsigned long long id_base, int* d_n_tracks, cudaStream_t st);
 // the kept features of the frame -> the tracks' feature blocks; false when the frame has none (no launch)
 bool launch_feat_store(const Params& p, const TrackStore& ts, const Frame& f, cudaStream_t st);
